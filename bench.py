@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- queries/sec of SearchArray's scoring hot path on B200 (see BASELINE.json).
+"""bench.py -- queries/sec of SearchArray's scoring hot path on H100 (see BASELINE.json).
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
     python bench.py --impl reference --gpus N --steps K --warmup W   # the CPU reference arm
+    python bench.py ... --dump-outputs DIR     # also write the last timed step's top-k to DIR/*.npy
 
 Workload (config.workload): BASELINE.json configs[1] -- 10M-doc synthetic MSMARCO-shaped corpus
 (searcharray_b200/synth.py, seeded, generated as postings), single-term BM25.  One "step" = one
@@ -17,7 +18,8 @@ the per-shard top-k per batch.
           (sa_score_batch_topk: H2D of the query descriptors, kernels, D2H of the top-k).
   e2e_dense : the literal `.score()` drop-in (sa_score_term), D2H of the dense float32[N] per query.
   roofline  : term_tile_kernel, algorithmic bytes 8*W + 4*df + 4*N per query (SURVEY 8d) over the
-          kernel's CUDA-event time, against MEASURED_PEAKS.json's hbm_gbs; per-df-bucket fractions.
+          kernel's CUDA-event time, against MEASURED_PEAKS.json's hbm_gbs (the H100 SXM data sheet's
+          3.35 TB/s when that file is absent); per-df-bucket fractions.
   cpu_baseline : the reference's own `SearchArray.score` (oracle/_ref, `kind: "reference"`; the
           oracle port when that build is absent) on the host cores, bounded sample, NO top-k
           (the reference's stock call returns the dense vector; a top-k variant is reported apart).
@@ -40,6 +42,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 K1, B = 1.2, 0.75
+NOMINAL_HBM_GBS = 3350.0        # H100 SXM HBM3, data sheet
 
 
 def log(*a):
@@ -423,26 +426,13 @@ class Ours:
 
 
 def peak_hbm():
-    peak, src = 6650.0, "fallback (B200_PROFILING.md)"
+    peak, src = NOMINAL_HBM_GBS, "H100 SXM data sheet, nominal (not a measured peak)"
     try:
         mp = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         peak, src = float(mp["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs"
     except Exception:
         pass
     return peak, src
-
-
-def committed_traffic(kernel, cfg):
-    """DRAM bytes per launch of `kernel` from the committed `ncu --set full` capture of this very
-    workload (it cannot be measured live); None for any other configuration."""
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "kernel_traffic.json")))
-        for ent in tj.get(kernel, []):
-            if ent["config"] == cfg:
-                return float(ent["dram_bytes_read_per_launch"] + ent["dram_bytes_write_per_launch"]), ent["source"]
-    except Exception:
-        pass
-    return None, None
 
 
 def oracle_topk_term(full, avgdl, idf, term_id, k):
@@ -463,6 +453,16 @@ def topk_of_dense(dense, k):
     docs[:len(d)] = d
     scores[:len(s)] = s
     return docs, scores
+
+
+def dump_outputs(out_dir, **arrays):
+    """What the timed path handed its caller in its last step, as <name>.npy: the global top-k doc ids
+    (float64, exact for uint32; NO_DOC = 4294967295 pads a short list) and their float32 scores."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32 if a.dtype == np.float32 else np.float64))
+    log(f"outputs of the last timed step written to {out_dir}: {', '.join(arrays)}")
 
 
 def bench_ours(args, rank, world):
@@ -498,6 +498,8 @@ def bench_ours(args, rank, world):
     launches_value = int(o.stats().total_launches)
     o.download(out_docs, out_scores)
     value = args.steps * Q / (dev_ms / 1e3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, topk_docs=out_docs, topk_scores=out_scores)
     dbg("device-timed steps done")
 
     # ---- e2e: host buffers in, top-k out, every step
@@ -542,10 +544,9 @@ def bench_ours(args, rank, world):
     launches_per_step = st.term_kernel_launches / prof_steps
     achieved = float(alg_q.sum()) / (term_ms / 1e3) / 1e9
     peak, peak_src = peak_hbm()
-    traffic, traffic_src = committed_traffic("term_tile_kernel", {"n_docs": args.docs, "queries_per_step": Q, "n_gpus": world})
     roofline = {"bound": "hbm", "kernel": "term_tile_kernel", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
-                "frac_of_nominal_8TBs": achieved / 8000.0,      # SURVEY 8d: both denominators
+                "frac": achieved / peak, "peak_source": peak_src,
+                "frac_of_nominal_3_35TBs": achieved / NOMINAL_HBM_GBS,      # SURVEY 8d: both denominators
                 "algorithmic_bytes_per_launch": float(alg_q.sum()) / launches_per_step,
                 "algorithmic_bytes": "postings + 4*df (norms) + 4*N (dense row) per query (SURVEY 8d), summed over the "
                                      "launch's queries; postings = 4*df for lists scanned through the upload-time "
@@ -626,7 +627,7 @@ def bench_ours(args, rank, world):
             o.upload(p_terms, p_starts, p_idf, slop, k); o.execute(); p_redo += o.download(p_docs, p_scores)
         dbg("  warm-up done, repairs", p_redo)
         o.upload(p_terms, p_starts, p_idf, slop, k)
-        p_steps = max(2, args.steps)
+        p_steps = args.steps
         p_ms = o.timed_executes(p_steps)
         dbg("  timed done")
         _lib.check(L.sa_stats_reset(h))
@@ -650,11 +651,8 @@ def bench_ours(args, rank, world):
             stp = o.profiled(min(p_steps, 3))
             k_ms = stp.phrase_kernel_ms / min(p_steps, 3)
             alg = 8.0 * float(Wp.sum()) + 16.0 * st1.phrase_cont_words + 4.0 * host.n_docs * PQ + 4.0 * st1.phrase_matched_docs
-            tr, tr_src = committed_traffic("phrase_kernel", {"n_docs": args.docs, "queries_per_step": PQ, "n_gpus": world,
-                                                            "workload": label})
             blk["roofline"] = {"bound": "hbm", "kernel": "phrase kernels (slop 0)", "achieved": alg / (k_ms / 1e3) / 1e9,
                                "peak": peak, "unit": "GB/s", "frac": alg / (k_ms / 1e3) / 1e9 / peak,
-                               "traffic": tr, "traffic_source": tr_src,
                                "algorithmic_bytes": "B_phrase = 8*sum(W) + 16*sum(C_s) + 4*N + 4*M (SURVEY 8d)",
                                "algorithmic_bytes_per_step": alg, "sum_W_words": float(Wp.sum()),
                                "sum_C_words": int(st1.phrase_cont_words), "matched_docs": int(st1.phrase_matched_docs),
@@ -907,7 +905,11 @@ def main():
                          "(default 48 at 1 GPU, 16 sharded -- rank 0 then re-generates the FULL corpus; 0 = off)")
     ap.add_argument("--verify-phrases", type=int, default=12)
     ap.add_argument("--verify-edismax", type=int, default=2)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the top-k doc ids and scores of the last step to DIR/*.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if args.impl == "reference":

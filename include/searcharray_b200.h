@@ -1,5 +1,5 @@
 /*
- * searcharray_b200.h -- C ABI of libsearcharray_b200.so (sm_100a CUDA kernels).
+ * searcharray_b200.h -- C ABI of libsearcharray_b200.so (sm_90a CUDA kernels, H100).
  *
  * Drop-in boundary for SearchArray's scoring hot path (SURVEY.md section 8b).  The
  * reference (softwaredoug/searcharray, paths below relative to its repo root) has no C

@@ -1,4 +1,4 @@
-"""searcharray_b200 -- SearchArray's scoring hot path on NVIDIA B200 (sm_100a).
+"""searcharray_b200 -- SearchArray's scoring hot path on NVIDIA H100 (sm_90a).
 
 Term-at-a-time BM25 over roaringish posting words and the positional phrase / slop matcher as
 hand-written CUDA kernels behind the reference's SearchArray.index / .score / .termfreqs

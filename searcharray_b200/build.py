@@ -1,4 +1,4 @@
-"""Builds libsearcharray_b200.so in-tree with nvcc for sm_100a (no GPU needed to compile)."""
+"""Builds libsearcharray_b200.so in-tree with nvcc for sm_90a (H100; no GPU needed to compile)."""
 import os
 import subprocess
 import sys
@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsearcharray_b200.so")
 SOURCES = ["sa_index.cu", "sa_term.cu", "sa_topk.cu", "sa_phrase.cu", "sa_span.cu", "sa_filter.cu", "sa_edismax.cu", "sa_similarity.cu", "sa_comm.cu", "sa_setops.cu", "sa_build.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-fmad=false"]
 
 

@@ -1,4 +1,4 @@
-// sa_common.cuh -- shared definitions for libsearcharray_b200 (sm_100a).
+// sa_common.cuh -- shared definitions for libsearcharray_b200 (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -24,7 +24,7 @@ typedef int64_t i64;
 #define SA_BIT17 (1ull << 17)
 #define SA_ONE_BLOCK (1ull << SA_LSB_BITS)
 
-#define SA_NUM_SMS_FALLBACK 148
+#define SA_NUM_SMS_FALLBACK 132          // H100 SXM
 
 // ---- error plumbing -------------------------------------------------------------
 void sa_set_error(const char *fmt, ...);

@@ -1341,8 +1341,8 @@ int sa_phrase_enqueue(sa_index *ix, const PhraseQuery *d_pqs, PhraseStats *d_sta
         ix->stats.total_launches++;
         return SA_OK;
     }
-    // the same regime as persistent CTAs with a double-buffered TMA pipeline (kept for comparison: measured slower,
-    // profiles/README.md): SA_PHRASE_TMA_PIPELINE=1
+    // the same regime as persistent CTAs with a double-buffered TMA pipeline (kept for comparison; not the
+    // default): SA_PHRASE_TMA_PIPELINE=1
     const u32 stage_words = sa_phrase_stage_words();
     u32 ctas = 0;
     if ((rc = staged_grid(ix, stage_words, &ctas))) return rc;

@@ -5,7 +5,7 @@
 //   as_dense/scatter    searcharray/roaringish/roaringish_ops.pyx:84-98, scatter_assign.h:8-29
 //   bm25_score          searcharray/bm25/bm25.pyx:11-41
 //
-// Design (B200).  The dense float32[N] score vector is cut into tiles of SA_TILE_DOCS docs; one
+// Design.  The dense float32[N] score vector is cut into tiles of SA_TILE_DOCS docs; one
 // CTA owns one (query, tile) and builds the tile in 32 KB of shared memory:
 //   1. the slice [lo,hi) of the term's posting words whose docs fall in the tile comes from the
 //      term's tile directory (two loads; built at upload for long lists) or, for short lists,
@@ -24,11 +24,10 @@
 // The grid is (queries, tiles) -- the query index runs fastest -- so that the CTAs resident on an
 // SM at any time belong to MANY queries: dense terms (issue-bound CTAs) and sparse terms
 // (store-bound CTAs) overlap, and a tile's norm sectors are shared in L2 by all queries.  With the
-// tiles of one query back to back the same kernel was 17 % slower (profiles/README.md).
+// tiles of one query back to back the same kernel was slower.
 // HBM traffic: 8*W (words) + the 32 B sectors holding the 4*df norms + 4*N (scores), less whatever
-// the queries of one launch share in L2.  History (profiles/): v1 evaluated BM25 for all 16 docs of
-// every thread under divergence with shared-memory atomics and was instruction-bound at 21 % of
-// the HBM roofline; variants that staged the postings with TMA bulk copies (cp.async.bulk +
+// the queries of one launch share in L2.  Evaluating BM25 for all 16 docs of every thread under
+// divergence with shared-memory atomics was instruction-bound; variants that staged the postings with TMA bulk copies (cp.async.bulk +
 // mbarrier), wrote zeros straight to HBM for sparse tiles, or pinned the norm table in L2 measured
 // slower and were dropped.
 #include <algorithm>

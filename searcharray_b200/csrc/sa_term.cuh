@@ -5,6 +5,7 @@
 #define SA_TILE_DOCS 8192          // docs per CTA tile (32 KB of float32 scores)
 #define SA_TERM_UNROLL 4           // 30-word windows loaded per warp before processing
 #define SA_TERM_THREADS 256
+// The three tf-table knobs below were swept on H100 (DESIGN.md §3.1); these values were the fastest on the bench mix.
 #define SA_STAGED_NORM_MIN_WORDS 1024   // tiles with at least this many posting words stage the tile's norms (sa_term.cu)
 #define SA_STAGED_NORM_MIN_RECS 48      // ... or this many (doc, tf) records on the tf-table path
 #define SA_TERM_PREFETCH_TILES 8         // L2 prefetch distance of the tf-table path, in tiles (sa_term.cu)

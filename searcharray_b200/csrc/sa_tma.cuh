@@ -1,4 +1,4 @@
-// sa_tma.cuh -- 1-D bulk asynchronous copies (TMA, cp.async.bulk) + mbarrier helpers for sm_100a.
+// sa_tma.cuh -- 1-D bulk asynchronous copies (TMA, cp.async.bulk) + mbarrier helpers (sm_90a: Hopper TMA).
 //
 // Posting blocks are plain contiguous uint64 runs, so the 1-D bulk form of the Tensor Memory
 // Accelerator is all that is needed: one elected thread arms an mbarrier with the byte count and

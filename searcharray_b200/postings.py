@@ -1,4 +1,4 @@
-"""SearchArray -- the reference's search surface, backed by the B200 kernels.
+"""SearchArray -- the reference's search surface, backed by the CUDA kernels.
 
 Mirrors the Search API of reference searcharray/postings.py (`SearchArray.index` :249-300,
 `termfreqs` :607-638, `docfreq` :640-647, `doclengths` :649-650, `score` :652-680,

@@ -1,12 +1,16 @@
-"""The oracle port (oracle/search.py + oracle/sa_oracle.c) against the REAL reference built into
-oracle/_ref (oracle/build_ref.py) on the seeded synthetic corpus -- the same index object both arms of
-bench.py run on.  Skips where oracle/_ref was never built (it needs /root/reference to build)."""
+"""The oracle port (oracle/search.py + oracle/sa_oracle.c) against the REAL reference on the seeded synthetic
+corpus -- the same index object both arms of bench.py run on.  What the reference returned on it is stored as
+whole-vector SHA-256 digests in tests/golden/ref_synth.json (tests/golden/make_golden_ref_outputs.py)."""
+import hashlib
+import json
+import os
+
 import numpy as np
 import pytest
 
-from oracle import ref_runner
+from conftest import GOLDEN
 
-pytestmark = pytest.mark.skipif(not ref_runner.available(), reason="oracle/_ref not built (python oracle/build_ref.py)")
+G = json.load(open(os.path.join(GOLDEN, "ref_synth.json")))
 
 
 @pytest.fixture(scope="module")
@@ -16,41 +20,42 @@ def corpus():
     spec = synth.SynthSpec(300_000, terms_per_bucket=5, n_phrases=16, n_bigrams=4)
     host, _, _ = synth.generate_shard(spec)
     avgdl = synth.global_avg_doc_length(spec)
-    arr = ref_runner.reference_array(host, avg_doc_length=avgdl)
     oidx = osearch.OracleIndex({t: host.term_words(t) for t in range(host.n_terms)}, host.doc_lens,
                                avg_doc_length=avgdl, corpus_size=host.n_docs, cache=True)
-    return spec, host, arr, oidx
+    return spec, host, oidx
 
 
-def same_bits(a, b):
-    a, b = np.asarray(a), np.asarray(b)
-    return a.dtype == b.dtype and a.shape == b.shape and np.array_equal(a.view(np.uint32), b.view(np.uint32))
+def sha(a):
+    a = np.asarray(a)
+    assert a.dtype == np.float32
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
 
 
 def test_terms_match_the_reference(corpus):
-    spec, host, arr, oidx = corpus
-    sim = ref_runner.bm25(1.2, 0.75)
+    spec, host, oidx = corpus
+    assert sorted(G["terms"]) == sorted(name for name, _, _ in spec.terms)
     for t, (name, _, _) in enumerate(spec.terms):
-        assert int(arr.docfreq(name)) == int(oidx.docfreq(t))
-        assert same_bits(arr.termfreqs(name), oidx.termfreqs(t)), name
-        assert same_bits(arr.score(name, similarity=sim), oidx.score(t, k1=1.2, b=0.75)), name
-    assert same_bits(arr.score("nope"), oidx.score(None))
+        want = G["terms"][name]
+        assert int(oidx.docfreq(t)) == want["df"], name
+        assert sha(oidx.termfreqs(t)) == want["tf"], name
+        assert sha(oidx.score(t, k1=1.2, b=0.75)) == want["score"], name
+    assert sha(oidx.score(None)) == G["missing_score"]
 
 
 def test_phrases_and_slop_match_the_reference(corpus):
-    spec, host, arr, oidx = corpus
-    sim = ref_runner.bm25(1.2, 0.75)
+    spec, host, oidx = corpus
     n_match = 0
-    for ph in spec.phrases:
+    assert [ph["terms"] for ph in spec.phrases] == [w["terms"] for w in G["phrases"]]
+    for ph, want in zip(spec.phrases, G["phrases"]):
         ids = [spec.term_index[t] for t in ph["terms"]]
-        want = arr.termfreqs(ph["terms"])
-        assert same_bits(want, oidx.termfreqs(ids)), ph
-        assert same_bits(arr.score(ph["terms"], similarity=sim), oidx.score(ids, k1=1.2, b=0.75)), ph
-        n_match += int(np.count_nonzero(want))
+        got = oidx.termfreqs(ids)
+        assert sha(got) == want["tf"], ph
+        assert sha(oidx.score(ids, k1=1.2, b=0.75)) == want["score"], ph
+        n_match += int(np.count_nonzero(got))
     assert n_match > 0
     from oracle import ops as oops
-    for ph in spec.phrases[::3]:
+    for ph, want in zip(spec.phrases[::3], G["slop2"]):
         ids = [spec.term_index[t] for t in ph["terms"]]
         got = oidx.termfreqs(ids, slop=2)
         if not oops.last_span_undefined:
-            assert same_bits(arr.termfreqs(ph["terms"], slop=2), got), ph
+            assert sha(got) == want["tf"], ph

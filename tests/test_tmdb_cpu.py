@@ -1,8 +1,9 @@
 """BASELINE configs[0]: the TMDB fixture (27,846 real documents) -- the host indexer and the CPU
 oracle against what the REAL reference produced on it (tests/golden/tmdb.json: digests, counts and
-top-10 lists; made by tests/golden/make_golden_tmdb.py).  The corpus stays in the reference tree, so
-these tests run where /root/reference exists (the build container) and skip elsewhere."""
-import gzip
+top-10 lists; made by tests/golden/make_golden_tmdb.py).  The corpus enters as the stored index of both
+fields (tests/golden/tmdb_index.npz, the same file the GPU tests upload), which is first checked against
+the reference's own index digest.  The indexer is checked by re-indexing the token streams that index
+holds (every token of every document at its position, joined by single spaces)."""
 import hashlib
 import json
 import os
@@ -10,10 +11,8 @@ import os
 import numpy as np
 import pytest
 
+from _tmdb_index import load_field
 from conftest import GOLDEN
-
-FIXTURE = "/root/reference/fixtures/tmdb.json.gz"
-pytestmark = pytest.mark.skipif(not os.path.exists(FIXTURE), reason="TMDB fixture lives in the reference tree")
 
 G = json.load(open(os.path.join(GOLDEN, "tmdb.json")))
 
@@ -22,17 +21,51 @@ def sha(a):
     return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
 
 
+def index_digest(host):
+    """The reference's canonical digest (make_golden_tmdb.index_digest) of a HostIndex."""
+    h = hashlib.sha256()
+    t2i = host.term_dict.term_to_ids
+    for t in sorted(t2i.keys()):
+        h.update(t.encode("utf-8"))
+        h.update(np.ascontiguousarray(host.term_words(t2i[t]), dtype=np.uint64).tobytes())
+    return {"n_terms": host.n_terms, "n_words": len(host.words), "sha256": h.hexdigest(),
+            "doc_lens_sha256": sha(host.doc_lens.astype(np.float32)), "avg_doc_length": float(host.avg_doc_length)}
+
+
+def token_streams(host):
+    """Each document's tokens in position order, decoded from the roaringish words
+    (doc id << 36 | position block << 18 | one bit per position in the block)."""
+    from searcharray_b200.roaringish import LSB_BITS
+    words = host.words.astype(np.uint64)
+    order = np.argsort(host.term_offsets, kind="stable")
+    term_of_word = np.repeat(order, host.term_lengths[order].astype(np.int64))
+    assert len(term_of_word) == len(words)
+    doc = (words >> np.uint64(36)).astype(np.int64)
+    base = ((words >> np.uint64(LSB_BITS)) & np.uint64(0x3FFFF)).astype(np.int64) * LSB_BITS
+    d, p, t = [], [], []
+    for bit in range(LSB_BITS):
+        on = ((words >> np.uint64(bit)) & np.uint64(1)).astype(bool)
+        d.append(doc[on]); p.append(base[on] + bit); t.append(term_of_word[on])
+    d, p, t = np.concatenate(d), np.concatenate(p), np.concatenate(t)
+    srt = np.lexsort((p, d))
+    d, p, t = d[srt], p[srt], t[srt]
+    names = [host.term_dict.get_term(i) for i in range(host.n_terms)]
+    counts = np.bincount(d, minlength=host.n_docs)
+    assert np.array_equal(counts, host.doc_lens.astype(np.int64))
+    starts = np.concatenate(([0], np.cumsum(counts)))
+    assert np.array_equal(p, np.arange(len(p)) - np.repeat(starts[:-1], counts))   # positions 0..len-1
+    return [" ".join(names[i] for i in t[starts[k]:starts[k + 1]]) for k in range(host.n_docs)]
+
+
 @pytest.fixture(scope="module")
 def fields():
     from oracle import search as osearch, solr as osolr
-    from searcharray_b200.indexing import build_index
-    with gzip.open(FIXTURE) as f:
-        raw = json.load(f)
-    titles = [(raw[k].get("title", "") or "") for k in raw.keys()]
-    overviews = [(raw[k].get("overview", "") or "") for k in raw.keys()]
+    z = np.load(os.path.join(GOLDEN, "tmdb_index.npz"))
     out = {}
-    for name, docs in (("title_tokens", titles), ("overview_tokens", overviews)):
-        host = build_index(docs, str.split)
+    for name in ("title_tokens", "overview_tokens"):
+        host = load_field(z, name)
+        assert index_digest(host) == G["fields"][name]["index"], name      # the reference's index, word for word
+        assert host.n_docs == G["n_docs"]
         idx = osearch.OracleIndex({t: host.term_words(t) for t in range(host.n_terms)}, host.doc_lens,
                                   avg_doc_length=host.avg_doc_length)
         out[name] = (host, osolr.OracleField(idx, host.term_dict.term_to_ids))
@@ -51,18 +84,11 @@ def check_vec(got, rec, what):
 
 @pytest.mark.parametrize("field", ["title_tokens", "overview_tokens"])
 def test_host_indexer_matches_reference_index(fields, field):
-    """searcharray_b200.indexing.build_index on real text == the reference's index, word for word."""
-    host, _ = fields[field]
-    want = G["fields"][field]["index"]
-    h = hashlib.sha256()
-    t2i = host.term_dict.term_to_ids
-    for t in sorted(t2i.keys()):
-        h.update(t.encode("utf-8"))
-        h.update(np.ascontiguousarray(host.term_words(t2i[t]), dtype=np.uint64).tobytes())
-    assert (host.n_terms, len(host.words)) == (want["n_terms"], want["n_words"])
-    assert h.hexdigest() == want["sha256"]
-    assert sha(host.doc_lens.astype(np.float32)) == want["doc_lens_sha256"]
-    assert float(host.avg_doc_length) == want["avg_doc_length"]
+    """searcharray_b200.indexing.build_index on the corpus's token streams == the reference's index, word for word."""
+    from searcharray_b200.indexing import build_index
+    stored, _ = fields[field]
+    host = build_index(token_streams(stored), str.split)
+    assert index_digest(host) == G["fields"][field]["index"]
     assert host.n_docs == G["n_docs"]
 
 

@@ -1,4 +1,4 @@
-// bw_probe.cu -- what HBM bandwidth does a write-dominated stream reach on this B200?
+// bw_probe.cu -- what HBM bandwidth does a write-dominated stream reach on this H100?
 // (fill / copy / 70-30 mix), to put the term kernel's 4N-write-dominated traffic in context.
 #include <cstdio>
 #include <cuda_runtime.h>
@@ -36,7 +36,7 @@ int main() {
             float ms; cudaEventElapsedTime(&ms, e0, e1); if (ms < best) best = ms; }
         printf("%-28s %8.3f ms  %8.1f GB/s\n", name, best, bytes / best / 1e6);
     };
-    for (int blocks : {148 * 8, 148 * 16, 148 * 64}) {
+    for (int blocks : {132 * 8, 132 * 16, 132 * 64}) {
         printf("grid %d x 256\n", blocks);
         time("fill (st.cs)", [&] { fill<<<blocks, 256>>>(b, n); }, n * 16.0);
         time("fill (plain st)", [&] { fill_plain<<<blocks, 256>>>(b, n); }, n * 16.0);
