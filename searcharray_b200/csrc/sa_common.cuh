@@ -127,7 +127,6 @@ struct sa_index {
     u32 *d_recs = nullptr;
     u32 *d_rec_dir = nullptr;
     std::vector<u64> h_rec_off;
-    std::vector<u32> h_max_tile_words;   // per term: the longest per-tile slice of its list (its length without a directory)
     // per-doc BM25 length norm k1*((1-b)+b*dl/avgdl) for the last used (k1, b, avgdl)
     float *d_norm = nullptr;         // [padded n_docs]
     float norm_k1 = 0, norm_b = 0, norm_avgdl = 0;
@@ -159,7 +158,6 @@ struct sa_index {
     DevBuf cand_meta;    // per-query counters / thresholds
     DevBuf topk_out;     // per-query (doc, score) results
     DevBuf phrase_scratch;
-    DevBuf phrase_slabs;  // per-CTA scratch of the persistent phrase kernel (merge regime)
     DevBuf filt;         // filtered (sliced / position-filtered) copies of posting lists
     DevBuf misc;
     void *h_pinned = nullptr;   // pinned staging

@@ -485,7 +485,7 @@ extern "C" int sa_multi_phrases(sa_multi *m, uint32_t field, uint32_t n_phrases,
     }
     PhraseDump nodump;
     memset(&nodump, 0, sizeof(nodump));
-    return sa_phrase_run_sync(ix, pqs, ix->filt.as<u64>(), 1, p, 0, nodump, 0);
+    return sa_phrase_run_sync(ix, pqs, ix->filt.as<u64>(), 1, p, 0, nodump, false);
 }
 
 extern "C" int sa_multi_add_phase(sa_multi *m, uint32_t n_entries, const uint32_t *entry_field,

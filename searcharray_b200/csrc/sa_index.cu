@@ -161,18 +161,6 @@ __global__ void tile_dir_kernel(const u64 *__restrict__ words, u64 n_words,
         for (u32 t = t_i + 1; t <= n_tiles; t++) d[t] = (u32)len;
 }
 
-// longest per-tile slice of every list that has a directory (sizes the merge regime's per-CTA scratch)
-__global__ void dir_max_kernel(const u32 *__restrict__ dir, const u64 *__restrict__ slot_dir_off, u32 n_slots, u32 n_tiles,
-                               u32 *__restrict__ slot_max) {
-    const u32 slot = blockIdx.x;                 // (terms can outnumber the 65,535 limit of grid.y)
-    if (slot >= n_slots || slot_dir_off[slot] == SA_NO_DIR) return;
-    const u32 *d = dir + slot_dir_off[slot];
-    u32 m = 0;
-    for (u32 t = blockIdx.y * blockDim.x + threadIdx.x; t < n_tiles; t += gridDim.y * blockDim.x) m = max(m, d[t + 1] - d[t]);
-    m = __reduce_max_sync(0xffffffffu, m);
-    if ((threadIdx.x & 31) == 0 && m) atomicMax(&slot_max[slot], m);
-}
-
 // ---- tf table (see sa_index::d_recs).  Pass 1 counts the doc heads of every 1024-word block, a one-CTA scan
 // turns the counts into ranks, pass 2 writes each head's record at (term's record offset + rank within the
 // term) and fills the term's record directory like tile_dir_kernel fills the word directory.
@@ -324,7 +312,6 @@ extern "C" int sa_index_create(const uint64_t *words, uint64_t n_words,
     ix->h_df.assign(n_terms, 0);
     ix->h_dir_off.assign(n_terms, SA_NO_DIR);
     ix->h_first0.assign(n_terms, 0);
-    ix->h_max_tile_words.assign(n_terms, 0);
     ix->h_rec_off.assign(n_terms, SA_NO_DIR);
     for (u32 t = 0; t < n_terms; t++)
         if (term_lengths[t] && (words[term_offsets[t]] & SA_HDR_MASK) == 0) ix->h_first0[t] = 1;
@@ -420,25 +407,7 @@ extern "C" int sa_index_create(const uint64_t *words, uint64_t n_words,
             CREATE_CUDA(cudaGetLastError());
             ix->stats.total_launches++;
         }
-        ix->h_max_tile_words.assign(n_terms, 0);
-        for (u32 t = 0; t < n_terms; t++) ix->h_max_tile_words[t] = (u32)std::min<u64>(term_lengths[t], 0xFFFFFFFFull);
-        std::vector<u32> slot_max(n_slots, 0);
-        u32 *d_slot_max = nullptr;
-        if (dir_words) {
-            CREATE_CUDA(cudaMalloc(&d_slot_max, n_slots * sizeof(u32)));
-            CREATE_CUDA(cudaMemsetAsync(d_slot_max, 0, n_slots * sizeof(u32), ix->stream));
-            dir_max_kernel<<<dim3(n_slots, std::min<u32>(32, (n_tiles + 255) / 256)), 256, 0, ix->stream>>>(
-                ix->d_tile_dir, d_slot_dir, n_slots, n_tiles, d_slot_max);
-            CREATE_CUDA(cudaGetLastError());
-            ix->stats.total_launches++;
-            CREATE_CUDA(cudaMemcpyAsync(slot_max.data(), d_slot_max, n_slots * sizeof(u32), cudaMemcpyDeviceToHost, ix->stream));
-        }
         CREATE_CUDA(cudaStreamSynchronize(ix->stream));         // h_df is final from here on
-        if (dir_words) {
-            for (u32 sI = 0; sI < n_slots; sI++)
-                if (slot_dir[sI] != SA_NO_DIR) ix->h_max_tile_words[term_of_slot[sI]] = slot_max[sI];
-            cudaFree(d_slot_max);
-        }
         // tf table for the terms that have a directory (the long lists: that is where the scan's time goes)
         static const bool no_tf_table = getenv("SA_NO_TF_TABLE") && atoi(getenv("SA_NO_TF_TABLE")) != 0;
         ix->h_rec_off.assign(n_terms, SA_NO_DIR);
@@ -516,7 +485,6 @@ extern "C" int sa_index_destroy(sa_index *ix) {
     ix->cand_meta.release();
     ix->topk_out.release();
     ix->phrase_scratch.release();
-    ix->phrase_slabs.release();
     ix->filt.release();
     ix->misc.release();
     ix->gather.release();
@@ -696,9 +664,8 @@ struct BatchChunk {
     Bm25Params params;
     u32 phrase_chunks = 1;          // doc-range chunks per phrase query
     u64 arena_words = 64;
-    // phrase queries by regime (indices relative to phrase0, stored at B.d_sel + sel0: search first, then staged)
-    u32 sel0 = 0, n_search = 0, n_staged = 0, staged_chunks = 1;
-    u64 slab_cap = 0;
+    // phrase queries by regime (indices relative to phrase0, stored at B.d_sel + sel0: search first, then conjunction)
+    u32 sel0 = 0, n_search = 0, n_conj = 0;
 };
 
 struct BatchState {
@@ -718,7 +685,7 @@ struct BatchState {
     DevBuf d_tq, d_pq, d_row_query;
     DevBuf d_meta;                            // u32 overflow[nq] (row space)
     DevBuf d_pstats;                          // PhraseStats[#phrase queries]
-    std::vector<u32> sel;                     // per chunk: search-regime then merge-regime phrase indices
+    std::vector<u32> sel;                     // per chunk: search-regime then conjunction-regime phrase indices
     DevBuf d_sel;
     DevBuf d_missing;                         // phrase_missing on the device (batch_summary_kernel)
 };
@@ -855,10 +822,7 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
                     else for (u32 i = 0; i < nt; i++)
                         if (ix->h_dir_off[tids[i]] != SA_NO_DIR) pq.dir_plus1[i] = ix->h_dir_off[tids[i]] + 1;
                     sa_phrase_plan(pq, tids);
-                    if (!missing && sa_phrase_is_staged(pq, ix->n_docs)) {
-                        pq.pad = 1;                                               // merge regime (see below)
-                        C.slab_cap = std::max(C.slab_cap, sa_phrase_slab_cap(ix, tids, nt));
-                    }
+                    pq.use_conj = !missing && sa_phrase_use_conjunction(pq, ix->n_docs);
                     B.pqs.push_back(pq);
                     B.phrase_query.push_back(q);
                     B.phrase_missing.push_back(missing);
@@ -878,15 +842,14 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
         C.n_phrase = (u32)B.pqs.size() - C.phrase0;
         if (C.n_phrase) {
             C.sel0 = (u32)B.sel.size();
-            for (u32 i = 0; i < C.n_phrase; i++) if (!B.pqs[C.phrase0 + i].pad) B.sel.push_back(i);
+            for (u32 i = 0; i < C.n_phrase; i++) if (!B.pqs[C.phrase0 + i].use_conj) B.sel.push_back(i);
             C.n_search = (u32)B.sel.size() - C.sel0;
-            for (u32 i = 0; i < C.n_phrase; i++) if (B.pqs[C.phrase0 + i].pad) B.sel.push_back(i);
-            C.n_staged = C.n_phrase - C.n_search;
-            C.staged_chunks = sa_phrase_staged_chunks(ix);
+            for (u32 i = 0; i < C.n_phrase; i++) if (B.pqs[C.phrase0 + i].use_conj) B.sel.push_back(i);
+            C.n_conj = C.n_phrase - C.n_search;
             u64 want = std::max<u64>(1, (u64)ix->num_sms * 16 / std::max<u32>(C.n_search, 1));
             C.phrase_chunks = sa_phrase_chunks(ix, (u32)std::max<u64>(1, std::min<u64>(want, std::max<u64>(1, ix->n_docs / 512))));
             for (u32 i = 0; i < C.n_phrase; i++)                     // only the search regime bump-allocates
-                if (!B.pqs[C.phrase0 + i].pad) C.arena_words += sa_phrase_arena_words(B.pqs[C.phrase0 + i], C.phrase_chunks);
+                if (!B.pqs[C.phrase0 + i].use_conj) C.arena_words += sa_phrase_arena_words(B.pqs[C.phrase0 + i], C.phrase_chunks);
             max_arena = std::max(max_arena, C.arena_words);
         }
         B.chunks.push_back(C);
@@ -1017,10 +980,8 @@ int sa_batch_execute_locked(sa_index *ix) {
             PhraseSplit sp;
             sp.d_search = B.d_sel.as<u32>() + C.sel0;
             sp.n_search = C.n_search;
-            sp.d_staged = sp.d_search + C.n_search;
-            sp.n_staged = C.n_staged;
-            sp.staged_chunks = C.staged_chunks;
-            sp.slab_cap = C.slab_cap;
+            sp.d_conj = sp.d_search + C.n_search;
+            sp.n_conj = C.n_conj;
             if ((rc = sa_phrase_enqueue(ix, B.d_pq.as<PhraseQuery>() + C.phrase0, B.d_pstats.as<PhraseStats>() + C.phrase0,
                                         C.n_phrase, rows, stride, C.phrase_chunks, (u64 *)ix->phrase_scratch.p + 8,
                                         d_used, C.arena_words, 1, C.params, &t, C.n_term, &sp))) return rc;
@@ -1057,7 +1018,7 @@ static int redo_query(sa_index *ix, BatchState &B, bool is_phrase, u32 idx, u32 
         std::vector<PhraseQuery> one(1, B.pqs[idx]);
         PhraseDump nodump;
         memset(&nodump, 0, sizeof(nodump));
-        if ((rc = sa_phrase_run_sync(ix, one, ix->d_words, 1, p, 0, nodump, 0))) return rc;   // loops until the guess holds
+        if ((rc = sa_phrase_run_sync(ix, one, ix->d_words, 1, p, 0, nodump, false))) return rc;   // loops until the guess holds
         B.pqs[idx] = one[0];
         if ((rc = launch_dense_topk_tiles(ix, ix->dense.as<float>(), stride, 0, 1, t, nullptr))) return rc;
     }

@@ -28,14 +28,13 @@
 #include "sa_phrase.cuh"
 #include "sa_span.cuh"
 #include "sa_term.cuh"
-#include "sa_tma.cuh"
 
 int sa_filter_terms(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, bool use_rows,
                     u64 pay_lo, u64 pay_hi, bool use_payload, std::vector<u64> &offs, std::vector<u64> &lens);
 int sa_gather_rows(sa_index *ix, const float *d_dense, float *out_host);
 
 #define PT SA_PHRASE_THREADS
-#define PW_SUB_DOCS (SA_TILE_DOCS / (SA_PHRASE_THREADS / 32))   // docs of a tile that one warp of the merge regime owns (1,024)
+#define PW_SUB_DOCS (SA_TILE_DOCS / (SA_PHRASE_THREADS / 32))   // docs of a tile that one warp of the conjunction regime owns (1,024)
 
 static u64 docs_per_chunk_of(const sa_index *ix, u32 n_chunks);
 
@@ -534,315 +533,6 @@ phrase_kernel(const PhraseArgs a) {
     }
 }
 
-
-// ---------------------------------------------------------------------------------------------------------------
-// The MERGE regime (balanced lists; chosen per query by the host, sa_phrase_is_staged): persistent CTAs, each claiming
-// (query, 16-tile chunk) work items.  A work item is cut into SEGMENTS of whole tiles whose posting slices fit in one
-// half of the CTA's staging buffer.  Warp 0 plans a segment from the chunk's tile-directory entries (preloaded into
-// shared memory) and its lane 0 arms an mbarrier and issues one TMA bulk copy per term
-// (cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes); the NEXT segment is planned and issued into
-// the other half before the current one is consumed, so the copy engine streams every list from HBM exactly once,
-// sequentially, while the SM works (double buffering).  Per tile:
-//   1. a doc can only match if it holds EVERY term, so each term's slice sets bits in a doc-presence bitmap
-//      (shared-memory atomicOr) and the bitmaps are ANDed.  Conjunctions of common terms are rare (df/N of .3, .1,
-//      .03, .01: 9e-6 of the docs), so almost every tile ends here and is written as zeros;
-//   2. otherwise each of the eight warps takes 1,024 docs of the tile: it compacts the candidate docs' words of
-//      every term in order (ballots) and runs the whole bigram chain on them at warp scope (sa_phrase_warp.cuh);
-//   3. the tile is materialised (zeros + BM25-scored matches) and its top-k candidates collected.
-// The pair statistics of the same-term speculation cover the candidate docs only -- enough to CONFIRM a guess, not
-// to derive the reference's global decision from; any disagreement re-runs the query in the search regime
-// (sa_phrase_run_sync / redo_query), which keeps the result exact.
-#define PS_MAX_CHUNK_TILES 32
-
-struct SegPlan {                                   // one per staging-buffer half
-    u32 te, any;
-    u32 n[SA_MAX_PHRASE_TERMS];                    // words of each term in the segment
-    u32 dir0[SA_MAX_PHRASE_TERMS];                 // directory entry of the segment's first tile (tile slices by subtraction)
-    const u64 *ptr[SA_MAX_PHRASE_TERMS];           // where the segment's slice is read from (staged copy, or global)
-};
-
-struct StagedShared {
-    u32 dirs[SA_MAX_PHRASE_TERMS][PS_MAX_CHUNK_TILES + 1];   // tile-directory entries of the chunk's tile boundaries
-    u32 has_dir[SA_MAX_PHRASE_TERMS];
-    u64 c_lo[SA_MAX_PHRASE_TERMS], c_n[SA_MAX_PHRASE_TERMS];  // chunk slices (lists without a directory are searched)
-    SegPlan plan[2];
-    const u64 *sptr[PT / 32][SA_MAX_PHRASE_TERMS]; // every warp's chain inputs (compacted candidates, or plain sub-slices)
-    u32 sn[PT / 32][SA_MAX_PHRASE_TERMS];
-    u32 wmatch[2][PT / 32];                        // matches of every warp, alternating between consecutive tiles
-    u32 ncand, tile_max, work, ok;
-    u32 top[(PT / 32) * 8];
-    __align__(16) float tile[SA_TILE_DOCS];        // bitmaps / compaction buffers first, then the dense tile
-    __align__(8) u64 bar[2];
-};
-
-// warp 0 only: plan the segment that starts at tile `ts` and issue its copies into staging half `h`
-__device__ __forceinline__ void staged_plan(const PhraseArgs &a, const PhraseQuery &pq, StagedShared &P, u64 *stage_half,
-                                            u32 h, u32 ts, u32 tile0, u32 tile1, u64 dend) {
-    const unsigned lane = threadIdx.x & 31;
-    const u32 n_terms = pq.n_terms;
-    SegPlan &pl = P.plan[h];
-    const bool has = lane < n_terms;
-    const bool hd = has && P.has_dir[lane];
-    const u32 base = hd ? P.dirs[lane][ts - tile0] : 0u;
-    const u32 fixed = (has && !hd) ? (u32)min(P.c_n[lane], (u64)0x7FFFFFFFu) : 0u;
-    u32 best = ts + 1;
-    for (u32 cand = ts + 1; cand <= tile1; cand++) {
-        const u32 mine = has ? ((hd ? P.dirs[lane][cand - tile0] - base : fixed) + 4u) : 0u;     // + alignment slack
-        const u32 sum = __reduce_add_sync(0xffffffffu, mine);
-        if (cand > ts + 1 && sum > a.stage_words) break;
-        best = cand;
-        if (sum > a.stage_words) break;
-    }
-    const u32 te = best;
-    // every term's slice of the segment
-    u64 lo = 0;
-    u32 n = 0;
-    if (has) {
-        if (hd) {
-            lo = base;
-            n = P.dirs[lane][te - tile0] - base;
-        } else {                                   // short list without a directory: search its chunk slice
-            const u64 *lst = a.words + pq.off[lane] + P.c_lo[lane];
-            const u64 seg_d0 = a.doc_base + (u64)ts * SA_TILE_DOCS, seg_d1 = min(a.doc_base + (u64)te * SA_TILE_DOCS, dend);
-            u32 l2 = 0, h2 = (u32)P.c_n[lane];
-            while (l2 < h2) { const u32 m = (l2 + h2) >> 1; if ((lst[m] >> SA_KEY_SHIFT) < seg_d0) l2 = m + 1; else h2 = m; }
-            u32 l3 = l2, h3 = (u32)P.c_n[lane];
-            while (l3 < h3) { const u32 m = (l3 + h3) >> 1; if ((lst[m] >> SA_KEY_SHIFT) < seg_d1) l3 = m + 1; else h3 = m; }
-            lo = P.c_lo[lane] + l2;
-            n = l3 - l2;
-        }
-    }
-    // staging layout: terms in order while they fit (exclusive scan over the lanes)
-    const u64 *lst = has ? a.words + pq.off[lane] : nullptr;
-    const u32 wds = (has && n) ? sa_stage_bytes(lst, lo, n) / 8u : 0u;
-    u32 incl = wds;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const u32 t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= (unsigned)o) incl += t; }
-    const bool st = wds && incl <= a.stage_words;                 // (a term that does not fit is read from global memory)
-    const u32 so = incl - wds;
-    const u32 total = __reduce_add_sync(0xffffffffu, st ? wds * 8u : 0u);
-    if (lane == 0 && total) {
-        sa_fence_proxy_async();                                  // the half's previous readers are behind a barrier
-        sa_mbar_expect_tx(&P.bar[h], total);
-    }
-    __syncwarp();
-    if (has) {
-        pl.n[lane] = n;
-        pl.dir0[lane] = base;
-        if (st) {
-            const u32 head = sa_stage_issue(stage_half + so, lst, lo, n, &P.bar[h]);
-            pl.ptr[lane] = stage_half + so + head;
-        } else {
-            pl.ptr[lane] = lst + lo;
-        }
-    }
-    if (lane == 0) { pl.te = te; pl.any = total ? 1u : 0u; }
-    __syncwarp();
-}
-
-__device__ void phrase_work_staged(const PhraseArgs &a, const u32 q, const u32 chunk, StagedShared &P, u64 *stage,
-                                   u32 (&bar_phase)[2], u64 *cta_slab, const u64 cap) {
-    const PhraseQuery &pq = a.queries[q];
-    const u32 n_terms = pq.n_terms;
-    const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const u64 d0 = a.doc_base + (u64)chunk * a.docs_per_chunk;
-    const u64 dend = a.doc_base + a.n_docs;
-    if (d0 >= dend) return;
-    const u64 d1 = min(d0 + a.docs_per_chunk, dend);
-    const u32 tile0 = (u32)(((u64)chunk * a.docs_per_chunk) / SA_TILE_DOCS);
-    const u32 tile1 = (u32)((d1 - a.doc_base + SA_TILE_DOCS - 1) / SA_TILE_DOCS);
-    const u32 nt = tile1 - tile0;                                 // <= PS_MAX_CHUNK_TILES (host: sa_phrase_staged_chunks)
-    float *out = a.out + (u64)q * a.out_stride;
-    Bm25Params p = a.bm25;
-    p.idf = pq.idf;
-    const u32 row = a.topk_row0 + q;
-
-    // ---- the chunk's directory entries -> shared memory; chunk slices of the lists without a directory
-    __syncthreads();                                              // the previous work item is done with P
-    for (u32 idx = tid; idx < n_terms * (nt + 1); idx += PT) {
-        const u32 t = idx / (nt + 1), j = idx % (nt + 1);
-        const bool hd = pq.dir_plus1[t] && a.tile_dir;
-        P.dirs[t][j] = hd ? __ldg(a.tile_dir + (pq.dir_plus1[t] - 1) + tile0 + j) : 0u;
-        if (j == 0) P.has_dir[t] = hd ? 1u : 0u;
-    }
-    for (u32 t = warp; t < n_terms; t += PT / 32) {
-        if (pq.dir_plus1[t] && a.tile_dir) continue;
-        const u64 *lst = a.words + pq.off[t];
-        const u64 lo = warp_lower_bound_shifted(lst, 0, pq.len[t], d0, SA_KEY_SHIFT);
-        const u64 hi = warp_lower_bound_shifted(lst, lo, pq.len[t], d1, SA_KEY_SHIFT);
-        if (lane == 0) { P.c_lo[t] = lo; P.c_n[t] = hi - lo; }
-    }
-    if (tid == 0) P.ok = 1;
-    __syncthreads();
-    u32 widest = 0;
-    for (u32 t = 0; t < n_terms; t++) {
-        const u64 n = P.has_dir[t] ? (u64)(P.dirs[t][nt] - P.dirs[t][0]) : P.c_n[t];
-        if (n) widest++;
-        if (n + 2 > cap && !P.has_dir[t]) { if (tid == 0) { P.ok = 0; atomicExch(&a.stats[q].overflow, 1u); } }
-    }
-    const bool run = widest >= 2;                                 // fewer than two terms present: no pairs at any step
-
-    if (run && warp == 0) staged_plan(a, pq, P, stage, 0, tile0, tile0, tile1, dend);
-    __syncthreads();
-    const bool ok = P.ok != 0;
-
-    u32 ts = tile0, seg = 0, tile_no = 0;
-    while (ts < tile1) {
-        const u32 h = seg & 1u;
-        u32 te = tile1;
-        if (run) {
-            te = P.plan[h].te;
-            // prefetch: plan the next segment and issue its copies into the other half before consuming this one
-            if (te < tile1 && warp == 0) staged_plan(a, pq, P, stage + (u64)(h ^ 1u) * a.stage_words, h ^ 1u, te, tile0, tile1, dend);
-            if (P.plan[h].any) {
-                sa_mbar_wait(&P.bar[h], bar_phase[h]);
-                bar_phase[h] ^= 1u;
-            }
-        }
-        const SegPlan &pl = P.plan[h];
-        for (u32 tile = ts; tile < te; tile++, tile_no++) {
-            // ---- every warp takes 1,024 docs of the tile and works on them WITHOUT block barriers: sub-slice bounds
-            //      (lane-parallel binary searches), doc-presence bitmaps of the terms (one 32-bit word per lane), their
-            //      AND, ordered compaction of the candidate docs' words, the bigram chain, and its 4 KB of the dense tile.
-            //      The warp's scratch overlays its own slice of the tile.
-            const u64 td0 = a.doc_base + (u64)tile * SA_TILE_DOCS;
-            const u64 w_d0 = td0 + (u64)warp * PW_SUB_DOCS, w_d1 = w_d0 + PW_SUB_DOCS;
-            float *my_slice = P.tile + warp * PW_SUB_DOCS;
-            u32 *wbm = reinterpret_cast<u32 *>(my_slice);                       // [n_terms][32] presence bitmaps
-            u32 *wcand = wbm + n_terms * 32;                                    // [32] candidate docs
-            u64 *fbw = reinterpret_cast<u64 *>(wcand + 32);                     // compaction area
-            const u32 fb_cap = ((PW_SUB_DOCS * 4 - (n_terms + 1) * 128) / 8) / n_terms;
-            WarpFin wf;
-            wf.docs = nullptr;
-            wf.n_docs = 0;
-            if (run && ok) {
-                // the tile's slice of term `lane`
-                const u64 *t_ptr = nullptr;
-                u32 t_n = 0;
-                if (lane < n_terms) {
-                    const u64 *base = pl.ptr[lane];
-                    const u32 n = pl.n[lane];
-                    u32 lo = 0, hi = n;
-                    if (te - ts > 1) {
-                        if (P.has_dir[lane]) {
-                            lo = P.dirs[lane][tile - tile0] - pl.dir0[lane];
-                            hi = P.dirs[lane][tile + 1 - tile0] - pl.dir0[lane];
-                        } else {
-                            lo = w_lower_bound_doc(base, n, td0);
-                            hi = lo + w_lower_bound_doc(base + lo, n - lo, td0 + SA_TILE_DOCS);
-                        }
-                    }
-                    t_ptr = base + lo;
-                    t_n = hi - lo;
-                }
-                // this warp's sub-slice bounds: lane 2t searches the lower, lane 2t+1 the upper doc bound of term t
-                u32 bound = 0;
-                {
-                    const u32 t = lane >> 1;
-                    const u64 ptr_bits = __shfl_sync(0xffffffffu, (u64)(uintptr_t)t_ptr, t);
-                    const u32 n = __shfl_sync(0xffffffffu, t_n, t);
-                    if (t < n_terms) bound = w_lower_bound_doc(reinterpret_cast<const u64 *>((uintptr_t)ptr_bits), n, (lane & 1u) ? w_d1 : w_d0);
-                }
-                bool all_present = true;
-                for (u32 t = 0; t < n_terms; t++) wbm[t * 32 + lane] = 0u;
-                __syncwarp();
-                for (u32 t = 0; t < n_terms; t++) {
-                    const u64 *base = reinterpret_cast<const u64 *>((uintptr_t)__shfl_sync(0xffffffffu, (u64)(uintptr_t)t_ptr, t));
-                    const u32 lo = __shfl_sync(0xffffffffu, bound, 2 * t), hi = __shfl_sync(0xffffffffu, bound, 2 * t + 1);
-                    all_present = all_present && hi > lo;
-                    if (!all_present) break;                                    // warp-uniform
-                    u32 *bm = wbm + t * 32;
-                    for (u32 i = lo + lane; i < hi; i += 32) {
-                        const u32 rel = (u32)((base[i] >> SA_KEY_SHIFT) - w_d0);
-                        atomicOr(&bm[rel >> 5], 1u << (rel & 31u));
-                    }
-                }
-                __syncwarp();
-                u32 c = 0;
-                if (all_present) {
-                    c = wbm[lane];
-                    for (u32 t = 1; t < n_terms; t++) c &= wbm[t * 32 + lane];
-                }
-                if (__reduce_add_sync(0xffffffffu, (u32)__popc(c))) {          // warp-uniform: candidates in this sub-range
-                    wcand[lane] = c;
-                    __syncwarp();
-                    for (u32 t = 0; t < n_terms; t++) {
-                        const u64 *base = reinterpret_cast<const u64 *>((uintptr_t)__shfl_sync(0xffffffffu, (u64)(uintptr_t)t_ptr, t));
-                        const u32 lo = __shfl_sync(0xffffffffu, bound, 2 * t), hi = __shfl_sync(0xffffffffu, bound, 2 * t + 1);
-                        u64 *dst = fbw + (u64)t * fb_cap;
-                        u32 kept = 0;
-                        for (u32 i0 = lo; i0 < hi; i0 += 32) {                 // ordered compaction by ballots
-                            const u32 i = i0 + lane;
-                            u64 w = 0;
-                            bool keep = false;
-                            if (i < hi) {
-                                w = base[i];
-                                const u32 rel = (u32)((w >> SA_KEY_SHIFT) - w_d0);
-                                keep = (wcand[rel >> 5] >> (rel & 31u)) & 1u;
-                            }
-                            const unsigned m = __ballot_sync(0xffffffffu, keep);
-                            const u32 at = kept + __popc(m & ((1u << lane) - 1u));
-                            if (keep && at < fb_cap) dst[at] = w;
-                            kept += __popc(m);
-                        }
-                        if (lane == 0) {
-                            // (a list too long to compact enters the chain whole: its extra docs die at the other terms)
-                            P.sptr[warp][t] = kept <= fb_cap ? dst : base + lo;
-                            P.sn[warp][t] = kept <= fb_cap ? kept : hi - lo;
-                        }
-                    }
-                    __syncwarp();
-                    wf = warp_phrase_chain(pq, P.sptr[warp], P.sn[warp], cta_slab + (u64)warp * 6ull * cap, cap, &a.stats[q]);
-                }
-            }
-            // ---- this warp's 4 KB of the dense tile: zeros + its matches
-            __syncwarp();
-#pragma unroll
-            for (int i = 0; i < PW_SUB_DOCS / 32 / 4; i++)
-                reinterpret_cast<float4 *>(my_slice)[lane + i * 32] = make_float4(0.f, 0.f, 0.f, 0.f);
-            __syncwarp();
-            u32 my_max = 0, my_match = 0;
-            for (u32 i = lane; i < wf.n_docs; i += 32) {
-                const u64 e = wf.docs[i];
-                const u32 c = (u32)(e & 0xFFFFFFFFull);
-                if (c == 0) continue;
-                const u64 d = (e >> 32) - a.doc_base;
-                if (d >= a.n_docs) continue;
-                my_match++;
-                const float v = a.score ? bm25_one((float)c, __ldg(a.doc_lens + d), p) : (float)c;
-                P.tile[d - (u64)tile * SA_TILE_DOCS] = v;
-                if (v > 0.0f) my_max = max(my_max, __float_as_uint(v));
-            }
-            my_match = __reduce_add_sync(0xffffffffu, my_match);
-            if (lane == 0) {
-                if (my_match) atomicAdd(&a.stats[q].n_match, my_match);
-                P.wmatch[tile_no & 1u][warp] = my_match;
-            }
-            __syncthreads();                                                  // the tile's only block barrier (besides the flush's own)
-            u32 total = 0, holders = 0;
-#pragma unroll
-            for (int w = 0; w < PT / 32; w++) { const u32 m = P.wmatch[tile_no & 1u][w]; total += m; holders += min(m, 32u); }
-            if (total == 0) {
-                float4 *__restrict__ out4 = reinterpret_cast<float4 *>(out + (u64)tile * SA_TILE_DOCS);
-                const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-                for (int i = 0; i < SA_TILE_DOCS / PT / 4; i++) __stcs(out4 + tid + i * PT, z);
-                if (a.topk.k && tid == 0) {
-                    const u64 t_idx = (u64)row * a.topk.n_tiles + tile;
-                    a.topk.tile_cnt[t_idx] = 0;
-                    a.topk.tile_max[t_idx] = 0;
-                }
-                continue;                                                      // (the next tile's scratch lives in the warps' own slices)
-            }
-            flush_tile_collect(P.tile, out + (u64)tile * SA_TILE_DOCS, a.topk, row, tile, my_max, total, holders,
-                               P.top, &P.ncand, &P.tile_max);
-        }
-        __syncthreads();                    // every read of this half of the staging buffer is done: it may be refilled
-        ts = te;
-        seg++;
-    }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // The CONJUNCTION regime (balanced lists): one CTA per (query, 8192-doc tile), like the term scan -- small shared
 // memory footprint, five CTAs per SM, latency hidden by occupancy.  A doc can only match if it holds EVERY term of the
@@ -853,6 +543,8 @@ __device__ void phrase_work_staged(const PhraseArgs &a, const u32 q, const u32 c
 // 4 KB of the tile.  HBM traffic: 8 * sum(W) + 4 * N, each list read once, sequentially: the B_phrase of SURVEY 8d
 // without its continuation term.  A sub-range whose candidates do not fit its compaction area flags the query for
 // the exact re-run in the search regime (the host routes phrases whose terms co-occur that often there up front).
+// The pair statistics of the same-term speculation cover the candidate docs only: enough to CONFIRM a guess, not to
+// derive the reference's global decision from, so any disagreement also re-runs the query in the search regime.
 __global__ void __launch_bounds__(PT, 5)
 phrase_tile_kernel(const PhraseArgs a) {
     __shared__ __align__(16) float s_tile[SA_TILE_DOCS];
@@ -1019,33 +711,6 @@ phrase_tile_kernel(const PhraseArgs a) {
     flush_tile_collect(s_tile, out + (u64)tile * SA_TILE_DOCS, a.topk, row, tile, my_max, total, holders, s_top, &s_ncand, &s_tile_max);
 }
 
-// Persistent CTAs (grid = resident CTAs of the device): work items (query, chunk) are claimed with an atomic
-// counter, each CTA keeps its staging buffer (dynamic shared memory, two halves), its mbarriers and its scratch slab.
-__global__ void __launch_bounds__(PT, 2)
-phrase_staged_kernel(const PhraseArgs a) {
-    __shared__ StagedShared P;
-    extern __shared__ __align__(16) u64 s_stage[];
-    if (threadIdx.x == 0) {
-        sa_mbar_init(&P.bar[0], 1);
-        sa_mbar_init(&P.bar[1], 1);
-        sa_mbar_fence_init();
-    }
-    __syncthreads();
-    u32 phase[2] = {0u, 0u};
-    u64 *slab = a.slabs + (u64)blockIdx.x * (PT / 32) * 6ull * a.slab_cap;      // six buffers for each of the CTA's warps
-    const u32 n_work = a.n_sel * a.n_chunks;
-    for (;;) {
-        __syncthreads();
-        if (threadIdx.x == 0) P.work = atomicAdd(a.work_counter, 1u);
-        __syncthreads();
-        const u32 w = P.work;
-        if (w >= n_work) break;
-        // consecutive work items belong to different queries (dense and sparse lists interleave on an SM)
-        const u32 q = a.qsel[w % a.n_sel], chunk = w / a.n_sel;
-        phrase_work_staged(a, q, chunk, P, s_stage, phase, slab, a.slab_cap);
-    }
-}
-
 int launch_phrase(sa_index *ix, const PhraseArgs &a, u32 n_queries) {
     if (n_queries == 0 || a.n_docs == 0) return SA_OK;
     dim3 grid(n_queries, a.n_chunks);
@@ -1058,29 +723,22 @@ int launch_phrase(sa_index *ix, const PhraseArgs &a, u32 n_queries) {
     return SA_OK;
 }
 
-// resident CTAs of phrase_staged_kernel with `stage_words` words of dynamic shared memory
-static int staged_grid(sa_index *ix, u32 stage_words, u32 *ctas_out) {
-    static bool attr_set = false;
-    const size_t dyn = 2 * (size_t)stage_words * sizeof(u64);            // two halves (double buffering)
-    if (!attr_set) {
-        SA_CUDA(cudaFuncSetAttribute(phrase_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-        attr_set = true;
-    }
-    int per_sm = 0;
-    SA_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, phrase_staged_kernel, PT, dyn));
-    SA_CHECK(per_sm >= 1, "phrase_staged_kernel does not fit on an SM with %u staged words", stage_words);
-    *ctas_out = (u32)per_sm * (u32)ix->num_sms;
+// conjunction regime: one CTA per (query, tile), like the term scan
+static int launch_phrase_tile(sa_index *ix, const PhraseArgs &a, u32 n_queries) {
+    if (n_queries == 0 || a.n_docs == 0) return SA_OK;
+    const unsigned n_tiles = (unsigned)((a.n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS);
+    KernelTimer t(ix, 2);
+    phrase_tile_kernel<<<dim3(n_queries, n_tiles), PT, 0, ix->stream>>>(a);
+    SA_CUDA(cudaGetLastError());
+    t.stop();
+    ix->stats.phrase_kernel_launches++;
+    ix->stats.total_launches++;
     return SA_OK;
 }
 
-u32 sa_phrase_stage_words() {
-    static const long env = getenv("SA_PHRASE_STAGE_WORDS") ? atol(getenv("SA_PHRASE_STAGE_WORDS")) : 0;
-    return env > 0 ? (u32)std::min<long>(env, 9 * 1024) : 4608u;        // per half; 2 x 36 KB + 38 KB static: two CTAs per SM
-}
-
-// Merge regime or search regime?  Staging reads every list once (8 * sum(W) bytes); the search path costs about
-// `ratio` bytes (a dozen 32-byte sectors of dependent probes) per driver element of the first step.
-bool sa_phrase_is_staged(const PhraseQuery &pq, u64 n_docs) {
+// Conjunction regime or search regime?  The conjunction regime reads every list once (8 * sum(W) bytes); the search
+// path costs about `ratio` bytes (a dozen 32-byte sectors of dependent probes) per driver element of the first step.
+bool sa_phrase_use_conjunction(const PhraseQuery &pq, u64 n_docs) {
     static const long env = getenv("SA_PHRASE_STAGE_RATIO") ? atol(getenv("SA_PHRASE_STAGE_RATIO")) : -1;
     const u64 ratio = env >= 0 ? (u64)env : 50;
     if (ratio == 0) return false;
@@ -1147,10 +805,37 @@ static void step_order(const PhraseQuery &pq, std::vector<u32> &order) {
     }
 }
 
+// Launch arguments of both regimes.  The kernels write every tile of the dense rows themselves: no zero-fill pass.
+static PhraseArgs phrase_args(const sa_index *ix, const u64 *d_words, const PhraseQuery *d_pqs, PhraseStats *d_stats,
+                              float *dense_rows, u64 stride, u32 n_chunks, u64 *d_arena,
+                              unsigned long long *d_arena_used, u64 arena_words, int score, const Bm25Params &p) {
+    PhraseArgs a;
+    memset(&a, 0, sizeof(a));
+    a.words = d_words;
+    a.tile_dir = (d_words == ix->d_words) ? ix->d_tile_dir : nullptr;
+    a.doc_lens = ix->d_doc_lens;
+    a.n_docs = ix->n_docs;
+    a.doc_base = ix->doc_base;
+    a.queries = d_pqs;
+    a.stats = d_stats;
+    a.out = dense_rows;
+    a.out_stride = stride;
+    a.n_chunks = n_chunks;
+    a.docs_per_chunk = docs_per_chunk_of(ix, n_chunks);
+    a.arena = d_arena;
+    a.arena_used = d_arena_used;
+    a.arena_cap = arena_words;
+    a.bm25 = p;
+    a.score = score;
+    return a;
+}
+
 // Runs phrase queries (already planned) into ix->dense; loops until the same-term speculation
 // of every query is confirmed.  lists may live in ix->d_words (off = absolute word offsets).
+// allow_conj: a single query on the index's own lists may take the conjunction regime; otherwise
+// every query runs in the search regime, whose pair statistics cover every pair.
 int sa_phrase_run_sync(sa_index *ix, std::vector<PhraseQuery> &pqs, const u64 *d_words,
-                              int score, const Bm25Params &p, u32 n_chunks_hint, PhraseDump dump, u64 staged_slab_cap) {
+                       int score, const Bm25Params &p, u32 n_chunks_hint, PhraseDump dump, bool allow_conj) {
     const u32 Q = (u32)pqs.size();
     const u64 stride = padded(ix->n_docs);
     int rc;
@@ -1165,87 +850,44 @@ int sa_phrase_run_sync(sa_index *ix, std::vector<PhraseQuery> &pqs, const u64 *d
         n_chunks = std::max<u32>(n_chunks, 1);
     }
     n_chunks = sa_phrase_chunks(ix, n_chunks);
-    const u64 docs_per_chunk = docs_per_chunk_of(ix, n_chunks);
     u64 arena_words = 64;
     for (auto &pq : pqs) {
         u64 sum = 0;
         for (u32 t = 0; t < pq.n_terms; t++) sum += pq.len[t];
         arena_words += 6 * (sum + 2ull * n_chunks);
     }
-    // merge regime (single query on the index's own lists): persistent CTAs + TMA staging, no bump arena
-    bool staged = staged_slab_cap && Q == 1 && d_words == ix->d_words && !dump.cont && sa_phrase_is_staged(pqs[0], ix->n_docs);
+    // the conjunction regime needs no bump arena
+    bool conj = allow_conj && Q == 1 && d_words == ix->d_words && !dump.cont && sa_phrase_use_conjunction(pqs[0], ix->n_docs);
     const u64 full_arena_words = arena_words;
     const std::vector<PhraseQuery> pqs_in = pqs;
-    if (staged) arena_words = 64;
+    if (conj) arena_words = 64;
     if ((rc = ix->phrase_scratch.reserve(arena_words * sizeof(u64) + 64))) return rc;
     unsigned long long *d_used = (unsigned long long *)ix->phrase_scratch.p;
     u64 *d_arena = (u64 *)ix->phrase_scratch.p + 8;
     PhraseStats *d_stats = (PhraseStats *)ix->cand_meta.p;
     std::vector<PhraseStats> h_stats(Q);
-    std::vector<u32> order;
-    if (staged) {
-        if ((rc = ix->misc.reserve(256))) return rc;
-        SA_CUDA(cudaMemsetAsync(ix->misc.p, 0, sizeof(u32), ix->stream));      // qsel = {0}
-    }
 
     for (int attempt = 0; attempt < (int)SA_MAX_PHRASE_TERMS + 2; attempt++) {
         SA_CUDA(cudaMemcpyAsync(ix->queries.p, pqs.data(), (size_t)Q * sizeof(PhraseQuery), cudaMemcpyHostToDevice, ix->stream));
         SA_CUDA(cudaMemsetAsync(d_stats, 0, (size_t)Q * sizeof(PhraseStats), ix->stream));
         SA_CUDA(cudaMemsetAsync(d_used, 0, 64, ix->stream));
-        if (staged) {
-            PhraseSplit sp;
-            memset(&sp, 0, sizeof(sp));
-            sp.d_staged = (const u32 *)ix->misc.p;
-            sp.n_staged = 1;
-            sp.staged_chunks = sa_phrase_staged_chunks(ix);
-            sp.slab_cap = staged_slab_cap;
-            if ((rc = sa_phrase_enqueue(ix, ix->queries.as<PhraseQuery>(), d_stats, 1, ix->dense.as<float>(), stride, 1, d_arena,
-                                        d_used, arena_words, score, p, nullptr, 0, &sp))) return rc;
-        } else {
-        PhraseArgs a;      // (the kernel writes every tile of the dense rows itself: no zero-fill pass)
-        memset(&a, 0, sizeof(a));
-        a.words = d_words;
-        a.tile_dir = (d_words == ix->d_words) ? ix->d_tile_dir : nullptr;
-        a.doc_lens = ix->d_doc_lens;
-        a.n_docs = ix->n_docs;
-        a.doc_base = ix->doc_base;
-        a.queries = ix->queries.as<PhraseQuery>();
-        a.stats = d_stats;
-        a.out = ix->dense.as<float>();
-        a.out_stride = stride;
-        a.n_chunks = n_chunks;
-        a.docs_per_chunk = docs_per_chunk;
-        a.arena = d_arena;
-        a.arena_used = d_used;
-        a.arena_cap = arena_words;
-        a.bm25 = p;
-        a.score = score;
+        PhraseArgs a = phrase_args(ix, d_words, ix->queries.as<PhraseQuery>(), d_stats, ix->dense.as<float>(), stride,
+                                   n_chunks, d_arena, d_used, arena_words, score, p);
         a.dump = dump;
-        if ((rc = launch_phrase(ix, a, Q))) return rc;
-        }
+        if ((rc = conj ? launch_phrase_tile(ix, a, Q) : launch_phrase(ix, a, Q))) return rc;
         SA_CUDA(cudaMemcpyAsync(h_stats.data(), d_stats, (size_t)Q * sizeof(PhraseStats), cudaMemcpyDeviceToHost, ix->stream));
         SA_CUDA(cudaStreamSynchronize(ix->stream));
         bool again = false;
         for (u32 q = 0; q < Q; q++) {
             SA_CHECK(h_stats[q].overflow != 1, "phrase scratch arena exhausted (internal sizing error)");
-            if (h_stats[q].overflow == 2) { again = true; continue; }      // dense conjunction: the search regime takes it
-            step_order(pqs[q], order);
-            for (u32 s : order) {
-                bool actual = h_stats[q].n_inner[s] > 0 && h_stats[q].n_diff[s] == 0;
-                bool guess = (pqs[q].same_guess >> s) & 1u;
-                if (actual != guess) {      // later steps ran on a wrong premise: fix this one, redo
-                    pqs[q].same_guess ^= 1u << s;
-                    again = true;
-                    break;
-                }
-            }
+            // overflow 2: dense conjunction, the search regime takes it; a wrong guess is flipped for the next attempt
+            if (h_stats[q].overflow == 2 || !sa_phrase_guess_ok(pqs[q], h_stats[q])) again = true;
         }
         if (!again) return SA_OK;
-        if (staged) {
-            // The merge regime counts equal-header pairs in the candidate docs only (docs holding every term): enough to
-            // CONFIRM a guess, not to derive the reference's global same-term decision from.  On any disagreement the
-            // query starts over in the search regime, whose statistics cover every pair.
-            staged = false;
+        if (conj) {
+            // The conjunction regime's pair statistics only CONFIRM a guess (phrase_tile_kernel): on any disagreement
+            // the query starts over in the search regime, whose statistics cover every pair.
+            conj = false;
             pqs = pqs_in;
             arena_words = full_arena_words;
             if ((rc = ix->phrase_scratch.reserve(arena_words * sizeof(u64) + 64))) return rc;
@@ -1297,87 +939,16 @@ int sa_phrase_enqueue(sa_index *ix, const PhraseQuery *d_pqs, PhraseStats *d_sta
                       float *dense_rows, u64 stride, u32 n_chunks, u64 *d_arena,
                       unsigned long long *d_arena_used, u64 arena_words, int score, const Bm25Params &p,
                       const TopkCtx *topk, u32 topk_row0, const PhraseSplit *split) {
-    PhraseArgs a;
-    memset(&a, 0, sizeof(a));
-    a.words = ix->d_words;
-    a.tile_dir = ix->d_tile_dir;
-    a.doc_lens = ix->d_doc_lens;
-    a.n_docs = ix->n_docs;
-    a.doc_base = ix->doc_base;
-    a.queries = d_pqs;
-    a.stats = d_stats;
-    a.out = dense_rows;
-    a.out_stride = stride;
-    a.n_chunks = n_chunks;
-    a.docs_per_chunk = docs_per_chunk_of(ix, n_chunks);
-    a.arena = d_arena;
-    a.arena_used = d_arena_used;
-    a.arena_cap = arena_words;
-    a.bm25 = p;
-    a.score = score;
+    PhraseArgs a = phrase_args(ix, ix->d_words, d_pqs, d_stats, dense_rows, stride, n_chunks, d_arena, d_arena_used,
+                               arena_words, score, p);
     if (topk) a.topk = *topk;
     a.topk_row0 = topk_row0;
-    if (!split || split->n_staged == 0) {
-        if (split) { a.qsel = split->d_search; a.n_sel = split->n_search; }
-        return launch_phrase(ix, a, split ? split->n_search : Q);
-    }
+    if (!split) return launch_phrase(ix, a, Q);
     int rc;
-    if (split->n_search) {                      // search regime: one CTA per (query, chunk)
-        a.qsel = split->d_search;
-        a.n_sel = split->n_search;
-        if ((rc = launch_phrase(ix, a, split->n_search))) return rc;
-    }
-    a.qsel = split->d_staged;
-    a.n_sel = split->n_staged;
-    static const bool use_tma_pipeline = getenv("SA_PHRASE_TMA_PIPELINE") && atoi(getenv("SA_PHRASE_TMA_PIPELINE")) != 0;
-    if (!use_tma_pipeline) {
-        // conjunction regime: one CTA per (query, tile), like the term scan
-        const unsigned n_tiles = (unsigned)((ix->n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS);
-        KernelTimer t(ix, 2);
-        phrase_tile_kernel<<<dim3(split->n_staged, n_tiles), PT, 0, ix->stream>>>(a);
-        SA_CUDA(cudaGetLastError());
-        t.stop();
-        ix->stats.phrase_kernel_launches++;
-        ix->stats.total_launches++;
-        return SA_OK;
-    }
-    // the same regime as persistent CTAs with a double-buffered TMA pipeline (kept for comparison; not the
-    // default): SA_PHRASE_TMA_PIPELINE=1
-    const u32 stage_words = sa_phrase_stage_words();
-    u32 ctas = 0;
-    if ((rc = staged_grid(ix, stage_words, &ctas))) return rc;
-    if ((rc = ix->phrase_slabs.reserve((size_t)ctas * (PT / 32) * 6 * split->slab_cap * sizeof(u64)))) return rc;
-    a.qsel = split->d_staged;
-    a.n_sel = split->n_staged;
-    a.n_chunks = split->staged_chunks;
-    a.docs_per_chunk = docs_per_chunk_of(ix, split->staged_chunks);
-    a.stage_words = stage_words;
-    a.slabs = ix->phrase_slabs.as<u64>();
-    a.slab_cap = split->slab_cap;
-    a.work_counter = (u32 *)(d_arena_used + 1);                 // zeroed with the arena counter
-    const u64 n_work = (u64)a.n_sel * a.n_chunks;
-    KernelTimer t(ix, 2);
-    phrase_staged_kernel<<<(unsigned)std::min<u64>(ctas, n_work), PT, 2 * (size_t)stage_words * sizeof(u64), ix->stream>>>(a);
-    SA_CUDA(cudaGetLastError());
-    t.stop();
-    ix->stats.phrase_kernel_launches++;
-    ix->stats.total_launches++;
-    return SA_OK;
-}
-
-// chunks of the merge regime: whole tiles, ~16 tiles each (segments are cut inside the kernel)
-u32 sa_phrase_staged_chunks(const sa_index *ix) {
-    const u64 n_tiles = (ix->n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS;
-    return sa_phrase_chunks(ix, (u32)std::max<u64>(1, (n_tiles + 15) / 16));
-}
-
-// scratch entries per buffer a persistent CTA needs for this query: no segment slice is longer than the largest
-// per-tile slice of its terms (one-tile segments) or the staging capacity (multi-tile segments)
-u64 sa_phrase_slab_cap(const sa_index *ix, const u32 *term_ids, u32 n_terms) {
-    u64 cap = sa_phrase_stage_words();
-    for (u32 i = 0; i < n_terms; i++)
-        if (term_ids[i] != SA_NO_TERM && term_ids[i] < ix->n_terms) cap = std::max<u64>(cap, ix->h_max_tile_words[term_ids[i]]);
-    return cap + 8;
+    a.qsel = split->d_search;                   // search regime: one CTA per (query, chunk)
+    if ((rc = launch_phrase(ix, a, split->n_search))) return rc;
+    a.qsel = split->d_conj;
+    return launch_phrase_tile(ix, a, split->n_conj);
 }
 
 static int phrase_common(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, uint32_t slop,
@@ -1450,8 +1021,7 @@ static int phrase_common(sa_index *ix, const uint32_t *term_ids, uint32_t n_term
         PhraseDump nodump;
         memset(&nodump, 0, sizeof(nodump));
         // raw counts first when BM25 must touch every doc
-        if ((rc = sa_phrase_run_sync(ix, pqs, d_lists, score && p.sparse_ok, p, 0, nodump,
-                                     d_lists == ix->d_words ? sa_phrase_slab_cap(ix, term_ids, n_terms) : 0))) return rc;
+        if ((rc = sa_phrase_run_sync(ix, pqs, d_lists, score && p.sparse_ok, p, 0, nodump, true))) return rc;
         raw_counts = score && !p.sparse_ok;
     } else {
         if ((rc = ix->dense.reserve(stride * sizeof(float)))) return rc;
@@ -1522,7 +1092,7 @@ extern "C" int sa_op_bigram_freqs(const uint64_t *lhs, uint64_t n_lhs, const uin
             cudaMemsetAsync(dump.n_cont, 0, 2 * sizeof(u64), ix->stream);
             Bm25Params p;
             memset(&p, 0, sizeof(p));
-            rc = sa_phrase_run_sync(ix, pqs, ix->d_words, 0, p, 1, dump, 0);
+            rc = sa_phrase_run_sync(ix, pqs, ix->d_words, 0, p, 1, dump, false);
             if (!rc) {
                 u64 n[2];
                 cudaMemcpy(n, dump.n_cont, 2 * sizeof(u64), cudaMemcpyDeviceToHost);

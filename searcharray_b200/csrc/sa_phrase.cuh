@@ -18,7 +18,7 @@ struct PhraseQuery {
     u64 len[SA_MAX_PHRASE_TERMS];
     u64 dir_plus1[SA_MAX_PHRASE_TERMS];   // 1 + offset of the list's tile directory in d_tile_dir; 0 = none
     float idf;
-    u32 pad;
+    u32 use_conj;         // batches: 1 = the conjunction regime runs it (sa_phrase_use_conjunction); the kernels ignore it
 };
 
 struct PhraseStats {      // per query, accumulated over all chunks (global atomics)
@@ -61,22 +61,14 @@ struct PhraseArgs {
     u32 topk_row0;
     const u32 *tile_dir;        // word tile directories (sa_index::d_tile_dir) or NULL (filtered lists)
     const u32 *qsel;            // launch only these queries (indices into `queries`); NULL = all, in order
-    u32 n_sel;
-    // merge regime (phrase_staged_kernel, persistent CTAs)
-    u32 stage_words;            // capacity of a CTA's staging buffer (dynamic shared memory), in words
-    u64 *slabs;                 // per-CTA scratch: 6 * slab_cap words each
-    u64 slab_cap;
-    u32 *work_counter;
 };
 
 // Which queries of a batch run in which regime (device index lists into the PhraseQuery array)
 struct PhraseSplit {
     const u32 *d_search;
     u32 n_search;
-    const u32 *d_staged;
-    u32 n_staged;
-    u32 staged_chunks;
-    u64 slab_cap;
+    const u32 *d_conj;
+    u32 n_conj;
 };
 
 int launch_phrase(sa_index *ix, const PhraseArgs &a, u32 n_queries);
@@ -87,10 +79,7 @@ int sa_phrase_enqueue(sa_index *ix, const PhraseQuery *d_pqs, PhraseStats *d_sta
                       float *dense_rows, u64 stride, u32 n_chunks, u64 *d_arena,
                       unsigned long long *d_arena_used, u64 arena_words, int score, const Bm25Params &p,
                       const TopkCtx *topk, u32 topk_row0, const PhraseSplit *split);
-u32 sa_phrase_staged_chunks(const sa_index *ix);
-u64 sa_phrase_slab_cap(const sa_index *ix, const u32 *term_ids, u32 n_terms);
 u32 sa_phrase_chunks(const sa_index *ix, u32 wanted);
-bool sa_phrase_is_staged(const PhraseQuery &pq, u64 n_docs);
-u32 sa_phrase_stage_words();
+bool sa_phrase_use_conjunction(const PhraseQuery &pq, u64 n_docs);
 int sa_phrase_run_sync(sa_index *ix, std::vector<PhraseQuery> &pqs, const u64 *d_words,
-                       int score, const Bm25Params &p, u32 n_chunks_hint, PhraseDump dump, u64 staged_slab_cap);
+                       int score, const Bm25Params &p, u32 n_chunks_hint, PhraseDump dump, bool allow_conj);

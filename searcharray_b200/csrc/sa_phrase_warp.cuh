@@ -1,12 +1,11 @@
-// sa_phrase_warp.cuh -- the bigram chain at WARP scope, for the merge regime of sa_phrase.cu.
+// sa_phrase_warp.cuh -- the bigram chain at WARP scope, for the conjunction regime of sa_phrase.cu (phrase_tile_kernel).
 //
-// Once a segment's posting slices sit in shared memory (TMA-staged, sa_phrase.cu), the CTA's eight warps cut the
-// segment's doc range into eight sub-ranges and every warp runs the whole n-term chain on its own sub-range without
-// a single block barrier: driver elements are taken 32 at a time, partners are found by binary search in shared
-// memory, continuation words are emitted in order through ballots (`__ballot_sync` + popcount prefix), the per-doc
-// counts are a segmented warp reduction (`__match_any_sync` groups of equal doc id, `__reduce_add_sync` inside the
-// group), and a doc run crossing an iteration boundary is carried in registers.  Phrase matching never crosses a
-// document, so the sub-ranges are independent (reference phrase/bigram_freqs.py:213-307 semantics per doc).
+// A warp runs the whole n-term chain on its own sub-range of docs without a single block barrier: driver elements are
+// taken 32 at a time, partners are found by binary search, continuation words are emitted in order through ballots
+// (`__ballot_sync` + popcount prefix), the per-doc counts are a segmented warp reduction (`__match_any_sync` groups of
+// equal doc id, `__reduce_add_sync` inside the group), and a doc run crossing an iteration boundary is carried in
+// registers.  Phrase matching never crosses a document, so the sub-ranges are independent (reference
+// phrase/bigram_freqs.py:213-307 semantics per doc).
 #pragma once
 #include "sa_phrase.cuh"
 

@@ -20,7 +20,7 @@
 //     the other list); grouped sums are head flags + a scan + integer atomics (deterministic);
 //   * everything that compacts goes through one flags -> exclusive scan -> ordered write pipeline.
 // Host in, host out: these exports exist for kernel-level parity tests; the scoring path proper keeps its
-// data in HBM (sa_phrase.cu uses the same staging primitive, sa_tma.cuh).
+// data in HBM.
 #include <algorithm>
 #include <vector>
 
