@@ -293,7 +293,7 @@ extern "C" int sa_multi_create(sa_index *const *fields, uint32_t n_fields, sa_mu
     m->device = fields[0]->device;
     m->n_docs = fields[0]->n_docs;
     m->doc_base = fields[0]->doc_base;
-    m->stride = (m->n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS * SA_TILE_DOCS;
+    m->stride = sa_padded_docs(m->n_docs);
     m->filt_offs.resize(n_fields);
     m->filt_lens.resize(n_fields);
     m->phrase_rows.assign(n_fields, 0);
@@ -359,33 +359,18 @@ extern "C" int sa_multi_qf(sa_multi *m, int field_centric, const uint32_t *n_ter
         if (T && (avg_doc_len[f] == 0.0f || m->n_docs == 0)) {         // similarity.py:31-32: zeros
             SA_CUDA(cudaMemsetAsync(ix->dense.p, 0, (size_t)T * m->stride * sizeof(float), m->stream));
         } else if (T) {
+            if ((rc = sa_check_term_ids(ix, term_ids + at, T))) return rc;
             std::vector<TermQuery> tqs(T);
-            Bm25Params p = sa_make_bm25(ix, 1.0f, avg_doc_len[f], k1[f], b[f]);
+            Bm25Params p = make_bm25(1.0f, avg_doc_len[f], k1[f], b[f], ix->doc_lens_nonneg);
             for (u32 t = 0; t < T; t++) {
-                const u32 id = term_ids[at + t];
-                SA_CHECK(id == SA_NO_TERM || id < ix->n_terms, "term id %u out of range", id);
-                tqs[t] = sa_make_term_query(ix, id, idf[at + t]);
-                if (!sa_make_bm25(ix, idf[at + t], avg_doc_len[f], k1[f], b[f]).sparse_ok) p.sparse_ok = 0;
+                tqs[t] = make_term_query(ix, term_ids[at + t], idf[at + t]);
+                if (!make_bm25(idf[at + t], avg_doc_len[f], k1[f], b[f], ix->doc_lens_nonneg).sparse_ok) p.sparse_ok = 0;
             }
             if ((rc = ix->queries.reserve(T * sizeof(TermQuery)))) return rc;
             SA_CUDA(cudaMemcpyAsync(ix->queries.p, tqs.data(), T * sizeof(TermQuery), cudaMemcpyHostToDevice, m->stream));
             TopkCtx none;
             memset(&none, 0, sizeof(none));
-            TermBatchArgs ta;
-            memset(&ta, 0, sizeof(ta));
-            ta.words = ix->d_words;
-            ta.doc_lens = ix->d_doc_lens;
-            ta.n_docs = ix->n_docs;
-            ta.doc_base = ix->doc_base;
-            ta.queries = ix->queries.as<TermQuery>();
-            ta.out = ix->dense.as<float>();
-            ta.out_stride = m->stride;
-            ta.bm25 = p;
-            ta.min_payload = 0;
-            ta.max_payload = SA_ALL_BITS;
-            ta.mode = TERM_MODE_SCORE;
-            ta.topk = none;
-            if ((rc = launch_term_batch(ix, ta, T))) return rc;
+            if ((rc = launch_term_batch(ix, make_term_args(ix, ix->queries.as<TermQuery>(), p, none), T))) return rc;
             SA_CUDA(cudaStreamSynchronize(m->stream));                  // tqs leaves scope
         }
         at += T;
@@ -419,8 +404,8 @@ extern "C" int sa_multi_filter(sa_multi *m, uint32_t field, const uint32_t *term
     std::lock_guard<std::mutex> g(m->mu);
     SA_CUDA(cudaSetDevice(m->device));
     sa_index *ix = m->fields[field];
-    for (u32 t = 0; t < n_terms; t++)
-        SA_CHECK(term_ids[t] == SA_NO_TERM || term_ids[t] < ix->n_terms, "term id %u out of range", term_ids[t]);
+    int rc = sa_check_term_ids(ix, term_ids, n_terms);
+    if (rc) return rc;
     FieldGuard fg(ix, m->stream);
     std::vector<u64> dfs;
     if (m->filt_bound[field] == 0) {
@@ -436,9 +421,8 @@ extern "C" int sa_multi_filter(sa_multi *m, uint32_t field, const uint32_t *term
         int rc0 = ix->filt.reserve(m->filt_bound[field] * sizeof(u64));
         if (rc0) return rc0;
     }
-    int rc = sa_filter_terms_mask(ix, term_ids, n_terms, m->d_mask, 0, SA_ALL_BITS, false,
-                                  m->filt_offs[field], m->filt_lens[field], &dfs);
-    if (rc) return rc;
+    if ((rc = sa_filter_terms_mask(ix, term_ids, n_terms, m->d_mask, 0, SA_ALL_BITS, false,
+                                   m->filt_offs[field], m->filt_lens[field], &dfs))) return rc;
     for (u32 t = 0; t < n_terms; t++) df_out[t] = dfs[t];
     return SA_OK;
 }
@@ -462,30 +446,26 @@ extern "C" int sa_multi_phrases(sa_multi *m, uint32_t field, uint32_t n_phrases,
         return SA_OK;
     }
     std::vector<PhraseQuery> pqs(n_phrases);
-    Bm25Params p = sa_make_bm25(ix, 1.0f, avg_doc_len, k1, b);
+    const Bm25Params p = make_bm25(1.0f, avg_doc_len, k1, b, ix->doc_lens_nonneg);
     for (u32 i = 0; i < n_phrases; i++) {
-        PhraseQuery &pq = pqs[i];
-        memset(&pq, 0, sizeof(pq));
         const u32 s0 = phrase_starts[i], nt = phrase_starts[i + 1] - s0;
         SA_CHECK(nt >= 2 && nt <= SA_MAX_PHRASE_TERMS, "phrase %u: 2..%d terms", i, SA_MAX_PHRASE_TERMS);
-        pq.n_terms = nt;
-        pq.idf = idf[i];
-        SA_CHECK(sa_make_bm25(ix, idf[i], avg_doc_len, k1, b).sparse_ok,
+        SA_CHECK(make_bm25(idf[i], avg_doc_len, k1, b, ix->doc_lens_nonneg).sparse_ok,
                  "edismax phrase phases need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite idf >= 0)");
+        u64 p_offs[SA_MAX_PHRASE_TERMS], p_lens[SA_MAX_PHRASE_TERMS];
         bool missing = false;
         for (u32 j = 0; j < nt; j++) {
             const u32 slot = term_slots[s0 + j];
             SA_CHECK(slot < offs.size(), "term slot out of range");
             if (term_ids[s0 + j] == SA_NO_TERM || lens[slot] == 0) missing = true;
-            pq.off[j] = offs[slot];
-            pq.len[j] = lens[slot];
+            p_offs[j] = offs[slot];
+            p_lens[j] = lens[slot];
         }
-        if (missing) for (u32 j = 0; j < nt; j++) pq.len[j] = 0;       // unknown term -> zeros (postings.py:705-708)
-        sa_phrase_plan(pq, term_ids + s0);
+        pqs[i] = make_phrase_query(term_ids + s0, nt, p_offs, p_lens, nullptr, idf[i], missing);
     }
     PhraseDump nodump;
     memset(&nodump, 0, sizeof(nodump));
-    return sa_phrase_run_sync(ix, pqs, ix->filt.as<u64>(), 1, p, 0, nodump, false);
+    return sa_phrase_run_sync(ix, pqs, ix->filt.as<u64>(), 1, p, nodump, false);
 }
 
 extern "C" int sa_multi_add_phase(sa_multi *m, uint32_t n_entries, const uint32_t *entry_field,
@@ -548,25 +528,18 @@ extern "C" int sa_multi_topk(sa_multi *m, uint32_t k, uint32_t *out_docs, double
     if (m->n_docs == 0) return SA_OK;
     sa_index *ix = m->fields[0];
     FieldGuard fg(ix, m->stream);
-    const u32 T = (u32)(m->stride / SA_TILE_DOCS);
+    const u32 T = sa_n_tiles(m->n_docs);
     int rc;
     unsigned blocks = (unsigned)((m->stride + 255) / 256);
     edismax_proxy_kernel<<<blocks, 256, 0, m->stream>>>(m->d_qf, m->d_proxy, m->stride);
     SA_CUDA(cudaGetLastError());
     u32 slots = sa_topk_slots(k);
     for (int attempt = 0; attempt < 2; attempt++) {
-        if ((rc = m->cand.reserve((size_t)T * ((size_t)slots * sizeof(u64) + 2 * sizeof(u32)) + 64))) return rc;
+        if ((rc = m->cand.reserve(cand_bytes(T, 1, slots)))) return rc;
         if ((rc = m->meta.reserve(256))) return rc;
         if ((rc = m->keys.reserve((size_t)k * (sizeof(u64) + sizeof(double) + sizeof(u32)) + 64))) return rc;
         SA_CUDA(cudaMemsetAsync(m->meta.p, 0, 256, m->stream));
-        TopkCtx t;
-        t.tile_cand = m->cand.as<u64>();
-        t.tile_cnt = (u32 *)(t.tile_cand + (u64)T * slots);
-        t.tile_max = t.tile_cnt + T;
-        t.overflow = m->meta.as<u32>();
-        t.n_tiles = T;
-        t.slots = slots;
-        t.k = k;
+        const TopkCtx t = make_topk_ctx(m->cand.p, T, 1, slots, k, m->meta.as<u32>());
         if ((rc = launch_dense_topk_tiles(ix, m->d_proxy, m->stride, 0, 1, t, nullptr))) return rc;
         if ((rc = launch_topk_select(ix, t, 1, 0, m->keys.as<u64>(), nullptr))) return rc;
         u32 ovf = 0;

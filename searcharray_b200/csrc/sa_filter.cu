@@ -189,11 +189,16 @@ int sa_filter_terms(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, bo
                                 offs, lens, nullptr);
 }
 
-int sa_gather_rows(sa_index *ix, const float *d_dense, float *out_host) {
+int sa_copy_out_dense(sa_index *ix, float *out_host) {
+    if (!ix->rows_active) {
+        SA_CUDA(cudaMemcpyAsync(out_host, ix->dense.p, ix->n_docs * sizeof(float), cudaMemcpyDeviceToHost, ix->stream));
+        SA_CUDA(cudaStreamSynchronize(ix->stream));
+        return SA_OK;
+    }
     int rc;
     if ((rc = ix->gather.reserve(ix->n_rows * sizeof(float) + 64))) return rc;
-    gather_rows_kernel<<<(unsigned)((ix->n_rows + 255) / 256), 256, 0, ix->stream>>>(d_dense, ix->d_rows, ix->n_rows,
-                                                                                   ix->gather.as<float>());
+    gather_rows_kernel<<<(unsigned)((ix->n_rows + 255) / 256), 256, 0, ix->stream>>>(ix->dense.as<float>(), ix->d_rows,
+                                                                                   ix->n_rows, ix->gather.as<float>());
     SA_CUDA(cudaGetLastError());
     ix->stats.total_launches++;
     SA_CUDA(cudaMemcpyAsync(out_host, ix->gather.p, ix->n_rows * sizeof(float), cudaMemcpyDeviceToHost, ix->stream));
@@ -232,13 +237,13 @@ extern "C" int sa_index_set_rows(sa_index *ix, const uint64_t *rows, uint64_t n_
 extern "C" int sa_docfreq_rows(sa_index *ix, uint32_t term_id, uint64_t *df_out) {
     SA_CHECK(ix && df_out, "NULL argument");
     if (term_id == SA_NO_TERM) { *df_out = 0; return SA_OK; }
-    SA_CHECK(term_id < ix->n_terms, "term id %u out of range", term_id);
+    int rc = sa_check_term_ids(ix, &term_id, 1);
+    if (rc) return rc;
     std::lock_guard<std::mutex> g(ix->mu);
     SA_CUDA(cudaSetDevice(ix->device));
     if (!ix->rows_active) { *df_out = ix->h_df[term_id]; return SA_OK; }
     std::vector<u64> offs, lens, dfs;
-    int rc = sa_filter_terms_mask(ix, &term_id, 1, ix->d_row_mask, 0, SA_ALL_BITS, false, offs, lens, &dfs);
-    if (rc) return rc;
+    if ((rc = sa_filter_terms_mask(ix, &term_id, 1, ix->d_row_mask, 0, SA_ALL_BITS, false, offs, lens, &dfs))) return rc;
     *df_out = dfs[0];
     return SA_OK;
 }

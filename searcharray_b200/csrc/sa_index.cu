@@ -2,7 +2,6 @@
 // points of the term path (see include/searcharray_b200.h for the reference mapping).
 #include <stdarg.h>
 #include <algorithm>
-#include <cmath>
 
 #include "sa_term.cuh"
 #include "sa_phrase.cuh"
@@ -372,7 +371,7 @@ extern "C" int sa_index_create(const uint64_t *words, uint64_t n_words,
         u32 *d_slot = nullptr;
         u32 n_slots = (u32)off_sorted.size();
         // tile directories for long lists (short ones are searched: they stay cache resident)
-        const u32 n_tiles = (u32)((n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS);
+        const u32 n_tiles = sa_n_tiles(n_docs);
         const u64 dir_min_words = std::max<u64>(1024, n_tiles / 2);
         std::vector<u64> slot_len(n_slots), slot_dir(n_slots, SA_NO_DIR);
         u64 dir_words = 0;
@@ -524,7 +523,8 @@ extern "C" int sa_index_upload_mode(const sa_index *ix, int *mode_out) {
 extern "C" int sa_docfreq(sa_index *ix, uint32_t term_id, uint64_t *df_out) {
     SA_CHECK(ix && df_out, "NULL argument");
     if (term_id == SA_NO_TERM) { *df_out = 0; return SA_OK; }
-    SA_CHECK(term_id < ix->n_terms, "term id %u out of range", term_id);
+    int rc = sa_check_term_ids(ix, &term_id, 1);
+    if (rc) return rc;
     *df_out = ix->h_df[term_id];
     return SA_OK;
 }
@@ -554,87 +554,46 @@ extern "C" int sa_set_profiling(sa_index *ix, int enabled) {
 }
 
 // ----------------------------------------------------------------- term path
-static Bm25Params make_bm25(const sa_index *ix, float idf, float avg_doc_len, float k1, float b) {
-    Bm25Params p;
-    p.idf = idf;
-    p.avg_doc_len = avg_doc_len;
-    p.k1 = k1;
-    p.b = b;
-    p.one_minus_b = 1 - b;       // float arithmetic, as `cdef float one_minus_b = 1 - b` (bm25.pyx:19)
-    p.sparse_ok = (ix->doc_lens_nonneg && k1 > 0.0f && std::isfinite(k1) && b >= 0.0f && b < 1.0f &&
-                   avg_doc_len > 0.0f && std::isfinite(avg_doc_len) && std::isfinite(idf) &&
-                   idf >= 0.0f && !std::signbit(idf)) ? 1 : 0;
-    return p;
-}
-
-static u64 padded_docs(u64 n_docs) { return (n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS * SA_TILE_DOCS; }
-
-int sa_filter_terms(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, bool use_rows,
-                    u64 pay_lo, u64 pay_hi, bool use_payload, std::vector<u64> &offs, std::vector<u64> &lens);
-int sa_gather_rows(sa_index *ix, const float *d_dense, float *out_host);
-
 static int single_term(sa_index *ix, uint32_t term_id, int mode, const Bm25Params &p,
                        u64 min_payload, u64 max_payload, float *out_host) {
     SA_CHECK(ix && out_host, "NULL argument");
-    SA_CHECK(term_id == SA_NO_TERM || term_id < ix->n_terms, "term id %u out of range", term_id);
+    int rc = sa_check_term_ids(ix, &term_id, 1);
+    if (rc) return rc;
     std::lock_guard<std::mutex> g(ix->mu);
     SA_CUDA(cudaSetDevice(ix->device));
     if (ix->n_docs == 0) return SA_OK;
     const bool rows = ix->rows_active;
     SA_CHECK(!(rows && mode == TERM_MODE_SCORE), "score on a sliced array: call termfreqs + bm25 (the Python layer does)");
-    const u64 stride = padded_docs(ix->n_docs);
-    int rc = ix->dense.reserve(stride * sizeof(float));
-    if (rc) return rc;
-    rc = ix->queries.reserve(sizeof(TermQuery));
-    if (rc) return rc;
-    TermQuery tq;
-    memset(&tq, 0, sizeof(tq));
-    tq.word_off = term_id == SA_NO_TERM ? 0 : ix->h_off[term_id];
-    tq.n_words = term_id == SA_NO_TERM ? 0 : ix->h_len[term_id];
-    tq.dir_off = term_id == SA_NO_TERM ? SA_NO_DIR : ix->h_dir_off[term_id];
-    tq.rec_off = (term_id == SA_NO_TERM || ix->h_rec_off.empty()) ? SA_NO_DIR : ix->h_rec_off[term_id];
-    tq.idf = p.idf;
-    const u64 *words = ix->d_words;
-    bool filter = !(min_payload == 0 && max_payload == SA_ALL_BITS);
+    if ((rc = ix->dense.reserve(sa_padded_docs(ix->n_docs) * sizeof(float)))) return rc;
+    if ((rc = ix->queries.reserve(sizeof(TermQuery)))) return rc;
+    TermQuery tq = make_term_query(ix, term_id, p.idf);
+    TopkCtx none;
+    memset(&none, 0, sizeof(none));
+    TermBatchArgs a = make_term_args(ix, ix->queries.as<TermQuery>(), p, none);
+    a.min_payload = min_payload;
+    a.max_payload = max_payload;
+    a.filter = !(min_payload == 0 && max_payload == SA_ALL_BITS);
+    a.mode = mode;
     if (rows && term_id != SA_NO_TERM) {
         // sliced array: run on the materialised FilteredPosns list (rows and block filter applied)
         std::vector<u64> offs, lens;
-        if ((rc = sa_filter_terms(ix, &term_id, 1, true, min_payload, max_payload, filter, offs, lens))) return rc;
-        words = ix->filt.as<u64>();
+        if ((rc = sa_filter_terms(ix, &term_id, 1, true, min_payload, max_payload, a.filter, offs, lens))) return rc;
+        a.words = ix->filt.as<u64>();
         tq.word_off = offs[0];
         tq.n_words = lens[0];
         tq.dir_off = SA_NO_DIR;
         tq.rec_off = SA_NO_DIR;
-        filter = false;
+        a.filter = 0;
     }
     SA_CUDA(cudaMemcpyAsync(ix->queries.p, &tq, sizeof(tq), cudaMemcpyHostToDevice, ix->stream));
-    TermBatchArgs a;
-    memset(&a, 0, sizeof(a));
-    a.words = words;
-    a.doc_lens = ix->d_doc_lens;
-    a.n_docs = ix->n_docs;
-    a.doc_base = ix->doc_base;
-    a.queries = ix->queries.as<TermQuery>();
-    a.out = ix->dense.as<float>();
-    a.out_stride = stride;
-    a.bm25 = p;
-    a.min_payload = min_payload;
-    a.max_payload = max_payload;
-    a.filter = filter;
-    a.mode = mode;
-    a.topk.k = 0;
-    rc = launch_term_batch(ix, a, 1);
-    if (rc) return rc;
-    if (rows) return sa_gather_rows(ix, ix->dense.as<float>(), out_host);
-    SA_CUDA(cudaMemcpyAsync(out_host, ix->dense.p, ix->n_docs * sizeof(float), cudaMemcpyDeviceToHost, ix->stream));
-    SA_CUDA(cudaStreamSynchronize(ix->stream));
-    return SA_OK;
+    if ((rc = launch_term_batch(ix, a, 1))) return rc;
+    return sa_copy_out_dense(ix, out_host);
 }
 
 extern "C" int sa_termfreqs(sa_index *ix, uint32_t term_id, uint64_t min_payload, uint64_t max_payload,
                             float *out_host) {
     SA_CHECK(ix, "index is NULL");
-    Bm25Params p = make_bm25(ix, 0, 1, 1, 0);
+    Bm25Params p = make_bm25(0, 1, 1, 0, ix->doc_lens_nonneg);
     return single_term(ix, term_id, TERM_MODE_TF, p, min_payload, max_payload, out_host);
 }
 
@@ -647,7 +606,7 @@ extern "C" int sa_score_term(sa_index *ix, uint32_t term_id, float idf, float av
         memset(out_host, 0, ix->n_docs * sizeof(float));
         return SA_OK;
     }
-    Bm25Params p = make_bm25(ix, idf, avg_doc_len, k1, b);
+    Bm25Params p = make_bm25(idf, avg_doc_len, k1, b, ix->doc_lens_nonneg);
     return single_term(ix, term_id, TERM_MODE_SCORE, p, min_payload, max_payload, out_host);
 }
 
@@ -662,7 +621,7 @@ struct BatchChunk {
     u32 n_term = 0, n_phrase = 0;
     u32 term0 = 0, phrase0 = 0;     // offsets into the batch-wide TermQuery / PhraseQuery arrays
     Bm25Params params;
-    u32 phrase_chunks = 1;          // doc-range chunks per phrase query
+    DocChunks phrase_chunks{};      // doc ranges of every phrase query
     u64 arena_words = 64;
     // phrase queries by regime (indices relative to phrase0, stored at B.d_sel + sel0: search first, then conjunction)
     u32 sel0 = 0, n_search = 0, n_conj = 0;
@@ -690,58 +649,6 @@ struct BatchState {
     DevBuf d_missing;                         // phrase_missing on the device (batch_summary_kernel)
 };
 
-static TermQuery make_term_query(const sa_index *ix, u32 t, float idf) {
-    TermQuery tq;
-    memset(&tq, 0, sizeof(tq));
-    tq.word_off = t == SA_NO_TERM ? 0 : ix->h_off[t];
-    tq.n_words = t == SA_NO_TERM ? 0 : ix->h_len[t];
-    tq.dir_off = t == SA_NO_TERM ? SA_NO_DIR : ix->h_dir_off[t];
-    tq.rec_off = (t == SA_NO_TERM || ix->h_rec_off.empty()) ? SA_NO_DIR : ix->h_rec_off[t];
-    tq.idf = idf;
-    return tq;
-}
-
-Bm25Params sa_make_bm25(const sa_index *ix, float idf, float avg_doc_len, float k1, float b) { return make_bm25(ix, idf, avg_doc_len, k1, b); }
-TermQuery sa_make_term_query(const sa_index *ix, u32 term_id, float idf) { return make_term_query(ix, term_id, idf); }
-
-static u32 n_tiles_of(const sa_index *ix) { return (u32)((ix->n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS); }
-
-static size_t cand_bytes(const sa_index *ix, u32 Q, u32 slots) {
-    return (size_t)Q * n_tiles_of(ix) * ((size_t)slots * sizeof(u64) + 2 * sizeof(u32)) + 64;
-}
-
-static TopkCtx make_topk_ctx(sa_index *ix, u32 Q, u32 slots, u32 k, u32 *d_overflow) {
-    const u32 T = n_tiles_of(ix);
-    TopkCtx t;
-    t.tile_cand = ix->cand.as<u64>();
-    t.tile_cnt = (u32 *)(t.tile_cand + (u64)Q * T * slots);
-    t.tile_max = t.tile_cnt + (u64)Q * T;
-    t.overflow = d_overflow;
-    t.n_tiles = T;
-    t.slots = slots;
-    t.k = k;
-    return t;
-}
-
-static TermBatchArgs make_term_args(sa_index *ix, const TermQuery *d_queries, const Bm25Params &p, const TopkCtx &t) {
-    TermBatchArgs a;
-    memset(&a, 0, sizeof(a));
-    a.words = ix->d_words;
-    a.doc_lens = ix->d_doc_lens;
-    a.n_docs = ix->n_docs;
-    a.doc_base = ix->doc_base;
-    a.queries = d_queries;
-    a.out = ix->dense.as<float>();
-    a.out_stride = padded_docs(ix->n_docs);
-    a.bm25 = p;
-    a.min_payload = 0;
-    a.max_payload = SA_ALL_BITS;
-    a.filter = 0;
-    a.mode = TERM_MODE_SCORE;
-    a.topk = t;
-    return a;
-}
-
 int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *term_starts,
                            const float *idf, uint32_t n_queries, uint32_t slop,
                            float avg_doc_len, float k1, float b, uint32_t k) {
@@ -764,7 +671,7 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
     int rc;
     if ((rc = ix->topk_out.reserve(std::max<size_t>(((size_t)n_queries * k + SA_BATCH_TAIL) * sizeof(u64), 256)))) return rc;
     if (n_queries == 0) { B.ready = true; return SA_OK; }
-    const u64 stride = padded_docs(std::max<u64>(ix->n_docs, 1));
+    const u64 stride = sa_padded_docs(std::max<u64>(ix->n_docs, 1));
     // chunk so the dense score vectors of one chunk stay within ~4 GB of HBM
     u32 chunk = (u32)std::max<u64>(1, std::min<u64>(n_queries, (4ull << 30) / (stride * sizeof(float))));
     B.chunk = std::min<u32>(chunk, 65535);
@@ -777,51 +684,29 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
         C.row0 = (u32)B.row_query.size();
         C.term0 = (u32)B.tqs.size();
         C.phrase0 = (u32)B.pqs.size();
-        C.params = make_bm25(ix, 1.0f, avg_doc_len, k1, b);
+        C.params = make_bm25(1.0f, avg_doc_len, k1, b, ix->doc_lens_nonneg);
         SpanPlan plan;
         for (int pass = 0; pass < 2; pass++) {               // term queries first, then phrases
             for (u32 q = q0; q < q1; q++) {
                 const u32 nt = term_starts[q + 1] - term_starts[q];
                 SA_CHECK(nt >= 1 && nt <= SA_MAX_PHRASE_TERMS, "query %u: bad number of terms", q);
                 const u32 *tids = terms + term_starts[q];
-                for (u32 i = 0; i < nt; i++)
-                    SA_CHECK(tids[i] == SA_NO_TERM || tids[i] < ix->n_terms, "term id %u out of range", tids[i]);
+                u64 offs[SA_MAX_PHRASE_TERMS], lens[SA_MAX_PHRASE_TERMS], dirs[SA_MAX_PHRASE_TERMS];
+                bool missing, literal;
+                if ((rc = sa_resolve_terms(ix, tids, nt, offs, lens, dirs, &missing, &literal))) return rc;
                 if ((nt == 1) != (pass == 0)) continue;
-                if (!make_bm25(ix, idf[q], avg_doc_len, k1, b).sparse_ok) C.params.sparse_ok = 0;
+                if (!make_bm25(idf[q], avg_doc_len, k1, b, ix->doc_lens_nonneg).sparse_ok) C.params.sparse_ok = 0;
                 B.row_query.push_back(q);
                 if (nt == 1) {
                     B.tqs.push_back(make_term_query(ix, tids[0], idf[q]));
                     B.term_query.push_back(q);
                 } else if (slop > 0) {
                     // phrase with slop: span search (spans.py:171-187) on the index's own lists
-                    u64 offs[SA_MAX_PHRASE_TERMS], lens[SA_MAX_PHRASE_TERMS], dirs[SA_MAX_PHRASE_TERMS];
-                    bool missing = false, literal = true;
-                    for (u32 i = 0; i < nt; i++)
-                        if (tids[i] == SA_NO_TERM || ix->h_len[tids[i]] == 0) missing = true;
-                    for (u32 i = 0; i < nt; i++) {
-                        offs[i] = missing ? 0 : ix->h_off[tids[i]];
-                        lens[i] = missing ? 0 : ix->h_len[tids[i]];
-                        dirs[i] = missing ? SA_NO_DIR : ix->h_dir_off[tids[i]];
-                        literal = literal && !missing && ix->h_first0[tids[i]];
-                    }
                     sa_span_plan_add(plan, offs, lens, dirs, nt, slop, idf[q], literal, missing ? 0 : ix->n_docs);
                     B.span_idf.push_back(idf[q]);
                     B.phrase_query.push_back(q);
                 } else {
-                    PhraseQuery pq;
-                    memset(&pq, 0, sizeof(pq));
-                    pq.n_terms = nt;
-                    pq.idf = idf[q];
-                    u32 missing = 0;
-                    for (u32 i = 0; i < nt; i++) {
-                        if (tids[i] == SA_NO_TERM || ix->h_len[tids[i]] == 0) { missing = 1; continue; }
-                        pq.off[i] = ix->h_off[tids[i]];
-                        pq.len[i] = ix->h_len[tids[i]];
-                    }
-                    if (missing) for (u32 i = 0; i < nt; i++) pq.len[i] = 0;     // no pairs -> zeros
-                    else for (u32 i = 0; i < nt; i++)
-                        if (ix->h_dir_off[tids[i]] != SA_NO_DIR) pq.dir_plus1[i] = ix->h_dir_off[tids[i]] + 1;
-                    sa_phrase_plan(pq, tids);
+                    PhraseQuery pq = make_phrase_query(tids, nt, offs, lens, dirs, idf[q], missing);
                     pq.use_conj = !missing && sa_phrase_use_conjunction(pq, ix->n_docs);
                     B.pqs.push_back(pq);
                     B.phrase_query.push_back(q);
@@ -846,10 +731,10 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
             C.n_search = (u32)B.sel.size() - C.sel0;
             for (u32 i = 0; i < C.n_phrase; i++) if (B.pqs[C.phrase0 + i].use_conj) B.sel.push_back(i);
             C.n_conj = C.n_phrase - C.n_search;
-            u64 want = std::max<u64>(1, (u64)ix->num_sms * 16 / std::max<u32>(C.n_search, 1));
-            C.phrase_chunks = sa_phrase_chunks(ix, (u32)std::max<u64>(1, std::min<u64>(want, std::max<u64>(1, ix->n_docs / 512))));
+            C.phrase_chunks = phrase_doc_chunks(ix, C.n_search, 16);
             for (u32 i = 0; i < C.n_phrase; i++)                     // only the search regime bump-allocates
-                if (!B.pqs[C.phrase0 + i].use_conj) C.arena_words += sa_phrase_arena_words(B.pqs[C.phrase0 + i], C.phrase_chunks);
+                if (!B.pqs[C.phrase0 + i].use_conj)
+                    C.arena_words += sa_phrase_arena_words(B.pqs[C.phrase0 + i], C.phrase_chunks.n_chunks);
             max_arena = std::max(max_arena, C.arena_words);
         }
         B.chunks.push_back(C);
@@ -857,7 +742,7 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
     SA_CHECK(B.chunks.empty() || B.chunks[0].params.sparse_ok || (B.pqs.empty() && n_span == 0),
              "phrase queries in a batch need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite idf)");
     if ((rc = ix->dense.reserve((size_t)B.chunk * stride * sizeof(float)))) return rc;
-    if ((rc = ix->cand.reserve(cand_bytes(ix, B.chunk, B.slots)))) return rc;
+    if ((rc = ix->cand.reserve(cand_bytes(sa_n_tiles(ix->n_docs), B.chunk, B.slots)))) return rc;
     if ((rc = B.d_tq.reserve(std::max<size_t>(B.tqs.size() * sizeof(TermQuery), 64)))) return rc;
     if ((rc = B.d_pq.reserve(std::max<size_t>(B.pqs.size() * sizeof(PhraseQuery), 64)))) return rc;
     if ((rc = B.d_row_query.reserve((size_t)n_queries * sizeof(u32)))) return rc;
@@ -948,7 +833,7 @@ int sa_batch_execute_locked(sa_index *ix) {
         SA_CUDA(cudaMemsetAsync(d_keys, 0, ((size_t)B.nq * B.k + SA_BATCH_TAIL) * sizeof(u64), ix->stream));
         return SA_OK;
     }
-    const u64 stride = padded_docs(ix->n_docs);
+    const u64 stride = sa_padded_docs(ix->n_docs);
     u32 *d_ovf = B.d_meta.as<u32>();
     SA_CUDA(cudaMemsetAsync(d_ovf, 0, (size_t)B.nq * sizeof(u32), ix->stream));
     if (!B.pqs.empty())
@@ -957,7 +842,7 @@ int sa_batch_execute_locked(sa_index *ix) {
     size_t chunk_i = 0;
     for (const BatchChunk &C : B.chunks) {
         const u32 Q = C.n_term + C.n_phrase;
-        TopkCtx t = make_topk_ctx(ix, Q, B.slots, B.k, d_ovf + C.row0);
+        TopkCtx t = make_topk_ctx(ix->cand.p, sa_n_tiles(ix->n_docs), Q, B.slots, B.k, d_ovf + C.row0);
         if (C.n_term) {
             TermBatchArgs a = make_term_args(ix, B.d_tq.as<TermQuery>() + C.term0, C.params, t);
             if ((rc = launch_term_batch(ix, a, C.n_term))) return rc;
@@ -1000,12 +885,13 @@ int sa_batch_execute_locked(sa_index *ix) {
 // same-term speculation was wrong.  Uses a slot per doc of the tile -- cannot overflow.
 static int redo_query(sa_index *ix, BatchState &B, bool is_phrase, u32 idx, u32 q, const SpanQuery *sq = nullptr) {
     int rc;
-    const u64 stride = padded_docs(ix->n_docs);
-    if ((rc = ix->cand.reserve(cand_bytes(ix, 1, SA_TILE_DOCS)))) return rc;
+    const u64 stride = sa_padded_docs(ix->n_docs);
+    const u32 n_tiles = sa_n_tiles(ix->n_docs);
+    if ((rc = ix->cand.reserve(cand_bytes(n_tiles, 1, SA_TILE_DOCS)))) return rc;
     SA_CUDA(cudaMemsetAsync(B.d_meta.p, 0, sizeof(u32), ix->stream));
-    TopkCtx t = make_topk_ctx(ix, 1, SA_TILE_DOCS, B.k, B.d_meta.as<u32>());
+    TopkCtx t = make_topk_ctx(ix->cand.p, n_tiles, 1, SA_TILE_DOCS, B.k, B.d_meta.as<u32>());
     if (!is_phrase) {
-        Bm25Params p = make_bm25(ix, B.tqs[idx].idf, B.avg_doc_len, B.k1, B.b);
+        Bm25Params p = make_bm25(B.tqs[idx].idf, B.avg_doc_len, B.k1, B.b, ix->doc_lens_nonneg);
         TermBatchArgs a = make_term_args(ix, B.d_tq.as<TermQuery>() + idx, p, t);
         if ((rc = launch_term_batch(ix, a, 1))) return rc;
     } else if (sq) {
@@ -1014,11 +900,11 @@ static int redo_query(sa_index *ix, BatchState &B, bool is_phrase, u32 idx, u32 
         SA_CUDA(cudaMemcpyAsync(B.d_sidf.p, &sq->idf, sizeof(float), cudaMemcpyHostToDevice, ix->stream));
         if ((rc = launch_dense_topk_tiles(ix, ix->dense.as<float>(), stride, 0, 1, t, B.d_sidf.as<float>()))) return rc;
     } else {
-        Bm25Params p = make_bm25(ix, B.pqs[idx].idf, B.avg_doc_len, B.k1, B.b);
+        Bm25Params p = make_bm25(B.pqs[idx].idf, B.avg_doc_len, B.k1, B.b, ix->doc_lens_nonneg);
         std::vector<PhraseQuery> one(1, B.pqs[idx]);
         PhraseDump nodump;
         memset(&nodump, 0, sizeof(nodump));
-        if ((rc = sa_phrase_run_sync(ix, one, ix->d_words, 1, p, 0, nodump, false))) return rc;   // loops until the guess holds
+        if ((rc = sa_phrase_run_sync(ix, one, ix->d_words, 1, p, nodump, false))) return rc;   // loops until the guess holds
         B.pqs[idx] = one[0];
         if ((rc = launch_dense_topk_tiles(ix, ix->dense.as<float>(), stride, 0, 1, t, nullptr))) return rc;
     }
@@ -1069,7 +955,7 @@ int sa_batch_fix_overflow_locked(sa_index *ix, u32 *n_redone) {
     for (const Redo &r : redo)
         if ((rc = redo_query(ix, B, r.phrase, r.idx, r.q, r.sq))) return rc;
     // the repair buffers are larger than the batch's: restore the normal ones and descriptors
-    if ((rc = ix->cand.reserve(cand_bytes(ix, B.chunk, B.slots)))) return rc;
+    if ((rc = ix->cand.reserve(cand_bytes(sa_n_tiles(ix->n_docs), B.chunk, B.slots)))) return rc;
     SA_CUDA(cudaMemcpyAsync(B.d_row_query.p, B.row_query.data(), (size_t)B.nq * sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
     if (!B.pqs.empty())
         SA_CUDA(cudaMemcpyAsync(B.d_pq.p, B.pqs.data(), B.pqs.size() * sizeof(PhraseQuery), cudaMemcpyHostToDevice, ix->stream));

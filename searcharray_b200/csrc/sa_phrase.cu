@@ -29,14 +29,8 @@
 #include "sa_span.cuh"
 #include "sa_term.cuh"
 
-int sa_filter_terms(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, bool use_rows,
-                    u64 pay_lo, u64 pay_hi, bool use_payload, std::vector<u64> &offs, std::vector<u64> &lens);
-int sa_gather_rows(sa_index *ix, const float *d_dense, float *out_host);
-
 #define PT SA_PHRASE_THREADS
 #define PW_SUB_DOCS (SA_TILE_DOCS / (SA_PHRASE_THREADS / 32))   // docs of a tile that one warp of the conjunction regime owns (1,024)
-
-static u64 docs_per_chunk_of(const sa_index *ix, u32 n_chunks);
 
 struct Elem {
     u64 w0, w1;
@@ -726,9 +720,8 @@ int launch_phrase(sa_index *ix, const PhraseArgs &a, u32 n_queries) {
 // conjunction regime: one CTA per (query, tile), like the term scan
 static int launch_phrase_tile(sa_index *ix, const PhraseArgs &a, u32 n_queries) {
     if (n_queries == 0 || a.n_docs == 0) return SA_OK;
-    const unsigned n_tiles = (unsigned)((a.n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS);
     KernelTimer t(ix, 2);
-    phrase_tile_kernel<<<dim3(n_queries, n_tiles), PT, 0, ix->stream>>>(a);
+    phrase_tile_kernel<<<dim3(n_queries, sa_n_tiles(a.n_docs)), PT, 0, ix->stream>>>(a);
     SA_CUDA(cudaGetLastError());
     t.stop();
     ix->stats.phrase_kernel_launches++;
@@ -771,8 +764,6 @@ __global__ void bm25_dense_kernel(float *__restrict__ tf, const float *__restric
     if (i < n) tf[i] = bm25_one(tf[i], dl[i], p);
 }
 
-static u64 padded(u64 n_docs) { return (n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS * SA_TILE_DOCS; }
-
 // direction / speculation plan exactly as compute_phrase_freqs picks it (middle_out.py:154-168)
 void sa_phrase_plan(PhraseQuery &pq, const u32 *term_ids) {
     const u32 n = pq.n_terms;
@@ -793,6 +784,21 @@ void sa_phrase_plan(PhraseQuery &pq, const u32 *term_ids) {
     }
 }
 
+PhraseQuery make_phrase_query(const u32 *term_ids, u32 n, const u64 *offs, const u64 *lens, const u64 *dirs,
+                              float idf, bool missing) {
+    PhraseQuery pq;
+    memset(&pq, 0, sizeof(pq));
+    pq.n_terms = n;
+    pq.idf = idf;
+    for (u32 i = 0; i < n; i++) {
+        pq.off[i] = offs[i];
+        pq.len[i] = missing ? 0 : lens[i];       // unknown term -> no pairs -> zeros (postings.py:705-708)
+        if (!missing && dirs && dirs[i] != SA_NO_DIR) pq.dir_plus1[i] = dirs[i] + 1;
+    }
+    sa_phrase_plan(pq, term_ids);               // after the zeroing: the plan follows the lengths
+    return pq;
+}
+
 // order in which the steps of a plan run (for verifying the speculation)
 static void step_order(const PhraseQuery &pq, std::vector<u32> &order) {
     order.clear();
@@ -807,7 +813,7 @@ static void step_order(const PhraseQuery &pq, std::vector<u32> &order) {
 
 // Launch arguments of both regimes.  The kernels write every tile of the dense rows themselves: no zero-fill pass.
 static PhraseArgs phrase_args(const sa_index *ix, const u64 *d_words, const PhraseQuery *d_pqs, PhraseStats *d_stats,
-                              float *dense_rows, u64 stride, u32 n_chunks, u64 *d_arena,
+                              float *dense_rows, u64 stride, DocChunks chunks, u64 *d_arena,
                               unsigned long long *d_arena_used, u64 arena_words, int score, const Bm25Params &p) {
     PhraseArgs a;
     memset(&a, 0, sizeof(a));
@@ -820,8 +826,8 @@ static PhraseArgs phrase_args(const sa_index *ix, const u64 *d_words, const Phra
     a.stats = d_stats;
     a.out = dense_rows;
     a.out_stride = stride;
-    a.n_chunks = n_chunks;
-    a.docs_per_chunk = docs_per_chunk_of(ix, n_chunks);
+    a.n_chunks = chunks.n_chunks;
+    a.docs_per_chunk = chunks.docs_per_chunk;
     a.arena = d_arena;
     a.arena_used = d_arena_used;
     a.arena_cap = arena_words;
@@ -833,29 +839,18 @@ static PhraseArgs phrase_args(const sa_index *ix, const u64 *d_words, const Phra
 // Runs phrase queries (already planned) into ix->dense; loops until the same-term speculation
 // of every query is confirmed.  lists may live in ix->d_words (off = absolute word offsets).
 // allow_conj: a single query on the index's own lists may take the conjunction regime; otherwise
-// every query runs in the search regime, whose pair statistics cover every pair.
+// every query runs in the search regime, whose pair statistics cover every pair.  A dump runs as one chunk.
 int sa_phrase_run_sync(sa_index *ix, std::vector<PhraseQuery> &pqs, const u64 *d_words,
-                       int score, const Bm25Params &p, u32 n_chunks_hint, PhraseDump dump, bool allow_conj) {
+                       int score, const Bm25Params &p, PhraseDump dump, bool allow_conj) {
     const u32 Q = (u32)pqs.size();
-    const u64 stride = padded(ix->n_docs);
+    const u64 stride = sa_padded_docs(ix->n_docs);
     int rc;
     if ((rc = ix->dense.reserve((size_t)Q * stride * sizeof(float)))) return rc;
     if ((rc = ix->queries.reserve((size_t)Q * sizeof(PhraseQuery)))) return rc;
     if ((rc = ix->cand_meta.reserve((size_t)Q * sizeof(PhraseStats) + 64))) return rc;
-    // scratch arena: per query <= 6 * (sum of list lengths + 2 per chunk)
-    u32 n_chunks = n_chunks_hint;
-    if (n_chunks == 0) {
-        u64 want = std::max<u64>(1, (u64)ix->num_sms * 8 / std::max<u32>(Q, 1));
-        n_chunks = (u32)std::min<u64>(want, std::max<u64>(1, ix->n_docs / 512));
-        n_chunks = std::max<u32>(n_chunks, 1);
-    }
-    n_chunks = sa_phrase_chunks(ix, n_chunks);
+    const DocChunks chunks = dump.cont ? DocChunks{1, stride} : phrase_doc_chunks(ix, Q, 8);
     u64 arena_words = 64;
-    for (auto &pq : pqs) {
-        u64 sum = 0;
-        for (u32 t = 0; t < pq.n_terms; t++) sum += pq.len[t];
-        arena_words += 6 * (sum + 2ull * n_chunks);
-    }
+    for (auto &pq : pqs) arena_words += sa_phrase_arena_words(pq, chunks.n_chunks);
     // the conjunction regime needs no bump arena
     bool conj = allow_conj && Q == 1 && d_words == ix->d_words && !dump.cont && sa_phrase_use_conjunction(pqs[0], ix->n_docs);
     const u64 full_arena_words = arena_words;
@@ -872,7 +867,7 @@ int sa_phrase_run_sync(sa_index *ix, std::vector<PhraseQuery> &pqs, const u64 *d
         SA_CUDA(cudaMemsetAsync(d_stats, 0, (size_t)Q * sizeof(PhraseStats), ix->stream));
         SA_CUDA(cudaMemsetAsync(d_used, 0, 64, ix->stream));
         PhraseArgs a = phrase_args(ix, d_words, ix->queries.as<PhraseQuery>(), d_stats, ix->dense.as<float>(), stride,
-                                   n_chunks, d_arena, d_used, arena_words, score, p);
+                                   chunks, d_arena, d_used, arena_words, score, p);
         a.dump = dump;
         if ((rc = conj ? launch_phrase_tile(ix, a, Q) : launch_phrase(ix, a, Q))) return rc;
         SA_CUDA(cudaMemcpyAsync(h_stats.data(), d_stats, (size_t)Q * sizeof(PhraseStats), cudaMemcpyDeviceToHost, ix->stream));
@@ -921,25 +916,25 @@ u64 sa_phrase_arena_words(const PhraseQuery &pq, u32 n_chunks) {
     return 6 * (sum + 2ull * n_chunks);
 }
 
+// About `ctas_per_sm` CTAs per SM over `n_queries` queries, in chunks of whole tiles: the tile count per chunk is
+// rounded up, then the tiles are spread evenly over the chunks that takes.
+DocChunks phrase_doc_chunks(const sa_index *ix, u32 n_queries, u32 ctas_per_sm) {
+    const u64 n_tiles = sa_n_tiles(ix->n_docs);
+    const u64 wanted = std::max<u64>(1, (u64)ix->num_sms * ctas_per_sm / std::max<u32>(n_queries, 1));
+    const u64 tiles_per_chunk = std::max<u64>(1, (n_tiles + wanted - 1) / wanted);
+    DocChunks c;
+    c.n_chunks = (u32)((n_tiles + tiles_per_chunk - 1) / tiles_per_chunk);
+    c.docs_per_chunk = c.n_chunks ? (n_tiles + c.n_chunks - 1) / c.n_chunks * SA_TILE_DOCS : 0;
+    return c;
+}
+
 // Asynchronous launch of already planned phrase queries living in device memory; dense rows,
 // stats and the arena counter must have been zeroed by the caller.
-// chunks are whole tiles: returns the chunk count actually used for `wanted` chunks per query
-u32 sa_phrase_chunks(const sa_index *ix, u32 wanted) {
-    const u64 n_tiles = (ix->n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS;
-    const u64 tiles_per_chunk = std::max<u64>(1, (n_tiles + std::max<u32>(wanted, 1) - 1) / std::max<u32>(wanted, 1));
-    return (u32)((n_tiles + tiles_per_chunk - 1) / tiles_per_chunk);
-}
-
-static u64 docs_per_chunk_of(const sa_index *ix, u32 n_chunks) {
-    const u64 n_tiles = (ix->n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS;
-    return ((n_tiles + n_chunks - 1) / n_chunks) * SA_TILE_DOCS;
-}
-
 int sa_phrase_enqueue(sa_index *ix, const PhraseQuery *d_pqs, PhraseStats *d_stats, u32 Q,
-                      float *dense_rows, u64 stride, u32 n_chunks, u64 *d_arena,
+                      float *dense_rows, u64 stride, DocChunks chunks, u64 *d_arena,
                       unsigned long long *d_arena_used, u64 arena_words, int score, const Bm25Params &p,
                       const TopkCtx *topk, u32 topk_row0, const PhraseSplit *split) {
-    PhraseArgs a = phrase_args(ix, ix->d_words, d_pqs, d_stats, dense_rows, stride, n_chunks, d_arena, d_arena_used,
+    PhraseArgs a = phrase_args(ix, ix->d_words, d_pqs, d_stats, dense_rows, stride, chunks, d_arena, d_arena_used,
                                arena_words, score, p);
     if (topk) a.topk = *topk;
     a.topk_row0 = topk_row0;
@@ -960,68 +955,42 @@ static int phrase_common(sa_index *ix, const uint32_t *term_ids, uint32_t n_term
     std::lock_guard<std::mutex> g(ix->mu);
     SA_CUDA(cudaSetDevice(ix->device));
     if (ix->n_docs == 0) return SA_OK;
-    bool missing = false;
-    for (u32 i = 0; i < n_terms; i++) {
-        SA_CHECK(term_ids[i] == SA_NO_TERM || term_ids[i] < ix->n_terms, "term id %u out of range", term_ids[i]);
-        if (term_ids[i] == SA_NO_TERM || ix->h_len[term_ids[i]] == 0) missing = true;
-    }
+    u64 offs[SA_MAX_PHRASE_TERMS], lens[SA_MAX_PHRASE_TERMS], dirs[SA_MAX_PHRASE_TERMS];
+    bool missing, literal;
+    int rc = sa_resolve_terms(ix, term_ids, n_terms, offs, lens, dirs, &missing, &literal);
+    if (rc) return rc;
     if (missing || (score && avg_doc_len == 0.0f)) {
         // unknown term inside a phrase -> zeros (postings.py:705-708); with tf == 0 everywhere BM25
         // still runs over all docs in the reference, which only matters for exotic parameters
         memset(out_host, 0, (ix->rows_active ? ix->n_rows : ix->n_docs) * sizeof(float));
         if (!(score && avg_doc_len != 0.0f) || ix->rows_active) return SA_OK;
     }
-    Bm25Params p;
-    p.idf = idf; p.avg_doc_len = avg_doc_len; p.k1 = k1; p.b = b; p.one_minus_b = 1 - b;
-    p.sparse_ok = (ix->doc_lens_nonneg && k1 > 0.0f && std::isfinite(k1) && b >= 0.0f && b < 1.0f &&
-                   avg_doc_len > 0.0f && std::isfinite(avg_doc_len) && std::isfinite(idf) && idf >= 0.0f &&
-                   !std::signbit(idf)) ? 1 : 0;
-    const u64 stride = padded(ix->n_docs);
-    int rc;
+    const Bm25Params p = make_bm25(idf, avg_doc_len, k1, b, ix->doc_lens_nonneg);
+    const u64 stride = sa_padded_docs(ix->n_docs);
     bool raw_counts = false;          // dense row holds raw phrase freqs that still need BM25
     const bool use_payload = !(min_payload == 0 && max_payload == SA_ALL_BITS);
     const bool rows = ix->rows_active;
     SA_CHECK(!(rows && score), "score on a sliced array: call termfreqs + bm25 (the Python layer does)");
     // term lists: the index's own, or filtered copies (sliced array / min-max posn), which is what
     // the reference runs on (middle_out.py:427-437: encoder.slice per term, then the same algorithm)
-    std::vector<u64> offs(n_terms), lens(n_terms);
     const u64 *d_lists = ix->d_words;
     if (!missing && (rows || use_payload)) {
-        if ((rc = sa_filter_terms(ix, term_ids, n_terms, rows, min_payload, max_payload, use_payload, offs, lens))) return rc;
+        std::vector<u64> f_offs, f_lens;
+        if ((rc = sa_filter_terms(ix, term_ids, n_terms, rows, min_payload, max_payload, use_payload, f_offs, f_lens))) return rc;
         d_lists = ix->filt.as<u64>();
-    } else if (!missing) {
-        for (u32 i = 0; i < n_terms; i++) { offs[i] = ix->h_off[term_ids[i]]; lens[i] = ix->h_len[term_ids[i]]; }
+        for (u32 i = 0; i < n_terms; i++) { offs[i] = f_offs[i]; lens[i] = f_lens[i]; dirs[i] = SA_NO_DIR; }
+        if (slop > 0 && (rc = sa_span_is_literal(ix, d_lists, offs, lens, n_terms, &literal))) return rc;
     }
     if (!missing && slop > 0) {
         // span search (phrase/spans.py + roaringish/spans.pyx): raw counts, BM25 afterwards
-        std::vector<u64> dirs(n_terms, SA_NO_DIR);
-        bool literal = true;
-        if (d_lists == ix->d_words) {
-            for (u32 i = 0; i < n_terms; i++) {
-                dirs[i] = ix->h_dir_off[term_ids[i]];
-                literal = literal && ix->h_first0[term_ids[i]];
-            }
-        } else if ((rc = sa_span_is_literal(ix, d_lists, offs.data(), lens.data(), n_terms, &literal))) {
-            return rc;
-        }
-        if ((rc = sa_span_run(ix, d_lists, offs.data(), lens.data(), dirs.data(), n_terms, slop, literal, nullptr))) return rc;
+        if ((rc = sa_span_run(ix, d_lists, offs, lens, dirs, n_terms, slop, literal, nullptr))) return rc;
         raw_counts = score != 0;
     } else if (!missing) {
-        std::vector<PhraseQuery> pqs(1);
-        PhraseQuery &pq = pqs[0];
-        memset(&pq, 0, sizeof(pq));
-        pq.n_terms = n_terms;
-        pq.idf = idf;
-        for (u32 i = 0; i < n_terms; i++) {
-            pq.off[i] = offs[i];
-            pq.len[i] = lens[i];
-            if (d_lists == ix->d_words && ix->h_dir_off[term_ids[i]] != SA_NO_DIR) pq.dir_plus1[i] = ix->h_dir_off[term_ids[i]] + 1;
-        }
-        sa_phrase_plan(pq, term_ids);
+        std::vector<PhraseQuery> pqs(1, make_phrase_query(term_ids, n_terms, offs, lens, dirs, idf, false));
         PhraseDump nodump;
         memset(&nodump, 0, sizeof(nodump));
         // raw counts first when BM25 must touch every doc
-        if ((rc = sa_phrase_run_sync(ix, pqs, d_lists, score && p.sparse_ok, p, 0, nodump, true))) return rc;
+        if ((rc = sa_phrase_run_sync(ix, pqs, d_lists, score && p.sparse_ok, p, nodump, true))) return rc;
         raw_counts = score && !p.sparse_ok;
     } else {
         if ((rc = ix->dense.reserve(stride * sizeof(float)))) return rc;
@@ -1034,10 +1003,7 @@ static int phrase_common(sa_index *ix, const uint32_t *term_ids, uint32_t n_term
         SA_CUDA(cudaGetLastError());
         ix->stats.total_launches++;
     }
-    if (rows) return sa_gather_rows(ix, ix->dense.as<float>(), out_host);
-    SA_CUDA(cudaMemcpyAsync(out_host, ix->dense.p, ix->n_docs * sizeof(float), cudaMemcpyDeviceToHost, ix->stream));
-    SA_CUDA(cudaStreamSynchronize(ix->stream));
-    return SA_OK;
+    return sa_copy_out_dense(ix, out_host);
 }
 
 extern "C" int sa_phrase_freqs(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, uint32_t slop,
@@ -1092,7 +1058,7 @@ extern "C" int sa_op_bigram_freqs(const uint64_t *lhs, uint64_t n_lhs, const uin
             cudaMemsetAsync(dump.n_cont, 0, 2 * sizeof(u64), ix->stream);
             Bm25Params p;
             memset(&p, 0, sizeof(p));
-            rc = sa_phrase_run_sync(ix, pqs, ix->d_words, 0, p, 1, dump, false);
+            rc = sa_phrase_run_sync(ix, pqs, ix->d_words, 0, p, dump, false);
             if (!rc) {
                 u64 n[2];
                 cudaMemcpy(n, dump.n_cont, 2 * sizeof(u64), cudaMemcpyDeviceToHost);
@@ -1150,9 +1116,7 @@ extern "C" int sa_op_bm25_score(float *tf_inout, const float *doc_lens, uint64_t
     if (cudaMalloc(&d_dl, n * sizeof(float)) != cudaSuccess) { cudaFree(d_tf); sa_set_error("cudaMalloc failed"); return SA_ERR_NOMEM; }
     cudaMemcpy(d_tf, tf_inout, n * sizeof(float), cudaMemcpyHostToDevice);
     cudaMemcpy(d_dl, doc_lens, n * sizeof(float), cudaMemcpyHostToDevice);
-    Bm25Params p;
-    p.idf = idf; p.avg_doc_len = avg_doc_len; p.k1 = k1; p.b = b; p.one_minus_b = 1 - b; p.sparse_ok = 0;
-    bm25_dense_kernel<<<(unsigned)((n + 255) / 256), 256>>>(d_tf, d_dl, n, p);
+    bm25_dense_kernel<<<(unsigned)((n + 255) / 256), 256>>>(d_tf, d_dl, n, make_bm25(idf, avg_doc_len, k1, b, false));
     cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaMemcpy(tf_inout, d_tf, n * sizeof(float), cudaMemcpyDeviceToHost);
     cudaFree(d_tf);

@@ -71,15 +71,25 @@ struct PhraseSplit {
     u32 n_conj;
 };
 
+// Doc ranges of a phrase or span launch: n_chunks per query, each docs_per_chunk docs (whole tiles) long.
+struct DocChunks {
+    u32 n_chunks;
+    u64 docs_per_chunk;
+};
+
 int launch_phrase(sa_index *ix, const PhraseArgs &a, u32 n_queries);
 void sa_phrase_plan(PhraseQuery &pq, const u32 *term_ids);
+// A planned descriptor.  missing: some term matches nothing -- every length is zeroed (the rows stay zero).
+// dirs: tile directory offsets (SA_NO_DIR = none), or NULL for lists outside the index.
+PhraseQuery make_phrase_query(const u32 *term_ids, u32 n, const u64 *offs, const u64 *lens, const u64 *dirs,
+                              float idf, bool missing);
 bool sa_phrase_guess_ok(PhraseQuery &pq, const PhraseStats &st);
 u64 sa_phrase_arena_words(const PhraseQuery &pq, u32 n_chunks);
 int sa_phrase_enqueue(sa_index *ix, const PhraseQuery *d_pqs, PhraseStats *d_stats, u32 Q,
-                      float *dense_rows, u64 stride, u32 n_chunks, u64 *d_arena,
+                      float *dense_rows, u64 stride, DocChunks chunks, u64 *d_arena,
                       unsigned long long *d_arena_used, u64 arena_words, int score, const Bm25Params &p,
                       const TopkCtx *topk, u32 topk_row0, const PhraseSplit *split);
-u32 sa_phrase_chunks(const sa_index *ix, u32 wanted);
+DocChunks phrase_doc_chunks(const sa_index *ix, u32 n_queries, u32 ctas_per_sm);
 bool sa_phrase_use_conjunction(const PhraseQuery &pq, u64 n_docs);
 int sa_phrase_run_sync(sa_index *ix, std::vector<PhraseQuery> &pqs, const u64 *d_words,
-                       int score, const Bm25Params &p, u32 n_chunks_hint, PhraseDump dump, bool allow_conj);
+                       int score, const Bm25Params &p, PhraseDump dump, bool allow_conj);

@@ -28,6 +28,7 @@
 // ballots.  Counts are accumulated per `last_key` like the reference's Counter.
 #include <algorithm>
 
+#include "sa_phrase.cuh"
 #include "sa_span.cuh"
 #include "sa_term.cuh"
 
@@ -850,7 +851,6 @@ span_tiles_kernel(const SpanArgs a) {
 }
 
 // --------------------------------------------------------------------------------- host
-static u64 padded_stride(u64 n_docs) { return (n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS * SA_TILE_DOCS; }
 static u64 align_up(u64 v, u64 a) { return (v + a - 1) / a * a; }
 
 void sa_span_plan_add(SpanPlan &plan, const u64 *offs, const u64 *lens, const u64 *dir_offs, u32 n_terms,
@@ -898,7 +898,7 @@ void sa_span_plan_add(SpanPlan &plan, const u64 *offs, const u64 *lens, const u6
         for (u32 t = 0; t < n_terms; t++) { sum += lens[t]; dirs = dirs && dir_offs[t] != SA_NO_DIR; }
         if (dirs && ratio && shortest_len * ratio > sum) {
             sq.cand_off = plan.cand_total;
-            plan.cand_total += (n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS * (SA_TILE_DOCS / 32);
+            plan.cand_total += (u64)sa_n_tiles(n_docs) * (SA_TILE_DOCS / 32);
             plan.conj.push_back((u32)plan.qs.size());
         }
     }
@@ -964,11 +964,9 @@ int sa_span_enqueue(sa_index *ix, const u64 *d_lists, const SpanPlan &plan, cons
         a.norm = ix->d_norm;
         a.topk = *topk;
         a.topk_row0 = topk_row0;
-        const u64 n_tiles = (ix->n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS;
-        const u64 want = std::max<u64>(1, (u64)ix->num_sms * 16 / Q);
-        const u64 tiles_per_chunk = std::max<u64>(1, (n_tiles + want - 1) / want);
-        a.n_chunks = (u32)((n_tiles + tiles_per_chunk - 1) / tiles_per_chunk);
-        a.docs_per_chunk = tiles_per_chunk * SA_TILE_DOCS;
+        const DocChunks chunks = phrase_doc_chunks(ix, Q, 16);
+        a.n_chunks = chunks.n_chunks;
+        a.docs_per_chunk = chunks.docs_per_chunk;
         // rows are addressed by absolute row (topk_row0 + q) in span_tiles_kernel
         a.out = dense_rows - (u64)topk_row0 * stride;
     } else {
@@ -980,8 +978,7 @@ int sa_span_enqueue(sa_index *ix, const u64 *d_lists, const SpanPlan &plan, cons
     if (!plan.conj.empty()) {
         SA_CHECK(a.tile_dir, "span conjunction prefilter needs the index's own lists");
         SA_CUDA(cudaMemcpyAsync(base + L.conj, plan.conj.data(), plan.conj.size() * sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
-        const unsigned n_tiles = (unsigned)((ix->n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS);
-        span_cand_kernel<<<dim3((unsigned)plan.conj.size(), n_tiles), 256, 0, ix->stream>>>(a);
+        span_cand_kernel<<<dim3((unsigned)plan.conj.size(), sa_n_tiles(ix->n_docs)), 256, 0, ix->stream>>>(a);
         SA_CUDA(cudaGetLastError());
         ix->stats.phrase_kernel_launches += 1;
         ix->stats.total_launches += 1;
@@ -1041,7 +1038,7 @@ int sa_span_enqueue(sa_index *ix, const u64 *d_lists, const SpanPlan &plan, cons
 // Span search of one query into ix->dense row 0 (raw counts).  Caller holds ix->mu.
 int sa_span_run(sa_index *ix, const u64 *d_lists, const u64 *offs, const u64 *lens, const u64 *dir_offs,
                 uint32_t n_terms, uint32_t slop, bool literal, u32 *n_undefined) {
-    const u64 stride = padded_stride(ix->n_docs);
+    const u64 stride = sa_padded_docs(ix->n_docs);
     int rc;
     if ((rc = ix->dense.reserve(stride * sizeof(float)))) return rc;
     SpanPlan plan;

@@ -477,15 +477,14 @@ __global__ void norm_kernel(const float *__restrict__ dl, float *__restrict__ no
 
 int sa_ensure_norm(sa_index *ix, float k1, float b, float avg_doc_len) {
     if (ix->norm_valid && ix->norm_k1 == k1 && ix->norm_b == b && ix->norm_avgdl == avg_doc_len) return SA_OK;
-    const u64 n_pad = (ix->n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS * SA_TILE_DOCS;
+    const u64 n_pad = sa_padded_docs(ix->n_docs);
     if (!ix->d_norm) {
         SA_CUDA(cudaMalloc(&ix->d_norm, std::max<u64>(n_pad, 1) * sizeof(float)));
         ix->device_bytes += n_pad * sizeof(float);
     }
-    Bm25Params p;
-    p.idf = 0; p.avg_doc_len = avg_doc_len; p.k1 = k1; p.b = b; p.one_minus_b = 1 - b; p.sparse_ok = 1;
     if (n_pad) {
-        norm_kernel<<<(unsigned)((n_pad + 255) / 256), 256, 0, ix->stream>>>(ix->d_doc_lens, ix->d_norm, ix->n_docs, n_pad, p);
+        norm_kernel<<<(unsigned)((n_pad + 255) / 256), 256, 0, ix->stream>>>(ix->d_doc_lens, ix->d_norm, ix->n_docs, n_pad,
+                                                                           make_bm25(0, avg_doc_len, k1, b, ix->doc_lens_nonneg));
         SA_CUDA(cudaGetLastError());
         ix->stats.total_launches++;
     }
@@ -516,7 +515,7 @@ int launch_term_batch(sa_index *ix, const TermBatchArgs &a_in, u32 n_queries) {
         if (rc) return rc;
         a.norm = ix->d_norm;
     }
-    const unsigned n_tiles = (unsigned)((a.n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS);
+    const unsigned n_tiles = sa_n_tiles(a.n_docs);
     static const bool env_qmajor = getenv("SA_TERM_QUERY_MAJOR") && atoi(getenv("SA_TERM_QUERY_MAJOR")) != 0;
     a.query_major = (env_qmajor || n_tiles > 65535) ? 1 : 0;
     dim3 grid = a.query_major ? dim3(n_tiles, n_queries) : dim3(n_queries, n_tiles);

@@ -1,5 +1,7 @@
 // sa_term.cuh -- kernel-side declarations shared by the term-path translation units.
 #pragma once
+#include <cmath>
+
 #include "sa_common.cuh"
 
 #define SA_TILE_DOCS 8192          // docs per CTA tile (32 KB of float32 scores)
@@ -54,8 +56,6 @@ int sa_ensure_norm(sa_index *ix, float k1, float b, float avg_doc_len);
 int launch_topk_select(sa_index *ix, const TopkCtx &t, u32 n_queries, u64 doc_base, u64 *d_out_keys,
                        const u32 *d_out_index);
 u32 sa_topk_slots(u32 k);
-Bm25Params sa_make_bm25(const sa_index *ix, float idf, float avg_doc_len, float k1, float b);
-TermQuery sa_make_term_query(const sa_index *ix, u32 term_id, float idf);
 // d_row_idf != NULL: the rows hold raw match counts; BM25 (norm table of the last sa_ensure_norm) is applied in
 // place on the way (row_idf[i] = idf of row row0 + i)
 int launch_dense_topk_tiles(sa_index *ix, float *dense, u64 stride, u32 row0, u32 n_rows, const TopkCtx &t,
@@ -75,6 +75,103 @@ int sa_batch_execute_locked(sa_index *ix);
 int sa_batch_fix_overflow_locked(sa_index *ix, u32 *n_redone);
 void sa_batch_dims(sa_index *ix, u32 *nq, u32 *k);
 void sa_unpack_keys(const u64 *keys, u64 n, uint32_t *out_docs, float *out_scores);
+int sa_filter_terms(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, bool use_rows,
+                    u64 pay_lo, u64 pay_hi, bool use_payload, std::vector<u64> &offs, std::vector<u64> &lens);
+// Dense row 0 of ix->dense to the host (the selected rows only, when a row filter is installed), synchronously.
+int sa_copy_out_dense(sa_index *ix, float *out_host);
+
+// ---- host-side query set-up shared by every entry point
+// Dense rows are padded to whole tiles.
+inline u32 sa_n_tiles(u64 n_docs) { return (u32)((n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS); }
+inline u64 sa_padded_docs(u64 n_docs) { return (u64)sa_n_tiles(n_docs) * SA_TILE_DOCS; }
+
+inline Bm25Params make_bm25(float idf, float avg_doc_len, float k1, float b, bool doc_lens_nonneg) {
+    Bm25Params p;
+    p.idf = idf;
+    p.avg_doc_len = avg_doc_len;
+    p.k1 = k1;
+    p.b = b;
+    p.one_minus_b = 1 - b;       // float arithmetic, as `cdef float one_minus_b = 1 - b` (bm25.pyx:19)
+    p.sparse_ok = (doc_lens_nonneg && k1 > 0.0f && std::isfinite(k1) && b >= 0.0f && b < 1.0f &&
+                   avg_doc_len > 0.0f && std::isfinite(avg_doc_len) && std::isfinite(idf) &&
+                   idf >= 0.0f && !std::signbit(idf)) ? 1 : 0;
+    return p;
+}
+
+// Every id is SA_NO_TERM or a term of the index.
+inline int sa_check_term_ids(const sa_index *ix, const u32 *term_ids, u32 n) {
+    for (u32 i = 0; i < n; i++)
+        SA_CHECK(term_ids[i] == SA_NO_TERM || term_ids[i] < ix->n_terms, "term id %u out of range", term_ids[i]);
+    return SA_OK;
+}
+
+// The index's lists of a query's terms (offsets, lengths, tile directories).  *missing: some term is SA_NO_TERM or has
+// an empty list, so the query matches nothing; every list is then reported empty.  *literal: every list starts with a
+// word at (doc 0, block 0), the span search's replayed corner (SpanQuery::literal).
+inline int sa_resolve_terms(const sa_index *ix, const u32 *term_ids, u32 n, u64 *offs, u64 *lens, u64 *dirs,
+                            bool *missing, bool *literal) {
+    int rc = sa_check_term_ids(ix, term_ids, n);
+    if (rc) return rc;
+    *missing = false;
+    for (u32 i = 0; i < n; i++)
+        if (term_ids[i] == SA_NO_TERM || ix->h_len[term_ids[i]] == 0) *missing = true;
+    *literal = !*missing;
+    for (u32 i = 0; i < n; i++) {
+        offs[i] = *missing ? 0 : ix->h_off[term_ids[i]];
+        lens[i] = *missing ? 0 : ix->h_len[term_ids[i]];
+        dirs[i] = *missing ? SA_NO_DIR : ix->h_dir_off[term_ids[i]];
+        *literal = *literal && ix->h_first0[term_ids[i]];
+    }
+    return SA_OK;
+}
+
+inline TermQuery make_term_query(const sa_index *ix, u32 t, float idf) {
+    TermQuery tq;
+    memset(&tq, 0, sizeof(tq));
+    tq.word_off = t == SA_NO_TERM ? 0 : ix->h_off[t];
+    tq.n_words = t == SA_NO_TERM ? 0 : ix->h_len[t];
+    tq.dir_off = t == SA_NO_TERM ? SA_NO_DIR : ix->h_dir_off[t];
+    tq.rec_off = (t == SA_NO_TERM || ix->h_rec_off.empty()) ? SA_NO_DIR : ix->h_rec_off[t];
+    tq.idf = idf;
+    return tq;
+}
+
+// Top-k candidate buffer of Q queries: keys [Q][n_tiles][slots], then counts and maxima [Q][n_tiles] each.
+inline size_t cand_bytes(u32 n_tiles, u32 Q, u32 slots) {
+    return (size_t)Q * n_tiles * ((size_t)slots * sizeof(u64) + 2 * sizeof(u32)) + 64;
+}
+
+inline TopkCtx make_topk_ctx(void *cand, u32 n_tiles, u32 Q, u32 slots, u32 k, u32 *d_overflow) {
+    TopkCtx t;
+    t.tile_cand = (u64 *)cand;
+    t.tile_cnt = (u32 *)(t.tile_cand + (u64)Q * n_tiles * slots);
+    t.tile_max = t.tile_cnt + (u64)Q * n_tiles;
+    t.overflow = d_overflow;
+    t.n_tiles = n_tiles;
+    t.slots = slots;
+    t.k = k;
+    return t;
+}
+
+// BM25 scores of the index's own lists into ix->dense, one row per query
+inline TermBatchArgs make_term_args(sa_index *ix, const TermQuery *d_queries, const Bm25Params &p, const TopkCtx &t) {
+    TermBatchArgs a;
+    memset(&a, 0, sizeof(a));
+    a.words = ix->d_words;
+    a.doc_lens = ix->d_doc_lens;
+    a.n_docs = ix->n_docs;
+    a.doc_base = ix->doc_base;
+    a.queries = d_queries;
+    a.out = ix->dense.as<float>();
+    a.out_stride = sa_padded_docs(ix->n_docs);
+    a.bm25 = p;
+    a.min_payload = 0;
+    a.max_payload = SA_ALL_BITS;
+    a.filter = 0;
+    a.mode = TERM_MODE_SCORE;
+    a.topk = t;
+    return a;
+}
 
 #ifdef __CUDACC__
 // The j-th round of "take the warp maximum, then clear it" (REDUX.MAX: one instruction per round on sm_80+).
