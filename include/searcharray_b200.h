@@ -82,6 +82,10 @@ int sa_docfreq(sa_index *index, uint32_t term_id, uint64_t *df_out);
 int sa_index_set_rows(sa_index *index, const uint64_t *rows, uint64_t n_rows);
 /* docfreq on the filtered postings (reference quirk iii: df is taken on the slice). */
 int sa_docfreq_rows(sa_index *index, uint32_t term_id, uint64_t *df_out);
+/* The same for n_terms terms in one device pass (what SearchArray.docfreq returns on the slice for each of them;
+ * PosnBitArray.docfreq on FilteredPosns, middle_out.py:521-528 and 291-317).  SA_NO_TERM -> 0; no row filter
+ * installed -> the shard's df.  Counts the docs of every list that lie in the filter; writes no filtered list. */
+int sa_docfreq_rows_batch(sa_index *index, const uint32_t *term_ids, uint32_t n_terms, uint64_t *df_out);
 
 /* ------------------------------------------------------------------ term path
  * SearchArray.termfreqs(token) (postings.py:607-638): popcount64_reduce + as_dense fused;
@@ -123,6 +127,16 @@ int sa_score_batch_topk(sa_index *index, const uint32_t *terms, const uint32_t *
                         const float *idf, uint32_t n_queries, uint32_t slop,
                         float avg_doc_len, float k1, float b, uint32_t k,
                         uint32_t *out_docs, float *out_scores);
+/* The batched top-k on a sliced array: the top k of SearchArray.score on the view (postings.py:652-680 on
+ * FilteredPosns, middle_out.py:291-317; np.argpartition as above).  Row filter installed by sa_index_set_rows;
+ * idf[q] from sa_docfreq_rows_batch's slice document frequencies; view_doc_lens = float32[n_rows], the lengths the
+ * view's BM25 uses (bm25/bm25.pyx:28-41); avg_doc_len the parent's.  Counts come from the filtered postings.
+ * out_pos = positions in the view (< n_rows, which must be < 2^32 - 1), not doc ids; order and empty slots as
+ * sa_score_batch_topk. */
+int sa_score_batch_topk_rows(sa_index *index, const uint32_t *terms, const uint32_t *term_starts,
+                             const float *idf, uint32_t n_queries, uint32_t slop, const float *view_doc_lens,
+                             float avg_doc_len, float k1, float b, uint32_t k,
+                             uint32_t *out_pos, float *out_scores);
 
 /* The same batch in three stages, so a serving loop (or the benchmark) can keep the query
  * descriptors resident and time the device work alone: upload (H2D of descriptors), execute

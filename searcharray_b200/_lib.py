@@ -42,12 +42,15 @@ SIGNATURES = {
     "sa_docfreq": (c_int, [P_void, c_u32, P_u64]),
     "sa_index_set_rows": (c_int, [P_void, P_u64, c_u64]),
     "sa_docfreq_rows": (c_int, [P_void, c_u32, P_u64]),
+    "sa_docfreq_rows_batch": (c_int, [P_void, P_u32, c_u32, P_u64]),
     "sa_termfreqs": (c_int, [P_void, c_u32, c_u64, c_u64, P_f32]),
     "sa_score_term": (c_int, [P_void, c_u32, c_f32, c_f32, c_f32, c_f32, c_u64, c_u64, P_f32]),
     "sa_phrase_freqs": (c_int, [P_void, P_u32, c_u32, c_u32, c_u64, c_u64, P_f32]),
     "sa_score_phrase": (c_int, [P_void, P_u32, c_u32, c_u32, c_f32, c_f32, c_f32, c_f32, c_u64, c_u64, P_f32]),
     "sa_score_batch_topk": (c_int, [P_void, P_u32, P_u32, P_f32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32,
                                     P_u32, P_f32]),
+    "sa_score_batch_topk_rows": (c_int, [P_void, P_u32, P_u32, P_f32, c_u32, c_u32, P_f32, c_f32, c_f32, c_f32,
+                                         c_u32, P_u32, P_f32]),
     "sa_batch_upload": (c_int, [P_void, P_u32, P_u32, P_f32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32]),
     "sa_batch_execute": (c_int, [P_void]),
     "sa_batch_download": (c_int, [P_void, P_u32, P_f32, P_u32]),

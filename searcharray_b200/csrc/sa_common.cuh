@@ -104,6 +104,7 @@ struct TermQuery {
 // ---- the index handle ---------------------------------------------------------------
 struct TimedLaunch;
 struct BatchState;
+struct ViewState;
 struct sa_index {
     int device = 0;
     int num_sms = SA_NUM_SMS_FALLBACK;
@@ -148,6 +149,7 @@ struct sa_index {
     std::vector<struct TimedLaunch> *pending_timers = nullptr;
     std::vector<cudaEvent_t> *free_events = nullptr;
     struct BatchState *batch = nullptr;
+    struct ViewState *view = nullptr;   // buffers of sa_score_batch_topk_rows (sa_view.cu)
     sa_stats stats;
     std::mutex mu;
 

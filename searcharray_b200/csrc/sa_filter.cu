@@ -233,17 +233,109 @@ extern "C" int sa_index_set_rows(sa_index *ix, const uint64_t *rows, uint64_t n_
     return SA_OK;
 }
 
-// PosnBitArray.docfreq on FilteredPosns (quirk iii: df of the filtered postings)
-extern "C" int sa_docfreq_rows(sa_index *ix, uint32_t term_id, uint64_t *df_out) {
-    SA_CHECK(ix && df_out, "NULL argument");
-    if (term_id == SA_NO_TERM) { *df_out = 0; return SA_OK; }
-    int rc = sa_check_term_ids(ix, &term_id, 1);
+// ---- PosnBitArray.docfreq on FilteredPosns (quirk iii: df of the filtered postings) without materialising them.
+// df = the distinct docs of the term's list whose row-mask byte is set.  Terms with a tf table have one record per
+// (term, doc), so their df is the sum of mask[doc] over the records (4 bytes per doc of the list); the other terms
+// count the doc-head words of their posting list that lie in the mask (8 bytes per word).  One CTA per job, integer
+// sums only: the result does not depend on the launch geometry.
+struct DfJob {
+    u64 src_off;        // first record (d_recs) or word (d_words) of the term
+    u64 begin, end;     // records: tiles [begin, end); words: list indices [begin, end)
+    u64 dir_off;        // record directory of the term (records only)
+    u32 slot;           // output index
+    u32 recs;           // 1 = records, 0 = posting words
+};
+#define DF_TILES_PER_JOB 8
+#define DF_WORDS_PER_JOB (FILT_THREADS * 16)
+
+__global__ void __launch_bounds__(FILT_THREADS)
+docfreq_rows_kernel(const u64 *__restrict__ words, const u32 *__restrict__ recs, const u32 *__restrict__ rec_dir,
+                    const DfJob *__restrict__ jobs, const unsigned char *__restrict__ row_mask, u64 doc_base, u64 n_docs,
+                    unsigned long long *__restrict__ df) {
+    const DfJob job = jobs[blockIdx.x];
+    u32 cnt = 0;
+    if (job.recs) {
+        const u32 *__restrict__ r = recs + job.src_off;
+        const u32 *__restrict__ dir = rec_dir + job.dir_off;
+        for (u64 tile = job.begin; tile < job.end; tile++) {
+            const u32 lo = __ldg(dir + tile), hi = __ldg(dir + tile + 1);
+            const unsigned char *__restrict__ m = row_mask + tile * SA_TILE_DOCS;
+            for (u32 i = lo + threadIdx.x; i < hi; i += FILT_THREADS) cnt += m[__ldg(r + i) >> SA_REC_TF_BITS];
+        }
+    } else {
+        const u64 *__restrict__ w = words + job.src_off;
+        for (u64 i = job.begin + threadIdx.x; i < job.end; i += FILT_THREADS) {
+            const u64 doc = __ldg(w + i) >> SA_KEY_SHIFT;
+            const bool head = i == 0 || (__ldg(w + i - 1) >> SA_KEY_SHIFT) != doc;
+            if (head && doc - doc_base < n_docs) cnt += row_mask[doc - doc_base];
+        }
+    }
+    cnt = __reduce_add_sync(0xffffffffu, cnt);
+    if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(df + job.slot, (unsigned long long)cnt);
+}
+
+// Caller holds ix->mu; term ids already checked.
+static int docfreq_rows_locked(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, uint64_t *df_out) {
+    SA_CUDA(cudaSetDevice(ix->device));
+    if (!ix->rows_active) {
+        for (u32 i = 0; i < n_terms; i++) df_out[i] = term_ids[i] == SA_NO_TERM ? 0 : ix->h_df[term_ids[i]];
+        return SA_OK;
+    }
+    std::vector<DfJob> jobs;
+    const u32 n_tiles = sa_n_tiles(ix->n_docs);
+    for (u32 i = 0; i < n_terms; i++) {
+        const u32 t = term_ids[i];
+        if (t == SA_NO_TERM || ix->h_len[t] == 0) continue;
+        DfJob j;
+        j.slot = i;
+        if (ix->d_recs && ix->h_rec_off[t] != SA_NO_DIR && ix->h_dir_off[t] != SA_NO_DIR) {
+            j.recs = 1;
+            j.src_off = ix->h_rec_off[t];
+            j.dir_off = ix->h_dir_off[t];
+            for (u64 b = 0; b < n_tiles; b += DF_TILES_PER_JOB) {
+                j.begin = b;
+                j.end = std::min<u64>(n_tiles, b + DF_TILES_PER_JOB);
+                jobs.push_back(j);
+            }
+        } else {
+            j.recs = 0;
+            j.src_off = ix->h_off[t];
+            j.dir_off = 0;
+            for (u64 b = 0; b < ix->h_len[t]; b += DF_WORDS_PER_JOB) {
+                j.begin = b;
+                j.end = std::min<u64>(ix->h_len[t], b + DF_WORDS_PER_JOB);
+                jobs.push_back(j);
+            }
+        }
+    }
+    std::vector<u64> h_df(n_terms, 0);
+    if (!jobs.empty()) {
+        const size_t jobs_bytes = (jobs.size() * sizeof(DfJob) + 255) / 256 * 256;
+        int rc;
+        if ((rc = ix->misc.reserve(jobs_bytes + (size_t)n_terms * sizeof(u64)))) return rc;
+        DfJob *d_jobs = ix->misc.as<DfJob>();
+        unsigned long long *d_df = (unsigned long long *)((char *)ix->misc.p + jobs_bytes);
+        SA_CUDA(cudaMemcpyAsync(d_jobs, jobs.data(), jobs.size() * sizeof(DfJob), cudaMemcpyHostToDevice, ix->stream));
+        SA_CUDA(cudaMemsetAsync(d_df, 0, (size_t)n_terms * sizeof(u64), ix->stream));
+        docfreq_rows_kernel<<<(unsigned)jobs.size(), FILT_THREADS, 0, ix->stream>>>(ix->d_words, ix->d_recs, ix->d_rec_dir, d_jobs,
+                                                                               ix->d_row_mask, ix->doc_base, ix->n_docs, d_df);
+        SA_CUDA(cudaGetLastError());
+        ix->stats.total_launches++;
+        SA_CUDA(cudaMemcpyAsync(h_df.data(), d_df, (size_t)n_terms * sizeof(u64), cudaMemcpyDeviceToHost, ix->stream));
+        SA_CUDA(cudaStreamSynchronize(ix->stream));
+    }
+    memcpy(df_out, h_df.data(), (size_t)n_terms * sizeof(u64));
+    return SA_OK;
+}
+
+extern "C" int sa_docfreq_rows_batch(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, uint64_t *df_out) {
+    SA_CHECK(ix && (n_terms == 0 || (term_ids && df_out)), "NULL argument");
+    int rc = sa_check_term_ids(ix, term_ids, n_terms);
     if (rc) return rc;
     std::lock_guard<std::mutex> g(ix->mu);
-    SA_CUDA(cudaSetDevice(ix->device));
-    if (!ix->rows_active) { *df_out = ix->h_df[term_id]; return SA_OK; }
-    std::vector<u64> offs, lens, dfs;
-    if ((rc = sa_filter_terms_mask(ix, &term_id, 1, ix->d_row_mask, 0, SA_ALL_BITS, false, offs, lens, &dfs))) return rc;
-    *df_out = dfs[0];
-    return SA_OK;
+    return docfreq_rows_locked(ix, term_ids, n_terms, df_out);
+}
+
+extern "C" int sa_docfreq_rows(sa_index *ix, uint32_t term_id, uint64_t *df_out) {
+    return sa_docfreq_rows_batch(ix, &term_id, 1, df_out);
 }

@@ -488,6 +488,7 @@ extern "C" int sa_index_destroy(sa_index *ix) {
     ix->misc.release();
     ix->gather.release();
     sa_free_batch(ix);
+    sa_free_view(ix);
     if (ix->pending_timers) {
         for (auto &t : *ix->pending_timers) { cudaEventDestroy(t.e0); cudaEventDestroy(t.e1); }
         delete ix->pending_timers;

@@ -77,6 +77,10 @@ void sa_batch_dims(sa_index *ix, u32 *nq, u32 *k);
 void sa_unpack_keys(const u64 *keys, u64 n, uint32_t *out_docs, float *out_scores);
 int sa_filter_terms(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, bool use_rows,
                     u64 pay_lo, u64 pay_hi, bool use_payload, std::vector<u64> &offs, std::vector<u64> &lens);
+int sa_filter_terms_mask(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, const unsigned char *d_mask,
+                         u64 pay_lo, u64 pay_hi, bool use_payload, std::vector<u64> &offs, std::vector<u64> &lens,
+                         std::vector<u64> *df_out);
+void sa_free_view(sa_index *ix);     // sa_view.cu
 // Dense row 0 of ix->dense to the host (the selected rows only, when a row filter is installed), synchronously.
 int sa_copy_out_dense(sa_index *ix, float *out_host);
 

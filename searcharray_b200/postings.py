@@ -423,6 +423,12 @@ class SearchArray(ExtensionArray):
             return self.doc_lens
         return self.doc_lens[self.rows.astype(np.int64)]
 
+    def _view_bm25_doc_lens(self) -> np.ndarray:
+        """The doc lengths BM25 uses on this view: the stepped-slice quirk's (see __getitem__) or the view's own.
+        Shared by .score and .search_topk so that the two rank with the same lengths."""
+        dl = getattr(self, "_bm25_doc_lens", None)
+        return np.ascontiguousarray(self.doclengths()) if dl is None else dl
+
     def score(self, token: Union[str, List[str]], similarity: Similarity = default_bm25, slop: int = 0,
               min_posn: Optional[int] = None, max_posn: Optional[int] = None) -> np.ndarray:
         """Score each doc (reference postings.py:652-680).  With a bm25_similarity the whole
@@ -442,11 +448,9 @@ class SearchArray(ExtensionArray):
             tfs = self.termfreqs(token, min_posn=min_posn, max_posn=max_posn, slop=slop)
             if self.avg_doc_length == 0:
                 return np.zeros_like(tfs)
-            dl = getattr(self, "_bm25_doc_lens", None)
-            if dl is None:
-                dl = np.ascontiguousarray(self.doclengths())
             idf = compute_idf(self.corpus_size, all_dfs)
-            return ops.bm25_score(tfs, dl, self.avg_doc_length, idf, similarity.k1, similarity.b, device=self.device)
+            return ops.bm25_score(tfs, self._view_bm25_doc_lens(), self.avg_doc_length, idf, similarity.k1,
+                                  similarity.b, device=self.device)
         out = _pool.empty_f32(len(self))
         if self.avg_doc_length == 0:
             out[:] = 0
@@ -483,11 +487,16 @@ class SearchArray(ExtensionArray):
     # -------------------------------------------------- batched, HBM-resident path
     def search_topk(self, queries, k=10, similarity: Bm25Similarity = default_bm25, slop=0):
         """queries: list of str (term) or list[str] (phrase).  Returns (docs uint32[Q,k],
-        scores float32[Q,k]); scores never leave HBM except the top-k (sa_score_batch_topk).
-        Defined on unsliced arrays only: a sliced view scores through .score() (FilteredPosns semantics)."""
+        scores float32[Q,k]): per query the k best scores > 0, by score descending then id ascending, empty
+        slots NO_DOC / 0.  Scores never leave HBM except the top-k (sa_score_batch_topk).
+
+        On a view (arr[mask], arr[a:b], arr[::s], arr.take(idx), a view of a view) the result is the top k of
+        `view.score(q, similarity=similarity, slop=slop)`, and the returned ids are POSITIONS IN THE VIEW
+        (0 .. len(view) - 1, the index space of view.score), not the parent's doc ids.  Views of a sharded array
+        (built with a comm or a global_df) raise ValueError: their document frequencies would need a sum over
+        the ranks."""
         if self.rows is not None:
-            raise ValueError("search_topk on a sliced SearchArray is not supported: the batched path scores the "
-                             "whole shard; use .score() on the slice")
+            return self._search_topk_view(queries, k, similarity, slop)
         terms, starts, idfs = [], [0], []
         for q in queries:
             toks = [q] if isinstance(q, str) else list(q)
@@ -505,4 +514,41 @@ class SearchArray(ExtensionArray):
                                                       _lib.p_f32(idfs), len(queries), int(slop),
                                                       self.avg_doc_length, similarity.k1, similarity.b, k,
                                                       _lib.p_u32(docs), _lib.p_f32(scores)))
+        return docs, scores
+
+    def _search_topk_view(self, queries, k, similarity, slop):
+        """search_topk on a view: the slice's dfs of every distinct token in one device pass, idf per query as
+        .score computes it, then the batched top-k over the view's positions (sa_score_batch_topk_rows)."""
+        if self.comm is not None or self.global_df is not None:
+            raise ValueError("search_topk on a view of a sharded SearchArray is not supported: the slice's document "
+                             "frequencies would need a sum over the ranks; use .score() on the view")
+        toks = [[q] if isinstance(q, str) else list(q) for q in queries]
+        docs = np.full((len(toks), k), _lib.NO_DOC, dtype=np.uint32)
+        scores = np.zeros((len(toks), k), dtype=np.float32)
+        if self.avg_doc_length == 0 or not toks:          # .score is all zeros there: nothing ranks
+            return docs, scores
+        ids = {t: self._term_id(t) for ts in toks for t in ts}
+        known = [t for t, tid in ids.items() if tid != _lib.NO_TERM]
+        dl = np.ascontiguousarray(self._view_bm25_doc_lens(), dtype=np.float32)
+        dev = self._device()
+        with self._shared["lock"]:
+            self._apply_rows(dev)
+            dfs = np.zeros(len(known), dtype=np.uint64)
+            if known:
+                tids = np.asarray([ids[t] for t in known], dtype=np.uint32)
+                _lib.check(_lib.lib().sa_docfreq_rows_batch(dev.handle, _lib.p_u32(tids), len(tids), _lib.p_u64(dfs)))
+            # the values .docfreq returns: np.uint64 for a known token, 0 for an unknown one
+            df = dict(zip(known, dfs))
+            terms, starts, idfs = [], [0], []
+            for ts in toks:
+                terms.extend(ids[t] for t in ts)
+                starts.append(len(terms))
+                idfs.append(compute_idf(self.corpus_size, np.asarray([df.get(t, 0) for t in ts])))
+            terms = np.asarray(terms, dtype=np.uint32)
+            starts = np.asarray(starts, dtype=np.uint32)
+            idfs = np.asarray(idfs, dtype=np.float32)
+            _lib.check(_lib.lib().sa_score_batch_topk_rows(dev.handle, _lib.p_u32(terms), _lib.p_u32(starts),
+                                                           _lib.p_f32(idfs), len(toks), int(slop), _lib.p_f32(dl),
+                                                           self.avg_doc_length, similarity.k1, similarity.b, k,
+                                                           _lib.p_u32(docs), _lib.p_f32(scores)))
         return docs, scores
