@@ -137,6 +137,18 @@ int sa_score_batch_topk_rows(sa_index *index, const uint32_t *terms, const uint3
                              const float *idf, uint32_t n_queries, uint32_t slop, const float *view_doc_lens,
                              float avg_doc_len, float k1, float b, uint32_t k,
                              uint32_t *out_pos, float *out_scores);
+/* The batched top-k under another similarity (kind = SA_SIM_*, below): the top k of SearchArray.score(q,
+ * similarity=...), i.e. of sa_op_similarity over the query's counts, on the view the installed row filter selects
+ * or, with no filter, on the whole array.  Counts as SearchArray.termfreqs (the filtered postings on a view); doc
+ * lengths the index's own (gathered through the row filter: SearchArray.doclengths()); idf[q] the similarity's own
+ * float64 idf of the query's document frequencies (must be finite; unused by SA_SIM_BM25_IMPACT); avg_doc_len, k1,
+ * b the Python values (numpy's float32 promotion is applied here).  avg_doc_len == 0 -> nothing ranks, except under
+ * SA_SIM_CLASSIC.  out_scores are float64 (the float32 impact scores widened).  Only scores > 0 rank (+inf does,
+ * NaN never); order score desc, then id asc; empty slots SA_NO_DOC / 0.  Ids: positions in the view, or GLOBAL doc
+ * ids (doc_base added) on an unsliced array; fewer than 2^32 - 1 of them. */
+int sa_score_batch_topk_sim(sa_index *index, int kind, const uint32_t *terms, const uint32_t *term_starts,
+                            const double *idf, uint32_t n_queries, uint32_t slop, double avg_doc_len,
+                            double k1, double b, uint32_t k, uint32_t *out_ids, double *out_scores);
 
 /* The same batch in three stages, so a serving loop (or the benchmark) can keep the query
  * descriptors resident and time the device work alone: upload (H2D of descriptors), execute

@@ -1,27 +1,19 @@
 // sa_similarity.cu -- the reference's non-default similarities as device kernels (SURVEY.md 8f-3).
 //
 // Replaces the numpy closures of searcharray/similarity.py:41-89 (bm25_impact,
-// bm25_legacy_similarity, classic_similarity).  What parity depends on is numpy's dtype promotion:
-// the Python-float parameters become float32 next to the float32 arrays (k1, b, `1 - b` and `k1 + 1`
-// are computed in double and THEN rounded), the idf scalars are float64 and make the final product
-// float64 (legacy, classic).  Every operation is individually rounded (-fmad=false, *_rn).
+// bm25_legacy_similarity, classic_similarity).  The formulas, and how they reproduce numpy's
+// dtype promotion, are in sa_sim.cuh (shared with the batched top-k of sa_view.cu).
 #include <cmath>
 
-#include "sa_common.cuh"
+#include "sa_sim.cuh"
 
 struct SimArgs {
     const float *tf, *dl;
     u64 n;
-    float k1, b, one_minus_b, k1_plus_1, avgdl;
+    SimParams p;
     double idf;
     void *out;
 };
-
-__device__ __forceinline__ float saturation_denominator(float tf, float dl, const SimArgs &a) {
-    // tf + k1 * (1 - b + b * doc_lens / avg_doc_lens), left to right as numpy evaluates it
-    const float ratio = __fdiv_rn(__fmul_rn(a.b, dl), a.avgdl);
-    return __fadd_rn(tf, __fmul_rn(a.k1, __fadd_rn(a.one_minus_b, ratio)));
-}
 
 template <int KIND>
 __global__ void __launch_bounds__(256) similarity_kernel(const SimArgs a) {
@@ -29,13 +21,11 @@ __global__ void __launch_bounds__(256) similarity_kernel(const SimArgs a) {
     if (i >= a.n) return;
     const float tf = a.tf[i], dl = a.dl[i];
     if (KIND == SA_SIM_BM25_IMPACT) {
-        ((float *)a.out)[i] = __fdiv_rn(tf, saturation_denominator(tf, dl, a));
+        ((float *)a.out)[i] = sim_impact(tf, dl, a.p);
     } else if (KIND == SA_SIM_BM25_LEGACY) {
-        const float sat = __fdiv_rn(__fmul_rn(tf, a.k1_plus_1), saturation_denominator(tf, dl, a));
-        ((double *)a.out)[i] = __dmul_rn(a.idf, (double)sat);
+        ((double *)a.out)[i] = sim_legacy(a.idf, sim_legacy_sat(tf, dl, a.p));
     } else {
-        const float length_norm = __fdiv_rn(1.0f, __fsqrt_rn(dl));
-        ((double *)a.out)[i] = __dmul_rn(__dmul_rn(a.idf, (double)__fsqrt_rn(tf)), (double)length_norm);
+        ((double *)a.out)[i] = sim_classic(a.idf, tf, dl);
     }
 }
 
@@ -56,10 +46,7 @@ extern "C" int sa_op_similarity(int kind, const float *term_freqs, const float *
     if (e == cudaSuccess) {
         SimArgs a;
         a.tf = d_tf; a.dl = d_dl; a.n = n;
-        a.k1 = (float)k1; a.b = (float)b;
-        a.one_minus_b = (float)(1 - b);          // Python: `1 - b` in double, rounded when it meets the array
-        a.k1_plus_1 = (float)(k1 + 1);
-        a.avgdl = (float)avg_doc_len;
+        a.p = make_sim_params(avg_doc_len, k1, b);
         a.idf = idf;
         a.out = d_out;
         const unsigned blocks = (unsigned)((n + 255) / 256);

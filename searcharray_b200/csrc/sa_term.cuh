@@ -56,6 +56,10 @@ int sa_ensure_norm(sa_index *ix, float k1, float b, float avg_doc_len);
 int launch_topk_select(sa_index *ix, const TopkCtx &t, u32 n_queries, u64 doc_base, u64 *d_out_keys,
                        const u32 *d_out_index);
 u32 sa_topk_slots(u32 k);
+// topk_select_kernel for candidates whose key carries a float32 proxy of a float64 score (d_tile_d: the score bits,
+// slot for slot); exact in float64, see sa_topk.cu.  d_out_scores[out_index[q] * k + i] = the float64 scores.
+int launch_topk_select_f64(sa_index *ix, const TopkCtx &t, const u64 *d_tile_d, u32 n_queries, u64 doc_base,
+                           u64 *d_out_keys, double *d_out_scores, const u32 *d_out_index);
 // d_row_idf != NULL: the rows hold raw match counts; BM25 (norm table of the last sa_ensure_norm) is applied in
 // place on the way (row_idf[i] = idf of row row0 + i)
 int launch_dense_topk_tiles(sa_index *ix, float *dense, u64 stride, u32 row0, u32 n_rows, const TopkCtx &t,

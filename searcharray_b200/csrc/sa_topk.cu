@@ -174,6 +174,106 @@ topk_select_kernel(TopkCtx t, u64 doc_base, u64 *__restrict__ out_keys, const u3
     }
 }
 
+// k-th largest, with multiplicity, of the BITS-bit keys `visit` yields (0 when it yields fewer than k): an 8-bit
+// radix select from the most significant digit, as in topk_select_kernel.  All threads call; all get the result.
+template <typename K, int BITS, typename V>
+__device__ K radix_kth_largest(u32 k, u32 *s_hist, K *s_prefix, u32 *s_krem, V visit) {
+    if (threadIdx.x == 0) { *s_prefix = 0; *s_krem = k; }
+    __syncthreads();
+    for (int shift = BITS - 8; shift >= 0; shift -= 8) {
+        for (u32 i = threadIdx.x; i < 256; i += blockDim.x) s_hist[i] = 0;
+        __syncthreads();
+        const K prefix = *s_prefix;
+        visit([&](K key) {
+            if (shift == BITS - 8 || (key >> (shift + 8)) == (prefix >> (shift + 8)))
+                atomicAdd(&s_hist[(u32)(key >> shift) & 255u], 1u);
+        });
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            u32 rem = *s_krem;
+            int b;
+            radix_pick(s_hist, rem, b);
+            *s_krem = rem;
+            *s_prefix = prefix | ((K)(u32)b << shift);
+        }
+        __syncthreads();
+    }
+    return *s_prefix;
+}
+
+typedef unsigned __int128 u128;
+
+// The exact top k of a query whose candidates carry a float32 PROXY of a float64 score (classic similarity,
+// sim_tile_kernel): the candidate key is proxy_bits << 32 | ~position as usual and tile_d[] holds the float64 score
+// bits of the same slot.  The proxy is monotone but not injective, so distinct scores can share it; the tiles kept
+// EVERY position at or above their bound (no tie cut), hence every position whose proxy is >= the k-th largest
+// proxy P_k is a candidate, and the true top k lies among them (a position below P_k has k better ones).
+//   A. thr = k-th largest tile maximum (<= P_k: the maxima belong to distinct positions);
+//   B. over the candidates with proxy >= thr, a radix select of the 96-bit key (score bits, ~position) -- exact
+//      float64 order, ties to the lower position -- gives the k-th key; the keys >= it are the result, ranked.
+// Result: out_keys as topk_select_kernel writes them (ids only) and out_scores the float64 scores; empty = 0 / 0.
+__global__ void __launch_bounds__(SEL_THREADS)
+topk_select_f64_kernel(TopkCtx t, const u64 *__restrict__ tile_d, u64 doc_base, u64 *__restrict__ out_keys,
+                       double *__restrict__ out_scores, const u32 *__restrict__ out_index) {
+    __shared__ u32 s_hist[256];
+    __shared__ u32 s_krem, s_n;
+    __shared__ u32 s_thr;
+    __shared__ u128 s_prefix;
+    __shared__ u128 s_win[SA_TOPK_MAX];
+    const u32 q = blockIdx.x, k = t.k, T = t.n_tiles;
+    const u32 *tmax = t.tile_max + (u64)q * T;
+    u32 thr = radix_kth_largest<u32, 32>(k, s_hist, &s_thr, &s_krem, [&](auto f) {
+        for (u32 tile = threadIdx.x; tile < T; tile += blockDim.x) f(tmax[tile]);
+    });
+    if (thr == 0) thr = 1;
+    const u64 *d = tile_d + (u64)q * T * t.slots;
+    const u64 *cand = t.tile_cand + (u64)q * T * t.slots;
+    const u32 *cnt = t.tile_cnt + (u64)q * T;
+    auto survivors = [&](auto f) {
+        for (u32 tile = threadIdx.x; tile < T; tile += blockDim.x) {
+            if (tmax[tile] < thr) continue;
+            const u64 base = (u64)tile * t.slots;
+            for (u32 j = 0; j < cnt[tile]; j++)
+                if ((u32)(cand[base + j] >> 32) >= thr) f(((u128)d[base + j] << 32) | (u32)cand[base + j]);
+        }
+    };
+    const u128 kth = radix_kth_largest<u128, 96>(k, s_hist, &s_prefix, &s_krem, survivors);
+    if (threadIdx.x == 0) s_n = 0;
+    __syncthreads();
+    survivors([&](u128 key) {                   // keys are distinct (positions are): at most k reach kth
+        if (key >= kth) {
+            const u32 slot = atomicAdd(&s_n, 1u);
+            if (slot < SA_TOPK_MAX) s_win[slot] = key;
+        }
+    });
+    __syncthreads();
+    const u32 n = min(s_n, k);
+    const u64 row = out_index ? out_index[q] : q;
+    if (threadIdx.x < n) {
+        const u128 key = s_win[threadIdx.x];
+        u32 rank = 0;
+        for (u32 j = 0; j < n; j++) rank += s_win[j] > key;
+        out_keys[row * k + rank] = ((u64)1 << 32) | (u64)((u32)key - (u32)doc_base);   // (~local) - base == ~(local + base)
+        out_scores[row * k + rank] = __longlong_as_double((long long)(u64)(key >> 32));
+    } else if (threadIdx.x < k) {
+        out_keys[row * k + threadIdx.x] = 0ull;
+        out_scores[row * k + threadIdx.x] = 0.0;
+    }
+}
+
+int launch_topk_select_f64(sa_index *ix, const TopkCtx &t, const u64 *d_tile_d, u32 n_queries, u64 doc_base,
+                           u64 *d_out_keys, double *d_out_scores, const u32 *d_out_index) {
+    if (n_queries == 0) return SA_OK;
+    KernelTimer tm(ix, 1);
+    topk_select_f64_kernel<<<n_queries, SEL_THREADS, 0, ix->stream>>>(t, d_tile_d, doc_base, d_out_keys, d_out_scores,
+                                                                      d_out_index);
+    SA_CUDA(cudaGetLastError());
+    tm.stop();
+    ix->stats.topk_kernel_launches++;
+    ix->stats.total_launches++;
+    return SA_OK;
+}
+
 // Merge per-shard top-k lists after the all-gather: in[r][q][k] -> out[q][k].
 __global__ void __launch_bounds__(SEL_THREADS)
 topk_merge_kernel(const u64 *__restrict__ in, u64 rank_stride, u32 world, u32 n_queries, u32 k, u64 *__restrict__ out) {

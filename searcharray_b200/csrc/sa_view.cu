@@ -18,9 +18,16 @@
 // does for the unsliced batch.
 // HBM traffic of a term query: the term scan's own bytes + 4*N (its doc-space row) + 20 per view position (8 row
 // index, 4 doc length, 4 gathered count, 4 view-space row).
+//
+// sa_score_batch_topk_sim runs the same steps under bm25_impact, bm25_legacy_similarity and classic_similarity, on a
+// view or on the unsliced array: the result of a query is the top k of SearchArray.score(q, similarity=sim), whose
+// formulas sim_tile_kernel shares with sa_op_similarity (sa_sim.cuh).  Only the tile kernel and, for classic, the
+// selection differ; see sim_tile_kernel.
 #include <algorithm>
+#include <cmath>
 
 #include "sa_phrase.cuh"
+#include "sa_sim.cuh"
 #include "sa_span.cuh"
 #include "sa_term.cuh"
 
@@ -28,10 +35,12 @@ struct ViewState {
     DevBuf d_dl;           // float [padded n_rows]: the doc lengths the view's BM25 uses
     DevBuf d_vrows;        // float [chunk][padded n_rows]: view-space score rows
     DevBuf d_tq;           // TermQuery [chunk]
-    DevBuf d_idf;          // float [n_queries], row order
+    DevBuf d_idf;          // float [n_queries], row order (double for sa_score_batch_topk_sim)
     DevBuf d_row_query;    // u32 [n_queries]: row -> query
     DevBuf d_ovf;          // u32 [n_queries], row order: candidate slots overflowed
     DevBuf d_keys;         // u64 [n_queries * k]: the result keys
+    DevBuf d_cand_d;       // u64 [chunk][tiles][slots]: float64 score bits of the classic candidates
+    DevBuf d_scores;       // double [n_queries * k]: the classic result scores
 };
 
 void sa_free_view(sa_index *ix) {
@@ -44,6 +53,8 @@ void sa_free_view(sa_index *ix) {
     V.d_row_query.release();
     V.d_ovf.release();
     V.d_keys.release();
+    V.d_cand_d.release();
+    V.d_scores.release();
     delete ix->view;
     ix->view = nullptr;
 }
@@ -296,4 +307,347 @@ extern "C" int sa_score_batch_topk_rows(sa_index *ix, const uint32_t *terms, con
     }
     if (!redone) return SA_OK;
     return view_download(ix, n_queries, k, out_pos, out_scores, nullptr);
+}
+
+// ------------------------------------------------ the other similarities (sa_score_batch_topk_sim)
+// grid = (tiles of positions, queries), as view_tile_kernel.  Position i reads its count at doc = rows[i] on a view
+// (rows == NULL: the unsliced array, doc = i) and its doc length at doc_lens[doc], which is SearchArray.doclengths()
+// -- not the stepped-slice lengths view_tile_kernel uses, a quirk of bm25_score only.  A zero count never scores
+// > 0 under any of the three formulas (0 / x, 0 * l and sqrt(0) give +-0 or NaN, and the idf is finite), so the
+// doc length is loaded only where the count is > 0.  What the tile ranks by, and how:
+//   impact:  the float32 score itself; flush_tile_collect and topk_select_kernel apply unchanged.
+//   legacy:  score = fl64(idf * (double)sat), sat the float32 saturation, idf finite.  For idf > 0 it is strictly
+//            increasing in sat: two distinct float32 sats differ by a relative 2^-24 at least, the double product
+//            of each is exact to a relative 2^-53 -- their order survives the rounding (and both the float32 and
+//            float64 ranges are wide enough that nothing overflows or underflows).  So sat is an EXACT key with the
+//            same ties, and the existing collector and select are exact; for idf < 0 the key is -sat (the score
+//            is > 0 only where sat < 0), for idf == 0 nothing ranks.  The score is formed on the host for the k
+//            winners only: |idf| * key, the same rounding as idf * sat.
+//   classic: score = fl64(fl64(idf * sqrt_tf) * inv_sqrt_dl) has no exact float32 key.  The tile ranks by a
+//            PROXY, the score rounded toward zero to float32 (at least the smallest subnormal for a score > 0):
+//            monotone, but distinct scores can share it.  So the tile keeps EVERY position at or above its bound
+//            -- flush_tile_collect's tie retry would cut positions tied at the bound by index, dropping larger
+//            float64 scores -- stores each candidate's float64 score beside its key (tile_d), and a tile with more
+//            candidates than slots sends the query to the exact re-run; topk_select_f64_kernel ranks in float64.
+template <int KIND>
+__global__ void __launch_bounds__(SA_TERM_THREADS)
+sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *__restrict__ rows,
+                const float *__restrict__ doc_lens, u64 n_pos, SimParams p, const double *__restrict__ idf,
+                float *__restrict__ out_rows, u64 out_stride, u32 row0, const TopkCtx t, u64 *__restrict__ tile_d) {
+    constexpr int PER_THREAD = SA_TILE_DOCS / SA_TERM_THREADS;
+    __shared__ __align__(16) float s_out[KIND == SA_SIM_CLASSIC ? 4 : SA_TILE_DOCS];
+    __shared__ u32 s_top[(SA_TERM_THREADS / 32) * 8];
+    __shared__ u32 s_ncand, s_tile_max;
+    const unsigned tid = threadIdx.x;
+    const u32 tile = blockIdx.x, row = row0 + blockIdx.y;
+    const u64 pos0 = (u64)tile * SA_TILE_DOCS;
+    const float *__restrict__ counts = doc_rows + (u64)blockIdx.y * doc_stride;
+    const double q_idf = idf[blockIdx.y];
+    u32 my_max = 0;
+    u32 key[PER_THREAD];          // classic: the proxy bits of the thread's positions
+    // thread tid owns positions 4g .. 4g+3 of the tile for g = tid + j * SA_TERM_THREADS (flush_tile_collect's layout)
+#pragma unroll
+    for (int j = 0; j < PER_THREAD / 4; j++) {
+        const unsigned g = tid + j * SA_TERM_THREADS;
+        float v[4];
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            const u64 i = pos0 + g * 4 + e;
+            v[e] = 0.0f;
+            if (i < n_pos) {
+                const u64 doc = rows ? __ldg(rows + i) : i;
+                const float tf = __ldg(counts + doc);
+                if (tf > 0.0f) {
+                    const float dl = __ldg(doc_lens + doc);
+                    if (KIND == SA_SIM_BM25_IMPACT) {
+                        v[e] = sim_impact(tf, dl, p);
+                    } else if (KIND == SA_SIM_BM25_LEGACY) {
+                        const float sat = sim_legacy_sat(tf, dl, p);
+                        v[e] = q_idf > 0.0 ? sat : (q_idf < 0.0 ? -sat : 0.0f);
+                    } else {
+                        const double s = sim_classic(q_idf, tf, dl);
+                        if (s > 0.0) v[e] = __uint_as_float(max(1u, __float_as_uint(__double2float_rz(s))));
+                    }
+                    if (v[e] > 0.0f) my_max = max(my_max, __float_as_uint(v[e]));   // NaN and <= 0 never rank
+                }
+            }
+            key[j * 4 + e] = v[e] > 0.0f ? __float_as_uint(v[e]) : 0u;
+        }
+        if (KIND != SA_SIM_CLASSIC) reinterpret_cast<float4 *>(s_out)[g] = make_float4(v[0], v[1], v[2], v[3]);
+    }
+    const u32 n_items = (u32)min((u64)SA_TILE_DOCS, n_pos - pos0);
+    if (KIND != SA_SIM_CLASSIC) {
+        flush_tile_collect(s_out, out_rows + (u64)row * out_stride + pos0, t, row, tile, my_max, n_items,
+                           min((u32)SA_TERM_THREADS, (n_items + 3) / 4), s_top, &s_ncand, &s_tile_max);
+        return;
+    }
+    // classic: the tile bound as flush_tile_collect computes it (8 values per warp), then every proxy >= it
+    const unsigned warp = tid >> 5, lane = tid & 31;
+    const bool need_bound = n_items > t.k;                           // CTA-uniform
+    if (need_bound) {
+        u32 v = my_max;
+        for (u32 r = 0; r < 8; r++) {
+            const u32 m = warp_pop_max(v);
+            if (lane == r) s_top[warp * 8 + r] = m;
+        }
+    }
+    if (tid == 0) { s_ncand = 0; s_tile_max = 0; }
+    __syncthreads();
+    const u32 thr = need_bound ? max(cta_kth_bound(s_top, t.k, true), 1u) : 1u;
+    const u64 slot0 = ((u64)row * t.n_tiles + tile) * t.slots;
+    u32 cand_max = 0;
+#pragma unroll
+    for (int j = 0; j < PER_THREAD / 4; j++) {
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            if (key[j * 4 + e] >= thr) {
+                const u32 local = (tid + j * SA_TERM_THREADS) * 4 + e;
+                const u32 slot = atomicAdd(&s_ncand, 1u);
+                if (slot < t.slots) {
+                    // the float64 score again, for the few candidates (cheaper than holding 32 doubles per thread)
+                    const u64 doc = rows ? __ldg(rows + pos0 + local) : pos0 + local;
+                    const double s = sim_classic(q_idf, __ldg(counts + doc), __ldg(doc_lens + doc));
+                    t.tile_cand[slot0 + slot] = ((u64)key[j * 4 + e] << 32) | (u64)(0xFFFFFFFFu - (tile * SA_TILE_DOCS + local));
+                    tile_d[slot0 + slot] = (u64)__double_as_longlong(s);
+                }
+                cand_max = max(cand_max, key[j * 4 + e]);
+            }
+        }
+    }
+    if (cand_max) atomicMax(&s_tile_max, cand_max);
+    __syncthreads();
+    if (tid == 0) {
+        const u64 t_idx = (u64)row * t.n_tiles + tile;
+        t.tile_cnt[t_idx] = min(s_ncand, t.slots);
+        t.tile_max[t_idx] = s_tile_max;
+        if (s_ncand > t.slots) t.overflow[row] = 1u;
+    }
+}
+
+// counts of row r (rows [row0, row0 + n_queries) of the chunk) in doc_rows + r * doc_stride
+static int launch_sim_tiles(sa_index *ix, int kind, const float *doc_rows, u64 doc_stride, const double *d_idf,
+                            u32 n_queries, u32 row0, const SimParams &p, const TopkCtx &t) {
+    ViewState &V = *ix->view;
+    if (n_queries == 0 || t.n_tiles == 0) return SA_OK;
+    const u64 *rows = ix->rows_active ? ix->d_rows : nullptr;
+    const u64 n_pos = ix->rows_active ? ix->n_rows : ix->n_docs;
+    const dim3 grid(t.n_tiles, n_queries);
+    KernelTimer tm(ix, 1);
+#define SA_SIM_TILES(KIND)                                                                                         \
+    sim_tile_kernel<KIND><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(doc_rows, doc_stride, rows, ix->d_doc_lens,    \
+        n_pos, p, d_idf, V.d_vrows.as<float>(), sa_padded_docs(n_pos), row0, t, V.d_cand_d.as<u64>())
+    if (kind == SA_SIM_BM25_IMPACT) SA_SIM_TILES(SA_SIM_BM25_IMPACT);
+    else if (kind == SA_SIM_BM25_LEGACY) SA_SIM_TILES(SA_SIM_BM25_LEGACY);
+    else SA_SIM_TILES(SA_SIM_CLASSIC);
+#undef SA_SIM_TILES
+    SA_CUDA(cudaGetLastError());
+    tm.stop();
+    ix->stats.topk_kernel_launches++;
+    ix->stats.total_launches++;
+    return SA_OK;
+}
+
+static int launch_sim_select(sa_index *ix, int kind, const TopkCtx &t, u32 n_queries, const u32 *d_out_index) {
+    ViewState &V = *ix->view;
+    const u64 doc_base = ix->rows_active ? 0 : ix->doc_base;    // a view returns positions, an array doc ids
+    if (kind == SA_SIM_CLASSIC)
+        return launch_topk_select_f64(ix, t, V.d_cand_d.as<u64>(), n_queries, doc_base, V.d_keys.as<u64>(),
+                                      V.d_scores.as<double>(), d_out_index);
+    return launch_topk_select(ix, t, n_queries, doc_base, V.d_keys.as<u64>(), d_out_index);
+}
+
+// Raw counts of one phrase / slop query on the index's own lists into ix->dense row 0: what phrase_common computes
+// for sa_phrase_freqs on an unsliced array.
+static int own_phrase_counts(sa_index *ix, const u32 *tids, u32 nt, u32 slop) {
+    u64 offs[SA_MAX_PHRASE_TERMS], lens[SA_MAX_PHRASE_TERMS], dirs[SA_MAX_PHRASE_TERMS];
+    bool missing, literal;
+    int rc = sa_resolve_terms(ix, tids, nt, offs, lens, dirs, &missing, &literal);
+    if (rc) return rc;
+    if (missing) return view_phrase_counts(ix, tids, nt, slop, true, nullptr, nullptr);    // zeros
+    if (slop > 0) return sa_span_run(ix, ix->d_words, offs, lens, dirs, nt, slop, literal, nullptr);
+    std::vector<PhraseQuery> pqs(1, make_phrase_query(tids, nt, offs, lens, dirs, 0.0f, false));
+    PhraseDump nodump;
+    memset(&nodump, 0, sizeof(nodump));
+    return sa_phrase_run_sync(ix, pqs, ix->d_words, 0, make_bm25(0, 1, 1, 0, ix->doc_lens_nonneg), nodump, true);
+}
+
+// keys (the classic scores, the overflow flags) to the host in one copy each and one synchronise
+static int sim_download(sa_index *ix, bool classic, u32 nq, u32 k, std::vector<u64> &keys, std::vector<double> &scores,
+                        std::vector<u32> *ovf) {
+    ViewState &V = *ix->view;
+    const size_t nk = (size_t)nq * k;
+    int rc;
+    if ((rc = sa_pinned_reserve(ix, nk * (sizeof(u64) + sizeof(double)) + (size_t)nq * sizeof(u32)))) return rc;
+    u64 *h_keys = (u64 *)ix->h_pinned;
+    double *h_scores = (double *)(h_keys + nk);
+    u32 *h_ovf = (u32 *)(h_scores + nk);
+    SA_CUDA(cudaMemcpyAsync(h_keys, V.d_keys.p, nk * sizeof(u64), cudaMemcpyDeviceToHost, ix->stream));
+    if (classic)
+        SA_CUDA(cudaMemcpyAsync(h_scores, V.d_scores.p, nk * sizeof(double), cudaMemcpyDeviceToHost, ix->stream));
+    if (ovf) SA_CUDA(cudaMemcpyAsync(h_ovf, V.d_ovf.p, nq * sizeof(u32), cudaMemcpyDeviceToHost, ix->stream));
+    SA_CUDA(cudaStreamSynchronize(ix->stream));
+    keys.assign(h_keys, h_keys + nk);
+    if (classic) scores.assign(h_scores, h_scores + nk);
+    if (ovf) ovf->assign(h_ovf, h_ovf + nq);
+    return SA_OK;
+}
+
+extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *terms, const uint32_t *term_starts,
+                                       const double *idf, uint32_t n_queries, uint32_t slop, double avg_doc_len,
+                                       double k1, double b, uint32_t k, uint32_t *out_ids, double *out_scores) {
+    SA_CHECK(ix, "index is NULL");
+    SA_CHECK(n_queries == 0 || (terms && term_starts && idf && out_ids && out_scores), "NULL argument");
+    SA_CHECK(kind == SA_SIM_BM25_IMPACT || kind == SA_SIM_BM25_LEGACY || kind == SA_SIM_CLASSIC, "unknown similarity %d", kind);
+    SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
+    int rc;
+    for (u32 q = 0; q < n_queries; q++) {
+        const u32 nt = term_starts[q + 1] - term_starts[q];
+        SA_CHECK(nt >= 1 && nt <= SA_MAX_PHRASE_TERMS, "query %u: bad number of terms", q);
+        if ((rc = sa_check_term_ids(ix, terms + term_starts[q], nt))) return rc;
+        SA_CHECK(kind == SA_SIM_BM25_IMPACT || std::isfinite(idf[q]), "query %u: idf is not finite", q);
+    }
+    std::lock_guard<std::mutex> g(ix->mu);
+    const bool view = ix->rows_active;
+    const u64 n_pos = view ? ix->n_rows : ix->n_docs;
+    SA_CHECK(n_pos < 0xFFFFFFFFull, "the array must have fewer than 2^32 - 1 rows");
+    SA_CUDA(cudaSetDevice(ix->device));
+    const size_t nk = (size_t)n_queries * k;
+    for (size_t i = 0; i < nk; i++) { out_ids[i] = SA_NO_DOC; out_scores[i] = 0.0; }
+    // impact and legacy score zeros at avgdl == 0 (similarity.py:49-50, 66-67); classic has no such branch
+    if (n_queries == 0 || n_pos == 0 || (kind != SA_SIM_CLASSIC && avg_doc_len == 0.0)) return SA_OK;
+    if (!ix->view) ix->view = new ViewState();
+    ViewState &V = *ix->view;
+    const bool classic = kind == SA_SIM_CLASSIC;
+    const u64 stride = sa_padded_docs(ix->n_docs), pstride = sa_padded_docs(n_pos);
+    const u32 n_ptiles = sa_n_tiles(n_pos), slots = classic ? 256u : sa_topk_slots(k);
+    // chunk so the doc-space and position-space rows of one chunk stay within ~4 GB of HBM
+    const u32 chunk = (u32)std::min<u64>(65535, std::max<u64>(1, std::min<u64>(n_queries,
+                                         (4ull << 30) / ((stride + pstride) * sizeof(float)))));
+    // Every buffer is reserved before the first write: DevBuf::reserve does not keep the contents.  ix->dense is the
+    // exception -- each step reserves it and consumes what it wrote before the next reserve.
+    if (!classic && (rc = V.d_vrows.reserve((size_t)chunk * pstride * sizeof(float)))) return rc;
+    if ((rc = V.d_tq.reserve((size_t)chunk * sizeof(TermQuery)))) return rc;
+    if ((rc = V.d_idf.reserve((size_t)n_queries * sizeof(double)))) return rc;
+    if ((rc = V.d_row_query.reserve((size_t)n_queries * sizeof(u32)))) return rc;
+    if ((rc = V.d_ovf.reserve((size_t)n_queries * sizeof(u32)))) return rc;
+    if ((rc = V.d_keys.reserve(nk * sizeof(u64)))) return rc;
+    if ((rc = ix->cand.reserve(cand_bytes(n_ptiles, chunk, slots)))) return rc;
+    if (classic && (rc = V.d_scores.reserve(nk * sizeof(double)))) return rc;
+    if (classic && (rc = V.d_cand_d.reserve((size_t)chunk * n_ptiles * slots * sizeof(u64)))) return rc;
+
+    // rows: chunk by chunk, the term queries first, then the phrase queries
+    struct Chunk { u32 row0, n_term, n_phrase; };
+    std::vector<Chunk> chunks;
+    std::vector<u32> row_query;
+    std::vector<double> row_idf;
+    row_query.reserve(n_queries);
+    row_idf.reserve(n_queries);
+    for (u32 q0 = 0; q0 < n_queries; q0 += chunk) {
+        const u32 q1 = std::min(n_queries, q0 + chunk);
+        Chunk C{(u32)row_query.size(), 0, 0};
+        for (int pass = 0; pass < 2; pass++)
+            for (u32 q = q0; q < q1; q++) {
+                const bool term = term_starts[q + 1] - term_starts[q] == 1;
+                if (term != (pass == 0)) continue;
+                row_query.push_back(q);
+                row_idf.push_back(idf[q]);
+                (term ? C.n_term : C.n_phrase)++;
+            }
+        chunks.push_back(C);
+    }
+    SA_CUDA(cudaMemcpyAsync(V.d_idf.p, row_idf.data(), n_queries * sizeof(double), cudaMemcpyHostToDevice, ix->stream));
+    SA_CUDA(cudaMemcpyAsync(V.d_row_query.p, row_query.data(), n_queries * sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
+    SA_CUDA(cudaMemsetAsync(V.d_ovf.p, 0, n_queries * sizeof(u32), ix->stream));
+    const SimParams p = make_sim_params(avg_doc_len, k1, b);
+    const double *d_idf = V.d_idf.as<double>();
+
+    for (const Chunk &C : chunks) {
+        const u32 Q = C.n_term + C.n_phrase;
+        TopkCtx t = make_topk_ctx(ix->cand.p, n_ptiles, Q, slots, k, V.d_ovf.as<u32>() + C.row0);
+        if (C.n_phrase) {
+            // on a view, one filter pass over every list of the chunk's phrases (a phrase with a missing term has none)
+            std::vector<u32> ftids, fstart;
+            std::vector<unsigned char> missing;
+            for (u32 j = 0; j < C.n_phrase && view; j++) {
+                const u32 q = row_query[C.row0 + C.n_term + j];
+                const u32 *tids = terms + term_starts[q];
+                const u32 nt = term_starts[q + 1] - term_starts[q];
+                fstart.push_back((u32)ftids.size());
+                missing.push_back(query_missing(ix, tids, nt));
+                if (!missing.back()) ftids.insert(ftids.end(), tids, tids + nt);
+            }
+            std::vector<u64> f_offs, f_lens;
+            if (!ftids.empty() && (rc = sa_filter_terms_mask(ix, ftids.data(), (u32)ftids.size(), ix->d_row_mask, 0,
+                                                             SA_ALL_BITS, false, f_offs, f_lens, nullptr))) return rc;
+            for (u32 j = 0; j < C.n_phrase; j++) {
+                const u32 q = row_query[C.row0 + C.n_term + j];
+                const u32 *tids = terms + term_starts[q];
+                const u32 nt = term_starts[q + 1] - term_starts[q];
+                if (view) {
+                    const u64 *fo = missing[j] ? nullptr : f_offs.data() + fstart[j];
+                    const u64 *fl = missing[j] ? nullptr : f_lens.data() + fstart[j];
+                    rc = view_phrase_counts(ix, tids, nt, slop, missing[j], fo, fl);
+                } else {
+                    rc = own_phrase_counts(ix, tids, nt, slop);
+                }
+                if (rc) return rc;
+                if ((rc = launch_sim_tiles(ix, kind, ix->dense.as<float>(), stride, d_idf + C.row0 + C.n_term + j, 1,
+                                           C.n_term + j, p, t))) return rc;
+            }
+        }
+        if (C.n_term) {
+            // the index's own lists, on a view too: a view keeps or drops whole docs (see sa_score_batch_topk_rows)
+            std::vector<TermQuery> tqs(C.n_term);
+            for (u32 j = 0; j < C.n_term; j++) tqs[j] = make_term_query(ix, terms[term_starts[row_query[C.row0 + j]]], 0.0f);
+            if ((rc = view_term_counts(ix, tqs.data(), C.n_term))) return rc;
+            if ((rc = launch_sim_tiles(ix, kind, ix->dense.as<float>(), stride, d_idf + C.row0, C.n_term, 0, p, t))) return rc;
+        }
+        if ((rc = launch_sim_select(ix, kind, t, Q, V.d_row_query.as<u32>() + C.row0))) return rc;
+    }
+    std::vector<u64> keys;
+    std::vector<double> scores;
+    std::vector<u32> ovf;
+    if ((rc = sim_download(ix, classic, n_queries, k, keys, scores, &ovf))) return rc;
+    bool redone = false;
+    for (u32 r = 0; r < n_queries; r++) {
+        if (!ovf[r]) continue;
+        // exact re-run of one query: a candidate slot per position of the tile cannot overflow
+        const u32 q = row_query[r];
+        const u32 *tids = terms + term_starts[q];
+        const u32 nt = term_starts[q + 1] - term_starts[q];
+        if (nt == 1) {
+            TermQuery tq = make_term_query(ix, tids[0], 0.0f);
+            if ((rc = view_term_counts(ix, &tq, 1))) return rc;
+        } else if (view) {
+            const bool miss = query_missing(ix, tids, nt);
+            std::vector<u64> f_offs, f_lens;
+            if (!miss && (rc = sa_filter_terms_mask(ix, tids, nt, ix->d_row_mask, 0, SA_ALL_BITS, false, f_offs, f_lens,
+                                                    nullptr))) return rc;
+            if ((rc = view_phrase_counts(ix, tids, nt, slop, miss, f_offs.data(), f_lens.data()))) return rc;
+        } else if ((rc = own_phrase_counts(ix, tids, nt, slop))) {
+            return rc;
+        }
+        if ((rc = ix->cand.reserve(cand_bytes(n_ptiles, 1, SA_TILE_DOCS)))) return rc;
+        if (classic && (rc = V.d_cand_d.reserve((size_t)n_ptiles * SA_TILE_DOCS * sizeof(u64)))) return rc;
+        SA_CUDA(cudaMemsetAsync(V.d_ovf.as<u32>() + r, 0, sizeof(u32), ix->stream));
+        TopkCtx t = make_topk_ctx(ix->cand.p, n_ptiles, 1, SA_TILE_DOCS, k, V.d_ovf.as<u32>() + r);
+        if ((rc = launch_sim_tiles(ix, kind, ix->dense.as<float>(), stride, d_idf + r, 1, 0, p, t))) return rc;
+        if ((rc = launch_sim_select(ix, kind, t, 1, V.d_row_query.as<u32>() + r))) return rc;
+        redone = true;
+    }
+    if (redone && (rc = sim_download(ix, classic, n_queries, k, keys, scores, nullptr))) return rc;
+    for (u32 q = 0; q < n_queries; q++)
+        for (u32 i = 0; i < k; i++) {
+            const size_t j = (size_t)q * k + i;
+            const u64 key = keys[j];
+            if (key == 0) continue;
+            out_ids[j] = 0xFFFFFFFFu - (u32)key;
+            float f;
+            const u32 bits = (u32)(key >> 32);
+            memcpy(&f, &bits, sizeof(f));
+            if (kind == SA_SIM_BM25_IMPACT) out_scores[j] = f;
+            else if (kind == SA_SIM_BM25_LEGACY) out_scores[j] = std::fabs(idf[q]) * (double)f;   // f = sign(idf) * sat
+            else out_scores[j] = scores[j];
+        }
+    return SA_OK;
 }

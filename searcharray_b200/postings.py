@@ -24,7 +24,8 @@ from pandas.api.types import is_list_like
 from . import _lib
 from .indexing import HostIndex, TermMissingError, build_index
 from .roaringish import decode_positions
-from .similarity import Bm25Similarity, Similarity, compute_idf, default_bm25
+from .similarity import (Bm25Impact, Bm25Legacy, Bm25Similarity, ClassicSimilarity, Similarity, compute_idf,
+                         default_bm25)
 
 
 def ws_tokenizer(string):
@@ -485,7 +486,7 @@ class SearchArray(ExtensionArray):
         return out
 
     # -------------------------------------------------- batched, HBM-resident path
-    def search_topk(self, queries, k=10, similarity: Bm25Similarity = default_bm25, slop=0):
+    def search_topk(self, queries, k=10, similarity: Similarity = default_bm25, slop=0):
         """queries: list of str (term) or list[str] (phrase).  Returns (docs uint32[Q,k],
         scores float32[Q,k]): per query the k best scores > 0, by score descending then id ascending, empty
         slots NO_DOC / 0.  Scores never leave HBM except the top-k (sa_score_batch_topk).
@@ -494,7 +495,15 @@ class SearchArray(ExtensionArray):
         `view.score(q, similarity=similarity, slop=slop)`, and the returned ids are POSITIONS IN THE VIEW
         (0 .. len(view) - 1, the index space of view.score), not the parent's doc ids.  Views of a sharded array
         (built with a comm or a global_df) raise ValueError: their document frequencies would need a sum over
-        the ranks."""
+        the ranks.
+
+        similarity: bm25_similarity, bm25_impact, bm25_legacy_similarity or classic_similarity; any other
+        callable raises TypeError.  Under the last three the result is, bit for bit, the top k of
+        `.score(q, similarity=similarity, slop=slop)` on the same array or view, and the scores have its dtype
+        (float32 for bm25_impact, float64 for the other two, also where .score returns float32 zeros because
+        avg_doc_length is 0); +inf ranks, NaN never does."""
+        if not isinstance(similarity, Bm25Similarity):
+            return self._search_topk_sim(queries, k, similarity, slop)
         if self.rows is not None:
             return self._search_topk_view(queries, k, similarity, slop)
         terms, starts, idfs = [], [0], []
@@ -552,3 +561,47 @@ class SearchArray(ExtensionArray):
                                                            self.avg_doc_length, similarity.k1, similarity.b, k,
                                                            _lib.p_u32(docs), _lib.p_f32(scores)))
         return docs, scores
+
+    def _search_topk_sim(self, queries, k, similarity, slop):
+        """search_topk under bm25_impact, bm25_legacy_similarity or classic_similarity (sa_score_batch_topk_sim):
+        the counts, document frequencies, doc lengths, avgdl and corpus size .score hands the similarity, with
+        the similarity's own idf computed here, on the host, from the same dfs."""
+        if not isinstance(similarity, (Bm25Impact, Bm25Legacy, ClassicSimilarity)):
+            raise TypeError("search_topk supports bm25_similarity, bm25_impact, bm25_legacy_similarity and "
+                            f"classic_similarity, not {similarity!r}")
+        if self.rows is not None and (self.comm is not None or self.global_df is not None):
+            raise ValueError("search_topk on a view of a sharded SearchArray is not supported: the slice's document "
+                             "frequencies would need a sum over the ranks; use .score() on the view")
+        toks = [[q] if isinstance(q, str) else list(q) for q in queries]
+        docs = np.full((len(toks), k), _lib.NO_DOC, dtype=np.uint32)
+        scores = np.zeros((len(toks), k), dtype=np.float64)
+        ids = {t: self._term_id(t) for ts in toks for t in ts}
+        dev = self._device()
+        with self._shared["lock"]:
+            self._apply_rows(dev)
+            if self.rows is None:
+                df = {t: self.docfreq(t) for t in ids}
+            else:
+                # the slice dfs of every distinct known token in one device pass; .docfreq's values: np.uint64 for
+                # a known token, 0 for an unknown one
+                known = [t for t, tid in ids.items() if tid != _lib.NO_TERM]
+                dfs = np.zeros(len(known), dtype=np.uint64)
+                if known:
+                    tids = np.asarray([ids[t] for t in known], dtype=np.uint32)
+                    _lib.check(_lib.lib().sa_docfreq_rows_batch(dev.handle, _lib.p_u32(tids), len(tids),
+                                                                _lib.p_u64(dfs)))
+                df = dict(zip(known, dfs))
+            terms, starts, idfs = [], [0], []
+            for ts in toks:
+                terms.extend(ids[t] for t in ts)
+                starts.append(len(terms))
+                idfs.append(float(similarity._idf(np.asarray([df.get(t, 0) for t in ts]), self.corpus_size)))
+            terms = np.asarray(terms, dtype=np.uint32)
+            starts = np.asarray(starts, dtype=np.uint32)
+            idfs = np.asarray(idfs, dtype=np.float64)
+            dbl = ctypes.POINTER(ctypes.c_double)
+            _lib.check(_lib.lib().sa_score_batch_topk_sim(
+                dev.handle, similarity.kind, _lib.p_u32(terms), _lib.p_u32(starts), idfs.ctypes.data_as(dbl),
+                len(toks), int(slop), float(self.avg_doc_length), float(similarity.k1), float(similarity.b), k,
+                _lib.p_u32(docs), scores.ctypes.data_as(dbl)))
+        return docs, scores.astype(similarity.out_dtype, copy=False)
