@@ -127,28 +127,26 @@ int sa_score_batch_topk(sa_index *index, const uint32_t *terms, const uint32_t *
                         const float *idf, uint32_t n_queries, uint32_t slop,
                         float avg_doc_len, float k1, float b, uint32_t k,
                         uint32_t *out_docs, float *out_scores);
-/* The batched top-k on a sliced array: the top k of SearchArray.score on the view (postings.py:652-680 on
- * FilteredPosns, middle_out.py:291-317; np.argpartition as above).  Row filter installed by sa_index_set_rows;
- * idf[q] from sa_docfreq_rows_batch's slice document frequencies; view_doc_lens = float32[n_rows], the lengths the
- * view's BM25 uses (bm25/bm25.pyx:28-41); avg_doc_len the parent's.  Counts come from the filtered postings.
- * out_pos = positions in the view (< n_rows, which must be < 2^32 - 1), not doc ids; order and empty slots as
- * sa_score_batch_topk. */
-int sa_score_batch_topk_rows(sa_index *index, const uint32_t *terms, const uint32_t *term_starts,
-                             const float *idf, uint32_t n_queries, uint32_t slop, const float *view_doc_lens,
-                             float avg_doc_len, float k1, float b, uint32_t k,
-                             uint32_t *out_pos, float *out_scores);
-/* The batched top-k under another similarity (kind = SA_SIM_*, below): the top k of SearchArray.score(q,
- * similarity=...), i.e. of sa_op_similarity over the query's counts, on the view the installed row filter selects
- * or, with no filter, on the whole array.  Counts as SearchArray.termfreqs (the filtered postings on a view); doc
- * lengths the index's own (gathered through the row filter: SearchArray.doclengths()); idf[q] the similarity's own
- * float64 idf of the query's document frequencies (must be finite; unused by SA_SIM_BM25_IMPACT); avg_doc_len, k1,
- * b the Python values (numpy's float32 promotion is applied here).  avg_doc_len == 0 -> nothing ranks, except under
- * SA_SIM_CLASSIC.  out_scores are float64 (the float32 impact scores widened).  Only scores > 0 rank (+inf does,
- * NaN never); order score desc, then id asc; empty slots SA_NO_DOC / 0.  Ids: positions in the view, or GLOBAL doc
- * ids (doc_base added) on an unsliced array; fewer than 2^32 - 1 of them. */
+/* The batched top-k on a sliced array, and under the other similarities (kind = SA_SIM_*, below): the top k of
+ * SearchArray.score(q, similarity=...) on the view the installed row filter selects (sa_index_set_rows;
+ * postings.py:652-680 on FilteredPosns, middle_out.py:291-317) or, with no filter, on the whole array.  Counts as
+ * SearchArray.termfreqs (the filtered postings on a view); avg_doc_len the parent's.
+ *   SA_SIM_BM25 (on a view only; the unsliced array takes sa_score_batch_topk): BM25 as sa_score_term computes it,
+ *     idf[q] the float32 idf of the slice's document frequencies (sa_docfreq_rows_batch), widened;
+ *     view_doc_lens = float32[n_rows], the lengths the view's BM25 uses (bm25/bm25.pyx:28-41); avg_doc_len, k1 and b
+ *     are rounded to float32.
+ *   The others: sa_op_similarity over the query's counts; doc lengths the index's own (gathered through the row
+ *     filter: SearchArray.doclengths()), view_doc_lens is ignored; idf[q] the similarity's own float64 idf (must be
+ *     finite for SA_SIM_BM25_LEGACY and SA_SIM_CLASSIC; unused by SA_SIM_BM25_IMPACT); avg_doc_len, k1, b the
+ *     Python values (numpy's float32 promotion is applied here).
+ * avg_doc_len == 0 -> nothing ranks, except under SA_SIM_CLASSIC.  out_scores are float64 (the float32 BM25 and
+ * impact scores widened).  Only scores > 0 rank (+inf does, NaN never); order score desc, then id asc
+ * (np.argpartition as above); empty slots SA_NO_DOC / 0.  Ids: positions in the view, or GLOBAL doc ids (doc_base
+ * added) on an unsliced array; fewer than 2^32 - 1 of them. */
 int sa_score_batch_topk_sim(sa_index *index, int kind, const uint32_t *terms, const uint32_t *term_starts,
-                            const double *idf, uint32_t n_queries, uint32_t slop, double avg_doc_len,
-                            double k1, double b, uint32_t k, uint32_t *out_ids, double *out_scores);
+                            const double *idf, uint32_t n_queries, uint32_t slop, const float *view_doc_lens,
+                            double avg_doc_len, double k1, double b, uint32_t k, uint32_t *out_ids,
+                            double *out_scores);
 
 /* The same batch in three stages, so a serving loop (or the benchmark) can keep the query
  * descriptors resident and time the device work alone: upload (H2D of descriptors), execute
@@ -262,6 +260,8 @@ int sa_op_bm25_score(float *tf_inout, const float *doc_lens, uint64_t n, float a
 #define SA_SIM_BM25_IMPACT 0
 #define SA_SIM_BM25_LEGACY 1
 #define SA_SIM_CLASSIC 2
+/* BM25 on a view, for sa_score_batch_topk_sim only (sa_op_similarity rejects it) */
+#define SA_SIM_BM25 3
 int sa_op_similarity(int kind, const float *term_freqs, const float *doc_lens, uint64_t n,
                      double avg_doc_len, double idf, double k1, double b, int device, void *out);
 /* bigram_freqs (phrase/bigram_freqs.py:213-307): cont_rhs=1 -> Continuation.RHS else LHS.

@@ -49,10 +49,8 @@ SIGNATURES = {
     "sa_score_phrase": (c_int, [P_void, P_u32, c_u32, c_u32, c_f32, c_f32, c_f32, c_f32, c_u64, c_u64, P_f32]),
     "sa_score_batch_topk": (c_int, [P_void, P_u32, P_u32, P_f32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32,
                                     P_u32, P_f32]),
-    "sa_score_batch_topk_rows": (c_int, [P_void, P_u32, P_u32, P_f32, c_u32, c_u32, P_f32, c_f32, c_f32, c_f32,
-                                         c_u32, P_u32, P_f32]),
     "sa_score_batch_topk_sim": (c_int, [P_void, c_int, P_u32, P_u32, ctypes.POINTER(ctypes.c_double), c_u32, c_u32,
-                                        ctypes.c_double, ctypes.c_double, ctypes.c_double, c_u32, P_u32,
+                                        P_f32, ctypes.c_double, ctypes.c_double, ctypes.c_double, c_u32, P_u32,
                                         ctypes.POINTER(ctypes.c_double)]),
     "sa_batch_upload": (c_int, [P_void, P_u32, P_u32, P_f32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32]),
     "sa_batch_execute": (c_int, [P_void]),

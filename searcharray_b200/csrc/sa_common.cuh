@@ -149,7 +149,7 @@ struct sa_index {
     std::vector<struct TimedLaunch> *pending_timers = nullptr;
     std::vector<cudaEvent_t> *free_events = nullptr;
     struct BatchState *batch = nullptr;
-    struct ViewState *view = nullptr;   // buffers of sa_score_batch_topk_rows (sa_view.cu)
+    struct ViewState *view = nullptr;   // buffers of sa_score_batch_topk_sim (sa_view.cu)
     sa_stats stats;
     std::mutex mu;
 

@@ -289,6 +289,8 @@ __device__ __forceinline__ u32 tile_bound_width(u32 k, u32 n_holders) { return (
 // collect the tile's top-k candidates (private slots, count, maximum): the same step the term kernel
 // ends with, shared with the phrase kernel.  `my_max` = largest score bits this thread put into the
 // tile, `n_items` = number of scores in the tile, `n_holders` = how many threads can hold one of them.  All SA_TERM_THREADS threads must call.
+// STORE = false: collect only (out_tile unused); the tile stays in shared memory for the tie retry either way.
+template <bool STORE = true>
 __device__ __forceinline__ void flush_tile_collect(const float *s_out, float *__restrict__ out_tile, const TopkCtx &t,
                                                    u32 row, u32 tile, u32 my_max, u32 n_items, u32 n_holders, u32 *s_top,
                                                    u32 *s_ncand, u32 *s_tile_max) {
@@ -319,7 +321,7 @@ __device__ __forceinline__ void flush_tile_collect(const float *s_out, float *__
     for (int jj = 0; jj < SA_TILE_DOCS / SA_TERM_THREADS / 4; jj++) {
         const unsigned g = tid + jj * SA_TERM_THREADS;
         const float4 v = reinterpret_cast<const float4 *>(s_out)[g];
-        __stcs(out4 + g, v);
+        if constexpr (STORE) __stcs(out4 + g, v);
         if (k && ((v.x >= thr_f) | (v.y >= thr_f) | (v.z >= thr_f) | (v.w >= thr_f))) {
             const float vs[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll

@@ -1,30 +1,26 @@
-// sa_view.cu -- the batched top-k path on a sliced array (a view: SearchArray.search_topk on arr[key]).
+// sa_view.cu -- sa_score_batch_topk_sim: SearchArray.search_topk on a sliced array (a view: arr[key]) under every
+// similarity, and on the unsliced array under bm25_impact, bm25_legacy_similarity and classic_similarity.
 //
-// The result of a query is the top k of what SearchArray.score returns on the view (reference postings.py:652-680
-// on FilteredPosns, middle_out.py:291-317): per-doc counts of the FILTERED postings, BM25 over the view's positions
-// with the view's doc lengths and the parent's avgdl, and an idf the caller derived from the view's document
-// frequencies (sa_docfreq_rows_batch).  Ids are positions in the view.  Per chunk of queries:
+// The result of a query is the top k of SearchArray.score(q, similarity=sim, slop=slop) on the same array or view
+// (reference postings.py:652-680 on FilteredPosns, middle_out.py:291-317): per-doc counts of the (on a view:
+// filtered) postings, the similarity's formula over the positions, and an idf the caller derived from the document
+// frequencies (a view's from sa_docfreq_rows_batch).  Ids are positions in the view, or doc ids on an unsliced
+// array.  Per chunk of queries:
 //   1. per-doc counts in DOC space, one row per query in ix->dense:
-//        phrase / slop queries: the chunk's phrase terms are filtered once (sa_filter_terms_mask), then every query
-//          takes the raw-count route phrase_common takes for a view (sa_phrase_run_sync / sa_span_run) into row 0,
+//        phrase / slop queries: on a view the chunk's phrase terms are filtered once (sa_filter_terms_mask), then
+//          every query takes the raw-count route phrase_common takes (sa_phrase_run_sync / sa_span_run) into row 0,
 //          which step 2 consumes before the next query overwrites it;
-//        term queries: the term kernel in tf mode on the index's own lists, rows [0, n_term) (see the call);
-//   2. view_tile_kernel: one CTA per (8,192 view positions, query) gathers count = row[rows[i]] and evaluates
-//      bm25_one(count, view_doc_lens[i]) for EVERY position, as bm25_dense_kernel does for .score, so exotic
-//      k1 / b and zero counts give the same bits; the tile is staged in shared memory and flush_tile_collect writes
-//      the view-space row and the tile's top-k candidates;
-//   3. launch_topk_select over the view's tiles (doc_base 0: the keys carry view positions).
+//        term queries: the term kernel in tf mode on the index's own lists, rows [0, n_term) (see term_tiles);
+//   2. sim_tile_kernel: one CTA per (8,192 positions, query) gathers each position's count, scores it and collects
+//      the tile's top-k candidates;
+//   3. launch_topk_select (launch_topk_select_f64 for classic) over the tiles.
 // A query whose candidate slots overflowed is re-run alone with a slot per position of the tile, as redo_query
 // does for the unsliced batch.
-// HBM traffic of a term query: the term scan's own bytes + 4*N (its doc-space row) + 20 per view position (8 row
-// index, 4 doc length, 4 gathered count, 4 view-space row).
-//
-// sa_score_batch_topk_sim runs the same steps under bm25_impact, bm25_legacy_similarity and classic_similarity, on a
-// view or on the unsliced array: the result of a query is the top k of SearchArray.score(q, similarity=sim), whose
-// formulas sim_tile_kernel shares with sa_op_similarity (sa_sim.cuh).  Only the tile kernel and, for classic, the
-// selection differ; see sim_tile_kernel.
+// HBM traffic of a term query: the term scan's own bytes + 4*N (its doc-space row), then per position 4 (gathered
+// count) and 8 (row index, views only), and 4 (doc length) per position whose count is > 0.
 #include <algorithm>
 #include <cmath>
+#include <type_traits>
 
 #include "sa_phrase.cuh"
 #include "sa_sim.cuh"
@@ -32,10 +28,9 @@
 #include "sa_term.cuh"
 
 struct ViewState {
-    DevBuf d_dl;           // float [padded n_rows]: the doc lengths the view's BM25 uses
-    DevBuf d_vrows;        // float [chunk][padded n_rows]: view-space score rows
+    DevBuf d_dl;           // float [n_rows]: the doc lengths BM25 uses on the view
     DevBuf d_tq;           // TermQuery [chunk]
-    DevBuf d_idf;          // float [n_queries], row order (double for sa_score_batch_topk_sim)
+    DevBuf d_idf;          // double [n_queries], row order
     DevBuf d_row_query;    // u32 [n_queries]: row -> query
     DevBuf d_ovf;          // u32 [n_queries], row order: candidate slots overflowed
     DevBuf d_keys;         // u64 [n_queries * k]: the result keys
@@ -47,7 +42,6 @@ void sa_free_view(sa_index *ix) {
     if (!ix->view) return;
     ViewState &V = *ix->view;
     V.d_dl.release();
-    V.d_vrows.release();
     V.d_tq.release();
     V.d_idf.release();
     V.d_row_query.release();
@@ -59,263 +53,19 @@ void sa_free_view(sa_index *ix) {
     ix->view = nullptr;
 }
 
-// grid = (view tiles, queries).  row = row0 + blockIdx.y indexes the view-space rows, the candidate slots and the
-// overflow flags; doc_rows + blockIdx.y * doc_stride is the query's doc-space count row, idf[blockIdx.y] its idf.
-__global__ void __launch_bounds__(SA_TERM_THREADS)
-view_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *__restrict__ rows,
-                 const float *__restrict__ view_dl, u64 n_rows, Bm25Params p, const float *__restrict__ idf,
-                 float *__restrict__ view_rows, u64 view_stride, u32 row0, const TopkCtx t) {
-    __shared__ __align__(16) float s_out[SA_TILE_DOCS];
-    __shared__ u32 s_top[(SA_TERM_THREADS / 32) * 8];
-    __shared__ u32 s_ncand, s_tile_max;
-    const u32 tile = blockIdx.x, row = row0 + blockIdx.y;
-    const u64 pos0 = (u64)tile * SA_TILE_DOCS;
-    const float *__restrict__ counts = doc_rows + (u64)blockIdx.y * doc_stride;
-    p.idf = idf[blockIdx.y];
-    u32 my_max = 0;
-    // thread tid owns positions 4g .. 4g+3 of the tile for g = tid + j * SA_TERM_THREADS: the float4 layout
-    // flush_tile_collect reads, so every thread reads back only what it wrote
-#pragma unroll
-    for (int j = 0; j < SA_TILE_DOCS / SA_TERM_THREADS / 4; j++) {
-        const unsigned g = threadIdx.x + j * SA_TERM_THREADS;
-        float v[4];
-#pragma unroll
-        for (int e = 0; e < 4; e++) {
-            const u64 i = pos0 + g * 4 + e;
-            v[e] = 0.0f;
-            if (i < n_rows) {
-                v[e] = bm25_one(__ldg(counts + __ldg(rows + i)), __ldg(view_dl + i), p);
-                if (v[e] > 0.0f) my_max = max(my_max, __float_as_uint(v[e]));   // NaN and <= 0 never rank
-            }
-        }
-        reinterpret_cast<float4 *>(s_out)[g] = make_float4(v[0], v[1], v[2], v[3]);
-    }
-    const u32 n_items = (u32)min((u64)SA_TILE_DOCS, n_rows - pos0);
-    flush_tile_collect(s_out, view_rows + (u64)row * view_stride + pos0, t, row, tile, my_max, n_items,
-                       min((u32)SA_TERM_THREADS, (n_items + 3) / 4), s_top, &s_ncand, &s_tile_max);
-}
+template <int KIND> using TileParams = std::conditional_t<KIND == SA_SIM_BM25, Bm25Params, SimParams>;
 
-static int launch_view_tiles(sa_index *ix, const float *doc_rows, u64 doc_stride, const float *d_idf, u32 n_queries,
-                             u32 row0, const Bm25Params &p, const TopkCtx &t) {
-    ViewState &V = *ix->view;
-    if (n_queries == 0 || t.n_tiles == 0) return SA_OK;
-    KernelTimer tm(ix, 1);
-    view_tile_kernel<<<dim3(t.n_tiles, n_queries), SA_TERM_THREADS, 0, ix->stream>>>(
-        doc_rows, doc_stride, ix->d_rows, V.d_dl.as<float>(), ix->n_rows, p, d_idf, V.d_vrows.as<float>(),
-        sa_padded_docs(ix->n_rows), row0, t);
-    SA_CUDA(cudaGetLastError());
-    tm.stop();
-    ix->stats.topk_kernel_launches++;
-    ix->stats.total_launches++;
-    return SA_OK;
-}
-
-// tf of n term queries into ix->dense rows [0, n), on the index's own lists (tf-table fast path, no top-k)
-static int view_term_counts(sa_index *ix, const TermQuery *h_tq, u32 n) {
-    ViewState &V = *ix->view;
-    int rc;
-    if ((rc = ix->dense.reserve((size_t)n * sa_padded_docs(ix->n_docs) * sizeof(float)))) return rc;
-    SA_CUDA(cudaMemcpyAsync(V.d_tq.p, h_tq, n * sizeof(TermQuery), cudaMemcpyHostToDevice, ix->stream));
-    TopkCtx none;
-    memset(&none, 0, sizeof(none));
-    TermBatchArgs a = make_term_args(ix, V.d_tq.as<TermQuery>(), make_bm25(0, 1, 1, 0, ix->doc_lens_nonneg), none);
-    a.mode = TERM_MODE_TF;
-    return launch_term_batch(ix, a, n);
-}
-
-// Raw counts of one phrase / slop query on the view's filtered lists into ix->dense row 0: what phrase_common
-// computes for sa_phrase_freqs on a sliced array.  f_offs / f_lens: the query's filtered lists in ix->filt.
-static int view_phrase_counts(sa_index *ix, const u32 *tids, u32 nt, u32 slop, bool missing, const u64 *f_offs,
-                              const u64 *f_lens) {
-    const u64 stride = sa_padded_docs(ix->n_docs);
-    int rc;
-    if (missing) {                                   // an unknown term: zeros (postings.py:705-708)
-        if ((rc = ix->dense.reserve(stride * sizeof(float)))) return rc;
-        SA_CUDA(cudaMemsetAsync(ix->dense.p, 0, stride * sizeof(float), ix->stream));
-        return SA_OK;
-    }
-    u64 offs[SA_MAX_PHRASE_TERMS], lens[SA_MAX_PHRASE_TERMS], dirs[SA_MAX_PHRASE_TERMS];
-    for (u32 i = 0; i < nt; i++) { offs[i] = f_offs[i]; lens[i] = f_lens[i]; dirs[i] = SA_NO_DIR; }
-    const u64 *d_lists = ix->filt.as<u64>();
-    if (slop > 0) {
-        bool literal;
-        if ((rc = sa_span_is_literal(ix, d_lists, offs, lens, nt, &literal))) return rc;
-        return sa_span_run(ix, d_lists, offs, lens, dirs, nt, slop, literal, nullptr);
-    }
-    std::vector<PhraseQuery> pqs(1, make_phrase_query(tids, nt, offs, lens, dirs, 0.0f, false));
-    PhraseDump nodump;
-    memset(&nodump, 0, sizeof(nodump));
-    return sa_phrase_run_sync(ix, pqs, d_lists, 0, make_bm25(0, 1, 1, 0, ix->doc_lens_nonneg), nodump, true);
-}
-
-static bool query_missing(const sa_index *ix, const u32 *tids, u32 nt) {
-    for (u32 i = 0; i < nt; i++)
-        if (tids[i] == SA_NO_TERM || ix->h_len[tids[i]] == 0) return true;
-    return false;
-}
-
-// keys (and the overflow flags) to the host in one copy and one synchronise
-static int view_download(sa_index *ix, u32 nq, u32 k, uint32_t *out_pos, float *out_scores, std::vector<u32> *ovf) {
-    ViewState &V = *ix->view;
-    const size_t nk = (size_t)nq * k, ovf_bytes = ovf ? (size_t)nq * sizeof(u32) : 0;
-    int rc;
-    if ((rc = sa_pinned_reserve(ix, nk * sizeof(u64) + ovf_bytes))) return rc;
-    SA_CUDA(cudaMemcpyAsync(ix->h_pinned, V.d_keys.p, nk * sizeof(u64), cudaMemcpyDeviceToHost, ix->stream));
-    if (ovf)
-        SA_CUDA(cudaMemcpyAsync((u64 *)ix->h_pinned + nk, V.d_ovf.p, ovf_bytes, cudaMemcpyDeviceToHost, ix->stream));
-    SA_CUDA(cudaStreamSynchronize(ix->stream));
-    sa_unpack_keys((const u64 *)ix->h_pinned, nk, out_pos, out_scores);
-    if (ovf) ovf->assign((const u32 *)((u64 *)ix->h_pinned + nk), (const u32 *)((u64 *)ix->h_pinned + nk) + nq);
-    return SA_OK;
-}
-
-extern "C" int sa_score_batch_topk_rows(sa_index *ix, const uint32_t *terms, const uint32_t *term_starts,
-                                        const float *idf, uint32_t n_queries, uint32_t slop,
-                                        const float *view_doc_lens, float avg_doc_len, float k1, float b, uint32_t k,
-                                        uint32_t *out_pos, float *out_scores) {
-    SA_CHECK(ix, "index is NULL");
-    SA_CHECK(n_queries == 0 || (terms && term_starts && idf && out_pos && out_scores), "NULL argument");
-    SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
-    int rc;
-    for (u32 q = 0; q < n_queries; q++) {
-        const u32 nt = term_starts[q + 1] - term_starts[q];
-        SA_CHECK(nt >= 1 && nt <= SA_MAX_PHRASE_TERMS, "query %u: bad number of terms", q);
-        if ((rc = sa_check_term_ids(ix, terms + term_starts[q], nt))) return rc;
-    }
-    std::lock_guard<std::mutex> g(ix->mu);
-    SA_CHECK(ix->rows_active, "no row filter installed (sa_index_set_rows)");
-    const u64 n_rows = ix->n_rows;
-    SA_CHECK(n_rows < 0xFFFFFFFFull, "a view must have fewer than 2^32 - 1 rows");
-    SA_CHECK(n_rows == 0 || view_doc_lens, "view_doc_lens is NULL");
-    SA_CUDA(cudaSetDevice(ix->device));
-    const size_t nk = (size_t)n_queries * k;
-    if (n_queries == 0 || n_rows == 0 || avg_doc_len == 0.0f) {     // .score is all zeros: nothing ranks
-        for (size_t i = 0; i < nk; i++) { out_pos[i] = SA_NO_DOC; out_scores[i] = 0.0f; }
-        return SA_OK;
-    }
-    if (!ix->view) ix->view = new ViewState();
-    ViewState &V = *ix->view;
-    const u64 stride = sa_padded_docs(ix->n_docs), vstride = sa_padded_docs(n_rows);
-    const u32 n_vtiles = sa_n_tiles(n_rows), slots = sa_topk_slots(k);
-    // chunk so the doc-space and view-space rows of one chunk stay within ~4 GB of HBM
-    const u32 chunk = (u32)std::min<u64>(65535, std::max<u64>(1, std::min<u64>(n_queries,
-                                         (4ull << 30) / ((stride + vstride) * sizeof(float)))));
-    // Every buffer is reserved before the first write: DevBuf::reserve does not keep the contents.  ix->dense is the
-    // exception -- each step reserves it and consumes what it wrote before the next reserve.
-    if ((rc = V.d_dl.reserve(vstride * sizeof(float)))) return rc;
-    if ((rc = V.d_vrows.reserve((size_t)chunk * vstride * sizeof(float)))) return rc;
-    if ((rc = V.d_tq.reserve((size_t)chunk * sizeof(TermQuery)))) return rc;
-    if ((rc = V.d_idf.reserve((size_t)n_queries * sizeof(float)))) return rc;
-    if ((rc = V.d_row_query.reserve((size_t)n_queries * sizeof(u32)))) return rc;
-    if ((rc = V.d_ovf.reserve((size_t)n_queries * sizeof(u32)))) return rc;
-    if ((rc = V.d_keys.reserve(nk * sizeof(u64)))) return rc;
-    if ((rc = ix->cand.reserve(cand_bytes(n_vtiles, chunk, slots)))) return rc;
-
-    // rows: chunk by chunk, the term queries first, then the phrase queries
-    struct Chunk { u32 row0, n_term, n_phrase; };
-    std::vector<Chunk> chunks;
-    std::vector<u32> row_query;
-    std::vector<float> row_idf;
-    row_query.reserve(n_queries);
-    row_idf.reserve(n_queries);
-    for (u32 q0 = 0; q0 < n_queries; q0 += chunk) {
-        const u32 q1 = std::min(n_queries, q0 + chunk);
-        Chunk C{(u32)row_query.size(), 0, 0};
-        for (int pass = 0; pass < 2; pass++)
-            for (u32 q = q0; q < q1; q++) {
-                const bool term = term_starts[q + 1] - term_starts[q] == 1;
-                if (term != (pass == 0)) continue;
-                row_query.push_back(q);
-                row_idf.push_back(idf[q]);
-                (term ? C.n_term : C.n_phrase)++;
-            }
-        chunks.push_back(C);
-    }
-    SA_CUDA(cudaMemcpyAsync(V.d_dl.p, view_doc_lens, n_rows * sizeof(float), cudaMemcpyHostToDevice, ix->stream));
-    SA_CUDA(cudaMemcpyAsync(V.d_idf.p, row_idf.data(), n_queries * sizeof(float), cudaMemcpyHostToDevice, ix->stream));
-    SA_CUDA(cudaMemcpyAsync(V.d_row_query.p, row_query.data(), n_queries * sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
-    SA_CUDA(cudaMemsetAsync(V.d_ovf.p, 0, n_queries * sizeof(u32), ix->stream));
-    // BM25 exactly as ops.bm25_score -> sa_op_bm25_score sets it up (idf per row, in the kernel)
-    const Bm25Params p = make_bm25(0.0f, avg_doc_len, k1, b, false);
-    const float *d_idf = V.d_idf.as<float>();
-
-    for (const Chunk &C : chunks) {
-        const u32 Q = C.n_term + C.n_phrase;
-        TopkCtx t = make_topk_ctx(ix->cand.p, n_vtiles, Q, slots, k, V.d_ovf.as<u32>() + C.row0);
-        if (C.n_phrase) {
-            // one filter pass over every list of the chunk's phrases (a phrase with a missing term has none)
-            std::vector<u32> ftids, fstart;
-            std::vector<unsigned char> missing;
-            for (u32 j = 0; j < C.n_phrase; j++) {
-                const u32 q = row_query[C.row0 + C.n_term + j];
-                const u32 *tids = terms + term_starts[q];
-                const u32 nt = term_starts[q + 1] - term_starts[q];
-                fstart.push_back((u32)ftids.size());
-                missing.push_back(query_missing(ix, tids, nt));
-                if (!missing.back()) ftids.insert(ftids.end(), tids, tids + nt);
-            }
-            std::vector<u64> f_offs, f_lens;
-            if (!ftids.empty() && (rc = sa_filter_terms_mask(ix, ftids.data(), (u32)ftids.size(), ix->d_row_mask, 0,
-                                                             SA_ALL_BITS, false, f_offs, f_lens, nullptr))) return rc;
-            for (u32 j = 0; j < C.n_phrase; j++) {
-                const u32 q = row_query[C.row0 + C.n_term + j];
-                const u32 *tids = terms + term_starts[q];
-                const u32 nt = term_starts[q + 1] - term_starts[q];
-                const u64 *fo = missing[j] ? nullptr : f_offs.data() + fstart[j];
-                const u64 *fl = missing[j] ? nullptr : f_lens.data() + fstart[j];
-                if ((rc = view_phrase_counts(ix, tids, nt, slop, missing[j], fo, fl))) return rc;
-                if ((rc = launch_view_tiles(ix, ix->dense.as<float>(), stride, d_idf + C.row0 + C.n_term + j, 1,
-                                            C.n_term + j, p, t))) return rc;
-            }
-        }
-        if (C.n_term) {
-            // A view keeps or drops WHOLE docs (no position filter here), so a doc of the view has the same tf in the
-            // filtered list as in the index's own list: the term kernel runs on the own lists, with the tf table, and
-            // no compaction.  Docs outside the view get counts too; view_tile_kernel never gathers them.
-            std::vector<TermQuery> tqs(C.n_term);
-            for (u32 j = 0; j < C.n_term; j++) tqs[j] = make_term_query(ix, terms[term_starts[row_query[C.row0 + j]]], 0.0f);
-            if ((rc = view_term_counts(ix, tqs.data(), C.n_term))) return rc;
-            if ((rc = launch_view_tiles(ix, ix->dense.as<float>(), stride, d_idf + C.row0, C.n_term, 0, p, t))) return rc;
-        }
-        if ((rc = launch_topk_select(ix, t, Q, 0, V.d_keys.as<u64>(), V.d_row_query.as<u32>() + C.row0))) return rc;
-    }
-    std::vector<u32> ovf;
-    if ((rc = view_download(ix, n_queries, k, out_pos, out_scores, &ovf))) return rc;
-    bool redone = false;
-    for (u32 r = 0; r < n_queries; r++) {
-        if (!ovf[r]) continue;
-        // exact re-run of one query: a candidate slot per position of the tile cannot overflow
-        const u32 q = row_query[r];
-        const u32 *tids = terms + term_starts[q];
-        const u32 nt = term_starts[q + 1] - term_starts[q];
-        if (nt == 1) {
-            TermQuery tq = make_term_query(ix, tids[0], 0.0f);
-            if ((rc = view_term_counts(ix, &tq, 1))) return rc;
-        } else {
-            const bool miss = query_missing(ix, tids, nt);
-            std::vector<u64> f_offs, f_lens;
-            if (!miss && (rc = sa_filter_terms_mask(ix, tids, nt, ix->d_row_mask, 0, SA_ALL_BITS, false, f_offs, f_lens,
-                                                    nullptr))) return rc;
-            if ((rc = view_phrase_counts(ix, tids, nt, slop, miss, f_offs.data(), f_lens.data()))) return rc;
-        }
-        if ((rc = ix->cand.reserve(cand_bytes(n_vtiles, 1, SA_TILE_DOCS)))) return rc;
-        SA_CUDA(cudaMemsetAsync(V.d_ovf.as<u32>() + r, 0, sizeof(u32), ix->stream));
-        TopkCtx t = make_topk_ctx(ix->cand.p, n_vtiles, 1, SA_TILE_DOCS, k, V.d_ovf.as<u32>() + r);
-        if ((rc = launch_view_tiles(ix, ix->dense.as<float>(), stride, d_idf + r, 1, 0, p, t))) return rc;
-        if ((rc = launch_topk_select(ix, t, 1, 0, V.d_keys.as<u64>(), V.d_row_query.as<u32>() + r))) return rc;
-        redone = true;
-    }
-    if (!redone) return SA_OK;
-    return view_download(ix, n_queries, k, out_pos, out_scores, nullptr);
-}
-
-// ------------------------------------------------ the other similarities (sa_score_batch_topk_sim)
-// grid = (tiles of positions, queries), as view_tile_kernel.  Position i reads its count at doc = rows[i] on a view
-// (rows == NULL: the unsliced array, doc = i) and its doc length at doc_lens[doc], which is SearchArray.doclengths()
-// -- not the stepped-slice lengths view_tile_kernel uses, a quirk of bm25_score only.  A zero count never scores
-// > 0 under any of the three formulas (0 / x, 0 * l and sqrt(0) give +-0 or NaN, and the idf is finite), so the
-// doc length is loaded only where the count is > 0.  What the tile ranks by, and how:
-//   impact:  the float32 score itself; flush_tile_collect and topk_select_kernel apply unchanged.
+// grid = (tiles of positions, queries).  row = row0 + blockIdx.y indexes the candidate slots and the overflow flags;
+// doc_rows + blockIdx.y * doc_stride is the query's doc-space count row, idf[blockIdx.y] its idf.  Position i reads
+// its count at doc = rows[i] on a view (rows == NULL: the unsliced array, doc = i) and its doc length at
+//   SA_SIM_BM25: doc_lens[i], the lengths the view's BM25 uses (the stepped-slice quirk of bm25_score);
+//   the others:  doc_lens[doc], SearchArray.doclengths().
+// A zero count never scores > 0 under any of the formulas (0 / x, 0 * l and sqrt(0) give +-0 or NaN, and the idf
+// cannot turn them positive), so the doc length is loaded only where the count is > 0.  What the tile ranks by, and
+// how:
+//   BM25:    the float32 score bm25_one(count, dl, p), with the row's idf narrowed back to the float32 the caller
+//            rounded it from; flush_tile_collect and topk_select_kernel apply unchanged.
+//   impact:  the float32 score itself, as BM25.
 //   legacy:  score = fl64(idf * (double)sat), sat the float32 saturation, idf finite.  For idf > 0 it is strictly
 //            increasing in sat: two distinct float32 sats differ by a relative 2^-24 at least, the double product
 //            of each is exact to a relative 2^-53 -- their order survives the rounding (and both the float32 and
@@ -332,8 +82,8 @@ extern "C" int sa_score_batch_topk_rows(sa_index *ix, const uint32_t *terms, con
 template <int KIND>
 __global__ void __launch_bounds__(SA_TERM_THREADS)
 sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *__restrict__ rows,
-                const float *__restrict__ doc_lens, u64 n_pos, SimParams p, const double *__restrict__ idf,
-                float *__restrict__ out_rows, u64 out_stride, u32 row0, const TopkCtx t, u64 *__restrict__ tile_d) {
+                const float *__restrict__ doc_lens, u64 n_pos, TileParams<KIND> p, const double *__restrict__ idf,
+                u32 row0, const TopkCtx t, u64 *__restrict__ tile_d) {
     constexpr int PER_THREAD = SA_TILE_DOCS / SA_TERM_THREADS;
     __shared__ __align__(16) float s_out[KIND == SA_SIM_CLASSIC ? 4 : SA_TILE_DOCS];
     __shared__ u32 s_top[(SA_TERM_THREADS / 32) * 8];
@@ -343,6 +93,7 @@ sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *_
     const u64 pos0 = (u64)tile * SA_TILE_DOCS;
     const float *__restrict__ counts = doc_rows + (u64)blockIdx.y * doc_stride;
     const double q_idf = idf[blockIdx.y];
+    if constexpr (KIND == SA_SIM_BM25) p.idf = (float)q_idf;
     u32 my_max = 0;
     u32 key[PER_THREAD];          // classic: the proxy bits of the thread's positions
     // thread tid owns positions 4g .. 4g+3 of the tile for g = tid + j * SA_TERM_THREADS (flush_tile_collect's layout)
@@ -358,10 +109,12 @@ sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *_
                 const u64 doc = rows ? __ldg(rows + i) : i;
                 const float tf = __ldg(counts + doc);
                 if (tf > 0.0f) {
-                    const float dl = __ldg(doc_lens + doc);
-                    if (KIND == SA_SIM_BM25_IMPACT) {
+                    const float dl = __ldg(doc_lens + (KIND == SA_SIM_BM25 ? i : doc));
+                    if constexpr (KIND == SA_SIM_BM25) {
+                        v[e] = bm25_one(tf, dl, p);
+                    } else if constexpr (KIND == SA_SIM_BM25_IMPACT) {
                         v[e] = sim_impact(tf, dl, p);
-                    } else if (KIND == SA_SIM_BM25_LEGACY) {
+                    } else if constexpr (KIND == SA_SIM_BM25_LEGACY) {
                         const float sat = sim_legacy_sat(tf, dl, p);
                         v[e] = q_idf > 0.0 ? sat : (q_idf < 0.0 ? -sat : 0.0f);
                     } else {
@@ -377,8 +130,9 @@ sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *_
     }
     const u32 n_items = (u32)min((u64)SA_TILE_DOCS, n_pos - pos0);
     if (KIND != SA_SIM_CLASSIC) {
-        flush_tile_collect(s_out, out_rows + (u64)row * out_stride + pos0, t, row, tile, my_max, n_items,
-                           min((u32)SA_TERM_THREADS, (n_items + 3) / 4), s_top, &s_ncand, &s_tile_max);
+        // nothing reads the scores outside the tile: collect the candidates without storing the row
+        flush_tile_collect<false>(s_out, nullptr, t, row, tile, my_max, n_items,
+                                  min((u32)SA_TERM_THREADS, (n_items + 3) / 4), s_top, &s_ncand, &s_tile_max);
         return;
     }
     // classic: the tile bound as flush_tile_collect computes it (8 values per warp), then every proxy >= it
@@ -424,21 +178,34 @@ sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *_
     }
 }
 
-// counts of row r (rows [row0, row0 + n_queries) of the chunk) in doc_rows + r * doc_stride
-static int launch_sim_tiles(sa_index *ix, int kind, const float *doc_rows, u64 doc_stride, const double *d_idf,
-                            u32 n_queries, u32 row0, const SimParams &p, const TopkCtx &t) {
+// One call's queries and scoring.
+struct SimRun {
+    int kind;                 // SA_SIM_*
+    Bm25Params bm25;          // SA_SIM_BM25 (the idf is set per row, in the kernel)
+    SimParams sim;            // the other kinds
+    const u32 *terms, *term_starts;
+    u32 slop;
+    const u32 *tids(u32 q) const { return terms + term_starts[q]; }
+    u32 n_terms(u32 q) const { return term_starts[q + 1] - term_starts[q]; }
+};
+
+// The tile pass over ix->dense rows [0, n): row j holds the counts of row row0 + j of t, d_idf[j] is its idf.
+static int launch_tiles(sa_index *ix, const SimRun &R, const double *d_idf, u32 n, u32 row0, const TopkCtx &t) {
     ViewState &V = *ix->view;
-    if (n_queries == 0 || t.n_tiles == 0) return SA_OK;
+    if (n == 0 || t.n_tiles == 0) return SA_OK;
+    const float *counts = ix->dense.as<float>();
+    const u64 stride = sa_padded_docs(ix->n_docs);
     const u64 *rows = ix->rows_active ? ix->d_rows : nullptr;
     const u64 n_pos = ix->rows_active ? ix->n_rows : ix->n_docs;
-    const dim3 grid(t.n_tiles, n_queries);
+    const dim3 grid(t.n_tiles, n);
     KernelTimer tm(ix, 1);
-#define SA_SIM_TILES(KIND)                                                                                         \
-    sim_tile_kernel<KIND><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(doc_rows, doc_stride, rows, ix->d_doc_lens,    \
-        n_pos, p, d_idf, V.d_vrows.as<float>(), sa_padded_docs(n_pos), row0, t, V.d_cand_d.as<u64>())
-    if (kind == SA_SIM_BM25_IMPACT) SA_SIM_TILES(SA_SIM_BM25_IMPACT);
-    else if (kind == SA_SIM_BM25_LEGACY) SA_SIM_TILES(SA_SIM_BM25_LEGACY);
-    else SA_SIM_TILES(SA_SIM_CLASSIC);
+#define SA_SIM_TILES(KIND, DOC_LENS, P)                                                                              \
+    sim_tile_kernel<KIND><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(counts, stride, rows, DOC_LENS, n_pos, P, d_idf, \
+                                                                    row0, t, V.d_cand_d.as<u64>())
+    if (R.kind == SA_SIM_BM25) SA_SIM_TILES(SA_SIM_BM25, V.d_dl.as<float>(), R.bm25);
+    else if (R.kind == SA_SIM_BM25_IMPACT) SA_SIM_TILES(SA_SIM_BM25_IMPACT, ix->d_doc_lens, R.sim);
+    else if (R.kind == SA_SIM_BM25_LEGACY) SA_SIM_TILES(SA_SIM_BM25_LEGACY, ix->d_doc_lens, R.sim);
+    else SA_SIM_TILES(SA_SIM_CLASSIC, ix->d_doc_lens, R.sim);
 #undef SA_SIM_TILES
     SA_CUDA(cudaGetLastError());
     tm.stop();
@@ -447,13 +214,59 @@ static int launch_sim_tiles(sa_index *ix, int kind, const float *doc_rows, u64 d
     return SA_OK;
 }
 
-static int launch_sim_select(sa_index *ix, int kind, const TopkCtx &t, u32 n_queries, const u32 *d_out_index) {
+static int launch_select(sa_index *ix, int kind, const TopkCtx &t, u32 n_queries, const u32 *d_out_index) {
     ViewState &V = *ix->view;
     const u64 doc_base = ix->rows_active ? 0 : ix->doc_base;    // a view returns positions, an array doc ids
     if (kind == SA_SIM_CLASSIC)
         return launch_topk_select_f64(ix, t, V.d_cand_d.as<u64>(), n_queries, doc_base, V.d_keys.as<u64>(),
                                       V.d_scores.as<double>(), d_out_index);
     return launch_topk_select(ix, t, n_queries, doc_base, V.d_keys.as<u64>(), d_out_index);
+}
+
+// Term queries qs[0, n): their tf into ix->dense rows [0, n), then their tile pass (rows row0 + j of t, idf
+// d_idf[j]).  A view keeps or drops WHOLE docs (no position filter here), so a doc of the view has the same tf in the
+// filtered list as in the index's own list: the term kernel runs on the own lists, with the tf table, and no
+// compaction.  Docs outside the view get counts too; the tile pass never gathers them.
+static int term_tiles(sa_index *ix, const SimRun &R, const u32 *qs, u32 n, const double *d_idf, u32 row0,
+                      const TopkCtx &t) {
+    ViewState &V = *ix->view;
+    if (n == 0) return SA_OK;
+    std::vector<TermQuery> tqs(n);
+    for (u32 j = 0; j < n; j++) tqs[j] = make_term_query(ix, R.tids(qs[j])[0], 0.0f);
+    int rc;
+    if ((rc = ix->dense.reserve((size_t)n * sa_padded_docs(ix->n_docs) * sizeof(float)))) return rc;
+    SA_CUDA(cudaMemcpyAsync(V.d_tq.p, tqs.data(), n * sizeof(TermQuery), cudaMemcpyHostToDevice, ix->stream));
+    TopkCtx none;
+    memset(&none, 0, sizeof(none));
+    TermBatchArgs a = make_term_args(ix, V.d_tq.as<TermQuery>(), make_bm25(0, 1, 1, 0, ix->doc_lens_nonneg), none);
+    a.mode = TERM_MODE_TF;
+    if ((rc = launch_term_batch(ix, a, n))) return rc;
+    return launch_tiles(ix, R, d_idf, n, row0, t);
+}
+
+// Raw counts of one phrase / slop query on the view's filtered lists into ix->dense row 0: what phrase_common
+// computes for sa_phrase_freqs on a sliced array.  f_offs / f_lens: the query's filtered lists in ix->filt.
+static int view_phrase_counts(sa_index *ix, const u32 *tids, u32 nt, u32 slop, bool missing, const u64 *f_offs,
+                              const u64 *f_lens) {
+    const u64 stride = sa_padded_docs(ix->n_docs);
+    int rc;
+    if (missing) {                                   // an unknown term: zeros (postings.py:705-708)
+        if ((rc = ix->dense.reserve(stride * sizeof(float)))) return rc;
+        SA_CUDA(cudaMemsetAsync(ix->dense.p, 0, stride * sizeof(float), ix->stream));
+        return SA_OK;
+    }
+    u64 offs[SA_MAX_PHRASE_TERMS], lens[SA_MAX_PHRASE_TERMS], dirs[SA_MAX_PHRASE_TERMS];
+    for (u32 i = 0; i < nt; i++) { offs[i] = f_offs[i]; lens[i] = f_lens[i]; dirs[i] = SA_NO_DIR; }
+    const u64 *d_lists = ix->filt.as<u64>();
+    if (slop > 0) {
+        bool literal;
+        if ((rc = sa_span_is_literal(ix, d_lists, offs, lens, nt, &literal))) return rc;
+        return sa_span_run(ix, d_lists, offs, lens, dirs, nt, slop, literal, nullptr);
+    }
+    std::vector<PhraseQuery> pqs(1, make_phrase_query(tids, nt, offs, lens, dirs, 0.0f, false));
+    PhraseDump nodump;
+    memset(&nodump, 0, sizeof(nodump));
+    return sa_phrase_run_sync(ix, pqs, d_lists, 0, make_bm25(0, 1, 1, 0, ix->doc_lens_nonneg), nodump, true);
 }
 
 // Raw counts of one phrase / slop query on the index's own lists into ix->dense row 0: what phrase_common computes
@@ -471,9 +284,45 @@ static int own_phrase_counts(sa_index *ix, const u32 *tids, u32 nt, u32 slop) {
     return sa_phrase_run_sync(ix, pqs, ix->d_words, 0, make_bm25(0, 1, 1, 0, ix->doc_lens_nonneg), nodump, true);
 }
 
+static bool query_missing(const sa_index *ix, const u32 *tids, u32 nt) {
+    for (u32 i = 0; i < nt; i++)
+        if (tids[i] == SA_NO_TERM || ix->h_len[tids[i]] == 0) return true;
+    return false;
+}
+
+// Phrase / slop queries qs[0, n), one at a time: raw counts into ix->dense row 0, then the query's tile pass (row
+// row0 + j of t, idf d_idf[j]).  On a view, one filter pass over every list of the n queries comes first (a query
+// with a missing term has none).
+static int phrase_tiles(sa_index *ix, const SimRun &R, const u32 *qs, u32 n, const double *d_idf, u32 row0,
+                        const TopkCtx &t) {
+    const bool view = ix->rows_active;
+    std::vector<u32> ftids, fstart;
+    std::vector<unsigned char> missing;
+    std::vector<u64> f_offs, f_lens;
+    int rc;
+    for (u32 j = 0; j < n && view; j++) {
+        const u32 *tids = R.tids(qs[j]);
+        const u32 nt = R.n_terms(qs[j]);
+        fstart.push_back((u32)ftids.size());
+        missing.push_back(query_missing(ix, tids, nt));
+        if (!missing.back()) ftids.insert(ftids.end(), tids, tids + nt);
+    }
+    if (!ftids.empty() && (rc = sa_filter_terms_mask(ix, ftids.data(), (u32)ftids.size(), ix->d_row_mask, 0,
+                                                     SA_ALL_BITS, false, f_offs, f_lens, nullptr))) return rc;
+    for (u32 j = 0; j < n; j++) {
+        const u32 *tids = R.tids(qs[j]);
+        const u32 nt = R.n_terms(qs[j]);
+        if (!view) rc = own_phrase_counts(ix, tids, nt, R.slop);
+        else if (missing[j]) rc = view_phrase_counts(ix, tids, nt, R.slop, true, nullptr, nullptr);
+        else rc = view_phrase_counts(ix, tids, nt, R.slop, false, f_offs.data() + fstart[j], f_lens.data() + fstart[j]);
+        if (rc || (rc = launch_tiles(ix, R, d_idf + j, 1, row0 + j, t))) return rc;
+    }
+    return SA_OK;
+}
+
 // keys (the classic scores, the overflow flags) to the host in one copy each and one synchronise
-static int sim_download(sa_index *ix, bool classic, u32 nq, u32 k, std::vector<u64> &keys, std::vector<double> &scores,
-                        std::vector<u32> *ovf) {
+static int download(sa_index *ix, bool classic, u32 nq, u32 k, std::vector<u64> &keys, std::vector<double> &scores,
+                    std::vector<u32> *ovf) {
     ViewState &V = *ix->view;
     const size_t nk = (size_t)nq * k;
     int rc;
@@ -493,47 +342,55 @@ static int sim_download(sa_index *ix, bool classic, u32 nq, u32 k, std::vector<u
 }
 
 extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *terms, const uint32_t *term_starts,
-                                       const double *idf, uint32_t n_queries, uint32_t slop, double avg_doc_len,
-                                       double k1, double b, uint32_t k, uint32_t *out_ids, double *out_scores) {
+                                       const double *idf, uint32_t n_queries, uint32_t slop,
+                                       const float *view_doc_lens, double avg_doc_len, double k1, double b,
+                                       uint32_t k, uint32_t *out_ids, double *out_scores) {
     SA_CHECK(ix, "index is NULL");
     SA_CHECK(n_queries == 0 || (terms && term_starts && idf && out_ids && out_scores), "NULL argument");
-    SA_CHECK(kind == SA_SIM_BM25_IMPACT || kind == SA_SIM_BM25_LEGACY || kind == SA_SIM_CLASSIC, "unknown similarity %d", kind);
+    SA_CHECK(kind == SA_SIM_BM25 || kind == SA_SIM_BM25_IMPACT || kind == SA_SIM_BM25_LEGACY || kind == SA_SIM_CLASSIC,
+             "unknown similarity %d", kind);
     SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
+    const bool classic = kind == SA_SIM_CLASSIC;
     int rc;
     for (u32 q = 0; q < n_queries; q++) {
         const u32 nt = term_starts[q + 1] - term_starts[q];
         SA_CHECK(nt >= 1 && nt <= SA_MAX_PHRASE_TERMS, "query %u: bad number of terms", q);
         if ((rc = sa_check_term_ids(ix, terms + term_starts[q], nt))) return rc;
-        SA_CHECK(kind == SA_SIM_BM25_IMPACT || std::isfinite(idf[q]), "query %u: idf is not finite", q);
+        SA_CHECK((kind != SA_SIM_BM25_LEGACY && !classic) || std::isfinite(idf[q]), "query %u: idf is not finite", q);
     }
     std::lock_guard<std::mutex> g(ix->mu);
     const bool view = ix->rows_active;
+    SA_CHECK(view || kind != SA_SIM_BM25, "no row filter installed (sa_index_set_rows)");
     const u64 n_pos = view ? ix->n_rows : ix->n_docs;
     SA_CHECK(n_pos < 0xFFFFFFFFull, "the array must have fewer than 2^32 - 1 rows");
+    SA_CHECK(kind != SA_SIM_BM25 || n_pos == 0 || view_doc_lens, "view_doc_lens is NULL");
     SA_CUDA(cudaSetDevice(ix->device));
     const size_t nk = (size_t)n_queries * k;
     for (size_t i = 0; i < nk; i++) { out_ids[i] = SA_NO_DOC; out_scores[i] = 0.0; }
-    // impact and legacy score zeros at avgdl == 0 (similarity.py:49-50, 66-67); classic has no such branch
-    if (n_queries == 0 || n_pos == 0 || (kind != SA_SIM_CLASSIC && avg_doc_len == 0.0)) return SA_OK;
+    // BM25 (its float32 avgdl, as it runs), impact and legacy score zeros at avgdl == 0 (similarity.py:49-50, 66-67);
+    // classic has no such branch
+    const bool zero_avgdl = kind == SA_SIM_BM25 ? (float)avg_doc_len == 0.0f : avg_doc_len == 0.0;
+    if (n_queries == 0 || n_pos == 0 || (!classic && zero_avgdl)) return SA_OK;
     if (!ix->view) ix->view = new ViewState();
     ViewState &V = *ix->view;
-    const bool classic = kind == SA_SIM_CLASSIC;
-    const u64 stride = sa_padded_docs(ix->n_docs), pstride = sa_padded_docs(n_pos);
-    const u32 n_ptiles = sa_n_tiles(n_pos), slots = classic ? 256u : sa_topk_slots(k);
-    // chunk so the doc-space and position-space rows of one chunk stay within ~4 GB of HBM
+    // BM25 exactly as ops.bm25_score -> sa_op_bm25_score sets it up: float32 parameters, `1 - b` in float32
+    const SimRun R{kind, make_bm25(0.0f, (float)avg_doc_len, (float)k1, (float)b, false),
+                   make_sim_params(avg_doc_len, k1, b), terms, term_starts, slop};
+    const u32 n_tiles = sa_n_tiles(n_pos), slots = classic ? 256u : sa_topk_slots(k);
+    // chunk so the doc-space count rows of one chunk stay within ~4 GB of HBM, as sa_batch_upload_locked does
     const u32 chunk = (u32)std::min<u64>(65535, std::max<u64>(1, std::min<u64>(n_queries,
-                                         (4ull << 30) / ((stride + pstride) * sizeof(float)))));
+                                         (4ull << 30) / (sa_padded_docs(ix->n_docs) * sizeof(float)))));
     // Every buffer is reserved before the first write: DevBuf::reserve does not keep the contents.  ix->dense is the
     // exception -- each step reserves it and consumes what it wrote before the next reserve.
-    if (!classic && (rc = V.d_vrows.reserve((size_t)chunk * pstride * sizeof(float)))) return rc;
+    if (kind == SA_SIM_BM25 && (rc = V.d_dl.reserve(n_pos * sizeof(float)))) return rc;
     if ((rc = V.d_tq.reserve((size_t)chunk * sizeof(TermQuery)))) return rc;
     if ((rc = V.d_idf.reserve((size_t)n_queries * sizeof(double)))) return rc;
     if ((rc = V.d_row_query.reserve((size_t)n_queries * sizeof(u32)))) return rc;
     if ((rc = V.d_ovf.reserve((size_t)n_queries * sizeof(u32)))) return rc;
     if ((rc = V.d_keys.reserve(nk * sizeof(u64)))) return rc;
-    if ((rc = ix->cand.reserve(cand_bytes(n_ptiles, chunk, slots)))) return rc;
+    if ((rc = ix->cand.reserve(cand_bytes(n_tiles, chunk, slots)))) return rc;
     if (classic && (rc = V.d_scores.reserve(nk * sizeof(double)))) return rc;
-    if (classic && (rc = V.d_cand_d.reserve((size_t)chunk * n_ptiles * slots * sizeof(u64)))) return rc;
+    if (classic && (rc = V.d_cand_d.reserve((size_t)chunk * n_tiles * slots * sizeof(u64)))) return rc;
 
     // rows: chunk by chunk, the term queries first, then the phrase queries
     struct Chunk { u32 row0, n_term, n_phrase; };
@@ -547,7 +404,7 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
         Chunk C{(u32)row_query.size(), 0, 0};
         for (int pass = 0; pass < 2; pass++)
             for (u32 q = q0; q < q1; q++) {
-                const bool term = term_starts[q + 1] - term_starts[q] == 1;
+                const bool term = R.n_terms(q) == 1;
                 if (term != (pass == 0)) continue;
                 row_query.push_back(q);
                 row_idf.push_back(idf[q]);
@@ -555,87 +412,39 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
             }
         chunks.push_back(C);
     }
+    if (kind == SA_SIM_BM25)
+        SA_CUDA(cudaMemcpyAsync(V.d_dl.p, view_doc_lens, n_pos * sizeof(float), cudaMemcpyHostToDevice, ix->stream));
     SA_CUDA(cudaMemcpyAsync(V.d_idf.p, row_idf.data(), n_queries * sizeof(double), cudaMemcpyHostToDevice, ix->stream));
     SA_CUDA(cudaMemcpyAsync(V.d_row_query.p, row_query.data(), n_queries * sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
     SA_CUDA(cudaMemsetAsync(V.d_ovf.p, 0, n_queries * sizeof(u32), ix->stream));
-    const SimParams p = make_sim_params(avg_doc_len, k1, b);
     const double *d_idf = V.d_idf.as<double>();
 
     for (const Chunk &C : chunks) {
         const u32 Q = C.n_term + C.n_phrase;
-        TopkCtx t = make_topk_ctx(ix->cand.p, n_ptiles, Q, slots, k, V.d_ovf.as<u32>() + C.row0);
-        if (C.n_phrase) {
-            // on a view, one filter pass over every list of the chunk's phrases (a phrase with a missing term has none)
-            std::vector<u32> ftids, fstart;
-            std::vector<unsigned char> missing;
-            for (u32 j = 0; j < C.n_phrase && view; j++) {
-                const u32 q = row_query[C.row0 + C.n_term + j];
-                const u32 *tids = terms + term_starts[q];
-                const u32 nt = term_starts[q + 1] - term_starts[q];
-                fstart.push_back((u32)ftids.size());
-                missing.push_back(query_missing(ix, tids, nt));
-                if (!missing.back()) ftids.insert(ftids.end(), tids, tids + nt);
-            }
-            std::vector<u64> f_offs, f_lens;
-            if (!ftids.empty() && (rc = sa_filter_terms_mask(ix, ftids.data(), (u32)ftids.size(), ix->d_row_mask, 0,
-                                                             SA_ALL_BITS, false, f_offs, f_lens, nullptr))) return rc;
-            for (u32 j = 0; j < C.n_phrase; j++) {
-                const u32 q = row_query[C.row0 + C.n_term + j];
-                const u32 *tids = terms + term_starts[q];
-                const u32 nt = term_starts[q + 1] - term_starts[q];
-                if (view) {
-                    const u64 *fo = missing[j] ? nullptr : f_offs.data() + fstart[j];
-                    const u64 *fl = missing[j] ? nullptr : f_lens.data() + fstart[j];
-                    rc = view_phrase_counts(ix, tids, nt, slop, missing[j], fo, fl);
-                } else {
-                    rc = own_phrase_counts(ix, tids, nt, slop);
-                }
-                if (rc) return rc;
-                if ((rc = launch_sim_tiles(ix, kind, ix->dense.as<float>(), stride, d_idf + C.row0 + C.n_term + j, 1,
-                                           C.n_term + j, p, t))) return rc;
-            }
-        }
-        if (C.n_term) {
-            // the index's own lists, on a view too: a view keeps or drops whole docs (see sa_score_batch_topk_rows)
-            std::vector<TermQuery> tqs(C.n_term);
-            for (u32 j = 0; j < C.n_term; j++) tqs[j] = make_term_query(ix, terms[term_starts[row_query[C.row0 + j]]], 0.0f);
-            if ((rc = view_term_counts(ix, tqs.data(), C.n_term))) return rc;
-            if ((rc = launch_sim_tiles(ix, kind, ix->dense.as<float>(), stride, d_idf + C.row0, C.n_term, 0, p, t))) return rc;
-        }
-        if ((rc = launch_sim_select(ix, kind, t, Q, V.d_row_query.as<u32>() + C.row0))) return rc;
+        const u32 *qs = row_query.data() + C.row0;
+        TopkCtx t = make_topk_ctx(ix->cand.p, n_tiles, Q, slots, k, V.d_ovf.as<u32>() + C.row0);
+        if ((rc = phrase_tiles(ix, R, qs + C.n_term, C.n_phrase, d_idf + C.row0 + C.n_term, C.n_term, t))) return rc;
+        if ((rc = term_tiles(ix, R, qs, C.n_term, d_idf + C.row0, 0, t))) return rc;
+        if ((rc = launch_select(ix, kind, t, Q, V.d_row_query.as<u32>() + C.row0))) return rc;
     }
     std::vector<u64> keys;
     std::vector<double> scores;
     std::vector<u32> ovf;
-    if ((rc = sim_download(ix, classic, n_queries, k, keys, scores, &ovf))) return rc;
+    if ((rc = download(ix, classic, n_queries, k, keys, scores, &ovf))) return rc;
     bool redone = false;
     for (u32 r = 0; r < n_queries; r++) {
         if (!ovf[r]) continue;
         // exact re-run of one query: a candidate slot per position of the tile cannot overflow
-        const u32 q = row_query[r];
-        const u32 *tids = terms + term_starts[q];
-        const u32 nt = term_starts[q + 1] - term_starts[q];
-        if (nt == 1) {
-            TermQuery tq = make_term_query(ix, tids[0], 0.0f);
-            if ((rc = view_term_counts(ix, &tq, 1))) return rc;
-        } else if (view) {
-            const bool miss = query_missing(ix, tids, nt);
-            std::vector<u64> f_offs, f_lens;
-            if (!miss && (rc = sa_filter_terms_mask(ix, tids, nt, ix->d_row_mask, 0, SA_ALL_BITS, false, f_offs, f_lens,
-                                                    nullptr))) return rc;
-            if ((rc = view_phrase_counts(ix, tids, nt, slop, miss, f_offs.data(), f_lens.data()))) return rc;
-        } else if ((rc = own_phrase_counts(ix, tids, nt, slop))) {
-            return rc;
-        }
-        if ((rc = ix->cand.reserve(cand_bytes(n_ptiles, 1, SA_TILE_DOCS)))) return rc;
-        if (classic && (rc = V.d_cand_d.reserve((size_t)n_ptiles * SA_TILE_DOCS * sizeof(u64)))) return rc;
+        if ((rc = ix->cand.reserve(cand_bytes(n_tiles, 1, SA_TILE_DOCS)))) return rc;
+        if (classic && (rc = V.d_cand_d.reserve((size_t)n_tiles * SA_TILE_DOCS * sizeof(u64)))) return rc;
         SA_CUDA(cudaMemsetAsync(V.d_ovf.as<u32>() + r, 0, sizeof(u32), ix->stream));
-        TopkCtx t = make_topk_ctx(ix->cand.p, n_ptiles, 1, SA_TILE_DOCS, k, V.d_ovf.as<u32>() + r);
-        if ((rc = launch_sim_tiles(ix, kind, ix->dense.as<float>(), stride, d_idf + r, 1, 0, p, t))) return rc;
-        if ((rc = launch_sim_select(ix, kind, t, 1, V.d_row_query.as<u32>() + r))) return rc;
+        TopkCtx t = make_topk_ctx(ix->cand.p, n_tiles, 1, SA_TILE_DOCS, k, V.d_ovf.as<u32>() + r);
+        const bool term = R.n_terms(row_query[r]) == 1;
+        if ((rc = (term ? term_tiles : phrase_tiles)(ix, R, &row_query[r], 1, d_idf + r, 0, t))) return rc;
+        if ((rc = launch_select(ix, kind, t, 1, V.d_row_query.as<u32>() + r))) return rc;
         redone = true;
     }
-    if (redone && (rc = sim_download(ix, classic, n_queries, k, keys, scores, nullptr))) return rc;
+    if (redone && (rc = download(ix, classic, n_queries, k, keys, scores, nullptr))) return rc;
     for (u32 q = 0; q < n_queries; q++)
         for (u32 i = 0; i < k; i++) {
             const size_t j = (size_t)q * k + i;
@@ -645,9 +454,9 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
             float f;
             const u32 bits = (u32)(key >> 32);
             memcpy(&f, &bits, sizeof(f));
-            if (kind == SA_SIM_BM25_IMPACT) out_scores[j] = f;
-            else if (kind == SA_SIM_BM25_LEGACY) out_scores[j] = std::fabs(idf[q]) * (double)f;   // f = sign(idf) * sat
-            else out_scores[j] = scores[j];
+            if (kind == SA_SIM_BM25_LEGACY) out_scores[j] = std::fabs(idf[q]) * (double)f;   // f = sign(idf) * sat
+            else if (classic) out_scores[j] = scores[j];
+            else out_scores[j] = f;                                                      // BM25 and impact
         }
     return SA_OK;
 }

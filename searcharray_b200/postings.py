@@ -502,106 +502,72 @@ class SearchArray(ExtensionArray):
         `.score(q, similarity=similarity, slop=slop)` on the same array or view, and the scores have its dtype
         (float32 for bm25_impact, float64 for the other two, also where .score returns float32 zeros because
         avg_doc_length is 0); +inf ranks, NaN never does."""
-        if not isinstance(similarity, Bm25Similarity):
+        if not isinstance(similarity, (Bm25Similarity, Bm25Impact, Bm25Legacy, ClassicSimilarity)):
+            raise TypeError("search_topk supports bm25_similarity, bm25_impact, bm25_legacy_similarity and "
+                            f"classic_similarity, not {similarity!r}")
+        if self.rows is not None or not isinstance(similarity, Bm25Similarity):
             return self._search_topk_sim(queries, k, similarity, slop)
-        if self.rows is not None:
-            return self._search_topk_view(queries, k, similarity, slop)
-        terms, starts, idfs = [], [0], []
-        for q in queries:
-            toks = [q] if isinstance(q, str) else list(q)
-            terms.extend(self._term_id(t) for t in toks)
-            starts.append(len(terms))
-            idfs.append(compute_idf(self.corpus_size, np.asarray([self.docfreq(t) for t in toks])))
-        terms = np.asarray(terms, dtype=np.uint32)
-        starts = np.asarray(starts, dtype=np.uint32)
+        terms, starts, idfs = self._topk_queries(queries, lambda dfs: compute_idf(self.corpus_size, dfs))
         idfs = np.asarray(idfs, dtype=np.float32)
-        docs = np.empty((len(queries), k), dtype=np.uint32)
-        scores = np.empty((len(queries), k), dtype=np.float32)
+        docs = np.empty((len(idfs), k), dtype=np.uint32)
+        scores = np.empty((len(idfs), k), dtype=np.float32)
         dev = self._device()
         with self._shared["lock"]:
             _lib.check(_lib.lib().sa_score_batch_topk(dev.handle, _lib.p_u32(terms), _lib.p_u32(starts),
-                                                      _lib.p_f32(idfs), len(queries), int(slop),
+                                                      _lib.p_f32(idfs), len(idfs), int(slop),
                                                       self.avg_doc_length, similarity.k1, similarity.b, k,
                                                       _lib.p_u32(docs), _lib.p_f32(scores)))
         return docs, scores
 
-    def _search_topk_view(self, queries, k, similarity, slop):
-        """search_topk on a view: the slice's dfs of every distinct token in one device pass, idf per query as
-        .score computes it, then the batched top-k over the view's positions (sa_score_batch_topk_rows)."""
-        if self.comm is not None or self.global_df is not None:
-            raise ValueError("search_topk on a view of a sharded SearchArray is not supported: the slice's document "
-                             "frequencies would need a sum over the ranks; use .score() on the view")
+    def _topk_queries(self, queries, idf):
+        """The queries as the batched top-k entries take them: term ids, start offsets and, per query, idf(dfs) of
+        its tokens' document frequencies -- .docfreq's values, on a view the slice's from one sa_docfreq_rows_batch
+        over the distinct known tokens (call it with the view's rows applied and the lock held)."""
         toks = [[q] if isinstance(q, str) else list(q) for q in queries]
-        docs = np.full((len(toks), k), _lib.NO_DOC, dtype=np.uint32)
-        scores = np.zeros((len(toks), k), dtype=np.float32)
-        if self.avg_doc_length == 0 or not toks:          # .score is all zeros there: nothing ranks
-            return docs, scores
         ids = {t: self._term_id(t) for ts in toks for t in ts}
-        known = [t for t, tid in ids.items() if tid != _lib.NO_TERM]
-        dl = np.ascontiguousarray(self._view_bm25_doc_lens(), dtype=np.float32)
-        dev = self._device()
-        with self._shared["lock"]:
-            self._apply_rows(dev)
+        if self.rows is None:
+            df = {t: self.docfreq(t) for t in ids}
+        else:
+            # .docfreq's values: np.uint64 for a known token, 0 for an unknown one
+            known = [t for t, tid in ids.items() if tid != _lib.NO_TERM]
             dfs = np.zeros(len(known), dtype=np.uint64)
             if known:
                 tids = np.asarray([ids[t] for t in known], dtype=np.uint32)
-                _lib.check(_lib.lib().sa_docfreq_rows_batch(dev.handle, _lib.p_u32(tids), len(tids), _lib.p_u64(dfs)))
-            # the values .docfreq returns: np.uint64 for a known token, 0 for an unknown one
+                _lib.check(_lib.lib().sa_docfreq_rows_batch(self._device().handle, _lib.p_u32(tids), len(tids),
+                                                            _lib.p_u64(dfs)))
             df = dict(zip(known, dfs))
-            terms, starts, idfs = [], [0], []
-            for ts in toks:
-                terms.extend(ids[t] for t in ts)
-                starts.append(len(terms))
-                idfs.append(compute_idf(self.corpus_size, np.asarray([df.get(t, 0) for t in ts])))
-            terms = np.asarray(terms, dtype=np.uint32)
-            starts = np.asarray(starts, dtype=np.uint32)
-            idfs = np.asarray(idfs, dtype=np.float32)
-            _lib.check(_lib.lib().sa_score_batch_topk_rows(dev.handle, _lib.p_u32(terms), _lib.p_u32(starts),
-                                                           _lib.p_f32(idfs), len(toks), int(slop), _lib.p_f32(dl),
-                                                           self.avg_doc_length, similarity.k1, similarity.b, k,
-                                                           _lib.p_u32(docs), _lib.p_f32(scores)))
-        return docs, scores
+        terms, starts, idfs = [], [0], []
+        for ts in toks:
+            terms.extend(ids[t] for t in ts)
+            starts.append(len(terms))
+            idfs.append(idf(np.asarray([df.get(t, 0) for t in ts])))
+        return np.asarray(terms, dtype=np.uint32), np.asarray(starts, dtype=np.uint32), idfs
 
     def _search_topk_sim(self, queries, k, similarity, slop):
-        """search_topk under bm25_impact, bm25_legacy_similarity or classic_similarity (sa_score_batch_topk_sim):
-        the counts, document frequencies, doc lengths, avgdl and corpus size .score hands the similarity, with
-        the similarity's own idf computed here, on the host, from the same dfs."""
-        if not isinstance(similarity, (Bm25Impact, Bm25Legacy, ClassicSimilarity)):
-            raise TypeError("search_topk supports bm25_similarity, bm25_impact, bm25_legacy_similarity and "
-                            f"classic_similarity, not {similarity!r}")
+        """search_topk on a view, and under bm25_impact, bm25_legacy_similarity or classic_similarity on any array
+        (sa_score_batch_topk_sim): the counts, document frequencies, doc lengths, avgdl and corpus size .score
+        uses, with the idf computed here, on the host, from the same dfs."""
         if self.rows is not None and (self.comm is not None or self.global_df is not None):
             raise ValueError("search_topk on a view of a sharded SearchArray is not supported: the slice's document "
                              "frequencies would need a sum over the ranks; use .score() on the view")
-        toks = [[q] if isinstance(q, str) else list(q) for q in queries]
-        docs = np.full((len(toks), k), _lib.NO_DOC, dtype=np.uint32)
-        scores = np.zeros((len(toks), k), dtype=np.float64)
-        ids = {t: self._term_id(t) for ts in toks for t in ts}
+        bm25 = isinstance(similarity, Bm25Similarity)
+        # BM25 ranks a view with the doc lengths .score's BM25 uses there (the stepped-slice quirk)
+        dl = np.ascontiguousarray(self._view_bm25_doc_lens(), dtype=np.float32) if bm25 else None
         dev = self._device()
         with self._shared["lock"]:
             self._apply_rows(dev)
-            if self.rows is None:
-                df = {t: self.docfreq(t) for t in ids}
+            if bm25:        # the float32 idf .score's BM25 takes
+                terms, starts, idfs = self._topk_queries(queries, lambda dfs: compute_idf(self.corpus_size, dfs))
+                idfs = np.asarray(idfs, dtype=np.float32)
             else:
-                # the slice dfs of every distinct known token in one device pass; .docfreq's values: np.uint64 for
-                # a known token, 0 for an unknown one
-                known = [t for t, tid in ids.items() if tid != _lib.NO_TERM]
-                dfs = np.zeros(len(known), dtype=np.uint64)
-                if known:
-                    tids = np.asarray([ids[t] for t in known], dtype=np.uint32)
-                    _lib.check(_lib.lib().sa_docfreq_rows_batch(dev.handle, _lib.p_u32(tids), len(tids),
-                                                                _lib.p_u64(dfs)))
-                df = dict(zip(known, dfs))
-            terms, starts, idfs = [], [0], []
-            for ts in toks:
-                terms.extend(ids[t] for t in ts)
-                starts.append(len(terms))
-                idfs.append(float(similarity._idf(np.asarray([df.get(t, 0) for t in ts]), self.corpus_size)))
-            terms = np.asarray(terms, dtype=np.uint32)
-            starts = np.asarray(starts, dtype=np.uint32)
+                terms, starts, idfs = self._topk_queries(
+                    queries, lambda dfs: float(similarity._idf(dfs, self.corpus_size)))
             idfs = np.asarray(idfs, dtype=np.float64)
+            docs = np.full((len(idfs), k), _lib.NO_DOC, dtype=np.uint32)
+            scores = np.zeros((len(idfs), k), dtype=np.float64)
             dbl = ctypes.POINTER(ctypes.c_double)
             _lib.check(_lib.lib().sa_score_batch_topk_sim(
                 dev.handle, similarity.kind, _lib.p_u32(terms), _lib.p_u32(starts), idfs.ctypes.data_as(dbl),
-                len(toks), int(slop), float(self.avg_doc_length), float(similarity.k1), float(similarity.b), k,
-                _lib.p_u32(docs), scores.ctypes.data_as(dbl)))
+                len(idfs), int(slop), None if dl is None else _lib.p_f32(dl), float(self.avg_doc_length),
+                float(similarity.k1), float(similarity.b), k, _lib.p_u32(docs), scores.ctypes.data_as(dbl)))
         return docs, scores.astype(similarity.out_dtype, copy=False)

@@ -24,6 +24,8 @@ def compute_idf(num_docs, dfs):
 
 class Bm25Similarity:
     """BM25 as in Lucene 9 (reference similarity.py:24-38), evaluated on the GPU."""
+    kind = 3                  # SA_SIM_BM25: search_topk on a view (sa_score_batch_topk_sim)
+    out_dtype = np.float32
 
     def __init__(self, k1=1.2, b=0.75):
         self.k1 = k1

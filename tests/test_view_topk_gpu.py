@@ -166,7 +166,7 @@ def test_terms_and_phrases_mixed(small_vocab, slop):
                 assert_topk(docs[i], scores[i], dense[i], (vname, q, slop, k))
 
 
-@pytest.mark.parametrize("k1,b", [(0.0, 0.75), (1.2, 1.0), (1.2, 0.0)])
+@pytest.mark.parametrize("k1,b", [(0.0, 0.75), (1.2, 1.0), (1.2, 0.0), (1.2, 1.5)])
 def test_exotic_bm25_parameters(corpus, k1, b):
     from searcharray_b200 import bm25_similarity
     host, arr, oidx = corpus

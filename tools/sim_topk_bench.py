@@ -11,7 +11,7 @@ has been checked against .score(q, similarity=sim) (ids, score bits, dtype):
   bm25_qps       the same batch with the default bm25_similarity;
   bytes / gbs    algorithmic bytes per term query and the rate they are moved at over the whole call:
                  P + 4*N (the tf scan and its doc-space count row), then per position 4 (count) + 8 (row index, views
-                 only) + 4 (score row, impact and legacy only), and 4 per position with a count > 0 (doc length);
+                 only), and 4 per position with a count > 0 (doc length);
                  P = 4*df for terms with a tf table, 8*W for the others;
   score_argpartition_qps   the alternative: .score(q, similarity=sim) + np.argpartition, for 32 queries.
 The card name and power limit come from a read-only nvidia-smi query in the same run.  Prints one JSON line.
@@ -99,7 +99,7 @@ def main():
                         np.array_equal(s[i].view(np.uint8), ws.view(np.uint8))):
                     raise SystemExit(f"{label}/{sname}: search_topk differs from .score's top k for {q!r}")
             t_med = timed(lambda: view.search_topk(names, k=args.k, similarity=sim), args.warmup, args.reps)
-            per_pos = 4 + (8 if sliced else 0) + (0 if sname == "classic" else 4)
+            per_pos = 4 + (8 if sliced else 0)
             per_query = P + 4 * n + per_pos * len(view) + 4 * df * frac
             bq = names[:args.baseline_queries]
             t0 = time.perf_counter()

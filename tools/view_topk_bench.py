@@ -9,9 +9,9 @@ results has been checked against view.score (positions and score bits):
   qps            search_topk over the whole batch, host clock around the synchronous call, after warm-up;
   docfreq_ms     one sa_docfreq_rows_batch over the batch's distinct terms (views only);
   bytes / gbs    algorithmic bytes per term query and the rate they are moved at over the whole call: views
-                 P + 4*N + 20*len(view) (the tf scan in doc space, its row, then row index, doc length, gathered
-                 count and view-space score per position), the unsliced path DESIGN.md 3.1's P + 4*df + 4*N;
-                 P = 4*df for terms with a tf table, 8*W for the others;
+                 P + 4*N + 12*len(view) + 4*df*len(view)/N (the tf scan in doc space, its row, then row index and
+                 gathered count per position, and the doc length of each position with a count), the unsliced path
+                 DESIGN.md 3.1's P + 4*df + 4*N; P = 4*df for terms with a tf table, 8*W for the others;
   score_argpartition_qps   the alternative a view had before: view.score(q) + np.argpartition, for 32 queries.
 The card name and power limit come from a read-only nvidia-smi query in the same run.  Prints one JSON line.
 """
@@ -101,7 +101,7 @@ def main():
         rec = {"rows": len(view), "verified_queries": len(sample), "qps_median": len(names) / t_med,
                "qps_best": len(names) / t_best, "ms_per_batch_median": 1e3 * t_med}
         if sliced:
-            per_query = P + 4 * n + 20 * len(view)
+            per_query = P + 4 * n + 12 * len(view) + 4 * df * len(view) / n
             dev = view._device()
             uniq = np.unique(tids)
             dfs = np.zeros(len(uniq), dtype=np.uint64)
