@@ -17,10 +17,10 @@
 //                        filtered lists (BM25 applied in the kernel).
 //   sa_multi_add_phase   solr.py:335-353: float32 sum of the phase's boosted vectors in list order,
 //                        added to qf where qf != 0.
-//   sa_multi_topk        exact top-k of the float64 vector: the high 32 bits of a positive double
-//                        order like the double itself, so the float32 top-k machinery (sa_topk.cu)
-//                        finds the k-th largest high word; every doc at or above it is then sorted
-//                        exactly (score desc, doc asc).
+//   sa_multi_topk        exact top-k of the float64 vector (score desc, doc asc): edismax_tile_kernel
+//                        ranks each tile by f64_proxy_key and keeps every doc at or above the tile's
+//                        bound with its float64 score (collect_tile_f64, as classic_similarity's
+//                        search_topk does), topk_select_f64_kernel orders the candidates in float64.
 #include <algorithm>
 #include <cmath>
 #include <functional>
@@ -34,7 +34,6 @@ int sa_filter_terms_mask(sa_index *ix, const uint32_t *term_ids, uint32_t n_term
 
 #define ED_MAX_FIELDS 8
 #define ED_MAX_ROWS 64
-#define ED_TOPK_CAP 2048
 
 struct sa_multi {
     std::vector<sa_index *> fields;
@@ -43,14 +42,13 @@ struct sa_multi {
     cudaStream_t stream = nullptr;
     double *d_qf = nullptr;              // [stride] combined scores (float32 values widened in field-centric mode)
     unsigned char *d_mask = nullptr;     // [stride] qf > 0 after the qf phase
-    float *d_proxy = nullptr;            // [stride] high words of qf (top-k)
     unsigned long long *d_count = nullptr;
-    u64 *d_pairs = nullptr;              // top-k candidates: score bits, doc
     bool f32_mode = false, has_qf = false;
     std::vector<std::vector<u64>> filt_offs, filt_lens;   // per field: last sa_multi_filter
     std::vector<u32> phrase_rows;        // per field: rows produced by the last sa_multi_phrases
     std::vector<u64> filt_bound;         // per field: words reserved for filtered lists (0 = not computed yet)
-    DevBuf cand, meta, keys;
+    DevBuf cand;                         // top-k: candidate slots, then their float64 scores
+    DevBuf keys;                         // top-k result: k keys, k float64 scores, the overflow flag
     std::mutex mu;
 };
 
@@ -176,108 +174,27 @@ edismax_add_phase_kernel(const PhaseArgs a) {
     else a.qf[d] = __dadd_rn(cur, (double)acc);
 }
 
-__global__ void __launch_bounds__(256)
-edismax_proxy_kernel(const double *__restrict__ qf, float *__restrict__ proxy, u64 stride) {
-    const u64 d = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (d >= stride) return;
-    const double v = qf[d];
-    proxy[d] = v > 0.0 ? __uint_as_float((u32)((u64)__double_as_longlong(v) >> 32)) : 0.0f;
-}
-
-// every doc whose high word is >= the k-th best high word (keys[k-1] of the proxy top-k; 0 = fewer than k matches)
-__global__ void __launch_bounds__(256)
-edismax_gather_kernel(const double *__restrict__ qf, u64 n_docs, const u64 *__restrict__ proxy_keys, u32 k,
-                      u64 *__restrict__ pairs, unsigned long long *__restrict__ count, u32 cap) {
-    const u64 d = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (d >= n_docs) return;
-    const double v = qf[d];
-    if (!(v > 0.0)) return;
-    const u32 kth_hi = (u32)(proxy_keys[k - 1] >> 32);
-    const u64 bits = (u64)__double_as_longlong(v);
-    if ((u32)(bits >> 32) < kth_hi) return;
-    const unsigned long long slot = atomicAdd(count, 1ull);
-    if (slot < cap) { pairs[2 * slot] = bits; pairs[2 * slot + 1] = d; }
-}
-
-// one CTA: exact order of <= ED_TOPK_CAP candidates by (score desc, doc asc), first k out
-__global__ void __launch_bounds__(1024)
-edismax_sort_kernel(const u64 *__restrict__ pairs, const unsigned long long *__restrict__ count, u32 k, u64 doc_base,
-                    double *__restrict__ out_scores, u32 *__restrict__ out_docs) {
-    __shared__ u64 s_key[ED_TOPK_CAP];
-    __shared__ u32 s_doc[ED_TOPK_CAP];
-    const u32 n = (u32)min((unsigned long long)ED_TOPK_CAP, *count);
-    for (u32 i = threadIdx.x; i < ED_TOPK_CAP; i += blockDim.x) {
-        s_key[i] = i < n ? pairs[2 * i] : 0ull;
-        s_doc[i] = i < n ? (u32)pairs[2 * i + 1] : 0xFFFFFFFFu;
-    }
-    __syncthreads();
-    for (u32 size = 2; size <= ED_TOPK_CAP; size <<= 1) {
-        for (u32 strideI = size >> 1; strideI > 0; strideI >>= 1) {
-            for (u32 i = threadIdx.x; i < ED_TOPK_CAP / 2; i += blockDim.x) {
-                const u32 lo = 2 * i - (i & (strideI - 1));
-                const u32 hi = lo + strideI;
-                const bool desc_block = ((lo & size) == 0);
-                // "a before b": larger score first, then smaller doc
-                const bool a_first = s_key[lo] > s_key[hi] || (s_key[lo] == s_key[hi] && s_doc[lo] < s_doc[hi]);
-                if (a_first != desc_block) {
-                    const u64 tk = s_key[lo]; s_key[lo] = s_key[hi]; s_key[hi] = tk;
-                    const u32 td = s_doc[lo]; s_doc[lo] = s_doc[hi]; s_doc[hi] = td;
-                }
-            }
-            __syncthreads();
+// Top-k candidates of one tile of qf (positions [0, n_docs)), ranked by f64_proxy_key with the float64 scores beside
+// them: the collection classic_similarity's search_topk uses (sim_tile_kernel).  The tile is read whole: the combine
+// kernels write qf's padding past n_docs with zeros, which never rank.
+__global__ void __launch_bounds__(SA_TERM_THREADS)
+edismax_tile_kernel(const double *__restrict__ qf, u64 n_docs, const TopkCtx t, u64 *__restrict__ tile_d) {
+    __shared__ u32 s_top[(SA_TERM_THREADS / 32) * 8];
+    __shared__ u32 s_ncand, s_tile_max;
+    const u32 tile = blockIdx.x;
+    const u64 pos0 = (u64)tile * SA_TILE_DOCS;
+    u32 key[SA_TILE_DOCS / SA_TERM_THREADS], my_max = 0;
+#pragma unroll
+    for (int j = 0; j < SA_TILE_DOCS / SA_TERM_THREADS / 4; j++) {
+        const u64 i0 = pos0 + (threadIdx.x + j * SA_TERM_THREADS) * 4;
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            key[j * 4 + e] = f64_proxy_key(__ldg(qf + i0 + e));
+            my_max = max(my_max, key[j * 4 + e]);
         }
     }
-    for (u32 i = threadIdx.x; i < k; i += blockDim.x) {
-        const bool ok = i < n && s_key[i] != 0ull;
-        out_scores[i] = ok ? __longlong_as_double((long long)s_key[i]) : 0.0;
-        out_docs[i] = ok ? (u32)(s_doc[i] + doc_base) : SA_NO_DOC;
-    }
-}
-
-// ---- exact fallback of the top-k when more than ED_TOPK_CAP docs share the leading 32 bits of the k-th score
-// (BM25 scores are a function of (tf, doc length): on a field of uniform short docs thousands of docs tie exactly).
-// hist[b] = docs with score > 0 whose bits match `prefix` above `shift + 8` and whose next byte is b
-__global__ void __launch_bounds__(256)
-edismax_hist_kernel(const double *__restrict__ qf, u64 n_docs, u64 prefix, int shift, unsigned long long *__restrict__ hist) {
-    __shared__ unsigned int s_h[256];
-    s_h[threadIdx.x] = 0;
-    __syncthreads();
-    for (u64 d = (u64)blockIdx.x * blockDim.x + threadIdx.x; d < n_docs; d += (u64)gridDim.x * blockDim.x) {
-        const double v = qf[d];
-        if (!(v > 0.0)) continue;
-        const u64 bits = (u64)__double_as_longlong(v);
-        if (shift < 56 && (bits >> (shift + 8)) != (prefix >> (shift + 8))) continue;
-        atomicAdd(&s_h[(bits >> shift) & 255u], 1u);
-    }
-    __syncthreads();
-    if (s_h[threadIdx.x]) atomicAdd(&hist[threadIdx.x], (unsigned long long)s_h[threadIdx.x]);
-}
-
-// docs scoring strictly more than `kth_bits` (fewer than k of them) -> pairs; ties per 1024-doc block -> tie_cnt
-__global__ void __launch_bounds__(256)
-edismax_above_kernel(const double *__restrict__ qf, u64 n_docs, u64 kth_bits, u64 *__restrict__ pairs,
-                     unsigned long long *__restrict__ count, u32 cap, u32 *__restrict__ tie_cnt) {
-    __shared__ unsigned int s_t;
-    if (threadIdx.x == 0) s_t = 0;
-    __syncthreads();
-    const u64 d0 = (u64)blockIdx.x * 1024;
-    u32 mine = 0;
-    for (u32 i = threadIdx.x; i < 1024; i += 256) {
-        const u64 d = d0 + i;
-        if (d >= n_docs) break;
-        const double v = qf[d];
-        if (!(v > 0.0)) continue;
-        const u64 bits = (u64)__double_as_longlong(v);
-        if (bits > kth_bits) {
-            const unsigned long long slot = atomicAdd(count, 1ull);
-            if (slot < cap) { pairs[2 * slot] = bits; pairs[2 * slot + 1] = d; }
-        } else if (bits == kth_bits) {
-            mine++;
-        }
-    }
-    if (mine) atomicAdd(&s_t, mine);
-    __syncthreads();
-    if (threadIdx.x == 0) tie_cnt[blockIdx.x] = s_t;
+    collect_tile_f64(key, my_max, (u32)min((u64)SA_TILE_DOCS, n_docs - pos0), t, tile_d, 0, tile, s_top, &s_ncand,
+                     &s_tile_max, [&](u32 local) { return __ldg(qf + pos0 + local); });
 }
 
 // ------------------------------------------------------------------------------ host
@@ -303,9 +220,7 @@ extern "C" int sa_multi_create(sa_index *const *fields, uint32_t n_fields, sa_mu
     bool ok = cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) == cudaSuccess &&
               cudaMalloc(&m->d_qf, s * sizeof(double)) == cudaSuccess &&
               cudaMalloc(&m->d_mask, s) == cudaSuccess &&
-              cudaMalloc(&m->d_proxy, s * sizeof(float)) == cudaSuccess &&
-              cudaMalloc(&m->d_count, 64) == cudaSuccess &&
-              cudaMalloc(&m->d_pairs, 2ull * ED_TOPK_CAP * sizeof(u64)) == cudaSuccess;
+              cudaMalloc(&m->d_count, 64) == cudaSuccess;
     if (!ok) {
         sa_set_error("sa_multi_create: %s", cudaGetErrorString(cudaGetLastError()));
         sa_multi_destroy(m);
@@ -321,11 +236,8 @@ extern "C" int sa_multi_destroy(sa_multi *m) {
     if (m->stream) { cudaStreamSynchronize(m->stream); cudaStreamDestroy(m->stream); }
     cudaFree(m->d_qf);
     cudaFree(m->d_mask);
-    cudaFree(m->d_proxy);
     cudaFree(m->d_count);
-    cudaFree(m->d_pairs);
     m->cand.release();
-    m->meta.release();
     m->keys.release();
     delete m;
     return SA_OK;
@@ -530,98 +442,36 @@ extern "C" int sa_multi_topk(sa_multi *m, uint32_t k, uint32_t *out_docs, double
     FieldGuard fg(ix, m->stream);
     const u32 T = sa_n_tiles(m->n_docs);
     int rc;
-    unsigned blocks = (unsigned)((m->stride + 255) / 256);
-    edismax_proxy_kernel<<<blocks, 256, 0, m->stream>>>(m->d_qf, m->d_proxy, m->stride);
-    SA_CUDA(cudaGetLastError());
-    u32 slots = sa_topk_slots(k);
-    for (int attempt = 0; attempt < 2; attempt++) {
-        if ((rc = m->cand.reserve(cand_bytes(T, 1, slots)))) return rc;
-        if ((rc = m->meta.reserve(256))) return rc;
-        if ((rc = m->keys.reserve((size_t)k * (sizeof(u64) + sizeof(double) + sizeof(u32)) + 64))) return rc;
-        SA_CUDA(cudaMemsetAsync(m->meta.p, 0, 256, m->stream));
-        const TopkCtx t = make_topk_ctx(m->cand.p, T, 1, slots, k, m->meta.as<u32>());
-        if ((rc = launch_dense_topk_tiles(ix, m->d_proxy, m->stride, 0, 1, t, nullptr))) return rc;
-        if ((rc = launch_topk_select(ix, t, 1, 0, m->keys.as<u64>(), nullptr))) return rc;
-        u32 ovf = 0;
-        SA_CUDA(cudaMemcpyAsync(&ovf, m->meta.p, sizeof(u32), cudaMemcpyDeviceToHost, m->stream));
-        SA_CUDA(cudaStreamSynchronize(m->stream));
-        if (!ovf) break;
-        slots = SA_TILE_DOCS;                                           // cannot overflow
-    }
-    SA_CUDA(cudaMemsetAsync(m->d_count, 0, sizeof(unsigned long long), m->stream));
-    edismax_gather_kernel<<<(unsigned)((m->n_docs + 255) / 256), 256, 0, m->stream>>>(m->d_qf, m->n_docs, m->keys.as<u64>(), k,
-                                                                                   m->d_pairs, m->d_count, ED_TOPK_CAP);
-    SA_CUDA(cudaGetLastError());
-    double *d_scores = (double *)(m->keys.as<u64>() + k);
-    u32 *d_docs = (u32 *)(d_scores + k);
-    edismax_sort_kernel<<<1, 1024, 0, m->stream>>>(m->d_pairs, m->d_count, k, m->doc_base, d_scores, d_docs);
-    SA_CUDA(cudaGetLastError());
-    unsigned long long cnt = 0;
-    SA_CUDA(cudaMemcpyAsync(&cnt, m->d_count, sizeof(cnt), cudaMemcpyDeviceToHost, m->stream));
-    SA_CUDA(cudaMemcpyAsync(out_scores, d_scores, k * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
-    SA_CUDA(cudaMemcpyAsync(out_docs, d_docs, k * sizeof(u32), cudaMemcpyDeviceToHost, m->stream));
-    SA_CUDA(cudaStreamSynchronize(m->stream));
-    if (cnt <= ED_TOPK_CAP) return SA_OK;
-
-    // ---- more than ED_TOPK_CAP docs share the k-th score's leading bits: exact selection on the full 64 bits
-    // 1. the k-th largest score (with multiplicity): 8-pass byte-wise radix select over all docs
-    unsigned long long *d_hist = (unsigned long long *)m->d_pairs;             // 256 counters (the pairs buffer is free)
-    unsigned long long h_hist[256];
-    u64 prefix = 0, need = k;
-    const unsigned hb = (unsigned)std::min<u64>(1024, (m->n_docs + 255) / 256);
-    for (int shift = 56; shift >= 0; shift -= 8) {
-        SA_CUDA(cudaMemsetAsync(d_hist, 0, sizeof(h_hist), m->stream));
-        edismax_hist_kernel<<<hb, 256, 0, m->stream>>>(m->d_qf, m->n_docs, prefix, shift, d_hist);
-        SA_CUDA(cudaGetLastError());
-        SA_CUDA(cudaMemcpyAsync(h_hist, d_hist, sizeof(h_hist), cudaMemcpyDeviceToHost, m->stream));
-        SA_CUDA(cudaStreamSynchronize(m->stream));
-        int b = 255;
-        for (; b > 0; b--) {
-            if (h_hist[b] >= need) break;
-            need -= h_hist[b];
+    if ((rc = m->keys.reserve((size_t)k * (sizeof(u64) + sizeof(double)) + sizeof(u32)))) return rc;
+    u64 *d_keys = m->keys.as<u64>();
+    double *d_scores = (double *)(d_keys + k);
+    u32 *d_ovf = (u32 *)(d_scores + k);
+    std::vector<u64> h(2 * (size_t)k + 1);          // the keys, the scores' bits, the overflow flag
+    // a tile with more candidates than slots sends the query once more with a slot per position, which cannot overflow
+    for (u32 slots = sa_topk_slots(k);; slots = SA_TILE_DOCS) {
+        const size_t cb = cand_bytes(T, 1, slots);
+        if ((rc = m->cand.reserve(cb + (size_t)T * slots * sizeof(u64)))) return rc;
+        u64 *tile_d = (u64 *)((char *)m->cand.p + cb);
+        SA_CUDA(cudaMemsetAsync(d_ovf, 0, sizeof(u32), m->stream));
+        const TopkCtx t = make_topk_ctx(m->cand.p, T, 1, slots, k, d_ovf);
+        {
+            KernelTimer tm(ix, 1);
+            edismax_tile_kernel<<<T, SA_TERM_THREADS, 0, m->stream>>>(m->d_qf, m->n_docs, t, tile_d);
+            SA_CUDA(cudaGetLastError());
+            tm.stop();
+            ix->stats.topk_kernel_launches++;
+            ix->stats.total_launches++;
         }
-        prefix |= (u64)b << shift;
-    }
-    const u64 kth_bits = prefix;                     // `need` docs with exactly this score belong to the top k
-    // 2. docs above it (fewer than k) + ties per 1024-doc block
-    const u32 n_blocks = (u32)((m->n_docs + 1023) / 1024);
-    if ((rc = m->cand.reserve((size_t)n_blocks * sizeof(u32) + 64))) return rc;
-    std::vector<u32> tie_cnt(n_blocks);
-    std::vector<u64> above(2 * (size_t)k);
-    SA_CUDA(cudaMemsetAsync(m->d_count, 0, sizeof(unsigned long long), m->stream));
-    edismax_above_kernel<<<n_blocks, 256, 0, m->stream>>>(m->d_qf, m->n_docs, kth_bits, m->d_pairs, m->d_count, k, m->cand.as<u32>());
-    SA_CUDA(cudaGetLastError());
-    SA_CUDA(cudaMemcpyAsync(&cnt, m->d_count, sizeof(cnt), cudaMemcpyDeviceToHost, m->stream));
-    SA_CUDA(cudaMemcpyAsync(tie_cnt.data(), m->cand.p, (size_t)n_blocks * sizeof(u32), cudaMemcpyDeviceToHost, m->stream));
-    SA_CUDA(cudaStreamSynchronize(m->stream));
-    SA_CHECK(cnt < k, "top-k fallback: inconsistent selection");
-    if (cnt) SA_CUDA(cudaMemcpy(above.data(), m->d_pairs, 2 * (size_t)cnt * sizeof(u64), cudaMemcpyDeviceToHost));
-    std::vector<std::pair<u64, u64>> best;           // (score bits, doc)
-    for (u64 i = 0; i < cnt; i++) best.push_back({above[2 * i], above[2 * i + 1]});
-    std::sort(best.begin(), best.end(), [](const std::pair<u64, u64> &x, const std::pair<u64, u64> &y) {
-        return x.first > y.first || (x.first == y.first && x.second < y.second);
-    });
-    // 3. the `need` tied docs with the smallest ids: walk the blocks in order, read only the blocks that hold them
-    u64 want_ties = std::min<u64>(need, (u64)k - cnt);
-    std::vector<double> blk(1024);
-    for (u32 bI = 0; bI < n_blocks && want_ties; bI++) {
-        if (!tie_cnt[bI]) continue;
-        const u64 d0 = (u64)bI * 1024, nb = std::min<u64>(1024, m->n_docs - d0);
-        SA_CUDA(cudaMemcpy(blk.data(), m->d_qf + d0, nb * sizeof(double), cudaMemcpyDeviceToHost));
-        for (u64 i = 0; i < nb && want_ties; i++) {
-            u64 bits;
-            memcpy(&bits, &blk[i], 8);
-            if (blk[i] > 0.0 && bits == kth_bits) { best.push_back({bits, d0 + i}); want_ties--; }
-        }
+        if ((rc = launch_topk_select_f64(ix, t, tile_d, 1, m->doc_base, d_keys, d_scores, nullptr))) return rc;
+        SA_CUDA(cudaMemcpyAsync(h.data(), d_keys, (size_t)k * (sizeof(u64) + sizeof(double)) + sizeof(u32),
+                                cudaMemcpyDeviceToHost, m->stream));
+        SA_CUDA(cudaStreamSynchronize(m->stream));
+        if (!(u32)h[2 * k] || slots == SA_TILE_DOCS) break;
     }
     for (u32 i = 0; i < k; i++) {
-        if (i < best.size()) {
-            memcpy(&out_scores[i], &best[i].first, 8);
-            out_docs[i] = (u32)(best[i].second + m->doc_base);
-        } else {
-            out_scores[i] = 0.0;
-            out_docs[i] = SA_NO_DOC;
-        }
+        if (h[i] == 0) continue;
+        out_docs[i] = 0xFFFFFFFFu - (u32)h[i];                           // the select added doc_base
+        memcpy(&out_scores[i], &h[k + i], sizeof(double));
     }
     return SA_OK;
 }

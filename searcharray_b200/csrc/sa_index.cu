@@ -5,6 +5,7 @@
 
 #include "sa_term.cuh"
 #include "sa_phrase.cuh"
+#include "sa_sim.cuh"
 #include "sa_span.cuh"
 
 // ------------------------------------------------------------------ error text
@@ -640,8 +641,7 @@ struct BatchState {
     std::vector<BatchChunk> chunks;
     // slop > 0: the multi-term queries are span queries (one plan per chunk, descriptors concatenated)
     std::vector<SpanPlan> span_plans;
-    std::vector<float> span_idf;
-    DevBuf d_sq, d_scounts, d_sidf;
+    DevBuf d_sq, d_scounts;
     DevBuf d_tq, d_pq, d_row_query;
     DevBuf d_meta;                            // u32 overflow[nq] (row space)
     DevBuf d_pstats;                          // PhraseStats[#phrase queries]
@@ -666,7 +666,7 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
     B.k1 = k1;
     B.b = b;
     B.slop = slop;
-    B.span_plans.clear(); B.span_idf.clear();
+    B.span_plans.clear();
     B.tqs.clear(); B.pqs.clear(); B.row_query.clear(); B.term_query.clear(); B.phrase_query.clear();
     B.phrase_missing.clear(); B.chunks.clear(); B.sel.clear();
     int rc;
@@ -704,7 +704,6 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
                 } else if (slop > 0) {
                     // phrase with slop: span search (spans.py:171-187) on the index's own lists
                     sa_span_plan_add(plan, offs, lens, dirs, nt, slop, idf[q], literal, missing ? 0 : ix->n_docs);
-                    B.span_idf.push_back(idf[q]);
                     B.phrase_query.push_back(q);
                 } else {
                     PhraseQuery pq = make_phrase_query(tids, nt, offs, lens, dirs, idf[q], missing);
@@ -756,7 +755,6 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
         if ((rc = ix->phrase_scratch.reserve(max_span_scratch))) return rc;
         if ((rc = B.d_sq.reserve((size_t)n_span * sizeof(SpanQuery)))) return rc;
         if ((rc = B.d_scounts.reserve((size_t)n_span * sizeof(SpanCounts)))) return rc;
-        if ((rc = B.d_sidf.reserve((size_t)n_span * sizeof(float)))) return rc;
         u32 at = 0;
         for (const SpanPlan &pl : B.span_plans) {
             if (pl.qs.empty()) continue;
@@ -764,7 +762,6 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
                                     cudaMemcpyHostToDevice, ix->stream));
             at += (u32)pl.qs.size();
         }
-        SA_CUDA(cudaMemcpyAsync(B.d_sidf.p, B.span_idf.data(), (size_t)n_span * sizeof(float), cudaMemcpyHostToDevice, ix->stream));
         SA_CUDA(cudaStreamSynchronize(ix->stream));      // the plans' host vectors may be reallocated later
     }
     if (!B.tqs.empty())
@@ -883,10 +880,12 @@ int sa_batch_execute_locked(sa_index *ix) {
 }
 
 // Re-run one query exactly (synchronously): a tile overflowed its candidate slots, or a phrase's
-// same-term speculation was wrong.  Uses a slot per doc of the tile -- cannot overflow.
+// same-term speculation was wrong.  Uses a slot per doc of the tile -- cannot overflow.  A phrase or span query
+// writes its raw counts into ix->dense row 0, and the BM25 tile pass (launch_sim_tiles) scores and collects them:
+// bm25_one performs the rounded operations of the batch kernels' BM25 in the same order, and a zero count scores +0
+// (a batch with phrase queries has ordinary parameters, sa_batch_upload_locked), so the scores are the batch's bits.
 static int redo_query(sa_index *ix, BatchState &B, bool is_phrase, u32 idx, u32 q, const SpanQuery *sq = nullptr) {
     int rc;
-    const u64 stride = sa_padded_docs(ix->n_docs);
     const u32 n_tiles = sa_n_tiles(ix->n_docs);
     if ((rc = ix->cand.reserve(cand_bytes(n_tiles, 1, SA_TILE_DOCS)))) return rc;
     SA_CUDA(cudaMemsetAsync(B.d_meta.p, 0, sizeof(u32), ix->stream));
@@ -895,19 +894,22 @@ static int redo_query(sa_index *ix, BatchState &B, bool is_phrase, u32 idx, u32 
         Bm25Params p = make_bm25(B.tqs[idx].idf, B.avg_doc_len, B.k1, B.b, ix->doc_lens_nonneg);
         TermBatchArgs a = make_term_args(ix, B.d_tq.as<TermQuery>() + idx, p, t);
         if ((rc = launch_term_batch(ix, a, 1))) return rc;
-    } else if (sq) {
-        if ((rc = sa_ensure_norm(ix, B.k1, B.b, B.avg_doc_len))) return rc;
-        if ((rc = sa_span_run(ix, ix->d_words, sq->off, sq->len, sq->dir_off, sq->n_terms, sq->slop, sq->literal != 0, nullptr))) return rc;
-        SA_CUDA(cudaMemcpyAsync(B.d_sidf.p, &sq->idf, sizeof(float), cudaMemcpyHostToDevice, ix->stream));
-        if ((rc = launch_dense_topk_tiles(ix, ix->dense.as<float>(), stride, 0, 1, t, B.d_sidf.as<float>()))) return rc;
     } else {
-        Bm25Params p = make_bm25(B.pqs[idx].idf, B.avg_doc_len, B.k1, B.b, ix->doc_lens_nonneg);
-        std::vector<PhraseQuery> one(1, B.pqs[idx]);
-        PhraseDump nodump;
-        memset(&nodump, 0, sizeof(nodump));
-        if ((rc = sa_phrase_run_sync(ix, one, ix->d_words, 1, p, nodump, false))) return rc;   // loops until the guess holds
-        B.pqs[idx] = one[0];
-        if ((rc = launch_dense_topk_tiles(ix, ix->dense.as<float>(), stride, 0, 1, t, nullptr))) return rc;
+        const Bm25Params p = make_bm25(sq ? sq->idf : B.pqs[idx].idf, B.avg_doc_len, B.k1, B.b, ix->doc_lens_nonneg);
+        if (sq) {
+            if ((rc = sa_span_run(ix, ix->d_words, sq->off, sq->len, sq->dir_off, sq->n_terms, sq->slop, sq->literal != 0, nullptr))) return rc;
+        } else {
+            std::vector<PhraseQuery> one(1, B.pqs[idx]);
+            PhraseDump nodump;
+            memset(&nodump, 0, sizeof(nodump));
+            if ((rc = sa_phrase_run_sync(ix, one, ix->d_words, 0, p, nodump, false))) return rc;   // loops until the guess holds
+            B.pqs[idx] = one[0];
+        }
+        const double idf = p.idf;
+        if ((rc = ix->misc.reserve(sizeof(double)))) return rc;
+        SA_CUDA(cudaMemcpyAsync(ix->misc.p, &idf, sizeof(double), cudaMemcpyHostToDevice, ix->stream));
+        if ((rc = launch_sim_tiles(ix, SA_SIM_BM25, ix->dense.as<float>(), nullptr, ix->d_doc_lens, ix->n_docs, p,
+                                   SimParams{}, ix->misc.as<double>(), 1, 0, t, nullptr))) return rc;
     }
     SA_CUDA(cudaMemcpyAsync(B.d_row_query.p, &q, sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
     if ((rc = launch_topk_select(ix, t, 1, ix->doc_base, ix->topk_out.as<u64>(), B.d_row_query.as<u32>()))) return rc;
@@ -960,11 +962,10 @@ int sa_batch_fix_overflow_locked(sa_index *ix, u32 *n_redone) {
     SA_CUDA(cudaMemcpyAsync(B.d_row_query.p, B.row_query.data(), (size_t)B.nq * sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
     if (!B.pqs.empty())
         SA_CUDA(cudaMemcpyAsync(B.d_pq.p, B.pqs.data(), B.pqs.size() * sizeof(PhraseQuery), cudaMemcpyHostToDevice, ix->stream));
-    if (!B.span_idf.empty()) {
+    if (B.slop > 0) {
         size_t need = 0;
         for (const SpanPlan &pl : B.span_plans) need = std::max(need, sa_span_scratch_bytes(pl));
         if ((rc = ix->phrase_scratch.reserve(need))) return rc;
-        SA_CUDA(cudaMemcpyAsync(B.d_sidf.p, B.span_idf.data(), B.span_idf.size() * sizeof(float), cudaMemcpyHostToDevice, ix->stream));
     }
     SA_CUDA(cudaStreamSynchronize(ix->stream));
     if (n_redone) *n_redone = (u32)redo.size();
@@ -1110,7 +1111,6 @@ void sa_free_batch(sa_index *ix) {
     ix->batch->d_missing.release();
     ix->batch->d_sq.release();
     ix->batch->d_scounts.release();
-    ix->batch->d_sidf.release();
     delete ix->batch;
     ix->batch = nullptr;
 }

@@ -377,94 +377,6 @@ term_tile_kernel(const TermBatchArgs a) {
     }
 }
 
-// Top-k candidate collection for an already materialised dense score vector (phrase queries:
-// their kernel scatters sparse matches, so the collector runs as a separate tile scan).  Same
-// outputs as step 3/4 of term_tile_kernel: per-tile candidate slots, count and maximum.
-template <bool SCORE>
-__global__ void __launch_bounds__(SA_TERM_THREADS)
-dense_topk_tiles_kernel(float *__restrict__ dense, u64 stride, u32 row0, const TopkCtx t,
-                        const float *__restrict__ norm, const float *__restrict__ row_idf) {
-    __shared__ u32 s_top[(SA_TERM_THREADS / 32) * 8];
-    __shared__ u32 s_ncand, s_tile_max;
-    const u32 q = blockIdx.y + row0;
-    const u32 tile = blockIdx.x;
-    const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const u32 tile_doc0 = tile * SA_TILE_DOCS;
-    const u32 k = t.k;
-    constexpr int NV = SA_TILE_DOCS / SA_TERM_THREADS / 4;
-    float4 *__restrict__ src = reinterpret_cast<float4 *>(dense + (u64)q * stride + tile_doc0);
-    float4 v[NV];
-    u32 my_max = 0;
-    const float idf = SCORE ? row_idf[blockIdx.y] : 0.0f;
-#pragma unroll
-    for (int j = 0; j < NV; j++) {
-        v[j] = __ldcs(src + tid + j * SA_TERM_THREADS);
-        float vs[4] = {v[j].x, v[j].y, v[j].z, v[j].w};
-        if (SCORE) {
-            // raw counts -> BM25 (bm25.pyx:20-25; a zero count scores +0.0 for ordinary parameters)
-            if ((vs[0] != 0.0f) | (vs[1] != 0.0f) | (vs[2] != 0.0f) | (vs[3] != 0.0f)) {
-                const u32 d0 = tile_doc0 + (tid + j * SA_TERM_THREADS) * 4;
-#pragma unroll
-                for (int e = 0; e < 4; e++)
-                    if (vs[e] != 0.0f) vs[e] = bm25_from_norm(vs[e], __ldg(norm + d0 + e), idf);
-                v[j] = make_float4(vs[0], vs[1], vs[2], vs[3]);
-                __stcs(src + tid + j * SA_TERM_THREADS, v[j]);
-            }
-        }
-#pragma unroll
-        for (int e = 0; e < 4; e++)
-            if (vs[e] > 0.0f) my_max = max(my_max, __float_as_uint(vs[e]));
-    }
-    const u32 M = 8u;
-    u32 mv = my_max;
-    for (u32 r = 0; r < M; r++) {
-        u32 m = warp_pop_max(mv);
-        if (lane == r) s_top[warp * 8 + r] = m;
-    }
-    if (tid == 0) { s_ncand = 0; s_tile_max = 0; }
-    __syncthreads();
-    const float thr_f = __uint_as_float(max(cta_kth_bound(s_top, k, true), 1u));
-    u64 *__restrict__ my_cand = t.tile_cand + ((u64)q * t.n_tiles + tile) * t.slots;
-    u32 cand_max = 0;
-#pragma unroll
-    for (int j = 0; j < NV; j++) {
-        const float vs[4] = {v[j].x, v[j].y, v[j].z, v[j].w};
-#pragma unroll
-        for (int e = 0; e < 4; e++) {
-            if (vs[e] >= thr_f) {
-                u32 slot = atomicAdd(&s_ncand, 1u);
-                if (slot < t.slots)
-                    my_cand[slot] = ((u64)__float_as_uint(vs[e]) << 32) |
-                                    (u64)(0xFFFFFFFFu - (tile_doc0 + (tid + j * SA_TERM_THREADS) * 4 + e));
-                cand_max = max(cand_max, __float_as_uint(vs[e]));
-            }
-        }
-    }
-    if (cand_max) atomicMax(&s_tile_max, cand_max);
-    __syncthreads();
-    if (tid == 0) {
-        const u32 n = s_ncand;
-        const u64 t_idx = (u64)q * t.n_tiles + tile;
-        t.tile_cnt[t_idx] = min(n, t.slots);
-        t.tile_max[t_idx] = s_tile_max;
-        if (n > t.slots) t.overflow[q] = 1u;
-    }
-}
-
-int launch_dense_topk_tiles(sa_index *ix, float *dense, u64 stride, u32 row0, u32 n_rows, const TopkCtx &t,
-                            const float *d_row_idf) {
-    if (n_rows == 0 || t.n_tiles == 0) return SA_OK;
-    dim3 grid(t.n_tiles, n_rows);
-    KernelTimer tm(ix, 1);
-    if (d_row_idf) dense_topk_tiles_kernel<true><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(dense, stride, row0, t, ix->d_norm, d_row_idf);
-    else dense_topk_tiles_kernel<false><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(dense, stride, row0, t, nullptr, nullptr);
-    SA_CUDA(cudaGetLastError());
-    tm.stop();
-    ix->stats.topk_kernel_launches++;
-    ix->stats.total_launches++;
-    return SA_OK;
-}
-
 // per-doc BM25 length norm, the inner part of bm25.pyx:21-23 with the same rounding sequence
 __global__ void norm_kernel(const float *__restrict__ dl, float *__restrict__ norm, u64 n, u64 n_pad,
                             Bm25Params p) {

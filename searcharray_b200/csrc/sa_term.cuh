@@ -1,4 +1,6 @@
-// sa_term.cuh -- kernel-side declarations shared by the term-path translation units.
+// sa_term.cuh -- kernel-side declarations shared by the term-path translation units, and the per-tile top-k
+// collectors every scoring kernel ends with: flush_tile_collect for float32 scores, collect_tile_f64 for float64
+// scores ranked by a float32 proxy (classic similarity, edismax).
 #pragma once
 #include <cmath>
 
@@ -60,10 +62,14 @@ u32 sa_topk_slots(u32 k);
 // slot for slot); exact in float64, see sa_topk.cu.  d_out_scores[out_index[q] * k + i] = the float64 scores.
 int launch_topk_select_f64(sa_index *ix, const TopkCtx &t, const u64 *d_tile_d, u32 n_queries, u64 doc_base,
                            u64 *d_out_keys, double *d_out_scores, const u32 *d_out_index);
-// d_row_idf != NULL: the rows hold raw match counts; BM25 (norm table of the last sa_ensure_norm) is applied in
-// place on the way (row_idf[i] = idf of row row0 + i)
-int launch_dense_topk_tiles(sa_index *ix, float *dense, u64 stride, u32 row0, u32 n_rows, const TopkCtx &t,
-                            const float *d_row_idf);
+// sim_tile_kernel<kind> (sa_view.cu) over n doc-space count rows of ix->dense's stride: counts + j * stride is row j,
+// d_idf[j] its idf, row row0 + j of t takes its candidates.  Position i < n_pos reads its count at doc rows[i] (rows ==
+// NULL: doc i) and its doc length from doc_lens as sim_tile_kernel describes.  bm25 / sim: the parameters of the
+// kind; tile_d: the float64 candidate scores (SA_SIM_CLASSIC only).
+struct SimParams;
+int launch_sim_tiles(sa_index *ix, int kind, const float *counts, const u64 *rows, const float *doc_lens, u64 n_pos,
+                     const Bm25Params &bm25, const SimParams &sim, const double *d_idf, u32 n, u32 row0,
+                     const TopkCtx &t, u64 *tile_d);
 int launch_topk_merge(sa_index *ix, const u64 *d_in, u64 rank_stride, u32 world, u32 n_queries, u32 k, u64 *d_out);
 // A batch's result block in HBM: nq * k keys followed by SA_BATCH_TAIL summary words written by the batch's last
 // kernel -- [0] queries that need the exact host-side re-run (candidate overflow, wrong same-term guess, scratch
@@ -349,5 +355,62 @@ __device__ __forceinline__ void flush_tile_collect(const float *s_out, float *__
         }
     }
     __syncthreads();
+}
+
+// The float32 key a float64 score s ranks by when no float32 value is exact: s rounded toward zero, at least the
+// smallest subnormal for s > 0 (0 = never ranks: s <= 0 or NaN).  Monotone in s, but distinct scores can share it.
+__device__ __forceinline__ u32 f64_proxy_key(double s) {
+    return s > 0.0 ? max(1u, __float_as_uint(__double2float_rz(s))) : 0u;
+}
+
+// flush_tile_collect for float64 scores ranked by f64_proxy_key (classic similarity, edismax): the tile bound from 8
+// maxima per warp, then EVERY position whose key is at or above it -- no tie cut, which would drop positions tied in
+// the key by index although their float64 scores can be larger -- with the float64 score bits beside each candidate
+// in tile_d (slot for slot), for topk_select_f64_kernel.  key[]: the thread's keys in flush_tile_collect's layout
+// (position 4g + e of the tile, g = tid + j * SA_TERM_THREADS), my_max their maximum, n_items the positions of the
+// tile; score(local) returns the float64 score of tile position `local` and runs for the stored candidates only.
+// More candidates than slots flags the query's overflow: the caller re-runs it with SA_TILE_DOCS slots, which cannot
+// overflow.  All SA_TERM_THREADS threads must call.
+template <typename F>
+__device__ __forceinline__ void collect_tile_f64(const u32 (&key)[SA_TILE_DOCS / SA_TERM_THREADS], u32 my_max,
+                                                 u32 n_items, const TopkCtx &t, u64 *__restrict__ tile_d, u32 row,
+                                                 u32 tile, u32 *s_top, u32 *s_ncand, u32 *s_tile_max, F score) {
+    const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const bool need_bound = n_items > t.k;                           // CTA-uniform
+    if (need_bound) {
+        u32 v = my_max;
+        for (u32 r = 0; r < 8; r++) {
+            const u32 m = warp_pop_max(v);
+            if (lane == r) s_top[warp * 8 + r] = m;
+        }
+    }
+    if (tid == 0) { *s_ncand = 0; *s_tile_max = 0; }
+    __syncthreads();
+    const u32 thr = need_bound ? max(cta_kth_bound(s_top, t.k, true), 1u) : 1u;
+    const u64 slot0 = ((u64)row * t.n_tiles + tile) * t.slots;
+    u32 cand_max = 0;
+#pragma unroll
+    for (int j = 0; j < SA_TILE_DOCS / SA_TERM_THREADS / 4; j++) {
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            if (key[j * 4 + e] >= thr) {
+                const u32 local = (tid + j * SA_TERM_THREADS) * 4 + e;
+                const u32 slot = atomicAdd(s_ncand, 1u);
+                if (slot < t.slots) {
+                    t.tile_cand[slot0 + slot] = ((u64)key[j * 4 + e] << 32) | (u64)(0xFFFFFFFFu - (tile * SA_TILE_DOCS + local));
+                    tile_d[slot0 + slot] = (u64)__double_as_longlong(score(local));
+                }
+                cand_max = max(cand_max, key[j * 4 + e]);
+            }
+        }
+    }
+    if (cand_max) atomicMax(s_tile_max, cand_max);
+    __syncthreads();
+    if (tid == 0) {
+        const u64 t_idx = (u64)row * t.n_tiles + tile;
+        t.tile_cnt[t_idx] = min(*s_ncand, t.slots);
+        t.tile_max[t_idx] = *s_tile_max;
+        if (*s_ncand > t.slots) t.overflow[row] = 1u;
+    }
 }
 #endif

@@ -203,8 +203,8 @@ __device__ K radix_kth_largest(u32 k, u32 *s_hist, K *s_prefix, u32 *s_krem, V v
 
 typedef unsigned __int128 u128;
 
-// The exact top k of a query whose candidates carry a float32 PROXY of a float64 score (classic similarity,
-// sim_tile_kernel): the candidate key is proxy_bits << 32 | ~position as usual and tile_d[] holds the float64 score
+// The exact top k of a query whose candidates carry a float32 PROXY of a float64 score (collect_tile_f64: classic
+// similarity, edismax): the candidate key is proxy_bits << 32 | ~position as usual and tile_d[] holds the float64 score
 // bits of the same slot.  The proxy is monotone but not injective, so distinct scores can share it; the tiles kept
 // EVERY position at or above their bound (no tie cut), hence every position whose proxy is >= the k-th largest
 // proxy P_k is a candidate, and the true top k lies among them (a position below P_k has k better ones).

@@ -15,7 +15,8 @@
 //      the tile's top-k candidates;
 //   3. launch_topk_select (launch_topk_select_f64 for classic) over the tiles.
 // A query whose candidate slots overflowed is re-run alone with a slot per position of the tile, as redo_query
-// does for the unsliced batch.
+// does for the unsliced batch.  Step 2 (launch_sim_tiles) is also the BM25 scoring of redo_query's phrase and span
+// re-runs, over the raw counts in row 0 of the unsliced array.
 // HBM traffic of a term query: the term scan's own bytes + 4*N (its doc-space row), then per position 4 (gathered
 // count) and 8 (row index, views only), and 4 (doc length) per position whose count is > 0.
 #include <algorithm>
@@ -58,7 +59,8 @@ template <int KIND> using TileParams = std::conditional_t<KIND == SA_SIM_BM25, B
 // grid = (tiles of positions, queries).  row = row0 + blockIdx.y indexes the candidate slots and the overflow flags;
 // doc_rows + blockIdx.y * doc_stride is the query's doc-space count row, idf[blockIdx.y] its idf.  Position i reads
 // its count at doc = rows[i] on a view (rows == NULL: the unsliced array, doc = i) and its doc length at
-//   SA_SIM_BM25: doc_lens[i], the lengths the view's BM25 uses (the stepped-slice quirk of bm25_score);
+//   SA_SIM_BM25: doc_lens[i], the lengths the view's BM25 uses (the stepped-slice quirk of bm25_score), or the
+//                index's own on the unsliced array;
 //   the others:  doc_lens[doc], SearchArray.doclengths().
 // A zero count never scores > 0 under any of the formulas (0 / x, 0 * l and sqrt(0) give +-0 or NaN, and the idf
 // cannot turn them positive), so the doc length is loaded only where the count is > 0.  What the tile ranks by, and
@@ -73,12 +75,9 @@ template <int KIND> using TileParams = std::conditional_t<KIND == SA_SIM_BM25, B
 //            same ties, and the existing collector and select are exact; for idf < 0 the key is -sat (the score
 //            is > 0 only where sat < 0), for idf == 0 nothing ranks.  The score is formed on the host for the k
 //            winners only: |idf| * key, the same rounding as idf * sat.
-//   classic: score = fl64(fl64(idf * sqrt_tf) * inv_sqrt_dl) has no exact float32 key.  The tile ranks by a
-//            PROXY, the score rounded toward zero to float32 (at least the smallest subnormal for a score > 0):
-//            monotone, but distinct scores can share it.  So the tile keeps EVERY position at or above its bound
-//            -- flush_tile_collect's tie retry would cut positions tied at the bound by index, dropping larger
-//            float64 scores -- stores each candidate's float64 score beside its key (tile_d), and a tile with more
-//            candidates than slots sends the query to the exact re-run; topk_select_f64_kernel ranks in float64.
+//   classic: score = fl64(fl64(idf * sqrt_tf) * inv_sqrt_dl) has no exact float32 key.  The tile ranks by
+//            f64_proxy_key(score) and collects with collect_tile_f64 (every position at or above the bound, the
+//            float64 scores in tile_d, overflow -> the exact re-run); topk_select_f64_kernel ranks in float64.
 template <int KIND>
 __global__ void __launch_bounds__(SA_TERM_THREADS)
 sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *__restrict__ rows,
@@ -118,8 +117,7 @@ sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *_
                         const float sat = sim_legacy_sat(tf, dl, p);
                         v[e] = q_idf > 0.0 ? sat : (q_idf < 0.0 ? -sat : 0.0f);
                     } else {
-                        const double s = sim_classic(q_idf, tf, dl);
-                        if (s > 0.0) v[e] = __uint_as_float(max(1u, __float_as_uint(__double2float_rz(s))));
+                        v[e] = __uint_as_float(f64_proxy_key(sim_classic(q_idf, tf, dl)));
                     }
                     if (v[e] > 0.0f) my_max = max(my_max, __float_as_uint(v[e]));   // NaN and <= 0 never rank
                 }
@@ -129,52 +127,16 @@ sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *_
         if (KIND != SA_SIM_CLASSIC) reinterpret_cast<float4 *>(s_out)[g] = make_float4(v[0], v[1], v[2], v[3]);
     }
     const u32 n_items = (u32)min((u64)SA_TILE_DOCS, n_pos - pos0);
-    if (KIND != SA_SIM_CLASSIC) {
+    if constexpr (KIND == SA_SIM_CLASSIC) {
+        collect_tile_f64(key, my_max, n_items, t, tile_d, row, tile, s_top, &s_ncand, &s_tile_max, [&](u32 local) {
+            // the float64 score again, for the few candidates (cheaper than holding 32 doubles per thread)
+            const u64 doc = rows ? __ldg(rows + pos0 + local) : pos0 + local;
+            return sim_classic(q_idf, __ldg(counts + doc), __ldg(doc_lens + doc));
+        });
+    } else {
         // nothing reads the scores outside the tile: collect the candidates without storing the row
         flush_tile_collect<false>(s_out, nullptr, t, row, tile, my_max, n_items,
                                   min((u32)SA_TERM_THREADS, (n_items + 3) / 4), s_top, &s_ncand, &s_tile_max);
-        return;
-    }
-    // classic: the tile bound as flush_tile_collect computes it (8 values per warp), then every proxy >= it
-    const unsigned warp = tid >> 5, lane = tid & 31;
-    const bool need_bound = n_items > t.k;                           // CTA-uniform
-    if (need_bound) {
-        u32 v = my_max;
-        for (u32 r = 0; r < 8; r++) {
-            const u32 m = warp_pop_max(v);
-            if (lane == r) s_top[warp * 8 + r] = m;
-        }
-    }
-    if (tid == 0) { s_ncand = 0; s_tile_max = 0; }
-    __syncthreads();
-    const u32 thr = need_bound ? max(cta_kth_bound(s_top, t.k, true), 1u) : 1u;
-    const u64 slot0 = ((u64)row * t.n_tiles + tile) * t.slots;
-    u32 cand_max = 0;
-#pragma unroll
-    for (int j = 0; j < PER_THREAD / 4; j++) {
-#pragma unroll
-        for (int e = 0; e < 4; e++) {
-            if (key[j * 4 + e] >= thr) {
-                const u32 local = (tid + j * SA_TERM_THREADS) * 4 + e;
-                const u32 slot = atomicAdd(&s_ncand, 1u);
-                if (slot < t.slots) {
-                    // the float64 score again, for the few candidates (cheaper than holding 32 doubles per thread)
-                    const u64 doc = rows ? __ldg(rows + pos0 + local) : pos0 + local;
-                    const double s = sim_classic(q_idf, __ldg(counts + doc), __ldg(doc_lens + doc));
-                    t.tile_cand[slot0 + slot] = ((u64)key[j * 4 + e] << 32) | (u64)(0xFFFFFFFFu - (tile * SA_TILE_DOCS + local));
-                    tile_d[slot0 + slot] = (u64)__double_as_longlong(s);
-                }
-                cand_max = max(cand_max, key[j * 4 + e]);
-            }
-        }
-    }
-    if (cand_max) atomicMax(&s_tile_max, cand_max);
-    __syncthreads();
-    if (tid == 0) {
-        const u64 t_idx = (u64)row * t.n_tiles + tile;
-        t.tile_cnt[t_idx] = min(s_ncand, t.slots);
-        t.tile_max[t_idx] = s_tile_max;
-        if (s_ncand > t.slots) t.overflow[row] = 1u;
     }
 }
 
@@ -189,29 +151,35 @@ struct SimRun {
     u32 n_terms(u32 q) const { return term_starts[q + 1] - term_starts[q]; }
 };
 
-// The tile pass over ix->dense rows [0, n): row j holds the counts of row row0 + j of t, d_idf[j] is its idf.
-static int launch_tiles(sa_index *ix, const SimRun &R, const double *d_idf, u32 n, u32 row0, const TopkCtx &t) {
-    ViewState &V = *ix->view;
+int launch_sim_tiles(sa_index *ix, int kind, const float *counts, const u64 *rows, const float *doc_lens, u64 n_pos,
+                     const Bm25Params &bm25, const SimParams &sim, const double *d_idf, u32 n, u32 row0,
+                     const TopkCtx &t, u64 *tile_d) {
     if (n == 0 || t.n_tiles == 0) return SA_OK;
-    const float *counts = ix->dense.as<float>();
     const u64 stride = sa_padded_docs(ix->n_docs);
-    const u64 *rows = ix->rows_active ? ix->d_rows : nullptr;
-    const u64 n_pos = ix->rows_active ? ix->n_rows : ix->n_docs;
     const dim3 grid(t.n_tiles, n);
     KernelTimer tm(ix, 1);
-#define SA_SIM_TILES(KIND, DOC_LENS, P)                                                                              \
-    sim_tile_kernel<KIND><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(counts, stride, rows, DOC_LENS, n_pos, P, d_idf, \
-                                                                    row0, t, V.d_cand_d.as<u64>())
-    if (R.kind == SA_SIM_BM25) SA_SIM_TILES(SA_SIM_BM25, V.d_dl.as<float>(), R.bm25);
-    else if (R.kind == SA_SIM_BM25_IMPACT) SA_SIM_TILES(SA_SIM_BM25_IMPACT, ix->d_doc_lens, R.sim);
-    else if (R.kind == SA_SIM_BM25_LEGACY) SA_SIM_TILES(SA_SIM_BM25_LEGACY, ix->d_doc_lens, R.sim);
-    else SA_SIM_TILES(SA_SIM_CLASSIC, ix->d_doc_lens, R.sim);
+#define SA_SIM_TILES(KIND, P)                                                                                       \
+    sim_tile_kernel<KIND><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(counts, stride, rows, doc_lens, n_pos, P, d_idf, \
+                                                                    row0, t, tile_d)
+    if (kind == SA_SIM_BM25) SA_SIM_TILES(SA_SIM_BM25, bm25);
+    else if (kind == SA_SIM_BM25_IMPACT) SA_SIM_TILES(SA_SIM_BM25_IMPACT, sim);
+    else if (kind == SA_SIM_BM25_LEGACY) SA_SIM_TILES(SA_SIM_BM25_LEGACY, sim);
+    else SA_SIM_TILES(SA_SIM_CLASSIC, sim);
 #undef SA_SIM_TILES
     SA_CUDA(cudaGetLastError());
     tm.stop();
     ix->stats.topk_kernel_launches++;
     ix->stats.total_launches++;
     return SA_OK;
+}
+
+// The tile pass over ix->dense rows [0, n): row j holds the counts of row row0 + j of t, d_idf[j] is its idf.
+static int launch_tiles(sa_index *ix, const SimRun &R, const double *d_idf, u32 n, u32 row0, const TopkCtx &t) {
+    ViewState &V = *ix->view;
+    const bool view = ix->rows_active;
+    return launch_sim_tiles(ix, R.kind, ix->dense.as<float>(), view ? ix->d_rows : nullptr,
+                            R.kind == SA_SIM_BM25 ? V.d_dl.as<float>() : ix->d_doc_lens, view ? ix->n_rows : ix->n_docs,
+                            R.bm25, R.sim, d_idf, n, row0, t, V.d_cand_d.as<u64>());
 }
 
 static int launch_select(sa_index *ix, int kind, const TopkCtx &t, u32 n_queries, const u32 *d_out_index) {
