@@ -46,6 +46,9 @@ int sa_device_count(int *n_out);
 /* Pinned host memory for result vectors (D2H of a dense float32[N] at full PCIe rate). */
 int sa_host_alloc(void **ptr_out, uint64_t bytes);
 int sa_host_free(void *ptr);
+/* Device buffers the library holds right now in this process, and their bytes (every index, multi-field handle and
+ * in-flight call).  Returns to its earlier value once everything created since is destroyed. */
+int sa_device_allocations(uint64_t *live_buffers, uint64_t *live_bytes);
 
 /* ---------------------------------------------------------------------- index
  * Uploads one shard of the inverted index into HBM.  Replaces the host-side state the

@@ -34,6 +34,7 @@ SIGNATURES = {
     "sa_device_count": (c_int, [ctypes.POINTER(c_int)]),
     "sa_host_alloc": (c_int, [ctypes.POINTER(P_void), c_u64]),
     "sa_host_free": (c_int, [P_void]),
+    "sa_device_allocations": (c_int, [P_u64, P_u64]),
     "sa_index_create": (c_int, [P_u64, c_u64, P_u64, P_u64, c_u32, P_f32, c_u64, c_u64, c_int,
                                 ctypes.POINTER(P_void)]),
     "sa_index_destroy": (c_int, [P_void]),

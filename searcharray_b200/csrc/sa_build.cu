@@ -21,17 +21,6 @@
 
 namespace {
 
-struct DevMemB {
-    std::vector<void *> ptrs;
-    ~DevMemB() { for (void *p : ptrs) cudaFree(p); }
-    template <typename T> T *alloc(size_t n) {
-        void *p = nullptr;
-        if (cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T) + 64) != cudaSuccess) return nullptr;
-        ptrs.push_back(p);
-        return (T *)p;
-    }
-};
-
 __global__ void iota_kernel(u32 *__restrict__ a, u64 n) {
     const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) a[i] = (u32)i;
@@ -140,7 +129,7 @@ extern "C" int sa_op_build_index(const uint32_t *term_ids, const uint32_t *doc_i
     SA_CHECK(n_triples < (1ull << 32), "too many tokens for one build call (batch them like the reference's batch_size)");
     SA_CUDA(cudaSetDevice(device));
     const u64 n = n_triples;
-    DevMemB m;
+    DevMem m;
     u32 *d_t = m.alloc<u32>(n), *d_ts = m.alloc<u32>(n), *d_i = m.alloc<u32>(n), *d_is = m.alloc<u32>(n);
     u32 *d_doc = m.alloc<u32>(n), *d_pos = m.alloc<u32>(n), *d_head = m.alloc<u32>(n), *d_offs = m.alloc<u32>(n);
     const u32 n_blocks = (u32)((n + 1023) / 1024);

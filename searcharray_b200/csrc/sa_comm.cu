@@ -148,8 +148,8 @@ static int download_merged(sa_index *ix, size_t nq, u32 k, uint32_t *out_docs, f
                            bool count_stats) {
     const size_t nk = nq * k, blk = nk + SA_BATCH_TAIL;
     int rc;
-    if ((rc = sa_pinned_reserve(ix, (nk + (size_t)ix->world * SA_BATCH_TAIL) * sizeof(u64)))) return rc;
-    u64 *h = (u64 *)ix->h_pinned;
+    if ((rc = ix->h_pinned.reserve((nk + (size_t)ix->world * SA_BATCH_TAIL) * sizeof(u64)))) return rc;
+    u64 *h = ix->h_pinned.as<u64>();
     const u64 *d_all = ix->gather.as<u64>();
     const u64 *d_merged = d_all + (size_t)ix->world * blk;
     if (nk) SA_CUDA(cudaMemcpyAsync(h, d_merged, nk * sizeof(u64), cudaMemcpyDeviceToHost, ix->stream));

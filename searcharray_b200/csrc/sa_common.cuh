@@ -5,8 +5,11 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <string.h>
+#include <atomic>
+#include <memory>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/searcharray_b200.h"
@@ -46,33 +49,93 @@ void sa_set_error(const char *fmt, ...);
         }                                                                              \
     } while (0)
 
-// ---- a growable device buffer -----------------------------------------------------
-struct DevBuf {
+// ---- owned memory ---------------------------------------------------------------------
+// Every cudaMalloc / cudaHostAlloc of the library is made by a Buffer (apart from sa_host_alloc's, which hands its
+// memory to the caller), and the Buffer frees it when its owner goes away, on every return path.  A device buffer is
+// destroyed while its device is current: ~sa_index and ~sa_multi set the device first, and locals live inside calls
+// that have set it.
+inline std::atomic<uint64_t> g_live_dev_buffers{0}, g_live_dev_bytes{0};   // sa_device_allocations
+
+struct DeviceSpace {
+    static constexpr const char *name = "cudaMalloc";
+    static cudaError_t alloc(void **p, size_t bytes) {
+        cudaError_t e = cudaMalloc(p, bytes);
+        if (e == cudaSuccess && *p) { g_live_dev_buffers++; g_live_dev_bytes += bytes; }
+        return e;
+    }
+    static void free(void *p, size_t bytes) {
+        cudaFree(p);
+        g_live_dev_buffers--;
+        g_live_dev_bytes -= bytes;
+    }
+};
+
+struct PinnedSpace {
+    static constexpr const char *name = "cudaHostAlloc";
+    static cudaError_t alloc(void **p, size_t bytes) { return cudaHostAlloc(p, bytes, cudaHostAllocDefault); }
+    static void free(void *p, size_t) { cudaFreeHost(p); }
+};
+
+template <typename Space> struct Buffer {
     void *p = nullptr;
     size_t cap = 0;
+    Buffer() = default;
+    Buffer(const Buffer &) = delete;
+    Buffer &operator=(const Buffer &) = delete;
+    Buffer(Buffer &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    Buffer &operator=(Buffer &&o) noexcept {
+        if (this != &o) {
+            reset();
+            std::swap(p, o.p);
+            std::swap(cap, o.cap);
+        }
+        return *this;
+    }
+    ~Buffer() { reset(); }
+    // At least `bytes`; the contents are not kept.  Grows geometrically: cudaFree + cudaMalloc synchronise the
+    // device, so a buffer that creeps up query by query must not be reallocated on every new maximum.
     int reserve(size_t bytes) {
         if (bytes <= cap) return SA_OK;
-        // grow geometrically: cudaFree + cudaMalloc synchronise the device, so a buffer that creeps up
-        // query by query must not be reallocated on every new maximum
-        const size_t want = std::max(bytes + (bytes >> 3), cap + (cap >> 1)) + 256;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        cudaError_t e = cudaMalloc(&p, want);
+        return allocate(std::max(bytes + (bytes >> 3), cap + (cap >> 1)) + 256);
+    }
+    // Exactly `bytes` (the index's fixed arrays); the contents are not kept.
+    int allocate(size_t bytes) {
+        reset();
+        cudaError_t e = Space::alloc(&p, bytes);
         if (e != cudaSuccess) {
-            sa_set_error("cudaMalloc(%zu) failed: %s", want, cudaGetErrorString(e));
+            sa_set_error("%s(%zu) failed: %s", Space::name, bytes, cudaGetErrorString(e));
             p = nullptr;
             return SA_ERR_NOMEM;
         }
-        cap = want;
+        cap = bytes;
         return SA_OK;
     }
-    void release() {
-        if (p) cudaFree(p);
+    void reset() {
+        if (p) Space::free(p, cap);
         p = nullptr;
         cap = 0;
     }
     template <typename T> T *as() const { return (T *)p; }
+};
+using DevBuf = Buffer<DeviceSpace>;
+using PinnedBuf = Buffer<PinnedSpace>;
+static_assert(!std::is_copy_constructible<DevBuf>::value, "a DevBuf has exactly one owner");
+
+// The scratch arrays of one call, freed when the set goes out of scope.
+struct DevMem {
+    std::vector<DevBuf> bufs;
+    template <typename T> T *alloc(size_t n) {
+        DevBuf b;
+        if (b.allocate(std::max<size_t>(n, 1) * sizeof(T) + 64)) return nullptr;
+        bufs.push_back(std::move(b));
+        return bufs.back().as<T>();
+    }
+    template <typename T> T *upload(const T *h, size_t n) {
+        T *d = alloc<T>(n + 4);                       // pad: staged copies read up to 2 words past a slice
+        if (!d || cudaMemset(d + n, 0, 4 * sizeof(T)) != cudaSuccess) return nullptr;
+        if (n && cudaMemcpy(d, h, n * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
+        return d;
+    }
 };
 
 // ---- BM25 parameters as the reference passes them to bm25_score ---------------------
@@ -102,10 +165,13 @@ struct TermQuery {
 #define SA_REC_TF_MASK 0x7FFFFu
 
 // ---- the index handle ---------------------------------------------------------------
-struct TimedLaunch;
+struct TimedLaunch { cudaEvent_t e0, e1; int kind; };   // kind: 0 term, 1 topk, 2 phrase (see KernelTimer)
 struct BatchState;
 struct ViewState;
+struct BatchStateDelete { void operator()(BatchState *b) const; };   // sa_index.cu
+struct ViewStateDelete { void operator()(ViewState *v) const; };     // sa_view.cu
 struct sa_index {
+    ~sa_index();
     int device = 0;
     int num_sms = SA_NUM_SMS_FALLBACK;
     u64 n_docs = 0, n_words = 0, doc_base = 0;
@@ -114,22 +180,22 @@ struct sa_index {
     int upload_mode = 0;             // how the posting words reached HBM (sa_index_upload_mode)
 
     // HBM-resident index
-    u64 *d_words = nullptr;          // [n_words + 1] (one readable pad word)
-    float *d_doc_lens = nullptr;     // [n_docs]
-    u32 *d_df = nullptr;             // [n_terms] distinct docs per term (this shard)
+    DevBuf d_words;                  // u64 [n_words + 1] (one readable pad word)
+    DevBuf d_doc_lens;               // float [n_docs]
+    DevBuf d_df;                     // u32 [n_terms] distinct docs per term (this shard)
     // tile directory of long posting lists: for term t with h_dir_off[t] != SA_NO_DIR,
     // d_tile_dir[h_dir_off[t] + j] = index (within the term's list) of the first word whose
     // doc lies in tile >= j, j = 0..n_tiles  (tile = 4096 docs).  Built on the device at upload.
-    u32 *d_tile_dir = nullptr;
+    DevBuf d_tile_dir;               // u32
     std::vector<u64> h_dir_off;
     // per-term tf table (the analogue of the reference's termfreq_cache, middle_out.py:501-509, built on the
     // device at upload): for every term WITH a tile directory, one u32 record per (term, doc) in doc order,
     // (doc - tile_doc0) << 19 | tf; d_rec_dir mirrors d_tile_dir (same offsets) with indices into the records.
-    u32 *d_recs = nullptr;
-    u32 *d_rec_dir = nullptr;
+    DevBuf d_recs;                   // u32
+    DevBuf d_rec_dir;                // u32
     std::vector<u64> h_rec_off;
     // per-doc BM25 length norm k1*((1-b)+b*dl/avgdl) for the last used (k1, b, avgdl)
-    float *d_norm = nullptr;         // [padded n_docs]
+    DevBuf d_norm;                   // float [padded n_docs]
     float norm_k1 = 0, norm_b = 0, norm_avgdl = 0;
     bool norm_valid = false;
     // host mirrors for query set-up
@@ -140,16 +206,20 @@ struct sa_index {
     // sliced-array filter (FilteredPosns semantics)
     u64 n_rows = 0;                  // number of selected rows
     bool rows_active = false;        // a row filter is installed (n_rows may be 0)
-    u64 *d_rows = nullptr;           // sorted local doc indices
-    unsigned char *d_row_mask = nullptr;  // [n_docs] 1 if doc selected
+    // one buffer, so that installing a filter allocates once: the row mask (unsigned char [n_docs], 1 if doc selected),
+    // then the rows (u64, sorted local doc indices) at row_mask_bytes()
+    DevBuf row_filter;
+    size_t row_mask_bytes() const { return (std::max<u64>(n_docs, 1) + 15) & ~(size_t)15; }
+    unsigned char *d_row_mask() const { return row_filter.as<unsigned char>(); }
+    u64 *d_rows() const { return row_filter.p ? (u64 *)(row_filter.as<char>() + row_mask_bytes()) : nullptr; }
 
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;   // sa_timer_start / sa_timer_stop
     bool profiling = false;
-    std::vector<struct TimedLaunch> *pending_timers = nullptr;
-    std::vector<cudaEvent_t> *free_events = nullptr;
-    struct BatchState *batch = nullptr;
-    struct ViewState *view = nullptr;   // buffers of sa_score_batch_topk_sim (sa_view.cu)
+    std::vector<TimedLaunch> pending_timers;
+    std::vector<cudaEvent_t> free_events;
+    std::unique_ptr<BatchState, BatchStateDelete> batch;
+    std::unique_ptr<ViewState, ViewStateDelete> view;   // buffers of sa_score_batch_topk_sim (sa_view.cu)
     sa_stats stats;
     std::mutex mu;
 
@@ -162,8 +232,7 @@ struct sa_index {
     DevBuf phrase_scratch;
     DevBuf filt;         // filtered (sliced / position-filtered) copies of posting lists
     DevBuf misc;
-    void *h_pinned = nullptr;   // pinned staging
-    size_t h_pinned_cap = 0;
+    PinnedBuf h_pinned;  // pinned staging
 
     // NCCL
     void *nccl_comm = nullptr;
@@ -173,11 +242,8 @@ struct sa_index {
     size_t device_bytes = 0;
 };
 
-int sa_pinned_reserve(sa_index *ix, size_t bytes);
-
 // Kernel timing without serialising the stream: when profiling is on every timed launch gets
 // an event pair from a pool; elapsed times are resolved lazily (sa_stats_get syncs once).
-struct TimedLaunch { cudaEvent_t e0, e1; int kind; };   // kind: 0 term, 1 topk, 2 phrase
 struct KernelTimer {
     sa_index *ix;
     int kind;

@@ -36,13 +36,17 @@ int sa_filter_terms_mask(sa_index *ix, const uint32_t *term_ids, uint32_t n_term
 #define ED_MAX_ROWS 64
 
 struct sa_multi {
+    ~sa_multi() {
+        cudaSetDevice(device);          // the buffers below are freed after this body, on this device
+        if (stream) { cudaStreamSynchronize(stream); cudaStreamDestroy(stream); }
+    }
     std::vector<sa_index *> fields;
     int device = 0;
     u64 n_docs = 0, doc_base = 0, stride = 0;
     cudaStream_t stream = nullptr;
-    double *d_qf = nullptr;              // [stride] combined scores (float32 values widened in field-centric mode)
-    unsigned char *d_mask = nullptr;     // [stride] qf > 0 after the qf phase
-    unsigned long long *d_count = nullptr;
+    DevBuf d_qf;                         // double [stride] combined scores (float32 values widened in field-centric mode)
+    DevBuf d_mask;                       // unsigned char [stride] qf > 0 after the qf phase
+    DevBuf d_count;                      // unsigned long long
     bool f32_mode = false, has_qf = false;
     std::vector<std::vector<u64>> filt_offs, filt_lens;   // per field: last sa_multi_filter
     std::vector<u32> phrase_rows;        // per field: rows produced by the last sa_multi_phrases
@@ -205,7 +209,7 @@ extern "C" int sa_multi_create(sa_index *const *fields, uint32_t n_fields, sa_mu
         SA_CHECK(fields[f]->device == fields[0]->device && fields[f]->n_docs == fields[0]->n_docs &&
                  fields[f]->doc_base == fields[0]->doc_base, "fields must share device, doc range and size");
     }
-    sa_multi *m = new sa_multi();
+    std::unique_ptr<sa_multi> m(new sa_multi());
     m->fields.assign(fields, fields + n_fields);
     m->device = fields[0]->device;
     m->n_docs = fields[0]->n_docs;
@@ -215,30 +219,16 @@ extern "C" int sa_multi_create(sa_index *const *fields, uint32_t n_fields, sa_mu
     m->filt_lens.resize(n_fields);
     m->phrase_rows.assign(n_fields, 0);
     m->filt_bound.assign(n_fields, 0);
-    cudaSetDevice(m->device);
+    SA_CUDA(cudaSetDevice(m->device));
     const u64 s = std::max<u64>(m->stride, SA_TILE_DOCS);
-    bool ok = cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking) == cudaSuccess &&
-              cudaMalloc(&m->d_qf, s * sizeof(double)) == cudaSuccess &&
-              cudaMalloc(&m->d_mask, s) == cudaSuccess &&
-              cudaMalloc(&m->d_count, 64) == cudaSuccess;
-    if (!ok) {
-        sa_set_error("sa_multi_create: %s", cudaGetErrorString(cudaGetLastError()));
-        sa_multi_destroy(m);
-        return SA_ERR_NOMEM;
-    }
-    *out = m;
+    SA_CUDA(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
+    int rc;
+    if ((rc = m->d_qf.allocate(s * sizeof(double))) || (rc = m->d_mask.allocate(s)) || (rc = m->d_count.allocate(64))) return rc;
+    *out = m.release();
     return SA_OK;
 }
 
 extern "C" int sa_multi_destroy(sa_multi *m) {
-    if (!m) return SA_OK;
-    cudaSetDevice(m->device);
-    if (m->stream) { cudaStreamSynchronize(m->stream); cudaStreamDestroy(m->stream); }
-    cudaFree(m->d_qf);
-    cudaFree(m->d_mask);
-    cudaFree(m->d_count);
-    m->cand.release();
-    m->keys.release();
     delete m;
     return SA_OK;
 }
@@ -291,16 +281,16 @@ extern "C" int sa_multi_qf(sa_multi *m, int field_centric, const uint32_t *n_ter
     a.tie = tie;
     a.n_docs = m->n_docs;
     a.stride = m->stride;
-    a.qf = m->d_qf;
-    a.mask = m->d_mask;
-    a.count = m->d_count;
-    SA_CUDA(cudaMemsetAsync(m->d_count, 0, sizeof(unsigned long long), m->stream));
+    a.qf = m->d_qf.as<double>();
+    a.mask = m->d_mask.as<unsigned char>();
+    a.count = m->d_count.as<unsigned long long>();
+    SA_CUDA(cudaMemsetAsync(m->d_count.p, 0, sizeof(unsigned long long), m->stream));
     const unsigned blocks = (unsigned)((std::max<u64>(m->stride, 1) + 255) / 256);
     if (field_centric) edismax_combine_fields_kernel<<<blocks, 256, 0, m->stream>>>(a);
     else edismax_combine_terms_kernel<<<blocks, 256, 0, m->stream>>>(a);
     SA_CUDA(cudaGetLastError());
     unsigned long long cnt = 0;
-    SA_CUDA(cudaMemcpyAsync(&cnt, m->d_count, sizeof(cnt), cudaMemcpyDeviceToHost, m->stream));
+    SA_CUDA(cudaMemcpyAsync(&cnt, m->d_count.p, sizeof(cnt), cudaMemcpyDeviceToHost, m->stream));
     SA_CUDA(cudaStreamSynchronize(m->stream));
     *n_matches = cnt;
     m->f32_mode = field_centric != 0;
@@ -333,7 +323,7 @@ extern "C" int sa_multi_filter(sa_multi *m, uint32_t field, const uint32_t *term
         int rc0 = ix->filt.reserve(m->filt_bound[field] * sizeof(u64));
         if (rc0) return rc0;
     }
-    if ((rc = sa_filter_terms_mask(ix, term_ids, n_terms, m->d_mask, 0, SA_ALL_BITS, false,
+    if ((rc = sa_filter_terms_mask(ix, term_ids, n_terms, m->d_mask.as<unsigned char>(), 0, SA_ALL_BITS, false,
                                    m->filt_offs[field], m->filt_lens[field], &dfs))) return rc;
     for (u32 t = 0; t < n_terms; t++) df_out[t] = dfs[t];
     return SA_OK;
@@ -397,7 +387,7 @@ extern "C" int sa_multi_add_phase(sa_multi *m, uint32_t n_entries, const uint32_
     }
     a.n = n_entries;
     a.n_docs = m->n_docs;
-    a.qf = m->d_qf;
+    a.qf = m->d_qf.as<double>();
     a.f32_mode = m->f32_mode ? 1 : 0;
     if (m->n_docs) {
         edismax_add_phase_kernel<<<(unsigned)((m->n_docs + 255) / 256), 256, 0, m->stream>>>(a);
@@ -413,12 +403,12 @@ extern "C" int sa_multi_download(sa_multi *m, void *out, int as_float32) {
     SA_CUDA(cudaSetDevice(m->device));
     if (m->n_docs == 0) return SA_OK;
     if (!as_float32) {
-        SA_CUDA(cudaMemcpyAsync(out, m->d_qf, m->n_docs * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+        SA_CUDA(cudaMemcpyAsync(out, m->d_qf.as<double>(), m->n_docs * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
         SA_CUDA(cudaStreamSynchronize(m->stream));
         return SA_OK;
     }
     std::vector<double> tmp(m->n_docs);
-    SA_CUDA(cudaMemcpyAsync(tmp.data(), m->d_qf, m->n_docs * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
+    SA_CUDA(cudaMemcpyAsync(tmp.data(), m->d_qf.as<double>(), m->n_docs * sizeof(double), cudaMemcpyDeviceToHost, m->stream));
     SA_CUDA(cudaStreamSynchronize(m->stream));
     float *o = (float *)out;
     for (u64 i = 0; i < m->n_docs; i++) o[i] = (float)tmp[i];           // exact: the values are float32
@@ -456,7 +446,7 @@ extern "C" int sa_multi_topk(sa_multi *m, uint32_t k, uint32_t *out_docs, double
         const TopkCtx t = make_topk_ctx(m->cand.p, T, 1, slots, k, d_ovf);
         {
             KernelTimer tm(ix, 1);
-            edismax_tile_kernel<<<T, SA_TERM_THREADS, 0, m->stream>>>(m->d_qf, m->n_docs, t, tile_d);
+            edismax_tile_kernel<<<T, SA_TERM_THREADS, 0, m->stream>>>(m->d_qf.as<double>(), m->n_docs, t, tile_d);
             SA_CUDA(cudaGetLastError());
             tm.stop();
             ix->stats.topk_kernel_launches++;

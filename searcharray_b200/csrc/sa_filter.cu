@@ -152,13 +152,15 @@ int sa_filter_terms_mask(sa_index *ix, const uint32_t *term_ids, uint32_t n_term
     u32 *d_df = d_totals + n_terms;
     SA_CUDA(cudaMemcpyAsync(d_jobs, jobs.data(), n_terms * sizeof(FilterJob), cudaMemcpyHostToDevice, ix->stream));
     dim3 grid((unsigned)max_chunks, n_terms);
-    filter_lists_kernel<false><<<grid, FILT_THREADS, 0, ix->stream>>>(ix->d_words, d_jobs, ix->filt.as<u64>(), d_chunks, d_mask,
-                                                                     ix->doc_base, ix->n_docs, pay_lo, pay_hi, use_payload ? 1 : 0);
+    filter_lists_kernel<false><<<grid, FILT_THREADS, 0, ix->stream>>>(ix->d_words.as<u64>(), d_jobs, ix->filt.as<u64>(), d_chunks,
+                                                                     d_mask, ix->doc_base, ix->n_docs, pay_lo, pay_hi,
+                                                                     use_payload ? 1 : 0);
     SA_CUDA(cudaGetLastError());
     filter_scan_kernel<<<n_terms, FILT_THREADS, 0, ix->stream>>>(d_jobs, d_chunks, d_totals);
     SA_CUDA(cudaGetLastError());
-    filter_lists_kernel<true><<<grid, FILT_THREADS, 0, ix->stream>>>(ix->d_words, d_jobs, ix->filt.as<u64>(), d_chunks, d_mask,
-                                                                    ix->doc_base, ix->n_docs, pay_lo, pay_hi, use_payload ? 1 : 0);
+    filter_lists_kernel<true><<<grid, FILT_THREADS, 0, ix->stream>>>(ix->d_words.as<u64>(), d_jobs, ix->filt.as<u64>(), d_chunks,
+                                                                    d_mask, ix->doc_base, ix->n_docs, pay_lo, pay_hi,
+                                                                    use_payload ? 1 : 0);
     SA_CUDA(cudaGetLastError());
     ix->stats.total_launches += 3;
     std::vector<u32> h_counts(n_terms);
@@ -185,8 +187,8 @@ int sa_filter_terms_mask(sa_index *ix, const uint32_t *term_ids, uint32_t n_term
 
 int sa_filter_terms(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, bool use_rows,
                     u64 pay_lo, u64 pay_hi, bool use_payload, std::vector<u64> &offs, std::vector<u64> &lens) {
-    return sa_filter_terms_mask(ix, term_ids, n_terms, use_rows ? ix->d_row_mask : nullptr, pay_lo, pay_hi, use_payload,
-                                offs, lens, nullptr);
+    return sa_filter_terms_mask(ix, term_ids, n_terms, use_rows ? ix->d_row_mask() : nullptr, pay_lo, pay_hi,
+                                use_payload, offs, lens, nullptr);
 }
 
 int sa_copy_out_dense(sa_index *ix, float *out_host) {
@@ -197,7 +199,7 @@ int sa_copy_out_dense(sa_index *ix, float *out_host) {
     }
     int rc;
     if ((rc = ix->gather.reserve(ix->n_rows * sizeof(float) + 64))) return rc;
-    gather_rows_kernel<<<(unsigned)((ix->n_rows + 255) / 256), 256, 0, ix->stream>>>(ix->dense.as<float>(), ix->d_rows,
+    gather_rows_kernel<<<(unsigned)((ix->n_rows + 255) / 256), 256, 0, ix->stream>>>(ix->dense.as<float>(), ix->d_rows(),
                                                                                    ix->n_rows, ix->gather.as<float>());
     SA_CUDA(cudaGetLastError());
     ix->stats.total_launches++;
@@ -221,13 +223,16 @@ extern "C" int sa_index_set_rows(sa_index *ix, const uint64_t *rows, uint64_t n_
         SA_CHECK(rows[i] < ix->n_docs, "row %llu out of range", (unsigned long long)rows[i]);
         mask[rows[i]] = 1;
     }
-    cudaFree(ix->d_rows);
-    ix->d_rows = nullptr;
-    SA_CUDA(cudaMalloc(&ix->d_rows, std::max<u64>(n_rows, 1) * sizeof(u64)));
-    if (!ix->d_row_mask) SA_CUDA(cudaMalloc(&ix->d_row_mask, std::max<u64>(ix->n_docs, 1)));
-    if (n_rows) SA_CUDA(cudaMemcpyAsync(ix->d_rows, rows, n_rows * sizeof(u64), cudaMemcpyHostToDevice, ix->stream));
-    if (ix->n_docs) SA_CUDA(cudaMemcpyAsync(ix->d_row_mask, mask.data(), ix->n_docs, cudaMemcpyHostToDevice, ix->stream));
+    // the new filter is built aside and swapped in only once complete: a failed call leaves the previous one installed
+    const size_t mask_bytes = ix->row_mask_bytes();
+    DevBuf filter;
+    int rc;
+    if ((rc = filter.allocate(mask_bytes + std::max<u64>(n_rows, 1) * sizeof(u64)))) return rc;
+    if (ix->n_docs) SA_CUDA(cudaMemcpyAsync(filter.p, mask.data(), ix->n_docs, cudaMemcpyHostToDevice, ix->stream));
+    if (n_rows)
+        SA_CUDA(cudaMemcpyAsync(filter.as<char>() + mask_bytes, rows, n_rows * sizeof(u64), cudaMemcpyHostToDevice, ix->stream));
     SA_CUDA(cudaStreamSynchronize(ix->stream));
+    ix->row_filter = std::move(filter);
     ix->n_rows = n_rows;
     ix->rows_active = true;
     return SA_OK;
@@ -288,7 +293,7 @@ static int docfreq_rows_locked(sa_index *ix, const uint32_t *term_ids, uint32_t 
         if (t == SA_NO_TERM || ix->h_len[t] == 0) continue;
         DfJob j;
         j.slot = i;
-        if (ix->d_recs && ix->h_rec_off[t] != SA_NO_DIR && ix->h_dir_off[t] != SA_NO_DIR) {
+        if (ix->d_recs.p && ix->h_rec_off[t] != SA_NO_DIR && ix->h_dir_off[t] != SA_NO_DIR) {
             j.recs = 1;
             j.src_off = ix->h_rec_off[t];
             j.dir_off = ix->h_dir_off[t];
@@ -317,8 +322,9 @@ static int docfreq_rows_locked(sa_index *ix, const uint32_t *term_ids, uint32_t 
         unsigned long long *d_df = (unsigned long long *)((char *)ix->misc.p + jobs_bytes);
         SA_CUDA(cudaMemcpyAsync(d_jobs, jobs.data(), jobs.size() * sizeof(DfJob), cudaMemcpyHostToDevice, ix->stream));
         SA_CUDA(cudaMemsetAsync(d_df, 0, (size_t)n_terms * sizeof(u64), ix->stream));
-        docfreq_rows_kernel<<<(unsigned)jobs.size(), FILT_THREADS, 0, ix->stream>>>(ix->d_words, ix->d_recs, ix->d_rec_dir, d_jobs,
-                                                                               ix->d_row_mask, ix->doc_base, ix->n_docs, d_df);
+        docfreq_rows_kernel<<<(unsigned)jobs.size(), FILT_THREADS, 0, ix->stream>>>(
+            ix->d_words.as<u64>(), ix->d_recs.as<u32>(), ix->d_rec_dir.as<u32>(), d_jobs, ix->d_row_mask(),
+            ix->doc_base, ix->n_docs, d_df);
         SA_CUDA(cudaGetLastError());
         ix->stats.total_launches++;
         SA_CUDA(cudaMemcpyAsync(h_df.data(), d_df, (size_t)n_terms * sizeof(u64), cudaMemcpyDeviceToHost, ix->stream));

@@ -39,13 +39,10 @@ extern "C" int sa_host_free(void *ptr) {
     return SA_OK;
 }
 
-int sa_pinned_reserve(sa_index *ix, size_t bytes) {
-    if (bytes <= ix->h_pinned_cap) return SA_OK;
-    if (ix->h_pinned) cudaFreeHost(ix->h_pinned);
-    ix->h_pinned = nullptr;
-    ix->h_pinned_cap = 0;
-    SA_CUDA(cudaHostAlloc(&ix->h_pinned, bytes, cudaHostAllocDefault));
-    ix->h_pinned_cap = bytes;
+extern "C" int sa_device_allocations(uint64_t *live_buffers, uint64_t *live_bytes) {
+    SA_CHECK(live_buffers && live_bytes, "NULL argument");
+    *live_buffers = g_live_dev_buffers;
+    *live_bytes = g_live_dev_bytes;
     return SA_OK;
 }
 
@@ -71,32 +68,34 @@ static int upload_bulk(void *dst, const void *src, size_t bytes, cudaStream_t st
         }
         cudaGetLastError();                                   // registration refused: clear the error, bounce instead
         const size_t CH = 32u << 20;
-        void *pin[2] = {nullptr, nullptr};
-        cudaEvent_t ev[2] = {nullptr, nullptr};
-        bool ok = cudaHostAlloc(&pin[0], CH, cudaHostAllocDefault) == cudaSuccess &&
-                  cudaHostAlloc(&pin[1], CH, cudaHostAllocDefault) == cudaSuccess &&
-                  cudaEventCreate(&ev[0]) == cudaSuccess && cudaEventCreate(&ev[1]) == cudaSuccess;
+        struct EventDestroy { void operator()(cudaEvent_t e) const { cudaEventDestroy(e); } };
+        PinnedBuf pin[2];
+        std::unique_ptr<CUevent_st, EventDestroy> ev[2];
+        bool ok = pin[0].allocate(CH) == SA_OK && pin[1].allocate(CH) == SA_OK;
+        for (int i = 0; i < 2 && ok; i++) {
+            cudaEvent_t e = nullptr;
+            ok = cudaEventCreate(&e) == cudaSuccess;
+            ev[i].reset(e);
+        }
         if (ok) {
             size_t at = 0;
             int b = 0;
             cudaError_t e = cudaSuccess;
             while (at < bytes && e == cudaSuccess) {
                 const size_t n = std::min(CH, bytes - at);
-                e = cudaEventSynchronize(ev[b]);              // the previous copy out of this buffer is done
+                e = cudaEventSynchronize(ev[b].get());        // the previous copy out of this buffer is done
                 if (e != cudaSuccess) break;
-                memcpy(pin[b], (const char *)src + at, n);
-                e = cudaMemcpyAsync((char *)dst + at, pin[b], n, cudaMemcpyHostToDevice, stream);
-                if (e == cudaSuccess) e = cudaEventRecord(ev[b], stream);
+                memcpy(pin[b].p, (const char *)src + at, n);
+                e = cudaMemcpyAsync((char *)dst + at, pin[b].p, n, cudaMemcpyHostToDevice, stream);
+                if (e == cudaSuccess) e = cudaEventRecord(ev[b].get(), stream);
                 at += n;
                 b ^= 1;
             }
             if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
-            for (int i = 0; i < 2; i++) { cudaFreeHost(pin[i]); cudaEventDestroy(ev[i]); }
             if (e != cudaSuccess) { sa_set_error("bounce upload failed: %s", cudaGetErrorString(e)); return SA_ERR_CUDA; }
             *mode_out = 2;
             return SA_OK;
         }
-        for (int i = 0; i < 2; i++) { if (pin[i]) cudaFreeHost(pin[i]); if (ev[i]) cudaEventDestroy(ev[i]); }
         cudaGetLastError();
     }
     SA_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, stream));
@@ -298,7 +297,7 @@ extern "C" int sa_index_create(const uint64_t *words, uint64_t n_words,
         SA_CHECK(term_offsets[t] + term_lengths[t] <= n_words, "term %u slice out of range", t);
     SA_CUDA(cudaSetDevice(device));
 
-    sa_index *ix = new sa_index();
+    std::unique_ptr<sa_index> ix(new sa_index());
     ix->device = device;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) ix->num_sms = prop.multiProcessorCount;
@@ -316,30 +315,26 @@ extern "C" int sa_index_create(const uint64_t *words, uint64_t n_words,
     for (u32 t = 0; t < n_terms; t++)
         if (term_lengths[t] && (words[term_offsets[t]] & SA_HDR_MASK) == 0) ix->h_first0[t] = 1;
 
-#define CREATE_CUDA(call)                                                              \
-    do {                                                                               \
-        cudaError_t e_ = (call);                                                       \
-        if (e_ != cudaSuccess) {                                                       \
-            sa_set_error("%s:%d %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); \
-            sa_index_destroy(ix);                                                      \
-            return SA_ERR_CUDA;                                                        \
-        }                                                                              \
-    } while (0)
-
-    CREATE_CUDA(cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking));
-    CREATE_CUDA(cudaEventCreate(&ix->ev0));
-    CREATE_CUDA(cudaEventCreate(&ix->ev1));
-    CREATE_CUDA(cudaMalloc(&ix->d_words, (n_words + 4) * sizeof(u64)));
-    CREATE_CUDA(cudaMemsetAsync(ix->d_words + n_words, 0, 4 * sizeof(u64), ix->stream));
-    if (n_words && upload_bulk(ix->d_words, words, n_words * sizeof(u64), ix->stream, &ix->upload_mode) != SA_OK) {
-        sa_index_destroy(ix);
-        return SA_ERR_CUDA;
-    }
-    CREATE_CUDA(cudaMalloc(&ix->d_doc_lens, (n_docs + 1) * sizeof(float)));
+    // a host table in a new device buffer of exactly its size, copied on the index's stream
+    auto upload_table = [&](DevBuf &d, const auto &h) -> int {
+        const size_t bytes = h.size() * sizeof(h[0]);
+        int rc = d.allocate(bytes);
+        if (rc) return rc;
+        SA_CUDA(cudaMemcpyAsync(d.p, h.data(), bytes, cudaMemcpyHostToDevice, ix->stream));
+        return SA_OK;
+    };
+    int rc;
+    SA_CUDA(cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking));
+    SA_CUDA(cudaEventCreate(&ix->ev0));
+    SA_CUDA(cudaEventCreate(&ix->ev1));
+    if ((rc = ix->d_words.allocate((n_words + 4) * sizeof(u64)))) return rc;
+    SA_CUDA(cudaMemsetAsync(ix->d_words.as<u64>() + n_words, 0, 4 * sizeof(u64), ix->stream));
+    if (n_words && (rc = upload_bulk(ix->d_words.p, words, n_words * sizeof(u64), ix->stream, &ix->upload_mode))) return rc;
+    if ((rc = ix->d_doc_lens.allocate((n_docs + 1) * sizeof(float)))) return rc;
     if (n_docs)
-        CREATE_CUDA(cudaMemcpyAsync(ix->d_doc_lens, doc_lens, n_docs * sizeof(float), cudaMemcpyHostToDevice, ix->stream));
-    CREATE_CUDA(cudaMalloc(&ix->d_df, (size_t)(n_terms + 1) * sizeof(u32)));
-    CREATE_CUDA(cudaMemsetAsync(ix->d_df, 0, (size_t)(n_terms + 1) * sizeof(u32), ix->stream));
+        SA_CUDA(cudaMemcpyAsync(ix->d_doc_lens.p, doc_lens, n_docs * sizeof(float), cudaMemcpyHostToDevice, ix->stream));
+    if ((rc = ix->d_df.allocate((size_t)(n_terms + 1) * sizeof(u32)))) return rc;
+    SA_CUDA(cudaMemsetAsync(ix->d_df.p, 0, (size_t)(n_terms + 1) * sizeof(u32), ix->stream));
     ix->device_bytes = (n_words + 1) * sizeof(u64) + (n_docs + 1) * sizeof(float) + (size_t)(n_terms + 1) * 4;
 
     ix->doc_lens_nonneg = true;
@@ -363,13 +358,7 @@ extern "C" int sa_index_create(const uint64_t *words, uint64_t n_words,
             term_of_slot.push_back(t);
             covered += term_lengths[t];
         }
-        if (!full_cover || covered != n_words) {
-            sa_set_error("term slices must tile `words` exactly (ArrayDict.compact layout)");
-            sa_index_destroy(ix);
-            return SA_ERR_ARG;
-        }
-        u64 *d_off = nullptr;
-        u32 *d_slot = nullptr;
+        SA_CHECK(full_cover && covered == n_words, "term slices must tile `words` exactly (ArrayDict.compact layout)");
         u32 n_slots = (u32)off_sorted.size();
         // tile directories for long lists (short ones are searched: they stay cache resident)
         const u32 n_tiles = sa_n_tiles(n_docs);
@@ -385,29 +374,25 @@ extern "C" int sa_index_create(const uint64_t *words, uint64_t n_words,
                 dir_words += (u64)n_tiles + 1;
             }
         }
-        CREATE_CUDA(cudaMalloc(&d_off, n_slots * sizeof(u64)));
-        CREATE_CUDA(cudaMalloc(&d_slot, n_slots * sizeof(u32)));
-        CREATE_CUDA(cudaMemcpyAsync(d_off, off_sorted.data(), n_slots * sizeof(u64), cudaMemcpyHostToDevice, ix->stream));
-        CREATE_CUDA(cudaMemcpyAsync(d_slot, term_of_slot.data(), n_slots * sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
+        DevBuf d_off, d_slot, d_slot_len, d_slot_dir;
+        if ((rc = upload_table(d_off, off_sorted)) || (rc = upload_table(d_slot, term_of_slot))) return rc;
         unsigned blocks = (unsigned)((n_words + 255) / 256);
-        df_kernel<<<blocks, 256, 0, ix->stream>>>(ix->d_words, n_words, d_off, d_slot, n_slots, ix->d_df);
-        CREATE_CUDA(cudaGetLastError());
+        df_kernel<<<blocks, 256, 0, ix->stream>>>(ix->d_words.as<u64>(), n_words, d_off.as<u64>(), d_slot.as<u32>(), n_slots,
+                                                  ix->d_df.as<u32>());
+        SA_CUDA(cudaGetLastError());
         ix->stats.total_launches++;
-        CREATE_CUDA(cudaMemcpyAsync(ix->h_df.data(), ix->d_df, n_terms * sizeof(u32), cudaMemcpyDeviceToHost, ix->stream));
-        u64 *d_slot_len = nullptr, *d_slot_dir = nullptr;
+        SA_CUDA(cudaMemcpyAsync(ix->h_df.data(), ix->d_df.p, n_terms * sizeof(u32), cudaMemcpyDeviceToHost, ix->stream));
         if (dir_words) {
-            CREATE_CUDA(cudaMalloc(&ix->d_tile_dir, dir_words * sizeof(u32)));
+            if ((rc = ix->d_tile_dir.allocate(dir_words * sizeof(u32)))) return rc;
             ix->device_bytes += dir_words * sizeof(u32);
-            CREATE_CUDA(cudaMalloc(&d_slot_len, n_slots * sizeof(u64)));
-            CREATE_CUDA(cudaMalloc(&d_slot_dir, n_slots * sizeof(u64)));
-            CREATE_CUDA(cudaMemcpyAsync(d_slot_len, slot_len.data(), n_slots * sizeof(u64), cudaMemcpyHostToDevice, ix->stream));
-            CREATE_CUDA(cudaMemcpyAsync(d_slot_dir, slot_dir.data(), n_slots * sizeof(u64), cudaMemcpyHostToDevice, ix->stream));
-            tile_dir_kernel<<<blocks, 256, 0, ix->stream>>>(ix->d_words, n_words, d_off, d_slot_len, d_slot_dir, n_slots,
-                                                           ix->d_tile_dir, doc_base, n_tiles);
-            CREATE_CUDA(cudaGetLastError());
+            if ((rc = upload_table(d_slot_len, slot_len)) || (rc = upload_table(d_slot_dir, slot_dir))) return rc;
+            tile_dir_kernel<<<blocks, 256, 0, ix->stream>>>(ix->d_words.as<u64>(), n_words, d_off.as<u64>(),
+                                                           d_slot_len.as<u64>(), d_slot_dir.as<u64>(), n_slots,
+                                                           ix->d_tile_dir.as<u32>(), doc_base, n_tiles);
+            SA_CUDA(cudaGetLastError());
             ix->stats.total_launches++;
         }
-        CREATE_CUDA(cudaStreamSynchronize(ix->stream));         // h_df is final from here on
+        SA_CUDA(cudaStreamSynchronize(ix->stream));         // h_df is final from here on
         // tf table for the terms that have a directory (the long lists: that is where the scan's time goes)
         static const bool no_tf_table = getenv("SA_NO_TF_TABLE") && atoi(getenv("SA_NO_TF_TABLE")) != 0;
         ix->h_rec_off.assign(n_terms, SA_NO_DIR);
@@ -427,81 +412,47 @@ extern "C" int sa_index_create(const uint64_t *words, uint64_t n_words,
                 }
             }
             const u32 n_rblocks = (u32)((n_words + REC_BLOCK - 1) / REC_BLOCK);
-            u32 *d_bcount = nullptr, *d_slot_df = nullptr;
-            u64 *d_bbase = nullptr, *d_slot_rec = nullptr, *d_slot_hb = nullptr;
-            CREATE_CUDA(cudaMalloc(&ix->d_recs, (total_recs + 8) * sizeof(u32)));
-            CREATE_CUDA(cudaMemsetAsync(ix->d_recs, 0, (total_recs + 8) * sizeof(u32), ix->stream));
-            CREATE_CUDA(cudaMalloc(&ix->d_rec_dir, dir_words * sizeof(u32)));
+            DevBuf d_bcount, d_bbase, d_slot_rec, d_slot_hb, d_slot_df;
+            if ((rc = ix->d_recs.allocate((total_recs + 8) * sizeof(u32)))) return rc;
+            SA_CUDA(cudaMemsetAsync(ix->d_recs.p, 0, (total_recs + 8) * sizeof(u32), ix->stream));
+            if ((rc = ix->d_rec_dir.allocate(dir_words * sizeof(u32)))) return rc;
             ix->device_bytes += (total_recs + 8) * sizeof(u32) + dir_words * sizeof(u32);
-            CREATE_CUDA(cudaMalloc(&d_bcount, (size_t)n_rblocks * sizeof(u32)));
-            CREATE_CUDA(cudaMalloc(&d_bbase, (size_t)n_rblocks * sizeof(u64)));
-            CREATE_CUDA(cudaMalloc(&d_slot_rec, n_slots * sizeof(u64)));
-            CREATE_CUDA(cudaMalloc(&d_slot_hb, n_slots * sizeof(u64)));
-            CREATE_CUDA(cudaMalloc(&d_slot_df, n_slots * sizeof(u32)));
-            CREATE_CUDA(cudaMemcpyAsync(d_slot_rec, slot_rec.data(), n_slots * sizeof(u64), cudaMemcpyHostToDevice, ix->stream));
-            CREATE_CUDA(cudaMemcpyAsync(d_slot_hb, slot_head_base.data(), n_slots * sizeof(u64), cudaMemcpyHostToDevice, ix->stream));
-            CREATE_CUDA(cudaMemcpyAsync(d_slot_df, slot_df.data(), n_slots * sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
-            rec_count_kernel<<<n_rblocks, 256, 0, ix->stream>>>(ix->d_words, n_words, d_off, n_slots, d_bcount);
-            rec_scan_kernel<<<1, 1024, 0, ix->stream>>>(d_bcount, d_bbase, n_rblocks);
-            rec_write_kernel<<<n_rblocks, 256, 0, ix->stream>>>(ix->d_words, n_words, d_off, d_slot_len, d_slot_dir, d_slot_rec,
-                                                                d_slot_hb, d_slot_df, n_slots, d_bbase, ix->d_recs, ix->d_rec_dir,
-                                                                doc_base, n_tiles);
-            CREATE_CUDA(cudaGetLastError());
+            if ((rc = d_bcount.allocate((size_t)n_rblocks * sizeof(u32))) ||
+                (rc = d_bbase.allocate((size_t)n_rblocks * sizeof(u64))) || (rc = upload_table(d_slot_rec, slot_rec)) ||
+                (rc = upload_table(d_slot_hb, slot_head_base)) || (rc = upload_table(d_slot_df, slot_df)))
+                return rc;
+            rec_count_kernel<<<n_rblocks, 256, 0, ix->stream>>>(ix->d_words.as<u64>(), n_words, d_off.as<u64>(), n_slots,
+                                                                d_bcount.as<u32>());
+            rec_scan_kernel<<<1, 1024, 0, ix->stream>>>(d_bcount.as<u32>(), d_bbase.as<u64>(), n_rblocks);
+            rec_write_kernel<<<n_rblocks, 256, 0, ix->stream>>>(
+                ix->d_words.as<u64>(), n_words, d_off.as<u64>(), d_slot_len.as<u64>(), d_slot_dir.as<u64>(), d_slot_rec.as<u64>(),
+                d_slot_hb.as<u64>(), d_slot_df.as<u32>(), n_slots, d_bbase.as<u64>(), ix->d_recs.as<u32>(), ix->d_rec_dir.as<u32>(),
+                doc_base, n_tiles);
+            SA_CUDA(cudaGetLastError());
             ix->stats.total_launches += 3;
-            CREATE_CUDA(cudaStreamSynchronize(ix->stream));
-            cudaFree(d_bcount); cudaFree(d_bbase); cudaFree(d_slot_rec); cudaFree(d_slot_hb); cudaFree(d_slot_df);
+            SA_CUDA(cudaStreamSynchronize(ix->stream));
         }
-        cudaFree(d_off);
-        cudaFree(d_slot);
-        cudaFree(d_slot_len);
-        cudaFree(d_slot_dir);
     } else {
-        CREATE_CUDA(cudaStreamSynchronize(ix->stream));
+        SA_CUDA(cudaStreamSynchronize(ix->stream));
     }
-#undef CREATE_CUDA
-    *index_out = ix;
+    *index_out = ix.release();
     return SA_OK;
 }
 
-void sa_free_batch(sa_index *ix);
+// Order matters: the stream drains before anything it uses is freed; the members (every device buffer, the batch
+// and view states, the pinned staging) free themselves after this body, with the device still current.
+sa_index::~sa_index() {
+    cudaSetDevice(device);
+    if (stream) cudaStreamSynchronize(stream);
+    sa_comm_destroy(this);
+    for (auto &t : pending_timers) { cudaEventDestroy(t.e0); cudaEventDestroy(t.e1); }
+    for (auto e : free_events) cudaEventDestroy(e);
+    if (ev0) cudaEventDestroy(ev0);
+    if (ev1) cudaEventDestroy(ev1);
+    if (stream) cudaStreamDestroy(stream);
+}
 
 extern "C" int sa_index_destroy(sa_index *ix) {
-    if (!ix) return SA_OK;
-    cudaSetDevice(ix->device);
-    if (ix->stream) cudaStreamSynchronize(ix->stream);
-    sa_comm_destroy(ix);
-    cudaFree(ix->d_words);
-    cudaFree(ix->d_doc_lens);
-    cudaFree(ix->d_df);
-    cudaFree(ix->d_tile_dir);
-    cudaFree(ix->d_recs);
-    cudaFree(ix->d_rec_dir);
-    cudaFree(ix->d_norm);
-    cudaFree(ix->d_rows);
-    cudaFree(ix->d_row_mask);
-    ix->dense.release();
-    ix->queries.release();
-    ix->cand.release();
-    ix->cand_meta.release();
-    ix->topk_out.release();
-    ix->phrase_scratch.release();
-    ix->filt.release();
-    ix->misc.release();
-    ix->gather.release();
-    sa_free_batch(ix);
-    sa_free_view(ix);
-    if (ix->pending_timers) {
-        for (auto &t : *ix->pending_timers) { cudaEventDestroy(t.e0); cudaEventDestroy(t.e1); }
-        delete ix->pending_timers;
-    }
-    if (ix->free_events) {
-        for (auto e : *ix->free_events) cudaEventDestroy(e);
-        delete ix->free_events;
-    }
-    if (ix->h_pinned) cudaFreeHost(ix->h_pinned);
-    if (ix->ev0) cudaEventDestroy(ix->ev0);
-    if (ix->ev1) cudaEventDestroy(ix->ev1);
-    if (ix->stream) cudaStreamDestroy(ix->stream);
     delete ix;
     return SA_OK;
 }
@@ -656,7 +607,7 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
     SA_CHECK(ix && (n_queries == 0 || (terms && term_starts && idf)), "NULL argument");
     SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
     SA_CUDA(cudaSetDevice(ix->device));
-    if (!ix->batch) ix->batch = new BatchState();
+    if (!ix->batch) ix->batch.reset(new BatchState());
     BatchState &B = *ix->batch;
     B.ready = false;
     B.nq = n_queries;
@@ -851,7 +802,7 @@ int sa_batch_execute_locked(sa_index *ix) {
                 // span matches become records; one tile pass writes the rows (zeros + BM25) and collects top-k
                 float *rows = ix->dense.as<float>() + (u64)C.n_term * stride;
                 if ((rc = sa_ensure_norm(ix, B.k1, B.b, B.avg_doc_len))) return rc;
-                if ((rc = sa_span_enqueue(ix, ix->d_words, plan, B.d_sq.as<SpanQuery>() + C.phrase0,
+                if ((rc = sa_span_enqueue(ix, ix->d_words.as<u64>(), plan, B.d_sq.as<SpanQuery>() + C.phrase0,
                                           B.d_scounts.as<SpanCounts>() + C.phrase0, ix->phrase_scratch.p, rows, stride,
                                           &t, C.n_term))) return rc;
             }
@@ -897,18 +848,20 @@ static int redo_query(sa_index *ix, BatchState &B, bool is_phrase, u32 idx, u32 
     } else {
         const Bm25Params p = make_bm25(sq ? sq->idf : B.pqs[idx].idf, B.avg_doc_len, B.k1, B.b, ix->doc_lens_nonneg);
         if (sq) {
-            if ((rc = sa_span_run(ix, ix->d_words, sq->off, sq->len, sq->dir_off, sq->n_terms, sq->slop, sq->literal != 0, nullptr))) return rc;
+            if ((rc = sa_span_run(ix, ix->d_words.as<u64>(), sq->off, sq->len, sq->dir_off, sq->n_terms, sq->slop,
+                                  sq->literal != 0, nullptr))) return rc;
         } else {
             std::vector<PhraseQuery> one(1, B.pqs[idx]);
             PhraseDump nodump;
             memset(&nodump, 0, sizeof(nodump));
-            if ((rc = sa_phrase_run_sync(ix, one, ix->d_words, 0, p, nodump, false))) return rc;   // loops until the guess holds
+            // loops until the guess holds
+            if ((rc = sa_phrase_run_sync(ix, one, ix->d_words.as<u64>(), 0, p, nodump, false))) return rc;
             B.pqs[idx] = one[0];
         }
         const double idf = p.idf;
         if ((rc = ix->misc.reserve(sizeof(double)))) return rc;
         SA_CUDA(cudaMemcpyAsync(ix->misc.p, &idf, sizeof(double), cudaMemcpyHostToDevice, ix->stream));
-        if ((rc = launch_sim_tiles(ix, SA_SIM_BM25, ix->dense.as<float>(), nullptr, ix->d_doc_lens, ix->n_docs, p,
+        if ((rc = launch_sim_tiles(ix, SA_SIM_BM25, ix->dense.as<float>(), nullptr, ix->d_doc_lens.as<float>(), ix->n_docs, p,
                                    SimParams{}, ix->misc.as<double>(), 1, 0, t, nullptr))) return rc;
     }
     SA_CUDA(cudaMemcpyAsync(B.d_row_query.p, &q, sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
@@ -924,14 +877,14 @@ int sa_batch_fix_overflow_locked(sa_index *ix, u32 *n_redone) {
     if (B.nq == 0 || ix->n_docs == 0 || B.avg_doc_len == 0.0f) return SA_OK;
     int rc;
     const size_t ovf_bytes = (size_t)B.nq * sizeof(u32), st_bytes = B.pqs.size() * sizeof(PhraseStats);
-    if ((rc = sa_pinned_reserve(ix, std::max<size_t>(ovf_bytes + st_bytes, 4096)))) return rc;
-    SA_CUDA(cudaMemcpyAsync(ix->h_pinned, B.d_meta.p, ovf_bytes, cudaMemcpyDeviceToHost, ix->stream));
+    if ((rc = ix->h_pinned.reserve(std::max<size_t>(ovf_bytes + st_bytes, 4096)))) return rc;
+    SA_CUDA(cudaMemcpyAsync(ix->h_pinned.p, B.d_meta.p, ovf_bytes, cudaMemcpyDeviceToHost, ix->stream));
     if (st_bytes)
-        SA_CUDA(cudaMemcpyAsync((char *)ix->h_pinned + ovf_bytes, B.d_pstats.p, st_bytes, cudaMemcpyDeviceToHost, ix->stream));
+        SA_CUDA(cudaMemcpyAsync(ix->h_pinned.as<char>() + ovf_bytes, B.d_pstats.p, st_bytes, cudaMemcpyDeviceToHost, ix->stream));
     SA_CUDA(cudaStreamSynchronize(ix->stream));
-    std::vector<u32> ovf((const u32 *)ix->h_pinned, (const u32 *)ix->h_pinned + B.nq);       // row space
+    std::vector<u32> ovf(ix->h_pinned.as<const u32>(), ix->h_pinned.as<const u32>() + B.nq);       // row space
     std::vector<PhraseStats> st(B.pqs.size());
-    if (st_bytes) memcpy(st.data(), (char *)ix->h_pinned + ovf_bytes, st_bytes);
+    if (st_bytes) memcpy(st.data(), ix->h_pinned.as<char>() + ovf_bytes, st_bytes);
 
     struct Redo { bool phrase; u32 idx, q; const SpanQuery *sq; };
     std::vector<Redo> redo;
@@ -985,11 +938,11 @@ void sa_unpack_keys(const u64 *keys, u64 n, uint32_t *out_docs, float *out_score
 // keys + the batch's summary tail in ONE device-to-host copy and ONE synchronise
 static int download_keys(sa_index *ix, const u64 *d_keys, size_t nk, uint32_t *out_docs, float *out_scores, u64 *tail) {
     int rc;
-    if ((rc = sa_pinned_reserve(ix, (nk + SA_BATCH_TAIL) * sizeof(u64)))) return rc;
-    SA_CUDA(cudaMemcpyAsync(ix->h_pinned, d_keys, (nk + SA_BATCH_TAIL) * sizeof(u64), cudaMemcpyDeviceToHost, ix->stream));
+    if ((rc = ix->h_pinned.reserve((nk + SA_BATCH_TAIL) * sizeof(u64)))) return rc;
+    SA_CUDA(cudaMemcpyAsync(ix->h_pinned.p, d_keys, (nk + SA_BATCH_TAIL) * sizeof(u64), cudaMemcpyDeviceToHost, ix->stream));
     SA_CUDA(cudaStreamSynchronize(ix->stream));
-    sa_unpack_keys((const u64 *)ix->h_pinned, nk, out_docs, out_scores);
-    if (tail) memcpy(tail, (const u64 *)ix->h_pinned + nk, SA_BATCH_TAIL * sizeof(u64));
+    sa_unpack_keys(ix->h_pinned.as<const u64>(), nk, out_docs, out_scores);
+    if (tail) memcpy(tail, ix->h_pinned.as<const u64>() + nk, SA_BATCH_TAIL * sizeof(u64));
     return SA_OK;
 }
 
@@ -1043,11 +996,9 @@ extern "C" int sa_score_batch_topk(sa_index *ix, const uint32_t *terms, const ui
 // ------------------------------------------------------------------- timers
 KernelTimer::KernelTimer(sa_index *ix_, int kind_) : ix(ix_), kind(kind_), on(ix_->profiling) {
     if (!on) return;
-    if (!ix->pending_timers) ix->pending_timers = new std::vector<TimedLaunch>();
-    if (!ix->free_events) ix->free_events = new std::vector<cudaEvent_t>();
     auto get = [&]() {
         cudaEvent_t e = nullptr;
-        if (!ix->free_events->empty()) { e = ix->free_events->back(); ix->free_events->pop_back(); }
+        if (!ix->free_events.empty()) { e = ix->free_events.back(); ix->free_events.pop_back(); }
         else cudaEventCreate(&e);
         return e;
     };
@@ -1059,23 +1010,23 @@ KernelTimer::KernelTimer(sa_index *ix_, int kind_) : ix(ix_), kind(kind_), on(ix
 void KernelTimer::stop() {
     if (!on) return;
     cudaEventRecord(e1, ix->stream);
-    ix->pending_timers->push_back(TimedLaunch{e0, e1, kind});
+    ix->pending_timers.push_back(TimedLaunch{e0, e1, kind});
     on = false;
 }
 
 int sa_resolve_timers(sa_index *ix) {
-    if (!ix->pending_timers || ix->pending_timers->empty()) return SA_OK;
+    if (ix->pending_timers.empty()) return SA_OK;
     SA_CUDA(cudaStreamSynchronize(ix->stream));
-    for (auto &t : *ix->pending_timers) {
+    for (auto &t : ix->pending_timers) {
         float ms = 0;
         cudaEventElapsedTime(&ms, t.e0, t.e1);
         if (t.kind == 0) ix->stats.term_kernel_ms += ms;
         else if (t.kind == 1) ix->stats.topk_kernel_ms += ms;
         else ix->stats.phrase_kernel_ms += ms;
-        ix->free_events->push_back(t.e0);
-        ix->free_events->push_back(t.e1);
+        ix->free_events.push_back(t.e0);
+        ix->free_events.push_back(t.e1);
     }
-    ix->pending_timers->clear();
+    ix->pending_timers.clear();
     return SA_OK;
 }
 
@@ -1100,20 +1051,7 @@ extern "C" int sa_timer_stop(sa_index *ix, double *ms_out) {
     return SA_OK;
 }
 
-void sa_free_batch(sa_index *ix) {
-    if (!ix->batch) return;
-    ix->batch->d_tq.release();
-    ix->batch->d_pq.release();
-    ix->batch->d_row_query.release();
-    ix->batch->d_meta.release();
-    ix->batch->d_pstats.release();
-    ix->batch->d_sel.release();
-    ix->batch->d_missing.release();
-    ix->batch->d_sq.release();
-    ix->batch->d_scounts.release();
-    delete ix->batch;
-    ix->batch = nullptr;
-}
+void BatchStateDelete::operator()(BatchState *b) const { delete b; }
 
 void sa_batch_dims(sa_index *ix, u32 *nq, u32 *k) {
     *nq = ix->batch ? ix->batch->nq : 0;

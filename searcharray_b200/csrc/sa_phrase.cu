@@ -818,8 +818,8 @@ static PhraseArgs phrase_args(const sa_index *ix, const u64 *d_words, const Phra
     PhraseArgs a;
     memset(&a, 0, sizeof(a));
     a.words = d_words;
-    a.tile_dir = (d_words == ix->d_words) ? ix->d_tile_dir : nullptr;
-    a.doc_lens = ix->d_doc_lens;
+    a.tile_dir = (d_words == ix->d_words.as<u64>()) ? ix->d_tile_dir.as<u32>() : nullptr;
+    a.doc_lens = ix->d_doc_lens.as<float>();
     a.n_docs = ix->n_docs;
     a.doc_base = ix->doc_base;
     a.queries = d_pqs;
@@ -852,7 +852,7 @@ int sa_phrase_run_sync(sa_index *ix, std::vector<PhraseQuery> &pqs, const u64 *d
     u64 arena_words = 64;
     for (auto &pq : pqs) arena_words += sa_phrase_arena_words(pq, chunks.n_chunks);
     // the conjunction regime needs no bump arena
-    bool conj = allow_conj && Q == 1 && d_words == ix->d_words && !dump.cont && sa_phrase_use_conjunction(pqs[0], ix->n_docs);
+    bool conj = allow_conj && Q == 1 && d_words == ix->d_words.as<u64>() && !dump.cont && sa_phrase_use_conjunction(pqs[0], ix->n_docs);
     const u64 full_arena_words = arena_words;
     const std::vector<PhraseQuery> pqs_in = pqs;
     if (conj) arena_words = 64;
@@ -934,7 +934,7 @@ int sa_phrase_enqueue(sa_index *ix, const PhraseQuery *d_pqs, PhraseStats *d_sta
                       float *dense_rows, u64 stride, DocChunks chunks, u64 *d_arena,
                       unsigned long long *d_arena_used, u64 arena_words, int score, const Bm25Params &p,
                       const TopkCtx *topk, u32 topk_row0, const PhraseSplit *split) {
-    PhraseArgs a = phrase_args(ix, ix->d_words, d_pqs, d_stats, dense_rows, stride, chunks, d_arena, d_arena_used,
+    PhraseArgs a = phrase_args(ix, ix->d_words.as<u64>(), d_pqs, d_stats, dense_rows, stride, chunks, d_arena, d_arena_used,
                                arena_words, score, p);
     if (topk) a.topk = *topk;
     a.topk_row0 = topk_row0;
@@ -973,7 +973,7 @@ static int phrase_common(sa_index *ix, const uint32_t *term_ids, uint32_t n_term
     SA_CHECK(!(rows && score), "score on a sliced array: call termfreqs + bm25 (the Python layer does)");
     // term lists: the index's own, or filtered copies (sliced array / min-max posn), which is what
     // the reference runs on (middle_out.py:427-437: encoder.slice per term, then the same algorithm)
-    const u64 *d_lists = ix->d_words;
+    const u64 *d_lists = ix->d_words.as<u64>();
     if (!missing && (rows || use_payload)) {
         std::vector<u64> f_offs, f_lens;
         if ((rc = sa_filter_terms(ix, term_ids, n_terms, rows, min_payload, max_payload, use_payload, f_offs, f_lens))) return rc;
@@ -999,7 +999,7 @@ static int phrase_common(sa_index *ix, const uint32_t *term_ids, uint32_t n_term
     }
     if (raw_counts) {     // bm25.pyx:20-25 over every doc (tf == 0 scores +0.0 for ordinary parameters)
         unsigned blocks = (unsigned)((ix->n_docs + 255) / 256);
-        bm25_dense_kernel<<<blocks, 256, 0, ix->stream>>>(ix->dense.as<float>(), ix->d_doc_lens, ix->n_docs, p);
+        bm25_dense_kernel<<<blocks, 256, 0, ix->stream>>>(ix->dense.as<float>(), ix->d_doc_lens.as<float>(), ix->n_docs, p);
         SA_CUDA(cudaGetLastError());
         ix->stats.total_launches++;
     }
@@ -1033,50 +1033,43 @@ extern "C" int sa_op_bigram_freqs(const uint64_t *lhs, uint64_t n_lhs, const uin
     u64 max_doc = std::max(lhs[n_lhs - 1], rhs[n_rhs - 1]) >> SA_KEY_SHIFT;
     std::vector<float> dl(max_doc + 1, 1.0f);
     u64 offs[2] = {0, n_lhs}, lens[2] = {n_lhs, n_rhs};
-    sa_index *ix = nullptr;
-    int rc = sa_index_create(words.data(), words.size(), offs, lens, 2, dl.data(), max_doc + 1, 0, device, &ix);
+    sa_index *created = nullptr;
+    int rc = sa_index_create(words.data(), words.size(), offs, lens, 2, dl.data(), max_doc + 1, 0, device, &created);
     if (rc) return rc;
-    {
-        std::lock_guard<std::mutex> g(ix->mu);
-        std::vector<PhraseQuery> pqs(1);
-        PhraseQuery &pq = pqs[0];
-        memset(&pq, 0, sizeof(pq));
-        pq.n_terms = 2;
-        pq.off[0] = 0; pq.len[0] = n_lhs;
-        pq.off[1] = n_lhs; pq.len[1] = n_rhs;
-        pq.mode = cont_rhs ? SA_PHRASE_MODE_LR : SA_PHRASE_MODE_RL;
-        pq.same_guess = 0;
-        const u64 cap = 2 * std::min(n_lhs, n_rhs) + std::max(n_lhs, n_rhs) + 8;
-        DevBuf dbuf;
-        rc = dbuf.reserve((2 * cap + 2) * sizeof(u64));
-        if (!rc) {
-            PhraseDump dump;
-            dump.cont = dbuf.as<u64>();
-            dump.docs = dump.cont + cap;
-            dump.n_cont = dump.docs + cap;
-            dump.n_docs = dump.n_cont + 1;
-            cudaMemsetAsync(dump.n_cont, 0, 2 * sizeof(u64), ix->stream);
-            Bm25Params p;
-            memset(&p, 0, sizeof(p));
-            rc = sa_phrase_run_sync(ix, pqs, ix->d_words, 0, p, dump, false);
-            if (!rc) {
-                u64 n[2];
-                cudaMemcpy(n, dump.n_cont, 2 * sizeof(u64), cudaMemcpyDeviceToHost);
-                std::vector<u64> docs(n[1]);
-                cudaMemcpy(next_out, dump.cont, n[0] * sizeof(u64), cudaMemcpyDeviceToHost);
-                if (n[1]) cudaMemcpy(docs.data(), dump.docs, n[1] * sizeof(u64), cudaMemcpyDeviceToHost);
-                for (u64 i = 0; i < n[1]; i++) {
-                    ids_out[i] = docs[i] >> 32;
-                    counts_out[i] = (float)(u32)(docs[i] & 0xFFFFFFFFull);
-                }
-                *n_next_out = n[0];
-                *n_ids_out = n[1];
-            }
-        }
-        dbuf.release();
+    std::unique_ptr<sa_index> ix(created);
+    std::lock_guard<std::mutex> g(ix->mu);
+    std::vector<PhraseQuery> pqs(1);
+    PhraseQuery &pq = pqs[0];
+    memset(&pq, 0, sizeof(pq));
+    pq.n_terms = 2;
+    pq.off[0] = 0; pq.len[0] = n_lhs;
+    pq.off[1] = n_lhs; pq.len[1] = n_rhs;
+    pq.mode = cont_rhs ? SA_PHRASE_MODE_LR : SA_PHRASE_MODE_RL;
+    pq.same_guess = 0;
+    const u64 cap = 2 * std::min(n_lhs, n_rhs) + std::max(n_lhs, n_rhs) + 8;
+    DevBuf dbuf;
+    if ((rc = dbuf.reserve((2 * cap + 2) * sizeof(u64)))) return rc;
+    PhraseDump dump;
+    dump.cont = dbuf.as<u64>();
+    dump.docs = dump.cont + cap;
+    dump.n_cont = dump.docs + cap;
+    dump.n_docs = dump.n_cont + 1;
+    SA_CUDA(cudaMemsetAsync(dump.n_cont, 0, 2 * sizeof(u64), ix->stream));
+    Bm25Params p;
+    memset(&p, 0, sizeof(p));
+    if ((rc = sa_phrase_run_sync(ix.get(), pqs, ix->d_words.as<u64>(), 0, p, dump, false))) return rc;
+    u64 n[2];
+    SA_CUDA(cudaMemcpy(n, dump.n_cont, 2 * sizeof(u64), cudaMemcpyDeviceToHost));
+    std::vector<u64> docs(n[1]);
+    SA_CUDA(cudaMemcpy(next_out, dump.cont, n[0] * sizeof(u64), cudaMemcpyDeviceToHost));
+    if (n[1]) SA_CUDA(cudaMemcpy(docs.data(), dump.docs, n[1] * sizeof(u64), cudaMemcpyDeviceToHost));
+    for (u64 i = 0; i < n[1]; i++) {
+        ids_out[i] = docs[i] >> 32;
+        counts_out[i] = (float)(u32)(docs[i] & 0xFFFFFFFFull);
     }
-    sa_index_destroy(ix);
-    return rc;
+    *n_next_out = n[0];
+    *n_ids_out = n[1];
+    return SA_OK;
 }
 
 // popcount64_reduce / as_dense / bm25_score on raw arrays: the term kernel on a one-term index
@@ -1090,12 +1083,11 @@ extern "C" int sa_op_popcount64_reduce(const uint64_t *words, uint64_t n, int de
     u64 nd = max_doc - min_doc + 1;
     std::vector<float> dl(nd, 1.0f), tf(nd);
     u64 off = 0, len = n;
-    sa_index *ix = nullptr;
-    int rc = sa_index_create(words, n, &off, &len, 1, dl.data(), nd, min_doc, device, &ix);
+    sa_index *created = nullptr;
+    int rc = sa_index_create(words, n, &off, &len, 1, dl.data(), nd, min_doc, device, &created);
     if (rc) return rc;
-    rc = sa_termfreqs(ix, 0, 0, SA_ALL_BITS, tf.data());
-    sa_index_destroy(ix);
-    if (rc) return rc;
+    std::unique_ptr<sa_index> ix(created);
+    if ((rc = sa_termfreqs(ix.get(), 0, 0, SA_ALL_BITS, tf.data()))) return rc;
     // docs present in the list keep their (possibly zero) count: walk the keys on the host
     u64 m = 0, last = ~0ull;
     for (u64 i = 0; i < n; i++) {
@@ -1111,17 +1103,15 @@ extern "C" int sa_op_bm25_score(float *tf_inout, const float *doc_lens, uint64_t
     if (n == 0) return SA_OK;
     SA_CHECK(tf_inout && doc_lens, "NULL argument");
     SA_CUDA(cudaSetDevice(device));
-    float *d_tf = nullptr, *d_dl = nullptr;
-    SA_CUDA(cudaMalloc(&d_tf, n * sizeof(float)));
-    if (cudaMalloc(&d_dl, n * sizeof(float)) != cudaSuccess) { cudaFree(d_tf); sa_set_error("cudaMalloc failed"); return SA_ERR_NOMEM; }
-    cudaMemcpy(d_tf, tf_inout, n * sizeof(float), cudaMemcpyHostToDevice);
-    cudaMemcpy(d_dl, doc_lens, n * sizeof(float), cudaMemcpyHostToDevice);
-    bm25_dense_kernel<<<(unsigned)((n + 255) / 256), 256>>>(d_tf, d_dl, n, make_bm25(idf, avg_doc_len, k1, b, false));
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpy(tf_inout, d_tf, n * sizeof(float), cudaMemcpyDeviceToHost);
-    cudaFree(d_tf);
-    cudaFree(d_dl);
-    if (e != cudaSuccess) { sa_set_error("sa_op_bm25_score: %s", cudaGetErrorString(e)); return SA_ERR_CUDA; }
+    DevBuf d_tf, d_dl;
+    int rc;
+    if ((rc = d_tf.allocate(n * sizeof(float))) || (rc = d_dl.allocate(n * sizeof(float)))) return rc;
+    SA_CUDA(cudaMemcpy(d_tf.p, tf_inout, n * sizeof(float), cudaMemcpyHostToDevice));
+    SA_CUDA(cudaMemcpy(d_dl.p, doc_lens, n * sizeof(float), cudaMemcpyHostToDevice));
+    bm25_dense_kernel<<<(unsigned)((n + 255) / 256), 256>>>(d_tf.as<float>(), d_dl.as<float>(), n,
+                                                          make_bm25(idf, avg_doc_len, k1, b, false));
+    SA_CUDA(cudaGetLastError());
+    SA_CUDA(cudaMemcpy(tf_inout, d_tf.p, n * sizeof(float), cudaMemcpyDeviceToHost));
     return SA_OK;
 }
 

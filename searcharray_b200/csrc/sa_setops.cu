@@ -37,24 +37,6 @@ static thread_local uint64_t g_last_staged = 0;
 
 namespace {
 
-struct DevMem {                         // scratch for one op call
-    std::vector<void *> ptrs;
-    ~DevMem() { for (void *p : ptrs) cudaFree(p); }
-    template <typename T> T *alloc(size_t n) {
-        void *p = nullptr;
-        if (cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T) + 64) != cudaSuccess) return nullptr;
-        ptrs.push_back(p);
-        return (T *)p;
-    }
-    template <typename T> T *upload(const T *h, size_t n) {
-        T *d = alloc<T>(n + 4);                       // pad: staged copies read up to 2 words past a slice
-        if (!d) return nullptr;
-        cudaMemset(d + n, 0, 4 * sizeof(T));
-        if (n && cudaMemcpy(d, h, n * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) return nullptr;
-        return d;
-    }
-};
-
 #define SO_ALLOC_CHECK(p)                                              \
     do {                                                               \
         if (!(p)) {                                                    \

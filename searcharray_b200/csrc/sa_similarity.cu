@@ -36,29 +36,22 @@ extern "C" int sa_op_similarity(int kind, const float *term_freqs, const float *
     SA_CHECK(kind == SA_SIM_BM25_IMPACT || kind == SA_SIM_BM25_LEGACY || kind == SA_SIM_CLASSIC, "unknown similarity %d", kind);
     SA_CUDA(cudaSetDevice(device));
     const size_t out_bytes = n * (kind == SA_SIM_BM25_IMPACT ? sizeof(float) : sizeof(double));
-    float *d_tf = nullptr, *d_dl = nullptr;
-    void *d_out = nullptr;
-    cudaError_t e = cudaMalloc(&d_tf, n * sizeof(float));
-    if (e == cudaSuccess) e = cudaMalloc(&d_dl, n * sizeof(float));
-    if (e == cudaSuccess) e = cudaMalloc(&d_out, out_bytes);
-    if (e == cudaSuccess) e = cudaMemcpy(d_tf, term_freqs, n * sizeof(float), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaMemcpy(d_dl, doc_lens, n * sizeof(float), cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) {
-        SimArgs a;
-        a.tf = d_tf; a.dl = d_dl; a.n = n;
-        a.p = make_sim_params(avg_doc_len, k1, b);
-        a.idf = idf;
-        a.out = d_out;
-        const unsigned blocks = (unsigned)((n + 255) / 256);
-        if (kind == SA_SIM_BM25_IMPACT) similarity_kernel<SA_SIM_BM25_IMPACT><<<blocks, 256>>>(a);
-        else if (kind == SA_SIM_BM25_LEGACY) similarity_kernel<SA_SIM_BM25_LEGACY><<<blocks, 256>>>(a);
-        else similarity_kernel<SA_SIM_CLASSIC><<<blocks, 256>>>(a);
-        e = cudaGetLastError();
-        if (e == cudaSuccess) e = cudaMemcpy(out, d_out, out_bytes, cudaMemcpyDeviceToHost);
-    }
-    cudaFree(d_tf);
-    cudaFree(d_dl);
-    cudaFree(d_out);
-    if (e != cudaSuccess) { sa_set_error("sa_op_similarity: %s", cudaGetErrorString(e)); return SA_ERR_CUDA; }
+    DevBuf d_tf, d_dl, d_out;
+    int rc;
+    if ((rc = d_tf.allocate(n * sizeof(float))) || (rc = d_dl.allocate(n * sizeof(float))) || (rc = d_out.allocate(out_bytes)))
+        return rc;
+    SA_CUDA(cudaMemcpy(d_tf.p, term_freqs, n * sizeof(float), cudaMemcpyHostToDevice));
+    SA_CUDA(cudaMemcpy(d_dl.p, doc_lens, n * sizeof(float), cudaMemcpyHostToDevice));
+    SimArgs a;
+    a.tf = d_tf.as<float>(); a.dl = d_dl.as<float>(); a.n = n;
+    a.p = make_sim_params(avg_doc_len, k1, b);
+    a.idf = idf;
+    a.out = d_out.p;
+    const unsigned blocks = (unsigned)((n + 255) / 256);
+    if (kind == SA_SIM_BM25_IMPACT) similarity_kernel<SA_SIM_BM25_IMPACT><<<blocks, 256>>>(a);
+    else if (kind == SA_SIM_BM25_LEGACY) similarity_kernel<SA_SIM_BM25_LEGACY><<<blocks, 256>>>(a);
+    else similarity_kernel<SA_SIM_CLASSIC><<<blocks, 256>>>(a);
+    SA_CUDA(cudaGetLastError());
+    SA_CUDA(cudaMemcpy(out, d_out.p, out_bytes, cudaMemcpyDeviceToHost));
     return SA_OK;
 }

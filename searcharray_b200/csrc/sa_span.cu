@@ -946,7 +946,7 @@ int sa_span_enqueue(sa_index *ix, const u64 *d_lists, const SpanPlan &plan, cons
     SpanArgs a;
     memset(&a, 0, sizeof(a));
     a.words = d_lists;
-    a.tile_dir = (d_lists == ix->d_words) ? ix->d_tile_dir : nullptr;
+    a.tile_dir = (d_lists == ix->d_words.as<u64>()) ? ix->d_tile_dir.as<u32>() : nullptr;
     a.queries = d_qs;
     a.counts = d_counts;
     a.word_arena = (u64 *)(base + L.words);
@@ -961,7 +961,7 @@ int sa_span_enqueue(sa_index *ix, const u64 *d_lists, const SpanPlan &plan, cons
     SA_CUDA(cudaMemsetAsync(d_counts, 0, (size_t)Q * sizeof(SpanCounts), ix->stream));
     if (topk) {
         a.matches = (u64 *)(base + L.matches);
-        a.norm = ix->d_norm;
+        a.norm = ix->d_norm.as<float>();
         a.topk = *topk;
         a.topk_row0 = topk_row0;
         const DocChunks chunks = phrase_doc_chunks(ix, Q, 16);
@@ -1008,7 +1008,6 @@ int sa_span_enqueue(sa_index *ix, const u64 *d_lists, const SpanPlan &plan, cons
             span_groups_build_kernel<<<1, GEN_THREADS, 0, ix->stream>>>(a, q);
             SA_CUDA(cudaGetLastError());
             SA_CUDA(cudaStreamSynchronize(ix->stream));
-            lit.release();
             ix->stats.phrase_kernel_launches += 2;
             ix->stats.total_launches += 2;
         }
@@ -1042,7 +1041,7 @@ int sa_span_run(sa_index *ix, const u64 *d_lists, const u64 *offs, const u64 *le
     int rc;
     if ((rc = ix->dense.reserve(stride * sizeof(float)))) return rc;
     SpanPlan plan;
-    sa_span_plan_add(plan, offs, lens, dir_offs, n_terms, slop, 0.0f, literal, d_lists == ix->d_words ? ix->n_docs : 0);
+    sa_span_plan_add(plan, offs, lens, dir_offs, n_terms, slop, 0.0f, literal, d_lists == ix->d_words.as<u64>() ? ix->n_docs : 0);
     if ((rc = ix->phrase_scratch.reserve(sa_span_scratch_bytes(plan)))) return rc;
     if ((rc = ix->queries.reserve(sizeof(SpanQuery)))) return rc;
     if ((rc = ix->cand_meta.reserve(sizeof(SpanCounts)))) return rc;

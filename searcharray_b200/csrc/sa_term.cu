@@ -390,12 +390,14 @@ __global__ void norm_kernel(const float *__restrict__ dl, float *__restrict__ no
 int sa_ensure_norm(sa_index *ix, float k1, float b, float avg_doc_len) {
     if (ix->norm_valid && ix->norm_k1 == k1 && ix->norm_b == b && ix->norm_avgdl == avg_doc_len) return SA_OK;
     const u64 n_pad = sa_padded_docs(ix->n_docs);
-    if (!ix->d_norm) {
-        SA_CUDA(cudaMalloc(&ix->d_norm, std::max<u64>(n_pad, 1) * sizeof(float)));
+    if (!ix->d_norm.p) {
+        int rc = ix->d_norm.allocate(std::max<u64>(n_pad, 1) * sizeof(float));
+        if (rc) return rc;
         ix->device_bytes += n_pad * sizeof(float);
     }
     if (n_pad) {
-        norm_kernel<<<(unsigned)((n_pad + 255) / 256), 256, 0, ix->stream>>>(ix->d_doc_lens, ix->d_norm, ix->n_docs, n_pad,
+        norm_kernel<<<(unsigned)((n_pad + 255) / 256), 256, 0, ix->stream>>>(ix->d_doc_lens.as<float>(), ix->d_norm.as<float>(),
+                                                                           ix->n_docs, n_pad,
                                                                            make_bm25(0, avg_doc_len, k1, b, ix->doc_lens_nonneg));
         SA_CUDA(cudaGetLastError());
         ix->stats.total_launches++;
@@ -417,15 +419,16 @@ int launch_term_batch(sa_index *ix, const TermBatchArgs &a_in, u32 n_queries) {
         a.prefetch_tiles = (e = getenv("SA_TERM_PREFETCH_TILES")) ? (u32)atol(e) : SA_TERM_PREFETCH_TILES;
         a.quad_min_recs = std::max(a.quad_min_recs, a.staged_norm_min_recs);   // the quad path reads norms from the staged tile only
     }
-    a.tile_dir = ix->d_tile_dir;
-    a.recs = (a.words == ix->d_words) ? ix->d_recs : nullptr;     // the tf table describes the index's own lists only
-    a.rec_dir = ix->d_rec_dir;
-    a.norm = ix->d_norm;
+    a.tile_dir = ix->d_tile_dir.as<u32>();
+    // the tf table describes the index's own lists only
+    a.recs = (a.words == ix->d_words.as<u64>()) ? ix->d_recs.as<u32>() : nullptr;
+    a.rec_dir = ix->d_rec_dir.as<u32>();
+    a.norm = ix->d_norm.as<float>();
     const bool sparse_score = (a.mode == TERM_MODE_SCORE) && a.bm25.sparse_ok;
     if (sparse_score) {
         int rc = sa_ensure_norm(ix, a.bm25.k1, a.bm25.b, a.bm25.avg_doc_len);
         if (rc) return rc;
-        a.norm = ix->d_norm;
+        a.norm = ix->d_norm.as<float>();
     }
     const unsigned n_tiles = sa_n_tiles(a.n_docs);
     static const bool env_qmajor = getenv("SA_TERM_QUERY_MAJOR") && atoi(getenv("SA_TERM_QUERY_MAJOR")) != 0;

@@ -90,7 +90,6 @@ int sa_filter_terms(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, bo
 int sa_filter_terms_mask(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, const unsigned char *d_mask,
                          u64 pay_lo, u64 pay_hi, bool use_payload, std::vector<u64> &offs, std::vector<u64> &lens,
                          std::vector<u64> *df_out);
-void sa_free_view(sa_index *ix);     // sa_view.cu
 // Dense row 0 of ix->dense to the host (the selected rows only, when a row filter is installed), synchronously.
 int sa_copy_out_dense(sa_index *ix, float *out_host);
 
@@ -171,8 +170,8 @@ inline TopkCtx make_topk_ctx(void *cand, u32 n_tiles, u32 Q, u32 slots, u32 k, u
 inline TermBatchArgs make_term_args(sa_index *ix, const TermQuery *d_queries, const Bm25Params &p, const TopkCtx &t) {
     TermBatchArgs a;
     memset(&a, 0, sizeof(a));
-    a.words = ix->d_words;
-    a.doc_lens = ix->d_doc_lens;
+    a.words = ix->d_words.as<u64>();
+    a.doc_lens = ix->d_doc_lens.as<float>();
     a.n_docs = ix->n_docs;
     a.doc_base = ix->doc_base;
     a.queries = d_queries;

@@ -39,20 +39,7 @@ struct ViewState {
     DevBuf d_scores;       // double [n_queries * k]: the classic result scores
 };
 
-void sa_free_view(sa_index *ix) {
-    if (!ix->view) return;
-    ViewState &V = *ix->view;
-    V.d_dl.release();
-    V.d_tq.release();
-    V.d_idf.release();
-    V.d_row_query.release();
-    V.d_ovf.release();
-    V.d_keys.release();
-    V.d_cand_d.release();
-    V.d_scores.release();
-    delete ix->view;
-    ix->view = nullptr;
-}
+void ViewStateDelete::operator()(ViewState *v) const { delete v; }
 
 template <int KIND> using TileParams = std::conditional_t<KIND == SA_SIM_BM25, Bm25Params, SimParams>;
 
@@ -177,9 +164,9 @@ int launch_sim_tiles(sa_index *ix, int kind, const float *counts, const u64 *row
 static int launch_tiles(sa_index *ix, const SimRun &R, const double *d_idf, u32 n, u32 row0, const TopkCtx &t) {
     ViewState &V = *ix->view;
     const bool view = ix->rows_active;
-    return launch_sim_tiles(ix, R.kind, ix->dense.as<float>(), view ? ix->d_rows : nullptr,
-                            R.kind == SA_SIM_BM25 ? V.d_dl.as<float>() : ix->d_doc_lens, view ? ix->n_rows : ix->n_docs,
-                            R.bm25, R.sim, d_idf, n, row0, t, V.d_cand_d.as<u64>());
+    return launch_sim_tiles(ix, R.kind, ix->dense.as<float>(), view ? ix->d_rows() : nullptr,
+                            R.kind == SA_SIM_BM25 ? V.d_dl.as<float>() : ix->d_doc_lens.as<float>(),
+                            view ? ix->n_rows : ix->n_docs, R.bm25, R.sim, d_idf, n, row0, t, V.d_cand_d.as<u64>());
 }
 
 static int launch_select(sa_index *ix, int kind, const TopkCtx &t, u32 n_queries, const u32 *d_out_index) {
@@ -245,11 +232,11 @@ static int own_phrase_counts(sa_index *ix, const u32 *tids, u32 nt, u32 slop) {
     int rc = sa_resolve_terms(ix, tids, nt, offs, lens, dirs, &missing, &literal);
     if (rc) return rc;
     if (missing) return view_phrase_counts(ix, tids, nt, slop, true, nullptr, nullptr);    // zeros
-    if (slop > 0) return sa_span_run(ix, ix->d_words, offs, lens, dirs, nt, slop, literal, nullptr);
+    if (slop > 0) return sa_span_run(ix, ix->d_words.as<u64>(), offs, lens, dirs, nt, slop, literal, nullptr);
     std::vector<PhraseQuery> pqs(1, make_phrase_query(tids, nt, offs, lens, dirs, 0.0f, false));
     PhraseDump nodump;
     memset(&nodump, 0, sizeof(nodump));
-    return sa_phrase_run_sync(ix, pqs, ix->d_words, 0, make_bm25(0, 1, 1, 0, ix->doc_lens_nonneg), nodump, true);
+    return sa_phrase_run_sync(ix, pqs, ix->d_words.as<u64>(), 0, make_bm25(0, 1, 1, 0, ix->doc_lens_nonneg), nodump, true);
 }
 
 static bool query_missing(const sa_index *ix, const u32 *tids, u32 nt) {
@@ -275,7 +262,7 @@ static int phrase_tiles(sa_index *ix, const SimRun &R, const u32 *qs, u32 n, con
         missing.push_back(query_missing(ix, tids, nt));
         if (!missing.back()) ftids.insert(ftids.end(), tids, tids + nt);
     }
-    if (!ftids.empty() && (rc = sa_filter_terms_mask(ix, ftids.data(), (u32)ftids.size(), ix->d_row_mask, 0,
+    if (!ftids.empty() && (rc = sa_filter_terms_mask(ix, ftids.data(), (u32)ftids.size(), ix->d_row_mask(), 0,
                                                      SA_ALL_BITS, false, f_offs, f_lens, nullptr))) return rc;
     for (u32 j = 0; j < n; j++) {
         const u32 *tids = R.tids(qs[j]);
@@ -294,8 +281,8 @@ static int download(sa_index *ix, bool classic, u32 nq, u32 k, std::vector<u64> 
     ViewState &V = *ix->view;
     const size_t nk = (size_t)nq * k;
     int rc;
-    if ((rc = sa_pinned_reserve(ix, nk * (sizeof(u64) + sizeof(double)) + (size_t)nq * sizeof(u32)))) return rc;
-    u64 *h_keys = (u64 *)ix->h_pinned;
+    if ((rc = ix->h_pinned.reserve(nk * (sizeof(u64) + sizeof(double)) + (size_t)nq * sizeof(u32)))) return rc;
+    u64 *h_keys = ix->h_pinned.as<u64>();
     double *h_scores = (double *)(h_keys + nk);
     u32 *h_ovf = (u32 *)(h_scores + nk);
     SA_CUDA(cudaMemcpyAsync(h_keys, V.d_keys.p, nk * sizeof(u64), cudaMemcpyDeviceToHost, ix->stream));
@@ -339,7 +326,7 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
     // classic has no such branch
     const bool zero_avgdl = kind == SA_SIM_BM25 ? (float)avg_doc_len == 0.0f : avg_doc_len == 0.0;
     if (n_queries == 0 || n_pos == 0 || (!classic && zero_avgdl)) return SA_OK;
-    if (!ix->view) ix->view = new ViewState();
+    if (!ix->view) ix->view.reset(new ViewState());
     ViewState &V = *ix->view;
     // BM25 exactly as ops.bm25_score -> sa_op_bm25_score sets it up: float32 parameters, `1 - b` in float32
     const SimRun R{kind, make_bm25(0.0f, (float)avg_doc_len, (float)k1, (float)b, false),

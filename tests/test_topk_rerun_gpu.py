@@ -107,15 +107,11 @@ def test_edismax_tie_breaker_scores_that_share_a_float32_key():
         assert np.array_equal(scores.view(np.uint64), ws.view(np.uint64)), k
 
 
-@pytest.mark.parametrize("slop", [0, 2])
-def test_batch_phrase_rerun_scores_the_counts(slop):
-    """The thread layout of test_sim_topk_gpu's overflow test on the unsliced BM25 batch: 992 docs held by 31
-    threads of tile 0 tie at the best phrase score, 32 docs of 32 other threads score less.  More tied docs than
-    candidate slots reach the tile bound, so the phrase (slop 0) or span (slop 2) query takes the re-run, which
-    scores the raw counts in the tile pass.  Docs and score bits must be the top k of .score, also when the same
-    upload runs a second time."""
-    from searcharray_b200 import SearchArray, _lib
-    from searcharray_b200.similarity import compute_idf, default_bm25
+def phrase_overflow_array():
+    """The thread layout of test_sim_topk_gpu's overflow test: 992 docs held by 31 threads of tile 0 tie at the best
+    score of the phrase ["a", "b"] (slop 0 or 2), 32 docs of 32 other threads score less.  Returns the array and the
+    number of tied docs."""
+    from searcharray_b200 import SearchArray
     n = 10_000
     high = [4 * (t + 256 * j) + e for t in range(31) for j in range(8) for e in range(4)]
     low = [4 * t for t in range(31, 63)]
@@ -125,12 +121,24 @@ def test_batch_phrase_rerun_scores_the_counts(slop):
     host = host_index({"a": (ab, [2 * np.arange(r) for r in reps]),
                        "b": (ab, [2 * np.arange(r) + 1 for r in reps]),
                        "w": (w_docs, [np.zeros(1, dtype=np.int64)] * len(w_docs))}, np.full(n, 10.0))
-    arr = SearchArray.from_host_index(host)
+    return SearchArray.from_host_index(host), len(high)
+
+
+@pytest.mark.parametrize("slop", [0, 2])
+def test_batch_phrase_rerun_scores_the_counts(slop):
+    """The thread layout of test_sim_topk_gpu's overflow test on the unsliced BM25 batch: 992 docs held by 31
+    threads of tile 0 tie at the best phrase score, 32 docs of 32 other threads score less.  More tied docs than
+    candidate slots reach the tile bound, so the phrase (slop 0) or span (slop 2) query takes the re-run, which
+    scores the raw counts in the tile pass.  Docs and score bits must be the top k of .score, also when the same
+    upload runs a second time."""
+    from searcharray_b200 import _lib
+    from searcharray_b200.similarity import compute_idf, default_bm25
+    arr, n_high = phrase_overflow_array()
     queries = [["a", "b"], "w"]
     terms, starts, idfs = arr._topk_queries(queries, lambda dfs: compute_idf(arr.corpus_size, dfs))
     idfs = np.asarray(idfs, dtype=np.float32)
     dense = [arr.score(q, slop=slop) for q in queries]
-    assert np.count_nonzero(dense[0] == dense[0].max()) == len(high)
+    assert np.count_nonzero(dense[0] == dense[0].max()) == n_high
     L, h = _lib.lib(), arr._device().handle
     for k in (10, 32):
         with arr._shared["lock"]:
