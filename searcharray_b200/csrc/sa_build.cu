@@ -11,13 +11,15 @@
 // emits them.  The only sort needed is the STABLE sort by term id: a least-significant-digit radix sort of
 // (term id, original index) pairs -- cub::DeviceRadixSort, NVIDIA's library sort shipped with the CUDA toolkit, used
 // as a plain library primitive the way a BLAS call would be; everything around it (header / bit construction,
-// segmented OR by head flags, compaction, term slices) is this file's kernels.
+// segmented OR by head flags, compaction, term slices) is this file's kernels.  The head flags are ranked by
+// sa_scan.cuh's `scan_flags`, the same device-wide scan the set ops compact with.
 #include <cub/device/device_radix_sort.cuh>
 
 #include <algorithm>
 #include <vector>
 
 #include "sa_common.cuh"
+#include "sa_scan.cuh"
 
 namespace {
 
@@ -42,64 +44,15 @@ __global__ void word_head_kernel(const u32 *__restrict__ terms_sorted, const u32
     head[i] = h ? 1u : 0u;
 }
 
-// block-local exclusive scan of head flags + per-block totals (1024 entries per block)
-__global__ void __launch_bounds__(256)
-build_scan_kernel(const u32 *__restrict__ flags, u32 *__restrict__ offs, u64 n, u32 *__restrict__ bsum) {
-    __shared__ u32 warp_sums[8];
-    const u64 base = (u64)blockIdx.x * 1024 + (u64)threadIdx.x * 4;
-    u32 v[4], sum = 0;
-#pragma unroll
-    for (int e = 0; e < 4; e++) { v[e] = (base + e < n) ? flags[base + e] : 0u; sum += v[e]; }
-    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    u32 incl = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { u32 t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-    if (lane == 31) warp_sums[warp] = incl;
-    __syncthreads();
-    u32 wbase = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < 8; w++) { if (w < (int)warp) wbase += warp_sums[w]; total += warp_sums[w]; }
-    u32 run = wbase + incl - sum;
-#pragma unroll
-    for (int e = 0; e < 4; e++) { if (base + e < n) offs[base + e] = run; run += v[e]; }
-    if (threadIdx.x == 0) bsum[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(1024)
-build_bsum_kernel(u32 *__restrict__ bsum, u32 n_blocks, u32 *__restrict__ total_out) {
-    __shared__ u32 warp_sums[32];
-    __shared__ u32 carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (u32 b0 = 0; b0 < n_blocks; b0 += 1024) {
-        const u32 i = b0 + threadIdx.x;
-        const u32 v = i < n_blocks ? bsum[i] : 0u;
-        const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-        u32 incl = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) { u32 t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-        if (lane == 31) warp_sums[warp] = incl;
-        __syncthreads();
-        u32 wbase = 0, tot = 0;
-        for (int w = 0; w < 32; w++) { if (w < (int)warp) wbase += warp_sums[w]; tot += warp_sums[w]; }
-        const u32 c = carry;
-        if (i < n_blocks) bsum[i] = c + wbase + incl - v;
-        __syncthreads();
-        if (threadIdx.x == 0) carry = c + tot;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *total_out = carry;
-}
-
 // every head writes its word at its rank; the first word of a term records the term's slice start, and every
 // head bumps its term's length
 __global__ void word_write_kernel(const u32 *__restrict__ terms_sorted, const u32 *__restrict__ order,
                                   const u32 *__restrict__ docs, const u32 *__restrict__ posns, u64 n,
-                                  const u32 *__restrict__ head, const u32 *__restrict__ offs, const u32 *__restrict__ bsum,
+                                  const u32 *__restrict__ head, const u32 *__restrict__ offs,
                                   u64 *__restrict__ words, u64 *__restrict__ term_off, u64 *__restrict__ term_len) {
     const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n || !head[i]) return;
-    const u32 rank = offs[i] + bsum[i / 1024];
+    const u32 rank = offs[i];
     const u32 term = terms_sorted[i];
     const u32 a = order[i];
     const u32 doc = docs[a], blk = posns[a] / SA_LSB_BITS;
@@ -132,10 +85,8 @@ extern "C" int sa_op_build_index(const uint32_t *term_ids, const uint32_t *doc_i
     DevMem m;
     u32 *d_t = m.alloc<u32>(n), *d_ts = m.alloc<u32>(n), *d_i = m.alloc<u32>(n), *d_is = m.alloc<u32>(n);
     u32 *d_doc = m.alloc<u32>(n), *d_pos = m.alloc<u32>(n), *d_head = m.alloc<u32>(n), *d_offs = m.alloc<u32>(n);
-    const u32 n_blocks = (u32)((n + 1023) / 1024);
-    u32 *d_bsum = m.alloc<u32>(n_blocks + 1);
     u64 *d_words = m.alloc<u64>(n), *d_toff = m.alloc<u64>(n_terms), *d_tlen = m.alloc<u64>(n_terms);
-    if (!(d_t && d_ts && d_i && d_is && d_doc && d_pos && d_head && d_offs && d_bsum && d_words && d_toff && d_tlen)) {
+    if (!(d_t && d_ts && d_i && d_is && d_doc && d_pos && d_head && d_offs && d_words && d_toff && d_tlen)) {
         sa_set_error("device allocation failed");
         return SA_ERR_NOMEM;
     }
@@ -155,12 +106,11 @@ extern "C" int sa_op_build_index(const uint32_t *term_ids, const uint32_t *doc_i
     if (!d_tmp) { sa_set_error("device allocation failed"); return SA_ERR_NOMEM; }
     SA_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, d_t, d_ts, d_i, d_is, (int)n, 0, end_bit));
     word_head_kernel<<<blocks, 256>>>(d_ts, d_is, d_doc, d_pos, n, d_head);
-    build_scan_kernel<<<n_blocks, 256>>>(d_head, d_offs, n, d_bsum);
-    build_bsum_kernel<<<1, 1024>>>(d_bsum, n_blocks, d_bsum + n_blocks);
-    word_write_kernel<<<blocks, 256>>>(d_ts, d_is, d_doc, d_pos, n, d_head, d_offs, d_bsum, d_words, d_toff, d_tlen);
+    u64 total = 0;
+    int rc = scan_flags(m, d_head, d_offs, n, &total, 0);
+    if (rc) return rc;
+    word_write_kernel<<<blocks, 256>>>(d_ts, d_is, d_doc, d_pos, n, d_head, d_offs, d_words, d_toff, d_tlen);
     SA_CUDA(cudaGetLastError());
-    u32 total = 0;
-    SA_CUDA(cudaMemcpy(&total, d_bsum + n_blocks, sizeof(u32), cudaMemcpyDeviceToHost));
     SA_CUDA(cudaMemcpy(words_out, d_words, (size_t)total * sizeof(u64), cudaMemcpyDeviceToHost));
     if (n_terms) {
         SA_CUDA(cudaMemcpy(term_off_out, d_toff, n_terms * sizeof(u64), cudaMemcpyDeviceToHost));

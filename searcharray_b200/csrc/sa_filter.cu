@@ -10,6 +10,7 @@
 #include <algorithm>
 
 #include "sa_phrase.cuh"
+#include "sa_scan.cuh"
 #include "sa_term.cuh"
 
 struct FilterJob { u64 src_off, src_len, dst_off, chunk_off; };   // chunk_off: first entry in the chunk-count table
@@ -44,7 +45,7 @@ filter_lists_kernel(const u64 *__restrict__ words, const FilterJob *__restrict__
     const u64 base = (u64)blockIdx.x * FILT_CHUNK;
     if (base >= job.src_len) return;
     const u64 *__restrict__ src = words + job.src_off;
-    const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const unsigned tid = threadIdx.x;
     // thread t owns words base + t*ITEMS .. +ITEMS-1 (contiguous: the output order is the thread order)
     u64 w[FILT_ITEMS];
     u32 keep_bits = 0;
@@ -57,18 +58,8 @@ filter_lists_kernel(const u64 *__restrict__ words, const FilterJob *__restrict__
             if (filter_keep(w[j], row_mask, doc_base, n_docs, pay_lo, pay_hi, use_payload)) keep_bits |= 1u << j;
         }
     }
-    const u32 cnt = __popc(keep_bits);
-    u32 incl = cnt;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        u32 t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += t;
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    u32 off = incl - cnt, tot = 0;
-#pragma unroll
-    for (int wI = 0; wI < FILT_THREADS / 32; wI++) { u32 c = s_warp[wI]; if (wI < (int)warp) off += c; tot += c; }
+    u32 tot;
+    const u32 off = block_exclusive_sum<FILT_THREADS>((u32)__popc(keep_bits), s_warp, tot);
     if (!WRITE) {
         if (tid == 0) chunk_counts[job.chunk_off + blockIdx.x] = tot;
         return;
@@ -82,31 +73,9 @@ filter_lists_kernel(const u64 *__restrict__ words, const FilterJob *__restrict__
 // one CTA per list: exclusive scan of its chunk counts (in place); totals[job] = kept words
 __global__ void __launch_bounds__(FILT_THREADS)
 filter_scan_kernel(const FilterJob *__restrict__ jobs, u32 *__restrict__ chunk_counts, u32 *__restrict__ totals) {
-    __shared__ u32 s_warp[FILT_THREADS / 32];
     const FilterJob job = jobs[blockIdx.x];
-    const u32 n_chunks = (u32)((job.src_len + FILT_CHUNK - 1) / FILT_CHUNK);
-    u32 *cc = chunk_counts + job.chunk_off;
-    const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    u32 carry = 0;
-    for (u32 base = 0; base < n_chunks; base += FILT_THREADS) {
-        const u32 c = base + tid;
-        const u32 v = c < n_chunks ? cc[c] : 0u;
-        u32 incl = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            u32 t = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += t;
-        }
-        __syncthreads();
-        if (lane == 31) s_warp[warp] = incl;
-        __syncthreads();
-        u32 off = incl - v, tot = 0;
-#pragma unroll
-        for (int wI = 0; wI < FILT_THREADS / 32; wI++) { u32 x = s_warp[wI]; if (wI < (int)warp) off += x; tot += x; }
-        if (c < n_chunks) cc[c] = carry + off;
-        carry += tot;
-    }
-    if (tid == 0) totals[blockIdx.x] = carry;
+    cta_exclusive_scan<FILT_THREADS>(chunk_counts + job.chunk_off, (u32)((job.src_len + FILT_CHUNK - 1) / FILT_CHUNK),
+                                     totals + blockIdx.x);
 }
 
 __global__ void gather_rows_kernel(const float *__restrict__ dense, const u64 *__restrict__ rows, u64 n_rows,

@@ -5,6 +5,7 @@
 
 #include "sa_term.cuh"
 #include "sa_phrase.cuh"
+#include "sa_scan.cuh"
 #include "sa_sim.cuh"
 #include "sa_span.cuh"
 
@@ -102,25 +103,53 @@ static int upload_bulk(void *dst, const void *src, size_t bytes, cudaStream_t st
     return SA_OK;
 }
 
-// --------------------------------------------------------------- df at upload
+// --------------------------------------------------------------- df, tile directories and the tf table at upload
+// The upload kernels run one thread per posting word of the whole index; a word finds its term through the slots
+// (the terms' slices, sorted by offset, covering `words` exactly).
+
+// slot = last j with term_off_sorted[j] <= i   (slots cover [off, off+len) disjointly)
+__device__ __forceinline__ u32 slot_of_word(const u64 *__restrict__ term_off_sorted, u32 n_slots, u64 i) {
+    u32 lo = 0, hi = n_slots;
+    while (hi - lo > 1) {
+        u32 mid = (lo + hi) >> 1;
+        if (term_off_sorted[mid] <= i) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+// word i is a "doc head" when it starts its term's list (at `start`) or its doc id differs from its predecessor's
+__device__ __forceinline__ bool is_doc_head(const u64 *__restrict__ words, u64 i, u64 start) {
+    return i == start || (words[i] >> SA_KEY_SHIFT) != (words[i - 1] >> SA_KEY_SHIFT);
+}
+
+__device__ __forceinline__ u32 tile_of_word(u64 w, u64 doc_base) {
+    return (u32)(((w >> SA_KEY_SHIFT) - doc_base) / SA_TILE_DOCS);
+}
+
+// The directory entries that word i of the list [start, start + len) fills: dir[t] = value for the tiles after its
+// predecessor's, up to its own (from tile 0 for the list's first word), and dir[t] = end for the tiles after the list's
+// last word.  A word of the same doc as its predecessor fills no tile of the first kind.
+__device__ __forceinline__ void fill_tile_dir(u32 *__restrict__ dir, const u64 *__restrict__ words, u64 i, u64 start,
+                                              u64 len, u32 value, u32 end, u64 doc_base, u32 n_tiles) {
+    const u32 t_i = tile_of_word(words[i], doc_base);
+    const u32 t0 = i == start ? 0 : tile_of_word(words[i - 1], doc_base) + 1;
+    for (u32 t = t0; t <= t_i && t <= n_tiles; t++) dir[t] = value;
+    if (i == start + len - 1)
+        for (u32 t = t_i + 1; t <= n_tiles; t++) dir[t] = end;
+}
+
 // docfreq = number of distinct doc ids among a term's words (reference: unique(words >> 36)
-// .size, roaringish/unique.pyx:87-104 via middle_out.py:521-528).  One thread per word; a word
-// is a "doc head" when it starts its term or its doc id differs from its predecessor's.
+// .size, roaringish/unique.pyx:87-104 via middle_out.py:521-528) = its doc heads.
 __global__ void df_kernel(const u64 *__restrict__ words, u64 n_words,
                           const u64 *__restrict__ term_off_sorted, const u32 *__restrict__ term_of_slot,
                           u32 n_slots, u32 *__restrict__ df) {
     u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     const bool live = i < n_words;
-    // slot = last j with term_off_sorted[j] <= i   (slots cover [off, off+len) disjointly)
-    u32 lo = 0, hi = n_slots;
+    u32 lo = 0;
     bool head = false;
     if (live) {
-        while (hi - lo > 1) {
-            u32 mid = (lo + hi) >> 1;
-            if (term_off_sorted[mid] <= i) lo = mid; else hi = mid;
-        }
-        const u64 start = term_off_sorted[lo];
-        head = (i == start) || ((words[i] >> SA_KEY_SHIFT) != (words[i - 1] >> SA_KEY_SHIFT));
+        lo = slot_of_word(term_off_sorted, n_slots, i);
+        head = is_doc_head(words, i, term_off_sorted[lo]);
     }
     // a warp's 32 consecutive words almost always belong to one term: one atomic per (warp, term) instead of one
     // per doc head (a billion same-address atomics on a 10M-doc index)
@@ -132,50 +161,28 @@ __global__ void df_kernel(const u64 *__restrict__ words, u64 n_words,
 }
 
 // Tile directory of a long posting list: dir[j] = index (within the list) of the first word whose
-// doc falls in tile >= j, for j = 0..n_tiles.  One thread per word fills the entries it starts.
+// doc falls in tile >= j, for j = 0..n_tiles.
 __global__ void tile_dir_kernel(const u64 *__restrict__ words, u64 n_words,
                                 const u64 *__restrict__ term_off_sorted, const u64 *__restrict__ slot_len,
                                 const u64 *__restrict__ slot_dir_off, u32 n_slots,
                                 u32 *__restrict__ dir, u64 doc_base, u32 n_tiles) {
     u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_words) return;
-    u32 lo = 0, hi = n_slots;
-    while (hi - lo > 1) {
-        u32 mid = (lo + hi) >> 1;
-        if (term_off_sorted[mid] <= i) lo = mid; else hi = mid;
-    }
-    const u64 doff = slot_dir_off[lo];
+    const u32 slot = slot_of_word(term_off_sorted, n_slots, i);
+    const u64 doff = slot_dir_off[slot];
     if (doff == SA_NO_DIR) return;
-    const u64 start = term_off_sorted[lo], len = slot_len[lo];
-    const u32 local = (u32)(i - start);
-    u32 *d = dir + doff;
-    const u32 t_i = (u32)(((words[i] >> SA_KEY_SHIFT) - doc_base) / SA_TILE_DOCS);
-    if (local == 0) {
-        for (u32 t = 0; t <= t_i && t <= n_tiles; t++) d[t] = 0;
-    } else {
-        const u32 t_p = (u32)(((words[i - 1] >> SA_KEY_SHIFT) - doc_base) / SA_TILE_DOCS);
-        for (u32 t = t_p + 1; t <= t_i && t <= n_tiles; t++) d[t] = local;
-    }
-    if (local == len - 1)
-        for (u32 t = t_i + 1; t <= n_tiles; t++) d[t] = (u32)len;
+    const u64 start = term_off_sorted[slot], len = slot_len[slot];
+    fill_tile_dir(dir + doff, words, i, start, len, (u32)(i - start), (u32)len, doc_base, n_tiles);
 }
 
 // ---- tf table (see sa_index::d_recs).  Pass 1 counts the doc heads of every 1024-word block, a one-CTA scan
-// turns the counts into ranks, pass 2 writes each head's record at (term's record offset + rank within the
-// term) and fills the term's record directory like tile_dir_kernel fills the word directory.
+// (cta_scan_kernel, sa_scan.cuh) turns the counts into ranks in place, pass 2 writes each head's record at (term's
+// record offset + rank within the term) and fills the term's record directory with the heads' ranks.
 #define REC_BLOCK 1024
-__device__ __forceinline__ u32 slot_of_word(const u64 *__restrict__ term_off_sorted, u32 n_slots, u64 i) {
-    u32 lo = 0, hi = n_slots;
-    while (hi - lo > 1) {
-        u32 mid = (lo + hi) >> 1;
-        if (term_off_sorted[mid] <= i) lo = mid; else hi = mid;
-    }
-    return lo;
-}
 
 __global__ void __launch_bounds__(256)
 rec_count_kernel(const u64 *__restrict__ words, u64 n_words, const u64 *__restrict__ term_off_sorted, u32 n_slots,
-                 u32 *__restrict__ bcount) {
+                 u64 *__restrict__ bcount) {
     __shared__ u32 s_cnt;
     if (threadIdx.x == 0) s_cnt = 0;
     __syncthreads();
@@ -183,45 +190,12 @@ rec_count_kernel(const u64 *__restrict__ words, u64 n_words, const u64 *__restri
     for (int e = 0; e < REC_BLOCK / 256; e++) {
         const u64 i = (u64)blockIdx.x * REC_BLOCK + e * 256 + threadIdx.x;
         if (i >= n_words) break;
-        const u64 start = term_off_sorted[slot_of_word(term_off_sorted, n_slots, i)];
-        if (i == start || (words[i] >> SA_KEY_SHIFT) != (words[i - 1] >> SA_KEY_SHIFT)) mine++;
+        if (is_doc_head(words, i, term_off_sorted[slot_of_word(term_off_sorted, n_slots, i)])) mine++;
     }
     mine = __reduce_add_sync(0xffffffffu, mine);
     if ((threadIdx.x & 31) == 0 && mine) atomicAdd(&s_cnt, mine);
     __syncthreads();
     if (threadIdx.x == 0) bcount[blockIdx.x] = s_cnt;
-}
-
-// exclusive scan of u64-accumulated u32 counts by ONE CTA (n ~ 1e6 entries: a few hundred microseconds)
-__global__ void __launch_bounds__(1024)
-rec_scan_kernel(const u32 *__restrict__ bcount, u64 *__restrict__ bbase, u32 n) {
-    __shared__ u64 warp_sums[32];
-    __shared__ u64 carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (u32 b0 = 0; b0 < n; b0 += 1024) {
-        const u32 i = b0 + threadIdx.x;
-        const u64 v = i < n ? bcount[i] : 0;
-        const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-        u64 incl = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            u64 t = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += t;
-        }
-        if (lane == 31) warp_sums[warp] = incl;
-        __syncthreads();
-        u64 wbase = 0, tot = 0;
-        for (int w = 0; w < 32; w++) {
-            if (w < (int)warp) wbase += warp_sums[w];
-            tot += warp_sums[w];
-        }
-        const u64 c = carry;
-        if (i < n) bbase[i] = c + wbase + incl - v;
-        __syncthreads();
-        if (threadIdx.x == 0) carry = c + tot;
-        __syncthreads();
-    }
 }
 
 __global__ void __launch_bounds__(256)
@@ -231,55 +205,35 @@ rec_write_kernel(const u64 *__restrict__ words, u64 n_words, const u64 *__restri
                  const u32 *__restrict__ slot_df, u32 n_slots, const u64 *__restrict__ bbase,
                  u32 *__restrict__ recs, u32 *__restrict__ rec_dir, u64 doc_base, u32 n_tiles) {
     __shared__ u32 s_warp[8];
-    __shared__ u32 s_run;
-    if (threadIdx.x == 0) s_run = 0;
-    __syncthreads();
-    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    u32 run = 0;                                                                      // heads of the earlier rounds
     for (int e = 0; e < REC_BLOCK / 256; e++) {
         const u64 i = (u64)blockIdx.x * REC_BLOCK + e * 256 + threadIdx.x;
         bool head = false;
         u32 slot = 0;
-        u64 start = 0, w = 0;
+        u64 start = 0;
         if (i < n_words) {
             slot = slot_of_word(term_off_sorted, n_slots, i);
             start = term_off_sorted[slot];
-            w = words[i];
-            head = (i == start) || ((w >> SA_KEY_SHIFT) != (words[i - 1] >> SA_KEY_SHIFT));
+            head = is_doc_head(words, i, start);
         }
-        // rank of this head among the block's heads (block-wide exclusive scan of the head flags)
-        const unsigned m = __ballot_sync(0xffffffffu, head);
-        if (lane == 0) s_warp[warp] = __popc(m);
-        __syncthreads();
-        u32 before = s_run;
-        for (unsigned x = 0; x < warp; x++) before += s_warp[x];
-        u32 round_total = 0;
-        for (unsigned x = 0; x < 8; x++) round_total += s_warp[x];
-        const u64 g = bbase[blockIdx.x] + before + __popc(m & ((1u << lane) - 1u));   // global head rank
-        __syncthreads();
-        if (threadIdx.x == 0) s_run += round_total;
+        u32 round_total;
+        const u64 g = bbase[blockIdx.x] + run + block_exclusive_sum<256>(head ? 1u : 0u, s_warp, round_total);   // global head rank
+        run += round_total;
         if (i < n_words && slot_dir_off[slot] != SA_NO_DIR) {
             const u64 len = slot_len[slot];
-            const u64 doc = (w >> SA_KEY_SHIFT) - doc_base;
-            const u32 t_i = (u32)(doc / SA_TILE_DOCS);
-            u32 *d = rec_dir + slot_dir_off[slot];
+            const u32 rank = (u32)(g - slot_head_base[slot]);                         // within the term
             if (head) {
-                const u32 rank = (u32)(g - slot_head_base[slot]);                     // within the term
+                const u64 w = words[i];
                 u32 tf = 0;
                 for (u64 j = i; j < start + len; j++) {                                // the doc's run of words
                     const u64 w2 = words[j];
                     if ((w2 >> SA_KEY_SHIFT) != (w >> SA_KEY_SHIFT)) break;
                     tf += (u32)__popcll(w2 & SA_LSB_MASK);
                 }
+                const u64 doc = (w >> SA_KEY_SHIFT) - doc_base;
                 recs[slot_rec_off[slot] + rank] = ((u32)(doc % SA_TILE_DOCS) << SA_REC_TF_BITS) | (tf & SA_REC_TF_MASK);
-                if (i == start) {
-                    for (u32 t = 0; t <= t_i && t <= n_tiles; t++) d[t] = 0;
-                } else {
-                    const u32 t_p = (u32)(((words[i - 1] >> SA_KEY_SHIFT) - doc_base) / SA_TILE_DOCS);
-                    for (u32 t = t_p + 1; t <= t_i && t <= n_tiles; t++) d[t] = rank;
-                }
             }
-            if (i == start + len - 1)
-                for (u32 t = t_i + 1; t <= n_tiles; t++) d[t] = slot_df[slot];
+            fill_tile_dir(rec_dir + slot_dir_off[slot], words, i, start, len, rank, slot_df[slot], doc_base, n_tiles);
         }
     }
 }
@@ -412,18 +366,17 @@ extern "C" int sa_index_create(const uint64_t *words, uint64_t n_words,
                 }
             }
             const u32 n_rblocks = (u32)((n_words + REC_BLOCK - 1) / REC_BLOCK);
-            DevBuf d_bcount, d_bbase, d_slot_rec, d_slot_hb, d_slot_df;
+            DevBuf d_bbase, d_slot_rec, d_slot_hb, d_slot_df;
             if ((rc = ix->d_recs.allocate((total_recs + 8) * sizeof(u32)))) return rc;
             SA_CUDA(cudaMemsetAsync(ix->d_recs.p, 0, (total_recs + 8) * sizeof(u32), ix->stream));
             if ((rc = ix->d_rec_dir.allocate(dir_words * sizeof(u32)))) return rc;
             ix->device_bytes += (total_recs + 8) * sizeof(u32) + dir_words * sizeof(u32);
-            if ((rc = d_bcount.allocate((size_t)n_rblocks * sizeof(u32))) ||
-                (rc = d_bbase.allocate((size_t)n_rblocks * sizeof(u64))) || (rc = upload_table(d_slot_rec, slot_rec)) ||
+            if ((rc = d_bbase.allocate((size_t)(n_rblocks + 1) * sizeof(u64))) || (rc = upload_table(d_slot_rec, slot_rec)) ||
                 (rc = upload_table(d_slot_hb, slot_head_base)) || (rc = upload_table(d_slot_df, slot_df)))
                 return rc;
             rec_count_kernel<<<n_rblocks, 256, 0, ix->stream>>>(ix->d_words.as<u64>(), n_words, d_off.as<u64>(), n_slots,
-                                                                d_bcount.as<u32>());
-            rec_scan_kernel<<<1, 1024, 0, ix->stream>>>(d_bcount.as<u32>(), d_bbase.as<u64>(), n_rblocks);
+                                                                d_bbase.as<u64>());
+            cta_scan_kernel<1024><<<1, 1024, 0, ix->stream>>>(d_bbase.as<u64>(), n_rblocks, d_bbase.as<u64>() + n_rblocks);
             rec_write_kernel<<<n_rblocks, 256, 0, ix->stream>>>(
                 ix->d_words.as<u64>(), n_words, d_off.as<u64>(), d_slot_len.as<u64>(), d_slot_dir.as<u64>(), d_slot_rec.as<u64>(),
                 d_slot_hb.as<u64>(), d_slot_df.as<u32>(), n_slots, d_bbase.as<u64>(), ix->d_recs.as<u32>(), ix->d_rec_dir.as<u32>(),

@@ -26,6 +26,7 @@
 #include <algorithm>
 
 #include "sa_phrase.cuh"
+#include "sa_scan.cuh"
 #include "sa_span.cuh"
 #include "sa_term.cuh"
 
@@ -177,29 +178,6 @@ struct StepShared {
     u64 n_cont, n_docs;
 };
 
-// exclusive block scan (all PT threads call); returns the exclusive prefix, `total` = block sum
-__device__ __forceinline__ u32 block_excl_scan(u32 v, u32 *warp_sums, u32 &total) {
-    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    u32 incl = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        u32 t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += t;
-    }
-    __syncthreads();                 // protect warp_sums from the previous use
-    if (lane == 31) warp_sums[warp] = incl;
-    __syncthreads();
-    u32 base = 0, tot = 0;
-#pragma unroll
-    for (int w = 0; w < PT / 32; w++) {
-        u32 s = warp_sums[w];
-        if (w < (int)warp) base += s;
-        tot += s;
-    }
-    total = tot;
-    return base + incl - v;
-}
-
 // One bigram step over this CTA's chunk.  Writes the continuation list (sorted) to cont_out and
 // the per-doc counts (doc << 32 | count, sorted by doc, zero counts kept) to docs_out.
 template <bool CONT_RHS, bool DRIVER_LHS>
@@ -231,13 +209,13 @@ __device__ void bigram_step(const u64 *__restrict__ D, u64 nD, const u64 *__rest
         }
         // continuation words, in order
         u32 total;
-        u32 off = block_excl_scan(e.n_emit, S.warp_sums, total);
+        u32 off = block_exclusive_sum<PT>(e.n_emit, S.warp_sums, total);
         const u64 cbase = S.n_cont;
         if (e.n_emit >= 1) cont_out[cbase + off] = e.w0;
         if (e.n_emit == 2) cont_out[cbase + off + 1] = e.w1;
         // (doc, count) entries of this tile, compacted into shared memory
         u32 etotal;
-        u32 eoff = block_excl_scan(e.entry ? 1u : 0u, S.warp_sums, etotal);
+        u32 eoff = block_exclusive_sum<PT>(e.entry ? 1u : 0u, S.warp_sums, etotal);
         if (e.entry) {
             S.edoc[eoff] = e.doc;
             S.ecnt[eoff] = e.cnt;
@@ -264,7 +242,7 @@ __device__ void bigram_step(const u64 *__restrict__ D, u64 nD, const u64 *__rest
                 }
             }
             u32 htotal;
-            u32 hoff = block_excl_scan(emit ? 1u : 0u, S.warp_sums, htotal);
+            u32 hoff = block_exclusive_sum<PT>(emit ? 1u : 0u, S.warp_sums, htotal);
             const u64 obase = dbase + (flush ? 1 : 0);
             if (emit) docs_out[obase + hoff] = ((u64)doc << 32) | sum;
             if (tid == 0 && flush) docs_out[dbase] = ((u64)c_doc << 32) | c_cnt;

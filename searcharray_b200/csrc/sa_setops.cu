@@ -18,13 +18,15 @@
 //     tile (|lhs| << |rhs|) staging would read words nobody needs, so the CTA searches global memory instead;
 //   * merges are rank computations (merge-path: an element's output slot is its own index plus its rank in
 //     the other list); grouped sums are head flags + a scan + integer atomics (deterministic);
-//   * everything that compacts goes through one flags -> exclusive scan -> ordered write pipeline.
+//   * everything that compacts goes through one flags -> exclusive scan -> ordered write pipeline; the scan is
+//     sa_scan.cuh's device-wide `scan_flags`.
 // Host in, host out: these exports exist for kernel-level parity tests; the scoring path proper keeps its
 // data in HBM.
 #include <algorithm>
 #include <vector>
 
 #include "sa_common.cuh"
+#include "sa_scan.cuh"
 #include "sa_tma.cuh"
 
 #define SO_THREADS 256
@@ -35,8 +37,6 @@
 
 static thread_local uint64_t g_last_staged = 0;
 
-namespace {
-
 #define SO_ALLOC_CHECK(p)                                              \
     do {                                                               \
         if (!(p)) {                                                    \
@@ -45,7 +45,7 @@ namespace {
         }                                                              \
     } while (0)
 
-// ------------------------------------------------------------------ exclusive scan of u32 flags
+// ------------------------------------------------------------------ exclusive scan of u32 flags (sa_scan.cuh)
 __global__ void __launch_bounds__(SO_THREADS)
 scan_block_kernel(const u32 *__restrict__ flags, u32 *__restrict__ offs, u64 n, u32 *__restrict__ bsum) {
     __shared__ u32 warp_sums[SO_THREADS / 32];
@@ -56,22 +56,8 @@ scan_block_kernel(const u32 *__restrict__ flags, u32 *__restrict__ offs, u64 n, 
         v[e] = (base + e < n) ? flags[base + e] : 0u;
         sum += v[e];
     }
-    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    u32 incl = sum;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        u32 t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += t;
-    }
-    if (lane == 31) warp_sums[warp] = incl;
-    __syncthreads();
-    u32 wbase = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < SO_THREADS / 32; w++) {
-        if (w < (int)warp) wbase += warp_sums[w];
-        total += warp_sums[w];
-    }
-    u32 run = wbase + incl - sum;
+    u32 total;
+    u32 run = block_exclusive_sum<SO_THREADS>(sum, warp_sums, total);
 #pragma unroll
     for (int e = 0; e < SO_ITEMS; e++) {
         if (base + e < n) offs[base + e] = run;
@@ -80,60 +66,31 @@ scan_block_kernel(const u32 *__restrict__ flags, u32 *__restrict__ offs, u64 n, 
     if (threadIdx.x == 0) bsum[blockIdx.x] = total;
 }
 
-__global__ void __launch_bounds__(1024)
-scan_bsums_kernel(u32 *__restrict__ bsum, u32 n_blocks, u32 *__restrict__ total_out) {
-    __shared__ u32 warp_sums[32];
-    __shared__ u32 carry;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (u32 b0 = 0; b0 < n_blocks; b0 += 1024) {
-        const u32 i = b0 + threadIdx.x;
-        const u32 v = i < n_blocks ? bsum[i] : 0u;
-        const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-        u32 incl = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            u32 t = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += t;
-        }
-        if (lane == 31) warp_sums[warp] = incl;
-        __syncthreads();
-        u32 wbase = 0, tot = 0;
-        for (int w = 0; w < 32; w++) {
-            if (w < (int)warp) wbase += warp_sums[w];
-            tot += warp_sums[w];
-        }
-        const u32 c = carry;
-        if (i < n_blocks) bsum[i] = c + wbase + incl - v;
-        __syncthreads();
-        if (threadIdx.x == 0) carry = c + tot;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *total_out = carry;
-}
-
 __global__ void add_bsums_kernel(u32 *__restrict__ offs, u64 n, const u32 *__restrict__ bsum) {
     const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) offs[i] += bsum[i / SO_TILE];
 }
 
 // offs[i] = number of set flags before i; *total = number of set flags
-int scan_flags(DevMem &m, const u32 *d_flags, u32 *d_offs, u64 n, u64 *total) {
+int scan_flags(DevMem &m, const u32 *d_flags, u32 *d_offs, u64 n, u64 *total, cudaStream_t stream) {
     *total = 0;
     if (n == 0) return SA_OK;
     SA_CHECK(n < (1ull << 32), "array too long for the per-op exports");
     const u32 n_blocks = (u32)((n + SO_TILE - 1) / SO_TILE);
     u32 *d_bsum = m.alloc<u32>(n_blocks + 1);
     SO_ALLOC_CHECK(d_bsum);
-    scan_block_kernel<<<n_blocks, SO_THREADS>>>(d_flags, d_offs, n, d_bsum);
-    scan_bsums_kernel<<<1, 1024>>>(d_bsum, n_blocks, d_bsum + n_blocks);
-    add_bsums_kernel<<<(unsigned)((n + 255) / 256), 256>>>(d_offs, n, d_bsum);
+    scan_block_kernel<<<n_blocks, SO_THREADS, 0, stream>>>(d_flags, d_offs, n, d_bsum);
+    cta_scan_kernel<1024><<<1, 1024, 0, stream>>>(d_bsum, n_blocks, d_bsum + n_blocks);
+    add_bsums_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(d_offs, n, d_bsum);
     SA_CUDA(cudaGetLastError());
     u32 t = 0;
-    SA_CUDA(cudaMemcpy(&t, d_bsum + n_blocks, sizeof(u32), cudaMemcpyDeviceToHost));
+    SA_CUDA(cudaMemcpyAsync(&t, d_bsum + n_blocks, sizeof(u32), cudaMemcpyDeviceToHost, stream));
+    SA_CUDA(cudaStreamSynchronize(stream));
     *total = t;
     return SA_OK;
 }
+
+namespace {
 
 // ------------------------------------------------------------------ the intersect kernel
 // warp-cooperative lower bound on masked values: first i in [lo, hi) with (a[i] & mask) >= key
@@ -277,7 +234,7 @@ int run_partner(DevMem &m, const u64 *d_lhs, u64 nl, const u64 *d_rhs, u64 nr, u
     pair_flag_kernel<<<blocks, 256>>>(d_pos, d_first, nl, need_first, d_flag);
     SA_CUDA(cudaGetLastError());
     u64 total = 0;
-    int rc = scan_flags(m, d_flag, d_offs, nl, &total);
+    int rc = scan_flags(m, d_flag, d_offs, nl, &total, 0);
     if (rc) return rc;
     if (total) {
         u64 *d_oi = m.alloc<u64>(total), *d_op = h_partner ? m.alloc<u64>(total) : nullptr;
@@ -486,7 +443,7 @@ static int merge_common(const u64 *lhs, u64 nl, const u64 *rhs, u64 nr, int drop
         kept_before = m.alloc<u32>(nr + 1);
         SO_ALLOC_CHECK(keep_r && kept_before);
         invert_kernel<<<blocks_for(nr), 256>>>(hit_r, keep_r, nr);
-        int rc = scan_flags(m, keep_r, kept_before, nr, &kept);
+        int rc = scan_flags(m, keep_r, kept_before, nr, &kept, 0);
         if (rc) return rc;
         const u32 k32 = (u32)kept;
         SA_CUDA(cudaMemcpy(kept_before + nr, &k32, sizeof(u32), cudaMemcpyHostToDevice));
@@ -534,7 +491,7 @@ extern "C" int sa_op_unique(const uint64_t *arr, uint64_t n, uint64_t rshift, in
     SO_ALLOC_CHECK(d_a && flag && offs);
     head_flag_kernel<<<blocks_for(n), 256>>>(d_a, n, rshift, flag);
     u64 total = 0;
-    int rc = scan_flags(m, flag, offs, n, &total);
+    int rc = scan_flags(m, flag, offs, n, &total, 0);
     if (rc) return rc;
     u64 *d_out = m.alloc<u64>(total);
     SO_ALLOC_CHECK(d_out);
@@ -569,7 +526,7 @@ static int grouped(const u64 *ids, const u64 *val, u64 n, int popcount, int devi
     SO_ALLOC_CHECK(d_i && d_v && flag && offs);
     head_flag_kernel<<<blocks_for(n), 256>>>(d_i, n, 0, flag);
     u64 total = 0;
-    int rc = scan_flags(m, flag, offs, n, &total);
+    int rc = scan_flags(m, flag, offs, n, &total, 0);
     if (rc) return rc;
     u64 *d_io = m.alloc<u64>(total);
     unsigned long long *d_s = m.alloc<unsigned long long>(total);
@@ -609,7 +566,7 @@ extern "C" int sa_op_payload_slice(const uint64_t *arr, uint64_t n, uint64_t msb
     SO_ALLOC_CHECK(d_a && flag && offs);
     payload_flag_kernel<<<blocks_for(n), 256>>>(d_a, n, msb_mask, min_payload, max_payload, flag);
     u64 total = 0;
-    int rc = scan_flags(m, flag, offs, n, &total);
+    int rc = scan_flags(m, flag, offs, n, &total, 0);
     if (rc) return rc;
     u64 *d_out = m.alloc<u64>(total);
     SO_ALLOC_CHECK(d_out);

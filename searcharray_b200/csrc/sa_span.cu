@@ -29,6 +29,7 @@
 #include <algorithm>
 
 #include "sa_phrase.cuh"
+#include "sa_scan.cuh"
 #include "sa_span.cuh"
 #include "sa_term.cuh"
 
@@ -84,28 +85,6 @@ __device__ __forceinline__ u32 lb_hdr(const u64 *__restrict__ a, u64 len, const 
         if ((__ldg(a + mid) & SA_HDR_MASK) < target) lo = mid + 1; else hi = mid;
     }
     return (u32)lo;
-}
-
-__device__ __forceinline__ u32 block_scan_excl(u32 v, u32 *warp_sums, u32 &total) {
-    const unsigned lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    u32 incl = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        u32 t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += t;
-    }
-    __syncthreads();
-    if (lane == 31) warp_sums[warp] = incl;
-    __syncthreads();
-    u32 base = 0, tot = 0;
-#pragma unroll
-    for (int w = 0; w < GEN_THREADS / 32; w++) {
-        u32 s = warp_sums[w];
-        if (w < (int)warp) base += s;
-        tot += s;
-    }
-    total = tot;
-    return base + incl - v;
 }
 
 // exclusive running maximum (0 = nothing before); `total` = maximum over the block
@@ -273,7 +252,7 @@ span_presence_kernel(const SpanArgs a) {
             prev_p1 = doc_p1;
         }
         u32 total;
-        const u32 off = block_scan_excl(cnt | ((u32)__popc(start5) << 16), s_warp, total);
+        const u32 off = block_exclusive_sum<GEN_THREADS>(cnt | ((u32)__popc(start5) << 16), s_warp, total);
         if (tid == 0) s_first = 0;
         __syncthreads();
         if (cnt && (off & 0xFFFFu) == 0) s_first = first_p1;            // the CTA's first kept word
@@ -312,8 +291,8 @@ span_scan_kernel(const SpanArgs a) {
             u32 blk_last, tot_w, tot_g;
             const u32 prev_last = max(block_scan_excl_max(r.last_p1, s_warp, blk_last), carry_last);
             const u32 adj = (r.count && r.first_p1 == prev_last) ? 1u : 0u;
-            const u32 w_off = block_scan_excl(r.count, s_warp, tot_w) + carry_w;
-            const u32 g_off = block_scan_excl(r.starts - adj, s_warp, tot_g) + carry_g;
+            const u32 w_off = block_exclusive_sum<GEN_THREADS>(r.count, s_warp, tot_w) + carry_w;
+            const u32 g_off = block_exclusive_sum<GEN_THREADS>(r.starts - adj, s_warp, tot_g) + carry_g;
             if (c < sq.n_ctas) {
                 r.count = w_off; r.starts = g_off; r.first_p1 = adj;
                 recs[c] = r;
@@ -385,7 +364,7 @@ span_groups_build_kernel(const SpanArgs a, u32 q) {
             bool start = false;
             if (i < cnt) start = (i == 0) || ((sl[i] >> SA_KEY_SHIFT) != (sl[i - 1] >> SA_KEY_SHIFT));
             u32 total;
-            u32 off = block_scan_excl(start ? 1u : 0u, s_warp, total);
+            u32 off = block_exclusive_sum<GEN_THREADS>(start ? 1u : 0u, s_warp, total);
             const u32 g0 = s_groups;
             if (start) a.group_arena[sq.g_off[t] + g0 + off] = i;
             __syncthreads();
