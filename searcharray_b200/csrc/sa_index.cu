@@ -518,19 +518,20 @@ extern "C" int sa_score_term(sa_index *ix, uint32_t term_id, float idf, float av
 
 // ------------------------------------------------ batched, HBM-resident top-k
 // A prepared batch: query descriptors live in HBM; sa_batch_execute only enqueues kernels.
-// Queries are processed in chunks (bounded dense-vector memory).  Inside a chunk the term queries
+// Queries are processed in the chunks of sa_plan_rows (bounded dense-vector memory).  Inside a chunk the term queries
 // take dense rows [0, nT) (one fused launch) and the phrase queries rows [nT, nT + nP) (phrase
 // kernel + tile scan); one select launch covers the chunk and writes each result at its
 // original query index.
 struct BatchChunk {
     u32 row0 = 0;          // first row (in the permuted "row space") of this chunk
     u32 n_term = 0, n_phrase = 0;
-    u32 term0 = 0, phrase0 = 0;     // offsets into the batch-wide TermQuery / PhraseQuery arrays
+    u32 term0 = 0, phrase0 = 0;     // offsets into the batch-wide TermQuery / PhraseQuery (slop > 0: SpanQuery) arrays
     Bm25Params params;
     DocChunks phrase_chunks{};      // doc ranges of every phrase query
     u64 arena_words = 64;
     // phrase queries by regime (indices relative to phrase0, stored at B.d_sel + sel0: search first, then conjunction)
     u32 sel0 = 0, n_search = 0, n_conj = 0;
+    SpanPlan span;                  // slop > 0: the chunk's multi-term queries as span queries
 };
 
 struct BatchState {
@@ -543,9 +544,7 @@ struct BatchState {
     std::vector<u32> term_query, phrase_query;  // index in tqs / pqs -> original query index
     std::vector<u32> phrase_missing;          // 1 = a term is unknown: result stays empty
     std::vector<BatchChunk> chunks;
-    // slop > 0: the multi-term queries are span queries (one plan per chunk, descriptors concatenated)
-    std::vector<SpanPlan> span_plans;
-    DevBuf d_sq, d_scounts;
+    DevBuf d_sq, d_scounts;                   // slop > 0: every chunk's span descriptors, concatenated, and counts
     DevBuf d_tq, d_pq, d_row_query;
     DevBuf d_meta;                            // u32 overflow[nq] (row space)
     DevBuf d_pstats;                          // PhraseStats[#phrase queries]
@@ -570,65 +569,60 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
     B.k1 = k1;
     B.b = b;
     B.slop = slop;
-    B.span_plans.clear();
     B.tqs.clear(); B.pqs.clear(); B.row_query.clear(); B.term_query.clear(); B.phrase_query.clear();
     B.phrase_missing.clear(); B.chunks.clear(); B.sel.clear();
     int rc;
     if ((rc = ix->topk_out.reserve(std::max<size_t>(((size_t)n_queries * k + SA_BATCH_TAIL) * sizeof(u64), 256)))) return rc;
     if (n_queries == 0) { B.ready = true; return SA_OK; }
+    for (u32 q = 0; q < n_queries; q++) {
+        const u32 nt = term_starts[q + 1] - term_starts[q];
+        SA_CHECK(nt >= 1 && nt <= SA_MAX_PHRASE_TERMS, "query %u: bad number of terms", q);
+        if ((rc = sa_check_term_ids(ix, terms + term_starts[q], nt))) return rc;
+    }
+    RowPlan plan = sa_plan_rows(ix->n_docs, term_starts, n_queries);
     const u64 stride = sa_padded_docs(std::max<u64>(ix->n_docs, 1));
-    // chunk so the dense score vectors of one chunk stay within ~4 GB of HBM
-    u32 chunk = (u32)std::max<u64>(1, std::min<u64>(n_queries, (4ull << 30) / (stride * sizeof(float))));
-    B.chunk = std::min<u32>(chunk, 65535);
+    B.chunk = plan.chunk;
+    B.row_query = std::move(plan.row_query);
     u64 max_arena = 64;
     size_t max_span_scratch = 0;
     u32 n_span = 0;
-    for (u32 q0 = 0; q0 < n_queries; q0 += B.chunk) {
-        const u32 q1 = std::min(n_queries, q0 + B.chunk);
+    for (const RowChunk &R : plan.chunks) {
         BatchChunk C;
-        C.row0 = (u32)B.row_query.size();
+        C.row0 = R.row0;
+        C.n_term = R.n_term;
+        C.n_phrase = R.n_phrase;
         C.term0 = (u32)B.tqs.size();
-        C.phrase0 = (u32)B.pqs.size();
+        C.phrase0 = slop > 0 ? n_span : (u32)B.pqs.size();
         C.params = make_bm25(1.0f, avg_doc_len, k1, b, ix->doc_lens_nonneg);
-        SpanPlan plan;
-        for (int pass = 0; pass < 2; pass++) {               // term queries first, then phrases
-            for (u32 q = q0; q < q1; q++) {
-                const u32 nt = term_starts[q + 1] - term_starts[q];
-                SA_CHECK(nt >= 1 && nt <= SA_MAX_PHRASE_TERMS, "query %u: bad number of terms", q);
-                const u32 *tids = terms + term_starts[q];
-                u64 offs[SA_MAX_PHRASE_TERMS], lens[SA_MAX_PHRASE_TERMS], dirs[SA_MAX_PHRASE_TERMS];
-                bool missing, literal;
-                if ((rc = sa_resolve_terms(ix, tids, nt, offs, lens, dirs, &missing, &literal))) return rc;
-                if ((nt == 1) != (pass == 0)) continue;
-                if (!make_bm25(idf[q], avg_doc_len, k1, b, ix->doc_lens_nonneg).sparse_ok) C.params.sparse_ok = 0;
-                B.row_query.push_back(q);
-                if (nt == 1) {
-                    B.tqs.push_back(make_term_query(ix, tids[0], idf[q]));
-                    B.term_query.push_back(q);
-                } else if (slop > 0) {
-                    // phrase with slop: span search (spans.py:171-187) on the index's own lists
-                    sa_span_plan_add(plan, offs, lens, dirs, nt, slop, idf[q], literal, missing ? 0 : ix->n_docs);
-                    B.phrase_query.push_back(q);
-                } else {
-                    PhraseQuery pq = make_phrase_query(tids, nt, offs, lens, dirs, idf[q], missing);
-                    pq.use_conj = !missing && sa_phrase_use_conjunction(pq, ix->n_docs);
-                    B.pqs.push_back(pq);
-                    B.phrase_query.push_back(q);
-                    B.phrase_missing.push_back(missing);
-                }
+        for (u32 r = R.row0; r < R.row0 + R.n_term + R.n_phrase; r++) {
+            const u32 q = B.row_query[r];
+            const u32 nt = term_starts[q + 1] - term_starts[q];
+            const u32 *tids = terms + term_starts[q];
+            u64 offs[SA_MAX_PHRASE_TERMS], lens[SA_MAX_PHRASE_TERMS], dirs[SA_MAX_PHRASE_TERMS];
+            bool missing, literal;
+            if ((rc = sa_resolve_terms(ix, tids, nt, offs, lens, dirs, &missing, &literal))) return rc;
+            if (!make_bm25(idf[q], avg_doc_len, k1, b, ix->doc_lens_nonneg).sparse_ok) C.params.sparse_ok = 0;
+            if (nt == 1) {
+                B.tqs.push_back(make_term_query(ix, tids[0], idf[q]));
+                B.term_query.push_back(q);
+            } else if (slop > 0) {
+                // phrase with slop: span search (spans.py:171-187) on the index's own lists
+                sa_span_plan_add(C.span, offs, lens, dirs, nt, slop, idf[q], literal, missing ? 0 : ix->n_docs);
+                B.phrase_query.push_back(q);
+            } else {
+                PhraseQuery pq = make_phrase_query(tids, nt, offs, lens, dirs, idf[q], missing);
+                pq.use_conj = !missing && sa_phrase_use_conjunction(pq, ix->n_docs);
+                B.pqs.push_back(pq);
+                B.phrase_query.push_back(q);
+                B.phrase_missing.push_back(missing);
             }
         }
-        C.n_term = (u32)B.tqs.size() - C.term0;
         if (slop > 0) {
-            C.phrase0 = n_span;
-            C.n_phrase = (u32)plan.qs.size();
             n_span += C.n_phrase;
-            max_span_scratch = std::max(max_span_scratch, sa_span_scratch_bytes(plan));
-            B.span_plans.push_back(std::move(plan));
-            B.chunks.push_back(C);
+            max_span_scratch = std::max(max_span_scratch, sa_span_scratch_bytes(C.span));
+            B.chunks.push_back(std::move(C));
             continue;
         }
-        C.n_phrase = (u32)B.pqs.size() - C.phrase0;
         if (C.n_phrase) {
             C.sel0 = (u32)B.sel.size();
             for (u32 i = 0; i < C.n_phrase; i++) if (!B.pqs[C.phrase0 + i].use_conj) B.sel.push_back(i);
@@ -641,7 +635,7 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
                     C.arena_words += sa_phrase_arena_words(B.pqs[C.phrase0 + i], C.phrase_chunks.n_chunks);
             max_arena = std::max(max_arena, C.arena_words);
         }
-        B.chunks.push_back(C);
+        B.chunks.push_back(std::move(C));
     }
     SA_CHECK(B.chunks.empty() || B.chunks[0].params.sparse_ok || (B.pqs.empty() && n_span == 0),
              "phrase queries in a batch need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite idf)");
@@ -659,12 +653,10 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
         if ((rc = ix->phrase_scratch.reserve(max_span_scratch))) return rc;
         if ((rc = B.d_sq.reserve((size_t)n_span * sizeof(SpanQuery)))) return rc;
         if ((rc = B.d_scounts.reserve((size_t)n_span * sizeof(SpanCounts)))) return rc;
-        u32 at = 0;
-        for (const SpanPlan &pl : B.span_plans) {
-            if (pl.qs.empty()) continue;
-            SA_CUDA(cudaMemcpyAsync(B.d_sq.as<SpanQuery>() + at, pl.qs.data(), pl.qs.size() * sizeof(SpanQuery),
+        for (const BatchChunk &C : B.chunks) {
+            if (C.span.qs.empty()) continue;
+            SA_CUDA(cudaMemcpyAsync(B.d_sq.as<SpanQuery>() + C.phrase0, C.span.qs.data(), C.span.qs.size() * sizeof(SpanQuery),
                                     cudaMemcpyHostToDevice, ix->stream));
-            at += (u32)pl.qs.size();
         }
         SA_CUDA(cudaStreamSynchronize(ix->stream));      // the plans' host vectors may be reallocated later
     }
@@ -741,7 +733,6 @@ int sa_batch_execute_locked(sa_index *ix) {
     if (!B.pqs.empty())
         SA_CUDA(cudaMemsetAsync(B.d_pstats.p, 0, B.pqs.size() * sizeof(PhraseStats), ix->stream));
     int rc;
-    size_t chunk_i = 0;
     for (const BatchChunk &C : B.chunks) {
         const u32 Q = C.n_term + C.n_phrase;
         TopkCtx t = make_topk_ctx(ix->cand.p, sa_n_tiles(ix->n_docs), Q, B.slots, B.k, d_ovf + C.row0);
@@ -750,12 +741,11 @@ int sa_batch_execute_locked(sa_index *ix) {
             if ((rc = launch_term_batch(ix, a, C.n_term))) return rc;
         }
         if (B.slop > 0) {
-            const SpanPlan &plan = B.span_plans[chunk_i++];
             if (C.n_phrase) {
                 // span matches become records; one tile pass writes the rows (zeros + BM25) and collects top-k
                 float *rows = ix->dense.as<float>() + (u64)C.n_term * stride;
                 if ((rc = sa_ensure_norm(ix, B.k1, B.b, B.avg_doc_len))) return rc;
-                if ((rc = sa_span_enqueue(ix, ix->d_words.as<u64>(), plan, B.d_sq.as<SpanQuery>() + C.phrase0,
+                if ((rc = sa_span_enqueue(ix, ix->d_words.as<u64>(), C.span, B.d_sq.as<SpanQuery>() + C.phrase0,
                                           B.d_scounts.as<SpanCounts>() + C.phrase0, ix->phrase_scratch.p, rows, stride,
                                           &t, C.n_term))) return rc;
             }
@@ -802,7 +792,7 @@ static int redo_query(sa_index *ix, BatchState &B, bool is_phrase, u32 idx, u32 
         const Bm25Params p = make_bm25(sq ? sq->idf : B.pqs[idx].idf, B.avg_doc_len, B.k1, B.b, ix->doc_lens_nonneg);
         if (sq) {
             if ((rc = sa_span_run(ix, ix->d_words.as<u64>(), sq->off, sq->len, sq->dir_off, sq->n_terms, sq->slop,
-                                  sq->literal != 0, nullptr))) return rc;
+                                  sq->literal != 0))) return rc;
         } else {
             std::vector<PhraseQuery> one(1, B.pqs[idx]);
             PhraseDump nodump;
@@ -841,15 +831,13 @@ int sa_batch_fix_overflow_locked(sa_index *ix, u32 *n_redone) {
 
     struct Redo { bool phrase; u32 idx, q; const SpanQuery *sq; };
     std::vector<Redo> redo;
-    size_t chunk_i = 0;
     for (const BatchChunk &C : B.chunks) {
         for (u32 i = 0; i < C.n_term; i++)
             if (ovf[C.row0 + i]) redo.push_back({false, C.term0 + i, B.term_query[C.term0 + i], nullptr});
         if (B.slop > 0) {
-            const SpanPlan &plan = B.span_plans[chunk_i++];
             for (u32 i = 0; i < C.n_phrase; i++)
                 if (ovf[C.row0 + C.n_term + i])
-                    redo.push_back({true, C.phrase0 + i, B.phrase_query[C.phrase0 + i], &plan.qs[i]});
+                    redo.push_back({true, C.phrase0 + i, B.phrase_query[C.phrase0 + i], &C.span.qs[i]});
             continue;
         }
         for (u32 i = 0; i < C.n_phrase; i++) {
@@ -870,7 +858,7 @@ int sa_batch_fix_overflow_locked(sa_index *ix, u32 *n_redone) {
         SA_CUDA(cudaMemcpyAsync(B.d_pq.p, B.pqs.data(), B.pqs.size() * sizeof(PhraseQuery), cudaMemcpyHostToDevice, ix->stream));
     if (B.slop > 0) {
         size_t need = 0;
-        for (const SpanPlan &pl : B.span_plans) need = std::max(need, sa_span_scratch_bytes(pl));
+        for (const BatchChunk &C : B.chunks) need = std::max(need, sa_span_scratch_bytes(C.span));
         if ((rc = ix->phrase_scratch.reserve(need))) return rc;
     }
     SA_CUDA(cudaStreamSynchronize(ix->stream));

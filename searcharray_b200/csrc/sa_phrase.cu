@@ -924,6 +924,36 @@ int sa_phrase_enqueue(sa_index *ix, const PhraseQuery *d_pqs, PhraseStats *d_sta
     return launch_phrase_tile(ix, a, split->n_conj);
 }
 
+int sa_phrase_row(sa_index *ix, const u32 *term_ids, u32 n_terms, u32 slop, const u64 *f_offs, const u64 *f_lens,
+                  const Bm25Params *bm25, bool *scored) {
+    u64 offs[SA_MAX_PHRASE_TERMS], lens[SA_MAX_PHRASE_TERMS], dirs[SA_MAX_PHRASE_TERMS];
+    bool missing, literal;
+    int rc = sa_resolve_terms(ix, term_ids, n_terms, offs, lens, dirs, &missing, &literal);
+    if (rc) return rc;
+    const Bm25Params p = bm25 ? *bm25 : make_bm25(0.0f, 1.0f, 1.0f, 0.0f, ix->doc_lens_nonneg);
+    // sparse_ok: a zero count scores +0, so the phrase kernels may score the matches alone, and a zero row is scored
+    const bool score = bm25 && p.sparse_ok;
+    *scored = score && (slop == 0 || missing);
+    if (missing) {                   // an unknown term inside a phrase -> zeros (postings.py:705-708)
+        const u64 stride = sa_padded_docs(ix->n_docs);
+        if ((rc = ix->dense.reserve(stride * sizeof(float)))) return rc;
+        SA_CUDA(cudaMemsetAsync(ix->dense.p, 0, stride * sizeof(float), ix->stream));
+        return SA_OK;
+    }
+    const u64 *d_lists = ix->d_words.as<u64>();
+    if (f_offs) {
+        d_lists = ix->filt.as<u64>();
+        for (u32 i = 0; i < n_terms; i++) { offs[i] = f_offs[i]; lens[i] = f_lens[i]; dirs[i] = SA_NO_DIR; }
+        if (slop > 0 && (rc = sa_span_is_literal(ix, d_lists, offs, lens, n_terms, &literal))) return rc;
+    }
+    // span search (phrase/spans.py + roaringish/spans.pyx): raw counts
+    if (slop > 0) return sa_span_run(ix, d_lists, offs, lens, dirs, n_terms, slop, literal);
+    std::vector<PhraseQuery> pqs(1, make_phrase_query(term_ids, n_terms, offs, lens, dirs, p.idf, false));
+    PhraseDump nodump;
+    memset(&nodump, 0, sizeof(nodump));
+    return sa_phrase_run_sync(ix, pqs, d_lists, score, p, nodump, true);
+}
+
 static int phrase_common(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, uint32_t slop,
                          int score, float idf, float avg_doc_len, float k1, float b,
                          uint64_t min_payload, uint64_t max_payload, float *out_host) {
@@ -944,38 +974,19 @@ static int phrase_common(sa_index *ix, const uint32_t *term_ids, uint32_t n_term
         if (!(score && avg_doc_len != 0.0f) || ix->rows_active) return SA_OK;
     }
     const Bm25Params p = make_bm25(idf, avg_doc_len, k1, b, ix->doc_lens_nonneg);
-    const u64 stride = sa_padded_docs(ix->n_docs);
-    bool raw_counts = false;          // dense row holds raw phrase freqs that still need BM25
     const bool use_payload = !(min_payload == 0 && max_payload == SA_ALL_BITS);
     const bool rows = ix->rows_active;
     SA_CHECK(!(rows && score), "score on a sliced array: call termfreqs + bm25 (the Python layer does)");
     // term lists: the index's own, or filtered copies (sliced array / min-max posn), which is what
     // the reference runs on (middle_out.py:427-437: encoder.slice per term, then the same algorithm)
-    const u64 *d_lists = ix->d_words.as<u64>();
-    if (!missing && (rows || use_payload)) {
-        std::vector<u64> f_offs, f_lens;
-        if ((rc = sa_filter_terms(ix, term_ids, n_terms, rows, min_payload, max_payload, use_payload, f_offs, f_lens))) return rc;
-        d_lists = ix->filt.as<u64>();
-        for (u32 i = 0; i < n_terms; i++) { offs[i] = f_offs[i]; lens[i] = f_lens[i]; dirs[i] = SA_NO_DIR; }
-        if (slop > 0 && (rc = sa_span_is_literal(ix, d_lists, offs, lens, n_terms, &literal))) return rc;
-    }
-    if (!missing && slop > 0) {
-        // span search (phrase/spans.py + roaringish/spans.pyx): raw counts, BM25 afterwards
-        if ((rc = sa_span_run(ix, d_lists, offs, lens, dirs, n_terms, slop, literal, nullptr))) return rc;
-        raw_counts = score != 0;
-    } else if (!missing) {
-        std::vector<PhraseQuery> pqs(1, make_phrase_query(term_ids, n_terms, offs, lens, dirs, idf, false));
-        PhraseDump nodump;
-        memset(&nodump, 0, sizeof(nodump));
-        // raw counts first when BM25 must touch every doc
-        if ((rc = sa_phrase_run_sync(ix, pqs, d_lists, score && p.sparse_ok, p, nodump, true))) return rc;
-        raw_counts = score && !p.sparse_ok;
-    } else {
-        if ((rc = ix->dense.reserve(stride * sizeof(float)))) return rc;
-        SA_CUDA(cudaMemsetAsync(ix->dense.p, 0, stride * sizeof(float), ix->stream));
-        raw_counts = score && !p.sparse_ok;
-    }
-    if (raw_counts) {     // bm25.pyx:20-25 over every doc (tf == 0 scores +0.0 for ordinary parameters)
+    const bool filtered = !missing && (rows || use_payload);
+    std::vector<u64> f_offs, f_lens;
+    if (filtered && (rc = sa_filter_terms(ix, term_ids, n_terms, rows, min_payload, max_payload, use_payload, f_offs,
+                                          f_lens))) return rc;
+    bool scored;
+    if ((rc = sa_phrase_row(ix, term_ids, n_terms, slop, filtered ? f_offs.data() : nullptr,
+                            filtered ? f_lens.data() : nullptr, score ? &p : nullptr, &scored))) return rc;
+    if (score && !scored) {     // bm25.pyx:20-25 over every doc (tf == 0 scores +0.0 for ordinary parameters)
         unsigned blocks = (unsigned)((ix->n_docs + 255) / 256);
         bm25_dense_kernel<<<blocks, 256, 0, ix->stream>>>(ix->dense.as<float>(), ix->d_doc_lens.as<float>(), ix->n_docs, p);
         SA_CUDA(cudaGetLastError());

@@ -93,3 +93,11 @@ DocChunks phrase_doc_chunks(const sa_index *ix, u32 n_queries, u32 ctas_per_sm);
 bool sa_phrase_use_conjunction(const PhraseQuery &pq, u64 n_docs);
 int sa_phrase_run_sync(sa_index *ix, std::vector<PhraseQuery> &pqs, const u64 *d_words,
                        int score, const Bm25Params &p, PhraseDump dump, bool allow_conj);
+// One phrase (slop 0) or span (slop > 0) query's per-doc counts into ix->dense row 0, synchronously.  The caller
+// holds ix->mu and has checked n_terms and the term ids.  Lists: the index's own (f_offs == NULL), or the filtered
+// copies in ix->filt at f_offs / f_lens (sa_filter_terms / sa_filter_terms_mask).  A missing query (sa_resolve_terms)
+// gets a zero row without a launch and reads no f_offs.  bm25: NULL for raw counts; otherwise, where bm25->sparse_ok,
+// a slop-0 query is scored in the phrase kernels under *bm25 (its idf included).  *scored: the row holds BM25 scores
+// (that case, or a missing query's zero row under sparse_ok parameters) rather than counts.
+int sa_phrase_row(sa_index *ix, const u32 *term_ids, u32 n_terms, u32 slop, const u64 *f_offs, const u64 *f_lens,
+                  const Bm25Params *bm25, bool *scored);

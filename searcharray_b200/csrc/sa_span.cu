@@ -1015,7 +1015,7 @@ int sa_span_enqueue(sa_index *ix, const u64 *d_lists, const SpanPlan &plan, cons
 
 // Span search of one query into ix->dense row 0 (raw counts).  Caller holds ix->mu.
 int sa_span_run(sa_index *ix, const u64 *d_lists, const u64 *offs, const u64 *lens, const u64 *dir_offs,
-                uint32_t n_terms, uint32_t slop, bool literal, u32 *n_undefined) {
+                uint32_t n_terms, uint32_t slop, bool literal) {
     const u64 stride = sa_padded_docs(ix->n_docs);
     int rc;
     if ((rc = ix->dense.reserve(stride * sizeof(float)))) return rc;
@@ -1031,6 +1031,5 @@ int sa_span_run(sa_index *ix, const u64 *d_lists, const u64 *offs, const u64 *le
     SA_CUDA(cudaMemcpyAsync(&h, ix->cand_meta.p, sizeof(h), cudaMemcpyDeviceToHost, ix->stream));
     SA_CUDA(cudaStreamSynchronize(ix->stream));
     SA_CHECK(!h.overflow, "span candidate arena exhausted (internal sizing error)");
-    if (n_undefined) *n_undefined = h.undefined;
     return SA_OK;
 }

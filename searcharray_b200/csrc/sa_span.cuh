@@ -55,8 +55,10 @@ size_t sa_span_scratch_bytes(const SpanPlan &plan);
 int sa_span_enqueue(sa_index *ix, const u64 *d_lists, const SpanPlan &plan, const SpanQuery *d_qs,
                     SpanCounts *d_counts, void *d_scratch, float *dense_rows, u64 stride,
                     const struct TopkCtx *topk = nullptr, u32 topk_row0 = 0);
-// One query, synchronously, into ix->dense row 0 (raw counts).
+// One query, synchronously, into ix->dense row 0 (raw counts).  sa_phrase_row runs it for a query given by term ids;
+// the batch re-run calls it with a stored descriptor.
 int sa_span_run(sa_index *ix, const u64 *d_lists, const u64 *offs, const u64 *lens, const u64 *dir_offs,
-                uint32_t n_terms, uint32_t slop, bool literal, u32 *n_undefined);
-// "Every list starts with a word at (doc 0, block 0)" for lists that live in d_lists (device check).
+                uint32_t n_terms, uint32_t slop, bool literal);
+// "Every list starts with a word at (doc 0, block 0)" for lists that live in d_lists (device check, one synchronise
+// per list): the literal flag of filtered lists, for sa_phrase_row.
 int sa_span_is_literal(sa_index *ix, const u64 *d_lists, const u64 *offs, const u64 *lens, u32 n_terms, bool *out);

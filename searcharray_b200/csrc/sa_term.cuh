@@ -138,6 +138,36 @@ inline int sa_resolve_terms(const sa_index *ix, const u32 *term_ids, u32 n, u64 
     return SA_OK;
 }
 
+// The dense rows of a batch of queries.  The queries are cut, in order, into chunks of `chunk` queries: one chunk's
+// doc-space rows stay within about 4 GB of HBM, and its queries fit one grid dimension (65,535).  Inside a chunk the
+// term queries take the first rows, then the multi-term queries, each group in query order.
+struct RowChunk { u32 row0, n_term, n_phrase; };
+struct RowPlan {
+    u32 chunk;
+    std::vector<RowChunk> chunks;
+    std::vector<u32> row_query;      // row -> query
+};
+
+inline RowPlan sa_plan_rows(u64 n_docs, const u32 *term_starts, u32 n_queries) {
+    RowPlan P;
+    const u64 row_bytes = sa_padded_docs(std::max<u64>(n_docs, 1)) * sizeof(float);
+    P.chunk = (u32)std::min<u64>(65535, std::max<u64>(1, std::min<u64>(n_queries, (4ull << 30) / row_bytes)));
+    P.row_query.reserve(n_queries);
+    for (u32 q0 = 0; q0 < n_queries; q0 += P.chunk) {
+        const u32 q1 = std::min(n_queries, q0 + P.chunk);
+        RowChunk C{(u32)P.row_query.size(), 0, 0};
+        for (int pass = 0; pass < 2; pass++)
+            for (u32 q = q0; q < q1; q++) {
+                const bool term = term_starts[q + 1] - term_starts[q] == 1;
+                if (term != (pass == 0)) continue;
+                P.row_query.push_back(q);
+                (term ? C.n_term : C.n_phrase)++;
+            }
+        P.chunks.push_back(C);
+    }
+    return P;
+}
+
 inline TermQuery make_term_query(const sa_index *ix, u32 t, float idf) {
     TermQuery tq;
     memset(&tq, 0, sizeof(tq));

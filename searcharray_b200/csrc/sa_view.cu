@@ -5,11 +5,11 @@
 // (reference postings.py:652-680 on FilteredPosns, middle_out.py:291-317): per-doc counts of the (on a view:
 // filtered) postings, the similarity's formula over the positions, and an idf the caller derived from the document
 // frequencies (a view's from sa_docfreq_rows_batch).  Ids are positions in the view, or doc ids on an unsliced
-// array.  Per chunk of queries:
+// array.  Per chunk of queries (sa_plan_rows, the chunks and row order of the unsliced BM25 batch):
 //   1. per-doc counts in DOC space, one row per query in ix->dense:
 //        phrase / slop queries: on a view the chunk's phrase terms are filtered once (sa_filter_terms_mask), then
-//          every query takes the raw-count route phrase_common takes (sa_phrase_run_sync / sa_span_run) into row 0,
-//          which step 2 consumes before the next query overwrites it;
+//          every query takes sa_phrase_row, the raw-count route of sa_phrase_freqs, into row 0, which step 2
+//          consumes before the next query overwrites it;
 //        term queries: the term kernel in tf mode on the index's own lists, rows [0, n_term) (see term_tiles);
 //   2. sim_tile_kernel: one CTA per (8,192 positions, query) gathers each position's count, scores it and collects
 //      the tile's top-k candidates;
@@ -199,78 +199,31 @@ static int term_tiles(sa_index *ix, const SimRun &R, const u32 *qs, u32 n, const
     return launch_tiles(ix, R, d_idf, n, row0, t);
 }
 
-// Raw counts of one phrase / slop query on the view's filtered lists into ix->dense row 0: what phrase_common
-// computes for sa_phrase_freqs on a sliced array.  f_offs / f_lens: the query's filtered lists in ix->filt.
-static int view_phrase_counts(sa_index *ix, const u32 *tids, u32 nt, u32 slop, bool missing, const u64 *f_offs,
-                              const u64 *f_lens) {
-    const u64 stride = sa_padded_docs(ix->n_docs);
-    int rc;
-    if (missing) {                                   // an unknown term: zeros (postings.py:705-708)
-        if ((rc = ix->dense.reserve(stride * sizeof(float)))) return rc;
-        SA_CUDA(cudaMemsetAsync(ix->dense.p, 0, stride * sizeof(float), ix->stream));
-        return SA_OK;
-    }
-    u64 offs[SA_MAX_PHRASE_TERMS], lens[SA_MAX_PHRASE_TERMS], dirs[SA_MAX_PHRASE_TERMS];
-    for (u32 i = 0; i < nt; i++) { offs[i] = f_offs[i]; lens[i] = f_lens[i]; dirs[i] = SA_NO_DIR; }
-    const u64 *d_lists = ix->filt.as<u64>();
-    if (slop > 0) {
-        bool literal;
-        if ((rc = sa_span_is_literal(ix, d_lists, offs, lens, nt, &literal))) return rc;
-        return sa_span_run(ix, d_lists, offs, lens, dirs, nt, slop, literal, nullptr);
-    }
-    std::vector<PhraseQuery> pqs(1, make_phrase_query(tids, nt, offs, lens, dirs, 0.0f, false));
-    PhraseDump nodump;
-    memset(&nodump, 0, sizeof(nodump));
-    return sa_phrase_run_sync(ix, pqs, d_lists, 0, make_bm25(0, 1, 1, 0, ix->doc_lens_nonneg), nodump, true);
-}
-
-// Raw counts of one phrase / slop query on the index's own lists into ix->dense row 0: what phrase_common computes
-// for sa_phrase_freqs on an unsliced array.
-static int own_phrase_counts(sa_index *ix, const u32 *tids, u32 nt, u32 slop) {
-    u64 offs[SA_MAX_PHRASE_TERMS], lens[SA_MAX_PHRASE_TERMS], dirs[SA_MAX_PHRASE_TERMS];
-    bool missing, literal;
-    int rc = sa_resolve_terms(ix, tids, nt, offs, lens, dirs, &missing, &literal);
-    if (rc) return rc;
-    if (missing) return view_phrase_counts(ix, tids, nt, slop, true, nullptr, nullptr);    // zeros
-    if (slop > 0) return sa_span_run(ix, ix->d_words.as<u64>(), offs, lens, dirs, nt, slop, literal, nullptr);
-    std::vector<PhraseQuery> pqs(1, make_phrase_query(tids, nt, offs, lens, dirs, 0.0f, false));
-    PhraseDump nodump;
-    memset(&nodump, 0, sizeof(nodump));
-    return sa_phrase_run_sync(ix, pqs, ix->d_words.as<u64>(), 0, make_bm25(0, 1, 1, 0, ix->doc_lens_nonneg), nodump, true);
-}
-
-static bool query_missing(const sa_index *ix, const u32 *tids, u32 nt) {
-    for (u32 i = 0; i < nt; i++)
-        if (tids[i] == SA_NO_TERM || ix->h_len[tids[i]] == 0) return true;
-    return false;
-}
-
-// Phrase / slop queries qs[0, n), one at a time: raw counts into ix->dense row 0, then the query's tile pass (row
-// row0 + j of t, idf d_idf[j]).  On a view, one filter pass over every list of the n queries comes first (a query
-// with a missing term has none).
+// Phrase / slop queries qs[0, n), one at a time: raw counts into ix->dense row 0 (sa_phrase_row), then the query's
+// tile pass (row row0 + j of t, idf d_idf[j]).  On a view, one filter pass over every list of the n queries comes
+// first; a missing query has no filtered lists, and sa_phrase_row reads none for it.
 static int phrase_tiles(sa_index *ix, const SimRun &R, const u32 *qs, u32 n, const double *d_idf, u32 row0,
                         const TopkCtx &t) {
     const bool view = ix->rows_active;
     std::vector<u32> ftids, fstart;
-    std::vector<unsigned char> missing;
     std::vector<u64> f_offs, f_lens;
     int rc;
     for (u32 j = 0; j < n && view; j++) {
         const u32 *tids = R.tids(qs[j]);
         const u32 nt = R.n_terms(qs[j]);
+        u64 offs[SA_MAX_PHRASE_TERMS], lens[SA_MAX_PHRASE_TERMS], dirs[SA_MAX_PHRASE_TERMS];
+        bool missing, literal;
+        if ((rc = sa_resolve_terms(ix, tids, nt, offs, lens, dirs, &missing, &literal))) return rc;
         fstart.push_back((u32)ftids.size());
-        missing.push_back(query_missing(ix, tids, nt));
-        if (!missing.back()) ftids.insert(ftids.end(), tids, tids + nt);
+        if (!missing) ftids.insert(ftids.end(), tids, tids + nt);
     }
     if (!ftids.empty() && (rc = sa_filter_terms_mask(ix, ftids.data(), (u32)ftids.size(), ix->d_row_mask(), 0,
                                                      SA_ALL_BITS, false, f_offs, f_lens, nullptr))) return rc;
     for (u32 j = 0; j < n; j++) {
-        const u32 *tids = R.tids(qs[j]);
-        const u32 nt = R.n_terms(qs[j]);
-        if (!view) rc = own_phrase_counts(ix, tids, nt, R.slop);
-        else if (missing[j]) rc = view_phrase_counts(ix, tids, nt, R.slop, true, nullptr, nullptr);
-        else rc = view_phrase_counts(ix, tids, nt, R.slop, false, f_offs.data() + fstart[j], f_lens.data() + fstart[j]);
-        if (rc || (rc = launch_tiles(ix, R, d_idf + j, 1, row0 + j, t))) return rc;
+        bool scored;
+        if ((rc = sa_phrase_row(ix, R.tids(qs[j]), R.n_terms(qs[j]), R.slop, view ? f_offs.data() + fstart[j] : nullptr,
+                                view ? f_lens.data() + fstart[j] : nullptr, nullptr, &scored)) ||
+            (rc = launch_tiles(ix, R, d_idf + j, 1, row0 + j, t))) return rc;
     }
     return SA_OK;
 }
@@ -332,9 +285,9 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
     const SimRun R{kind, make_bm25(0.0f, (float)avg_doc_len, (float)k1, (float)b, false),
                    make_sim_params(avg_doc_len, k1, b), terms, term_starts, slop};
     const u32 n_tiles = sa_n_tiles(n_pos), slots = classic ? 256u : sa_topk_slots(k);
-    // chunk so the doc-space count rows of one chunk stay within ~4 GB of HBM, as sa_batch_upload_locked does
-    const u32 chunk = (u32)std::min<u64>(65535, std::max<u64>(1, std::min<u64>(n_queries,
-                                         (4ull << 30) / (sa_padded_docs(ix->n_docs) * sizeof(float)))));
+    const RowPlan plan = sa_plan_rows(ix->n_docs, term_starts, n_queries);
+    const u32 chunk = plan.chunk;
+    const std::vector<u32> &row_query = plan.row_query;
     // Every buffer is reserved before the first write: DevBuf::reserve does not keep the contents.  ix->dense is the
     // exception -- each step reserves it and consumes what it wrote before the next reserve.
     if (kind == SA_SIM_BM25 && (rc = V.d_dl.reserve(n_pos * sizeof(float)))) return rc;
@@ -347,26 +300,8 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
     if (classic && (rc = V.d_scores.reserve(nk * sizeof(double)))) return rc;
     if (classic && (rc = V.d_cand_d.reserve((size_t)chunk * n_tiles * slots * sizeof(u64)))) return rc;
 
-    // rows: chunk by chunk, the term queries first, then the phrase queries
-    struct Chunk { u32 row0, n_term, n_phrase; };
-    std::vector<Chunk> chunks;
-    std::vector<u32> row_query;
-    std::vector<double> row_idf;
-    row_query.reserve(n_queries);
-    row_idf.reserve(n_queries);
-    for (u32 q0 = 0; q0 < n_queries; q0 += chunk) {
-        const u32 q1 = std::min(n_queries, q0 + chunk);
-        Chunk C{(u32)row_query.size(), 0, 0};
-        for (int pass = 0; pass < 2; pass++)
-            for (u32 q = q0; q < q1; q++) {
-                const bool term = R.n_terms(q) == 1;
-                if (term != (pass == 0)) continue;
-                row_query.push_back(q);
-                row_idf.push_back(idf[q]);
-                (term ? C.n_term : C.n_phrase)++;
-            }
-        chunks.push_back(C);
-    }
+    std::vector<double> row_idf(n_queries);
+    for (u32 r = 0; r < n_queries; r++) row_idf[r] = idf[row_query[r]];
     if (kind == SA_SIM_BM25)
         SA_CUDA(cudaMemcpyAsync(V.d_dl.p, view_doc_lens, n_pos * sizeof(float), cudaMemcpyHostToDevice, ix->stream));
     SA_CUDA(cudaMemcpyAsync(V.d_idf.p, row_idf.data(), n_queries * sizeof(double), cudaMemcpyHostToDevice, ix->stream));
@@ -374,7 +309,7 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
     SA_CUDA(cudaMemsetAsync(V.d_ovf.p, 0, n_queries * sizeof(u32), ix->stream));
     const double *d_idf = V.d_idf.as<double>();
 
-    for (const Chunk &C : chunks) {
+    for (const RowChunk &C : plan.chunks) {
         const u32 Q = C.n_term + C.n_phrase;
         const u32 *qs = row_query.data() + C.row0;
         TopkCtx t = make_topk_ctx(ix->cand.p, n_tiles, Q, slots, k, V.d_ovf.as<u32>() + C.row0);
