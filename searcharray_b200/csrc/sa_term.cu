@@ -147,7 +147,9 @@ term_tile_kernel(const TermBatchArgs a) {
             // look-ahead lanes may read into the next tile (another doc) but never past the list
             w[u] = (i < n_words && i < hi + 2) ? __ldg(words + i) : ~0ull;
         }
-        u32 pk[UN];                                       // rel << 18 | tf, ~0 = not a head
+        // rel << 19 | tf, the tf records' layout: tf <= 2^18 (positions < 2^18) needs 19 bits, and rel < 2^13 keeps
+        // every packed value below ~0 = not a head
+        u32 pk[UN];
         float nr[UN];
 #pragma unroll
         for (int u = 0; u < UN; u++) {
@@ -180,7 +182,7 @@ term_tile_kernel(const TermBatchArgs a) {
                         }
                     }
                 }
-                pk[u] = (rel << 18) | tf;
+                pk[u] = (rel << SA_REC_TF_BITS) | tf;
                 if (MODE == TERM_MODE_SCORE && !ALL_DOCS && tf && !staged_norm) nr[u] = __ldg(norm + rel);
             }
         }
@@ -192,7 +194,7 @@ term_tile_kernel(const TermBatchArgs a) {
 #pragma unroll
         for (int u = 0; u < UN; u++) {
             if (pk[u] != ~0u) {
-                const u32 rel = pk[u] >> 18, tf = pk[u] & 0x3FFFFu;
+                const u32 rel = pk[u] >> SA_REC_TF_BITS, tf = pk[u] & SA_REC_TF_MASK;
                 float v;
                 if (MODE == TERM_MODE_TF || ALL_DOCS) {
                     v = (float)tf;
@@ -413,8 +415,10 @@ int launch_term_batch(sa_index *ix, const TermBatchArgs &a_in, u32 n_queries) {
     {
         // tuning knobs, read per launch (a getenv costs nanoseconds; tools/term_buckets.py sweeps them in one process)
         const char *e;
-        a.staged_norm_min_words = (e = getenv("SA_STAGED_NORM_MIN_WORDS")) ? (u32)atol(e) : SA_STAGED_NORM_MIN_WORDS;
-        a.staged_norm_min_recs = (e = getenv("SA_STAGED_NORM_MIN_RECS")) ? (u32)atol(e) : SA_STAGED_NORM_MIN_RECS;
+        // the staged-norm thresholds are at least 1: a tile with no records or words must not stage norms, since it
+        // would exit with its cp.async copies still in flight
+        a.staged_norm_min_words = std::max(1u, (e = getenv("SA_STAGED_NORM_MIN_WORDS")) ? (u32)atol(e) : SA_STAGED_NORM_MIN_WORDS);
+        a.staged_norm_min_recs = std::max(1u, (e = getenv("SA_STAGED_NORM_MIN_RECS")) ? (u32)atol(e) : SA_STAGED_NORM_MIN_RECS);
         a.quad_min_recs = (e = getenv("SA_TERM_QUAD_MIN_RECS")) ? (u32)atol(e) : SA_TERM_QUAD_MIN_RECS;
         a.prefetch_tiles = (e = getenv("SA_TERM_PREFETCH_TILES")) ? (u32)atol(e) : SA_TERM_PREFETCH_TILES;
         a.quad_min_recs = std::max(a.quad_min_recs, a.staged_norm_min_recs);   // the quad path reads norms from the staged tile only
