@@ -150,6 +150,20 @@ int sa_score_batch_topk_sim(sa_index *index, int kind, const uint32_t *terms, co
                             const double *idf, uint32_t n_queries, uint32_t slop, const float *view_doc_lens,
                             double avg_doc_len, double k1, double b, uint32_t k, uint32_t *out_ids,
                             double *out_scores);
+/* Batched boolean queries: OR / AND / min-should-match over term and phrase clauses (the reference's composition in
+ * test/test_search.py:126-226).  Query q = clauses [query_clause_starts[q], query_clause_starts[q+1]) (1 to
+ * SA_BOOL_MAX_CLAUSES of them; query_clause_starts[0] == 0); clause c = clause_terms[clause_term_starts[c] ..
+ * clause_term_starts[c+1]) (1 term, or a phrase with `slop`), scored exactly as sa_score_term / sa_score_phrase with
+ * idf clause_idf[c].  Per query, s = score(c0) + score(c1) + ... folded left in float32; a doc ranks iff s > 0 and at
+ * least mm[q] (<= its clauses) clauses score > 0 there.  Result: the top k by (score desc, doc id asc; as
+ * np.argpartition, searcharray/utils/sort.py:24), GLOBAL doc ids (doc_base added), empty slots SA_NO_DOC / 0.
+ * Phrase clauses need ordinary BM25 parameters (k1 > 0, 0 <= b < 1).  *n_redone (nullable): queries re-run exactly
+ * because a tile had more candidates than slots. */
+#define SA_BOOL_MAX_CLAUSES 64
+int sa_score_batch_topk_bool(sa_index *index, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
+                             const uint32_t *clause_term_starts, const float *clause_idf, const uint32_t *mm,
+                             uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
+                             uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
 
 /* The same batch in three stages, so a serving loop (or the benchmark) can keep the query
  * descriptors resident and time the device work alone: upload (H2D of descriptors), execute

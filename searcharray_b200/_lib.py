@@ -53,6 +53,8 @@ SIGNATURES = {
     "sa_score_batch_topk_sim": (c_int, [P_void, c_int, P_u32, P_u32, ctypes.POINTER(ctypes.c_double), c_u32, c_u32,
                                         P_f32, ctypes.c_double, ctypes.c_double, ctypes.c_double, c_u32, P_u32,
                                         ctypes.POINTER(ctypes.c_double)]),
+    "sa_score_batch_topk_bool": (c_int, [P_void, P_u32, P_u32, P_u32, P_f32, P_u32, c_u32, c_u32, c_f32, c_f32, c_f32,
+                                         c_u32, P_u32, P_f32, P_u32]),
     "sa_batch_upload": (c_int, [P_void, P_u32, P_u32, P_f32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32]),
     "sa_batch_execute": (c_int, [P_void]),
     "sa_batch_download": (c_int, [P_void, P_u32, P_f32, P_u32]),

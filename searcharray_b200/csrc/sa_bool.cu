@@ -1,0 +1,377 @@
+// sa_bool.cu -- batched boolean queries (OR / AND / min-should-match over term and phrase clauses), ranked on the
+// device.
+//
+// Replaces the reference's own composition of multi-clause queries (test/test_search.py:126-226):
+//   scores = arr.score(c0) + arr.score(c1) + ...                              float32, clause order
+//   ok     = np.sum(np.array([arr.score(c) for c in clauses]) > 0, axis=0) >= mm
+//   top    = np.argpartition(np.where(ok, scores, 0), -k)[-k:]               utils/sort.py:24
+//
+// Design.  One CTA per (query, 8192-doc tile), the query index fastest (as term_tile_kernel).  Every thread owns
+// the 32 docs of the tile that flush_tile_collect hands it (4 g .. 4 g + 3, g = tid + j * 256) and keeps their
+// running sums and hit counts in registers; the clauses are folded in order, so each sum is the exact left fold
+// above.  A term clause is scanned in place -- its (doc, tf) records, or its posting words with run heads summing
+// popcounts -- and scattered as BM25 scores (bm25_from_norm over the cached norms) into a shared tile, which the
+// owners read back after a barrier.  A phrase clause reads its count row (materialised beforehand by
+// sa_phrase_row) coalesced.  Under parameters that are not sparse-safe a term clause scatters tf and the owners
+// evaluate bm25_one over every doc, as the ALL_DOCS term scan does.  Before the fold the CTA counts the clauses that
+// have anything in the tile; fewer than mm -> no doc of the tile can rank, and the tile is published empty.
+// Then the docs below mm are zeroed and the tile goes through flush_tile_collect, the float32 collector of every
+// other path, and topk_select_kernel ranks the candidates.
+#include "sa_term.cuh"
+#include "sa_phrase.cuh"
+
+#define SA_BOOL_NO_ROW 0xFFFFFFFFu
+
+struct BoolClause {
+    u64 word_off, n_words, dir_off, rec_off;   // a term clause's list (TermQuery's fields); n_words == 0: no doc
+    float idf;
+    u32 row;        // a phrase clause's count row in BoolState::rows (within its group); SA_BOOL_NO_ROW: a term
+    u32 sparse;     // Bm25Params::sparse_ok under this clause's idf
+    u32 pad;
+};
+
+struct BoolQuery { u32 c0, n, mm, pad; };   // clauses [c0, c0 + n) of the batch
+
+struct BoolArgs {
+    const u64 *words;
+    const u32 *tile_dir, *recs, *rec_dir;   // see sa_index; recs NULL: no tf table
+    const float *norm, *doc_lens;
+    const float *rows;                      // phrase clauses' count rows, row_stride floats apart
+    u64 row_stride, n_docs, doc_base;
+    const BoolClause *clauses;
+    const BoolQuery *queries;               // [gridDim.x]
+    Bm25Params bm25;                        // idf unused (per clause)
+    TopkCtx topk;
+};
+
+struct BoolState {
+    DevBuf d_clauses, d_queries, d_out_index;
+    DevBuf d_keys;       // nq * k result keys, then u32 overflow[nq]: one device-to-host copy
+    DevBuf rows;
+};
+void BoolStateDelete::operator()(BoolState *s) const { delete s; }
+
+__device__ __forceinline__ bool bool_uses_recs(const BoolArgs &a, const BoolClause &cl) {
+    return a.recs != nullptr && cl.rec_off != SA_NO_DIR && cl.dir_off != SA_NO_DIR;
+}
+
+// A term clause's docs of this tile into s_tile: BM25 scores (sparse) or tf.  Slice [lo, hi) of its records or words.
+__device__ __forceinline__ void bool_scatter_term(const BoolArgs &a, const BoolClause &cl, u32 lo, u32 hi,
+                                                  u32 tile_doc0, u64 tile_doc0_abs, float *s_tile) {
+    const float *__restrict__ norm = a.norm + tile_doc0;
+    if (bool_uses_recs(a, cl)) {
+        const u32 *__restrict__ recs = a.recs + cl.rec_off;
+        for (u32 i = lo + threadIdx.x; i < hi; i += SA_TERM_THREADS) {
+            const u32 r = __ldg(recs + i), rel = r >> SA_REC_TF_BITS, tf = r & SA_REC_TF_MASK;
+            s_tile[rel] = cl.sparse ? bm25_from_norm((float)tf, __ldg(norm + rel), cl.idf) : (float)tf;
+        }
+        return;
+    }
+    // words: the thread holding a doc's first word sums the popcounts of the doc's run (a doc never spans tiles)
+    const u64 *__restrict__ words = a.words + cl.word_off;
+    for (u32 i = lo + threadIdx.x; i < hi; i += SA_TERM_THREADS) {
+        const u64 doc = __ldg(words + i) >> SA_KEY_SHIFT;
+        if (i > lo && (__ldg(words + i - 1) >> SA_KEY_SHIFT) == doc) continue;
+        u32 tf = 0;
+        for (u32 j = i; j < hi; j++) {
+            const u64 w = __ldg(words + j);
+            if ((w >> SA_KEY_SHIFT) != doc) break;
+            tf += (u32)__popcll(w & SA_LSB_MASK);
+        }
+        const u32 rel = (u32)(doc - tile_doc0_abs);
+        s_tile[rel] = cl.sparse ? bm25_from_norm((float)tf, __ldg(norm + rel), cl.idf) : (float)tf;
+    }
+}
+
+__global__ void __launch_bounds__(SA_TERM_THREADS)
+bool_tile_kernel(const BoolArgs a) {
+    constexpr int PER = SA_TILE_DOCS / SA_TERM_THREADS / 4;        // float4 groups per thread
+    __shared__ __align__(16) float s_tile[SA_TILE_DOCS];
+    __shared__ u32 s_lo[SA_BOOL_MAX_CLAUSES], s_hi[SA_BOOL_MAX_CLAUSES];
+    __shared__ u32 s_top[(SA_TERM_THREADS / 32) * 8];
+    __shared__ u32 s_ncand, s_tile_max, s_present;
+    const u32 q = blockIdx.x, tile = blockIdx.y;
+    const BoolQuery bq = a.queries[q];
+    const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const u32 tile_doc0 = tile * SA_TILE_DOCS;
+    const u64 tile_doc0_abs = a.doc_base + tile_doc0;              // as stored in the words
+    float4 *s_tile4 = reinterpret_cast<float4 *>(s_tile);
+
+    // 1. zero the tile; every clause's slice of the tile, and how many clauses have anything in it
+#pragma unroll
+    for (int j = 0; j < PER; j++) s_tile4[tid + j * SA_TERM_THREADS] = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (tid == 0) s_present = 0;
+    __syncthreads();
+    for (u32 c = warp; c < bq.n; c += SA_TERM_THREADS / 32) {      // warp-uniform
+        const BoolClause cl = a.clauses[bq.c0 + c];
+        u32 lo = 0, hi = 0;
+        if (cl.row != SA_BOOL_NO_ROW) {
+            hi = 1;                                                 // a phrase row counts as present
+        } else if (cl.n_words == 0) {
+        } else if (cl.dir_off != SA_NO_DIR) {
+            const u32 *dir = (bool_uses_recs(a, cl) ? a.rec_dir : a.tile_dir) + cl.dir_off + tile;
+            lo = __ldg(dir);
+            hi = __ldg(dir + 1);
+        } else {
+            const u64 *w = a.words + cl.word_off;
+            lo = (u32)warp_lower_bound_shifted(w, 0, cl.n_words, tile_doc0_abs, SA_KEY_SHIFT);
+            hi = (u32)warp_lower_bound_shifted(w, lo, cl.n_words, tile_doc0_abs + SA_TILE_DOCS, SA_KEY_SHIFT);
+        }
+        if (lane == 0) {
+            s_lo[c] = lo;
+            s_hi[c] = hi;
+            if (hi > lo) atomicAdd(&s_present, 1u);
+        }
+    }
+    __syncthreads();
+    // 2. a clause with nothing in the tile scores > 0 at no doc of it: fewer such clauses than mm, nothing ranks
+    if (s_present < bq.mm) {                                        // CTA-uniform
+        if (tid == 0) {
+            const u64 t_idx = (u64)q * a.topk.n_tiles + tile;
+            a.topk.tile_cnt[t_idx] = 0;
+            a.topk.tile_max[t_idx] = 0;
+        }
+        return;
+    }
+
+    // 3. the fold, clause by clause in order
+    float acc[PER * 4];
+    u32 hits[PER];                         // byte e of hits[j]: clauses scoring > 0 at doc 4 g + e (<= 64 clauses)
+#pragma unroll
+    for (int i = 0; i < PER * 4; i++) acc[i] = 0.0f;
+#pragma unroll
+    for (int j = 0; j < PER; j++) hits[j] = 0;
+    Bm25Params p = a.bm25;
+    for (u32 c = 0; c < bq.n; c++) {
+        const BoolClause cl = a.clauses[bq.c0 + c];
+        const u32 lo = s_lo[c], hi = s_hi[c];
+        if (cl.sparse && hi <= lo) continue;                        // CTA-uniform: +0 at every doc of the tile
+        p.idf = cl.idf;
+        if (cl.row != SA_BOOL_NO_ROW) {
+            // phrase clause (sparse-safe parameters only): BM25 of its counts, zero counts score +0
+            const float4 *__restrict__ r4 = reinterpret_cast<const float4 *>(a.rows + (u64)cl.row * a.row_stride + tile_doc0);
+#pragma unroll
+            for (int j = 0; j < PER; j++) {
+                const unsigned g = tid + j * SA_TERM_THREADS;
+                const float4 x = __ldcs(r4 + g);
+                const float xs[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+                for (int e = 0; e < 4; e++) {
+                    const u64 d = (u64)tile_doc0 + g * 4 + e;
+                    float v = 0.0f;
+                    if (xs[e] > 0.0f && d < a.n_docs) v = bm25_from_norm(xs[e], __ldg(a.norm + d), cl.idf);
+                    acc[j * 4 + e] = __fadd_rn(acc[j * 4 + e], v);
+                    hits[j] += (v > 0.0f ? 1u : 0u) << (8 * e);
+                }
+            }
+        } else {
+            bool_scatter_term(a, cl, lo, hi, tile_doc0, tile_doc0_abs, s_tile);
+            __syncthreads();
+#pragma unroll
+            for (int j = 0; j < PER; j++) {
+                const unsigned g = tid + j * SA_TERM_THREADS;
+                const float4 x = s_tile4[g];
+                s_tile4[g] = make_float4(0.f, 0.f, 0.f, 0.f);
+                const float xs[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+                for (int e = 0; e < 4; e++) {
+                    const u64 d = (u64)tile_doc0 + g * 4 + e;
+                    float v = xs[e];
+                    // bm25.pyx:20-25 over every doc (NaN / inf / -0.0 of exotic parameters)
+                    if (!cl.sparse) v = d < a.n_docs ? bm25_one(xs[e], __ldg(a.doc_lens + d), p) : 0.0f;
+                    acc[j * 4 + e] = __fadd_rn(acc[j * 4 + e], v);
+                    hits[j] += (v > 0.0f ? 1u : 0u) << (8 * e);
+                }
+            }
+            __syncthreads();
+        }
+    }
+
+    // 4. docs with fewer than mm hits (or a sum <= 0 / NaN) do not rank; collect the tile's top-k candidates
+    u32 my_max = 0;
+#pragma unroll
+    for (int j = 0; j < PER; j++) {
+        float o[4];
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            const float s = acc[j * 4 + e];
+            o[e] = (((hits[j] >> (8 * e)) & 0xFFu) >= bq.mm && s > 0.0f) ? s : 0.0f;
+            my_max = max(my_max, __float_as_uint(o[e]));
+        }
+        s_tile4[tid + j * SA_TERM_THREADS] = make_float4(o[0], o[1], o[2], o[3]);
+    }
+    flush_tile_collect<false>(s_tile, nullptr, a.topk, q, tile, my_max, SA_TILE_DOCS, 0, s_top, &s_ncand, &s_tile_max);
+}
+
+// ------------------------------------------------------------------------------------------------------------ host
+namespace {
+
+struct BoolPlan {
+    std::vector<BoolClause> clauses;
+    std::vector<BoolQuery> queries;
+    std::vector<u32> group_start;       // queries [group_start[i], group_start[i + 1]) share one launch and its rows
+    u32 max_group = 1, max_rows = 0;
+    bool any_sparse = false;
+};
+
+// The count rows of the phrase clauses of queries [q0, q1) (rows are numbered within the group), synchronously.
+int bool_build_rows(sa_index *ix, BoolState &S, const BoolPlan &P, const uint32_t *clause_terms,
+                    const uint32_t *clause_term_starts, u32 slop, u32 q0, u32 q1) {
+    const u64 stride = sa_padded_docs(ix->n_docs);
+    int rc;
+    for (u32 q = q0; q < q1; q++) {
+        const BoolQuery &bq = P.queries[q];
+        for (u32 c = bq.c0; c < bq.c0 + bq.n; c++) {
+            const BoolClause &cl = P.clauses[c];
+            if (cl.row == SA_BOOL_NO_ROW) continue;
+            bool scored;
+            if ((rc = sa_phrase_row(ix, clause_terms + clause_term_starts[c], clause_term_starts[c + 1] - clause_term_starts[c],
+                                    slop, nullptr, nullptr, nullptr, &scored))) return rc;
+            SA_CUDA(cudaMemcpyAsync(S.rows.as<float>() + (u64)cl.row * stride, ix->dense.p, ix->n_docs * sizeof(float),
+                                    cudaMemcpyDeviceToDevice, ix->stream));
+        }
+    }
+    return SA_OK;
+}
+
+// Queries [q0, q1) with `slots` candidate slots per tile: their rows, the tile kernel and the selection, enqueued.
+int bool_run_group(sa_index *ix, BoolState &S, const BoolPlan &P, const uint32_t *clause_terms,
+                   const uint32_t *clause_term_starts, u32 slop, const Bm25Params &bm25, u32 k, u32 slots,
+                   u32 q0, u32 q1) {
+    const u32 n_tiles = sa_n_tiles(ix->n_docs), nq = q1 - q0;
+    int rc;
+    if ((rc = bool_build_rows(ix, S, P, clause_terms, clause_term_starts, slop, q0, q1))) return rc;
+    if ((rc = ix->cand.reserve(cand_bytes(n_tiles, nq, slots)))) return rc;
+    u64 *d_keys = S.d_keys.as<u64>();
+    u32 *d_ovf = (u32 *)(d_keys + (size_t)P.queries.size() * k);
+    TopkCtx t = make_topk_ctx(ix->cand.p, n_tiles, nq, slots, k, d_ovf + q0);
+    BoolArgs a;
+    memset(&a, 0, sizeof(a));
+    a.words = ix->d_words.as<u64>();
+    a.tile_dir = ix->d_tile_dir.as<u32>();
+    a.recs = ix->d_recs.as<u32>();
+    a.rec_dir = ix->d_rec_dir.as<u32>();
+    a.norm = ix->d_norm.as<float>();
+    a.doc_lens = ix->d_doc_lens.as<float>();
+    a.rows = S.rows.as<float>();
+    a.row_stride = sa_padded_docs(ix->n_docs);
+    a.n_docs = ix->n_docs;
+    a.doc_base = ix->doc_base;
+    a.clauses = S.d_clauses.as<BoolClause>();
+    a.queries = S.d_queries.as<BoolQuery>() + q0;
+    a.bm25 = bm25;
+    a.topk = t;
+    bool_tile_kernel<<<dim3(nq, n_tiles), SA_TERM_THREADS, 0, ix->stream>>>(a);
+    SA_CUDA(cudaGetLastError());
+    ix->stats.total_launches++;
+    return launch_topk_select(ix, t, nq, ix->doc_base, d_keys, S.d_out_index.as<u32>() + q0);
+}
+
+}  // namespace
+
+extern "C" int sa_score_batch_topk_bool(sa_index *ix, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
+                                        const uint32_t *clause_term_starts, const float *clause_idf, const uint32_t *mm,
+                                        uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
+                                        uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+    SA_CHECK(ix && out_docs && out_scores, "NULL argument");
+    SA_CHECK(n_queries == 0 || (query_clause_starts && clause_terms && clause_term_starts && clause_idf && mm),
+             "NULL argument");
+    SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
+    if (n_redone) *n_redone = 0;
+    std::lock_guard<std::mutex> g(ix->mu);
+    SA_CUDA(cudaSetDevice(ix->device));
+    int rc;
+    SA_CHECK(n_queries == 0 || query_clause_starts[0] == 0, "query_clause_starts[0] must be 0");
+    for (u32 q = 0; q < n_queries; q++) {
+        SA_CHECK(query_clause_starts[q + 1] > query_clause_starts[q] &&
+                 query_clause_starts[q + 1] - query_clause_starts[q] <= SA_BOOL_MAX_CLAUSES,
+                 "query %u: a boolean query has 1 to %d clauses", q, SA_BOOL_MAX_CLAUSES);
+        SA_CHECK(mm[q] <= query_clause_starts[q + 1] - query_clause_starts[q], "query %u: mm exceeds its clauses", q);
+    }
+    const u32 c_begin = n_queries ? query_clause_starts[0] : 0, c_end = n_queries ? query_clause_starts[n_queries] : 0;
+    for (u32 c = c_begin; c < c_end; c++) {
+        const u32 nt = clause_term_starts[c + 1] - clause_term_starts[c];
+        SA_CHECK(clause_term_starts[c + 1] > clause_term_starts[c] && nt <= SA_MAX_PHRASE_TERMS,
+                 "clause %u: bad number of terms", c);
+        if ((rc = sa_check_term_ids(ix, clause_terms + clause_term_starts[c], nt))) return rc;
+    }
+    const size_t nk = (size_t)n_queries * k;
+    for (size_t i = 0; i < nk; i++) { out_docs[i] = SA_NO_DOC; out_scores[i] = 0.0f; }
+    if (n_queries == 0 || ix->n_docs == 0 || avg_doc_len == 0.0f) return SA_OK;   // .score is all zeros: nothing ranks
+
+    // descriptors, and the groups: at most ~1 GB of candidate slots and ~4 GB of phrase rows per launch
+    const u32 n_tiles = sa_n_tiles(ix->n_docs), slots = sa_topk_slots(k);
+    const u64 stride = sa_padded_docs(ix->n_docs);
+    const u32 group_q = (u32)std::min<u64>(65535, std::max<u64>(1, (1ull << 30) / ((u64)n_tiles * (slots * sizeof(u64) + 8))));
+    const u32 group_rows = (u32)std::max<u64>(1, (4ull << 30) / (stride * sizeof(float)));
+    const Bm25Params bm25 = make_bm25(1.0f, avg_doc_len, k1, b, ix->doc_lens_nonneg);
+    BoolPlan P;
+    P.queries.resize(n_queries);
+    P.group_start.push_back(0);
+    u32 rows = 0;
+    for (u32 q = 0; q < n_queries; q++) {
+        const u32 c0 = query_clause_starts[q], c1 = query_clause_starts[q + 1];
+        u32 nr = 0;
+        for (u32 c = c0; c < c1; c++) nr += clause_term_starts[c + 1] - clause_term_starts[c] > 1;
+        if (q > P.group_start.back() && (q - P.group_start.back() == group_q || rows + nr > group_rows)) {
+            P.group_start.push_back(q);
+            rows = 0;
+        }
+        P.queries[q] = BoolQuery{(u32)P.clauses.size(), c1 - c0, mm[q], 0};
+        for (u32 c = c0; c < c1; c++) {
+            const u32 *tids = clause_terms + clause_term_starts[c];
+            const u32 nt = clause_term_starts[c + 1] - clause_term_starts[c];
+            const bool sparse = make_bm25(clause_idf[c], avg_doc_len, k1, b, ix->doc_lens_nonneg).sparse_ok != 0;
+            SA_CHECK(nt == 1 || sparse, "phrase queries in a batch need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite idf)");
+            const TermQuery tq = make_term_query(ix, nt == 1 ? tids[0] : SA_NO_TERM, clause_idf[c]);
+            P.clauses.push_back(BoolClause{tq.word_off, tq.n_words, tq.dir_off, tq.rec_off, clause_idf[c],
+                                           nt == 1 ? SA_BOOL_NO_ROW : rows++, sparse ? 1u : 0u, 0});
+            P.any_sparse = P.any_sparse || sparse;
+        }
+        P.max_group = std::max(P.max_group, q + 1 - P.group_start.back());
+        P.max_rows = std::max(P.max_rows, rows);
+    }
+    P.group_start.push_back(n_queries);
+
+    if (!ix->boolq) ix->boolq.reset(new BoolState());
+    BoolState &S = *ix->boolq;
+    const size_t key_bytes = nk * sizeof(u64) + (size_t)n_queries * sizeof(u32);
+    if ((rc = S.d_clauses.reserve(P.clauses.size() * sizeof(BoolClause))) ||
+        (rc = S.d_queries.reserve(P.queries.size() * sizeof(BoolQuery))) ||
+        (rc = S.d_out_index.reserve((size_t)n_queries * sizeof(u32))) || (rc = S.d_keys.reserve(key_bytes)) ||
+        (rc = S.rows.reserve(std::max<size_t>((size_t)P.max_rows * stride * sizeof(float), 64))) ||
+        (rc = ix->h_pinned.reserve(key_bytes)))
+        return rc;
+    if (P.any_sparse && (rc = sa_ensure_norm(ix, k1, b, avg_doc_len))) return rc;
+    std::vector<u32> identity(n_queries);
+    for (u32 q = 0; q < n_queries; q++) identity[q] = q;
+    SA_CUDA(cudaMemcpyAsync(S.d_clauses.p, P.clauses.data(), P.clauses.size() * sizeof(BoolClause), cudaMemcpyHostToDevice, ix->stream));
+    SA_CUDA(cudaMemcpyAsync(S.d_queries.p, P.queries.data(), P.queries.size() * sizeof(BoolQuery), cudaMemcpyHostToDevice, ix->stream));
+    SA_CUDA(cudaMemcpyAsync(S.d_out_index.p, identity.data(), (size_t)n_queries * sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
+    u32 *d_ovf = (u32 *)(S.d_keys.as<u64>() + nk);
+    SA_CUDA(cudaMemsetAsync(d_ovf, 0, (size_t)n_queries * sizeof(u32), ix->stream));
+    for (size_t i = 0; i + 1 < P.group_start.size(); i++)
+        if ((rc = bool_run_group(ix, S, P, clause_terms, clause_term_starts, slop, bm25, k, slots, P.group_start[i],
+                                 P.group_start[i + 1]))) return rc;
+
+    // keys and overflow flags in one copy and one synchronise; a query whose tile overflowed is re-run alone with a
+    // slot per doc of the tile, which cannot overflow
+    SA_CUDA(cudaMemcpyAsync(ix->h_pinned.p, S.d_keys.p, key_bytes, cudaMemcpyDeviceToHost, ix->stream));
+    SA_CUDA(cudaStreamSynchronize(ix->stream));
+    std::vector<u32> ovf(n_queries);
+    memcpy(ovf.data(), ix->h_pinned.as<const u64>() + nk, (size_t)n_queries * sizeof(u32));
+    sa_unpack_keys(ix->h_pinned.as<const u64>(), nk, out_docs, out_scores);
+    u32 redone = 0;
+    for (u32 q = 0; q < n_queries; q++) {
+        if (!ovf[q]) continue;
+        SA_CUDA(cudaMemsetAsync(d_ovf + q, 0, sizeof(u32), ix->stream));
+        if ((rc = bool_run_group(ix, S, P, clause_terms, clause_term_starts, slop, bm25, k, SA_TILE_DOCS, q, q + 1))) return rc;
+        SA_CUDA(cudaMemcpyAsync(ix->h_pinned.p, S.d_keys.as<u64>() + (size_t)q * k, k * sizeof(u64), cudaMemcpyDeviceToHost,
+                                ix->stream));
+        SA_CUDA(cudaStreamSynchronize(ix->stream));
+        sa_unpack_keys(ix->h_pinned.as<const u64>(), k, out_docs + (size_t)q * k, out_scores + (size_t)q * k);
+        redone++;
+    }
+    if (n_redone) *n_redone = redone;
+    return SA_OK;
+}

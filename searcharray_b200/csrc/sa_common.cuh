@@ -170,6 +170,8 @@ struct BatchState;
 struct ViewState;
 struct BatchStateDelete { void operator()(BatchState *b) const; };   // sa_index.cu
 struct ViewStateDelete { void operator()(ViewState *v) const; };     // sa_view.cu
+struct BoolState;
+struct BoolStateDelete { void operator()(BoolState *s) const; };     // sa_bool.cu
 struct sa_index {
     ~sa_index();
     int device = 0;
@@ -220,6 +222,7 @@ struct sa_index {
     std::vector<cudaEvent_t> free_events;
     std::unique_ptr<BatchState, BatchStateDelete> batch;
     std::unique_ptr<ViewState, ViewStateDelete> view;   // buffers of sa_score_batch_topk_sim (sa_view.cu)
+    std::unique_ptr<BoolState, BoolStateDelete> boolq;  // buffers of sa_score_batch_topk_bool (sa_bool.cu)
     sa_stats stats;
     std::mutex mu;
 

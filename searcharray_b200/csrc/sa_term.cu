@@ -41,10 +41,6 @@ __device__ __forceinline__ bool payload_keep(u64 w, u64 lo, u64 hi) {
     return v >= lo && v <= hi;
 }
 
-__device__ __forceinline__ float bm25_from_norm(float tf, float norm, float idf) {
-    return __fmul_rn(__fdiv_rn(tf, __fadd_rn(tf, norm)), idf);
-}
-
 template <int MODE, bool ALL_DOCS, bool FILTER>
 __global__ void __launch_bounds__(SA_TERM_THREADS, 6)
 term_tile_kernel(const TermBatchArgs a) {

@@ -217,6 +217,11 @@ inline TermBatchArgs make_term_args(sa_index *ix, const TermQuery *d_queries, co
 }
 
 #ifdef __CUDACC__
+// BM25 of tf from the doc's cached length norm (sa_ensure_norm): the last two rounded operations of bm25_one
+__device__ __forceinline__ float bm25_from_norm(float tf, float norm, float idf) {
+    return __fmul_rn(__fdiv_rn(tf, __fadd_rn(tf, norm)), idf);
+}
+
 // The j-th round of "take the warp maximum, then clear it" (REDUX.MAX: one instruction per round on sm_80+).
 // Exactly ONE lane gives up its value per round, so equal values are counted with their multiplicity: BM25
 // scores are a function of (tf, doc length) only and repeat a lot -- collapsing duplicates used to leave fewer

@@ -501,7 +501,15 @@ class SearchArray(ExtensionArray):
         callable raises TypeError.  Under the last three the result is, bit for bit, the top k of
         `.score(q, similarity=similarity, slop=slop)` on the same array or view, and the scores have its dtype
         (float32 for bm25_impact, float64 for the other two, also where .score returns float32 zeros because
-        avg_doc_length is 0); +inf ranks, NaN never does."""
+        avg_doc_length is 0); +inf ranks, NaN never does.
+
+        queries may also hold boolean queries (query.Or / query.And), mixed freely with the others: per boolean query
+        the top k of s = .score(c0) + .score(c1) + ... (float32, clause order) over the docs where s > 0 and at least
+        mm clauses score > 0 (sa_score_batch_topk_bool).  They run on the whole array under bm25_similarity only: on
+        a view they raise NotImplementedError, under another similarity TypeError."""
+        from .query import Or
+        if any(isinstance(q, Or) for q in queries):
+            return self._search_topk_mixed(list(queries), k, similarity, slop)
         if not isinstance(similarity, (Bm25Similarity, Bm25Impact, Bm25Legacy, ClassicSimilarity)):
             raise TypeError("search_topk supports bm25_similarity, bm25_impact, bm25_legacy_similarity and "
                             f"classic_similarity, not {similarity!r}")
@@ -518,6 +526,44 @@ class SearchArray(ExtensionArray):
                                                       self.avg_doc_length, similarity.k1, similarity.b, k,
                                                       _lib.p_u32(docs), _lib.p_f32(scores)))
         return docs, scores
+
+    def _search_topk_mixed(self, queries, k, similarity, slop):
+        """search_topk of a batch holding boolean queries: the plain ones through search_topk as before, the boolean
+        ones through sa_score_batch_topk_bool, each clause with the idf .score gives it; results in query order."""
+        from .query import Or
+        if self.rows is not None:
+            raise NotImplementedError("boolean queries on a view (arr[mask]) are not supported yet; "
+                                      "compose .score() on the view")
+        if not isinstance(similarity, Bm25Similarity):
+            raise TypeError(f"boolean queries support bm25_similarity only, not {similarity!r}")
+        is_bool = np.asarray([isinstance(q, Or) for q in queries], dtype=bool)
+        docs = np.empty((len(queries), k), dtype=np.uint32)
+        scores = np.empty((len(queries), k), dtype=np.float32)
+        plain = [q for q, b in zip(queries, is_bool) if not b]
+        if plain:
+            docs[~is_bool], scores[~is_bool] = self.search_topk(plain, k=k, similarity=similarity, slop=slop)
+        bq = [q for q in queries if isinstance(q, Or)]
+        bdocs, bscores, _ = self._search_topk_bool(bq, k, similarity, slop)
+        docs[is_bool], scores[is_bool] = bdocs, bscores
+        return docs, scores
+
+    def _search_topk_bool(self, queries, k, similarity, slop):
+        """Boolean queries through sa_score_batch_topk_bool: (docs, scores, queries re-run exactly)."""
+        from .query import flatten
+        clauses, q_starts, mm = flatten(queries)
+        dev = self._device()
+        docs = np.empty((len(queries), k), dtype=np.uint32)
+        scores = np.empty((len(queries), k), dtype=np.float32)
+        n_redone = ctypes.c_uint32(0)
+        terms, c_starts, idfs = self._topk_queries(clauses, lambda dfs: compute_idf(self.corpus_size, dfs))
+        idfs = np.asarray(idfs, dtype=np.float32)
+        with self._shared["lock"]:
+            self._apply_rows(dev)
+            _lib.check(_lib.lib().sa_score_batch_topk_bool(
+                dev.handle, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
+                _lib.p_u32(mm), len(queries), int(slop), self.avg_doc_length, similarity.k1, similarity.b, k,
+                _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
+        return docs, scores, n_redone.value
 
     def _topk_queries(self, queries, idf):
         """The queries as the batched top-k entries take them: term ids, start offsets and, per query, idf(dfs) of
