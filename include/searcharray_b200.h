@@ -164,6 +164,23 @@ int sa_score_batch_topk_bool(sa_index *index, const uint32_t *query_clause_start
                              const uint32_t *clause_term_starts, const float *clause_idf, const uint32_t *mm,
                              uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
+/* Boolean queries with clause roles and per-clause weights (Lucene's MUST / SHOULD / FILTER / MUST_NOT): the
+ * arguments of sa_score_batch_topk_bool plus, per clause, clause_weight[c] (finite, >= 0) and clause_occur[c] (one of
+ * SA_OCCUR_*).  Per query, over its MUST and SHOULD clauses in clause order, s = w0 * score(c0), then
+ * s = s + w1 * score(c1), ..., every product and sum rounded to float32 (no fused multiply-add).  A doc ranks iff
+ * s > 0, at least mm[q] (<= its SHOULD clauses) SHOULD clauses score > 0 there (unweighted: a weight of 0 still
+ * matches), every MUST and FILTER clause scores > 0 there, and no MUST_NOT clause does.  FILTER and MUST_NOT clauses
+ * add nothing to s.  Every clause, whatever its role, is scored exactly as in sa_score_batch_topk_bool, with its own
+ * idf.  With every clause SHOULD and weight 1 the result equals sa_score_batch_topk_bool's, bit for bit. */
+#define SA_OCCUR_SHOULD 0
+#define SA_OCCUR_MUST 1
+#define SA_OCCUR_FILTER 2
+#define SA_OCCUR_MUST_NOT 3
+int sa_score_batch_topk_bool_occur(sa_index *index, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
+                                   const uint32_t *clause_term_starts, const float *clause_idf,
+                                   const float *clause_weight, const uint8_t *clause_occur, const uint32_t *mm,
+                                   uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
+                                   uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
 
 /* The same batch in three stages, so a serving loop (or the benchmark) can keep the query
  * descriptors resident and time the device work alone: upload (H2D of descriptors), execute

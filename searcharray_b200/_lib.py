@@ -17,6 +17,7 @@ ALL_BITS = 0xFFFFFFFFFFFFFFFF
 
 c_u64, c_u32, c_f32, c_int = ctypes.c_uint64, ctypes.c_uint32, ctypes.c_float, ctypes.c_int
 P_u64, P_u32, P_f32 = ctypes.POINTER(c_u64), ctypes.POINTER(c_u32), ctypes.POINTER(c_f32)
+P_u8 = ctypes.POINTER(ctypes.c_uint8)
 P_void = ctypes.c_void_p
 
 
@@ -55,6 +56,8 @@ SIGNATURES = {
                                         ctypes.POINTER(ctypes.c_double)]),
     "sa_score_batch_topk_bool": (c_int, [P_void, P_u32, P_u32, P_u32, P_f32, P_u32, c_u32, c_u32, c_f32, c_f32, c_f32,
                                          c_u32, P_u32, P_f32, P_u32]),
+    "sa_score_batch_topk_bool_occur": (c_int, [P_void, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8, P_u32, c_u32, c_u32,
+                                               c_f32, c_f32, c_f32, c_u32, P_u32, P_f32, P_u32]),
     "sa_batch_upload": (c_int, [P_void, P_u32, P_u32, P_f32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32]),
     "sa_batch_execute": (c_int, [P_void]),
     "sa_batch_download": (c_int, [P_void, P_u32, P_f32, P_u32]),
@@ -144,3 +147,7 @@ def p_u32(a):
 
 def p_f32(a):
     return a.ctypes.data_as(P_f32)
+
+
+def p_u8(a):
+    return a.ctypes.data_as(P_u8)

@@ -17,6 +17,12 @@
 // have anything in the tile; fewer than mm -> no doc of the tile can rank, and the tile is published empty.
 // Then the docs below mm are zeroed and the tile goes through flush_tile_collect, the float32 collector of every
 // other path, and topk_select_kernel ranks the candidates.
+//
+// bool_tile_kernel<true> (sa_score_batch_topk_bool_occur) adds Lucene's clause roles and per-clause weights, from a
+// separate BoolOccur array: MUST / SHOULD clauses add weight * score, only SHOULD clauses count towards mm, and two
+// per-thread masks over the thread's 32 docs record where a MUST / FILTER clause misses (`req`) and where a MUST_NOT
+// clause matches (`veto`).  A tile where a MUST / FILTER clause has no doc, or with fewer SHOULD clauses than mm, is
+// published empty before the fold.
 #include "sa_term.cuh"
 #include "sa_phrase.cuh"
 
@@ -44,8 +50,16 @@ struct BoolArgs {
     TopkCtx topk;
 };
 
+// A clause's role and weight (sa_score_batch_topk_bool_occur), read by bool_tile_kernel<true> only, so the plain
+// instance's loads stay those of BoolClause.
+struct BoolOccur {
+    float weight;   // MUST / SHOULD: s += weight * score (rounded once, then added)
+    u32 occur;      // SA_OCCUR_*
+};
+
 struct BoolState {
     DevBuf d_clauses, d_queries, d_out_index;
+    DevBuf d_occur;
     DevBuf d_keys;       // nq * k result keys, then u32 overflow[nq]: one device-to-host copy
     DevBuf rows;
 };
@@ -83,8 +97,24 @@ __device__ __forceinline__ void bool_scatter_term(const BoolArgs &a, const BoolC
     }
 }
 
+// bool_tile_kernel<true>: doc i = 4 j + e of the thread's 32 gets the clause's exact score v.  MUST / SHOULD add
+// weight * v, each product rounded before the add as numpy rounds it (no FMA contraction); only SHOULD counts a hit,
+// on the unweighted v, so a zero weight still matches; MUST / FILTER clear the doc's `req` bit where v is not > 0;
+// MUST_NOT sets its `veto` bit where v > 0.  The occur tests are clause-uniform branches, which skip the work of the
+// other roles (a branch-free select form measured slower).
+__device__ __forceinline__ void bool_fold_occur(float &acc, u32 &hits, u32 &req, u32 &veto, int i, float v,
+                                                const BoolOccur &oc) {
+    if (oc.occur == SA_OCCUR_SHOULD || oc.occur == SA_OCCUR_MUST) acc = __fadd_rn(acc, __fmul_rn(oc.weight, v));
+    if (oc.occur == SA_OCCUR_SHOULD) hits += (v > 0.0f ? 1u : 0u) << (8 * (i & 3));
+    if ((oc.occur == SA_OCCUR_MUST || oc.occur == SA_OCCUR_FILTER) && !(v > 0.0f)) req &= ~(1u << i);
+    if (oc.occur == SA_OCCUR_MUST_NOT && v > 0.0f) veto |= 1u << i;
+}
+
+// OCCUR = false: Or / And (every clause SHOULD, weight 1).  OCCUR = true: per-clause roles and weights in occ[],
+// indexed as a.clauses; a query's mm counts its SHOULD clauses.
+template <bool OCCUR>
 __global__ void __launch_bounds__(SA_TERM_THREADS)
-bool_tile_kernel(const BoolArgs a) {
+bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ) {
     constexpr int PER = SA_TILE_DOCS / SA_TERM_THREADS / 4;        // float4 groups per thread
     __shared__ __align__(16) float s_tile[SA_TILE_DOCS];
     __shared__ u32 s_lo[SA_BOOL_MAX_CLAUSES], s_hi[SA_BOOL_MAX_CLAUSES];
@@ -120,12 +150,21 @@ bool_tile_kernel(const BoolArgs a) {
         if (lane == 0) {
             s_lo[c] = lo;
             s_hi[c] = hi;
-            if (hi > lo) atomicAdd(&s_present, 1u);
+            if (OCCUR) {
+                // low 16 bits: SHOULD clauses present; high bits: MUST / FILTER clauses absent (<= 64 clauses)
+                const u32 o = occ[bq.c0 + c].occur;
+                const u32 add = o == SA_OCCUR_SHOULD ? (hi > lo ? 1u : 0u)
+                              : (o == SA_OCCUR_MUST || o == SA_OCCUR_FILTER) && hi <= lo ? 1u << 16 : 0u;
+                if (add) atomicAdd(&s_present, add);
+            } else if (hi > lo) {
+                atomicAdd(&s_present, 1u);
+            }
         }
     }
     __syncthreads();
-    // 2. a clause with nothing in the tile scores > 0 at no doc of it: fewer such clauses than mm, nothing ranks
-    if (s_present < bq.mm) {                                        // CTA-uniform
+    // 2. a clause with nothing in the tile scores > 0 at no doc of it: fewer such clauses than mm, nothing ranks;
+    //    nor does anything where a MUST / FILTER clause is absent
+    if (OCCUR ? ((s_present & 0xFFFFu) < bq.mm || (s_present >> 16) != 0) : s_present < bq.mm) {   // CTA-uniform
         if (tid == 0) {
             const u64 t_idx = (u64)q * a.topk.n_tiles + tile;
             a.topk.tile_cnt[t_idx] = 0;
@@ -141,11 +180,15 @@ bool_tile_kernel(const BoolArgs a) {
     for (int i = 0; i < PER * 4; i++) acc[i] = 0.0f;
 #pragma unroll
     for (int j = 0; j < PER; j++) hits[j] = 0;
+    u32 req = ~0u, veto = 0;               // OCCUR: bit 4 j + e of the thread's docs (PER * 4 == 32)
+    static_assert(PER * 4 == 32, "one u32 mask bit per owned doc");
     Bm25Params p = a.bm25;
     for (u32 c = 0; c < bq.n; c++) {
         const BoolClause cl = a.clauses[bq.c0 + c];
         const u32 lo = s_lo[c], hi = s_hi[c];
         if (cl.sparse && hi <= lo) continue;                        // CTA-uniform: +0 at every doc of the tile
+        BoolOccur oc{1.0f, SA_OCCUR_SHOULD};
+        if (OCCUR) oc = occ[bq.c0 + c];
         p.idf = cl.idf;
         if (cl.row != SA_BOOL_NO_ROW) {
             // phrase clause (sparse-safe parameters only): BM25 of its counts, zero counts score +0
@@ -160,8 +203,12 @@ bool_tile_kernel(const BoolArgs a) {
                     const u64 d = (u64)tile_doc0 + g * 4 + e;
                     float v = 0.0f;
                     if (xs[e] > 0.0f && d < a.n_docs) v = bm25_from_norm(xs[e], __ldg(a.norm + d), cl.idf);
-                    acc[j * 4 + e] = __fadd_rn(acc[j * 4 + e], v);
-                    hits[j] += (v > 0.0f ? 1u : 0u) << (8 * e);
+                    if (OCCUR) {
+                        bool_fold_occur(acc[j * 4 + e], hits[j], req, veto, j * 4 + e, v, oc);
+                    } else {
+                        acc[j * 4 + e] = __fadd_rn(acc[j * 4 + e], v);
+                        hits[j] += (v > 0.0f ? 1u : 0u) << (8 * e);
+                    }
                 }
             }
         } else {
@@ -179,15 +226,21 @@ bool_tile_kernel(const BoolArgs a) {
                     float v = xs[e];
                     // bm25.pyx:20-25 over every doc (NaN / inf / -0.0 of exotic parameters)
                     if (!cl.sparse) v = d < a.n_docs ? bm25_one(xs[e], __ldg(a.doc_lens + d), p) : 0.0f;
-                    acc[j * 4 + e] = __fadd_rn(acc[j * 4 + e], v);
-                    hits[j] += (v > 0.0f ? 1u : 0u) << (8 * e);
+                    if (OCCUR) {
+                        bool_fold_occur(acc[j * 4 + e], hits[j], req, veto, j * 4 + e, v, oc);
+                    } else {
+                        acc[j * 4 + e] = __fadd_rn(acc[j * 4 + e], v);
+                        hits[j] += (v > 0.0f ? 1u : 0u) << (8 * e);
+                    }
                 }
             }
             __syncthreads();
         }
     }
 
-    // 4. docs with fewer than mm hits (or a sum <= 0 / NaN) do not rank; collect the tile's top-k candidates
+    // 4. docs with fewer than mm hits (or a sum <= 0 / NaN), and under OCCUR docs a MUST / FILTER clause misses or a
+    //    MUST_NOT clause matches, do not rank; collect the tile's top-k candidates
+    const u32 keep = req & ~veto;
     u32 my_max = 0;
 #pragma unroll
     for (int j = 0; j < PER; j++) {
@@ -195,7 +248,8 @@ bool_tile_kernel(const BoolArgs a) {
 #pragma unroll
         for (int e = 0; e < 4; e++) {
             const float s = acc[j * 4 + e];
-            o[e] = (((hits[j] >> (8 * e)) & 0xFFu) >= bq.mm && s > 0.0f) ? s : 0.0f;
+            const bool ok = OCCUR ? ((keep >> (j * 4 + e)) & 1u) != 0 : true;
+            o[e] = (ok && ((hits[j] >> (8 * e)) & 0xFFu) >= bq.mm && s > 0.0f) ? s : 0.0f;
             my_max = max(my_max, __float_as_uint(o[e]));
         }
         s_tile4[tid + j * SA_TERM_THREADS] = make_float4(o[0], o[1], o[2], o[3]);
@@ -210,6 +264,7 @@ struct BoolPlan {
     std::vector<BoolClause> clauses;
     std::vector<BoolQuery> queries;
     std::vector<u32> group_start;       // queries [group_start[i], group_start[i + 1]) share one launch and its rows
+    std::vector<BoolOccur> occur;       // per clause, as clauses; empty: Or / And (bool_tile_kernel<false>)
     u32 max_group = 1, max_rows = 0;
     bool any_sparse = false;
 };
@@ -261,18 +316,20 @@ int bool_run_group(sa_index *ix, BoolState &S, const BoolPlan &P, const uint32_t
     a.queries = S.d_queries.as<BoolQuery>() + q0;
     a.bm25 = bm25;
     a.topk = t;
-    bool_tile_kernel<<<dim3(nq, n_tiles), SA_TERM_THREADS, 0, ix->stream>>>(a);
+    if (P.occur.empty())
+        bool_tile_kernel<false><<<dim3(nq, n_tiles), SA_TERM_THREADS, 0, ix->stream>>>(a, nullptr);
+    else
+        bool_tile_kernel<true><<<dim3(nq, n_tiles), SA_TERM_THREADS, 0, ix->stream>>>(a, S.d_occur.as<BoolOccur>());
     SA_CUDA(cudaGetLastError());
     ix->stats.total_launches++;
     return launch_topk_select(ix, t, nq, ix->doc_base, d_keys, S.d_out_index.as<u32>() + q0);
 }
 
-}  // namespace
-
-extern "C" int sa_score_batch_topk_bool(sa_index *ix, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
-                                        const uint32_t *clause_term_starts, const float *clause_idf, const uint32_t *mm,
-                                        uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
-                                        uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+// Both entry points.  clause_weight / clause_occur NULL: Or / And, every clause SHOULD with weight 1, mm over all.
+int bool_topk(sa_index *ix, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
+              const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
+              const uint8_t *clause_occur, const uint32_t *mm, uint32_t n_queries, uint32_t slop, float avg_doc_len,
+              float k1, float b, uint32_t k, uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
     SA_CHECK(ix && out_docs && out_scores, "NULL argument");
     SA_CHECK(n_queries == 0 || (query_clause_starts && clause_terms && clause_term_starts && clause_idf && mm),
              "NULL argument");
@@ -281,12 +338,24 @@ extern "C" int sa_score_batch_topk_bool(sa_index *ix, const uint32_t *query_clau
     std::lock_guard<std::mutex> g(ix->mu);
     SA_CUDA(cudaSetDevice(ix->device));
     int rc;
+    const bool occur = clause_occur != nullptr;
     SA_CHECK(n_queries == 0 || query_clause_starts[0] == 0, "query_clause_starts[0] must be 0");
     for (u32 q = 0; q < n_queries; q++) {
         SA_CHECK(query_clause_starts[q + 1] > query_clause_starts[q] &&
                  query_clause_starts[q + 1] - query_clause_starts[q] <= SA_BOOL_MAX_CLAUSES,
                  "query %u: a boolean query has 1 to %d clauses", q, SA_BOOL_MAX_CLAUSES);
-        SA_CHECK(mm[q] <= query_clause_starts[q + 1] - query_clause_starts[q], "query %u: mm exceeds its clauses", q);
+        u32 n_should = query_clause_starts[q + 1] - query_clause_starts[q];
+        if (occur) {
+            n_should = 0;
+            for (u32 c = query_clause_starts[q]; c < query_clause_starts[q + 1]; c++) {
+                SA_CHECK(clause_occur[c] <= SA_OCCUR_MUST_NOT, "clause %u: occur %u is not an SA_OCCUR_* value", c,
+                         (unsigned)clause_occur[c]);
+                SA_CHECK(std::isfinite(clause_weight[c]) && clause_weight[c] >= 0.0f,
+                         "clause %u: a weight is finite and >= 0", c);
+                n_should += clause_occur[c] == SA_OCCUR_SHOULD;
+            }
+        }
+        SA_CHECK(mm[q] <= n_should, "query %u: mm exceeds its %sclauses", q, occur ? "SHOULD " : "");
     }
     const u32 c_begin = n_queries ? query_clause_starts[0] : 0, c_end = n_queries ? query_clause_starts[n_queries] : 0;
     for (u32 c = c_begin; c < c_end; c++) {
@@ -326,6 +395,7 @@ extern "C" int sa_score_batch_topk_bool(sa_index *ix, const uint32_t *query_clau
             const TermQuery tq = make_term_query(ix, nt == 1 ? tids[0] : SA_NO_TERM, clause_idf[c]);
             P.clauses.push_back(BoolClause{tq.word_off, tq.n_words, tq.dir_off, tq.rec_off, clause_idf[c],
                                            nt == 1 ? SA_BOOL_NO_ROW : rows++, sparse ? 1u : 0u, 0});
+            if (occur) P.occur.push_back(BoolOccur{clause_weight[c], clause_occur[c]});
             P.any_sparse = P.any_sparse || sparse;
         }
         P.max_group = std::max(P.max_group, q + 1 - P.group_start.back());
@@ -340,12 +410,16 @@ extern "C" int sa_score_batch_topk_bool(sa_index *ix, const uint32_t *query_clau
         (rc = S.d_queries.reserve(P.queries.size() * sizeof(BoolQuery))) ||
         (rc = S.d_out_index.reserve((size_t)n_queries * sizeof(u32))) || (rc = S.d_keys.reserve(key_bytes)) ||
         (rc = S.rows.reserve(std::max<size_t>((size_t)P.max_rows * stride * sizeof(float), 64))) ||
+        (rc = S.d_occur.reserve(P.occur.size() * sizeof(BoolOccur))) ||
         (rc = ix->h_pinned.reserve(key_bytes)))
         return rc;
     if (P.any_sparse && (rc = sa_ensure_norm(ix, k1, b, avg_doc_len))) return rc;
     std::vector<u32> identity(n_queries);
     for (u32 q = 0; q < n_queries; q++) identity[q] = q;
     SA_CUDA(cudaMemcpyAsync(S.d_clauses.p, P.clauses.data(), P.clauses.size() * sizeof(BoolClause), cudaMemcpyHostToDevice, ix->stream));
+    if (occur) {
+        SA_CUDA(cudaMemcpyAsync(S.d_occur.p, P.occur.data(), P.occur.size() * sizeof(BoolOccur), cudaMemcpyHostToDevice, ix->stream));
+    }
     SA_CUDA(cudaMemcpyAsync(S.d_queries.p, P.queries.data(), P.queries.size() * sizeof(BoolQuery), cudaMemcpyHostToDevice, ix->stream));
     SA_CUDA(cudaMemcpyAsync(S.d_out_index.p, identity.data(), (size_t)n_queries * sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
     u32 *d_ovf = (u32 *)(S.d_keys.as<u64>() + nk);
@@ -374,4 +448,25 @@ extern "C" int sa_score_batch_topk_bool(sa_index *ix, const uint32_t *query_clau
     }
     if (n_redone) *n_redone = redone;
     return SA_OK;
+}
+
+}  // namespace
+
+extern "C" int sa_score_batch_topk_bool(sa_index *ix, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
+                                        const uint32_t *clause_term_starts, const float *clause_idf, const uint32_t *mm,
+                                        uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
+                                        uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+    return bool_topk(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, nullptr, nullptr, mm,
+                     n_queries, slop, avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
+}
+
+extern "C" int sa_score_batch_topk_bool_occur(sa_index *ix, const uint32_t *query_clause_starts,
+                                              const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                              const float *clause_idf, const float *clause_weight,
+                                              const uint8_t *clause_occur, const uint32_t *mm, uint32_t n_queries,
+                                              uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
+                                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+    SA_CHECK(n_queries == 0 || (clause_weight && clause_occur), "NULL argument");
+    return bool_topk(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, clause_weight,
+                     clause_occur, mm, n_queries, slop, avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
 }

@@ -506,9 +506,14 @@ class SearchArray(ExtensionArray):
         queries may also hold boolean queries (query.Or / query.And), mixed freely with the others: per boolean query
         the top k of s = .score(c0) + .score(c1) + ... (float32, clause order) over the docs where s > 0 and at least
         mm clauses score > 0 (sa_score_batch_topk_bool).  They run on the whole array under bm25_similarity only: on
-        a view they raise NotImplementedError, under another similarity TypeError."""
-        from .query import Or
-        if any(isinstance(q, Or) for q in queries):
+        a view they raise NotImplementedError, under another similarity TypeError.
+
+        query.Bool(must, should, filter, must_not, mm) and query.Boost(clause, weight) clauses are accepted the same
+        way: s = w0 * .score(c0) + w1 * .score(c1) + ... over must + should (float32, each product rounded), ranked
+        where s > 0, every must and filter clause scores > 0, no must_not clause does and at least mm should clauses
+        do (sa_score_batch_topk_bool_occur).  An Or / And whose weights are all 1 takes the path above unchanged."""
+        from .query import is_boolean
+        if any(is_boolean(q) for q in queries):
             return self._search_topk_mixed(list(queries), k, similarity, slop)
         if not isinstance(similarity, (Bm25Similarity, Bm25Impact, Bm25Legacy, ClassicSimilarity)):
             raise TypeError("search_topk supports bm25_similarity, bm25_impact, bm25_legacy_similarity and "
@@ -529,28 +534,37 @@ class SearchArray(ExtensionArray):
 
     def _search_topk_mixed(self, queries, k, similarity, slop):
         """search_topk of a batch holding boolean queries: the plain ones through search_topk as before, the boolean
-        ones through sa_score_batch_topk_bool, each clause with the idf .score gives it; results in query order."""
-        from .query import Or
+        ones through sa_score_batch_topk_bool (Or / And with weights 1) or sa_score_batch_topk_bool_occur (Bool,
+        boosted Or / And), each clause with the idf .score gives it; results in query order."""
+        from .query import is_boolean, needs_occur
         if self.rows is not None:
             raise NotImplementedError("boolean queries on a view (arr[mask]) are not supported yet; "
                                       "compose .score() on the view")
         if not isinstance(similarity, Bm25Similarity):
             raise TypeError(f"boolean queries support bm25_similarity only, not {similarity!r}")
-        is_bool = np.asarray([isinstance(q, Or) for q in queries], dtype=bool)
+        kind = np.asarray([(needs_occur(q) + 1) if is_boolean(q) else 0 for q in queries])   # plain, Or, occur
         docs = np.empty((len(queries), k), dtype=np.uint32)
         scores = np.empty((len(queries), k), dtype=np.float32)
-        plain = [q for q, b in zip(queries, is_bool) if not b]
-        if plain:
-            docs[~is_bool], scores[~is_bool] = self.search_topk(plain, k=k, similarity=similarity, slop=slop)
-        bq = [q for q in queries if isinstance(q, Or)]
-        bdocs, bscores, _ = self._search_topk_bool(bq, k, similarity, slop)
-        docs[is_bool], scores[is_bool] = bdocs, bscores
+        for kd in (0, 1, 2):
+            sel = kind == kd
+            part = [q for q, s in zip(queries, sel) if s]
+            if not part:
+                continue
+            if kd == 0:
+                docs[sel], scores[sel] = self.search_topk(part, k=k, similarity=similarity, slop=slop)
+            else:
+                docs[sel], scores[sel], _ = self._search_topk_bool(part, k, similarity, slop)
         return docs, scores
 
     def _search_topk_bool(self, queries, k, similarity, slop):
-        """Boolean queries through sa_score_batch_topk_bool: (docs, scores, queries re-run exactly)."""
-        from .query import flatten
-        clauses, q_starts, mm = flatten(queries)
+        """Boolean queries through sa_score_batch_topk_bool, or through sa_score_batch_topk_bool_occur when one of
+        them is a Bool or has a weight other than 1: (docs, scores, queries re-run exactly)."""
+        from .query import flatten, flatten_occur, needs_occur
+        occur = any(needs_occur(q) for q in queries)
+        if occur:
+            clauses, q_starts, mm, weights, occurs = flatten_occur(queries)
+        else:
+            clauses, q_starts, mm = flatten(queries)
         dev = self._device()
         docs = np.empty((len(queries), k), dtype=np.uint32)
         scores = np.empty((len(queries), k), dtype=np.float32)
@@ -559,10 +573,17 @@ class SearchArray(ExtensionArray):
         idfs = np.asarray(idfs, dtype=np.float32)
         with self._shared["lock"]:
             self._apply_rows(dev)
-            _lib.check(_lib.lib().sa_score_batch_topk_bool(
-                dev.handle, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
-                _lib.p_u32(mm), len(queries), int(slop), self.avg_doc_length, similarity.k1, similarity.b, k,
-                _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
+            if occur:
+                _lib.check(_lib.lib().sa_score_batch_topk_bool_occur(
+                    dev.handle, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
+                    _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(mm), len(queries), int(slop),
+                    self.avg_doc_length, similarity.k1, similarity.b, k, _lib.p_u32(docs), _lib.p_f32(scores),
+                    ctypes.byref(n_redone)))
+            else:
+                _lib.check(_lib.lib().sa_score_batch_topk_bool(
+                    dev.handle, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
+                    _lib.p_u32(mm), len(queries), int(slop), self.avg_doc_length, similarity.k1, similarity.b, k,
+                    _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
         return docs, scores, n_redone.value
 
     def _topk_queries(self, queries, idf):

@@ -1,9 +1,12 @@
-"""Boolean queries for SearchArray.search_topk: OR / AND / min-should-match over term and phrase clauses.
+"""Boolean queries for SearchArray.search_topk: OR / AND / min-should-match over term and phrase clauses, and
+Lucene-style required / optional / filter / prohibited clauses with per-clause boosts.
 
 Or(clauses, mm) ranks, per doc, s = score(c0) + score(c1) + ... (float32, folded left in clause order) among the docs
 where at least mm clauses score > 0 -- the reference's own composition of multi-clause queries
 (test/test_search.py:126-226) -- and search_topk returns the top k of it by (score desc, doc asc), computed on the
-device (sa_score_batch_topk_bool)."""
+device (sa_score_batch_topk_bool).  Bool(must, should, filter, must_not, mm) and Boost(clause, weight) extend that
+composition (sa_score_batch_topk_bool_occur)."""
+import math
 from typing import List, Union
 
 import numpy as np
@@ -11,35 +14,79 @@ import numpy as np
 from .solr import parse_min_should_match
 
 SA_BOOL_MAX_CLAUSES = 64          # include/searcharray_b200.h
+SA_OCCUR_SHOULD, SA_OCCUR_MUST, SA_OCCUR_FILTER, SA_OCCUR_MUST_NOT = 0, 1, 2, 3
 
 Clause = Union[str, List[str]]
+
+
+def _clause(c):
+    """A clause as search_topk's query form: str (term) or list[str] (phrase); anything else is a TypeError."""
+    if isinstance(c, str):
+        return c
+    if isinstance(c, (list, tuple)) and c and all(isinstance(t, str) for t in c):
+        return list(c)
+    raise TypeError(f"a clause is a str (term) or a non-empty list of str (phrase), not {c!r}")
+
+
+class Boost:
+    """A term or phrase clause whose score is multiplied by `weight` (Lucene's `title^2`) before it is added:
+    s = s + float32(weight) * score(clause), the product rounded to float32.  `weight` is finite and >= 0 and is
+    rounded to float32 once.  A doc still counts as matched by the clause where its unweighted score is > 0, so a
+    weight of 0 matches without scoring.  Accepted where a clause scores: in Or, And, Bool's must and should."""
+
+    def __init__(self, clause, weight):
+        self.clause = _clause(clause)
+        w = float(weight)
+        if not math.isfinite(w) or w < 0:
+            raise ValueError(f"a boost is finite and >= 0, not {weight!r}")
+        self.weight = np.float32(w)
+
+    def __repr__(self):
+        return f"Boost({self.clause!r}, {float(self.weight)!r})"
+
+
+def _scoring(clauses):
+    """(clauses, float32 weights) of a list of clauses and Boosts."""
+    out, weights = [], []
+    for c in clauses:
+        if isinstance(c, Boost):
+            out.append(c.clause)
+            weights.append(c.weight)
+        else:
+            out.append(_clause(c))
+            weights.append(np.float32(1.0))
+    return out, weights
+
+
+def _check_count(n):
+    if n > SA_BOOL_MAX_CLAUSES:
+        raise ValueError(f"a boolean query has at most {SA_BOOL_MAX_CLAUSES} clauses, not {n}")
 
 
 class Or:
     """A query matching docs where at least `mm` of `clauses` score > 0, scored by the sum of the clauses' scores.
 
-    clauses: a str (a term) or a list[str] (a phrase, matched with search_topk's `slop`); duplicates count twice.
-    mm: an int or a Solr min-should-match spec ("2", "-1", "75%", "2<-25%"), clamped to [0, len(clauses)] as
-    edismax clamps it (solr.parse_min_should_match)."""
+    clauses: a str (a term), a list[str] (a phrase, matched with search_topk's `slop`) or a Boost of either;
+    duplicates count twice.  mm: an int or a Solr min-should-match spec ("2", "-1", "75%", "2<-25%"), clamped to
+    [0, len(clauses)] as edismax clamps it (solr.parse_min_should_match)."""
 
     def __init__(self, clauses, mm=1):
         clauses = list(clauses)
         if not clauses:
             raise ValueError("a boolean query needs at least one clause")
-        if len(clauses) > SA_BOOL_MAX_CLAUSES:
-            raise ValueError(f"a boolean query has at most {SA_BOOL_MAX_CLAUSES} clauses, not {len(clauses)}")
-        out = []
-        for c in clauses:
-            if isinstance(c, str):
-                out.append(c)
-            elif isinstance(c, (list, tuple)) and c and all(isinstance(t, str) for t in c):
-                out.append(list(c))
-            else:
-                raise TypeError(f"a clause is a str (term) or a non-empty list of str (phrase), not {c!r}")
-        self.clauses = out
-        self.mm = parse_min_should_match(len(out), str(mm))
+        _check_count(len(clauses))
+        self.clauses, self.weights = _scoring(clauses)
+        self.mm = parse_min_should_match(len(self.clauses), str(mm))
+
+    @property
+    def boosted(self):
+        """Whether any clause has a weight other than 1 (such a query takes sa_score_batch_topk_bool_occur)."""
+        return any(w != 1.0 for w in self.weights)
 
     def __repr__(self):
+        if self.boosted:
+            shown = [Boost(c, w) if w != 1.0 else c for c, w in zip(self.clauses, self.weights)]
+            return f"{type(self).__name__}({shown!r}, mm={self.mm})"
         return f"{type(self).__name__}({self.clauses!r}, mm={self.mm})"
 
 
@@ -51,6 +98,60 @@ class And(Or):
         super().__init__(clauses, mm=len(clauses))
 
 
+class Bool:
+    """Lucene's boolean query: a doc ranks iff every `must` and `filter` clause scores > 0 there, no `must_not`
+    clause does, at least `mm` of the `should` clauses do, and s > 0, where
+    s = w0 * score(c0) + w1 * score(c1) + ... over must + should in that order (float32, each product rounded, folded
+    left).  `filter` and `must_not` clauses add nothing to s and take no Boost.
+
+    mm counts `should` clauses only: an int or a Solr spec (solr.parse_min_should_match(len(should), str(mm))); by
+    default 0 when there are must or filter clauses, else 1.  At least one must or should clause is needed (without
+    one nothing can score > 0), and at most SA_BOOL_MAX_CLAUSES clauses in the four lists together."""
+
+    def __init__(self, must=(), should=(), filter=(), must_not=(), mm=None):
+        must, should, filter, must_not = list(must), list(should), list(filter), list(must_not)
+        for role, cs in (("filter", filter), ("must_not", must_not)):
+            for c in cs:
+                if isinstance(c, Boost):
+                    raise ValueError(f"a {role} clause adds nothing to the score and takes no Boost: {c!r}")
+        self.must, self.must_weights = _scoring(must)
+        self.should, self.should_weights = _scoring(should)
+        self.filter = [_clause(c) for c in filter]
+        self.must_not = [_clause(c) for c in must_not]
+        if not self.must and not self.should:
+            raise ValueError("a Bool query needs at least one must or should clause: nothing else scores")
+        _check_count(len(must) + len(should) + len(filter) + len(must_not))
+        if mm is None:
+            mm = 0 if (self.must or self.filter) else 1
+        self.mm = parse_min_should_match(len(self.should), str(mm))
+
+    def occur_clauses(self):
+        """(clauses, float32 weights, occurs) in the order the device folds them: must, should, filter, must_not."""
+        clauses = self.must + self.should + self.filter + self.must_not
+        one = np.float32(1.0)
+        weights = self.must_weights + self.should_weights + [one] * (len(self.filter) + len(self.must_not))
+        occurs = ([SA_OCCUR_MUST] * len(self.must) + [SA_OCCUR_SHOULD] * len(self.should) +
+                  [SA_OCCUR_FILTER] * len(self.filter) + [SA_OCCUR_MUST_NOT] * len(self.must_not))
+        return clauses, weights, occurs
+
+    def __repr__(self):
+        def shown(cs, ws):
+            return [Boost(c, w) if w != 1.0 else c for c, w in zip(cs, ws)]
+        return (f"Bool(must={shown(self.must, self.must_weights)!r}, "
+                f"should={shown(self.should, self.should_weights)!r}, filter={self.filter!r}, "
+                f"must_not={self.must_not!r}, mm={self.mm})")
+
+
+def is_boolean(q):
+    """Whether search_topk routes q to the boolean path."""
+    return isinstance(q, (Or, Bool))
+
+
+def needs_occur(q):
+    """Whether q takes sa_score_batch_topk_bool_occur: a Bool, or an Or / And with a weight other than 1."""
+    return isinstance(q, Bool) or q.boosted
+
+
 def flatten(queries):
     """Boolean queries as sa_score_batch_topk_bool takes them: (clause list in query order, query_clause_starts,
     mm), the clause list being search_topk's query form (str or list[str])."""
@@ -60,3 +161,22 @@ def flatten(queries):
         starts.append(len(clauses))
         mm.append(q.mm)
     return clauses, np.asarray(starts, dtype=np.uint32), np.asarray(mm, dtype=np.uint32)
+
+
+def flatten_occur(queries):
+    """Or / And / Bool queries as sa_score_batch_topk_bool_occur takes them: flatten's (clauses,
+    query_clause_starts, mm) and, per clause, float32 weights and uint8 SA_OCCUR_* roles.  An Or's clauses are all
+    SHOULD; a Bool's come as must, should, filter, must_not."""
+    clauses, starts, mm, weights, occurs = [], [0], [], [], []
+    for q in queries:
+        if isinstance(q, Bool):
+            cs, ws, os_ = q.occur_clauses()
+        else:
+            cs, ws, os_ = q.clauses, q.weights, [SA_OCCUR_SHOULD] * len(q.clauses)
+        clauses.extend(cs)
+        weights.extend(ws)
+        occurs.extend(os_)
+        starts.append(len(clauses))
+        mm.append(q.mm)
+    return (clauses, np.asarray(starts, dtype=np.uint32), np.asarray(mm, dtype=np.uint32),
+            np.asarray(weights, dtype=np.float32), np.asarray(occurs, dtype=np.uint8))

@@ -1,0 +1,23 @@
+"""Worker for tests/test_bool_occur_gpu.py: the Bool role checks in a process started with SA_NO_TF_TABLE=1, which
+the library reads once per process, so the long lists take the words path with a tile directory.  Prints OK when
+every check passes."""
+import os
+import sys
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+sys.path.insert(0, os.path.dirname(HERE))
+sys.path.insert(0, HERE)
+
+import test_bool_occur_gpu as occ  # noqa: E402
+from test_bool_topk_gpu import Synth  # noqa: E402
+
+
+def main():
+    assert os.environ.get("SA_NO_TF_TABLE") == "1"
+    synth = Synth()
+    occ.check_roles(synth.arr, synth.oracle(), "no tf table")
+    print("OK")
+
+
+if __name__ == "__main__":
+    main()
