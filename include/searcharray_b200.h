@@ -276,6 +276,20 @@ int sa_multi_add_phase(sa_multi *multi, uint32_t n_entries, const uint32_t *entr
 int sa_multi_download(sa_multi *multi, void *out, int as_float32);
 int sa_multi_is_float32(sa_multi *multi, int *out);
 int sa_multi_topk(sa_multi *multi, uint32_t k, uint32_t *out_docs, double *out_scores);
+/* Boolean queries over several fields of one document set (Elasticsearch's `+title:star overview:war`): the arguments
+ * of sa_score_batch_topk_bool_occur, with clause c on field clause_field[c] (< the multi's fields) and its term ids
+ * that field's.  Field f of the multi is scored with avg_doc_len[f], k1[f] and b[f]; each clause's idf is the
+ * caller's, from its own field.  Per query the result is sa_score_batch_topk_bool_occur's composition with
+ * score(c) = .score of the clause on its field; a field whose avg_doc_len is 0 scores 0 at every doc (a MUST / FILTER
+ * clause on it ranks nothing, a MUST_NOT clause on it vetoes nothing).  Or / And take it with every clause SHOULD and
+ * weight 1.  Fields that share one sa_index must share (avg_doc_len, k1, b): the index caches one norm table.  Result
+ * ids are global doc ids (doc_base added). */
+int sa_multi_score_batch_topk_bool(sa_multi *multi, const uint32_t *query_clause_starts, const uint32_t *clause_field,
+                                   const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                   const float *clause_idf, const float *clause_weight, const uint8_t *clause_occur,
+                                   const uint32_t *mm, uint32_t n_queries, uint32_t slop, const float *avg_doc_len,
+                                   const float *k1, const float *b, uint32_t k, uint32_t *out_docs, float *out_scores,
+                                   uint32_t *n_redone);
 
 /* ------------------------------------------------- per-op exports (parity tests)
  * Device implementations of the reference's native ops on raw arrays (host in, host out),

@@ -23,6 +23,11 @@
 // per-thread masks over the thread's 32 docs record where a MUST / FILTER clause misses (`req`) and where a MUST_NOT
 // clause matches (`veto`).  A tile where a MUST / FILTER clause has no doc, or with fewer SHOULD clauses than mm, is
 // published empty before the fold.
+//
+// bool_fields_tile_kernel (sa_multi_score_batch_topk_bool) is the same fold with clauses on several fields of one
+// document set: a clause carries its field's slot, and every step reads that field's lists, norms, doc lengths and
+// BM25 parameters from a small per-call table (BoolField) instead of the index in BoolArgs.
+#include "sa_multi.cuh"
 #include "sa_term.cuh"
 #include "sa_phrase.cuh"
 
@@ -33,7 +38,7 @@ struct BoolClause {
     float idf;
     u32 row;        // a phrase clause's count row in BoolState::rows (within its group); SA_BOOL_NO_ROW: a term
     u32 sparse;     // Bm25Params::sparse_ok under this clause's idf
-    u32 pad;
+    u32 field;      // bool_fields_tile_kernel: the clause's slot in the field table; 0 otherwise
 };
 
 struct BoolQuery { u32 c0, n, mm, pad; };   // clauses [c0, c0 + n) of the batch
@@ -57,9 +62,18 @@ struct BoolOccur {
     u32 occur;      // SA_OCCUR_*
 };
 
+// One field of sa_multi_score_batch_topk_bool, as bool_fields_tile_kernel reads it: BoolArgs' per-index members.
+struct BoolField {
+    const u64 *words;
+    const u32 *tile_dir, *recs, *rec_dir;
+    const float *norm, *doc_lens;
+    Bm25Params bm25;                        // idf unused (per clause)
+};
+
 struct BoolState {
     DevBuf d_clauses, d_queries, d_out_index;
     DevBuf d_occur;
+    DevBuf d_fields;     // BoolField[] of a multi-field call
     DevBuf d_keys;       // nq * k result keys, then u32 overflow[nq]: one device-to-host copy
     DevBuf rows;
 };
@@ -110,11 +124,28 @@ __device__ __forceinline__ void bool_fold_occur(float &acc, u32 &hits, u32 &req,
     if (oc.occur == SA_OCCUR_MUST_NOT && v > 0.0f) veto |= 1u << i;
 }
 
-// OCCUR = false: Or / And (every clause SHOULD, weight 1).  OCCUR = true: per-clause roles and weights in occ[],
-// indexed as a.clauses; a query's mm counts its SHOULD clauses.
-template <bool OCCUR>
-__global__ void __launch_bounds__(SA_TERM_THREADS)
-bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ) {
+// FIELDS: point the view `v` (a copy of the kernel's BoolArgs) at field slot f of the table: its lists, norms, doc
+// lengths and BM25 parameters.  The entry's address is CTA-uniform, so its loads are broadcasts that stay cached.
+template <bool FIELDS>
+__device__ __forceinline__ void bool_set_field(BoolArgs &v, const BoolField *__restrict__ fld, u32 f) {
+    if (!FIELDS) return;
+    const BoolField &e = fld[f];
+    v.words = e.words;
+    v.tile_dir = e.tile_dir;
+    v.recs = e.recs;
+    v.rec_dir = e.rec_dir;
+    v.norm = e.norm;
+    v.doc_lens = e.doc_lens;
+    v.bm25 = e.bm25;
+}
+
+// The tile fold of one (query, tile).  OCCUR = false: Or / And (every clause SHOULD, weight 1).  OCCUR = true:
+// per-clause roles and weights in occ[], indexed as a.clauses; a query's mm counts its SHOULD clauses.  FIELDS: each
+// clause reads the field fld[clause.field] (bool_set_field) in place of the index in `a`; n_docs, doc_base, the
+// phrase rows and the top-k context stay common.
+template <bool OCCUR, bool FIELDS>
+__device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__restrict__ occ,
+                                          const BoolField *__restrict__ fld) {
     constexpr int PER = SA_TILE_DOCS / SA_TERM_THREADS / 4;        // float4 groups per thread
     __shared__ __align__(16) float s_tile[SA_TILE_DOCS];
     __shared__ u32 s_lo[SA_BOOL_MAX_CLAUSES], s_hi[SA_BOOL_MAX_CLAUSES];
@@ -126,6 +157,7 @@ bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ) {
     const u32 tile_doc0 = tile * SA_TILE_DOCS;
     const u64 tile_doc0_abs = a.doc_base + tile_doc0;              // as stored in the words
     float4 *s_tile4 = reinterpret_cast<float4 *>(s_tile);
+    BoolArgs view = a;                                              // FIELDS: the clause's field (bool_set_field)
 
     // 1. zero the tile; every clause's slice of the tile, and how many clauses have anything in it
 #pragma unroll
@@ -134,16 +166,18 @@ bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ) {
     __syncthreads();
     for (u32 c = warp; c < bq.n; c += SA_TERM_THREADS / 32) {      // warp-uniform
         const BoolClause cl = a.clauses[bq.c0 + c];
+        bool_set_field<FIELDS>(view, fld, cl.field);
+        const BoolArgs &ca = FIELDS ? view : a;
         u32 lo = 0, hi = 0;
         if (cl.row != SA_BOOL_NO_ROW) {
             hi = 1;                                                 // a phrase row counts as present
         } else if (cl.n_words == 0) {
         } else if (cl.dir_off != SA_NO_DIR) {
-            const u32 *dir = (bool_uses_recs(a, cl) ? a.rec_dir : a.tile_dir) + cl.dir_off + tile;
+            const u32 *dir = (bool_uses_recs(ca, cl) ? ca.rec_dir : ca.tile_dir) + cl.dir_off + tile;
             lo = __ldg(dir);
             hi = __ldg(dir + 1);
         } else {
-            const u64 *w = a.words + cl.word_off;
+            const u64 *w = ca.words + cl.word_off;
             lo = (u32)warp_lower_bound_shifted(w, 0, cl.n_words, tile_doc0_abs, SA_KEY_SHIFT);
             hi = (u32)warp_lower_bound_shifted(w, lo, cl.n_words, tile_doc0_abs + SA_TILE_DOCS, SA_KEY_SHIFT);
         }
@@ -189,6 +223,9 @@ bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ) {
         if (cl.sparse && hi <= lo) continue;                        // CTA-uniform: +0 at every doc of the tile
         BoolOccur oc{1.0f, SA_OCCUR_SHOULD};
         if (OCCUR) oc = occ[bq.c0 + c];
+        bool_set_field<FIELDS>(view, fld, cl.field);
+        const BoolArgs &ca = FIELDS ? view : a;
+        if (FIELDS) p = ca.bm25;
         p.idf = cl.idf;
         if (cl.row != SA_BOOL_NO_ROW) {
             // phrase clause (sparse-safe parameters only): BM25 of its counts, zero counts score +0
@@ -202,7 +239,7 @@ bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ) {
                 for (int e = 0; e < 4; e++) {
                     const u64 d = (u64)tile_doc0 + g * 4 + e;
                     float v = 0.0f;
-                    if (xs[e] > 0.0f && d < a.n_docs) v = bm25_from_norm(xs[e], __ldg(a.norm + d), cl.idf);
+                    if (xs[e] > 0.0f && d < a.n_docs) v = bm25_from_norm(xs[e], __ldg(ca.norm + d), cl.idf);
                     if (OCCUR) {
                         bool_fold_occur(acc[j * 4 + e], hits[j], req, veto, j * 4 + e, v, oc);
                     } else {
@@ -212,7 +249,7 @@ bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ) {
                 }
             }
         } else {
-            bool_scatter_term(a, cl, lo, hi, tile_doc0, tile_doc0_abs, s_tile);
+            bool_scatter_term(ca, cl, lo, hi, tile_doc0, tile_doc0_abs, s_tile);
             __syncthreads();
 #pragma unroll
             for (int j = 0; j < PER; j++) {
@@ -225,7 +262,7 @@ bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ) {
                     const u64 d = (u64)tile_doc0 + g * 4 + e;
                     float v = xs[e];
                     // bm25.pyx:20-25 over every doc (NaN / inf / -0.0 of exotic parameters)
-                    if (!cl.sparse) v = d < a.n_docs ? bm25_one(xs[e], __ldg(a.doc_lens + d), p) : 0.0f;
+                    if (!cl.sparse) v = d < a.n_docs ? bm25_one(xs[e], __ldg(ca.doc_lens + d), p) : 0.0f;
                     if (OCCUR) {
                         bool_fold_occur(acc[j * 4 + e], hits[j], req, veto, j * 4 + e, v, oc);
                     } else {
@@ -257,32 +294,61 @@ bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ) {
     flush_tile_collect<false>(s_tile, nullptr, a.topk, q, tile, my_max, SA_TILE_DOCS, 0, s_top, &s_ncand, &s_tile_max);
 }
 
+template <bool OCCUR>
+__global__ void __launch_bounds__(SA_TERM_THREADS)
+bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ) {
+    bool_tile<OCCUR, false>(a, occ, nullptr);
+}
+
+// sa_multi_score_batch_topk_bool: roles and weights as bool_tile_kernel<true>, each clause on its own field.  Held to
+// three CTAs per SM, as the single-field instance runs (80 registers, no spills); at two (90 registers) it ran 23-24%
+// slower.
+__global__ void __launch_bounds__(SA_TERM_THREADS, 3)
+bool_fields_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld) {
+    bool_tile<true, true>(a, occ, fld);
+}
+
 // ------------------------------------------------------------------------------------------------------------ host
 namespace {
+
+// The fields of one call and where the call keeps its state.  The single-index entry points pass one field and the
+// index's own buffers (ix->boolq, ix->cand, ix->h_pinned); sa_multi_score_batch_topk_bool passes the multi's fields,
+// its BoolState and candidate buffer, and field 0's pinned staging.  Every field's stream is `lead`'s (FieldGuard).
+struct BoolCall {
+    std::vector<sa_index *> ix;         // per field slot
+    std::vector<float> avgdl, k1, b;    // per field slot
+    bool fields_kernel = false;         // bool_fields_tile_kernel (clauses carry their field slot)
+    BoolState *S = nullptr;
+    DevBuf *cand = nullptr;
+    PinnedBuf *h_pinned = nullptr;
+    sa_index *lead() const { return ix[0]; }
+};
 
 struct BoolPlan {
     std::vector<BoolClause> clauses;
     std::vector<BoolQuery> queries;
     std::vector<u32> group_start;       // queries [group_start[i], group_start[i + 1]) share one launch and its rows
     std::vector<BoolOccur> occur;       // per clause, as clauses; empty: Or / And (bool_tile_kernel<false>)
+    std::vector<BoolField> fields;      // per field slot (bool_fields_tile_kernel only)
     u32 max_group = 1, max_rows = 0;
-    bool any_sparse = false;
 };
 
-// The count rows of the phrase clauses of queries [q0, q1) (rows are numbered within the group), synchronously.
-int bool_build_rows(sa_index *ix, BoolState &S, const BoolPlan &P, const uint32_t *clause_terms,
+// The count rows of the phrase clauses of queries [q0, q1) (rows are numbered within the group), each on its clause's
+// field, synchronously.
+int bool_build_rows(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_terms,
                     const uint32_t *clause_term_starts, u32 slop, u32 q0, u32 q1) {
-    const u64 stride = sa_padded_docs(ix->n_docs);
+    const u64 stride = sa_padded_docs(X.lead()->n_docs);
     int rc;
     for (u32 q = q0; q < q1; q++) {
         const BoolQuery &bq = P.queries[q];
         for (u32 c = bq.c0; c < bq.c0 + bq.n; c++) {
             const BoolClause &cl = P.clauses[c];
             if (cl.row == SA_BOOL_NO_ROW) continue;
+            sa_index *ix = X.ix[cl.field];
             bool scored;
             if ((rc = sa_phrase_row(ix, clause_terms + clause_term_starts[c], clause_term_starts[c + 1] - clause_term_starts[c],
                                     slop, nullptr, nullptr, nullptr, &scored))) return rc;
-            SA_CUDA(cudaMemcpyAsync(S.rows.as<float>() + (u64)cl.row * stride, ix->dense.p, ix->n_docs * sizeof(float),
+            SA_CUDA(cudaMemcpyAsync(X.S->rows.as<float>() + (u64)cl.row * stride, ix->dense.p, ix->n_docs * sizeof(float),
                                     cudaMemcpyDeviceToDevice, ix->stream));
         }
     }
@@ -290,33 +356,39 @@ int bool_build_rows(sa_index *ix, BoolState &S, const BoolPlan &P, const uint32_
 }
 
 // Queries [q0, q1) with `slots` candidate slots per tile: their rows, the tile kernel and the selection, enqueued.
-int bool_run_group(sa_index *ix, BoolState &S, const BoolPlan &P, const uint32_t *clause_terms,
-                   const uint32_t *clause_term_starts, u32 slop, const Bm25Params &bm25, u32 k, u32 slots,
-                   u32 q0, u32 q1) {
+int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_terms,
+                   const uint32_t *clause_term_starts, u32 slop, u32 k, u32 slots, u32 q0, u32 q1) {
+    sa_index *ix = X.lead();
+    BoolState &S = *X.S;
     const u32 n_tiles = sa_n_tiles(ix->n_docs), nq = q1 - q0;
     int rc;
-    if ((rc = bool_build_rows(ix, S, P, clause_terms, clause_term_starts, slop, q0, q1))) return rc;
-    if ((rc = ix->cand.reserve(cand_bytes(n_tiles, nq, slots)))) return rc;
+    if ((rc = bool_build_rows(X, P, clause_terms, clause_term_starts, slop, q0, q1))) return rc;
+    if ((rc = X.cand->reserve(cand_bytes(n_tiles, nq, slots)))) return rc;
     u64 *d_keys = S.d_keys.as<u64>();
     u32 *d_ovf = (u32 *)(d_keys + (size_t)P.queries.size() * k);
-    TopkCtx t = make_topk_ctx(ix->cand.p, n_tiles, nq, slots, k, d_ovf + q0);
+    TopkCtx t = make_topk_ctx(X.cand->p, n_tiles, nq, slots, k, d_ovf + q0);
     BoolArgs a;
     memset(&a, 0, sizeof(a));
-    a.words = ix->d_words.as<u64>();
-    a.tile_dir = ix->d_tile_dir.as<u32>();
-    a.recs = ix->d_recs.as<u32>();
-    a.rec_dir = ix->d_rec_dir.as<u32>();
-    a.norm = ix->d_norm.as<float>();
-    a.doc_lens = ix->d_doc_lens.as<float>();
+    if (!X.fields_kernel) {                 // the multi-field kernel reads these per clause from S.d_fields
+        a.words = ix->d_words.as<u64>();
+        a.tile_dir = ix->d_tile_dir.as<u32>();
+        a.recs = ix->d_recs.as<u32>();
+        a.rec_dir = ix->d_rec_dir.as<u32>();
+        a.norm = ix->d_norm.as<float>();
+        a.doc_lens = ix->d_doc_lens.as<float>();
+        a.bm25 = make_bm25(1.0f, X.avgdl[0], X.k1[0], X.b[0], ix->doc_lens_nonneg);
+    }
     a.rows = S.rows.as<float>();
     a.row_stride = sa_padded_docs(ix->n_docs);
     a.n_docs = ix->n_docs;
     a.doc_base = ix->doc_base;
     a.clauses = S.d_clauses.as<BoolClause>();
     a.queries = S.d_queries.as<BoolQuery>() + q0;
-    a.bm25 = bm25;
     a.topk = t;
-    if (P.occur.empty())
+    if (X.fields_kernel)
+        bool_fields_tile_kernel<<<dim3(nq, n_tiles), SA_TERM_THREADS, 0, ix->stream>>>(a, S.d_occur.as<BoolOccur>(),
+                                                                                        S.d_fields.as<BoolField>());
+    else if (P.occur.empty())
         bool_tile_kernel<false><<<dim3(nq, n_tiles), SA_TERM_THREADS, 0, ix->stream>>>(a, nullptr);
     else
         bool_tile_kernel<true><<<dim3(nq, n_tiles), SA_TERM_THREADS, 0, ix->stream>>>(a, S.d_occur.as<BoolOccur>());
@@ -325,18 +397,14 @@ int bool_run_group(sa_index *ix, BoolState &S, const BoolPlan &P, const uint32_t
     return launch_topk_select(ix, t, nq, ix->doc_base, d_keys, S.d_out_index.as<u32>() + q0);
 }
 
-// Both entry points.  clause_weight / clause_occur NULL: Or / And, every clause SHOULD with weight 1, mm over all.
-int bool_topk(sa_index *ix, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
-              const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
-              const uint8_t *clause_occur, const uint32_t *mm, uint32_t n_queries, uint32_t slop, float avg_doc_len,
-              float k1, float b, uint32_t k, uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
-    SA_CHECK(ix && out_docs && out_scores, "NULL argument");
-    SA_CHECK(n_queries == 0 || (query_clause_starts && clause_terms && clause_term_starts && clause_idf && mm),
-             "NULL argument");
-    SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
-    if (n_redone) *n_redone = 0;
-    std::lock_guard<std::mutex> g(ix->mu);
-    SA_CUDA(cudaSetDevice(ix->device));
+// Every entry point, with the call's indexes locked and their device current.  clause_weight / clause_occur NULL:
+// Or / And, every clause SHOULD with weight 1, mm over all.  clause_field NULL: every clause on field 0.
+int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint32_t *clause_field,
+              const uint32_t *clause_terms, const uint32_t *clause_term_starts, const float *clause_idf,
+              const float *clause_weight, const uint8_t *clause_occur, const uint32_t *mm, uint32_t n_queries,
+              uint32_t slop, uint32_t k, uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+    sa_index *lead = X.lead();
+    const u32 n_fields = (u32)X.ix.size();
     int rc;
     const bool occur = clause_occur != nullptr;
     SA_CHECK(n_queries == 0 || query_clause_starts[0] == 0, "query_clause_starts[0] must be 0");
@@ -362,92 +430,145 @@ int bool_topk(sa_index *ix, const uint32_t *query_clause_starts, const uint32_t 
         const u32 nt = clause_term_starts[c + 1] - clause_term_starts[c];
         SA_CHECK(clause_term_starts[c + 1] > clause_term_starts[c] && nt <= SA_MAX_PHRASE_TERMS,
                  "clause %u: bad number of terms", c);
-        if ((rc = sa_check_term_ids(ix, clause_terms + clause_term_starts[c], nt))) return rc;
+        const u32 f = clause_field ? clause_field[c] : 0;
+        SA_CHECK(f < n_fields, "clause %u: field %u out of range (%u fields)", c, f, n_fields);
+        if ((rc = sa_check_term_ids(X.ix[f], clause_terms + clause_term_starts[c], nt))) return rc;
     }
     const size_t nk = (size_t)n_queries * k;
     for (size_t i = 0; i < nk; i++) { out_docs[i] = SA_NO_DOC; out_scores[i] = 0.0f; }
-    if (n_queries == 0 || ix->n_docs == 0 || avg_doc_len == 0.0f) return SA_OK;   // .score is all zeros: nothing ranks
+    // .score is all zeros on a field whose avgdl is 0: its clauses are empty (below), and without any other field
+    // nothing ranks
+    bool any_avgdl = false;
+    for (u32 f = 0; f < n_fields; f++) any_avgdl = any_avgdl || X.avgdl[f] != 0.0f;
+    if (n_queries == 0 || lead->n_docs == 0 || !any_avgdl) return SA_OK;
 
     // descriptors, and the groups: at most ~1 GB of candidate slots and ~4 GB of phrase rows per launch
-    const u32 n_tiles = sa_n_tiles(ix->n_docs), slots = sa_topk_slots(k);
-    const u64 stride = sa_padded_docs(ix->n_docs);
+    const u32 n_tiles = sa_n_tiles(lead->n_docs), slots = sa_topk_slots(k);
+    const u64 stride = sa_padded_docs(lead->n_docs);
     const u32 group_q = (u32)std::min<u64>(65535, std::max<u64>(1, (1ull << 30) / ((u64)n_tiles * (slots * sizeof(u64) + 8))));
     const u32 group_rows = (u32)std::max<u64>(1, (4ull << 30) / (stride * sizeof(float)));
-    const Bm25Params bm25 = make_bm25(1.0f, avg_doc_len, k1, b, ix->doc_lens_nonneg);
     BoolPlan P;
     P.queries.resize(n_queries);
     P.group_start.push_back(0);
+    std::vector<char> field_sparse(n_fields, 0);      // fields with a sparse-safe clause: their norms are cached
     u32 rows = 0;
     for (u32 q = 0; q < n_queries; q++) {
         const u32 c0 = query_clause_starts[q], c1 = query_clause_starts[q + 1];
         u32 nr = 0;
-        for (u32 c = c0; c < c1; c++) nr += clause_term_starts[c + 1] - clause_term_starts[c] > 1;
+        for (u32 c = c0; c < c1; c++) {
+            const u32 f = clause_field ? clause_field[c] : 0;
+            nr += clause_term_starts[c + 1] - clause_term_starts[c] > 1 && X.avgdl[f] != 0.0f;
+        }
         if (q > P.group_start.back() && (q - P.group_start.back() == group_q || rows + nr > group_rows)) {
             P.group_start.push_back(q);
             rows = 0;
         }
         P.queries[q] = BoolQuery{(u32)P.clauses.size(), c1 - c0, mm[q], 0};
         for (u32 c = c0; c < c1; c++) {
+            const u32 f = clause_field ? clause_field[c] : 0;
+            sa_index *ix = X.ix[f];
             const u32 *tids = clause_terms + clause_term_starts[c];
             const u32 nt = clause_term_starts[c + 1] - clause_term_starts[c];
-            const bool sparse = make_bm25(clause_idf[c], avg_doc_len, k1, b, ix->doc_lens_nonneg).sparse_ok != 0;
+            if (occur) P.occur.push_back(BoolOccur{clause_weight[c], clause_occur[c]});
+            if (X.avgdl[f] == 0.0f) {       // scores +0 at every doc: no list, no row
+                P.clauses.push_back(BoolClause{0, 0, SA_NO_DIR, SA_NO_DIR, clause_idf[c], SA_BOOL_NO_ROW, 1u, f});
+                continue;
+            }
+            const bool sparse = make_bm25(clause_idf[c], X.avgdl[f], X.k1[f], X.b[f], ix->doc_lens_nonneg).sparse_ok != 0;
             SA_CHECK(nt == 1 || sparse, "phrase queries in a batch need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite idf)");
             const TermQuery tq = make_term_query(ix, nt == 1 ? tids[0] : SA_NO_TERM, clause_idf[c]);
             P.clauses.push_back(BoolClause{tq.word_off, tq.n_words, tq.dir_off, tq.rec_off, clause_idf[c],
-                                           nt == 1 ? SA_BOOL_NO_ROW : rows++, sparse ? 1u : 0u, 0});
-            if (occur) P.occur.push_back(BoolOccur{clause_weight[c], clause_occur[c]});
-            P.any_sparse = P.any_sparse || sparse;
+                                           nt == 1 ? SA_BOOL_NO_ROW : rows++, sparse ? 1u : 0u, f});
+            field_sparse[f] = field_sparse[f] || sparse;
         }
         P.max_group = std::max(P.max_group, q + 1 - P.group_start.back());
         P.max_rows = std::max(P.max_rows, rows);
     }
     P.group_start.push_back(n_queries);
 
-    if (!ix->boolq) ix->boolq.reset(new BoolState());
-    BoolState &S = *ix->boolq;
+    BoolState &S = *X.S;
     const size_t key_bytes = nk * sizeof(u64) + (size_t)n_queries * sizeof(u32);
     if ((rc = S.d_clauses.reserve(P.clauses.size() * sizeof(BoolClause))) ||
         (rc = S.d_queries.reserve(P.queries.size() * sizeof(BoolQuery))) ||
         (rc = S.d_out_index.reserve((size_t)n_queries * sizeof(u32))) || (rc = S.d_keys.reserve(key_bytes)) ||
         (rc = S.rows.reserve(std::max<size_t>((size_t)P.max_rows * stride * sizeof(float), 64))) ||
         (rc = S.d_occur.reserve(P.occur.size() * sizeof(BoolOccur))) ||
-        (rc = ix->h_pinned.reserve(key_bytes)))
+        (rc = X.h_pinned->reserve(key_bytes)))
         return rc;
-    if (P.any_sparse && (rc = sa_ensure_norm(ix, k1, b, avg_doc_len))) return rc;
+    for (u32 f = 0; f < n_fields; f++)
+        if (field_sparse[f] && (rc = sa_ensure_norm(X.ix[f], X.k1[f], X.b[f], X.avgdl[f]))) return rc;
+    if (X.fields_kernel) {
+        for (u32 f = 0; f < n_fields; f++) {
+            sa_index *ix = X.ix[f];
+            P.fields.push_back(BoolField{ix->d_words.as<u64>(), ix->d_tile_dir.as<u32>(), ix->d_recs.as<u32>(),
+                                         ix->d_rec_dir.as<u32>(), ix->d_norm.as<float>(), ix->d_doc_lens.as<float>(),
+                                         make_bm25(1.0f, X.avgdl[f], X.k1[f], X.b[f], ix->doc_lens_nonneg)});
+        }
+        if ((rc = S.d_fields.reserve(P.fields.size() * sizeof(BoolField)))) return rc;
+        SA_CUDA(cudaMemcpyAsync(S.d_fields.p, P.fields.data(), P.fields.size() * sizeof(BoolField), cudaMemcpyHostToDevice,
+                                lead->stream));
+    }
     std::vector<u32> identity(n_queries);
     for (u32 q = 0; q < n_queries; q++) identity[q] = q;
-    SA_CUDA(cudaMemcpyAsync(S.d_clauses.p, P.clauses.data(), P.clauses.size() * sizeof(BoolClause), cudaMemcpyHostToDevice, ix->stream));
+    SA_CUDA(cudaMemcpyAsync(S.d_clauses.p, P.clauses.data(), P.clauses.size() * sizeof(BoolClause), cudaMemcpyHostToDevice, lead->stream));
     if (occur) {
-        SA_CUDA(cudaMemcpyAsync(S.d_occur.p, P.occur.data(), P.occur.size() * sizeof(BoolOccur), cudaMemcpyHostToDevice, ix->stream));
+        SA_CUDA(cudaMemcpyAsync(S.d_occur.p, P.occur.data(), P.occur.size() * sizeof(BoolOccur), cudaMemcpyHostToDevice, lead->stream));
     }
-    SA_CUDA(cudaMemcpyAsync(S.d_queries.p, P.queries.data(), P.queries.size() * sizeof(BoolQuery), cudaMemcpyHostToDevice, ix->stream));
-    SA_CUDA(cudaMemcpyAsync(S.d_out_index.p, identity.data(), (size_t)n_queries * sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
+    SA_CUDA(cudaMemcpyAsync(S.d_queries.p, P.queries.data(), P.queries.size() * sizeof(BoolQuery), cudaMemcpyHostToDevice, lead->stream));
+    SA_CUDA(cudaMemcpyAsync(S.d_out_index.p, identity.data(), (size_t)n_queries * sizeof(u32), cudaMemcpyHostToDevice, lead->stream));
     u32 *d_ovf = (u32 *)(S.d_keys.as<u64>() + nk);
-    SA_CUDA(cudaMemsetAsync(d_ovf, 0, (size_t)n_queries * sizeof(u32), ix->stream));
+    SA_CUDA(cudaMemsetAsync(d_ovf, 0, (size_t)n_queries * sizeof(u32), lead->stream));
     for (size_t i = 0; i + 1 < P.group_start.size(); i++)
-        if ((rc = bool_run_group(ix, S, P, clause_terms, clause_term_starts, slop, bm25, k, slots, P.group_start[i],
+        if ((rc = bool_run_group(X, P, clause_terms, clause_term_starts, slop, k, slots, P.group_start[i],
                                  P.group_start[i + 1]))) return rc;
 
     // keys and overflow flags in one copy and one synchronise; a query whose tile overflowed is re-run alone with a
     // slot per doc of the tile, which cannot overflow
-    SA_CUDA(cudaMemcpyAsync(ix->h_pinned.p, S.d_keys.p, key_bytes, cudaMemcpyDeviceToHost, ix->stream));
-    SA_CUDA(cudaStreamSynchronize(ix->stream));
+    PinnedBuf &h = *X.h_pinned;
+    SA_CUDA(cudaMemcpyAsync(h.p, S.d_keys.p, key_bytes, cudaMemcpyDeviceToHost, lead->stream));
+    SA_CUDA(cudaStreamSynchronize(lead->stream));
     std::vector<u32> ovf(n_queries);
-    memcpy(ovf.data(), ix->h_pinned.as<const u64>() + nk, (size_t)n_queries * sizeof(u32));
-    sa_unpack_keys(ix->h_pinned.as<const u64>(), nk, out_docs, out_scores);
+    memcpy(ovf.data(), h.as<const u64>() + nk, (size_t)n_queries * sizeof(u32));
+    sa_unpack_keys(h.as<const u64>(), nk, out_docs, out_scores);
     u32 redone = 0;
     for (u32 q = 0; q < n_queries; q++) {
         if (!ovf[q]) continue;
-        SA_CUDA(cudaMemsetAsync(d_ovf + q, 0, sizeof(u32), ix->stream));
-        if ((rc = bool_run_group(ix, S, P, clause_terms, clause_term_starts, slop, bm25, k, SA_TILE_DOCS, q, q + 1))) return rc;
-        SA_CUDA(cudaMemcpyAsync(ix->h_pinned.p, S.d_keys.as<u64>() + (size_t)q * k, k * sizeof(u64), cudaMemcpyDeviceToHost,
-                                ix->stream));
-        SA_CUDA(cudaStreamSynchronize(ix->stream));
-        sa_unpack_keys(ix->h_pinned.as<const u64>(), k, out_docs + (size_t)q * k, out_scores + (size_t)q * k);
+        SA_CUDA(cudaMemsetAsync(d_ovf + q, 0, sizeof(u32), lead->stream));
+        if ((rc = bool_run_group(X, P, clause_terms, clause_term_starts, slop, k, SA_TILE_DOCS, q, q + 1))) return rc;
+        SA_CUDA(cudaMemcpyAsync(h.p, S.d_keys.as<u64>() + (size_t)q * k, k * sizeof(u64), cudaMemcpyDeviceToHost,
+                                lead->stream));
+        SA_CUDA(cudaStreamSynchronize(lead->stream));
+        sa_unpack_keys(h.as<const u64>(), k, out_docs + (size_t)q * k, out_scores + (size_t)q * k);
         redone++;
     }
     if (n_redone) *n_redone = redone;
     return SA_OK;
+}
+
+// The single-index entry points: the index's own lock, state and buffers.
+int bool_topk_index(sa_index *ix, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
+                    const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
+                    const uint8_t *clause_occur, const uint32_t *mm, uint32_t n_queries, uint32_t slop,
+                    float avg_doc_len, float k1, float b, uint32_t k, uint32_t *out_docs, float *out_scores,
+                    uint32_t *n_redone) {
+    SA_CHECK(ix && out_docs && out_scores, "NULL argument");
+    SA_CHECK(n_queries == 0 || (query_clause_starts && clause_terms && clause_term_starts && clause_idf && mm),
+             "NULL argument");
+    SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
+    if (n_redone) *n_redone = 0;
+    std::lock_guard<std::mutex> g(ix->mu);
+    SA_CUDA(cudaSetDevice(ix->device));
+    if (!ix->boolq) ix->boolq.reset(new BoolState());
+    BoolCall X;
+    X.ix = {ix};
+    X.avgdl = {avg_doc_len};
+    X.k1 = {k1};
+    X.b = {b};
+    X.S = ix->boolq.get();
+    X.cand = &ix->cand;
+    X.h_pinned = &ix->h_pinned;
+    return bool_topk(X, query_clause_starts, nullptr, clause_terms, clause_term_starts, clause_idf, clause_weight,
+                     clause_occur, mm, n_queries, slop, k, out_docs, out_scores, n_redone);
 }
 
 }  // namespace
@@ -456,8 +577,8 @@ extern "C" int sa_score_batch_topk_bool(sa_index *ix, const uint32_t *query_clau
                                         const uint32_t *clause_term_starts, const float *clause_idf, const uint32_t *mm,
                                         uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
                                         uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
-    return bool_topk(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, nullptr, nullptr, mm,
-                     n_queries, slop, avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
+    return bool_topk_index(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, nullptr, nullptr, mm,
+                           n_queries, slop, avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
 }
 
 extern "C" int sa_score_batch_topk_bool_occur(sa_index *ix, const uint32_t *query_clause_starts,
@@ -467,6 +588,48 @@ extern "C" int sa_score_batch_topk_bool_occur(sa_index *ix, const uint32_t *quer
                                               uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
                                               uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
     SA_CHECK(n_queries == 0 || (clause_weight && clause_occur), "NULL argument");
-    return bool_topk(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, clause_weight,
-                     clause_occur, mm, n_queries, slop, avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
+    return bool_topk_index(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, clause_weight,
+                           clause_occur, mm, n_queries, slop, avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
+}
+
+extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, const uint32_t *query_clause_starts,
+                                              const uint32_t *clause_field, const uint32_t *clause_terms,
+                                              const uint32_t *clause_term_starts, const float *clause_idf,
+                                              const float *clause_weight, const uint8_t *clause_occur,
+                                              const uint32_t *mm, uint32_t n_queries, uint32_t slop,
+                                              const float *avg_doc_len, const float *k1, const float *b, uint32_t k,
+                                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+    SA_CHECK(m && out_docs && out_scores && avg_doc_len && k1 && b, "NULL argument");
+    SA_CHECK(n_queries == 0 || (query_clause_starts && clause_field && clause_terms && clause_term_starts &&
+                                clause_idf && clause_weight && clause_occur && mm), "NULL argument");
+    SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
+    if (n_redone) *n_redone = 0;
+    std::lock_guard<std::mutex> g(m->mu);
+    SA_CUDA(cudaSetDevice(m->device));
+    const u32 n_fields = (u32)m->fields.size();
+    // fields that share an index share its norm cache, which holds one parameter set; each index is locked once, in
+    // address order, and its stream swapped to the multi's for the whole call
+    std::vector<sa_index *> distinct;
+    for (u32 f = 0; f < n_fields; f++) {
+        for (u32 e = 0; e < f; e++)
+            SA_CHECK(m->fields[e] != m->fields[f] ||
+                     (avg_doc_len[e] == avg_doc_len[f] && k1[e] == k1[f] && b[e] == b[f]),
+                     "fields %u and %u share an index but not their BM25 parameters", e, f);
+        if (std::find(distinct.begin(), distinct.end(), m->fields[f]) == distinct.end()) distinct.push_back(m->fields[f]);
+    }
+    std::sort(distinct.begin(), distinct.end());
+    std::vector<std::unique_ptr<FieldGuard>> guards;
+    for (sa_index *ix : distinct) guards.emplace_back(new FieldGuard(ix, m->stream));
+    if (!m->boolq) m->boolq.reset(new BoolState());
+    BoolCall X;
+    X.ix = m->fields;
+    X.avgdl.assign(avg_doc_len, avg_doc_len + n_fields);
+    X.k1.assign(k1, k1 + n_fields);
+    X.b.assign(b, b + n_fields);
+    X.fields_kernel = true;
+    X.S = m->boolq.get();
+    X.cand = &m->cand;
+    X.h_pinned = &m->fields[0]->h_pinned;
+    return bool_topk(X, query_clause_starts, clause_field, clause_terms, clause_term_starts, clause_idf, clause_weight,
+                     clause_occur, mm, n_queries, slop, k, out_docs, out_scores, n_redone);
 }

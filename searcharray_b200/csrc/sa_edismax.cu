@@ -25,52 +25,13 @@
 #include <cmath>
 #include <functional>
 
+#include "sa_multi.cuh"
 #include "sa_phrase.cuh"
 #include "sa_term.cuh"
 
 int sa_filter_terms_mask(sa_index *ix, const uint32_t *term_ids, uint32_t n_terms, const unsigned char *d_mask,
                          u64 pay_lo, u64 pay_hi, bool use_payload, std::vector<u64> &offs, std::vector<u64> &lens,
                          std::vector<u64> *df_out);
-
-#define ED_MAX_FIELDS 8
-#define ED_MAX_ROWS 64
-
-struct sa_multi {
-    ~sa_multi() {
-        cudaSetDevice(device);          // the buffers below are freed after this body, on this device
-        if (stream) { cudaStreamSynchronize(stream); cudaStreamDestroy(stream); }
-    }
-    std::vector<sa_index *> fields;
-    int device = 0;
-    u64 n_docs = 0, doc_base = 0, stride = 0;
-    cudaStream_t stream = nullptr;
-    DevBuf d_qf;                         // double [stride] combined scores (float32 values widened in field-centric mode)
-    DevBuf d_mask;                       // unsigned char [stride] qf > 0 after the qf phase
-    DevBuf d_count;                      // unsigned long long
-    bool f32_mode = false, has_qf = false;
-    std::vector<std::vector<u64>> filt_offs, filt_lens;   // per field: last sa_multi_filter
-    std::vector<u32> phrase_rows;        // per field: rows produced by the last sa_multi_phrases
-    std::vector<u64> filt_bound;         // per field: words reserved for filtered lists (0 = not computed yet)
-    DevBuf cand;                         // top-k: candidate slots, then their float64 scores
-    DevBuf keys;                         // top-k result: k keys, k float64 scores, the overflow flag
-    std::mutex mu;
-};
-
-// All kernels of one multi call run on the multi's stream, including the ones the per-field
-// helpers launch on `ix->stream`: the field streams are swapped for the duration of the call.
-struct FieldGuard {
-    sa_index *ix;
-    cudaStream_t saved;
-    std::unique_lock<std::mutex> lk;
-    FieldGuard(sa_index *ix_, cudaStream_t s) : ix(ix_), saved(ix_->stream), lk(ix_->mu) {
-        cudaStreamSynchronize(saved);
-        ix->stream = s;
-    }
-    ~FieldGuard() {
-        cudaStreamSynchronize(ix->stream);
-        ix->stream = saved;
-    }
-};
 
 struct CombineArgs {
     const float *rows[ED_MAX_FIELDS];    // field f: [n_terms[f]][stride]

@@ -536,7 +536,10 @@ class SearchArray(ExtensionArray):
         """search_topk of a batch holding boolean queries: the plain ones through search_topk as before, the boolean
         ones through sa_score_batch_topk_bool (Or / And with weights 1) or sa_score_batch_topk_bool_occur (Bool,
         boosted Or / And), each clause with the idf .score gives it; results in query order."""
-        from .query import is_boolean, needs_occur
+        from .query import has_field, is_boolean, needs_occur
+        if any(has_field(q) for q in queries if is_boolean(q)):
+            raise ValueError("a Field clause names a DataFrame column: run queries over columns with "
+                             "solr.fields_topk(frame, queries), not SearchArray.search_topk")
         if self.rows is not None:
             raise NotImplementedError("boolean queries on a view (arr[mask]) are not supported yet; "
                                       "compose .score() on the view")

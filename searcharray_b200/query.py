@@ -5,7 +5,8 @@ Or(clauses, mm) ranks, per doc, s = score(c0) + score(c1) + ... (float32, folded
 where at least mm clauses score > 0 -- the reference's own composition of multi-clause queries
 (test/test_search.py:126-226) -- and search_topk returns the top k of it by (score desc, doc asc), computed on the
 device (sa_score_batch_topk_bool).  Bool(must, should, filter, must_not, mm) and Boost(clause, weight) extend that
-composition (sa_score_batch_topk_bool_occur)."""
+composition (sa_score_batch_topk_bool_occur).  Field(field, clause) names the DataFrame column a clause scores on,
+for queries over several columns (solr.fields_topk, sa_multi_score_batch_topk_bool)."""
 import math
 from typing import List, Union
 
@@ -14,18 +15,38 @@ import numpy as np
 from .solr import parse_min_should_match
 
 SA_BOOL_MAX_CLAUSES = 64          # include/searcharray_b200.h
+ED_MAX_FIELDS = 8                 # fields of one sa_multi (sa_multi.cuh)
 SA_OCCUR_SHOULD, SA_OCCUR_MUST, SA_OCCUR_FILTER, SA_OCCUR_MUST_NOT = 0, 1, 2, 3
 
 Clause = Union[str, List[str]]
 
 
 def _clause(c):
-    """A clause as search_topk's query form: str (term) or list[str] (phrase); anything else is a TypeError."""
-    if isinstance(c, str):
+    """A clause as search_topk's query form: str (term) or list[str] (phrase), or a Field of one; anything else is a
+    TypeError."""
+    if isinstance(c, (str, Field)):
         return c
     if isinstance(c, (list, tuple)) and c and all(isinstance(t, str) for t in c):
         return list(c)
     raise TypeError(f"a clause is a str (term) or a non-empty list of str (phrase), not {c!r}")
+
+
+class Field:
+    """A term (str) or phrase (non-empty list of str) clause scored on the DataFrame column `field`, as
+    frame[field].array.score(clause) scores it -- Lucene's `title:star`.  Accepted wherever a clause is (Or, And, the
+    four lists of Bool) by solr.fields_topk, which needs every clause to name its field; SearchArray.search_topk
+    refuses it.  A boosted field clause is Boost(Field(field, clause), weight); a Field holds no Boost or Field."""
+
+    def __init__(self, field, clause):
+        if not isinstance(field, str):
+            raise TypeError(f"a field is a column name (str), not {field!r}")
+        if isinstance(clause, (Boost, Field)):
+            raise TypeError(f"a Field holds a term or a phrase; boost a field clause as Boost(Field(...), w), not {clause!r}")
+        self.field = field
+        self.clause = _clause(clause)
+
+    def __repr__(self):
+        return f"Field({self.field!r}, {self.clause!r})"
 
 
 class Boost:
@@ -145,6 +166,12 @@ class Bool:
 def is_boolean(q):
     """Whether search_topk routes q to the boolean path."""
     return isinstance(q, (Or, Bool))
+
+
+def has_field(q):
+    """Whether a boolean query holds a Field clause (solr.fields_topk's form)."""
+    clauses = q.occur_clauses()[0] if isinstance(q, Bool) else q.clauses
+    return any(isinstance(c, Field) for c in clauses)
 
 
 def needs_occur(q):

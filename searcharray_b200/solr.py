@@ -405,3 +405,115 @@ def edismax_topk(frame: pd.DataFrame, q: str, qf: List[str], k: int = 10, mm: Op
     if comm is not None:                  # one all-gather of the per-shard top-k, merged on every rank
         return comm.merge_topk_f64(docs, scores, k)
     return docs, scores
+
+
+def _fields_plan(frame, queries, similarity):
+    """fields_topk's refusals and field slots, before any device work: (flatten_occur's arrays, the Field clauses,
+    field name -> slot, per-slot arrays, per-slot similarities)."""
+    from .query import ED_MAX_FIELDS, Field, flatten_occur, is_boolean
+    queries = list(queries)
+    for q in queries:
+        if not is_boolean(q):
+            raise TypeError(f"fields_topk takes Or / And / Bool queries, not {q!r}")
+    clauses, q_starts, mm, weights, occurs = flatten_occur(queries)
+    for c in clauses:
+        if not isinstance(c, Field):
+            raise ValueError(f"every clause of fields_topk names its column: Field(field, {c!r})")
+    names = list(dict.fromkeys(c.field for c in clauses))
+    if len(names) > ED_MAX_FIELDS:
+        raise ValueError(f"fields_topk takes at most {ED_MAX_FIELDS} distinct fields in one call, not {len(names)}")
+    arrays = {f: get_field(frame, f) for f in names}
+    sims = {}
+    for f in names:
+        sim = similarity.get(f, default_bm25) if isinstance(similarity, dict) else similarity
+        if not isinstance(sim, Bm25Similarity):
+            raise TypeError(f"fields_topk supports bm25_similarity only, not {sim!r} on {f!r}")
+        sims[f] = sim
+    for f, a in arrays.items():
+        if a.rows is not None:
+            raise NotImplementedError(f"fields_topk on a view (frame[mask]) is not supported yet: {f!r} is sliced; "
+                                      "compose .score() on the view")
+    if len({len(a) for a in arrays.values()}) > 1:
+        raise ValueError("fields_topk needs columns of one length: " + ", ".join(f"{f}: {len(a)}" for f, a in arrays.items()))
+    if len({a.device for a in arrays.values()}) > 1:
+        raise ValueError("fields_topk needs columns on one device: " + ", ".join(f"{f}: {a.device}" for f, a in arrays.items()))
+    # columns that share one device index (a copy of a column) are one slot: the index caches one BM25 norm table
+    slot_of, slot_key, slot_arrays, slot_sims, slot_name = {}, {}, [], [], []
+    for f in names:
+        a, sim = arrays[f], sims[f]
+        params = (np.float32(a.avg_doc_length), np.float32(sim.k1), np.float32(sim.b))
+        s = slot_key.get(id(a._shared))
+        if s is not None:
+            if (np.float32(arrays[slot_name[s]].avg_doc_length), np.float32(slot_sims[s].k1),
+                    np.float32(slot_sims[s].b)) != params:
+                raise ValueError(f"{f!r} shares its device index with {slot_name[s]!r} but not its similarity: "
+                                 "one index caches one set of BM25 parameters")
+            slot_of[f] = s
+            continue
+        slot_of[f] = slot_key[id(a._shared)] = len(slot_arrays)
+        slot_arrays.append(a)
+        slot_sims.append(sim)
+        slot_name.append(f)
+    return (clauses, q_starts, mm, weights, occurs), slot_of, slot_arrays, slot_sims
+
+
+def _fields_clauses(clauses, slot_of, arrays):
+    """Each clause's term ids and idf from its own field, as that column's .score takes them: (terms, clause term
+    starts, float32 idf, field slots).  Call it with the fields locked (_locked)."""
+    c_terms, c_idf = [None] * len(clauses), np.empty(len(clauses), dtype=np.float32)
+    for s, arr in enumerate(arrays):
+        idx = [i for i, c in enumerate(clauses) if slot_of[c.field] == s]
+        t, st, idf = arr._topk_queries([clauses[i].clause for i in idx],
+                                       lambda dfs, arr=arr: compute_idf(arr.corpus_size, dfs))
+        for j, i in enumerate(idx):
+            c_terms[i] = t[st[j]:st[j + 1]]
+            c_idf[i] = idf[j]
+    c_starts = _u32(np.cumsum([0] + [len(t) for t in c_terms]))
+    terms = _u32(np.concatenate(c_terms) if c_terms else [])
+    return terms, c_starts, c_idf, _u32([slot_of[c.field] for c in clauses])
+
+
+def _fields_call(multi, arrays, sims, flat, prepared, k, slop):
+    """sa_multi_score_batch_topk_bool on prepared arrays (the fields locked): (docs, scores, queries re-run)."""
+    _, q_starts, mm, weights, occurs = flat
+    terms, c_starts, c_idf, c_field = prepared
+    nq = len(q_starts) - 1
+    docs = np.empty((nq, k), dtype=np.uint32)
+    scores = np.empty((nq, k), dtype=np.float32)
+    n_redone = ctypes.c_uint32(0)
+    avgdl = _f32([a.avg_doc_length for a in arrays])
+    k1, b = _f32([s.k1 for s in sims]), _f32([s.b for s in sims])
+    _lib.check(_lib.lib().sa_multi_score_batch_topk_bool(
+        multi.handle, _lib.p_u32(q_starts), _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts),
+        _lib.p_f32(c_idf), _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(mm), nq, int(slop), _lib.p_f32(avgdl),
+        _lib.p_f32(k1), _lib.p_f32(b), k, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
+    return docs, scores, n_redone.value
+
+
+def _fields_topk(frame, queries, k, similarity, slop):
+    """fields_topk and the number of queries re-run exactly (candidate overflow)."""
+    flat, slot_of, arrays, sims = _fields_plan(frame, queries, similarity)
+    multi = _multi_for(arrays)
+    with _locked(multi, arrays):
+        for arr in arrays:                 # a sliced view of the same column may have left its row filter installed
+            arr._apply_rows(arr._device())
+        prepared = _fields_clauses(flat[0], slot_of, arrays)
+        return _fields_call(multi, arrays, sims, flat, prepared, k, slop)
+
+
+def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
+                similarity: Union[Similarity, Dict[str, Similarity]] = default_bm25, slop: int = 0):
+    """Batched Or / And / Bool queries whose clauses are on several columns of `frame` -- Lucene's
+    `+title:star overview:war -overview:trek`, or Elasticsearch's most_fields `title:alien^2 overview:alien` -- ranked
+    on the device in one batch.  Every clause is a query.Field(field, term or phrase), or a Boost of one; phrases match
+    with `slop`.  similarity: one bm25_similarity, or a dict {field: bm25_similarity} (missing fields take the
+    default), as in edismax.
+
+    Per query the result is the top k (score desc, doc asc) of the composition search_topk ranks for a Bool, with
+    score(Field(f, c)) = frame[f].array.score(c, similarity=similarity[f], slop=slop): each clause with its own
+    column's idf, avgdl and doc lengths.  Returns (rows uint32[Q, k], scores float32[Q, k]); empty slots are NO_DOC /
+    0; on a shard the rows are global doc ids.  Views, non-BM25 similarities, more than 8 distinct fields, columns of
+    different lengths or devices, and two names of one column under different similarities are refused before any
+    device work."""
+    docs, scores, _ = _fields_topk(frame, queries, k, similarity, slop)
+    return docs, scores
