@@ -211,6 +211,9 @@ typedef struct {
      * data-dependent terms of SURVEY 8d's B_phrase = 8*sum(W) + 16*sum(C_s) + 4*N + 4*M */
     uint64_t phrase_cont_words;
     uint64_t phrase_matched_docs;
+    /* launches of the conjunction regime's phrase_tile_kernel (also counted in phrase_kernel_launches): 0 = the
+     * search regime alone ran, phrase_kernel_launches > phrase_tile_launches after one = a re-run in the search regime */
+    uint64_t phrase_tile_launches;
 } sa_stats;
 int sa_stats_reset(sa_index *index);
 int sa_stats_get(sa_index *index, sa_stats *out);

@@ -703,6 +703,7 @@ static int launch_phrase_tile(sa_index *ix, const PhraseArgs &a, u32 n_queries) 
     SA_CUDA(cudaGetLastError());
     t.stop();
     ix->stats.phrase_kernel_launches++;
+    ix->stats.phrase_tile_launches++;
     ix->stats.total_launches++;
     return SA_OK;
 }
@@ -710,7 +711,8 @@ static int launch_phrase_tile(sa_index *ix, const PhraseArgs &a, u32 n_queries) 
 // Conjunction regime or search regime?  The conjunction regime reads every list once (8 * sum(W) bytes); the search
 // path costs about `ratio` bytes (a dozen 32-byte sectors of dependent probes) per driver element of the first step.
 bool sa_phrase_use_conjunction(const PhraseQuery &pq, u64 n_docs) {
-    static const long env = getenv("SA_PHRASE_STAGE_RATIO") ? atol(getenv("SA_PHRASE_STAGE_RATIO")) : -1;
+    const char *s = getenv("SA_PHRASE_STAGE_RATIO");             // read on every call, like the term knobs
+    const long env = s ? atol(s) : -1;
     const u64 ratio = env >= 0 ? (u64)env : 50;
     if (ratio == 0) return false;
     const u32 n = pq.n_terms;

@@ -708,6 +708,12 @@ span_groups_kernel(const SpanArgs a) {
 
 // ---------------------------------------------------------------------------- phase 3 (batched path)
 // are the match records of every query in doc order?  (they are whenever the terms' doc groups pair up)
+// Record i carries the doc of doc group i of the last term that has one.  Outside the literal corner every term's
+// sliced list holds words in the same docs (a candidate header has every term within one block, and positions stay
+// below 2^18, so one block more or less never reaches another doc), so group i is one doc for every term and the records
+// ascend; a record is ~0 only for a doc outside the shard, which the shard's own lists cannot hold.  Only the literal
+// corner's replayed lists can pair groups of different docs, and no literal input found so far does: the unsorted
+// loop of span_tiles_kernel is a guard that no known index reaches, and no test covers it.
 __global__ void __launch_bounds__(GEN_THREADS)
 span_sorted_kernel(const SpanArgs a) {
     const u32 q = blockIdx.y;
@@ -870,7 +876,8 @@ void sa_span_plan_add(SpanPlan &plan, const u64 *offs, const u64 *lens, const u6
     // conjunction prefilter: balanced lists (the generator list is not much shorter than the rest), all with a directory
     sq.cand_off = SA_NO_DIR;
     if (n_docs && !literal && dir_offs && n_terms >= 2) {
-        static const long env = getenv("SA_SPAN_CONJ_RATIO") ? atol(getenv("SA_SPAN_CONJ_RATIO")) : -1;
+        const char *s = getenv("SA_SPAN_CONJ_RATIO");             // read on every call, like the term knobs
+        const long env = s ? atol(s) : -1;
         const u64 ratio = env >= 0 ? (u64)env : 50;
         u64 sum = 0;
         bool dirs = true;
