@@ -181,6 +181,22 @@ int sa_score_batch_topk_bool_occur(sa_index *index, const uint32_t *query_clause
                                    const float *clause_weight, const uint8_t *clause_occur, const uint32_t *mm,
                                    uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
                                    uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
+/* Boolean queries with disjunction-max clauses (Lucene's DisjunctionMaxQuery, edismax's per-term qf): the arguments of
+ * sa_score_batch_topk_bool_occur plus, per clause, clause_group[c], the batch-wide index of the first clause of c's
+ * group (c itself for a plain clause), and clause_tie[c], read at a group's first clause (finite, in [0, 1]; checked
+ * at every group's first clause).  A group is a run of consecutive clauses of one query with one occur, and is one
+ * clause of its query: with v_j = w_j * score(c_j) over its members, m = max_j v_j, t = v_0 + v_1 + ... (left fold),
+ * it contributes d = m + (t - m) * tie (every step rounded to float32, no fused multiply-add) with weight 1 to s under
+ * its occur, and it matches a doc where any member scores > 0 (unweighted).  mm[q] counts SHOULD groups (<= their
+ * number).  Members of a group of two or more clauses need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite
+ * idf >= 0), so that every v >= +0; a group of one is a plain clause.  Queries without a group of two or more score
+ * as in sa_score_batch_topk_bool_occur, bit for bit. */
+int sa_score_batch_topk_bool_dismax(sa_index *index, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
+                                    const uint32_t *clause_term_starts, const float *clause_idf,
+                                    const float *clause_weight, const uint8_t *clause_occur,
+                                    const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
+                                    uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
+                                    uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
 
 /* The same batch in three stages, so a serving loop (or the benchmark) can keep the query
  * descriptors resident and time the device work alone: upload (H2D of descriptors), execute
@@ -293,6 +309,17 @@ int sa_multi_score_batch_topk_bool(sa_multi *multi, const uint32_t *query_clause
                                    const uint32_t *mm, uint32_t n_queries, uint32_t slop, const float *avg_doc_len,
                                    const float *k1, const float *b, uint32_t k, uint32_t *out_docs, float *out_scores,
                                    uint32_t *n_redone);
+/* sa_multi_score_batch_topk_bool with the DisMax groups of sa_score_batch_topk_bool_dismax (clause_group, clause_tie):
+ * Elasticsearch's best_fields, and per-term groups inside an Or with mm for edismax's term-centric qf.  A group's
+ * members may sit on different fields; each is scored on its own. */
+int sa_multi_score_batch_topk_bool_dismax(sa_multi *multi, const uint32_t *query_clause_starts,
+                                          const uint32_t *clause_field, const uint32_t *clause_terms,
+                                          const uint32_t *clause_term_starts, const float *clause_idf,
+                                          const float *clause_weight, const uint8_t *clause_occur,
+                                          const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
+                                          uint32_t n_queries, uint32_t slop, const float *avg_doc_len, const float *k1,
+                                          const float *b, uint32_t k, uint32_t *out_docs, float *out_scores,
+                                          uint32_t *n_redone);
 
 /* ------------------------------------------------- per-op exports (parity tests)
  * Device implementations of the reference's native ops on raw arrays (host in, host out),

@@ -27,6 +27,13 @@
 // bool_fields_tile_kernel (sa_multi_score_batch_topk_bool) is the same fold with clauses on several fields of one
 // document set: a clause carries its field's slot, and every step reads that field's lists, norms, doc lengths and
 // BM25 parameters from a small per-call table (BoolField) instead of the index in BoolArgs.
+//
+// bool_dismax_tile_kernel (sa_score_batch_topk_bool_dismax, sa_multi_score_batch_topk_bool_dismax; the single-index
+// entry passes a one-entry field table) adds disjunction-max groups: a run of consecutive clauses that is one clause
+// of its query.  A member's v = weight * score goes into the group's running max m and left-folded sum t, kept per
+// owned doc in per-thread strips of dynamic shared memory, and a u32 mask records where any member scores > 0; at the
+// group's last member d = m + (t - m) * tie is folded with weight 1 under the group's role, its hit being the mask.
+// A group is present in a tile iff any member is.
 #include "sa_multi.cuh"
 #include "sa_term.cuh"
 #include "sa_phrase.cuh"
@@ -70,9 +77,19 @@ struct BoolField {
     Bm25Params bm25;                        // idf unused (per clause)
 };
 
+// A clause's disjunction-max group (bool_dismax_tile_kernel only).  A clause outside a DisMax, or the one member of a
+// single-member DisMax, is a group of one (member == 0) and folds exactly as in bool_fields_tile_kernel.
+struct BoolGroup {
+    float tie;      // the group's tie (member clauses)
+    u32 first;      // the group's first clause, within its query
+    u32 member;     // 1: a member of a group of two or more clauses
+    u32 last;       // 1: the group's last member
+};
+
 struct BoolState {
     DevBuf d_clauses, d_queries, d_out_index;
     DevBuf d_occur;
+    DevBuf d_groups;     // BoolGroup[] of a DisMax call
     DevBuf d_fields;     // BoolField[] of a multi-field call
     DevBuf d_keys;       // nq * k result keys, then u32 overflow[nq]: one device-to-host copy
     DevBuf rows;
@@ -124,6 +141,48 @@ __device__ __forceinline__ void bool_fold_occur(float &acc, u32 &hits, u32 &req,
     if (oc.occur == SA_OCCUR_MUST_NOT && v > 0.0f) veto |= 1u << i;
 }
 
+// bool_dismax_tile_kernel: bool_fold_occur of a DisMax group's d, with the group's hit (any member > 0) in place of
+// d > 0 and weight 1.
+__device__ __forceinline__ void bool_fold_group(float &acc, u32 &hits, u32 &req, u32 &veto, int i, float d, bool hit,
+                                                u32 occur) {
+    if (occur == SA_OCCUR_SHOULD || occur == SA_OCCUR_MUST) acc = __fadd_rn(acc, d);
+    if (occur == SA_OCCUR_SHOULD) hits += (hit ? 1u : 0u) << (8 * (i & 3));
+    if ((occur == SA_OCCUR_MUST || occur == SA_OCCUR_FILTER) && !hit) req &= ~(1u << i);
+    if (occur == SA_OCCUR_MUST_NOT && hit) veto |= 1u << i;
+}
+
+// DISMAX: member v of a group at owned doc i (sparse-safe, so v >= +0): the running max and left-folded sum of the
+// weighted scores where the group scores (MUST / SHOULD), the hit mask in every role.  s_m / s_t: the thread's strips,
+// doc i at [i * SA_TERM_THREADS].
+__device__ __forceinline__ void bool_dismax_member(float *s_m, float *s_t, u32 &any, int i, float v,
+                                                   const BoolOccur &oc) {
+    if (oc.occur == SA_OCCUR_SHOULD || oc.occur == SA_OCCUR_MUST) {
+        const float w = __fmul_rn(oc.weight, v);
+        s_m[i * SA_TERM_THREADS] = fmaxf(s_m[i * SA_TERM_THREADS], w);
+        s_t[i * SA_TERM_THREADS] = __fadd_rn(s_t[i * SA_TERM_THREADS], w);
+    }
+    any |= (v > 0.0f ? 1u : 0u) << i;
+}
+
+// DISMAX, at a group's last member: d = m + (t - m) * tie at each owned doc, rounded step by step as numpy (no FMA),
+// folded under the group's role with the hit mask; the strips and the mask are reset for the next group.
+template <int N>
+__device__ __forceinline__ void bool_dismax_group_end(float (&acc)[N * 4], u32 (&hits)[N], u32 &req, u32 &veto,
+                                                      u32 &any, float *s_m, float *s_t, float tie, u32 occur) {
+    const bool scoring = occur == SA_OCCUR_SHOULD || occur == SA_OCCUR_MUST;
+#pragma unroll
+    for (int i = 0; i < N * 4; i++) {
+        float d = 0.0f;
+        if (scoring) {
+            const float m = s_m[i * SA_TERM_THREADS], t = s_t[i * SA_TERM_THREADS];
+            d = __fadd_rn(m, __fmul_rn(__fsub_rn(t, m), tie));
+            s_m[i * SA_TERM_THREADS] = s_t[i * SA_TERM_THREADS] = 0.0f;
+        }
+        bool_fold_group(acc[i], hits[i >> 2], req, veto, i, d, ((any >> i) & 1u) != 0, occur);
+    }
+    any = 0;
+}
+
 // FIELDS: point the view `v` (a copy of the kernel's BoolArgs) at field slot f of the table: its lists, norms, doc
 // lengths and BM25 parameters.  The entry's address is CTA-uniform, so its loads are broadcasts that stay cached.
 template <bool FIELDS>
@@ -142,15 +201,22 @@ __device__ __forceinline__ void bool_set_field(BoolArgs &v, const BoolField *__r
 // The tile fold of one (query, tile).  OCCUR = false: Or / And (every clause SHOULD, weight 1).  OCCUR = true:
 // per-clause roles and weights in occ[], indexed as a.clauses; a query's mm counts its SHOULD clauses.  FIELDS: each
 // clause reads the field fld[clause.field] (bool_set_field) in place of the index in `a`; n_docs, doc_base, the
-// phrase rows and the top-k context stay common.
-template <bool OCCUR, bool FIELDS>
+// phrase rows and the top-k context stay common.  DISMAX (with OCCUR and FIELDS): clauses form groups (grp[], indexed
+// as a.clauses); mm counts SHOULD groups; s_dyn holds the groups' running max and sum, 2 * 32 floats per thread, and
+// s_g[3] (shared) the groups' presence masks.
+template <bool OCCUR, bool FIELDS, bool DISMAX = false>
 __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__restrict__ occ,
-                                          const BoolField *__restrict__ fld) {
+                                          const BoolField *__restrict__ fld,
+                                          const BoolGroup *__restrict__ grp = nullptr, float *s_dyn = nullptr,
+                                          unsigned long long *s_g = nullptr) {
     constexpr int PER = SA_TILE_DOCS / SA_TERM_THREADS / 4;        // float4 groups per thread
     __shared__ __align__(16) float s_tile[SA_TILE_DOCS];
     __shared__ u32 s_lo[SA_BOOL_MAX_CLAUSES], s_hi[SA_BOOL_MAX_CLAUSES];
     __shared__ u32 s_top[(SA_TERM_THREADS / 32) * 8];
     __shared__ u32 s_ncand, s_tile_max, s_present;
+    // DISMAX: bit g of s_g[0] / [1] / [2]: the group whose first clause is the query's clause g has a member in the
+    // tile / is SHOULD / is MUST or FILTER
+    unsigned long long &s_g_present = s_g[0], &s_g_should = s_g[1], &s_g_req = s_g[2];
     const u32 q = blockIdx.x, tile = blockIdx.y;
     const BoolQuery bq = a.queries[q];
     const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -163,6 +229,7 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
 #pragma unroll
     for (int j = 0; j < PER; j++) s_tile4[tid + j * SA_TERM_THREADS] = make_float4(0.f, 0.f, 0.f, 0.f);
     if (tid == 0) s_present = 0;
+    if (DISMAX && tid == 0) s_g_present = s_g_should = s_g_req = 0;
     __syncthreads();
     for (u32 c = warp; c < bq.n; c += SA_TERM_THREADS / 32) {      // warp-uniform
         const BoolClause cl = a.clauses[bq.c0 + c];
@@ -184,7 +251,13 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
         if (lane == 0) {
             s_lo[c] = lo;
             s_hi[c] = hi;
-            if (OCCUR) {
+            if (DISMAX) {
+                const u32 o = occ[bq.c0 + c].occur;
+                const unsigned long long bit = 1ull << grp[bq.c0 + c].first;
+                if (hi > lo) atomicOr(&s_g_present, bit);
+                if (o == SA_OCCUR_SHOULD) atomicOr(&s_g_should, bit);
+                if (o == SA_OCCUR_MUST || o == SA_OCCUR_FILTER) atomicOr(&s_g_req, bit);
+            } else if (OCCUR) {
                 // low 16 bits: SHOULD clauses present; high bits: MUST / FILTER clauses absent (<= 64 clauses)
                 const u32 o = occ[bq.c0 + c].occur;
                 const u32 add = o == SA_OCCUR_SHOULD ? (hi > lo ? 1u : 0u)
@@ -198,7 +271,9 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
     __syncthreads();
     // 2. a clause with nothing in the tile scores > 0 at no doc of it: fewer such clauses than mm, nothing ranks;
     //    nor does anything where a MUST / FILTER clause is absent
-    if (OCCUR ? ((s_present & 0xFFFFu) < bq.mm || (s_present >> 16) != 0) : s_present < bq.mm) {   // CTA-uniform
+    //    (DISMAX: fewer SHOULD groups with a member in the tile than mm, or a MUST / FILTER group without one)
+    if (DISMAX ? ((u32)__popcll(s_g_present & s_g_should) < bq.mm || (s_g_req & ~s_g_present) != 0)
+               : OCCUR ? ((s_present & 0xFFFFu) < bq.mm || (s_present >> 16) != 0) : s_present < bq.mm) {   // CTA-uniform
         if (tid == 0) {
             const u64 t_idx = (u64)q * a.topk.n_tiles + tile;
             a.topk.tile_cnt[t_idx] = 0;
@@ -216,13 +291,28 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
     for (int j = 0; j < PER; j++) hits[j] = 0;
     u32 req = ~0u, veto = 0;               // OCCUR: bit 4 j + e of the thread's docs (PER * 4 == 32)
     static_assert(PER * 4 == 32, "one u32 mask bit per owned doc");
+    u32 any = 0;                           // DISMAX: bit 4 j + e: a member of the current group scores > 0 there
+    float *s_m = s_dyn + tid, *s_t = s_dyn + PER * 4 * SA_TERM_THREADS + tid;
+    if (DISMAX) {
+#pragma unroll
+        for (int i = 0; i < PER * 4; i++) s_m[i * SA_TERM_THREADS] = s_t[i * SA_TERM_THREADS] = 0.0f;
+    }
     Bm25Params p = a.bm25;
     for (u32 c = 0; c < bq.n; c++) {
         const BoolClause cl = a.clauses[bq.c0 + c];
         const u32 lo = s_lo[c], hi = s_hi[c];
-        if (cl.sparse && hi <= lo) continue;                        // CTA-uniform: +0 at every doc of the tile
+        BoolGroup gr{0.0f, 0u, 0u, 0u};
+        if (DISMAX) gr = grp[bq.c0 + c];
+        // CTA-uniform: +0 at every doc of the tile, which changes neither a group's max nor its sum (v >= +0); a
+        // group's last member still folds the group
+        const bool absent = cl.sparse && hi <= lo;
+        if (absent && !(DISMAX && gr.last)) continue;
         BoolOccur oc{1.0f, SA_OCCUR_SHOULD};
         if (OCCUR) oc = occ[bq.c0 + c];
+        if (DISMAX && absent) {
+            bool_dismax_group_end(acc, hits, req, veto, any, s_m, s_t, gr.tie, oc.occur);
+            continue;
+        }
         bool_set_field<FIELDS>(view, fld, cl.field);
         const BoolArgs &ca = FIELDS ? view : a;
         if (FIELDS) p = ca.bm25;
@@ -240,7 +330,9 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
                     const u64 d = (u64)tile_doc0 + g * 4 + e;
                     float v = 0.0f;
                     if (xs[e] > 0.0f && d < a.n_docs) v = bm25_from_norm(xs[e], __ldg(ca.norm + d), cl.idf);
-                    if (OCCUR) {
+                    if (DISMAX && gr.member) {
+                        bool_dismax_member(s_m, s_t, any, j * 4 + e, v, oc);
+                    } else if (OCCUR) {
                         bool_fold_occur(acc[j * 4 + e], hits[j], req, veto, j * 4 + e, v, oc);
                     } else {
                         acc[j * 4 + e] = __fadd_rn(acc[j * 4 + e], v);
@@ -263,7 +355,9 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
                     float v = xs[e];
                     // bm25.pyx:20-25 over every doc (NaN / inf / -0.0 of exotic parameters)
                     if (!cl.sparse) v = d < a.n_docs ? bm25_one(xs[e], __ldg(ca.doc_lens + d), p) : 0.0f;
-                    if (OCCUR) {
+                    if (DISMAX && gr.member) {
+                        bool_dismax_member(s_m, s_t, any, j * 4 + e, v, oc);
+                    } else if (OCCUR) {
                         bool_fold_occur(acc[j * 4 + e], hits[j], req, veto, j * 4 + e, v, oc);
                     } else {
                         acc[j * 4 + e] = __fadd_rn(acc[j * 4 + e], v);
@@ -273,6 +367,7 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
             }
             __syncthreads();
         }
+        if (DISMAX && gr.last) bool_dismax_group_end(acc, hits, req, veto, any, s_m, s_t, gr.tie, oc.occur);
     }
 
     // 4. docs with fewer than mm hits (or a sum <= 0 / NaN), and under OCCUR docs a MUST / FILTER clause misses or a
@@ -298,6 +393,18 @@ template <bool OCCUR>
 __global__ void __launch_bounds__(SA_TERM_THREADS)
 bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ) {
     bool_tile<OCCUR, false>(a, occ, nullptr);
+}
+
+// sa_score_batch_topk_bool_dismax / sa_multi_score_batch_topk_bool_dismax: bool_fields_tile_kernel with DisMax groups.
+// The groups' running max and sum live in SA_BOOL_DISMAX_SMEM bytes of dynamic shared memory (a thread's strips,
+// owner-only, so no extra barriers); see DESIGN.md section 3.10.3 for registers and occupancy.
+#define SA_BOOL_DISMAX_SMEM (2 * SA_TILE_DOCS * sizeof(float))
+__global__ void __launch_bounds__(SA_TERM_THREADS, 2)
+bool_dismax_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
+                        const BoolGroup *__restrict__ grp) {
+    extern __shared__ __align__(16) float s_dyn[];
+    __shared__ unsigned long long s_g[3];
+    bool_tile<true, true, true>(a, occ, fld, grp, s_dyn, s_g);
 }
 
 // sa_multi_score_batch_topk_bool: roles and weights as bool_tile_kernel<true>, each clause on its own field.  Held to
@@ -329,7 +436,8 @@ struct BoolPlan {
     std::vector<BoolQuery> queries;
     std::vector<u32> group_start;       // queries [group_start[i], group_start[i + 1]) share one launch and its rows
     std::vector<BoolOccur> occur;       // per clause, as clauses; empty: Or / And (bool_tile_kernel<false>)
-    std::vector<BoolField> fields;      // per field slot (bool_fields_tile_kernel only)
+    std::vector<BoolField> fields;      // per field slot (bool_fields_tile_kernel, bool_dismax_tile_kernel)
+    std::vector<BoolGroup> groups;      // per clause, as clauses; non-empty: bool_dismax_tile_kernel
     u32 max_group = 1, max_rows = 0;
 };
 
@@ -369,7 +477,7 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
     TopkCtx t = make_topk_ctx(X.cand->p, n_tiles, nq, slots, k, d_ovf + q0);
     BoolArgs a;
     memset(&a, 0, sizeof(a));
-    if (!X.fields_kernel) {                 // the multi-field kernel reads these per clause from S.d_fields
+    if (P.fields.empty()) {                 // the field-table kernels read these per clause from S.d_fields
         a.words = ix->d_words.as<u64>();
         a.tile_dir = ix->d_tile_dir.as<u32>();
         a.recs = ix->d_recs.as<u32>();
@@ -385,7 +493,10 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
     a.clauses = S.d_clauses.as<BoolClause>();
     a.queries = S.d_queries.as<BoolQuery>() + q0;
     a.topk = t;
-    if (X.fields_kernel)
+    if (!P.groups.empty())
+        bool_dismax_tile_kernel<<<dim3(nq, n_tiles), SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
+            a, S.d_occur.as<BoolOccur>(), S.d_fields.as<BoolField>(), S.d_groups.as<BoolGroup>());
+    else if (X.fields_kernel)
         bool_fields_tile_kernel<<<dim3(nq, n_tiles), SA_TERM_THREADS, 0, ix->stream>>>(a, S.d_occur.as<BoolOccur>(),
                                                                                         S.d_fields.as<BoolField>());
     else if (P.occur.empty())
@@ -397,16 +508,28 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
     return launch_topk_select(ix, t, nq, ix->doc_base, d_keys, S.d_out_index.as<u32>() + q0);
 }
 
+// bool_dismax_tile_kernel's dynamic shared memory above the default 48 KB, and the carveout that fits two CTAs per SM
+// (~2 x 98 KB of shared memory), on the current device (function attributes are per device).
+int bool_dismax_smem() {
+    SA_CUDA(cudaFuncSetAttribute(bool_dismax_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)SA_BOOL_DISMAX_SMEM));
+    SA_CUDA(cudaFuncSetAttribute(bool_dismax_tile_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                 (int)cudaSharedmemCarveoutMaxShared));
+    return SA_OK;
+}
+
 // Every entry point, with the call's indexes locked and their device current.  clause_weight / clause_occur NULL:
 // Or / And, every clause SHOULD with weight 1, mm over all.  clause_field NULL: every clause on field 0.
+// clause_group / clause_tie non-NULL (with clause_occur): DisMax groups, bool_dismax_tile_kernel with a field table.
 int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint32_t *clause_field,
               const uint32_t *clause_terms, const uint32_t *clause_term_starts, const float *clause_idf,
-              const float *clause_weight, const uint8_t *clause_occur, const uint32_t *mm, uint32_t n_queries,
-              uint32_t slop, uint32_t k, uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+              const float *clause_weight, const uint8_t *clause_occur, const uint32_t *clause_group,
+              const float *clause_tie, const uint32_t *mm, uint32_t n_queries, uint32_t slop, uint32_t k,
+              uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
     sa_index *lead = X.lead();
     const u32 n_fields = (u32)X.ix.size();
     int rc;
-    const bool occur = clause_occur != nullptr;
+    const bool occur = clause_occur != nullptr, dismax = clause_group != nullptr;
     SA_CHECK(n_queries == 0 || query_clause_starts[0] == 0, "query_clause_starts[0] must be 0");
     for (u32 q = 0; q < n_queries; q++) {
         SA_CHECK(query_clause_starts[q + 1] > query_clause_starts[q] &&
@@ -420,10 +543,25 @@ int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint
                          (unsigned)clause_occur[c]);
                 SA_CHECK(std::isfinite(clause_weight[c]) && clause_weight[c] >= 0.0f,
                          "clause %u: a weight is finite and >= 0", c);
+                if (dismax) {
+                    // a group: consecutive clauses of one query, one occur; its tie at its first clause
+                    const u32 g = clause_group[c];
+                    SA_CHECK(g >= query_clause_starts[q] && g <= c && (g == c || clause_group[c - 1] == g),
+                             "clause %u: group %u is not a run of consecutive clauses of query %u", c, g, q);
+                    SA_CHECK(clause_occur[c] == clause_occur[g], "clause %u: the members of group %u differ in occur",
+                             c, g);
+                    if (g == c) {
+                        SA_CHECK(std::isfinite(clause_tie[c]) && clause_tie[c] >= 0.0f && clause_tie[c] <= 1.0f,
+                                 "clause %u: a tie is finite and in [0, 1]", c);
+                    } else {
+                        continue;   // mm counts groups
+                    }
+                }
                 n_should += clause_occur[c] == SA_OCCUR_SHOULD;
             }
         }
-        SA_CHECK(mm[q] <= n_should, "query %u: mm exceeds its %sclauses", q, occur ? "SHOULD " : "");
+        SA_CHECK(mm[q] <= n_should, "query %u: mm exceeds its %s", q,
+                 dismax ? "SHOULD groups" : occur ? "SHOULD clauses" : "clauses");
     }
     const u32 c_begin = n_queries ? query_clause_starts[0] : 0, c_end = n_queries ? query_clause_starts[n_queries] : 0;
     for (u32 c = c_begin; c < c_end; c++) {
@@ -470,12 +608,20 @@ int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint
             const u32 *tids = clause_terms + clause_term_starts[c];
             const u32 nt = clause_term_starts[c + 1] - clause_term_starts[c];
             if (occur) P.occur.push_back(BoolOccur{clause_weight[c], clause_occur[c]});
+            // a member of a group of two or more: scores >= +0 everywhere (sparse-safe), which its max relies on
+            const bool member = dismax && ((c > c0 && clause_group[c] == clause_group[c - 1]) ||
+                                           (c + 1 < c1 && clause_group[c + 1] == clause_group[c]));
+            if (dismax)
+                P.groups.push_back(BoolGroup{clause_tie[clause_group[c]], clause_group[c] - c0, member ? 1u : 0u,
+                                             member && (c + 1 == c1 || clause_group[c + 1] != clause_group[c]) ? 1u : 0u});
             if (X.avgdl[f] == 0.0f) {       // scores +0 at every doc: no list, no row
                 P.clauses.push_back(BoolClause{0, 0, SA_NO_DIR, SA_NO_DIR, clause_idf[c], SA_BOOL_NO_ROW, 1u, f});
                 continue;
             }
             const bool sparse = make_bm25(clause_idf[c], X.avgdl[f], X.k1[f], X.b[f], ix->doc_lens_nonneg).sparse_ok != 0;
             SA_CHECK(nt == 1 || sparse, "phrase queries in a batch need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite idf)");
+            SA_CHECK(!member || sparse, "clause %u: DisMax members need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, "
+                     "finite idf >= 0)", c);
             const TermQuery tq = make_term_query(ix, nt == 1 ? tids[0] : SA_NO_TERM, clause_idf[c]);
             P.clauses.push_back(BoolClause{tq.word_off, tq.n_words, tq.dir_off, tq.rec_off, clause_idf[c],
                                            nt == 1 ? SA_BOOL_NO_ROW : rows++, sparse ? 1u : 0u, f});
@@ -493,11 +639,12 @@ int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint
         (rc = S.d_out_index.reserve((size_t)n_queries * sizeof(u32))) || (rc = S.d_keys.reserve(key_bytes)) ||
         (rc = S.rows.reserve(std::max<size_t>((size_t)P.max_rows * stride * sizeof(float), 64))) ||
         (rc = S.d_occur.reserve(P.occur.size() * sizeof(BoolOccur))) ||
+        (rc = S.d_groups.reserve(P.groups.size() * sizeof(BoolGroup))) ||
         (rc = X.h_pinned->reserve(key_bytes)))
         return rc;
     for (u32 f = 0; f < n_fields; f++)
         if (field_sparse[f] && (rc = sa_ensure_norm(X.ix[f], X.k1[f], X.b[f], X.avgdl[f]))) return rc;
-    if (X.fields_kernel) {
+    if (X.fields_kernel || dismax) {
         for (u32 f = 0; f < n_fields; f++) {
             sa_index *ix = X.ix[f];
             P.fields.push_back(BoolField{ix->d_words.as<u64>(), ix->d_tile_dir.as<u32>(), ix->d_recs.as<u32>(),
@@ -513,6 +660,10 @@ int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint
     SA_CUDA(cudaMemcpyAsync(S.d_clauses.p, P.clauses.data(), P.clauses.size() * sizeof(BoolClause), cudaMemcpyHostToDevice, lead->stream));
     if (occur) {
         SA_CUDA(cudaMemcpyAsync(S.d_occur.p, P.occur.data(), P.occur.size() * sizeof(BoolOccur), cudaMemcpyHostToDevice, lead->stream));
+    }
+    if (dismax) {
+        if ((rc = bool_dismax_smem())) return rc;
+        SA_CUDA(cudaMemcpyAsync(S.d_groups.p, P.groups.data(), P.groups.size() * sizeof(BoolGroup), cudaMemcpyHostToDevice, lead->stream));
     }
     SA_CUDA(cudaMemcpyAsync(S.d_queries.p, P.queries.data(), P.queries.size() * sizeof(BoolQuery), cudaMemcpyHostToDevice, lead->stream));
     SA_CUDA(cudaMemcpyAsync(S.d_out_index.p, identity.data(), (size_t)n_queries * sizeof(u32), cudaMemcpyHostToDevice, lead->stream));
@@ -548,7 +699,8 @@ int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint
 // The single-index entry points: the index's own lock, state and buffers.
 int bool_topk_index(sa_index *ix, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
                     const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
-                    const uint8_t *clause_occur, const uint32_t *mm, uint32_t n_queries, uint32_t slop,
+                    const uint8_t *clause_occur, const uint32_t *clause_group, const float *clause_tie,
+                    const uint32_t *mm, uint32_t n_queries, uint32_t slop,
                     float avg_doc_len, float k1, float b, uint32_t k, uint32_t *out_docs, float *out_scores,
                     uint32_t *n_redone) {
     SA_CHECK(ix && out_docs && out_scores, "NULL argument");
@@ -568,37 +720,16 @@ int bool_topk_index(sa_index *ix, const uint32_t *query_clause_starts, const uin
     X.cand = &ix->cand;
     X.h_pinned = &ix->h_pinned;
     return bool_topk(X, query_clause_starts, nullptr, clause_terms, clause_term_starts, clause_idf, clause_weight,
-                     clause_occur, mm, n_queries, slop, k, out_docs, out_scores, n_redone);
+                     clause_occur, clause_group, clause_tie, mm, n_queries, slop, k, out_docs, out_scores, n_redone);
 }
 
-}  // namespace
-
-extern "C" int sa_score_batch_topk_bool(sa_index *ix, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
-                                        const uint32_t *clause_term_starts, const float *clause_idf, const uint32_t *mm,
-                                        uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
-                                        uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
-    return bool_topk_index(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, nullptr, nullptr, mm,
-                           n_queries, slop, avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
-}
-
-extern "C" int sa_score_batch_topk_bool_occur(sa_index *ix, const uint32_t *query_clause_starts,
-                                              const uint32_t *clause_terms, const uint32_t *clause_term_starts,
-                                              const float *clause_idf, const float *clause_weight,
-                                              const uint8_t *clause_occur, const uint32_t *mm, uint32_t n_queries,
-                                              uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
-                                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
-    SA_CHECK(n_queries == 0 || (clause_weight && clause_occur), "NULL argument");
-    return bool_topk_index(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, clause_weight,
-                           clause_occur, mm, n_queries, slop, avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
-}
-
-extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, const uint32_t *query_clause_starts,
-                                              const uint32_t *clause_field, const uint32_t *clause_terms,
-                                              const uint32_t *clause_term_starts, const float *clause_idf,
-                                              const float *clause_weight, const uint8_t *clause_occur,
-                                              const uint32_t *mm, uint32_t n_queries, uint32_t slop,
-                                              const float *avg_doc_len, const float *k1, const float *b, uint32_t k,
-                                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+// The multi-field entry points: the multi's lock, state and candidate buffer.
+int bool_topk_multi(sa_multi *m, const uint32_t *query_clause_starts, const uint32_t *clause_field,
+                    const uint32_t *clause_terms, const uint32_t *clause_term_starts, const float *clause_idf,
+                    const float *clause_weight, const uint8_t *clause_occur, const uint32_t *clause_group,
+                    const float *clause_tie, const uint32_t *mm, uint32_t n_queries, uint32_t slop,
+                    const float *avg_doc_len, const float *k1, const float *b, uint32_t k, uint32_t *out_docs,
+                    float *out_scores, uint32_t *n_redone) {
     SA_CHECK(m && out_docs && out_scores && avg_doc_len && k1 && b, "NULL argument");
     SA_CHECK(n_queries == 0 || (query_clause_starts && clause_field && clause_terms && clause_term_starts &&
                                 clause_idf && clause_weight && clause_occur && mm), "NULL argument");
@@ -631,5 +762,67 @@ extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, const uint32_t *query
     X.cand = &m->cand;
     X.h_pinned = &m->fields[0]->h_pinned;
     return bool_topk(X, query_clause_starts, clause_field, clause_terms, clause_term_starts, clause_idf, clause_weight,
-                     clause_occur, mm, n_queries, slop, k, out_docs, out_scores, n_redone);
+                     clause_occur, clause_group, clause_tie, mm, n_queries, slop, k, out_docs, out_scores, n_redone);
+}
+
+}  // namespace
+
+extern "C" int sa_score_batch_topk_bool(sa_index *ix, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
+                                        const uint32_t *clause_term_starts, const float *clause_idf, const uint32_t *mm,
+                                        uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
+                                        uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+    return bool_topk_index(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, nullptr, nullptr,
+                           nullptr, nullptr, mm, n_queries, slop, avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
+}
+
+extern "C" int sa_score_batch_topk_bool_occur(sa_index *ix, const uint32_t *query_clause_starts,
+                                              const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                              const float *clause_idf, const float *clause_weight,
+                                              const uint8_t *clause_occur, const uint32_t *mm, uint32_t n_queries,
+                                              uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
+                                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+    SA_CHECK(n_queries == 0 || (clause_weight && clause_occur), "NULL argument");
+    return bool_topk_index(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, clause_weight,
+                           clause_occur, nullptr, nullptr, mm, n_queries, slop, avg_doc_len, k1, b, k, out_docs,
+                           out_scores, n_redone);
+}
+
+extern "C" int sa_score_batch_topk_bool_dismax(sa_index *ix, const uint32_t *query_clause_starts,
+                                               const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                               const float *clause_idf, const float *clause_weight,
+                                               const uint8_t *clause_occur, const uint32_t *clause_group,
+                                               const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
+                                               uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
+                                               uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+    SA_CHECK(n_queries == 0 || (clause_weight && clause_occur && clause_group && clause_tie), "NULL argument");
+    return bool_topk_index(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, clause_weight,
+                           clause_occur, clause_group, clause_tie, mm, n_queries, slop, avg_doc_len, k1, b, k,
+                           out_docs, out_scores, n_redone);
+}
+
+extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, const uint32_t *query_clause_starts,
+                                              const uint32_t *clause_field, const uint32_t *clause_terms,
+                                              const uint32_t *clause_term_starts, const float *clause_idf,
+                                              const float *clause_weight, const uint8_t *clause_occur,
+                                              const uint32_t *mm, uint32_t n_queries, uint32_t slop,
+                                              const float *avg_doc_len, const float *k1, const float *b, uint32_t k,
+                                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+    return bool_topk_multi(m, query_clause_starts, clause_field, clause_terms, clause_term_starts, clause_idf,
+                           clause_weight, clause_occur, nullptr, nullptr, mm, n_queries, slop, avg_doc_len, k1, b, k,
+                           out_docs, out_scores, n_redone);
+}
+
+extern "C" int sa_multi_score_batch_topk_bool_dismax(sa_multi *m, const uint32_t *query_clause_starts,
+                                                     const uint32_t *clause_field, const uint32_t *clause_terms,
+                                                     const uint32_t *clause_term_starts, const float *clause_idf,
+                                                     const float *clause_weight, const uint8_t *clause_occur,
+                                                     const uint32_t *clause_group, const float *clause_tie,
+                                                     const uint32_t *mm, uint32_t n_queries, uint32_t slop,
+                                                     const float *avg_doc_len, const float *k1, const float *b,
+                                                     uint32_t k, uint32_t *out_docs, float *out_scores,
+                                                     uint32_t *n_redone) {
+    SA_CHECK(n_queries == 0 || (clause_group && clause_tie), "NULL argument");
+    return bool_topk_multi(m, query_clause_starts, clause_field, clause_terms, clause_term_starts, clause_idf,
+                           clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, avg_doc_len,
+                           k1, b, k, out_docs, out_scores, n_redone);
 }

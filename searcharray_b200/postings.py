@@ -511,7 +511,12 @@ class SearchArray(ExtensionArray):
         query.Bool(must, should, filter, must_not, mm) and query.Boost(clause, weight) clauses are accepted the same
         way: s = w0 * .score(c0) + w1 * .score(c1) + ... over must + should (float32, each product rounded), ranked
         where s > 0, every must and filter clause scores > 0, no must_not clause does and at least mm should clauses
-        do (sa_score_batch_topk_bool_occur).  An Or / And whose weights are all 1 takes the path above unchanged."""
+        do (sa_score_batch_topk_bool_occur).  An Or / And whose weights are all 1 takes the path above unchanged.
+
+        query.DisMax(clauses, tie) is accepted as a clause of these, and as a query of its own (Bool(should=[it])):
+        one clause scoring d = max_j v_j + (sum_j v_j - max_j v_j) * tie over its members' v_j = w_j * .score(c_j),
+        matched where any member scores > 0 (sa_score_batch_topk_bool_dismax) -- synonyms as
+        DisMax(["film", "movie"], tie=0.1).  Its members need k1 > 0 and 0 <= b < 1 (ValueError otherwise)."""
         from .query import is_boolean
         if any(is_boolean(q) for q in queries):
             return self._search_topk_mixed(list(queries), k, similarity, slop)
@@ -536,7 +541,7 @@ class SearchArray(ExtensionArray):
         """search_topk of a batch holding boolean queries: the plain ones through search_topk as before, the boolean
         ones through sa_score_batch_topk_bool (Or / And with weights 1) or sa_score_batch_topk_bool_occur (Bool,
         boosted Or / And), each clause with the idf .score gives it; results in query order."""
-        from .query import has_field, is_boolean, needs_occur
+        from .query import has_dismax, has_field, is_boolean, needs_occur
         if any(has_field(q) for q in queries if is_boolean(q)):
             raise ValueError("a Field clause names a DataFrame column: run queries over columns with "
                              "solr.fields_topk(frame, queries), not SearchArray.search_topk")
@@ -545,19 +550,51 @@ class SearchArray(ExtensionArray):
                                       "compose .score() on the view")
         if not isinstance(similarity, Bm25Similarity):
             raise TypeError(f"boolean queries support bm25_similarity only, not {similarity!r}")
-        kind = np.asarray([(needs_occur(q) + 1) if is_boolean(q) else 0 for q in queries])   # plain, Or, occur
+        kind = np.asarray([(3 if has_dismax(q) else needs_occur(q) + 1) if is_boolean(q) else 0
+                           for q in queries])                       # plain, Or, occur, DisMax
+        if np.any(kind == 3):
+            self._check_dismax_params(similarity)
         docs = np.empty((len(queries), k), dtype=np.uint32)
         scores = np.empty((len(queries), k), dtype=np.float32)
-        for kd in (0, 1, 2):
+        for kd in (0, 1, 2, 3):
             sel = kind == kd
             part = [q for q, s in zip(queries, sel) if s]
             if not part:
                 continue
             if kd == 0:
                 docs[sel], scores[sel] = self.search_topk(part, k=k, similarity=similarity, slop=slop)
+            elif kd == 3:
+                docs[sel], scores[sel], _ = self._search_topk_dismax(part, k, similarity, slop)
             else:
                 docs[sel], scores[sel], _ = self._search_topk_bool(part, k, similarity, slop)
         return docs, scores
+
+    def _check_dismax_params(self, similarity):
+        """ValueError, before any device work, where DisMax members would not be sparse-safe for k1 / b."""
+        from .query import check_dismax_members
+        check_dismax_members([(0, "DisMax member")], lambda i: (similarity.k1, similarity.b, self.avg_doc_length, 0.0))
+
+    def _search_topk_dismax(self, queries, k, similarity, slop):
+        """Boolean queries holding a DisMax through sa_score_batch_topk_bool_dismax: (docs, scores, queries re-run
+        exactly).  Every DisMax member needs sparse-safe BM25 parameters (ValueError before any device work)."""
+        from .query import check_dismax_members, dismax_members, flatten_dismax
+        clauses, q_starts, mm, weights, occurs, groups, ties = flatten_dismax(queries)
+        dev = self._device()
+        docs = np.empty((len(queries), k), dtype=np.uint32)
+        scores = np.empty((len(queries), k), dtype=np.float32)
+        n_redone = ctypes.c_uint32(0)
+        terms, c_starts, idfs = self._topk_queries(clauses, lambda dfs: compute_idf(self.corpus_size, dfs))
+        idfs = np.asarray(idfs, dtype=np.float32)
+        check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
+                             lambda i: (similarity.k1, similarity.b, self.avg_doc_length, idfs[i]))
+        with self._shared["lock"]:
+            self._apply_rows(dev)
+            _lib.check(_lib.lib().sa_score_batch_topk_bool_dismax(
+                dev.handle, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
+                _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(groups), _lib.p_f32(ties), _lib.p_u32(mm),
+                len(queries), int(slop), self.avg_doc_length, similarity.k1, similarity.b, k, _lib.p_u32(docs),
+                _lib.p_f32(scores), ctypes.byref(n_redone)))
+        return docs, scores, n_redone.value
 
     def _search_topk_bool(self, queries, k, similarity, slop):
         """Boolean queries through sa_score_batch_topk_bool, or through sa_score_batch_topk_bool_occur when one of

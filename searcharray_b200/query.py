@@ -6,7 +6,9 @@ where at least mm clauses score > 0 -- the reference's own composition of multi-
 (test/test_search.py:126-226) -- and search_topk returns the top k of it by (score desc, doc asc), computed on the
 device (sa_score_batch_topk_bool).  Bool(must, should, filter, must_not, mm) and Boost(clause, weight) extend that
 composition (sa_score_batch_topk_bool_occur).  Field(field, clause) names the DataFrame column a clause scores on,
-for queries over several columns (solr.fields_topk, sa_multi_score_batch_topk_bool)."""
+for queries over several columns (solr.fields_topk, sa_multi_score_batch_topk_bool).  DisMax(clauses, tie) is one
+clause scored by its best member plus tie times the others (Lucene's DisjunctionMaxQuery;
+sa_score_batch_topk_bool_dismax, sa_multi_score_batch_topk_bool_dismax)."""
 import math
 from typing import List, Union
 
@@ -22,9 +24,9 @@ Clause = Union[str, List[str]]
 
 
 def _clause(c):
-    """A clause as search_topk's query form: str (term) or list[str] (phrase), or a Field of one; anything else is a
-    TypeError."""
-    if isinstance(c, (str, Field)):
+    """A clause as search_topk's query form: str (term) or list[str] (phrase), a Field of one, or a DisMax; anything
+    else is a TypeError."""
+    if isinstance(c, (str, Field, DisMax)):
         return c
     if isinstance(c, (list, tuple)) and c and all(isinstance(t, str) for t in c):
         return list(c)
@@ -40,7 +42,7 @@ class Field:
     def __init__(self, field, clause):
         if not isinstance(field, str):
             raise TypeError(f"a field is a column name (str), not {field!r}")
-        if isinstance(clause, (Boost, Field)):
+        if isinstance(clause, (Boost, Field, DisMax)):
             raise TypeError(f"a Field holds a term or a phrase; boost a field clause as Boost(Field(...), w), not {clause!r}")
         self.field = field
         self.clause = _clause(clause)
@@ -56,6 +58,8 @@ class Boost:
     weight of 0 matches without scoring.  Accepted where a clause scores: in Or, And, Bool's must and should."""
 
     def __init__(self, clause, weight):
+        if isinstance(clause, DisMax):
+            raise TypeError(f"a DisMax takes no Boost: boost its members instead, as edismax's qf boosts do: {clause!r}")
         self.clause = _clause(clause)
         w = float(weight)
         if not math.isfinite(w) or w < 0:
@@ -79,6 +83,49 @@ def _scoring(clauses):
     return out, weights
 
 
+class DisMax:
+    """One clause scored by its best member: Lucene's DisjunctionMaxQuery, Elasticsearch's dis_max, the per-term qf
+    part of edismax.  With v_j = float32(w_j * score(c_j)) (w_j the member's Boost, 1 without one),
+    d = m + (t - m) * tie, m = max_j v_j, t = v_0 + v_1 + ... folded left in member order, every operation rounded to
+    float32.  The DisMax matches a doc where any member scores > 0 (unweighted, so a zero-weight member still matches).
+
+    clauses: at least one member, each a term (str), a phrase (list[str], matched with the call's slop), a Field of
+    either, or a Boost of any of these; a DisMax, Or, And or Bool member is a TypeError.  tie: finite, in [0, 1],
+    rounded to float32 once.  Accepted wherever a clause is (Or, And, the four lists of Bool), where it is one clause
+    (it counts once towards mm and adds d with weight 1); as a query of its own it is Bool(should=[it]).  It takes no
+    Boost itself.  Members need sparse-safe BM25 parameters (k1 > 0, 0 <= b < 1), as phrase clauses do.
+    DisMax([c]) scores exactly as c."""
+
+    def __init__(self, clauses, tie=0.0):
+        clauses = list(clauses)
+        if not clauses:
+            raise ValueError("a DisMax needs at least one member")
+        for c in clauses:
+            inner = c.clause if isinstance(c, Boost) else c
+            if isinstance(inner, (DisMax, Or, Bool)):
+                raise TypeError(f"a DisMax member is a term, a phrase or a Field of one (boosted or not), not {c!r}")
+        self.clauses, self.weights = _scoring(clauses)
+        t = float(tie)
+        if not math.isfinite(t) or not 0.0 <= t <= 1.0:
+            raise ValueError(f"a DisMax tie is finite and in [0, 1], not {tie!r}")
+        self.tie = np.float32(t)
+        _check_count(len(self.clauses))
+
+    @property
+    def boosted(self):
+        """Whether any member has a weight other than 1."""
+        return any(w != 1.0 for w in self.weights)
+
+    def __repr__(self):
+        shown = [Boost(c, w) if w != 1.0 else c for c, w in zip(self.clauses, self.weights)]
+        return f"DisMax({shown!r}, tie={float(self.tie)!r})"
+
+
+def _n_clauses(clauses):
+    """The clauses a list holds as the device counts them: a DisMax counts its members."""
+    return sum(len(c.clauses) if isinstance(c, DisMax) else 1 for c in clauses)
+
+
 def _check_count(n):
     if n > SA_BOOL_MAX_CLAUSES:
         raise ValueError(f"a boolean query has at most {SA_BOOL_MAX_CLAUSES} clauses, not {n}")
@@ -95,7 +142,7 @@ class Or:
         clauses = list(clauses)
         if not clauses:
             raise ValueError("a boolean query needs at least one clause")
-        _check_count(len(clauses))
+        _check_count(_n_clauses(clauses))
         self.clauses, self.weights = _scoring(clauses)
         self.mm = parse_min_should_match(len(self.clauses), str(mm))
 
@@ -133,7 +180,7 @@ class Bool:
         must, should, filter, must_not = list(must), list(should), list(filter), list(must_not)
         for role, cs in (("filter", filter), ("must_not", must_not)):
             for c in cs:
-                if isinstance(c, Boost):
+                if isinstance(c, Boost) or (isinstance(c, DisMax) and c.boosted):
                     raise ValueError(f"a {role} clause adds nothing to the score and takes no Boost: {c!r}")
         self.must, self.must_weights = _scoring(must)
         self.should, self.should_weights = _scoring(should)
@@ -141,7 +188,7 @@ class Bool:
         self.must_not = [_clause(c) for c in must_not]
         if not self.must and not self.should:
             raise ValueError("a Bool query needs at least one must or should clause: nothing else scores")
-        _check_count(len(must) + len(should) + len(filter) + len(must_not))
+        _check_count(_n_clauses(must + should + filter + must_not))
         if mm is None:
             mm = 0 if (self.must or self.filter) else 1
         self.mm = parse_min_should_match(len(self.should), str(mm))
@@ -165,13 +212,24 @@ class Bool:
 
 def is_boolean(q):
     """Whether search_topk routes q to the boolean path."""
-    return isinstance(q, (Or, Bool))
+    return isinstance(q, (Or, Bool, DisMax))
+
+
+def _top_clauses(q):
+    """The clauses of an Or / And / Bool, or a top-level DisMax as the one clause it is."""
+    if isinstance(q, DisMax):
+        return [q]
+    return q.occur_clauses()[0] if isinstance(q, Bool) else q.clauses
 
 
 def has_field(q):
-    """Whether a boolean query holds a Field clause (solr.fields_topk's form)."""
-    clauses = q.occur_clauses()[0] if isinstance(q, Bool) else q.clauses
-    return any(isinstance(c, Field) for c in clauses)
+    """Whether a boolean query holds a Field clause (solr.fields_topk's form), a DisMax's members included."""
+    return any(isinstance(m, Field) for c in _top_clauses(q) for m in (c.clauses if isinstance(c, DisMax) else [c]))
+
+
+def has_dismax(q):
+    """Whether q is or holds a DisMax (sa_score_batch_topk_bool_dismax's form)."""
+    return any(isinstance(c, DisMax) for c in _top_clauses(q))
 
 
 def needs_occur(q):
@@ -207,3 +265,65 @@ def flatten_occur(queries):
         mm.append(q.mm)
     return (clauses, np.asarray(starts, dtype=np.uint32), np.asarray(mm, dtype=np.uint32),
             np.asarray(weights, dtype=np.float32), np.asarray(occurs, dtype=np.uint8))
+
+
+def flatten_dismax(queries):
+    """Or / And / Bool / DisMax queries as sa_score_batch_topk_bool_dismax takes them: flatten_occur's arrays, with
+    each DisMax expanded into its members (their own weights, the DisMax's role), and per clause uint32 clause_group
+    (the batch-wide index of the first clause of its group; the clause itself outside a DisMax) and float32
+    clause_tie (the group's tie; 0 outside a DisMax).  A top-level DisMax is Bool(should=[it])."""
+    clauses, starts, mm, weights, occurs, groups, ties = [], [0], [], [], [], [], []
+    for q in queries:
+        if isinstance(q, DisMax):
+            cs, ws, os_, qmm = [q], [np.float32(1.0)], [SA_OCCUR_SHOULD], 1
+        elif isinstance(q, Bool):
+            cs, ws, os_ = q.occur_clauses()
+            qmm = q.mm
+        else:
+            cs, ws, os_, qmm = q.clauses, q.weights, [SA_OCCUR_SHOULD] * len(q.clauses), q.mm
+        for c, w, o in zip(cs, ws, os_):
+            first = len(clauses)
+            if isinstance(c, DisMax):
+                for m, mw in zip(c.clauses, c.weights):
+                    clauses.append(m)
+                    weights.append(mw)
+                    occurs.append(o)
+                    groups.append(first)
+                    ties.append(c.tie)
+            else:
+                clauses.append(c)
+                weights.append(w)
+                occurs.append(o)
+                groups.append(first)
+                ties.append(np.float32(0.0))
+        starts.append(len(clauses))
+        mm.append(qmm)
+    return (clauses, np.asarray(starts, dtype=np.uint32), np.asarray(mm, dtype=np.uint32),
+            np.asarray(weights, dtype=np.float32), np.asarray(occurs, dtype=np.uint8),
+            np.asarray(groups, dtype=np.uint32), np.asarray(ties, dtype=np.float32))
+
+
+def dismax_members(queries):
+    """Indices, into flatten_dismax's clause list, of the clauses that are DisMax members."""
+    out, n = [], 0
+    for q in queries:
+        for c in _top_clauses(q):
+            k = len(c.clauses) if isinstance(c, DisMax) else 1
+            if isinstance(c, DisMax):
+                out.extend(range(n, n + k))
+            n += k
+    return out
+
+
+def check_dismax_members(members, params):
+    """ValueError unless every DisMax member can be ranked by its max: params(i) -> (k1, b, avgdl, idf) of member i
+    must be sparse-safe (k1 > 0, 0 <= b < 1, finite idf >= 0), so that every weighted score is >= +0.  A member on a
+    column whose avgdl is 0 scores 0 everywhere and is accepted.  members: (index, clause) pairs."""
+    for i, c in members:
+        k1, b, avgdl, idf = (np.float32(x) for x in params(i))
+        if avgdl == 0:
+            continue
+        if not (np.isfinite(k1) and k1 > 0 and 0 <= b < 1 and np.isfinite(avgdl) and avgdl > 0 and np.isfinite(idf)
+                and idf >= 0 and not np.signbit(idf)):
+            raise ValueError(f"DisMax members need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite idf >= 0): "
+                             f"{c!r} has k1={float(k1)}, b={float(b)}, idf={float(idf)}")

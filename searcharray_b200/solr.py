@@ -408,14 +408,15 @@ def edismax_topk(frame: pd.DataFrame, q: str, qf: List[str], k: int = 10, mm: Op
 
 
 def _fields_plan(frame, queries, similarity):
-    """fields_topk's refusals and field slots, before any device work: (flatten_occur's arrays, the Field clauses,
-    field name -> slot, per-slot arrays, per-slot similarities)."""
-    from .query import ED_MAX_FIELDS, Field, flatten_occur, is_boolean
+    """fields_topk's refusals and field slots, before any device work: (flatten_occur's arrays, or flatten_dismax's
+    when a query holds a DisMax, field name -> slot, per-slot arrays, per-slot similarities)."""
+    from .query import ED_MAX_FIELDS, Field, flatten_dismax, flatten_occur, has_dismax, is_boolean
     queries = list(queries)
     for q in queries:
         if not is_boolean(q):
-            raise TypeError(f"fields_topk takes Or / And / Bool queries, not {q!r}")
-    clauses, q_starts, mm, weights, occurs = flatten_occur(queries)
+            raise TypeError(f"fields_topk takes Or / And / Bool / DisMax queries, not {q!r}")
+    flat = flatten_dismax(queries) if any(has_dismax(q) for q in queries) else flatten_occur(queries)
+    clauses = flat[0]
     for c in clauses:
         if not isinstance(c, Field):
             raise ValueError(f"every clause of fields_topk names its column: Field(field, {c!r})")
@@ -454,7 +455,12 @@ def _fields_plan(frame, queries, similarity):
         slot_arrays.append(a)
         slot_sims.append(sim)
         slot_name.append(f)
-    return (clauses, q_starts, mm, weights, occurs), slot_of, slot_arrays, slot_sims
+    if len(flat) == 7:                    # DisMax members: sparse-safe k1 / b on their fields (idf: _fields_clauses)
+        from .query import check_dismax_members, dismax_members
+        check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
+                             lambda i: (sims[clauses[i].field].k1, sims[clauses[i].field].b,
+                                        arrays[clauses[i].field].avg_doc_length, 0.0))
+    return flat, slot_of, slot_arrays, slot_sims
 
 
 def _fields_clauses(clauses, slot_of, arrays):
@@ -474,8 +480,9 @@ def _fields_clauses(clauses, slot_of, arrays):
 
 
 def _fields_call(multi, arrays, sims, flat, prepared, k, slop):
-    """sa_multi_score_batch_topk_bool on prepared arrays (the fields locked): (docs, scores, queries re-run)."""
-    _, q_starts, mm, weights, occurs = flat
+    """sa_multi_score_batch_topk_bool, or sa_multi_score_batch_topk_bool_dismax for flatten_dismax's arrays, on
+    prepared arrays (the fields locked): (docs, scores, queries re-run)."""
+    q_starts, mm, weights, occurs = flat[1:5]
     terms, c_starts, c_idf, c_field = prepared
     nq = len(q_starts) - 1
     docs = np.empty((nq, k), dtype=np.uint32)
@@ -483,6 +490,14 @@ def _fields_call(multi, arrays, sims, flat, prepared, k, slop):
     n_redone = ctypes.c_uint32(0)
     avgdl = _f32([a.avg_doc_length for a in arrays])
     k1, b = _f32([s.k1 for s in sims]), _f32([s.b for s in sims])
+    if len(flat) == 7:
+        groups, ties = flat[5:]
+        _lib.check(_lib.lib().sa_multi_score_batch_topk_bool_dismax(
+            multi.handle, _lib.p_u32(q_starts), _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts),
+            _lib.p_f32(c_idf), _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(groups), _lib.p_f32(ties),
+            _lib.p_u32(mm), nq, int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1), _lib.p_f32(b), k, _lib.p_u32(docs),
+            _lib.p_f32(scores), ctypes.byref(n_redone)))
+        return docs, scores, n_redone.value
     _lib.check(_lib.lib().sa_multi_score_batch_topk_bool(
         multi.handle, _lib.p_u32(q_starts), _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts),
         _lib.p_f32(c_idf), _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(mm), nq, int(slop), _lib.p_f32(avgdl),
@@ -492,12 +507,19 @@ def _fields_call(multi, arrays, sims, flat, prepared, k, slop):
 
 def _fields_topk(frame, queries, k, similarity, slop):
     """fields_topk and the number of queries re-run exactly (candidate overflow)."""
+    queries = list(queries)
     flat, slot_of, arrays, sims = _fields_plan(frame, queries, similarity)
     multi = _multi_for(arrays)
     with _locked(multi, arrays):
         for arr in arrays:                 # a sliced view of the same column may have left its row filter installed
             arr._apply_rows(arr._device())
         prepared = _fields_clauses(flat[0], slot_of, arrays)
+        if len(flat) == 7:                # DisMax members: sparse-safe idf from their own fields
+            from .query import check_dismax_members, dismax_members
+            clauses = flat[0]
+            check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
+                                 lambda i: (sims[slot_of[clauses[i].field]].k1, sims[slot_of[clauses[i].field]].b,
+                                            arrays[slot_of[clauses[i].field]].avg_doc_length, prepared[2][i]))
         return _fields_call(multi, arrays, sims, flat, prepared, k, slop)
 
 
@@ -514,6 +536,12 @@ def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
     column's idf, avgdl and doc lengths.  Returns (rows uint32[Q, k], scores float32[Q, k]); empty slots are NO_DOC /
     0; on a shard the rows are global doc ids.  Views, non-BM25 similarities, more than 8 distinct fields, columns of
     different lengths or devices, and two names of one column under different similarities are refused before any
-    device work."""
+    device work.
+
+    A query.DisMax of Field members is one clause scoring d = max_j v_j + (sum_j v_j - max_j v_j) * tie over
+    v_j = w_j * score(member j), each member on its own column (sa_multi_score_batch_topk_bool_dismax): Elasticsearch's
+    best_fields as DisMax([Boost(Field("title", "alien"), 2), Field("overview", "alien")], tie=0.3), and edismax's
+    term-centric qf as an Or of one such DisMax per term with a Solr mm.  Its members need k1 > 0 and 0 <= b < 1 on
+    their fields (ValueError otherwise)."""
     docs, scores, _ = _fields_topk(frame, queries, k, similarity, slop)
     return docs, scores
