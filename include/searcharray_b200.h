@@ -197,6 +197,24 @@ int sa_score_batch_topk_bool_dismax(sa_index *index, const uint32_t *query_claus
                                     const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
                                     uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
                                     uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
+/* Nested boolean queries: an Or / And / Bool used as a clause of another.  Nodes 0 .. n_queries-1 are the queries
+ * whose top k is returned; nodes n_queries .. n_nodes-1 are nested queries.  Node n owns clauses
+ * [node_clause_starts[n], node_clause_starts[n+1]) (node_clause_starts[0] == 0), with the per-clause arrays, DisMax
+ * groups and mm[n] of sa_score_batch_topk_bool_dismax, checked per node.  clause_node[c] == SA_NO_NODE: a leaf, its terms
+ * clause_terms[clause_term_starts[c] ..).  Otherwise c is nested node clause_node[c]: it has no terms, the node's index
+ * is above that of the node holding c, no other clause references it, and c is not a DisMax member; every nested node
+ * is referenced.  A nested node N scores r_N(d) = the score N ranks doc d with as a query of its own (s_N(d) where
+ * all its conditions hold and s_N(d) > 0, +0 elsewhere), and matches where r_N(d) > 0: it adds w * r_N under MUST /
+ * SHOULD (rounded, then added), counts once towards its holder's mm, and under FILTER / MUST_NOT plays a leaf's role.
+ * Queries without a nested clause score as in sa_score_batch_topk_bool_dismax, bit for bit. */
+#define SA_NO_NODE 0xFFFFFFFFu
+int sa_score_batch_topk_bool_nested(sa_index *index, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                    const uint32_t *clause_node, const uint32_t *clause_terms,
+                                    const uint32_t *clause_term_starts, const float *clause_idf,
+                                    const float *clause_weight, const uint8_t *clause_occur,
+                                    const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
+                                    uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
+                                    uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
 
 /* The same batch in three stages, so a serving loop (or the benchmark) can keep the query
  * descriptors resident and time the device work alone: upload (H2D of descriptors), execute
@@ -320,6 +338,16 @@ int sa_multi_score_batch_topk_bool_dismax(sa_multi *multi, const uint32_t *query
                                           uint32_t n_queries, uint32_t slop, const float *avg_doc_len, const float *k1,
                                           const float *b, uint32_t k, uint32_t *out_docs, float *out_scores,
                                           uint32_t *n_redone);
+/* sa_multi_score_batch_topk_bool_dismax with the nested nodes of sa_score_batch_topk_bool_nested: clause_field[c] is
+ * read for leaves only. */
+int sa_multi_score_batch_topk_bool_nested(sa_multi *multi, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                          const uint32_t *clause_node, const uint32_t *clause_field,
+                                          const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                          const float *clause_idf, const float *clause_weight,
+                                          const uint8_t *clause_occur, const uint32_t *clause_group,
+                                          const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
+                                          uint32_t slop, const float *avg_doc_len, const float *k1, const float *b,
+                                          uint32_t k, uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
 
 /* ------------------------------------------------- per-op exports (parity tests)
  * Device implementations of the reference's native ops on raw arrays (host in, host out),

@@ -34,6 +34,13 @@
 // owned doc in per-thread strips of dynamic shared memory, and a u32 mask records where any member scores > 0; at the
 // group's last member d = m + (t - m) * tie is folded with weight 1 under the group's role, its hit being the mask.
 // A group is present in a tile iff any member is.
+//
+// bool_nested_tile_kernel (sa_score_batch_topk_bool_nested, sa_multi_score_batch_topk_bool_nested) is the DisMax fold
+// with nested queries: an Or / And / Bool used as a clause of another.  Each nested node is materialised first, deepest
+// level first, by the same fold in a store pass: its ranked values (0 where it does not rank) go to its row in
+// BoolState::rows and a per-(row, tile) flag records whether anything ranked, a tile that ranks nothing writing only
+// its flag.  A parent reads a nested clause's row as the clause's score (no BM25), present in a tile iff the child's
+// flag is set; the top-level nodes are collected and selected as in every other instance.
 #include "sa_multi.cuh"
 #include "sa_term.cuh"
 #include "sa_phrase.cuh"
@@ -86,9 +93,21 @@ struct BoolGroup {
     u32 last;       // 1: the group's last member
 };
 
+// The nested-query part of bool_nested_tile_kernel's arguments.  A nested node's row is BoolQuery::pad (its slot in
+// BoolState::rows, numbered with the phrase rows of its launch group); a nested clause's BoolClause::row is its
+// child's row.
+struct BoolNest {
+    const u32 *nested;  // per clause, as a.clauses: 1: a nested clause, scored by its child's row as stored
+    u32 *flags;         // [row * n_tiles + tile]: 1 where the nested node of that row ranks a doc of the tile
+    float *store;       // the store pass: a.rows, written at each node's row; NULL: top-level nodes, collected
+    u32 n_tiles;
+};
+
 struct BoolState {
     DevBuf d_clauses, d_queries, d_out_index;
     DevBuf d_occur;
+    DevBuf d_nest;       // u32[] per clause of a nested call (BoolNest::nested)
+    DevBuf d_flags;      // BoolNest::flags
     DevBuf d_groups;     // BoolGroup[] of a DisMax call
     DevBuf d_fields;     // BoolField[] of a multi-field call
     DevBuf d_keys;       // nq * k result keys, then u32 overflow[nq]: one device-to-host copy
@@ -203,12 +222,12 @@ __device__ __forceinline__ void bool_set_field(BoolArgs &v, const BoolField *__r
 // clause reads the field fld[clause.field] (bool_set_field) in place of the index in `a`; n_docs, doc_base, the
 // phrase rows and the top-k context stay common.  DISMAX (with OCCUR and FIELDS): clauses form groups (grp[], indexed
 // as a.clauses); mm counts SHOULD groups; s_dyn holds the groups' running max and sum, 2 * 32 floats per thread, and
-// s_g[3] (shared) the groups' presence masks.
-template <bool OCCUR, bool FIELDS, bool DISMAX = false>
+// s_g[3] (shared) the groups' presence masks.  NESTED (with DISMAX): nested clauses and the store pass (BoolNest).
+template <bool OCCUR, bool FIELDS, bool DISMAX = false, bool NESTED = false>
 __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__restrict__ occ,
                                           const BoolField *__restrict__ fld,
                                           const BoolGroup *__restrict__ grp = nullptr, float *s_dyn = nullptr,
-                                          unsigned long long *s_g = nullptr) {
+                                          unsigned long long *s_g = nullptr, const BoolNest nb = BoolNest{}) {
     constexpr int PER = SA_TILE_DOCS / SA_TERM_THREADS / 4;        // float4 groups per thread
     __shared__ __align__(16) float s_tile[SA_TILE_DOCS];
     __shared__ u32 s_lo[SA_BOOL_MAX_CLAUSES], s_hi[SA_BOOL_MAX_CLAUSES];
@@ -236,7 +255,9 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
         bool_set_field<FIELDS>(view, fld, cl.field);
         const BoolArgs &ca = FIELDS ? view : a;
         u32 lo = 0, hi = 0;
-        if (cl.row != SA_BOOL_NO_ROW) {
+        if (NESTED && nb.nested[bq.c0 + c]) {
+            hi = nb.flags[(u64)cl.row * nb.n_tiles + tile] != 0;   // the child ranks a doc of the tile
+        } else if (cl.row != SA_BOOL_NO_ROW) {
             hi = 1;                                                 // a phrase row counts as present
         } else if (cl.n_words == 0) {
         } else if (cl.dir_off != SA_NO_DIR) {
@@ -274,6 +295,10 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
     //    (DISMAX: fewer SHOULD groups with a member in the tile than mm, or a MUST / FILTER group without one)
     if (DISMAX ? ((u32)__popcll(s_g_present & s_g_should) < bq.mm || (s_g_req & ~s_g_present) != 0)
                : OCCUR ? ((s_present & 0xFFFFu) < bq.mm || (s_present >> 16) != 0) : s_present < bq.mm) {   // CTA-uniform
+        if (NESTED && nb.store != nullptr) {                        // a nested node: its flag only
+            if (tid == 0) nb.flags[(u64)bq.pad * nb.n_tiles + tile] = 0;
+            return;
+        }
         if (tid == 0) {
             const u64 t_idx = (u64)q * a.topk.n_tiles + tile;
             a.topk.tile_cnt[t_idx] = 0;
@@ -318,7 +343,9 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
         if (FIELDS) p = ca.bm25;
         p.idf = cl.idf;
         if (cl.row != SA_BOOL_NO_ROW) {
-            // phrase clause (sparse-safe parameters only): BM25 of its counts, zero counts score +0
+            // phrase clause (sparse-safe parameters only): BM25 of its counts, zero counts score +0.  NESTED: a nested
+            // clause's row holds its child's ranked scores (>= +0), read as they are
+            const bool nested = NESTED && nb.nested[bq.c0 + c];
             const float4 *__restrict__ r4 = reinterpret_cast<const float4 *>(a.rows + (u64)cl.row * a.row_stride + tile_doc0);
 #pragma unroll
             for (int j = 0; j < PER; j++) {
@@ -329,7 +356,8 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
                 for (int e = 0; e < 4; e++) {
                     const u64 d = (u64)tile_doc0 + g * 4 + e;
                     float v = 0.0f;
-                    if (xs[e] > 0.0f && d < a.n_docs) v = bm25_from_norm(xs[e], __ldg(ca.norm + d), cl.idf);
+                    if (NESTED && nested) v = xs[e];
+                    else if (xs[e] > 0.0f && d < a.n_docs) v = bm25_from_norm(xs[e], __ldg(ca.norm + d), cl.idf);
                     if (DISMAX && gr.member) {
                         bool_dismax_member(s_m, s_t, any, j * 4 + e, v, oc);
                     } else if (OCCUR) {
@@ -386,6 +414,18 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
         }
         s_tile4[tid + j * SA_TERM_THREADS] = make_float4(o[0], o[1], o[2], o[3]);
     }
+    if (NESTED && nb.store != nullptr) {
+        // a nested node: its ranked values to its row where anything ranks (each thread its own float4s), and the
+        // tile's flag
+        const int ranked = __syncthreads_or(my_max != 0);
+        if (ranked) {
+            float4 *dst = reinterpret_cast<float4 *>(nb.store + (u64)bq.pad * a.row_stride + tile_doc0);
+#pragma unroll
+            for (int j = 0; j < PER; j++) dst[tid + j * SA_TERM_THREADS] = s_tile4[tid + j * SA_TERM_THREADS];
+        }
+        if (tid == 0) nb.flags[(u64)bq.pad * nb.n_tiles + tile] = ranked ? 1u : 0u;
+        return;
+    }
     flush_tile_collect<false>(s_tile, nullptr, a.topk, q, tile, my_max, SA_TILE_DOCS, 0, s_top, &s_ncand, &s_tile_max);
 }
 
@@ -405,6 +445,17 @@ bool_dismax_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, con
     extern __shared__ __align__(16) float s_dyn[];
     __shared__ unsigned long long s_g[3];
     bool_tile<true, true, true>(a, occ, fld, grp, s_dyn, s_g);
+}
+
+// sa_score_batch_topk_bool_nested / sa_multi_score_batch_topk_bool_nested: bool_dismax_tile_kernel with nested
+// clauses, launched once per level of nested nodes (nb.store set) and once for the top-level nodes; see DESIGN.md
+// section 3.10.4 for registers and occupancy.
+__global__ void __launch_bounds__(SA_TERM_THREADS, 2)
+bool_nested_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
+                        const BoolGroup *__restrict__ grp, const BoolNest nb) {
+    extern __shared__ __align__(16) float s_dyn[];
+    __shared__ unsigned long long s_g[3];
+    bool_tile<true, true, true, true>(a, occ, fld, grp, s_dyn, s_g, nb);
 }
 
 // sa_multi_score_batch_topk_bool: roles and weights as bool_tile_kernel<true>, each clause on its own field.  Held to
@@ -439,19 +490,29 @@ struct BoolPlan {
     std::vector<BoolField> fields;      // per field slot (bool_fields_tile_kernel, bool_dismax_tile_kernel)
     std::vector<BoolGroup> groups;      // per clause, as clauses; non-empty: bool_dismax_tile_kernel
     u32 max_group = 1, max_rows = 0;
+    // nested calls: nodes 0 .. n_top - 1 are the top-level queries (queries[0 .. n_top)), the others nested nodes
+    u32 n_top = 0;
+    std::vector<u32> node_starts;       // node n's clauses [node_starts[n], node_starts[n + 1])
+    std::vector<u32> root, depth;       // per node: its top-level query, and its depth below it
+    std::vector<u32> nested;            // nested nodes by (launch group, depth desc, top-level query); queries[n_top + i]
+                                        // is nested[i]'s descriptor
+    std::vector<u32> nest;              // per clause, as clauses: 1 for a nested clause; non-empty: bool_nested_tile_kernel
 };
 
-// The count rows of the phrase clauses of queries [q0, q1) (rows are numbered within the group), each on its clause's
-// field, synchronously.
+// The count rows of the phrase clauses of queries [q0, q1) and of their nested nodes (rows are numbered within the
+// group), each on its clause's field, synchronously.
 int bool_build_rows(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_terms,
                     const uint32_t *clause_term_starts, u32 slop, u32 q0, u32 q1) {
     const u64 stride = sa_padded_docs(X.lead()->n_docs);
     int rc;
-    for (u32 q = q0; q < q1; q++) {
-        const BoolQuery &bq = P.queries[q];
-        for (u32 c = bq.c0; c < bq.c0 + bq.n; c++) {
+    std::vector<u32> nodes;
+    for (u32 q = q0; q < q1; q++) nodes.push_back(q);
+    for (u32 n : P.nested)
+        if (P.root[n] >= q0 && P.root[n] < q1) nodes.push_back(n);
+    for (u32 n : nodes) {
+        for (u32 c = P.node_starts[n]; c < P.node_starts[n + 1]; c++) {
             const BoolClause &cl = P.clauses[c];
-            if (cl.row == SA_BOOL_NO_ROW) continue;
+            if (cl.row == SA_BOOL_NO_ROW || (!P.nest.empty() && P.nest[c])) continue;
             sa_index *ix = X.ix[cl.field];
             bool scored;
             if ((rc = sa_phrase_row(ix, clause_terms + clause_term_starts[c], clause_term_starts[c + 1] - clause_term_starts[c],
@@ -473,7 +534,7 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
     if ((rc = bool_build_rows(X, P, clause_terms, clause_term_starts, slop, q0, q1))) return rc;
     if ((rc = X.cand->reserve(cand_bytes(n_tiles, nq, slots)))) return rc;
     u64 *d_keys = S.d_keys.as<u64>();
-    u32 *d_ovf = (u32 *)(d_keys + (size_t)P.queries.size() * k);
+    u32 *d_ovf = (u32 *)(d_keys + (size_t)P.n_top * k);
     TopkCtx t = make_topk_ctx(X.cand->p, n_tiles, nq, slots, k, d_ovf + q0);
     BoolArgs a;
     memset(&a, 0, sizeof(a));
@@ -493,7 +554,27 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
     a.clauses = S.d_clauses.as<BoolClause>();
     a.queries = S.d_queries.as<BoolQuery>() + q0;
     a.topk = t;
-    if (!P.groups.empty())
+    if (!P.nest.empty()) {
+        // the nested nodes of these queries, deepest level first (one launch per level: a level's nodes of the run
+        // are consecutive in P.nested), each into its row and flags; then the top-level nodes, collected
+        BoolNest nb{S.d_nest.as<u32>(), S.d_flags.as<u32>(), S.rows.as<float>(), n_tiles};
+        for (size_t i = 0; i < P.nested.size();) {
+            auto in_run = [&](size_t x) { return P.root[P.nested[x]] >= q0 && P.root[P.nested[x]] < q1; };
+            if (!in_run(i)) { i++; continue; }
+            size_t j = i + 1;
+            while (j < P.nested.size() && in_run(j) && P.depth[P.nested[j]] == P.depth[P.nested[i]]) j++;
+            BoolArgs an = a;
+            an.queries = S.d_queries.as<BoolQuery>() + P.n_top + i;
+            bool_nested_tile_kernel<<<dim3((u32)(j - i), n_tiles), SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
+                an, S.d_occur.as<BoolOccur>(), S.d_fields.as<BoolField>(), S.d_groups.as<BoolGroup>(), nb);
+            SA_CUDA(cudaGetLastError());
+            ix->stats.total_launches++;
+            i = j;
+        }
+        nb.store = nullptr;
+        bool_nested_tile_kernel<<<dim3(nq, n_tiles), SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
+            a, S.d_occur.as<BoolOccur>(), S.d_fields.as<BoolField>(), S.d_groups.as<BoolGroup>(), nb);
+    } else if (!P.groups.empty())
         bool_dismax_tile_kernel<<<dim3(nq, n_tiles), SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
             a, S.d_occur.as<BoolOccur>(), S.d_fields.as<BoolField>(), S.d_groups.as<BoolGroup>());
     else if (X.fields_kernel)
@@ -508,12 +589,13 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
     return launch_topk_select(ix, t, nq, ix->doc_base, d_keys, S.d_out_index.as<u32>() + q0);
 }
 
-// bool_dismax_tile_kernel's dynamic shared memory above the default 48 KB, and the carveout that fits two CTAs per SM
-// (~2 x 98 KB of shared memory), on the current device (function attributes are per device).
-int bool_dismax_smem() {
-    SA_CUDA(cudaFuncSetAttribute(bool_dismax_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)SA_BOOL_DISMAX_SMEM));
-    SA_CUDA(cudaFuncSetAttribute(bool_dismax_tile_kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
+// bool_dismax_tile_kernel's (bool_nested_tile_kernel's) dynamic shared memory above the default 48 KB, and the
+// carveout that fits two CTAs per SM (~2 x 98 KB of shared memory), on the current device (function attributes are
+// per device).
+template <typename Kernel>
+int bool_dismax_smem(Kernel kernel) {
+    SA_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SA_BOOL_DISMAX_SMEM));
+    SA_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
                                  (int)cudaSharedmemCarveoutMaxShared));
     return SA_OK;
 }
@@ -521,17 +603,21 @@ int bool_dismax_smem() {
 // Every entry point, with the call's indexes locked and their device current.  clause_weight / clause_occur NULL:
 // Or / And, every clause SHOULD with weight 1, mm over all.  clause_field NULL: every clause on field 0.
 // clause_group / clause_tie non-NULL (with clause_occur): DisMax groups, bool_dismax_tile_kernel with a field table.
-int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint32_t *clause_field,
-              const uint32_t *clause_terms, const uint32_t *clause_term_starts, const float *clause_idf,
-              const float *clause_weight, const uint8_t *clause_occur, const uint32_t *clause_group,
-              const float *clause_tie, const uint32_t *mm, uint32_t n_queries, uint32_t slop, uint32_t k,
-              uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+// clause_node non-NULL (with the DisMax arrays): n_nodes nodes, the first n_queries top-level, clause c being nested
+// node clause_node[c] unless SA_NO_NODE (sa_score_batch_topk_bool_nested); otherwise n_nodes == n_queries.
+int bool_topk(const BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts, const uint32_t *clause_node,
+              const uint32_t *clause_field, const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+              const float *clause_idf, const float *clause_weight, const uint8_t *clause_occur,
+              const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
+              uint32_t slop, uint32_t k, uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
     sa_index *lead = X.lead();
     const u32 n_fields = (u32)X.ix.size();
     int rc;
-    const bool occur = clause_occur != nullptr, dismax = clause_group != nullptr;
-    SA_CHECK(n_queries == 0 || query_clause_starts[0] == 0, "query_clause_starts[0] must be 0");
-    for (u32 q = 0; q < n_queries; q++) {
+    const bool occur = clause_occur != nullptr, dismax = clause_group != nullptr, nested = clause_node != nullptr;
+    auto is_nested = [&](u32 c) { return nested && clause_node[c] != SA_NO_NODE; };
+    SA_CHECK(n_nodes >= n_queries, "n_nodes (%u) is below n_queries (%u)", n_nodes, n_queries);
+    SA_CHECK(n_nodes == 0 || query_clause_starts[0] == 0, "query_clause_starts[0] must be 0");
+    for (u32 q = 0; q < n_nodes; q++) {
         SA_CHECK(query_clause_starts[q + 1] > query_clause_starts[q] &&
                  query_clause_starts[q + 1] - query_clause_starts[q] <= SA_BOOL_MAX_CLAUSES,
                  "query %u: a boolean query has 1 to %d clauses", q, SA_BOOL_MAX_CLAUSES);
@@ -563,8 +649,26 @@ int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint
         SA_CHECK(mm[q] <= n_should, "query %u: mm exceeds its %s", q,
                  dismax ? "SHOULD groups" : occur ? "SHOULD clauses" : "clauses");
     }
-    const u32 c_begin = n_queries ? query_clause_starts[0] : 0, c_end = n_queries ? query_clause_starts[n_queries] : 0;
+    // nested nodes: each referenced by exactly one clause of an earlier node, as a clause of its own (no terms, not a
+    // DisMax member); the top-level nodes by none
+    std::vector<u32> refs(nested ? n_nodes : 0, 0);
+    for (u32 n = 0; nested && n < n_nodes; n++) {
+        for (u32 c = query_clause_starts[n]; c < query_clause_starts[n + 1]; c++) {
+            if (!is_nested(c)) continue;
+            const u32 ch = clause_node[c];
+            SA_CHECK(ch < n_nodes && ch >= n_queries && ch > n,
+                     "clause %u: node %u is not a nested node after its holder %u (%u nodes, %u top-level)", c, ch, n,
+                     n_nodes, n_queries);
+            SA_CHECK(refs[ch]++ == 0, "node %u is referenced by more than one clause", ch);
+            SA_CHECK(clause_term_starts[c + 1] == clause_term_starts[c], "clause %u: a nested clause has no terms", c);
+            SA_CHECK(clause_group[c] == c && (c + 1 == query_clause_starts[n + 1] || clause_group[c + 1] != c),
+                     "clause %u: a nested clause is not a DisMax member", c);
+        }
+    }
+    for (u32 n = n_queries; nested && n < n_nodes; n++) SA_CHECK(refs[n] == 1, "node %u is referenced by no clause", n);
+    const u32 c_begin = n_nodes ? query_clause_starts[0] : 0, c_end = n_nodes ? query_clause_starts[n_nodes] : 0;
     for (u32 c = c_begin; c < c_end; c++) {
+        if (is_nested(c)) continue;
         const u32 nt = clause_term_starts[c + 1] - clause_term_starts[c];
         SA_CHECK(clause_term_starts[c + 1] > clause_term_starts[c] && nt <= SA_MAX_PHRASE_TERMS,
                  "clause %u: bad number of terms", c);
@@ -586,23 +690,67 @@ int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint
     const u32 group_q = (u32)std::min<u64>(65535, std::max<u64>(1, (1ull << 30) / ((u64)n_tiles * (slots * sizeof(u64) + 8))));
     const u32 group_rows = (u32)std::max<u64>(1, (4ull << 30) / (stride * sizeof(float)));
     BoolPlan P;
-    P.queries.resize(n_queries);
+    P.n_top = n_queries;
+    P.node_starts.assign(query_clause_starts, query_clause_starts + n_nodes + 1);
+    P.root.resize(n_nodes);
+    P.depth.assign(n_nodes, 0);
+    // every node's top-level query and depth (references point forward, so a holder is seen before its children), and
+    // the rows each top-level query needs: its phrase leaves and its nested nodes
+    std::vector<u32> q_rows(n_queries, 0);
+    for (u32 n = 0; n < n_nodes; n++) {
+        if (n < n_queries) P.root[n] = n;
+        else q_rows[P.root[n]]++;
+        for (u32 c = query_clause_starts[n]; c < query_clause_starts[n + 1]; c++) {
+            if (is_nested(c)) {
+                P.root[clause_node[c]] = P.root[n];
+                P.depth[clause_node[c]] = P.depth[n] + 1;
+                continue;
+            }
+            const u32 f = clause_field ? clause_field[c] : 0;
+            q_rows[P.root[n]] += clause_term_starts[c + 1] - clause_term_starts[c] > 1 && X.avgdl[f] != 0.0f;
+        }
+    }
     P.group_start.push_back(0);
-    std::vector<char> field_sparse(n_fields, 0);      // fields with a sparse-safe clause: their norms are cached
+    std::vector<u32> group_of(n_queries), g_rows;       // per launch group: its rows so far
     u32 rows = 0;
     for (u32 q = 0; q < n_queries; q++) {
-        const u32 c0 = query_clause_starts[q], c1 = query_clause_starts[q + 1];
-        u32 nr = 0;
-        for (u32 c = c0; c < c1; c++) {
-            const u32 f = clause_field ? clause_field[c] : 0;
-            nr += clause_term_starts[c + 1] - clause_term_starts[c] > 1 && X.avgdl[f] != 0.0f;
-        }
-        if (q > P.group_start.back() && (q - P.group_start.back() == group_q || rows + nr > group_rows)) {
+        if (q > P.group_start.back() && (q - P.group_start.back() == group_q || rows + q_rows[q] > group_rows)) {
             P.group_start.push_back(q);
             rows = 0;
         }
-        P.queries[q] = BoolQuery{(u32)P.clauses.size(), c1 - c0, mm[q], 0};
+        rows += q_rows[q];
+        group_of[q] = (u32)P.group_start.size() - 1;
+        P.max_group = std::max(P.max_group, q + 1 - P.group_start.back());
+        P.max_rows = std::max(P.max_rows, rows);
+    }
+    P.group_start.push_back(n_queries);
+    g_rows.assign(P.group_start.size() - 1, 0);
+    // the nested nodes' rows first (a parent's clause names its child's row), then the phrase rows
+    std::vector<u32> node_row(n_nodes, 0);
+    for (u32 n = n_queries; n < n_nodes; n++) {
+        P.nested.push_back(n);
+        node_row[n] = g_rows[group_of[P.root[n]]]++;
+    }
+    std::stable_sort(P.nested.begin(), P.nested.end(), [&](u32 x, u32 y) {
+        const u32 gx = group_of[P.root[x]], gy = group_of[P.root[y]];
+        if (gx != gy) return gx < gy;
+        if (P.depth[x] != P.depth[y]) return P.depth[x] > P.depth[y];
+        return P.root[x] < P.root[y];
+    });
+    P.queries.resize(n_queries);                      // then the nested nodes' descriptors, in P.nested's order
+    std::vector<char> field_sparse(n_fields, 0);      // fields with a sparse-safe clause: their norms are cached
+    for (u32 q = 0; q < n_nodes; q++) {
+        const u32 c0 = query_clause_starts[q], c1 = query_clause_starts[q + 1];
+        u32 &next_row = g_rows[group_of[P.root[q]]];
+        if (q < n_queries) P.queries[q] = BoolQuery{(u32)P.clauses.size(), c1 - c0, mm[q], 0};
         for (u32 c = c0; c < c1; c++) {
+            if (nested) P.nest.push_back(is_nested(c) ? 1u : 0u);
+            if (is_nested(c)) {             // scored by its child's row, present where the child ranks
+                P.occur.push_back(BoolOccur{clause_weight[c], clause_occur[c]});
+                P.groups.push_back(BoolGroup{0.0f, c - c0, 0u, 0u});
+                P.clauses.push_back(BoolClause{0, 0, SA_NO_DIR, SA_NO_DIR, 0.0f, node_row[clause_node[c]], 1u, 0u});
+                continue;
+            }
             const u32 f = clause_field ? clause_field[c] : 0;
             sa_index *ix = X.ix[f];
             const u32 *tids = clause_terms + clause_term_starts[c];
@@ -624,13 +772,13 @@ int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint
                      "finite idf >= 0)", c);
             const TermQuery tq = make_term_query(ix, nt == 1 ? tids[0] : SA_NO_TERM, clause_idf[c]);
             P.clauses.push_back(BoolClause{tq.word_off, tq.n_words, tq.dir_off, tq.rec_off, clause_idf[c],
-                                           nt == 1 ? SA_BOOL_NO_ROW : rows++, sparse ? 1u : 0u, f});
+                                           nt == 1 ? SA_BOOL_NO_ROW : next_row++, sparse ? 1u : 0u, f});
             field_sparse[f] = field_sparse[f] || sparse;
         }
-        P.max_group = std::max(P.max_group, q + 1 - P.group_start.back());
-        P.max_rows = std::max(P.max_rows, rows);
     }
-    P.group_start.push_back(n_queries);
+    for (u32 n : P.nested)
+        P.queries.push_back(BoolQuery{query_clause_starts[n], query_clause_starts[n + 1] - query_clause_starts[n], mm[n],
+                                      node_row[n]});
 
     BoolState &S = *X.S;
     const size_t key_bytes = nk * sizeof(u64) + (size_t)n_queries * sizeof(u32);
@@ -640,6 +788,8 @@ int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint
         (rc = S.rows.reserve(std::max<size_t>((size_t)P.max_rows * stride * sizeof(float), 64))) ||
         (rc = S.d_occur.reserve(P.occur.size() * sizeof(BoolOccur))) ||
         (rc = S.d_groups.reserve(P.groups.size() * sizeof(BoolGroup))) ||
+        (rc = S.d_nest.reserve(P.nest.size() * sizeof(u32))) ||
+        (rc = S.d_flags.reserve(nested ? (size_t)P.max_rows * n_tiles * sizeof(u32) : 0)) ||
         (rc = X.h_pinned->reserve(key_bytes)))
         return rc;
     for (u32 f = 0; f < n_fields; f++)
@@ -662,8 +812,13 @@ int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint
         SA_CUDA(cudaMemcpyAsync(S.d_occur.p, P.occur.data(), P.occur.size() * sizeof(BoolOccur), cudaMemcpyHostToDevice, lead->stream));
     }
     if (dismax) {
-        if ((rc = bool_dismax_smem())) return rc;
+        if ((rc = nested ? bool_dismax_smem(bool_nested_tile_kernel) : bool_dismax_smem(bool_dismax_tile_kernel)))
+            return rc;
         SA_CUDA(cudaMemcpyAsync(S.d_groups.p, P.groups.data(), P.groups.size() * sizeof(BoolGroup), cudaMemcpyHostToDevice, lead->stream));
+    }
+    if (nested) {
+        SA_CUDA(cudaMemcpyAsync(S.d_nest.p, P.nest.data(), P.nest.size() * sizeof(u32), cudaMemcpyHostToDevice,
+                                lead->stream));
     }
     SA_CUDA(cudaMemcpyAsync(S.d_queries.p, P.queries.data(), P.queries.size() * sizeof(BoolQuery), cudaMemcpyHostToDevice, lead->stream));
     SA_CUDA(cudaMemcpyAsync(S.d_out_index.p, identity.data(), (size_t)n_queries * sizeof(u32), cudaMemcpyHostToDevice, lead->stream));
@@ -697,14 +852,15 @@ int bool_topk(const BoolCall &X, const uint32_t *query_clause_starts, const uint
 }
 
 // The single-index entry points: the index's own lock, state and buffers.
-int bool_topk_index(sa_index *ix, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
+int bool_topk_index(sa_index *ix, uint32_t n_nodes, const uint32_t *query_clause_starts,
+                    const uint32_t *clause_node, const uint32_t *clause_terms,
                     const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
                     const uint8_t *clause_occur, const uint32_t *clause_group, const float *clause_tie,
                     const uint32_t *mm, uint32_t n_queries, uint32_t slop,
                     float avg_doc_len, float k1, float b, uint32_t k, uint32_t *out_docs, float *out_scores,
                     uint32_t *n_redone) {
     SA_CHECK(ix && out_docs && out_scores, "NULL argument");
-    SA_CHECK(n_queries == 0 || (query_clause_starts && clause_terms && clause_term_starts && clause_idf && mm),
+    SA_CHECK(n_nodes == 0 || (query_clause_starts && clause_terms && clause_term_starts && clause_idf && mm),
              "NULL argument");
     SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
     if (n_redone) *n_redone = 0;
@@ -719,19 +875,21 @@ int bool_topk_index(sa_index *ix, const uint32_t *query_clause_starts, const uin
     X.S = ix->boolq.get();
     X.cand = &ix->cand;
     X.h_pinned = &ix->h_pinned;
-    return bool_topk(X, query_clause_starts, nullptr, clause_terms, clause_term_starts, clause_idf, clause_weight,
-                     clause_occur, clause_group, clause_tie, mm, n_queries, slop, k, out_docs, out_scores, n_redone);
+    return bool_topk(X, n_nodes, query_clause_starts, clause_node, nullptr, clause_terms, clause_term_starts,
+                     clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
+                     out_docs, out_scores, n_redone);
 }
 
 // The multi-field entry points: the multi's lock, state and candidate buffer.
-int bool_topk_multi(sa_multi *m, const uint32_t *query_clause_starts, const uint32_t *clause_field,
+int bool_topk_multi(sa_multi *m, uint32_t n_nodes, const uint32_t *query_clause_starts,
+                    const uint32_t *clause_node, const uint32_t *clause_field,
                     const uint32_t *clause_terms, const uint32_t *clause_term_starts, const float *clause_idf,
                     const float *clause_weight, const uint8_t *clause_occur, const uint32_t *clause_group,
                     const float *clause_tie, const uint32_t *mm, uint32_t n_queries, uint32_t slop,
                     const float *avg_doc_len, const float *k1, const float *b, uint32_t k, uint32_t *out_docs,
                     float *out_scores, uint32_t *n_redone) {
     SA_CHECK(m && out_docs && out_scores && avg_doc_len && k1 && b, "NULL argument");
-    SA_CHECK(n_queries == 0 || (query_clause_starts && clause_field && clause_terms && clause_term_starts &&
+    SA_CHECK(n_nodes == 0 || (query_clause_starts && clause_field && clause_terms && clause_term_starts &&
                                 clause_idf && clause_weight && clause_occur && mm), "NULL argument");
     SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
     if (n_redone) *n_redone = 0;
@@ -761,8 +919,9 @@ int bool_topk_multi(sa_multi *m, const uint32_t *query_clause_starts, const uint
     X.S = m->boolq.get();
     X.cand = &m->cand;
     X.h_pinned = &m->fields[0]->h_pinned;
-    return bool_topk(X, query_clause_starts, clause_field, clause_terms, clause_term_starts, clause_idf, clause_weight,
-                     clause_occur, clause_group, clause_tie, mm, n_queries, slop, k, out_docs, out_scores, n_redone);
+    return bool_topk(X, n_nodes, query_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
+                     clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
+                     out_docs, out_scores, n_redone);
 }
 
 }  // namespace
@@ -771,8 +930,9 @@ extern "C" int sa_score_batch_topk_bool(sa_index *ix, const uint32_t *query_clau
                                         const uint32_t *clause_term_starts, const float *clause_idf, const uint32_t *mm,
                                         uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
                                         uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
-    return bool_topk_index(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, nullptr, nullptr,
-                           nullptr, nullptr, mm, n_queries, slop, avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
+    return bool_topk_index(ix, n_queries, query_clause_starts, nullptr, clause_terms, clause_term_starts, clause_idf,
+                           nullptr, nullptr, nullptr, nullptr, mm, n_queries, slop, avg_doc_len, k1, b, k, out_docs,
+                           out_scores, n_redone);
 }
 
 extern "C" int sa_score_batch_topk_bool_occur(sa_index *ix, const uint32_t *query_clause_starts,
@@ -782,9 +942,9 @@ extern "C" int sa_score_batch_topk_bool_occur(sa_index *ix, const uint32_t *quer
                                               uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
                                               uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
     SA_CHECK(n_queries == 0 || (clause_weight && clause_occur), "NULL argument");
-    return bool_topk_index(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, clause_weight,
-                           clause_occur, nullptr, nullptr, mm, n_queries, slop, avg_doc_len, k1, b, k, out_docs,
-                           out_scores, n_redone);
+    return bool_topk_index(ix, n_queries, query_clause_starts, nullptr, clause_terms, clause_term_starts, clause_idf,
+                           clause_weight, clause_occur, nullptr, nullptr, mm, n_queries, slop, avg_doc_len, k1, b, k,
+                           out_docs, out_scores, n_redone);
 }
 
 extern "C" int sa_score_batch_topk_bool_dismax(sa_index *ix, const uint32_t *query_clause_starts,
@@ -795,9 +955,9 @@ extern "C" int sa_score_batch_topk_bool_dismax(sa_index *ix, const uint32_t *que
                                                uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
                                                uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
     SA_CHECK(n_queries == 0 || (clause_weight && clause_occur && clause_group && clause_tie), "NULL argument");
-    return bool_topk_index(ix, query_clause_starts, clause_terms, clause_term_starts, clause_idf, clause_weight,
-                           clause_occur, clause_group, clause_tie, mm, n_queries, slop, avg_doc_len, k1, b, k,
-                           out_docs, out_scores, n_redone);
+    return bool_topk_index(ix, n_queries, query_clause_starts, nullptr, clause_terms, clause_term_starts, clause_idf,
+                           clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, avg_doc_len, k1,
+                           b, k, out_docs, out_scores, n_redone);
 }
 
 extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, const uint32_t *query_clause_starts,
@@ -807,9 +967,9 @@ extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, const uint32_t *query
                                               const uint32_t *mm, uint32_t n_queries, uint32_t slop,
                                               const float *avg_doc_len, const float *k1, const float *b, uint32_t k,
                                               uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
-    return bool_topk_multi(m, query_clause_starts, clause_field, clause_terms, clause_term_starts, clause_idf,
-                           clause_weight, clause_occur, nullptr, nullptr, mm, n_queries, slop, avg_doc_len, k1, b, k,
-                           out_docs, out_scores, n_redone);
+    return bool_topk_multi(m, n_queries, query_clause_starts, nullptr, clause_field, clause_terms, clause_term_starts,
+                           clause_idf, clause_weight, clause_occur, nullptr, nullptr, mm, n_queries, slop, avg_doc_len,
+                           k1, b, k, out_docs, out_scores, n_redone);
 }
 
 extern "C" int sa_multi_score_batch_topk_bool_dismax(sa_multi *m, const uint32_t *query_clause_starts,
@@ -822,7 +982,37 @@ extern "C" int sa_multi_score_batch_topk_bool_dismax(sa_multi *m, const uint32_t
                                                      uint32_t k, uint32_t *out_docs, float *out_scores,
                                                      uint32_t *n_redone) {
     SA_CHECK(n_queries == 0 || (clause_group && clause_tie), "NULL argument");
-    return bool_topk_multi(m, query_clause_starts, clause_field, clause_terms, clause_term_starts, clause_idf,
+    return bool_topk_multi(m, n_queries, query_clause_starts, nullptr, clause_field, clause_terms, clause_term_starts,
+                           clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop,
+                           avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
+}
+
+extern "C" int sa_score_batch_topk_bool_nested(sa_index *ix, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                               const uint32_t *clause_node, const uint32_t *clause_terms,
+                                               const uint32_t *clause_term_starts, const float *clause_idf,
+                                               const float *clause_weight, const uint8_t *clause_occur,
+                                               const uint32_t *clause_group, const float *clause_tie,
+                                               const uint32_t *mm, uint32_t n_queries, uint32_t slop,
+                                               float avg_doc_len, float k1, float b, uint32_t k, uint32_t *out_docs,
+                                               float *out_scores, uint32_t *n_redone) {
+    SA_CHECK(n_nodes == 0 || (clause_node && clause_weight && clause_occur && clause_group && clause_tie),
+             "NULL argument");
+    return bool_topk_index(ix, n_nodes, node_clause_starts, clause_node, clause_terms, clause_term_starts, clause_idf,
                            clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, avg_doc_len,
                            k1, b, k, out_docs, out_scores, n_redone);
+}
+
+extern "C" int sa_multi_score_batch_topk_bool_nested(sa_multi *m, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                                     const uint32_t *clause_node, const uint32_t *clause_field,
+                                                     const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                                     const float *clause_idf, const float *clause_weight,
+                                                     const uint8_t *clause_occur, const uint32_t *clause_group,
+                                                     const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
+                                                     uint32_t slop, const float *avg_doc_len, const float *k1,
+                                                     const float *b, uint32_t k, uint32_t *out_docs,
+                                                     float *out_scores, uint32_t *n_redone) {
+    SA_CHECK(n_nodes == 0 || (clause_node && clause_group && clause_tie), "NULL argument");
+    return bool_topk_multi(m, n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
+                           clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop,
+                           avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
 }

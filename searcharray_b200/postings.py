@@ -516,7 +516,11 @@ class SearchArray(ExtensionArray):
         query.DisMax(clauses, tie) is accepted as a clause of these, and as a query of its own (Bool(should=[it])):
         one clause scoring d = max_j v_j + (sum_j v_j - max_j v_j) * tie over its members' v_j = w_j * .score(c_j),
         matched where any member scores > 0 (sa_score_batch_topk_bool_dismax) -- synonyms as
-        DisMax(["film", "movie"], tie=0.1).  Its members need k1 > 0 and 0 <= b < 1 (ValueError otherwise)."""
+        DisMax(["film", "movie"], tie=0.1).  Its members need k1 > 0 and 0 <= b < 1 (ValueError otherwise).
+
+        An Or / And / Bool may be a clause of another, at any depth (Or([And(["star", "wars"]), And(["star", "trek"])])):
+        it scores what it would rank as a query of its own and matches where that is > 0
+        (sa_score_batch_topk_bool_nested); see query.Or."""
         from .query import is_boolean
         if any(is_boolean(q) for q in queries):
             return self._search_topk_mixed(list(queries), k, similarity, slop)
@@ -541,7 +545,7 @@ class SearchArray(ExtensionArray):
         """search_topk of a batch holding boolean queries: the plain ones through search_topk as before, the boolean
         ones through sa_score_batch_topk_bool (Or / And with weights 1) or sa_score_batch_topk_bool_occur (Bool,
         boosted Or / And), each clause with the idf .score gives it; results in query order."""
-        from .query import has_dismax, has_field, is_boolean, needs_occur
+        from .query import has_dismax, has_field, is_boolean, is_nested, needs_occur
         if any(has_field(q) for q in queries if is_boolean(q)):
             raise ValueError("a Field clause names a DataFrame column: run queries over columns with "
                              "solr.fields_topk(frame, queries), not SearchArray.search_topk")
@@ -550,13 +554,13 @@ class SearchArray(ExtensionArray):
                                       "compose .score() on the view")
         if not isinstance(similarity, Bm25Similarity):
             raise TypeError(f"boolean queries support bm25_similarity only, not {similarity!r}")
-        kind = np.asarray([(3 if has_dismax(q) else needs_occur(q) + 1) if is_boolean(q) else 0
-                           for q in queries])                       # plain, Or, occur, DisMax
-        if np.any(kind == 3):
+        kind = np.asarray([(4 if is_nested(q) else 3 if has_dismax(q) else needs_occur(q) + 1) if is_boolean(q) else 0
+                           for q in queries])                       # plain, Or, occur, DisMax, nested
+        if any(has_dismax(q) for q, kd in zip(queries, kind) if kd >= 3):
             self._check_dismax_params(similarity)
         docs = np.empty((len(queries), k), dtype=np.uint32)
         scores = np.empty((len(queries), k), dtype=np.float32)
-        for kd in (0, 1, 2, 3):
+        for kd in (0, 1, 2, 3, 4):
             sel = kind == kd
             part = [q for q, s in zip(queries, sel) if s]
             if not part:
@@ -565,6 +569,8 @@ class SearchArray(ExtensionArray):
                 docs[sel], scores[sel] = self.search_topk(part, k=k, similarity=similarity, slop=slop)
             elif kd == 3:
                 docs[sel], scores[sel], _ = self._search_topk_dismax(part, k, similarity, slop)
+            elif kd == 4:
+                docs[sel], scores[sel], _ = self._search_topk_nested(part, k, similarity, slop)
             else:
                 docs[sel], scores[sel], _ = self._search_topk_bool(part, k, similarity, slop)
         return docs, scores
@@ -594,6 +600,34 @@ class SearchArray(ExtensionArray):
                 _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(groups), _lib.p_f32(ties), _lib.p_u32(mm),
                 len(queries), int(slop), self.avg_doc_length, similarity.k1, similarity.b, k, _lib.p_u32(docs),
                 _lib.p_f32(scores), ctypes.byref(n_redone)))
+        return docs, scores, n_redone.value
+
+    def _search_topk_nested(self, queries, k, similarity, slop):
+        """Boolean queries holding nested queries through sa_score_batch_topk_bool_nested: (docs, scores, queries
+        re-run exactly).  DisMax members anywhere in the trees need sparse-safe BM25 parameters (ValueError before any
+        device work)."""
+        from .query import check_dismax_members, dismax_members, flatten_nested
+        clauses, n_starts, c_node, mm, weights, occurs, groups, ties = flatten_nested(queries)
+        dev = self._device()
+        docs = np.empty((len(queries), k), dtype=np.uint32)
+        scores = np.empty((len(queries), k), dtype=np.float32)
+        n_redone = ctypes.c_uint32(0)
+        leaf = [i for i, c in enumerate(clauses) if c is not None]
+        terms, l_starts, l_idfs = self._topk_queries([clauses[i] for i in leaf],
+                                                     lambda dfs: compute_idf(self.corpus_size, dfs))
+        idfs, n_terms = np.zeros(len(clauses), dtype=np.float32), np.zeros(len(clauses), dtype=np.int64)
+        idfs[leaf] = l_idfs
+        n_terms[leaf] = np.diff(l_starts)
+        c_starts = np.concatenate([[0], np.cumsum(n_terms)]).astype(np.uint32)   # nested clauses: no terms
+        check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
+                             lambda i: (similarity.k1, similarity.b, self.avg_doc_length, idfs[i]))
+        with self._shared["lock"]:
+            self._apply_rows(dev)
+            _lib.check(_lib.lib().sa_score_batch_topk_bool_nested(
+                dev.handle, len(n_starts) - 1, _lib.p_u32(n_starts), _lib.p_u32(c_node), _lib.p_u32(terms),
+                _lib.p_u32(c_starts), _lib.p_f32(idfs), _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(groups),
+                _lib.p_f32(ties), _lib.p_u32(mm), len(queries), int(slop), self.avg_doc_length, similarity.k1,
+                similarity.b, k, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
         return docs, scores, n_redone.value
 
     def _search_topk_bool(self, queries, k, similarity, slop):

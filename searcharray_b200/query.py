@@ -8,7 +8,9 @@ device (sa_score_batch_topk_bool).  Bool(must, should, filter, must_not, mm) and
 composition (sa_score_batch_topk_bool_occur).  Field(field, clause) names the DataFrame column a clause scores on,
 for queries over several columns (solr.fields_topk, sa_multi_score_batch_topk_bool).  DisMax(clauses, tie) is one
 clause scored by its best member plus tie times the others (Lucene's DisjunctionMaxQuery;
-sa_score_batch_topk_bool_dismax, sa_multi_score_batch_topk_bool_dismax)."""
+sa_score_batch_topk_bool_dismax, sa_multi_score_batch_topk_bool_dismax).  An Or / And / Bool may itself be a clause of
+another (a nested query, scored by what it ranks as a query of its own; sa_score_batch_topk_bool_nested,
+sa_multi_score_batch_topk_bool_nested)."""
 import math
 from typing import List, Union
 
@@ -17,6 +19,8 @@ import numpy as np
 from .solr import parse_min_should_match
 
 SA_BOOL_MAX_CLAUSES = 64          # include/searcharray_b200.h
+SA_BOOL_MAX_NESTED = 64           # nested queries in one top-level query, at any depth
+SA_NO_NODE = 0xFFFFFFFF           # include/searcharray_b200.h
 ED_MAX_FIELDS = 8                 # fields of one sa_multi (sa_multi.cuh)
 SA_OCCUR_SHOULD, SA_OCCUR_MUST, SA_OCCUR_FILTER, SA_OCCUR_MUST_NOT = 0, 1, 2, 3
 
@@ -24,9 +28,9 @@ Clause = Union[str, List[str]]
 
 
 def _clause(c):
-    """A clause as search_topk's query form: str (term) or list[str] (phrase), a Field of one, or a DisMax; anything
-    else is a TypeError."""
-    if isinstance(c, (str, Field, DisMax)):
+    """A clause as search_topk's query form: str (term) or list[str] (phrase), a Field of one, a DisMax, or a nested
+    Or / And / Bool; anything else is a TypeError."""
+    if isinstance(c, (str, Field, DisMax, Or, Bool)):
         return c
     if isinstance(c, (list, tuple)) and c and all(isinstance(t, str) for t in c):
         return list(c)
@@ -42,7 +46,7 @@ class Field:
     def __init__(self, field, clause):
         if not isinstance(field, str):
             raise TypeError(f"a field is a column name (str), not {field!r}")
-        if isinstance(clause, (Boost, Field, DisMax)):
+        if isinstance(clause, (Boost, Field, DisMax, Or, Bool)):
             raise TypeError(f"a Field holds a term or a phrase; boost a field clause as Boost(Field(...), w), not {clause!r}")
         self.field = field
         self.clause = _clause(clause)
@@ -55,7 +59,8 @@ class Boost:
     """A term or phrase clause whose score is multiplied by `weight` (Lucene's `title^2`) before it is added:
     s = s + float32(weight) * score(clause), the product rounded to float32.  `weight` is finite and >= 0 and is
     rounded to float32 once.  A doc still counts as matched by the clause where its unweighted score is > 0, so a
-    weight of 0 matches without scoring.  Accepted where a clause scores: in Or, And, Bool's must and should."""
+    weight of 0 matches without scoring.  Accepted where a clause scores: in Or, And, Bool's must and should.  A
+    nested Or / And / Bool may be boosted the same way: it adds float32(weight) * (what it ranks)."""
 
     def __init__(self, clause, weight):
         if isinstance(clause, DisMax):
@@ -121,9 +126,24 @@ class DisMax:
         return f"DisMax({shown!r}, tie={float(self.tie)!r})"
 
 
+def _inner(c):
+    """A clause without its Boost."""
+    return c.clause if isinstance(c, Boost) else c
+
+
+def _is_node(c):
+    """Whether a clause (boosted or not) is a nested Or / And / Bool."""
+    return isinstance(_inner(c), (Or, Bool))
+
+
 def _n_clauses(clauses):
-    """The clauses a list holds as the device counts them: a DisMax counts its members."""
-    return sum(len(c.clauses) if isinstance(c, DisMax) else 1 for c in clauses)
+    """The leaves a list holds as the device counts them: a DisMax counts its members, a nested query its leaves."""
+    return sum(_inner(c).n_leaves if _is_node(c) else len(c.clauses) if isinstance(c, DisMax) else 1 for c in clauses)
+
+
+def _n_nodes(clauses):
+    """The nested queries a list holds, at any depth; a query object used twice counts twice."""
+    return sum(1 + _inner(c).n_nested for c in clauses if _is_node(c))
 
 
 def _check_count(n):
@@ -131,18 +151,33 @@ def _check_count(n):
         raise ValueError(f"a boolean query has at most {SA_BOOL_MAX_CLAUSES} clauses, not {n}")
 
 
+def _check_nodes(n):
+    if n > SA_BOOL_MAX_NESTED:
+        raise ValueError(f"a boolean query holds at most {SA_BOOL_MAX_NESTED} nested queries, not {n}")
+
+
 class Or:
     """A query matching docs where at least `mm` of `clauses` score > 0, scored by the sum of the clauses' scores.
 
     clauses: a str (a term), a list[str] (a phrase, matched with search_topk's `slop`) or a Boost of either;
     duplicates count twice.  mm: an int or a Solr min-should-match spec ("2", "-1", "75%", "2<-25%"), clamped to
-    [0, len(clauses)] as edismax clamps it (solr.parse_min_should_match)."""
+    [0, len(clauses)] as edismax clamps it (solr.parse_min_should_match).
+
+    A clause may also be a nested Or / And / Bool N (or a Boost of one), at any depth.  It is one clause: its score
+    at doc d is r_N(d), what N ranks d with as a query of its own (its sum where all its conditions hold and the sum
+    is > 0, else 0), it matches where r_N(d) > 0 and counts once towards mm.  So, unlike Lucene, a nested query whose
+    sum is <= 0 (all its boosts 0, say) does not match.  Or([a, Or([b])]) scores as Or([a, b]); flattening a larger
+    nested Or in general changes the fold order and the mm counts.  A top-level query holds at most
+    SA_BOOL_MAX_CLAUSES leaves in its whole tree (DisMax members counted) and SA_BOOL_MAX_NESTED nested queries; a
+    sub-query object used twice counts twice."""
 
     def __init__(self, clauses, mm=1):
         clauses = list(clauses)
         if not clauses:
             raise ValueError("a boolean query needs at least one clause")
-        _check_count(_n_clauses(clauses))
+        self.n_leaves, self.n_nested = _n_clauses(clauses), _n_nodes(clauses)
+        _check_count(self.n_leaves)
+        _check_nodes(self.n_nested)
         self.clauses, self.weights = _scoring(clauses)
         self.mm = parse_min_should_match(len(self.clauses), str(mm))
 
@@ -174,7 +209,9 @@ class Bool:
 
     mm counts `should` clauses only: an int or a Solr spec (solr.parse_min_should_match(len(should), str(mm))); by
     default 0 when there are must or filter clauses, else 1.  At least one must or should clause is needed (without
-    one nothing can score > 0), and at most SA_BOOL_MAX_CLAUSES clauses in the four lists together."""
+    one nothing can score > 0), and at most SA_BOOL_MAX_CLAUSES clauses in the four lists together.  Every list
+    accepts a nested Or / And / Bool as Or does (a Boost of one in must and should only); under filter / must_not it
+    plays a leaf's role, matching where what it ranks is > 0."""
 
     def __init__(self, must=(), should=(), filter=(), must_not=(), mm=None):
         must, should, filter, must_not = list(must), list(should), list(filter), list(must_not)
@@ -188,7 +225,10 @@ class Bool:
         self.must_not = [_clause(c) for c in must_not]
         if not self.must and not self.should:
             raise ValueError("a Bool query needs at least one must or should clause: nothing else scores")
-        _check_count(_n_clauses(must + should + filter + must_not))
+        every = must + should + filter + must_not
+        self.n_leaves, self.n_nested = _n_clauses(every), _n_nodes(every)
+        _check_count(self.n_leaves)
+        _check_nodes(self.n_nested)
         if mm is None:
             mm = 0 if (self.must or self.filter) else 1
         self.mm = parse_min_should_match(len(self.should), str(mm))
@@ -222,14 +262,32 @@ def _top_clauses(q):
     return q.occur_clauses()[0] if isinstance(q, Bool) else q.clauses
 
 
+def _leaves(q):
+    """Every clause of a boolean query's tree that is not a nested query: its DisMax clauses and their members, and
+    the leaves of its nested queries at any depth."""
+    for c in _top_clauses(q):
+        if isinstance(c, (Or, Bool)):
+            yield from _leaves(c)
+        else:
+            yield c
+            if isinstance(c, DisMax):
+                yield from c.clauses
+
+
 def has_field(q):
-    """Whether a boolean query holds a Field clause (solr.fields_topk's form), a DisMax's members included."""
-    return any(isinstance(m, Field) for c in _top_clauses(q) for m in (c.clauses if isinstance(c, DisMax) else [c]))
+    """Whether a boolean query holds a Field clause (solr.fields_topk's form), a DisMax's members and nested queries
+    included."""
+    return any(isinstance(c, Field) for c in _leaves(q))
 
 
 def has_dismax(q):
-    """Whether q is or holds a DisMax (sa_score_batch_topk_bool_dismax's form)."""
-    return any(isinstance(c, DisMax) for c in _top_clauses(q))
+    """Whether q is or holds a DisMax (sa_score_batch_topk_bool_dismax's form), nested queries included."""
+    return any(isinstance(c, DisMax) for c in _leaves(q))
+
+
+def is_nested(q):
+    """Whether a boolean query holds a nested Or / And / Bool (sa_score_batch_topk_bool_nested's form)."""
+    return not isinstance(q, DisMax) and any(isinstance(c, (Or, Bool)) for c in _top_clauses(q))
 
 
 def needs_occur(q):
@@ -303,10 +361,72 @@ def flatten_dismax(queries):
             np.asarray(groups, dtype=np.uint32), np.asarray(ties, dtype=np.float32))
 
 
+def _node_parts(q):
+    """(clauses, float32 weights, occurs, mm) of one node as the device folds it: an Or's clauses all SHOULD, a Bool's
+    as must, should, filter, must_not, a top-level DisMax as Bool(should=[it])."""
+    if isinstance(q, DisMax):
+        return [q], [np.float32(1.0)], [SA_OCCUR_SHOULD], 1
+    if isinstance(q, Bool):
+        cs, ws, os_ = q.occur_clauses()
+        return cs, ws, os_, q.mm
+    return q.clauses, q.weights, [SA_OCCUR_SHOULD] * len(q.clauses), q.mm
+
+
+def _nodes(queries):
+    """The nodes of a batch in flatten_nested's order: the queries, then each query's nested queries in pre-order
+    (a sub-query object used twice is two nodes); and per node, the node indices of its nested clauses in order."""
+    nodes, children = list(queries), [[] for _ in queries]
+
+    def visit(n):
+        for c in _node_parts(nodes[n])[0]:
+            if isinstance(c, (Or, Bool)):
+                nodes.append(c)
+                children.append([])
+                children[n].append(len(nodes) - 1)
+                visit(len(nodes) - 1)
+    for q in range(len(queries)):
+        visit(q)
+    return nodes, children
+
+
+def flatten_nested(queries):
+    """Boolean queries, nested ones included, as sa_score_batch_topk_bool_nested takes them: (clauses,
+    node_clause_starts, clause_node, mm, weights, occurs, groups, ties), every array per node or per clause as
+    flatten_dismax's per query or per clause.  Nodes 0 .. len(queries) - 1 are the queries, then each query's nested
+    queries in pre-order, so that every child comes after its parent.  A nested clause is None in `clauses`, with
+    clause_node its node (SA_NO_NODE for the others), its Boost's weight, its role and a group of its own."""
+    nodes, children = _nodes(queries)
+    clauses, starts, cnode, mm, weights, occurs, groups, ties = [], [0], [], [], [], [], [], []
+    for n, node in enumerate(nodes):
+        cs, ws, os_, qmm = _node_parts(node)
+        kids = iter(children[n])
+        for c, w, o in zip(cs, ws, os_):
+            first = len(clauses)
+            if isinstance(c, (Or, Bool)):
+                members, tie, child = [(None, w)], np.float32(0.0), next(kids)
+            elif isinstance(c, DisMax):
+                members, tie, child = list(zip(c.clauses, c.weights)), c.tie, SA_NO_NODE
+            else:
+                members, tie, child = [(c, w)], np.float32(0.0), SA_NO_NODE
+            for m, mw in members:
+                clauses.append(m)
+                cnode.append(child)
+                weights.append(mw)
+                occurs.append(o)
+                groups.append(first)
+                ties.append(tie)
+        starts.append(len(clauses))
+        mm.append(qmm)
+    u32 = lambda x: np.asarray(x, dtype=np.uint32)      # noqa: E731
+    return (clauses, u32(starts), u32(cnode), u32(mm), np.asarray(weights, dtype=np.float32),
+            np.asarray(occurs, dtype=np.uint8), u32(groups), np.asarray(ties, dtype=np.float32))
+
+
 def dismax_members(queries):
-    """Indices, into flatten_dismax's clause list, of the clauses that are DisMax members."""
+    """Indices of the clauses that are DisMax members, into the clause list of flatten_nested (which is
+    flatten_dismax's for a batch without nested queries)."""
     out, n = [], 0
-    for q in queries:
+    for q in _nodes(queries)[0]:
         for c in _top_clauses(q):
             k = len(c.clauses) if isinstance(c, DisMax) else 1
             if isinstance(c, DisMax):

@@ -408,15 +408,20 @@ def edismax_topk(frame: pd.DataFrame, q: str, qf: List[str], k: int = 10, mm: Op
 
 
 def _fields_plan(frame, queries, similarity):
-    """fields_topk's refusals and field slots, before any device work: (flatten_occur's arrays, or flatten_dismax's
-    when a query holds a DisMax, field name -> slot, per-slot arrays, per-slot similarities)."""
-    from .query import ED_MAX_FIELDS, Field, flatten_dismax, flatten_occur, has_dismax, is_boolean
+    """fields_topk's refusals and field slots, before any device work: (flatten_occur's arrays, flatten_dismax's
+    when a query holds a DisMax, or flatten_nested's when one holds a nested query, field name -> slot, per-slot
+    arrays, per-slot similarities)."""
+    from .query import ED_MAX_FIELDS, Field, flatten_dismax, flatten_nested, flatten_occur, has_dismax, is_boolean, \
+        is_nested
     queries = list(queries)
     for q in queries:
         if not is_boolean(q):
             raise TypeError(f"fields_topk takes Or / And / Bool / DisMax queries, not {q!r}")
-    flat = flatten_dismax(queries) if any(has_dismax(q) for q in queries) else flatten_occur(queries)
-    clauses = flat[0]
+    if any(is_nested(q) for q in queries):
+        flat = flatten_nested(queries)
+    else:
+        flat = flatten_dismax(queries) if any(has_dismax(q) for q in queries) else flatten_occur(queries)
+    clauses = [c for c in flat[0] if c is not None]          # flatten_nested: None for a nested clause
     for c in clauses:
         if not isinstance(c, Field):
             raise ValueError(f"every clause of fields_topk names its column: Field(field, {c!r})")
@@ -455,8 +460,9 @@ def _fields_plan(frame, queries, similarity):
         slot_arrays.append(a)
         slot_sims.append(sim)
         slot_name.append(f)
-    if len(flat) == 7:                    # DisMax members: sparse-safe k1 / b on their fields (idf: _fields_clauses)
+    if len(flat) >= 7:                    # DisMax members: sparse-safe k1 / b on their fields (idf: _fields_clauses)
         from .query import check_dismax_members, dismax_members
+        clauses = flat[0]
         check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
                              lambda i: (sims[clauses[i].field].k1, sims[clauses[i].field].b,
                                         arrays[clauses[i].field].avg_doc_length, 0.0))
@@ -465,10 +471,11 @@ def _fields_plan(frame, queries, similarity):
 
 def _fields_clauses(clauses, slot_of, arrays):
     """Each clause's term ids and idf from its own field, as that column's .score takes them: (terms, clause term
-    starts, float32 idf, field slots).  Call it with the fields locked (_locked)."""
-    c_terms, c_idf = [None] * len(clauses), np.empty(len(clauses), dtype=np.float32)
+    starts, float32 idf, field slots).  A nested clause (None) has no terms, idf 0 and slot 0.  Call it with the
+    fields locked (_locked)."""
+    c_terms, c_idf = [[]] * len(clauses), np.zeros(len(clauses), dtype=np.float32)
     for s, arr in enumerate(arrays):
-        idx = [i for i, c in enumerate(clauses) if slot_of[c.field] == s]
+        idx = [i for i, c in enumerate(clauses) if c is not None and slot_of[c.field] == s]
         t, st, idf = arr._topk_queries([clauses[i].clause for i in idx],
                                        lambda dfs, arr=arr: compute_idf(arr.corpus_size, dfs))
         for j, i in enumerate(idx):
@@ -476,20 +483,33 @@ def _fields_clauses(clauses, slot_of, arrays):
             c_idf[i] = idf[j]
     c_starts = _u32(np.cumsum([0] + [len(t) for t in c_terms]))
     terms = _u32(np.concatenate(c_terms) if c_terms else [])
-    return terms, c_starts, c_idf, _u32([slot_of[c.field] for c in clauses])
+    return terms, c_starts, c_idf, _u32([0 if c is None else slot_of[c.field] for c in clauses])
 
 
 def _fields_call(multi, arrays, sims, flat, prepared, k, slop):
-    """sa_multi_score_batch_topk_bool, or sa_multi_score_batch_topk_bool_dismax for flatten_dismax's arrays, on
-    prepared arrays (the fields locked): (docs, scores, queries re-run)."""
-    q_starts, mm, weights, occurs = flat[1:5]
+    """sa_multi_score_batch_topk_bool, sa_multi_score_batch_topk_bool_dismax for flatten_dismax's arrays, or
+    sa_multi_score_batch_topk_bool_nested for flatten_nested's, on prepared arrays (the fields locked): (docs, scores,
+    queries re-run)."""
     terms, c_starts, c_idf, c_field = prepared
-    nq = len(q_starts) - 1
-    docs = np.empty((nq, k), dtype=np.uint32)
-    scores = np.empty((nq, k), dtype=np.float32)
     n_redone = ctypes.c_uint32(0)
     avgdl = _f32([a.avg_doc_length for a in arrays])
     k1, b = _f32([s.k1 for s in sims]), _f32([s.b for s in sims])
+    if len(flat) == 8:
+        from .query import SA_NO_NODE
+        n_starts, c_node, mm, weights, occurs, groups, ties = flat[1:]
+        nq = len(n_starts) - 1 - int(np.count_nonzero(c_node != SA_NO_NODE))   # each nested node: one reference
+        docs = np.empty((nq, k), dtype=np.uint32)
+        scores = np.empty((nq, k), dtype=np.float32)
+        _lib.check(_lib.lib().sa_multi_score_batch_topk_bool_nested(
+            multi.handle, len(n_starts) - 1, _lib.p_u32(n_starts), _lib.p_u32(c_node), _lib.p_u32(c_field),
+            _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(c_idf), _lib.p_f32(weights), _lib.p_u8(occurs),
+            _lib.p_u32(groups), _lib.p_f32(ties), _lib.p_u32(mm), nq, int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1),
+            _lib.p_f32(b), k, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
+        return docs, scores, n_redone.value
+    q_starts, mm, weights, occurs = flat[1:5]
+    nq = len(q_starts) - 1
+    docs = np.empty((nq, k), dtype=np.uint32)
+    scores = np.empty((nq, k), dtype=np.float32)
     if len(flat) == 7:
         groups, ties = flat[5:]
         _lib.check(_lib.lib().sa_multi_score_batch_topk_bool_dismax(
@@ -514,7 +534,7 @@ def _fields_topk(frame, queries, k, similarity, slop):
         for arr in arrays:                 # a sliced view of the same column may have left its row filter installed
             arr._apply_rows(arr._device())
         prepared = _fields_clauses(flat[0], slot_of, arrays)
-        if len(flat) == 7:                # DisMax members: sparse-safe idf from their own fields
+        if len(flat) >= 7:                # DisMax members: sparse-safe idf from their own fields
             from .query import check_dismax_members, dismax_members
             clauses = flat[0]
             check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
@@ -542,6 +562,10 @@ def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
     v_j = w_j * score(member j), each member on its own column (sa_multi_score_batch_topk_bool_dismax): Elasticsearch's
     best_fields as DisMax([Boost(Field("title", "alien"), 2), Field("overview", "alien")], tie=0.3), and edismax's
     term-centric qf as an Or of one such DisMax per term with a Solr mm.  Its members need k1 > 0 and 0 <= b < 1 on
-    their fields (ValueError otherwise)."""
+    their fields (ValueError otherwise).
+
+    An Or / And / Bool may be a clause of another, at any depth, as in SearchArray.search_topk: edismax's qf + pf as
+    Bool(must=[Or([DisMax(...), DisMax(...)], mm="75%")], should=[Boost(Field("title", ["a", "b"]), 3)])
+    (sa_multi_score_batch_topk_bool_nested)."""
     docs, scores, _ = _fields_topk(frame, queries, k, similarity, slop)
     return docs, scores
