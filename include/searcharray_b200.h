@@ -150,6 +150,22 @@ int sa_score_batch_topk_sim(sa_index *index, int kind, const uint32_t *terms, co
                             const double *idf, uint32_t n_queries, uint32_t slop, const float *view_doc_lens,
                             double avg_doc_len, double k1, double b, uint32_t k, uint32_t *out_ids,
                             double *out_scores);
+/* A document mask for the batched top-k (the `_where` entry points below): the result is the top k of
+ * where(mask_q, S_q, 0), S_q being the scores the call without a mask ranks for query q, under the same selection rule.
+ * The mask never changes a score -- idf, document frequencies, avgdl and doc lengths stay the unmasked call's -- it
+ * only removes docs from the ranking.  where_bits: u32 words, one row of SA_WHERE_WORDS(where_n) words covering
+ * where_n docs (the index's docs, or a view's positions under sa_score_batch_topk_sim_where), for the whole batch
+ * (where_stride == 0) or one row per query (where_stride == that row length; row q is query q's).  Within a row the
+ * bits are in the tile kernels' owner order, not doc order: word t * 256 + i holds, at bit 4 j + e, doc
+ * t * 8192 + 4 (i + 256 j) + e (t: the 8,192-doc tile, i: the owning thread, j < 8, e < 4); bits past where_n are 0.
+ * where_n must equal the doc (position) count the call ranks; anything else is SA_ERR_ARG before any device work.
+ * where_bits NULL: no mask. */
+#define SA_WHERE_WORDS(n) ((((uint64_t)(n) + 8191u) / 8192u) * 256u)
+/* sa_score_batch_topk_sim with a document mask over the positions it ranks (a view's, or the array's docs). */
+int sa_score_batch_topk_sim_where(sa_index *index, int kind, const uint32_t *terms, const uint32_t *term_starts,
+                                  const double *idf, uint32_t n_queries, uint32_t slop, const float *view_doc_lens,
+                                  double avg_doc_len, double k1, double b, uint32_t k, const uint32_t *where_bits,
+                                  uint64_t where_n, uint64_t where_stride, uint32_t *out_ids, double *out_scores);
 /* Batched boolean queries: OR / AND / min-should-match over term and phrase clauses (the reference's composition in
  * test/test_search.py:126-226).  Query q = clauses [query_clause_starts[q], query_clause_starts[q+1]) (1 to
  * SA_BOOL_MAX_CLAUSES of them; query_clause_starts[0] == 0); clause c = clause_terms[clause_term_starts[c] ..
@@ -215,6 +231,20 @@ int sa_score_batch_topk_bool_nested(sa_index *index, uint32_t n_nodes, const uin
                                     const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
                                     uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
                                     uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
+/* Every boolean entry point above with a document mask (SA_WHERE_WORDS): the arguments of
+ * sa_score_batch_topk_bool_nested, whose nullable arrays pick the form -- clause_weight / clause_occur NULL: Or / And
+ * (sa_score_batch_topk_bool); clause_group / clause_tie NULL: no DisMax groups (sa_score_batch_topk_bool_occur);
+ * clause_node NULL: no nested nodes, n_nodes == n_queries (sa_score_batch_topk_bool_dismax) -- plus the mask over the
+ * index's n_docs docs.  Per query the result is the top k of the unmasked call's scores where the query's mask is
+ * set; every score equals the unmasked one bit for bit. */
+int sa_score_batch_topk_bool_where(sa_index *index, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                   const uint32_t *clause_node, const uint32_t *clause_terms,
+                                   const uint32_t *clause_term_starts, const float *clause_idf,
+                                   const float *clause_weight, const uint8_t *clause_occur,
+                                   const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
+                                   uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
+                                   const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
+                                   uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
 
 /* The same batch in three stages, so a serving loop (or the benchmark) can keep the query
  * descriptors resident and time the device work alone: upload (H2D of descriptors), execute
@@ -348,6 +378,20 @@ int sa_multi_score_batch_topk_bool_nested(sa_multi *multi, uint32_t n_nodes, con
                                           const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
                                           uint32_t slop, const float *avg_doc_len, const float *k1, const float *b,
                                           uint32_t k, uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
+/* The multi-field entry points above with a document mask, as sa_score_batch_topk_bool_where: the arguments of
+ * sa_multi_score_batch_topk_bool_nested (clause_weight and clause_occur required; clause_group / clause_tie NULL: no
+ * DisMax groups; clause_node NULL: no nested nodes, n_nodes == n_queries) plus the mask over the fields' n_docs
+ * docs. */
+int sa_multi_score_batch_topk_bool_where(sa_multi *multi, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                         const uint32_t *clause_node, const uint32_t *clause_field,
+                                         const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                         const float *clause_idf, const float *clause_weight,
+                                         const uint8_t *clause_occur, const uint32_t *clause_group,
+                                         const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
+                                         uint32_t slop, const float *avg_doc_len, const float *k1, const float *b,
+                                         uint32_t k, const uint32_t *where_bits, uint64_t where_n,
+                                         uint64_t where_stride, uint32_t *out_docs, float *out_scores,
+                                         uint32_t *n_redone);
 
 /* ------------------------------------------------- per-op exports (parity tests)
  * Device implementations of the reference's native ops on raw arrays (host in, host out),

@@ -41,6 +41,12 @@
 // BoolState::rows and a per-(row, tile) flag records whether anything ranked, a tile that ranks nothing writing only
 // its flag.  A parent reads a nested clause's row as the clause's score (no BM25), present in a tile iff the child's
 // flag is set; the top-level nodes are collected and selected as in every other instance.
+//
+// bool_where_tile_kernel (sa_score_batch_topk_bool_where, sa_multi_score_batch_topk_bool_where) is each of the five
+// instances with a document mask (WhereMask, sa_term.cuh): a tile without an allowed doc is published empty before
+// any of its lists is read, and a disallowed doc is zeroed with the docs below mm, before the tile's bound is taken,
+// so the mask never changes a score, only which docs rank.  In a nested call only the top-level launch is masked:
+// a disallowed doc never ranks whatever its nested rows hold.
 #include "sa_multi.cuh"
 #include "sa_term.cuh"
 #include "sa_phrase.cuh"
@@ -112,6 +118,7 @@ struct BoolState {
     DevBuf d_fields;     // BoolField[] of a multi-field call
     DevBuf d_keys;       // nq * k result keys, then u32 overflow[nq]: one device-to-host copy
     DevBuf rows;
+    DevBuf d_where;      // the WhereMask rows of a `_where` call
 };
 void BoolStateDelete::operator()(BoolState *s) const { delete s; }
 
@@ -217,17 +224,37 @@ __device__ __forceinline__ void bool_set_field(BoolArgs &v, const BoolField *__r
     v.bm25 = e.bm25;
 }
 
+// The thread index read afresh (asm volatile, never merged with other reads), so that a rare `tid == 0` test in the
+// masked instances does not hold a predicate live through the fold (at the fields instance's 80-register cap it spilled).
+__device__ __forceinline__ unsigned bool_fresh_tid() {
+    unsigned t;
+    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+    return t;
+}
+
+// A (query, tile) where nothing ranks: no candidates, bound 0.  FRESH: thread 0 found by bool_fresh_tid.
+template <bool FRESH = false>
+__device__ __forceinline__ void bool_publish_empty(const TopkCtx &t, u32 q, u32 tile) {
+    if ((FRESH ? bool_fresh_tid() : threadIdx.x) == 0) {
+        const u64 t_idx = (u64)q * t.n_tiles + tile;
+        t.tile_cnt[t_idx] = 0;
+        t.tile_max[t_idx] = 0;
+    }
+}
+
 // The tile fold of one (query, tile).  OCCUR = false: Or / And (every clause SHOULD, weight 1).  OCCUR = true:
 // per-clause roles and weights in occ[], indexed as a.clauses; a query's mm counts its SHOULD clauses.  FIELDS: each
 // clause reads the field fld[clause.field] (bool_set_field) in place of the index in `a`; n_docs, doc_base, the
 // phrase rows and the top-k context stay common.  DISMAX (with OCCUR and FIELDS): clauses form groups (grp[], indexed
 // as a.clauses); mm counts SHOULD groups; s_dyn holds the groups' running max and sum, 2 * 32 floats per thread, and
 // s_g[3] (shared) the groups' presence masks.  NESTED (with DISMAX): nested clauses and the store pass (BoolNest).
-template <bool OCCUR, bool FIELDS, bool DISMAX = false, bool NESTED = false>
+// WHERE: only docs whose bit of the mask row of query blockIdx.x is set rank (never in a store pass).
+template <bool OCCUR, bool FIELDS, bool DISMAX = false, bool NESTED = false, bool WHERE = false>
 __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__restrict__ occ,
                                           const BoolField *__restrict__ fld,
                                           const BoolGroup *__restrict__ grp = nullptr, float *s_dyn = nullptr,
-                                          unsigned long long *s_g = nullptr, const BoolNest nb = BoolNest{}) {
+                                          unsigned long long *s_g = nullptr, const BoolNest nb = BoolNest{},
+                                          const WhereMask wh = WhereMask{nullptr, 0}) {
     constexpr int PER = SA_TILE_DOCS / SA_TERM_THREADS / 4;        // float4 groups per thread
     __shared__ __align__(16) float s_tile[SA_TILE_DOCS];
     __shared__ u32 s_lo[SA_BOOL_MAX_CLAUSES], s_hi[SA_BOOL_MAX_CLAUSES];
@@ -247,9 +274,20 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
     // 1. zero the tile; every clause's slice of the tile, and how many clauses have anything in it
 #pragma unroll
     for (int j = 0; j < PER; j++) s_tile4[tid + j * SA_TERM_THREADS] = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (tid == 0) s_present = 0;
-    if (DISMAX && tid == 0) s_g_present = s_g_should = s_g_req = 0;
-    __syncthreads();
+    const bool tid0 = WHERE ? bool_fresh_tid() == 0 : tid == 0;
+    if (tid0) s_present = 0;
+    if (DISMAX && tid0) s_g_present = s_g_should = s_g_req = 0;
+    u32 allow = ~0u;                       // WHERE: bit 4 j + e: the mask allows doc 4 g + e
+    if (WHERE) {
+        // no allowed doc in the tile: nothing ranks, and no list is read (contiguous filters skip whole tiles)
+        allow = where_word(wh, q, tile);
+        if (!__syncthreads_or(allow != 0)) {
+            bool_publish_empty<true>(a.topk, q, tile);
+            return;
+        }
+    } else {
+        __syncthreads();
+    }
     for (u32 c = warp; c < bq.n; c += SA_TERM_THREADS / 32) {      // warp-uniform
         const BoolClause cl = a.clauses[bq.c0 + c];
         bool_set_field<FIELDS>(view, fld, cl.field);
@@ -299,11 +337,7 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
             if (tid == 0) nb.flags[(u64)bq.pad * nb.n_tiles + tile] = 0;
             return;
         }
-        if (tid == 0) {
-            const u64 t_idx = (u64)q * a.topk.n_tiles + tile;
-            a.topk.tile_cnt[t_idx] = 0;
-            a.topk.tile_max[t_idx] = 0;
-        }
+        bool_publish_empty(a.topk, q, tile);
         return;
     }
 
@@ -314,7 +348,9 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
     for (int i = 0; i < PER * 4; i++) acc[i] = 0.0f;
 #pragma unroll
     for (int j = 0; j < PER; j++) hits[j] = 0;
-    u32 req = ~0u, veto = 0;               // OCCUR: bit 4 j + e of the thread's docs (PER * 4 == 32)
+    // OCCUR: bit 4 j + e of the thread's docs (PER * 4 == 32).  WHERE: a doc the mask leaves out starts as a missed
+    // requirement, so step 4 drops it with the others without another register held through the fold
+    u32 req = allow, veto = 0;
     static_assert(PER * 4 == 32, "one u32 mask bit per owned doc");
     u32 any = 0;                           // DISMAX: bit 4 j + e: a member of the current group scores > 0 there
     float *s_m = s_dyn + tid, *s_t = s_dyn + PER * 4 * SA_TERM_THREADS + tid;
@@ -399,7 +435,9 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
     }
 
     // 4. docs with fewer than mm hits (or a sum <= 0 / NaN), and under OCCUR docs a MUST / FILTER clause misses or a
-    //    MUST_NOT clause matches, do not rank; collect the tile's top-k candidates
+    //    MUST_NOT clause matches, do not rank, nor under WHERE docs the mask leaves out (in `req`; zeroed here,
+    //    before my_max: a bound taken over disallowed scores could push allowed docs out of the candidates); collect
+    //    the tile's top-k candidates
     const u32 keep = req & ~veto;
     u32 my_max = 0;
 #pragma unroll
@@ -408,7 +446,7 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
 #pragma unroll
         for (int e = 0; e < 4; e++) {
             const float s = acc[j * 4 + e];
-            const bool ok = OCCUR ? ((keep >> (j * 4 + e)) & 1u) != 0 : true;
+            const bool ok = (OCCUR || WHERE) ? ((keep >> (j * 4 + e)) & 1u) != 0 : true;
             o[e] = (ok && ((hits[j] >> (8 * e)) & 0xFFu) >= bq.mm && s > 0.0f) ? s : 0.0f;
             my_max = max(my_max, __float_as_uint(o[e]));
         }
@@ -466,6 +504,20 @@ bool_fields_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, con
     bool_tile<true, true>(a, occ, fld);
 }
 
+// sa_score_batch_topk_bool_where / sa_multi_score_batch_topk_bool_where: the instances above with a document mask,
+// each held to its unmasked instance's CTAs per SM (MIN_CTAS; see DESIGN.md section 3.11).  Template arguments
+// (OCCUR, FIELDS, DISMAX, NESTED) of bool_tile_kernel<false>: (false, false, false, false), <true>: (true, false, ...),
+// bool_fields_tile_kernel: (true, true, false, false), bool_dismax_tile_kernel: (true, true, true, false),
+// bool_nested_tile_kernel's top-level launch: (true, true, true, true).
+template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, int MIN_CTAS>
+__global__ void __launch_bounds__(SA_TERM_THREADS, MIN_CTAS)
+bool_where_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
+                       const BoolGroup *__restrict__ grp, const BoolNest nb, const WhereMask wh) {
+    extern __shared__ __align__(16) float s_dyn[];
+    __shared__ unsigned long long s_g[3];
+    bool_tile<OCCUR, FIELDS, DISMAX, NESTED, true>(a, occ, fld, grp, s_dyn, s_g, nb, wh);
+}
+
 // ------------------------------------------------------------------------------------------------------------ host
 namespace {
 
@@ -479,6 +531,10 @@ struct BoolCall {
     BoolState *S = nullptr;
     DevBuf *cand = nullptr;
     PinnedBuf *h_pinned = nullptr;
+    // the `_where` entry points' mask, as passed (host; where_bits NULL: no mask), and its rows on the device
+    const uint32_t *where_bits = nullptr;
+    uint64_t where_n = 0, where_stride = 0;
+    WhereMask where{nullptr, 0};
     sa_index *lead() const { return ix[0]; }
 };
 
@@ -554,6 +610,10 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
     a.clauses = S.d_clauses.as<BoolClause>();
     a.queries = S.d_queries.as<BoolQuery>() + q0;
     a.topk = t;
+    WhereMask wh = X.where;                 // row 0 of the launch is query q0's
+    if (wh.bits) wh.bits += (u64)q0 * wh.stride;
+    const dim3 grid(nq, n_tiles);
+    const BoolNest no_nest{nullptr, nullptr, nullptr, 0};
     if (!P.nest.empty()) {
         // the nested nodes of these queries, deepest level first (one launch per level: a level's nodes of the run
         // are consecutive in P.nested), each into its row and flags; then the top-level nodes, collected
@@ -572,8 +632,27 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
             i = j;
         }
         nb.store = nullptr;
-        bool_nested_tile_kernel<<<dim3(nq, n_tiles), SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
-            a, S.d_occur.as<BoolOccur>(), S.d_fields.as<BoolField>(), S.d_groups.as<BoolGroup>(), nb);
+        if (wh.bits)
+            bool_where_tile_kernel<true, true, true, true, 2><<<grid, SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
+                a, S.d_occur.as<BoolOccur>(), S.d_fields.as<BoolField>(), S.d_groups.as<BoolGroup>(), nb, wh);
+        else
+            bool_nested_tile_kernel<<<dim3(nq, n_tiles), SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
+                a, S.d_occur.as<BoolOccur>(), S.d_fields.as<BoolField>(), S.d_groups.as<BoolGroup>(), nb);
+    } else if (wh.bits) {
+        const BoolOccur *occ = S.d_occur.as<BoolOccur>();
+        const BoolField *fld = S.d_fields.as<BoolField>();
+        if (!P.groups.empty())
+            bool_where_tile_kernel<true, true, true, false, 2><<<grid, SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
+                a, occ, fld, S.d_groups.as<BoolGroup>(), no_nest, wh);
+        else if (X.fields_kernel)
+            bool_where_tile_kernel<true, true, false, false, 3><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(
+                a, occ, fld, nullptr, no_nest, wh);
+        else if (P.occur.empty())
+            bool_where_tile_kernel<false, false, false, false, 2><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(
+                a, nullptr, nullptr, nullptr, no_nest, wh);
+        else
+            bool_where_tile_kernel<true, false, false, false, 3><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(
+                a, occ, nullptr, nullptr, no_nest, wh);
     } else if (!P.groups.empty())
         bool_dismax_tile_kernel<<<dim3(nq, n_tiles), SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
             a, S.d_occur.as<BoolOccur>(), S.d_fields.as<BoolField>(), S.d_groups.as<BoolGroup>());
@@ -605,7 +684,8 @@ int bool_dismax_smem(Kernel kernel) {
 // clause_group / clause_tie non-NULL (with clause_occur): DisMax groups, bool_dismax_tile_kernel with a field table.
 // clause_node non-NULL (with the DisMax arrays): n_nodes nodes, the first n_queries top-level, clause c being nested
 // node clause_node[c] unless SA_NO_NODE (sa_score_batch_topk_bool_nested); otherwise n_nodes == n_queries.
-int bool_topk(const BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts, const uint32_t *clause_node,
+// X.where_bits non-NULL: the document mask of the `_where` entry points, checked before any device work.
+int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts, const uint32_t *clause_node,
               const uint32_t *clause_field, const uint32_t *clause_terms, const uint32_t *clause_term_starts,
               const float *clause_idf, const float *clause_weight, const uint8_t *clause_occur,
               const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
@@ -666,6 +746,7 @@ int bool_topk(const BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_
         }
     }
     for (u32 n = n_queries; nested && n < n_nodes; n++) SA_CHECK(refs[n] == 1, "node %u is referenced by no clause", n);
+    if ((rc = sa_where_check(X.where_bits, X.where_n, X.where_stride, lead->n_docs))) return rc;
     const u32 c_begin = n_nodes ? query_clause_starts[0] : 0, c_end = n_nodes ? query_clause_starts[n_nodes] : 0;
     for (u32 c = c_begin; c < c_end; c++) {
         if (is_nested(c)) continue;
@@ -811,8 +892,13 @@ int bool_topk(const BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_
     if (occur) {
         SA_CUDA(cudaMemcpyAsync(S.d_occur.p, P.occur.data(), P.occur.size() * sizeof(BoolOccur), cudaMemcpyHostToDevice, lead->stream));
     }
+    if ((rc = sa_where_upload(lead, S.d_where, X.where_bits, lead->n_docs, X.where_stride, n_queries, &X.where)))
+        return rc;
     if (dismax) {
         if ((rc = nested ? bool_dismax_smem(bool_nested_tile_kernel) : bool_dismax_smem(bool_dismax_tile_kernel)))
+            return rc;
+        if (X.where.bits && (rc = nested ? bool_dismax_smem(bool_where_tile_kernel<true, true, true, true, 2>)
+                                         : bool_dismax_smem(bool_where_tile_kernel<true, true, true, false, 2>)))
             return rc;
         SA_CUDA(cudaMemcpyAsync(S.d_groups.p, P.groups.data(), P.groups.size() * sizeof(BoolGroup), cudaMemcpyHostToDevice, lead->stream));
     }
@@ -857,8 +943,8 @@ int bool_topk_index(sa_index *ix, uint32_t n_nodes, const uint32_t *query_clause
                     const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
                     const uint8_t *clause_occur, const uint32_t *clause_group, const float *clause_tie,
                     const uint32_t *mm, uint32_t n_queries, uint32_t slop,
-                    float avg_doc_len, float k1, float b, uint32_t k, uint32_t *out_docs, float *out_scores,
-                    uint32_t *n_redone) {
+                    float avg_doc_len, float k1, float b, uint32_t k, const uint32_t *where_bits, uint64_t where_n,
+                    uint64_t where_stride, uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
     SA_CHECK(ix && out_docs && out_scores, "NULL argument");
     SA_CHECK(n_nodes == 0 || (query_clause_starts && clause_terms && clause_term_starts && clause_idf && mm),
              "NULL argument");
@@ -875,6 +961,9 @@ int bool_topk_index(sa_index *ix, uint32_t n_nodes, const uint32_t *query_clause
     X.S = ix->boolq.get();
     X.cand = &ix->cand;
     X.h_pinned = &ix->h_pinned;
+    X.where_bits = where_bits;
+    X.where_n = where_n;
+    X.where_stride = where_stride;
     return bool_topk(X, n_nodes, query_clause_starts, clause_node, nullptr, clause_terms, clause_term_starts,
                      clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
                      out_docs, out_scores, n_redone);
@@ -886,7 +975,8 @@ int bool_topk_multi(sa_multi *m, uint32_t n_nodes, const uint32_t *query_clause_
                     const uint32_t *clause_terms, const uint32_t *clause_term_starts, const float *clause_idf,
                     const float *clause_weight, const uint8_t *clause_occur, const uint32_t *clause_group,
                     const float *clause_tie, const uint32_t *mm, uint32_t n_queries, uint32_t slop,
-                    const float *avg_doc_len, const float *k1, const float *b, uint32_t k, uint32_t *out_docs,
+                    const float *avg_doc_len, const float *k1, const float *b, uint32_t k,
+                    const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride, uint32_t *out_docs,
                     float *out_scores, uint32_t *n_redone) {
     SA_CHECK(m && out_docs && out_scores && avg_doc_len && k1 && b, "NULL argument");
     SA_CHECK(n_nodes == 0 || (query_clause_starts && clause_field && clause_terms && clause_term_starts &&
@@ -919,6 +1009,9 @@ int bool_topk_multi(sa_multi *m, uint32_t n_nodes, const uint32_t *query_clause_
     X.S = m->boolq.get();
     X.cand = &m->cand;
     X.h_pinned = &m->fields[0]->h_pinned;
+    X.where_bits = where_bits;
+    X.where_n = where_n;
+    X.where_stride = where_stride;
     return bool_topk(X, n_nodes, query_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
                      clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
                      out_docs, out_scores, n_redone);
@@ -931,8 +1024,8 @@ extern "C" int sa_score_batch_topk_bool(sa_index *ix, const uint32_t *query_clau
                                         uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
                                         uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
     return bool_topk_index(ix, n_queries, query_clause_starts, nullptr, clause_terms, clause_term_starts, clause_idf,
-                           nullptr, nullptr, nullptr, nullptr, mm, n_queries, slop, avg_doc_len, k1, b, k, out_docs,
-                           out_scores, n_redone);
+                           nullptr, nullptr, nullptr, nullptr, mm, n_queries, slop, avg_doc_len, k1, b, k, nullptr, 0,
+                           0, out_docs, out_scores, n_redone);
 }
 
 extern "C" int sa_score_batch_topk_bool_occur(sa_index *ix, const uint32_t *query_clause_starts,
@@ -944,7 +1037,7 @@ extern "C" int sa_score_batch_topk_bool_occur(sa_index *ix, const uint32_t *quer
     SA_CHECK(n_queries == 0 || (clause_weight && clause_occur), "NULL argument");
     return bool_topk_index(ix, n_queries, query_clause_starts, nullptr, clause_terms, clause_term_starts, clause_idf,
                            clause_weight, clause_occur, nullptr, nullptr, mm, n_queries, slop, avg_doc_len, k1, b, k,
-                           out_docs, out_scores, n_redone);
+                           nullptr, 0, 0, out_docs, out_scores, n_redone);
 }
 
 extern "C" int sa_score_batch_topk_bool_dismax(sa_index *ix, const uint32_t *query_clause_starts,
@@ -957,7 +1050,7 @@ extern "C" int sa_score_batch_topk_bool_dismax(sa_index *ix, const uint32_t *que
     SA_CHECK(n_queries == 0 || (clause_weight && clause_occur && clause_group && clause_tie), "NULL argument");
     return bool_topk_index(ix, n_queries, query_clause_starts, nullptr, clause_terms, clause_term_starts, clause_idf,
                            clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, avg_doc_len, k1,
-                           b, k, out_docs, out_scores, n_redone);
+                           b, k, nullptr, 0, 0, out_docs, out_scores, n_redone);
 }
 
 extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, const uint32_t *query_clause_starts,
@@ -969,7 +1062,7 @@ extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, const uint32_t *query
                                               uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
     return bool_topk_multi(m, n_queries, query_clause_starts, nullptr, clause_field, clause_terms, clause_term_starts,
                            clause_idf, clause_weight, clause_occur, nullptr, nullptr, mm, n_queries, slop, avg_doc_len,
-                           k1, b, k, out_docs, out_scores, n_redone);
+                           k1, b, k, nullptr, 0, 0, out_docs, out_scores, n_redone);
 }
 
 extern "C" int sa_multi_score_batch_topk_bool_dismax(sa_multi *m, const uint32_t *query_clause_starts,
@@ -984,7 +1077,7 @@ extern "C" int sa_multi_score_batch_topk_bool_dismax(sa_multi *m, const uint32_t
     SA_CHECK(n_queries == 0 || (clause_group && clause_tie), "NULL argument");
     return bool_topk_multi(m, n_queries, query_clause_starts, nullptr, clause_field, clause_terms, clause_term_starts,
                            clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop,
-                           avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
+                           avg_doc_len, k1, b, k, nullptr, 0, 0, out_docs, out_scores, n_redone);
 }
 
 extern "C" int sa_score_batch_topk_bool_nested(sa_index *ix, uint32_t n_nodes, const uint32_t *node_clause_starts,
@@ -999,7 +1092,7 @@ extern "C" int sa_score_batch_topk_bool_nested(sa_index *ix, uint32_t n_nodes, c
              "NULL argument");
     return bool_topk_index(ix, n_nodes, node_clause_starts, clause_node, clause_terms, clause_term_starts, clause_idf,
                            clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, avg_doc_len,
-                           k1, b, k, out_docs, out_scores, n_redone);
+                           k1, b, k, nullptr, 0, 0, out_docs, out_scores, n_redone);
 }
 
 extern "C" int sa_multi_score_batch_topk_bool_nested(sa_multi *m, uint32_t n_nodes, const uint32_t *node_clause_starts,
@@ -1014,5 +1107,42 @@ extern "C" int sa_multi_score_batch_topk_bool_nested(sa_multi *m, uint32_t n_nod
     SA_CHECK(n_nodes == 0 || (clause_node && clause_group && clause_tie), "NULL argument");
     return bool_topk_multi(m, n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
                            clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop,
-                           avg_doc_len, k1, b, k, out_docs, out_scores, n_redone);
+                           avg_doc_len, k1, b, k, nullptr, 0, 0, out_docs, out_scores, n_redone);
+}
+
+extern "C" int sa_score_batch_topk_bool_where(sa_index *ix, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                              const uint32_t *clause_node, const uint32_t *clause_terms,
+                                              const uint32_t *clause_term_starts, const float *clause_idf,
+                                              const float *clause_weight, const uint8_t *clause_occur,
+                                              const uint32_t *clause_group, const float *clause_tie,
+                                              const uint32_t *mm, uint32_t n_queries, uint32_t slop,
+                                              float avg_doc_len, float k1, float b, uint32_t k,
+                                              const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
+                                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+    SA_CHECK(!clause_weight == !clause_occur, "clause_weight and clause_occur are both given or both NULL");
+    SA_CHECK(!clause_group == !clause_tie && (!clause_group || clause_occur),
+             "clause_group and clause_tie are both given (with clause_occur) or both NULL");
+    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
+             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
+    return bool_topk_index(ix, n_nodes, node_clause_starts, clause_node, clause_terms, clause_term_starts, clause_idf,
+                           clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, avg_doc_len,
+                           k1, b, k, where_bits, where_n, where_stride, out_docs, out_scores, n_redone);
+}
+
+extern "C" int sa_multi_score_batch_topk_bool_where(sa_multi *m, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                                    const uint32_t *clause_node, const uint32_t *clause_field,
+                                                    const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                                    const float *clause_idf, const float *clause_weight,
+                                                    const uint8_t *clause_occur, const uint32_t *clause_group,
+                                                    const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
+                                                    uint32_t slop, const float *avg_doc_len, const float *k1,
+                                                    const float *b, uint32_t k, const uint32_t *where_bits,
+                                                    uint64_t where_n, uint64_t where_stride, uint32_t *out_docs,
+                                                    float *out_scores, uint32_t *n_redone) {
+    SA_CHECK(!clause_group == !clause_tie, "clause_group and clause_tie are both given or both NULL");
+    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
+             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
+    return bool_topk_multi(m, n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
+                           clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop,
+                           avg_doc_len, k1, b, k, where_bits, where_n, where_stride, out_docs, out_scores, n_redone);
 }

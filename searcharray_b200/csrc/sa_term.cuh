@@ -30,6 +30,25 @@ struct TopkCtx {
     u32 k;             // 0 => no top-k collection
 };
 
+// A document mask of the batched top-k (the `_where` entry points): one row of packed bits for the batch, or one per
+// query.  The tile kernels that take it (bool_tile, sim_tile) have thread tid own docs 4 g .. 4 g + 3 of a tile,
+// g = tid + j * SA_TERM_THREADS (flush_tile_collect's layout), so a row stores its bits in that owner order, not in
+// doc order: word tile * SA_TERM_THREADS + tid holds, at bit 4 j + e, doc tile * SA_TILE_DOCS + 4 g + e.  A thread
+// then reads its 32 bits as one u32 and a warp one 128-byte line; in doc order each thread would gather a nibble
+// from each of 8 words.  Bits past the last doc are 0.
+struct WhereMask {
+    const u32 *bits;   // row 0 of the mask on the device; NULL: no mask
+    u64 stride;        // words from one query's row to the next; 0: one row for every query
+};
+
+// The calling thread's 32 mask bits of `tile` in mask row `row`.  The thread index is read afresh (asm volatile):
+// merged with the kernel's other reads, its 64-bit widening stayed live through the tile fold and spilled.
+__device__ __forceinline__ u32 where_word(const WhereMask &w, u64 row, u32 tile) {
+    unsigned tid;
+    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(tid));
+    return __ldg(w.bits + row * w.stride + (u64)tile * SA_TERM_THREADS + tid);
+}
+
 struct TermBatchArgs {
     const u64 *words;
     const float *doc_lens;
@@ -67,9 +86,12 @@ int launch_topk_select_f64(sa_index *ix, const TopkCtx &t, const u64 *d_tile_d, 
 // NULL: doc i) and its doc length from doc_lens as sim_tile_kernel describes.  bm25 / sim: the parameters of the
 // kind; tile_d: the float64 candidate scores (SA_SIM_CLASSIC only).
 struct SimParams;
+// wh (sim_where_tile_kernel): position i ranks only where its mask bit is set, in the mask row of query
+// d_row_query[j] for row j.
 int launch_sim_tiles(sa_index *ix, int kind, const float *counts, const u64 *rows, const float *doc_lens, u64 n_pos,
                      const Bm25Params &bm25, const SimParams &sim, const double *d_idf, u32 n, u32 row0,
-                     const TopkCtx &t, u64 *tile_d);
+                     const TopkCtx &t, u64 *tile_d, const WhereMask &wh = WhereMask{nullptr, 0},
+                     const u32 *d_row_query = nullptr);
 int launch_topk_merge(sa_index *ix, const u64 *d_in, u64 rank_stride, u32 world, u32 n_queries, u32 k, u64 *d_out);
 // A batch's result block in HBM: nq * k keys followed by SA_BATCH_TAIL summary words written by the batch's last
 // kernel -- [0] queries that need the exact host-side re-run (candidate overflow, wrong same-term guess, scratch
@@ -97,6 +119,15 @@ int sa_copy_out_dense(sa_index *ix, float *out_host);
 // Dense rows are padded to whole tiles.
 inline u32 sa_n_tiles(u64 n_docs) { return (u32)((n_docs + SA_TILE_DOCS - 1) / SA_TILE_DOCS); }
 inline u64 sa_padded_docs(u64 n_docs) { return (u64)sa_n_tiles(n_docs) * SA_TILE_DOCS; }
+static_assert(SA_WHERE_WORDS(1) == SA_TERM_THREADS && SA_WHERE_WORDS(SA_TILE_DOCS + 1) == 2 * SA_TERM_THREADS,
+              "a WhereMask row is SA_TERM_THREADS words per tile");
+// The `_where` entry points' mask arguments against the n docs (positions) the call ranks, on the host: where_bits
+// NULL (no mask), or where_n == n and where_stride 0 or SA_WHERE_WORDS(n).
+int sa_where_check(const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride, u64 n);
+// A checked mask's rows over n docs (one, or n_queries when where_stride != 0) into buf on ix->stream; *out addresses
+// them (bits NULL without a mask).
+int sa_where_upload(sa_index *ix, DevBuf &buf, const uint32_t *where_bits, u64 n, uint64_t where_stride, u32 n_queries,
+                    WhereMask *out);
 
 inline Bm25Params make_bm25(float idf, float avg_doc_len, float k1, float b, bool doc_lens_nonneg) {
     Bm25Params p;

@@ -37,6 +37,7 @@ struct ViewState {
     DevBuf d_keys;         // u64 [n_queries * k]: the result keys
     DevBuf d_cand_d;       // u64 [chunk][tiles][slots]: float64 score bits of the classic candidates
     DevBuf d_scores;       // double [n_queries * k]: the classic result scores
+    DevBuf d_where;        // the WhereMask rows of sa_score_batch_topk_sim_where
 };
 
 void ViewStateDelete::operator()(ViewState *v) const { delete v; }
@@ -65,11 +66,13 @@ template <int KIND> using TileParams = std::conditional_t<KIND == SA_SIM_BM25, B
 //   classic: score = fl64(fl64(idf * sqrt_tf) * inv_sqrt_dl) has no exact float32 key.  The tile ranks by
 //            f64_proxy_key(score) and collects with collect_tile_f64 (every position at or above the bound, the
 //            float64 scores in tile_d, overflow -> the exact re-run); topk_select_f64_kernel ranks in float64.
-template <int KIND>
-__global__ void __launch_bounds__(SA_TERM_THREADS)
-sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *__restrict__ rows,
-                const float *__restrict__ doc_lens, u64 n_pos, TileParams<KIND> p, const double *__restrict__ idf,
-                u32 row0, const TopkCtx t, u64 *__restrict__ tile_d) {
+// WHERE (sim_where_tile_kernel): position i scores only where its bit of the mask row of query
+// row_query[blockIdx.y] is set; the others are +0, as a position without the term, before the tile's bound is taken.
+template <int KIND, bool WHERE>
+__device__ __forceinline__ void sim_tile(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *__restrict__ rows,
+                                         const float *__restrict__ doc_lens, u64 n_pos, TileParams<KIND> p,
+                                         const double *__restrict__ idf, u32 row0, const TopkCtx &t,
+                                         u64 *__restrict__ tile_d, const WhereMask &wh, const u32 *__restrict__ row_query) {
     constexpr int PER_THREAD = SA_TILE_DOCS / SA_TERM_THREADS;
     __shared__ __align__(16) float s_out[KIND == SA_SIM_CLASSIC ? 4 : SA_TILE_DOCS];
     __shared__ u32 s_top[(SA_TERM_THREADS / 32) * 8];
@@ -82,6 +85,8 @@ sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *_
     if constexpr (KIND == SA_SIM_BM25) p.idf = (float)q_idf;
     u32 my_max = 0;
     u32 key[PER_THREAD];          // classic: the proxy bits of the thread's positions
+    u32 allow = ~0u;              // bit 4 j + e: position 4 g + e may rank
+    if (WHERE) allow = where_word(wh, __ldg(row_query + blockIdx.y), tile);
     // thread tid owns positions 4g .. 4g+3 of the tile for g = tid + j * SA_TERM_THREADS (flush_tile_collect's layout)
 #pragma unroll
     for (int j = 0; j < PER_THREAD / 4; j++) {
@@ -91,7 +96,7 @@ sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *_
         for (int e = 0; e < 4; e++) {
             const u64 i = pos0 + g * 4 + e;
             v[e] = 0.0f;
-            if (i < n_pos) {
+            if (i < n_pos && ((allow >> (j * 4 + e)) & 1u)) {
                 const u64 doc = rows ? __ldg(rows + i) : i;
                 const float tf = __ldg(counts + doc);
                 if (tf > 0.0f) {
@@ -127,6 +132,25 @@ sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *_
     }
 }
 
+template <int KIND>
+__global__ void __launch_bounds__(SA_TERM_THREADS)
+sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *__restrict__ rows,
+                const float *__restrict__ doc_lens, u64 n_pos, TileParams<KIND> p, const double *__restrict__ idf,
+                u32 row0, const TopkCtx t, u64 *__restrict__ tile_d) {
+    sim_tile<KIND, false>(doc_rows, doc_stride, rows, doc_lens, n_pos, p, idf, row0, t, tile_d, WhereMask{nullptr, 0},
+                          nullptr);
+}
+
+// sa_score_batch_topk_sim_where: sim_tile_kernel with a document mask over the positions.
+template <int KIND>
+__global__ void __launch_bounds__(SA_TERM_THREADS)
+sim_where_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *__restrict__ rows,
+                      const float *__restrict__ doc_lens, u64 n_pos, TileParams<KIND> p, const double *__restrict__ idf,
+                      u32 row0, const TopkCtx t, u64 *__restrict__ tile_d, const WhereMask wh,
+                      const u32 *__restrict__ row_query) {
+    sim_tile<KIND, true>(doc_rows, doc_stride, rows, doc_lens, n_pos, p, idf, row0, t, tile_d, wh, row_query);
+}
+
 // One call's queries and scoring.
 struct SimRun {
     int kind;                 // SA_SIM_*
@@ -134,24 +158,30 @@ struct SimRun {
     SimParams sim;            // the other kinds
     const u32 *terms, *term_starts;
     u32 slop;
+    WhereMask where;          // bits NULL: no mask
     const u32 *tids(u32 q) const { return terms + term_starts[q]; }
     u32 n_terms(u32 q) const { return term_starts[q + 1] - term_starts[q]; }
 };
 
 int launch_sim_tiles(sa_index *ix, int kind, const float *counts, const u64 *rows, const float *doc_lens, u64 n_pos,
                      const Bm25Params &bm25, const SimParams &sim, const double *d_idf, u32 n, u32 row0,
-                     const TopkCtx &t, u64 *tile_d) {
+                     const TopkCtx &t, u64 *tile_d, const WhereMask &wh, const u32 *d_row_query) {
     if (n == 0 || t.n_tiles == 0) return SA_OK;
     const u64 stride = sa_padded_docs(ix->n_docs);
     const dim3 grid(t.n_tiles, n);
     KernelTimer tm(ix, 1);
 #define SA_SIM_TILES(KIND, P)                                                                                       \
-    sim_tile_kernel<KIND><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(counts, stride, rows, doc_lens, n_pos, P, d_idf, \
-                                                                    row0, t, tile_d)
-    if (kind == SA_SIM_BM25) SA_SIM_TILES(SA_SIM_BM25, bm25);
-    else if (kind == SA_SIM_BM25_IMPACT) SA_SIM_TILES(SA_SIM_BM25_IMPACT, sim);
-    else if (kind == SA_SIM_BM25_LEGACY) SA_SIM_TILES(SA_SIM_BM25_LEGACY, sim);
-    else SA_SIM_TILES(SA_SIM_CLASSIC, sim);
+    if (wh.bits)                                                                                                    \
+        sim_where_tile_kernel<KIND><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(counts, stride, rows, doc_lens, n_pos, \
+                                                                              P, d_idf, row0, t, tile_d, wh,       \
+                                                                              d_row_query);                        \
+    else                                                                                                            \
+        sim_tile_kernel<KIND><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(counts, stride, rows, doc_lens, n_pos, P,   \
+                                                                        d_idf, row0, t, tile_d)
+    if (kind == SA_SIM_BM25) { SA_SIM_TILES(SA_SIM_BM25, bm25); }
+    else if (kind == SA_SIM_BM25_IMPACT) { SA_SIM_TILES(SA_SIM_BM25_IMPACT, sim); }
+    else if (kind == SA_SIM_BM25_LEGACY) { SA_SIM_TILES(SA_SIM_BM25_LEGACY, sim); }
+    else { SA_SIM_TILES(SA_SIM_CLASSIC, sim); }
 #undef SA_SIM_TILES
     SA_CUDA(cudaGetLastError());
     tm.stop();
@@ -160,13 +190,15 @@ int launch_sim_tiles(sa_index *ix, int kind, const float *counts, const u64 *row
     return SA_OK;
 }
 
-// The tile pass over ix->dense rows [0, n): row j holds the counts of row row0 + j of t, d_idf[j] is its idf.
-static int launch_tiles(sa_index *ix, const SimRun &R, const double *d_idf, u32 n, u32 row0, const TopkCtx &t) {
+// The tile pass over ix->dense rows [0, n): row j holds the counts of call row call_row + j (its idf
+// V.d_idf[call_row + j], its query V.d_row_query[call_row + j]), collected into row row0 + j of t.
+static int launch_tiles(sa_index *ix, const SimRun &R, u32 call_row, u32 n, u32 row0, const TopkCtx &t) {
     ViewState &V = *ix->view;
     const bool view = ix->rows_active;
     return launch_sim_tiles(ix, R.kind, ix->dense.as<float>(), view ? ix->d_rows() : nullptr,
                             R.kind == SA_SIM_BM25 ? V.d_dl.as<float>() : ix->d_doc_lens.as<float>(),
-                            view ? ix->n_rows : ix->n_docs, R.bm25, R.sim, d_idf, n, row0, t, V.d_cand_d.as<u64>());
+                            view ? ix->n_rows : ix->n_docs, R.bm25, R.sim, V.d_idf.as<double>() + call_row, n, row0,
+                            t, V.d_cand_d.as<u64>(), R.where, V.d_row_query.as<u32>() + call_row);
 }
 
 static int launch_select(sa_index *ix, int kind, const TopkCtx &t, u32 n_queries, const u32 *d_out_index) {
@@ -178,11 +210,11 @@ static int launch_select(sa_index *ix, int kind, const TopkCtx &t, u32 n_queries
     return launch_topk_select(ix, t, n_queries, doc_base, V.d_keys.as<u64>(), d_out_index);
 }
 
-// Term queries qs[0, n): their tf into ix->dense rows [0, n), then their tile pass (rows row0 + j of t, idf
-// d_idf[j]).  A view keeps or drops WHOLE docs (no position filter here), so a doc of the view has the same tf in the
+// Term queries qs[0, n): their tf into ix->dense rows [0, n), then their tile pass (rows row0 + j of t, call
+// rows call_row + j).  A view keeps or drops WHOLE docs (no position filter here), so a doc of the view has the same tf in the
 // filtered list as in the index's own list: the term kernel runs on the own lists, with the tf table, and no
 // compaction.  Docs outside the view get counts too; the tile pass never gathers them.
-static int term_tiles(sa_index *ix, const SimRun &R, const u32 *qs, u32 n, const double *d_idf, u32 row0,
+static int term_tiles(sa_index *ix, const SimRun &R, const u32 *qs, u32 n, u32 call_row, u32 row0,
                       const TopkCtx &t) {
     ViewState &V = *ix->view;
     if (n == 0) return SA_OK;
@@ -196,13 +228,13 @@ static int term_tiles(sa_index *ix, const SimRun &R, const u32 *qs, u32 n, const
     TermBatchArgs a = make_term_args(ix, V.d_tq.as<TermQuery>(), make_bm25(0, 1, 1, 0, ix->doc_lens_nonneg), none);
     a.mode = TERM_MODE_TF;
     if ((rc = launch_term_batch(ix, a, n))) return rc;
-    return launch_tiles(ix, R, d_idf, n, row0, t);
+    return launch_tiles(ix, R, call_row, n, row0, t);
 }
 
 // Phrase / slop queries qs[0, n), one at a time: raw counts into ix->dense row 0 (sa_phrase_row), then the query's
-// tile pass (row row0 + j of t, idf d_idf[j]).  On a view, one filter pass over every list of the n queries comes
+// tile pass (row row0 + j of t, call row call_row + j).  On a view, one filter pass over every list of the n queries comes
 // first; a missing query has no filtered lists, and sa_phrase_row reads none for it.
-static int phrase_tiles(sa_index *ix, const SimRun &R, const u32 *qs, u32 n, const double *d_idf, u32 row0,
+static int phrase_tiles(sa_index *ix, const SimRun &R, const u32 *qs, u32 n, u32 call_row, u32 row0,
                         const TopkCtx &t) {
     const bool view = ix->rows_active;
     std::vector<u32> ftids, fstart;
@@ -223,7 +255,7 @@ static int phrase_tiles(sa_index *ix, const SimRun &R, const u32 *qs, u32 n, con
         bool scored;
         if ((rc = sa_phrase_row(ix, R.tids(qs[j]), R.n_terms(qs[j]), R.slop, view ? f_offs.data() + fstart[j] : nullptr,
                                 view ? f_lens.data() + fstart[j] : nullptr, nullptr, &scored)) ||
-            (rc = launch_tiles(ix, R, d_idf + j, 1, row0 + j, t))) return rc;
+            (rc = launch_tiles(ix, R, call_row + j, 1, row0 + j, t))) return rc;
     }
     return SA_OK;
 }
@@ -249,10 +281,41 @@ static int download(sa_index *ix, bool classic, u32 nq, u32 k, std::vector<u64> 
     return SA_OK;
 }
 
+int sa_where_check(const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride, u64 n) {
+    if (!where_bits) return SA_OK;
+    SA_CHECK(where_n == n, "the mask covers %llu docs, the call ranks %llu", (unsigned long long)where_n,
+             (unsigned long long)n);
+    SA_CHECK(where_stride == 0 || where_stride == SA_WHERE_WORDS(n),
+             "where_stride must be 0 (one mask) or %llu words (a mask per query), not %llu",
+             (unsigned long long)SA_WHERE_WORDS(n), (unsigned long long)where_stride);
+    return SA_OK;
+}
+
+int sa_where_upload(sa_index *ix, DevBuf &buf, const uint32_t *where_bits, u64 n, uint64_t where_stride, u32 n_queries,
+                    WhereMask *out) {
+    *out = WhereMask{nullptr, where_stride};
+    if (!where_bits) return SA_OK;
+    const size_t bytes = (where_stride ? (size_t)n_queries : 1) * SA_WHERE_WORDS(n) * sizeof(u32);
+    int rc;
+    if ((rc = buf.reserve(std::max<size_t>(bytes, 4)))) return rc;
+    SA_CUDA(cudaMemcpyAsync(buf.p, where_bits, bytes, cudaMemcpyHostToDevice, ix->stream));
+    out->bits = buf.as<u32>();
+    return SA_OK;
+}
+
 extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *terms, const uint32_t *term_starts,
                                        const double *idf, uint32_t n_queries, uint32_t slop,
                                        const float *view_doc_lens, double avg_doc_len, double k1, double b,
                                        uint32_t k, uint32_t *out_ids, double *out_scores) {
+    return sa_score_batch_topk_sim_where(ix, kind, terms, term_starts, idf, n_queries, slop, view_doc_lens,
+                                         avg_doc_len, k1, b, k, nullptr, 0, 0, out_ids, out_scores);
+}
+
+extern "C" int sa_score_batch_topk_sim_where(sa_index *ix, int kind, const uint32_t *terms,
+                                             const uint32_t *term_starts, const double *idf, uint32_t n_queries,
+                                             uint32_t slop, const float *view_doc_lens, double avg_doc_len, double k1,
+                                             double b, uint32_t k, const uint32_t *where_bits, uint64_t where_n,
+                                             uint64_t where_stride, uint32_t *out_ids, double *out_scores) {
     SA_CHECK(ix, "index is NULL");
     SA_CHECK(n_queries == 0 || (terms && term_starts && idf && out_ids && out_scores), "NULL argument");
     SA_CHECK(kind == SA_SIM_BM25 || kind == SA_SIM_BM25_IMPACT || kind == SA_SIM_BM25_LEGACY || kind == SA_SIM_CLASSIC,
@@ -272,6 +335,7 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
     const u64 n_pos = view ? ix->n_rows : ix->n_docs;
     SA_CHECK(n_pos < 0xFFFFFFFFull, "the array must have fewer than 2^32 - 1 rows");
     SA_CHECK(kind != SA_SIM_BM25 || n_pos == 0 || view_doc_lens, "view_doc_lens is NULL");
+    if ((rc = sa_where_check(where_bits, where_n, where_stride, n_pos))) return rc;
     SA_CUDA(cudaSetDevice(ix->device));
     const size_t nk = (size_t)n_queries * k;
     for (size_t i = 0; i < nk; i++) { out_ids[i] = SA_NO_DOC; out_scores[i] = 0.0; }
@@ -282,8 +346,8 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
     if (!ix->view) ix->view.reset(new ViewState());
     ViewState &V = *ix->view;
     // BM25 exactly as ops.bm25_score -> sa_op_bm25_score sets it up: float32 parameters, `1 - b` in float32
-    const SimRun R{kind, make_bm25(0.0f, (float)avg_doc_len, (float)k1, (float)b, false),
-                   make_sim_params(avg_doc_len, k1, b), terms, term_starts, slop};
+    SimRun R{kind, make_bm25(0.0f, (float)avg_doc_len, (float)k1, (float)b, false),
+             make_sim_params(avg_doc_len, k1, b), terms, term_starts, slop, WhereMask{nullptr, 0}};
     const u32 n_tiles = sa_n_tiles(n_pos), slots = classic ? 256u : sa_topk_slots(k);
     const RowPlan plan = sa_plan_rows(ix->n_docs, term_starts, n_queries);
     const u32 chunk = plan.chunk;
@@ -299,6 +363,7 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
     if ((rc = ix->cand.reserve(cand_bytes(n_tiles, chunk, slots)))) return rc;
     if (classic && (rc = V.d_scores.reserve(nk * sizeof(double)))) return rc;
     if (classic && (rc = V.d_cand_d.reserve((size_t)chunk * n_tiles * slots * sizeof(u64)))) return rc;
+    if ((rc = sa_where_upload(ix, V.d_where, where_bits, n_pos, where_stride, n_queries, &R.where))) return rc;
 
     std::vector<double> row_idf(n_queries);
     for (u32 r = 0; r < n_queries; r++) row_idf[r] = idf[row_query[r]];
@@ -307,14 +372,13 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
     SA_CUDA(cudaMemcpyAsync(V.d_idf.p, row_idf.data(), n_queries * sizeof(double), cudaMemcpyHostToDevice, ix->stream));
     SA_CUDA(cudaMemcpyAsync(V.d_row_query.p, row_query.data(), n_queries * sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
     SA_CUDA(cudaMemsetAsync(V.d_ovf.p, 0, n_queries * sizeof(u32), ix->stream));
-    const double *d_idf = V.d_idf.as<double>();
 
     for (const RowChunk &C : plan.chunks) {
         const u32 Q = C.n_term + C.n_phrase;
         const u32 *qs = row_query.data() + C.row0;
         TopkCtx t = make_topk_ctx(ix->cand.p, n_tiles, Q, slots, k, V.d_ovf.as<u32>() + C.row0);
-        if ((rc = phrase_tiles(ix, R, qs + C.n_term, C.n_phrase, d_idf + C.row0 + C.n_term, C.n_term, t))) return rc;
-        if ((rc = term_tiles(ix, R, qs, C.n_term, d_idf + C.row0, 0, t))) return rc;
+        if ((rc = phrase_tiles(ix, R, qs + C.n_term, C.n_phrase, C.row0 + C.n_term, C.n_term, t))) return rc;
+        if ((rc = term_tiles(ix, R, qs, C.n_term, C.row0, 0, t))) return rc;
         if ((rc = launch_select(ix, kind, t, Q, V.d_row_query.as<u32>() + C.row0))) return rc;
     }
     std::vector<u64> keys;
@@ -330,7 +394,7 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
         SA_CUDA(cudaMemsetAsync(V.d_ovf.as<u32>() + r, 0, sizeof(u32), ix->stream));
         TopkCtx t = make_topk_ctx(ix->cand.p, n_tiles, 1, SA_TILE_DOCS, k, V.d_ovf.as<u32>() + r);
         const bool term = R.n_terms(row_query[r]) == 1;
-        if ((rc = (term ? term_tiles : phrase_tiles)(ix, R, &row_query[r], 1, d_idf + r, 0, t))) return rc;
+        if ((rc = (term ? term_tiles : phrase_tiles)(ix, R, &row_query[r], 1, r, 0, t))) return rc;
         if ((rc = launch_select(ix, kind, t, 1, V.d_row_query.as<u32>() + r))) return rc;
         redone = true;
     }

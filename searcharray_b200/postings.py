@@ -144,6 +144,42 @@ class _PinnedPool:
 
 _pool = _PinnedPool()
 
+_TILE_DOCS, _TILE_THREADS = 8192, 256          # SA_TILE_DOCS, SA_TERM_THREADS (csrc/sa_term.cuh)
+
+
+def pack_where(where, n, n_queries):
+    """The `where=` mask of search_topk / fields_topk over n docs for n_queries queries, checked before any device
+    work -- a dtype other than bool raises TypeError, a shape other than (n,) or (n_queries, n) ValueError -- and
+    packed as the `_where` entry points take it: uint32[R, SA_WHERE_WORDS(n)], R = 1 (one mask for the batch) or
+    n_queries.  Bits are in the tile kernels' owner order (include/searcharray_b200.h): bit 4 j + e of word
+    t * 256 + i is doc t * 8192 + 4 (i + 256 j) + e; bits past n are 0."""
+    w = np.asarray(where)
+    if w.dtype != np.bool_:
+        raise TypeError(f"where must be a boolean mask (dtype bool), not dtype {w.dtype}")
+    if w.shape != (n,) and w.shape != (n_queries, n):
+        raise ValueError(f"where must have shape ({n},) or ({n_queries}, {n}) (one mask per query), not {w.shape}")
+    rows = w.reshape(1 if w.ndim == 1 else n_queries, n)
+    n_tiles = -(-n // _TILE_DOCS)
+    padded = np.zeros((rows.shape[0], n_tiles * _TILE_DOCS), dtype=bool)
+    padded[:, :n] = rows
+    # [row, tile, j, i, e] -> [row, tile, i, j, e]: thread i's 32 docs, bit 4 j + e
+    owner = padded.reshape(rows.shape[0], n_tiles, 32 // 4, _TILE_THREADS, 4).transpose(0, 1, 3, 2, 4)
+    packed = np.packbits(owner.reshape(rows.shape[0], n_tiles * _TILE_THREADS, 32), axis=-1, bitorder="little")
+    return np.ascontiguousarray(packed).view("<u4").reshape(rows.shape[0], n_tiles * _TILE_THREADS).astype(
+        np.uint32, copy=False)
+
+
+def _where_args(bits):
+    """A packed mask as the C calls take it: (where_bits, where_stride); one row is the batch's mask, None no mask."""
+    if bits is None:
+        return None, 0
+    return _lib.p_u32(bits), (bits.shape[1] if bits.shape[0] > 1 else 0)
+
+
+def _where_part(bits, sel):
+    """The packed mask of the queries `sel` selects (a one-row mask is every query's)."""
+    return bits if bits is None or bits.shape[0] == 1 else np.ascontiguousarray(bits[sel])
+
 
 class DeviceIndex:
     """Owns one sa_index handle (one shard in one GPU's HBM)."""
@@ -486,7 +522,7 @@ class SearchArray(ExtensionArray):
         return out
 
     # -------------------------------------------------- batched, HBM-resident path
-    def search_topk(self, queries, k=10, similarity: Similarity = default_bm25, slop=0):
+    def search_topk(self, queries, k=10, similarity: Similarity = default_bm25, slop=0, where=None):
         """queries: list of str (term) or list[str] (phrase).  Returns (docs uint32[Q,k],
         scores float32[Q,k]): per query the k best scores > 0, by score descending then id ascending, empty
         slots NO_DOC / 0.  Scores never leave HBM except the top-k (sa_score_batch_topk).
@@ -520,13 +556,28 @@ class SearchArray(ExtensionArray):
 
         An Or / And / Bool may be a clause of another, at any depth (Or([And(["star", "wars"]), And(["star", "trek"])])):
         it scores what it would rank as a query of its own and matches where that is > 0
-        (sa_score_batch_topk_bool_nested); see query.Or."""
+        (sa_score_batch_topk_bool_nested); see query.Or.
+
+        where: a document filter -- a boolean array-like (a boolean pd.Series too) of shape (len(self),), one mask for
+        the batch, or (len(queries), len(self)), one per query -- ranks each query only among the docs its mask
+        allows, as Lucene's filter context does: the result is the top k of np.where(mask_q, S_q, 0), S_q being what
+        the call without `where` ranks (.score, or the boolean composition), under the same rule, ids and dtypes.
+        The mask never changes a score: idf, document frequencies, avgdl and doc lengths stay those of the whole
+        array (of the view, on a view).  On a view it indexes the view's positions, on a shard the shard's rows.
+        A dtype other than bool raises TypeError and another shape ValueError, before any device work; every input
+        refused without `where` is refused the same way with it.  Plain BM25 queries on the unsliced array rank as
+        one-clause Or queries (sa_score_batch_topk_bool_where); the others take sa_score_batch_topk_sim_where.  A
+        mask per query costs len(self) / 8 bytes of host-to-device copy and device memory per query."""
         from .query import is_boolean
+        if where is not None:
+            queries = list(queries)
+            bits = pack_where(where, len(self), len(queries))
+            if any(is_boolean(q) for q in queries):
+                return self._search_topk_mixed(queries, k, similarity, slop, bits)
+            return self._search_topk_plain_where(queries, k, similarity, slop, bits)
         if any(is_boolean(q) for q in queries):
             return self._search_topk_mixed(list(queries), k, similarity, slop)
-        if not isinstance(similarity, (Bm25Similarity, Bm25Impact, Bm25Legacy, ClassicSimilarity)):
-            raise TypeError("search_topk supports bm25_similarity, bm25_impact, bm25_legacy_similarity and "
-                            f"classic_similarity, not {similarity!r}")
+        self._check_topk_similarity(similarity)
         if self.rows is not None or not isinstance(similarity, Bm25Similarity):
             return self._search_topk_sim(queries, k, similarity, slop)
         terms, starts, idfs = self._topk_queries(queries, lambda dfs: compute_idf(self.corpus_size, dfs))
@@ -541,10 +592,38 @@ class SearchArray(ExtensionArray):
                                                       _lib.p_u32(docs), _lib.p_f32(scores)))
         return docs, scores
 
-    def _search_topk_mixed(self, queries, k, similarity, slop):
+    @staticmethod
+    def _check_topk_similarity(similarity):
+        if not isinstance(similarity, (Bm25Similarity, Bm25Impact, Bm25Legacy, ClassicSimilarity)):
+            raise TypeError("search_topk supports bm25_similarity, bm25_impact, bm25_legacy_similarity and "
+                            f"classic_similarity, not {similarity!r}")
+
+    def _search_topk_plain_where(self, queries, k, similarity, slop, where):
+        """search_topk of plain queries with a packed mask (pack_where): on a view or under a non-BM25 similarity
+        through sa_score_batch_topk_sim_where, else each query as a one-clause Or through the boolean fold, which
+        scores a clause exactly as .score(c, slop=slop).  The clauses are taken as the unmasked batch takes its
+        queries (_topk_queries: a str is a term, any other iterable of str a phrase), and the C call checks their
+        term counts as the unmasked one does."""
+        self._check_topk_similarity(similarity)
+        if self.rows is not None or not isinstance(similarity, Bm25Similarity):
+            return self._search_topk_sim(queries, k, similarity, slop, where)
+        docs = np.empty((len(queries), k), dtype=np.uint32)
+        scores = np.empty((len(queries), k), dtype=np.float32)
+        dev = self._device()
+        with self._shared["lock"]:
+            self._apply_rows(dev)
+            terms, c_starts, idfs = self._topk_queries(queries, lambda dfs: compute_idf(self.corpus_size, dfs))
+            starts = np.arange(len(queries) + 1, dtype=np.uint32)             # query q: clause q, mm 1
+            self._bool_where(dev, len(queries), starts, None, terms, c_starts, np.asarray(idfs, dtype=np.float32),
+                             None, None, None, None, np.ones(len(queries), dtype=np.uint32), len(queries), slop,
+                             similarity, k, docs, scores, ctypes.c_uint32(0), where)
+        return docs, scores
+
+    def _search_topk_mixed(self, queries, k, similarity, slop, where=None):
         """search_topk of a batch holding boolean queries: the plain ones through search_topk as before, the boolean
         ones through sa_score_batch_topk_bool (Or / And with weights 1) or sa_score_batch_topk_bool_occur (Bool,
-        boosted Or / And), each clause with the idf .score gives it; results in query order."""
+        boosted Or / And), each clause with the idf .score gives it; results in query order.  where: a packed mask
+        (pack_where), its rows split with the queries."""
         from .query import has_dismax, has_field, is_boolean, is_nested, needs_occur
         if any(has_field(q) for q in queries if is_boolean(q)):
             raise ValueError("a Field clause names a DataFrame column: run queries over columns with "
@@ -565,14 +644,17 @@ class SearchArray(ExtensionArray):
             part = [q for q, s in zip(queries, sel) if s]
             if not part:
                 continue
-            if kd == 0:
+            w = _where_part(where, sel)
+            if kd == 0 and where is not None:
+                docs[sel], scores[sel] = self._search_topk_plain_where(part, k, similarity, slop, w)
+            elif kd == 0:
                 docs[sel], scores[sel] = self.search_topk(part, k=k, similarity=similarity, slop=slop)
             elif kd == 3:
-                docs[sel], scores[sel], _ = self._search_topk_dismax(part, k, similarity, slop)
+                docs[sel], scores[sel], _ = self._search_topk_dismax(part, k, similarity, slop, w)
             elif kd == 4:
-                docs[sel], scores[sel], _ = self._search_topk_nested(part, k, similarity, slop)
+                docs[sel], scores[sel], _ = self._search_topk_nested(part, k, similarity, slop, w)
             else:
-                docs[sel], scores[sel], _ = self._search_topk_bool(part, k, similarity, slop)
+                docs[sel], scores[sel], _ = self._search_topk_bool(part, k, similarity, slop, w)
         return docs, scores
 
     def _check_dismax_params(self, similarity):
@@ -580,7 +662,20 @@ class SearchArray(ExtensionArray):
         from .query import check_dismax_members
         check_dismax_members([(0, "DisMax member")], lambda i: (similarity.k1, similarity.b, self.avg_doc_length, 0.0))
 
-    def _search_topk_dismax(self, queries, k, similarity, slop):
+    def _bool_where(self, dev, n_nodes, n_starts, c_node, terms, c_starts, idfs, weights, occurs, groups, ties, mm,
+                    n_queries, slop, similarity, k, docs, scores, n_redone, where):
+        """sa_score_batch_topk_bool_where: the boolean entry point the NULL arrays select, with a packed mask (None:
+        no mask, the unmasked instances)."""
+        p_w, stride = _where_args(where)
+        _lib.check(_lib.lib().sa_score_batch_topk_bool_where(
+            dev.handle, n_nodes, _lib.p_u32(n_starts), None if c_node is None else _lib.p_u32(c_node),
+            _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs), None if weights is None else _lib.p_f32(weights),
+            None if occurs is None else _lib.p_u8(occurs), None if groups is None else _lib.p_u32(groups),
+            None if ties is None else _lib.p_f32(ties), _lib.p_u32(mm), n_queries, int(slop), self.avg_doc_length,
+            similarity.k1, similarity.b, k, p_w, len(self), stride, _lib.p_u32(docs), _lib.p_f32(scores),
+            ctypes.byref(n_redone)))
+
+    def _search_topk_dismax(self, queries, k, similarity, slop, where=None):
         """Boolean queries holding a DisMax through sa_score_batch_topk_bool_dismax: (docs, scores, queries re-run
         exactly).  Every DisMax member needs sparse-safe BM25 parameters (ValueError before any device work)."""
         from .query import check_dismax_members, dismax_members, flatten_dismax
@@ -595,6 +690,10 @@ class SearchArray(ExtensionArray):
                              lambda i: (similarity.k1, similarity.b, self.avg_doc_length, idfs[i]))
         with self._shared["lock"]:
             self._apply_rows(dev)
+            if where is not None:
+                self._bool_where(dev, len(queries), q_starts, None, terms, c_starts, idfs, weights, occurs, groups,
+                                 ties, mm, len(queries), slop, similarity, k, docs, scores, n_redone, where)
+                return docs, scores, n_redone.value
             _lib.check(_lib.lib().sa_score_batch_topk_bool_dismax(
                 dev.handle, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
                 _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(groups), _lib.p_f32(ties), _lib.p_u32(mm),
@@ -602,7 +701,7 @@ class SearchArray(ExtensionArray):
                 _lib.p_f32(scores), ctypes.byref(n_redone)))
         return docs, scores, n_redone.value
 
-    def _search_topk_nested(self, queries, k, similarity, slop):
+    def _search_topk_nested(self, queries, k, similarity, slop, where=None):
         """Boolean queries holding nested queries through sa_score_batch_topk_bool_nested: (docs, scores, queries
         re-run exactly).  DisMax members anywhere in the trees need sparse-safe BM25 parameters (ValueError before any
         device work)."""
@@ -623,6 +722,10 @@ class SearchArray(ExtensionArray):
                              lambda i: (similarity.k1, similarity.b, self.avg_doc_length, idfs[i]))
         with self._shared["lock"]:
             self._apply_rows(dev)
+            if where is not None:
+                self._bool_where(dev, len(n_starts) - 1, n_starts, c_node, terms, c_starts, idfs, weights, occurs,
+                                 groups, ties, mm, len(queries), slop, similarity, k, docs, scores, n_redone, where)
+                return docs, scores, n_redone.value
             _lib.check(_lib.lib().sa_score_batch_topk_bool_nested(
                 dev.handle, len(n_starts) - 1, _lib.p_u32(n_starts), _lib.p_u32(c_node), _lib.p_u32(terms),
                 _lib.p_u32(c_starts), _lib.p_f32(idfs), _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(groups),
@@ -630,9 +733,10 @@ class SearchArray(ExtensionArray):
                 similarity.b, k, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
         return docs, scores, n_redone.value
 
-    def _search_topk_bool(self, queries, k, similarity, slop):
+    def _search_topk_bool(self, queries, k, similarity, slop, where=None):
         """Boolean queries through sa_score_batch_topk_bool, or through sa_score_batch_topk_bool_occur when one of
-        them is a Bool or has a weight other than 1: (docs, scores, queries re-run exactly)."""
+        them is a Bool or has a weight other than 1: (docs, scores, queries re-run exactly).  where: a packed mask
+        (pack_where), through sa_score_batch_topk_bool_where."""
         from .query import flatten, flatten_occur, needs_occur
         occur = any(needs_occur(q) for q in queries)
         if occur:
@@ -647,7 +751,11 @@ class SearchArray(ExtensionArray):
         idfs = np.asarray(idfs, dtype=np.float32)
         with self._shared["lock"]:
             self._apply_rows(dev)
-            if occur:
+            if where is not None:
+                self._bool_where(dev, len(queries), q_starts, None, terms, c_starts, idfs, weights if occur else None,
+                                 occurs if occur else None, None, None, mm, len(queries), slop, similarity, k, docs,
+                                 scores, n_redone, where)
+            elif occur:
                 _lib.check(_lib.lib().sa_score_batch_topk_bool_occur(
                     dev.handle, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
                     _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(mm), len(queries), int(slop),
@@ -684,10 +792,11 @@ class SearchArray(ExtensionArray):
             idfs.append(idf(np.asarray([df.get(t, 0) for t in ts])))
         return np.asarray(terms, dtype=np.uint32), np.asarray(starts, dtype=np.uint32), idfs
 
-    def _search_topk_sim(self, queries, k, similarity, slop):
+    def _search_topk_sim(self, queries, k, similarity, slop, where=None):
         """search_topk on a view, and under bm25_impact, bm25_legacy_similarity or classic_similarity on any array
         (sa_score_batch_topk_sim): the counts, document frequencies, doc lengths, avgdl and corpus size .score
-        uses, with the idf computed here, on the host, from the same dfs."""
+        uses, with the idf computed here, on the host, from the same dfs.  where: a packed mask over the positions
+        (pack_where), through sa_score_batch_topk_sim_where."""
         if self.rows is not None and (self.comm is not None or self.global_df is not None):
             raise ValueError("search_topk on a view of a sharded SearchArray is not supported: the slice's document "
                              "frequencies would need a sum over the ranks; use .score() on the view")
@@ -707,8 +816,16 @@ class SearchArray(ExtensionArray):
             docs = np.full((len(idfs), k), _lib.NO_DOC, dtype=np.uint32)
             scores = np.zeros((len(idfs), k), dtype=np.float64)
             dbl = ctypes.POINTER(ctypes.c_double)
-            _lib.check(_lib.lib().sa_score_batch_topk_sim(
-                dev.handle, similarity.kind, _lib.p_u32(terms), _lib.p_u32(starts), idfs.ctypes.data_as(dbl),
-                len(idfs), int(slop), None if dl is None else _lib.p_f32(dl), float(self.avg_doc_length),
-                float(similarity.k1), float(similarity.b), k, _lib.p_u32(docs), scores.ctypes.data_as(dbl)))
+            if where is not None:
+                p_w, stride = _where_args(where)
+                _lib.check(_lib.lib().sa_score_batch_topk_sim_where(
+                    dev.handle, similarity.kind, _lib.p_u32(terms), _lib.p_u32(starts), idfs.ctypes.data_as(dbl),
+                    len(idfs), int(slop), None if dl is None else _lib.p_f32(dl), float(self.avg_doc_length),
+                    float(similarity.k1), float(similarity.b), k, p_w, len(self), stride, _lib.p_u32(docs),
+                    scores.ctypes.data_as(dbl)))
+            else:
+                _lib.check(_lib.lib().sa_score_batch_topk_sim(
+                    dev.handle, similarity.kind, _lib.p_u32(terms), _lib.p_u32(starts), idfs.ctypes.data_as(dbl),
+                    len(idfs), int(slop), None if dl is None else _lib.p_f32(dl), float(self.avg_doc_length),
+                    float(similarity.k1), float(similarity.b), k, _lib.p_u32(docs), scores.ctypes.data_as(dbl)))
         return docs, scores.astype(similarity.out_dtype, copy=False)

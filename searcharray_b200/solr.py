@@ -19,7 +19,7 @@ import numpy as np
 import pandas as pd
 
 from . import _lib
-from .postings import SearchArray
+from .postings import SearchArray, _where_args, pack_where
 from .similarity import Bm25Similarity, Similarity, compute_idf, default_bm25
 
 
@@ -486,48 +486,60 @@ def _fields_clauses(clauses, slot_of, arrays):
     return terms, c_starts, c_idf, _u32([0 if c is None else slot_of[c.field] for c in clauses])
 
 
-def _fields_call(multi, arrays, sims, flat, prepared, k, slop):
+def _fields_call(multi, arrays, sims, flat, prepared, k, slop, where=None):
     """sa_multi_score_batch_topk_bool, sa_multi_score_batch_topk_bool_dismax for flatten_dismax's arrays, or
     sa_multi_score_batch_topk_bool_nested for flatten_nested's, on prepared arrays (the fields locked): (docs, scores,
-    queries re-run)."""
+    queries re-run).  where: a packed mask (postings.pack_where), through sa_multi_score_batch_topk_bool_where."""
+    from .query import SA_NO_NODE
     terms, c_starts, c_idf, c_field = prepared
     n_redone = ctypes.c_uint32(0)
     avgdl = _f32([a.avg_doc_length for a in arrays])
     k1, b = _f32([s.k1 for s in sims]), _f32([s.b for s in sims])
+    c_node = groups = ties = None
     if len(flat) == 8:
-        from .query import SA_NO_NODE
         n_starts, c_node, mm, weights, occurs, groups, ties = flat[1:]
         nq = len(n_starts) - 1 - int(np.count_nonzero(c_node != SA_NO_NODE))   # each nested node: one reference
-        docs = np.empty((nq, k), dtype=np.uint32)
-        scores = np.empty((nq, k), dtype=np.float32)
+    else:
+        n_starts, mm, weights, occurs = flat[1:5]
+        if len(flat) == 7:
+            groups, ties = flat[5:]
+        nq = len(n_starts) - 1
+    docs = np.empty((nq, k), dtype=np.uint32)
+    scores = np.empty((nq, k), dtype=np.float32)
+    if where is not None:
+        p_w, stride = _where_args(where)
+        _lib.check(_lib.lib().sa_multi_score_batch_topk_bool_where(
+            multi.handle, len(n_starts) - 1, _lib.p_u32(n_starts), None if c_node is None else _lib.p_u32(c_node),
+            _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(c_idf), _lib.p_f32(weights),
+            _lib.p_u8(occurs), None if groups is None else _lib.p_u32(groups), None if ties is None else _lib.p_f32(ties),
+            _lib.p_u32(mm), nq, int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1), _lib.p_f32(b), k, p_w,
+            len(arrays[0]), stride, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
+    elif c_node is not None:
         _lib.check(_lib.lib().sa_multi_score_batch_topk_bool_nested(
             multi.handle, len(n_starts) - 1, _lib.p_u32(n_starts), _lib.p_u32(c_node), _lib.p_u32(c_field),
             _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(c_idf), _lib.p_f32(weights), _lib.p_u8(occurs),
             _lib.p_u32(groups), _lib.p_f32(ties), _lib.p_u32(mm), nq, int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1),
             _lib.p_f32(b), k, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
-        return docs, scores, n_redone.value
-    q_starts, mm, weights, occurs = flat[1:5]
-    nq = len(q_starts) - 1
-    docs = np.empty((nq, k), dtype=np.uint32)
-    scores = np.empty((nq, k), dtype=np.float32)
-    if len(flat) == 7:
-        groups, ties = flat[5:]
+    elif groups is not None:
         _lib.check(_lib.lib().sa_multi_score_batch_topk_bool_dismax(
-            multi.handle, _lib.p_u32(q_starts), _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts),
+            multi.handle, _lib.p_u32(n_starts), _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts),
             _lib.p_f32(c_idf), _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(groups), _lib.p_f32(ties),
             _lib.p_u32(mm), nq, int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1), _lib.p_f32(b), k, _lib.p_u32(docs),
             _lib.p_f32(scores), ctypes.byref(n_redone)))
-        return docs, scores, n_redone.value
-    _lib.check(_lib.lib().sa_multi_score_batch_topk_bool(
-        multi.handle, _lib.p_u32(q_starts), _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts),
-        _lib.p_f32(c_idf), _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(mm), nq, int(slop), _lib.p_f32(avgdl),
-        _lib.p_f32(k1), _lib.p_f32(b), k, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
+    else:
+        _lib.check(_lib.lib().sa_multi_score_batch_topk_bool(
+            multi.handle, _lib.p_u32(n_starts), _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts),
+            _lib.p_f32(c_idf), _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(mm), nq, int(slop),
+            _lib.p_f32(avgdl), _lib.p_f32(k1), _lib.p_f32(b), k, _lib.p_u32(docs), _lib.p_f32(scores),
+            ctypes.byref(n_redone)))
     return docs, scores, n_redone.value
 
 
-def _fields_topk(frame, queries, k, similarity, slop):
+def _fields_topk(frame, queries, k, similarity, slop, where=None):
     """fields_topk and the number of queries re-run exactly (candidate overflow)."""
     queries = list(queries)
+    if where is not None:
+        where = pack_where(where, len(frame), len(queries))
     flat, slot_of, arrays, sims = _fields_plan(frame, queries, similarity)
     multi = _multi_for(arrays)
     with _locked(multi, arrays):
@@ -540,11 +552,11 @@ def _fields_topk(frame, queries, k, similarity, slop):
             check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
                                  lambda i: (sims[slot_of[clauses[i].field]].k1, sims[slot_of[clauses[i].field]].b,
                                             arrays[slot_of[clauses[i].field]].avg_doc_length, prepared[2][i]))
-        return _fields_call(multi, arrays, sims, flat, prepared, k, slop)
+        return _fields_call(multi, arrays, sims, flat, prepared, k, slop, where)
 
 
 def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
-                similarity: Union[Similarity, Dict[str, Similarity]] = default_bm25, slop: int = 0):
+                similarity: Union[Similarity, Dict[str, Similarity]] = default_bm25, slop: int = 0, where=None):
     """Batched Or / And / Bool queries whose clauses are on several columns of `frame` -- Lucene's
     `+title:star overview:war -overview:trek`, or Elasticsearch's most_fields `title:alien^2 overview:alien` -- ranked
     on the device in one batch.  Every clause is a query.Field(field, term or phrase), or a Boost of one; phrases match
@@ -566,6 +578,12 @@ def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
 
     An Or / And / Bool may be a clause of another, at any depth, as in SearchArray.search_topk: edismax's qf + pf as
     Bool(must=[Or([DisMax(...), DisMax(...)], mm="75%")], should=[Boost(Field("title", ["a", "b"]), 3)])
-    (sa_multi_score_batch_topk_bool_nested)."""
-    docs, scores, _ = _fields_topk(frame, queries, k, similarity, slop)
+    (sa_multi_score_batch_topk_bool_nested).
+
+    where: a document filter, as in SearchArray.search_topk -- a boolean array-like (a boolean pd.Series too) of
+    shape (len(frame),), one mask for the batch, or (len(queries), len(frame)), one per query.  Per query the
+    result is the top k of np.where(mask_q, S_q, 0), S_q the composition above; the mask never changes a score
+    (each column's idf, avgdl and doc lengths stay those of the whole column).  A dtype other than bool raises
+    TypeError and another shape ValueError, before any device work (sa_multi_score_batch_topk_bool_where)."""
+    docs, scores, _ = _fields_topk(frame, queries, k, similarity, slop, where)
     return docs, scores
