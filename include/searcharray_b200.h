@@ -145,106 +145,85 @@ int sa_score_batch_topk(sa_index *index, const uint32_t *terms, const uint32_t *
  * avg_doc_len == 0 -> nothing ranks, except under SA_SIM_CLASSIC.  out_scores are float64 (the float32 BM25 and
  * impact scores widened).  Only scores > 0 rank (+inf does, NaN never); order score desc, then id asc
  * (np.argpartition as above); empty slots SA_NO_DOC / 0.  Ids: positions in the view, or GLOBAL doc ids (doc_base
- * added) on an unsliced array; fewer than 2^32 - 1 of them. */
+ * added) on an unsliced array; fewer than 2^32 - 1 of them.  where_bits / where_n / where_stride: a document mask
+ * over the positions it ranks (a view's, or the array's docs), as below; where_bits NULL: no mask. */
 int sa_score_batch_topk_sim(sa_index *index, int kind, const uint32_t *terms, const uint32_t *term_starts,
                             const double *idf, uint32_t n_queries, uint32_t slop, const float *view_doc_lens,
-                            double avg_doc_len, double k1, double b, uint32_t k, uint32_t *out_ids,
-                            double *out_scores);
-/* A document mask for the batched top-k (the `_where` entry points below): the result is the top k of
- * where(mask_q, S_q, 0), S_q being the scores the call without a mask ranks for query q, under the same selection rule.
- * The mask never changes a score -- idf, document frequencies, avgdl and doc lengths stay the unmasked call's -- it
- * only removes docs from the ranking.  where_bits: u32 words, one row of SA_WHERE_WORDS(where_n) words covering
- * where_n docs (the index's docs, or a view's positions under sa_score_batch_topk_sim_where), for the whole batch
- * (where_stride == 0) or one row per query (where_stride == that row length; row q is query q's).  Within a row the
- * bits are in the tile kernels' owner order, not doc order: word t * 256 + i holds, at bit 4 j + e, doc
+                            double avg_doc_len, double k1, double b, uint32_t k, const uint32_t *where_bits,
+                            uint64_t where_n, uint64_t where_stride, uint32_t *out_ids, double *out_scores);
+/* A document mask for the batched top-k (sa_score_batch_topk_sim and the boolean entry points below): the result is
+ * the top k of where(mask_q, S_q, 0), S_q being the scores the call without a mask ranks for query q, under the same
+ * selection rule.  The mask never changes a score -- idf, document frequencies, avgdl and doc lengths stay the
+ * unmasked call's -- it only removes docs from the ranking.  where_bits: u32 words, one row of SA_WHERE_WORDS(where_n)
+ * words covering where_n docs (the index's docs, or a view's positions under sa_score_batch_topk_sim), for the whole
+ * batch (where_stride == 0) or one row per query (where_stride == that row length; row q is query q's).  Within a row
+ * the bits are in the tile kernels' owner order, not doc order: word t * 256 + i holds, at bit 4 j + e, doc
  * t * 8192 + 4 (i + 256 j) + e (t: the 8,192-doc tile, i: the owning thread, j < 8, e < 4); bits past where_n are 0.
  * where_n must equal the doc (position) count the call ranks; anything else is SA_ERR_ARG before any device work.
- * where_bits NULL: no mask. */
+ * where_bits NULL: no mask (where_n and where_stride are then ignored). */
 #define SA_WHERE_WORDS(n) ((((uint64_t)(n) + 8191u) / 8192u) * 256u)
-/* sa_score_batch_topk_sim with a document mask over the positions it ranks (a view's, or the array's docs). */
-int sa_score_batch_topk_sim_where(sa_index *index, int kind, const uint32_t *terms, const uint32_t *term_starts,
-                                  const double *idf, uint32_t n_queries, uint32_t slop, const float *view_doc_lens,
-                                  double avg_doc_len, double k1, double b, uint32_t k, const uint32_t *where_bits,
-                                  uint64_t where_n, uint64_t where_stride, uint32_t *out_ids, double *out_scores);
-/* Batched boolean queries: OR / AND / min-should-match over term and phrase clauses (the reference's composition in
- * test/test_search.py:126-226).  Query q = clauses [query_clause_starts[q], query_clause_starts[q+1]) (1 to
- * SA_BOOL_MAX_CLAUSES of them; query_clause_starts[0] == 0); clause c = clause_terms[clause_term_starts[c] ..
- * clause_term_starts[c+1]) (1 term, or a phrase with `slop`), scored exactly as sa_score_term / sa_score_phrase with
- * idf clause_idf[c].  Per query, s = score(c0) + score(c1) + ... folded left in float32; a doc ranks iff s > 0 and at
- * least mm[q] (<= its clauses) clauses score > 0 there.  Result: the top k by (score desc, doc id asc; as
- * np.argpartition, searcharray/utils/sort.py:24), GLOBAL doc ids (doc_base added), empty slots SA_NO_DOC / 0.
- * Phrase clauses need ordinary BM25 parameters (k1 > 0, 0 <= b < 1).  *n_redone (nullable): queries re-run exactly
- * because a tile had more candidates than slots. */
-#define SA_BOOL_MAX_CLAUSES 64
-int sa_score_batch_topk_bool(sa_index *index, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
-                             const uint32_t *clause_term_starts, const float *clause_idf, const uint32_t *mm,
-                             uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
-                             uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
-/* Boolean queries with clause roles and per-clause weights (Lucene's MUST / SHOULD / FILTER / MUST_NOT): the
- * arguments of sa_score_batch_topk_bool plus, per clause, clause_weight[c] (finite, >= 0) and clause_occur[c] (one of
- * SA_OCCUR_*).  Per query, over its MUST and SHOULD clauses in clause order, s = w0 * score(c0), then
- * s = s + w1 * score(c1), ..., every product and sum rounded to float32 (no fused multiply-add).  A doc ranks iff
- * s > 0, at least mm[q] (<= its SHOULD clauses) SHOULD clauses score > 0 there (unweighted: a weight of 0 still
- * matches), every MUST and FILTER clause scores > 0 there, and no MUST_NOT clause does.  FILTER and MUST_NOT clauses
- * add nothing to s.  Every clause, whatever its role, is scored exactly as in sa_score_batch_topk_bool, with its own
- * idf.  With every clause SHOULD and weight 1 the result equals sa_score_batch_topk_bool's, bit for bit. */
-#define SA_OCCUR_SHOULD 0
-#define SA_OCCUR_MUST 1
-#define SA_OCCUR_FILTER 2
-#define SA_OCCUR_MUST_NOT 3
-int sa_score_batch_topk_bool_occur(sa_index *index, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
-                                   const uint32_t *clause_term_starts, const float *clause_idf,
-                                   const float *clause_weight, const uint8_t *clause_occur, const uint32_t *mm,
-                                   uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
-                                   uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
-/* Boolean queries with disjunction-max clauses (Lucene's DisjunctionMaxQuery, edismax's per-term qf): the arguments of
- * sa_score_batch_topk_bool_occur plus, per clause, clause_group[c], the batch-wide index of the first clause of c's
- * group (c itself for a plain clause), and clause_tie[c], read at a group's first clause (finite, in [0, 1]; checked
+/* Batched boolean queries, one entry point for every form; the nullable per-clause arrays select it.  Each layer below
+ * adds to the one before, and a batch that does not use a layer's arrays scores as the layer before, bit for bit.
+ *
+ * Or / And (clause_weight, clause_occur, clause_group, clause_tie and clause_node NULL; n_nodes == n_queries): OR /
+ * AND / min-should-match over term and phrase clauses (the reference's composition in test/test_search.py:126-226).
+ * Query q = clauses [node_clause_starts[q], node_clause_starts[q+1]) (1 to SA_BOOL_MAX_CLAUSES of them;
+ * node_clause_starts[0] == 0); clause c = clause_terms[clause_term_starts[c] .. clause_term_starts[c+1]) (1 term, or a
+ * phrase with `slop`), scored exactly as sa_score_term / sa_score_phrase with idf clause_idf[c].  Per query,
+ * s = score(c0) + score(c1) + ... folded left in float32; a doc ranks iff s > 0 and at least mm[q] (<= its clauses)
+ * clauses score > 0 there.  Result: the top k by (score desc, doc id asc; as np.argpartition,
+ * searcharray/utils/sort.py:24), GLOBAL doc ids (doc_base added), empty slots SA_NO_DOC / 0.  Phrase clauses need
+ * ordinary BM25 parameters (k1 > 0, 0 <= b < 1).  *n_redone (nullable): queries re-run exactly because a tile had more
+ * candidates than slots.
+ *
+ * Roles and weights (clause_weight and clause_occur given, both or neither): Lucene's MUST / SHOULD / FILTER /
+ * MUST_NOT, per clause clause_weight[c] (finite, >= 0) and clause_occur[c] (one of SA_OCCUR_*).  Per query, over its
+ * MUST and SHOULD clauses in clause order, s = w0 * score(c0), then s = s + w1 * score(c1), ..., every product and sum
+ * rounded to float32 (no fused multiply-add).  A doc ranks iff s > 0, at least mm[q] (<= its SHOULD clauses) SHOULD
+ * clauses score > 0 there (unweighted: a weight of 0 still matches), every MUST and FILTER clause scores > 0 there,
+ * and no MUST_NOT clause does.  FILTER and MUST_NOT clauses add nothing to s.  Every clause, whatever its role, is
+ * scored as above, with its own idf.  With every clause SHOULD and weight 1 the result equals Or / And's, bit for bit.
+ *
+ * Disjunction-max groups (clause_group and clause_tie given, both or neither, and only with clause_occur): Lucene's
+ * DisjunctionMaxQuery, edismax's per-term qf.  clause_group[c] is the batch-wide index of the first clause of c's
+ * group (c itself for a plain clause), and clause_tie[c] is read at a group's first clause (finite, in [0, 1]; checked
  * at every group's first clause).  A group is a run of consecutive clauses of one query with one occur, and is one
  * clause of its query: with v_j = w_j * score(c_j) over its members, m = max_j v_j, t = v_0 + v_1 + ... (left fold),
  * it contributes d = m + (t - m) * tie (every step rounded to float32, no fused multiply-add) with weight 1 to s under
  * its occur, and it matches a doc where any member scores > 0 (unweighted).  mm[q] counts SHOULD groups (<= their
  * number).  Members of a group of two or more clauses need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite
- * idf >= 0), so that every v >= +0; a group of one is a plain clause.  Queries without a group of two or more score
- * as in sa_score_batch_topk_bool_occur, bit for bit. */
-int sa_score_batch_topk_bool_dismax(sa_index *index, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
-                                    const uint32_t *clause_term_starts, const float *clause_idf,
-                                    const float *clause_weight, const uint8_t *clause_occur,
-                                    const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
-                                    uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
-                                    uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
-/* Nested boolean queries: an Or / And / Bool used as a clause of another.  Nodes 0 .. n_queries-1 are the queries
- * whose top k is returned; nodes n_queries .. n_nodes-1 are nested queries.  Node n owns clauses
- * [node_clause_starts[n], node_clause_starts[n+1]) (node_clause_starts[0] == 0), with the per-clause arrays, DisMax
- * groups and mm[n] of sa_score_batch_topk_bool_dismax, checked per node.  clause_node[c] == SA_NO_NODE: a leaf, its terms
- * clause_terms[clause_term_starts[c] ..).  Otherwise c is nested node clause_node[c]: it has no terms, the node's index
- * is above that of the node holding c, no other clause references it, and c is not a DisMax member; every nested node
- * is referenced.  A nested node N scores r_N(d) = the score N ranks doc d with as a query of its own (s_N(d) where
- * all its conditions hold and s_N(d) > 0, +0 elsewhere), and matches where r_N(d) > 0: it adds w * r_N under MUST /
- * SHOULD (rounded, then added), counts once towards its holder's mm, and under FILTER / MUST_NOT plays a leaf's role.
- * Queries without a nested clause score as in sa_score_batch_topk_bool_dismax, bit for bit. */
+ * idf >= 0), so that every v >= +0; a group of one is a plain clause.
+ *
+ * Nested queries (clause_node given, only with the group arrays): an Or / And / Bool used as a clause of another.
+ * Nodes 0 .. n_queries-1 are the queries whose top k is returned; nodes n_queries .. n_nodes-1 are nested queries.
+ * Node n owns clauses [node_clause_starts[n], node_clause_starts[n+1]), with the per-clause arrays, groups and mm[n]
+ * above, checked per node.  clause_node[c] == SA_NO_NODE: a leaf, its terms clause_terms[clause_term_starts[c] ..).
+ * Otherwise c is nested node clause_node[c]: it has no terms, the node's index is above that of the node holding c,
+ * no other clause references it, and c is not a DisMax member; every nested node is referenced.  A nested node N
+ * scores r_N(d) = the score N ranks doc d with as a query of its own (s_N(d) where all its conditions hold and
+ * s_N(d) > 0, +0 elsewhere), and matches where r_N(d) > 0: it adds w * r_N under MUST / SHOULD (rounded, then added),
+ * counts once towards its holder's mm, and under FILTER / MUST_NOT plays a leaf's role.  Without clause_node,
+ * n_nodes == n_queries.
+ *
+ * Document mask (where_bits, where_n, where_stride; SA_WHERE_WORDS): over the index's n_docs docs.  Per query the
+ * result is the top k of the unmasked call's scores where the query's mask is set; every score equals the unmasked
+ * one bit for bit.
+ *
+ * Arrays given in a pairing other than those above (weights without occurs, groups without ties or without occurs,
+ * clause_node without groups, n_nodes != n_queries without clause_node) are SA_ERR_ARG before any device work. */
+#define SA_BOOL_MAX_CLAUSES 64
+#define SA_OCCUR_SHOULD 0
+#define SA_OCCUR_MUST 1
+#define SA_OCCUR_FILTER 2
+#define SA_OCCUR_MUST_NOT 3
 #define SA_NO_NODE 0xFFFFFFFFu
-int sa_score_batch_topk_bool_nested(sa_index *index, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                    const uint32_t *clause_node, const uint32_t *clause_terms,
-                                    const uint32_t *clause_term_starts, const float *clause_idf,
-                                    const float *clause_weight, const uint8_t *clause_occur,
-                                    const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
-                                    uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
-                                    uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
-/* Every boolean entry point above with a document mask (SA_WHERE_WORDS): the arguments of
- * sa_score_batch_topk_bool_nested, whose nullable arrays pick the form -- clause_weight / clause_occur NULL: Or / And
- * (sa_score_batch_topk_bool); clause_group / clause_tie NULL: no DisMax groups (sa_score_batch_topk_bool_occur);
- * clause_node NULL: no nested nodes, n_nodes == n_queries (sa_score_batch_topk_bool_dismax) -- plus the mask over the
- * index's n_docs docs.  Per query the result is the top k of the unmasked call's scores where the query's mask is
- * set; every score equals the unmasked one bit for bit. */
-int sa_score_batch_topk_bool_where(sa_index *index, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                   const uint32_t *clause_node, const uint32_t *clause_terms,
-                                   const uint32_t *clause_term_starts, const float *clause_idf,
-                                   const float *clause_weight, const uint8_t *clause_occur,
-                                   const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
-                                   uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
-                                   const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
-                                   uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
+int sa_score_batch_topk_bool(sa_index *index, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                             const uint32_t *clause_node, const uint32_t *clause_terms,
+                             const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
+                             const uint8_t *clause_occur, const uint32_t *clause_group, const float *clause_tie,
+                             const uint32_t *mm, uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1,
+                             float b, uint32_t k, const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
+                             uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
 
 /* The same batch in three stages, so a serving loop (or the benchmark) can keep the query
  * descriptors resident and time the device work alone: upload (H2D of descriptors), execute
@@ -344,54 +323,24 @@ int sa_multi_download(sa_multi *multi, void *out, int as_float32);
 int sa_multi_is_float32(sa_multi *multi, int *out);
 int sa_multi_topk(sa_multi *multi, uint32_t k, uint32_t *out_docs, double *out_scores);
 /* Boolean queries over several fields of one document set (Elasticsearch's `+title:star overview:war`): the arguments
- * of sa_score_batch_topk_bool_occur, with clause c on field clause_field[c] (< the multi's fields) and its term ids
- * that field's.  Field f of the multi is scored with avg_doc_len[f], k1[f] and b[f]; each clause's idf is the
- * caller's, from its own field.  Per query the result is sa_score_batch_topk_bool_occur's composition with
+ * and layers of sa_score_batch_topk_bool, with clause c on field clause_field[c] (< the multi's fields; read for leaves
+ * only) and its term ids that field's.  clause_weight and clause_occur are required (Or / And take every clause
+ * SHOULD with weight 1); clause_group / clause_tie and clause_node are optional as there, and the mask is over the
+ * fields' n_docs docs.  Field f of the multi is scored with avg_doc_len[f], k1[f] and b[f]; each clause's idf is the
+ * caller's, from its own field.  Per query the result is sa_score_batch_topk_bool's composition with
  * score(c) = .score of the clause on its field; a field whose avg_doc_len is 0 scores 0 at every doc (a MUST / FILTER
- * clause on it ranks nothing, a MUST_NOT clause on it vetoes nothing).  Or / And take it with every clause SHOULD and
- * weight 1.  Fields that share one sa_index must share (avg_doc_len, k1, b): the index caches one norm table.  Result
- * ids are global doc ids (doc_base added). */
-int sa_multi_score_batch_topk_bool(sa_multi *multi, const uint32_t *query_clause_starts, const uint32_t *clause_field,
+ * clause on it ranks nothing, a MUST_NOT clause on it vetoes nothing).  A DisMax group's members may sit on different
+ * fields, each scored on its own: Elasticsearch's best_fields, and per-term groups inside an Or with mm for edismax's
+ * term-centric qf.  Fields that share one sa_index must share (avg_doc_len, k1, b): the index caches one norm table.
+ * Result ids are global doc ids (doc_base added). */
+int sa_multi_score_batch_topk_bool(sa_multi *multi, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                   const uint32_t *clause_node, const uint32_t *clause_field,
                                    const uint32_t *clause_terms, const uint32_t *clause_term_starts,
                                    const float *clause_idf, const float *clause_weight, const uint8_t *clause_occur,
-                                   const uint32_t *mm, uint32_t n_queries, uint32_t slop, const float *avg_doc_len,
-                                   const float *k1, const float *b, uint32_t k, uint32_t *out_docs, float *out_scores,
-                                   uint32_t *n_redone);
-/* sa_multi_score_batch_topk_bool with the DisMax groups of sa_score_batch_topk_bool_dismax (clause_group, clause_tie):
- * Elasticsearch's best_fields, and per-term groups inside an Or with mm for edismax's term-centric qf.  A group's
- * members may sit on different fields; each is scored on its own. */
-int sa_multi_score_batch_topk_bool_dismax(sa_multi *multi, const uint32_t *query_clause_starts,
-                                          const uint32_t *clause_field, const uint32_t *clause_terms,
-                                          const uint32_t *clause_term_starts, const float *clause_idf,
-                                          const float *clause_weight, const uint8_t *clause_occur,
-                                          const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
-                                          uint32_t n_queries, uint32_t slop, const float *avg_doc_len, const float *k1,
-                                          const float *b, uint32_t k, uint32_t *out_docs, float *out_scores,
-                                          uint32_t *n_redone);
-/* sa_multi_score_batch_topk_bool_dismax with the nested nodes of sa_score_batch_topk_bool_nested: clause_field[c] is
- * read for leaves only. */
-int sa_multi_score_batch_topk_bool_nested(sa_multi *multi, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                          const uint32_t *clause_node, const uint32_t *clause_field,
-                                          const uint32_t *clause_terms, const uint32_t *clause_term_starts,
-                                          const float *clause_idf, const float *clause_weight,
-                                          const uint8_t *clause_occur, const uint32_t *clause_group,
-                                          const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
-                                          uint32_t slop, const float *avg_doc_len, const float *k1, const float *b,
-                                          uint32_t k, uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
-/* The multi-field entry points above with a document mask, as sa_score_batch_topk_bool_where: the arguments of
- * sa_multi_score_batch_topk_bool_nested (clause_weight and clause_occur required; clause_group / clause_tie NULL: no
- * DisMax groups; clause_node NULL: no nested nodes, n_nodes == n_queries) plus the mask over the fields' n_docs
- * docs. */
-int sa_multi_score_batch_topk_bool_where(sa_multi *multi, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                         const uint32_t *clause_node, const uint32_t *clause_field,
-                                         const uint32_t *clause_terms, const uint32_t *clause_term_starts,
-                                         const float *clause_idf, const float *clause_weight,
-                                         const uint8_t *clause_occur, const uint32_t *clause_group,
-                                         const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
-                                         uint32_t slop, const float *avg_doc_len, const float *k1, const float *b,
-                                         uint32_t k, const uint32_t *where_bits, uint64_t where_n,
-                                         uint64_t where_stride, uint32_t *out_docs, float *out_scores,
-                                         uint32_t *n_redone);
+                                   const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
+                                   uint32_t n_queries, uint32_t slop, const float *avg_doc_len, const float *k1,
+                                   const float *b, uint32_t k, const uint32_t *where_bits, uint64_t where_n,
+                                   uint64_t where_stride, uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
 
 /* ------------------------------------------------- per-op exports (parity tests)
  * Device implementations of the reference's native ops on raw arrays (host in, host out),

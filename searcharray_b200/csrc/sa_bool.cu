@@ -18,35 +18,35 @@
 // Then the docs below mm are zeroed and the tile goes through flush_tile_collect, the float32 collector of every
 // other path, and topk_select_kernel ranks the candidates.
 //
-// bool_tile_kernel<true> (sa_score_batch_topk_bool_occur) adds Lucene's clause roles and per-clause weights, from a
-// separate BoolOccur array: MUST / SHOULD clauses add weight * score, only SHOULD clauses count towards mm, and two
-// per-thread masks over the thread's 32 docs record where a MUST / FILTER clause misses (`req`) and where a MUST_NOT
-// clause matches (`veto`).  A tile where a MUST / FILTER clause has no doc, or with fewer SHOULD clauses than mm, is
-// published empty before the fold.
+// One entry point per handle (sa_score_batch_topk_bool, sa_multi_score_batch_topk_bool) runs every form; the arrays
+// it is given select the form, and the form and the mask select one instance of bool_tile_kernel (bool_kernel).  The
+// flags add, in order:
 //
-// bool_fields_tile_kernel (sa_multi_score_batch_topk_bool) is the same fold with clauses on several fields of one
-// document set: a clause carries its field's slot, and every step reads that field's lists, norms, doc lengths and
-// BM25 parameters from a small per-call table (BoolField) instead of the index in BoolArgs.
+// OCCUR: Lucene's clause roles and per-clause weights, from a separate BoolOccur array: MUST / SHOULD clauses add
+// weight * score, only SHOULD clauses count towards mm, and two per-thread masks over the thread's 32 docs record
+// where a MUST / FILTER clause misses (`req`) and where a MUST_NOT clause matches (`veto`).  A tile where a MUST /
+// FILTER clause has no doc, or with fewer SHOULD clauses than mm, is published empty before the fold.
 //
-// bool_dismax_tile_kernel (sa_score_batch_topk_bool_dismax, sa_multi_score_batch_topk_bool_dismax; the single-index
-// entry passes a one-entry field table) adds disjunction-max groups: a run of consecutive clauses that is one clause
-// of its query.  A member's v = weight * score goes into the group's running max m and left-folded sum t, kept per
-// owned doc in per-thread strips of dynamic shared memory, and a u32 mask records where any member scores > 0; at the
-// group's last member d = m + (t - m) * tie is folded with weight 1 under the group's role, its hit being the mask.
-// A group is present in a tile iff any member is.
+// FIELDS (every multi-field call): clauses on several fields of one document set: a clause carries its field's slot,
+// and every step reads that field's lists, norms, doc lengths and BM25 parameters from a small per-call table
+// (BoolField) instead of the index in BoolArgs.
 //
-// bool_nested_tile_kernel (sa_score_batch_topk_bool_nested, sa_multi_score_batch_topk_bool_nested) is the DisMax fold
-// with nested queries: an Or / And / Bool used as a clause of another.  Each nested node is materialised first, deepest
-// level first, by the same fold in a store pass: its ranked values (0 where it does not rank) go to its row in
+// DISMAX (a single-index call passes a one-entry field table): disjunction-max groups, a run of consecutive clauses
+// that is one clause of its query.  A member's v = weight * score goes into the group's running max m and left-folded
+// sum t, kept per owned doc in per-thread strips of dynamic shared memory, and a u32 mask records where any member
+// scores > 0; at the group's last member d = m + (t - m) * tie is folded with weight 1 under the group's role, its hit
+// being the mask.  A group is present in a tile iff any member is.
+//
+// NESTED: nested queries, an Or / And / Bool used as a clause of another.  Each nested node is materialised first,
+// deepest level first, by the same fold in a store pass: its ranked values (0 where it does not rank) go to its row in
 // BoolState::rows and a per-(row, tile) flag records whether anything ranked, a tile that ranks nothing writing only
 // its flag.  A parent reads a nested clause's row as the clause's score (no BM25), present in a tile iff the child's
 // flag is set; the top-level nodes are collected and selected as in every other instance.
 //
-// bool_where_tile_kernel (sa_score_batch_topk_bool_where, sa_multi_score_batch_topk_bool_where) is each of the five
-// instances with a document mask (WhereMask, sa_term.cuh): a tile without an allowed doc is published empty before
-// any of its lists is read, and a disallowed doc is zeroed with the docs below mm, before the tile's bound is taken,
-// so the mask never changes a score, only which docs rank.  In a nested call only the top-level launch is masked:
-// a disallowed doc never ranks whatever its nested rows hold.
+// WHERE: a document mask (WhereMask, sa_term.cuh) on any of the five forms: a tile without an allowed doc is published
+// empty before any of its lists is read, and a disallowed doc is zeroed with the docs below mm, before the tile's
+// bound is taken, so the mask never changes a score, only which docs rank.  In a nested call only the top-level launch
+// is masked: a disallowed doc never ranks whatever its nested rows hold.
 #include "sa_multi.cuh"
 #include "sa_term.cuh"
 #include "sa_phrase.cuh"
@@ -58,7 +58,7 @@ struct BoolClause {
     float idf;
     u32 row;        // a phrase clause's count row in BoolState::rows (within its group); SA_BOOL_NO_ROW: a term
     u32 sparse;     // Bm25Params::sparse_ok under this clause's idf
-    u32 field;      // bool_fields_tile_kernel: the clause's slot in the field table; 0 otherwise
+    u32 field;      // FIELDS: the clause's slot in the field table; 0 otherwise
 };
 
 struct BoolQuery { u32 c0, n, mm, pad; };   // clauses [c0, c0 + n) of the batch
@@ -75,14 +75,14 @@ struct BoolArgs {
     TopkCtx topk;
 };
 
-// A clause's role and weight (sa_score_batch_topk_bool_occur), read by bool_tile_kernel<true> only, so the plain
+// A clause's role and weight (clause_weight, clause_occur), read by the OCCUR instances only, so the Or / And
 // instance's loads stay those of BoolClause.
 struct BoolOccur {
     float weight;   // MUST / SHOULD: s += weight * score (rounded once, then added)
     u32 occur;      // SA_OCCUR_*
 };
 
-// One field of sa_multi_score_batch_topk_bool, as bool_fields_tile_kernel reads it: BoolArgs' per-index members.
+// One field of sa_multi_score_batch_topk_bool, as the FIELDS instances read it: BoolArgs' per-index members.
 struct BoolField {
     const u64 *words;
     const u32 *tile_dir, *recs, *rec_dir;
@@ -90,8 +90,8 @@ struct BoolField {
     Bm25Params bm25;                        // idf unused (per clause)
 };
 
-// A clause's disjunction-max group (bool_dismax_tile_kernel only).  A clause outside a DisMax, or the one member of a
-// single-member DisMax, is a group of one (member == 0) and folds exactly as in bool_fields_tile_kernel.
+// A clause's disjunction-max group (DISMAX instances only).  A clause outside a DisMax, or the one member of a
+// single-member DisMax, is a group of one (member == 0) and folds exactly as in the FIELDS instance.
 struct BoolGroup {
     float tie;      // the group's tie (member clauses)
     u32 first;      // the group's first clause, within its query
@@ -99,7 +99,7 @@ struct BoolGroup {
     u32 last;       // 1: the group's last member
 };
 
-// The nested-query part of bool_nested_tile_kernel's arguments.  A nested node's row is BoolQuery::pad (its slot in
+// The nested-query part of the NESTED instances' arguments.  A nested node's row is BoolQuery::pad (its slot in
 // BoolState::rows, numbered with the phrase rows of its launch group); a nested clause's BoolClause::row is its
 // child's row.
 struct BoolNest {
@@ -118,7 +118,7 @@ struct BoolState {
     DevBuf d_fields;     // BoolField[] of a multi-field call
     DevBuf d_keys;       // nq * k result keys, then u32 overflow[nq]: one device-to-host copy
     DevBuf rows;
-    DevBuf d_where;      // the WhereMask rows of a `_where` call
+    DevBuf d_where;      // the WhereMask rows of a masked call
 };
 void BoolStateDelete::operator()(BoolState *s) const { delete s; }
 
@@ -154,7 +154,7 @@ __device__ __forceinline__ void bool_scatter_term(const BoolArgs &a, const BoolC
     }
 }
 
-// bool_tile_kernel<true>: doc i = 4 j + e of the thread's 32 gets the clause's exact score v.  MUST / SHOULD add
+// OCCUR: doc i = 4 j + e of the thread's 32 gets the clause's exact score v.  MUST / SHOULD add
 // weight * v, each product rounded before the add as numpy rounds it (no FMA contraction); only SHOULD counts a hit,
 // on the unweighted v, so a zero weight still matches; MUST / FILTER clear the doc's `req` bit where v is not > 0;
 // MUST_NOT sets its `veto` bit where v > 0.  The occur tests are clause-uniform branches, which skip the work of the
@@ -167,7 +167,7 @@ __device__ __forceinline__ void bool_fold_occur(float &acc, u32 &hits, u32 &req,
     if (oc.occur == SA_OCCUR_MUST_NOT && v > 0.0f) veto |= 1u << i;
 }
 
-// bool_dismax_tile_kernel: bool_fold_occur of a DisMax group's d, with the group's hit (any member > 0) in place of
+// DISMAX: bool_fold_occur of a DisMax group's d, with the group's hit (any member > 0) in place of
 // d > 0 and weight 1.
 __device__ __forceinline__ void bool_fold_group(float &acc, u32 &hits, u32 &req, u32 &veto, int i, float d, bool hit,
                                                 u32 occur) {
@@ -467,71 +467,69 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
     flush_tile_collect<false>(s_tile, nullptr, a.topk, q, tile, my_max, SA_TILE_DOCS, 0, s_top, &s_ncand, &s_tile_max);
 }
 
-template <bool OCCUR>
-__global__ void __launch_bounds__(SA_TERM_THREADS)
-bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ) {
-    bool_tile<OCCUR, false>(a, occ, nullptr);
-}
-
-// sa_score_batch_topk_bool_dismax / sa_multi_score_batch_topk_bool_dismax: bool_fields_tile_kernel with DisMax groups.
-// The groups' running max and sum live in SA_BOOL_DISMAX_SMEM bytes of dynamic shared memory (a thread's strips,
-// owner-only, so no extra barriers); see DESIGN.md section 3.10.3 for registers and occupancy.
+// Every instance of the fold: bool_tile with the arguments its form reads (the others are NULL and never read).
+// MIN_CTAS holds an instance to the CTAs per SM it was tuned for (0: no minimum); bool_kernel lists the ten instances.
+// DISMAX: the groups' running max and sum live in SA_BOOL_DISMAX_SMEM bytes of dynamic shared memory (a thread's
+// strips, owner-only, so no extra barriers).
 #define SA_BOOL_DISMAX_SMEM (2 * SA_TILE_DOCS * sizeof(float))
-__global__ void __launch_bounds__(SA_TERM_THREADS, 2)
-bool_dismax_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
-                        const BoolGroup *__restrict__ grp) {
-    extern __shared__ __align__(16) float s_dyn[];
+
+// bool_tile's s_g placed ahead of the fold's own shared arrays.  Where the compiler places a __shared__ array follows
+// where it is declared: the unmasked DisMax instances were tuned with s_g first (a local of this helper, one instance
+// per kernel), the masked ones with it last (a local of the kernel), and each keeps its layout.
+template <bool NESTED>
+__device__ __forceinline__ unsigned long long *bool_s_g_first() {
     __shared__ unsigned long long s_g[3];
-    bool_tile<true, true, true>(a, occ, fld, grp, s_dyn, s_g);
+    return s_g;
 }
 
-// sa_score_batch_topk_bool_nested / sa_multi_score_batch_topk_bool_nested: bool_dismax_tile_kernel with nested
-// clauses, launched once per level of nested nodes (nb.store set) and once for the top-level nodes; see DESIGN.md
-// section 3.10.4 for registers and occupancy.
-__global__ void __launch_bounds__(SA_TERM_THREADS, 2)
-bool_nested_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
-                        const BoolGroup *__restrict__ grp, const BoolNest nb) {
-    extern __shared__ __align__(16) float s_dyn[];
-    __shared__ unsigned long long s_g[3];
-    bool_tile<true, true, true, true>(a, occ, fld, grp, s_dyn, s_g, nb);
-}
-
-// sa_multi_score_batch_topk_bool: roles and weights as bool_tile_kernel<true>, each clause on its own field.  Held to
-// three CTAs per SM, as the single-field instance runs (80 registers, no spills); at two (90 registers) it ran 23-24%
-// slower.
-__global__ void __launch_bounds__(SA_TERM_THREADS, 3)
-bool_fields_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld) {
-    bool_tile<true, true>(a, occ, fld);
-}
-
-// sa_score_batch_topk_bool_where / sa_multi_score_batch_topk_bool_where: the instances above with a document mask,
-// each held to its unmasked instance's CTAs per SM (MIN_CTAS; see DESIGN.md section 3.11).  Template arguments
-// (OCCUR, FIELDS, DISMAX, NESTED) of bool_tile_kernel<false>: (false, false, false, false), <true>: (true, false, ...),
-// bool_fields_tile_kernel: (true, true, false, false), bool_dismax_tile_kernel: (true, true, true, false),
-// bool_nested_tile_kernel's top-level launch: (true, true, true, true).
-template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, int MIN_CTAS>
+template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, int MIN_CTAS>
 __global__ void __launch_bounds__(SA_TERM_THREADS, MIN_CTAS)
-bool_where_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
-                       const BoolGroup *__restrict__ grp, const BoolNest nb, const WhereMask wh) {
+bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
+                 const BoolGroup *__restrict__ grp, const BoolNest nb, const WhereMask wh) {
     extern __shared__ __align__(16) float s_dyn[];
-    __shared__ unsigned long long s_g[3];
-    bool_tile<OCCUR, FIELDS, DISMAX, NESTED, true>(a, occ, fld, grp, s_dyn, s_g, nb, wh);
+    if constexpr (DISMAX && !WHERE) {
+        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE>(a, occ, fld, grp, s_dyn, bool_s_g_first<NESTED>(), nb, wh);
+    } else {
+        __shared__ unsigned long long s_g[3];
+        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE>(a, occ, fld, grp, s_dyn, s_g, nb, wh);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------------------ host
 namespace {
 
-// The fields of one call and where the call keeps its state.  The single-index entry points pass one field and the
+// The form of a call, which picks its instance: Or / And; roles and weights (OCCUR); every multi-field call (FIELDS);
+// DisMax groups (on a field table, a single-index call passing one field); nested nodes.
+enum BoolForm { BOOL_OR_AND, BOOL_OCCUR, BOOL_FIELDS, BOOL_DISMAX, BOOL_NESTED };
+
+typedef void (*BoolKernel)(BoolArgs, const BoolOccur *, const BoolField *, const BoolGroup *, BoolNest, WhereMask);
+
+// The instance a launch of `form` runs, with or without a document mask.  The fields instance is held to three CTAs per
+// SM, as the single-field roles instance runs (80 registers, no spills; at two, 90 registers, it ran 23-24% slower);
+// the DisMax and nested ones to two (DESIGN.md sections 3.10.3, 3.10.4); each masked instance to its unmasked
+// instance's CTAs per SM (section 3.11).  A nested call's store passes run the unmasked nested instance.
+BoolKernel bool_kernel(BoolForm form, bool masked) {
+    static const BoolKernel instances[5][2] = {
+        {bool_tile_kernel<false, false, false, false, false, 0>, bool_tile_kernel<false, false, false, false, true, 2>},
+        {bool_tile_kernel<true, false, false, false, false, 0>, bool_tile_kernel<true, false, false, false, true, 3>},
+        {bool_tile_kernel<true, true, false, false, false, 3>, bool_tile_kernel<true, true, false, false, true, 3>},
+        {bool_tile_kernel<true, true, true, false, false, 2>, bool_tile_kernel<true, true, true, false, true, 2>},
+        {bool_tile_kernel<true, true, true, true, false, 2>, bool_tile_kernel<true, true, true, true, true, 2>},
+    };
+    return instances[form][masked];
+}
+
+// The fields of one call and where the call keeps its state.  The single-index entry point passes one field and the
 // index's own buffers (ix->boolq, ix->cand, ix->h_pinned); sa_multi_score_batch_topk_bool passes the multi's fields,
 // its BoolState and candidate buffer, and field 0's pinned staging.  Every field's stream is `lead`'s (FieldGuard).
 struct BoolCall {
     std::vector<sa_index *> ix;         // per field slot
     std::vector<float> avgdl, k1, b;    // per field slot
-    bool fields_kernel = false;         // bool_fields_tile_kernel (clauses carry their field slot)
+    bool fields_kernel = false;         // a multi-field call: BOOL_FIELDS at least (clauses carry their field slot)
     BoolState *S = nullptr;
     DevBuf *cand = nullptr;
     PinnedBuf *h_pinned = nullptr;
-    // the `_where` entry points' mask, as passed (host; where_bits NULL: no mask), and its rows on the device
+    // the call's document mask, as passed (host; where_bits NULL: no mask), and its rows on the device
     const uint32_t *where_bits = nullptr;
     uint64_t where_n = 0, where_stride = 0;
     WhereMask where{nullptr, 0};
@@ -539,12 +537,13 @@ struct BoolCall {
 };
 
 struct BoolPlan {
+    BoolForm form = BOOL_OR_AND;
     std::vector<BoolClause> clauses;
     std::vector<BoolQuery> queries;
     std::vector<u32> group_start;       // queries [group_start[i], group_start[i + 1]) share one launch and its rows
-    std::vector<BoolOccur> occur;       // per clause, as clauses; empty: Or / And (bool_tile_kernel<false>)
-    std::vector<BoolField> fields;      // per field slot (bool_fields_tile_kernel, bool_dismax_tile_kernel)
-    std::vector<BoolGroup> groups;      // per clause, as clauses; non-empty: bool_dismax_tile_kernel
+    std::vector<BoolOccur> occur;       // per clause, as clauses (from BOOL_OCCUR up)
+    std::vector<BoolField> fields;      // per field slot (from BOOL_FIELDS up)
+    std::vector<BoolGroup> groups;      // per clause, as clauses (from BOOL_DISMAX up)
     u32 max_group = 1, max_rows = 0;
     // nested calls: nodes 0 .. n_top - 1 are the top-level queries (queries[0 .. n_top)), the others nested nodes
     u32 n_top = 0;
@@ -552,7 +551,7 @@ struct BoolPlan {
     std::vector<u32> root, depth;       // per node: its top-level query, and its depth below it
     std::vector<u32> nested;            // nested nodes by (launch group, depth desc, top-level query); queries[n_top + i]
                                         // is nested[i]'s descriptor
-    std::vector<u32> nest;              // per clause, as clauses: 1 for a nested clause; non-empty: bool_nested_tile_kernel
+    std::vector<u32> nest;              // per clause, as clauses: 1 for a nested clause (BOOL_NESTED)
 };
 
 // The count rows of the phrase clauses of queries [q0, q1) and of their nested nodes (rows are numbered within the
@@ -612,12 +611,17 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
     a.topk = t;
     WhereMask wh = X.where;                 // row 0 of the launch is query q0's
     if (wh.bits) wh.bits += (u64)q0 * wh.stride;
-    const dim3 grid(nq, n_tiles);
-    const BoolNest no_nest{nullptr, nullptr, nullptr, 0};
-    if (!P.nest.empty()) {
+    // the arrays P.form reads, NULL above it
+    const BoolOccur *occ = P.form >= BOOL_OCCUR ? S.d_occur.as<BoolOccur>() : nullptr;
+    const BoolField *fld = P.form >= BOOL_FIELDS ? S.d_fields.as<BoolField>() : nullptr;
+    const BoolGroup *grp = P.form >= BOOL_DISMAX ? S.d_groups.as<BoolGroup>() : nullptr;
+    BoolNest nb{nullptr, nullptr, nullptr, 0};
+    const size_t smem = P.form >= BOOL_DISMAX ? SA_BOOL_DISMAX_SMEM : 0;
+    if (P.form == BOOL_NESTED) {
         // the nested nodes of these queries, deepest level first (one launch per level: a level's nodes of the run
-        // are consecutive in P.nested), each into its row and flags; then the top-level nodes, collected
-        BoolNest nb{S.d_nest.as<u32>(), S.d_flags.as<u32>(), S.rows.as<float>(), n_tiles};
+        // are consecutive in P.nested), each into its row and flags, unmasked; then the top-level nodes, collected
+        nb = BoolNest{S.d_nest.as<u32>(), S.d_flags.as<u32>(), S.rows.as<float>(), n_tiles};
+        const BoolKernel store = bool_kernel(BOOL_NESTED, false);
         for (size_t i = 0; i < P.nested.size();) {
             auto in_run = [&](size_t x) { return P.root[P.nested[x]] >= q0 && P.root[P.nested[x]] < q1; };
             if (!in_run(i)) { i++; continue; }
@@ -625,66 +629,36 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
             while (j < P.nested.size() && in_run(j) && P.depth[P.nested[j]] == P.depth[P.nested[i]]) j++;
             BoolArgs an = a;
             an.queries = S.d_queries.as<BoolQuery>() + P.n_top + i;
-            bool_nested_tile_kernel<<<dim3((u32)(j - i), n_tiles), SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
-                an, S.d_occur.as<BoolOccur>(), S.d_fields.as<BoolField>(), S.d_groups.as<BoolGroup>(), nb);
+            store<<<dim3((u32)(j - i), n_tiles), SA_TERM_THREADS, smem, ix->stream>>>(an, occ, fld, grp, nb,
+                                                                                     WhereMask{nullptr, 0});
             SA_CUDA(cudaGetLastError());
             ix->stats.total_launches++;
             i = j;
         }
         nb.store = nullptr;
-        if (wh.bits)
-            bool_where_tile_kernel<true, true, true, true, 2><<<grid, SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
-                a, S.d_occur.as<BoolOccur>(), S.d_fields.as<BoolField>(), S.d_groups.as<BoolGroup>(), nb, wh);
-        else
-            bool_nested_tile_kernel<<<dim3(nq, n_tiles), SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
-                a, S.d_occur.as<BoolOccur>(), S.d_fields.as<BoolField>(), S.d_groups.as<BoolGroup>(), nb);
-    } else if (wh.bits) {
-        const BoolOccur *occ = S.d_occur.as<BoolOccur>();
-        const BoolField *fld = S.d_fields.as<BoolField>();
-        if (!P.groups.empty())
-            bool_where_tile_kernel<true, true, true, false, 2><<<grid, SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
-                a, occ, fld, S.d_groups.as<BoolGroup>(), no_nest, wh);
-        else if (X.fields_kernel)
-            bool_where_tile_kernel<true, true, false, false, 3><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(
-                a, occ, fld, nullptr, no_nest, wh);
-        else if (P.occur.empty())
-            bool_where_tile_kernel<false, false, false, false, 2><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(
-                a, nullptr, nullptr, nullptr, no_nest, wh);
-        else
-            bool_where_tile_kernel<true, false, false, false, 3><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(
-                a, occ, nullptr, nullptr, no_nest, wh);
-    } else if (!P.groups.empty())
-        bool_dismax_tile_kernel<<<dim3(nq, n_tiles), SA_TERM_THREADS, SA_BOOL_DISMAX_SMEM, ix->stream>>>(
-            a, S.d_occur.as<BoolOccur>(), S.d_fields.as<BoolField>(), S.d_groups.as<BoolGroup>());
-    else if (X.fields_kernel)
-        bool_fields_tile_kernel<<<dim3(nq, n_tiles), SA_TERM_THREADS, 0, ix->stream>>>(a, S.d_occur.as<BoolOccur>(),
-                                                                                        S.d_fields.as<BoolField>());
-    else if (P.occur.empty())
-        bool_tile_kernel<false><<<dim3(nq, n_tiles), SA_TERM_THREADS, 0, ix->stream>>>(a, nullptr);
-    else
-        bool_tile_kernel<true><<<dim3(nq, n_tiles), SA_TERM_THREADS, 0, ix->stream>>>(a, S.d_occur.as<BoolOccur>());
+    }
+    bool_kernel(P.form, wh.bits != nullptr)<<<dim3(nq, n_tiles), SA_TERM_THREADS, smem, ix->stream>>>(
+        a, occ, fld, grp, nb, wh);
     SA_CUDA(cudaGetLastError());
     ix->stats.total_launches++;
     return launch_topk_select(ix, t, nq, ix->doc_base, d_keys, S.d_out_index.as<u32>() + q0);
 }
 
-// bool_dismax_tile_kernel's (bool_nested_tile_kernel's) dynamic shared memory above the default 48 KB, and the
-// carveout that fits two CTAs per SM (~2 x 98 KB of shared memory), on the current device (function attributes are
-// per device).
-template <typename Kernel>
-int bool_dismax_smem(Kernel kernel) {
+// The DisMax instances' dynamic shared memory above the default 48 KB, and the carveout that fits two CTAs per SM
+// (~2 x 98 KB of shared memory), on the current device (function attributes are per device).
+int bool_dismax_smem(BoolKernel kernel) {
     SA_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SA_BOOL_DISMAX_SMEM));
     SA_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
                                  (int)cudaSharedmemCarveoutMaxShared));
     return SA_OK;
 }
 
-// Every entry point, with the call's indexes locked and their device current.  clause_weight / clause_occur NULL:
+// Both entry points, with the call's indexes locked and their device current.  clause_weight / clause_occur NULL:
 // Or / And, every clause SHOULD with weight 1, mm over all.  clause_field NULL: every clause on field 0.
-// clause_group / clause_tie non-NULL (with clause_occur): DisMax groups, bool_dismax_tile_kernel with a field table.
-// clause_node non-NULL (with the DisMax arrays): n_nodes nodes, the first n_queries top-level, clause c being nested
-// node clause_node[c] unless SA_NO_NODE (sa_score_batch_topk_bool_nested); otherwise n_nodes == n_queries.
-// X.where_bits non-NULL: the document mask of the `_where` entry points, checked before any device work.
+// clause_group / clause_tie non-NULL (with clause_occur): DisMax groups, on a field table.  clause_node non-NULL (with
+// the DisMax arrays): n_nodes nodes, the first n_queries top-level, clause c being nested node clause_node[c] unless
+// SA_NO_NODE; otherwise n_nodes == n_queries.  X.where_bits non-NULL: the document mask, checked before any device
+// work.
 int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts, const uint32_t *clause_node,
               const uint32_t *clause_field, const uint32_t *clause_terms, const uint32_t *clause_term_starts,
               const float *clause_idf, const float *clause_weight, const uint8_t *clause_occur,
@@ -771,6 +745,7 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
     const u32 group_q = (u32)std::min<u64>(65535, std::max<u64>(1, (1ull << 30) / ((u64)n_tiles * (slots * sizeof(u64) + 8))));
     const u32 group_rows = (u32)std::max<u64>(1, (4ull << 30) / (stride * sizeof(float)));
     BoolPlan P;
+    P.form = nested ? BOOL_NESTED : dismax ? BOOL_DISMAX : X.fields_kernel ? BOOL_FIELDS : occur ? BOOL_OCCUR : BOOL_OR_AND;
     P.n_top = n_queries;
     P.node_starts.assign(query_clause_starts, query_clause_starts + n_nodes + 1);
     P.root.resize(n_nodes);
@@ -875,7 +850,7 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
         return rc;
     for (u32 f = 0; f < n_fields; f++)
         if (field_sparse[f] && (rc = sa_ensure_norm(X.ix[f], X.k1[f], X.b[f], X.avgdl[f]))) return rc;
-    if (X.fields_kernel || dismax) {
+    if (P.form >= BOOL_FIELDS) {
         for (u32 f = 0; f < n_fields; f++) {
             sa_index *ix = X.ix[f];
             P.fields.push_back(BoolField{ix->d_words.as<u64>(), ix->d_tile_dir.as<u32>(), ix->d_recs.as<u32>(),
@@ -895,10 +870,8 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
     if ((rc = sa_where_upload(lead, S.d_where, X.where_bits, lead->n_docs, X.where_stride, n_queries, &X.where)))
         return rc;
     if (dismax) {
-        if ((rc = nested ? bool_dismax_smem(bool_nested_tile_kernel) : bool_dismax_smem(bool_dismax_tile_kernel)))
-            return rc;
-        if (X.where.bits && (rc = nested ? bool_dismax_smem(bool_where_tile_kernel<true, true, true, true, 2>)
-                                         : bool_dismax_smem(bool_where_tile_kernel<true, true, true, false, 2>)))
+        if ((rc = bool_dismax_smem(bool_kernel(P.form, false))) ||
+            (X.where.bits && (rc = bool_dismax_smem(bool_kernel(P.form, true)))))
             return rc;
         SA_CUDA(cudaMemcpyAsync(S.d_groups.p, P.groups.data(), P.groups.size() * sizeof(BoolGroup), cudaMemcpyHostToDevice, lead->stream));
     }
@@ -937,7 +910,7 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
     return SA_OK;
 }
 
-// The single-index entry points: the index's own lock, state and buffers.
+// sa_score_batch_topk_bool: the index's own lock, state and buffers.
 int bool_topk_index(sa_index *ix, uint32_t n_nodes, const uint32_t *query_clause_starts,
                     const uint32_t *clause_node, const uint32_t *clause_terms,
                     const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
@@ -969,7 +942,7 @@ int bool_topk_index(sa_index *ix, uint32_t n_nodes, const uint32_t *query_clause
                      out_docs, out_scores, n_redone);
 }
 
-// The multi-field entry points: the multi's lock, state and candidate buffer.
+// sa_multi_score_batch_topk_bool: the multi's lock, state and candidate buffer.
 int bool_topk_multi(sa_multi *m, uint32_t n_nodes, const uint32_t *query_clause_starts,
                     const uint32_t *clause_node, const uint32_t *clause_field,
                     const uint32_t *clause_terms, const uint32_t *clause_term_starts, const float *clause_idf,
@@ -1019,106 +992,15 @@ int bool_topk_multi(sa_multi *m, uint32_t n_nodes, const uint32_t *query_clause_
 
 }  // namespace
 
-extern "C" int sa_score_batch_topk_bool(sa_index *ix, const uint32_t *query_clause_starts, const uint32_t *clause_terms,
-                                        const uint32_t *clause_term_starts, const float *clause_idf, const uint32_t *mm,
-                                        uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
-                                        uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
-    return bool_topk_index(ix, n_queries, query_clause_starts, nullptr, clause_terms, clause_term_starts, clause_idf,
-                           nullptr, nullptr, nullptr, nullptr, mm, n_queries, slop, avg_doc_len, k1, b, k, nullptr, 0,
-                           0, out_docs, out_scores, n_redone);
-}
-
-extern "C" int sa_score_batch_topk_bool_occur(sa_index *ix, const uint32_t *query_clause_starts,
-                                              const uint32_t *clause_terms, const uint32_t *clause_term_starts,
-                                              const float *clause_idf, const float *clause_weight,
-                                              const uint8_t *clause_occur, const uint32_t *mm, uint32_t n_queries,
-                                              uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
-                                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
-    SA_CHECK(n_queries == 0 || (clause_weight && clause_occur), "NULL argument");
-    return bool_topk_index(ix, n_queries, query_clause_starts, nullptr, clause_terms, clause_term_starts, clause_idf,
-                           clause_weight, clause_occur, nullptr, nullptr, mm, n_queries, slop, avg_doc_len, k1, b, k,
-                           nullptr, 0, 0, out_docs, out_scores, n_redone);
-}
-
-extern "C" int sa_score_batch_topk_bool_dismax(sa_index *ix, const uint32_t *query_clause_starts,
-                                               const uint32_t *clause_terms, const uint32_t *clause_term_starts,
-                                               const float *clause_idf, const float *clause_weight,
-                                               const uint8_t *clause_occur, const uint32_t *clause_group,
-                                               const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
-                                               uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
-                                               uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
-    SA_CHECK(n_queries == 0 || (clause_weight && clause_occur && clause_group && clause_tie), "NULL argument");
-    return bool_topk_index(ix, n_queries, query_clause_starts, nullptr, clause_terms, clause_term_starts, clause_idf,
-                           clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, avg_doc_len, k1,
-                           b, k, nullptr, 0, 0, out_docs, out_scores, n_redone);
-}
-
-extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, const uint32_t *query_clause_starts,
-                                              const uint32_t *clause_field, const uint32_t *clause_terms,
-                                              const uint32_t *clause_term_starts, const float *clause_idf,
-                                              const float *clause_weight, const uint8_t *clause_occur,
-                                              const uint32_t *mm, uint32_t n_queries, uint32_t slop,
-                                              const float *avg_doc_len, const float *k1, const float *b, uint32_t k,
-                                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
-    return bool_topk_multi(m, n_queries, query_clause_starts, nullptr, clause_field, clause_terms, clause_term_starts,
-                           clause_idf, clause_weight, clause_occur, nullptr, nullptr, mm, n_queries, slop, avg_doc_len,
-                           k1, b, k, nullptr, 0, 0, out_docs, out_scores, n_redone);
-}
-
-extern "C" int sa_multi_score_batch_topk_bool_dismax(sa_multi *m, const uint32_t *query_clause_starts,
-                                                     const uint32_t *clause_field, const uint32_t *clause_terms,
-                                                     const uint32_t *clause_term_starts, const float *clause_idf,
-                                                     const float *clause_weight, const uint8_t *clause_occur,
-                                                     const uint32_t *clause_group, const float *clause_tie,
-                                                     const uint32_t *mm, uint32_t n_queries, uint32_t slop,
-                                                     const float *avg_doc_len, const float *k1, const float *b,
-                                                     uint32_t k, uint32_t *out_docs, float *out_scores,
-                                                     uint32_t *n_redone) {
-    SA_CHECK(n_queries == 0 || (clause_group && clause_tie), "NULL argument");
-    return bool_topk_multi(m, n_queries, query_clause_starts, nullptr, clause_field, clause_terms, clause_term_starts,
-                           clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop,
-                           avg_doc_len, k1, b, k, nullptr, 0, 0, out_docs, out_scores, n_redone);
-}
-
-extern "C" int sa_score_batch_topk_bool_nested(sa_index *ix, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                               const uint32_t *clause_node, const uint32_t *clause_terms,
-                                               const uint32_t *clause_term_starts, const float *clause_idf,
-                                               const float *clause_weight, const uint8_t *clause_occur,
-                                               const uint32_t *clause_group, const float *clause_tie,
-                                               const uint32_t *mm, uint32_t n_queries, uint32_t slop,
-                                               float avg_doc_len, float k1, float b, uint32_t k, uint32_t *out_docs,
-                                               float *out_scores, uint32_t *n_redone) {
-    SA_CHECK(n_nodes == 0 || (clause_node && clause_weight && clause_occur && clause_group && clause_tie),
-             "NULL argument");
-    return bool_topk_index(ix, n_nodes, node_clause_starts, clause_node, clause_terms, clause_term_starts, clause_idf,
-                           clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, avg_doc_len,
-                           k1, b, k, nullptr, 0, 0, out_docs, out_scores, n_redone);
-}
-
-extern "C" int sa_multi_score_batch_topk_bool_nested(sa_multi *m, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                                     const uint32_t *clause_node, const uint32_t *clause_field,
-                                                     const uint32_t *clause_terms, const uint32_t *clause_term_starts,
-                                                     const float *clause_idf, const float *clause_weight,
-                                                     const uint8_t *clause_occur, const uint32_t *clause_group,
-                                                     const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
-                                                     uint32_t slop, const float *avg_doc_len, const float *k1,
-                                                     const float *b, uint32_t k, uint32_t *out_docs,
-                                                     float *out_scores, uint32_t *n_redone) {
-    SA_CHECK(n_nodes == 0 || (clause_node && clause_group && clause_tie), "NULL argument");
-    return bool_topk_multi(m, n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
-                           clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop,
-                           avg_doc_len, k1, b, k, nullptr, 0, 0, out_docs, out_scores, n_redone);
-}
-
-extern "C" int sa_score_batch_topk_bool_where(sa_index *ix, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                              const uint32_t *clause_node, const uint32_t *clause_terms,
-                                              const uint32_t *clause_term_starts, const float *clause_idf,
-                                              const float *clause_weight, const uint8_t *clause_occur,
-                                              const uint32_t *clause_group, const float *clause_tie,
-                                              const uint32_t *mm, uint32_t n_queries, uint32_t slop,
-                                              float avg_doc_len, float k1, float b, uint32_t k,
-                                              const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
-                                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+extern "C" int sa_score_batch_topk_bool(sa_index *ix, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                        const uint32_t *clause_node, const uint32_t *clause_terms,
+                                        const uint32_t *clause_term_starts, const float *clause_idf,
+                                        const float *clause_weight, const uint8_t *clause_occur,
+                                        const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
+                                        uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b,
+                                        uint32_t k, const uint32_t *where_bits, uint64_t where_n,
+                                        uint64_t where_stride, uint32_t *out_docs, float *out_scores,
+                                        uint32_t *n_redone) {
     SA_CHECK(!clause_weight == !clause_occur, "clause_weight and clause_occur are both given or both NULL");
     SA_CHECK(!clause_group == !clause_tie && (!clause_group || clause_occur),
              "clause_group and clause_tie are both given (with clause_occur) or both NULL");
@@ -1129,16 +1011,16 @@ extern "C" int sa_score_batch_topk_bool_where(sa_index *ix, uint32_t n_nodes, co
                            k1, b, k, where_bits, where_n, where_stride, out_docs, out_scores, n_redone);
 }
 
-extern "C" int sa_multi_score_batch_topk_bool_where(sa_multi *m, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                                    const uint32_t *clause_node, const uint32_t *clause_field,
-                                                    const uint32_t *clause_terms, const uint32_t *clause_term_starts,
-                                                    const float *clause_idf, const float *clause_weight,
-                                                    const uint8_t *clause_occur, const uint32_t *clause_group,
-                                                    const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
-                                                    uint32_t slop, const float *avg_doc_len, const float *k1,
-                                                    const float *b, uint32_t k, const uint32_t *where_bits,
-                                                    uint64_t where_n, uint64_t where_stride, uint32_t *out_docs,
-                                                    float *out_scores, uint32_t *n_redone) {
+extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                              const uint32_t *clause_node, const uint32_t *clause_field,
+                                              const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                              const float *clause_idf, const float *clause_weight,
+                                              const uint8_t *clause_occur, const uint32_t *clause_group,
+                                              const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
+                                              uint32_t slop, const float *avg_doc_len, const float *k1, const float *b,
+                                              uint32_t k, const uint32_t *where_bits, uint64_t where_n,
+                                              uint64_t where_stride, uint32_t *out_docs, float *out_scores,
+                                              uint32_t *n_redone) {
     SA_CHECK(!clause_group == !clause_tie, "clause_group and clause_tie are both given or both NULL");
     SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
              "clause_node needs the DisMax arrays; without it n_nodes == n_queries");

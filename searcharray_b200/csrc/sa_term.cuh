@@ -30,7 +30,7 @@ struct TopkCtx {
     u32 k;             // 0 => no top-k collection
 };
 
-// A document mask of the batched top-k (the `_where` entry points): one row of packed bits for the batch, or one per
+// A document mask of the batched top-k (the entry points' where_bits): one row of packed bits for the batch, or one per
 // query.  The tile kernels that take it (bool_tile, sim_tile) have thread tid own docs 4 g .. 4 g + 3 of a tile,
 // g = tid + j * SA_TERM_THREADS (flush_tile_collect's layout), so a row stores its bits in that owner order, not in
 // doc order: word tile * SA_TERM_THREADS + tid holds, at bit 4 j + e, doc tile * SA_TILE_DOCS + 4 g + e.  A thread
@@ -121,7 +121,7 @@ inline u32 sa_n_tiles(u64 n_docs) { return (u32)((n_docs + SA_TILE_DOCS - 1) / S
 inline u64 sa_padded_docs(u64 n_docs) { return (u64)sa_n_tiles(n_docs) * SA_TILE_DOCS; }
 static_assert(SA_WHERE_WORDS(1) == SA_TERM_THREADS && SA_WHERE_WORDS(SA_TILE_DOCS + 1) == 2 * SA_TERM_THREADS,
               "a WhereMask row is SA_TERM_THREADS words per tile");
-// The `_where` entry points' mask arguments against the n docs (positions) the call ranks, on the host: where_bits
+// The entry points' mask arguments against the n docs (positions) the call ranks, on the host: where_bits
 // NULL (no mask), or where_n == n and where_stride 0 or SA_WHERE_WORDS(n).
 int sa_where_check(const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride, u64 n);
 // A checked mask's rows over n docs (one, or n_queries when where_stride != 0) into buf on ix->stream; *out addresses

@@ -37,7 +37,7 @@ struct ViewState {
     DevBuf d_keys;         // u64 [n_queries * k]: the result keys
     DevBuf d_cand_d;       // u64 [chunk][tiles][slots]: float64 score bits of the classic candidates
     DevBuf d_scores;       // double [n_queries * k]: the classic result scores
-    DevBuf d_where;        // the WhereMask rows of sa_score_batch_topk_sim_where
+    DevBuf d_where;        // the WhereMask rows of a masked sa_score_batch_topk_sim
 };
 
 void ViewStateDelete::operator()(ViewState *v) const { delete v; }
@@ -141,7 +141,7 @@ sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *_
                           nullptr);
 }
 
-// sa_score_batch_topk_sim_where: sim_tile_kernel with a document mask over the positions.
+// sa_score_batch_topk_sim with where_bits: sim_tile_kernel with a document mask over the positions.
 template <int KIND>
 __global__ void __launch_bounds__(SA_TERM_THREADS)
 sim_where_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *__restrict__ rows,
@@ -306,16 +306,8 @@ int sa_where_upload(sa_index *ix, DevBuf &buf, const uint32_t *where_bits, u64 n
 extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *terms, const uint32_t *term_starts,
                                        const double *idf, uint32_t n_queries, uint32_t slop,
                                        const float *view_doc_lens, double avg_doc_len, double k1, double b,
-                                       uint32_t k, uint32_t *out_ids, double *out_scores) {
-    return sa_score_batch_topk_sim_where(ix, kind, terms, term_starts, idf, n_queries, slop, view_doc_lens,
-                                         avg_doc_len, k1, b, k, nullptr, 0, 0, out_ids, out_scores);
-}
-
-extern "C" int sa_score_batch_topk_sim_where(sa_index *ix, int kind, const uint32_t *terms,
-                                             const uint32_t *term_starts, const double *idf, uint32_t n_queries,
-                                             uint32_t slop, const float *view_doc_lens, double avg_doc_len, double k1,
-                                             double b, uint32_t k, const uint32_t *where_bits, uint64_t where_n,
-                                             uint64_t where_stride, uint32_t *out_ids, double *out_scores) {
+                                       uint32_t k, const uint32_t *where_bits, uint64_t where_n,
+                                       uint64_t where_stride, uint32_t *out_ids, double *out_scores) {
     SA_CHECK(ix, "index is NULL");
     SA_CHECK(n_queries == 0 || (terms && term_starts && idf && out_ids && out_scores), "NULL argument");
     SA_CHECK(kind == SA_SIM_BM25 || kind == SA_SIM_BM25_IMPACT || kind == SA_SIM_BM25_LEGACY || kind == SA_SIM_CLASSIC,

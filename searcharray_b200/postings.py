@@ -547,16 +547,15 @@ class SearchArray(ExtensionArray):
         query.Bool(must, should, filter, must_not, mm) and query.Boost(clause, weight) clauses are accepted the same
         way: s = w0 * .score(c0) + w1 * .score(c1) + ... over must + should (float32, each product rounded), ranked
         where s > 0, every must and filter clause scores > 0, no must_not clause does and at least mm should clauses
-        do (sa_score_batch_topk_bool_occur).  An Or / And whose weights are all 1 takes the path above unchanged.
+        do.  An Or / And whose weights are all 1 runs exactly as above.
 
         query.DisMax(clauses, tie) is accepted as a clause of these, and as a query of its own (Bool(should=[it])):
         one clause scoring d = max_j v_j + (sum_j v_j - max_j v_j) * tie over its members' v_j = w_j * .score(c_j),
-        matched where any member scores > 0 (sa_score_batch_topk_bool_dismax) -- synonyms as
+        matched where any member scores > 0 -- synonyms as
         DisMax(["film", "movie"], tie=0.1).  Its members need k1 > 0 and 0 <= b < 1 (ValueError otherwise).
 
         An Or / And / Bool may be a clause of another, at any depth (Or([And(["star", "wars"]), And(["star", "trek"])])):
-        it scores what it would rank as a query of its own and matches where that is > 0
-        (sa_score_batch_topk_bool_nested); see query.Or.
+        it scores what it would rank as a query of its own and matches where that is > 0; see query.Or.
 
         where: a document filter -- a boolean array-like (a boolean pd.Series too) of shape (len(self),), one mask for
         the batch, or (len(queries), len(self)), one per query -- ranks each query only among the docs its mask
@@ -566,7 +565,7 @@ class SearchArray(ExtensionArray):
         array (of the view, on a view).  On a view it indexes the view's positions, on a shard the shard's rows.
         A dtype other than bool raises TypeError and another shape ValueError, before any device work; every input
         refused without `where` is refused the same way with it.  Plain BM25 queries on the unsliced array rank as
-        one-clause Or queries (sa_score_batch_topk_bool_where); the others take sa_score_batch_topk_sim_where.  A
+        one-clause Or queries (sa_score_batch_topk_bool); the others take sa_score_batch_topk_sim.  A
         mask per query costs len(self) / 8 bytes of host-to-device copy and device memory per query."""
         from .query import is_boolean
         if where is not None:
@@ -600,31 +599,32 @@ class SearchArray(ExtensionArray):
 
     def _search_topk_plain_where(self, queries, k, similarity, slop, where):
         """search_topk of plain queries with a packed mask (pack_where): on a view or under a non-BM25 similarity
-        through sa_score_batch_topk_sim_where, else each query as a one-clause Or through the boolean fold, which
+        through sa_score_batch_topk_sim, else each query as a one-clause Or through the boolean fold, which
         scores a clause exactly as .score(c, slop=slop).  The clauses are taken as the unmasked batch takes its
         queries (_topk_queries: a str is a term, any other iterable of str a phrase), and the C call checks their
         term counts as the unmasked one does."""
         self._check_topk_similarity(similarity)
         if self.rows is not None or not isinstance(similarity, Bm25Similarity):
             return self._search_topk_sim(queries, k, similarity, slop, where)
-        docs = np.empty((len(queries), k), dtype=np.uint32)
-        scores = np.empty((len(queries), k), dtype=np.float32)
+        from .query import BoolBatch
+        n = len(queries)
         dev = self._device()
         with self._shared["lock"]:
             self._apply_rows(dev)
             terms, c_starts, idfs = self._topk_queries(queries, lambda dfs: compute_idf(self.corpus_size, dfs))
-            starts = np.arange(len(queries) + 1, dtype=np.uint32)             # query q: clause q, mm 1
-            self._bool_where(dev, len(queries), starts, None, terms, c_starts, np.asarray(idfs, dtype=np.float32),
-                             None, None, None, None, np.ones(len(queries), dtype=np.uint32), len(queries), slop,
-                             similarity, k, docs, scores, ctypes.c_uint32(0), where)
+            # query q: clause q, mm 1
+            batch = BoolBatch(queries, np.arange(n + 1, dtype=np.uint32), None, np.ones(n, dtype=np.uint32), None,
+                              None, None, None, n)
+            docs, scores, _ = self._bool_call(dev, batch, terms, c_starts, np.asarray(idfs, dtype=np.float32),
+                                              similarity, slop, k, where)
         return docs, scores
 
     def _search_topk_mixed(self, queries, k, similarity, slop, where=None):
         """search_topk of a batch holding boolean queries: the plain ones through search_topk as before, the boolean
-        ones through sa_score_batch_topk_bool (Or / And with weights 1) or sa_score_batch_topk_bool_occur (Bool,
-        boosted Or / And), each clause with the idf .score gives it; results in query order.  where: a packed mask
-        (pack_where), its rows split with the queries."""
-        from .query import has_dismax, has_field, is_boolean, is_nested, needs_occur
+        ones in one _search_topk_bool call per form present (query.bool_form), so that each runs the lightest
+        instance that scores it, each clause with the idf .score gives it; results in query order.  where: a packed
+        mask (pack_where), its rows split with the queries."""
+        from .query import DISMAX, NESTED, OCCUR, OR_AND, bool_form, has_dismax, has_field, is_boolean
         if any(has_field(q) for q in queries if is_boolean(q)):
             raise ValueError("a Field clause names a DataFrame column: run queries over columns with "
                              "solr.fields_topk(frame, queries), not SearchArray.search_topk")
@@ -633,13 +633,12 @@ class SearchArray(ExtensionArray):
                                       "compose .score() on the view")
         if not isinstance(similarity, Bm25Similarity):
             raise TypeError(f"boolean queries support bm25_similarity only, not {similarity!r}")
-        kind = np.asarray([(4 if is_nested(q) else 3 if has_dismax(q) else needs_occur(q) + 1) if is_boolean(q) else 0
-                           for q in queries])                       # plain, Or, occur, DisMax, nested
-        if any(has_dismax(q) for q, kd in zip(queries, kind) if kd >= 3):
+        kind = np.asarray([bool_form(q) if is_boolean(q) else 0 for q in queries])     # 0: plain
+        if any(has_dismax(q) for q, kd in zip(queries, kind) if kd >= DISMAX):
             self._check_dismax_params(similarity)
         docs = np.empty((len(queries), k), dtype=np.uint32)
         scores = np.empty((len(queries), k), dtype=np.float32)
-        for kd in (0, 1, 2, 3, 4):
+        for kd in (0, OR_AND, OCCUR, DISMAX, NESTED):
             sel = kind == kd
             part = [q for q, s in zip(queries, sel) if s]
             if not part:
@@ -649,10 +648,6 @@ class SearchArray(ExtensionArray):
                 docs[sel], scores[sel] = self._search_topk_plain_where(part, k, similarity, slop, w)
             elif kd == 0:
                 docs[sel], scores[sel] = self.search_topk(part, k=k, similarity=similarity, slop=slop)
-            elif kd == 3:
-                docs[sel], scores[sel], _ = self._search_topk_dismax(part, k, similarity, slop, w)
-            elif kd == 4:
-                docs[sel], scores[sel], _ = self._search_topk_nested(part, k, similarity, slop, w)
             else:
                 docs[sel], scores[sel], _ = self._search_topk_bool(part, k, similarity, slop, w)
         return docs, scores
@@ -662,111 +657,49 @@ class SearchArray(ExtensionArray):
         from .query import check_dismax_members
         check_dismax_members([(0, "DisMax member")], lambda i: (similarity.k1, similarity.b, self.avg_doc_length, 0.0))
 
-    def _bool_where(self, dev, n_nodes, n_starts, c_node, terms, c_starts, idfs, weights, occurs, groups, ties, mm,
-                    n_queries, slop, similarity, k, docs, scores, n_redone, where):
-        """sa_score_batch_topk_bool_where: the boolean entry point the NULL arrays select, with a packed mask (None:
-        no mask, the unmasked instances)."""
+    def _bool_call(self, dev, batch, terms, c_starts, idfs, similarity, slop, k, where):
+        """sa_score_batch_topk_bool on a flattened batch (query.BoolBatch; its None arrays passed as NULL select the
+        instance) and a packed mask (None: no mask): (docs, scores, queries re-run exactly).  Call it with the lock
+        held and the rows applied."""
+        docs = np.empty((batch.n_queries, k), dtype=np.uint32)
+        scores = np.empty((batch.n_queries, k), dtype=np.float32)
+        n_redone = ctypes.c_uint32(0)
+        opt = lambda a, p: None if a is None else p(a)      # noqa: E731
         p_w, stride = _where_args(where)
-        _lib.check(_lib.lib().sa_score_batch_topk_bool_where(
-            dev.handle, n_nodes, _lib.p_u32(n_starts), None if c_node is None else _lib.p_u32(c_node),
-            _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs), None if weights is None else _lib.p_f32(weights),
-            None if occurs is None else _lib.p_u8(occurs), None if groups is None else _lib.p_u32(groups),
-            None if ties is None else _lib.p_f32(ties), _lib.p_u32(mm), n_queries, int(slop), self.avg_doc_length,
-            similarity.k1, similarity.b, k, p_w, len(self), stride, _lib.p_u32(docs), _lib.p_f32(scores),
-            ctypes.byref(n_redone)))
-
-    def _search_topk_dismax(self, queries, k, similarity, slop, where=None):
-        """Boolean queries holding a DisMax through sa_score_batch_topk_bool_dismax: (docs, scores, queries re-run
-        exactly).  Every DisMax member needs sparse-safe BM25 parameters (ValueError before any device work)."""
-        from .query import check_dismax_members, dismax_members, flatten_dismax
-        clauses, q_starts, mm, weights, occurs, groups, ties = flatten_dismax(queries)
-        dev = self._device()
-        docs = np.empty((len(queries), k), dtype=np.uint32)
-        scores = np.empty((len(queries), k), dtype=np.float32)
-        n_redone = ctypes.c_uint32(0)
-        terms, c_starts, idfs = self._topk_queries(clauses, lambda dfs: compute_idf(self.corpus_size, dfs))
-        idfs = np.asarray(idfs, dtype=np.float32)
-        check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
-                             lambda i: (similarity.k1, similarity.b, self.avg_doc_length, idfs[i]))
-        with self._shared["lock"]:
-            self._apply_rows(dev)
-            if where is not None:
-                self._bool_where(dev, len(queries), q_starts, None, terms, c_starts, idfs, weights, occurs, groups,
-                                 ties, mm, len(queries), slop, similarity, k, docs, scores, n_redone, where)
-                return docs, scores, n_redone.value
-            _lib.check(_lib.lib().sa_score_batch_topk_bool_dismax(
-                dev.handle, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
-                _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(groups), _lib.p_f32(ties), _lib.p_u32(mm),
-                len(queries), int(slop), self.avg_doc_length, similarity.k1, similarity.b, k, _lib.p_u32(docs),
-                _lib.p_f32(scores), ctypes.byref(n_redone)))
-        return docs, scores, n_redone.value
-
-    def _search_topk_nested(self, queries, k, similarity, slop, where=None):
-        """Boolean queries holding nested queries through sa_score_batch_topk_bool_nested: (docs, scores, queries
-        re-run exactly).  DisMax members anywhere in the trees need sparse-safe BM25 parameters (ValueError before any
-        device work)."""
-        from .query import check_dismax_members, dismax_members, flatten_nested
-        clauses, n_starts, c_node, mm, weights, occurs, groups, ties = flatten_nested(queries)
-        dev = self._device()
-        docs = np.empty((len(queries), k), dtype=np.uint32)
-        scores = np.empty((len(queries), k), dtype=np.float32)
-        n_redone = ctypes.c_uint32(0)
-        leaf = [i for i, c in enumerate(clauses) if c is not None]
-        terms, l_starts, l_idfs = self._topk_queries([clauses[i] for i in leaf],
-                                                     lambda dfs: compute_idf(self.corpus_size, dfs))
-        idfs, n_terms = np.zeros(len(clauses), dtype=np.float32), np.zeros(len(clauses), dtype=np.int64)
-        idfs[leaf] = l_idfs
-        n_terms[leaf] = np.diff(l_starts)
-        c_starts = np.concatenate([[0], np.cumsum(n_terms)]).astype(np.uint32)   # nested clauses: no terms
-        check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
-                             lambda i: (similarity.k1, similarity.b, self.avg_doc_length, idfs[i]))
-        with self._shared["lock"]:
-            self._apply_rows(dev)
-            if where is not None:
-                self._bool_where(dev, len(n_starts) - 1, n_starts, c_node, terms, c_starts, idfs, weights, occurs,
-                                 groups, ties, mm, len(queries), slop, similarity, k, docs, scores, n_redone, where)
-                return docs, scores, n_redone.value
-            _lib.check(_lib.lib().sa_score_batch_topk_bool_nested(
-                dev.handle, len(n_starts) - 1, _lib.p_u32(n_starts), _lib.p_u32(c_node), _lib.p_u32(terms),
-                _lib.p_u32(c_starts), _lib.p_f32(idfs), _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(groups),
-                _lib.p_f32(ties), _lib.p_u32(mm), len(queries), int(slop), self.avg_doc_length, similarity.k1,
-                similarity.b, k, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
+        _lib.check(_lib.lib().sa_score_batch_topk_bool(
+            dev.handle, len(batch.node_starts) - 1, _lib.p_u32(batch.node_starts), opt(batch.clause_node, _lib.p_u32),
+            _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs), opt(batch.weights, _lib.p_f32),
+            opt(batch.occurs, _lib.p_u8), opt(batch.groups, _lib.p_u32), opt(batch.ties, _lib.p_f32),
+            _lib.p_u32(batch.mm), batch.n_queries, int(slop), self.avg_doc_length, similarity.k1, similarity.b, k,
+            p_w, len(self), stride, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
         return docs, scores, n_redone.value
 
     def _search_topk_bool(self, queries, k, similarity, slop, where=None):
-        """Boolean queries through sa_score_batch_topk_bool, or through sa_score_batch_topk_bool_occur when one of
-        them is a Bool or has a weight other than 1: (docs, scores, queries re-run exactly).  where: a packed mask
-        (pack_where), through sa_score_batch_topk_bool_where."""
-        from .query import flatten, flatten_occur, needs_occur
-        occur = any(needs_occur(q) for q in queries)
-        if occur:
-            clauses, q_starts, mm, weights, occurs = flatten_occur(queries)
-        else:
-            clauses, q_starts, mm = flatten(queries)
+        """Boolean queries of any form through sa_score_batch_topk_bool, flattened for the heaviest form among them
+        (query.bool_form, flatten_bool): (docs, scores, queries re-run exactly).  DisMax members anywhere in the trees
+        need sparse-safe BM25 parameters (ValueError before any device work).  where: a packed mask (pack_where)."""
+        from .query import DISMAX, OR_AND, bool_form, check_dismax_members, dismax_members, flatten_bool
+        form = max(map(bool_form, queries), default=OR_AND)
+        batch = flatten_bool(queries, form)
+        clauses = batch.clauses
+        idf = lambda dfs: compute_idf(self.corpus_size, dfs)      # noqa: E731
+        if batch.clause_node is None:
+            terms, c_starts, idfs = self._topk_queries(clauses, idf)
+            idfs = np.asarray(idfs, dtype=np.float32)
+        else:                                           # nested clauses (None): no terms, idf 0
+            leaf = [i for i, c in enumerate(clauses) if c is not None]
+            terms, l_starts, l_idfs = self._topk_queries([clauses[i] for i in leaf], idf)
+            idfs, n_terms = np.zeros(len(clauses), dtype=np.float32), np.zeros(len(clauses), dtype=np.int64)
+            idfs[leaf] = l_idfs
+            n_terms[leaf] = np.diff(l_starts)
+            c_starts = np.concatenate([[0], np.cumsum(n_terms)]).astype(np.uint32)
+        if form >= DISMAX:
+            check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
+                                 lambda i: (similarity.k1, similarity.b, self.avg_doc_length, idfs[i]))
         dev = self._device()
-        docs = np.empty((len(queries), k), dtype=np.uint32)
-        scores = np.empty((len(queries), k), dtype=np.float32)
-        n_redone = ctypes.c_uint32(0)
-        terms, c_starts, idfs = self._topk_queries(clauses, lambda dfs: compute_idf(self.corpus_size, dfs))
-        idfs = np.asarray(idfs, dtype=np.float32)
         with self._shared["lock"]:
             self._apply_rows(dev)
-            if where is not None:
-                self._bool_where(dev, len(queries), q_starts, None, terms, c_starts, idfs, weights if occur else None,
-                                 occurs if occur else None, None, None, mm, len(queries), slop, similarity, k, docs,
-                                 scores, n_redone, where)
-            elif occur:
-                _lib.check(_lib.lib().sa_score_batch_topk_bool_occur(
-                    dev.handle, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
-                    _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(mm), len(queries), int(slop),
-                    self.avg_doc_length, similarity.k1, similarity.b, k, _lib.p_u32(docs), _lib.p_f32(scores),
-                    ctypes.byref(n_redone)))
-            else:
-                _lib.check(_lib.lib().sa_score_batch_topk_bool(
-                    dev.handle, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
-                    _lib.p_u32(mm), len(queries), int(slop), self.avg_doc_length, similarity.k1, similarity.b, k,
-                    _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
-        return docs, scores, n_redone.value
+            return self._bool_call(dev, batch, terms, c_starts, idfs, similarity, slop, k, where)
 
     def _topk_queries(self, queries, idf):
         """The queries as the batched top-k entries take them: term ids, start offsets and, per query, idf(dfs) of
@@ -796,7 +729,7 @@ class SearchArray(ExtensionArray):
         """search_topk on a view, and under bm25_impact, bm25_legacy_similarity or classic_similarity on any array
         (sa_score_batch_topk_sim): the counts, document frequencies, doc lengths, avgdl and corpus size .score
         uses, with the idf computed here, on the host, from the same dfs.  where: a packed mask over the positions
-        (pack_where), through sa_score_batch_topk_sim_where."""
+        (pack_where)."""
         if self.rows is not None and (self.comm is not None or self.global_df is not None):
             raise ValueError("search_topk on a view of a sharded SearchArray is not supported: the slice's document "
                              "frequencies would need a sum over the ranks; use .score() on the view")
@@ -816,16 +749,10 @@ class SearchArray(ExtensionArray):
             docs = np.full((len(idfs), k), _lib.NO_DOC, dtype=np.uint32)
             scores = np.zeros((len(idfs), k), dtype=np.float64)
             dbl = ctypes.POINTER(ctypes.c_double)
-            if where is not None:
-                p_w, stride = _where_args(where)
-                _lib.check(_lib.lib().sa_score_batch_topk_sim_where(
-                    dev.handle, similarity.kind, _lib.p_u32(terms), _lib.p_u32(starts), idfs.ctypes.data_as(dbl),
-                    len(idfs), int(slop), None if dl is None else _lib.p_f32(dl), float(self.avg_doc_length),
-                    float(similarity.k1), float(similarity.b), k, p_w, len(self), stride, _lib.p_u32(docs),
-                    scores.ctypes.data_as(dbl)))
-            else:
-                _lib.check(_lib.lib().sa_score_batch_topk_sim(
-                    dev.handle, similarity.kind, _lib.p_u32(terms), _lib.p_u32(starts), idfs.ctypes.data_as(dbl),
-                    len(idfs), int(slop), None if dl is None else _lib.p_f32(dl), float(self.avg_doc_length),
-                    float(similarity.k1), float(similarity.b), k, _lib.p_u32(docs), scores.ctypes.data_as(dbl)))
+            p_w, stride = _where_args(where)
+            _lib.check(_lib.lib().sa_score_batch_topk_sim(
+                dev.handle, similarity.kind, _lib.p_u32(terms), _lib.p_u32(starts), idfs.ctypes.data_as(dbl),
+                len(idfs), int(slop), None if dl is None else _lib.p_f32(dl), float(self.avg_doc_length),
+                float(similarity.k1), float(similarity.b), k, p_w, len(self), stride, _lib.p_u32(docs),
+                scores.ctypes.data_as(dbl)))
         return docs, scores.astype(similarity.out_dtype, copy=False)

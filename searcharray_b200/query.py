@@ -5,14 +5,13 @@ Or(clauses, mm) ranks, per doc, s = score(c0) + score(c1) + ... (float32, folded
 where at least mm clauses score > 0 -- the reference's own composition of multi-clause queries
 (test/test_search.py:126-226) -- and search_topk returns the top k of it by (score desc, doc asc), computed on the
 device (sa_score_batch_topk_bool).  Bool(must, should, filter, must_not, mm) and Boost(clause, weight) extend that
-composition (sa_score_batch_topk_bool_occur).  Field(field, clause) names the DataFrame column a clause scores on,
-for queries over several columns (solr.fields_topk, sa_multi_score_batch_topk_bool).  DisMax(clauses, tie) is one
-clause scored by its best member plus tie times the others (Lucene's DisjunctionMaxQuery;
-sa_score_batch_topk_bool_dismax, sa_multi_score_batch_topk_bool_dismax).  An Or / And / Bool may itself be a clause of
-another (a nested query, scored by what it ranks as a query of its own; sa_score_batch_topk_bool_nested,
-sa_multi_score_batch_topk_bool_nested)."""
+composition.  Field(field, clause) names the DataFrame column a clause scores on, for queries over several columns
+(solr.fields_topk, sa_multi_score_batch_topk_bool).  DisMax(clauses, tie) is one clause scored by its best member
+plus tie times the others (Lucene's DisjunctionMaxQuery).  An Or / And / Bool may itself be a clause of another (a
+nested query, scored by what it ranks as a query of its own).  The device entry points take the queries flattened
+for their form (bool_form, flatten_bool)."""
 import math
-from typing import List, Union
+from typing import List, NamedTuple, Optional, Union
 
 import numpy as np
 
@@ -180,10 +179,11 @@ class Or:
         _check_nodes(self.n_nested)
         self.clauses, self.weights = _scoring(clauses)
         self.mm = parse_min_should_match(len(self.clauses), str(mm))
+        self.form = _form(self.clauses, self.boosted)       # bool_form
 
     @property
     def boosted(self):
-        """Whether any clause has a weight other than 1 (such a query takes sa_score_batch_topk_bool_occur)."""
+        """Whether any clause has a weight other than 1 (such a query takes the OCCUR form)."""
         return any(w != 1.0 for w in self.weights)
 
     def __repr__(self):
@@ -232,6 +232,7 @@ class Bool:
         if mm is None:
             mm = 0 if (self.must or self.filter) else 1
         self.mm = parse_min_should_match(len(self.should), str(mm))
+        self.form = _form(self.must + self.should + self.filter + self.must_not, True)   # bool_form
 
     def occur_clauses(self):
         """(clauses, float32 weights, occurs) in the order the device folds them: must, should, filter, must_not."""
@@ -281,84 +282,55 @@ def has_field(q):
 
 
 def has_dismax(q):
-    """Whether q is or holds a DisMax (sa_score_batch_topk_bool_dismax's form), nested queries included."""
+    """Whether q is or holds a DisMax (the DISMAX form), nested queries included."""
     return any(isinstance(c, DisMax) for c in _leaves(q))
 
 
 def is_nested(q):
-    """Whether a boolean query holds a nested Or / And / Bool (sa_score_batch_topk_bool_nested's form)."""
+    """Whether a boolean query holds a nested Or / And / Bool (the NESTED form)."""
     return not isinstance(q, DisMax) and any(isinstance(c, (Or, Bool)) for c in _top_clauses(q))
 
 
 def needs_occur(q):
-    """Whether q takes sa_score_batch_topk_bool_occur: a Bool, or an Or / And with a weight other than 1."""
+    """Whether q takes at least the OCCUR form: a Bool, or an Or / And with a weight other than 1."""
     return isinstance(q, Bool) or q.boosted
 
 
-def flatten(queries):
-    """Boolean queries as sa_score_batch_topk_bool takes them: (clause list in query order, query_clause_starts,
-    mm), the clause list being search_topk's query form (str or list[str])."""
-    clauses, starts, mm = [], [0], []
-    for q in queries:
-        clauses.extend(q.clauses)
-        starts.append(len(clauses))
-        mm.append(q.mm)
-    return clauses, np.asarray(starts, dtype=np.uint32), np.asarray(mm, dtype=np.uint32)
+# The forms of a boolean batch, ordered: each form's arrays are those of the one before plus its own, and the C entry
+# points run the instance the non-NULL arrays select.
+OR_AND, OCCUR, DISMAX, NESTED = 1, 2, 3, 4
 
 
-def flatten_occur(queries):
-    """Or / And / Bool queries as sa_score_batch_topk_bool_occur takes them: flatten's (clauses,
-    query_clause_starts, mm) and, per clause, float32 weights and uint8 SA_OCCUR_* roles.  An Or's clauses are all
-    SHOULD; a Bool's come as must, should, filter, must_not."""
-    clauses, starts, mm, weights, occurs = [], [0], [], [], []
-    for q in queries:
-        if isinstance(q, Bool):
-            cs, ws, os_ = q.occur_clauses()
-        else:
-            cs, ws, os_ = q.clauses, q.weights, [SA_OCCUR_SHOULD] * len(q.clauses)
-        clauses.extend(cs)
-        weights.extend(ws)
-        occurs.extend(os_)
-        starts.append(len(clauses))
-        mm.append(q.mm)
-    return (clauses, np.asarray(starts, dtype=np.uint32), np.asarray(mm, dtype=np.uint32),
-            np.asarray(weights, dtype=np.float32), np.asarray(occurs, dtype=np.uint8))
+def bool_form(q):
+    """The form a boolean query takes: NESTED if it holds a nested Or / And / Bool, else DISMAX if it is or holds a
+    DisMax, else OCCUR if it is a Bool or has a weight other than 1, else OR_AND."""
+    return DISMAX if isinstance(q, DisMax) else q.form
 
 
-def flatten_dismax(queries):
-    """Or / And / Bool / DisMax queries as sa_score_batch_topk_bool_dismax takes them: flatten_occur's arrays, with
-    each DisMax expanded into its members (their own weights, the DisMax's role), and per clause uint32 clause_group
-    (the batch-wide index of the first clause of its group; the clause itself outside a DisMax) and float32
-    clause_tie (the group's tie; 0 outside a DisMax).  A top-level DisMax is Bool(should=[it])."""
-    clauses, starts, mm, weights, occurs, groups, ties = [], [0], [], [], [], [], []
-    for q in queries:
-        if isinstance(q, DisMax):
-            cs, ws, os_, qmm = [q], [np.float32(1.0)], [SA_OCCUR_SHOULD], 1
-        elif isinstance(q, Bool):
-            cs, ws, os_ = q.occur_clauses()
-            qmm = q.mm
-        else:
-            cs, ws, os_, qmm = q.clauses, q.weights, [SA_OCCUR_SHOULD] * len(q.clauses), q.mm
-        for c, w, o in zip(cs, ws, os_):
-            first = len(clauses)
-            if isinstance(c, DisMax):
-                for m, mw in zip(c.clauses, c.weights):
-                    clauses.append(m)
-                    weights.append(mw)
-                    occurs.append(o)
-                    groups.append(first)
-                    ties.append(c.tie)
-            else:
-                clauses.append(c)
-                weights.append(w)
-                occurs.append(o)
-                groups.append(first)
-                ties.append(np.float32(0.0))
-        starts.append(len(clauses))
-        mm.append(qmm)
-    return (clauses, np.asarray(starts, dtype=np.uint32), np.asarray(mm, dtype=np.uint32),
-            np.asarray(weights, dtype=np.float32), np.asarray(occurs, dtype=np.uint8),
-            np.asarray(groups, dtype=np.uint32), np.asarray(ties, dtype=np.float32))
+def _form(clauses, occur):
+    """bool_form of an Or / And / Bool with these top-level clauses (Boosts removed); occur: it is a Bool or boosted.
+    Without a nested query, every DisMax of the tree is a top-level clause."""
+    form = OCCUR if occur else OR_AND
+    for c in clauses:
+        if isinstance(c, (Or, Bool)):
+            return NESTED
+        if isinstance(c, DisMax):
+            form = DISMAX
+    return form
+
+
+class BoolBatch(NamedTuple):
+    """Boolean queries as sa_score_batch_topk_bool takes them (flatten_bool).  Arrays the form does not use are None,
+    passed as NULL."""
+    clauses: list                   # per clause: search_topk's query form (str or list[str]); None for a nested clause
+    node_starts: np.ndarray         # uint32: node n's clauses are [node_starts[n], node_starts[n + 1])
+    clause_node: Optional[np.ndarray]   # uint32 per clause: its nested node, else SA_NO_NODE (NESTED)
+    mm: np.ndarray                  # uint32 per node
+    weights: Optional[np.ndarray]   # float32 per clause (OCCUR up)
+    occurs: Optional[np.ndarray]    # uint8 SA_OCCUR_* per clause (OCCUR up)
+    groups: Optional[np.ndarray]    # uint32 per clause: the batch-wide index of its group's first clause (DISMAX up)
+    ties: Optional[np.ndarray]      # float32 per clause: its group's tie, 0 outside a DisMax (DISMAX up)
+    n_queries: int                  # the top-level queries: nodes 0 .. n_queries - 1
 
 
 def _node_parts(q):
@@ -373,7 +345,7 @@ def _node_parts(q):
 
 
 def _nodes(queries):
-    """The nodes of a batch in flatten_nested's order: the queries, then each query's nested queries in pre-order
+    """The nodes of a batch in flatten_bool's order: the queries, then each query's nested queries in pre-order
     (a sub-query object used twice is two nodes); and per node, the node indices of its nested clauses in order."""
     nodes, children = list(queries), [[] for _ in queries]
 
@@ -389,42 +361,66 @@ def _nodes(queries):
     return nodes, children
 
 
-def flatten_nested(queries):
-    """Boolean queries, nested ones included, as sa_score_batch_topk_bool_nested takes them: (clauses,
-    node_clause_starts, clause_node, mm, weights, occurs, groups, ties), every array per node or per clause as
-    flatten_dismax's per query or per clause.  Nodes 0 .. len(queries) - 1 are the queries, then each query's nested
-    queries in pre-order, so that every child comes after its parent.  A nested clause is None in `clauses`, with
-    clause_node its node (SA_NO_NODE for the others), its Boost's weight, its role and a group of its own."""
-    nodes, children = _nodes(queries)
-    clauses, starts, cnode, mm, weights, occurs, groups, ties = [], [0], [], [], [], [], [], []
+def flatten_bool(queries, form):
+    """Boolean queries as sa_score_batch_topk_bool takes them, for a form at least that of every query (bool_form):
+    a BoolBatch with only the arrays `form` reads, so a lighter form neither builds nor passes the others.
+
+    OR_AND: Or / And queries; clauses, node_starts (one node per query) and mm.  OCCUR adds per clause float32 weights
+    and uint8 SA_OCCUR_* roles: an Or's clauses all SHOULD, a Bool's as must, should, filter, must_not.  DISMAX expands
+    each DisMax into its members (their own weights, the DisMax's role) and adds per clause groups and ties; a top-level
+    DisMax is Bool(should=[it]).  NESTED adds the nested queries as nodes after the queries, each query's in pre-order
+    (every child after its parent), and clause_node: a nested clause is None in `clauses`, with its node, its Boost's
+    weight, its role and a group of its own.  A batch flattened for a heavier form than its own carries the lighter
+    form's arrays unchanged, plus self-groups, zero ties and SA_NO_NODE."""
+    queries = list(queries)
+    clauses, starts, mm = [], [0], []
+    if form == OR_AND:
+        for q in queries:
+            clauses.extend(q.clauses)
+            starts.append(len(clauses))
+            mm.append(q.mm)
+        return BoolBatch(clauses, _u32(starts), None, _u32(mm), None, None, None, None, len(queries))
+    nodes, children = _nodes(queries) if form == NESTED else (queries, None)
+    weights, occurs, cnode, groups, ties = [], [], [], [], []
+    zero = np.float32(0.0)
     for n, node in enumerate(nodes):
         cs, ws, os_, qmm = _node_parts(node)
-        kids = iter(children[n])
-        for c, w, o in zip(cs, ws, os_):
-            first = len(clauses)
-            if isinstance(c, (Or, Bool)):
-                members, tie, child = [(None, w)], np.float32(0.0), next(kids)
-            elif isinstance(c, DisMax):
-                members, tie, child = list(zip(c.clauses, c.weights)), c.tie, SA_NO_NODE
-            else:
-                members, tie, child = [(c, w)], np.float32(0.0), SA_NO_NODE
-            for m, mw in members:
-                clauses.append(m)
-                cnode.append(child)
-                weights.append(mw)
-                occurs.append(o)
-                groups.append(first)
-                ties.append(tie)
+        if form == OCCUR:
+            clauses.extend(cs)
+            weights.extend(ws)
+            occurs.extend(os_)
+        else:
+            kids = iter(children[n]) if children else None
+            for c, w, o in zip(cs, ws, os_):
+                first = len(clauses)
+                if isinstance(c, (Or, Bool)):
+                    members, tie, child = [(None, w)], zero, next(kids)
+                elif isinstance(c, DisMax):
+                    members, tie, child = list(zip(c.clauses, c.weights)), c.tie, SA_NO_NODE
+                else:
+                    members, tie, child = [(c, w)], zero, SA_NO_NODE
+                for m, mw in members:
+                    clauses.append(m)
+                    cnode.append(child)
+                    weights.append(mw)
+                    occurs.append(o)
+                    groups.append(first)
+                    ties.append(tie)
         starts.append(len(clauses))
         mm.append(qmm)
-    u32 = lambda x: np.asarray(x, dtype=np.uint32)      # noqa: E731
-    return (clauses, u32(starts), u32(cnode), u32(mm), np.asarray(weights, dtype=np.float32),
-            np.asarray(occurs, dtype=np.uint8), u32(groups), np.asarray(ties, dtype=np.float32))
+    dismax = form >= DISMAX
+    return BoolBatch(clauses, _u32(starts), _u32(cnode) if form == NESTED else None, _u32(mm),
+                     np.asarray(weights, dtype=np.float32), np.asarray(occurs, dtype=np.uint8),
+                     _u32(groups) if dismax else None, np.asarray(ties, dtype=np.float32) if dismax else None,
+                     len(queries))
+
+
+def _u32(x):
+    return np.asarray(x, dtype=np.uint32)
 
 
 def dismax_members(queries):
-    """Indices of the clauses that are DisMax members, into the clause list of flatten_nested (which is
-    flatten_dismax's for a batch without nested queries)."""
+    """Indices of the clauses that are DisMax members, into the clause list of flatten_bool for DISMAX or NESTED."""
     out, n = [], 0
     for q in _nodes(queries)[0]:
         for c in _top_clauses(q):

@@ -408,20 +408,16 @@ def edismax_topk(frame: pd.DataFrame, q: str, qf: List[str], k: int = 10, mm: Op
 
 
 def _fields_plan(frame, queries, similarity):
-    """fields_topk's refusals and field slots, before any device work: (flatten_occur's arrays, flatten_dismax's
-    when a query holds a DisMax, or flatten_nested's when one holds a nested query, field name -> slot, per-slot
+    """fields_topk's refusals and field slots, before any device work: (the batch flattened for its form, at least
+    OCCUR since the multi-field entry takes weights and roles (query.flatten_bool), field name -> slot, per-slot
     arrays, per-slot similarities)."""
-    from .query import ED_MAX_FIELDS, Field, flatten_dismax, flatten_nested, flatten_occur, has_dismax, is_boolean, \
-        is_nested
+    from .query import ED_MAX_FIELDS, OCCUR, Field, bool_form, flatten_bool, is_boolean
     queries = list(queries)
     for q in queries:
         if not is_boolean(q):
             raise TypeError(f"fields_topk takes Or / And / Bool / DisMax queries, not {q!r}")
-    if any(is_nested(q) for q in queries):
-        flat = flatten_nested(queries)
-    else:
-        flat = flatten_dismax(queries) if any(has_dismax(q) for q in queries) else flatten_occur(queries)
-    clauses = [c for c in flat[0] if c is not None]          # flatten_nested: None for a nested clause
+    batch = flatten_bool(queries, max([OCCUR] + [bool_form(q) for q in queries]))
+    clauses = [c for c in batch.clauses if c is not None]    # None: a nested clause
     for c in clauses:
         if not isinstance(c, Field):
             raise ValueError(f"every clause of fields_topk names its column: Field(field, {c!r})")
@@ -460,13 +456,13 @@ def _fields_plan(frame, queries, similarity):
         slot_arrays.append(a)
         slot_sims.append(sim)
         slot_name.append(f)
-    if len(flat) >= 7:                    # DisMax members: sparse-safe k1 / b on their fields (idf: _fields_clauses)
+    if batch.groups is not None:          # DisMax members: sparse-safe k1 / b on their fields (idf: _fields_clauses)
         from .query import check_dismax_members, dismax_members
-        clauses = flat[0]
+        clauses = batch.clauses
         check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
                              lambda i: (sims[clauses[i].field].k1, sims[clauses[i].field].b,
                                         arrays[clauses[i].field].avg_doc_length, 0.0))
-    return flat, slot_of, slot_arrays, slot_sims
+    return batch, slot_of, slot_arrays, slot_sims
 
 
 def _fields_clauses(clauses, slot_of, arrays):
@@ -486,52 +482,25 @@ def _fields_clauses(clauses, slot_of, arrays):
     return terms, c_starts, c_idf, _u32([0 if c is None else slot_of[c.field] for c in clauses])
 
 
-def _fields_call(multi, arrays, sims, flat, prepared, k, slop, where=None):
-    """sa_multi_score_batch_topk_bool, sa_multi_score_batch_topk_bool_dismax for flatten_dismax's arrays, or
-    sa_multi_score_batch_topk_bool_nested for flatten_nested's, on prepared arrays (the fields locked): (docs, scores,
-    queries re-run).  where: a packed mask (postings.pack_where), through sa_multi_score_batch_topk_bool_where."""
-    from .query import SA_NO_NODE
+def _fields_call(multi, arrays, sims, batch, prepared, k, slop, where=None):
+    """sa_multi_score_batch_topk_bool on a flattened batch (query.BoolBatch; its None arrays passed as NULL select the
+    instance) and prepared arrays (the fields locked): (docs, scores, queries re-run).  where: a packed mask
+    (postings.pack_where), None: no mask."""
     terms, c_starts, c_idf, c_field = prepared
     n_redone = ctypes.c_uint32(0)
     avgdl = _f32([a.avg_doc_length for a in arrays])
     k1, b = _f32([s.k1 for s in sims]), _f32([s.b for s in sims])
-    c_node = groups = ties = None
-    if len(flat) == 8:
-        n_starts, c_node, mm, weights, occurs, groups, ties = flat[1:]
-        nq = len(n_starts) - 1 - int(np.count_nonzero(c_node != SA_NO_NODE))   # each nested node: one reference
-    else:
-        n_starts, mm, weights, occurs = flat[1:5]
-        if len(flat) == 7:
-            groups, ties = flat[5:]
-        nq = len(n_starts) - 1
+    nq = batch.n_queries
     docs = np.empty((nq, k), dtype=np.uint32)
     scores = np.empty((nq, k), dtype=np.float32)
-    if where is not None:
-        p_w, stride = _where_args(where)
-        _lib.check(_lib.lib().sa_multi_score_batch_topk_bool_where(
-            multi.handle, len(n_starts) - 1, _lib.p_u32(n_starts), None if c_node is None else _lib.p_u32(c_node),
-            _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(c_idf), _lib.p_f32(weights),
-            _lib.p_u8(occurs), None if groups is None else _lib.p_u32(groups), None if ties is None else _lib.p_f32(ties),
-            _lib.p_u32(mm), nq, int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1), _lib.p_f32(b), k, p_w,
-            len(arrays[0]), stride, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
-    elif c_node is not None:
-        _lib.check(_lib.lib().sa_multi_score_batch_topk_bool_nested(
-            multi.handle, len(n_starts) - 1, _lib.p_u32(n_starts), _lib.p_u32(c_node), _lib.p_u32(c_field),
-            _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(c_idf), _lib.p_f32(weights), _lib.p_u8(occurs),
-            _lib.p_u32(groups), _lib.p_f32(ties), _lib.p_u32(mm), nq, int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1),
-            _lib.p_f32(b), k, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
-    elif groups is not None:
-        _lib.check(_lib.lib().sa_multi_score_batch_topk_bool_dismax(
-            multi.handle, _lib.p_u32(n_starts), _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts),
-            _lib.p_f32(c_idf), _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(groups), _lib.p_f32(ties),
-            _lib.p_u32(mm), nq, int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1), _lib.p_f32(b), k, _lib.p_u32(docs),
-            _lib.p_f32(scores), ctypes.byref(n_redone)))
-    else:
-        _lib.check(_lib.lib().sa_multi_score_batch_topk_bool(
-            multi.handle, _lib.p_u32(n_starts), _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts),
-            _lib.p_f32(c_idf), _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(mm), nq, int(slop),
-            _lib.p_f32(avgdl), _lib.p_f32(k1), _lib.p_f32(b), k, _lib.p_u32(docs), _lib.p_f32(scores),
-            ctypes.byref(n_redone)))
+    opt = lambda a, p: None if a is None else p(a)      # noqa: E731
+    p_w, stride = _where_args(where)
+    _lib.check(_lib.lib().sa_multi_score_batch_topk_bool(
+        multi.handle, len(batch.node_starts) - 1, _lib.p_u32(batch.node_starts), opt(batch.clause_node, _lib.p_u32),
+        _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(c_idf), _lib.p_f32(batch.weights),
+        _lib.p_u8(batch.occurs), opt(batch.groups, _lib.p_u32), opt(batch.ties, _lib.p_f32), _lib.p_u32(batch.mm), nq,
+        int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1), _lib.p_f32(b), k, p_w, len(arrays[0]), stride,
+        _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
     return docs, scores, n_redone.value
 
 
@@ -540,19 +509,19 @@ def _fields_topk(frame, queries, k, similarity, slop, where=None):
     queries = list(queries)
     if where is not None:
         where = pack_where(where, len(frame), len(queries))
-    flat, slot_of, arrays, sims = _fields_plan(frame, queries, similarity)
+    batch, slot_of, arrays, sims = _fields_plan(frame, queries, similarity)
     multi = _multi_for(arrays)
     with _locked(multi, arrays):
         for arr in arrays:                 # a sliced view of the same column may have left its row filter installed
             arr._apply_rows(arr._device())
-        prepared = _fields_clauses(flat[0], slot_of, arrays)
-        if len(flat) >= 7:                # DisMax members: sparse-safe idf from their own fields
+        prepared = _fields_clauses(batch.clauses, slot_of, arrays)
+        if batch.groups is not None:      # DisMax members: sparse-safe idf from their own fields
             from .query import check_dismax_members, dismax_members
-            clauses = flat[0]
+            clauses = batch.clauses
             check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
                                  lambda i: (sims[slot_of[clauses[i].field]].k1, sims[slot_of[clauses[i].field]].b,
                                             arrays[slot_of[clauses[i].field]].avg_doc_length, prepared[2][i]))
-        return _fields_call(multi, arrays, sims, flat, prepared, k, slop, where)
+        return _fields_call(multi, arrays, sims, batch, prepared, k, slop, where)
 
 
 def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
@@ -571,19 +540,18 @@ def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
     device work.
 
     A query.DisMax of Field members is one clause scoring d = max_j v_j + (sum_j v_j - max_j v_j) * tie over
-    v_j = w_j * score(member j), each member on its own column (sa_multi_score_batch_topk_bool_dismax): Elasticsearch's
+    v_j = w_j * score(member j), each member on its own column: Elasticsearch's
     best_fields as DisMax([Boost(Field("title", "alien"), 2), Field("overview", "alien")], tie=0.3), and edismax's
     term-centric qf as an Or of one such DisMax per term with a Solr mm.  Its members need k1 > 0 and 0 <= b < 1 on
     their fields (ValueError otherwise).
 
     An Or / And / Bool may be a clause of another, at any depth, as in SearchArray.search_topk: edismax's qf + pf as
-    Bool(must=[Or([DisMax(...), DisMax(...)], mm="75%")], should=[Boost(Field("title", ["a", "b"]), 3)])
-    (sa_multi_score_batch_topk_bool_nested).
+    Bool(must=[Or([DisMax(...), DisMax(...)], mm="75%")], should=[Boost(Field("title", ["a", "b"]), 3)]).
 
     where: a document filter, as in SearchArray.search_topk -- a boolean array-like (a boolean pd.Series too) of
     shape (len(frame),), one mask for the batch, or (len(queries), len(frame)), one per query.  Per query the
     result is the top k of np.where(mask_q, S_q, 0), S_q the composition above; the mask never changes a score
     (each column's idf, avgdl and doc lengths stay those of the whole column).  A dtype other than bool raises
-    TypeError and another shape ValueError, before any device work (sa_multi_score_batch_topk_bool_where)."""
+    TypeError and another shape ValueError, before any device work."""
     docs, scores, _ = _fields_topk(frame, queries, k, similarity, slop, where)
     return docs, scores

@@ -64,7 +64,9 @@ def test_flatten_to_field_slots():
     queries = [Or([Field("o", "a"), Boost(Field("t", ["a", "b"]), 2)], mm=2),
                Bool(must=[Field("t2", "b")], should=[Field("p", "c")], filter=[Field("o", "x")],
                     must_not=[Field("t", "c")], mm=1)]
-    (clauses, starts, mm, weights, occurs), slot_of, arrays, sims = _fields_plan(fr, queries, {})
+    batch, slot_of, arrays, sims = _fields_plan(fr, queries, {})
+    clauses, starts, mm, weights, occurs = batch.clauses, batch.node_starts, batch.mm, batch.weights, batch.occurs
+    assert batch.clause_node is None and batch.groups is None and batch.ties is None and batch.n_queries == 2
     assert [c.field for c in clauses] == ["o", "t", "t2", "p", "o", "t"]
     assert slot_of == {"o": 0, "t": 1, "t2": 1, "p": 2} and len(arrays) == 3 and len(sims) == 3
     assert arrays[1] is not None and arrays[1]._shared is fr["t2"].array._shared

@@ -1,5 +1,5 @@
-"""GPU: boolean queries over several DataFrame fields (solr.fields_topk, sa_multi_score_batch_topk_bool,
-bool_fields_tile_kernel in sa_bool.cu) against compose_occur with each clause scored by its own column's .score: ids
+"""GPU: boolean queries over several DataFrame fields (solr.fields_topk, sa_multi_score_batch_topk_bool, the FIELDS
+instance of bool_tile_kernel in sa_bool.cu) against compose_occur with each clause scored by its own column's .score: ids
 and float32 score bits must be equal.
 
 The synthetic frame spans five 8192-doc tiles and has fields that differ in vocabulary, doc lengths and avgdl:
@@ -357,9 +357,9 @@ def test_c_abi_validation(synth):
         avgdl = np.asarray(avgdl, dtype=np.float32)
         kk, bb = np.asarray(k1, dtype=np.float32), np.full(len(k1), 0.75, dtype=np.float32)
         return _lib.lib().sa_multi_score_batch_topk_bool(
-            multi.handle, _lib.p_u32(q_starts), _lib.p_u32(f), _lib.p_u32(t), _lib.p_u32(c_starts), _lib.p_f32(ones),
-            _lib.p_f32(ones), _lib.p_u8(occ), _lib.p_u32(mm), 1, 0, _lib.p_f32(avgdl), _lib.p_f32(kk), _lib.p_f32(bb),
-            10, _lib.p_u32(docs), _lib.p_f32(scores), None)
+            multi.handle, 1, _lib.p_u32(q_starts), None, _lib.p_u32(f), _lib.p_u32(t), _lib.p_u32(c_starts),
+            _lib.p_f32(ones), _lib.p_f32(ones), _lib.p_u8(occ), None, None, _lib.p_u32(mm), 1, 0, _lib.p_f32(avgdl),
+            _lib.p_f32(kk), _lib.p_f32(bb), 10, None, 0, 0, _lib.p_u32(docs), _lib.p_f32(scores), None)
     m, ab = _Multi([a, b]), (a.avg_doc_length, b.avg_doc_length)
     assert call(m, [0, 1], [ta["w0"], tb["b1"]], ab) == 0
     assert call(m, [0, 2], [ta["w0"], tb["b1"]], ab) != 0                 # no field slot 2
@@ -369,6 +369,71 @@ def test_c_abi_validation(synth):
     assert call(same, [0, 1], [ta["w0"], ta["w1"]], aa, k1=(1.2, 2.0)) != 0
     assert call(same, [0, 1], [ta["w0"], ta["w1"]], ab) != 0
     assert b"share an index" in _lib.lib().sa_last_error()
+
+
+def test_c_abi_pairings(synth):
+    """The nullable arrays alone select the form, so a pairing no form takes is SA_ERR_ARG before any device work:
+    weights without roles, groups without ties or without roles, clause_node without groups, n_nodes != n_queries
+    without clause_node, and on the multi-field entry NULL weights or roles.  The same call with the pairing
+    completed runs."""
+    from searcharray_b200 import _lib
+    from searcharray_b200.solr import _Multi
+    a, b = synth.frame[A].array, synth.frame[B].array
+    ta, tb = a.host.term_dict.term_to_ids, b.host.term_dict.term_to_ids
+    docs = np.empty(10, dtype=np.uint32)
+    scores = np.empty(10, dtype=np.float32)
+    n_starts = np.asarray([0, 2], dtype=np.uint32)
+    c_starts = np.arange(3, dtype=np.uint32)
+    ones = np.ones(2, dtype=np.float32)
+    occ = np.zeros(2, dtype=np.uint8)
+    groups = np.arange(2, dtype=np.uint32)
+    ties = np.zeros(2, dtype=np.float32)
+    nodes = np.full(2, 0xFFFFFFFF, dtype=np.uint32)
+    mm = np.asarray([1], dtype=np.uint32)
+    opt = lambda x, p: None if x is None else p(x)      # noqa: E731
+
+    def single(w, o, g, t, node, n_nodes=1):
+        terms = np.asarray([ta["w0"], ta["w1"]], dtype=np.uint32)
+        return _lib.lib().sa_score_batch_topk_bool(
+            a._device().handle, n_nodes, _lib.p_u32(n_starts), opt(node, _lib.p_u32), _lib.p_u32(terms),
+            _lib.p_u32(c_starts), _lib.p_f32(ones), opt(w, _lib.p_f32), opt(o, _lib.p_u8), opt(g, _lib.p_u32),
+            opt(t, _lib.p_f32), _lib.p_u32(mm), 1, 0, a.avg_doc_length, 1.2, 0.75, 10, None, 0, 0, _lib.p_u32(docs),
+            _lib.p_f32(scores), None)
+    assert single(None, None, None, None, None) == 0
+    assert single(ones, occ, None, None, None) == 0
+    assert single(ones, occ, groups, ties, None) == 0
+    assert single(ones, occ, groups, ties, nodes) == 0
+    assert single(ones, None, None, None, None) == 2                          # weights without roles
+    assert b"clause_weight and clause_occur" in _lib.lib().sa_last_error()
+    assert single(None, occ, None, None, None) == 2
+    assert single(ones, occ, groups, None, None) == 2                         # groups without ties
+    assert b"clause_group and clause_tie" in _lib.lib().sa_last_error()
+    assert single(None, None, groups, ties, None) == 2                        # groups without roles
+    assert b"clause_group and clause_tie" in _lib.lib().sa_last_error()
+    assert single(ones, occ, None, None, nodes) == 2                          # clause_node without groups
+    assert b"clause_node needs the DisMax arrays" in _lib.lib().sa_last_error()
+    assert single(ones, occ, groups, ties, None, n_nodes=2) == 2              # n_nodes != n_queries without clause_node
+    assert b"n_nodes == n_queries" in _lib.lib().sa_last_error()
+
+    def multi(w, o, g=None, t=None):
+        f = np.asarray([0, 1], dtype=np.uint32)
+        terms = np.asarray([ta["w0"], tb["b1"]], dtype=np.uint32)
+        avgdl = np.asarray([a.avg_doc_length, b.avg_doc_length], dtype=np.float32)
+        kk, bb = np.full(2, 1.2, dtype=np.float32), np.full(2, 0.75, dtype=np.float32)
+        return _lib.lib().sa_multi_score_batch_topk_bool(
+            mh.handle, 1, _lib.p_u32(n_starts), None, _lib.p_u32(f), _lib.p_u32(terms), _lib.p_u32(c_starts),
+            _lib.p_f32(ones), opt(w, _lib.p_f32), opt(o, _lib.p_u8), opt(g, _lib.p_u32), opt(t, _lib.p_f32),
+            _lib.p_u32(mm), 1, 0, _lib.p_f32(avgdl), _lib.p_f32(kk), _lib.p_f32(bb), 10, None, 0, 0,
+            _lib.p_u32(docs), _lib.p_f32(scores), None)
+    mh = _Multi([a, b])
+    assert multi(ones, occ) == 0
+    assert multi(ones, occ, groups, ties) == 0
+    assert multi(None, occ) == 2                                              # NULL weights
+    assert b"NULL argument" in _lib.lib().sa_last_error()
+    assert multi(ones, None) == 2                                             # NULL roles
+    assert multi(None, None) == 2
+    assert multi(ones, occ, groups, None) == 2
+    assert b"clause_group and clause_tie" in _lib.lib().sa_last_error()
 
 
 def test_launches_one_tile_launch_per_group(synth):

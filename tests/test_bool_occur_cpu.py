@@ -1,5 +1,5 @@
 """CPU: Bool (must / should / filter / must_not) and Boost in search_topk (searcharray_b200/query.py) --
-validation, mm defaults, the clause limit, flattening into sa_score_batch_topk_bool_occur's arrays -- and the oracle
+validation, mm defaults, the clause limit, flattening into the OCCUR arrays -- and the oracle
 composition against the real reference's composed results (tests/golden/bool_occur.json,
 make_golden_bool_occur.py)."""
 import json
@@ -79,19 +79,24 @@ def test_bool_validation_and_mm():
 
 def test_flatten_occur():
     from searcharray_b200 import And, Bool, Boost, Or
-    from searcharray_b200.query import flatten, flatten_occur
+    from searcharray_b200.query import OCCUR, OR_AND, flatten_bool
     queries = [Or(["a", Boost(["b", "c"], 2)], mm=2), And(["d"]),
                Bool(must=[Boost("m", 0.5)], should=["s", "t"], filter=[["f", "g"]], must_not=["n"], mm=1),
                Bool(must_not=["x"], should=[Boost("y", 3)])]
-    clauses, starts, mm, weights, occurs = flatten_occur(queries)
+    clauses, starts, _, mm, weights, occurs, _, _, _ = flatten_bool(queries, OCCUR)
     assert clauses == ["a", ["b", "c"], "d", "m", "s", "t", ["f", "g"], "n", "y", "x"]
     assert starts.dtype == np.uint32 and starts.tolist() == [0, 2, 3, 8, 10]
     assert mm.dtype == np.uint32 and mm.tolist() == [2, 1, 1, 1]
     assert weights.dtype == np.float32 and weights.tolist() == [1, 2, 1, 0.5, 1, 1, 1, 1, 3, 1]
     assert occurs.dtype == np.uint8 and occurs.tolist() == [0, 0, 0, 1, 0, 0, 2, 3, 0, 3]
     # the plain flatten of unboosted Or / And is what it was; a boosted Or flattens to its clauses
-    c, s, m = flatten([Or(["a", ["b", "c"]], mm=2), And(["d"]), Or(["a", Boost("e", 2)], mm=0)])
+    c, s, _, m, *_ = flatten_bool([Or(["a", ["b", "c"]], mm=2), And(["d"]), Or(["a", Boost("e", 2)], mm=0)], OR_AND)
     assert c == ["a", ["b", "c"], "d", "a", "e"] and s.tolist() == [0, 2, 3, 5] and m.tolist() == [2, 1, 0]
+    # an Or / And batch flattened for OCCUR: the same arrays, every clause SHOULD with weight 1
+    plain = [Or(["a", ["b", "c"]], mm=2), And(["d"])]
+    lo, hi = flatten_bool(plain, OR_AND), flatten_bool(plain, OCCUR)
+    assert hi.clauses == lo.clauses and np.array_equal(hi.node_starts, lo.node_starts)
+    assert np.array_equal(hi.mm, lo.mm) and hi.weights.tolist() == [1, 1, 1] and hi.occurs.tolist() == [0, 0, 0]
 
 
 def test_rejected_without_a_device():

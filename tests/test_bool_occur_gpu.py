@@ -1,5 +1,5 @@
-"""GPU: Bool (must / should / filter / must_not) and Boost in search_topk (sa_score_batch_topk_bool_occur,
-bool_tile_kernel<true> in sa_bool.cu) against the composition of tests/_bool_occur_compose.py: ids and float32 score
+"""GPU: Bool (must / should / filter / must_not) and Boost in search_topk (sa_score_batch_topk_bool with weights and
+roles, the OCCUR instances of bool_tile_kernel in sa_bool.cu) against the composition of tests/_bool_occur_compose.py: ids and float32 score
 bits must be equal.
 
 The corpus is test_bool_topk_gpu.py's synthetic five-tile corpus: `w0` / `w1` / `w2` have a tile directory and a tf
@@ -166,9 +166,10 @@ def test_mixed_batch(synth):
 
 
 def test_unit_weights_take_the_or_path(synth, monkeypatch):
-    """An Or / And whose weights are all 1.0 gives the unboosted query's bits, through sa_score_batch_topk_bool;
-    a Bool with only SHOULD clauses of weight 1 gives the same bits through the new entry point."""
-    from searcharray_b200 import And, Bool, Boost, Or, query
+    """An Or / And whose weights are all 1.0 gives the unboosted query's bits, through the Or / And instance (NULL
+    weights and roles); a Bool with only SHOULD clauses of weight 1 gives the same bits through the occur instance."""
+    from searcharray_b200 import And, Bool, Boost, Or
+    from searcharray_b200.query import OR_AND, bool_form
     arr = synth.arr
     plain = [Or(["w0", ["pa", "pb"], "s1"], mm=2), And(["w1", "w2"]), Or(["t0", "w0", "t3"])]
     unit = [Or([Boost("w0", 1), ["pa", "pb"], Boost("s1", 1.0)], mm=2), And([Boost("w1", 1), Boost("w2", 1)]),
@@ -177,9 +178,16 @@ def test_unit_weights_take_the_or_path(synth, monkeypatch):
     for k in (1, 10, 32):
         wd, ws = arr.search_topk(plain, k=k)
         bd, bs = arr.search_topk(as_bool, k=k)
+        assert [bool_form(q) for q in unit] == [OR_AND] * len(unit)
+        seen, real = [], type(arr)._bool_call
+
+        def spy(self, dev, batch, *a):
+            seen.append((batch.weights, batch.occurs))
+            return real(self, dev, batch, *a)
         with monkeypatch.context() as m:
-            m.setattr(query, "flatten_occur", lambda *a: pytest.fail("unit weights took the occur entry point"))
+            m.setattr(type(arr), "_bool_call", spy)
             gd, gs = arr.search_topk(unit, k=k)
+        assert seen == [(None, None)], "unit weights took the occur instance"
         assert np.array_equal(gd, wd) and np.array_equal(gs.view(np.uint32), ws.view(np.uint32))
         assert np.array_equal(bd, wd) and np.array_equal(bs.view(np.uint32), ws.view(np.uint32))
 
@@ -218,10 +226,10 @@ def test_c_abi_validation(synth):
         w = np.asarray(weights, dtype=np.float32)
         o = np.asarray(occurs, dtype=np.uint8)
         m = np.asarray([mm], dtype=np.uint32)
-        return _lib.lib().sa_score_batch_topk_bool_occur(
-            h, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idf), _lib.p_f32(w),
-            _lib.p_u8(o), _lib.p_u32(m), 1, 0, arr.avg_doc_length, 1.2, 0.75, 10, _lib.p_u32(docs),
-            _lib.p_f32(scores), None)
+        return _lib.lib().sa_score_batch_topk_bool(
+            h, 1, _lib.p_u32(q_starts), None, _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idf), _lib.p_f32(w),
+            _lib.p_u8(o), None, None, _lib.p_u32(m), 1, 0, arr.avg_doc_length, 1.2, 0.75, 10, None, 0, 0,
+            _lib.p_u32(docs), _lib.p_f32(scores), None)
     assert call([1, 1], [1, 0], 1) == 0
     assert call([1, 1], [1, 0], 2) != 0                       # one SHOULD clause
     assert call([1, 1], [1, 4], 0) != 0

@@ -50,11 +50,33 @@ def test_mm_parsing(mm, n, want):
 
 def test_flatten():
     from searcharray_b200 import And, Or
-    from searcharray_b200.query import flatten
-    clauses, starts, mm = flatten([Or(["a", ["b", "c"]], mm=2), And(["d"]), Or(["a", "a", "e"], mm=0)])
+    from searcharray_b200.query import OR_AND, flatten_bool
+    clauses, starts, _, mm, *_ = flatten_bool([Or(["a", ["b", "c"]], mm=2), And(["d"]), Or(["a", "a", "e"], mm=0)],
+                                             OR_AND)
     assert clauses == ["a", ["b", "c"], "d", "a", "a", "e"]
     assert starts.dtype == np.uint32 and starts.tolist() == [0, 2, 3, 6]
     assert mm.dtype == np.uint32 and mm.tolist() == [2, 1, 0]
+
+
+def test_bool_form_and_the_arrays_each_form_leaves_none():
+    """bool_form orders the query kinds OR_AND < OCCUR < DISMAX < NESTED, and flatten_bool builds only the arrays the
+    form reads: the others are None, passed as NULL, which selects that form's instance."""
+    from searcharray_b200 import And, Bool, Boost, DisMax, Or
+    from searcharray_b200.query import DISMAX, NESTED, OCCUR, OR_AND, bool_form, flatten_bool
+    assert OR_AND < OCCUR < DISMAX < NESTED
+    kinds = {OR_AND: [Or(["a", "b"]), And(["a", ["b", "c"]]), Or(["a", Boost("b", 1.0)])],
+             OCCUR: [Or(["a", Boost("b", 2)]), Bool(must=["a"]), Bool(should=["a"], must_not=["b"])],
+             DISMAX: [DisMax(["a", "b"]), Or(["a", DisMax(["b"])]), Bool(filter=[DisMax(["a", "b"])], should=["c"])],
+             NESTED: [Or(["a", And(["b", "c"])]), Bool(must=[Boost(Or(["a"]), 2)]),
+                      Or([DisMax(["a", "b"]), Bool(should=["c"])])]}
+    for form, qs in kinds.items():
+        assert [bool_form(q) for q in qs] == [form] * len(qs), form
+    for form, qs in kinds.items():
+        b = flatten_bool(qs, form)
+        assert b.n_queries == len(qs) and b.node_starts is not None and b.mm is not None
+        assert (b.weights is None, b.occurs is None) == ((form == OR_AND,) * 2)
+        assert (b.groups is None, b.ties is None) == ((form < DISMAX,) * 2)
+        assert (b.clause_node is None) == (form < NESTED)
 
 
 def test_rejected_without_a_device():

@@ -82,14 +82,15 @@ def test_dismax_validation():
 def test_flatten_groups_and_ties():
     from searcharray_b200 import Bool, Boost, DisMax, Field, Or
     from searcharray_b200.query import (SA_OCCUR_FILTER, SA_OCCUR_MUST, SA_OCCUR_MUST_NOT, SA_OCCUR_SHOULD,
-                                        dismax_members, flatten, flatten_dismax, flatten_occur, has_dismax, has_field,
+                                        DISMAX, OCCUR, OR_AND, dismax_members, flatten_bool, has_dismax, has_field,
                                         is_boolean)
     qs = [Or(["a", DisMax(["b", Boost("c", 2)], tie=0.25)], mm=2),
           Bool(must=[DisMax([["p", "q"], "r"], tie=1)], should=["s", DisMax(["t"], tie=0.5)],
                filter=[DisMax(["u", "v"])], must_not=["w", DisMax(["x", "y", "z"], tie=0.1)]),
           DisMax(["m", Boost("n", 3)], tie=0.3),
           Bool(must=["plain"], should=[Boost("k", 2)])]
-    clauses, starts, mm, weights, occurs, groups, ties = flatten_dismax(qs)
+    clauses, starts, cnode, mm, weights, occurs, groups, ties, nq = flatten_bool(qs, DISMAX)
+    assert cnode is None and nq == 4
     assert clauses == ["a", "b", "c", ["p", "q"], "r", "s", "t", "u", "v", "w", "x", "y", "z", "m", "n", "plain", "k"]
     assert starts.tolist() == [0, 3, 13, 15, 17] and starts.dtype == np.uint32
     assert mm.tolist() == [2, 0, 1, 0]
@@ -102,12 +103,14 @@ def test_flatten_groups_and_ties():
                              np.float32(.3), np.float32(.3), 0, 0]
     assert dismax_members(qs) == [1, 2, 3, 4, 6, 7, 8, 10, 11, 12, 13, 14]
     assert [has_dismax(q) for q in qs] == [True, True, True, False] and all(is_boolean(q) for q in qs)
-    # queries without a DisMax: flatten_dismax is flatten_occur plus plain groups; flatten / flatten_occur unchanged
+    # queries without a DisMax: flattened for DISMAX, the OCCUR arrays plus plain groups; OR_AND / OCCUR unchanged
     plain = [Or(["a", "b"]), Bool(must=["c"], should=[Boost("d", 2)], must_not=["e"])]
-    got, want = flatten_dismax(plain), flatten_occur(plain)
-    assert got[0] == want[0] and all(np.array_equal(x, y) for x, y in zip(got[1:5], want[1:]))
-    assert got[5].tolist() == [0, 1, 2, 3, 4] and not got[6].any()
-    assert flatten(plain[:1])[0] == ["a", "b"]
+    got, want = flatten_bool(plain, DISMAX), flatten_bool(plain, OCCUR)
+    assert got.clauses == want.clauses and want.groups is None and want.ties is None
+    for f in ("node_starts", "mm", "weights", "occurs"):
+        assert np.array_equal(getattr(got, f), getattr(want, f))
+    assert got.groups.tolist() == [0, 1, 2, 3, 4] and not got.ties.any()
+    assert flatten_bool(plain[:1], OR_AND).clauses == ["a", "b"]
     # Field members are seen inside a DisMax
     assert has_field(Or([DisMax(["a", Field("t", "b")])])) and has_field(DisMax([Field("t", "b")]))
     assert not has_field(Or([DisMax(["a", "b"])]))

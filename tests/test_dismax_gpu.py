@@ -1,5 +1,5 @@
-"""GPU: disjunction-max clauses (query.DisMax; sa_score_batch_topk_bool_dismax, sa_multi_score_batch_topk_bool_dismax,
-bool_dismax_tile_kernel in sa_bool.cu) against compose_dismax with each clause scored by this library's .score: ids
+"""GPU: disjunction-max clauses (query.DisMax; sa_score_batch_topk_bool and sa_multi_score_batch_topk_bool with
+groups, the DISMAX instances of bool_tile_kernel in sa_bool.cu) against compose_dismax with each clause scored by this library's .score: ids
 and float32 score bits must be equal.
 
 The synthetic frame is tests/test_bool_fields_gpu.py's: five 8192-doc tiles, `fa` (`w0` / `w1` / `w2` with a tile
@@ -142,7 +142,7 @@ def test_overflow_rerun(synth):
         for i, q in enumerate(queries):
             assert_topk(docs[i], scores[i], compose_dismax(synth.score(), q), k, f"overflow {q!r} k={k}")
     arr = synth.frame[A].array
-    docs, scores, n_redone = arr._search_topk_dismax([DisMax(["hot", "cold"], tie=0.3)], 10, bm25_similarity(), 0)
+    docs, scores, n_redone = arr._search_topk_bool([DisMax(["hot", "cold"], tie=0.3)], 10, bm25_similarity(), 0)
     assert n_redone == 1
     assert_topk(docs[0], scores[0], compose_dismax(arr.score, DisMax(["hot", "cold"], tie=0.3)), 10, "single overflow")
 
@@ -328,10 +328,10 @@ def test_c_abi_rejections(synth):
         t = np.asarray(ties, dtype=np.float32)
         o = np.asarray(occurs, dtype=np.uint8)
         m = np.asarray(mm, dtype=np.uint32)
-        return _lib.lib().sa_score_batch_topk_bool_dismax(
-            a._device().handle, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idf),
-            _lib.p_f32(idf), _lib.p_u8(o), _lib.p_u32(g), _lib.p_f32(t), _lib.p_u32(m), len(q_starts) - 1, 0,
-            a.avg_doc_length, k1, bb, 10, _lib.p_u32(docs), _lib.p_f32(scores), None)
+        return _lib.lib().sa_score_batch_topk_bool(
+            a._device().handle, len(q_starts) - 1, _lib.p_u32(q_starts), None, _lib.p_u32(terms), _lib.p_u32(c_starts),
+            _lib.p_f32(idf), _lib.p_f32(idf), _lib.p_u8(o), _lib.p_u32(g), _lib.p_f32(t), _lib.p_u32(m),
+            len(q_starts) - 1, 0, a.avg_doc_length, k1, bb, 10, None, 0, 0, _lib.p_u32(docs), _lib.p_f32(scores), None)
     assert single([0, 2, 4], [0, 0, 2, 2], [0.1, 0, 0.3, 0]) == 0
     assert single([0, 2, 4], [0, 1, 2, 2], [0, 0, 0, 0]) == 0               # plain clauses
     assert single([0, 4], [0, 0, 2, 2], [0.1, 0, 0.3, 0], mm=(2,)) == 0
@@ -360,11 +360,11 @@ def test_c_abi_rejections(synth):
         m = np.asarray([1], dtype=np.uint32)
         avgdl = np.asarray([a.avg_doc_length, b.avg_doc_length], dtype=np.float32)
         kk, bb = np.asarray(k1, dtype=np.float32), np.full(2, 0.75, dtype=np.float32)
-        return _lib.lib().sa_multi_score_batch_topk_bool_dismax(
-            mh.handle, _lib.p_u32(q_starts), _lib.p_u32(f), _lib.p_u32(t), _lib.p_u32(c_starts), _lib.p_f32(ones),
-            _lib.p_f32(ones), _lib.p_u8(occ), _lib.p_u32(np.asarray(groups, dtype=np.uint32)),
+        return _lib.lib().sa_multi_score_batch_topk_bool(
+            mh.handle, 1, _lib.p_u32(q_starts), None, _lib.p_u32(f), _lib.p_u32(t), _lib.p_u32(c_starts),
+            _lib.p_f32(ones), _lib.p_f32(ones), _lib.p_u8(occ), _lib.p_u32(np.asarray(groups, dtype=np.uint32)),
             _lib.p_f32(np.asarray(ties, dtype=np.float32)), _lib.p_u32(m), 1, 0, _lib.p_f32(avgdl), _lib.p_f32(kk),
-            _lib.p_f32(bb), 10, _lib.p_u32(docs), _lib.p_f32(scores), None)
+            _lib.p_f32(bb), 10, None, 0, 0, _lib.p_u32(docs), _lib.p_f32(scores), None)
     mh = _Multi([a, b])
     assert multi([0, 0], [0.3, 0]) == 0
     assert multi([0, 1], [0, 0]) == 0

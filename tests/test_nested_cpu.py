@@ -1,5 +1,5 @@
 """CPU: nested boolean queries (an Or / And / Bool as a clause of another) -- accepted forms, every refusal (raised
-before any device work, so on CPU-built arrays), flatten_nested's node arrays, and the oracle composition against the
+before any device work, so on CPU-built arrays), flatten_bool's node arrays, and the oracle composition against the
 real reference's composed results (tests/golden/nested.json, make_golden_nested.py)."""
 import json
 import os
@@ -88,12 +88,13 @@ def test_refusals_in_the_api():
 def test_flatten_nested_arrays():
     """A hand-written tree: nodes in pre-order after the top-level queries, a shared sub-query as two nodes."""
     from searcharray_b200 import And, Bool, Boost, DisMax, Or
-    from searcharray_b200.query import SA_NO_NODE as X, dismax_members, flatten_dismax, flatten_nested
+    from searcharray_b200.query import SA_NO_NODE as X, DISMAX, NESTED, dismax_members, flatten_bool
     shared = And(["s", "t"])
     q0 = Bool(must=["a", Or([shared, ["p", "q"]], mm=2)], should=[Boost(shared, 2), DisMax(["d", "e"], tie=0.5)],
               must_not=[shared])
     q1 = Or(["z"])
-    clauses, starts, cnode, mm, weights, occurs, groups, ties = flatten_nested([q0, q1])
+    clauses, starts, cnode, mm, weights, occurs, groups, ties, nq = flatten_bool([q0, q1], NESTED)
+    assert nq == 2
     # nodes: 0 q0, 1 q1, 2 Or([shared, p q]), 3 shared (in 2), 4 Boost(shared), 5 shared (must_not)
     assert starts.tolist() == [0, 6, 7, 9, 11, 13, 15]
     assert clauses == ["a", None, None, "d", "e", None, "z", None, ["p", "q"], "s", "t", "s", "t", "s", "t"]
@@ -110,13 +111,13 @@ def test_flatten_nested_arrays():
     for n in range(len(starts) - 1):
         for c in range(starts[n], starts[n + 1]):
             assert cnode[c] == X or cnode[c] > n
-    # a batch without nested queries flattens as flatten_dismax, with no nested clause
+    # a batch without nested queries flattened for NESTED: the DISMAX arrays, with no nested clause
     plain = [Or(["a", DisMax(["b", "c"])]), Bool(must=["m"], should=[Boost("s", 2)], must_not=["n"])]
-    got, want = flatten_nested(plain), flatten_dismax(plain)
-    assert got[0] == want[0] and all(c == X for c in got[2])
-    for g, w in zip(got[3:], want[2:]):
-        assert np.array_equal(g, w)
-    assert np.array_equal(got[1], want[1])
+    got, want = flatten_bool(plain, NESTED), flatten_bool(plain, DISMAX)
+    assert got.clauses == want.clauses and all(c == X for c in got.clause_node) and want.clause_node is None
+    for f in ("node_starts", "mm", "weights", "occurs", "groups", "ties"):
+        assert np.array_equal(getattr(got, f), getattr(want, f))
+    assert got.n_queries == want.n_queries == 2
 
 
 def test_helpers_see_inside_nested_queries():

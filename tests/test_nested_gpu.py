@@ -1,5 +1,5 @@
-"""GPU: nested boolean queries (an Or / And / Bool as a clause of another; sa_score_batch_topk_bool_nested,
-sa_multi_score_batch_topk_bool_nested, bool_nested_tile_kernel in sa_bool.cu) against compose_nested with each clause
+"""GPU: nested boolean queries (an Or / And / Bool as a clause of another; sa_score_batch_topk_bool and
+sa_multi_score_batch_topk_bool with clause_node, the NESTED instances of bool_tile_kernel in sa_bool.cu) against compose_nested with each clause
 scored by this library's .score: ids and float32 score bits must be equal.
 
 The synthetic frame is tests/test_bool_fields_gpu.py's: five 8192-doc tiles, `fa` (`w0` / `w1` / `w2` with a tile
@@ -164,7 +164,7 @@ def test_overflow_rerun(synth):
             assert_topk(docs[i], scores[i], compose_nested(synth.score(), q), k, f"overflow {q!r} k={k}")
     arr = synth.frame[A].array
     q = Or([Or(["hot", "cold"])])
-    docs, scores, n_redone = arr._search_topk_nested([q, Or(["w1", And(["s1", "w2"])])], 10, bm25_similarity(), 0)
+    docs, scores, n_redone = arr._search_topk_bool([q, Or(["w1", And(["s1", "w2"])])], 10, bm25_similarity(), 0)
     assert n_redone >= 1
     assert_topk(docs[0], scores[0], compose_nested(arr.score, q), 10, "single overflow")
 
@@ -301,11 +301,11 @@ def test_c_abi_rejections(synth):
         g = np.asarray(range(nc) if groups is None else groups, dtype=np.uint32)
         t = np.zeros(nc, dtype=np.float32)
         m = np.asarray(mm or [1] * (len(n_starts) - 1), dtype=np.uint32)
-        return _lib.lib().sa_score_batch_topk_bool_nested(
+        return _lib.lib().sa_score_batch_topk_bool(
             a._device().handle, len(n_starts) - 1, _lib.p_u32(n_starts), _lib.p_u32(np.asarray(c_node, dtype=np.uint32)),
             _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(ones), _lib.p_f32(ones), _lib.p_u8(occ), _lib.p_u32(g),
-            _lib.p_f32(t), _lib.p_u32(m), nq, 0, a.avg_doc_length, 1.2, 0.75, 10, _lib.p_u32(docs), _lib.p_f32(scores),
-            None)
+            _lib.p_f32(t), _lib.p_u32(m), nq, 0, a.avg_doc_length, 1.2, 0.75, 10, None, 0, 0, _lib.p_u32(docs),
+            _lib.p_f32(scores), None)
     # query 0 = Or(w0, node 1); node 1 = Or(w1, s1)
     assert call([0, 2, 4], [X, 1, X, X], [["w0"], [], ["w1"], ["s1"]]) == 0
     assert call([0, 2, 4], [X, 2, X, X], [["w0"], [], ["w1"], ["s1"]]) != 0          # out of range

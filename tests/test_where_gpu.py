@@ -1,5 +1,5 @@
-"""GPU: the `where=` document mask of search_topk and fields_topk (sa_score_batch_topk_bool_where,
-sa_multi_score_batch_topk_bool_where, sa_score_batch_topk_sim_where; bool_where_tile_kernel in sa_bool.cu,
+"""GPU: the `where=` document mask of search_topk and fields_topk (where_bits of sa_score_batch_topk_bool,
+sa_multi_score_batch_topk_bool and sa_score_batch_topk_sim; the WHERE instances of bool_tile_kernel in sa_bool.cu,
 sim_where_tile_kernel in sa_view.cu).  For every query the result must be the top k of np.where(mask_q, S_q, 0),
 S_q being what the call without a mask ranks -- .score for a plain query, compose_nested over .score for a boolean
 one, the per-field composition for fields_topk -- ids exact and score bits exact, so a mask never changes a score.

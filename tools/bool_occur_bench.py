@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Bool queries (must / should / filter / must_not) and boosted Or in search_topk (sa_score_batch_topk_bool_occur) on
+"""Bool queries (must / should / filter / must_not) and boosted Or in search_topk (sa_score_batch_topk_bool) on
 the bench corpus, next to the plain Or / And they extend, measured in the same run.
 
     python tools/bool_occur_bench.py [--docs 10000000] [--queries 1024] [--phrase-queries 64] [--k 10] [--reps 5]
@@ -57,8 +57,8 @@ def main():
     ap.add_argument("--verify", type=int, default=8)
     args = ap.parse_args()
 
-    from searcharray_b200 import And, Bool, Boost, Or, SearchArray, _lib, bm25_similarity, compute_idf, synth
-    from searcharray_b200.query import flatten, flatten_occur, needs_occur
+    from searcharray_b200 import And, Bool, Boost, Or, SearchArray, bm25_similarity, compute_idf, synth
+    from searcharray_b200.query import bool_form, flatten_bool
     info = card()
     spec = synth.SynthSpec(args.docs)
     host, _, _ = synth.generate_shard(spec)
@@ -133,35 +133,21 @@ def main():
         per_query = np.asarray([query_bytes(q) for q in queries], dtype=np.float64)
         # the Python side of the call alone: flattening and the per-clause idf (part of every timed call)
         t0 = time.perf_counter()
-        occur = any(needs_occur(q) for q in queries)
-        flat = flatten_occur(queries) if occur else flatten(queries)
-        terms, c_starts, idfs = arr._topk_queries(flat[0], lambda d: compute_idf(arr.corpus_size, d))
+        batch = flatten_bool(queries, max(map(bool_form, queries)))
+        terms, c_starts, idfs = arr._topk_queries(batch.clauses, lambda d: compute_idf(arr.corpus_size, d))
         prep_ms = 1e3 * (time.perf_counter() - t0)
         # the C call alone on the prepared arrays: planning, uploads, kernels, the result copy
         idfs = np.asarray(idfs, dtype=np.float32)
-        docs = np.empty((len(queries), args.k), dtype=np.uint32)
-        scores = np.empty((len(queries), args.k), dtype=np.float32)
-        h, L = arr._device().handle, _lib.lib()
+        dev = arr._device()
 
         def c_call():
-            if occur:
-                _, q_starts, mm, weights, occurs = flat
-                _lib.check(L.sa_score_batch_topk_bool_occur(
-                    h, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
-                    _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(mm), len(queries), 0, arr.avg_doc_length,
-                    sim.k1, sim.b, args.k, _lib.p_u32(docs), _lib.p_f32(scores), None))
-            else:
-                _, q_starts, mm = flat
-                _lib.check(L.sa_score_batch_topk_bool(
-                    h, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
-                    _lib.p_u32(mm), len(queries), 0, arr.avg_doc_length, sim.k1, sim.b, args.k,
-                    _lib.p_u32(docs), _lib.p_f32(scores), None))
+            return arr._bool_call(dev, batch, terms, c_starts, idfs, sim, 0, args.k, None)
         for _ in range(args.warmup):
             c_call()
         c_times = []
         for _ in range(args.reps):
             t0 = time.perf_counter()
-            c_call()
+            docs, scores, _ = c_call()
             c_times.append(time.perf_counter() - t0)
         d_ref, s_ref, _ = arr._search_topk_bool(queries, args.k, sim, 0)
         if not (np.array_equal(docs, d_ref) and np.array_equal(scores.view(np.uint32), s_ref.view(np.uint32))):

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Disjunction-max clauses (query.DisMax) on the bench corpus: best_fields over two DataFrame fields through
-solr.fields_topk (sa_multi_score_batch_topk_bool_dismax), next to the same leaves as most_fields (an Or of the Field
+solr.fields_topk (sa_multi_score_batch_topk_bool with groups), next to the same leaves as most_fields (an Or of the Field
 clauses, sa_multi_score_batch_topk_bool) measured in the same run, and single-column synonyms through search_topk.
 
     python tools/dismax_topk_bench.py [--docs 10000000] [--queries 1024] [--k 10] [--reps 5] [--edismax-queries 4]
@@ -118,11 +118,11 @@ def main():
            "workloads": {}}
 
     def c_time(queries):
-        flat, slot_of, arrays, sims = _fields_plan(frame, queries, sim)
+        batch, slot_of, arrays, sims = _fields_plan(frame, queries, sim)
         multi = _multi_for(arrays)
         with _locked(multi, arrays):
-            prepared = _fields_clauses(flat[0], slot_of, arrays)
-            return median_time(lambda: _fields_call(multi, arrays, sims, flat, prepared, args.k, 0), args.warmup,
+            prepared = _fields_clauses(batch.clauses, slot_of, arrays)
+            return median_time(lambda: _fields_call(multi, arrays, sims, batch, prepared, args.k, 0), args.warmup,
                                args.reps)
 
     def verify(label, queries, run, scorer):
@@ -163,37 +163,27 @@ def main():
         print(f"[dismax_topk_bench] {label}: {json.dumps(rec)}", file=sys.stderr, flush=True)
 
     # single-column synonyms through search_topk, against Or of the same terms
-    from searcharray_b200 import _lib
     sq = [DisMax([t(i, 0), t(i, 1)], tie=0.1) for i in range(nq)]
     oq = [Or([t(i, 0), t(i, 1)]) for i in range(nq)]
     n_ver = verify("synonyms", sq, lambda qs: f1.search_topk(qs, k=args.k), f1.score)
     t_api = median_time(lambda: f1.search_topk(sq, k=args.k), args.warmup, args.reps)
     t_or_api = median_time(lambda: f1.search_topk(oq, k=args.k), args.warmup, args.reps)
-    from searcharray_b200.query import flatten, flatten_dismax
+    from searcharray_b200.query import DISMAX, OR_AND, flatten_bool
     from searcharray_b200 import compute_idf
-    h = f1._device().handle
-    docs = np.empty((nq, args.k), dtype=np.uint32)
-    scores = np.empty((nq, args.k), dtype=np.float32)
-    clauses, q_starts, mm, weights, occurs, groups, ties = flatten_dismax(sq)
-    terms, c_starts, idfs = f1._topk_queries(clauses, lambda x: compute_idf(f1.corpus_size, x))
+    dev = f1._device()
+    batch = flatten_bool(sq, DISMAX)
+    terms, c_starts, idfs = f1._topk_queries(batch.clauses, lambda x: compute_idf(f1.corpus_size, x))
     idfs = np.asarray(idfs, dtype=np.float32)
     redone = []
 
     def dismax_c():
-        n = np.zeros(1, dtype=np.uint32)
-        _lib.check(_lib.lib().sa_score_batch_topk_bool_dismax(
-            h, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs), _lib.p_f32(weights),
-            _lib.p_u8(occurs), _lib.p_u32(groups), _lib.p_f32(ties), _lib.p_u32(mm), nq, 0, f1.avg_doc_length,
-            sim.k1, sim.b, args.k, _lib.p_u32(docs), _lib.p_f32(scores), _lib.p_u32(n)))
-        redone.append(int(n[0]))
-    oc, oqs, omm = flatten(oq)
-    oterms, oc_starts, oidfs = f1._topk_queries(oc, lambda x: compute_idf(f1.corpus_size, x))
+        redone.append(f1._bool_call(dev, batch, terms, c_starts, idfs, sim, 0, args.k, None)[2])
+    obatch = flatten_bool(oq, OR_AND)
+    oterms, oc_starts, oidfs = f1._topk_queries(obatch.clauses, lambda x: compute_idf(f1.corpus_size, x))
     oidfs = np.asarray(oidfs, dtype=np.float32)
 
     def or_c():
-        _lib.check(_lib.lib().sa_score_batch_topk_bool(
-            h, _lib.p_u32(oqs), _lib.p_u32(oterms), _lib.p_u32(oc_starts), _lib.p_f32(oidfs), _lib.p_u32(omm), nq, 0,
-            f1.avg_doc_length, sim.k1, sim.b, args.k, _lib.p_u32(docs), _lib.p_f32(scores), None))
+        f1._bool_call(dev, obatch, oterms, oc_starts, oidfs, sim, 0, args.k, None)
     t_c = median_time(dismax_c, args.warmup, args.reps)
     t_or_c = median_time(or_c, args.warmup, args.reps)
     rec = {"queries": nq, "verified_queries": n_ver, "qps": nq / t_api, "or_qps": nq / t_or_api, "c_call_qps": nq / t_c,

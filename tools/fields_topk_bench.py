@@ -70,9 +70,8 @@ def main():
 
     import pandas as pd
     from searcharray_b200 import Bool, Boost, Field, Or, SearchArray, bm25_similarity, compute_idf, synth
-    from searcharray_b200.query import flatten_occur
+    from searcharray_b200.query import OCCUR, flatten_bool
     from searcharray_b200.solr import _fields_call, _fields_clauses, _fields_plan, _fields_topk, _locked, _multi_for
-    from searcharray_b200 import _lib
     info = card()
     spec = synth.SynthSpec(args.docs)
     host, _, _ = synth.generate_shard(spec)
@@ -144,26 +143,21 @@ def main():
         # the C calls alone on prepared arrays: the two-column queries, the same with every clause on f1 (the
         # field-aware kernel on one index's data), and the single-field Bool
         def fields_c_time(queries):
-            flat, slot_of, arrays, sims = _fields_plan(frame, queries, sim)
+            batch, slot_of, arrays, sims = _fields_plan(frame, queries, sim)
             multi = _multi_for(arrays)
             with _locked(multi, arrays):
-                prepared = _fields_clauses(flat[0], slot_of, arrays)
-                return median_time(lambda: _fields_call(multi, arrays, sims, flat, prepared, args.k, 0), args.warmup,
+                prepared = _fields_clauses(batch.clauses, slot_of, arrays)
+                return median_time(lambda: _fields_call(multi, arrays, sims, batch, prepared, args.k, 0), args.warmup,
                                    args.reps)
         t_c = fields_c_time(fq)
         t_c1 = fields_c_time(build(lambda f, c: Field("f1", c), label))
-        clauses, q_starts, mm, weights, occurs = flatten_occur(sq)
-        terms, c_starts, idfs = f1._topk_queries(clauses, lambda x: compute_idf(f1.corpus_size, x))
+        sbatch = flatten_bool(sq, OCCUR)
+        terms, c_starts, idfs = f1._topk_queries(sbatch.clauses, lambda x: compute_idf(f1.corpus_size, x))
         idfs = np.asarray(idfs, dtype=np.float32)
-        docs = np.empty((len(sq), args.k), dtype=np.uint32)
-        scores = np.empty((len(sq), args.k), dtype=np.float32)
-        h = f1._device().handle
+        dev = f1._device()
 
         def single_c():
-            _lib.check(_lib.lib().sa_score_batch_topk_bool_occur(
-                h, _lib.p_u32(q_starts), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
-                _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(mm), len(sq), 0, f1.avg_doc_length, sim.k1, sim.b,
-                args.k, _lib.p_u32(docs), _lib.p_f32(scores), None))
+            f1._bool_call(dev, sbatch, terms, c_starts, idfs, sim, 0, args.k, None)
         t_single_c = median_time(single_c, args.warmup, args.reps)
 
         # the host composition of dense per-field .score vectors

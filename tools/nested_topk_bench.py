@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Nested boolean queries (an Or / And / Bool as a clause of another) on the bench corpus, through solr.fields_topk
-(sa_multi_score_batch_topk_bool_nested) and SearchArray.search_topk (sa_score_batch_topk_bool_nested).
+(sa_multi_score_batch_topk_bool) and SearchArray.search_topk (sa_score_batch_topk_bool), with clause_node.
 
     python tools/nested_topk_bench.py [--docs 10000000] [--queries 1024] [--k 10] [--reps 5]
 
@@ -63,9 +63,9 @@ def main():
     args = ap.parse_args()
 
     import pandas as pd
-    from searcharray_b200 import And, Bool, Boost, DisMax, Field, Or, SearchArray, _lib, bm25_similarity, compute_idf
+    from searcharray_b200 import And, Bool, Boost, DisMax, Field, Or, SearchArray, bm25_similarity, compute_idf
     from searcharray_b200 import synth
-    from searcharray_b200.query import _leaves, flatten_nested
+    from searcharray_b200.query import NESTED, _leaves, flatten_bool
     from searcharray_b200.solr import _fields_call, _fields_clauses, _fields_plan, _fields_topk, _locked, _multi_for
     info = card()
     spec = synth.SynthSpec(args.docs)
@@ -122,11 +122,11 @@ def main():
         def run():
             redone.append(_fields_topk(frame, qs, args.k, sim, 0)[2])
         t_api = median_time(run, args.warmup, args.reps)
-        flat, slot_of, arrays, sims = _fields_plan(frame, qs, sim)
+        batch, slot_of, arrays, sims = _fields_plan(frame, qs, sim)
         multi = _multi_for(arrays)
         with _locked(multi, arrays):
-            prepared = _fields_clauses(flat[0], slot_of, arrays)
-            t_c = median_time(lambda: _fields_call(multi, arrays, sims, flat, prepared, args.k, 0), args.warmup,
+            prepared = _fields_clauses(batch.clauses, slot_of, arrays)
+            t_c = median_time(lambda: _fields_call(multi, arrays, sims, batch, prepared, args.k, 0), args.warmup,
                               args.reps)
         rec = dict({"queries": nq, "verified_queries": n_ver, "qps": nq / t_api, "c_call_qps": nq / t_c,
                     "n_redone": redone[-args.reps:]}, **shape(qs))
@@ -137,25 +137,18 @@ def main():
     qs = [Or([And([t(i, 0), t(i, 1)]), And([t(i, 2), t(i, 3)])]) for i in range(nq)]
     n_ver = verify("or_of_ands", qs, lambda x: f1.search_topk(x, k=args.k), f1.score)
     t_api = median_time(lambda: f1.search_topk(qs, k=args.k), args.warmup, args.reps)
-    clauses, n_starts, c_node, mm, weights, occurs, groups, ties = flatten_nested(qs)
+    batch = flatten_bool(qs, NESTED)
+    clauses = batch.clauses
     leaf = [i for i, c in enumerate(clauses) if c is not None]
     terms, l_starts, l_idfs = f1._topk_queries([clauses[i] for i in leaf], lambda x: compute_idf(f1.corpus_size, x))
     idfs, n_terms = np.zeros(len(clauses), dtype=np.float32), np.zeros(len(clauses), dtype=np.int64)
     idfs[leaf], n_terms[leaf] = l_idfs, np.diff(l_starts)
     c_starts = np.concatenate([[0], np.cumsum(n_terms)]).astype(np.uint32)
-    h = f1._device().handle
-    docs = np.empty((nq, args.k), dtype=np.uint32)
-    scores = np.empty((nq, args.k), dtype=np.float32)
+    dev = f1._device()
     redone = []
 
     def c_call():
-        n = np.zeros(1, dtype=np.uint32)
-        _lib.check(_lib.lib().sa_score_batch_topk_bool_nested(
-            h, len(n_starts) - 1, _lib.p_u32(n_starts), _lib.p_u32(c_node), _lib.p_u32(terms), _lib.p_u32(c_starts),
-            _lib.p_f32(idfs), _lib.p_f32(weights), _lib.p_u8(occurs), _lib.p_u32(groups), _lib.p_f32(ties),
-            _lib.p_u32(mm), nq, 0, f1.avg_doc_length, sim.k1, sim.b, args.k, _lib.p_u32(docs), _lib.p_f32(scores),
-            _lib.p_u32(n)))
-        redone.append(int(n[0]))
+        redone.append(f1._bool_call(dev, batch, terms, c_starts, idfs, sim, 0, args.k, None)[2])
     t_c = median_time(c_call, args.warmup, args.reps)
     rec = dict({"queries": nq, "verified_queries": n_ver, "qps": nq / t_api, "c_call_qps": nq / t_c,
                 "n_redone": redone[-args.reps:]}, **shape(qs))

@@ -17,7 +17,7 @@ Masks: none (today's call, no `where`), all (all true), rand50 / rand10 / rand1 
 of 10M docs is 1.25 MB packed per query and N bytes per query as numpy bools).
 Per (workload, mask) cell:
   qps           the public call, host clock around the synchronous call (packing the mask included), median of --reps
-  c_call_qps    sa_score_batch_topk_bool_where on arrays and a mask packed once (the mask's upload included);
+  c_call_qps    sa_score_batch_topk_bool on arrays and a mask packed once (the mask's upload included);
                 for `none`: sa_score_batch_topk for term and phrase, and for the boolean workloads the same
                 prepared call without a mask (the unmasked instances)
   n_redone      queries re-run exactly in the timed C calls (candidate overflow)
@@ -27,7 +27,6 @@ Per workload, compose_qps: .score per clause + the boolean composition + np.wher
 Prints one JSON line.
 """
 import argparse
-import ctypes
 import json
 import os
 import sys
@@ -59,31 +58,20 @@ def median_time(fn, warmup, reps):
 def prepared_call(arr, queries, k, sim):
     """The C call of search_topk(queries, where=...) on arrays prepared once: fn(bits) -> n_redone."""
     from searcharray_b200 import Or, compute_idf
-    from searcharray_b200.query import flatten, flatten_nested, flatten_occur, is_boolean, is_nested, needs_occur
+    from searcharray_b200.query import bool_form, flatten_bool, is_boolean
     qs = [q if is_boolean(q) else Or([q]) for q in queries]
-    c_node = weights = occurs = groups = ties = None
-    if any(is_nested(q) for q in qs):
-        clauses, starts, c_node, mm, weights, occurs, groups, ties = flatten_nested(qs)
-    elif any(needs_occur(q) for q in qs):
-        clauses, starts, mm, weights, occurs = flatten_occur(qs)
-    else:
-        clauses, starts, mm = flatten(qs)
+    batch = flatten_bool(qs, max(map(bool_form, qs)))
+    clauses = batch.clauses
     leaf = [i for i, c in enumerate(clauses) if c is not None]
     terms, l_starts, l_idfs = arr._topk_queries([clauses[i] for i in leaf], lambda x: compute_idf(arr.corpus_size, x))
     idfs, n_terms = np.zeros(len(clauses), dtype=np.float32), np.zeros(len(clauses), dtype=np.int64)
     idfs[leaf], n_terms[leaf] = l_idfs, np.diff(l_starts)
     c_starts = np.concatenate([[0], np.cumsum(n_terms)]).astype(np.uint32)
-    docs = np.empty((len(qs), k), dtype=np.uint32)
-    scores = np.empty((len(qs), k), dtype=np.float32)
     dev = arr._device()
 
     def call(bits):
-        n = ctypes.c_uint32(0)
-        arr._bool_where(dev, len(starts) - 1, starts, c_node, terms, c_starts, idfs, weights, occurs, groups, ties, mm,
-                        len(qs), 0, sim, k, docs, scores, n, bits)
-        return n.value
+        return arr._bool_call(dev, batch, terms, c_starts, idfs, sim, 0, k, bits)[2]
     return call
-
 
 def main():
     ap = argparse.ArgumentParser()
