@@ -113,14 +113,16 @@ edismax_combine_fields_kernel(const CombineArgs a) {
 }
 
 struct PhaseArgs {
-    const float *rows[ED_MAX_ROWS];
-    float boost[ED_MAX_ROWS];
-    u32 has_boost[ED_MAX_ROWS];
+    const float *rows[ED_MAX_PHASE_ENTRIES];
+    float boost[ED_MAX_PHASE_ENTRIES];
+    u32 has_boost[ED_MAX_PHASE_ENTRIES];
     u32 n;
     u64 n_docs;
     double *qf;
     int f32_mode;
 };
+// a kernel parameter: one phase is one launch (one float32 fold in the reference's order), never split over two
+static_assert(sizeof(PhaseArgs) <= 4096, "PhaseArgs must fit the classic kernel parameter limit");
 
 // qf[where qf != 0] += float32 sum of the phase's vectors, in order (solr.py:335-353)
 __global__ void __launch_bounds__(256)
@@ -180,6 +182,11 @@ extern "C" int sa_multi_create(sa_index *const *fields, uint32_t n_fields, sa_mu
     m->filt_lens.resize(n_fields);
     m->phrase_rows.assign(n_fields, 0);
     m->filt_bound.assign(n_fields, 0);
+    m->shared.assign(n_fields, 0);
+    m->rows.resize(n_fields);
+    for (u32 f = 0; f < n_fields; f++)
+        for (u32 g = 0; g < n_fields; g++)
+            if (g != f && fields[g] == fields[f]) m->shared[f] = 1;
     SA_CUDA(cudaSetDevice(m->device));
     const u64 s = std::max<u64>(m->stride, SA_TILE_DOCS);
     SA_CUDA(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
@@ -213,14 +220,15 @@ extern "C" int sa_multi_qf(sa_multi *m, int field_centric, const uint32_t *n_ter
         sa_index *ix = m->fields[f];
         FieldGuard fg(ix, m->stream);
         int rc;
-        if ((rc = ix->dense.reserve(std::max<u64>(T, 1) * m->stride * sizeof(float)))) return rc;
-        a.rows[f] = ix->dense.as<float>();
+        if ((rc = (m->shared[f] ? m->rows[f] : ix->dense).reserve(std::max<u64>(T, 1) * m->stride * sizeof(float)))) return rc;
+        float *rows = m->field_rows(f);
+        a.rows[f] = rows;
         a.n_terms[f] = T;
         a.boost[f] = boost[f];
         a.has_boost[f] = has_boost[f];
         a.mm[f] = mm[f];
         if (T && (avg_doc_len[f] == 0.0f || m->n_docs == 0)) {         // similarity.py:31-32: zeros
-            SA_CUDA(cudaMemsetAsync(ix->dense.p, 0, (size_t)T * m->stride * sizeof(float), m->stream));
+            SA_CUDA(cudaMemsetAsync(rows, 0, (size_t)T * m->stride * sizeof(float), m->stream));
         } else if (T) {
             if ((rc = sa_check_term_ids(ix, term_ids + at, T))) return rc;
             std::vector<TermQuery> tqs(T);
@@ -233,7 +241,9 @@ extern "C" int sa_multi_qf(sa_multi *m, int field_centric, const uint32_t *n_ter
             SA_CUDA(cudaMemcpyAsync(ix->queries.p, tqs.data(), T * sizeof(TermQuery), cudaMemcpyHostToDevice, m->stream));
             TopkCtx none;
             memset(&none, 0, sizeof(none));
-            if ((rc = launch_term_batch(ix, make_term_args(ix, ix->queries.as<TermQuery>(), p, none), T))) return rc;
+            TermBatchArgs ta = make_term_args(ix, ix->queries.as<TermQuery>(), p, none);
+            ta.out = rows;
+            if ((rc = launch_term_batch(ix, ta, T))) return rc;
             SA_CUDA(cudaStreamSynchronize(m->stream));                  // tqs leaves scope
         }
         at += T;
@@ -303,9 +313,11 @@ extern "C" int sa_multi_phrases(sa_multi *m, uint32_t field, uint32_t n_phrases,
     FieldGuard fg(ix, m->stream);
     int rc;
     m->phrase_rows[field] = n_phrases;
+    const size_t row_bytes = (size_t)n_phrases * m->stride * sizeof(float);
+    if (m->shared[field] && (rc = m->rows[field].reserve(row_bytes))) return rc;
     if (avg_doc_len == 0.0f || m->n_docs == 0) {
-        if ((rc = ix->dense.reserve((size_t)n_phrases * m->stride * sizeof(float)))) return rc;
-        SA_CUDA(cudaMemsetAsync(ix->dense.p, 0, (size_t)n_phrases * m->stride * sizeof(float), m->stream));
+        if (!m->shared[field] && (rc = ix->dense.reserve(row_bytes))) return rc;
+        SA_CUDA(cudaMemsetAsync(m->field_rows(field), 0, row_bytes, m->stream));
         return SA_OK;
     }
     std::vector<PhraseQuery> pqs(n_phrases);
@@ -328,21 +340,25 @@ extern "C" int sa_multi_phrases(sa_multi *m, uint32_t field, uint32_t n_phrases,
     }
     PhraseDump nodump;
     memset(&nodump, 0, sizeof(nodump));
-    return sa_phrase_run_sync(ix, pqs, ix->filt.as<u64>(), 1, p, nodump, false);
+    if ((rc = sa_phrase_run_sync(ix, pqs, ix->filt.as<u64>(), 1, p, nodump, false))) return rc;
+    // the phrase kernel writes ix->dense: a field whose index another field shares keeps its own copy
+    if (m->shared[field]) SA_CUDA(cudaMemcpyAsync(m->rows[field].p, ix->dense.p, row_bytes, cudaMemcpyDeviceToDevice, m->stream));
+    return SA_OK;
 }
 
 extern "C" int sa_multi_add_phase(sa_multi *m, uint32_t n_entries, const uint32_t *entry_field,
                                   const uint32_t *entry_row, const float *entry_boost, const uint32_t *entry_has_boost) {
     SA_CHECK(m && m->has_qf, "sa_multi_qf has not run");
     if (n_entries == 0) return SA_OK;
-    SA_CHECK(entry_field && entry_row && entry_boost && entry_has_boost && n_entries <= ED_MAX_ROWS, "bad argument");
+    SA_CHECK(entry_field && entry_row && entry_boost && entry_has_boost, "NULL argument");
+    SA_CHECK(n_entries <= ED_MAX_PHASE_ENTRIES, "%u phase entries: at most %d", n_entries, ED_MAX_PHASE_ENTRIES);
     std::lock_guard<std::mutex> g(m->mu);
     SA_CUDA(cudaSetDevice(m->device));
     PhaseArgs a;
     memset(&a, 0, sizeof(a));
     for (u32 i = 0; i < n_entries; i++) {
         SA_CHECK(entry_field[i] < m->fields.size() && entry_row[i] < m->phrase_rows[entry_field[i]], "entry %u out of range", i);
-        a.rows[i] = m->fields[entry_field[i]]->dense.as<float>() + (u64)entry_row[i] * m->stride;
+        a.rows[i] = m->field_rows(entry_field[i]) + (u64)entry_row[i] * m->stride;
         a.boost[i] = entry_boost[i];
         a.has_boost[i] = entry_has_boost[i];
     }

@@ -4,7 +4,10 @@
 #include "sa_common.cuh"
 
 #define ED_MAX_FIELDS 8
-#define ED_MAX_ROWS 64
+#define ED_MAX_ROWS 64                                               // phrase rows of one field in one sa_multi_phrases
+// entries of one sa_multi_add_phase: pf2 on every field of a query of SA_MAX_PHRASE_TERMS tokens (T - 1 bigrams and
+// the last one repeated), the most searcharray_b200.solr._Plan.device_ok admits
+#define ED_MAX_PHASE_ENTRIES (ED_MAX_FIELDS * SA_MAX_PHRASE_TERMS)
 
 struct sa_multi {
     ~sa_multi() {
@@ -22,6 +25,12 @@ struct sa_multi {
     std::vector<std::vector<u64>> filt_offs, filt_lens;   // per field: last sa_multi_filter
     std::vector<u32> phrase_rows;        // per field: rows produced by the last sa_multi_phrases
     std::vector<u64> filt_bound;         // per field: words reserved for filtered lists (0 = not computed yet)
+    // per field: 1 when another field of the multi is the same index (two column names of one array).  Such a field
+    // keeps its term and phrase rows in rows[f] instead of its index's dense scratch, which the other field's calls
+    // overwrite before the combine / sa_multi_add_phase read them.
+    std::vector<char> shared;
+    std::vector<DevBuf> rows;
+    float *field_rows(u32 f) const { return shared[f] ? rows[f].as<float>() : fields[f]->dense.as<float>(); }
     DevBuf cand;                         // top-k: candidate slots (then, for sa_multi_topk, their float64 scores)
     DevBuf keys;                         // top-k result: k keys, k float64 scores, the overflow flag
     std::unique_ptr<BoolState, BoolStateDelete> boolq;   // buffers of sa_multi_score_batch_topk_bool (sa_bool.cu)

@@ -21,6 +21,9 @@ SA_BOOL_MAX_CLAUSES = 64          # include/searcharray_b200.h
 SA_BOOL_MAX_NESTED = 64           # nested queries in one top-level query, at any depth
 SA_NO_NODE = 0xFFFFFFFF           # include/searcharray_b200.h
 ED_MAX_FIELDS = 8                 # fields of one sa_multi (sa_multi.cuh)
+SA_MAX_PHRASE_TERMS = 16          # include/searcharray_b200.h
+ED_MAX_ROWS = 64                  # phrase rows of one field in one sa_multi_phrases call (sa_multi.cuh)
+ED_MAX_PHASE_ENTRIES = ED_MAX_FIELDS * SA_MAX_PHRASE_TERMS   # entries of one sa_multi_add_phase call (sa_multi.cuh)
 SA_OCCUR_SHOULD, SA_OCCUR_MUST, SA_OCCUR_FILTER, SA_OCCUR_MUST_NOT = 0, 1, 2, 3
 
 Clause = Union[str, List[str]]

@@ -185,10 +185,11 @@ class _Plan:
         self.num_terms, self.search_terms, self.term_centric = parse_query_terms(frame, q, self.names)
 
     def device_ok(self):
+        from .query import ED_MAX_FIELDS, SA_MAX_PHRASE_TERMS
         return (all(isinstance(self.similarity[f], Bm25Similarity) for f in self.names)
                 and all(a.rows is None for a in self.arrays)
-                and len({len(a) for a in self.arrays}) == 1 and len(self.names) <= 8
-                and all(len(t) <= 16 for t in self.search_terms.values()))
+                and len({len(a) for a in self.arrays}) == 1 and len(self.names) <= ED_MAX_FIELDS
+                and all(len(t) <= SA_MAX_PHRASE_TERMS for t in self.search_terms.values()))
 
     # explain strings, reference solr.py:133-147, 160-178, 199-200, 219-220, 241-242
     def explain_qf(self):
@@ -218,6 +219,29 @@ class _Plan:
                if len(self.search_terms[f]) >= 3]
         for name, items in (("pf", pf), ("pf2", pf2), ("pf3", pf3)):
             out.append((name, items))
+        return out
+
+    def phrase_rows(self):
+        """field -> [(phase name, phrase no)]: the rows of the field's one sa_multi_phrases launch, in row order."""
+        per_field: Dict[str, List[Tuple[str, int]]] = {}
+        for name, items in self.phases():
+            for f, _, phrases, _ in items:
+                if f not in self.query_fields:
+                    raise KeyError(f)                              # like the reference: pf fields must be in qf
+                per_field.setdefault(f, []).extend((name, i) for i in range(len(phrases)))
+        return per_field
+
+    def phase_entries(self):
+        """[(phase name, [(field, row, boost)])]: the entries of each phase's one sa_multi_add_phase call, in the
+        reference's summation order (pf2 adds its last bigram twice); row indexes phrase_rows()[field]."""
+        row_of = {(f, name, i): r for f, rows in self.phrase_rows().items() for r, (name, i) in enumerate(rows)}
+        out = []
+        for name, items in self.phases():
+            entries = []
+            for f, boost, phrases, repeat_last in items:
+                order = list(range(len(phrases))) + ([len(phrases) - 1] if repeat_last else [])
+                entries.extend((f, row_of[(f, name, i)], boost) for i in order)
+            out.append((name, entries))
         return out
 
     def explain_phases(self):
@@ -267,15 +291,7 @@ def _run_device(plan: _Plan, multi: _Multi) -> _Multi:
 
     # every phrase of one field runs in one launch on that field's lists filtered to qf > 0
     field_index = {f: i for i, f in enumerate(plan.names)}
-    per_field: Dict[str, List[Tuple[str, int]]] = {}          # field -> [(phase, phrase no)] in row order
-    for name, items in phases:
-        for f, _, phrases, _ in items:
-            if f not in field_index:
-                raise KeyError(f)                              # like the reference: pf fields must be in qf
-            rows = per_field.setdefault(f, [])
-            rows.extend((name, i) for i in range(len(phrases)))
-    row_of: Dict[Tuple[str, str, int], int] = {}
-    for f, rows in per_field.items():
+    for f, rows in plan.phrase_rows().items():
         fi, arr, sim = field_index[f], plan.arrays[field_index[f]], plan.similarity[f]
         toks = plan.search_terms[f]
         uniq = list(dict.fromkeys(toks))
@@ -287,9 +303,8 @@ def _run_device(plan: _Plan, multi: _Multi) -> _Multi:
             dfs = comm.sum_u64(dfs)
         starts, slots, ids, p_idf = [0], [], [], []
         phrase_lists = {name: phrases for name, items in phases for ff, _, phrases, _ in items if ff == f}
-        for r, (name, i) in enumerate(rows):
+        for name, i in rows:
             ph = phrase_lists[name][i]
-            row_of[(f, name, i)] = r
             slots.extend(slot[t] for t in ph)
             ids.extend(int(u_ids[slot[t]]) for t in ph)
             starts.append(len(slots))
@@ -297,18 +312,12 @@ def _run_device(plan: _Plan, multi: _Multi) -> _Multi:
         a_st, a_sl, a_id, a_pi = _u32(starts), _u32(slots), _u32(ids), _f32(p_idf)
         _lib.check(_timed("phrases", L.sa_multi_phrases, multi.handle, fi, len(rows), _lib.p_u32(a_st), _lib.p_u32(a_sl),
                                       _lib.p_u32(a_id), _lib.p_f32(a_pi), arr.avg_doc_length, sim.k1, sim.b))
-    for name, items in phases:
-        e_field, e_row, e_boost, e_hb = [], [], [], []
-        for f, boost, phrases, repeat_last in items:
-            order = list(range(len(phrases))) + ([len(phrases) - 1] if repeat_last else [])
-            for i in order:
-                e_field.append(field_index[f])
-                e_row.append(row_of[(f, name, i)])
-                e_boost.append(0.0 if boost is None else boost)
-                e_hb.append(0 if boost is None else 1)
-        if e_field:
-            a_f, a_r, a_bo, a_h = _u32(e_field), _u32(e_row), _f32(e_boost), _u32(e_hb)
-            _lib.check(_timed("add_phase", L.sa_multi_add_phase, multi.handle, len(e_field), _lib.p_u32(a_f), _lib.p_u32(a_r),
+    for _, entries in plan.phase_entries():
+        if entries:
+            a_f, a_r = _u32([field_index[f] for f, _, _ in entries]), _u32([r for _, r, _ in entries])
+            a_bo = _f32([0.0 if bo is None else bo for _, _, bo in entries])
+            a_h = _u32([0 if bo is None else 1 for _, _, bo in entries])
+            _lib.check(_timed("add_phase", L.sa_multi_add_phase, multi.handle, len(entries), _lib.p_u32(a_f), _lib.p_u32(a_r),
                                             _lib.p_f32(a_bo), _lib.p_u32(a_h)))
     return multi
 
