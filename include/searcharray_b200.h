@@ -209,6 +209,20 @@ int sa_score_batch_topk_sim(sa_index *index, int kind, const uint32_t *terms, co
  * result is the top k of the unmasked call's scores where the query's mask is set; every score equals the unmasked
  * one bit for bit.
  *
+ * Feature clauses (Lucene's FeatureField, Elasticsearch's rank_feature): a one-term leaf whose term id is
+ * SA_FEATURE_TERM(fn, slot) scores the index's feature column `slot` (sa_index_set_feature; on the clause's field in
+ * the multi-field call) through function fn, with its parameter in clause_idf[c].  With x the doc's value, v = +0
+ * where x is 0, and otherwise:
+ *   SA_FEATURE_LINEAR      v = x                                             (clause_idf[c] must be 0)
+ *   SA_FEATURE_SATURATION  v = x / (x + pivot), each step rounded to float32  (pivot = clause_idf[c], finite, > 0)
+ *   SA_FEATURE_LOG         v = float32(log(double(s) + double(x)))             (s = clause_idf[c], finite, >= 1)
+ * The clause matches where v > 0 and is otherwise a leaf like a term: counted once towards mm, w * v added under MUST
+ * / SHOULD, a leaf's role under FILTER / MUST_NOT.  It is not a DisMax member of a group of two or more.  An Or / And
+ * batch holding one runs as the roles layer with every clause SHOULD and weight 1 (the same result).  A reserved id
+ * naming an unknown function or a slot not set on the index, a reserved id inside a phrase, and a parameter out of
+ * range are SA_ERR_ARG before any device work.  Only the boolean entry points read reserved ids; every other entry
+ * point takes them as the out-of-range term ids they are.
+ *
  * Arrays given in a pairing other than those above (weights without occurs, groups without ties or without occurs,
  * clause_node without groups, n_nodes != n_queries without clause_node) are SA_ERR_ARG before any device work. */
 #define SA_BOOL_MAX_CLAUSES 64
@@ -217,6 +231,18 @@ int sa_score_batch_topk_sim(sa_index *index, int kind, const uint32_t *terms, co
 #define SA_OCCUR_FILTER 2
 #define SA_OCCUR_MUST_NOT 3
 #define SA_NO_NODE 0xFFFFFFFFu
+/* Per-document feature columns of an index (popularity, votes, a quality score), read by the feature clauses above.
+ * sa_index_set_feature copies values[0 .. n_values) (n_values == the index's n_docs; each finite and >= 0, 0 meaning
+ * the doc lacks the feature) into slot `slot` (< SA_MAX_FEATURES), replacing what the slot held, and records per
+ * 8,192-doc tile whether any value is > 0.  The index owns the copy and frees it with itself.  A bad argument, or an
+ * index whose n_terms reaches SA_FEATURE_TERM_BASE, is SA_ERR_ARG and leaves the index as it was. */
+#define SA_MAX_FEATURES 16
+#define SA_FEATURE_TERM_BASE 0xFF000000u
+#define SA_FEATURE_LINEAR 0
+#define SA_FEATURE_SATURATION 1
+#define SA_FEATURE_LOG 2
+#define SA_FEATURE_TERM(fn, slot) (SA_FEATURE_TERM_BASE | ((uint32_t)(fn) << 8) | (uint32_t)(slot))
+int sa_index_set_feature(sa_index *index, uint32_t slot, const float *values, uint64_t n_values);
 int sa_score_batch_topk_bool(sa_index *index, uint32_t n_nodes, const uint32_t *node_clause_starts,
                              const uint32_t *clause_node, const uint32_t *clause_terms,
                              const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,

@@ -54,6 +54,7 @@ SIGNATURES = {
     "sa_score_batch_topk_sim": (c_int, [P_void, c_int, P_u32, P_u32, ctypes.POINTER(ctypes.c_double), c_u32, c_u32,
                                         P_f32, ctypes.c_double, ctypes.c_double, ctypes.c_double, c_u32, P_u32, c_u64,
                                         c_u64, P_u32, ctypes.POINTER(ctypes.c_double)]),
+    "sa_index_set_feature": (c_int, [P_void, c_u32, P_f32, c_u64]),
     "sa_score_batch_topk_bool": (c_int, [P_void, c_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8, P_u32, P_f32,
                                          P_u32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32, P_u32, c_u64, c_u64, P_u32,
                                          P_f32, P_u32]),

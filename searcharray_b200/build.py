@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libsearcharray_b200.so")
 SOURCES = ["sa_index.cu", "sa_term.cu", "sa_topk.cu", "sa_phrase.cu", "sa_span.cu", "sa_filter.cu", "sa_edismax.cu", "sa_similarity.cu", "sa_comm.cu", "sa_setops.cu", "sa_build.cu",
-           "sa_view.cu", "sa_bool.cu"]
+           "sa_view.cu", "sa_bool.cu", "sa_feature.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall", "-fmad=false"]
 

@@ -47,11 +47,18 @@
 // empty before any of its lists is read, and a disallowed doc is zeroed with the docs below mm, before the tile's
 // bound is taken, so the mask never changes a score, only which docs rank.  In a nested call only the top-level launch
 // is masked: a disallowed doc never ranks whatever its nested rows hold.
+//
+// FEATURE: feature clauses (sa_index_set_feature) on the OCCUR, FIELDS, DISMAX and NESTED forms, in instances of
+// their own (bool_feature_kernel) so that a batch without one runs the instances above unchanged.  A feature clause
+// is present in a tile iff its column's tile flag is set; in the fold its owners read their float4s of the column with
+// cached loads (the CTAs of a batch's queries on one tile read the same 32 KB) and put v = f(x) into the shared tile,
+// which the term clauses' fold then reads as it reads BM25 scores.  An Or / And batch with a feature runs as OCCUR.
 #include "sa_multi.cuh"
 #include "sa_term.cuh"
 #include "sa_phrase.cuh"
 
 #define SA_BOOL_NO_ROW 0xFFFFFFFFu
+#define SA_BOOL_FEATURE_ROW 0xFFFFFFFEu     // BoolClause::row of a feature clause (FEATURE instances)
 
 struct BoolClause {
     u64 word_off, n_words, dir_off, rec_off;   // a term clause's list (TermQuery's fields); n_words == 0: no doc
@@ -109,6 +116,14 @@ struct BoolNest {
     u32 n_tiles;
 };
 
+// A feature clause's column and function (FEATURE instances only), per clause as a.clauses; unused at other clauses.
+struct BoolFeature {
+    const float *values;    // the column, float [padded n_docs], zero past n_docs
+    const u32 *tiles;       // its tile flags: 1 where some value of the tile is > 0
+    float param;            // SA_FEATURE_SATURATION: pivot; SA_FEATURE_LOG: scaling factor
+    u32 fn;                 // SA_FEATURE_*
+};
+
 struct BoolState {
     DevBuf d_clauses, d_queries, d_out_index;
     DevBuf d_occur;
@@ -119,6 +134,7 @@ struct BoolState {
     DevBuf d_keys;       // nq * k result keys, then u32 overflow[nq]: one device-to-host copy
     DevBuf rows;
     DevBuf d_where;      // the WhereMask rows of a masked call
+    DevBuf d_feat;       // BoolFeature[] of a call with feature clauses
 };
 void BoolStateDelete::operator()(BoolState *s) const { delete s; }
 
@@ -151,6 +167,28 @@ __device__ __forceinline__ void bool_scatter_term(const BoolArgs &a, const BoolC
         }
         const u32 rel = (u32)(doc - tile_doc0_abs);
         s_tile[rel] = cl.sparse ? bm25_from_norm((float)tf, __ldg(norm + rel), cl.idf) : (float)tf;
+    }
+}
+
+// FEATURE: v of a doc whose feature value is x: +0 where x is 0, else x, x / (x + pivot) rounded step by step, or
+// log(s + x) in double rounded once (Lucene's FeatureField functions).
+__device__ __forceinline__ float bool_feature_value(const BoolFeature &f, float x) {
+    if (!(x > 0.0f)) return 0.0f;
+    if (f.fn == SA_FEATURE_SATURATION) return __fdiv_rn(x, __fadd_rn(x, f.param));
+    if (f.fn == SA_FEATURE_LOG) return __double2float_rn(log(__dadd_rn((double)f.param, (double)x)));
+    return x;
+}
+
+// FEATURE: a feature clause's v at the thread's own docs into s_tile (each thread its own float4s, which it reads
+// back in the fold).  Not unrolled: the fold's registers stay live across it.
+__device__ __forceinline__ void bool_feature_tile(const BoolFeature &f, u32 tile_doc0, float4 *s_tile4) {
+    const float4 *__restrict__ v4 = reinterpret_cast<const float4 *>(f.values + tile_doc0);
+#pragma unroll 1
+    for (int j = 0; j < SA_TILE_DOCS / SA_TERM_THREADS / 4; j++) {
+        const unsigned g = threadIdx.x + j * SA_TERM_THREADS;
+        const float4 x = __ldg(v4 + g);
+        s_tile4[g] = make_float4(bool_feature_value(f, x.x), bool_feature_value(f, x.y), bool_feature_value(f, x.z),
+                                 bool_feature_value(f, x.w));
     }
 }
 
@@ -248,13 +286,15 @@ __device__ __forceinline__ void bool_publish_empty(const TopkCtx &t, u32 q, u32 
 // phrase rows and the top-k context stay common.  DISMAX (with OCCUR and FIELDS): clauses form groups (grp[], indexed
 // as a.clauses); mm counts SHOULD groups; s_dyn holds the groups' running max and sum, 2 * 32 floats per thread, and
 // s_g[3] (shared) the groups' presence masks.  NESTED (with DISMAX): nested clauses and the store pass (BoolNest).
-// WHERE: only docs whose bit of the mask row of query blockIdx.x is set rank (never in a store pass).
-template <bool OCCUR, bool FIELDS, bool DISMAX = false, bool NESTED = false, bool WHERE = false>
+// WHERE: only docs whose bit of the mask row of query blockIdx.x is set rank (never in a store pass).  FEATURE (with
+// OCCUR): clauses whose row is SA_BOOL_FEATURE_ROW score their column feat[clause] (BoolFeature).
+template <bool OCCUR, bool FIELDS, bool DISMAX = false, bool NESTED = false, bool WHERE = false, bool FEATURE = false>
 __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__restrict__ occ,
                                           const BoolField *__restrict__ fld,
                                           const BoolGroup *__restrict__ grp = nullptr, float *s_dyn = nullptr,
                                           unsigned long long *s_g = nullptr, const BoolNest nb = BoolNest{},
-                                          const WhereMask wh = WhereMask{nullptr, 0}) {
+                                          const WhereMask wh = WhereMask{nullptr, 0},
+                                          const BoolFeature *__restrict__ feat = nullptr) {
     constexpr int PER = SA_TILE_DOCS / SA_TERM_THREADS / 4;        // float4 groups per thread
     __shared__ __align__(16) float s_tile[SA_TILE_DOCS];
     __shared__ u32 s_lo[SA_BOOL_MAX_CLAUSES], s_hi[SA_BOOL_MAX_CLAUSES];
@@ -295,6 +335,8 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
         u32 lo = 0, hi = 0;
         if (NESTED && nb.nested[bq.c0 + c]) {
             hi = nb.flags[(u64)cl.row * nb.n_tiles + tile] != 0;   // the child ranks a doc of the tile
+        } else if (FEATURE && cl.row == SA_BOOL_FEATURE_ROW) {
+            hi = __ldg(feat[bq.c0 + c].tiles + tile) != 0;          // some doc of the tile has a value > 0
         } else if (cl.row != SA_BOOL_NO_ROW) {
             hi = 1;                                                 // a phrase row counts as present
         } else if (cl.n_words == 0) {
@@ -378,7 +420,8 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
         const BoolArgs &ca = FIELDS ? view : a;
         if (FIELDS) p = ca.bm25;
         p.idf = cl.idf;
-        if (cl.row != SA_BOOL_NO_ROW) {
+        const bool feature = FEATURE && cl.row == SA_BOOL_FEATURE_ROW;
+        if (cl.row != SA_BOOL_NO_ROW && !feature) {
             // phrase clause (sparse-safe parameters only): BM25 of its counts, zero counts score +0.  NESTED: a nested
             // clause's row holds its child's ranked scores (>= +0), read as they are
             const bool nested = NESTED && nb.nested[bq.c0 + c];
@@ -405,7 +448,9 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
                 }
             }
         } else {
-            bool_scatter_term(ca, cl, lo, hi, tile_doc0, tile_doc0_abs, s_tile);
+            // a feature clause (sparse, so v is read as it is) or a term clause
+            if (feature) bool_feature_tile(feat[bq.c0 + c], tile_doc0, s_tile4);
+            else bool_scatter_term(ca, cl, lo, hi, tile_doc0, tile_doc0_abs, s_tile);
             __syncthreads();
 #pragma unroll
             for (int j = 0; j < PER; j++) {
@@ -495,6 +540,18 @@ bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const Bool
     }
 }
 
+// The FEATURE instances: bool_tile_kernel's forms from OCCUR up, with the batch's feature table.  The DisMax shared
+// layout needs no tuned placement here (s_g a local of the kernel, as the masked instances have it).
+template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, int MIN_CTAS>
+__global__ void __launch_bounds__(SA_TERM_THREADS, MIN_CTAS)
+bool_feature_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
+                    const BoolGroup *__restrict__ grp, const BoolNest nb, const WhereMask wh,
+                    const BoolFeature *__restrict__ feat) {
+    extern __shared__ __align__(16) float s_dyn[];
+    __shared__ unsigned long long s_g[3];
+    bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, true>(a, occ, fld, grp, s_dyn, s_g, nb, wh, feat);
+}
+
 // ------------------------------------------------------------------------------------------------------------ host
 namespace {
 
@@ -517,6 +574,20 @@ BoolKernel bool_kernel(BoolForm form, bool masked) {
         {bool_tile_kernel<true, true, true, true, false, 2>, bool_tile_kernel<true, true, true, true, true, 2>},
     };
     return instances[form][masked];
+}
+
+typedef void (*BoolFeatureKernel)(BoolArgs, const BoolOccur *, const BoolField *, const BoolGroup *, BoolNest,
+                                  WhereMask, const BoolFeature *);
+
+// The FEATURE instance a launch of `form` (BOOL_OCCUR or above) runs, each at its form's CTAs per SM.
+BoolFeatureKernel bool_feature_kernel_for(BoolForm form, bool masked) {
+    static const BoolFeatureKernel instances[4][2] = {
+        {bool_feature_kernel<true, false, false, false, false, 3>, bool_feature_kernel<true, false, false, false, true, 3>},
+        {bool_feature_kernel<true, true, false, false, false, 3>, bool_feature_kernel<true, true, false, false, true, 3>},
+        {bool_feature_kernel<true, true, true, false, false, 2>, bool_feature_kernel<true, true, true, false, true, 2>},
+        {bool_feature_kernel<true, true, true, true, false, 2>, bool_feature_kernel<true, true, true, true, true, 2>},
+    };
+    return instances[form - BOOL_OCCUR][masked];
 }
 
 // The fields of one call and where the call keeps its state.  The single-index entry point passes one field and the
@@ -552,6 +623,7 @@ struct BoolPlan {
     std::vector<u32> nested;            // nested nodes by (launch group, depth desc, top-level query); queries[n_top + i]
                                         // is nested[i]'s descriptor
     std::vector<u32> nest;              // per clause, as clauses: 1 for a nested clause (BOOL_NESTED)
+    std::vector<BoolFeature> features;  // per clause, as clauses, when a clause is a feature (the FEATURE instances)
 };
 
 // The count rows of the phrase clauses of queries [q0, q1) and of their nested nodes (rows are numbered within the
@@ -567,7 +639,7 @@ int bool_build_rows(const BoolCall &X, const BoolPlan &P, const uint32_t *clause
     for (u32 n : nodes) {
         for (u32 c = P.node_starts[n]; c < P.node_starts[n + 1]; c++) {
             const BoolClause &cl = P.clauses[c];
-            if (cl.row == SA_BOOL_NO_ROW || (!P.nest.empty() && P.nest[c])) continue;
+            if (cl.row == SA_BOOL_NO_ROW || cl.row == SA_BOOL_FEATURE_ROW || (!P.nest.empty() && P.nest[c])) continue;
             sa_index *ix = X.ix[cl.field];
             bool scored;
             if ((rc = sa_phrase_row(ix, clause_terms + clause_term_starts[c], clause_term_starts[c + 1] - clause_term_starts[c],
@@ -617,11 +689,20 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
     const BoolGroup *grp = P.form >= BOOL_DISMAX ? S.d_groups.as<BoolGroup>() : nullptr;
     BoolNest nb{nullptr, nullptr, nullptr, 0};
     const size_t smem = P.form >= BOOL_DISMAX ? SA_BOOL_DISMAX_SMEM : 0;
+    // the form's instance, or its FEATURE instance when the call has feature clauses
+    const BoolFeature *feat = P.features.empty() ? nullptr : S.d_feat.as<BoolFeature>();
+    auto launch = [&](bool masked, u32 n_q, const BoolArgs &args, const BoolNest &n, const WhereMask &w) {
+        const dim3 grid(n_q, n_tiles);
+        if (feat)
+            bool_feature_kernel_for(P.form, masked)<<<grid, SA_TERM_THREADS, smem, ix->stream>>>(args, occ, fld, grp, n,
+                                                                                             w, feat);
+        else
+            bool_kernel(P.form, masked)<<<grid, SA_TERM_THREADS, smem, ix->stream>>>(args, occ, fld, grp, n, w);
+    };
     if (P.form == BOOL_NESTED) {
         // the nested nodes of these queries, deepest level first (one launch per level: a level's nodes of the run
         // are consecutive in P.nested), each into its row and flags, unmasked; then the top-level nodes, collected
         nb = BoolNest{S.d_nest.as<u32>(), S.d_flags.as<u32>(), S.rows.as<float>(), n_tiles};
-        const BoolKernel store = bool_kernel(BOOL_NESTED, false);
         for (size_t i = 0; i < P.nested.size();) {
             auto in_run = [&](size_t x) { return P.root[P.nested[x]] >= q0 && P.root[P.nested[x]] < q1; };
             if (!in_run(i)) { i++; continue; }
@@ -629,16 +710,14 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
             while (j < P.nested.size() && in_run(j) && P.depth[P.nested[j]] == P.depth[P.nested[i]]) j++;
             BoolArgs an = a;
             an.queries = S.d_queries.as<BoolQuery>() + P.n_top + i;
-            store<<<dim3((u32)(j - i), n_tiles), SA_TERM_THREADS, smem, ix->stream>>>(an, occ, fld, grp, nb,
-                                                                                     WhereMask{nullptr, 0});
+            launch(false, (u32)(j - i), an, nb, WhereMask{nullptr, 0});
             SA_CUDA(cudaGetLastError());
             ix->stats.total_launches++;
             i = j;
         }
         nb.store = nullptr;
     }
-    bool_kernel(P.form, wh.bits != nullptr)<<<dim3(nq, n_tiles), SA_TERM_THREADS, smem, ix->stream>>>(
-        a, occ, fld, grp, nb, wh);
+    launch(wh.bits != nullptr, nq, a, nb, wh);
     SA_CUDA(cudaGetLastError());
     ix->stats.total_launches++;
     return launch_topk_select(ix, t, nq, ix->doc_base, d_keys, S.d_out_index.as<u32>() + q0);
@@ -646,12 +725,30 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
 
 // The DisMax instances' dynamic shared memory above the default 48 KB, and the carveout that fits two CTAs per SM
 // (~2 x 98 KB of shared memory), on the current device (function attributes are per device).
-int bool_dismax_smem(BoolKernel kernel) {
+template <typename Kernel>
+int bool_dismax_smem(Kernel kernel) {
     SA_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SA_BOOL_DISMAX_SMEM));
     SA_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
                                  (int)cudaSharedmemCarveoutMaxShared));
     return SA_OK;
 }
+
+// A feature clause's reserved term id and parameter (include/searcharray_b200.h), on index ix: SA_ERR_ARG unless
+// its function is known, its slot set on ix and its parameter in range.
+int bool_check_feature(const sa_index *ix, u32 c, u32 term, float param) {
+    const u32 fn = (term >> 8) & 0xFFFFu, slot = term & 0xFFu;
+    SA_CHECK(fn <= SA_FEATURE_LOG, "clause %u: term id 0x%08x names no feature function", c, term);
+    SA_CHECK(slot < SA_MAX_FEATURES && (ix->feature_set >> slot & 1u), "clause %u: feature slot %u is not set", c,
+             slot);
+    SA_CHECK(fn != SA_FEATURE_LINEAR || param == 0.0f, "clause %u: a linear feature takes no parameter (0)", c);
+    SA_CHECK(fn != SA_FEATURE_SATURATION || (std::isfinite(param) && param > 0.0f),
+             "clause %u: a saturation pivot is finite and > 0", c);
+    SA_CHECK(fn != SA_FEATURE_LOG || (std::isfinite(param) && param >= 1.0f),
+             "clause %u: a log scaling factor is finite and >= 1", c);
+    return SA_OK;
+}
+
+bool bool_is_feature_term(u32 t) { return t >= SA_FEATURE_TERM_BASE && t != SA_NO_TERM; }
 
 // Both entry points, with the call's indexes locked and their device current.  clause_weight / clause_occur NULL:
 // Or / And, every clause SHOULD with weight 1, mm over all.  clause_field NULL: every clause on field 0.
@@ -722,6 +819,7 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
     for (u32 n = n_queries; nested && n < n_nodes; n++) SA_CHECK(refs[n] == 1, "node %u is referenced by no clause", n);
     if ((rc = sa_where_check(X.where_bits, X.where_n, X.where_stride, lead->n_docs))) return rc;
     const u32 c_begin = n_nodes ? query_clause_starts[0] : 0, c_end = n_nodes ? query_clause_starts[n_nodes] : 0;
+    bool features = false;
     for (u32 c = c_begin; c < c_end; c++) {
         if (is_nested(c)) continue;
         const u32 nt = clause_term_starts[c + 1] - clause_term_starts[c];
@@ -729,15 +827,36 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
                  "clause %u: bad number of terms", c);
         const u32 f = clause_field ? clause_field[c] : 0;
         SA_CHECK(f < n_fields, "clause %u: field %u out of range (%u fields)", c, f, n_fields);
-        if ((rc = sa_check_term_ids(X.ix[f], clause_terms + clause_term_starts[c], nt))) return rc;
+        const u32 *tids = clause_terms + clause_term_starts[c];
+        if (nt == 1 && bool_is_feature_term(tids[0])) {
+            if ((rc = bool_check_feature(X.ix[f], c, tids[0], clause_idf[c]))) return rc;
+            SA_CHECK(!dismax || ((c == c_begin || clause_group[c - 1] != clause_group[c]) &&
+                                 (c + 1 == c_end || clause_group[c + 1] != clause_group[c])),
+                     "clause %u: a feature clause is not a DisMax member", c);
+            features = true;
+            continue;
+        }
+        for (u32 i = 0; i < nt; i++)
+            SA_CHECK(!bool_is_feature_term(tids[i]), "clause %u: a feature term id inside a phrase", c);
+        if ((rc = sa_check_term_ids(X.ix[f], tids, nt))) return rc;
     }
+    // an Or / And batch with a feature clause runs as roles and weights, every clause SHOULD with weight 1
+    std::vector<float> ones;
+    std::vector<uint8_t> shoulds;
+    if (features && !occur) {
+        ones.assign(c_end, 1.0f);
+        shoulds.assign(c_end, SA_OCCUR_SHOULD);
+        clause_weight = ones.data();
+        clause_occur = shoulds.data();
+    }
+    const bool roles = occur || features;
     const size_t nk = (size_t)n_queries * k;
     for (size_t i = 0; i < nk; i++) { out_docs[i] = SA_NO_DOC; out_scores[i] = 0.0f; }
     // .score is all zeros on a field whose avgdl is 0: its clauses are empty (below), and without any other field
     // nothing ranks
     bool any_avgdl = false;
     for (u32 f = 0; f < n_fields; f++) any_avgdl = any_avgdl || X.avgdl[f] != 0.0f;
-    if (n_queries == 0 || lead->n_docs == 0 || !any_avgdl) return SA_OK;
+    if (n_queries == 0 || lead->n_docs == 0 || (!any_avgdl && !features)) return SA_OK;
 
     // descriptors, and the groups: at most ~1 GB of candidate slots and ~4 GB of phrase rows per launch
     const u32 n_tiles = sa_n_tiles(lead->n_docs), slots = sa_topk_slots(k);
@@ -745,7 +864,7 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
     const u32 group_q = (u32)std::min<u64>(65535, std::max<u64>(1, (1ull << 30) / ((u64)n_tiles * (slots * sizeof(u64) + 8))));
     const u32 group_rows = (u32)std::max<u64>(1, (4ull << 30) / (stride * sizeof(float)));
     BoolPlan P;
-    P.form = nested ? BOOL_NESTED : dismax ? BOOL_DISMAX : X.fields_kernel ? BOOL_FIELDS : occur ? BOOL_OCCUR : BOOL_OR_AND;
+    P.form = nested ? BOOL_NESTED : dismax ? BOOL_DISMAX : X.fields_kernel ? BOOL_FIELDS : roles ? BOOL_OCCUR : BOOL_OR_AND;
     P.n_top = n_queries;
     P.node_starts.assign(query_clause_starts, query_clause_starts + n_nodes + 1);
     P.root.resize(n_nodes);
@@ -811,13 +930,22 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
             sa_index *ix = X.ix[f];
             const u32 *tids = clause_terms + clause_term_starts[c];
             const u32 nt = clause_term_starts[c + 1] - clause_term_starts[c];
-            if (occur) P.occur.push_back(BoolOccur{clause_weight[c], clause_occur[c]});
+            if (roles) P.occur.push_back(BoolOccur{clause_weight[c], clause_occur[c]});
             // a member of a group of two or more: scores >= +0 everywhere (sparse-safe), which its max relies on
             const bool member = dismax && ((c > c0 && clause_group[c] == clause_group[c - 1]) ||
                                            (c + 1 < c1 && clause_group[c + 1] == clause_group[c]));
             if (dismax)
                 P.groups.push_back(BoolGroup{clause_tie[clause_group[c]], clause_group[c] - c0, member ? 1u : 0u,
                                              member && (c + 1 == c1 || clause_group[c + 1] != clause_group[c]) ? 1u : 0u});
+            if (nt == 1 && bool_is_feature_term(tids[0])) {   // its column on its field's index
+                const u32 slot = tids[0] & 0xFFu, fn = (tids[0] >> 8) & 0xFFFFu;
+                P.features.resize(c_end);
+                P.features[P.clauses.size()] = BoolFeature{ix->d_features[slot].as<float>(),
+                                                           ix->d_feature_tiles.as<u32>() + (size_t)slot * n_tiles,
+                                                           clause_idf[c], fn};
+                P.clauses.push_back(BoolClause{0, 0, SA_NO_DIR, SA_NO_DIR, 0.0f, SA_BOOL_FEATURE_ROW, 1u, f});
+                continue;
+            }
             if (X.avgdl[f] == 0.0f) {       // scores +0 at every doc: no list, no row
                 P.clauses.push_back(BoolClause{0, 0, SA_NO_DIR, SA_NO_DIR, clause_idf[c], SA_BOOL_NO_ROW, 1u, f});
                 continue;
@@ -864,14 +992,21 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
     std::vector<u32> identity(n_queries);
     for (u32 q = 0; q < n_queries; q++) identity[q] = q;
     SA_CUDA(cudaMemcpyAsync(S.d_clauses.p, P.clauses.data(), P.clauses.size() * sizeof(BoolClause), cudaMemcpyHostToDevice, lead->stream));
-    if (occur) {
+    if (roles) {
         SA_CUDA(cudaMemcpyAsync(S.d_occur.p, P.occur.data(), P.occur.size() * sizeof(BoolOccur), cudaMemcpyHostToDevice, lead->stream));
+    }
+    if (!P.features.empty()) {
+        if ((rc = S.d_feat.reserve(P.features.size() * sizeof(BoolFeature)))) return rc;
+        SA_CUDA(cudaMemcpyAsync(S.d_feat.p, P.features.data(), P.features.size() * sizeof(BoolFeature),
+                                cudaMemcpyHostToDevice, lead->stream));
     }
     if ((rc = sa_where_upload(lead, S.d_where, X.where_bits, lead->n_docs, X.where_stride, n_queries, &X.where)))
         return rc;
     if (dismax) {
-        if ((rc = bool_dismax_smem(bool_kernel(P.form, false))) ||
-            (X.where.bits && (rc = bool_dismax_smem(bool_kernel(P.form, true)))))
+        if (P.features.empty() ? ((rc = bool_dismax_smem(bool_kernel(P.form, false))) ||
+                                  (X.where.bits && (rc = bool_dismax_smem(bool_kernel(P.form, true)))))
+                               : ((rc = bool_dismax_smem(bool_feature_kernel_for(P.form, false))) ||
+                                  (X.where.bits && (rc = bool_dismax_smem(bool_feature_kernel_for(P.form, true))))))
             return rc;
         SA_CUDA(cudaMemcpyAsync(S.d_groups.p, P.groups.data(), P.groups.size() * sizeof(BoolGroup), cudaMemcpyHostToDevice, lead->stream));
     }

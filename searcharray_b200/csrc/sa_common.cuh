@@ -200,6 +200,12 @@ struct sa_index {
     DevBuf d_norm;                   // float [padded n_docs]
     float norm_k1 = 0, norm_b = 0, norm_avgdl = 0;
     bool norm_valid = false;
+    // feature columns (sa_index_set_feature, sa_feature.cu): slot s, when bit s of feature_set is set, is
+    // d_features[s] (float [padded n_docs], zero past n_docs) and its tile flags d_feature_tiles[s * n_tiles + t]
+    // (1: some doc of tile t has a value > 0)
+    DevBuf d_features[SA_MAX_FEATURES];
+    DevBuf d_feature_tiles;          // u32 [SA_MAX_FEATURES * n_tiles]
+    u32 feature_set = 0;
     // host mirrors for query set-up
     std::vector<u64> h_off, h_len;
     std::vector<u32> h_df;

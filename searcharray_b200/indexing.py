@@ -61,6 +61,9 @@ class HostIndex:
         if avg_doc_length is None:
             avg_doc_length = np.mean(self.doc_lens) if len(self.doc_lens) else 0
         self.avg_doc_length = avg_doc_length
+        # per-doc feature columns (SearchArray.set_feature): name -> float32[n_docs]; a name's slot on the device
+        # index is its position in this dict
+        self.features = {}
 
     # ---- on-disk posting words (reference phrase/memmap_arrays.py:145-208, MemoryMappedArrays): the words
     #      array written once to `<data_dir>/<n>.dat`, mapped back read-only; pickling stores the file name
@@ -87,6 +90,7 @@ class HostIndex:
 
     def __setstate__(self, st):
         self.__dict__.update(st)
+        self.__dict__.setdefault("features", {})
         if st.get("words_file"):
             self._map_words()
 
@@ -117,7 +121,9 @@ class HostIndex:
             lens.append(b - a)
             total += b - a
         words = np.concatenate(parts) if parts else np.empty(0, dtype=np.uint64)
-        return HostIndex(words, offs, lens, self.doc_lens[doc_lo:doc_hi], self.term_dict, self.avg_doc_length)
+        out = HostIndex(words, offs, lens, self.doc_lens[doc_lo:doc_hi], self.term_dict, self.avg_doc_length)
+        out.features = {name: v[doc_lo:doc_hi].copy() for name, v in self.features.items()}
+        return out
 
 
 def build_index(array, tokenizer, truncate=False, gpu_build=None):

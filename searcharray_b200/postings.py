@@ -195,6 +195,15 @@ class DeviceIndex:
             _lib.p_u64(host.term_lengths), host.n_terms, _lib.p_f32(host.doc_lens), host.n_docs,
             doc_base, device, ctypes.byref(self.handle)))
         self._finalizer = weakref.finalize(self, DeviceIndex._destroy, self.handle)
+        self.features = {}          # slot -> the host array last uploaded there
+        self.sync_features(host)
+
+    def sync_features(self, host: HostIndex):
+        """Uploads every feature column of `host` that this index does not hold yet (sa_index_set_feature)."""
+        for slot, values in enumerate(host.features.values()):
+            if self.features.get(slot) is not values:
+                _lib.check(_lib.lib().sa_index_set_feature(self.handle, slot, _lib.p_f32(values), len(values)))
+                self.features[slot] = values
 
     @staticmethod
     def _destroy(handle):
@@ -521,6 +530,44 @@ class SearchArray(ExtensionArray):
             out.append(decode_positions(w[a:b]))
         return out
 
+    # -------------------------------------------------------------------- features
+    def set_feature(self, name: str, values) -> None:
+        """Registers a per-document numeric column -- popularity, vote count, recency, a quality score -- for
+        query.Feature clauses of search_topk and solr.fields_topk.  values: one finite number >= 0 per doc of the
+        array (on a shard, per row of the shard), rounded once to float32; 0 means the doc lacks the feature.  Another
+        length, NaN, inf or a negative value is a ValueError, a non-numeric dtype a TypeError, both before any device
+        work.  Setting a name again replaces its values; at most 16 names per index.  Refused (ValueError) on a view,
+        whose positions are not the index's docs.  The values live with the index (copies and pickles carry them) and
+        go to the device when it is first used, or at once if it already is."""
+        from .query import SA_MAX_FEATURES
+        if not isinstance(name, str):
+            raise TypeError(f"a feature name is a str, not {name!r}")
+        if self.rows is not None:
+            raise ValueError("set_feature on a view (arr[mask]) is not supported: set it on the whole array")
+        v = np.asarray(values)
+        if v.dtype.kind not in "iuf":
+            raise TypeError(f"feature values are numbers (int or float), not dtype {v.dtype}")
+        if v.shape != (self.host.n_docs,):
+            raise ValueError(f"a feature has one value per doc: shape ({self.host.n_docs},), not {v.shape}")
+        with np.errstate(over="ignore"):
+            v32 = np.ascontiguousarray(v, dtype=np.float32).copy()
+        if not (np.all(np.isfinite(v)) and np.all(np.isfinite(v32))) or np.any(v < 0):
+            raise ValueError(f"feature values are finite and >= 0 (in float32): {name!r}")
+        feats = self.host.features
+        if name not in feats and len(feats) >= SA_MAX_FEATURES:
+            raise ValueError(f"an index holds at most {SA_MAX_FEATURES} features")
+        with self._shared["lock"]:
+            feats[name] = v32
+            if self._shared["dev"] is not None:
+                self._shared["dev"].sync_features(self.host)
+
+    def _feature_slot(self, name):
+        """The slot of feature `name` on this array's index; ValueError if it is not set."""
+        names = list(self.host.features)
+        if name not in names:
+            raise ValueError(f"feature {name!r} is not set on this array (set_feature); set: {names}")
+        return names.index(name)
+
     # -------------------------------------------------- batched, HBM-resident path
     def search_topk(self, queries, k=10, similarity: Similarity = default_bm25, slop=0, where=None):
         """queries: list of str (term) or list[str] (phrase).  Returns (docs uint32[Q,k],
@@ -567,9 +614,12 @@ class SearchArray(ExtensionArray):
         refused without `where` is refused the same way with it.  Plain BM25 queries on the unsliced array rank as
         one-clause Or queries (sa_score_batch_topk_bool); the others take sa_score_batch_topk_sim.  A
         mask per query costs len(self) / 8 bytes of host-to-device copy and device memory per query."""
-        from .query import is_boolean
+        from .query import Feature, is_boolean
+        queries = list(queries)
+        for q in queries:
+            if isinstance(q, Feature):
+                raise TypeError(f"a Feature is a clause, not a query: write Bool(should=[{q!r}])")
         if where is not None:
-            queries = list(queries)
             bits = pack_where(where, len(self), len(queries))
             if any(is_boolean(q) for q in queries):
                 return self._search_topk_mixed(queries, k, similarity, slop, bits)
@@ -678,12 +728,15 @@ class SearchArray(ExtensionArray):
         """Boolean queries of any form through sa_score_batch_topk_bool, flattened for the heaviest form among them
         (query.bool_form, flatten_bool): (docs, scores, queries re-run exactly).  DisMax members anywhere in the trees
         need sparse-safe BM25 parameters (ValueError before any device work).  where: a packed mask (pack_where)."""
-        from .query import DISMAX, OR_AND, bool_form, check_dismax_members, dismax_members, flatten_bool
+        from .query import DISMAX, OR_AND, bool_form, check_dismax_members, dismax_members, feature_terms, flatten_bool
         form = max(map(bool_form, queries), default=OR_AND)
         batch = flatten_bool(queries, form)
         clauses = batch.clauses
+        feats = feature_terms(clauses, lambda i, f: self._feature_slot(f.name))
         idf = lambda dfs: compute_idf(self.corpus_size, dfs)      # noqa: E731
-        if batch.clause_node is None:
+        if feats:                                       # feature clauses: a reserved term id and their parameter
+            terms, c_starts, idfs = self._feature_clauses(clauses, feats, idf)
+        elif batch.clause_node is None:
             terms, c_starts, idfs = self._topk_queries(clauses, idf)
             idfs = np.asarray(idfs, dtype=np.float32)
         else:                                           # nested clauses (None): no terms, idf 0
@@ -699,7 +752,24 @@ class SearchArray(ExtensionArray):
         dev = self._device()
         with self._shared["lock"]:
             self._apply_rows(dev)
+            if feats:
+                dev.sync_features(self.host)
             return self._bool_call(dev, batch, terms, c_starts, idfs, similarity, slop, k, where)
+
+    def _feature_clauses(self, clauses, feats, idf):
+        """(terms, clause term starts, float32 idf) of a flattened clause list holding feature clauses: a text clause
+        its term ids and idf (_topk_queries), a feature clause {index: (term id, parameter)} its reserved id and
+        parameter, a nested clause (None) no terms and 0."""
+        text = [i for i, c in enumerate(clauses) if c is not None and i not in feats]
+        t, l_starts, l_idfs = self._topk_queries([clauses[i] for i in text], idf)
+        c_terms, idfs = [np.empty(0, dtype=np.uint32)] * len(clauses), np.zeros(len(clauses), dtype=np.float32)
+        for j, i in enumerate(text):
+            c_terms[i], idfs[i] = t[l_starts[j]:l_starts[j + 1]], l_idfs[j]
+        for i, (tid, param) in feats.items():
+            c_terms[i], idfs[i] = np.asarray([tid], dtype=np.uint32), param
+        c_starts = np.concatenate([[0], np.cumsum([len(x) for x in c_terms])]).astype(np.uint32)
+        terms = np.concatenate(c_terms).astype(np.uint32) if c_terms else np.empty(0, dtype=np.uint32)
+        return terms, c_starts, idfs
 
     def _topk_queries(self, queries, idf):
         """The queries as the batched top-k entries take them: term ids, start offsets and, per query, idf(dfs) of

@@ -8,8 +8,9 @@ device (sa_score_batch_topk_bool).  Bool(must, should, filter, must_not, mm) and
 composition.  Field(field, clause) names the DataFrame column a clause scores on, for queries over several columns
 (solr.fields_topk, sa_multi_score_batch_topk_bool).  DisMax(clauses, tie) is one clause scored by its best member
 plus tie times the others (Lucene's DisjunctionMaxQuery).  An Or / And / Bool may itself be a clause of another (a
-nested query, scored by what it ranks as a query of its own).  The device entry points take the queries flattened
-for their form (bool_form, flatten_bool)."""
+nested query, scored by what it ranks as a query of its own).  Feature(name, function) is a leaf scored by a
+per-document numeric column registered with SearchArray.set_feature (Lucene's FeatureField).  The device entry points
+take the queries flattened for their form (bool_form, flatten_bool)."""
 import math
 from typing import List, NamedTuple, Optional, Union
 
@@ -25,25 +26,100 @@ SA_MAX_PHRASE_TERMS = 16          # include/searcharray_b200.h
 ED_MAX_ROWS = 64                  # phrase rows of one field in one sa_multi_phrases call (sa_multi.cuh)
 ED_MAX_PHASE_ENTRIES = ED_MAX_FIELDS * SA_MAX_PHRASE_TERMS   # entries of one sa_multi_add_phase call (sa_multi.cuh)
 SA_OCCUR_SHOULD, SA_OCCUR_MUST, SA_OCCUR_FILTER, SA_OCCUR_MUST_NOT = 0, 1, 2, 3
+SA_MAX_FEATURES = 16              # include/searcharray_b200.h
+SA_FEATURE_TERM_BASE = 0xFF000000
+FEATURE_FUNCTIONS = {"linear": 0, "saturation": 1, "log": 2}     # SA_FEATURE_LINEAR, _SATURATION, _LOG
 
 Clause = Union[str, List[str]]
 
 
 def _clause(c):
-    """A clause as search_topk's query form: str (term) or list[str] (phrase), a Field of one, a DisMax, or a nested
-    Or / And / Bool; anything else is a TypeError."""
-    if isinstance(c, (str, Field, DisMax, Or, Bool)):
+    """A clause as search_topk's query form: str (term) or list[str] (phrase), a Feature, a Field of one, a DisMax, or
+    a nested Or / And / Bool; anything else is a TypeError."""
+    if isinstance(c, (str, Feature, Field, DisMax, Or, Bool)):
         return c
     if isinstance(c, (list, tuple)) and c and all(isinstance(t, str) for t in c):
         return list(c)
     raise TypeError(f"a clause is a str (term) or a non-empty list of str (phrase), not {c!r}")
 
 
+class Feature:
+    """A clause scored by a per-document numeric column of the array's index (SearchArray.set_feature): Lucene's
+    FeatureField, Elasticsearch's rank_feature -- popularity, votes, a quality score added to the text score.  With x
+    the doc's value, v = 0 where x is 0, and otherwise:
+
+      "linear"      v = x
+      "saturation"  v = x / (x + pivot), in float32 (pivot finite and > 0)
+      "log"         v = float32(log(float64(scaling_factor) + float64(x))) (scaling_factor finite and >= 1)
+
+    Parameters are rounded to float32 once; a missing, extra or out-of-range one is a ValueError, a name that is not a
+    str a TypeError.  A Feature is a leaf like a term: it matches where v > 0, counts once towards mm, adds w * v under
+    must / should (Boost(Feature(...), w)) and plays a leaf's role under filter / must_not.  It is accepted in Or,
+    And, every list of Bool and nested queries; in solr.fields_topk as Field(column, Feature(...)), the column whose
+    index holds the values.  It is not a DisMax member (TypeError), and not a query of its own in search_topk
+    (TypeError: write Bool(should=[Feature(...)])).  apply(x) is the transform in numpy."""
+
+    def __init__(self, name, function="linear", pivot=None, scaling_factor=None):
+        if not isinstance(name, str):
+            raise TypeError(f"a feature name is a str, not {name!r}")
+        if function not in FEATURE_FUNCTIONS:
+            raise ValueError(f"a feature function is one of {sorted(FEATURE_FUNCTIONS)}, not {function!r}")
+        need = {"linear": None, "saturation": "pivot", "log": "scaling_factor"}[function]
+        for key, value in (("pivot", pivot), ("scaling_factor", scaling_factor)):
+            if key == need and value is None:
+                raise ValueError(f"a {function} feature needs {key}")
+            if key != need and value is not None:
+                raise ValueError(f"a {function} feature takes no {key}")
+        param = np.float32(0.0)
+        if need is not None:
+            value = pivot if need == "pivot" else scaling_factor
+            with np.errstate(over="ignore"):
+                param = np.float32(float(value))
+            low_ok = param > 0 if need == "pivot" else param >= 1
+            if not (np.isfinite(param) and low_ok):
+                raise ValueError(f"a {function} feature's {need} is finite and {'> 0' if need == 'pivot' else '>= 1'}"
+                                 f" in float32, not {value!r}")
+        self.name, self.function, self.param = name, function, param
+
+    @property
+    def fn(self):
+        """The SA_FEATURE_* code of the function."""
+        return FEATURE_FUNCTIONS[self.function]
+
+    def term_id(self, slot):
+        """The reserved term id (SA_FEATURE_TERM) naming this function on feature slot `slot` of an index."""
+        return SA_FEATURE_TERM_BASE | (self.fn << 8) | int(slot)
+
+    def apply(self, x):
+        """v = f(x) as float32[len(x)], as the device computes it: 0 where x is not > 0."""
+        x = np.asarray(x, dtype=np.float32)
+        pos = x > 0
+        if self.function == "linear":
+            v = x
+        elif self.function == "saturation":
+            with np.errstate(under="ignore"):
+                v = x / (x + self.param)
+        else:
+            v = np.log(np.float64(self.param) + x.astype(np.float64)).astype(np.float32)
+        return np.where(pos, v, np.float32(0)).astype(np.float32)
+
+    def __repr__(self):
+        extra = {"linear": "", "saturation": f", pivot={float(self.param)!r}",
+                 "log": f", scaling_factor={float(self.param)!r}"}[self.function]
+        return f"Feature({self.name!r}, {self.function!r}{extra})"
+
+
+def _is_feature(c):
+    """Whether a clause (without its Boost) is a Feature or a Field of one."""
+    return isinstance(c, Feature) or (isinstance(c, Field) and isinstance(c.clause, Feature))
+
+
 class Field:
     """A term (str) or phrase (non-empty list of str) clause scored on the DataFrame column `field`, as
     frame[field].array.score(clause) scores it -- Lucene's `title:star`.  Accepted wherever a clause is (Or, And, the
     four lists of Bool) by solr.fields_topk, which needs every clause to name its field; SearchArray.search_topk
-    refuses it.  A boosted field clause is Boost(Field(field, clause), weight); a Field holds no Boost or Field."""
+    refuses it.  A boosted field clause is Boost(Field(field, clause), weight); a Field holds no Boost or Field.
+    Field(field, Feature(...)) is a feature clause whose values are those set on that column's index."""
 
     def __init__(self, field, clause):
         if not isinstance(field, str):
@@ -109,7 +185,7 @@ class DisMax:
             raise ValueError("a DisMax needs at least one member")
         for c in clauses:
             inner = c.clause if isinstance(c, Boost) else c
-            if isinstance(inner, (DisMax, Or, Bool)):
+            if isinstance(inner, (DisMax, Or, Bool)) or _is_feature(inner):
                 raise TypeError(f"a DisMax member is a term, a phrase or a Field of one (boosted or not), not {c!r}")
         self.clauses, self.weights = _scoring(clauses)
         t = float(tie)
@@ -289,14 +365,19 @@ def has_dismax(q):
     return any(isinstance(c, DisMax) for c in _leaves(q))
 
 
+def has_feature(q):
+    """Whether a boolean query holds a feature clause (Feature, or Field of one), nested queries included."""
+    return any(_is_feature(c) for c in _leaves(q))
+
+
 def is_nested(q):
     """Whether a boolean query holds a nested Or / And / Bool (the NESTED form)."""
     return not isinstance(q, DisMax) and any(isinstance(c, (Or, Bool)) for c in _top_clauses(q))
 
 
 def needs_occur(q):
-    """Whether q takes at least the OCCUR form: a Bool, or an Or / And with a weight other than 1."""
-    return isinstance(q, Bool) or q.boosted
+    """Whether q takes at least the OCCUR form: a Bool, an Or / And with a weight other than 1 or a feature clause."""
+    return isinstance(q, Bool) or q.boosted or has_feature(q)
 
 
 # The forms of a boolean batch, ordered: each form's arrays are those of the one before plus its own, and the C entry
@@ -306,7 +387,7 @@ OR_AND, OCCUR, DISMAX, NESTED = 1, 2, 3, 4
 
 def bool_form(q):
     """The form a boolean query takes: NESTED if it holds a nested Or / And / Bool, else DISMAX if it is or holds a
-    DisMax, else OCCUR if it is a Bool or has a weight other than 1, else OR_AND."""
+    DisMax, else OCCUR if it is a Bool, has a weight other than 1 or a feature clause, else OR_AND."""
     return DISMAX if isinstance(q, DisMax) else q.form
 
 
@@ -319,13 +400,16 @@ def _form(clauses, occur):
             return NESTED
         if isinstance(c, DisMax):
             form = DISMAX
+        elif _is_feature(c):       # the FEATURE instances start at the roles form
+            form = max(form, OCCUR)
     return form
 
 
 class BoolBatch(NamedTuple):
     """Boolean queries as sa_score_batch_topk_bool takes them (flatten_bool).  Arrays the form does not use are None,
     passed as NULL."""
-    clauses: list                   # per clause: search_topk's query form (str or list[str]); None for a nested clause
+    clauses: list                   # per clause: search_topk's query form (str, list[str] or Feature); None for a
+                                    # nested clause
     node_starts: np.ndarray         # uint32: node n's clauses are [node_starts[n], node_starts[n + 1])
     clause_node: Optional[np.ndarray]   # uint32 per clause: its nested node, else SA_NO_NODE (NESTED)
     mm: np.ndarray                  # uint32 per node
@@ -446,3 +530,15 @@ def check_dismax_members(members, params):
                 and idf >= 0 and not np.signbit(idf)):
             raise ValueError(f"DisMax members need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite idf >= 0): "
                              f"{c!r} has k1={float(k1)}, b={float(b)}, idf={float(idf)}")
+
+
+def feature_terms(clauses, slot):
+    """The feature leaves of a flattened clause list (BoolBatch.clauses) as the C entry points take them:
+    {index: (reserved term id, float32 parameter)}.  slot(i, feature) -> the feature's slot on clause i's index (it
+    raises ValueError for a name that is not set there)."""
+    out = {}
+    for i, c in enumerate(clauses):
+        f = c.clause if isinstance(c, Field) else c
+        if isinstance(f, Feature):
+            out[i] = (f.term_id(slot(i, f)), f.param)
+    return out

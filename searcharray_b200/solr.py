@@ -471,16 +471,28 @@ def _fields_plan(frame, queries, similarity):
         check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
                              lambda i: (sims[clauses[i].field].k1, sims[clauses[i].field].b,
                                         arrays[clauses[i].field].avg_doc_length, 0.0))
+    _feature_terms(batch.clauses, slot_of, slot_arrays)       # feature names set on their columns
     return batch, slot_of, slot_arrays, slot_sims
+
+
+def _feature_terms(clauses, slot_of, arrays):
+    """Field(column, Feature) clauses as query.feature_terms encodes them, each on its column's index."""
+    from .query import feature_terms
+    return feature_terms(clauses, lambda i, f: arrays[slot_of[clauses[i].field]]._feature_slot(f.name))
 
 
 def _fields_clauses(clauses, slot_of, arrays):
     """Each clause's term ids and idf from its own field, as that column's .score takes them: (terms, clause term
-    starts, float32 idf, field slots).  A nested clause (None) has no terms, idf 0 and slot 0.  Call it with the
-    fields locked (_locked)."""
+    starts, float32 idf, field slots).  A nested clause (None) has no terms, idf 0 and slot 0; a feature clause its
+    reserved term id and its parameter.  Call it with the fields locked (_locked)."""
     c_terms, c_idf = [[]] * len(clauses), np.zeros(len(clauses), dtype=np.float32)
+    feats = _feature_terms(clauses, slot_of, arrays)
+    for i, (tid, param) in feats.items():         # a feature clause: its reserved term id and parameter
+        c_terms[i], c_idf[i] = _u32([tid]), param
     for s, arr in enumerate(arrays):
-        idx = [i for i, c in enumerate(clauses) if c is not None and slot_of[c.field] == s]
+        if any(slot_of[clauses[i].field] == s for i in feats):
+            arr._device().sync_features(arr.host)
+        idx = [i for i, c in enumerate(clauses) if c is not None and i not in feats and slot_of[c.field] == s]
         t, st, idf = arr._topk_queries([clauses[i].clause for i in idx],
                                        lambda dfs, arr=arr: compute_idf(arr.corpus_size, dfs))
         for j, i in enumerate(idx):
