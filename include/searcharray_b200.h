@@ -223,9 +223,22 @@ int sa_score_batch_topk_sim(sa_index *index, int kind, const uint32_t *terms, co
  * range are SA_ERR_ARG before any device work.  Only the boolean entry points read reserved ids; every other entry
  * point takes them as the out-of-range term ids they are.
  *
+ * Hit and facet counts (the _counts entry points below, out_total non-NULL): Lucene's totalHits and Elasticsearch's terms aggregations, counted where
+ * the fold decides which docs rank.  out_total[q] is the number of docs query q ranks (the docs whose score the top k
+ * is taken from: s > 0 and every condition above, mask included), over all of them, not only the top k.  With
+ * n_facets (<= SA_BOOL_MAX_FACETS) facets, facet i is the facet column facet_slot[i] (sa_index_set_facet) of the index
+ * of field facet_field[i] (0 on the single-index entry point; a field slot of the multi on the multi-field one), with
+ * B_i buckets, and out_facet_counts[q * (B_0 + ... + B_{n-1}) + B_0 + ... + B_{i-1} + b] is the number of docs query q
+ * ranks whose code in facet i is b (docs without a value are in no bucket).  The counts cover the index's own docs
+ * (a shard's, on a shard).  A slot not set, more than SA_BOOL_MAX_FACETS facets, a field out of range or
+ * out_facet_counts NULL with n_facets > 0 is SA_ERR_ARG before any device work.  The ranking is the same as without
+ * counting, bit for bit; an Or / And batch then runs as the roles layer with every clause SHOULD and weight 1.
+ * out_total NULL: no counting (n_facets, facet_field, facet_slot and out_facet_counts are ignored).
+ *
  * Arrays given in a pairing other than those above (weights without occurs, groups without ties or without occurs,
  * clause_node without groups, n_nodes != n_queries without clause_node) are SA_ERR_ARG before any device work. */
 #define SA_BOOL_MAX_CLAUSES 64
+#define SA_BOOL_MAX_FACETS 4
 #define SA_OCCUR_SHOULD 0
 #define SA_OCCUR_MUST 1
 #define SA_OCCUR_FILTER 2
@@ -243,6 +256,14 @@ int sa_score_batch_topk_sim(sa_index *index, int kind, const uint32_t *terms, co
 #define SA_FEATURE_LOG 2
 #define SA_FEATURE_TERM(fn, slot) (SA_FEATURE_TERM_BASE | ((uint32_t)(fn) << 8) | (uint32_t)(slot))
 int sa_index_set_feature(sa_index *index, uint32_t slot, const float *values, uint64_t n_values);
+/* Per-document facet columns of an index (a language, a decade, a category), counted by the facet counts above.
+ * sa_index_set_facet copies codes[0 .. n_values) (n_values == the index's n_docs) into slot `slot`
+ * (< SA_MAX_FACETS), replacing what the slot held: a code in [0, n_buckets) is the doc's bucket, -1 means the doc has
+ * no value.  1 <= n_buckets <= SA_FACET_MAX_BUCKETS.  The index owns the copy (uint16 per doc) and frees it with
+ * itself.  A bad argument is SA_ERR_ARG and leaves the index as it was. */
+#define SA_MAX_FACETS 8
+#define SA_FACET_MAX_BUCKETS 1024
+int sa_index_set_facet(sa_index *index, uint32_t slot, const int32_t *codes, uint64_t n_values, uint32_t n_buckets);
 int sa_score_batch_topk_bool(sa_index *index, uint32_t n_nodes, const uint32_t *node_clause_starts,
                              const uint32_t *clause_node, const uint32_t *clause_terms,
                              const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
@@ -250,6 +271,18 @@ int sa_score_batch_topk_bool(sa_index *index, uint32_t n_nodes, const uint32_t *
                              const uint32_t *mm, uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1,
                              float b, uint32_t k, const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
+/* sa_score_batch_topk_bool with the hit and facet counts above: the same arguments, then n_facets, facet_field,
+ * facet_slot, out_total and out_facet_counts.  sa_score_batch_topk_bool is this call with out_total NULL. */
+int sa_score_batch_topk_bool_counts(sa_index *index, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                    const uint32_t *clause_node, const uint32_t *clause_terms,
+                                    const uint32_t *clause_term_starts, const float *clause_idf,
+                                    const float *clause_weight, const uint8_t *clause_occur,
+                                    const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
+                                    uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b,
+                                    uint32_t k, const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
+                                    uint32_t *out_docs, float *out_scores, uint32_t *n_redone, uint32_t n_facets,
+                                    const uint32_t *facet_field, const uint32_t *facet_slot, uint32_t *out_total,
+                                    uint32_t *out_facet_counts);
 
 /* The same batch in three stages, so a serving loop (or the benchmark) can keep the query
  * descriptors resident and time the device work alone: upload (H2D of descriptors), execute
@@ -367,6 +400,20 @@ int sa_multi_score_batch_topk_bool(sa_multi *multi, uint32_t n_nodes, const uint
                                    uint32_t n_queries, uint32_t slop, const float *avg_doc_len, const float *k1,
                                    const float *b, uint32_t k, const uint32_t *where_bits, uint64_t where_n,
                                    uint64_t where_stride, uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
+/* sa_multi_score_batch_topk_bool with the hit and facet counts of sa_score_batch_topk_bool_counts, facet_field[i]
+ * being a field slot of the multi. */
+int sa_multi_score_batch_topk_bool_counts(sa_multi *multi, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                          const uint32_t *clause_node, const uint32_t *clause_field,
+                                          const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                          const float *clause_idf, const float *clause_weight,
+                                          const uint8_t *clause_occur, const uint32_t *clause_group,
+                                          const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
+                                          uint32_t slop, const float *avg_doc_len, const float *k1, const float *b,
+                                          uint32_t k, const uint32_t *where_bits, uint64_t where_n,
+                                          uint64_t where_stride, uint32_t *out_docs, float *out_scores,
+                                          uint32_t *n_redone, uint32_t n_facets, const uint32_t *facet_field,
+                                          const uint32_t *facet_slot, uint32_t *out_total,
+                                          uint32_t *out_facet_counts);
 
 /* ------------------------------------------------- per-op exports (parity tests)
  * Device implementations of the reference's native ops on raw arrays (host in, host out),

@@ -5,7 +5,7 @@ hand-written CUDA kernels behind the reference's SearchArray.index / .score / .t
 surface.  Host code is Python (numpy / pandas); the kernels are reached through the C ABI in
 include/searcharray_b200.h via ctypes.  No PyTorch, no Triton, no CPU fallback.
 """
-from .postings import SearchArray, Terms, TermsDtype, ws_tokenizer  # noqa: F401
+from .postings import Hits, SearchArray, Terms, TermsDtype, ws_tokenizer  # noqa: F401
 from .similarity import (Similarity, bm25_similarity, bm25_impact, bm25_legacy_similarity,  # noqa: F401
                          classic_similarity, compute_idf, default_bm25)
 from .indexing import HostIndex, TermDict, TermMissingError  # noqa: F401

@@ -18,6 +18,7 @@ ALL_BITS = 0xFFFFFFFFFFFFFFFF
 c_u64, c_u32, c_f32, c_int = ctypes.c_uint64, ctypes.c_uint32, ctypes.c_float, ctypes.c_int
 P_u64, P_u32, P_f32 = ctypes.POINTER(c_u64), ctypes.POINTER(c_u32), ctypes.POINTER(c_f32)
 P_u8 = ctypes.POINTER(ctypes.c_uint8)
+P_i32 = ctypes.POINTER(ctypes.c_int32)
 P_void = ctypes.c_void_p
 
 
@@ -55,9 +56,13 @@ SIGNATURES = {
                                         P_f32, ctypes.c_double, ctypes.c_double, ctypes.c_double, c_u32, P_u32, c_u64,
                                         c_u64, P_u32, ctypes.POINTER(ctypes.c_double)]),
     "sa_index_set_feature": (c_int, [P_void, c_u32, P_f32, c_u64]),
+    "sa_index_set_facet": (c_int, [P_void, c_u32, P_i32, c_u64, c_u32]),
     "sa_score_batch_topk_bool": (c_int, [P_void, c_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8, P_u32, P_f32,
                                          P_u32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32, P_u32, c_u64, c_u64, P_u32,
                                          P_f32, P_u32]),
+    "sa_score_batch_topk_bool_counts": (c_int, [P_void, c_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8, P_u32,
+                                                P_f32, P_u32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32, P_u32, c_u64,
+                                                c_u64, P_u32, P_f32, P_u32, c_u32, P_u32, P_u32, P_u32, P_u32]),
     "sa_batch_upload": (c_int, [P_void, P_u32, P_u32, P_f32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32]),
     "sa_batch_execute": (c_int, [P_void]),
     "sa_batch_download": (c_int, [P_void, P_u32, P_f32, P_u32]),
@@ -89,6 +94,10 @@ SIGNATURES = {
     "sa_multi_score_batch_topk_bool": (c_int, [P_void, c_u32, P_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8,
                                                P_u32, P_f32, P_u32, c_u32, c_u32, P_f32, P_f32, P_f32, c_u32, P_u32,
                                                c_u64, c_u64, P_u32, P_f32, P_u32]),
+    "sa_multi_score_batch_topk_bool_counts": (c_int, [P_void, c_u32, P_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32,
+                                                      P_u8, P_u32, P_f32, P_u32, c_u32, c_u32, P_f32, P_f32, P_f32,
+                                                      c_u32, P_u32, c_u64, c_u64, P_u32, P_f32, P_u32, c_u32, P_u32,
+                                                      P_u32, P_u32, P_u32]),
     "sa_op_popcount64_reduce": (c_int, [P_u64, c_u64, c_int, P_u64, P_f32, P_u64]),
     "sa_op_bm25_score": (c_int, [P_f32, P_f32, c_u64, c_f32, c_f32, c_f32, c_f32, c_int]),
     "sa_op_similarity": (c_int, [c_int, P_f32, P_f32, c_u64, ctypes.c_double, ctypes.c_double, ctypes.c_double,
@@ -150,6 +159,10 @@ def p_u32(a):
 
 def p_f32(a):
     return a.ctypes.data_as(P_f32)
+
+
+def p_i32(a):
+    return a.ctypes.data_as(P_i32)
 
 
 def p_u8(a):

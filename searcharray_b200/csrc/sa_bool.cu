@@ -53,6 +53,16 @@
 // is present in a tile iff its column's tile flag is set; in the fold its owners read their float4s of the column with
 // cached loads (the CTAs of a batch's queries on one tile read the same 32 KB) and put v = f(x) into the shared tile,
 // which the term clauses' fold then reads as it reads BM25 scores.  An Or / And batch with a feature runs as OCCUR.
+//
+// COUNT: hit and facet counts (sa_score_batch_topk_bool_counts), in instances of their own (bool_count_kernel, on the
+// FEATURE instances of OCCUR and above, an Or / And batch running as OCCUR) so that a batch without counts runs the
+// instances above unchanged.  After the tile's collect, s_tile still holds the ranked values (+0 where a doc does not
+// rank); each thread turns its 32 into a mask, a warp adds its popcounts into the query's total with one atomic, and
+// on a tile where anything ranks s_tile is reused as a shared histogram of the call's facets (<= 4 x 1,024 u32 =
+// 16 KB): each thread reads the codes of its ranked docs (one 8-byte load per float4 group with a ranked doc), one
+// shared atomic per ranked doc with a code, and the non-zero bins go to the query's counts with global atomics.  The
+// store passes of a nested call, and a query re-run after a candidate overflow, run the instances without COUNT: the
+// first pass has counted every tile of every query.
 #include "sa_multi.cuh"
 #include "sa_term.cuh"
 #include "sa_phrase.cuh"
@@ -124,6 +134,17 @@ struct BoolFeature {
     u32 fn;                 // SA_FEATURE_*
 };
 
+// The counts of a COUNT launch: per query of the launch its total and its facet rows, each facet's column and the
+// offset of its first bin in a row.  The kernel indexes the arrays with constants only (a dynamic index would copy the
+// struct to local memory).
+struct BoolCount {
+    u32 *total;                                         // [launch query]
+    u32 *counts;                                        // [launch query][n_bins]
+    const unsigned short *codes[SA_BOOL_MAX_FACETS];    // uint16 [padded n_docs] (sa_index::d_facets)
+    u32 offset[SA_BOOL_MAX_FACETS + 1];                 // offset[n_facets] == n_bins
+    u32 n_facets, n_bins;
+};
+
 struct BoolState {
     DevBuf d_clauses, d_queries, d_out_index;
     DevBuf d_occur;
@@ -131,7 +152,8 @@ struct BoolState {
     DevBuf d_flags;      // BoolNest::flags
     DevBuf d_groups;     // BoolGroup[] of a DisMax call
     DevBuf d_fields;     // BoolField[] of a multi-field call
-    DevBuf d_keys;       // nq * k result keys, then u32 overflow[nq]: one device-to-host copy
+    DevBuf d_keys;       // nq * k result keys, then u32 overflow[nq] (and, counting, total[nq] and the facet rows):
+                         // one device-to-host copy
     DevBuf rows;
     DevBuf d_where;      // the WhereMask rows of a masked call
     DevBuf d_feat;       // BoolFeature[] of a call with feature clauses
@@ -280,6 +302,54 @@ __device__ __forceinline__ void bool_publish_empty(const TopkCtx &t, u32 q, u32 
     }
 }
 
+// COUNT: the counting pass of one (query, tile), after flush_tile_collect (whose last barrier follows its last read
+// of s_tile): s_tile holds the tile's ranked values, +0 where a doc does not rank.  All threads must call.
+__device__ __forceinline__ void bool_count_tile(const BoolCount &cn, float *s_tile) {
+    constexpr int PER = SA_TILE_DOCS / SA_TERM_THREADS / 4;
+    const unsigned tid = bool_fresh_tid();
+    const u32 q = blockIdx.x, tile = blockIdx.y;
+    const float4 *s_tile4 = reinterpret_cast<const float4 *>(s_tile);
+    u32 ranked = 0;                        // bit 4 j + e: doc 4 g + e ranks
+#pragma unroll
+    for (int j = 0; j < PER; j++) {
+        const float4 x = s_tile4[tid + j * SA_TERM_THREADS];
+        ranked |= ((x.x > 0.0f ? 1u : 0u) | (x.y > 0.0f ? 2u : 0u) | (x.z > 0.0f ? 4u : 0u) | (x.w > 0.0f ? 8u : 0u))
+                  << (4 * j);
+    }
+    // the barrier also orders every read above before s_tile becomes the histogram
+    if (!__syncthreads_or(ranked != 0)) return;
+    const u32 n = __reduce_add_sync(0xFFFFFFFFu, (u32)__popc(ranked));
+    if ((tid & 31) == 0 && n) atomicAdd(cn.total + q, n);
+    if (cn.n_facets == 0) return;                                   // CTA-uniform
+    u32 *s_hist = reinterpret_cast<u32 *>(s_tile);
+    const u32 n_bins = cn.n_bins;
+    for (u32 i = tid; i < n_bins; i += SA_TERM_THREADS) s_hist[i] = 0;
+    __syncthreads();
+    const u32 tile_doc0 = tile * SA_TILE_DOCS;
+#pragma unroll
+    for (int f = 0; f < SA_BOOL_MAX_FACETS; f++) {
+        if (f >= (int)cn.n_facets) break;
+        const ushort4 *__restrict__ c4 = reinterpret_cast<const ushort4 *>(cn.codes[f] + tile_doc0);
+        u32 *h = s_hist + cn.offset[f];
+#pragma unroll
+        for (int j = 0; j < PER; j++) {
+            const u32 m = (ranked >> (4 * j)) & 0xFu;
+            if (!m) continue;
+            const ushort4 c = __ldg(c4 + tid + j * SA_TERM_THREADS);
+            if ((m & 1u) && c.x != SA_FACET_NONE) atomicAdd(h + c.x, 1u);
+            if ((m & 2u) && c.y != SA_FACET_NONE) atomicAdd(h + c.y, 1u);
+            if ((m & 4u) && c.z != SA_FACET_NONE) atomicAdd(h + c.z, 1u);
+            if ((m & 8u) && c.w != SA_FACET_NONE) atomicAdd(h + c.w, 1u);
+        }
+    }
+    __syncthreads();
+    u32 *dst = cn.counts + (u64)q * n_bins;
+    for (u32 i = tid; i < n_bins; i += SA_TERM_THREADS) {
+        const u32 v = s_hist[i];
+        if (v) atomicAdd(dst + i, v);
+    }
+}
+
 // The tile fold of one (query, tile).  OCCUR = false: Or / And (every clause SHOULD, weight 1).  OCCUR = true:
 // per-clause roles and weights in occ[], indexed as a.clauses; a query's mm counts its SHOULD clauses.  FIELDS: each
 // clause reads the field fld[clause.field] (bool_set_field) in place of the index in `a`; n_docs, doc_base, the
@@ -287,14 +357,17 @@ __device__ __forceinline__ void bool_publish_empty(const TopkCtx &t, u32 q, u32 
 // as a.clauses); mm counts SHOULD groups; s_dyn holds the groups' running max and sum, 2 * 32 floats per thread, and
 // s_g[3] (shared) the groups' presence masks.  NESTED (with DISMAX): nested clauses and the store pass (BoolNest).
 // WHERE: only docs whose bit of the mask row of query blockIdx.x is set rank (never in a store pass).  FEATURE (with
-// OCCUR): clauses whose row is SA_BOOL_FEATURE_ROW score their column feat[clause] (BoolFeature).
-template <bool OCCUR, bool FIELDS, bool DISMAX = false, bool NESTED = false, bool WHERE = false, bool FEATURE = false>
+// OCCUR): clauses whose row is SA_BOOL_FEATURE_ROW score their column feat[clause] (BoolFeature).  COUNT (with
+// FEATURE): the collected tile is counted into `cn` (bool_count_tile).
+template <bool OCCUR, bool FIELDS, bool DISMAX = false, bool NESTED = false, bool WHERE = false, bool FEATURE = false,
+          bool COUNT = false>
 __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__restrict__ occ,
                                           const BoolField *__restrict__ fld,
                                           const BoolGroup *__restrict__ grp = nullptr, float *s_dyn = nullptr,
                                           unsigned long long *s_g = nullptr, const BoolNest nb = BoolNest{},
                                           const WhereMask wh = WhereMask{nullptr, 0},
-                                          const BoolFeature *__restrict__ feat = nullptr) {
+                                          const BoolFeature *__restrict__ feat = nullptr,
+                                          const BoolCount cn = BoolCount{}) {
     constexpr int PER = SA_TILE_DOCS / SA_TERM_THREADS / 4;        // float4 groups per thread
     __shared__ __align__(16) float s_tile[SA_TILE_DOCS];
     __shared__ u32 s_lo[SA_BOOL_MAX_CLAUSES], s_hi[SA_BOOL_MAX_CLAUSES];
@@ -510,6 +583,7 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
         return;
     }
     flush_tile_collect<false>(s_tile, nullptr, a.topk, q, tile, my_max, SA_TILE_DOCS, 0, s_top, &s_ncand, &s_tile_max);
+    if (COUNT) bool_count_tile(cn, s_tile);
 }
 
 // Every instance of the fold: bool_tile with the arguments its form reads (the others are NULL and never read).
@@ -552,6 +626,17 @@ bool_feature_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const B
     bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, true>(a, occ, fld, grp, s_dyn, s_g, nb, wh, feat);
 }
 
+// The COUNT instances: bool_feature_kernel's, counting into `cn`.
+template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, int MIN_CTAS>
+__global__ void __launch_bounds__(SA_TERM_THREADS, MIN_CTAS)
+bool_count_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
+                  const BoolGroup *__restrict__ grp, const BoolNest nb, const WhereMask wh,
+                  const BoolFeature *__restrict__ feat, const BoolCount cn) {
+    extern __shared__ __align__(16) float s_dyn[];
+    __shared__ unsigned long long s_g[3];
+    bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, true, true>(a, occ, fld, grp, s_dyn, s_g, nb, wh, feat, cn);
+}
+
 // ------------------------------------------------------------------------------------------------------------ host
 namespace {
 
@@ -590,6 +675,21 @@ BoolFeatureKernel bool_feature_kernel_for(BoolForm form, bool masked) {
     return instances[form - BOOL_OCCUR][masked];
 }
 
+typedef void (*BoolCountKernel)(BoolArgs, const BoolOccur *, const BoolField *, const BoolGroup *, BoolNest,
+                                WhereMask, const BoolFeature *, BoolCount);
+
+// The COUNT instance of the first pass of a counting call of `form` (BOOL_OCCUR or above), each at its form's CTAs
+// per SM.
+BoolCountKernel bool_count_kernel_for(BoolForm form, bool masked) {
+    static const BoolCountKernel instances[4][2] = {
+        {bool_count_kernel<true, false, false, false, false, 3>, bool_count_kernel<true, false, false, false, true, 3>},
+        {bool_count_kernel<true, true, false, false, false, 3>, bool_count_kernel<true, true, false, false, true, 3>},
+        {bool_count_kernel<true, true, true, false, false, 2>, bool_count_kernel<true, true, true, false, true, 2>},
+        {bool_count_kernel<true, true, true, true, false, 2>, bool_count_kernel<true, true, true, true, true, 2>},
+    };
+    return instances[form - BOOL_OCCUR][masked];
+}
+
 // The fields of one call and where the call keeps its state.  The single-index entry point passes one field and the
 // index's own buffers (ix->boolq, ix->cand, ix->h_pinned); sa_multi_score_batch_topk_bool passes the multi's fields,
 // its BoolState and candidate buffer, and field 0's pinned staging.  Every field's stream is `lead`'s (FieldGuard).
@@ -604,6 +704,10 @@ struct BoolCall {
     const uint32_t *where_bits = nullptr;
     uint64_t where_n = 0, where_stride = 0;
     WhereMask where{nullptr, 0};
+    // the call's hit and facet counts, as passed (out_total NULL: no counting)
+    uint32_t n_facets = 0;
+    const uint32_t *facet_field = nullptr, *facet_slot = nullptr;
+    uint32_t *out_total = nullptr, *out_facet_counts = nullptr;
     sa_index *lead() const { return ix[0]; }
 };
 
@@ -624,6 +728,8 @@ struct BoolPlan {
                                         // is nested[i]'s descriptor
     std::vector<u32> nest;              // per clause, as clauses: 1 for a nested clause (BOOL_NESTED)
     std::vector<BoolFeature> features;  // per clause, as clauses, when a clause is a feature (the FEATURE instances)
+    bool counting = false;              // the first pass runs the COUNT instances into `count`
+    BoolCount count{};                  // total and counts: the call's rows (bool_run_group offsets them per launch)
 };
 
 // The count rows of the phrase clauses of queries [q0, q1) and of their nested nodes (rows are numbered within the
@@ -652,8 +758,9 @@ int bool_build_rows(const BoolCall &X, const BoolPlan &P, const uint32_t *clause
 }
 
 // Queries [q0, q1) with `slots` candidate slots per tile: their rows, the tile kernel and the selection, enqueued.
+// count: the first pass of a counting call (P.counting), the top-level launch counting into P.count.
 int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_terms,
-                   const uint32_t *clause_term_starts, u32 slop, u32 k, u32 slots, u32 q0, u32 q1) {
+                   const uint32_t *clause_term_starts, u32 slop, u32 k, u32 slots, u32 q0, u32 q1, bool count) {
     sa_index *ix = X.lead();
     BoolState &S = *X.S;
     const u32 n_tiles = sa_n_tiles(ix->n_docs), nq = q1 - q0;
@@ -691,9 +798,17 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
     const size_t smem = P.form >= BOOL_DISMAX ? SA_BOOL_DISMAX_SMEM : 0;
     // the form's instance, or its FEATURE instance when the call has feature clauses
     const BoolFeature *feat = P.features.empty() ? nullptr : S.d_feat.as<BoolFeature>();
-    auto launch = [&](bool masked, u32 n_q, const BoolArgs &args, const BoolNest &n, const WhereMask &w) {
+    BoolCount cn = P.count;                 // row 0 of the launch is query q0's
+    if (count) {
+        cn.total += q0;
+        cn.counts += (u64)q0 * cn.n_bins;
+    }
+    auto launch = [&](bool masked, u32 n_q, const BoolArgs &args, const BoolNest &n, const WhereMask &w, bool c) {
         const dim3 grid(n_q, n_tiles);
-        if (feat)
+        if (c)
+            bool_count_kernel_for(P.form, masked)<<<grid, SA_TERM_THREADS, smem, ix->stream>>>(args, occ, fld, grp, n, w,
+                                                                                             feat, cn);
+        else if (feat)
             bool_feature_kernel_for(P.form, masked)<<<grid, SA_TERM_THREADS, smem, ix->stream>>>(args, occ, fld, grp, n,
                                                                                              w, feat);
         else
@@ -710,14 +825,14 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
             while (j < P.nested.size() && in_run(j) && P.depth[P.nested[j]] == P.depth[P.nested[i]]) j++;
             BoolArgs an = a;
             an.queries = S.d_queries.as<BoolQuery>() + P.n_top + i;
-            launch(false, (u32)(j - i), an, nb, WhereMask{nullptr, 0});
+            launch(false, (u32)(j - i), an, nb, WhereMask{nullptr, 0}, false);
             SA_CUDA(cudaGetLastError());
             ix->stats.total_launches++;
             i = j;
         }
         nb.store = nullptr;
     }
-    launch(wh.bits != nullptr, nq, a, nb, wh);
+    launch(wh.bits != nullptr, nq, a, nb, wh, count);
     SA_CUDA(cudaGetLastError());
     ix->stats.total_launches++;
     return launch_topk_select(ix, t, nq, ix->doc_base, d_keys, S.d_out_index.as<u32>() + q0);
@@ -818,6 +933,24 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
     }
     for (u32 n = n_queries; nested && n < n_nodes; n++) SA_CHECK(refs[n] == 1, "node %u is referenced by no clause", n);
     if ((rc = sa_where_check(X.where_bits, X.where_n, X.where_stride, lead->n_docs))) return rc;
+    // hit and facet counts: each facet a set slot of its field's index
+    const bool counting = X.out_total != nullptr;
+    BoolCount count{};
+    if (counting) {
+        SA_CHECK(X.n_facets <= SA_BOOL_MAX_FACETS, "at most %d facets in one call, not %u", SA_BOOL_MAX_FACETS,
+                 X.n_facets);
+        SA_CHECK(X.n_facets == 0 || (X.facet_field && X.facet_slot && X.out_facet_counts), "NULL argument");
+        for (u32 i = 0; i < X.n_facets; i++) {
+            const u32 f = X.facet_field[i], slot = X.facet_slot[i];
+            SA_CHECK(f < n_fields, "facet %u: field %u out of range (%u fields)", i, f, n_fields);
+            SA_CHECK(slot < SA_MAX_FACETS && (X.ix[f]->facet_set >> slot & 1u), "facet %u: facet slot %u is not set",
+                     i, slot);
+            count.codes[i] = X.ix[f]->d_facets[slot].as<const unsigned short>();
+            count.offset[i + 1] = count.offset[i] + X.ix[f]->facet_buckets[slot];
+        }
+        count.n_facets = X.n_facets;
+        count.n_bins = count.offset[X.n_facets];
+    }
     const u32 c_begin = n_nodes ? query_clause_starts[0] : 0, c_end = n_nodes ? query_clause_starts[n_nodes] : 0;
     bool features = false;
     for (u32 c = c_begin; c < c_end; c++) {
@@ -840,18 +973,23 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
             SA_CHECK(!bool_is_feature_term(tids[i]), "clause %u: a feature term id inside a phrase", c);
         if ((rc = sa_check_term_ids(X.ix[f], tids, nt))) return rc;
     }
-    // an Or / And batch with a feature clause runs as roles and weights, every clause SHOULD with weight 1
+    // an Or / And batch with a feature clause or counts runs as roles and weights, every clause SHOULD with weight 1
     std::vector<float> ones;
     std::vector<uint8_t> shoulds;
-    if (features && !occur) {
+    if ((features || counting) && !occur) {
         ones.assign(c_end, 1.0f);
         shoulds.assign(c_end, SA_OCCUR_SHOULD);
         clause_weight = ones.data();
         clause_occur = shoulds.data();
     }
-    const bool roles = occur || features;
+    const bool roles = occur || features || counting;
     const size_t nk = (size_t)n_queries * k;
     for (size_t i = 0; i < nk; i++) { out_docs[i] = SA_NO_DOC; out_scores[i] = 0.0f; }
+    const size_t n_bins = count.n_bins;
+    if (counting) {
+        memset(X.out_total, 0, (size_t)n_queries * sizeof(u32));
+        if (n_bins) memset(X.out_facet_counts, 0, (size_t)n_queries * n_bins * sizeof(u32));
+    }
     // .score is all zeros on a field whose avgdl is 0: its clauses are empty (below), and without any other field
     // nothing ranks
     bool any_avgdl = false;
@@ -965,7 +1103,9 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
                                       node_row[n]});
 
     BoolState &S = *X.S;
-    const size_t key_bytes = nk * sizeof(u64) + (size_t)n_queries * sizeof(u32);
+    // counting: total[nq] and the facet rows [nq][n_bins] after the overflow flags, zeroed with them
+    const size_t count_bytes = counting ? (size_t)n_queries * (1 + n_bins) * sizeof(u32) : 0;
+    const size_t key_bytes = nk * sizeof(u64) + (size_t)n_queries * sizeof(u32) + count_bytes;
     if ((rc = S.d_clauses.reserve(P.clauses.size() * sizeof(BoolClause))) ||
         (rc = S.d_queries.reserve(P.queries.size() * sizeof(BoolQuery))) ||
         (rc = S.d_out_index.reserve((size_t)n_queries * sizeof(u32))) || (rc = S.d_keys.reserve(key_bytes)) ||
@@ -1008,6 +1148,9 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
                                : ((rc = bool_dismax_smem(bool_feature_kernel_for(P.form, false))) ||
                                   (X.where.bits && (rc = bool_dismax_smem(bool_feature_kernel_for(P.form, true))))))
             return rc;
+        if (counting && ((rc = bool_dismax_smem(bool_count_kernel_for(P.form, false))) ||
+                         (X.where.bits && (rc = bool_dismax_smem(bool_count_kernel_for(P.form, true))))))
+            return rc;
         SA_CUDA(cudaMemcpyAsync(S.d_groups.p, P.groups.data(), P.groups.size() * sizeof(BoolGroup), cudaMemcpyHostToDevice, lead->stream));
     }
     if (nested) {
@@ -1017,10 +1160,16 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
     SA_CUDA(cudaMemcpyAsync(S.d_queries.p, P.queries.data(), P.queries.size() * sizeof(BoolQuery), cudaMemcpyHostToDevice, lead->stream));
     SA_CUDA(cudaMemcpyAsync(S.d_out_index.p, identity.data(), (size_t)n_queries * sizeof(u32), cudaMemcpyHostToDevice, lead->stream));
     u32 *d_ovf = (u32 *)(S.d_keys.as<u64>() + nk);
-    SA_CUDA(cudaMemsetAsync(d_ovf, 0, (size_t)n_queries * sizeof(u32), lead->stream));
+    SA_CUDA(cudaMemsetAsync(d_ovf, 0, (size_t)n_queries * sizeof(u32) + count_bytes, lead->stream));
+    if (counting) {
+        P.counting = true;
+        P.count = count;
+        P.count.total = d_ovf + n_queries;
+        P.count.counts = d_ovf + 2 * (size_t)n_queries;
+    }
     for (size_t i = 0; i + 1 < P.group_start.size(); i++)
         if ((rc = bool_run_group(X, P, clause_terms, clause_term_starts, slop, k, slots, P.group_start[i],
-                                 P.group_start[i + 1]))) return rc;
+                                 P.group_start[i + 1], counting))) return rc;
 
     // keys and overflow flags in one copy and one synchronise; a query whose tile overflowed is re-run alone with a
     // slot per doc of the tile, which cannot overflow
@@ -1030,11 +1179,19 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
     std::vector<u32> ovf(n_queries);
     memcpy(ovf.data(), h.as<const u64>() + nk, (size_t)n_queries * sizeof(u32));
     sa_unpack_keys(h.as<const u64>(), nk, out_docs, out_scores);
+    if (counting) {
+        memcpy(X.out_total, h.as<const u32>() + 2 * nk + n_queries, (size_t)n_queries * sizeof(u32));
+        if (n_bins)
+            memcpy(X.out_facet_counts, h.as<const u32>() + 2 * nk + 2 * (size_t)n_queries,
+                   (size_t)n_queries * n_bins * sizeof(u32));
+    }
+    // a re-run query has been counted by the first pass, so its re-run does not count
     u32 redone = 0;
     for (u32 q = 0; q < n_queries; q++) {
         if (!ovf[q]) continue;
         SA_CUDA(cudaMemsetAsync(d_ovf + q, 0, sizeof(u32), lead->stream));
-        if ((rc = bool_run_group(X, P, clause_terms, clause_term_starts, slop, k, SA_TILE_DOCS, q, q + 1))) return rc;
+        if ((rc = bool_run_group(X, P, clause_terms, clause_term_starts, slop, k, SA_TILE_DOCS, q, q + 1, false)))
+            return rc;
         SA_CUDA(cudaMemcpyAsync(h.p, S.d_keys.as<u64>() + (size_t)q * k, k * sizeof(u64), cudaMemcpyDeviceToHost,
                                 lead->stream));
         SA_CUDA(cudaStreamSynchronize(lead->stream));
@@ -1052,7 +1209,9 @@ int bool_topk_index(sa_index *ix, uint32_t n_nodes, const uint32_t *query_clause
                     const uint8_t *clause_occur, const uint32_t *clause_group, const float *clause_tie,
                     const uint32_t *mm, uint32_t n_queries, uint32_t slop,
                     float avg_doc_len, float k1, float b, uint32_t k, const uint32_t *where_bits, uint64_t where_n,
-                    uint64_t where_stride, uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
+                    uint64_t where_stride, uint32_t *out_docs, float *out_scores, uint32_t *n_redone,
+                    uint32_t n_facets, const uint32_t *facet_field, const uint32_t *facet_slot, uint32_t *out_total,
+                    uint32_t *out_facet_counts) {
     SA_CHECK(ix && out_docs && out_scores, "NULL argument");
     SA_CHECK(n_nodes == 0 || (query_clause_starts && clause_terms && clause_term_starts && clause_idf && mm),
              "NULL argument");
@@ -1072,6 +1231,11 @@ int bool_topk_index(sa_index *ix, uint32_t n_nodes, const uint32_t *query_clause
     X.where_bits = where_bits;
     X.where_n = where_n;
     X.where_stride = where_stride;
+    X.n_facets = n_facets;
+    X.facet_field = facet_field;
+    X.facet_slot = facet_slot;
+    X.out_total = out_total;
+    X.out_facet_counts = out_facet_counts;
     return bool_topk(X, n_nodes, query_clause_starts, clause_node, nullptr, clause_terms, clause_term_starts,
                      clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
                      out_docs, out_scores, n_redone);
@@ -1085,7 +1249,8 @@ int bool_topk_multi(sa_multi *m, uint32_t n_nodes, const uint32_t *query_clause_
                     const float *clause_tie, const uint32_t *mm, uint32_t n_queries, uint32_t slop,
                     const float *avg_doc_len, const float *k1, const float *b, uint32_t k,
                     const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride, uint32_t *out_docs,
-                    float *out_scores, uint32_t *n_redone) {
+                    float *out_scores, uint32_t *n_redone, uint32_t n_facets, const uint32_t *facet_field,
+                    const uint32_t *facet_slot, uint32_t *out_total, uint32_t *out_facet_counts) {
     SA_CHECK(m && out_docs && out_scores && avg_doc_len && k1 && b, "NULL argument");
     SA_CHECK(n_nodes == 0 || (query_clause_starts && clause_field && clause_terms && clause_term_starts &&
                                 clause_idf && clause_weight && clause_occur && mm), "NULL argument");
@@ -1120,9 +1285,35 @@ int bool_topk_multi(sa_multi *m, uint32_t n_nodes, const uint32_t *query_clause_
     X.where_bits = where_bits;
     X.where_n = where_n;
     X.where_stride = where_stride;
+    X.n_facets = n_facets;
+    X.facet_field = facet_field;
+    X.facet_slot = facet_slot;
+    X.out_total = out_total;
+    X.out_facet_counts = out_facet_counts;
     return bool_topk(X, n_nodes, query_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
                      clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
                      out_docs, out_scores, n_redone);
+}
+
+// The argument pairings every form checks, at both single-index entry points.
+int bool_check_index_arrays(uint32_t n_nodes, const uint32_t *clause_node, const float *clause_weight,
+                            const uint8_t *clause_occur, const uint32_t *clause_group, const float *clause_tie,
+                            uint32_t n_queries) {
+    SA_CHECK(!clause_weight == !clause_occur, "clause_weight and clause_occur are both given or both NULL");
+    SA_CHECK(!clause_group == !clause_tie && (!clause_group || clause_occur),
+             "clause_group and clause_tie are both given (with clause_occur) or both NULL");
+    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
+             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
+    return SA_OK;
+}
+
+// ... and at both multi-field ones.
+int bool_check_multi_arrays(uint32_t n_nodes, const uint32_t *clause_node, const uint32_t *clause_group,
+                            const float *clause_tie, uint32_t n_queries) {
+    SA_CHECK(!clause_group == !clause_tie, "clause_group and clause_tie are both given or both NULL");
+    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
+             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
+    return SA_OK;
 }
 
 }  // namespace
@@ -1136,14 +1327,33 @@ extern "C" int sa_score_batch_topk_bool(sa_index *ix, uint32_t n_nodes, const ui
                                         uint32_t k, const uint32_t *where_bits, uint64_t where_n,
                                         uint64_t where_stride, uint32_t *out_docs, float *out_scores,
                                         uint32_t *n_redone) {
-    SA_CHECK(!clause_weight == !clause_occur, "clause_weight and clause_occur are both given or both NULL");
-    SA_CHECK(!clause_group == !clause_tie && (!clause_group || clause_occur),
-             "clause_group and clause_tie are both given (with clause_occur) or both NULL");
-    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
-             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
+    return sa_score_batch_topk_bool_counts(ix, n_nodes, node_clause_starts, clause_node, clause_terms,
+                                           clause_term_starts, clause_idf, clause_weight, clause_occur, clause_group,
+                                           clause_tie, mm, n_queries, slop, avg_doc_len, k1, b, k, where_bits, where_n,
+                                           where_stride, out_docs, out_scores, n_redone, 0, nullptr, nullptr, nullptr,
+                                           nullptr);
+}
+
+extern "C" int sa_score_batch_topk_bool_counts(sa_index *ix, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                               const uint32_t *clause_node, const uint32_t *clause_terms,
+                                               const uint32_t *clause_term_starts, const float *clause_idf,
+                                               const float *clause_weight, const uint8_t *clause_occur,
+                                               const uint32_t *clause_group, const float *clause_tie,
+                                               const uint32_t *mm, uint32_t n_queries, uint32_t slop,
+                                               float avg_doc_len, float k1, float b, uint32_t k,
+                                               const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
+                                               uint32_t *out_docs, float *out_scores, uint32_t *n_redone,
+                                               uint32_t n_facets, const uint32_t *facet_field,
+                                               const uint32_t *facet_slot, uint32_t *out_total,
+                                               uint32_t *out_facet_counts) {
+    int rc;
+    if ((rc = bool_check_index_arrays(n_nodes, clause_node, clause_weight, clause_occur, clause_group, clause_tie,
+                                      n_queries)))
+        return rc;
     return bool_topk_index(ix, n_nodes, node_clause_starts, clause_node, clause_terms, clause_term_starts, clause_idf,
                            clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, avg_doc_len,
-                           k1, b, k, where_bits, where_n, where_stride, out_docs, out_scores, n_redone);
+                           k1, b, k, where_bits, where_n, where_stride, out_docs, out_scores, n_redone, n_facets,
+                           facet_field, facet_slot, out_total, out_facet_counts);
 }
 
 extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, uint32_t n_nodes, const uint32_t *node_clause_starts,
@@ -1156,10 +1366,25 @@ extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, uint32_t n_nodes, con
                                               uint32_t k, const uint32_t *where_bits, uint64_t where_n,
                                               uint64_t where_stride, uint32_t *out_docs, float *out_scores,
                                               uint32_t *n_redone) {
-    SA_CHECK(!clause_group == !clause_tie, "clause_group and clause_tie are both given or both NULL");
-    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
-             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
+    return sa_multi_score_batch_topk_bool_counts(m, n_nodes, node_clause_starts, clause_node, clause_field,
+                                                 clause_terms, clause_term_starts, clause_idf, clause_weight,
+                                                 clause_occur, clause_group, clause_tie, mm, n_queries, slop,
+                                                 avg_doc_len, k1, b, k, where_bits, where_n, where_stride, out_docs,
+                                                 out_scores, n_redone, 0, nullptr, nullptr, nullptr, nullptr);
+}
+
+extern "C" int sa_multi_score_batch_topk_bool_counts(
+    sa_multi *m, uint32_t n_nodes, const uint32_t *node_clause_starts, const uint32_t *clause_node,
+    const uint32_t *clause_field, const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+    const float *clause_idf, const float *clause_weight, const uint8_t *clause_occur, const uint32_t *clause_group,
+    const float *clause_tie, const uint32_t *mm, uint32_t n_queries, uint32_t slop, const float *avg_doc_len,
+    const float *k1, const float *b, uint32_t k, const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
+    uint32_t *out_docs, float *out_scores, uint32_t *n_redone, uint32_t n_facets, const uint32_t *facet_field,
+    const uint32_t *facet_slot, uint32_t *out_total, uint32_t *out_facet_counts) {
+    int rc;
+    if ((rc = bool_check_multi_arrays(n_nodes, clause_node, clause_group, clause_tie, n_queries))) return rc;
     return bool_topk_multi(m, n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
                            clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop,
-                           avg_doc_len, k1, b, k, where_bits, where_n, where_stride, out_docs, out_scores, n_redone);
+                           avg_doc_len, k1, b, k, where_bits, where_n, where_stride, out_docs, out_scores, n_redone,
+                           n_facets, facet_field, facet_slot, out_total, out_facet_counts);
 }

@@ -150,6 +150,7 @@ struct Bm25Params {
 
 // A query against one shard, as the kernels see it.
 #define SA_NO_DIR 0xFFFFFFFFFFFFFFFFull
+#define SA_FACET_NONE 0xFFFFu           // a facet column's code of a doc without a value (sa_index::d_facets)
 struct TermQuery {
     u64 word_off;      // offset of the term's first word in d_words
     u64 n_words;       // 0 => unknown term (zeros)
@@ -206,6 +207,11 @@ struct sa_index {
     DevBuf d_features[SA_MAX_FEATURES];
     DevBuf d_feature_tiles;          // u32 [SA_MAX_FEATURES * n_tiles]
     u32 feature_set = 0;
+    // facet columns (sa_index_set_facet, sa_feature.cu): slot s, when bit s of facet_set is set, is d_facets[s]
+    // (uint16 [padded n_docs], a doc's bucket or 0xFFFF for none, 0xFFFF past n_docs) with facet_buckets[s] buckets
+    DevBuf d_facets[SA_MAX_FACETS];
+    u32 facet_buckets[SA_MAX_FACETS] = {};
+    u32 facet_set = 0;
     // host mirrors for query set-up
     std::vector<u64> h_off, h_len;
     std::vector<u32> h_df;

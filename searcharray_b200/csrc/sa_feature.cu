@@ -1,10 +1,14 @@
-// sa_feature.cu -- per-document feature columns of an index (sa_index_set_feature), read by the feature clauses of
-// the batched boolean queries (sa_bool.cu).
+// sa_feature.cu -- per-document columns of an index: feature columns (sa_index_set_feature), read by the feature
+// clauses of the batched boolean queries, and facet columns (sa_index_set_facet), read by their counting pass
+// (sa_bool.cu).
 //
-// A column is stored as float[padded n_docs], zero past n_docs, so the tile fold's float4 loads of a whole tile need
-// no bounds test.  Beside it, one u32 flag per (slot, tile): whether any value of the tile is > 0.  The fold takes a
-// feature clause as present in a tile iff its flag is set, as it takes a term clause present where its list has a
-// doc, so min-should-match and MUST pruning skip the tiles where the feature is absent.
+// A feature column is stored as float[padded n_docs], zero past n_docs, so the tile fold's float4 loads of a whole
+// tile need no bounds test.  Beside it, one u32 flag per (slot, tile): whether any value of the tile is > 0.  The fold
+// takes a feature clause as present in a tile iff its flag is set, as it takes a term clause present where its list
+// has a doc, so min-should-match and MUST pruning skip the tiles where the feature is absent.
+//
+// A facet column is stored as uint16[padded n_docs], 0xFFFF for "no value" and past n_docs, so the counting pass
+// reads a thread's four docs as one 8-byte load with no bounds test.
 #include <cmath>
 
 #include "sa_term.cuh"
@@ -58,5 +62,34 @@ extern "C" int sa_index_set_feature(sa_index *ix, uint32_t slot, const float *va
     SA_CUDA(cudaStreamSynchronize(ix->stream));     // `values` is borrowed for the call only
     ix->d_features[slot] = std::move(col);
     ix->feature_set |= 1u << slot;
+    return SA_OK;
+}
+
+extern "C" int sa_index_set_facet(sa_index *ix, uint32_t slot, const int32_t *codes, uint64_t n_values,
+                                  uint32_t n_buckets) {
+    SA_CHECK(ix && (codes || n_values == 0), "NULL argument");
+    SA_CHECK(slot < SA_MAX_FACETS, "facet slot %u out of range (%d slots)", slot, SA_MAX_FACETS);
+    SA_CHECK(n_buckets >= 1 && n_buckets <= SA_FACET_MAX_BUCKETS, "a facet has 1 to %d buckets, not %u",
+             SA_FACET_MAX_BUCKETS, n_buckets);
+    std::lock_guard<std::mutex> g(ix->mu);
+    SA_CHECK(n_values == ix->n_docs, "a facet has one code per doc: %llu codes for %llu docs",
+             (unsigned long long)n_values, (unsigned long long)ix->n_docs);
+    const u64 padded = sa_padded_docs(ix->n_docs);
+    std::vector<uint16_t> col(std::max<u64>(padded, 4), SA_FACET_NONE);
+    for (u64 i = 0; i < n_values; i++) {
+        SA_CHECK(codes[i] >= -1 && codes[i] < (int32_t)n_buckets, "facet code %llu (%d) is not -1 or in [0, %u)",
+                 (unsigned long long)i, codes[i], n_buckets);
+        if (codes[i] >= 0) col[i] = (uint16_t)codes[i];
+    }
+    SA_CUDA(cudaSetDevice(ix->device));
+    // into a new buffer, which replaces the slot's once it is filled: a failure leaves the slot as it was
+    DevBuf d;
+    int rc;
+    if ((rc = d.allocate(col.size() * sizeof(uint16_t)))) return rc;
+    SA_CUDA(cudaMemcpyAsync(d.p, col.data(), col.size() * sizeof(uint16_t), cudaMemcpyHostToDevice, ix->stream));
+    SA_CUDA(cudaStreamSynchronize(ix->stream));     // `col` is a local
+    ix->d_facets[slot] = std::move(d);
+    ix->facet_buckets[slot] = n_buckets;
+    ix->facet_set |= 1u << slot;
     return SA_OK;
 }

@@ -64,6 +64,9 @@ class HostIndex:
         # per-doc feature columns (SearchArray.set_feature): name -> float32[n_docs]; a name's slot on the device
         # index is its position in this dict
         self.features = {}
+        # per-doc facet columns (SearchArray.set_facet): name -> (int32[n_docs] codes, -1: no value; n_buckets); a
+        # name's slot on the device index is its position in this dict
+        self.facets = {}
 
     # ---- on-disk posting words (reference phrase/memmap_arrays.py:145-208, MemoryMappedArrays): the words
     #      array written once to `<data_dir>/<n>.dat`, mapped back read-only; pickling stores the file name
@@ -91,6 +94,7 @@ class HostIndex:
     def __setstate__(self, st):
         self.__dict__.update(st)
         self.__dict__.setdefault("features", {})
+        self.__dict__.setdefault("facets", {})
         if st.get("words_file"):
             self._map_words()
 
@@ -123,6 +127,7 @@ class HostIndex:
         words = np.concatenate(parts) if parts else np.empty(0, dtype=np.uint64)
         out = HostIndex(words, offs, lens, self.doc_lens[doc_lo:doc_hi], self.term_dict, self.avg_doc_length)
         out.features = {name: v[doc_lo:doc_hi].copy() for name, v in self.features.items()}
+        out.facets = {name: (c[doc_lo:doc_hi].copy(), nb) for name, (c, nb) in self.facets.items()}
         return out
 
 

@@ -14,7 +14,7 @@ import ctypes
 import numbers
 import threading
 import weakref
-from typing import List, Optional, Union
+from typing import Dict, List, NamedTuple, Optional, Union
 
 import numpy as np
 import pandas as pd
@@ -181,6 +181,52 @@ def _where_part(bits, sel):
     return bits if bits is None or bits.shape[0] == 1 else np.ascontiguousarray(bits[sel])
 
 
+class Hits(NamedTuple):
+    """The hit and facet counts of a batched top-k call with `facets=` (SearchArray.search_topk, solr.fields_topk).
+    total[q]: how many docs query q ranks (all of them, not only the top k).  facets[name][q, b]: how many of those
+    docs have code b in facet `name`."""
+    total: np.ndarray                   # int64[Q]
+    facets: Dict[object, np.ndarray]    # name -> int64[Q, n_buckets]
+
+
+class _Counts:
+    """The counts of one sa_score_batch_topk_bool_counts / sa_multi_score_batch_topk_bool_counts call: per facet its
+    key in Hits.facets, its field slot, its slot on that field's index and its bucket count, and the uint32 outputs
+    the call fills."""
+
+    def __init__(self, keys, fields, slots, n_buckets, n_queries):
+        self.keys, self.n_buckets = list(keys), list(n_buckets)
+        self.fields = np.asarray(fields, dtype=np.uint32)
+        self.slots = np.asarray(slots, dtype=np.uint32)
+        self.total = np.zeros(n_queries, dtype=np.uint32)
+        self.counts = np.zeros((n_queries, sum(self.n_buckets)), dtype=np.uint32)
+
+    def args(self):
+        """The trailing arguments of the _counts entry points."""
+        if not self.keys:
+            return 0, None, None, _lib.p_u32(self.total), None
+        return (len(self.keys), _lib.p_u32(self.fields), _lib.p_u32(self.slots), _lib.p_u32(self.total),
+                _lib.p_u32(self.counts))
+
+    def hits(self):
+        ends = np.cumsum(self.n_buckets)
+        return Hits(self.total.astype(np.int64), {key: self.counts[:, e - nb:e].astype(np.int64)
+                                                  for key, nb, e in zip(self.keys, self.n_buckets, ends)})
+
+
+def check_facet_keys(facets, what):
+    """facets= as a list of distinct keys, at most SA_BOOL_MAX_FACETS (ValueError), before any device work."""
+    from .query import SA_BOOL_MAX_FACETS
+    if isinstance(facets, (str, tuple)) or not is_list_like(facets):
+        raise TypeError(f"facets is a list of {what}, not {facets!r}")
+    facets = list(facets)
+    if len(facets) > SA_BOOL_MAX_FACETS:
+        raise ValueError(f"at most {SA_BOOL_MAX_FACETS} facets in one call, not {len(facets)}")
+    if len(set(facets)) != len(facets):
+        raise ValueError(f"facets are named once each: {facets}")
+    return facets
+
+
 class DeviceIndex:
     """Owns one sa_index handle (one shard in one GPU's HBM)."""
 
@@ -197,6 +243,8 @@ class DeviceIndex:
         self._finalizer = weakref.finalize(self, DeviceIndex._destroy, self.handle)
         self.features = {}          # slot -> the host array last uploaded there
         self.sync_features(host)
+        self.facets = {}            # slot -> the host codes last uploaded there
+        self.sync_facets(host)
 
     def sync_features(self, host: HostIndex):
         """Uploads every feature column of `host` that this index does not hold yet (sa_index_set_feature)."""
@@ -204,6 +252,13 @@ class DeviceIndex:
             if self.features.get(slot) is not values:
                 _lib.check(_lib.lib().sa_index_set_feature(self.handle, slot, _lib.p_f32(values), len(values)))
                 self.features[slot] = values
+
+    def sync_facets(self, host: HostIndex):
+        """Uploads every facet column of `host` that this index does not hold yet (sa_index_set_facet)."""
+        for slot, (codes, n_buckets) in enumerate(host.facets.values()):
+            if self.facets.get(slot) is not codes:
+                _lib.check(_lib.lib().sa_index_set_facet(self.handle, slot, _lib.p_i32(codes), len(codes), n_buckets))
+                self.facets[slot] = codes
 
     @staticmethod
     def _destroy(handle):
@@ -561,6 +616,55 @@ class SearchArray(ExtensionArray):
             if self._shared["dev"] is not None:
                 self._shared["dev"].sync_features(self.host)
 
+    def set_facet(self, name, codes, n_buckets=None) -> None:
+        """Registers a per-document category column -- a language, a decade, a genre -- whose counts search_topk and
+        solr.fields_topk return with `facets=`.  codes: one integer per doc of the array (on a shard, per row of the
+        shard); a code in [0, n_buckets) is the doc's bucket, -1 means the doc has no value.  n_buckets defaults to
+        max(codes) + 1, at least 1, and may be at most 1,024.  A non-integer dtype is a TypeError; another length, a
+        code below -1 or >= n_buckets, more than 1,024 buckets or more than 8 names per index a ValueError, all before
+        any device work.  Setting a name again replaces it.  Refused (ValueError) on a view, whose positions are not
+        the index's docs.  The codes live with the index (copies and pickles carry them) and go to the device when it
+        is first used, or at once if it already is."""
+        from .query import SA_FACET_MAX_BUCKETS, SA_MAX_FACETS
+        if not isinstance(name, str):
+            raise TypeError(f"a facet name is a str, not {name!r}")
+        if self.rows is not None:
+            raise ValueError("set_facet on a view (arr[mask]) is not supported: set it on the whole array")
+        c = np.asarray(codes)
+        if c.dtype.kind not in "iu":
+            raise TypeError(f"facet codes are integers, not dtype {c.dtype}")
+        if c.shape != (self.host.n_docs,):
+            raise ValueError(f"a facet has one code per doc: shape ({self.host.n_docs},), not {c.shape}")
+        if n_buckets is None:
+            n_buckets = max(int(c.max()) + 1 if len(c) else 1, 1)
+        if isinstance(n_buckets, bool) or not isinstance(n_buckets, numbers.Integral):
+            raise TypeError(f"n_buckets is an int, not {n_buckets!r}")
+        n_buckets = int(n_buckets)
+        if not 1 <= n_buckets <= SA_FACET_MAX_BUCKETS:
+            raise ValueError(f"a facet has 1 to {SA_FACET_MAX_BUCKETS} buckets, not {n_buckets}")
+        if len(c) and (int(c.min()) < -1 or int(c.max()) >= n_buckets):
+            raise ValueError(f"facet codes are -1 (no value) or in [0, {n_buckets}): {name!r} holds "
+                             f"[{int(c.min())}, {int(c.max())}]")
+        facets = self.host.facets
+        if name not in facets and len(facets) >= SA_MAX_FACETS:
+            raise ValueError(f"an index holds at most {SA_MAX_FACETS} facets")
+        with self._shared["lock"]:
+            facets[name] = (np.ascontiguousarray(c, dtype=np.int32).copy(), n_buckets)
+            if self._shared["dev"] is not None:
+                self._shared["dev"].sync_facets(self.host)
+
+    def _facet_slot(self, name):
+        """(slot, n_buckets) of facet `name` on this array's index; ValueError if it is not set."""
+        names = list(self.host.facets)
+        if name not in names:
+            raise ValueError(f"facet {name!r} is not set on this array (set_facet); set: {names}")
+        return names.index(name), self.host.facets[name][1]
+
+    def _counts(self, facets, n_queries):
+        """The _Counts of facet names `facets` (checked: check_facet_keys, _facet_slot) for n_queries queries."""
+        slots = [self._facet_slot(f) for f in facets]
+        return _Counts(facets, [0] * len(facets), [s for s, _ in slots], [nb for _, nb in slots], n_queries)
+
     def _feature_slot(self, name):
         """The slot of feature `name` on this array's index; ValueError if it is not set."""
         names = list(self.host.features)
@@ -569,7 +673,7 @@ class SearchArray(ExtensionArray):
         return names.index(name)
 
     # -------------------------------------------------- batched, HBM-resident path
-    def search_topk(self, queries, k=10, similarity: Similarity = default_bm25, slop=0, where=None):
+    def search_topk(self, queries, k=10, similarity: Similarity = default_bm25, slop=0, where=None, facets=None):
         """queries: list of str (term) or list[str] (phrase).  Returns (docs uint32[Q,k],
         scores float32[Q,k]): per query the k best scores > 0, by score descending then id ascending, empty
         slots NO_DOC / 0.  Scores never leave HBM except the top-k (sa_score_batch_topk).
@@ -613,12 +717,29 @@ class SearchArray(ExtensionArray):
         A dtype other than bool raises TypeError and another shape ValueError, before any device work; every input
         refused without `where` is refused the same way with it.  Plain BM25 queries on the unsliced array rank as
         one-clause Or queries (sa_score_batch_topk_bool); the others take sa_score_batch_topk_sim.  A
-        mask per query costs len(self) / 8 bytes of host-to-device copy and device memory per query."""
+        mask per query costs len(self) / 8 bytes of host-to-device copy and device memory per query.
+
+        facets: hit and facet counts, as Lucene's totalHits and Elasticsearch's terms aggregations return them with
+        the top k.  A list of at most 4 distinct facet names (set_facet), possibly empty, returns
+        (docs, scores, hits), hits a Hits: per query q, hits.total[q] == np.count_nonzero(S_q) and
+        hits.facets[name][q] == np.bincount(codes[(S_q > 0) & (codes >= 0)], minlength=n_buckets), S_q being the
+        dense vector the call without `facets` ranks from (`where` applied).  docs and scores are bit for bit those of
+        the call without `facets`.  The counts are made where the device fold decides which docs rank; only the
+        counts come back.  Every query form the boolean path takes is accepted, with or without `where`; plain
+        queries then rank as one-clause Or queries through the boolean fold, which is slower than the term scan
+        that ranks them without `facets`.  On a view (NotImplementedError), under another similarity than
+        bm25_similarity (TypeError), and for a name not set, a name given twice or more than 4 names (ValueError),
+        the call is refused before any device work.  On a shard the counts are the shard's own docs.  facets=None
+        (the default) returns (docs, scores) as above."""
         from .query import Feature, is_boolean
         queries = list(queries)
         for q in queries:
             if isinstance(q, Feature):
                 raise TypeError(f"a Feature is a clause, not a query: write Bool(should=[{q!r}])")
+        if facets is not None:
+            facets = check_facet_keys(facets, "facet names")
+            bits = None if where is None else pack_where(where, len(self), len(queries))
+            return self._search_topk_mixed(queries, k, similarity, slop, bits, facets)
         if where is not None:
             bits = pack_where(where, len(self), len(queries))
             if any(is_boolean(q) for q in queries):
@@ -647,12 +768,13 @@ class SearchArray(ExtensionArray):
             raise TypeError("search_topk supports bm25_similarity, bm25_impact, bm25_legacy_similarity and "
                             f"classic_similarity, not {similarity!r}")
 
-    def _search_topk_plain_where(self, queries, k, similarity, slop, where):
+    def _search_topk_plain_where(self, queries, k, similarity, slop, where, facets=None):
         """search_topk of plain queries with a packed mask (pack_where): on a view or under a non-BM25 similarity
         through sa_score_batch_topk_sim, else each query as a one-clause Or through the boolean fold, which
         scores a clause exactly as .score(c, slop=slop).  The clauses are taken as the unmasked batch takes its
         queries (_topk_queries: a str is a term, any other iterable of str a phrase), and the C call checks their
-        term counts as the unmasked one does."""
+        term counts as the unmasked one does.  facets: names (checked by the caller) whose counts come back as a third
+        value, a Hits."""
         self._check_topk_similarity(similarity)
         if self.rows is not None or not isinstance(similarity, Bm25Similarity):
             return self._search_topk_sim(queries, k, similarity, slop, where)
@@ -665,15 +787,20 @@ class SearchArray(ExtensionArray):
             # query q: clause q, mm 1
             batch = BoolBatch(queries, np.arange(n + 1, dtype=np.uint32), None, np.ones(n, dtype=np.uint32), None,
                               None, None, None, n)
+            counts = None if facets is None else self._counts(facets, n)
+            if counts is not None:
+                dev.sync_facets(self.host)
             docs, scores, _ = self._bool_call(dev, batch, terms, c_starts, np.asarray(idfs, dtype=np.float32),
-                                              similarity, slop, k, where)
-        return docs, scores
+                                              similarity, slop, k, where, counts)
+        return (docs, scores) if counts is None else (docs, scores, counts.hits())
 
-    def _search_topk_mixed(self, queries, k, similarity, slop, where=None):
+    def _search_topk_mixed(self, queries, k, similarity, slop, where=None, facets=None):
         """search_topk of a batch holding boolean queries: the plain ones through search_topk as before, the boolean
         ones in one _search_topk_bool call per form present (query.bool_form), so that each runs the lightest
         instance that scores it, each clause with the idf .score gives it; results in query order.  where: a packed
-        mask (pack_where), its rows split with the queries."""
+        mask (pack_where), its rows split with the queries.  facets: facet names (check_facet_keys): every query, plain
+        ones included, runs through the boolean fold and (docs, scores, hits) comes back, the counts in query
+        order."""
         from .query import DISMAX, NESTED, OCCUR, OR_AND, bool_form, has_dismax, has_field, is_boolean
         if any(has_field(q) for q in queries if is_boolean(q)):
             raise ValueError("a Field clause names a DataFrame column: run queries over columns with "
@@ -683,6 +810,9 @@ class SearchArray(ExtensionArray):
                                       "compose .score() on the view")
         if not isinstance(similarity, Bm25Similarity):
             raise TypeError(f"boolean queries support bm25_similarity only, not {similarity!r}")
+        counted = facets is not None
+        if counted:
+            hits = self._counts(facets, len(queries)).hits()      # the names checked, and zero counts
         kind = np.asarray([bool_form(q) if is_boolean(q) else 0 for q in queries])     # 0: plain
         if any(has_dismax(q) for q, kd in zip(queries, kind) if kd >= DISMAX):
             self._check_dismax_params(similarity)
@@ -694,40 +824,53 @@ class SearchArray(ExtensionArray):
             if not part:
                 continue
             w = _where_part(where, sel)
-            if kd == 0 and where is not None:
+            if counted:
+                if kd == 0:
+                    docs[sel], scores[sel], h = self._search_topk_plain_where(part, k, similarity, slop, w, facets)
+                else:
+                    docs[sel], scores[sel], _, h = self._search_topk_bool(part, k, similarity, slop, w, facets)
+                hits.total[sel] = h.total
+                for name in facets:
+                    hits.facets[name][sel] = h.facets[name]
+            elif kd == 0 and where is not None:
                 docs[sel], scores[sel] = self._search_topk_plain_where(part, k, similarity, slop, w)
             elif kd == 0:
                 docs[sel], scores[sel] = self.search_topk(part, k=k, similarity=similarity, slop=slop)
             else:
                 docs[sel], scores[sel], _ = self._search_topk_bool(part, k, similarity, slop, w)
-        return docs, scores
+        return (docs, scores, hits) if counted else (docs, scores)
 
     def _check_dismax_params(self, similarity):
         """ValueError, before any device work, where DisMax members would not be sparse-safe for k1 / b."""
         from .query import check_dismax_members
         check_dismax_members([(0, "DisMax member")], lambda i: (similarity.k1, similarity.b, self.avg_doc_length, 0.0))
 
-    def _bool_call(self, dev, batch, terms, c_starts, idfs, similarity, slop, k, where):
+    def _bool_call(self, dev, batch, terms, c_starts, idfs, similarity, slop, k, where, counts=None):
         """sa_score_batch_topk_bool on a flattened batch (query.BoolBatch; its None arrays passed as NULL select the
-        instance) and a packed mask (None: no mask): (docs, scores, queries re-run exactly).  Call it with the lock
-        held and the rows applied."""
+        instance) and a packed mask (None: no mask): (docs, scores, queries re-run exactly).  counts: a _Counts,
+        filled by sa_score_batch_topk_bool_counts.  Call it with the lock held and the rows applied."""
         docs = np.empty((batch.n_queries, k), dtype=np.uint32)
         scores = np.empty((batch.n_queries, k), dtype=np.float32)
         n_redone = ctypes.c_uint32(0)
         opt = lambda a, p: None if a is None else p(a)      # noqa: E731
         p_w, stride = _where_args(where)
-        _lib.check(_lib.lib().sa_score_batch_topk_bool(
-            dev.handle, len(batch.node_starts) - 1, _lib.p_u32(batch.node_starts), opt(batch.clause_node, _lib.p_u32),
-            _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs), opt(batch.weights, _lib.p_f32),
-            opt(batch.occurs, _lib.p_u8), opt(batch.groups, _lib.p_u32), opt(batch.ties, _lib.p_f32),
-            _lib.p_u32(batch.mm), batch.n_queries, int(slop), self.avg_doc_length, similarity.k1, similarity.b, k,
-            p_w, len(self), stride, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
+        args = (dev.handle, len(batch.node_starts) - 1, _lib.p_u32(batch.node_starts),
+                opt(batch.clause_node, _lib.p_u32), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
+                opt(batch.weights, _lib.p_f32), opt(batch.occurs, _lib.p_u8), opt(batch.groups, _lib.p_u32),
+                opt(batch.ties, _lib.p_f32), _lib.p_u32(batch.mm), batch.n_queries, int(slop), self.avg_doc_length,
+                similarity.k1, similarity.b, k, p_w, len(self), stride, _lib.p_u32(docs), _lib.p_f32(scores),
+                ctypes.byref(n_redone))
+        if counts is None:
+            _lib.check(_lib.lib().sa_score_batch_topk_bool(*args))
+        else:
+            _lib.check(_lib.lib().sa_score_batch_topk_bool_counts(*args, *counts.args()))
         return docs, scores, n_redone.value
 
-    def _search_topk_bool(self, queries, k, similarity, slop, where=None):
+    def _search_topk_bool(self, queries, k, similarity, slop, where=None, facets=None):
         """Boolean queries of any form through sa_score_batch_topk_bool, flattened for the heaviest form among them
         (query.bool_form, flatten_bool): (docs, scores, queries re-run exactly).  DisMax members anywhere in the trees
-        need sparse-safe BM25 parameters (ValueError before any device work).  where: a packed mask (pack_where)."""
+        need sparse-safe BM25 parameters (ValueError before any device work).  where: a packed mask (pack_where).
+        facets: facet names (check_facet_keys) whose counts come back as a fourth value, a Hits."""
         from .query import DISMAX, OR_AND, bool_form, check_dismax_members, dismax_members, feature_terms, flatten_bool
         form = max(map(bool_form, queries), default=OR_AND)
         batch = flatten_bool(queries, form)
@@ -749,12 +892,16 @@ class SearchArray(ExtensionArray):
         if form >= DISMAX:
             check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
                                  lambda i: (similarity.k1, similarity.b, self.avg_doc_length, idfs[i]))
+        counts = None if facets is None else self._counts(facets, batch.n_queries)
         dev = self._device()
         with self._shared["lock"]:
             self._apply_rows(dev)
             if feats:
                 dev.sync_features(self.host)
-            return self._bool_call(dev, batch, terms, c_starts, idfs, similarity, slop, k, where)
+            if counts is not None:
+                dev.sync_facets(self.host)
+            out = self._bool_call(dev, batch, terms, c_starts, idfs, similarity, slop, k, where, counts)
+        return out if counts is None else out + (counts.hits(),)
 
     def _feature_clauses(self, clauses, feats, idf):
         """(terms, clause term starts, float32 idf) of a flattened clause list holding feature clauses: a text clause

@@ -28,6 +28,9 @@ ED_MAX_PHASE_ENTRIES = ED_MAX_FIELDS * SA_MAX_PHRASE_TERMS   # entries of one sa
 SA_OCCUR_SHOULD, SA_OCCUR_MUST, SA_OCCUR_FILTER, SA_OCCUR_MUST_NOT = 0, 1, 2, 3
 SA_MAX_FEATURES = 16              # include/searcharray_b200.h
 SA_FEATURE_TERM_BASE = 0xFF000000
+SA_MAX_FACETS = 8                 # include/searcharray_b200.h: facet columns of one index
+SA_FACET_MAX_BUCKETS = 1024       # include/searcharray_b200.h
+SA_BOOL_MAX_FACETS = 4            # include/searcharray_b200.h: facets counted in one call
 FEATURE_FUNCTIONS = {"linear": 0, "saturation": 1, "log": 2}     # SA_FEATURE_LINEAR, _SATURATION, _LOG
 
 Clause = Union[str, List[str]]

@@ -19,7 +19,7 @@ import numpy as np
 import pandas as pd
 
 from . import _lib
-from .postings import SearchArray, _where_args, pack_where
+from .postings import SearchArray, _Counts, _where_args, check_facet_keys, pack_where
 from .similarity import Bm25Similarity, Similarity, compute_idf, default_bm25
 
 
@@ -416,10 +416,11 @@ def edismax_topk(frame: pd.DataFrame, q: str, qf: List[str], k: int = 10, mm: Op
     return docs, scores
 
 
-def _fields_plan(frame, queries, similarity):
+def _fields_plan(frame, queries, similarity, extra=()):
     """fields_topk's refusals and field slots, before any device work: (the batch flattened for its form, at least
     OCCUR since the multi-field entry takes weights and roles (query.flatten_bool), field name -> slot, per-slot
-    arrays, per-slot similarities)."""
+    arrays, per-slot similarities).  extra: columns the call reads that no clause may name (facet columns), given
+    slots after the clauses' fields."""
     from .query import ED_MAX_FIELDS, OCCUR, Field, bool_form, flatten_bool, is_boolean
     queries = list(queries)
     for q in queries:
@@ -430,7 +431,8 @@ def _fields_plan(frame, queries, similarity):
     for c in clauses:
         if not isinstance(c, Field):
             raise ValueError(f"every clause of fields_topk names its column: Field(field, {c!r})")
-    names = list(dict.fromkeys(c.field for c in clauses))
+    read = set(c.field for c in clauses)      # the columns a clause scores: their similarities count
+    names = list(dict.fromkeys([c.field for c in clauses] + list(extra)))
     if len(names) > ED_MAX_FIELDS:
         raise ValueError(f"fields_topk takes at most {ED_MAX_FIELDS} distinct fields in one call, not {len(names)}")
     arrays = {f: get_field(frame, f) for f in names}
@@ -455,7 +457,7 @@ def _fields_plan(frame, queries, similarity):
         params = (np.float32(a.avg_doc_length), np.float32(sim.k1), np.float32(sim.b))
         s = slot_key.get(id(a._shared))
         if s is not None:
-            if (np.float32(arrays[slot_name[s]].avg_doc_length), np.float32(slot_sims[s].k1),
+            if f in read and (np.float32(arrays[slot_name[s]].avg_doc_length), np.float32(slot_sims[s].k1),
                     np.float32(slot_sims[s].b)) != params:
                 raise ValueError(f"{f!r} shares its device index with {slot_name[s]!r} but not its similarity: "
                                  "one index caches one set of BM25 parameters")
@@ -503,10 +505,11 @@ def _fields_clauses(clauses, slot_of, arrays):
     return terms, c_starts, c_idf, _u32([0 if c is None else slot_of[c.field] for c in clauses])
 
 
-def _fields_call(multi, arrays, sims, batch, prepared, k, slop, where=None):
+def _fields_call(multi, arrays, sims, batch, prepared, k, slop, where=None, counts=None):
     """sa_multi_score_batch_topk_bool on a flattened batch (query.BoolBatch; its None arrays passed as NULL select the
     instance) and prepared arrays (the fields locked): (docs, scores, queries re-run).  where: a packed mask
-    (postings.pack_where), None: no mask."""
+    (postings.pack_where), None: no mask.  counts: a postings._Counts, filled by
+    sa_multi_score_batch_topk_bool_counts."""
     terms, c_starts, c_idf, c_field = prepared
     n_redone = ctypes.c_uint32(0)
     avgdl = _f32([a.avg_doc_length for a in arrays])
@@ -516,25 +519,51 @@ def _fields_call(multi, arrays, sims, batch, prepared, k, slop, where=None):
     scores = np.empty((nq, k), dtype=np.float32)
     opt = lambda a, p: None if a is None else p(a)      # noqa: E731
     p_w, stride = _where_args(where)
-    _lib.check(_lib.lib().sa_multi_score_batch_topk_bool(
-        multi.handle, len(batch.node_starts) - 1, _lib.p_u32(batch.node_starts), opt(batch.clause_node, _lib.p_u32),
-        _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(c_idf), _lib.p_f32(batch.weights),
-        _lib.p_u8(batch.occurs), opt(batch.groups, _lib.p_u32), opt(batch.ties, _lib.p_f32), _lib.p_u32(batch.mm), nq,
-        int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1), _lib.p_f32(b), k, p_w, len(arrays[0]), stride,
-        _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone)))
+    args = (multi.handle, len(batch.node_starts) - 1, _lib.p_u32(batch.node_starts), opt(batch.clause_node, _lib.p_u32),
+            _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(c_idf), _lib.p_f32(batch.weights),
+            _lib.p_u8(batch.occurs), opt(batch.groups, _lib.p_u32), opt(batch.ties, _lib.p_f32), _lib.p_u32(batch.mm),
+            nq, int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1), _lib.p_f32(b), k, p_w, len(arrays[0]), stride,
+            _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone))
+    if counts is None:
+        _lib.check(_lib.lib().sa_multi_score_batch_topk_bool(*args))
+    else:
+        _lib.check(_lib.lib().sa_multi_score_batch_topk_bool_counts(*args, *counts.args()))
     return docs, scores, n_redone.value
 
 
-def _fields_topk(frame, queries, k, similarity, slop, where=None):
-    """fields_topk and the number of queries re-run exactly (candidate overflow)."""
+def _facet_pairs(frame, facets):
+    """fields_topk's facets= as (column, name) pairs, checked before any device work: a list of at most 4 distinct
+    pairs, each column a SearchArray column of the frame (get_field) on whose index the name is set (ValueError)."""
+    facets = check_facet_keys(facets, "(column, name) pairs")
+    for pair in facets:
+        if not (isinstance(pair, tuple) and len(pair) == 2 and isinstance(pair[1], str)):
+            raise TypeError(f"a facet of fields_topk is a (column, name) pair, not {pair!r}")
+        get_field(frame, pair[0])._facet_slot(pair[1])
+    return facets
+
+
+def _fields_topk(frame, queries, k, similarity, slop, where=None, facets=None):
+    """fields_topk and the number of queries re-run exactly (candidate overflow); with facets (a list of
+    (column, name) pairs), (docs, scores, queries re-run, Hits)."""
     queries = list(queries)
     if where is not None:
         where = pack_where(where, len(frame), len(queries))
-    batch, slot_of, arrays, sims = _fields_plan(frame, queries, similarity)
+    if facets is not None:
+        facets = _facet_pairs(frame, facets)
+    batch, slot_of, arrays, sims = _fields_plan(frame, queries, similarity,
+                                                extra=[] if facets is None else [c for c, _ in facets])
+    counts = None
+    if facets is not None:
+        slots = [arrays[slot_of[c]]._facet_slot(name) for c, name in facets]
+        counts = _Counts(facets, [slot_of[c] for c, _ in facets], [s for s, _ in slots], [nb for _, nb in slots],
+                         len(queries))
     multi = _multi_for(arrays)
     with _locked(multi, arrays):
         for arr in arrays:                 # a sliced view of the same column may have left its row filter installed
             arr._apply_rows(arr._device())
+        if counts is not None:
+            for s in set(counts.fields.tolist()):
+                arrays[s]._device().sync_facets(arrays[s].host)
         prepared = _fields_clauses(batch.clauses, slot_of, arrays)
         if batch.groups is not None:      # DisMax members: sparse-safe idf from their own fields
             from .query import check_dismax_members, dismax_members
@@ -542,11 +571,13 @@ def _fields_topk(frame, queries, k, similarity, slop, where=None):
             check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
                                  lambda i: (sims[slot_of[clauses[i].field]].k1, sims[slot_of[clauses[i].field]].b,
                                             arrays[slot_of[clauses[i].field]].avg_doc_length, prepared[2][i]))
-        return _fields_call(multi, arrays, sims, batch, prepared, k, slop, where)
+        out = _fields_call(multi, arrays, sims, batch, prepared, k, slop, where, counts)
+    return out if counts is None else out + (counts.hits(),)
 
 
 def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
-                similarity: Union[Similarity, Dict[str, Similarity]] = default_bm25, slop: int = 0, where=None):
+                similarity: Union[Similarity, Dict[str, Similarity]] = default_bm25, slop: int = 0, where=None,
+                facets=None):
     """Batched Or / And / Bool queries whose clauses are on several columns of `frame` -- Lucene's
     `+title:star overview:war -overview:trek`, or Elasticsearch's most_fields `title:alien^2 overview:alien` -- ranked
     on the device in one batch.  Every clause is a query.Field(field, term or phrase), or a Boost of one; phrases match
@@ -573,6 +604,18 @@ def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
     shape (len(frame),), one mask for the batch, or (len(queries), len(frame)), one per query.  Per query the
     result is the top k of np.where(mask_q, S_q, 0), S_q the composition above; the mask never changes a score
     (each column's idf, avgdl and doc lengths stay those of the whole column).  A dtype other than bool raises
-    TypeError and another shape ValueError, before any device work."""
+    TypeError and another shape ValueError, before any device work.
+
+    facets: hit and facet counts, as in SearchArray.search_topk -- a list of at most 4 distinct (column, name) pairs,
+    name a facet set on that column (SearchArray.set_facet), possibly empty -- returns (rows, scores, hits), a Hits
+    whose facets are keyed by the pairs: hits.total[q] == np.count_nonzero(S_q) and
+    hits.facets[(column, name)][q] == np.bincount(codes[(S_q > 0) & (codes >= 0)], minlength=n_buckets), S_q the
+    composition above with `where` applied.  The column may be any SearchArray column of the frame, read by a clause
+    or not; it takes part in the column checks above.  rows and scores are bit for bit those of the call without
+    `facets`.  A pair whose name is not set, a pair given twice or more than 4 pairs is a ValueError before any device
+    work."""
+    if facets is not None:
+        docs, scores, _, hits = _fields_topk(frame, queries, k, similarity, slop, where, facets)
+        return docs, scores, hits
     docs, scores, _ = _fields_topk(frame, queries, k, similarity, slop, where)
     return docs, scores
