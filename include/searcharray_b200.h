@@ -223,9 +223,10 @@ int sa_score_batch_topk_sim(sa_index *index, int kind, const uint32_t *terms, co
  * range are SA_ERR_ARG before any device work.  Only the boolean entry points read reserved ids; every other entry
  * point takes them as the out-of-range term ids they are.
  *
- * Hit and facet counts (the _counts entry points below, out_total non-NULL): Lucene's totalHits and Elasticsearch's terms aggregations, counted where
- * the fold decides which docs rank.  out_total[q] is the number of docs query q ranks (the docs whose score the top k
- * is taken from: s > 0 and every condition above, mask included), over all of them, not only the top k.  With
+ * Hit and facet counts (n_facets, facet_field, facet_slot, out_total and out_facet_counts, the last arguments; out_total
+ * non-NULL): Lucene's totalHits and Elasticsearch's terms aggregations, counted where the fold decides which docs
+ * rank.  out_total[q] is the number of docs query q ranks (the docs whose score the top k is taken from: s > 0 and
+ * every condition above, mask included), over all of them, not only the top k.  With
  * n_facets (<= SA_BOOL_MAX_FACETS) facets, facet i is the facet column facet_slot[i] (sa_index_set_facet) of the index
  * of field facet_field[i] (0 on the single-index entry point; a field slot of the multi on the multi-field one), with
  * B_i buckets, and out_facet_counts[q * (B_0 + ... + B_{n-1}) + B_0 + ... + B_{i-1} + b] is the number of docs query q
@@ -270,19 +271,9 @@ int sa_score_batch_topk_bool(sa_index *index, uint32_t n_nodes, const uint32_t *
                              const uint8_t *clause_occur, const uint32_t *clause_group, const float *clause_tie,
                              const uint32_t *mm, uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1,
                              float b, uint32_t k, const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
-                             uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
-/* sa_score_batch_topk_bool with the hit and facet counts above: the same arguments, then n_facets, facet_field,
- * facet_slot, out_total and out_facet_counts.  sa_score_batch_topk_bool is this call with out_total NULL. */
-int sa_score_batch_topk_bool_counts(sa_index *index, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                    const uint32_t *clause_node, const uint32_t *clause_terms,
-                                    const uint32_t *clause_term_starts, const float *clause_idf,
-                                    const float *clause_weight, const uint8_t *clause_occur,
-                                    const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
-                                    uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b,
-                                    uint32_t k, const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
-                                    uint32_t *out_docs, float *out_scores, uint32_t *n_redone, uint32_t n_facets,
-                                    const uint32_t *facet_field, const uint32_t *facet_slot, uint32_t *out_total,
-                                    uint32_t *out_facet_counts);
+                             uint32_t *out_docs, float *out_scores, uint32_t *n_redone, uint32_t n_facets,
+                             const uint32_t *facet_field, const uint32_t *facet_slot, uint32_t *out_total,
+                             uint32_t *out_facet_counts);
 
 /* The same batch in three stages, so a serving loop (or the benchmark) can keep the query
  * descriptors resident and time the device work alone: upload (H2D of descriptors), execute
@@ -391,6 +382,7 @@ int sa_multi_topk(sa_multi *multi, uint32_t k, uint32_t *out_docs, double *out_s
  * clause on it ranks nothing, a MUST_NOT clause on it vetoes nothing).  A DisMax group's members may sit on different
  * fields, each scored on its own: Elasticsearch's best_fields, and per-term groups inside an Or with mm for edismax's
  * term-centric qf.  Fields that share one sa_index must share (avg_doc_len, k1, b): the index caches one norm table.
+ * The hit and facet counts are sa_score_batch_topk_bool's, facet_field[i] being a field slot of the multi.
  * Result ids are global doc ids (doc_base added). */
 int sa_multi_score_batch_topk_bool(sa_multi *multi, uint32_t n_nodes, const uint32_t *node_clause_starts,
                                    const uint32_t *clause_node, const uint32_t *clause_field,
@@ -399,21 +391,9 @@ int sa_multi_score_batch_topk_bool(sa_multi *multi, uint32_t n_nodes, const uint
                                    const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
                                    uint32_t n_queries, uint32_t slop, const float *avg_doc_len, const float *k1,
                                    const float *b, uint32_t k, const uint32_t *where_bits, uint64_t where_n,
-                                   uint64_t where_stride, uint32_t *out_docs, float *out_scores, uint32_t *n_redone);
-/* sa_multi_score_batch_topk_bool with the hit and facet counts of sa_score_batch_topk_bool_counts, facet_field[i]
- * being a field slot of the multi. */
-int sa_multi_score_batch_topk_bool_counts(sa_multi *multi, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                          const uint32_t *clause_node, const uint32_t *clause_field,
-                                          const uint32_t *clause_terms, const uint32_t *clause_term_starts,
-                                          const float *clause_idf, const float *clause_weight,
-                                          const uint8_t *clause_occur, const uint32_t *clause_group,
-                                          const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
-                                          uint32_t slop, const float *avg_doc_len, const float *k1, const float *b,
-                                          uint32_t k, const uint32_t *where_bits, uint64_t where_n,
-                                          uint64_t where_stride, uint32_t *out_docs, float *out_scores,
-                                          uint32_t *n_redone, uint32_t n_facets, const uint32_t *facet_field,
-                                          const uint32_t *facet_slot, uint32_t *out_total,
-                                          uint32_t *out_facet_counts);
+                                   uint64_t where_stride, uint32_t *out_docs, float *out_scores, uint32_t *n_redone,
+                                   uint32_t n_facets, const uint32_t *facet_field, const uint32_t *facet_slot,
+                                   uint32_t *out_total, uint32_t *out_facet_counts);
 
 /* ------------------------------------------------- per-op exports (parity tests)
  * Device implementations of the reference's native ops on raw arrays (host in, host out),

@@ -18,9 +18,9 @@
 // Then the docs below mm are zeroed and the tile goes through flush_tile_collect, the float32 collector of every
 // other path, and topk_select_kernel ranks the candidates.
 //
-// One entry point per handle (sa_score_batch_topk_bool, sa_multi_score_batch_topk_bool) runs every form; the arrays
-// it is given select the form, and the form and the mask select one instance of bool_tile_kernel (bool_kernel).  The
-// flags add, in order:
+// One entry point per handle (sa_score_batch_topk_bool, sa_multi_score_batch_topk_bool) runs every form, with or
+// without counts; the arrays it is given select the form, and the form, the mask and the variant (plain, FEATURE or
+// COUNT) select one instance of bool_tile_kernel (bool_kernel).  The flags add, in order:
 //
 // OCCUR: Lucene's clause roles and per-clause weights, from a separate BoolOccur array: MUST / SHOULD clauses add
 // weight * score, only SHOULD clauses count towards mm, and two per-thread masks over the thread's 32 docs record
@@ -49,20 +49,20 @@
 // is masked: a disallowed doc never ranks whatever its nested rows hold.
 //
 // FEATURE: feature clauses (sa_index_set_feature) on the OCCUR, FIELDS, DISMAX and NESTED forms, in instances of
-// their own (bool_feature_kernel) so that a batch without one runs the instances above unchanged.  A feature clause
-// is present in a tile iff its column's tile flag is set; in the fold its owners read their float4s of the column with
-// cached loads (the CTAs of a batch's queries on one tile read the same 32 KB) and put v = f(x) into the shared tile,
-// which the term clauses' fold then reads as it reads BM25 scores.  An Or / And batch with a feature runs as OCCUR.
+// their own so that a batch without one runs the instances above unchanged.  A feature clause is present in a tile iff
+// its column's tile flag is set; in the fold its owners read their float4s of the column with cached loads (the CTAs
+// of a batch's queries on one tile read the same 32 KB) and put v = f(x) into the shared tile, which the term clauses'
+// fold then reads as it reads BM25 scores.  An Or / And batch with a feature runs as OCCUR.
 //
-// COUNT: hit and facet counts (sa_score_batch_topk_bool_counts), in instances of their own (bool_count_kernel, on the
-// FEATURE instances of OCCUR and above, an Or / And batch running as OCCUR) so that a batch without counts runs the
-// instances above unchanged.  After the tile's collect, s_tile still holds the ranked values (+0 where a doc does not
-// rank); each thread turns its 32 into a mask, a warp adds its popcounts into the query's total with one atomic, and
-// on a tile where anything ranks s_tile is reused as a shared histogram of the call's facets (<= 4 x 1,024 u32 =
-// 16 KB): each thread reads the codes of its ranked docs (one 8-byte load per float4 group with a ranked doc), one
-// shared atomic per ranked doc with a code, and the non-zero bins go to the query's counts with global atomics.  The
-// store passes of a nested call, and a query re-run after a candidate overflow, run the instances without COUNT: the
-// first pass has counted every tile of every query.
+// COUNT: hit and facet counts (an entry point's out_total non-NULL), in instances of their own (the FEATURE instances
+// with COUNT, an Or / And batch running as OCCUR) so that a batch without counts runs the instances above unchanged.
+// After the tile's collect, s_tile still holds the ranked values (+0 where a doc does not rank); each thread turns its
+// 32 into a mask, a warp adds its popcounts into the query's total with one atomic, and on a tile where anything ranks
+// s_tile is reused as a shared histogram of the call's facets (<= 4 x 1,024 u32 = 16 KB): each thread reads the codes
+// of its ranked docs (one 8-byte load per float4 group with a ranked doc), one shared atomic per ranked doc with a
+// code, and the non-zero bins go to the query's counts with global atomics.  The store passes of a nested call, and a
+// query re-run after a candidate overflow, run the instances without COUNT: the first pass has counted every tile of
+// every query.
 #include "sa_multi.cuh"
 #include "sa_term.cuh"
 #include "sa_phrase.cuh"
@@ -359,15 +359,11 @@ __device__ __forceinline__ void bool_count_tile(const BoolCount &cn, float *s_ti
 // WHERE: only docs whose bit of the mask row of query blockIdx.x is set rank (never in a store pass).  FEATURE (with
 // OCCUR): clauses whose row is SA_BOOL_FEATURE_ROW score their column feat[clause] (BoolFeature).  COUNT (with
 // FEATURE): the collected tile is counted into `cn` (bool_count_tile).
-template <bool OCCUR, bool FIELDS, bool DISMAX = false, bool NESTED = false, bool WHERE = false, bool FEATURE = false,
-          bool COUNT = false>
+template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, bool FEATURE, bool COUNT>
 __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__restrict__ occ,
-                                          const BoolField *__restrict__ fld,
-                                          const BoolGroup *__restrict__ grp = nullptr, float *s_dyn = nullptr,
-                                          unsigned long long *s_g = nullptr, const BoolNest nb = BoolNest{},
-                                          const WhereMask wh = WhereMask{nullptr, 0},
-                                          const BoolFeature *__restrict__ feat = nullptr,
-                                          const BoolCount cn = BoolCount{}) {
+                                          const BoolField *__restrict__ fld, const BoolGroup *__restrict__ grp,
+                                          float *s_dyn, unsigned long long *s_g, const BoolNest nb, const WhereMask wh,
+                                          const BoolFeature *__restrict__ feat, const BoolCount cn) {
     constexpr int PER = SA_TILE_DOCS / SA_TERM_THREADS / 4;        // float4 groups per thread
     __shared__ __align__(16) float s_tile[SA_TILE_DOCS];
     __shared__ u32 s_lo[SA_BOOL_MAX_CLAUSES], s_hi[SA_BOOL_MAX_CLAUSES];
@@ -586,55 +582,34 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
     if (COUNT) bool_count_tile(cn, s_tile);
 }
 
-// Every instance of the fold: bool_tile with the arguments its form reads (the others are NULL and never read).
-// MIN_CTAS holds an instance to the CTAs per SM it was tuned for (0: no minimum); bool_kernel lists the ten instances.
-// DISMAX: the groups' running max and sum live in SA_BOOL_DISMAX_SMEM bytes of dynamic shared memory (a thread's
-// strips, owner-only, so no extra barriers).
+// Every instance of the fold: bool_tile with every argument, of which it reads those its flags name (the others are
+// NULL and never read).  MIN_CTAS holds an instance to the CTAs per SM it was tuned for (0: no minimum); bool_kernel
+// lists the instances.  DISMAX: the groups' running max and sum live in SA_BOOL_DISMAX_SMEM bytes of dynamic shared
+// memory (a thread's strips, owner-only, so no extra barriers).
 #define SA_BOOL_DISMAX_SMEM (2 * SA_TILE_DOCS * sizeof(float))
 
 // bool_tile's s_g placed ahead of the fold's own shared arrays.  Where the compiler places a __shared__ array follows
-// where it is declared: the unmasked DisMax instances were tuned with s_g first (a local of this helper, one instance
-// per kernel), the masked ones with it last (a local of the kernel), and each keeps its layout.
+// where it is declared: the unmasked DisMax instances without FEATURE were tuned with s_g first (a local of this
+// helper, one instance per kernel), the others with it last (a local of the kernel), and each keeps its layout.
 template <bool NESTED>
 __device__ __forceinline__ unsigned long long *bool_s_g_first() {
     __shared__ unsigned long long s_g[3];
     return s_g;
 }
 
-template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, int MIN_CTAS>
+template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, bool FEATURE, bool COUNT, int MIN_CTAS>
 __global__ void __launch_bounds__(SA_TERM_THREADS, MIN_CTAS)
 bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
-                 const BoolGroup *__restrict__ grp, const BoolNest nb, const WhereMask wh) {
+                 const BoolGroup *__restrict__ grp, const BoolNest nb, const WhereMask wh,
+                 const BoolFeature *__restrict__ feat, const BoolCount cn) {
     extern __shared__ __align__(16) float s_dyn[];
-    if constexpr (DISMAX && !WHERE) {
-        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE>(a, occ, fld, grp, s_dyn, bool_s_g_first<NESTED>(), nb, wh);
+    if constexpr (DISMAX && !WHERE && !FEATURE) {
+        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, FEATURE, COUNT>(a, occ, fld, grp, s_dyn,
+                                                                        bool_s_g_first<NESTED>(), nb, wh, feat, cn);
     } else {
         __shared__ unsigned long long s_g[3];
-        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE>(a, occ, fld, grp, s_dyn, s_g, nb, wh);
+        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, FEATURE, COUNT>(a, occ, fld, grp, s_dyn, s_g, nb, wh, feat, cn);
     }
-}
-
-// The FEATURE instances: bool_tile_kernel's forms from OCCUR up, with the batch's feature table.  The DisMax shared
-// layout needs no tuned placement here (s_g a local of the kernel, as the masked instances have it).
-template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, int MIN_CTAS>
-__global__ void __launch_bounds__(SA_TERM_THREADS, MIN_CTAS)
-bool_feature_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
-                    const BoolGroup *__restrict__ grp, const BoolNest nb, const WhereMask wh,
-                    const BoolFeature *__restrict__ feat) {
-    extern __shared__ __align__(16) float s_dyn[];
-    __shared__ unsigned long long s_g[3];
-    bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, true>(a, occ, fld, grp, s_dyn, s_g, nb, wh, feat);
-}
-
-// The COUNT instances: bool_feature_kernel's, counting into `cn`.
-template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, int MIN_CTAS>
-__global__ void __launch_bounds__(SA_TERM_THREADS, MIN_CTAS)
-bool_count_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
-                  const BoolGroup *__restrict__ grp, const BoolNest nb, const WhereMask wh,
-                  const BoolFeature *__restrict__ feat, const BoolCount cn) {
-    extern __shared__ __align__(16) float s_dyn[];
-    __shared__ unsigned long long s_g[3];
-    bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, true, true>(a, occ, fld, grp, s_dyn, s_g, nb, wh, feat, cn);
 }
 
 // ------------------------------------------------------------------------------------------------------------ host
@@ -644,50 +619,56 @@ namespace {
 // DisMax groups (on a field table, a single-index call passing one field); nested nodes.
 enum BoolForm { BOOL_OR_AND, BOOL_OCCUR, BOOL_FIELDS, BOOL_DISMAX, BOOL_NESTED };
 
-typedef void (*BoolKernel)(BoolArgs, const BoolOccur *, const BoolField *, const BoolGroup *, BoolNest, WhereMask);
+// The instances of a form: plain; FEATURE, for a batch with feature clauses; COUNT (with FEATURE), for the first pass
+// of a counting call.  The last two exist from BOOL_OCCUR up.
+enum BoolVariant { BOOL_PLAIN, BOOL_FEATURE, BOOL_COUNT };
+
+typedef void (*BoolKernel)(BoolArgs, const BoolOccur *, const BoolField *, const BoolGroup *, BoolNest, WhereMask,
+                           const BoolFeature *, BoolCount);
 
 // The instance a launch of `form` runs, with or without a document mask.  The fields instance is held to three CTAs per
 // SM, as the single-field roles instance runs (80 registers, no spills; at two, 90 registers, it ran 23-24% slower);
 // the DisMax and nested ones to two (DESIGN.md sections 3.10.3, 3.10.4); each masked instance to its unmasked
-// instance's CTAs per SM (section 3.11).  A nested call's store passes run the unmasked nested instance.
-BoolKernel bool_kernel(BoolForm form, bool masked) {
-    static const BoolKernel instances[5][2] = {
-        {bool_tile_kernel<false, false, false, false, false, 0>, bool_tile_kernel<false, false, false, false, true, 2>},
-        {bool_tile_kernel<true, false, false, false, false, 0>, bool_tile_kernel<true, false, false, false, true, 3>},
-        {bool_tile_kernel<true, true, false, false, false, 3>, bool_tile_kernel<true, true, false, false, true, 3>},
-        {bool_tile_kernel<true, true, true, false, false, 2>, bool_tile_kernel<true, true, true, false, true, 2>},
-        {bool_tile_kernel<true, true, true, true, false, 2>, bool_tile_kernel<true, true, true, true, true, 2>},
+// instance's CTAs per SM (section 3.11); the FEATURE and COUNT instances to their form's (three for the roles form).
+// A nested call's store passes run the unmasked nested instance.
+BoolKernel bool_kernel(BoolForm form, bool masked, BoolVariant variant) {
+    static const BoolKernel instances[3][5][2] = {
+        {
+            {bool_tile_kernel<false, false, false, false, false, false, false, 0>,
+             bool_tile_kernel<false, false, false, false, true, false, false, 2>},
+            {bool_tile_kernel<true, false, false, false, false, false, false, 0>,
+             bool_tile_kernel<true, false, false, false, true, false, false, 3>},
+            {bool_tile_kernel<true, true, false, false, false, false, false, 3>,
+             bool_tile_kernel<true, true, false, false, true, false, false, 3>},
+            {bool_tile_kernel<true, true, true, false, false, false, false, 2>,
+             bool_tile_kernel<true, true, true, false, true, false, false, 2>},
+            {bool_tile_kernel<true, true, true, true, false, false, false, 2>,
+             bool_tile_kernel<true, true, true, true, true, false, false, 2>},
+        },
+        {
+            {nullptr, nullptr},
+            {bool_tile_kernel<true, false, false, false, false, true, false, 3>,
+             bool_tile_kernel<true, false, false, false, true, true, false, 3>},
+            {bool_tile_kernel<true, true, false, false, false, true, false, 3>,
+             bool_tile_kernel<true, true, false, false, true, true, false, 3>},
+            {bool_tile_kernel<true, true, true, false, false, true, false, 2>,
+             bool_tile_kernel<true, true, true, false, true, true, false, 2>},
+            {bool_tile_kernel<true, true, true, true, false, true, false, 2>,
+             bool_tile_kernel<true, true, true, true, true, true, false, 2>},
+        },
+        {
+            {nullptr, nullptr},
+            {bool_tile_kernel<true, false, false, false, false, true, true, 3>,
+             bool_tile_kernel<true, false, false, false, true, true, true, 3>},
+            {bool_tile_kernel<true, true, false, false, false, true, true, 3>,
+             bool_tile_kernel<true, true, false, false, true, true, true, 3>},
+            {bool_tile_kernel<true, true, true, false, false, true, true, 2>,
+             bool_tile_kernel<true, true, true, false, true, true, true, 2>},
+            {bool_tile_kernel<true, true, true, true, false, true, true, 2>,
+             bool_tile_kernel<true, true, true, true, true, true, true, 2>},
+        },
     };
-    return instances[form][masked];
-}
-
-typedef void (*BoolFeatureKernel)(BoolArgs, const BoolOccur *, const BoolField *, const BoolGroup *, BoolNest,
-                                  WhereMask, const BoolFeature *);
-
-// The FEATURE instance a launch of `form` (BOOL_OCCUR or above) runs, each at its form's CTAs per SM.
-BoolFeatureKernel bool_feature_kernel_for(BoolForm form, bool masked) {
-    static const BoolFeatureKernel instances[4][2] = {
-        {bool_feature_kernel<true, false, false, false, false, 3>, bool_feature_kernel<true, false, false, false, true, 3>},
-        {bool_feature_kernel<true, true, false, false, false, 3>, bool_feature_kernel<true, true, false, false, true, 3>},
-        {bool_feature_kernel<true, true, true, false, false, 2>, bool_feature_kernel<true, true, true, false, true, 2>},
-        {bool_feature_kernel<true, true, true, true, false, 2>, bool_feature_kernel<true, true, true, true, true, 2>},
-    };
-    return instances[form - BOOL_OCCUR][masked];
-}
-
-typedef void (*BoolCountKernel)(BoolArgs, const BoolOccur *, const BoolField *, const BoolGroup *, BoolNest,
-                                WhereMask, const BoolFeature *, BoolCount);
-
-// The COUNT instance of the first pass of a counting call of `form` (BOOL_OCCUR or above), each at its form's CTAs
-// per SM.
-BoolCountKernel bool_count_kernel_for(BoolForm form, bool masked) {
-    static const BoolCountKernel instances[4][2] = {
-        {bool_count_kernel<true, false, false, false, false, 3>, bool_count_kernel<true, false, false, false, true, 3>},
-        {bool_count_kernel<true, true, false, false, false, 3>, bool_count_kernel<true, true, false, false, true, 3>},
-        {bool_count_kernel<true, true, true, false, false, 2>, bool_count_kernel<true, true, true, false, true, 2>},
-        {bool_count_kernel<true, true, true, true, false, 2>, bool_count_kernel<true, true, true, true, true, 2>},
-    };
-    return instances[form - BOOL_OCCUR][masked];
+    return instances[variant][form][masked];
 }
 
 // The fields of one call and where the call keeps its state.  The single-index entry point passes one field and the
@@ -728,9 +709,14 @@ struct BoolPlan {
                                         // is nested[i]'s descriptor
     std::vector<u32> nest;              // per clause, as clauses: 1 for a nested clause (BOOL_NESTED)
     std::vector<BoolFeature> features;  // per clause, as clauses, when a clause is a feature (the FEATURE instances)
-    bool counting = false;              // the first pass runs the COUNT instances into `count`
     BoolCount count{};                  // total and counts: the call's rows (bool_run_group offsets them per launch)
 };
+
+// The variant a launch runs: COUNT for the first pass of a counting call (count), otherwise FEATURE when the batch has
+// a feature clause.
+BoolVariant bool_variant(const BoolPlan &P, bool count) {
+    return count ? BOOL_COUNT : P.features.empty() ? BOOL_PLAIN : BOOL_FEATURE;
+}
 
 // The count rows of the phrase clauses of queries [q0, q1) and of their nested nodes (rows are numbered within the
 // group), each on its clause's field, synchronously.
@@ -758,7 +744,7 @@ int bool_build_rows(const BoolCall &X, const BoolPlan &P, const uint32_t *clause
 }
 
 // Queries [q0, q1) with `slots` candidate slots per tile: their rows, the tile kernel and the selection, enqueued.
-// count: the first pass of a counting call (P.counting), the top-level launch counting into P.count.
+// count: the first pass of a counting call, the top-level launch counting into P.count.
 int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_terms,
                    const uint32_t *clause_term_starts, u32 slop, u32 k, u32 slots, u32 q0, u32 q1, bool count) {
     sa_index *ix = X.lead();
@@ -796,23 +782,18 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
     const BoolGroup *grp = P.form >= BOOL_DISMAX ? S.d_groups.as<BoolGroup>() : nullptr;
     BoolNest nb{nullptr, nullptr, nullptr, 0};
     const size_t smem = P.form >= BOOL_DISMAX ? SA_BOOL_DISMAX_SMEM : 0;
-    // the form's instance, or its FEATURE instance when the call has feature clauses
     const BoolFeature *feat = P.features.empty() ? nullptr : S.d_feat.as<BoolFeature>();
     BoolCount cn = P.count;                 // row 0 of the launch is query q0's
     if (count) {
         cn.total += q0;
         cn.counts += (u64)q0 * cn.n_bins;
     }
-    auto launch = [&](bool masked, u32 n_q, const BoolArgs &args, const BoolNest &n, const WhereMask &w, bool c) {
-        const dim3 grid(n_q, n_tiles);
-        if (c)
-            bool_count_kernel_for(P.form, masked)<<<grid, SA_TERM_THREADS, smem, ix->stream>>>(args, occ, fld, grp, n, w,
-                                                                                             feat, cn);
-        else if (feat)
-            bool_feature_kernel_for(P.form, masked)<<<grid, SA_TERM_THREADS, smem, ix->stream>>>(args, occ, fld, grp, n,
-                                                                                             w, feat);
-        else
-            bool_kernel(P.form, masked)<<<grid, SA_TERM_THREADS, smem, ix->stream>>>(args, occ, fld, grp, n, w);
+    auto launch = [&](bool c, bool masked, u32 n_q, const BoolArgs &args, const BoolNest &n, const WhereMask &w) -> int {
+        bool_kernel(P.form, masked, bool_variant(P, c))<<<dim3(n_q, n_tiles), SA_TERM_THREADS, smem, ix->stream>>>(
+            args, occ, fld, grp, n, w, feat, cn);
+        SA_CUDA(cudaGetLastError());
+        ix->stats.total_launches++;
+        return SA_OK;
     };
     if (P.form == BOOL_NESTED) {
         // the nested nodes of these queries, deepest level first (one launch per level: a level's nodes of the run
@@ -825,23 +806,18 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
             while (j < P.nested.size() && in_run(j) && P.depth[P.nested[j]] == P.depth[P.nested[i]]) j++;
             BoolArgs an = a;
             an.queries = S.d_queries.as<BoolQuery>() + P.n_top + i;
-            launch(false, (u32)(j - i), an, nb, WhereMask{nullptr, 0}, false);
-            SA_CUDA(cudaGetLastError());
-            ix->stats.total_launches++;
+            if ((rc = launch(false, false, (u32)(j - i), an, nb, WhereMask{nullptr, 0}))) return rc;
             i = j;
         }
         nb.store = nullptr;
     }
-    launch(wh.bits != nullptr, nq, a, nb, wh, count);
-    SA_CUDA(cudaGetLastError());
-    ix->stats.total_launches++;
+    if ((rc = launch(count, wh.bits != nullptr, nq, a, nb, wh))) return rc;
     return launch_topk_select(ix, t, nq, ix->doc_base, d_keys, S.d_out_index.as<u32>() + q0);
 }
 
 // The DisMax instances' dynamic shared memory above the default 48 KB, and the carveout that fits two CTAs per SM
 // (~2 x 98 KB of shared memory), on the current device (function attributes are per device).
-template <typename Kernel>
-int bool_dismax_smem(Kernel kernel) {
+int bool_dismax_smem(BoolKernel kernel) {
     SA_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SA_BOOL_DISMAX_SMEM));
     SA_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
                                  (int)cudaSharedmemCarveoutMaxShared));
@@ -1143,14 +1119,12 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
     if ((rc = sa_where_upload(lead, S.d_where, X.where_bits, lead->n_docs, X.where_stride, n_queries, &X.where)))
         return rc;
     if (dismax) {
-        if (P.features.empty() ? ((rc = bool_dismax_smem(bool_kernel(P.form, false))) ||
-                                  (X.where.bits && (rc = bool_dismax_smem(bool_kernel(P.form, true)))))
-                               : ((rc = bool_dismax_smem(bool_feature_kernel_for(P.form, false))) ||
-                                  (X.where.bits && (rc = bool_dismax_smem(bool_feature_kernel_for(P.form, true))))))
-            return rc;
-        if (counting && ((rc = bool_dismax_smem(bool_count_kernel_for(P.form, false))) ||
-                         (X.where.bits && (rc = bool_dismax_smem(bool_count_kernel_for(P.form, true))))))
-            return rc;
+        // the first pass's variant and that of the store passes and re-runs, each masked only when the call is
+        const BoolVariant first = bool_variant(P, counting), rest = bool_variant(P, false);
+        for (int masked = 0; masked <= (X.where.bits != nullptr); masked++)
+            if ((rc = bool_dismax_smem(bool_kernel(P.form, masked, first))) ||
+                (rest != first && (rc = bool_dismax_smem(bool_kernel(P.form, masked, rest)))))
+                return rc;
         SA_CUDA(cudaMemcpyAsync(S.d_groups.p, P.groups.data(), P.groups.size() * sizeof(BoolGroup), cudaMemcpyHostToDevice, lead->stream));
     }
     if (nested) {
@@ -1162,7 +1136,6 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
     u32 *d_ovf = (u32 *)(S.d_keys.as<u64>() + nk);
     SA_CUDA(cudaMemsetAsync(d_ovf, 0, (size_t)n_queries * sizeof(u32) + count_bytes, lead->stream));
     if (counting) {
-        P.counting = true;
         P.count = count;
         P.count.total = d_ovf + n_queries;
         P.count.counts = d_ovf + 2 * (size_t)n_queries;
@@ -1202,18 +1175,26 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
     return SA_OK;
 }
 
-// sa_score_batch_topk_bool: the index's own lock, state and buffers.
-int bool_topk_index(sa_index *ix, uint32_t n_nodes, const uint32_t *query_clause_starts,
-                    const uint32_t *clause_node, const uint32_t *clause_terms,
-                    const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
-                    const uint8_t *clause_occur, const uint32_t *clause_group, const float *clause_tie,
-                    const uint32_t *mm, uint32_t n_queries, uint32_t slop,
-                    float avg_doc_len, float k1, float b, uint32_t k, const uint32_t *where_bits, uint64_t where_n,
-                    uint64_t where_stride, uint32_t *out_docs, float *out_scores, uint32_t *n_redone,
-                    uint32_t n_facets, const uint32_t *facet_field, const uint32_t *facet_slot, uint32_t *out_total,
-                    uint32_t *out_facet_counts) {
+}  // namespace
+
+// bool_topk under the index's own lock, with its state and buffers.
+extern "C" int sa_score_batch_topk_bool(sa_index *ix, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                        const uint32_t *clause_node, const uint32_t *clause_terms,
+                                        const uint32_t *clause_term_starts, const float *clause_idf,
+                                        const float *clause_weight, const uint8_t *clause_occur,
+                                        const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
+                                        uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b,
+                                        uint32_t k, const uint32_t *where_bits, uint64_t where_n,
+                                        uint64_t where_stride, uint32_t *out_docs, float *out_scores,
+                                        uint32_t *n_redone, uint32_t n_facets, const uint32_t *facet_field,
+                                        const uint32_t *facet_slot, uint32_t *out_total, uint32_t *out_facet_counts) {
+    SA_CHECK(!clause_weight == !clause_occur, "clause_weight and clause_occur are both given or both NULL");
+    SA_CHECK(!clause_group == !clause_tie && (!clause_group || clause_occur),
+             "clause_group and clause_tie are both given (with clause_occur) or both NULL");
+    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
+             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
     SA_CHECK(ix && out_docs && out_scores, "NULL argument");
-    SA_CHECK(n_nodes == 0 || (query_clause_starts && clause_terms && clause_term_starts && clause_idf && mm),
+    SA_CHECK(n_nodes == 0 || (node_clause_starts && clause_terms && clause_term_starts && clause_idf && mm),
              "NULL argument");
     SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
     if (n_redone) *n_redone = 0;
@@ -1236,23 +1217,29 @@ int bool_topk_index(sa_index *ix, uint32_t n_nodes, const uint32_t *query_clause
     X.facet_slot = facet_slot;
     X.out_total = out_total;
     X.out_facet_counts = out_facet_counts;
-    return bool_topk(X, n_nodes, query_clause_starts, clause_node, nullptr, clause_terms, clause_term_starts,
+    return bool_topk(X, n_nodes, node_clause_starts, clause_node, nullptr, clause_terms, clause_term_starts,
                      clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
                      out_docs, out_scores, n_redone);
 }
 
-// sa_multi_score_batch_topk_bool: the multi's lock, state and candidate buffer.
-int bool_topk_multi(sa_multi *m, uint32_t n_nodes, const uint32_t *query_clause_starts,
-                    const uint32_t *clause_node, const uint32_t *clause_field,
-                    const uint32_t *clause_terms, const uint32_t *clause_term_starts, const float *clause_idf,
-                    const float *clause_weight, const uint8_t *clause_occur, const uint32_t *clause_group,
-                    const float *clause_tie, const uint32_t *mm, uint32_t n_queries, uint32_t slop,
-                    const float *avg_doc_len, const float *k1, const float *b, uint32_t k,
-                    const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride, uint32_t *out_docs,
-                    float *out_scores, uint32_t *n_redone, uint32_t n_facets, const uint32_t *facet_field,
-                    const uint32_t *facet_slot, uint32_t *out_total, uint32_t *out_facet_counts) {
+// bool_topk under the multi's lock, with its state and candidate buffer.
+extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                              const uint32_t *clause_node, const uint32_t *clause_field,
+                                              const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                              const float *clause_idf, const float *clause_weight,
+                                              const uint8_t *clause_occur, const uint32_t *clause_group,
+                                              const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
+                                              uint32_t slop, const float *avg_doc_len, const float *k1, const float *b,
+                                              uint32_t k, const uint32_t *where_bits, uint64_t where_n,
+                                              uint64_t where_stride, uint32_t *out_docs, float *out_scores,
+                                              uint32_t *n_redone, uint32_t n_facets, const uint32_t *facet_field,
+                                              const uint32_t *facet_slot, uint32_t *out_total,
+                                              uint32_t *out_facet_counts) {
+    SA_CHECK(!clause_group == !clause_tie, "clause_group and clause_tie are both given or both NULL");
+    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
+             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
     SA_CHECK(m && out_docs && out_scores && avg_doc_len && k1 && b, "NULL argument");
-    SA_CHECK(n_nodes == 0 || (query_clause_starts && clause_field && clause_terms && clause_term_starts &&
+    SA_CHECK(n_nodes == 0 || (node_clause_starts && clause_field && clause_terms && clause_term_starts &&
                                 clause_idf && clause_weight && clause_occur && mm), "NULL argument");
     SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
     if (n_redone) *n_redone = 0;
@@ -1290,101 +1277,7 @@ int bool_topk_multi(sa_multi *m, uint32_t n_nodes, const uint32_t *query_clause_
     X.facet_slot = facet_slot;
     X.out_total = out_total;
     X.out_facet_counts = out_facet_counts;
-    return bool_topk(X, n_nodes, query_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
+    return bool_topk(X, n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
                      clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
                      out_docs, out_scores, n_redone);
-}
-
-// The argument pairings every form checks, at both single-index entry points.
-int bool_check_index_arrays(uint32_t n_nodes, const uint32_t *clause_node, const float *clause_weight,
-                            const uint8_t *clause_occur, const uint32_t *clause_group, const float *clause_tie,
-                            uint32_t n_queries) {
-    SA_CHECK(!clause_weight == !clause_occur, "clause_weight and clause_occur are both given or both NULL");
-    SA_CHECK(!clause_group == !clause_tie && (!clause_group || clause_occur),
-             "clause_group and clause_tie are both given (with clause_occur) or both NULL");
-    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
-             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
-    return SA_OK;
-}
-
-// ... and at both multi-field ones.
-int bool_check_multi_arrays(uint32_t n_nodes, const uint32_t *clause_node, const uint32_t *clause_group,
-                            const float *clause_tie, uint32_t n_queries) {
-    SA_CHECK(!clause_group == !clause_tie, "clause_group and clause_tie are both given or both NULL");
-    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
-             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
-    return SA_OK;
-}
-
-}  // namespace
-
-extern "C" int sa_score_batch_topk_bool(sa_index *ix, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                        const uint32_t *clause_node, const uint32_t *clause_terms,
-                                        const uint32_t *clause_term_starts, const float *clause_idf,
-                                        const float *clause_weight, const uint8_t *clause_occur,
-                                        const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
-                                        uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b,
-                                        uint32_t k, const uint32_t *where_bits, uint64_t where_n,
-                                        uint64_t where_stride, uint32_t *out_docs, float *out_scores,
-                                        uint32_t *n_redone) {
-    return sa_score_batch_topk_bool_counts(ix, n_nodes, node_clause_starts, clause_node, clause_terms,
-                                           clause_term_starts, clause_idf, clause_weight, clause_occur, clause_group,
-                                           clause_tie, mm, n_queries, slop, avg_doc_len, k1, b, k, where_bits, where_n,
-                                           where_stride, out_docs, out_scores, n_redone, 0, nullptr, nullptr, nullptr,
-                                           nullptr);
-}
-
-extern "C" int sa_score_batch_topk_bool_counts(sa_index *ix, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                               const uint32_t *clause_node, const uint32_t *clause_terms,
-                                               const uint32_t *clause_term_starts, const float *clause_idf,
-                                               const float *clause_weight, const uint8_t *clause_occur,
-                                               const uint32_t *clause_group, const float *clause_tie,
-                                               const uint32_t *mm, uint32_t n_queries, uint32_t slop,
-                                               float avg_doc_len, float k1, float b, uint32_t k,
-                                               const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
-                                               uint32_t *out_docs, float *out_scores, uint32_t *n_redone,
-                                               uint32_t n_facets, const uint32_t *facet_field,
-                                               const uint32_t *facet_slot, uint32_t *out_total,
-                                               uint32_t *out_facet_counts) {
-    int rc;
-    if ((rc = bool_check_index_arrays(n_nodes, clause_node, clause_weight, clause_occur, clause_group, clause_tie,
-                                      n_queries)))
-        return rc;
-    return bool_topk_index(ix, n_nodes, node_clause_starts, clause_node, clause_terms, clause_term_starts, clause_idf,
-                           clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, avg_doc_len,
-                           k1, b, k, where_bits, where_n, where_stride, out_docs, out_scores, n_redone, n_facets,
-                           facet_field, facet_slot, out_total, out_facet_counts);
-}
-
-extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                              const uint32_t *clause_node, const uint32_t *clause_field,
-                                              const uint32_t *clause_terms, const uint32_t *clause_term_starts,
-                                              const float *clause_idf, const float *clause_weight,
-                                              const uint8_t *clause_occur, const uint32_t *clause_group,
-                                              const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
-                                              uint32_t slop, const float *avg_doc_len, const float *k1, const float *b,
-                                              uint32_t k, const uint32_t *where_bits, uint64_t where_n,
-                                              uint64_t where_stride, uint32_t *out_docs, float *out_scores,
-                                              uint32_t *n_redone) {
-    return sa_multi_score_batch_topk_bool_counts(m, n_nodes, node_clause_starts, clause_node, clause_field,
-                                                 clause_terms, clause_term_starts, clause_idf, clause_weight,
-                                                 clause_occur, clause_group, clause_tie, mm, n_queries, slop,
-                                                 avg_doc_len, k1, b, k, where_bits, where_n, where_stride, out_docs,
-                                                 out_scores, n_redone, 0, nullptr, nullptr, nullptr, nullptr);
-}
-
-extern "C" int sa_multi_score_batch_topk_bool_counts(
-    sa_multi *m, uint32_t n_nodes, const uint32_t *node_clause_starts, const uint32_t *clause_node,
-    const uint32_t *clause_field, const uint32_t *clause_terms, const uint32_t *clause_term_starts,
-    const float *clause_idf, const float *clause_weight, const uint8_t *clause_occur, const uint32_t *clause_group,
-    const float *clause_tie, const uint32_t *mm, uint32_t n_queries, uint32_t slop, const float *avg_doc_len,
-    const float *k1, const float *b, uint32_t k, const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
-    uint32_t *out_docs, float *out_scores, uint32_t *n_redone, uint32_t n_facets, const uint32_t *facet_field,
-    const uint32_t *facet_slot, uint32_t *out_total, uint32_t *out_facet_counts) {
-    int rc;
-    if ((rc = bool_check_multi_arrays(n_nodes, clause_node, clause_group, clause_tie, n_queries))) return rc;
-    return bool_topk_multi(m, n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
-                           clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop,
-                           avg_doc_len, k1, b, k, where_bits, where_n, where_stride, out_docs, out_scores, n_redone,
-                           n_facets, facet_field, facet_slot, out_total, out_facet_counts);
 }

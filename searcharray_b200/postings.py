@@ -190,9 +190,9 @@ class Hits(NamedTuple):
 
 
 class _Counts:
-    """The counts of one sa_score_batch_topk_bool_counts / sa_multi_score_batch_topk_bool_counts call: per facet its
-    key in Hits.facets, its field slot, its slot on that field's index and its bucket count, and the uint32 outputs
-    the call fills."""
+    """The counts of one sa_score_batch_topk_bool / sa_multi_score_batch_topk_bool call: per facet its key in
+    Hits.facets, its field slot, its slot on that field's index and its bucket count, and the uint32 outputs the call
+    fills."""
 
     def __init__(self, keys, fields, slots, n_buckets, n_queries):
         self.keys, self.n_buckets = list(keys), list(n_buckets)
@@ -201,12 +201,16 @@ class _Counts:
         self.total = np.zeros(n_queries, dtype=np.uint32)
         self.counts = np.zeros((n_queries, sum(self.n_buckets)), dtype=np.uint32)
 
-    def args(self):
-        """The trailing arguments of the _counts entry points."""
-        if not self.keys:
-            return 0, None, None, _lib.p_u32(self.total), None
-        return (len(self.keys), _lib.p_u32(self.fields), _lib.p_u32(self.slots), _lib.p_u32(self.total),
-                _lib.p_u32(self.counts))
+    @staticmethod
+    def args(counts):
+        """The trailing arguments of the boolean entry points for `counts`, a _Counts or None (out_total NULL: no
+        counting)."""
+        if counts is None:
+            return 0, None, None, None, None
+        if not counts.keys:
+            return 0, None, None, _lib.p_u32(counts.total), None
+        return (len(counts.keys), _lib.p_u32(counts.fields), _lib.p_u32(counts.slots), _lib.p_u32(counts.total),
+                _lib.p_u32(counts.counts))
 
     def hits(self):
         ends = np.cumsum(self.n_buckets)
@@ -847,23 +851,19 @@ class SearchArray(ExtensionArray):
 
     def _bool_call(self, dev, batch, terms, c_starts, idfs, similarity, slop, k, where, counts=None):
         """sa_score_batch_topk_bool on a flattened batch (query.BoolBatch; its None arrays passed as NULL select the
-        instance) and a packed mask (None: no mask): (docs, scores, queries re-run exactly).  counts: a _Counts,
-        filled by sa_score_batch_topk_bool_counts.  Call it with the lock held and the rows applied."""
+        instance) and a packed mask (None: no mask): (docs, scores, queries re-run exactly).  counts: a _Counts the
+        call fills (None: no counting).  Call it with the lock held and the rows applied."""
         docs = np.empty((batch.n_queries, k), dtype=np.uint32)
         scores = np.empty((batch.n_queries, k), dtype=np.float32)
         n_redone = ctypes.c_uint32(0)
         opt = lambda a, p: None if a is None else p(a)      # noqa: E731
         p_w, stride = _where_args(where)
-        args = (dev.handle, len(batch.node_starts) - 1, _lib.p_u32(batch.node_starts),
-                opt(batch.clause_node, _lib.p_u32), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs),
-                opt(batch.weights, _lib.p_f32), opt(batch.occurs, _lib.p_u8), opt(batch.groups, _lib.p_u32),
-                opt(batch.ties, _lib.p_f32), _lib.p_u32(batch.mm), batch.n_queries, int(slop), self.avg_doc_length,
-                similarity.k1, similarity.b, k, p_w, len(self), stride, _lib.p_u32(docs), _lib.p_f32(scores),
-                ctypes.byref(n_redone))
-        if counts is None:
-            _lib.check(_lib.lib().sa_score_batch_topk_bool(*args))
-        else:
-            _lib.check(_lib.lib().sa_score_batch_topk_bool_counts(*args, *counts.args()))
+        _lib.check(_lib.lib().sa_score_batch_topk_bool(
+            dev.handle, len(batch.node_starts) - 1, _lib.p_u32(batch.node_starts), opt(batch.clause_node, _lib.p_u32),
+            _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs), opt(batch.weights, _lib.p_f32),
+            opt(batch.occurs, _lib.p_u8), opt(batch.groups, _lib.p_u32), opt(batch.ties, _lib.p_f32),
+            _lib.p_u32(batch.mm), batch.n_queries, int(slop), self.avg_doc_length, similarity.k1, similarity.b, k, p_w,
+            len(self), stride, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone), *_Counts.args(counts)))
         return docs, scores, n_redone.value
 
     def _search_topk_bool(self, queries, k, similarity, slop, where=None, facets=None):
@@ -877,18 +877,7 @@ class SearchArray(ExtensionArray):
         clauses = batch.clauses
         feats = feature_terms(clauses, lambda i, f: self._feature_slot(f.name))
         idf = lambda dfs: compute_idf(self.corpus_size, dfs)      # noqa: E731
-        if feats:                                       # feature clauses: a reserved term id and their parameter
-            terms, c_starts, idfs = self._feature_clauses(clauses, feats, idf)
-        elif batch.clause_node is None:
-            terms, c_starts, idfs = self._topk_queries(clauses, idf)
-            idfs = np.asarray(idfs, dtype=np.float32)
-        else:                                           # nested clauses (None): no terms, idf 0
-            leaf = [i for i, c in enumerate(clauses) if c is not None]
-            terms, l_starts, l_idfs = self._topk_queries([clauses[i] for i in leaf], idf)
-            idfs, n_terms = np.zeros(len(clauses), dtype=np.float32), np.zeros(len(clauses), dtype=np.int64)
-            idfs[leaf] = l_idfs
-            n_terms[leaf] = np.diff(l_starts)
-            c_starts = np.concatenate([[0], np.cumsum(n_terms)]).astype(np.uint32)
+        terms, c_starts, idfs = self._clause_terms(clauses, feats, idf)
         if form >= DISMAX:
             check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
                                  lambda i: (similarity.k1, similarity.b, self.avg_doc_length, idfs[i]))
@@ -903,19 +892,22 @@ class SearchArray(ExtensionArray):
             out = self._bool_call(dev, batch, terms, c_starts, idfs, similarity, slop, k, where, counts)
         return out if counts is None else out + (counts.hits(),)
 
-    def _feature_clauses(self, clauses, feats, idf):
-        """(terms, clause term starts, float32 idf) of a flattened clause list holding feature clauses: a text clause
-        its term ids and idf (_topk_queries), a feature clause {index: (term id, parameter)} its reserved id and
-        parameter, a nested clause (None) no terms and 0."""
+    def _clause_terms(self, clauses, feats, idf):
+        """(terms, clause term starts, float32 idf) of a flattened clause list, as the boolean entry points take them:
+        a text clause its term ids and idf (_topk_queries), a feature clause {index: (term id, parameter)} (feats) its
+        reserved id and parameter, a nested clause (None) no terms and 0."""
         text = [i for i, c in enumerate(clauses) if c is not None and i not in feats]
         t, l_starts, l_idfs = self._topk_queries([clauses[i] for i in text], idf)
-        c_terms, idfs = [np.empty(0, dtype=np.uint32)] * len(clauses), np.zeros(len(clauses), dtype=np.float32)
-        for j, i in enumerate(text):
-            c_terms[i], idfs[i] = t[l_starts[j]:l_starts[j + 1]], l_idfs[j]
-        for i, (tid, param) in feats.items():
-            c_terms[i], idfs[i] = np.asarray([tid], dtype=np.uint32), param
-        c_starts = np.concatenate([[0], np.cumsum([len(x) for x in c_terms])]).astype(np.uint32)
-        terms = np.concatenate(c_terms).astype(np.uint32) if c_terms else np.empty(0, dtype=np.uint32)
+        f = list(feats)
+        n_terms, idfs = np.zeros(len(clauses), dtype=np.int64), np.zeros(len(clauses), dtype=np.float32)
+        n_terms[text], idfs[text] = np.diff(l_starts), l_idfs
+        n_terms[f], idfs[f] = 1, [param for _, param in feats.values()]
+        c_starts = np.concatenate([[0], np.cumsum(n_terms)]).astype(np.uint32)
+        # the text clauses' terms in order, each feature clause's reserved id at its clause's start
+        is_feature = np.zeros(int(c_starts[-1]), dtype=bool)
+        is_feature[c_starts[f]] = True
+        terms = np.empty(len(is_feature), dtype=np.uint32)
+        terms[is_feature], terms[~is_feature] = [tid for tid, _ in feats.values()], t
         return terms, c_starts, idfs
 
     def _topk_queries(self, queries, idf):

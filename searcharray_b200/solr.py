@@ -508,8 +508,7 @@ def _fields_clauses(clauses, slot_of, arrays):
 def _fields_call(multi, arrays, sims, batch, prepared, k, slop, where=None, counts=None):
     """sa_multi_score_batch_topk_bool on a flattened batch (query.BoolBatch; its None arrays passed as NULL select the
     instance) and prepared arrays (the fields locked): (docs, scores, queries re-run).  where: a packed mask
-    (postings.pack_where), None: no mask.  counts: a postings._Counts, filled by
-    sa_multi_score_batch_topk_bool_counts."""
+    (postings.pack_where), None: no mask.  counts: a postings._Counts the call fills (None: no counting)."""
     terms, c_starts, c_idf, c_field = prepared
     n_redone = ctypes.c_uint32(0)
     avgdl = _f32([a.avg_doc_length for a in arrays])
@@ -519,15 +518,12 @@ def _fields_call(multi, arrays, sims, batch, prepared, k, slop, where=None, coun
     scores = np.empty((nq, k), dtype=np.float32)
     opt = lambda a, p: None if a is None else p(a)      # noqa: E731
     p_w, stride = _where_args(where)
-    args = (multi.handle, len(batch.node_starts) - 1, _lib.p_u32(batch.node_starts), opt(batch.clause_node, _lib.p_u32),
-            _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(c_idf), _lib.p_f32(batch.weights),
-            _lib.p_u8(batch.occurs), opt(batch.groups, _lib.p_u32), opt(batch.ties, _lib.p_f32), _lib.p_u32(batch.mm),
-            nq, int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1), _lib.p_f32(b), k, p_w, len(arrays[0]), stride,
-            _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone))
-    if counts is None:
-        _lib.check(_lib.lib().sa_multi_score_batch_topk_bool(*args))
-    else:
-        _lib.check(_lib.lib().sa_multi_score_batch_topk_bool_counts(*args, *counts.args()))
+    _lib.check(_lib.lib().sa_multi_score_batch_topk_bool(
+        multi.handle, len(batch.node_starts) - 1, _lib.p_u32(batch.node_starts), opt(batch.clause_node, _lib.p_u32),
+        _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(c_idf), _lib.p_f32(batch.weights),
+        _lib.p_u8(batch.occurs), opt(batch.groups, _lib.p_u32), opt(batch.ties, _lib.p_f32), _lib.p_u32(batch.mm),
+        nq, int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1), _lib.p_f32(b), k, p_w, len(arrays[0]), stride,
+        _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone), *_Counts.args(counts)))
     return docs, scores, n_redone.value
 
 

@@ -359,7 +359,8 @@ def test_c_abi_validation(synth):
         return _lib.lib().sa_multi_score_batch_topk_bool(
             multi.handle, 1, _lib.p_u32(q_starts), None, _lib.p_u32(f), _lib.p_u32(t), _lib.p_u32(c_starts),
             _lib.p_f32(ones), _lib.p_f32(ones), _lib.p_u8(occ), None, None, _lib.p_u32(mm), 1, 0, _lib.p_f32(avgdl),
-            _lib.p_f32(kk), _lib.p_f32(bb), 10, None, 0, 0, _lib.p_u32(docs), _lib.p_f32(scores), None)
+            _lib.p_f32(kk), _lib.p_f32(bb), 10, None, 0, 0, _lib.p_u32(docs), _lib.p_f32(scores), None,
+            0, None, None, None, None)
     m, ab = _Multi([a, b]), (a.avg_doc_length, b.avg_doc_length)
     assert call(m, [0, 1], [ta["w0"], tb["b1"]], ab) == 0
     assert call(m, [0, 2], [ta["w0"], tb["b1"]], ab) != 0                 # no field slot 2
@@ -398,7 +399,7 @@ def test_c_abi_pairings(synth):
             a._device().handle, n_nodes, _lib.p_u32(n_starts), opt(node, _lib.p_u32), _lib.p_u32(terms),
             _lib.p_u32(c_starts), _lib.p_f32(ones), opt(w, _lib.p_f32), opt(o, _lib.p_u8), opt(g, _lib.p_u32),
             opt(t, _lib.p_f32), _lib.p_u32(mm), 1, 0, a.avg_doc_length, 1.2, 0.75, 10, None, 0, 0, _lib.p_u32(docs),
-            _lib.p_f32(scores), None)
+            _lib.p_f32(scores), None, 0, None, None, None, None)
     assert single(None, None, None, None, None) == 0
     assert single(ones, occ, None, None, None) == 0
     assert single(ones, occ, groups, ties, None) == 0
@@ -424,7 +425,7 @@ def test_c_abi_pairings(synth):
             mh.handle, 1, _lib.p_u32(n_starts), None, _lib.p_u32(f), _lib.p_u32(terms), _lib.p_u32(c_starts),
             _lib.p_f32(ones), opt(w, _lib.p_f32), opt(o, _lib.p_u8), opt(g, _lib.p_u32), opt(t, _lib.p_f32),
             _lib.p_u32(mm), 1, 0, _lib.p_f32(avgdl), _lib.p_f32(kk), _lib.p_f32(bb), 10, None, 0, 0,
-            _lib.p_u32(docs), _lib.p_f32(scores), None)
+            _lib.p_u32(docs), _lib.p_f32(scores), None, 0, None, None, None, None)
     mh = _Multi([a, b])
     assert multi(ones, occ) == 0
     assert multi(ones, occ, groups, ties) == 0

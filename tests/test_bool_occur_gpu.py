@@ -229,7 +229,7 @@ def test_c_abi_validation(synth):
         return _lib.lib().sa_score_batch_topk_bool(
             h, 1, _lib.p_u32(q_starts), None, _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idf), _lib.p_f32(w),
             _lib.p_u8(o), None, None, _lib.p_u32(m), 1, 0, arr.avg_doc_length, 1.2, 0.75, 10, None, 0, 0,
-            _lib.p_u32(docs), _lib.p_f32(scores), None)
+            _lib.p_u32(docs), _lib.p_f32(scores), None, 0, None, None, None, None)
     assert call([1, 1], [1, 0], 1) == 0
     assert call([1, 1], [1, 0], 2) != 0                       # one SHOULD clause
     assert call([1, 1], [1, 4], 0) != 0

@@ -331,7 +331,8 @@ def test_c_abi_rejections(synth):
         return _lib.lib().sa_score_batch_topk_bool(
             a._device().handle, len(q_starts) - 1, _lib.p_u32(q_starts), None, _lib.p_u32(terms), _lib.p_u32(c_starts),
             _lib.p_f32(idf), _lib.p_f32(idf), _lib.p_u8(o), _lib.p_u32(g), _lib.p_f32(t), _lib.p_u32(m),
-            len(q_starts) - 1, 0, a.avg_doc_length, k1, bb, 10, None, 0, 0, _lib.p_u32(docs), _lib.p_f32(scores), None)
+            len(q_starts) - 1, 0, a.avg_doc_length, k1, bb, 10, None, 0, 0, _lib.p_u32(docs), _lib.p_f32(scores), None,
+            0, None, None, None, None)
     assert single([0, 2, 4], [0, 0, 2, 2], [0.1, 0, 0.3, 0]) == 0
     assert single([0, 2, 4], [0, 1, 2, 2], [0, 0, 0, 0]) == 0               # plain clauses
     assert single([0, 4], [0, 0, 2, 2], [0.1, 0, 0.3, 0], mm=(2,)) == 0
@@ -364,7 +365,7 @@ def test_c_abi_rejections(synth):
             mh.handle, 1, _lib.p_u32(q_starts), None, _lib.p_u32(f), _lib.p_u32(t), _lib.p_u32(c_starts),
             _lib.p_f32(ones), _lib.p_f32(ones), _lib.p_u8(occ), _lib.p_u32(np.asarray(groups, dtype=np.uint32)),
             _lib.p_f32(np.asarray(ties, dtype=np.float32)), _lib.p_u32(m), 1, 0, _lib.p_f32(avgdl), _lib.p_f32(kk),
-            _lib.p_f32(bb), 10, None, 0, 0, _lib.p_u32(docs), _lib.p_f32(scores), None)
+            _lib.p_f32(bb), 10, None, 0, 0, _lib.p_u32(docs), _lib.p_f32(scores), None, 0, None, None, None, None)
     mh = _Multi([a, b])
     assert multi([0, 0], [0.3, 0]) == 0
     assert multi([0, 1], [0, 0]) == 0

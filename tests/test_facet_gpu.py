@@ -158,6 +158,48 @@ def test_four_facets_and_reset(arr):
     check(b, [Or(["w0", "s2"])], ["x"], "set again")
 
 
+def test_c_abi_count_refusals(arr):
+    """The count arguments of sa_score_batch_topk_bool, which search_topk checks before it calls: each bad one is
+    SA_ERR_ARG with its message before any device work (out_docs and out_total untouched), and the same call with
+    valid ones counts."""
+    from searcharray_b200 import _lib
+    from searcharray_b200.similarity import compute_idf
+    u32 = lambda x: np.asarray(x, dtype=np.uint32)      # noqa: E731
+    w0 = arr.host.term_dict.get_term_id("w0")
+    idf = np.asarray([compute_idf(arr.corpus_size, np.asarray([arr.docfreq("w0")]))], dtype=np.float32)
+    lang, nb = arr._facet_slot("lang")
+    dev = arr._device()
+
+    def call(fields, slots, null_counts=False):
+        docs = np.full((1, 10), 7, dtype=np.uint32)
+        scores = np.zeros((1, 10), dtype=np.float32)
+        total = np.full(1, 7, dtype=np.uint32)
+        counts = np.zeros((1, nb), dtype=np.uint32)
+        with arr._shared["lock"]:
+            dev.sync_facets(arr.host)
+            rc = _lib.lib().sa_score_batch_topk_bool(
+                dev.handle, 1, _lib.p_u32(u32([0, 1])), None, _lib.p_u32(u32([w0])), _lib.p_u32(u32([0, 1])),
+                _lib.p_f32(idf), None, None, None, None, _lib.p_u32(u32([1])), 1, 0, arr.avg_doc_length, 1.2, 0.75, 10,
+                None, 0, 0, _lib.p_u32(docs), _lib.p_f32(scores), None, len(slots), _lib.p_u32(u32(fields)),
+                _lib.p_u32(u32(slots)), _lib.p_u32(total), None if null_counts else _lib.p_u32(counts))
+        return rc, docs, total, counts
+
+    for what, kw, msg in (("5 facets", dict(fields=[0] * 5, slots=range(5)), b"at most 4 facets in one call, not 5"),
+                          ("unset slot", dict(fields=[0], slots=[7]), b"facet 0: facet slot 7 is not set"),
+                          ("field 1", dict(fields=[1], slots=[lang]), b"facet 0: field 1 out of range (1 fields)"),
+                          ("NULL out_facet_counts", dict(fields=[0], slots=[lang], null_counts=True),
+                           b"NULL argument")):
+        rc, docs, total, _ = call(**kw)
+        assert rc == 2 and msg in _lib.lib().sa_last_error(), (what, rc, _lib.lib().sa_last_error())
+        assert (docs == 7).all() and total[0] == 7, what
+    rc, docs, total, counts = call([0], [lang])
+    assert rc == 0, _lib.lib().sa_last_error()
+    dense = arr.score("w0")
+    codes = arr.host.facets["lang"][0]
+    assert total[0] == np.count_nonzero(dense) > 0
+    assert np.array_equal(counts[0], np.bincount(codes[(dense > 0) & (codes >= 0)], minlength=nb))
+
+
 def test_shard_doc_base():
     from searcharray_b200 import And, Or, SearchArray
     base = 1_000_003

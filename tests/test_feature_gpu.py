@@ -254,7 +254,8 @@ def _c_call(arr, clauses, starts, terms, term_starts, idf, weights=None, occurs=
         rc = _lib.lib().sa_score_batch_topk_bool(
             dev.handle, nq, _lib.p_u32(starts), None, _lib.p_u32(terms), _lib.p_u32(term_starts), _lib.p_f32(idf),
             opt(w, _lib.p_f32), opt(o, _lib.p_u8), opt(g, _lib.p_u32), opt(t, _lib.p_f32), _lib.p_u32(mm), nq, 0,
-            arr.avg_doc_length, 1.2, 0.75, k, None, 0, 0, _lib.p_u32(docs), _lib.p_f32(scores), None)
+            arr.avg_doc_length, 1.2, 0.75, k, None, 0, 0, _lib.p_u32(docs), _lib.p_f32(scores), None,
+            0, None, None, None, None)
     return rc, docs, scores
 
 

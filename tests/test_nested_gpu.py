@@ -305,7 +305,7 @@ def test_c_abi_rejections(synth):
             a._device().handle, len(n_starts) - 1, _lib.p_u32(n_starts), _lib.p_u32(np.asarray(c_node, dtype=np.uint32)),
             _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(ones), _lib.p_f32(ones), _lib.p_u8(occ), _lib.p_u32(g),
             _lib.p_f32(t), _lib.p_u32(m), nq, 0, a.avg_doc_length, 1.2, 0.75, 10, None, 0, 0, _lib.p_u32(docs),
-            _lib.p_f32(scores), None)
+            _lib.p_f32(scores), None, 0, None, None, None, None)
     # query 0 = Or(w0, node 1); node 1 = Or(w1, s1)
     assert call([0, 2, 4], [X, 1, X, X], [["w0"], [], ["w1"], ["s1"]]) == 0
     assert call([0, 2, 4], [X, 2, X, X], [["w0"], [], ["w1"], ["s1"]]) != 0          # out of range

@@ -14,7 +14,7 @@ stratified terms), timed alternating in one run:
   term          a                               plain terms through the term scan
   term_total    a, facets=[]                    plain terms through the one-clause Or fold, totals only
 Per workload: qps (the public call, host clock around the synchronous call, median of --reps), c_call_qps for the
-Or workloads (sa_score_batch_topk_bool / sa_score_batch_topk_bool_counts on arrays prepared once), n_redone, and
+Or workloads (sa_score_batch_topk_bool, with or without counts, on arrays prepared once), n_redone, and
 verified: sampled queries whose total and facet rows equal numpy's count over the composed dense vector.  The card
 name and power limit come from a read-only nvidia-smi query in the same run.  Prints one JSON line.
 """

@@ -103,7 +103,7 @@ def main():
         """The C call of search_topk(queries) on arrays prepared once: fn() -> n_redone."""
         batch = flatten_bool(queries, max(map(bool_form, queries)))
         feats = feature_terms(batch.clauses, lambda i, f: arr._feature_slot(f.name))
-        terms, c_starts, idfs = arr._feature_clauses(batch.clauses, feats, lambda x: compute_idf(arr.corpus_size, x))
+        terms, c_starts, idfs = arr._clause_terms(batch.clauses, feats, lambda x: compute_idf(arr.corpus_size, x))
         dev = arr._device()
         dev.sync_features(arr.host)
         w = None if bits is None else pack_where(bits, n, len(queries))
