@@ -178,7 +178,7 @@ def _where_args(bits):
 
 def _where_part(bits, sel):
     """The packed mask of the queries `sel` selects (a one-row mask is every query's)."""
-    return bits if bits is None or bits.shape[0] == 1 else np.ascontiguousarray(bits[sel])
+    return bits if bits is None or bits.shape[0] == 1 or sel.all() else np.ascontiguousarray(bits[sel])
 
 
 class Hits(NamedTuple):
@@ -194,10 +194,12 @@ class _Counts:
     Hits.facets, its field slot, its slot on that field's index and its bucket count, and the uint32 outputs the call
     fills."""
 
-    def __init__(self, keys, fields, slots, n_buckets, n_queries):
-        self.keys, self.n_buckets = list(keys), list(n_buckets)
-        self.fields = np.asarray(fields, dtype=np.uint32)
-        self.slots = np.asarray(slots, dtype=np.uint32)
+    def __init__(self, facets, arrays, n_queries):
+        """facets: (key, field slot, name) triples, the name set on arrays[field slot] (ValueError otherwise)."""
+        found = [arrays[field]._facet_slot(name) for _, field, name in facets]
+        self.keys, self.n_buckets = [key for key, _, _ in facets], [nb for _, nb in found]
+        self.fields = np.asarray([field for _, field, _ in facets], dtype=np.uint32)
+        self.slots = np.asarray([slot for slot, _ in found], dtype=np.uint32)
         self.total = np.zeros(n_queries, dtype=np.uint32)
         self.counts = np.zeros((n_queries, sum(self.n_buckets)), dtype=np.uint32)
 
@@ -229,6 +231,100 @@ def check_facet_keys(facets, what):
     if len(set(facets)) != len(facets):
         raise ValueError(f"facets are named once each: {facets}")
     return facets
+
+
+def _check_dismax(members, clauses, clause_slot, arrays, sims, idfs=None):
+    """ValueError unless the DisMax members (indices into clauses) are sparse-safe (query.check_dismax_members) under
+    the k1, b and avgdl of their slot (clause_slot[i]: an index into arrays and sims) and their float32 idf.  idfs=None:
+    the check before any device work, with idf 0, of the parameters alone."""
+    from .query import check_dismax_members
+
+    def params(i):
+        s = clause_slot[i]
+        return sims[s].k1, sims[s].b, arrays[s].avg_doc_length, 0.0 if idfs is None else idfs[i]
+    check_dismax_members([(i, clauses[i]) for i in members], params)
+
+
+class _PreparedBool:
+    """One call of sa_score_batch_topk_bool over one SearchArray, or of sa_multi_score_batch_topk_bool over the columns
+    of a solr.fields_topk plan, prepared from a flattened batch (query.BoolBatch): each clause's term ids, term starts
+    and float32 idf from its own column, as that column's .score takes them, the feature columns its clauses read and
+    the counts it fills.  Build it and run it with the arrays' locks held (the array's lock; solr._locked for a
+    multi)."""
+
+    def __init__(self, arrays, sims, clause_slot, queries, batch, where=None, facets=None, multi=None):
+        """arrays, sims: per slot its SearchArray and similarity (one array: one slot).  clause_slot: uint32 per clause
+        of batch, its slot (0 for a nested clause).  batch: queries flattened (query.flatten_bool).  where: a packed
+        mask (pack_where), None: no mask.  facets: (key in Hits.facets, slot, name) triples, None: no counting.
+        multi: the solr._Multi over arrays for fields_topk, None for one array.  A facet or feature name not set on its
+        slot's array, and DisMax members whose idf is not sparse-safe, are ValueErrors, the names checked before any
+        device work."""
+        from .query import Field, dismax_members
+        self.arrays, self.batch, self.where = arrays, batch, where
+        self.counts = None if facets is None else _Counts(facets, arrays, batch.n_queries)
+        clauses = batch.clauses
+        feats = self.features(clauses, clause_slot, arrays)
+        text = np.asarray([i for i, c in enumerate(clauses) if c is not None and i not in feats], dtype=np.int64)
+        n_terms, self.idfs = np.zeros(len(clauses), dtype=np.int64), np.zeros(len(clauses), dtype=np.float32)
+        slot_terms = []
+        for s, arr in enumerate(arrays):
+            idx = text[clause_slot[text] == s]
+            t, starts, idf = arr._topk_queries([clauses[i].clause if isinstance(clauses[i], Field) else clauses[i]
+                                                for i in idx.tolist()],
+                                               lambda dfs, arr=arr: compute_idf(arr.corpus_size, dfs))
+            n_terms[idx], self.idfs[idx] = np.diff(starts), idf
+            slot_terms.append((idx, t, starts))
+        f = list(feats)
+        n_terms[f], self.idfs[f] = 1, [param for _, param in feats.values()]
+        self.c_starts = np.concatenate([[0], np.cumsum(n_terms)]).astype(np.uint32)
+        # each slot's text clauses' terms from their clause's start on, each feature clause's reserved id at its start
+        self.terms = np.empty(int(self.c_starts[-1]), dtype=np.uint32)
+        for idx, t, starts in slot_terms:
+            first = self.c_starts[idx].astype(np.int64) - starts[:-1]
+            self.terms[np.repeat(first, np.diff(starts)) + np.arange(len(t))] = t
+        self.terms[self.c_starts[f]] = [tid for tid, _ in feats.values()]
+        if batch.groups is not None:
+            _check_dismax(dismax_members(queries), clauses, clause_slot, arrays, sims, self.idfs)
+        for s in {int(clause_slot[i]) for i in feats}:
+            arrays[s]._device().sync_features(arrays[s].host)
+        if self.counts is not None:
+            for s in set(self.counts.fields.tolist()):
+                arrays[s]._device().sync_facets(arrays[s].host)
+        for arr in arrays:          # a sliced view of the same column may have left its row filter installed
+            arr._apply_rows(arr._device())
+        if multi is None:
+            self.entry, self.handle = _lib.lib().sa_score_batch_topk_bool, arrays[0]._device().handle
+            self.c_field, self.bm25 = (), (arrays[0].avg_doc_length, sims[0].k1, sims[0].b)
+        else:               # the clause slots, and avgdl, k1 and b per slot (a pointer keeps its array alive)
+            self.entry, self.handle = _lib.lib().sa_multi_score_batch_topk_bool, multi.handle
+            self.c_field = (_lib.p_u32(clause_slot),)
+            self.bm25 = tuple(_lib.p_f32(np.asarray(v, dtype=np.float32)) for v in
+                              ([a.avg_doc_length for a in arrays], [s.k1 for s in sims], [s.b for s in sims]))
+
+    @staticmethod
+    def features(clauses, clause_slot, arrays):
+        """The feature clauses as query.feature_terms encodes them, each on its slot's index: {index: (reserved term
+        id, float32 parameter)}; ValueError for a name not set there."""
+        from .query import feature_terms
+        return feature_terms(clauses, lambda i, f: arrays[clause_slot[i]]._feature_slot(f.name))
+
+    def run(self, k, slop):
+        """Makes the call: (docs uint32[Q, k], scores float32[Q, k], queries re-run exactly), and the Hits when
+        counting.  The batch's None arrays are passed as NULL, which selects the instance."""
+        b = self.batch
+        docs = np.empty((b.n_queries, k), dtype=np.uint32)
+        scores = np.empty((b.n_queries, k), dtype=np.float32)
+        n_redone = ctypes.c_uint32(0)
+        opt = lambda a, p: None if a is None else p(a)      # noqa: E731
+        p_w, stride = _where_args(self.where)
+        _lib.check(self.entry(
+            self.handle, len(b.node_starts) - 1, _lib.p_u32(b.node_starts), opt(b.clause_node, _lib.p_u32),
+            *self.c_field, _lib.p_u32(self.terms), _lib.p_u32(self.c_starts), _lib.p_f32(self.idfs),
+            opt(b.weights, _lib.p_f32), opt(b.occurs, _lib.p_u8), opt(b.groups, _lib.p_u32), opt(b.ties, _lib.p_f32),
+            _lib.p_u32(b.mm), b.n_queries, int(slop), *self.bm25, k, p_w, len(self.arrays[0]), stride,
+            _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone), *_Counts.args(self.counts)))
+        out = docs, scores, n_redone.value
+        return out if self.counts is None else out + (self.counts.hits(),)
 
 
 class DeviceIndex:
@@ -664,11 +760,6 @@ class SearchArray(ExtensionArray):
             raise ValueError(f"facet {name!r} is not set on this array (set_facet); set: {names}")
         return names.index(name), self.host.facets[name][1]
 
-    def _counts(self, facets, n_queries):
-        """The _Counts of facet names `facets` (checked: check_facet_keys, _facet_slot) for n_queries queries."""
-        slots = [self._facet_slot(f) for f in facets]
-        return _Counts(facets, [0] * len(facets), [s for s, _ in slots], [nb for _, nb in slots], n_queries)
-
     def _feature_slot(self, name):
         """The slot of feature `name` on this array's index; ValueError if it is not set."""
         names = list(self.host.features)
@@ -735,25 +826,62 @@ class SearchArray(ExtensionArray):
         bm25_similarity (TypeError), and for a name not set, a name given twice or more than 4 names (ValueError),
         the call is refused before any device work.  On a shard the counts are the shard's own docs.  facets=None
         (the default) returns (docs, scores) as above."""
-        from .query import Feature, is_boolean
+        from .query import DISMAX, NESTED, OCCUR, OR_AND, Feature, bool_form, has_dismax, has_field, is_boolean
         queries = list(queries)
         for q in queries:
             if isinstance(q, Feature):
                 raise TypeError(f"a Feature is a clause, not a query: write Bool(should=[{q!r}])")
         if facets is not None:
             facets = check_facet_keys(facets, "facet names")
-            bits = None if where is None else pack_where(where, len(self), len(queries))
-            return self._search_topk_mixed(queries, k, similarity, slop, bits, facets)
-        if where is not None:
-            bits = pack_where(where, len(self), len(queries))
-            if any(is_boolean(q) for q in queries):
-                return self._search_topk_mixed(queries, k, similarity, slop, bits)
-            return self._search_topk_plain_where(queries, k, similarity, slop, bits)
-        if any(is_boolean(q) for q in queries):
-            return self._search_topk_mixed(list(queries), k, similarity, slop)
-        self._check_topk_similarity(similarity)
-        if self.rows is not None or not isinstance(similarity, Bm25Similarity):
-            return self._search_topk_sim(queries, k, similarity, slop)
+        bits = None if where is None else pack_where(where, len(self), len(queries))
+        kind = np.asarray([bool_form(q) if is_boolean(q) else 0 for q in queries])     # 0: plain
+        if facets is None and not kind.any():
+            self._check_topk_similarity(similarity)
+            if self.rows is not None or not isinstance(similarity, Bm25Similarity):
+                return self._search_topk_sim(queries, k, similarity, slop, bits)
+            if bits is None:
+                return self._search_topk_plain(queries, k, similarity, slop)
+        else:                       # the boolean path's refusals
+            if any(has_field(q) for q in queries if is_boolean(q)):
+                raise ValueError("a Field clause names a DataFrame column: run queries over columns with "
+                                 "solr.fields_topk(frame, queries), not SearchArray.search_topk")
+            if self.rows is not None:
+                raise NotImplementedError("boolean queries on a view (arr[mask]) are not supported yet; "
+                                          "compose .score() on the view")
+            if not isinstance(similarity, Bm25Similarity):
+                raise TypeError(f"boolean queries support bm25_similarity only, not {similarity!r}")
+        hits = None if facets is None else Hits(np.zeros(len(queries), dtype=np.int64), {
+            f: np.zeros((len(queries), self._facet_slot(f)[1]), dtype=np.int64) for f in facets})
+        if any(has_dismax(q) for q, kd in zip(queries, kind) if kd >= DISMAX):      # k1 / b before any device work
+            _check_dismax([0], ["DisMax member"], [0], [self], [similarity])
+        # one call per form present, so that each runs the lightest instance that scores it; results in query order
+        docs = np.empty((len(queries), k), dtype=np.uint32)
+        scores = np.empty((len(queries), k), dtype=np.float32)
+        for kd in (0, OR_AND, OCCUR, DISMAX, NESTED):
+            sel = kind == kd
+            if not sel.any():
+                continue
+            part = [q for q, s in zip(queries, sel) if s]
+            if kd == 0 and bits is None and facets is None:
+                docs[sel], scores[sel] = self._search_topk_plain(part, k, similarity, slop)
+                continue
+            out = self._search_topk_bool(part, k, similarity, slop, _where_part(bits, sel), facets)
+            docs[sel], scores[sel] = out[:2]
+            if hits is not None:
+                hits.total[sel] = out[3].total
+                for f in facets:
+                    hits.facets[f][sel] = out[3].facets[f]
+        return (docs, scores) if hits is None else (docs, scores, hits)
+
+    @staticmethod
+    def _check_topk_similarity(similarity):
+        if not isinstance(similarity, (Bm25Similarity, Bm25Impact, Bm25Legacy, ClassicSimilarity)):
+            raise TypeError("search_topk supports bm25_similarity, bm25_impact, bm25_legacy_similarity and "
+                            f"classic_similarity, not {similarity!r}")
+
+    def _search_topk_plain(self, queries, k, similarity, slop):
+        """search_topk of plain queries under BM25 on the whole array, without a mask or counts: the term scan of
+        sa_score_batch_topk."""
         terms, starts, idfs = self._topk_queries(queries, lambda dfs: compute_idf(self.corpus_size, dfs))
         idfs = np.asarray(idfs, dtype=np.float32)
         docs = np.empty((len(idfs), k), dtype=np.uint32)
@@ -766,149 +894,21 @@ class SearchArray(ExtensionArray):
                                                       _lib.p_u32(docs), _lib.p_f32(scores)))
         return docs, scores
 
-    @staticmethod
-    def _check_topk_similarity(similarity):
-        if not isinstance(similarity, (Bm25Similarity, Bm25Impact, Bm25Legacy, ClassicSimilarity)):
-            raise TypeError("search_topk supports bm25_similarity, bm25_impact, bm25_legacy_similarity and "
-                            f"classic_similarity, not {similarity!r}")
-
-    def _search_topk_plain_where(self, queries, k, similarity, slop, where, facets=None):
-        """search_topk of plain queries with a packed mask (pack_where): on a view or under a non-BM25 similarity
-        through sa_score_batch_topk_sim, else each query as a one-clause Or through the boolean fold, which
-        scores a clause exactly as .score(c, slop=slop).  The clauses are taken as the unmasked batch takes its
-        queries (_topk_queries: a str is a term, any other iterable of str a phrase), and the C call checks their
-        term counts as the unmasked one does.  facets: names (checked by the caller) whose counts come back as a third
-        value, a Hits."""
-        self._check_topk_similarity(similarity)
-        if self.rows is not None or not isinstance(similarity, Bm25Similarity):
-            return self._search_topk_sim(queries, k, similarity, slop, where)
-        from .query import BoolBatch
-        n = len(queries)
-        dev = self._device()
-        with self._shared["lock"]:
-            self._apply_rows(dev)
-            terms, c_starts, idfs = self._topk_queries(queries, lambda dfs: compute_idf(self.corpus_size, dfs))
-            # query q: clause q, mm 1
-            batch = BoolBatch(queries, np.arange(n + 1, dtype=np.uint32), None, np.ones(n, dtype=np.uint32), None,
-                              None, None, None, n)
-            counts = None if facets is None else self._counts(facets, n)
-            if counts is not None:
-                dev.sync_facets(self.host)
-            docs, scores, _ = self._bool_call(dev, batch, terms, c_starts, np.asarray(idfs, dtype=np.float32),
-                                              similarity, slop, k, where, counts)
-        return (docs, scores) if counts is None else (docs, scores, counts.hits())
-
-    def _search_topk_mixed(self, queries, k, similarity, slop, where=None, facets=None):
-        """search_topk of a batch holding boolean queries: the plain ones through search_topk as before, the boolean
-        ones in one _search_topk_bool call per form present (query.bool_form), so that each runs the lightest
-        instance that scores it, each clause with the idf .score gives it; results in query order.  where: a packed
-        mask (pack_where), its rows split with the queries.  facets: facet names (check_facet_keys): every query, plain
-        ones included, runs through the boolean fold and (docs, scores, hits) comes back, the counts in query
-        order."""
-        from .query import DISMAX, NESTED, OCCUR, OR_AND, bool_form, has_dismax, has_field, is_boolean
-        if any(has_field(q) for q in queries if is_boolean(q)):
-            raise ValueError("a Field clause names a DataFrame column: run queries over columns with "
-                             "solr.fields_topk(frame, queries), not SearchArray.search_topk")
-        if self.rows is not None:
-            raise NotImplementedError("boolean queries on a view (arr[mask]) are not supported yet; "
-                                      "compose .score() on the view")
-        if not isinstance(similarity, Bm25Similarity):
-            raise TypeError(f"boolean queries support bm25_similarity only, not {similarity!r}")
-        counted = facets is not None
-        if counted:
-            hits = self._counts(facets, len(queries)).hits()      # the names checked, and zero counts
-        kind = np.asarray([bool_form(q) if is_boolean(q) else 0 for q in queries])     # 0: plain
-        if any(has_dismax(q) for q, kd in zip(queries, kind) if kd >= DISMAX):
-            self._check_dismax_params(similarity)
-        docs = np.empty((len(queries), k), dtype=np.uint32)
-        scores = np.empty((len(queries), k), dtype=np.float32)
-        for kd in (0, OR_AND, OCCUR, DISMAX, NESTED):
-            sel = kind == kd
-            part = [q for q, s in zip(queries, sel) if s]
-            if not part:
-                continue
-            w = _where_part(where, sel)
-            if counted:
-                if kd == 0:
-                    docs[sel], scores[sel], h = self._search_topk_plain_where(part, k, similarity, slop, w, facets)
-                else:
-                    docs[sel], scores[sel], _, h = self._search_topk_bool(part, k, similarity, slop, w, facets)
-                hits.total[sel] = h.total
-                for name in facets:
-                    hits.facets[name][sel] = h.facets[name]
-            elif kd == 0 and where is not None:
-                docs[sel], scores[sel] = self._search_topk_plain_where(part, k, similarity, slop, w)
-            elif kd == 0:
-                docs[sel], scores[sel] = self.search_topk(part, k=k, similarity=similarity, slop=slop)
-            else:
-                docs[sel], scores[sel], _ = self._search_topk_bool(part, k, similarity, slop, w)
-        return (docs, scores, hits) if counted else (docs, scores)
-
-    def _check_dismax_params(self, similarity):
-        """ValueError, before any device work, where DisMax members would not be sparse-safe for k1 / b."""
-        from .query import check_dismax_members
-        check_dismax_members([(0, "DisMax member")], lambda i: (similarity.k1, similarity.b, self.avg_doc_length, 0.0))
-
-    def _bool_call(self, dev, batch, terms, c_starts, idfs, similarity, slop, k, where, counts=None):
-        """sa_score_batch_topk_bool on a flattened batch (query.BoolBatch; its None arrays passed as NULL select the
-        instance) and a packed mask (None: no mask): (docs, scores, queries re-run exactly).  counts: a _Counts the
-        call fills (None: no counting).  Call it with the lock held and the rows applied."""
-        docs = np.empty((batch.n_queries, k), dtype=np.uint32)
-        scores = np.empty((batch.n_queries, k), dtype=np.float32)
-        n_redone = ctypes.c_uint32(0)
-        opt = lambda a, p: None if a is None else p(a)      # noqa: E731
-        p_w, stride = _where_args(where)
-        _lib.check(_lib.lib().sa_score_batch_topk_bool(
-            dev.handle, len(batch.node_starts) - 1, _lib.p_u32(batch.node_starts), opt(batch.clause_node, _lib.p_u32),
-            _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(idfs), opt(batch.weights, _lib.p_f32),
-            opt(batch.occurs, _lib.p_u8), opt(batch.groups, _lib.p_u32), opt(batch.ties, _lib.p_f32),
-            _lib.p_u32(batch.mm), batch.n_queries, int(slop), self.avg_doc_length, similarity.k1, similarity.b, k, p_w,
-            len(self), stride, _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone), *_Counts.args(counts)))
-        return docs, scores, n_redone.value
+    def _prepare_bool(self, queries, similarity, where=None, facets=None):
+        """Boolean queries of any forms, or plain ones (a batch of their own) as one-clause Or nodes, which score
+        exactly as .score(q, slop=slop), as one sa_score_batch_topk_bool call flattened for the heaviest form among
+        them (query.bool_form, flatten_bool): a _PreparedBool.  where: a packed mask (pack_where).  facets: facet names
+        (check_facet_keys) whose Hits the call returns.  Call it, and run the call, with the lock held."""
+        from .query import OR_AND, bool_form, flatten_bool, is_boolean
+        batch = flatten_bool(queries, max((bool_form(q) for q in queries if is_boolean(q)), default=OR_AND))
+        return _PreparedBool([self], [similarity], np.zeros(len(batch.clauses), dtype=np.uint32), queries, batch,
+                             where, None if facets is None else [(f, 0, f) for f in facets])
 
     def _search_topk_bool(self, queries, k, similarity, slop, where=None, facets=None):
-        """Boolean queries of any form through sa_score_batch_topk_bool, flattened for the heaviest form among them
-        (query.bool_form, flatten_bool): (docs, scores, queries re-run exactly).  DisMax members anywhere in the trees
-        need sparse-safe BM25 parameters (ValueError before any device work).  where: a packed mask (pack_where).
-        facets: facet names (check_facet_keys) whose counts come back as a fourth value, a Hits."""
-        from .query import DISMAX, OR_AND, bool_form, check_dismax_members, dismax_members, feature_terms, flatten_bool
-        form = max(map(bool_form, queries), default=OR_AND)
-        batch = flatten_bool(queries, form)
-        clauses = batch.clauses
-        feats = feature_terms(clauses, lambda i, f: self._feature_slot(f.name))
-        idf = lambda dfs: compute_idf(self.corpus_size, dfs)      # noqa: E731
-        terms, c_starts, idfs = self._clause_terms(clauses, feats, idf)
-        if form >= DISMAX:
-            check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
-                                 lambda i: (similarity.k1, similarity.b, self.avg_doc_length, idfs[i]))
-        counts = None if facets is None else self._counts(facets, batch.n_queries)
-        dev = self._device()
+        """_prepare_bool's call, made with the lock held: (docs, scores, queries re-run exactly), and the Hits with
+        facets."""
         with self._shared["lock"]:
-            self._apply_rows(dev)
-            if feats:
-                dev.sync_features(self.host)
-            if counts is not None:
-                dev.sync_facets(self.host)
-            out = self._bool_call(dev, batch, terms, c_starts, idfs, similarity, slop, k, where, counts)
-        return out if counts is None else out + (counts.hits(),)
-
-    def _clause_terms(self, clauses, feats, idf):
-        """(terms, clause term starts, float32 idf) of a flattened clause list, as the boolean entry points take them:
-        a text clause its term ids and idf (_topk_queries), a feature clause {index: (term id, parameter)} (feats) its
-        reserved id and parameter, a nested clause (None) no terms and 0."""
-        text = [i for i, c in enumerate(clauses) if c is not None and i not in feats]
-        t, l_starts, l_idfs = self._topk_queries([clauses[i] for i in text], idf)
-        f = list(feats)
-        n_terms, idfs = np.zeros(len(clauses), dtype=np.int64), np.zeros(len(clauses), dtype=np.float32)
-        n_terms[text], idfs[text] = np.diff(l_starts), l_idfs
-        n_terms[f], idfs[f] = 1, [param for _, param in feats.values()]
-        c_starts = np.concatenate([[0], np.cumsum(n_terms)]).astype(np.uint32)
-        # the text clauses' terms in order, each feature clause's reserved id at its clause's start
-        is_feature = np.zeros(int(c_starts[-1]), dtype=bool)
-        is_feature[c_starts[f]] = True
-        terms = np.empty(len(is_feature), dtype=np.uint32)
-        terms[is_feature], terms[~is_feature] = [tid for tid, _ in feats.values()], t
-        return terms, c_starts, idfs
+            return self._prepare_bool(queries, similarity, where, facets).run(k, slop)
 
     def _topk_queries(self, queries, idf):
         """The queries as the batched top-k entries take them: term ids, start offsets and, per query, idf(dfs) of

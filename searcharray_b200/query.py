@@ -455,7 +455,8 @@ def flatten_bool(queries, form):
     """Boolean queries as sa_score_batch_topk_bool takes them, for a form at least that of every query (bool_form):
     a BoolBatch with only the arrays `form` reads, so a lighter form neither builds nor passes the others.
 
-    OR_AND: Or / And queries; clauses, node_starts (one node per query) and mm.  OCCUR adds per clause float32 weights
+    OR_AND: Or / And queries, and plain ones (search_topk's terms and phrases) as one-clause nodes with mm 1; clauses,
+    node_starts (one node per query) and mm.  OCCUR adds per clause float32 weights
     and uint8 SA_OCCUR_* roles: an Or's clauses all SHOULD, a Bool's as must, should, filter, must_not.  DISMAX expands
     each DisMax into its members (their own weights, the DisMax's role) and adds per clause groups and ties; a top-level
     DisMax is Bool(should=[it]).  NESTED adds the nested queries as nodes after the queries, each query's in pre-order
@@ -466,9 +467,13 @@ def flatten_bool(queries, form):
     clauses, starts, mm = [], [0], []
     if form == OR_AND:
         for q in queries:
-            clauses.extend(q.clauses)
+            if isinstance(q, Or):
+                clauses.extend(q.clauses)
+                mm.append(q.mm)
+            else:
+                clauses.append(q)
+                mm.append(1)
             starts.append(len(clauses))
-            mm.append(q.mm)
         return BoolBatch(clauses, _u32(starts), None, _u32(mm), None, None, None, None, len(queries))
     nodes, children = _nodes(queries) if form == NESTED else (queries, None)
     weights, occurs, cnode, groups, ties = [], [], [], [], []

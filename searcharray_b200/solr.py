@@ -19,7 +19,7 @@ import numpy as np
 import pandas as pd
 
 from . import _lib
-from .postings import SearchArray, _Counts, _where_args, check_facet_keys, pack_where
+from .postings import SearchArray, _check_dismax, _PreparedBool, check_facet_keys, pack_where
 from .similarity import Bm25Similarity, Similarity, compute_idf, default_bm25
 
 
@@ -421,7 +421,7 @@ def _fields_plan(frame, queries, similarity, extra=()):
     OCCUR since the multi-field entry takes weights and roles (query.flatten_bool), field name -> slot, per-slot
     arrays, per-slot similarities).  extra: columns the call reads that no clause may name (facet columns), given
     slots after the clauses' fields."""
-    from .query import ED_MAX_FIELDS, OCCUR, Field, bool_form, flatten_bool, is_boolean
+    from .query import ED_MAX_FIELDS, OCCUR, Field, bool_form, dismax_members, flatten_bool, is_boolean
     queries = list(queries)
     for q in queries:
         if not is_boolean(q):
@@ -467,64 +467,16 @@ def _fields_plan(frame, queries, similarity, extra=()):
         slot_arrays.append(a)
         slot_sims.append(sim)
         slot_name.append(f)
-    if batch.groups is not None:          # DisMax members: sparse-safe k1 / b on their fields (idf: _fields_clauses)
-        from .query import check_dismax_members, dismax_members
-        clauses = batch.clauses
-        check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
-                             lambda i: (sims[clauses[i].field].k1, sims[clauses[i].field].b,
-                                        arrays[clauses[i].field].avg_doc_length, 0.0))
-    _feature_terms(batch.clauses, slot_of, slot_arrays)       # feature names set on their columns
+    clause_slot = _clause_slots(batch, slot_of)
+    if batch.groups is not None:          # DisMax members: sparse-safe k1 / b on their fields
+        _check_dismax(dismax_members(queries), batch.clauses, clause_slot, slot_arrays, slot_sims)
+    _PreparedBool.features(batch.clauses, clause_slot, slot_arrays)      # feature names set on their columns
     return batch, slot_of, slot_arrays, slot_sims
 
 
-def _feature_terms(clauses, slot_of, arrays):
-    """Field(column, Feature) clauses as query.feature_terms encodes them, each on its column's index."""
-    from .query import feature_terms
-    return feature_terms(clauses, lambda i, f: arrays[slot_of[clauses[i].field]]._feature_slot(f.name))
-
-
-def _fields_clauses(clauses, slot_of, arrays):
-    """Each clause's term ids and idf from its own field, as that column's .score takes them: (terms, clause term
-    starts, float32 idf, field slots).  A nested clause (None) has no terms, idf 0 and slot 0; a feature clause its
-    reserved term id and its parameter.  Call it with the fields locked (_locked)."""
-    c_terms, c_idf = [[]] * len(clauses), np.zeros(len(clauses), dtype=np.float32)
-    feats = _feature_terms(clauses, slot_of, arrays)
-    for i, (tid, param) in feats.items():         # a feature clause: its reserved term id and parameter
-        c_terms[i], c_idf[i] = _u32([tid]), param
-    for s, arr in enumerate(arrays):
-        if any(slot_of[clauses[i].field] == s for i in feats):
-            arr._device().sync_features(arr.host)
-        idx = [i for i, c in enumerate(clauses) if c is not None and i not in feats and slot_of[c.field] == s]
-        t, st, idf = arr._topk_queries([clauses[i].clause for i in idx],
-                                       lambda dfs, arr=arr: compute_idf(arr.corpus_size, dfs))
-        for j, i in enumerate(idx):
-            c_terms[i] = t[st[j]:st[j + 1]]
-            c_idf[i] = idf[j]
-    c_starts = _u32(np.cumsum([0] + [len(t) for t in c_terms]))
-    terms = _u32(np.concatenate(c_terms) if c_terms else [])
-    return terms, c_starts, c_idf, _u32([0 if c is None else slot_of[c.field] for c in clauses])
-
-
-def _fields_call(multi, arrays, sims, batch, prepared, k, slop, where=None, counts=None):
-    """sa_multi_score_batch_topk_bool on a flattened batch (query.BoolBatch; its None arrays passed as NULL select the
-    instance) and prepared arrays (the fields locked): (docs, scores, queries re-run).  where: a packed mask
-    (postings.pack_where), None: no mask.  counts: a postings._Counts the call fills (None: no counting)."""
-    terms, c_starts, c_idf, c_field = prepared
-    n_redone = ctypes.c_uint32(0)
-    avgdl = _f32([a.avg_doc_length for a in arrays])
-    k1, b = _f32([s.k1 for s in sims]), _f32([s.b for s in sims])
-    nq = batch.n_queries
-    docs = np.empty((nq, k), dtype=np.uint32)
-    scores = np.empty((nq, k), dtype=np.float32)
-    opt = lambda a, p: None if a is None else p(a)      # noqa: E731
-    p_w, stride = _where_args(where)
-    _lib.check(_lib.lib().sa_multi_score_batch_topk_bool(
-        multi.handle, len(batch.node_starts) - 1, _lib.p_u32(batch.node_starts), opt(batch.clause_node, _lib.p_u32),
-        _lib.p_u32(c_field), _lib.p_u32(terms), _lib.p_u32(c_starts), _lib.p_f32(c_idf), _lib.p_f32(batch.weights),
-        _lib.p_u8(batch.occurs), opt(batch.groups, _lib.p_u32), opt(batch.ties, _lib.p_f32), _lib.p_u32(batch.mm),
-        nq, int(slop), _lib.p_f32(avgdl), _lib.p_f32(k1), _lib.p_f32(b), k, p_w, len(arrays[0]), stride,
-        _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone), *_Counts.args(counts)))
-    return docs, scores, n_redone.value
+def _clause_slots(batch, slot_of):
+    """uint32 per clause of a fields_topk batch: the slot of its field (_fields_plan), 0 for a nested clause."""
+    return _u32([0 if c is None else slot_of[c.field] for c in batch.clauses])
 
 
 def _facet_pairs(frame, facets):
@@ -548,27 +500,10 @@ def _fields_topk(frame, queries, k, similarity, slop, where=None, facets=None):
         facets = _facet_pairs(frame, facets)
     batch, slot_of, arrays, sims = _fields_plan(frame, queries, similarity,
                                                 extra=[] if facets is None else [c for c, _ in facets])
-    counts = None
-    if facets is not None:
-        slots = [arrays[slot_of[c]]._facet_slot(name) for c, name in facets]
-        counts = _Counts(facets, [slot_of[c] for c, _ in facets], [s for s, _ in slots], [nb for _, nb in slots],
-                         len(queries))
     multi = _multi_for(arrays)
     with _locked(multi, arrays):
-        for arr in arrays:                 # a sliced view of the same column may have left its row filter installed
-            arr._apply_rows(arr._device())
-        if counts is not None:
-            for s in set(counts.fields.tolist()):
-                arrays[s]._device().sync_facets(arrays[s].host)
-        prepared = _fields_clauses(batch.clauses, slot_of, arrays)
-        if batch.groups is not None:      # DisMax members: sparse-safe idf from their own fields
-            from .query import check_dismax_members, dismax_members
-            clauses = batch.clauses
-            check_dismax_members([(i, clauses[i]) for i in dismax_members(queries)],
-                                 lambda i: (sims[slot_of[clauses[i].field]].k1, sims[slot_of[clauses[i].field]].b,
-                                            arrays[slot_of[clauses[i].field]].avg_doc_length, prepared[2][i]))
-        out = _fields_call(multi, arrays, sims, batch, prepared, k, slop, where, counts)
-    return out if counts is None else out + (counts.hits(),)
+        return _PreparedBool(arrays, sims, _clause_slots(batch, slot_of), queries, batch, where,
+                             None if facets is None else [(p, slot_of[p[0]], p[1]) for p in facets], multi).run(k, slop)
 
 
 def fields_topk(frame: pd.DataFrame, queries, k: int = 10,

@@ -179,13 +179,14 @@ def test_unit_weights_take_the_or_path(synth, monkeypatch):
         wd, ws = arr.search_topk(plain, k=k)
         bd, bs = arr.search_topk(as_bool, k=k)
         assert [bool_form(q) for q in unit] == [OR_AND] * len(unit)
-        seen, real = [], type(arr)._bool_call
+        from searcharray_b200.postings import _PreparedBool
+        seen, real = [], _PreparedBool.run
 
-        def spy(self, dev, batch, *a):
-            seen.append((batch.weights, batch.occurs))
-            return real(self, dev, batch, *a)
+        def spy(self, *a):
+            seen.append((self.batch.weights, self.batch.occurs))
+            return real(self, *a)
         with monkeypatch.context() as m:
-            m.setattr(type(arr), "_bool_call", spy)
+            m.setattr(_PreparedBool, "run", spy)
             gd, gs = arr.search_topk(unit, k=k)
         assert seen == [(None, None)], "unit weights took the occur instance"
         assert np.array_equal(gd, wd) and np.array_equal(gs.view(np.uint32), ws.view(np.uint32))

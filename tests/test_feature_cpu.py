@@ -212,7 +212,9 @@ def test_fields_topk_refusals(no_device):
     # columns sharing an index share its features: t2 is t's column
     batch, slot_of, arrays, sims = _fields_plan(fr, [Bool(must=[Field("t", "a")], should=[Field("t2", pop)])], {})
     assert slot_of["t"] == slot_of["t2"]
-    from searcharray_b200.solr import _feature_terms
-    assert _feature_terms(batch.clauses, slot_of, arrays) == {1: (pop.term_id(0), np.float32(1))}
+    from searcharray_b200.postings import _PreparedBool
+    from searcharray_b200.solr import _clause_slots
+    assert _PreparedBool.features(batch.clauses, _clause_slots(batch, slot_of), arrays) == {
+        1: (pop.term_id(0), np.float32(1))}
     with pytest.raises(DeviceTouched):
         fields_topk(fr, [Bool(must=[Field("t", "a")], should=[Field("t2", pop)])])

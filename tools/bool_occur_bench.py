@@ -57,8 +57,7 @@ def main():
     ap.add_argument("--verify", type=int, default=8)
     args = ap.parse_args()
 
-    from searcharray_b200 import And, Bool, Boost, Or, SearchArray, bm25_similarity, compute_idf, synth
-    from searcharray_b200.query import bool_form, flatten_bool
+    from searcharray_b200 import And, Bool, Boost, Or, SearchArray, bm25_similarity, synth
     info = card()
     spec = synth.SynthSpec(args.docs)
     host, _, _ = synth.generate_shard(spec)
@@ -133,21 +132,15 @@ def main():
         per_query = np.asarray([query_bytes(q) for q in queries], dtype=np.float64)
         # the Python side of the call alone: flattening and the per-clause idf (part of every timed call)
         t0 = time.perf_counter()
-        batch = flatten_bool(queries, max(map(bool_form, queries)))
-        terms, c_starts, idfs = arr._topk_queries(batch.clauses, lambda d: compute_idf(arr.corpus_size, d))
+        call = arr._prepare_bool(queries, sim)
         prep_ms = 1e3 * (time.perf_counter() - t0)
         # the C call alone on the prepared arrays: planning, uploads, kernels, the result copy
-        idfs = np.asarray(idfs, dtype=np.float32)
-        dev = arr._device()
-
-        def c_call():
-            return arr._bool_call(dev, batch, terms, c_starts, idfs, sim, 0, args.k, None)
         for _ in range(args.warmup):
-            c_call()
+            call.run(args.k, 0)
         c_times = []
         for _ in range(args.reps):
             t0 = time.perf_counter()
-            docs, scores, _ = c_call()
+            docs, scores, _ = call.run(args.k, 0)
             c_times.append(time.perf_counter() - t0)
         d_ref, s_ref, _ = arr._search_topk_bool(queries, args.k, sim, 0)
         if not (np.array_equal(docs, d_ref) and np.array_equal(scores.view(np.uint32), s_ref.view(np.uint32))):

@@ -65,7 +65,8 @@ def main():
 
     import pandas as pd
     from searcharray_b200 import Bool, Boost, DisMax, Field, Or, SearchArray, bm25_similarity, synth
-    from searcharray_b200.solr import _fields_call, _fields_clauses, _fields_plan, _fields_topk, _locked, _multi_for
+    from searcharray_b200.postings import _PreparedBool
+    from searcharray_b200.solr import _clause_slots, _fields_plan, _fields_topk, _multi_for
     from searcharray_b200 import solr
     info = card()
     spec = synth.SynthSpec(args.docs)
@@ -119,11 +120,9 @@ def main():
 
     def c_time(queries):
         batch, slot_of, arrays, sims = _fields_plan(frame, queries, sim)
-        multi = _multi_for(arrays)
-        with _locked(multi, arrays):
-            prepared = _fields_clauses(batch.clauses, slot_of, arrays)
-            return median_time(lambda: _fields_call(multi, arrays, sims, batch, prepared, args.k, 0), args.warmup,
-                               args.reps)
+        call = _PreparedBool(arrays, sims, _clause_slots(batch, slot_of), queries, batch,
+                             multi=_multi_for(arrays))
+        return median_time(lambda: call.run(args.k, 0), args.warmup, args.reps)
 
     def verify(label, queries, run, scorer):
         sample = queries[::max(1, len(queries) // args.verify)][:args.verify]
@@ -168,24 +167,10 @@ def main():
     n_ver = verify("synonyms", sq, lambda qs: f1.search_topk(qs, k=args.k), f1.score)
     t_api = median_time(lambda: f1.search_topk(sq, k=args.k), args.warmup, args.reps)
     t_or_api = median_time(lambda: f1.search_topk(oq, k=args.k), args.warmup, args.reps)
-    from searcharray_b200.query import DISMAX, OR_AND, flatten_bool
-    from searcharray_b200 import compute_idf
-    dev = f1._device()
-    batch = flatten_bool(sq, DISMAX)
-    terms, c_starts, idfs = f1._topk_queries(batch.clauses, lambda x: compute_idf(f1.corpus_size, x))
-    idfs = np.asarray(idfs, dtype=np.float32)
+    dismax_call, or_call = f1._prepare_bool(sq, sim), f1._prepare_bool(oq, sim)
     redone = []
-
-    def dismax_c():
-        redone.append(f1._bool_call(dev, batch, terms, c_starts, idfs, sim, 0, args.k, None)[2])
-    obatch = flatten_bool(oq, OR_AND)
-    oterms, oc_starts, oidfs = f1._topk_queries(obatch.clauses, lambda x: compute_idf(f1.corpus_size, x))
-    oidfs = np.asarray(oidfs, dtype=np.float32)
-
-    def or_c():
-        f1._bool_call(dev, obatch, oterms, oc_starts, oidfs, sim, 0, args.k, None)
-    t_c = median_time(dismax_c, args.warmup, args.reps)
-    t_or_c = median_time(or_c, args.warmup, args.reps)
+    t_c = median_time(lambda: redone.append(dismax_call.run(args.k, 0)[2]), args.warmup, args.reps)
+    t_or_c = median_time(lambda: or_call.run(args.k, 0), args.warmup, args.reps)
     rec = {"queries": nq, "verified_queries": n_ver, "qps": nq / t_api, "or_qps": nq / t_or_api, "c_call_qps": nq / t_c,
            "or_c_call_qps": nq / t_or_c, "ratio_c_call": t_or_c / t_c, "n_redone": redone[-args.reps:]}
     out["workloads"]["synonyms"] = rec

@@ -51,9 +51,8 @@ def main():
     ap.add_argument("--verify", type=int, default=4)
     args = ap.parse_args()
 
-    from searcharray_b200 import Or, SearchArray, bm25_similarity, compute_idf
+    from searcharray_b200 import Or, SearchArray, bm25_similarity
     from searcharray_b200 import synth
-    from searcharray_b200.query import bool_form, flatten_bool
     info = card()
     spec = synth.SynthSpec(args.docs)
     host, _, _ = synth.generate_shard(spec)
@@ -72,18 +71,10 @@ def main():
     terms = [names[perm[0][i]] for i in range(nq)]
     sim = bm25_similarity()
 
-    batch = flatten_bool(ors, max(map(bool_form, ors)))
-    t_ids, c_starts, idfs = arr._topk_queries(batch.clauses, lambda x: compute_idf(arr.corpus_size, x))
-    idfs = np.asarray(idfs, dtype=np.float32)
-    dev = arr._device()
-    dev.sync_facets(arr.host)
-
     def c_call(facets):
         """The C call of search_topk(ors, facets=facets) on arrays prepared once: fn() -> n_redone."""
-        def fn():
-            counts = None if facets is None else arr._counts(facets, nq)
-            return arr._bool_call(dev, batch, t_ids, c_starts, idfs, sim, 0, args.k, None, counts)[2]
-        return fn
+        call = arr._prepare_bool(ors, sim, facets=facets)
+        return lambda: call.run(args.k, 0)[2]
 
     cells = {
         "or": (lambda: arr.search_topk(ors, k=args.k), c_call(None), ors, None),

@@ -56,11 +56,10 @@ def main():
     args = ap.parse_args()
 
     import pandas as pd
-    from searcharray_b200 import Bool, Feature, Field, Or, SearchArray, bm25_similarity, compute_idf, fields_topk
+    from searcharray_b200 import Bool, Feature, Field, Or, SearchArray, bm25_similarity, fields_topk
     from searcharray_b200 import synth
-    from searcharray_b200.postings import pack_where
-    from searcharray_b200.query import bool_form, feature_terms, flatten_bool
-    from searcharray_b200.solr import _fields_call, _fields_clauses, _fields_plan, _locked, _multi_for
+    from searcharray_b200.postings import _PreparedBool, pack_where
+    from searcharray_b200.solr import _clause_slots, _fields_plan, _locked, _multi_for
     info = card()
     spec = synth.SynthSpec(args.docs)
     host, _, _ = synth.generate_shard(spec)
@@ -101,13 +100,8 @@ def main():
 
     def prepared(queries, bits=None):
         """The C call of search_topk(queries) on arrays prepared once: fn() -> n_redone."""
-        batch = flatten_bool(queries, max(map(bool_form, queries)))
-        feats = feature_terms(batch.clauses, lambda i, f: arr._feature_slot(f.name))
-        terms, c_starts, idfs = arr._clause_terms(batch.clauses, feats, lambda x: compute_idf(arr.corpus_size, x))
-        dev = arr._device()
-        dev.sync_features(arr.host)
-        w = None if bits is None else pack_where(bits, n, len(queries))
-        return lambda: arr._bool_call(dev, batch, terms, c_starts, idfs, sim, 0, args.k, w)[2]
+        call = arr._prepare_bool(queries, sim, None if bits is None else pack_where(bits, n, len(queries)))
+        return lambda: call.run(args.k, 0)[2]
 
     def verify(queries, docs, scores, where=None):
         ok = 0
@@ -130,12 +124,11 @@ def main():
     }
     batch, slot_of, arrays, sims = _fields_plan(frame, fields_q, sim)
     multi = _multi_for(arrays)
-    with _locked(multi, arrays):
-        prep = _fields_clauses(batch.clauses, slot_of, arrays)
+    fields_call = _PreparedBool(arrays, sims, _clause_slots(batch, slot_of), fields_q, batch, multi=multi)
 
     def fields_c():
         with _locked(multi, arrays):
-            return _fields_call(multi, arrays, sims, batch, prep, args.k, 0)[2]
+            return fields_call.run(args.k, 0)[2]
     cells["fields"] = (lambda: fields_topk(frame, fields_q, k=args.k), fields_c, fields_q, None)
     for fn_pub, fn_c, _, _ in cells.values():            # warm every shape
         for _ in range(args.warmup):

@@ -69,9 +69,9 @@ def main():
     args = ap.parse_args()
 
     import pandas as pd
-    from searcharray_b200 import Bool, Boost, Field, Or, SearchArray, bm25_similarity, compute_idf, synth
-    from searcharray_b200.query import OCCUR, flatten_bool
-    from searcharray_b200.solr import _fields_call, _fields_clauses, _fields_plan, _fields_topk, _locked, _multi_for
+    from searcharray_b200 import Bool, Boost, Field, Or, SearchArray, bm25_similarity, synth
+    from searcharray_b200.postings import _PreparedBool
+    from searcharray_b200.solr import _clause_slots, _fields_plan, _fields_topk, _multi_for
     info = card()
     spec = synth.SynthSpec(args.docs)
     host, _, _ = synth.generate_shard(spec)
@@ -144,21 +144,13 @@ def main():
         # field-aware kernel on one index's data), and the single-field Bool
         def fields_c_time(queries):
             batch, slot_of, arrays, sims = _fields_plan(frame, queries, sim)
-            multi = _multi_for(arrays)
-            with _locked(multi, arrays):
-                prepared = _fields_clauses(batch.clauses, slot_of, arrays)
-                return median_time(lambda: _fields_call(multi, arrays, sims, batch, prepared, args.k, 0), args.warmup,
-                                   args.reps)
+            call = _PreparedBool(arrays, sims, _clause_slots(batch, slot_of), queries, batch,
+                             multi=_multi_for(arrays))
+            return median_time(lambda: call.run(args.k, 0), args.warmup, args.reps)
         t_c = fields_c_time(fq)
         t_c1 = fields_c_time(build(lambda f, c: Field("f1", c), label))
-        sbatch = flatten_bool(sq, OCCUR)
-        terms, c_starts, idfs = f1._topk_queries(sbatch.clauses, lambda x: compute_idf(f1.corpus_size, x))
-        idfs = np.asarray(idfs, dtype=np.float32)
-        dev = f1._device()
-
-        def single_c():
-            f1._bool_call(dev, sbatch, terms, c_starts, idfs, sim, 0, args.k, None)
-        t_single_c = median_time(single_c, args.warmup, args.reps)
+        single_call = f1._prepare_bool(sq, sim)
+        t_single_c = median_time(lambda: single_call.run(args.k, 0), args.warmup, args.reps)
 
         # the host composition of dense per-field .score vectors
         nn = min(args.numpy_queries, len(fq))

@@ -63,10 +63,11 @@ def main():
     args = ap.parse_args()
 
     import pandas as pd
-    from searcharray_b200 import And, Bool, Boost, DisMax, Field, Or, SearchArray, bm25_similarity, compute_idf
+    from searcharray_b200 import And, Bool, Boost, DisMax, Field, Or, SearchArray, bm25_similarity
     from searcharray_b200 import synth
-    from searcharray_b200.query import NESTED, _leaves, flatten_bool
-    from searcharray_b200.solr import _fields_call, _fields_clauses, _fields_plan, _fields_topk, _locked, _multi_for
+    from searcharray_b200.postings import _PreparedBool
+    from searcharray_b200.query import _leaves
+    from searcharray_b200.solr import _clause_slots, _fields_plan, _fields_topk, _multi_for
     info = card()
     spec = synth.SynthSpec(args.docs)
     host, _, _ = synth.generate_shard(spec)
@@ -123,11 +124,8 @@ def main():
             redone.append(_fields_topk(frame, qs, args.k, sim, 0)[2])
         t_api = median_time(run, args.warmup, args.reps)
         batch, slot_of, arrays, sims = _fields_plan(frame, qs, sim)
-        multi = _multi_for(arrays)
-        with _locked(multi, arrays):
-            prepared = _fields_clauses(batch.clauses, slot_of, arrays)
-            t_c = median_time(lambda: _fields_call(multi, arrays, sims, batch, prepared, args.k, 0), args.warmup,
-                              args.reps)
+        call = _PreparedBool(arrays, sims, _clause_slots(batch, slot_of), qs, batch, multi=_multi_for(arrays))
+        t_c = median_time(lambda: call.run(args.k, 0), args.warmup, args.reps)
         rec = dict({"queries": nq, "verified_queries": n_ver, "qps": nq / t_api, "c_call_qps": nq / t_c,
                     "n_redone": redone[-args.reps:]}, **shape(qs))
         out["workloads"][label] = rec
@@ -137,19 +135,9 @@ def main():
     qs = [Or([And([t(i, 0), t(i, 1)]), And([t(i, 2), t(i, 3)])]) for i in range(nq)]
     n_ver = verify("or_of_ands", qs, lambda x: f1.search_topk(x, k=args.k), f1.score)
     t_api = median_time(lambda: f1.search_topk(qs, k=args.k), args.warmup, args.reps)
-    batch = flatten_bool(qs, NESTED)
-    clauses = batch.clauses
-    leaf = [i for i, c in enumerate(clauses) if c is not None]
-    terms, l_starts, l_idfs = f1._topk_queries([clauses[i] for i in leaf], lambda x: compute_idf(f1.corpus_size, x))
-    idfs, n_terms = np.zeros(len(clauses), dtype=np.float32), np.zeros(len(clauses), dtype=np.int64)
-    idfs[leaf], n_terms[leaf] = l_idfs, np.diff(l_starts)
-    c_starts = np.concatenate([[0], np.cumsum(n_terms)]).astype(np.uint32)
-    dev = f1._device()
+    call = f1._prepare_bool(qs, sim)
     redone = []
-
-    def c_call():
-        redone.append(f1._bool_call(dev, batch, terms, c_starts, idfs, sim, 0, args.k, None)[2])
-    t_c = median_time(c_call, args.warmup, args.reps)
+    t_c = median_time(lambda: redone.append(call.run(args.k, 0)[2]), args.warmup, args.reps)
     rec = dict({"queries": nq, "verified_queries": n_ver, "qps": nq / t_api, "c_call_qps": nq / t_c,
                 "n_redone": redone[-args.reps:]}, **shape(qs))
     out["workloads"]["or_of_ands"] = rec

@@ -55,24 +55,6 @@ def median_time(fn, warmup, reps):
     return float(np.median(times))
 
 
-def prepared_call(arr, queries, k, sim):
-    """The C call of search_topk(queries, where=...) on arrays prepared once: fn(bits) -> n_redone."""
-    from searcharray_b200 import Or, compute_idf
-    from searcharray_b200.query import bool_form, flatten_bool, is_boolean
-    qs = [q if is_boolean(q) else Or([q]) for q in queries]
-    batch = flatten_bool(qs, max(map(bool_form, qs)))
-    clauses = batch.clauses
-    leaf = [i for i, c in enumerate(clauses) if c is not None]
-    terms, l_starts, l_idfs = arr._topk_queries([clauses[i] for i in leaf], lambda x: compute_idf(arr.corpus_size, x))
-    idfs, n_terms = np.zeros(len(clauses), dtype=np.float32), np.zeros(len(clauses), dtype=np.int64)
-    idfs[leaf], n_terms[leaf] = l_idfs, np.diff(l_starts)
-    c_starts = np.concatenate([[0], np.cumsum(n_terms)]).astype(np.uint32)
-    dev = arr._device()
-
-    def call(bits):
-        return arr._bool_call(dev, batch, terms, c_starts, idfs, sim, 0, k, bits)[2]
-    return call
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--docs", type=int, default=10_000_000)
@@ -131,15 +113,13 @@ def main():
         sample_i = list(range(0, n_pq, max(1, n_pq // args.verify)))[:args.verify]
         dense = {i: compose_nested(arr.score, qs[i]) if not isinstance(qs[i], (str, list))
                  else np.asarray(arr.score(qs[i]), dtype=np.float32) for i in sample_i}
-        call = prepared_call(arr, qs, args.k, sim)
-        call_pq = prepared_call(arr, qs[:n_pq], args.k, sim)
         cells = {}
         for mname in list(masks) + ["perq10"]:
             if mname == "perq10":
                 m = np.random.default_rng(7).random((n_pq, n)) < 0.1
-                batch, c = qs[:n_pq], call_pq
+                batch = qs[:n_pq]
             else:
-                m, batch, c = masks[mname], qs, call
+                m, batch = masks[mname], qs
             d, s = arr.search_topk([batch[i] for i in sample_i], k=args.k, where=None if m is None else (
                 m[sample_i] if m is not None and m.ndim == 2 else m))
             for j, i in enumerate(sample_i):
@@ -158,12 +138,11 @@ def main():
                 t_c = median_time(lambda: _lib.check(_lib.lib().sa_score_batch_topk(
                     h, _lib.p_u32(terms), _lib.p_u32(starts), _lib.p_f32(idfs), len(idfs), 0, arr.avg_doc_length,
                     sim.k1, sim.b, args.k, _lib.p_u32(dd), _lib.p_f32(ss))), args.warmup, args.reps)
-            elif m is None:
-                # the same prepared arrays without a mask: the unmasked instances, for a kernel-level comparison
-                t_c = median_time(lambda: redone.append(c(None)), args.warmup, args.reps)
             else:
-                bits = pack_where(m, n, len(batch))
-                t_c = median_time(lambda: redone.append(c(bits)), args.warmup, args.reps)
+                # for `none`, the same prepared call without a mask: the unmasked instances, for a kernel-level
+                # comparison
+                call = arr._prepare_bool(batch, sim, None if m is None else pack_where(m, n, len(batch)))
+                t_c = median_time(lambda: redone.append(call.run(args.k, 0)[2]), args.warmup, args.reps)
             cells[mname] = {"queries": len(batch), "qps": len(batch) / t_api, "c_call_qps": len(batch) / t_c,
                             "n_redone": redone[-args.reps:], "verified": len(sample_i)}
             print(f"[where_topk_bench] {label} {mname}: {json.dumps(cells[mname])}", file=sys.stderr, flush=True)
