@@ -307,6 +307,9 @@ typedef struct {
     /* launches of the conjunction regime's phrase_tile_kernel (also counted in phrase_kernel_launches): 0 = the
      * search regime alone ran, phrase_kernel_launches > phrase_tile_launches after one = a re-run in the search regime */
     uint64_t phrase_tile_launches;
+    /* the bool_tile_kernel instances launched (sa_bool.cu, bool_kernel): bit variant * 10 + form * 2 + masked, with
+     * form 0 Or / And, 1 roles and weights, 2 fields, 3 DisMax, 4 nested and variant 0 plain, 1 FEATURE, 2 COUNT */
+    uint64_t bool_instances;
 } sa_stats;
 int sa_stats_reset(sa_index *index);
 int sa_stats_get(sa_index *index, sa_stats *out);

@@ -27,7 +27,8 @@ class SaStats(ctypes.Structure):
                 ("term_kernel_queries", c_u64), ("topk_kernel_ms", ctypes.c_double),
                 ("topk_kernel_launches", c_u64), ("phrase_kernel_ms", ctypes.c_double),
                 ("phrase_kernel_launches", c_u64), ("total_launches", c_u64),
-                ("phrase_cont_words", c_u64), ("phrase_matched_docs", c_u64), ("phrase_tile_launches", c_u64)]
+                ("phrase_cont_words", c_u64), ("phrase_matched_docs", c_u64), ("phrase_tile_launches", c_u64),
+                ("bool_instances", c_u64)]
 
 
 # name -> (restype, argtypes); must list EVERY symbol include/searcharray_b200.h declares

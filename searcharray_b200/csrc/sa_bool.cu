@@ -789,10 +789,12 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
         cn.counts += (u64)q0 * cn.n_bins;
     }
     auto launch = [&](bool c, bool masked, u32 n_q, const BoolArgs &args, const BoolNest &n, const WhereMask &w) -> int {
-        bool_kernel(P.form, masked, bool_variant(P, c))<<<dim3(n_q, n_tiles), SA_TERM_THREADS, smem, ix->stream>>>(
+        const BoolVariant variant = bool_variant(P, c);
+        bool_kernel(P.form, masked, variant)<<<dim3(n_q, n_tiles), SA_TERM_THREADS, smem, ix->stream>>>(
             args, occ, fld, grp, n, w, feat, cn);
         SA_CUDA(cudaGetLastError());
         ix->stats.total_launches++;
+        ix->stats.bool_instances |= 1ull << (variant * 10 + P.form * 2 + (masked ? 1 : 0));
         return SA_OK;
     };
     if (P.form == BOOL_NESTED) {
