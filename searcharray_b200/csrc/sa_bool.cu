@@ -146,17 +146,11 @@ struct BoolCount {
 };
 
 struct BoolState {
-    DevBuf d_clauses, d_queries, d_out_index;
-    DevBuf d_occur;
-    DevBuf d_nest;       // u32[] per clause of a nested call (BoolNest::nested)
-    DevBuf d_flags;      // BoolNest::flags
-    DevBuf d_groups;     // BoolGroup[] of a DisMax call
-    DevBuf d_fields;     // BoolField[] of a multi-field call
-    DevBuf d_keys;       // nq * k result keys, then u32 overflow[nq] (and, counting, total[nq] and the facet rows):
-                         // one device-to-host copy
+    DevBuf desc;         // the call's descriptor arrays, one section each (BoolDescs)
+    DevBuf d_keys;       // the call's result block (BoolResult): one device-to-host copy
     DevBuf rows;
+    DevBuf d_flags;      // BoolNest::flags
     DevBuf d_where;      // the WhereMask rows of a masked call
-    DevBuf d_feat;       // BoolFeature[] of a call with feature clauses
 };
 void BoolStateDelete::operator()(BoolState *s) const { delete s; }
 
@@ -677,39 +671,94 @@ BoolKernel bool_kernel(BoolForm form, bool masked, BoolVariant variant) {
 struct BoolCall {
     std::vector<sa_index *> ix;         // per field slot
     std::vector<float> avgdl, k1, b;    // per field slot
-    bool fields_kernel = false;         // a multi-field call: BOOL_FIELDS at least (clauses carry their field slot)
-    BoolState *S = nullptr;
-    DevBuf *cand = nullptr;
-    PinnedBuf *h_pinned = nullptr;
-    // the call's document mask, as passed (host; where_bits NULL: no mask), and its rows on the device
-    const uint32_t *where_bits = nullptr;
-    uint64_t where_n = 0, where_stride = 0;
-    WhereMask where{nullptr, 0};
-    // the call's hit and facet counts, as passed (out_total NULL: no counting)
-    uint32_t n_facets = 0;
-    const uint32_t *facet_field = nullptr, *facet_slot = nullptr;
-    uint32_t *out_total = nullptr, *out_facet_counts = nullptr;
+    bool fields_kernel;                 // a multi-field call: BOOL_FIELDS at least (clauses carry their field slot)
+    BoolState *S;
+    DevBuf *cand;
+    PinnedBuf *h_pinned;
     sa_index *lead() const { return ix[0]; }
+};
+
+bool bool_is_feature_term(u32 t) { return t >= SA_FEATURE_TERM_BASE && t != SA_NO_TERM; }
+
+// A call's arrays and scalars as its entry point was given them, in the entry points' argument order.
+// clause_weight / clause_occur NULL: Or / And, every clause SHOULD with weight 1, mm over all.  clause_field NULL:
+// every clause on field 0.  clause_group / clause_tie non-NULL (with clause_occur): DisMax groups, on a field table.
+// clause_node non-NULL (with the DisMax arrays): n_nodes nodes, the first n_queries top-level, clause c being nested
+// node clause_node[c] unless SA_NO_NODE; otherwise n_nodes == n_queries.  where_bits non-NULL: the document mask.
+// out_total non-NULL: hit counts, and counts over the n_facets facets.
+struct BoolInput {
+    u32 n_nodes;
+    const u32 *node_clause_starts, *clause_node, *clause_field, *clause_terms, *clause_term_starts;
+    const float *clause_idf, *clause_weight;
+    const uint8_t *clause_occur;
+    const u32 *clause_group;
+    const float *clause_tie;
+    const u32 *mm;
+    u32 n_queries, slop, k;
+    const u32 *where_bits;
+    uint64_t where_n, where_stride;
+    u32 *out_docs;
+    float *out_scores;
+    u32 *n_redone;
+    u32 n_facets;
+    const u32 *facet_field, *facet_slot;
+    u32 *out_total, *out_facet_counts;
+
+    bool nested(u32 c) const { return clause_node && clause_node[c] != SA_NO_NODE; }
+    u32 field(u32 c) const { return clause_field ? clause_field[c] : 0; }
+    const u32 *terms(u32 c) const { return clause_terms + clause_term_starts[c]; }
+    u32 n_terms(u32 c) const { return clause_term_starts[c + 1] - clause_term_starts[c]; }
+    bool feature(u32 c) const { return n_terms(c) == 1 && bool_is_feature_term(terms(c)[0]); }
+    // clause c of a node with clauses [c0, c1) is a member of a DisMax group of two or more clauses
+    bool member(u32 c, u32 c0, u32 c1) const {
+        return clause_group && ((c > c0 && clause_group[c] == clause_group[c - 1]) ||
+                                (c + 1 < c1 && clause_group[c + 1] == clause_group[c]));
+    }
+};
+
+// What bool_check learns of a call for the steps after it.
+struct BoolChecked {
+    bool features = false;  // some clause is a feature
+    bool empty = false;     // nothing can rank: no query, no doc, or every field's avgdl 0 and no feature
+    BoolCount count{};      // counting: the facets' columns and bins (the rows are placed per launch)
+};
+
+// Where each descriptor array of a call starts, in bytes, in BoolState::desc and in the host block it is uploaded
+// from in one copy: one section per array, each 256-byte aligned.
+struct BoolDescs { size_t clauses, queries, occur, groups, nest, fields, features, bytes; };
+
+// The result block of a call, in BoolState::d_keys and downloaded whole into the pinned staging: the keys
+// [n_queries][k], then the overflow flags [n_queries] and, counting, the totals [n_queries] and the facet rows
+// [n_queries][n_bins].  `base` is either copy.
+struct BoolResult {
+    size_t n_keys, n_queries, n_bins;
+    bool counting;
+    u64 *keys(void *base) const { return (u64 *)base; }
+    u32 *ovf(void *base) const { return (u32 *)(keys(base) + n_keys); }
+    u32 *total(void *base) const { return ovf(base) + n_queries; }
+    u32 *counts(void *base) const { return total(base) + n_queries; }
+    size_t bytes() const { return n_keys * sizeof(u64) + n_queries * sizeof(u32) * (counting ? 2 + n_bins : 1); }
 };
 
 struct BoolPlan {
     BoolForm form = BOOL_OR_AND;
+    u32 slots = 0;                      // candidate slots per tile of a first pass
     std::vector<BoolClause> clauses;
     std::vector<BoolQuery> queries;
     std::vector<u32> group_start;       // queries [group_start[i], group_start[i + 1]) share one launch and its rows
     std::vector<BoolOccur> occur;       // per clause, as clauses (from BOOL_OCCUR up)
-    std::vector<BoolField> fields;      // per field slot (from BOOL_FIELDS up)
     std::vector<BoolGroup> groups;      // per clause, as clauses (from BOOL_DISMAX up)
-    u32 max_group = 1, max_rows = 0;
-    // nested calls: nodes 0 .. n_top - 1 are the top-level queries (queries[0 .. n_top)), the others nested nodes
-    u32 n_top = 0;
-    std::vector<u32> node_starts;       // node n's clauses [node_starts[n], node_starts[n + 1])
+    u32 max_rows = 0;
+    // nested calls: nodes 0 .. n_queries - 1 are the top-level queries (queries[0 .. n_queries)), the others nested
     std::vector<u32> root, depth;       // per node: its top-level query, and its depth below it
-    std::vector<u32> nested;            // nested nodes by (launch group, depth desc, top-level query); queries[n_top + i]
-                                        // is nested[i]'s descriptor
+    std::vector<u32> nested;            // nested nodes by (launch group, depth desc, top-level query);
+                                        // queries[n_queries + i] is nested[i]'s descriptor
     std::vector<u32> nest;              // per clause, as clauses: 1 for a nested clause (BOOL_NESTED)
     std::vector<BoolFeature> features;  // per clause, as clauses, when a clause is a feature (the FEATURE instances)
-    BoolCount count{};                  // total and counts: the call's rows (bool_run_group offsets them per launch)
+    std::vector<char> field_sparse;     // per field slot: 1 with a sparse-safe clause (its norms are cached)
+    BoolCount count{};                  // the facet table of bool_check
+    BoolDescs descs{};
+    BoolResult result{};
 };
 
 // The variant a launch runs: COUNT for the first pass of a counting call (count), otherwise FEATURE when the batch has
@@ -720,8 +769,7 @@ BoolVariant bool_variant(const BoolPlan &P, bool count) {
 
 // The count rows of the phrase clauses of queries [q0, q1) and of their nested nodes (rows are numbered within the
 // group), each on its clause's field, synchronously.
-int bool_build_rows(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_terms,
-                    const uint32_t *clause_term_starts, u32 slop, u32 q0, u32 q1) {
+int bool_build_rows(const BoolCall &X, const BoolPlan &P, const BoolInput &in, u32 q0, u32 q1) {
     const u64 stride = sa_padded_docs(X.lead()->n_docs);
     int rc;
     std::vector<u32> nodes;
@@ -729,13 +777,13 @@ int bool_build_rows(const BoolCall &X, const BoolPlan &P, const uint32_t *clause
     for (u32 n : P.nested)
         if (P.root[n] >= q0 && P.root[n] < q1) nodes.push_back(n);
     for (u32 n : nodes) {
-        for (u32 c = P.node_starts[n]; c < P.node_starts[n + 1]; c++) {
+        for (u32 c = in.node_clause_starts[n]; c < in.node_clause_starts[n + 1]; c++) {
             const BoolClause &cl = P.clauses[c];
-            if (cl.row == SA_BOOL_NO_ROW || cl.row == SA_BOOL_FEATURE_ROW || (!P.nest.empty() && P.nest[c])) continue;
+            if (cl.row == SA_BOOL_NO_ROW || cl.row == SA_BOOL_FEATURE_ROW || in.nested(c)) continue;
             sa_index *ix = X.ix[cl.field];
             bool scored;
-            if ((rc = sa_phrase_row(ix, clause_terms + clause_term_starts[c], clause_term_starts[c + 1] - clause_term_starts[c],
-                                    slop, nullptr, nullptr, nullptr, &scored))) return rc;
+            if ((rc = sa_phrase_row(ix, in.terms(c), in.n_terms(c), in.slop, nullptr, nullptr, nullptr, &scored)))
+                return rc;
             SA_CUDA(cudaMemcpyAsync(X.S->rows.as<float>() + (u64)cl.row * stride, ix->dense.p, ix->n_docs * sizeof(float),
                                     cudaMemcpyDeviceToDevice, ix->stream));
         }
@@ -744,21 +792,19 @@ int bool_build_rows(const BoolCall &X, const BoolPlan &P, const uint32_t *clause
 }
 
 // Queries [q0, q1) with `slots` candidate slots per tile: their rows, the tile kernel and the selection, enqueued.
-// count: the first pass of a counting call, the top-level launch counting into P.count.
-int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_terms,
-                   const uint32_t *clause_term_starts, u32 slop, u32 k, u32 slots, u32 q0, u32 q1, bool count) {
+// count: the first pass of a counting call, the top-level launch counting into the call's rows.
+int bool_run_group(const BoolCall &X, const BoolPlan &P, const BoolInput &in, const WhereMask &where, u32 slots,
+                   u32 q0, u32 q1, bool count) {
     sa_index *ix = X.lead();
     BoolState &S = *X.S;
     const u32 n_tiles = sa_n_tiles(ix->n_docs), nq = q1 - q0;
     int rc;
-    if ((rc = bool_build_rows(X, P, clause_terms, clause_term_starts, slop, q0, q1))) return rc;
+    if ((rc = bool_build_rows(X, P, in, q0, q1))) return rc;
     if ((rc = X.cand->reserve(cand_bytes(n_tiles, nq, slots)))) return rc;
-    u64 *d_keys = S.d_keys.as<u64>();
-    u32 *d_ovf = (u32 *)(d_keys + (size_t)P.n_top * k);
-    TopkCtx t = make_topk_ctx(X.cand->p, n_tiles, nq, slots, k, d_ovf + q0);
+    TopkCtx t = make_topk_ctx(X.cand->p, n_tiles, nq, slots, in.k, P.result.ovf(S.d_keys.p) + q0);
     BoolArgs a;
     memset(&a, 0, sizeof(a));
-    if (P.fields.empty()) {                 // the field-table kernels read these per clause from S.d_fields
+    if (P.form < BOOL_FIELDS) {             // the field-table kernels read these per clause from the field table
         a.words = ix->d_words.as<u64>();
         a.tile_dir = ix->d_tile_dir.as<u32>();
         a.recs = ix->d_recs.as<u32>();
@@ -767,26 +813,29 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
         a.doc_lens = ix->d_doc_lens.as<float>();
         a.bm25 = make_bm25(1.0f, X.avgdl[0], X.k1[0], X.b[0], ix->doc_lens_nonneg);
     }
+    const char *d = S.desc.as<const char>();
+    const BoolQuery *queries = (const BoolQuery *)(d + P.descs.queries);
     a.rows = S.rows.as<float>();
     a.row_stride = sa_padded_docs(ix->n_docs);
     a.n_docs = ix->n_docs;
     a.doc_base = ix->doc_base;
-    a.clauses = S.d_clauses.as<BoolClause>();
-    a.queries = S.d_queries.as<BoolQuery>() + q0;
+    a.clauses = (const BoolClause *)(d + P.descs.clauses);
+    a.queries = queries + q0;
     a.topk = t;
-    WhereMask wh = X.where;                 // row 0 of the launch is query q0's
+    WhereMask wh = where;                   // row 0 of the launch is query q0's
     if (wh.bits) wh.bits += (u64)q0 * wh.stride;
     // the arrays P.form reads, NULL above it
-    const BoolOccur *occ = P.form >= BOOL_OCCUR ? S.d_occur.as<BoolOccur>() : nullptr;
-    const BoolField *fld = P.form >= BOOL_FIELDS ? S.d_fields.as<BoolField>() : nullptr;
-    const BoolGroup *grp = P.form >= BOOL_DISMAX ? S.d_groups.as<BoolGroup>() : nullptr;
+    const BoolOccur *occ = P.form >= BOOL_OCCUR ? (const BoolOccur *)(d + P.descs.occur) : nullptr;
+    const BoolField *fld = P.form >= BOOL_FIELDS ? (const BoolField *)(d + P.descs.fields) : nullptr;
+    const BoolGroup *grp = P.form >= BOOL_DISMAX ? (const BoolGroup *)(d + P.descs.groups) : nullptr;
     BoolNest nb{nullptr, nullptr, nullptr, 0};
     const size_t smem = P.form >= BOOL_DISMAX ? SA_BOOL_DISMAX_SMEM : 0;
-    const BoolFeature *feat = P.features.empty() ? nullptr : S.d_feat.as<BoolFeature>();
-    BoolCount cn = P.count;                 // row 0 of the launch is query q0's
-    if (count) {
-        cn.total += q0;
-        cn.counts += (u64)q0 * cn.n_bins;
+    const BoolFeature *feat = P.features.empty() ? nullptr : (const BoolFeature *)(d + P.descs.features);
+    BoolCount cn = P.count;                 // counting: the call's rows, from query q0's in the counting launch
+    if (in.out_total) {
+        const u32 row0 = count ? q0 : 0;
+        cn.total = P.result.total(S.d_keys.p) + row0;
+        cn.counts = P.result.counts(S.d_keys.p) + (u64)row0 * cn.n_bins;
     }
     auto launch = [&](bool c, bool masked, u32 n_q, const BoolArgs &args, const BoolNest &n, const WhereMask &w) -> int {
         const BoolVariant variant = bool_variant(P, c);
@@ -800,21 +849,21 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const uint32_t *clause_
     if (P.form == BOOL_NESTED) {
         // the nested nodes of these queries, deepest level first (one launch per level: a level's nodes of the run
         // are consecutive in P.nested), each into its row and flags, unmasked; then the top-level nodes, collected
-        nb = BoolNest{S.d_nest.as<u32>(), S.d_flags.as<u32>(), S.rows.as<float>(), n_tiles};
+        nb = BoolNest{(const u32 *)(d + P.descs.nest), S.d_flags.as<u32>(), S.rows.as<float>(), n_tiles};
         for (size_t i = 0; i < P.nested.size();) {
             auto in_run = [&](size_t x) { return P.root[P.nested[x]] >= q0 && P.root[P.nested[x]] < q1; };
             if (!in_run(i)) { i++; continue; }
             size_t j = i + 1;
             while (j < P.nested.size() && in_run(j) && P.depth[P.nested[j]] == P.depth[P.nested[i]]) j++;
             BoolArgs an = a;
-            an.queries = S.d_queries.as<BoolQuery>() + P.n_top + i;
+            an.queries = queries + in.n_queries + i;
             if ((rc = launch(false, false, (u32)(j - i), an, nb, WhereMask{nullptr, 0}))) return rc;
             i = j;
         }
         nb.store = nullptr;
     }
     if ((rc = launch(count, wh.bits != nullptr, nq, a, nb, wh))) return rc;
-    return launch_topk_select(ix, t, nq, ix->doc_base, d_keys, S.d_out_index.as<u32>() + q0);
+    return launch_topk_select(ix, t, nq, ix->doc_base, P.result.keys(S.d_keys.p) + (size_t)q0 * in.k, nullptr);
 }
 
 // The DisMax instances' dynamic shared memory above the default 48 KB, and the carveout that fits two CTAs per SM
@@ -841,148 +890,166 @@ int bool_check_feature(const sa_index *ix, u32 c, u32 term, float param) {
     return SA_OK;
 }
 
-bool bool_is_feature_term(u32 t) { return t >= SA_FEATURE_TERM_BASE && t != SA_NO_TERM; }
+// Bm25Params::sparse_ok of a clause with idf `idf` on field f.
+bool bool_sparse(const BoolCall &X, u32 f, float idf) {
+    return make_bm25(idf, X.avgdl[f], X.k1[f], X.b[f], X.ix[f]->doc_lens_nonneg).sparse_ok != 0;
+}
 
-// Both entry points, with the call's indexes locked and their device current.  clause_weight / clause_occur NULL:
-// Or / And, every clause SHOULD with weight 1, mm over all.  clause_field NULL: every clause on field 0.
-// clause_group / clause_tie non-NULL (with clause_occur): DisMax groups, on a field table.  clause_node non-NULL (with
-// the DisMax arrays): n_nodes nodes, the first n_queries top-level, clause c being nested node clause_node[c] unless
-// SA_NO_NODE; otherwise n_nodes == n_queries.  X.where_bits non-NULL: the document mask, checked before any device
-// work.
-int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts, const uint32_t *clause_node,
-              const uint32_t *clause_field, const uint32_t *clause_terms, const uint32_t *clause_term_starts,
-              const float *clause_idf, const float *clause_weight, const uint8_t *clause_occur,
-              const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
-              uint32_t slop, uint32_t k, uint32_t *out_docs, float *out_scores, uint32_t *n_redone) {
-    sa_index *lead = X.lead();
-    const u32 n_fields = (u32)X.ix.size();
+// Every refusal of a call (SA_ERR_ARG), with no CUDA API call.  The BM25-parameter refusals come last, and only where
+// something can rank, on fields with avgdl > 0: a call or a clause that scores nothing takes any parameters.
+int bool_check(const BoolCall &X, const BoolInput &in, BoolChecked *out) {
+    const u32 n_fields = (u32)X.ix.size(), n_nodes = in.n_nodes, n_queries = in.n_queries;
+    const u32 *starts = in.node_clause_starts;
+    const bool occur = in.clause_occur != nullptr, dismax = in.clause_group != nullptr;
     int rc;
-    const bool occur = clause_occur != nullptr, dismax = clause_group != nullptr, nested = clause_node != nullptr;
-    auto is_nested = [&](u32 c) { return nested && clause_node[c] != SA_NO_NODE; };
     SA_CHECK(n_nodes >= n_queries, "n_nodes (%u) is below n_queries (%u)", n_nodes, n_queries);
-    SA_CHECK(n_nodes == 0 || query_clause_starts[0] == 0, "query_clause_starts[0] must be 0");
+    SA_CHECK(n_nodes == 0 || starts[0] == 0, "query_clause_starts[0] must be 0");
     for (u32 q = 0; q < n_nodes; q++) {
-        SA_CHECK(query_clause_starts[q + 1] > query_clause_starts[q] &&
-                 query_clause_starts[q + 1] - query_clause_starts[q] <= SA_BOOL_MAX_CLAUSES,
+        SA_CHECK(starts[q + 1] > starts[q] && starts[q + 1] - starts[q] <= SA_BOOL_MAX_CLAUSES,
                  "query %u: a boolean query has 1 to %d clauses", q, SA_BOOL_MAX_CLAUSES);
-        u32 n_should = query_clause_starts[q + 1] - query_clause_starts[q];
+        u32 n_should = starts[q + 1] - starts[q];
         if (occur) {
             n_should = 0;
-            for (u32 c = query_clause_starts[q]; c < query_clause_starts[q + 1]; c++) {
-                SA_CHECK(clause_occur[c] <= SA_OCCUR_MUST_NOT, "clause %u: occur %u is not an SA_OCCUR_* value", c,
-                         (unsigned)clause_occur[c]);
-                SA_CHECK(std::isfinite(clause_weight[c]) && clause_weight[c] >= 0.0f,
+            for (u32 c = starts[q]; c < starts[q + 1]; c++) {
+                SA_CHECK(in.clause_occur[c] <= SA_OCCUR_MUST_NOT, "clause %u: occur %u is not an SA_OCCUR_* value", c,
+                         (unsigned)in.clause_occur[c]);
+                SA_CHECK(std::isfinite(in.clause_weight[c]) && in.clause_weight[c] >= 0.0f,
                          "clause %u: a weight is finite and >= 0", c);
                 if (dismax) {
                     // a group: consecutive clauses of one query, one occur; its tie at its first clause
-                    const u32 g = clause_group[c];
-                    SA_CHECK(g >= query_clause_starts[q] && g <= c && (g == c || clause_group[c - 1] == g),
+                    const u32 g = in.clause_group[c];
+                    SA_CHECK(g >= starts[q] && g <= c && (g == c || in.clause_group[c - 1] == g),
                              "clause %u: group %u is not a run of consecutive clauses of query %u", c, g, q);
-                    SA_CHECK(clause_occur[c] == clause_occur[g], "clause %u: the members of group %u differ in occur",
-                             c, g);
+                    SA_CHECK(in.clause_occur[c] == in.clause_occur[g],
+                             "clause %u: the members of group %u differ in occur", c, g);
                     if (g == c) {
-                        SA_CHECK(std::isfinite(clause_tie[c]) && clause_tie[c] >= 0.0f && clause_tie[c] <= 1.0f,
+                        SA_CHECK(std::isfinite(in.clause_tie[c]) && in.clause_tie[c] >= 0.0f && in.clause_tie[c] <= 1.0f,
                                  "clause %u: a tie is finite and in [0, 1]", c);
                     } else {
                         continue;   // mm counts groups
                     }
                 }
-                n_should += clause_occur[c] == SA_OCCUR_SHOULD;
+                n_should += in.clause_occur[c] == SA_OCCUR_SHOULD;
             }
         }
-        SA_CHECK(mm[q] <= n_should, "query %u: mm exceeds its %s", q,
+        SA_CHECK(in.mm[q] <= n_should, "query %u: mm exceeds its %s", q,
                  dismax ? "SHOULD groups" : occur ? "SHOULD clauses" : "clauses");
     }
     // nested nodes: each referenced by exactly one clause of an earlier node, as a clause of its own (no terms, not a
     // DisMax member); the top-level nodes by none
-    std::vector<u32> refs(nested ? n_nodes : 0, 0);
-    for (u32 n = 0; nested && n < n_nodes; n++) {
-        for (u32 c = query_clause_starts[n]; c < query_clause_starts[n + 1]; c++) {
-            if (!is_nested(c)) continue;
-            const u32 ch = clause_node[c];
+    std::vector<u32> refs(in.clause_node ? n_nodes : 0, 0);
+    for (u32 n = 0; in.clause_node && n < n_nodes; n++) {
+        for (u32 c = starts[n]; c < starts[n + 1]; c++) {
+            if (!in.nested(c)) continue;
+            const u32 ch = in.clause_node[c];
             SA_CHECK(ch < n_nodes && ch >= n_queries && ch > n,
                      "clause %u: node %u is not a nested node after its holder %u (%u nodes, %u top-level)", c, ch, n,
                      n_nodes, n_queries);
             SA_CHECK(refs[ch]++ == 0, "node %u is referenced by more than one clause", ch);
-            SA_CHECK(clause_term_starts[c + 1] == clause_term_starts[c], "clause %u: a nested clause has no terms", c);
-            SA_CHECK(clause_group[c] == c && (c + 1 == query_clause_starts[n + 1] || clause_group[c + 1] != c),
+            SA_CHECK(in.n_terms(c) == 0, "clause %u: a nested clause has no terms", c);
+            SA_CHECK(in.clause_group[c] == c && (c + 1 == starts[n + 1] || in.clause_group[c + 1] != c),
                      "clause %u: a nested clause is not a DisMax member", c);
         }
     }
-    for (u32 n = n_queries; nested && n < n_nodes; n++) SA_CHECK(refs[n] == 1, "node %u is referenced by no clause", n);
-    if ((rc = sa_where_check(X.where_bits, X.where_n, X.where_stride, lead->n_docs))) return rc;
+    for (u32 n = n_queries; in.clause_node && n < n_nodes; n++)
+        SA_CHECK(refs[n] == 1, "node %u is referenced by no clause", n);
+    if ((rc = sa_where_check(in.where_bits, in.where_n, in.where_stride, X.lead()->n_docs))) return rc;
     // hit and facet counts: each facet a set slot of its field's index
-    const bool counting = X.out_total != nullptr;
-    BoolCount count{};
-    if (counting) {
-        SA_CHECK(X.n_facets <= SA_BOOL_MAX_FACETS, "at most %d facets in one call, not %u", SA_BOOL_MAX_FACETS,
-                 X.n_facets);
-        SA_CHECK(X.n_facets == 0 || (X.facet_field && X.facet_slot && X.out_facet_counts), "NULL argument");
-        for (u32 i = 0; i < X.n_facets; i++) {
-            const u32 f = X.facet_field[i], slot = X.facet_slot[i];
+    BoolCount &count = out->count;
+    if (in.out_total) {
+        SA_CHECK(in.n_facets <= SA_BOOL_MAX_FACETS, "at most %d facets in one call, not %u", SA_BOOL_MAX_FACETS,
+                 in.n_facets);
+        SA_CHECK(in.n_facets == 0 || (in.facet_field && in.facet_slot && in.out_facet_counts), "NULL argument");
+        for (u32 i = 0; i < in.n_facets; i++) {
+            const u32 f = in.facet_field[i], slot = in.facet_slot[i];
             SA_CHECK(f < n_fields, "facet %u: field %u out of range (%u fields)", i, f, n_fields);
             SA_CHECK(slot < SA_MAX_FACETS && (X.ix[f]->facet_set >> slot & 1u), "facet %u: facet slot %u is not set",
                      i, slot);
             count.codes[i] = X.ix[f]->d_facets[slot].as<const unsigned short>();
             count.offset[i + 1] = count.offset[i] + X.ix[f]->facet_buckets[slot];
         }
-        count.n_facets = X.n_facets;
-        count.n_bins = count.offset[X.n_facets];
+        count.n_facets = in.n_facets;
+        count.n_bins = count.offset[in.n_facets];
     }
-    const u32 c_begin = n_nodes ? query_clause_starts[0] : 0, c_end = n_nodes ? query_clause_starts[n_nodes] : 0;
-    bool features = false;
+    const u32 c_begin = n_nodes ? starts[0] : 0, c_end = n_nodes ? starts[n_nodes] : 0;
     for (u32 c = c_begin; c < c_end; c++) {
-        if (is_nested(c)) continue;
-        const u32 nt = clause_term_starts[c + 1] - clause_term_starts[c];
-        SA_CHECK(clause_term_starts[c + 1] > clause_term_starts[c] && nt <= SA_MAX_PHRASE_TERMS,
+        if (in.nested(c)) continue;
+        const u32 nt = in.n_terms(c);
+        SA_CHECK(in.clause_term_starts[c + 1] > in.clause_term_starts[c] && nt <= SA_MAX_PHRASE_TERMS,
                  "clause %u: bad number of terms", c);
-        const u32 f = clause_field ? clause_field[c] : 0;
+        const u32 f = in.field(c);
         SA_CHECK(f < n_fields, "clause %u: field %u out of range (%u fields)", c, f, n_fields);
-        const u32 *tids = clause_terms + clause_term_starts[c];
-        if (nt == 1 && bool_is_feature_term(tids[0])) {
-            if ((rc = bool_check_feature(X.ix[f], c, tids[0], clause_idf[c]))) return rc;
-            SA_CHECK(!dismax || ((c == c_begin || clause_group[c - 1] != clause_group[c]) &&
-                                 (c + 1 == c_end || clause_group[c + 1] != clause_group[c])),
+        const u32 *tids = in.terms(c);
+        if (in.feature(c)) {
+            if ((rc = bool_check_feature(X.ix[f], c, tids[0], in.clause_idf[c]))) return rc;
+            SA_CHECK(!dismax || ((c == c_begin || in.clause_group[c - 1] != in.clause_group[c]) &&
+                                 (c + 1 == c_end || in.clause_group[c + 1] != in.clause_group[c])),
                      "clause %u: a feature clause is not a DisMax member", c);
-            features = true;
+            out->features = true;
             continue;
         }
         for (u32 i = 0; i < nt; i++)
             SA_CHECK(!bool_is_feature_term(tids[i]), "clause %u: a feature term id inside a phrase", c);
         if ((rc = sa_check_term_ids(X.ix[f], tids, nt))) return rc;
     }
-    // an Or / And batch with a feature clause or counts runs as roles and weights, every clause SHOULD with weight 1
-    std::vector<float> ones;
-    std::vector<uint8_t> shoulds;
-    if ((features || counting) && !occur) {
-        ones.assign(c_end, 1.0f);
-        shoulds.assign(c_end, SA_OCCUR_SHOULD);
-        clause_weight = ones.data();
-        clause_occur = shoulds.data();
-    }
-    const bool roles = occur || features || counting;
-    const size_t nk = (size_t)n_queries * k;
-    for (size_t i = 0; i < nk; i++) { out_docs[i] = SA_NO_DOC; out_scores[i] = 0.0f; }
-    const size_t n_bins = count.n_bins;
-    if (counting) {
-        memset(X.out_total, 0, (size_t)n_queries * sizeof(u32));
-        if (n_bins) memset(X.out_facet_counts, 0, (size_t)n_queries * n_bins * sizeof(u32));
-    }
-    // .score is all zeros on a field whose avgdl is 0: its clauses are empty (below), and without any other field
+    // .score is all zeros on a field whose avgdl is 0: its clauses are empty (bool_plan), and without any other field
     // nothing ranks
     bool any_avgdl = false;
     for (u32 f = 0; f < n_fields; f++) any_avgdl = any_avgdl || X.avgdl[f] != 0.0f;
-    if (n_queries == 0 || lead->n_docs == 0 || (!any_avgdl && !features)) return SA_OK;
+    out->empty = n_queries == 0 || X.lead()->n_docs == 0 || (!any_avgdl && !out->features);
+    if (out->empty) return SA_OK;
+    for (u32 n = 0; n < n_nodes; n++) {
+        for (u32 c = starts[n]; c < starts[n + 1]; c++) {
+            const u32 f = in.field(c);
+            if (in.nested(c) || in.feature(c) || X.avgdl[f] == 0.0f) continue;
+            const bool sparse = bool_sparse(X, f, in.clause_idf[c]);
+            SA_CHECK(in.n_terms(c) == 1 || sparse, "phrase queries in a batch need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite idf)");
+            SA_CHECK(!in.member(c, starts[n], starts[n + 1]) || sparse, "clause %u: DisMax members need ordinary BM25 "
+                     "parameters (k1 > 0, 0 <= b < 1, finite idf >= 0)", c);
+        }
+    }
+    return SA_OK;
+}
 
-    // descriptors, and the groups: at most ~1 GB of candidate slots and ~4 GB of phrase rows per launch
-    const u32 n_tiles = sa_n_tiles(lead->n_docs), slots = sa_topk_slots(k);
-    const u64 stride = sa_padded_docs(lead->n_docs);
-    const u32 group_q = (u32)std::min<u64>(65535, std::max<u64>(1, (1ull << 30) / ((u64)n_tiles * (slots * sizeof(u64) + 8))));
-    const u32 group_rows = (u32)std::max<u64>(1, (4ull << 30) / (stride * sizeof(float)));
+// Where the descriptor arrays of P go in BoolState::desc.
+BoolDescs bool_descs(const BoolPlan &P, size_t n_fields) {
+    size_t end = 0;
+    auto section = [&](size_t bytes) {
+        const size_t at = end;
+        end = (at + bytes + 255) & ~(size_t)255;
+        return at;
+    };
+    BoolDescs L;
+    L.clauses = section(P.clauses.size() * sizeof(BoolClause));
+    L.queries = section(P.queries.size() * sizeof(BoolQuery));
+    L.occur = section(P.occur.size() * sizeof(BoolOccur));
+    L.groups = section(P.groups.size() * sizeof(BoolGroup));
+    L.nest = section(P.nest.size() * sizeof(u32));
+    L.fields = section((P.form >= BOOL_FIELDS ? n_fields : 0) * sizeof(BoolField));
+    L.features = section(P.features.size() * sizeof(BoolFeature));
+    L.bytes = end;
+    return L;
+}
+
+// The launches of a checked call and its descriptors, on the host: the form, the launch groups (at most ~1 GB of
+// candidate slots and ~4 GB of phrase rows each), the row numbering and the per-clause arrays.  It makes no CUDA API
+// call and takes no d_norm pointer: bool_upload's sa_ensure_norm may move d_norm.
+BoolPlan bool_plan(const BoolCall &X, const BoolInput &in, const BoolChecked &chk) {
+    const u32 n_nodes = in.n_nodes, n_queries = in.n_queries, n_fields = (u32)X.ix.size();
+    const u32 *starts = in.node_clause_starts;
+    const bool occur = in.clause_occur != nullptr, dismax = in.clause_group != nullptr;
+    // an Or / And batch with a feature clause or counts runs as roles and weights, every clause SHOULD with weight 1
+    const bool roles = occur || chk.features || in.out_total != nullptr;
+    auto role = [&](u32 c) {
+        return occur ? BoolOccur{in.clause_weight[c], in.clause_occur[c]} : BoolOccur{1.0f, SA_OCCUR_SHOULD};
+    };
     BoolPlan P;
-    P.form = nested ? BOOL_NESTED : dismax ? BOOL_DISMAX : X.fields_kernel ? BOOL_FIELDS : roles ? BOOL_OCCUR : BOOL_OR_AND;
-    P.n_top = n_queries;
-    P.node_starts.assign(query_clause_starts, query_clause_starts + n_nodes + 1);
+    const u32 n_tiles = sa_n_tiles(X.lead()->n_docs);
+    P.slots = sa_topk_slots(in.k);
+    const u64 stride = sa_padded_docs(X.lead()->n_docs);
+    const u32 group_q = (u32)std::min<u64>(65535, std::max<u64>(1, (1ull << 30) / ((u64)n_tiles * (P.slots * sizeof(u64) + 8))));
+    const u32 group_rows = (u32)std::max<u64>(1, (4ull << 30) / (stride * sizeof(float)));
+    P.form = in.clause_node ? BOOL_NESTED : dismax ? BOOL_DISMAX : X.fields_kernel ? BOOL_FIELDS : roles ? BOOL_OCCUR : BOOL_OR_AND;
     P.root.resize(n_nodes);
     P.depth.assign(n_nodes, 0);
     // every node's top-level query and depth (references point forward, so a holder is seen before its children), and
@@ -991,14 +1058,13 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
     for (u32 n = 0; n < n_nodes; n++) {
         if (n < n_queries) P.root[n] = n;
         else q_rows[P.root[n]]++;
-        for (u32 c = query_clause_starts[n]; c < query_clause_starts[n + 1]; c++) {
-            if (is_nested(c)) {
-                P.root[clause_node[c]] = P.root[n];
-                P.depth[clause_node[c]] = P.depth[n] + 1;
+        for (u32 c = starts[n]; c < starts[n + 1]; c++) {
+            if (in.nested(c)) {
+                P.root[in.clause_node[c]] = P.root[n];
+                P.depth[in.clause_node[c]] = P.depth[n] + 1;
                 continue;
             }
-            const u32 f = clause_field ? clause_field[c] : 0;
-            q_rows[P.root[n]] += clause_term_starts[c + 1] - clause_term_starts[c] > 1 && X.avgdl[f] != 0.0f;
+            q_rows[P.root[n]] += in.n_terms(c) > 1 && X.avgdl[in.field(c)] != 0.0f;
         }
     }
     P.group_start.push_back(0);
@@ -1011,7 +1077,6 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
         }
         rows += q_rows[q];
         group_of[q] = (u32)P.group_start.size() - 1;
-        P.max_group = std::max(P.max_group, q + 1 - P.group_start.back());
         P.max_rows = std::max(P.max_rows, rows);
     }
     P.group_start.push_back(n_queries);
@@ -1029,152 +1094,160 @@ int bool_topk(BoolCall &X, uint32_t n_nodes, const uint32_t *query_clause_starts
         return P.root[x] < P.root[y];
     });
     P.queries.resize(n_queries);                      // then the nested nodes' descriptors, in P.nested's order
-    std::vector<char> field_sparse(n_fields, 0);      // fields with a sparse-safe clause: their norms are cached
+    P.field_sparse.assign(n_fields, 0);
+    const u32 c_end = n_nodes ? starts[n_nodes] : 0;
     for (u32 q = 0; q < n_nodes; q++) {
-        const u32 c0 = query_clause_starts[q], c1 = query_clause_starts[q + 1];
+        const u32 c0 = starts[q], c1 = starts[q + 1];
         u32 &next_row = g_rows[group_of[P.root[q]]];
-        if (q < n_queries) P.queries[q] = BoolQuery{(u32)P.clauses.size(), c1 - c0, mm[q], 0};
+        if (q < n_queries) P.queries[q] = BoolQuery{(u32)P.clauses.size(), c1 - c0, in.mm[q], 0};
         for (u32 c = c0; c < c1; c++) {
-            if (nested) P.nest.push_back(is_nested(c) ? 1u : 0u);
-            if (is_nested(c)) {             // scored by its child's row, present where the child ranks
-                P.occur.push_back(BoolOccur{clause_weight[c], clause_occur[c]});
+            if (in.clause_node) P.nest.push_back(in.nested(c) ? 1u : 0u);
+            if (in.nested(c)) {             // scored by its child's row, present where the child ranks
+                P.occur.push_back(role(c));
                 P.groups.push_back(BoolGroup{0.0f, c - c0, 0u, 0u});
-                P.clauses.push_back(BoolClause{0, 0, SA_NO_DIR, SA_NO_DIR, 0.0f, node_row[clause_node[c]], 1u, 0u});
+                P.clauses.push_back(BoolClause{0, 0, SA_NO_DIR, SA_NO_DIR, 0.0f, node_row[in.clause_node[c]], 1u, 0u});
                 continue;
             }
-            const u32 f = clause_field ? clause_field[c] : 0;
+            const u32 f = in.field(c);
             sa_index *ix = X.ix[f];
-            const u32 *tids = clause_terms + clause_term_starts[c];
-            const u32 nt = clause_term_starts[c + 1] - clause_term_starts[c];
-            if (roles) P.occur.push_back(BoolOccur{clause_weight[c], clause_occur[c]});
+            const u32 *tids = in.terms(c);
+            const u32 nt = in.n_terms(c);
+            if (roles) P.occur.push_back(role(c));
             // a member of a group of two or more: scores >= +0 everywhere (sparse-safe), which its max relies on
-            const bool member = dismax && ((c > c0 && clause_group[c] == clause_group[c - 1]) ||
-                                           (c + 1 < c1 && clause_group[c + 1] == clause_group[c]));
+            const bool member = in.member(c, c0, c1);
             if (dismax)
-                P.groups.push_back(BoolGroup{clause_tie[clause_group[c]], clause_group[c] - c0, member ? 1u : 0u,
-                                             member && (c + 1 == c1 || clause_group[c + 1] != clause_group[c]) ? 1u : 0u});
-            if (nt == 1 && bool_is_feature_term(tids[0])) {   // its column on its field's index
+                P.groups.push_back(BoolGroup{in.clause_tie[in.clause_group[c]], in.clause_group[c] - c0, member ? 1u : 0u,
+                                             member && (c + 1 == c1 || in.clause_group[c + 1] != in.clause_group[c]) ? 1u : 0u});
+            if (in.feature(c)) {            // its column on its field's index
                 const u32 slot = tids[0] & 0xFFu, fn = (tids[0] >> 8) & 0xFFFFu;
                 P.features.resize(c_end);
                 P.features[P.clauses.size()] = BoolFeature{ix->d_features[slot].as<float>(),
                                                            ix->d_feature_tiles.as<u32>() + (size_t)slot * n_tiles,
-                                                           clause_idf[c], fn};
+                                                           in.clause_idf[c], fn};
                 P.clauses.push_back(BoolClause{0, 0, SA_NO_DIR, SA_NO_DIR, 0.0f, SA_BOOL_FEATURE_ROW, 1u, f});
                 continue;
             }
             if (X.avgdl[f] == 0.0f) {       // scores +0 at every doc: no list, no row
-                P.clauses.push_back(BoolClause{0, 0, SA_NO_DIR, SA_NO_DIR, clause_idf[c], SA_BOOL_NO_ROW, 1u, f});
+                P.clauses.push_back(BoolClause{0, 0, SA_NO_DIR, SA_NO_DIR, in.clause_idf[c], SA_BOOL_NO_ROW, 1u, f});
                 continue;
             }
-            const bool sparse = make_bm25(clause_idf[c], X.avgdl[f], X.k1[f], X.b[f], ix->doc_lens_nonneg).sparse_ok != 0;
-            SA_CHECK(nt == 1 || sparse, "phrase queries in a batch need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite idf)");
-            SA_CHECK(!member || sparse, "clause %u: DisMax members need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, "
-                     "finite idf >= 0)", c);
-            const TermQuery tq = make_term_query(ix, nt == 1 ? tids[0] : SA_NO_TERM, clause_idf[c]);
-            P.clauses.push_back(BoolClause{tq.word_off, tq.n_words, tq.dir_off, tq.rec_off, clause_idf[c],
+            const bool sparse = bool_sparse(X, f, in.clause_idf[c]);   // phrases and members are (bool_check)
+            const TermQuery tq = make_term_query(ix, nt == 1 ? tids[0] : SA_NO_TERM, in.clause_idf[c]);
+            P.clauses.push_back(BoolClause{tq.word_off, tq.n_words, tq.dir_off, tq.rec_off, in.clause_idf[c],
                                            nt == 1 ? SA_BOOL_NO_ROW : next_row++, sparse ? 1u : 0u, f});
-            field_sparse[f] = field_sparse[f] || sparse;
+            P.field_sparse[f] = P.field_sparse[f] || sparse;
         }
     }
     for (u32 n : P.nested)
-        P.queries.push_back(BoolQuery{query_clause_starts[n], query_clause_starts[n + 1] - query_clause_starts[n], mm[n],
-                                      node_row[n]});
+        P.queries.push_back(BoolQuery{starts[n], starts[n + 1] - starts[n], in.mm[n], node_row[n]});
+    P.count = chk.count;
+    P.descs = bool_descs(P, n_fields);
+    P.result = BoolResult{(size_t)n_queries * in.k, n_queries, chk.count.n_bins, in.out_total != nullptr};
+    return P;
+}
 
+// The call's buffers, the norms of its sparse-safe fields, the descriptors in one copy (the field table after the
+// norms: sa_ensure_norm may move d_norm), the mask (*where), the DisMax shared memory, and zeroed flags and counts.
+int bool_upload(const BoolCall &X, const BoolInput &in, const BoolPlan &P, WhereMask *where) {
+    sa_index *lead = X.lead();
     BoolState &S = *X.S;
-    // counting: total[nq] and the facet rows [nq][n_bins] after the overflow flags, zeroed with them
-    const size_t count_bytes = counting ? (size_t)n_queries * (1 + n_bins) * sizeof(u32) : 0;
-    const size_t key_bytes = nk * sizeof(u64) + (size_t)n_queries * sizeof(u32) + count_bytes;
-    if ((rc = S.d_clauses.reserve(P.clauses.size() * sizeof(BoolClause))) ||
-        (rc = S.d_queries.reserve(P.queries.size() * sizeof(BoolQuery))) ||
-        (rc = S.d_out_index.reserve((size_t)n_queries * sizeof(u32))) || (rc = S.d_keys.reserve(key_bytes)) ||
+    const u32 n_fields = (u32)X.ix.size(), n_tiles = sa_n_tiles(lead->n_docs);
+    const u64 stride = sa_padded_docs(lead->n_docs);
+    int rc;
+    if ((rc = S.desc.reserve(P.descs.bytes)) || (rc = S.d_keys.reserve(P.result.bytes())) ||
         (rc = S.rows.reserve(std::max<size_t>((size_t)P.max_rows * stride * sizeof(float), 64))) ||
-        (rc = S.d_occur.reserve(P.occur.size() * sizeof(BoolOccur))) ||
-        (rc = S.d_groups.reserve(P.groups.size() * sizeof(BoolGroup))) ||
-        (rc = S.d_nest.reserve(P.nest.size() * sizeof(u32))) ||
-        (rc = S.d_flags.reserve(nested ? (size_t)P.max_rows * n_tiles * sizeof(u32) : 0)) ||
-        (rc = X.h_pinned->reserve(key_bytes)))
+        (rc = S.d_flags.reserve(P.form == BOOL_NESTED ? (size_t)P.max_rows * n_tiles * sizeof(u32) : 0)) ||
+        (rc = X.h_pinned->reserve(P.result.bytes())))
         return rc;
     for (u32 f = 0; f < n_fields; f++)
-        if (field_sparse[f] && (rc = sa_ensure_norm(X.ix[f], X.k1[f], X.b[f], X.avgdl[f]))) return rc;
+        if (P.field_sparse[f] && (rc = sa_ensure_norm(X.ix[f], X.k1[f], X.b[f], X.avgdl[f]))) return rc;
+    std::vector<char> staged(P.descs.bytes, 0);
+    auto put = [&](size_t at, const auto &v) {
+        if (!v.empty()) memcpy(staged.data() + at, v.data(), v.size() * sizeof(v[0]));
+    };
+    put(P.descs.clauses, P.clauses);
+    put(P.descs.queries, P.queries);
+    put(P.descs.occur, P.occur);
+    put(P.descs.groups, P.groups);
+    put(P.descs.nest, P.nest);
+    put(P.descs.features, P.features);
     if (P.form >= BOOL_FIELDS) {
+        std::vector<BoolField> fields;
         for (u32 f = 0; f < n_fields; f++) {
             sa_index *ix = X.ix[f];
-            P.fields.push_back(BoolField{ix->d_words.as<u64>(), ix->d_tile_dir.as<u32>(), ix->d_recs.as<u32>(),
-                                         ix->d_rec_dir.as<u32>(), ix->d_norm.as<float>(), ix->d_doc_lens.as<float>(),
-                                         make_bm25(1.0f, X.avgdl[f], X.k1[f], X.b[f], ix->doc_lens_nonneg)});
+            fields.push_back(BoolField{ix->d_words.as<u64>(), ix->d_tile_dir.as<u32>(), ix->d_recs.as<u32>(),
+                                       ix->d_rec_dir.as<u32>(), ix->d_norm.as<float>(), ix->d_doc_lens.as<float>(),
+                                       make_bm25(1.0f, X.avgdl[f], X.k1[f], X.b[f], ix->doc_lens_nonneg)});
         }
-        if ((rc = S.d_fields.reserve(P.fields.size() * sizeof(BoolField)))) return rc;
-        SA_CUDA(cudaMemcpyAsync(S.d_fields.p, P.fields.data(), P.fields.size() * sizeof(BoolField), cudaMemcpyHostToDevice,
-                                lead->stream));
+        put(P.descs.fields, fields);
     }
-    std::vector<u32> identity(n_queries);
-    for (u32 q = 0; q < n_queries; q++) identity[q] = q;
-    SA_CUDA(cudaMemcpyAsync(S.d_clauses.p, P.clauses.data(), P.clauses.size() * sizeof(BoolClause), cudaMemcpyHostToDevice, lead->stream));
-    if (roles) {
-        SA_CUDA(cudaMemcpyAsync(S.d_occur.p, P.occur.data(), P.occur.size() * sizeof(BoolOccur), cudaMemcpyHostToDevice, lead->stream));
-    }
-    if (!P.features.empty()) {
-        if ((rc = S.d_feat.reserve(P.features.size() * sizeof(BoolFeature)))) return rc;
-        SA_CUDA(cudaMemcpyAsync(S.d_feat.p, P.features.data(), P.features.size() * sizeof(BoolFeature),
-                                cudaMemcpyHostToDevice, lead->stream));
-    }
-    if ((rc = sa_where_upload(lead, S.d_where, X.where_bits, lead->n_docs, X.where_stride, n_queries, &X.where)))
+    SA_CUDA(cudaMemcpyAsync(S.desc.p, staged.data(), staged.size(), cudaMemcpyHostToDevice, lead->stream));
+    if ((rc = sa_where_upload(lead, S.d_where, in.where_bits, lead->n_docs, in.where_stride, in.n_queries, where)))
         return rc;
-    if (dismax) {
+    if (P.form >= BOOL_DISMAX) {
         // the first pass's variant and that of the store passes and re-runs, each masked only when the call is
-        const BoolVariant first = bool_variant(P, counting), rest = bool_variant(P, false);
-        for (int masked = 0; masked <= (X.where.bits != nullptr); masked++)
+        const BoolVariant first = bool_variant(P, in.out_total != nullptr), rest = bool_variant(P, false);
+        for (int masked = 0; masked <= (where->bits != nullptr); masked++)
             if ((rc = bool_dismax_smem(bool_kernel(P.form, masked, first))) ||
                 (rest != first && (rc = bool_dismax_smem(bool_kernel(P.form, masked, rest)))))
                 return rc;
-        SA_CUDA(cudaMemcpyAsync(S.d_groups.p, P.groups.data(), P.groups.size() * sizeof(BoolGroup), cudaMemcpyHostToDevice, lead->stream));
     }
-    if (nested) {
-        SA_CUDA(cudaMemcpyAsync(S.d_nest.p, P.nest.data(), P.nest.size() * sizeof(u32), cudaMemcpyHostToDevice,
-                                lead->stream));
-    }
-    SA_CUDA(cudaMemcpyAsync(S.d_queries.p, P.queries.data(), P.queries.size() * sizeof(BoolQuery), cudaMemcpyHostToDevice, lead->stream));
-    SA_CUDA(cudaMemcpyAsync(S.d_out_index.p, identity.data(), (size_t)n_queries * sizeof(u32), cudaMemcpyHostToDevice, lead->stream));
-    u32 *d_ovf = (u32 *)(S.d_keys.as<u64>() + nk);
-    SA_CUDA(cudaMemsetAsync(d_ovf, 0, (size_t)n_queries * sizeof(u32) + count_bytes, lead->stream));
-    if (counting) {
-        P.count = count;
-        P.count.total = d_ovf + n_queries;
-        P.count.counts = d_ovf + 2 * (size_t)n_queries;
-    }
-    for (size_t i = 0; i + 1 < P.group_start.size(); i++)
-        if ((rc = bool_run_group(X, P, clause_terms, clause_term_starts, slop, k, slots, P.group_start[i],
-                                 P.group_start[i + 1], counting))) return rc;
+    SA_CUDA(cudaMemsetAsync(P.result.ovf(S.d_keys.p), 0, P.result.bytes() - P.result.n_keys * sizeof(u64),
+                            lead->stream));
+    return SA_OK;
+}
 
-    // keys and overflow flags in one copy and one synchronise; a query whose tile overflowed is re-run alone with a
-    // slot per doc of the tile, which cannot overflow
-    PinnedBuf &h = *X.h_pinned;
-    SA_CUDA(cudaMemcpyAsync(h.p, S.d_keys.p, key_bytes, cudaMemcpyDeviceToHost, lead->stream));
+// The result block in one device-to-host copy and one synchronise: the keys into out_docs / out_scores and the counts
+// into out_total / out_facet_counts.  Then a query whose tile overflowed is re-run alone with a slot per doc of the
+// tile, which cannot overflow, and without counting: its first pass has counted it.
+int bool_collect(const BoolCall &X, const BoolPlan &P, const BoolInput &in, const WhereMask &where) {
+    sa_index *lead = X.lead();
+    const BoolResult &R = P.result;
+    void *d = X.S->d_keys.p, *h = X.h_pinned->p;
+    const u32 nq = in.n_queries, k = in.k;
+    int rc;
+    SA_CUDA(cudaMemcpyAsync(h, d, R.bytes(), cudaMemcpyDeviceToHost, lead->stream));
     SA_CUDA(cudaStreamSynchronize(lead->stream));
-    std::vector<u32> ovf(n_queries);
-    memcpy(ovf.data(), h.as<const u64>() + nk, (size_t)n_queries * sizeof(u32));
-    sa_unpack_keys(h.as<const u64>(), nk, out_docs, out_scores);
-    if (counting) {
-        memcpy(X.out_total, h.as<const u32>() + 2 * nk + n_queries, (size_t)n_queries * sizeof(u32));
-        if (n_bins)
-            memcpy(X.out_facet_counts, h.as<const u32>() + 2 * nk + 2 * (size_t)n_queries,
-                   (size_t)n_queries * n_bins * sizeof(u32));
+    const std::vector<u32> ovf(R.ovf(h), R.ovf(h) + nq);
+    sa_unpack_keys(R.keys(h), R.n_keys, in.out_docs, in.out_scores);
+    if (R.counting) {
+        memcpy(in.out_total, R.total(h), (size_t)nq * sizeof(u32));
+        if (R.n_bins) memcpy(in.out_facet_counts, R.counts(h), (size_t)nq * R.n_bins * sizeof(u32));
     }
-    // a re-run query has been counted by the first pass, so its re-run does not count
     u32 redone = 0;
-    for (u32 q = 0; q < n_queries; q++) {
+    for (u32 q = 0; q < nq; q++) {
         if (!ovf[q]) continue;
-        SA_CUDA(cudaMemsetAsync(d_ovf + q, 0, sizeof(u32), lead->stream));
-        if ((rc = bool_run_group(X, P, clause_terms, clause_term_starts, slop, k, SA_TILE_DOCS, q, q + 1, false)))
-            return rc;
-        SA_CUDA(cudaMemcpyAsync(h.p, S.d_keys.as<u64>() + (size_t)q * k, k * sizeof(u64), cudaMemcpyDeviceToHost,
-                                lead->stream));
+        SA_CUDA(cudaMemsetAsync(R.ovf(d) + q, 0, sizeof(u32), lead->stream));
+        if ((rc = bool_run_group(X, P, in, where, SA_TILE_DOCS, q, q + 1, false))) return rc;
+        SA_CUDA(cudaMemcpyAsync(h, R.keys(d) + (size_t)q * k, k * sizeof(u64), cudaMemcpyDeviceToHost, lead->stream));
         SA_CUDA(cudaStreamSynchronize(lead->stream));
-        sa_unpack_keys(h.as<const u64>(), k, out_docs + (size_t)q * k, out_scores + (size_t)q * k);
+        sa_unpack_keys(R.keys(h), k, in.out_docs + (size_t)q * k, in.out_scores + (size_t)q * k);
         redone++;
     }
-    if (n_redone) *n_redone = redone;
+    if (in.n_redone) *in.n_redone = redone;
     return SA_OK;
+}
+
+// Both entry points, with the call's indexes locked and their device current: the refusals, the outputs filled as
+// for no match, then the plan, its upload, the launch groups and the results.
+int bool_topk(const BoolCall &X, const BoolInput &in) {
+    BoolChecked chk;
+    int rc;
+    if ((rc = bool_check(X, in, &chk))) return rc;
+    const size_t nk = (size_t)in.n_queries * in.k;
+    for (size_t i = 0; i < nk; i++) { in.out_docs[i] = SA_NO_DOC; in.out_scores[i] = 0.0f; }
+    if (in.out_total) {
+        memset(in.out_total, 0, (size_t)in.n_queries * sizeof(u32));
+        if (chk.count.n_bins) memset(in.out_facet_counts, 0, (size_t)in.n_queries * chk.count.n_bins * sizeof(u32));
+    }
+    if (chk.empty) return SA_OK;
+    const BoolPlan P = bool_plan(X, in, chk);
+    WhereMask where;
+    if ((rc = bool_upload(X, in, P, &where))) return rc;
+    for (size_t i = 0; i + 1 < P.group_start.size(); i++)
+        if ((rc = bool_run_group(X, P, in, where, P.slots, P.group_start[i], P.group_start[i + 1],
+                                 in.out_total != nullptr))) return rc;
+    return bool_collect(X, P, in, where);
 }
 
 }  // namespace
@@ -1203,25 +1276,12 @@ extern "C" int sa_score_batch_topk_bool(sa_index *ix, uint32_t n_nodes, const ui
     std::lock_guard<std::mutex> g(ix->mu);
     SA_CUDA(cudaSetDevice(ix->device));
     if (!ix->boolq) ix->boolq.reset(new BoolState());
-    BoolCall X;
-    X.ix = {ix};
-    X.avgdl = {avg_doc_len};
-    X.k1 = {k1};
-    X.b = {b};
-    X.S = ix->boolq.get();
-    X.cand = &ix->cand;
-    X.h_pinned = &ix->h_pinned;
-    X.where_bits = where_bits;
-    X.where_n = where_n;
-    X.where_stride = where_stride;
-    X.n_facets = n_facets;
-    X.facet_field = facet_field;
-    X.facet_slot = facet_slot;
-    X.out_total = out_total;
-    X.out_facet_counts = out_facet_counts;
-    return bool_topk(X, n_nodes, node_clause_starts, clause_node, nullptr, clause_terms, clause_term_starts,
-                     clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
-                     out_docs, out_scores, n_redone);
+    const BoolCall X{{ix}, {avg_doc_len}, {k1}, {b}, false, ix->boolq.get(), &ix->cand, &ix->h_pinned};
+    const BoolInput in{n_nodes, node_clause_starts, clause_node, nullptr, clause_terms, clause_term_starts, clause_idf,
+                       clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k, where_bits,
+                       where_n, where_stride, out_docs, out_scores, n_redone, n_facets, facet_field, facet_slot,
+                       out_total, out_facet_counts};
+    return bool_topk(X, in);
 }
 
 // bool_topk under the multi's lock, with its state and candidate buffer.
@@ -1262,24 +1322,12 @@ extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, uint32_t n_nodes, con
     std::vector<std::unique_ptr<FieldGuard>> guards;
     for (sa_index *ix : distinct) guards.emplace_back(new FieldGuard(ix, m->stream));
     if (!m->boolq) m->boolq.reset(new BoolState());
-    BoolCall X;
-    X.ix = m->fields;
-    X.avgdl.assign(avg_doc_len, avg_doc_len + n_fields);
-    X.k1.assign(k1, k1 + n_fields);
-    X.b.assign(b, b + n_fields);
-    X.fields_kernel = true;
-    X.S = m->boolq.get();
-    X.cand = &m->cand;
-    X.h_pinned = &m->fields[0]->h_pinned;
-    X.where_bits = where_bits;
-    X.where_n = where_n;
-    X.where_stride = where_stride;
-    X.n_facets = n_facets;
-    X.facet_field = facet_field;
-    X.facet_slot = facet_slot;
-    X.out_total = out_total;
-    X.out_facet_counts = out_facet_counts;
-    return bool_topk(X, n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
-                     clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
-                     out_docs, out_scores, n_redone);
+    const BoolCall X{m->fields, std::vector<float>(avg_doc_len, avg_doc_len + n_fields),
+                     std::vector<float>(k1, k1 + n_fields), std::vector<float>(b, b + n_fields), true, m->boolq.get(),
+                     &m->cand, &m->fields[0]->h_pinned};
+    const BoolInput in{n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
+                       clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
+                       where_bits, where_n, where_stride, out_docs, out_scores, n_redone, n_facets, facet_field,
+                       facet_slot, out_total, out_facet_counts};
+    return bool_topk(X, in);
 }
