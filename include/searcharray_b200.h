@@ -310,6 +310,10 @@ typedef struct {
     /* the bool_tile_kernel instances launched (sa_bool.cu, bool_kernel): bit variant * 10 + form * 2 + masked, with
      * form 0 Or / And, 1 roles and weights, 2 fields, 3 DisMax, 4 nested and variant 0 plain, 1 FEATURE, 2 COUNT */
     uint64_t bool_instances;
+    /* the sim_tile_kernel / sim_where_tile_kernel instances launched (sa_view.cu, launch_sim_tiles): bit
+     * 2 * kind + masked, kind the SA_SIM_* value (0 impact, 1 legacy, 2 classic, 3 BM25, also the BM25 batch's phrase
+     * and span re-runs) and masked 1 for sim_where_tile_kernel */
+    uint64_t sim_instances;
 } sa_stats;
 int sa_stats_reset(sa_index *index);
 int sa_stats_get(sa_index *index, sa_stats *out);

@@ -187,6 +187,7 @@ int launch_sim_tiles(sa_index *ix, int kind, const float *counts, const u64 *row
     tm.stop();
     ix->stats.topk_kernel_launches++;
     ix->stats.total_launches++;
+    ix->stats.sim_instances |= 1ull << (2 * kind + (wh.bits ? 1 : 0));
     return SA_OK;
 }
 
