@@ -61,6 +61,8 @@ int sa_device_allocations(uint64_t *live_buffers, uint64_t *live_bytes);
  *   doc_lens     float32 length of every doc in the shard         [n_docs]
  *   doc_base     global id of the shard's first doc; the shard owns [doc_base, doc_base+n_docs)
  *                and every word's doc id must lie in that range (doc-range sharding, sec. 8e)
+ * A word whose block ((w >> 18) & 0x3FFFF) exceeds MAX_POSN / 18 = 14,563 (MAX_POSN = 2^18 - 1, the reference's
+ * per-doc position limit, roaringish.py:86) is SA_ERR_ARG: a doc's term frequency must fit the index's 19-bit counts.
  */
 int sa_index_create(const uint64_t *words, uint64_t n_words,
                     const uint64_t *term_offsets, const uint64_t *term_lengths, uint32_t n_terms,
@@ -405,7 +407,8 @@ int sa_multi_score_batch_topk_bool(sa_multi *multi, uint32_t n_nodes, const uint
 /* ------------------------------------------------- per-op exports (parity tests)
  * Device implementations of the reference's native ops on raw arrays (host in, host out),
  * for kernel-level parity tests against the Cython originals (SURVEY.md section 8b). */
-/* popcount64_reduce (roaringish/popcount.pyx:212-237): returns groups in *n_out */
+/* popcount64_reduce (roaringish/popcount.pyx:212-237): returns groups in *n_out; exact sums rounded once to float32,
+ * docs whose words carry no bits kept with count 0 */
 int sa_op_popcount64_reduce(const uint64_t *words, uint64_t n, int device,
                             uint64_t *keys_out, float *counts_out, uint64_t *n_out);
 /* bm25_score (bm25/bm25.pyx:28-41): in place over all n */
@@ -444,8 +447,13 @@ int sa_op_bigram_freqs(const uint64_t *lhs, uint64_t n_lhs, const uint64_t *rhs,
  *   sa_op_unique                   searcharray/roaringish/unique.pyx:139-145
  *   sa_op_popcount64 / sa_op_popcount_reduce_at / sa_op_key_sum_over   popcount.pyx:120-122, 150-165, 195-204
  *   sa_op_payload_slice / sa_op_as_dense   roaringish_ops.pyx:46-68, 84-98
+ * Inside a run of equal values, merge / sort_merge_counts pair the k-th lhs copy with the k-th rhs copy, as the
+ * reference's two-pointer loop does (drop_duplicates drops the paired rhs copies; counts add over pairs).
  * sa_op_last_staged_ctas: how many CTAs of the calling thread's last intersect-family call took the
- * TMA-staged shared-memory path (the rest searched global memory): a test hook. */
+ * TMA-staged shared-memory path: a test hook.
+ * sa_op_last_path_ctas: the same call's CTAs by path, out[0] staged, out[1] searched global memory, out[2] had an
+ * empty rhs range (no partner possible); summed over the partner passes of the call (keep mode and
+ * intersect_with_adjacents run two). */
 int sa_op_intersect(const uint64_t *lhs, uint64_t n_lhs, const uint64_t *rhs, uint64_t n_rhs,
                     uint64_t mask, int drop_duplicates, int device,
                     uint64_t *lhs_idx_out, uint64_t *rhs_idx_out, uint64_t *n_lhs_out, uint64_t *n_rhs_out);
@@ -470,12 +478,15 @@ int sa_op_payload_slice(const uint64_t *arr, uint64_t n, uint64_t msb_mask, uint
                         uint64_t max_payload, int device, uint64_t *out, uint64_t *n_out);
 int sa_op_as_dense(const uint64_t *indices, const float *values, uint64_t n, uint64_t size, int device, float *out);
 uint64_t sa_op_last_staged_ctas(void);
+void sa_op_last_path_ctas(uint64_t out[3]);
 
 /* ------------------------------------------------------------ index build (8f-4)
  * The numpy half of the reference's index build after tokenisation (searcharray/indexing.py:101-145:
  * stable sort of the (term, doc, posn) triples by term; searcharray/roaringish/roaringish.py:93-142: encode) on
- * the device.  Triples in document order as _gather_tokens emits them (indexing.py:64-98); term ids < n_terms.
- * words_out: room for n_triples words; term_off_out / term_len_out: every term's slice of words_out. */
+ * the device.  Triples in document order as _gather_tokens emits them (indexing.py:64-98).
+ * words_out: room for n_triples words; term_off_out / term_len_out: every term's slice of words_out (terms without
+ * triples: 0, 0).  SA_ERR_ARG before any device work for n_triples >= 2^31, a term id >= n_terms, a doc id >= 2^28
+ * or a position > 18 * 2^18 - 1 (the word's 18-bit block). */
 int sa_op_build_index(const uint32_t *term_ids, const uint32_t *doc_ids, const uint32_t *posns, uint64_t n_triples,
                       uint32_t n_terms, int device, uint64_t *words_out, uint64_t *n_words_out,
                       uint64_t *term_off_out, uint64_t *term_len_out);

@@ -110,6 +110,7 @@ SIGNATURES = {
     "sa_op_payload_slice": (c_int, [P_u64, c_u64, c_u64, c_u64, c_u64, c_int, P_u64, P_u64]),
     "sa_op_as_dense": (c_int, [P_u64, P_f32, c_u64, c_u64, c_int, P_f32]),
     "sa_op_last_staged_ctas": (c_u64, []),
+    "sa_op_last_path_ctas": (None, [P_u64]),
     "sa_op_build_index": (c_int, [P_u32, P_u32, P_u32, c_u64, c_u32, c_int, P_u64, P_u64, P_u64, P_u64]),
 }
 

@@ -79,7 +79,16 @@ extern "C" int sa_op_build_index(const uint32_t *term_ids, const uint32_t *doc_i
     for (u32 t = 0; t < n_terms; t++) { term_off_out[t] = 0; term_len_out[t] = 0; }
     if (n_triples == 0) return SA_OK;
     SA_CHECK(term_ids && doc_ids && posns && words_out, "NULL argument");
-    SA_CHECK(n_triples < (1ull << 32), "too many tokens for one build call (batch them like the reference's batch_size)");
+    // cub's sort counts items in an int
+    SA_CHECK(n_triples < (1ull << 31), "too many tokens for one build call (batch them like the reference's batch_size)");
+    // every triple must fit the word it lands in: a term slot, a 28-bit doc id, an 18-bit block
+    for (u64 i = 0; i < n_triples; i++) {
+        SA_CHECK(term_ids[i] < n_terms, "triple %llu: term id %u >= n_terms %u", (unsigned long long)i, term_ids[i], n_terms);
+        SA_CHECK(doc_ids[i] < (1u << 28), "triple %llu: doc id %u exceeds the 28-bit key space", (unsigned long long)i,
+                 doc_ids[i]);
+        SA_CHECK(posns[i] < SA_LSB_BITS * SA_ONE_BLOCK, "triple %llu: position %u exceeds %llu", (unsigned long long)i,
+                 posns[i], (unsigned long long)(SA_LSB_BITS * SA_ONE_BLOCK - 1));
+    }
     SA_CUDA(cudaSetDevice(device));
     const u64 n = n_triples;
     DevMem m;

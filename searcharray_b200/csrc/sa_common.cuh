@@ -26,6 +26,8 @@ typedef int64_t i64;
 #define SA_MSB_MASK 0x0000000FFFFC0000ull
 #define SA_BIT17 (1ull << 17)
 #define SA_ONE_BLOCK (1ull << SA_LSB_BITS)
+#define SA_MAX_POSN ((1u << 18) - 1)                   // reference roaringish.py:86: positions a doc may hold
+#define SA_MAX_BLOCK (SA_MAX_POSN / SA_LSB_BITS)       // 14,563: the last block a posting word may carry
 
 #define SA_NUM_SMS_FALLBACK 132          // H100 SXM
 
@@ -268,6 +270,12 @@ struct KernelTimer {
     void stop();
 };
 int sa_resolve_timers(sa_index *ix);
+// sa_index_create, or with refuse_past_max_posn == false an index that also accepts words whose block lies past
+// SA_MAX_BLOCK (sa_op_bigram_freqs: the reference's bigram_freqs takes any word; its count never reads a tf record)
+int sa_index_create_blocks(const uint64_t *words, uint64_t n_words,
+                           const uint64_t *term_offsets, const uint64_t *term_lengths, uint32_t n_terms,
+                           const float *doc_lens, uint64_t n_docs, uint64_t doc_base,
+                           int device, bool refuse_past_max_posn, sa_index **index_out);
 
 // ---- device helpers -------------------------------------------------------------------
 #ifdef __CUDACC__

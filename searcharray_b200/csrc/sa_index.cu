@@ -139,10 +139,11 @@ __device__ __forceinline__ void fill_tile_dir(u32 *__restrict__ dir, const u64 *
 }
 
 // docfreq = number of distinct doc ids among a term's words (reference: unique(words >> 36)
-// .size, roaringish/unique.pyx:87-104 via middle_out.py:521-528) = its doc heads.
+// .size, roaringish/unique.pyx:87-104 via middle_out.py:521-528) = its doc heads.  A word whose block lies past
+// MAX_POSN's sets *past_max_posn (one ballot per warp; an atomic only on a violation).
 __global__ void df_kernel(const u64 *__restrict__ words, u64 n_words,
                           const u64 *__restrict__ term_off_sorted, const u32 *__restrict__ term_of_slot,
-                          u32 n_slots, u32 *__restrict__ df) {
+                          u32 n_slots, u32 *__restrict__ df, u32 *__restrict__ past_max_posn) {
     u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     const bool live = i < n_words;
     u32 lo = 0;
@@ -151,6 +152,8 @@ __global__ void df_kernel(const u64 *__restrict__ words, u64 n_words,
         lo = slot_of_word(term_off_sorted, n_slots, i);
         head = is_doc_head(words, i, term_off_sorted[lo]);
     }
+    const bool past = live && ((words[i] >> SA_LSB_BITS) & SA_LSB_MASK) > SA_MAX_BLOCK;
+    if (__ballot_sync(0xffffffffu, past) && (threadIdx.x & 31) == 0) atomicOr(past_max_posn, 1u);
     // a warp's 32 consecutive words almost always belong to one term: one atomic per (warp, term) instead of one
     // per doc head (a billion same-address atomics on a 10M-doc index)
     const unsigned heads = __ballot_sync(0xffffffffu, head);
@@ -242,6 +245,14 @@ extern "C" int sa_index_create(const uint64_t *words, uint64_t n_words,
                                const uint64_t *term_offsets, const uint64_t *term_lengths, uint32_t n_terms,
                                const float *doc_lens, uint64_t n_docs, uint64_t doc_base,
                                int device, sa_index **index_out) {
+    return sa_index_create_blocks(words, n_words, term_offsets, term_lengths, n_terms, doc_lens, n_docs, doc_base,
+                                  device, true, index_out);
+}
+
+int sa_index_create_blocks(const uint64_t *words, uint64_t n_words,
+                           const uint64_t *term_offsets, const uint64_t *term_lengths, uint32_t n_terms,
+                           const float *doc_lens, uint64_t n_docs, uint64_t doc_base,
+                           int device, bool refuse_past_max_posn, sa_index **index_out) {
     SA_CHECK(index_out, "index_out is NULL");
     SA_CHECK(n_words == 0 || words, "words is NULL");
     SA_CHECK(n_terms == 0 || (term_offsets && term_lengths), "term tables are NULL");
@@ -289,6 +300,10 @@ extern "C" int sa_index_create(const uint64_t *words, uint64_t n_words,
         SA_CUDA(cudaMemcpyAsync(ix->d_doc_lens.p, doc_lens, n_docs * sizeof(float), cudaMemcpyHostToDevice, ix->stream));
     if ((rc = ix->d_df.allocate((size_t)(n_terms + 1) * sizeof(u32)))) return rc;
     SA_CUDA(cudaMemsetAsync(ix->d_df.p, 0, (size_t)(n_terms + 1) * sizeof(u32), ix->stream));
+    DevBuf d_past;
+    u32 past_max_posn = 0;
+    if ((rc = d_past.allocate(sizeof(u32)))) return rc;
+    SA_CUDA(cudaMemsetAsync(d_past.p, 0, sizeof(u32), ix->stream));
     ix->device_bytes = (n_words + 1) * sizeof(u64) + (n_docs + 1) * sizeof(float) + (size_t)(n_terms + 1) * 4;
 
     ix->doc_lens_nonneg = true;
@@ -332,10 +347,11 @@ extern "C" int sa_index_create(const uint64_t *words, uint64_t n_words,
         if ((rc = upload_table(d_off, off_sorted)) || (rc = upload_table(d_slot, term_of_slot))) return rc;
         unsigned blocks = (unsigned)((n_words + 255) / 256);
         df_kernel<<<blocks, 256, 0, ix->stream>>>(ix->d_words.as<u64>(), n_words, d_off.as<u64>(), d_slot.as<u32>(), n_slots,
-                                                  ix->d_df.as<u32>());
+                                                  ix->d_df.as<u32>(), d_past.as<u32>());
         SA_CUDA(cudaGetLastError());
         ix->stats.total_launches++;
         SA_CUDA(cudaMemcpyAsync(ix->h_df.data(), ix->d_df.p, n_terms * sizeof(u32), cudaMemcpyDeviceToHost, ix->stream));
+        SA_CUDA(cudaMemcpyAsync(&past_max_posn, d_past.p, sizeof(u32), cudaMemcpyDeviceToHost, ix->stream));
         if (dir_words) {
             if ((rc = ix->d_tile_dir.allocate(dir_words * sizeof(u32)))) return rc;
             ix->device_bytes += dir_words * sizeof(u32);
@@ -347,6 +363,10 @@ extern "C" int sa_index_create(const uint64_t *words, uint64_t n_words,
             ix->stats.total_launches++;
         }
         SA_CUDA(cudaStreamSynchronize(ix->stream));         // h_df is final from here on
+        // a block past MAX_POSN's would carry a doc's tf past the 19 bits of its record (and of the words path's count)
+        SA_CHECK(!(refuse_past_max_posn && past_max_posn),
+                 "posting words hold positions past MAX_POSN = %u (block > %u): the index counts at most %u positions per doc",
+                 SA_MAX_POSN, SA_MAX_BLOCK, SA_MAX_POSN + 1);
         // tf table for the terms that have a directory (the long lists: that is where the scan's time goes)
         static const bool no_tf_table = getenv("SA_NO_TF_TABLE") && atoi(getenv("SA_NO_TF_TABLE")) != 0;
         ix->h_rec_off.assign(n_terms, SA_NO_DIR);

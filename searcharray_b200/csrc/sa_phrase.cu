@@ -1025,7 +1025,8 @@ extern "C" int sa_op_bigram_freqs(const uint64_t *lhs, uint64_t n_lhs, const uin
     std::vector<float> dl(max_doc + 1, 1.0f);
     u64 offs[2] = {0, n_lhs}, lens[2] = {n_lhs, n_rhs};
     sa_index *created = nullptr;
-    int rc = sa_index_create(words.data(), words.size(), offs, lens, 2, dl.data(), max_doc + 1, 0, device, &created);
+    int rc = sa_index_create_blocks(words.data(), words.size(), offs, lens, 2, dl.data(), max_doc + 1, 0, device, false,
+                                    &created);
     if (rc) return rc;
     std::unique_ptr<sa_index> ix(created);
     std::lock_guard<std::mutex> g(ix->mu);
@@ -1063,32 +1064,7 @@ extern "C" int sa_op_bigram_freqs(const uint64_t *lhs, uint64_t n_lhs, const uin
     return SA_OK;
 }
 
-// popcount64_reduce / as_dense / bm25_score on raw arrays: the term kernel on a one-term index
-extern "C" int sa_op_popcount64_reduce(const uint64_t *words, uint64_t n, int device,
-                                       uint64_t *keys_out, float *counts_out, uint64_t *n_out) {
-    SA_CHECK(keys_out && counts_out && n_out, "NULL argument");
-    *n_out = 0;
-    if (n == 0) return SA_OK;
-    SA_CHECK(words, "NULL argument");
-    u64 min_doc = words[0] >> SA_KEY_SHIFT, max_doc = words[n - 1] >> SA_KEY_SHIFT;
-    u64 nd = max_doc - min_doc + 1;
-    std::vector<float> dl(nd, 1.0f), tf(nd);
-    u64 off = 0, len = n;
-    sa_index *created = nullptr;
-    int rc = sa_index_create(words, n, &off, &len, 1, dl.data(), nd, min_doc, device, &created);
-    if (rc) return rc;
-    std::unique_ptr<sa_index> ix(created);
-    if ((rc = sa_termfreqs(ix.get(), 0, 0, SA_ALL_BITS, tf.data()))) return rc;
-    // docs present in the list keep their (possibly zero) count: walk the keys on the host
-    u64 m = 0, last = ~0ull;
-    for (u64 i = 0; i < n; i++) {
-        u64 d = words[i] >> SA_KEY_SHIFT;
-        if (d != last) { keys_out[m] = d; counts_out[m] = tf[d - min_doc]; m++; last = d; }
-    }
-    *n_out = m;
-    return SA_OK;
-}
-
+// bm25_score on a raw array
 extern "C" int sa_op_bm25_score(float *tf_inout, const float *doc_lens, uint64_t n, float avg_doc_len,
                                 float idf, float k1, float b, int device) {
     if (n == 0) return SA_OK;

@@ -35,7 +35,8 @@
 #define SO_STAGE_WORDS 4096            // rhs words staged per round (32 KB)
 #define SO_NONE 0xFFFFFFFFFFFFFFFFull
 
-static thread_local uint64_t g_last_staged = 0;
+// CTAs of the calling thread's last intersect-family call, by path: staged, global search, empty partner range
+static thread_local uint64_t g_last_paths[3] = {0, 0, 0};
 
 #define SO_ALLOC_CHECK(p)                                              \
     do {                                                               \
@@ -116,7 +117,7 @@ __device__ __forceinline__ u64 warp_lower_bound_masked(const u64 *__restrict__ a
 // add == 0: intersect (intersect.pyx:32-128); add == lowest set bit of mask: adjacent (:131-190, :213-275).
 __global__ void __launch_bounds__(SO_THREADS)
 partner_kernel(const u64 *__restrict__ lhs, u64 nl, const u64 *__restrict__ rhs, u64 nr, u64 mask, u64 add,
-               u64 *__restrict__ pos_out, u32 *__restrict__ first_out, u32 *__restrict__ n_staged_ctas) {
+               u64 *__restrict__ pos_out, u32 *__restrict__ first_out, u32 *__restrict__ n_path_ctas /*[3]*/) {
     __shared__ __align__(16) u64 s_blk[SO_STAGE_WORDS + 4];
     __shared__ __align__(8) u64 s_bar;
     __shared__ u64 s_r[2];
@@ -155,10 +156,13 @@ partner_kernel(const u64 *__restrict__ lhs, u64 nl, const u64 *__restrict__ rhs,
     }
     __syncthreads();
     const u64 r0 = s_r[0], r1 = max(s_r[1], s_r[0]);
-    if (r1 == r0) goto done;
+    if (r1 == r0) {
+        if (tid == 0) atomicAdd(n_path_ctas + 2, 1u);
+        goto done;
+    }
     if (r1 - r0 <= 8ull * SO_TILE) {
         // ---- staged: the rhs range passes through shared memory in TMA-copied blocks
-        if (tid == 0) atomicAdd(n_staged_ctas, 1u);
+        if (tid == 0) atomicAdd(n_path_ctas + 0, 1u);
         u32 phase = 0;
         for (u64 b0 = r0; b0 < r1; b0 += SO_STAGE_WORDS) {
             const u32 nb = (u32)min((u64)SO_STAGE_WORDS, r1 - b0);
@@ -186,6 +190,7 @@ partner_kernel(const u64 *__restrict__ lhs, u64 nl, const u64 *__restrict__ rhs,
         }
     } else {
         // ---- skewed (|lhs tile| << |rhs range|): search global memory, touching only the probed sectors
+        if (tid == 0) atomicAdd(n_path_ctas + 1, 1u);
 #pragma unroll
         for (int e = 0; e < SO_ITEMS; e++) {
             if (!live[e]) continue;
@@ -221,14 +226,17 @@ __global__ void pair_write_kernel(const u64 *__restrict__ pos, const u32 *__rest
 }
 
 // One (lhs -> rhs) partner pass; results compacted to the host.  out_partner may be NULL (membership only).
-int run_partner(DevMem &m, const u64 *d_lhs, u64 nl, const u64 *d_rhs, u64 nr, u64 mask, u64 add, int need_first,
-                u64 *h_idx, u64 *h_partner, u64 *n_out) {
+// need_first (one pair per masked value) follows the reference's drop loops, which start `last` at all ones
+// (intersect.pyx:40,145,224): a pair whose masked value equals the mask is skipped while no pair precedes it.  That
+// value is the largest there is, so this drops it exactly when it is the only pair.
+int run_partner(DevMem &m, const u64 *h_lhs, const u64 *d_lhs, u64 nl, const u64 *d_rhs, u64 nr, u64 mask, u64 add,
+                int need_first, u64 *h_idx, u64 *h_partner, u64 *n_out) {
     *n_out = 0;
     if (nl == 0 || nr == 0) return SA_OK;
     u64 *d_pos = m.alloc<u64>(nl);
-    u32 *d_first = m.alloc<u32>(nl), *d_flag = m.alloc<u32>(nl), *d_offs = m.alloc<u32>(nl), *d_cnt = m.alloc<u32>(1);
+    u32 *d_first = m.alloc<u32>(nl), *d_flag = m.alloc<u32>(nl), *d_offs = m.alloc<u32>(nl), *d_cnt = m.alloc<u32>(3);
     SO_ALLOC_CHECK(d_pos && d_first && d_flag && d_offs && d_cnt);
-    cudaMemset(d_cnt, 0, sizeof(u32));
+    SA_CUDA(cudaMemset(d_cnt, 0, 3 * sizeof(u32)));
     const unsigned tiles = (unsigned)((nl + SO_TILE - 1) / SO_TILE), blocks = (unsigned)((nl + 255) / 256);
     partner_kernel<<<tiles, SO_THREADS>>>(d_lhs, nl, d_rhs, nr, mask, add, d_pos, d_first, d_cnt);
     pair_flag_kernel<<<blocks, 256>>>(d_pos, d_first, nl, need_first, d_flag);
@@ -244,48 +252,60 @@ int run_partner(DevMem &m, const u64 *d_lhs, u64 nl, const u64 *d_rhs, u64 nr, u
         SA_CUDA(cudaMemcpy(h_idx, d_oi, total * sizeof(u64), cudaMemcpyDeviceToHost));
         if (h_partner) SA_CUDA(cudaMemcpy(h_partner, d_op, total * sizeof(u64), cudaMemcpyDeviceToHost));
     }
-    u32 staged = 0;
-    SA_CUDA(cudaMemcpy(&staged, d_cnt, sizeof(u32), cudaMemcpyDeviceToHost));
-    g_last_staged += staged;
+    u32 paths[3];
+    SA_CUDA(cudaMemcpy(paths, d_cnt, sizeof(paths), cudaMemcpyDeviceToHost));
+    for (int k = 0; k < 3; k++) g_last_paths[k] += paths[k];
+    if (need_first && total == 1 && (h_lhs[h_idx[0]] & mask) == mask) total = 0;
     *n_out = total;
     return SA_OK;
 }
 
 // ------------------------------------------------------------------ ranks (merge-path)
-// rank[i] = number of b elements < a[i] (upper == 0) or <= a[i] (upper == 1); hit[i] = a[i] occurs in b
+#define SO_UNPAIRED 0xFFFFFFFFu
+
+__device__ __forceinline__ u64 bound(const u64 *__restrict__ a, u64 lo, u64 hi, u64 x, bool upper) {
+    while (lo < hi) {
+        const u64 mid = (lo + hi) >> 1;
+        const u64 y = __ldg(a + mid);
+        if (upper ? (y <= x) : (y < x)) lo = mid + 1; else hi = mid;
+    }
+    return lo;
+}
+
+// rank[i] = number of b elements < a[i] (upper == 0) or <= a[i] (upper == 1).  The reference's two-pointer merge
+// pairs the k-th copy of a value in a with the k-th copy in b (merge.pyx:64-77): pair[i] = the index in b of a[i]'s
+// partner, or SO_UNPAIRED when b holds fewer copies of the value than come up to a[i] in a.
 __global__ void rank_kernel(const u64 *__restrict__ a, u64 na, const u64 *__restrict__ b, u64 nb, int upper,
-                            u32 *__restrict__ rank, u32 *__restrict__ hit) {
+                            u32 *__restrict__ rank, u32 *__restrict__ pair) {
     const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= na) return;
     const u64 x = a[i];
-    u64 lo = 0, hi = nb;
-    while (lo < hi) {
-        const u64 mid = (lo + hi) >> 1;
-        const u64 y = __ldg(b + mid);
-        if (upper ? (y <= x) : (y < x)) lo = mid + 1; else hi = mid;
-    }
-    rank[i] = (u32)lo;
-    if (hit) hit[i] = upper ? ((lo > 0 && __ldg(b + lo - 1) == x) ? 1u : 0u) : ((lo < nb && __ldg(b + lo) == x) ? 1u : 0u);
+    const u64 lo = bound(b, 0, nb, x, false), hi = bound(b, lo, nb, x, true);
+    rank[i] = (u32)(upper ? hi : lo);
+    const u64 p = lo + (i - bound(a, 0, i, x, false));               // a[i] is copy number i - first of its value
+    pair[i] = p < hi ? (u32)p : SO_UNPAIRED;
 }
 
-__global__ void invert_kernel(const u32 *__restrict__ in, u32 *__restrict__ out, u64 n) {
+__global__ void unpaired_kernel(const u32 *__restrict__ pair, u32 *__restrict__ out, u64 n) {
     const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = in[i] ? 0u : 1u;
+    if (i < n) out[i] = pair[i] == SO_UNPAIRED ? 1u : 0u;
 }
 
-// merged[i + kept_before(rank_l[i])] = lhs[i];  merged[kept_before(j) + rank_r[j]] = rhs[j] (kept rhs only)
+// merged[i + kept_before(rank_l[i])] = lhs[i];  merged[kept_before(j) + rank_r[j]] = rhs[j] (kept rhs only).  Inside
+// a run of equal values the lhs copies come first, the paired ones first among them, then the kept rhs copies: the
+// order the reference's merge writes them in.
 __global__ void merge_write_kernel(const u64 *__restrict__ lhs, u64 nl, const u64 *__restrict__ rhs, u64 nr,
                                    const u32 *__restrict__ rank_l, const u32 *__restrict__ rank_r,
                                    const u32 *__restrict__ keep_r, const u32 *__restrict__ kept_before /*[nr + 1]*/,
                                    const float *__restrict__ lcnt, const float *__restrict__ rcnt,
-                                   const u32 *__restrict__ hit_l,
+                                   const u32 *__restrict__ pair_l,
                                    u64 *__restrict__ out, float *__restrict__ out_cnt) {
     const u64 i = (u64)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < nl) {
         const u32 r = rank_l[i];
         const u64 at = i + (kept_before ? kept_before[r] : r);
         out[at] = lhs[i];
-        if (out_cnt) out_cnt[at] = (hit_l && hit_l[i]) ? __fadd_rn(lcnt[i], rcnt[r]) : lcnt[i];
+        if (out_cnt) out_cnt[at] = (pair_l && pair_l[i] != SO_UNPAIRED) ? __fadd_rn(lcnt[i], rcnt[pair_l[i]]) : lcnt[i];
     } else if (i < nl + nr) {
         const u64 j = i - nl;
         if (keep_r && !keep_r[j]) return;
@@ -364,7 +384,7 @@ extern "C" int sa_op_intersect(const uint64_t *lhs, uint64_t n_lhs, const uint64
                                uint64_t *n_lhs_out, uint64_t *n_rhs_out) {
     SA_CHECK(lhs_idx_out && rhs_idx_out && n_lhs_out && n_rhs_out, "NULL argument");
     SA_CHECK(mask != 0, "Mask cannot be zero");                       // intersect.pyx:291-292 (ValueError)
-    g_last_staged = 0;
+    g_last_paths[0] = g_last_paths[1] = g_last_paths[2] = 0;
     *n_lhs_out = *n_rhs_out = 0;
     if (n_lhs == 0 || n_rhs == 0) return SA_OK;
     SA_CHECK(lhs && rhs, "NULL argument");
@@ -375,13 +395,13 @@ extern "C" int sa_op_intersect(const uint64_t *lhs, uint64_t n_lhs, const uint64
     int rc;
     if (drop_duplicates) {
         // one pair per distinct common masked value: first occurrence on both sides (intersect.pyx:32-74)
-        if ((rc = run_partner(m, d_l, n_lhs, d_r, n_rhs, mask, 0, 1, lhs_idx_out, rhs_idx_out, n_lhs_out))) return rc;
+        if ((rc = run_partner(m, lhs, d_l, n_lhs, d_r, n_rhs, mask, 0, 1, lhs_idx_out, rhs_idx_out, n_lhs_out))) return rc;
         *n_rhs_out = *n_lhs_out;
         return SA_OK;
     }
     // keep: every lhs index whose value occurs in rhs, every rhs index whose value occurs in lhs (:77-128)
-    if ((rc = run_partner(m, d_l, n_lhs, d_r, n_rhs, mask, 0, 0, lhs_idx_out, nullptr, n_lhs_out))) return rc;
-    return run_partner(m, d_r, n_rhs, d_l, n_lhs, mask, 0, 0, rhs_idx_out, nullptr, n_rhs_out);
+    if ((rc = run_partner(m, lhs, d_l, n_lhs, d_r, n_rhs, mask, 0, 0, lhs_idx_out, nullptr, n_lhs_out))) return rc;
+    return run_partner(m, rhs, d_r, n_rhs, d_l, n_lhs, mask, 0, 0, rhs_idx_out, nullptr, n_rhs_out);
 }
 
 extern "C" int sa_op_adjacent(const uint64_t *lhs, uint64_t n_lhs, const uint64_t *rhs, uint64_t n_rhs,
@@ -389,7 +409,7 @@ extern "C" int sa_op_adjacent(const uint64_t *lhs, uint64_t n_lhs, const uint64_
                               uint64_t *n_out) {
     SA_CHECK(lhs_idx_out && rhs_idx_out && n_out, "NULL argument");
     SA_CHECK(mask != 0, "Mask cannot be zero");
-    g_last_staged = 0;
+    g_last_paths[0] = g_last_paths[1] = g_last_paths[2] = 0;
     *n_out = 0;
     if (n_lhs == 0 || n_rhs == 0) return SA_OK;
     SA_CHECK(lhs && rhs, "NULL argument");
@@ -398,7 +418,7 @@ extern "C" int sa_op_adjacent(const uint64_t *lhs, uint64_t n_lhs, const uint64_
     u64 *d_l = m.upload(lhs, n_lhs), *d_r = m.upload(rhs, n_rhs);
     SO_ALLOC_CHECK(d_l && d_r);
     const u64 delta = mask & (~mask + 1);                            // lowest set bit (intersect.pyx:140)
-    return run_partner(m, d_l, n_lhs, d_r, n_rhs, mask, delta, 1, lhs_idx_out, rhs_idx_out, n_out);
+    return run_partner(m, lhs, d_l, n_lhs, d_r, n_rhs, mask, delta, 1, lhs_idx_out, rhs_idx_out, n_out);
 }
 
 extern "C" int sa_op_intersect_with_adjacents(const uint64_t *lhs, uint64_t n_lhs, const uint64_t *rhs, uint64_t n_rhs,
@@ -407,7 +427,7 @@ extern "C" int sa_op_intersect_with_adjacents(const uint64_t *lhs, uint64_t n_lh
                                               uint64_t *adj_lhs_idx_out, uint64_t *adj_rhs_idx_out, uint64_t *n_adj_out) {
     SA_CHECK(lhs_idx_out && rhs_idx_out && n_out && adj_lhs_idx_out && adj_rhs_idx_out && n_adj_out, "NULL argument");
     SA_CHECK(mask != 0, "Mask cannot be zero");
-    g_last_staged = 0;
+    g_last_paths[0] = g_last_paths[1] = g_last_paths[2] = 0;
     *n_out = *n_adj_out = 0;
     if (n_lhs == 0 || n_rhs == 0) return SA_OK;
     SA_CHECK(lhs && rhs, "NULL argument");
@@ -416,12 +436,13 @@ extern "C" int sa_op_intersect_with_adjacents(const uint64_t *lhs, uint64_t n_lh
     u64 *d_l = m.upload(lhs, n_lhs), *d_r = m.upload(rhs, n_rhs);
     SO_ALLOC_CHECK(d_l && d_r);
     const u64 delta = mask & (~mask + 1);
-    int rc = run_partner(m, d_l, n_lhs, d_r, n_rhs, mask, 0, 1, lhs_idx_out, rhs_idx_out, n_out);
+    int rc = run_partner(m, lhs, d_l, n_lhs, d_r, n_rhs, mask, 0, 1, lhs_idx_out, rhs_idx_out, n_out);
     if (rc) return rc;
-    return run_partner(m, d_l, n_lhs, d_r, n_rhs, mask, delta, 1, adj_lhs_idx_out, adj_rhs_idx_out, n_adj_out);
+    return run_partner(m, lhs, d_l, n_lhs, d_r, n_rhs, mask, delta, 1, adj_lhs_idx_out, adj_rhs_idx_out, n_adj_out);
 }
 
-// merge.pyx:54-158: sorted two-way merge; an element present in both lists appears twice unless drop_duplicates
+// merge.pyx:54-158: sorted two-way merge; an element present in both lists appears twice unless drop_duplicates,
+// which drops the rhs copies paired with an lhs copy
 static int merge_common(const u64 *lhs, u64 nl, const u64 *rhs, u64 nr, int drop, const float *lcnt, const float *rcnt,
                         int device, u64 *out, float *out_cnt, u64 *n_out) {
     *n_out = 0;
@@ -431,10 +452,10 @@ static int merge_common(const u64 *lhs, u64 nl, const u64 *rhs, u64 nr, int drop
     DevMem m;
     u64 *d_l = m.upload(lhs, nl), *d_r = m.upload(rhs, nr);
     float *d_lc = lcnt ? m.upload(lcnt, nl) : nullptr, *d_rc = rcnt ? m.upload(rcnt, nr) : nullptr;
-    u32 *rank_l = m.alloc<u32>(nl), *hit_l = m.alloc<u32>(nl), *rank_r = m.alloc<u32>(nr), *hit_r = m.alloc<u32>(nr);
-    SO_ALLOC_CHECK(d_l && d_r && rank_l && hit_l && rank_r && hit_r && (!lcnt || (d_lc && d_rc)));
-    if (nl) rank_kernel<<<blocks_for(nl), 256>>>(d_l, nl, d_r, nr, 0, rank_l, hit_l);          // # rhs <  lhs[i]
-    if (nr) rank_kernel<<<blocks_for(nr), 256>>>(d_r, nr, d_l, nl, 1, rank_r, hit_r);          // # lhs <= rhs[j]
+    u32 *rank_l = m.alloc<u32>(nl), *pair_l = m.alloc<u32>(nl), *rank_r = m.alloc<u32>(nr), *pair_r = m.alloc<u32>(nr);
+    SO_ALLOC_CHECK(d_l && d_r && rank_l && pair_l && rank_r && pair_r && (!lcnt || (d_lc && d_rc)));
+    if (nl) rank_kernel<<<blocks_for(nl), 256>>>(d_l, nl, d_r, nr, 0, rank_l, pair_l);         // # rhs <  lhs[i]
+    if (nr) rank_kernel<<<blocks_for(nr), 256>>>(d_r, nr, d_l, nl, 1, rank_r, pair_r);         // # lhs <= rhs[j]
     SA_CUDA(cudaGetLastError());
     u32 *keep_r = nullptr, *kept_before = nullptr;
     u64 kept = nr;
@@ -442,7 +463,7 @@ static int merge_common(const u64 *lhs, u64 nl, const u64 *rhs, u64 nr, int drop
         keep_r = m.alloc<u32>(nr);
         kept_before = m.alloc<u32>(nr + 1);
         SO_ALLOC_CHECK(keep_r && kept_before);
-        invert_kernel<<<blocks_for(nr), 256>>>(hit_r, keep_r, nr);
+        unpaired_kernel<<<blocks_for(nr), 256>>>(pair_r, keep_r, nr);
         int rc = scan_flags(m, keep_r, kept_before, nr, &kept, 0);
         if (rc) return rc;
         const u32 k32 = (u32)kept;
@@ -453,7 +474,7 @@ static int merge_common(const u64 *lhs, u64 nl, const u64 *rhs, u64 nr, int drop
     float *d_oc = out_cnt ? m.alloc<float>(total) : nullptr;
     SO_ALLOC_CHECK(d_out && (d_oc || !out_cnt));
     merge_write_kernel<<<blocks_for(nl + nr), 256>>>(d_l, nl, d_r, nr, rank_l, rank_r, keep_r, kept_before, d_lc, d_rc,
-                                                     out_cnt ? hit_l : nullptr, d_out, d_oc);
+                                                     out_cnt ? pair_l : nullptr, d_out, d_oc);
     SA_CUDA(cudaGetLastError());
     SA_CUDA(cudaMemcpy(out, d_out, total * sizeof(u64), cudaMemcpyDeviceToHost));
     if (out_cnt) SA_CUDA(cudaMemcpy(out_cnt, d_oc, total * sizeof(float), cudaMemcpyDeviceToHost));
@@ -554,6 +575,20 @@ extern "C" int sa_op_key_sum_over(const uint64_t *ids, const uint64_t *counts, u
     return grouped(ids, counts, n, 0, device, ids_out, counts_out, n_out);
 }
 
+// popcount.pyx:212-237,271-278 (popcount64_reduce with key_shift 36, value_mask 0x3FFFF): grouped() over (doc id,
+// position bits).  The sum per doc is exact in 64 bits and rounded to float32 once, as the reference's `(float)acc`;
+// a doc's count is not bounded by the 19-bit tf of the index's records (up to 18 * 2^18 positions per doc).
+extern "C" int sa_op_popcount64_reduce(const uint64_t *words, uint64_t n, int device,
+                                       uint64_t *keys_out, float *counts_out, uint64_t *n_out) {
+    SA_CHECK(keys_out && counts_out && n_out && (words || !n), "NULL argument");
+    std::vector<u64> docs(n), bits(n);
+    for (u64 i = 0; i < n; i++) {
+        docs[i] = words[i] >> SA_KEY_SHIFT;
+        bits[i] = words[i] & SA_LSB_MASK;
+    }
+    return grouped(docs.data(), bits.data(), n, 1, device, keys_out, counts_out, n_out);
+}
+
 extern "C" int sa_op_payload_slice(const uint64_t *arr, uint64_t n, uint64_t msb_mask, uint64_t min_payload,
                                    uint64_t max_payload, int device, uint64_t *out, uint64_t *n_out) {
     SA_CHECK(out && n_out && (arr || !n), "NULL argument");
@@ -600,4 +635,9 @@ extern "C" int sa_op_as_dense(const uint64_t *indices, const float *values, uint
 }
 
 // how many CTAs of this thread's last intersect-family call took the TMA-staged path (test hook)
-extern "C" uint64_t sa_op_last_staged_ctas(void) { return g_last_staged; }
+extern "C" uint64_t sa_op_last_staged_ctas(void) { return g_last_paths[0]; }
+
+// ... and how many took each path: staged, global search, empty partner range (test hook)
+extern "C" void sa_op_last_path_ctas(uint64_t out[3]) {
+    for (int k = 0; k < 3; k++) out[k] = g_last_paths[k];
+}

@@ -186,3 +186,10 @@ def as_dense(indices, values, size, device=0):
 
 def last_staged_ctas():
     return int(_lib.lib().sa_op_last_staged_ctas())
+
+
+def last_path_ctas():
+    """CTAs of this thread's last intersect-family call by path: (TMA-staged, global search, empty rhs range)."""
+    out = np.zeros(3, dtype=np.uint64)
+    _lib.lib().sa_op_last_path_ctas(_lib.p_u64(out))
+    return tuple(int(x) for x in out)
