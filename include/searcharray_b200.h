@@ -74,6 +74,12 @@ int sa_index_destroy(sa_index *index);
  * was page-locked in place with cudaHostRegister and DMA'd at PCIe rate, 2 = pipelined through pinned bounce
  * buffers because the range could not be registered. */
 int sa_index_upload_mode(const sa_index *index, int *mode_out);
+/* 1 when the last batch of sa_batch_upload / sa_score_batch_topk wrote its rare terms' dense rows (df < n_docs / 300)
+ * to compressible device memory.  The L2 then compresses their all-zero lines on the way to DRAM, and those terms
+ * are scanned in a launch of their own.  0 when no batch has had rare terms yet, or when every row is in plain
+ * cudaMalloc memory: the device has no compression support, the driver does not grant it, or the process started
+ * with SA_DENSE_PLAIN=1.  The results are the same bits either way. */
+int sa_index_dense_compressible(const sa_index *index, int *compressible_out);
 int sa_index_info(const sa_index *index, uint64_t *n_docs, uint64_t *n_words,
                   uint32_t *n_terms, uint64_t *device_bytes);
 

@@ -42,6 +42,7 @@ SIGNATURES = {
                                 ctypes.POINTER(P_void)]),
     "sa_index_destroy": (c_int, [P_void]),
     "sa_index_upload_mode": (c_int, [P_void, ctypes.POINTER(c_int)]),
+    "sa_index_dense_compressible": (c_int, [P_void, ctypes.POINTER(c_int)]),
     "sa_index_info": (c_int, [P_void, P_u64, P_u64, P_u32, P_u64]),
     "sa_docfreq": (c_int, [P_void, c_u32, P_u64]),
     "sa_index_set_rows": (c_int, [P_void, P_u64, c_u64]),

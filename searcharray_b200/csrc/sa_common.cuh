@@ -52,7 +52,7 @@ void sa_set_error(const char *fmt, ...);
     } while (0)
 
 // ---- owned memory ---------------------------------------------------------------------
-// Every cudaMalloc / cudaHostAlloc of the library is made by a Buffer (apart from sa_host_alloc's, which hands its
+// Every cudaMalloc / cuMemCreate / cudaHostAlloc of the library is made by a Buffer (apart from sa_host_alloc's, which hands its
 // memory to the caller), and the Buffer frees it when its owner goes away, on every return path.  A device buffer is
 // destroyed while its device is current: ~sa_index and ~sa_multi set the device first, and locals live inside calls
 // that have set it.
@@ -76,6 +76,20 @@ struct PinnedSpace {
     static constexpr const char *name = "cudaHostAlloc";
     static cudaError_t alloc(void **p, size_t bytes) { return cudaHostAlloc(p, bytes, cudaHostAllocDefault); }
     static void free(void *p, size_t) { cudaFreeHost(p); }
+};
+
+// Device memory the L2 may compress on its way to DRAM (Hopper's generic compute data compression): the term batch's
+// rows of rare terms, almost all of whose 128-byte lines are zero.  cuMemCreate with
+// CU_MEM_ALLOCATION_COMP_GENERIC, mapped at a reserved address for the current device; plain cudaMalloc where the
+// device does not support it, the driver does not grant it, or SA_DENSE_PLAIN=1 (read once per process).  Freeing
+// synchronises the device first, as cudaFree does: the rows may still be written on any of the library's streams.
+// Contents and addresses behave as cudaMalloc's; sa_device_allocations counts the mapped bytes.  sa_index.cu.
+struct CompressibleSpace {
+    static constexpr const char *name = "compressible device alloc";
+    static cudaError_t alloc(void **p, size_t bytes);
+    static void free(void *p, size_t bytes);
+    static bool compressible(const void *p);   // p came from cuMemCreate with compression granted
+    static bool available();                   // the current device supports it and SA_DENSE_PLAIN is unset
 };
 
 template <typename Space> struct Buffer {
@@ -121,6 +135,9 @@ template <typename Space> struct Buffer {
 };
 using DevBuf = Buffer<DeviceSpace>;
 using PinnedBuf = Buffer<PinnedSpace>;
+using RowBuf = Buffer<CompressibleSpace>;
+// A term of df < n_docs / SA_RARE_ROW_INV_DF has a rare row: at df/N = 1e-3, 97 % of its 128-byte lines are zero.
+#define SA_RARE_ROW_INV_DF 300
 static_assert(!std::is_copy_constructible<DevBuf>::value, "a DevBuf has exactly one owner");
 
 // The scratch arrays of one call, freed when the set goes out of scope.
@@ -242,6 +259,7 @@ struct sa_index {
 
     // scratch
     DevBuf dense;        // float [chunk][n_docs_padded]
+    RowBuf rare_rows;    // term batch: the rows of a chunk's rare terms, in compressible memory (sa_batch_upload)
     DevBuf queries;      // TermQuery[] / phrase descriptors
     DevBuf cand;         // top-k candidates
     DevBuf cand_meta;    // per-query counters / thresholds

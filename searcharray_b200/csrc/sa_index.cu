@@ -1,7 +1,10 @@
 // sa_index.cu -- index upload into HBM, per-term document frequencies, and the C-ABI entry
 // points of the term path (see include/searcharray_b200.h for the reference mapping).
+#include <cuda.h>
+#include <cudaTypedefs.h>
 #include <stdarg.h>
 #include <algorithm>
+#include <unordered_map>
 
 #include "sa_term.cuh"
 #include "sa_phrase.cuh"
@@ -45,6 +48,132 @@ extern "C" int sa_device_allocations(uint64_t *live_buffers, uint64_t *live_byte
     *live_buffers = g_live_dev_buffers;
     *live_bytes = g_live_dev_bytes;
     return SA_OK;
+}
+
+// --------------------------------------------------------------- compressible score rows (CompressibleSpace)
+// The driver's virtual memory calls are reached through the runtime, so the library links against cudart alone.
+namespace {
+struct VmmApi {
+    PFN_cuDeviceGetAttribute_v2000 getAttribute = nullptr;
+    PFN_cuMemGetAllocationGranularity_v10020 granularity = nullptr;
+    PFN_cuMemCreate_v10020 create = nullptr;
+    PFN_cuMemGetAllocationPropertiesFromHandle_v10020 properties = nullptr;
+    PFN_cuMemRelease_v10020 release = nullptr;
+    PFN_cuMemAddressReserve_v10020 reserve = nullptr;
+    PFN_cuMemAddressFree_v10020 addressFree = nullptr;
+    PFN_cuMemMap_v10020 map = nullptr;
+    PFN_cuMemUnmap_v10020 unmap = nullptr;
+    PFN_cuMemSetAccess_v10020 setAccess = nullptr;
+    bool ok = false;
+};
+
+template <typename F> bool driver_entry(const char *symbol, F *fn) {
+    cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+    return cudaGetDriverEntryPointByVersion(symbol, (void **)fn, 12000, cudaEnableDefault, &q) == cudaSuccess &&
+           q == cudaDriverEntryPointSuccess && *fn;
+}
+
+// nullptr when SA_DENSE_PLAIN=1 or the driver lacks an entry point
+const VmmApi *vmm_api() {
+    static const VmmApi api = [] {
+        VmmApi a;
+        if (getenv("SA_DENSE_PLAIN") && atoi(getenv("SA_DENSE_PLAIN")) != 0) return a;
+        a.ok = driver_entry("cuDeviceGetAttribute", &a.getAttribute) &&
+               driver_entry("cuMemGetAllocationGranularity", &a.granularity) && driver_entry("cuMemCreate", &a.create) &&
+               driver_entry("cuMemGetAllocationPropertiesFromHandle", &a.properties) &&
+               driver_entry("cuMemRelease", &a.release) && driver_entry("cuMemAddressReserve", &a.reserve) &&
+               driver_entry("cuMemAddressFree", &a.addressFree) && driver_entry("cuMemMap", &a.map) &&
+               driver_entry("cuMemUnmap", &a.unmap) && driver_entry("cuMemSetAccess", &a.setAccess);
+        return a;
+    }();
+    return api.ok ? &api : nullptr;
+}
+
+// The live compressible mappings: base address -> mapped bytes (the request rounded up to the granularity).
+std::mutex g_vmm_mu;
+std::unordered_map<const void *, size_t> g_vmm_maps;
+
+// cuMemCreate + reserve + map + access with compression granted, or nullptr (nothing left behind).
+void *map_compressible(const VmmApi &api, size_t bytes, size_t *mapped) {
+    int device = 0, supported = 0;
+    if (cudaGetDevice(&device) != cudaSuccess || cudaSetDevice(device) != cudaSuccess ||   // primary context current
+        api.getAttribute(&supported, CU_DEVICE_ATTRIBUTE_GENERIC_COMPRESSION_SUPPORTED, device) != CUDA_SUCCESS ||
+        !supported)
+        return nullptr;
+    CUmemAllocationProp prop = {};
+    prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
+    prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+    prop.location.id = device;
+    prop.allocFlags.compressionType = CU_MEM_ALLOCATION_COMP_GENERIC;
+    size_t gran = 0;
+    if (api.granularity(&gran, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM) != CUDA_SUCCESS || !gran) return nullptr;
+    const size_t size = (bytes + gran - 1) / gran * gran;
+    CUmemGenericAllocationHandle h;
+    if (api.create(&h, size, &prop, 0) != CUDA_SUCCESS) return nullptr;
+    CUmemAllocationProp got = {};
+    CUdeviceptr va = 0;
+    bool ok = api.properties(&got, h) == CUDA_SUCCESS && got.allocFlags.compressionType == CU_MEM_ALLOCATION_COMP_GENERIC;
+    ok = ok && api.reserve(&va, size, gran, 0, 0) == CUDA_SUCCESS;
+    bool mapped_ok = ok && api.map(va, size, 0, h, 0) == CUDA_SUCCESS;
+    api.release(h);                                   // the mapping keeps the memory until it is unmapped
+    CUmemAccessDesc access = {};
+    access.location = prop.location;
+    access.flags = CU_MEM_ACCESS_FLAGS_PROT_READWRITE;
+    if (mapped_ok && api.setAccess(va, size, &access, 1) == CUDA_SUCCESS) {
+        *mapped = size;
+        return (void *)va;
+    }
+    if (mapped_ok) api.unmap(va, size);
+    if (va) api.addressFree(va, size);
+    return nullptr;
+}
+}  // namespace
+
+cudaError_t CompressibleSpace::alloc(void **p, size_t bytes) {
+    if (const VmmApi *api = vmm_api()) {
+        size_t mapped = 0;
+        if (void *va = map_compressible(*api, bytes, &mapped)) {
+            std::lock_guard<std::mutex> lk(g_vmm_mu);
+            g_vmm_maps[va] = mapped;
+            *p = va;
+            g_live_dev_buffers++;
+            g_live_dev_bytes += mapped;
+            return cudaSuccess;
+        }
+    }
+    return DeviceSpace::alloc(p, bytes);
+}
+
+void CompressibleSpace::free(void *p, size_t bytes) {
+    size_t mapped = 0;
+    {
+        std::lock_guard<std::mutex> lk(g_vmm_mu);
+        auto it = g_vmm_maps.find(p);
+        if (it != g_vmm_maps.end()) {
+            mapped = it->second;
+            g_vmm_maps.erase(it);
+        }
+    }
+    if (!mapped) return DeviceSpace::free(p, bytes);
+    const VmmApi *api = vmm_api();
+    cudaDeviceSynchronize();                          // cudaFree's implicit synchronisation: no kernel still writes p
+    api->unmap((CUdeviceptr)p, mapped);
+    api->addressFree((CUdeviceptr)p, mapped);
+    g_live_dev_buffers--;
+    g_live_dev_bytes -= mapped;
+}
+
+bool CompressibleSpace::available() {
+    const VmmApi *api = vmm_api();
+    int device = 0, supported = 0;
+    return api && cudaGetDevice(&device) == cudaSuccess &&
+           api->getAttribute(&supported, CU_DEVICE_ATTRIBUTE_GENERIC_COMPRESSION_SUPPORTED, device) == CUDA_SUCCESS &&
+           supported;
+}
+
+bool CompressibleSpace::compressible(const void *p) {
+    std::lock_guard<std::mutex> lk(g_vmm_mu);
+    return p && g_vmm_maps.count(p);
 }
 
 // --------------------------------------------------------------- bulk upload
@@ -446,6 +575,12 @@ extern "C" int sa_index_upload_mode(const sa_index *ix, int *mode_out) {
     return SA_OK;
 }
 
+extern "C" int sa_index_dense_compressible(const sa_index *ix, int *compressible_out) {
+    SA_CHECK(ix && compressible_out, "NULL argument");
+    *compressible_out = CompressibleSpace::compressible(ix->rare_rows.p) ? 1 : 0;
+    return SA_OK;
+}
+
 extern "C" int sa_docfreq(sa_index *ix, uint32_t term_id, uint64_t *df_out) {
     SA_CHECK(ix && df_out, "NULL argument");
     if (term_id == SA_NO_TERM) { *df_out = 0; return SA_OK; }
@@ -551,6 +686,7 @@ struct BatchChunk {
     u64 arena_words = 64;
     // phrase queries by regime (indices relative to phrase0, stored at B.d_sel + sel0: search first, then conjunction)
     u32 sel0 = 0, n_search = 0, n_conj = 0;
+    u32 n_rare = 0;                 // the last n_rare term rows are rare terms' rows in ix->rare_rows
     SpanPlan span;                  // slop > 0: the chunk's multi-term queries as span queries
 };
 
@@ -603,6 +739,25 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
     const u64 stride = sa_padded_docs(std::max<u64>(ix->n_docs, 1));
     B.chunk = plan.chunk;
     B.row_query = std::move(plan.row_query);
+    // A rare term's row is almost all zero 128-byte lines, which compressible memory keeps off DRAM when the CTAs in
+    // flight write neighbouring tiles of few rows; the other terms' rows are faster in plain memory under the
+    // (queries, tiles) grid, which shares a tile's norms in L2 among the queries (DESIGN §3.1).  So where compressible
+    // memory is available, each chunk's rare terms take its last term rows, in ix->rare_rows, and a launch of their own.
+    auto is_rare = [&](u32 q) {
+        const u32 t = terms[term_starts[q]];
+        return t == SA_NO_TERM || (u64)ix->h_df[t] * SA_RARE_ROW_INV_DF < ix->n_docs;
+    };
+    u32 max_rare = 0;
+    for (const RowChunk &R : plan.chunks)
+        max_rare = std::max(max_rare, (u32)std::count_if(B.row_query.begin() + R.row0,
+                                                         B.row_query.begin() + R.row0 + R.n_term, is_rare));
+    bool split_rare = false;
+    if (max_rare && CompressibleSpace::available()) {
+        split_rare = ix->rare_rows.reserve((size_t)max_rare * stride * sizeof(float)) == SA_OK &&
+                     CompressibleSpace::compressible(ix->rare_rows.p);
+        if (!split_rare) ix->rare_rows.reset();
+    }
+    u32 max_dense_rows = 1;
     u64 max_arena = 64;
     size_t max_span_scratch = 0;
     u32 n_span = 0;
@@ -614,6 +769,11 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
         C.term0 = (u32)B.tqs.size();
         C.phrase0 = slop > 0 ? n_span : (u32)B.pqs.size();
         C.params = make_bm25(1.0f, avg_doc_len, k1, b, ix->doc_lens_nonneg);
+        if (split_rare) {
+            auto first = B.row_query.begin() + R.row0, last = first + R.n_term;
+            C.n_rare = (u32)(last - std::stable_partition(first, last, [&](u32 q) { return !is_rare(q); }));
+        }
+        max_dense_rows = std::max(max_dense_rows, R.n_term - C.n_rare + R.n_phrase);
         for (u32 r = R.row0; r < R.row0 + R.n_term + R.n_phrase; r++) {
             const u32 q = B.row_query[r];
             const u32 nt = term_starts[q + 1] - term_starts[q];
@@ -659,7 +819,7 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
     }
     SA_CHECK(B.chunks.empty() || B.chunks[0].params.sparse_ok || (B.pqs.empty() && n_span == 0),
              "phrase queries in a batch need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite idf)");
-    if ((rc = ix->dense.reserve((size_t)B.chunk * stride * sizeof(float)))) return rc;
+    if ((rc = ix->dense.reserve((size_t)max_dense_rows * stride * sizeof(float)))) return rc;
     if ((rc = ix->cand.reserve(cand_bytes(sa_n_tiles(ix->n_docs), B.chunk, B.slots)))) return rc;
     if ((rc = B.d_tq.reserve(std::max<size_t>(B.tqs.size() * sizeof(TermQuery), 64)))) return rc;
     if ((rc = B.d_pq.reserve(std::max<size_t>(B.pqs.size() * sizeof(PhraseQuery), 64)))) return rc;
@@ -756,21 +916,28 @@ int sa_batch_execute_locked(sa_index *ix) {
     for (const BatchChunk &C : B.chunks) {
         const u32 Q = C.n_term + C.n_phrase;
         TopkCtx t = make_topk_ctx(ix->cand.p, sa_n_tiles(ix->n_docs), Q, B.slots, B.k, d_ovf + C.row0);
+        const u32 n_plain = C.n_term - C.n_rare;          // term rows in ix->dense; the phrase rows follow them
         if (C.n_term) {
             TermBatchArgs a = make_term_args(ix, B.d_tq.as<TermQuery>() + C.term0, C.params, t);
-            if ((rc = launch_term_batch(ix, a, C.n_term))) return rc;
+            if ((rc = launch_term_batch(ix, a, n_plain))) return rc;
+            if (C.n_rare) {
+                a.queries += n_plain;
+                a.out = ix->rare_rows.as<float>();
+                a.topk = topk_ctx_from(t, n_plain);
+                if ((rc = launch_term_batch(ix, a, C.n_rare, /*tiles_fastest=*/true))) return rc;
+            }
         }
         if (B.slop > 0) {
             if (C.n_phrase) {
                 // span matches become records; one tile pass writes the rows (zeros + BM25) and collects top-k
-                float *rows = ix->dense.as<float>() + (u64)C.n_term * stride;
+                float *rows = ix->dense.as<float>() + (u64)n_plain * stride;
                 if ((rc = sa_ensure_norm(ix, B.k1, B.b, B.avg_doc_len))) return rc;
                 if ((rc = sa_span_enqueue(ix, ix->d_words.as<u64>(), C.span, B.d_sq.as<SpanQuery>() + C.phrase0,
                                           B.d_scounts.as<SpanCounts>() + C.phrase0, ix->phrase_scratch.p, rows, stride,
                                           &t, C.n_term))) return rc;
             }
         } else if (C.n_phrase) {
-            float *rows = ix->dense.as<float>() + (u64)C.n_term * stride;
+            float *rows = ix->dense.as<float>() + (u64)n_plain * stride;
             unsigned long long *d_used = (unsigned long long *)ix->phrase_scratch.p;
             SA_CUDA(cudaMemsetAsync(d_used, 0, 64, ix->stream));
             // the phrase kernel materialises its dense rows (zeros + matches) and their top-k candidates

@@ -405,7 +405,7 @@ int sa_ensure_norm(sa_index *ix, float k1, float b, float avg_doc_len) {
     return SA_OK;
 }
 
-int launch_term_batch(sa_index *ix, const TermBatchArgs &a_in, u32 n_queries) {
+int launch_term_batch(sa_index *ix, const TermBatchArgs &a_in, u32 n_queries, bool tiles_fastest) {
     if (n_queries == 0 || a_in.n_docs == 0) return SA_OK;
     TermBatchArgs a = a_in;
     {
@@ -432,7 +432,7 @@ int launch_term_batch(sa_index *ix, const TermBatchArgs &a_in, u32 n_queries) {
     }
     const unsigned n_tiles = sa_n_tiles(a.n_docs);
     static const bool env_qmajor = getenv("SA_TERM_QUERY_MAJOR") && atoi(getenv("SA_TERM_QUERY_MAJOR")) != 0;
-    a.query_major = (env_qmajor || n_tiles > 65535) ? 1 : 0;
+    a.query_major = (tiles_fastest || env_qmajor || n_tiles > 65535) ? 1 : 0;
     dim3 grid = a.query_major ? dim3(n_tiles, n_queries) : dim3(n_queries, n_tiles);
     dim3 block(SA_TERM_THREADS);
     KernelTimer t(ix, 0);

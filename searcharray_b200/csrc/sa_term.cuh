@@ -72,7 +72,9 @@ struct TermBatchArgs {
     TopkCtx topk;
 };
 
-int launch_term_batch(sa_index *ix, const TermBatchArgs &a, u32 n_queries);
+// tiles_fastest: a (tiles, queries) grid, so the CTAs in flight write neighbouring tiles of few rows (the rare terms'
+// rows in compressible memory, sa_batch_upload_locked); otherwise (queries, tiles) unless SA_TERM_QUERY_MAJOR=1.
+int launch_term_batch(sa_index *ix, const TermBatchArgs &a, u32 n_queries, bool tiles_fastest = false);
 int sa_ensure_norm(sa_index *ix, float k1, float b, float avg_doc_len);
 int launch_topk_select(sa_index *ix, const TopkCtx &t, u32 n_queries, u64 doc_base, u64 *d_out_keys,
                        const u32 *d_out_index);
@@ -213,6 +215,15 @@ inline TermQuery make_term_query(const sa_index *ix, u32 t, float idf) {
 // Top-k candidate buffer of Q queries: keys [Q][n_tiles][slots], then counts and maxima [Q][n_tiles] each.
 inline size_t cand_bytes(u32 n_tiles, u32 Q, u32 slots) {
     return (size_t)Q * n_tiles * ((size_t)slots * sizeof(u64) + 2 * sizeof(u32)) + 64;
+}
+
+// The same candidate buffer seen from row `row0` on: a launch over rows [row0, Q) of it indexes them from 0.
+inline TopkCtx topk_ctx_from(TopkCtx t, u32 row0) {
+    t.tile_cand += (u64)row0 * t.n_tiles * t.slots;
+    t.tile_cnt += (u64)row0 * t.n_tiles;
+    t.tile_max += (u64)row0 * t.n_tiles;
+    t.overflow += row0;
+    return t;
 }
 
 inline TopkCtx make_topk_ctx(void *cand, u32 n_tiles, u32 Q, u32 slots, u32 k, u32 *d_overflow) {
