@@ -74,9 +74,9 @@ int sa_index_destroy(sa_index *index);
  * was page-locked in place with cudaHostRegister and DMA'd at PCIe rate, 2 = pipelined through pinned bounce
  * buffers because the range could not be registered. */
 int sa_index_upload_mode(const sa_index *index, int *mode_out);
-/* 1 when the last batch of sa_batch_upload / sa_score_batch_topk wrote its rare terms' dense rows (df < n_docs / 300)
- * to compressible device memory.  The L2 then compresses their all-zero lines on the way to DRAM, and those terms
- * are scanned in a launch of their own.  0 when no batch has had rare terms yet, or when every row is in plain
+/* 1 when a batch of sa_batch_upload / sa_score_batch_topk has written its term queries' dense rows to compressible
+ * device memory.  The L2 then compresses their all-zero lines on the way to DRAM, and the term scan walks those rows
+ * in small query groups.  0 when no batch has had term queries yet, or when every row is in plain
  * cudaMalloc memory: the device has no compression support, the driver does not grant it, or the process started
  * with SA_DENSE_PLAIN=1.  The results are the same bits either way. */
 int sa_index_dense_compressible(const sa_index *index, int *compressible_out);
@@ -322,6 +322,9 @@ typedef struct {
      * 2 * kind + masked, kind the SA_SIM_* value (0 impact, 1 legacy, 2 classic, 3 BM25, also the BM25 batch's phrase
      * and span re-runs) and masked 1 for sim_where_tile_kernel */
     uint64_t sim_instances;
+    /* query groups the term launches walked (sa_term.cu): ceil(queries / G) per launch of group width G, so one per
+     * launch that walks every query as one group */
+    uint64_t term_kernel_groups;
 } sa_stats;
 int sa_stats_reset(sa_index *index);
 int sa_stats_get(sa_index *index, sa_stats *out);

@@ -28,7 +28,7 @@ class SaStats(ctypes.Structure):
                 ("topk_kernel_launches", c_u64), ("phrase_kernel_ms", ctypes.c_double),
                 ("phrase_kernel_launches", c_u64), ("total_launches", c_u64),
                 ("phrase_cont_words", c_u64), ("phrase_matched_docs", c_u64), ("phrase_tile_launches", c_u64),
-                ("bool_instances", c_u64), ("sim_instances", c_u64)]
+                ("bool_instances", c_u64), ("sim_instances", c_u64), ("term_kernel_groups", c_u64)]
 
 
 # name -> (restype, argtypes); must list EVERY symbol include/searcharray_b200.h declares

@@ -79,7 +79,7 @@ struct PinnedSpace {
 };
 
 // Device memory the L2 may compress on its way to DRAM (Hopper's generic compute data compression): the term batch's
-// rows of rare terms, almost all of whose 128-byte lines are zero.  cuMemCreate with
+// score rows, most of whose 128-byte lines are zero.  cuMemCreate with
 // CU_MEM_ALLOCATION_COMP_GENERIC, mapped at a reserved address for the current device; plain cudaMalloc where the
 // device does not support it, the driver does not grant it, or SA_DENSE_PLAIN=1 (read once per process).  Freeing
 // synchronises the device first, as cudaFree does: the rows may still be written on any of the library's streams.
@@ -89,7 +89,8 @@ struct CompressibleSpace {
     static cudaError_t alloc(void **p, size_t bytes);
     static void free(void *p, size_t bytes);
     static bool compressible(const void *p);   // p came from cuMemCreate with compression granted
-    static bool available();                   // the current device supports it and SA_DENSE_PLAIN is unset
+    // bytes a compressible mapping is rounded to; 0 when the current device has no support or SA_DENSE_PLAIN is set
+    static size_t granularity();
 };
 
 template <typename Space> struct Buffer {
@@ -136,8 +137,9 @@ template <typename Space> struct Buffer {
 using DevBuf = Buffer<DeviceSpace>;
 using PinnedBuf = Buffer<PinnedSpace>;
 using RowBuf = Buffer<CompressibleSpace>;
-// A term of df < n_docs / SA_RARE_ROW_INV_DF has a rare row: at df/N = 1e-3, 97 % of its 128-byte lines are zero.
-#define SA_RARE_ROW_INV_DF 300
+// The term batch scans its rows in compressible memory in query groups of SA_COMP_ROW_GROUP (0 = all), or of
+// SA_COMP_ROW_GROUP from the environment, read per launch.  Swept on H100 (DESIGN §6).
+#define SA_COMP_ROW_GROUP 16
 static_assert(!std::is_copy_constructible<DevBuf>::value, "a DevBuf has exactly one owner");
 
 // The scratch arrays of one call, freed when the set goes out of scope.
@@ -259,7 +261,7 @@ struct sa_index {
 
     // scratch
     DevBuf dense;        // float [chunk][n_docs_padded]
-    RowBuf rare_rows;    // term batch: the rows of a chunk's rare terms, in compressible memory (sa_batch_upload)
+    RowBuf comp_rows;    // term batch: a chunk's rows in compressible memory, each padded to the granularity (sa_batch_upload)
     DevBuf queries;      // TermQuery[] / phrase descriptors
     DevBuf cand;         // top-k candidates
     DevBuf cand_meta;    // per-query counters / thresholds

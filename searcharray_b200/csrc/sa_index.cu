@@ -93,20 +93,28 @@ const VmmApi *vmm_api() {
 std::mutex g_vmm_mu;
 std::unordered_map<const void *, size_t> g_vmm_maps;
 
-// cuMemCreate + reserve + map + access with compression granted, or nullptr (nothing left behind).
-void *map_compressible(const VmmApi &api, size_t bytes, size_t *mapped) {
+// The current device's compressible allocation properties and their granularity, or 0 when it has none.
+size_t compressible_prop(const VmmApi &api, CUmemAllocationProp *prop) {
     int device = 0, supported = 0;
     if (cudaGetDevice(&device) != cudaSuccess || cudaSetDevice(device) != cudaSuccess ||   // primary context current
         api.getAttribute(&supported, CU_DEVICE_ATTRIBUTE_GENERIC_COMPRESSION_SUPPORTED, device) != CUDA_SUCCESS ||
         !supported)
-        return nullptr;
-    CUmemAllocationProp prop = {};
-    prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
-    prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
-    prop.location.id = device;
-    prop.allocFlags.compressionType = CU_MEM_ALLOCATION_COMP_GENERIC;
+        return 0;
+    *prop = {};
+    prop->type = CU_MEM_ALLOCATION_TYPE_PINNED;
+    prop->location.type = CU_MEM_LOCATION_TYPE_DEVICE;
+    prop->location.id = device;
+    prop->allocFlags.compressionType = CU_MEM_ALLOCATION_COMP_GENERIC;
     size_t gran = 0;
-    if (api.granularity(&gran, &prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM) != CUDA_SUCCESS || !gran) return nullptr;
+    if (api.granularity(&gran, prop, CU_MEM_ALLOC_GRANULARITY_MINIMUM) != CUDA_SUCCESS) return 0;
+    return gran;
+}
+
+// cuMemCreate + reserve + map + access with compression granted, or nullptr (nothing left behind).
+void *map_compressible(const VmmApi &api, size_t bytes, size_t *mapped) {
+    CUmemAllocationProp prop;
+    const size_t gran = compressible_prop(api, &prop);
+    if (!gran) return nullptr;
     const size_t size = (bytes + gran - 1) / gran * gran;
     CUmemGenericAllocationHandle h;
     if (api.create(&h, size, &prop, 0) != CUDA_SUCCESS) return nullptr;
@@ -163,12 +171,10 @@ void CompressibleSpace::free(void *p, size_t bytes) {
     g_live_dev_bytes -= mapped;
 }
 
-bool CompressibleSpace::available() {
+size_t CompressibleSpace::granularity() {
     const VmmApi *api = vmm_api();
-    int device = 0, supported = 0;
-    return api && cudaGetDevice(&device) == cudaSuccess &&
-           api->getAttribute(&supported, CU_DEVICE_ATTRIBUTE_GENERIC_COMPRESSION_SUPPORTED, device) == CUDA_SUCCESS &&
-           supported;
+    CUmemAllocationProp prop;
+    return api ? compressible_prop(*api, &prop) : 0;
 }
 
 bool CompressibleSpace::compressible(const void *p) {
@@ -577,7 +583,7 @@ extern "C" int sa_index_upload_mode(const sa_index *ix, int *mode_out) {
 
 extern "C" int sa_index_dense_compressible(const sa_index *ix, int *compressible_out) {
     SA_CHECK(ix && compressible_out, "NULL argument");
-    *compressible_out = CompressibleSpace::compressible(ix->rare_rows.p) ? 1 : 0;
+    *compressible_out = CompressibleSpace::compressible(ix->comp_rows.p) ? 1 : 0;
     return SA_OK;
 }
 
@@ -686,7 +692,6 @@ struct BatchChunk {
     u64 arena_words = 64;
     // phrase queries by regime (indices relative to phrase0, stored at B.d_sel + sel0: search first, then conjunction)
     u32 sel0 = 0, n_search = 0, n_conj = 0;
-    u32 n_rare = 0;                 // the last n_rare term rows are rare terms' rows in ix->rare_rows
     SpanPlan span;                  // slop > 0: the chunk's multi-term queries as span queries
 };
 
@@ -700,6 +705,7 @@ struct BatchState {
     std::vector<u32> term_query, phrase_query;  // index in tqs / pqs -> original query index
     std::vector<u32> phrase_missing;          // 1 = a term is unknown: result stays empty
     std::vector<BatchChunk> chunks;
+    u64 comp_stride = 0;                      // term rows in ix->comp_rows, floats from one to the next; 0: in ix->dense
     DevBuf d_sq, d_scounts;                   // slop > 0: every chunk's span descriptors, concatenated, and counts
     DevBuf d_tq, d_pq, d_row_query;
     DevBuf d_meta;                            // u32 overflow[nq] (row space)
@@ -739,23 +745,27 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
     const u64 stride = sa_padded_docs(std::max<u64>(ix->n_docs, 1));
     B.chunk = plan.chunk;
     B.row_query = std::move(plan.row_query);
-    // A rare term's row is almost all zero 128-byte lines, which compressible memory keeps off DRAM when the CTAs in
-    // flight write neighbouring tiles of few rows; the other terms' rows are faster in plain memory under the
-    // (queries, tiles) grid, which shares a tile's norms in L2 among the queries (DESIGN §3.1).  So where compressible
-    // memory is available, each chunk's rare terms take its last term rows, in ix->rare_rows, and a launch of their own.
-    auto is_rare = [&](u32 q) {
-        const u32 t = terms[term_starts[q]];
-        return t == SA_NO_TERM || (u64)ix->h_df[t] * SA_RARE_ROW_INV_DF < ix->n_docs;
-    };
-    u32 max_rare = 0;
-    for (const RowChunk &R : plan.chunks)
-        max_rare = std::max(max_rare, (u32)std::count_if(B.row_query.begin() + R.row0,
-                                                         B.row_query.begin() + R.row0 + R.n_term, is_rare));
-    bool split_rare = false;
-    if (max_rare && CompressibleSpace::available()) {
-        split_rare = ix->rare_rows.reserve((size_t)max_rare * stride * sizeof(float)) == SA_OK &&
-                     CompressibleSpace::compressible(ix->rare_rows.p);
-        if (!split_rare) ix->rare_rows.reset();
+    // A term row is mostly zero 128-byte lines (72 % at df/N = 1e-2), which compressible memory keeps off DRAM when
+    // the CTAs in flight write neighbouring tiles of few rows: the term launch walks the rows in query groups of
+    // SA_COMP_ROW_GROUP (sa_term.cu, DESIGN §3.1).  So where compressible memory is available the chunks' term rows
+    // live in ix->comp_rows, the phrase rows in ix->dense.  A row that spans many granules starts on one of its own:
+    // written a group's time apart, neighbouring rows sharing one would be slow to compress.  The padding is kept to at
+    // most 1/8 of the row (always so for rows of >= 8 granules, 16 MiB); other rows stay packed -- a group's few short
+    // rows are in flight together anyway -- so a chunk's rows stay within sa_plan_rows' budget plus that 1/8.
+    u32 max_term = 0;
+    for (const RowChunk &R : plan.chunks) max_term = std::max(max_term, R.n_term);
+    const size_t gran = max_term ? CompressibleSpace::granularity() : 0;
+    B.comp_stride = 0;
+    if (gran) {
+        const size_t packed = stride * sizeof(float), padded = (packed + gran - 1) / gran * gran;
+        const size_t row_bytes = padded - packed <= packed / 8 ? padded : packed;
+        if (ix->comp_rows.reserve((size_t)max_term * row_bytes) == SA_OK && CompressibleSpace::compressible(ix->comp_rows.p)) {
+            B.comp_stride = row_bytes / sizeof(float);
+        } else {
+            // plain rows in ix->dense instead; a failed fallback cudaMalloc must not fail the batch's next launch check
+            ix->comp_rows.reset();
+            (void)cudaGetLastError();
+        }
     }
     u32 max_dense_rows = 1;
     u64 max_arena = 64;
@@ -769,11 +779,7 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
         C.term0 = (u32)B.tqs.size();
         C.phrase0 = slop > 0 ? n_span : (u32)B.pqs.size();
         C.params = make_bm25(1.0f, avg_doc_len, k1, b, ix->doc_lens_nonneg);
-        if (split_rare) {
-            auto first = B.row_query.begin() + R.row0, last = first + R.n_term;
-            C.n_rare = (u32)(last - std::stable_partition(first, last, [&](u32 q) { return !is_rare(q); }));
-        }
-        max_dense_rows = std::max(max_dense_rows, R.n_term - C.n_rare + R.n_phrase);
+        max_dense_rows = std::max(max_dense_rows, (B.comp_stride ? 0 : R.n_term) + R.n_phrase);
         for (u32 r = R.row0; r < R.row0 + R.n_term + R.n_phrase; r++) {
             const u32 q = B.row_query[r];
             const u32 nt = term_starts[q + 1] - term_starts[q];
@@ -908,6 +914,8 @@ int sa_batch_execute_locked(sa_index *ix) {
         return SA_OK;
     }
     const u64 stride = sa_padded_docs(ix->n_docs);
+    const char *e = getenv("SA_COMP_ROW_GROUP");
+    const u32 comp_group = e ? (u32)atol(e) : SA_COMP_ROW_GROUP;
     u32 *d_ovf = B.d_meta.as<u32>();
     SA_CUDA(cudaMemsetAsync(d_ovf, 0, (size_t)B.nq * sizeof(u32), ix->stream));
     if (!B.pqs.empty())
@@ -916,16 +924,14 @@ int sa_batch_execute_locked(sa_index *ix) {
     for (const BatchChunk &C : B.chunks) {
         const u32 Q = C.n_term + C.n_phrase;
         TopkCtx t = make_topk_ctx(ix->cand.p, sa_n_tiles(ix->n_docs), Q, B.slots, B.k, d_ovf + C.row0);
-        const u32 n_plain = C.n_term - C.n_rare;          // term rows in ix->dense; the phrase rows follow them
+        const u32 n_plain = B.comp_stride ? 0 : C.n_term;   // term rows in ix->dense; the phrase rows follow them
         if (C.n_term) {
             TermBatchArgs a = make_term_args(ix, B.d_tq.as<TermQuery>() + C.term0, C.params, t);
-            if ((rc = launch_term_batch(ix, a, n_plain))) return rc;
-            if (C.n_rare) {
-                a.queries += n_plain;
-                a.out = ix->rare_rows.as<float>();
-                a.topk = topk_ctx_from(t, n_plain);
-                if ((rc = launch_term_batch(ix, a, C.n_rare, /*tiles_fastest=*/true))) return rc;
+            if (B.comp_stride) {
+                a.out = ix->comp_rows.as<float>();
+                a.out_stride = B.comp_stride;
             }
+            if ((rc = launch_term_batch(ix, a, C.n_term, B.comp_stride ? comp_group : 0))) return rc;
         }
         if (B.slop > 0) {
             if (C.n_phrase) {

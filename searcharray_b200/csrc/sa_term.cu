@@ -21,10 +21,12 @@
 //   3. the tile is flushed once with 16-byte streaming stores; while it passes through registers
 //      every score >= a running, provably valid lower bound of the k-th best score is appended to
 //      the query's top-k candidate list (sa_topk.cu), so the dense vector is never re-read.
-// The grid is (queries, tiles) -- the query index runs fastest -- so that the CTAs resident on an
-// SM at any time belong to MANY queries: dense terms (issue-bound CTAs) and sparse terms
-// (store-bound CTAs) overlap, and a tile's norm sectors are shared in L2 by all queries.  With the
-// tiles of one query back to back the same kernel was slower.
+// The grid is one-dimensional, Q * n_tiles CTAs walked in groups of G consecutive queries: inside a group the query
+// runs fastest, then the tile, then the group.  The CTAs in flight (about 6 per SM) then cover about 6 * SMs / G
+// neighbouring tiles of G rows: dense terms (issue-bound CTAs) and sparse terms (store-bound CTAs) overlap, and a
+// staged tile's norms are read from DRAM about once per group and shared in L2 by its queries.  G = Q (every query of
+// the launch, the default) shares them the most; rows in compressible memory want a small G, whose CTAs write few
+// rows in long runs of neighbouring tiles (DESIGN §3.1).
 // HBM traffic: 8*W (words) + the 32 B sectors holding the 4*df norms + 4*N (scores), less whatever
 // the queries of one launch share in L2.  Evaluating BM25 for all 16 docs of every thread under
 // divergence with shared-memory atomics was instruction-bound; variants that staged the postings with TMA bulk copies (cp.async.bulk +
@@ -42,18 +44,21 @@ __device__ __forceinline__ bool payload_keep(u64 w, u64 lo, u64 hi) {
 }
 
 template <int MODE, bool ALL_DOCS, bool FILTER>
-__global__ void __launch_bounds__(SA_TERM_THREADS, 6)
+__global__ void __launch_bounds__(SA_TERM_THREADS, SA_TERM_CTAS_PER_SM)
 term_tile_kernel(const TermBatchArgs a) {
     __shared__ __align__(16) float s_out[SA_TILE_DOCS];
     __shared__ u32 s_range[2];
     __shared__ u32 s_top[(SA_TERM_THREADS / 32) * 8];
     __shared__ u32 s_ncand, s_tile_max;
 
-    // grid = (queries, tiles): consecutive CTAs work on the SAME tile of different queries, so at any
-    // moment an SM holds a mix of dense (issue-bound) and sparse (store-bound) terms, and the tile's
-    // norm sectors are shared in L2 by all queries of the launch
-    const u32 q = a.query_major ? blockIdx.y : blockIdx.x;
-    const u32 tile = a.query_major ? blockIdx.x : blockIdx.y;
+    // 1-D grid in groups of G queries: CTA b is in group g = b / (G T); inside it, consecutive CTAs work on the SAME
+    // tile of the group's Gg (<= G: the last group may be partial) queries, then on the next tile
+    const u32 grp = blockIdx.x / a.group_ctas;
+    const u32 rem = blockIdx.x - grp * a.group_ctas;
+    const u32 q0 = grp * a.group;
+    const u32 gg = min(a.group, a.n_queries - q0);
+    const u32 tile = rem / gg;
+    const u32 q = q0 + (rem - tile * gg);
     const TermQuery tq = a.queries[q];
     const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const u64 *__restrict__ words = a.words + tq.word_off;
@@ -73,10 +78,10 @@ term_tile_kernel(const TermBatchArgs a) {
         const u32 *dir = a.rec_dir + tq.dir_off + tile;
         lo = __ldg(dir);
         hi = __ldg(dir + 1);
-        // L2 prefetch of the records a LATER tile of this query will read: the grid is (queries, tiles) with the query
-        // fastest, so tile + prefetch_tiles is dispatched about one generation of resident CTAs after this one; its
-        // record loads -- the second of two dependent DRAM round trips (directory, then records) on a memory system
-        // saturated with the dense rows' stores -- then hit L2.  One 128-byte line per thread covers any tile (<= 32 KB).
+        // L2 prefetch of the records a LATER tile of this query will read: tile + d is dispatched Gg * d CTAs after this
+        // one, and launch_term_batch picks d so that this is about one generation of resident CTAs; its record loads --
+        // the second of two dependent DRAM round trips (directory, then records) on a memory system saturated with the
+        // dense rows' stores -- then hit L2.  One 128-byte line per thread covers any tile (<= 32 KB).
         const u32 pf_tile = tile + a.prefetch_tiles;
         if (a.prefetch_tiles && (u64)pf_tile * SA_TILE_DOCS < a.n_docs) {
             const u32 plo = __ldg(dir + a.prefetch_tiles), phi = __ldg(dir + a.prefetch_tiles + 1);
@@ -405,9 +410,18 @@ int sa_ensure_norm(sa_index *ix, float k1, float b, float avg_doc_len) {
     return SA_OK;
 }
 
-int launch_term_batch(sa_index *ix, const TermBatchArgs &a_in, u32 n_queries, bool tiles_fastest) {
+int launch_term_batch(sa_index *ix, const TermBatchArgs &a_in, u32 n_queries, u32 group) {
     if (n_queries == 0 || a_in.n_docs == 0) return SA_OK;
     TermBatchArgs a = a_in;
+    const unsigned n_tiles = sa_n_tiles(a.n_docs);
+    SA_CHECK((u64)n_queries * n_tiles <= 0x7fffffffu, "term launch of %u queries x %u tiles exceeds the grid", n_queries,
+             n_tiles);
+    static const bool env_qmajor = getenv("SA_TERM_QUERY_MAJOR") && atoi(getenv("SA_TERM_QUERY_MAJOR")) != 0;
+    if (env_qmajor) group = 1;
+    a.n_queries = n_queries;
+    a.n_tiles = n_tiles;
+    a.group = (group == 0 || group > n_queries) ? n_queries : group;
+    a.group_ctas = a.group * n_tiles;
     {
         // tuning knobs, read per launch (a getenv costs nanoseconds; tools/term_buckets.py sweeps them in one process)
         const char *e;
@@ -416,7 +430,10 @@ int launch_term_batch(sa_index *ix, const TermBatchArgs &a_in, u32 n_queries, bo
         a.staged_norm_min_words = std::max(1u, (e = getenv("SA_STAGED_NORM_MIN_WORDS")) ? (u32)atol(e) : SA_STAGED_NORM_MIN_WORDS);
         a.staged_norm_min_recs = std::max(1u, (e = getenv("SA_STAGED_NORM_MIN_RECS")) ? (u32)atol(e) : SA_STAGED_NORM_MIN_RECS);
         a.quad_min_recs = (e = getenv("SA_TERM_QUAD_MIN_RECS")) ? (u32)atol(e) : SA_TERM_QUAD_MIN_RECS;
-        a.prefetch_tiles = (e = getenv("SA_TERM_PREFETCH_TILES")) ? (u32)atol(e) : SA_TERM_PREFETCH_TILES;
+        // tile + d of a query is dispatched group * d CTAs later: d = one generation of resident CTAs, rounded up
+        a.prefetch_tiles = (e = getenv("SA_TERM_PREFETCH_TILES"))
+                               ? (u32)atol(e)
+                               : std::max(1u, (SA_TERM_CTAS_PER_SM * (u32)ix->num_sms + a.group - 1) / a.group);
         a.quad_min_recs = std::max(a.quad_min_recs, a.staged_norm_min_recs);   // the quad path reads norms from the staged tile only
     }
     a.tile_dir = ix->d_tile_dir.as<u32>();
@@ -430,11 +447,7 @@ int launch_term_batch(sa_index *ix, const TermBatchArgs &a_in, u32 n_queries, bo
         if (rc) return rc;
         a.norm = ix->d_norm.as<float>();
     }
-    const unsigned n_tiles = sa_n_tiles(a.n_docs);
-    static const bool env_qmajor = getenv("SA_TERM_QUERY_MAJOR") && atoi(getenv("SA_TERM_QUERY_MAJOR")) != 0;
-    a.query_major = (tiles_fastest || env_qmajor || n_tiles > 65535) ? 1 : 0;
-    dim3 grid = a.query_major ? dim3(n_tiles, n_queries) : dim3(n_queries, n_tiles);
-    dim3 block(SA_TERM_THREADS);
+    const dim3 grid(n_queries * n_tiles), block(SA_TERM_THREADS);
     KernelTimer t(ix, 0);
     if (a.mode == TERM_MODE_TF) {
         if (a.filter) term_tile_kernel<TERM_MODE_TF, false, true><<<grid, block, 0, ix->stream>>>(a);
@@ -450,6 +463,7 @@ int launch_term_batch(sa_index *ix, const TermBatchArgs &a_in, u32 n_queries, bo
     t.stop();
     ix->stats.term_kernel_launches++;
     ix->stats.term_kernel_queries += n_queries;
+    ix->stats.term_kernel_groups += (n_queries + a.group - 1) / a.group;
     ix->stats.total_launches++;
     return SA_OK;
 }

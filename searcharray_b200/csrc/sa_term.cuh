@@ -12,7 +12,7 @@
 // The three tf-table knobs below were swept on H100 (DESIGN.md §3.1); these values were the fastest on the bench mix.
 #define SA_STAGED_NORM_MIN_WORDS 1024   // tiles with at least this many posting words stage the tile's norms (sa_term.cu)
 #define SA_STAGED_NORM_MIN_RECS 48      // ... or this many (doc, tf) records on the tf-table path
-#define SA_TERM_PREFETCH_TILES 8         // L2 prefetch distance of the tf-table path, in tiles (sa_term.cu)
+#define SA_TERM_CTAS_PER_SM 6           // resident term CTAs per SM (the launch bound); sets the L2 prefetch distance (sa_term.cu)
 #define SA_TERM_QUAD_MIN_RECS 512       // four records per thread from this many records per tile on (and >= 16 * k, sa_term.cu)
 #define SA_TOPK_MAX 32             // warp-level threshold estimation handles k <= 32
 
@@ -68,13 +68,15 @@ struct TermBatchArgs {
     u32 staged_norm_min_words;  // set by launch_term_batch
     u32 staged_norm_min_recs, quad_min_recs;   // set by launch_term_batch
     u32 prefetch_tiles;         // L2 prefetch distance in tiles on the tf-table path (0 = off); set by launch_term_batch
-    u32 query_major;            // grid layout (set by launch_term_batch): 1 = (tiles, queries), 0 = (queries, tiles)
+    // CTA order (set by launch_term_batch): CTA b of the 1-D grid of n_queries * n_tiles walks the rows in groups of
+    // `group` consecutive queries, the queries of a group fastest, then the tiles, then the groups (sa_term.cu)
+    u32 n_queries, n_tiles, group, group_ctas;   // group_ctas = group * n_tiles
     TopkCtx topk;
 };
 
-// tiles_fastest: a (tiles, queries) grid, so the CTAs in flight write neighbouring tiles of few rows (the rare terms'
-// rows in compressible memory, sa_batch_upload_locked); otherwise (queries, tiles) unless SA_TERM_QUERY_MAJOR=1.
-int launch_term_batch(sa_index *ix, const TermBatchArgs &a, u32 n_queries, bool tiles_fastest = false);
+// group: the CTA order's query-group width G (0 = every query, the (queries, tiles) order).  G = 1 walks each row's
+// tiles back to back; SA_TERM_QUERY_MAJOR=1 forces it for every launch.
+int launch_term_batch(sa_index *ix, const TermBatchArgs &a, u32 n_queries, u32 group = 0);
 int sa_ensure_norm(sa_index *ix, float k1, float b, float avg_doc_len);
 int launch_topk_select(sa_index *ix, const TopkCtx &t, u32 n_queries, u64 doc_base, u64 *d_out_keys,
                        const u32 *d_out_index);
@@ -172,7 +174,8 @@ inline int sa_resolve_terms(const sa_index *ix, const u32 *term_ids, u32 n, u64 
 }
 
 // The dense rows of a batch of queries.  The queries are cut, in order, into chunks of `chunk` queries: one chunk's
-// doc-space rows stay within about 4 GB of HBM, and its queries fit one grid dimension (65,535).  Inside a chunk the
+// doc-space rows stay within about 4 GB of HBM (compressible term rows may add up to 1/8 of padding,
+// sa_batch_upload_locked), and its queries fit the span kernels' second grid dimension (65,535).  Inside a chunk the
 // term queries take the first rows, then the multi-term queries, each group in query order.
 struct RowChunk { u32 row0, n_term, n_phrase; };
 struct RowPlan {
@@ -215,15 +218,6 @@ inline TermQuery make_term_query(const sa_index *ix, u32 t, float idf) {
 // Top-k candidate buffer of Q queries: keys [Q][n_tiles][slots], then counts and maxima [Q][n_tiles] each.
 inline size_t cand_bytes(u32 n_tiles, u32 Q, u32 slots) {
     return (size_t)Q * n_tiles * ((size_t)slots * sizeof(u64) + 2 * sizeof(u32)) + 64;
-}
-
-// The same candidate buffer seen from row `row0` on: a launch over rows [row0, Q) of it indexes them from 0.
-inline TopkCtx topk_ctx_from(TopkCtx t, u32 row0) {
-    t.tile_cand += (u64)row0 * t.n_tiles * t.slots;
-    t.tile_cnt += (u64)row0 * t.n_tiles;
-    t.tile_max += (u64)row0 * t.n_tiles;
-    t.overflow += row0;
-    return t;
 }
 
 inline TopkCtx make_topk_ctx(void *cand, u32 n_tiles, u32 Q, u32 slots, u32 k, u32 *d_overflow) {

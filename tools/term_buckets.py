@@ -1,7 +1,8 @@
 """Times the batched term path per df bucket, optionally under several settings of the term kernel's tuning knobs
 (environment variables read per launch):
     python tools/term_buckets.py [n_docs] [buckets, e.g. 2,3] [queries] [KEY=v1,v2,... ...]
-e.g. python tools/term_buckets.py 10000000 1,2,3 128 SA_TERM_QUAD_MIN_RECS=160,512 SA_STAGED_NORM_MIN_RECS=384,768"""
+e.g. python tools/term_buckets.py 10000000 1,2,3 128 SA_TERM_QUAD_MIN_RECS=160,512 SA_STAGED_NORM_MIN_RECS=384,768
+The value `default` leaves a variable unset (the compiled-in default)."""
 import ctypes, itertools, os, sys, time
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -24,7 +25,10 @@ print(f'generated + uploaded in {time.time() - t0:.1f}s', flush=True)
 settings = list(itertools.product(*[[(name, v) for v in vals] for name, vals in knobs])) or [()]
 for setting in settings:
     for name, v in setting:
-        os.environ[name] = v
+        if v == 'default':
+            os.environ.pop(name, None)
+        else:
+            os.environ[name] = v
     print('== ' + (' '.join(f'{n}={v}' for n, v in setting) or 'defaults'), flush=True)
     for b, p in enumerate(synth.DF_BUCKETS):
         if only is not None and b not in only:
