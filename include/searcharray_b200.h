@@ -37,6 +37,10 @@ typedef struct sa_index sa_index;
 
 #define SA_NO_TERM 0xFFFFFFFFu      /* "token not in the term dictionary" (TermMissingError) */
 #define SA_NO_DOC 0xFFFFFFFFu       /* empty top-k slot */
+/* The largest k of the batched top-k entry points: sa_score_batch_topk, sa_batch_upload, the boolean ones,
+ * sa_score_batch_topk_sim (every kind), sa_multi_topk and sa_score_batch_topk_allgather take 1 <= k <=
+ * SA_TOPK_DEEP_MAX. */
+#define SA_TOPK_DEEP_MAX 1024
 #define SA_MAX_PHRASE_TERMS 16
 #define SA_ALL_BITS 0xFFFFFFFFFFFFFFFFull
 
@@ -325,6 +329,9 @@ typedef struct {
     /* query groups the term launches walked (sa_term.cu): ceil(queries / G) per launch of group width G, so one per
      * launch that walks every query as one group */
     uint64_t term_kernel_groups;
+    /* (query, tile) pairs whose candidates the deep collector took (k > 32: the tile's exact top k, sorted), over
+     * every batched top-k entry point */
+    uint64_t deep_tiles;
 } sa_stats;
 int sa_stats_reset(sa_index *index);
 int sa_stats_get(sa_index *index, sa_stats *out);
@@ -352,6 +359,13 @@ int sa_score_batch_topk_allgather(sa_index *index, const uint32_t *terms, const 
                                   const float *idf, uint32_t n_queries, uint32_t slop,
                                   float avg_doc_len, float k1, float b, uint32_t k,
                                   uint32_t *out_docs, float *out_scores);
+/* The merge step of sa_score_batch_topk_allgather on lists the caller holds: lists[r][q][i], world per-rank lists of
+ * k keys (score_bits << 32 | ~doc, as the batched top-k keeps them) per query, each sorted descending and 0-padded,
+ * the ranks' doc ranges disjoint; out[q][i] = the k largest keys of query q over the ranks, descending, 0-padded.
+ * Runs the device merge the all-gather uses (topk_merge_kernel, or topk_merge_ranked_kernel for world * k > 4,096)
+ * on the index's device; 1 <= k <= SA_TOPK_DEEP_MAX. */
+int sa_topk_merge(sa_index *index, const uint64_t *lists, uint32_t world, uint32_t n_queries, uint32_t k,
+                  uint64_t *out);
 
 /* ------------------------------------------------------ multi-field edismax (8f-1)
  * Replaces the numpy half of searcharray/solr.py:117-355 (edismax): the per-(term, field) BM25

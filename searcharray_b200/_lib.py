@@ -28,7 +28,8 @@ class SaStats(ctypes.Structure):
                 ("topk_kernel_launches", c_u64), ("phrase_kernel_ms", ctypes.c_double),
                 ("phrase_kernel_launches", c_u64), ("total_launches", c_u64),
                 ("phrase_cont_words", c_u64), ("phrase_matched_docs", c_u64), ("phrase_tile_launches", c_u64),
-                ("bool_instances", c_u64), ("sim_instances", c_u64), ("term_kernel_groups", c_u64)]
+                ("bool_instances", c_u64), ("sim_instances", c_u64), ("term_kernel_groups", c_u64),
+                ("deep_tiles", c_u64)]
 
 
 # name -> (restype, argtypes); must list EVERY symbol include/searcharray_b200.h declares
@@ -78,6 +79,7 @@ SIGNATURES = {
     "sa_comm_allreduce_sum_u64": (c_int, [P_void, P_u64, c_u64]),
     "sa_batch_execute_allgather": (c_int, [P_void]),
     "sa_batch_download_allgather": (c_int, [P_void, P_u32, P_f32, P_u32]),
+    "sa_topk_merge": (c_int, [P_void, P_u64, c_u32, c_u32, c_u32, P_u64]),
     "sa_score_batch_topk_allgather": (c_int, [P_void, P_u32, P_u32, P_f32, c_u32, c_u32, c_f32, c_f32, c_f32,
                                               c_u32, P_u32, P_f32]),
     "sa_multi_create": (c_int, [ctypes.POINTER(P_void), c_u32, ctypes.POINTER(P_void)]),

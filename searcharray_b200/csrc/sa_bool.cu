@@ -352,8 +352,9 @@ __device__ __forceinline__ void bool_count_tile(const BoolCount &cn, float *s_ti
 // s_g[3] (shared) the groups' presence masks.  NESTED (with DISMAX): nested clauses and the store pass (BoolNest).
 // WHERE: only docs whose bit of the mask row of query blockIdx.x is set rank (never in a store pass).  FEATURE (with
 // OCCUR): clauses whose row is SA_BOOL_FEATURE_ROW score their column feat[clause] (BoolFeature).  COUNT (with
-// FEATURE): the collected tile is counted into `cn` (bool_count_tile).
-template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, bool FEATURE, bool COUNT>
+// FEATURE): the collected tile is counted into `cn` (bool_count_tile).  DEEP: k > SA_TOPK_MAX, the tile's candidates
+// from deep_tile_collect.
+template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, bool FEATURE, bool COUNT, bool DEEP>
 __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__restrict__ occ,
                                           const BoolField *__restrict__ fld, const BoolGroup *__restrict__ grp,
                                           float *s_dyn, unsigned long long *s_g, const BoolNest nb, const WhereMask wh,
@@ -572,7 +573,8 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
         if (tid == 0) nb.flags[(u64)bq.pad * nb.n_tiles + tile] = ranked ? 1u : 0u;
         return;
     }
-    flush_tile_collect<false>(s_tile, nullptr, a.topk, q, tile, my_max, SA_TILE_DOCS, 0, s_top, &s_ncand, &s_tile_max);
+    flush_tile_collect<false, DEEP>(s_tile, nullptr, a.topk, q, tile, my_max, SA_TILE_DOCS, 0, s_top, &s_ncand,
+                                    &s_tile_max);
     if (COUNT) bool_count_tile(cn, s_tile);
 }
 
@@ -585,24 +587,25 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
 // bool_tile's s_g placed ahead of the fold's own shared arrays.  Where the compiler places a __shared__ array follows
 // where it is declared: the unmasked DisMax instances without FEATURE were tuned with s_g first (a local of this
 // helper, one instance per kernel), the others with it last (a local of the kernel), and each keeps its layout.
-template <bool NESTED>
+template <bool NESTED, bool DEEP>
 __device__ __forceinline__ unsigned long long *bool_s_g_first() {
     __shared__ unsigned long long s_g[3];
     return s_g;
 }
 
-template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, bool FEATURE, bool COUNT, int MIN_CTAS>
+template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, bool FEATURE, bool COUNT, bool DEEP,
+          int MIN_CTAS>
 __global__ void __launch_bounds__(SA_TERM_THREADS, MIN_CTAS)
 bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
                  const BoolGroup *__restrict__ grp, const BoolNest nb, const WhereMask wh,
                  const BoolFeature *__restrict__ feat, const BoolCount cn) {
     extern __shared__ __align__(16) float s_dyn[];
     if constexpr (DISMAX && !WHERE && !FEATURE) {
-        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, FEATURE, COUNT>(a, occ, fld, grp, s_dyn,
-                                                                        bool_s_g_first<NESTED>(), nb, wh, feat, cn);
+        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, FEATURE, COUNT, DEEP>(a, occ, fld, grp, s_dyn,
+                                                                        bool_s_g_first<NESTED, DEEP>(), nb, wh, feat, cn);
     } else {
         __shared__ unsigned long long s_g[3];
-        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, FEATURE, COUNT>(a, occ, fld, grp, s_dyn, s_g, nb, wh, feat, cn);
+        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, FEATURE, COUNT, DEEP>(a, occ, fld, grp, s_dyn, s_g, nb, wh, feat, cn);
     }
 }
 
@@ -625,44 +628,50 @@ typedef void (*BoolKernel)(BoolArgs, const BoolOccur *, const BoolField *, const
 // the DisMax and nested ones to two (DESIGN.md sections 3.10.3, 3.10.4); each masked instance to its unmasked
 // instance's CTAs per SM (section 3.11); the FEATURE and COUNT instances to their form's (three for the roles form).
 // A nested call's store passes run the unmasked nested instance.
-BoolKernel bool_kernel(BoolForm form, bool masked, BoolVariant variant) {
+template <bool DEEP>
+BoolKernel bool_instance(BoolForm form, bool masked, BoolVariant variant) {
     static const BoolKernel instances[3][5][2] = {
         {
-            {bool_tile_kernel<false, false, false, false, false, false, false, 0>,
-             bool_tile_kernel<false, false, false, false, true, false, false, 2>},
-            {bool_tile_kernel<true, false, false, false, false, false, false, 0>,
-             bool_tile_kernel<true, false, false, false, true, false, false, 3>},
-            {bool_tile_kernel<true, true, false, false, false, false, false, 3>,
-             bool_tile_kernel<true, true, false, false, true, false, false, 3>},
-            {bool_tile_kernel<true, true, true, false, false, false, false, 2>,
-             bool_tile_kernel<true, true, true, false, true, false, false, 2>},
-            {bool_tile_kernel<true, true, true, true, false, false, false, 2>,
-             bool_tile_kernel<true, true, true, true, true, false, false, 2>},
+            {bool_tile_kernel<false, false, false, false, false, false, false, DEEP, 0>,
+             bool_tile_kernel<false, false, false, false, true, false, false, DEEP, 2>},
+            {bool_tile_kernel<true, false, false, false, false, false, false, DEEP, 0>,
+             bool_tile_kernel<true, false, false, false, true, false, false, DEEP, 3>},
+            {bool_tile_kernel<true, true, false, false, false, false, false, DEEP, 3>,
+             bool_tile_kernel<true, true, false, false, true, false, false, DEEP, 3>},
+            {bool_tile_kernel<true, true, true, false, false, false, false, DEEP, 2>,
+             bool_tile_kernel<true, true, true, false, true, false, false, DEEP, 2>},
+            {bool_tile_kernel<true, true, true, true, false, false, false, DEEP, 2>,
+             bool_tile_kernel<true, true, true, true, true, false, false, DEEP, 2>},
         },
         {
             {nullptr, nullptr},
-            {bool_tile_kernel<true, false, false, false, false, true, false, 3>,
-             bool_tile_kernel<true, false, false, false, true, true, false, 3>},
-            {bool_tile_kernel<true, true, false, false, false, true, false, 3>,
-             bool_tile_kernel<true, true, false, false, true, true, false, 3>},
-            {bool_tile_kernel<true, true, true, false, false, true, false, 2>,
-             bool_tile_kernel<true, true, true, false, true, true, false, 2>},
-            {bool_tile_kernel<true, true, true, true, false, true, false, 2>,
-             bool_tile_kernel<true, true, true, true, true, true, false, 2>},
+            {bool_tile_kernel<true, false, false, false, false, true, false, DEEP, 3>,
+             bool_tile_kernel<true, false, false, false, true, true, false, DEEP, 3>},
+            {bool_tile_kernel<true, true, false, false, false, true, false, DEEP, 3>,
+             bool_tile_kernel<true, true, false, false, true, true, false, DEEP, 3>},
+            {bool_tile_kernel<true, true, true, false, false, true, false, DEEP, 2>,
+             bool_tile_kernel<true, true, true, false, true, true, false, DEEP, 2>},
+            {bool_tile_kernel<true, true, true, true, false, true, false, DEEP, 2>,
+             bool_tile_kernel<true, true, true, true, true, true, false, DEEP, 2>},
         },
         {
             {nullptr, nullptr},
-            {bool_tile_kernel<true, false, false, false, false, true, true, 3>,
-             bool_tile_kernel<true, false, false, false, true, true, true, 3>},
-            {bool_tile_kernel<true, true, false, false, false, true, true, 3>,
-             bool_tile_kernel<true, true, false, false, true, true, true, 3>},
-            {bool_tile_kernel<true, true, true, false, false, true, true, 2>,
-             bool_tile_kernel<true, true, true, false, true, true, true, 2>},
-            {bool_tile_kernel<true, true, true, true, false, true, true, 2>,
-             bool_tile_kernel<true, true, true, true, true, true, true, 2>},
+            {bool_tile_kernel<true, false, false, false, false, true, true, DEEP, 3>,
+             bool_tile_kernel<true, false, false, false, true, true, true, DEEP, 3>},
+            {bool_tile_kernel<true, true, false, false, false, true, true, DEEP, 3>,
+             bool_tile_kernel<true, true, false, false, true, true, true, DEEP, 3>},
+            {bool_tile_kernel<true, true, true, false, false, true, true, DEEP, 2>,
+             bool_tile_kernel<true, true, true, false, true, true, true, DEEP, 2>},
+            {bool_tile_kernel<true, true, true, true, false, true, true, DEEP, 2>,
+             bool_tile_kernel<true, true, true, true, true, true, true, DEEP, 2>},
         },
     };
     return instances[variant][form][masked];
+}
+
+// deep: k > SA_TOPK_MAX, the instance whose tiles collect with deep_tile_collect
+BoolKernel bool_kernel(BoolForm form, bool masked, BoolVariant variant, bool deep) {
+    return deep ? bool_instance<true>(form, masked, variant) : bool_instance<false>(form, masked, variant);
 }
 
 // The fields of one call and where the call keeps its state.  The single-index entry point passes one field and the
@@ -839,9 +848,10 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const BoolInput &in, co
     }
     auto launch = [&](bool c, bool masked, u32 n_q, const BoolArgs &args, const BoolNest &n, const WhereMask &w) -> int {
         const BoolVariant variant = bool_variant(P, c);
-        bool_kernel(P.form, masked, variant)<<<dim3(n_q, n_tiles), SA_TERM_THREADS, smem, ix->stream>>>(
-            args, occ, fld, grp, n, w, feat, cn);
+        bool_kernel(P.form, masked, variant, in.k > SA_TOPK_MAX)<<<dim3(n_q, n_tiles), SA_TERM_THREADS, smem,
+                                                                    ix->stream>>>(args, occ, fld, grp, n, w, feat, cn);
         SA_CUDA(cudaGetLastError());
+        if (in.k > SA_TOPK_MAX && !n.store) ix->stats.deep_tiles += (u64)n_q * n_tiles;
         ix->stats.total_launches++;
         ix->stats.bool_instances |= 1ull << (variant * 10 + P.form * 2 + (masked ? 1 : 0));
         return SA_OK;
@@ -1188,8 +1198,8 @@ int bool_upload(const BoolCall &X, const BoolInput &in, const BoolPlan &P, Where
         // the first pass's variant and that of the store passes and re-runs, each masked only when the call is
         const BoolVariant first = bool_variant(P, in.out_total != nullptr), rest = bool_variant(P, false);
         for (int masked = 0; masked <= (where->bits != nullptr); masked++)
-            if ((rc = bool_dismax_smem(bool_kernel(P.form, masked, first))) ||
-                (rest != first && (rc = bool_dismax_smem(bool_kernel(P.form, masked, rest)))))
+            if ((rc = bool_dismax_smem(bool_kernel(P.form, masked, first, in.k > SA_TOPK_MAX))) ||
+                (rest != first && (rc = bool_dismax_smem(bool_kernel(P.form, masked, rest, in.k > SA_TOPK_MAX)))))
                 return rc;
     }
     SA_CUDA(cudaMemsetAsync(P.result.ovf(S.d_keys.p), 0, P.result.bytes() - P.result.n_keys * sizeof(u64),
@@ -1271,7 +1281,7 @@ extern "C" int sa_score_batch_topk_bool(sa_index *ix, uint32_t n_nodes, const ui
     SA_CHECK(ix && out_docs && out_scores, "NULL argument");
     SA_CHECK(n_nodes == 0 || (node_clause_starts && clause_terms && clause_term_starts && clause_idf && mm),
              "NULL argument");
-    SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
+    SA_CHECK(k >= 1 && k <= SA_TOPK_DEEP_MAX, "k must be in [1, %d]", SA_TOPK_DEEP_MAX);
     if (n_redone) *n_redone = 0;
     std::lock_guard<std::mutex> g(ix->mu);
     SA_CUDA(cudaSetDevice(ix->device));
@@ -1303,7 +1313,7 @@ extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, uint32_t n_nodes, con
     SA_CHECK(m && out_docs && out_scores && avg_doc_len && k1 && b, "NULL argument");
     SA_CHECK(n_nodes == 0 || (node_clause_starts && clause_field && clause_terms && clause_term_starts &&
                                 clause_idf && clause_weight && clause_occur && mm), "NULL argument");
-    SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
+    SA_CHECK(k >= 1 && k <= SA_TOPK_DEEP_MAX, "k must be in [1, %d]", SA_TOPK_DEEP_MAX);
     if (n_redone) *n_redone = 0;
     std::lock_guard<std::mutex> g(m->mu);
     SA_CUDA(cudaSetDevice(m->device));

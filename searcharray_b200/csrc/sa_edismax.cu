@@ -144,6 +144,8 @@ edismax_add_phase_kernel(const PhaseArgs a) {
 // Top-k candidates of one tile of qf (positions [0, n_docs)), ranked by f64_proxy_key with the float64 scores beside
 // them: the collection classic_similarity's search_topk uses (sim_tile_kernel).  The tile is read whole: the combine
 // kernels write qf's padding past n_docs with zeros, which never rank.
+// DEEP: k > SA_TOPK_MAX, collect_tile_f64's exact tile bound.
+template <bool DEEP>
 __global__ void __launch_bounds__(SA_TERM_THREADS)
 edismax_tile_kernel(const double *__restrict__ qf, u64 n_docs, const TopkCtx t, u64 *__restrict__ tile_d) {
     __shared__ u32 s_top[(SA_TERM_THREADS / 32) * 8];
@@ -160,7 +162,7 @@ edismax_tile_kernel(const double *__restrict__ qf, u64 n_docs, const TopkCtx t, 
             my_max = max(my_max, key[j * 4 + e]);
         }
     }
-    collect_tile_f64(key, my_max, (u32)min((u64)SA_TILE_DOCS, n_docs - pos0), t, tile_d, 0, tile, s_top, &s_ncand,
+    collect_tile_f64<DEEP>(key, my_max, (u32)min((u64)SA_TILE_DOCS, n_docs - pos0), t, tile_d, 0, tile, s_top, &s_ncand,
                      &s_tile_max, [&](u32 local) { return __ldg(qf + pos0 + local); });
 }
 
@@ -400,7 +402,7 @@ extern "C" int sa_multi_is_float32(sa_multi *m, int *out) {
 
 extern "C" int sa_multi_topk(sa_multi *m, uint32_t k, uint32_t *out_docs, double *out_scores) {
     SA_CHECK(m && out_docs && out_scores && m->has_qf, "bad argument");
-    SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
+    SA_CHECK(k >= 1 && k <= SA_TOPK_DEEP_MAX, "k must be in [1, %d]", SA_TOPK_DEEP_MAX);
     std::lock_guard<std::mutex> g(m->mu);
     SA_CUDA(cudaSetDevice(m->device));
     for (u32 i = 0; i < k; i++) { out_docs[i] = SA_NO_DOC; out_scores[i] = 0.0; }
@@ -415,7 +417,7 @@ extern "C" int sa_multi_topk(sa_multi *m, uint32_t k, uint32_t *out_docs, double
     u32 *d_ovf = (u32 *)(d_scores + k);
     std::vector<u64> h(2 * (size_t)k + 1);          // the keys, the scores' bits, the overflow flag
     // a tile with more candidates than slots sends the query once more with a slot per position, which cannot overflow
-    for (u32 slots = sa_topk_slots(k);; slots = SA_TILE_DOCS) {
+    for (u32 slots = sa_topk_slots_f64(k, sa_topk_slots(k));; slots = SA_TILE_DOCS) {
         const size_t cb = cand_bytes(T, 1, slots);
         if ((rc = m->cand.reserve(cb + (size_t)T * slots * sizeof(u64)))) return rc;
         u64 *tile_d = (u64 *)((char *)m->cand.p + cb);
@@ -423,7 +425,12 @@ extern "C" int sa_multi_topk(sa_multi *m, uint32_t k, uint32_t *out_docs, double
         const TopkCtx t = make_topk_ctx(m->cand.p, T, 1, slots, k, d_ovf);
         {
             KernelTimer tm(ix, 1);
-            edismax_tile_kernel<<<T, SA_TERM_THREADS, 0, m->stream>>>(m->d_qf.as<double>(), m->n_docs, t, tile_d);
+            if (k > SA_TOPK_MAX) {
+                edismax_tile_kernel<true><<<T, SA_TERM_THREADS, 0, m->stream>>>(m->d_qf.as<double>(), m->n_docs, t, tile_d);
+                ix->stats.deep_tiles += T;
+            } else {
+                edismax_tile_kernel<false><<<T, SA_TERM_THREADS, 0, m->stream>>>(m->d_qf.as<double>(), m->n_docs, t, tile_d);
+            }
             SA_CUDA(cudaGetLastError());
             tm.stop();
             ix->stats.topk_kernel_launches++;

@@ -719,7 +719,7 @@ int sa_batch_upload_locked(sa_index *ix, const uint32_t *terms, const uint32_t *
                            const float *idf, uint32_t n_queries, uint32_t slop,
                            float avg_doc_len, float k1, float b, uint32_t k) {
     SA_CHECK(ix && (n_queries == 0 || (terms && term_starts && idf)), "NULL argument");
-    SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
+    SA_CHECK(k >= 1 && k <= SA_TOPK_DEEP_MAX, "k must be in [1, %d]", SA_TOPK_DEEP_MAX);
     SA_CUDA(cudaSetDevice(ix->device));
     if (!ix->batch) ix->batch.reset(new BatchState());
     BatchState &B = *ix->batch;

@@ -287,6 +287,8 @@ struct ChainResult { u64 *docs; u64 n_docs; u64 *cont; u64 n_cont; };
 // ---------------------------------------------------------------------------------------------------------------
 // The SEARCH regime (|shortest list| << |the others|): one CTA per (query, doc-range chunk) runs the whole chain once
 // over its chunk; a step's driver elements binary-search the other list in global memory, which skips most of it.
+// DEEP (here and in phrase_tile_kernel): k > SA_TOPK_MAX, collected by deep_tile_collect.
+template <bool DEEP>
 __global__ void __launch_bounds__(PT, 4)
 phrase_kernel(const PhraseArgs a) {
     __shared__ StepShared S;
@@ -500,7 +502,7 @@ phrase_kernel(const PhraseArgs a) {
         my_match = __reduce_add_sync(0xffffffffu, my_match);
         if (lane == 0 && my_match) atomicAdd(&a.stats[q].n_match, my_match);
         __syncthreads();
-        flush_tile_collect(s_tile, out + (u64)tile * SA_TILE_DOCS, a.topk, row, tile, my_max, (u32)(m1 - m0),
+        flush_tile_collect<true, DEEP>(s_tile, out + (u64)tile * SA_TILE_DOCS, a.topk, row, tile, my_max, (u32)(m1 - m0),
                            (u32)min(m1 - m0, (u64)PT), s_top, &s_ncand, &s_tile_max);
     }
 }
@@ -517,6 +519,7 @@ phrase_kernel(const PhraseArgs a) {
 // the exact re-run in the search regime (the host routes phrases whose terms co-occur that often there up front).
 // The pair statistics of the same-term speculation cover the candidate docs only: enough to CONFIRM a guess, not to
 // derive the reference's global decision from, so any disagreement also re-runs the query in the search regime.
+template <bool DEEP>
 __global__ void __launch_bounds__(PT, 5)
 phrase_tile_kernel(const PhraseArgs a) {
     __shared__ __align__(16) float s_tile[SA_TILE_DOCS];
@@ -680,15 +683,18 @@ phrase_tile_kernel(const PhraseArgs a) {
         }
         return;
     }
-    flush_tile_collect(s_tile, out + (u64)tile * SA_TILE_DOCS, a.topk, row, tile, my_max, total, holders, s_top, &s_ncand, &s_tile_max);
+    flush_tile_collect<true, DEEP>(s_tile, out + (u64)tile * SA_TILE_DOCS, a.topk, row, tile, my_max, total, holders, s_top,
+                                   &s_ncand, &s_tile_max);
 }
 
 int launch_phrase(sa_index *ix, const PhraseArgs &a, u32 n_queries) {
     if (n_queries == 0 || a.n_docs == 0) return SA_OK;
     dim3 grid(n_queries, a.n_chunks);
     KernelTimer t(ix, 2);
-    phrase_kernel<<<grid, PT, 0, ix->stream>>>(a);
+    if (a.topk.k > SA_TOPK_MAX) phrase_kernel<true><<<grid, PT, 0, ix->stream>>>(a);
+    else phrase_kernel<false><<<grid, PT, 0, ix->stream>>>(a);
     SA_CUDA(cudaGetLastError());
+    if (a.topk.k > SA_TOPK_MAX) ix->stats.deep_tiles += (u64)n_queries * sa_n_tiles(a.n_docs);
     t.stop();
     ix->stats.phrase_kernel_launches++;
     ix->stats.total_launches++;
@@ -699,8 +705,10 @@ int launch_phrase(sa_index *ix, const PhraseArgs &a, u32 n_queries) {
 static int launch_phrase_tile(sa_index *ix, const PhraseArgs &a, u32 n_queries) {
     if (n_queries == 0 || a.n_docs == 0) return SA_OK;
     KernelTimer t(ix, 2);
-    phrase_tile_kernel<<<dim3(n_queries, sa_n_tiles(a.n_docs)), PT, 0, ix->stream>>>(a);
+    if (a.topk.k > SA_TOPK_MAX) phrase_tile_kernel<true><<<dim3(n_queries, sa_n_tiles(a.n_docs)), PT, 0, ix->stream>>>(a);
+    else phrase_tile_kernel<false><<<dim3(n_queries, sa_n_tiles(a.n_docs)), PT, 0, ix->stream>>>(a);
     SA_CUDA(cudaGetLastError());
+    if (a.topk.k > SA_TOPK_MAX) ix->stats.deep_tiles += (u64)n_queries * sa_n_tiles(a.n_docs);
     t.stop();
     ix->stats.phrase_kernel_launches++;
     ix->stats.phrase_tile_launches++;

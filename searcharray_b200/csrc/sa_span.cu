@@ -729,6 +729,8 @@ span_sorted_kernel(const SpanArgs a) {
 
 // One CTA per (doc-range chunk, query): writes the chunk's dense tiles -- zeros, plus the BM25 of the
 // accumulated span counts where there are matches -- and collects every tile's top-k candidates.
+// DEEP: k > SA_TOPK_MAX, collected by deep_tile_collect.
+template <bool DEEP>
 __global__ void __launch_bounds__(SA_TERM_THREADS)
 span_tiles_kernel(const SpanArgs a) {
     __shared__ __align__(16) float s_tile[SA_TILE_DOCS];
@@ -831,7 +833,8 @@ span_tiles_kernel(const SpanArgs a) {
             }
         }
         __syncthreads();
-        flush_tile_collect(s_tile, out + t0, a.topk, row, tile, my_max, n_items, min(n_items, (u32)SA_TERM_THREADS), s_top, &s_ncand, &s_tile_max);
+        flush_tile_collect<true, DEEP>(s_tile, out + t0, a.topk, row, tile, my_max, n_items,
+                                       min(n_items, (u32)SA_TERM_THREADS), s_top, &s_ncand, &s_tile_max);
     }
 }
 
@@ -1011,8 +1014,10 @@ int sa_span_enqueue(sa_index *ix, const u64 *d_lists, const SpanPlan &plan, cons
     if (topk) {
         span_sorted_kernel<<<dim3(8, Q), GEN_THREADS, 0, ix->stream>>>(a);
         SA_CUDA(cudaGetLastError());
-        span_tiles_kernel<<<dim3(Q, a.n_chunks), SA_TERM_THREADS, 0, ix->stream>>>(a);
+        if (a.topk.k > SA_TOPK_MAX) span_tiles_kernel<true><<<dim3(Q, a.n_chunks), SA_TERM_THREADS, 0, ix->stream>>>(a);
+        else span_tiles_kernel<false><<<dim3(Q, a.n_chunks), SA_TERM_THREADS, 0, ix->stream>>>(a);
         SA_CUDA(cudaGetLastError());
+        if (a.topk.k > SA_TOPK_MAX) ix->stats.deep_tiles += (u64)Q * sa_n_tiles(ix->n_docs);
         ix->stats.phrase_kernel_launches += 2;
         ix->stats.total_launches += 2;
     }

@@ -43,8 +43,9 @@ __device__ __forceinline__ bool payload_keep(u64 w, u64 lo, u64 hi) {
     return v >= lo && v <= hi;
 }
 
-template <int MODE, bool ALL_DOCS, bool FILTER>
-__global__ void __launch_bounds__(SA_TERM_THREADS, SA_TERM_CTAS_PER_SM)
+// DEEP: k > SA_TOPK_MAX, the tile's candidates from deep_tile_collect (step 3').
+template <int MODE, bool ALL_DOCS, bool FILTER, bool DEEP>
+__global__ void __launch_bounds__(SA_TERM_THREADS, DEEP ? SA_TERM_DEEP_CTAS_PER_SM : SA_TERM_CTAS_PER_SM)
 term_tile_kernel(const TermBatchArgs a) {
     __shared__ __align__(16) float s_out[SA_TILE_DOCS];
     __shared__ u32 s_range[2];
@@ -93,7 +94,8 @@ term_tile_kernel(const TermBatchArgs a) {
         // tile bound is the k-th largest of (at most 8 per warp) thread maxima, and with fewer than k of them it
         // degenerates to "keep everything" -- 129 records in 32 threads of ONE warp overflowed the 128 slots (the short
         // last tile of a 2.5M-doc shard).  16 * k records = 4 * k quads = k / 8 full warps of 8 published maxima.
-        quads = hi - lo >= max(a.quad_min_recs, 16u * a.topk.k);
+        // (the deep collector takes no bound from thread maxima)
+        quads = hi - lo >= (DEEP ? a.quad_min_recs : max(a.quad_min_recs, 16u * a.topk.k));
     } else if (tq.dir_off != SA_NO_DIR) {                             // CTA-uniform
         const u32 *dir = a.tile_dir + tq.dir_off + tile;
         lo = __ldg(dir);
@@ -295,6 +297,40 @@ term_tile_kernel(const TermBatchArgs a) {
     }
     }
 
+    if constexpr (DEEP) {
+        // 3'. flush the tile's final scores -- de-negated on staged-norm tiles, formed over every doc on the ALL_DOCS
+        //     path -- and write them back to the tile, which the deep collector then ranks.  The barrier: a thread's
+        //     float4s hold scores other threads stored
+        __syncthreads();
+        float4 *__restrict__ out4 = reinterpret_cast<float4 *>(a.out + (u64)q * a.out_stride + tile_doc0);
+#pragma unroll
+        for (int jj = 0; jj < SA_TILE_DOCS / SA_TERM_THREADS / 4; jj++) {
+            const unsigned g = tid + jj * SA_TERM_THREADS;
+            float4 v = reinterpret_cast<const float4 *>(s_out)[g];
+            if (staged_norm) {
+                v.x = __float_as_int(v.x) < 0 ? -v.x : 0.0f;
+                v.y = __float_as_int(v.y) < 0 ? -v.y : 0.0f;
+                v.z = __float_as_int(v.z) < 0 ? -v.z : 0.0f;
+                v.w = __float_as_int(v.w) < 0 ? -v.w : 0.0f;
+            }
+            if (ALL_DOCS && MODE == TERM_MODE_SCORE) {
+                Bm25Params p = a.bm25;
+                p.idf = tq.idf;
+                const u64 d = (u64)tile_doc0 + (u64)g * 4;
+                const float *dl = a.doc_lens + d;
+                v.x = (d + 0 < a.n_docs) ? bm25_one(v.x, dl[0], p) : 0.0f;
+                v.y = (d + 1 < a.n_docs) ? bm25_one(v.y, dl[1], p) : 0.0f;
+                v.z = (d + 2 < a.n_docs) ? bm25_one(v.z, dl[2], p) : 0.0f;
+                v.w = (d + 3 < a.n_docs) ? bm25_one(v.w, dl[3], p) : 0.0f;
+            }
+            __stcs(out4 + g, v);
+            reinterpret_cast<float4 *>(s_out)[g] = v;
+        }
+        __syncthreads();
+        deep_tile_collect(s_out, a.topk, q, tile);
+        return;
+    }
+
     // 3. top-k.  A tile with no more words than candidate slots needs no bound: every positive
     //    score fits.  Otherwise each warp publishes its largest thread maxima and every warp
     //    derives the same tile bound; scores >= bound are this tile's candidates.
@@ -433,7 +469,8 @@ int launch_term_batch(sa_index *ix, const TermBatchArgs &a_in, u32 n_queries, u3
         // tile + d of a query is dispatched group * d CTAs later: d = one generation of resident CTAs, rounded up
         a.prefetch_tiles = (e = getenv("SA_TERM_PREFETCH_TILES"))
                                ? (u32)atol(e)
-                               : std::max(1u, (SA_TERM_CTAS_PER_SM * (u32)ix->num_sms + a.group - 1) / a.group);
+                               : std::max(1u, ((a.topk.k > SA_TOPK_MAX ? SA_TERM_DEEP_CTAS_PER_SM : SA_TERM_CTAS_PER_SM) *
+                                                   (u32)ix->num_sms + a.group - 1) / a.group);
         a.quad_min_recs = std::max(a.quad_min_recs, a.staged_norm_min_recs);   // the quad path reads norms from the staged tile only
     }
     a.tile_dir = ix->d_tile_dir.as<u32>();
@@ -449,16 +486,23 @@ int launch_term_batch(sa_index *ix, const TermBatchArgs &a_in, u32 n_queries, u3
     }
     const dim3 grid(n_queries * n_tiles), block(SA_TERM_THREADS);
     KernelTimer t(ix, 0);
+    // top-k launches score without a payload filter (TF-mode and filtered launches collect nothing): the deep
+    // instances exist for that case only
+    const bool deep = a.topk.k > SA_TOPK_MAX;
+    SA_CHECK(!deep || (a.mode == TERM_MODE_SCORE && !a.filter), "a deep top-k term launch scores without a filter");
     if (a.mode == TERM_MODE_TF) {
-        if (a.filter) term_tile_kernel<TERM_MODE_TF, false, true><<<grid, block, 0, ix->stream>>>(a);
-        else term_tile_kernel<TERM_MODE_TF, false, false><<<grid, block, 0, ix->stream>>>(a);
+        if (a.filter) term_tile_kernel<TERM_MODE_TF, false, true, false><<<grid, block, 0, ix->stream>>>(a);
+        else term_tile_kernel<TERM_MODE_TF, false, false, false><<<grid, block, 0, ix->stream>>>(a);
     } else if (sparse_score) {
-        if (a.filter) term_tile_kernel<TERM_MODE_SCORE, false, true><<<grid, block, 0, ix->stream>>>(a);
-        else term_tile_kernel<TERM_MODE_SCORE, false, false><<<grid, block, 0, ix->stream>>>(a);
+        if (deep) term_tile_kernel<TERM_MODE_SCORE, false, false, true><<<grid, block, 0, ix->stream>>>(a);
+        else if (a.filter) term_tile_kernel<TERM_MODE_SCORE, false, true, false><<<grid, block, 0, ix->stream>>>(a);
+        else term_tile_kernel<TERM_MODE_SCORE, false, false, false><<<grid, block, 0, ix->stream>>>(a);
     } else {
-        if (a.filter) term_tile_kernel<TERM_MODE_SCORE, true, true><<<grid, block, 0, ix->stream>>>(a);
-        else term_tile_kernel<TERM_MODE_SCORE, true, false><<<grid, block, 0, ix->stream>>>(a);
+        if (deep) term_tile_kernel<TERM_MODE_SCORE, true, false, true><<<grid, block, 0, ix->stream>>>(a);
+        else if (a.filter) term_tile_kernel<TERM_MODE_SCORE, true, true, false><<<grid, block, 0, ix->stream>>>(a);
+        else term_tile_kernel<TERM_MODE_SCORE, true, false, false><<<grid, block, 0, ix->stream>>>(a);
     }
+    if (deep) ix->stats.deep_tiles += (u64)n_queries * n_tiles;
     SA_CUDA(cudaGetLastError());
     t.stop();
     ix->stats.term_kernel_launches++;

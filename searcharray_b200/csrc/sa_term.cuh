@@ -13,8 +13,10 @@
 #define SA_STAGED_NORM_MIN_WORDS 1024   // tiles with at least this many posting words stage the tile's norms (sa_term.cu)
 #define SA_STAGED_NORM_MIN_RECS 48      // ... or this many (doc, tf) records on the tf-table path
 #define SA_TERM_CTAS_PER_SM 6           // resident term CTAs per SM (the launch bound); sets the L2 prefetch distance (sa_term.cu)
+#define SA_TERM_DEEP_CTAS_PER_SM 5      // the same for the deep instances: 32 KB tile + 9.3 KB run and histogram each
 #define SA_TERM_QUAD_MIN_RECS 512       // four records per thread from this many records per tile on (and >= 16 * k, sa_term.cu)
 #define SA_TOPK_MAX 32             // warp-level threshold estimation handles k <= 32
+// k in (SA_TOPK_MAX, SA_TOPK_DEEP_MAX] (searcharray_b200.h): each tile keeps its exact top k (deep_tile_collect)
 
 enum TermMode { TERM_MODE_TF = 0, TERM_MODE_SCORE = 1 };
 
@@ -26,7 +28,7 @@ struct TopkCtx {
     u64 *tile_cand;    // [Q][n_tiles][slots] key = score_bits << 32 | (0xFFFFFFFF - local_doc)
     u32 *overflow;     // [Q] set when some tile had more than `slots` candidates
     u32 n_tiles;
-    u32 slots;
+    u32 slots;         // k on the deep path: a tile's candidates are then one run sorted by key, descending
     u32 k;             // 0 => no top-k collection
 };
 
@@ -81,6 +83,9 @@ int sa_ensure_norm(sa_index *ix, float k1, float b, float avg_doc_len);
 int launch_topk_select(sa_index *ix, const TopkCtx &t, u32 n_queries, u64 doc_base, u64 *d_out_keys,
                        const u32 *d_out_index);
 u32 sa_topk_slots(u32 k);
+// Slots of a tile of collect_tile_f64: `shallow` for k <= SA_TOPK_MAX, max(k, 256) above (the deep bound keeps the k
+// best keys plus their ties)
+inline u32 sa_topk_slots_f64(u32 k, u32 shallow) { return k > SA_TOPK_MAX ? std::max(k, 256u) : shallow; }
 // topk_select_kernel for candidates whose key carries a float32 proxy of a float64 score (d_tile_d: the score bits,
 // slot for slot); exact in float64, see sa_topk.cu.  d_out_scores[out_index[q] * k + i] = the float64 scores.
 int launch_topk_select_f64(sa_index *ix, const TopkCtx &t, const u64 *d_tile_d, u32 n_queries, u64 doc_base,
@@ -253,6 +258,125 @@ inline TermBatchArgs make_term_args(sa_index *ix, const TermQuery *d_queries, co
 }
 
 #ifdef __CUDACC__
+// n_pow2 keys in shared memory sorted descending; all threads call
+__device__ inline void bitonic_sort_desc_smem(u64 *s, u32 n_pow2) {
+    for (u32 k = 2; k <= n_pow2; k <<= 1) {
+        for (u32 j = k >> 1; j > 0; j >>= 1) {
+            for (u32 i = threadIdx.x; i < n_pow2; i += blockDim.x) {
+                u32 ixj = i ^ j;
+                if (ixj > i) {
+                    u64 a = s[i], b = s[ixj];
+                    bool desc = ((i & k) == 0);
+                    if ((a < b) == desc) { s[i] = b; s[ixj] = a; }
+                }
+            }
+            __syncthreads();
+        }
+    }
+}
+
+// thread 0: walk the 256-bin histogram from the top until `rem` keys are covered
+__device__ __forceinline__ void radix_pick(const u32 *hist, u32 &rem, int &bin) {
+    u32 acc = 0;
+    int b = 255;
+    for (; b > 0; b--) {
+        if (acc + hist[b] >= rem) break;
+        acc += hist[b];
+    }
+    rem -= acc;
+    bin = b;
+}
+
+// k-th largest, with multiplicity, of the BITS-bit keys `visit` yields (0 when it yields fewer than k): an 8-bit
+// radix select from the most significant digit, as in topk_select_kernel.  All threads call; all get the result.
+template <typename K, int BITS, typename V>
+__device__ K radix_kth_largest(u32 k, u32 *s_hist, K *s_prefix, u32 *s_krem, V visit) {
+    if (threadIdx.x == 0) { *s_prefix = 0; *s_krem = k; }
+    __syncthreads();
+    for (int shift = BITS - 8; shift >= 0; shift -= 8) {
+        for (u32 i = threadIdx.x; i < 256; i += blockDim.x) s_hist[i] = 0;
+        __syncthreads();
+        const K prefix = *s_prefix;
+        visit([&](K key) {
+            if (shift == BITS - 8 || (key >> (shift + 8)) == (prefix >> (shift + 8)))
+                atomicAdd(&s_hist[(u32)(key >> shift) & 255u], 1u);
+        });
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            u32 rem = *s_krem;
+            int b;
+            radix_pick(s_hist, rem, b);
+            *s_krem = rem;
+            *s_prefix = prefix | ((K)(u32)b << shift);
+        }
+        __syncthreads();
+    }
+    return *s_prefix;
+}
+
+// The deep tile collector (k > SA_TOPK_MAX): the tile's EXACT top k by key score_bits << 32 | ~doc, written as one run
+// sorted by key, descending, so that topk_select_kernel<true> reads only the prefix of each run above its threshold.
+// s_tile holds the tile's final float32 scores (a doc ranks iff its score is > 0; NaN never does).  With n ranked
+// docs, n <= k keeps them all; otherwise a radix select over the 48-bit keys score_bits << 16 | (0xFFFF - local) -- the
+// same order, ties to the lower doc -- finds the k-th, and exactly k keys reach it (they are distinct).  The run is
+// sorted in shared memory (<= 8 KB) and stored; tile_cnt = its length, tile_max = its first score.  Never overflows.
+// All SA_TERM_THREADS threads call; returns after a barrier, so the caller may reuse s_tile.
+__device__ __forceinline__ void deep_tile_collect(const float *s_tile, const TopkCtx &t, u32 row, u32 tile) {
+    __shared__ u64 s_run[SA_TOPK_DEEP_MAX];
+    __shared__ u32 s_hist[256];
+    __shared__ u64 s_prefix;
+    __shared__ u32 s_krem, s_n, s_m;
+    const unsigned tid = threadIdx.x;
+    const u32 k = t.k;
+    auto visit = [&](auto f) {
+#pragma unroll
+        for (int jj = 0; jj < SA_TILE_DOCS / SA_TERM_THREADS / 4; jj++) {
+            const unsigned g = tid + jj * SA_TERM_THREADS;
+            const float4 v = reinterpret_cast<const float4 *>(s_tile)[g];
+            const float vs[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+            for (int e = 0; e < 4; e++)
+                if (vs[e] > 0.0f) f(((u64)__float_as_uint(vs[e]) << 16) | (u64)(0xFFFFu - (g * 4 + e)));
+        }
+    };
+    if (tid == 0) { s_n = 0; s_m = 0; }
+    __syncthreads();
+    u32 mine = 0;
+    visit([&](u64) { mine++; });
+    mine = __reduce_add_sync(0xffffffffu, mine);
+    if ((tid & 31) == 0 && mine) atomicAdd(&s_n, mine);
+    __syncthreads();
+    const u32 n = s_n;                                               // CTA-uniform
+    const u64 kth = n > k ? radix_kth_largest<u64, 48>(k, s_hist, &s_prefix, &s_krem, visit) : 0ull;
+    const u32 tile_doc0 = tile * SA_TILE_DOCS;
+    visit([&](u64 key) {
+        if (key >= kth) {
+            const u32 slot = atomicAdd(&s_m, 1u);
+            const u32 local = 0xFFFFu - (u32)(key & 0xFFFFu);
+            if (slot < k) s_run[slot] = ((key >> 16) << 32) | (u64)(0xFFFFFFFFu - (tile_doc0 + local));
+        }
+    });
+    const u32 m = min(n, k);
+    if (m > 1) {                                                     // CTA-uniform
+        u32 n2 = 2;
+        while (n2 < m) n2 <<= 1;
+        __syncthreads();
+        for (u32 i = m + tid; i < n2; i += blockDim.x) s_run[i] = 0ull;
+        __syncthreads();
+        bitonic_sort_desc_smem(s_run, n2);
+    } else {
+        __syncthreads();
+    }
+    const u64 t_idx = (u64)row * t.n_tiles + tile;
+    u64 *__restrict__ run = t.tile_cand + t_idx * t.slots;
+    for (u32 i = tid; i < m; i += blockDim.x) run[i] = s_run[i];
+    if (tid == 0) {
+        t.tile_cnt[t_idx] = m;
+        t.tile_max[t_idx] = m ? (u32)(s_run[0] >> 32) : 0u;
+    }
+    __syncthreads();
+}
+
 // BM25 of tf from the doc's cached length norm (sa_ensure_norm): the last two rounded operations of bm25_one
 __device__ __forceinline__ float bm25_from_norm(float tf, float norm, float idf) {
     return __fmul_rn(__fdiv_rn(tf, __fadd_rn(tf, norm)), idf);
@@ -366,11 +490,23 @@ __device__ __forceinline__ u32 tile_bound_width(u32 k, u32 n_holders) { return (
 // ends with, shared with the phrase kernel.  `my_max` = largest score bits this thread put into the
 // tile, `n_items` = number of scores in the tile, `n_holders` = how many threads can hold one of them.  All SA_TERM_THREADS threads must call.
 // STORE = false: collect only (out_tile unused); the tile stays in shared memory for the tie retry either way.
-template <bool STORE = true>
+// DEEP: k > SA_TOPK_MAX, the tile's candidates from deep_tile_collect (my_max, n_items and n_holders unused).
+template <bool STORE = true, bool DEEP = false>
 __device__ __forceinline__ void flush_tile_collect(const float *s_out, float *__restrict__ out_tile, const TopkCtx &t,
                                                    u32 row, u32 tile, u32 my_max, u32 n_items, u32 n_holders, u32 *s_top,
                                                    u32 *s_ncand, u32 *s_tile_max) {
     const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    if constexpr (DEEP) {
+        __syncthreads();                                             // the tile as every thread stored it
+        if constexpr (STORE) {
+#pragma unroll
+            for (int jj = 0; jj < SA_TILE_DOCS / SA_TERM_THREADS / 4; jj++)
+                __stcs(reinterpret_cast<float4 *>(out_tile) + tid + jj * SA_TERM_THREADS,
+                       reinterpret_cast<const float4 *>(s_out)[tid + jj * SA_TERM_THREADS]);
+        }
+        deep_tile_collect(s_out, t, row, tile);
+        return;
+    }
     const u32 k = t.k;
     const u32 tile_doc0 = tile * SA_TILE_DOCS;
     const bool need_bound = k && n_items > k;                        // CTA-uniform
@@ -440,12 +576,26 @@ __device__ __forceinline__ u32 f64_proxy_key(double s) {
 // (position 4g + e of the tile, g = tid + j * SA_TERM_THREADS), my_max their maximum, n_items the positions of the
 // tile; score(local) returns the float64 score of tile position `local` and runs for the stored candidates only.
 // More candidates than slots flags the query's overflow: the caller re-runs it with SA_TILE_DOCS slots, which cannot
-// overflow.  All SA_TERM_THREADS threads must call.
-template <typename F>
+// overflow.  All SA_TERM_THREADS threads must call.  DEEP (k > SA_TOPK_MAX): the bound is the EXACT k-th largest key
+// of the tile (a radix select over the keys in registers; 1 when fewer than k positions rank), and the caller gives
+// the tile max(k, 256) slots.
+template <bool DEEP = false, typename F>
 __device__ __forceinline__ void collect_tile_f64(const u32 (&key)[SA_TILE_DOCS / SA_TERM_THREADS], u32 my_max,
                                                  u32 n_items, const TopkCtx &t, u64 *__restrict__ tile_d, u32 row,
                                                  u32 tile, u32 *s_top, u32 *s_ncand, u32 *s_tile_max, F score) {
     const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    u32 thr;
+    if constexpr (DEEP) {
+        __shared__ u32 s_hist[256], s_kth, s_krem;
+        const u32 kth = radix_kth_largest<u32, 32>(t.k, s_hist, &s_kth, &s_krem, [&](auto f) {
+#pragma unroll
+            for (int i = 0; i < SA_TILE_DOCS / SA_TERM_THREADS; i++)
+                if (key[i]) f(key[i]);
+        });
+        if (tid == 0) { *s_ncand = 0; *s_tile_max = 0; }
+        __syncthreads();
+        thr = max(kth, 1u);
+    } else {
     const bool need_bound = n_items > t.k;                           // CTA-uniform
     if (need_bound) {
         u32 v = my_max;
@@ -456,7 +606,8 @@ __device__ __forceinline__ void collect_tile_f64(const u32 (&key)[SA_TILE_DOCS /
     }
     if (tid == 0) { *s_ncand = 0; *s_tile_max = 0; }
     __syncthreads();
-    const u32 thr = need_bound ? max(cta_kth_bound(s_top, t.k, true), 1u) : 1u;
+    thr = need_bound ? max(cta_kth_bound(s_top, t.k, true), 1u) : 1u;
+    }
     const u64 slot0 = ((u64)row * t.n_tiles + tile) * t.slots;
     u32 cand_max = 0;
 #pragma unroll

@@ -12,24 +12,9 @@
 #define SEL_THREADS 512
 #define SEL_SMEM_KEYS 4096
 
-__device__ void bitonic_sort_desc_smem(u64 *s, u32 n_pow2) {
-    for (u32 k = 2; k <= n_pow2; k <<= 1) {
-        for (u32 j = k >> 1; j > 0; j >>= 1) {
-            for (u32 i = threadIdx.x; i < n_pow2; i += blockDim.x) {
-                u32 ixj = i ^ j;
-                if (ixj > i) {
-                    u64 a = s[i], b = s[ixj];
-                    bool desc = ((i & k) == 0);
-                    if ((a < b) == desc) { s[i] = b; s[ixj] = a; }
-                }
-            }
-            __syncthreads();
-        }
-    }
-}
-
-// visit every candidate key of query q whose tile can hold a key with score bits >= min_score
-template <typename F>
+// visit every candidate key of query q whose tile can hold a key with score bits >= min_score.  RUNS: each tile's
+// candidates are sorted descending (deep_tile_collect), so the visit stops at the first key below min_score.
+template <bool RUNS, typename F>
 __device__ __forceinline__ void for_each_candidate(const TopkCtx &t, u32 q, u32 min_score, F f) {
     const u32 *cnt = t.tile_cnt + (u64)q * t.n_tiles;
     const u32 *tmax = t.tile_max + (u64)q * t.n_tiles;
@@ -38,22 +23,14 @@ __device__ __forceinline__ void for_each_candidate(const TopkCtx &t, u32 q, u32 
         if (tmax[tile] < min_score) continue;
         const u32 n = cnt[tile];
         const u64 *c = cand + (u64)tile * t.slots;
-        for (u32 j = 0; j < n; j++) f(c[j]);
+        for (u32 j = 0; j < n; j++) {
+            if (RUNS && (u32)(c[j] >> 32) < min_score) break;
+            f(c[j]);
+        }
     }
 }
 
-// thread 0: walk the 256-bin histogram from the top until `rem` keys are covered
-__device__ __forceinline__ void radix_pick(const u32 *hist, u32 &rem, int &bin) {
-    u32 acc = 0;
-    int b = 255;
-    for (; b > 0; b--) {
-        if (acc + hist[b] >= rem) break;
-        acc += hist[b];
-    }
-    rem -= acc;
-    bin = b;
-}
-
+template <bool RUNS>
 __global__ void __launch_bounds__(SEL_THREADS)
 topk_select_kernel(TopkCtx t, u64 doc_base, u64 *__restrict__ out_keys, const u32 *__restrict__ out_index) {
     __shared__ u64 s_keys[SEL_SMEM_KEYS];
@@ -109,7 +86,7 @@ topk_select_kernel(TopkCtx t, u64 doc_base, u64 *__restrict__ out_keys, const u3
     //    tiles whose best score is below the threshold are skipped without touching their slots
     if (threadIdx.x == 0) s_n = 0;
     __syncthreads();
-    for_each_candidate(t, q, thr_score, [&](u64 key) {
+    for_each_candidate<RUNS>(t, q, thr_score, [&](u64 key) {
         if ((u32)(key >> 32) >= thr_score) {
             u32 slot = atomicAdd(&s_n, 1u);
             if (slot < SEL_SMEM_KEYS) s_keys[slot] = key;
@@ -133,7 +110,7 @@ topk_select_kernel(TopkCtx t, u64 doc_base, u64 *__restrict__ out_keys, const u3
             for (u32 i = threadIdx.x; i < 256; i += blockDim.x) s_hist[i] = 0;
             __syncthreads();
             const u64 prefix = s_prefix;
-            for_each_candidate(t, q, thr_score, [&](u64 key) {
+            for_each_candidate<RUNS>(t, q, thr_score, [&](u64 key) {
                 if ((u32)(key >> 32) < thr_score) return;
                 bool match = (shift == 56) || ((key >> (shift + 8)) == (prefix >> (shift + 8)));
                 if (match) atomicAdd(&s_hist[(key >> shift) & 255], 1u);
@@ -151,7 +128,7 @@ topk_select_kernel(TopkCtx t, u64 doc_base, u64 *__restrict__ out_keys, const u3
         const u64 kth = s_prefix;
         if (threadIdx.x == 0) s_n = 0;
         __syncthreads();
-        for_each_candidate(t, q, thr_score, [&](u64 key) {
+        for_each_candidate<RUNS>(t, q, thr_score, [&](u64 key) {
             if (key >= kth) {
                 u32 slot = atomicAdd(&s_n, 1u);
                 if (slot < SEL_SMEM_KEYS) s_keys[slot] = key;
@@ -174,33 +151,6 @@ topk_select_kernel(TopkCtx t, u64 doc_base, u64 *__restrict__ out_keys, const u3
     }
 }
 
-// k-th largest, with multiplicity, of the BITS-bit keys `visit` yields (0 when it yields fewer than k): an 8-bit
-// radix select from the most significant digit, as in topk_select_kernel.  All threads call; all get the result.
-template <typename K, int BITS, typename V>
-__device__ K radix_kth_largest(u32 k, u32 *s_hist, K *s_prefix, u32 *s_krem, V visit) {
-    if (threadIdx.x == 0) { *s_prefix = 0; *s_krem = k; }
-    __syncthreads();
-    for (int shift = BITS - 8; shift >= 0; shift -= 8) {
-        for (u32 i = threadIdx.x; i < 256; i += blockDim.x) s_hist[i] = 0;
-        __syncthreads();
-        const K prefix = *s_prefix;
-        visit([&](K key) {
-            if (shift == BITS - 8 || (key >> (shift + 8)) == (prefix >> (shift + 8)))
-                atomicAdd(&s_hist[(u32)(key >> shift) & 255u], 1u);
-        });
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            u32 rem = *s_krem;
-            int b;
-            radix_pick(s_hist, rem, b);
-            *s_krem = rem;
-            *s_prefix = prefix | ((K)(u32)b << shift);
-        }
-        __syncthreads();
-    }
-    return *s_prefix;
-}
-
 typedef unsigned __int128 u128;
 
 // The exact top k of a query whose candidates carry a float32 PROXY of a float64 score (collect_tile_f64: classic
@@ -219,7 +169,8 @@ topk_select_f64_kernel(TopkCtx t, const u64 *__restrict__ tile_d, u64 doc_base, 
     __shared__ u32 s_krem, s_n;
     __shared__ u32 s_thr;
     __shared__ u128 s_prefix;
-    __shared__ u128 s_win[SA_TOPK_MAX];
+    extern __shared__ __align__(16) unsigned char s_dyn[];
+    u128 *s_win = reinterpret_cast<u128 *>(s_dyn);                 // [k], launch_topk_select_f64
     const u32 q = blockIdx.x, k = t.k, T = t.n_tiles;
     const u32 *tmax = t.tile_max + (u64)q * T;
     u32 thr = radix_kth_largest<u32, 32>(k, s_hist, &s_thr, &s_krem, [&](auto f) {
@@ -243,21 +194,23 @@ topk_select_f64_kernel(TopkCtx t, const u64 *__restrict__ tile_d, u64 doc_base, 
     survivors([&](u128 key) {                   // keys are distinct (positions are): at most k reach kth
         if (key >= kth) {
             const u32 slot = atomicAdd(&s_n, 1u);
-            if (slot < SA_TOPK_MAX) s_win[slot] = key;
+            if (slot < k) s_win[slot] = key;
         }
     });
     __syncthreads();
     const u32 n = min(s_n, k);
     const u64 row = out_index ? out_index[q] : q;
-    if (threadIdx.x < n) {
-        const u128 key = s_win[threadIdx.x];
-        u32 rank = 0;
-        for (u32 j = 0; j < n; j++) rank += s_win[j] > key;
-        out_keys[row * k + rank] = ((u64)1 << 32) | (u64)((u32)key - (u32)doc_base);   // (~local) - base == ~(local + base)
-        out_scores[row * k + rank] = __longlong_as_double((long long)(u64)(key >> 32));
-    } else if (threadIdx.x < k) {
-        out_keys[row * k + threadIdx.x] = 0ull;
-        out_scores[row * k + threadIdx.x] = 0.0;
+    for (u32 i = threadIdx.x; i < k; i += blockDim.x) {
+        if (i < n) {
+            const u128 key = s_win[i];
+            u32 rank = 0;
+            for (u32 j = 0; j < n; j++) rank += s_win[j] > key;
+            out_keys[row * k + rank] = ((u64)1 << 32) | (u64)((u32)key - (u32)doc_base);   // (~local) - base == ~(local + base)
+            out_scores[row * k + rank] = __longlong_as_double((long long)(u64)(key >> 32));
+        } else {
+            out_keys[row * k + i] = 0ull;
+            out_scores[row * k + i] = 0.0;
+        }
     }
 }
 
@@ -265,8 +218,9 @@ int launch_topk_select_f64(sa_index *ix, const TopkCtx &t, const u64 *d_tile_d, 
                            u64 *d_out_keys, double *d_out_scores, const u32 *d_out_index) {
     if (n_queries == 0) return SA_OK;
     KernelTimer tm(ix, 1);
-    topk_select_f64_kernel<<<n_queries, SEL_THREADS, 0, ix->stream>>>(t, d_tile_d, doc_base, d_out_keys, d_out_scores,
-                                                                      d_out_index);
+    SA_CHECK(t.k <= SA_TOPK_DEEP_MAX, "k = %u is above %d", t.k, SA_TOPK_DEEP_MAX);
+    topk_select_f64_kernel<<<n_queries, SEL_THREADS, (size_t)t.k * sizeof(u128), ix->stream>>>(
+        t, d_tile_d, doc_base, d_out_keys, d_out_scores, d_out_index);
     SA_CUDA(cudaGetLastError());
     tm.stop();
     ix->stats.topk_kernel_launches++;
@@ -295,11 +249,41 @@ topk_merge_kernel(const u64 *__restrict__ in, u64 rank_stride, u32 world, u32 n_
     for (u32 i = threadIdx.x; i < k; i += blockDim.x) out[(u64)q * k + i] = s_keys[i];
 }
 
+// topk_merge_kernel for world * k > SEL_SMEM_KEYS (k > SA_TOPK_MAX): every rank's list is sorted descending, 0-padded,
+// and its non-zero keys are distinct from every other rank's (the ranks own disjoint doc ranges), so key i of rank r
+// lands at i + (keys greater than it in the other lists), found by binary search: a merge without shared memory.
+__global__ void __launch_bounds__(SEL_THREADS)
+topk_merge_ranked_kernel(const u64 *__restrict__ in, u64 rank_stride, u32 world, u32 k, u64 *__restrict__ out) {
+    const u32 q = blockIdx.x;
+    for (u32 i = threadIdx.x; i < k; i += blockDim.x) out[(u64)q * k + i] = 0ull;
+    __syncthreads();
+    for (u32 x = threadIdx.x; x < world * k; x += blockDim.x) {
+        const u32 r = x / k, i = x % k;
+        const u64 key = in[(u64)r * rank_stride + (u64)q * k + i];
+        if (key == 0ull) continue;
+        u32 pos = i;
+        for (u32 o = 0; o < world && pos < k; o++) {
+            if (o == r) continue;
+            const u64 *l = in + (u64)o * rank_stride + (u64)q * k;
+            u32 lo = 0, hi = k;                                      // first index whose key is below `key`
+            while (lo < hi) {
+                const u32 mid = (lo + hi) >> 1;
+                if (l[mid] > key) lo = mid + 1; else hi = mid;
+            }
+            pos += lo;
+        }
+        if (pos < k) out[(u64)q * k + pos] = key;
+    }
+}
+
 int launch_topk_select(sa_index *ix, const TopkCtx &t, u32 n_queries, u64 doc_base, u64 *d_out_keys,
                        const u32 *d_out_index) {
     if (n_queries == 0) return SA_OK;
     KernelTimer tm(ix, 1);
-    topk_select_kernel<<<n_queries, SEL_THREADS, 0, ix->stream>>>(t, doc_base, d_out_keys, d_out_index);
+    if (t.k > SA_TOPK_MAX)
+        topk_select_kernel<true><<<n_queries, SEL_THREADS, 0, ix->stream>>>(t, doc_base, d_out_keys, d_out_index);
+    else
+        topk_select_kernel<false><<<n_queries, SEL_THREADS, 0, ix->stream>>>(t, doc_base, d_out_keys, d_out_index);
     SA_CUDA(cudaGetLastError());
     tm.stop();
     ix->stats.topk_kernel_launches++;
@@ -309,9 +293,12 @@ int launch_topk_select(sa_index *ix, const TopkCtx &t, u32 n_queries, u64 doc_ba
 
 int launch_topk_merge(sa_index *ix, const u64 *d_in, u64 rank_stride, u32 world, u32 n_queries, u32 k, u64 *d_out) {
     if (n_queries == 0) return SA_OK;
-    SA_CHECK((u64)world * k <= SEL_SMEM_KEYS, "world*k too large for the merge kernel");
+    SA_CHECK(k <= SA_TOPK_DEEP_MAX, "k = %u is above %d for the merge kernel", k, SA_TOPK_DEEP_MAX);
     KernelTimer tm(ix, 1);
-    topk_merge_kernel<<<n_queries, SEL_THREADS, 0, ix->stream>>>(d_in, rank_stride, world, n_queries, k, d_out);
+    if ((u64)world * k <= SEL_SMEM_KEYS)
+        topk_merge_kernel<<<n_queries, SEL_THREADS, 0, ix->stream>>>(d_in, rank_stride, world, n_queries, k, d_out);
+    else
+        topk_merge_ranked_kernel<<<n_queries, SEL_THREADS, 0, ix->stream>>>(d_in, rank_stride, world, k, d_out);
     SA_CUDA(cudaGetLastError());
     tm.stop();
     ix->stats.topk_kernel_launches++;
@@ -319,5 +306,25 @@ int launch_topk_merge(sa_index *ix, const u64 *d_in, u64 rank_stride, u32 world,
     return SA_OK;
 }
 
-// a tile keeps up to 4 * k docs at or above its bound (four docs per thread on the dense tf-table path) plus ties
-u32 sa_topk_slots(u32 k) { return k <= 16 ? 128u : 256u; }
+// a tile keeps up to 4 * k docs at or above its bound (four docs per thread on the dense tf-table path) plus ties; a
+// deep tile (k > SA_TOPK_MAX) keeps at most k
+u32 sa_topk_slots(u32 k) { return k > SA_TOPK_MAX ? k : k <= 16 ? 128u : 256u; }
+
+extern "C" int sa_topk_merge(sa_index *ix, const uint64_t *lists, uint32_t world, uint32_t n_queries, uint32_t k,
+                             uint64_t *out) {
+    SA_CHECK(ix && (n_queries == 0 || (lists && out)), "NULL argument");
+    SA_CHECK(world >= 1 && k >= 1 && k <= SA_TOPK_DEEP_MAX, "world >= 1 and k in [1, %d]", SA_TOPK_DEEP_MAX);
+    if (n_queries == 0) return SA_OK;
+    std::lock_guard<std::mutex> g(ix->mu);
+    SA_CUDA(cudaSetDevice(ix->device));
+    const size_t n_in = (size_t)world * n_queries * k, n_out = (size_t)n_queries * k;
+    DevBuf buf;
+    int rc;
+    if ((rc = buf.reserve((n_in + n_out) * sizeof(u64)))) return rc;
+    SA_CUDA(cudaMemcpyAsync(buf.p, lists, n_in * sizeof(u64), cudaMemcpyHostToDevice, ix->stream));
+    if ((rc = launch_topk_merge(ix, buf.as<u64>(), (u64)n_queries * k, world, n_queries, k, buf.as<u64>() + n_in)))
+        return rc;
+    SA_CUDA(cudaMemcpyAsync(out, buf.as<u64>() + n_in, n_out * sizeof(u64), cudaMemcpyDeviceToHost, ix->stream));
+    SA_CUDA(cudaStreamSynchronize(ix->stream));
+    return SA_OK;
+}

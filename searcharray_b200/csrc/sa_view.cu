@@ -68,7 +68,8 @@ template <int KIND> using TileParams = std::conditional_t<KIND == SA_SIM_BM25, B
 //            float64 scores in tile_d, overflow -> the exact re-run); topk_select_f64_kernel ranks in float64.
 // WHERE (sim_where_tile_kernel): position i scores only where its bit of the mask row of query
 // row_query[blockIdx.y] is set; the others are +0, as a position without the term, before the tile's bound is taken.
-template <int KIND, bool WHERE>
+// DEEP: k > SA_TOPK_MAX, the tile's candidates from deep_tile_collect (classic: collect_tile_f64's deep bound).
+template <int KIND, bool WHERE, bool DEEP>
 __device__ __forceinline__ void sim_tile(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *__restrict__ rows,
                                          const float *__restrict__ doc_lens, u64 n_pos, TileParams<KIND> p,
                                          const double *__restrict__ idf, u32 row0, const TopkCtx &t,
@@ -120,35 +121,35 @@ __device__ __forceinline__ void sim_tile(const float *__restrict__ doc_rows, u64
     }
     const u32 n_items = (u32)min((u64)SA_TILE_DOCS, n_pos - pos0);
     if constexpr (KIND == SA_SIM_CLASSIC) {
-        collect_tile_f64(key, my_max, n_items, t, tile_d, row, tile, s_top, &s_ncand, &s_tile_max, [&](u32 local) {
+        collect_tile_f64<DEEP>(key, my_max, n_items, t, tile_d, row, tile, s_top, &s_ncand, &s_tile_max, [&](u32 local) {
             // the float64 score again, for the few candidates (cheaper than holding 32 doubles per thread)
             const u64 doc = rows ? __ldg(rows + pos0 + local) : pos0 + local;
             return sim_classic(q_idf, __ldg(counts + doc), __ldg(doc_lens + doc));
         });
     } else {
         // nothing reads the scores outside the tile: collect the candidates without storing the row
-        flush_tile_collect<false>(s_out, nullptr, t, row, tile, my_max, n_items,
+        flush_tile_collect<false, DEEP>(s_out, nullptr, t, row, tile, my_max, n_items,
                                   min((u32)SA_TERM_THREADS, (n_items + 3) / 4), s_top, &s_ncand, &s_tile_max);
     }
 }
 
-template <int KIND>
+template <int KIND, bool DEEP>
 __global__ void __launch_bounds__(SA_TERM_THREADS)
 sim_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *__restrict__ rows,
                 const float *__restrict__ doc_lens, u64 n_pos, TileParams<KIND> p, const double *__restrict__ idf,
                 u32 row0, const TopkCtx t, u64 *__restrict__ tile_d) {
-    sim_tile<KIND, false>(doc_rows, doc_stride, rows, doc_lens, n_pos, p, idf, row0, t, tile_d, WhereMask{nullptr, 0},
+    sim_tile<KIND, false, DEEP>(doc_rows, doc_stride, rows, doc_lens, n_pos, p, idf, row0, t, tile_d, WhereMask{nullptr, 0},
                           nullptr);
 }
 
 // sa_score_batch_topk_sim with where_bits: sim_tile_kernel with a document mask over the positions.
-template <int KIND>
+template <int KIND, bool DEEP>
 __global__ void __launch_bounds__(SA_TERM_THREADS)
 sim_where_tile_kernel(const float *__restrict__ doc_rows, u64 doc_stride, const u64 *__restrict__ rows,
                       const float *__restrict__ doc_lens, u64 n_pos, TileParams<KIND> p, const double *__restrict__ idf,
                       u32 row0, const TopkCtx t, u64 *__restrict__ tile_d, const WhereMask wh,
                       const u32 *__restrict__ row_query) {
-    sim_tile<KIND, true>(doc_rows, doc_stride, rows, doc_lens, n_pos, p, idf, row0, t, tile_d, wh, row_query);
+    sim_tile<KIND, true, DEEP>(doc_rows, doc_stride, rows, doc_lens, n_pos, p, idf, row0, t, tile_d, wh, row_query);
 }
 
 // One call's queries and scoring.
@@ -170,24 +171,31 @@ int launch_sim_tiles(sa_index *ix, int kind, const float *counts, const u64 *row
     const u64 stride = sa_padded_docs(ix->n_docs);
     const dim3 grid(t.n_tiles, n);
     KernelTimer tm(ix, 1);
-#define SA_SIM_TILES(KIND, P)                                                                                       \
+#define SA_SIM_TILES(KIND, P, DEEP)                                                                                 \
     if (wh.bits)                                                                                                    \
-        sim_where_tile_kernel<KIND><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(counts, stride, rows, doc_lens, n_pos, \
-                                                                              P, d_idf, row0, t, tile_d, wh,       \
-                                                                              d_row_query);                        \
+        sim_where_tile_kernel<KIND, DEEP><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(counts, stride, rows, doc_lens, \
+                                                                                    n_pos, P, d_idf, row0, t,       \
+                                                                                    tile_d, wh, d_row_query);       \
     else                                                                                                            \
-        sim_tile_kernel<KIND><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(counts, stride, rows, doc_lens, n_pos, P,   \
-                                                                        d_idf, row0, t, tile_d)
-    if (kind == SA_SIM_BM25) { SA_SIM_TILES(SA_SIM_BM25, bm25); }
-    else if (kind == SA_SIM_BM25_IMPACT) { SA_SIM_TILES(SA_SIM_BM25_IMPACT, sim); }
-    else if (kind == SA_SIM_BM25_LEGACY) { SA_SIM_TILES(SA_SIM_BM25_LEGACY, sim); }
-    else { SA_SIM_TILES(SA_SIM_CLASSIC, sim); }
+        sim_tile_kernel<KIND, DEEP><<<grid, SA_TERM_THREADS, 0, ix->stream>>>(counts, stride, rows, doc_lens, n_pos, \
+                                                                              P, d_idf, row0, t, tile_d)
+    const bool deep = t.k > SA_TOPK_MAX;
+    if (kind == SA_SIM_BM25) {
+        if (deep) { SA_SIM_TILES(SA_SIM_BM25, bm25, true); } else { SA_SIM_TILES(SA_SIM_BM25, bm25, false); }
+    } else if (kind == SA_SIM_BM25_IMPACT) {
+        if (deep) { SA_SIM_TILES(SA_SIM_BM25_IMPACT, sim, true); } else { SA_SIM_TILES(SA_SIM_BM25_IMPACT, sim, false); }
+    } else if (kind == SA_SIM_BM25_LEGACY) {
+        if (deep) { SA_SIM_TILES(SA_SIM_BM25_LEGACY, sim, true); } else { SA_SIM_TILES(SA_SIM_BM25_LEGACY, sim, false); }
+    } else {
+        if (deep) { SA_SIM_TILES(SA_SIM_CLASSIC, sim, true); } else { SA_SIM_TILES(SA_SIM_CLASSIC, sim, false); }
+    }
 #undef SA_SIM_TILES
     SA_CUDA(cudaGetLastError());
     tm.stop();
     ix->stats.topk_kernel_launches++;
     ix->stats.total_launches++;
     ix->stats.sim_instances |= 1ull << (2 * kind + (wh.bits ? 1 : 0));
+    if (deep) ix->stats.deep_tiles += (u64)n * t.n_tiles;
     return SA_OK;
 }
 
@@ -313,7 +321,7 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
     SA_CHECK(n_queries == 0 || (terms && term_starts && idf && out_ids && out_scores), "NULL argument");
     SA_CHECK(kind == SA_SIM_BM25 || kind == SA_SIM_BM25_IMPACT || kind == SA_SIM_BM25_LEGACY || kind == SA_SIM_CLASSIC,
              "unknown similarity %d", kind);
-    SA_CHECK(k >= 1 && k <= SA_TOPK_MAX, "k must be in [1, %d]", SA_TOPK_MAX);
+    SA_CHECK(k >= 1 && k <= SA_TOPK_DEEP_MAX, "k must be in [1, %d]", SA_TOPK_DEEP_MAX);
     const bool classic = kind == SA_SIM_CLASSIC;
     int rc;
     for (u32 q = 0; q < n_queries; q++) {
@@ -341,7 +349,7 @@ extern "C" int sa_score_batch_topk_sim(sa_index *ix, int kind, const uint32_t *t
     // BM25 exactly as ops.bm25_score -> sa_op_bm25_score sets it up: float32 parameters, `1 - b` in float32
     SimRun R{kind, make_bm25(0.0f, (float)avg_doc_len, (float)k1, (float)b, false),
              make_sim_params(avg_doc_len, k1, b), terms, term_starts, slop, WhereMask{nullptr, 0}};
-    const u32 n_tiles = sa_n_tiles(n_pos), slots = classic ? 256u : sa_topk_slots(k);
+    const u32 n_tiles = sa_n_tiles(n_pos), slots = classic ? sa_topk_slots_f64(k, 256u) : sa_topk_slots(k);
     const RowPlan plan = sa_plan_rows(ix->n_docs, term_starts, n_queries);
     const u32 chunk = plan.chunk;
     const std::vector<u32> &row_query = plan.row_query;

@@ -773,6 +773,10 @@ class SearchArray(ExtensionArray):
         scores float32[Q,k]): per query the k best scores > 0, by score descending then id ascending, empty
         slots NO_DOC / 0.  Scores never leave HBM except the top-k (sa_score_batch_topk).
 
+        k: 1 <= k <= query.TOPK_MAX (1,024), e.g. k=1000 for first-stage retrieval ahead of a reranker; another k is a
+        ValueError before any device work.  Above 32 every tile keeps its own exact top k, so the first k' results of
+        a call are bit for bit those of the same call at k'.
+
         On a view (arr[mask], arr[a:b], arr[::s], arr.take(idx), a view of a view) the result is the top k of
         `view.score(q, similarity=similarity, slop=slop)`, and the returned ids are POSITIONS IN THE VIEW
         (0 .. len(view) - 1, the index space of view.score), not the parent's doc ids.  Views of a sharded array
@@ -826,7 +830,8 @@ class SearchArray(ExtensionArray):
         bm25_similarity (TypeError), and for a name not set, a name given twice or more than 4 names (ValueError),
         the call is refused before any device work.  On a shard the counts are the shard's own docs.  facets=None
         (the default) returns (docs, scores) as above."""
-        from .query import DISMAX, NESTED, OCCUR, OR_AND, Feature, bool_form, has_dismax, has_field, is_boolean
+        from .query import DISMAX, NESTED, OCCUR, OR_AND, Feature, bool_form, check_k, has_dismax, has_field, is_boolean
+        k = check_k(k)
         queries = list(queries)
         for q in queries:
             if isinstance(q, Feature):

@@ -550,3 +550,15 @@ def feature_terms(clauses, slot):
         if isinstance(f, Feature):
             out[i] = (f.term_id(slot(i, f)), f.param)
     return out
+
+
+# The largest k of the batched top-k (search_topk, fields_topk, edismax_topk): SA_TOPK_DEEP_MAX of
+# include/searcharray_b200.h.  Above 32 every tile keeps its exact top k (the deep collectors).
+TOPK_MAX = 1024
+
+
+def check_k(k, limit=TOPK_MAX):
+    """k as an int, or ValueError unless 1 <= k <= limit: refused before any device work."""
+    if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 1 <= k <= limit:
+        raise ValueError(f"k must be in [1, {limit}], not {k!r}")
+    return int(k)

@@ -399,7 +399,10 @@ def edismax_topk(frame: pd.DataFrame, q: str, qf: List[str], k: int = 10, mm: Op
                  tie: float = 0.0, q_op: str = "OR",
                  similarity: Union[Similarity, Dict[str, Similarity]] = default_bm25):
     """The k best rows of `edismax(...)` (score desc, row asc) without moving the score vector
-    off the GPU.  Returns (rows uint32[k], scores float64[k]); unused slots are 0xFFFFFFFF / 0."""
+    off the GPU.  Returns (rows uint32[k], scores float64[k]); unused slots are 0xFFFFFFFF / 0.  k: 1 <= k <= 1,024
+    (query.TOPK_MAX); another k is a ValueError before any device work."""
+    from .query import check_k
+    k = check_k(k)
     plan = _Plan(frame, q, qf, mm, pf, pf2, pf3, tie, q_op, similarity)
     if not plan.device_ok():
         raise NotImplementedError("edismax_topk needs BM25 similarities on unsliced SearchArray columns")
@@ -544,7 +547,10 @@ def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
     composition above with `where` applied.  The column may be any SearchArray column of the frame, read by a clause
     or not; it takes part in the column checks above.  rows and scores are bit for bit those of the call without
     `facets`.  A pair whose name is not set, a pair given twice or more than 4 pairs is a ValueError before any device
-    work."""
+    work.  k: 1 <= k <= query.TOPK_MAX (1,024), as in SearchArray.search_topk; another k is a ValueError before any
+    device work."""
+    from .query import check_k
+    k = check_k(k)
     if facets is not None:
         docs, scores, _, hits = _fields_topk(frame, queries, k, similarity, slop, where, facets)
         return docs, scores, hits
