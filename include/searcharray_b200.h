@@ -286,6 +286,25 @@ int sa_score_batch_topk_bool(sa_index *index, uint32_t n_nodes, const uint32_t *
                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone, uint32_t n_facets,
                              const uint32_t *facet_field, const uint32_t *facet_slot, uint32_t *out_total,
                              uint32_t *out_facet_counts);
+/* Scoring at given documents, the second stage after a batched top-k (reranker features, window rescoring): replaces
+ * the reference's `arr.score(q)[docs[q]]` (postings.py:652 `score`, indexed at the candidates) without a dense row.
+ * The descriptor arguments are sa_score_batch_topk_bool's, in its order and under its refusals; in place of k, the
+ * mask, the top-k outputs and the counts it takes docs[n_queries * n_per_query] and fills
+ * out_scores[n_queries * n_per_query]: out_scores[q * K + j] (K = n_per_query) is the value at doc docs[q * K + j] of
+ * the dense vector S_q the top-k entry point ranks from -- the fold's float32 s where the doc ranks (s > 0, mm met,
+ * every MUST / FILTER clause matching and no MUST_NOT clause, for top-level and nested nodes alike) and +0.0
+ * elsewhere.  Ids are global (doc_base added), as the top-k returns them; SA_NO_DOC gives 0.0; duplicates and any
+ * order are allowed.  Called on the docs of a top-k call with the same descriptors it returns that call's scores bit
+ * for bit.  Any other id outside [doc_base, doc_base + n_docs), n_queries * n_per_query >= 2^31, and a query with
+ * more than 64 nested nodes are SA_ERR_ARG before any device work.  Term, feature, DisMax and nested clauses are
+ * evaluated at each doc from the index's lists (one thread per (query, doc)); only phrase clauses write their count
+ * rows, as in the top-k. */
+int sa_score_docs_bool(sa_index *index, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                       const uint32_t *clause_node, const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                       const float *clause_idf, const float *clause_weight, const uint8_t *clause_occur,
+                       const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
+                       uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b,
+                       const uint32_t *docs, uint32_t n_per_query, float *out_scores);
 
 /* The same batch in three stages, so a serving loop (or the benchmark) can keep the query
  * descriptors resident and time the device work alone: upload (H2D of descriptors), execute
@@ -426,6 +445,16 @@ int sa_multi_score_batch_topk_bool(sa_multi *multi, uint32_t n_nodes, const uint
                                    uint64_t where_stride, uint32_t *out_docs, float *out_scores, uint32_t *n_redone,
                                    uint32_t n_facets, const uint32_t *facet_field, const uint32_t *facet_slot,
                                    uint32_t *out_total, uint32_t *out_facet_counts);
+/* sa_score_docs_bool over the fields of a multi: sa_multi_score_batch_topk_bool's descriptor arguments up to b, then
+ * the docs (global ids of the fields' document set), n_per_query and out_scores, under sa_score_docs_bool's contract
+ * with sa_multi_score_batch_topk_bool as the top-k it matches. */
+int sa_multi_score_docs_bool(sa_multi *multi, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                             const uint32_t *clause_node, const uint32_t *clause_field, const uint32_t *clause_terms,
+                             const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
+                             const uint8_t *clause_occur, const uint32_t *clause_group, const float *clause_tie,
+                             const uint32_t *mm, uint32_t n_queries, uint32_t slop, const float *avg_doc_len,
+                             const float *k1, const float *b, const uint32_t *docs, uint32_t n_per_query,
+                             float *out_scores);
 
 /* ------------------------------------------------- per-op exports (parity tests)
  * Device implementations of the reference's native ops on raw arrays (host in, host out),

@@ -63,6 +63,8 @@ SIGNATURES = {
     "sa_score_batch_topk_bool": (c_int, [P_void, c_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8, P_u32, P_f32,
                                          P_u32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32, P_u32, c_u64, c_u64, P_u32,
                                          P_f32, P_u32, c_u32, P_u32, P_u32, P_u32, P_u32]),
+    "sa_score_docs_bool": (c_int, [P_void, c_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8, P_u32, P_f32, P_u32,
+                                   c_u32, c_u32, c_f32, c_f32, c_f32, P_u32, c_u32, P_f32]),
     "sa_batch_upload": (c_int, [P_void, P_u32, P_u32, P_f32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32]),
     "sa_batch_execute": (c_int, [P_void]),
     "sa_batch_download": (c_int, [P_void, P_u32, P_f32, P_u32]),
@@ -95,6 +97,8 @@ SIGNATURES = {
     "sa_multi_score_batch_topk_bool": (c_int, [P_void, c_u32, P_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8,
                                                P_u32, P_f32, P_u32, c_u32, c_u32, P_f32, P_f32, P_f32, c_u32, P_u32,
                                                c_u64, c_u64, P_u32, P_f32, P_u32, c_u32, P_u32, P_u32, P_u32, P_u32]),
+    "sa_multi_score_docs_bool": (c_int, [P_void, c_u32, P_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8, P_u32,
+                                         P_f32, P_u32, c_u32, c_u32, P_f32, P_f32, P_f32, P_u32, c_u32, P_f32]),
     "sa_op_popcount64_reduce": (c_int, [P_u64, c_u64, c_int, P_u64, P_f32, P_u64]),
     "sa_op_bm25_score": (c_int, [P_f32, P_f32, c_u64, c_f32, c_f32, c_f32, c_f32, c_int]),
     "sa_op_similarity": (c_int, [c_int, P_f32, P_f32, c_u64, ctypes.c_double, ctypes.c_double, ctypes.c_double,

@@ -151,6 +151,7 @@ struct BoolState {
     DevBuf rows;
     DevBuf d_flags;      // BoolNest::flags
     DevBuf d_where;      // the WhereMask rows of a masked call
+    DevBuf d_docs;       // sa_score_docs_bool: the docs, the scores and the nested-node lists (BoolDocs)
 };
 void BoolStateDelete::operator()(BoolState *s) const { delete s; }
 
@@ -234,32 +235,35 @@ __device__ __forceinline__ void bool_fold_group(float &acc, u32 &hits, u32 &req,
 // DISMAX: member v of a group at owned doc i (sparse-safe, so v >= +0): the running max and left-folded sum of the
 // weighted scores where the group scores (MUST / SHOULD), the hit mask in every role.  s_m / s_t: the thread's strips,
 // doc i at [i * SA_TERM_THREADS].
-__device__ __forceinline__ void bool_dismax_member(float *s_m, float *s_t, u32 &any, int i, float v,
-                                                   const BoolOccur &oc) {
+__device__ __forceinline__ void bool_dismax_member(float &m, float &t, u32 &any, int i, float v, const BoolOccur &oc) {
     if (oc.occur == SA_OCCUR_SHOULD || oc.occur == SA_OCCUR_MUST) {
         const float w = __fmul_rn(oc.weight, v);
-        s_m[i * SA_TERM_THREADS] = fmaxf(s_m[i * SA_TERM_THREADS], w);
-        s_t[i * SA_TERM_THREADS] = __fadd_rn(s_t[i * SA_TERM_THREADS], w);
+        m = fmaxf(m, w);
+        t = __fadd_rn(t, w);
     }
     any |= (v > 0.0f ? 1u : 0u) << i;
 }
 
-// DISMAX, at a group's last member: d = m + (t - m) * tie at each owned doc, rounded step by step as numpy (no FMA),
-// folded under the group's role with the hit mask; the strips and the mask are reset for the next group.
+// DISMAX, at a group's last member, for owned doc i with running max m and sum t: d = m + (t - m) * tie, rounded step
+// by step as numpy (no FMA), folded under the group's role with the hit mask; m and t are reset for the next group.
+__device__ __forceinline__ void bool_dismax_doc_end(float &acc, u32 &hits, u32 &req, u32 &veto, int i, u32 any,
+                                                    float &m, float &t, float tie, u32 occur) {
+    float d = 0.0f;
+    if (occur == SA_OCCUR_SHOULD || occur == SA_OCCUR_MUST) {
+        d = __fadd_rn(m, __fmul_rn(__fsub_rn(t, m), tie));
+        m = t = 0.0f;
+    }
+    bool_fold_group(acc, hits, req, veto, i, d, ((any >> i) & 1u) != 0, occur);
+}
+
+// DISMAX, at a group's last member: bool_dismax_doc_end at each owned doc, then the hit mask is reset.
 template <int N>
 __device__ __forceinline__ void bool_dismax_group_end(float (&acc)[N * 4], u32 (&hits)[N], u32 &req, u32 &veto,
                                                       u32 &any, float *s_m, float *s_t, float tie, u32 occur) {
-    const bool scoring = occur == SA_OCCUR_SHOULD || occur == SA_OCCUR_MUST;
 #pragma unroll
-    for (int i = 0; i < N * 4; i++) {
-        float d = 0.0f;
-        if (scoring) {
-            const float m = s_m[i * SA_TERM_THREADS], t = s_t[i * SA_TERM_THREADS];
-            d = __fadd_rn(m, __fmul_rn(__fsub_rn(t, m), tie));
-            s_m[i * SA_TERM_THREADS] = s_t[i * SA_TERM_THREADS] = 0.0f;
-        }
-        bool_fold_group(acc[i], hits[i >> 2], req, veto, i, d, ((any >> i) & 1u) != 0, occur);
-    }
+    for (int i = 0; i < N * 4; i++)
+        bool_dismax_doc_end(acc[i], hits[i >> 2], req, veto, i, any, s_m[i * SA_TERM_THREADS], s_t[i * SA_TERM_THREADS],
+                            tie, occur);
     any = 0;
 }
 
@@ -502,7 +506,8 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
                     if (NESTED && nested) v = xs[e];
                     else if (xs[e] > 0.0f && d < a.n_docs) v = bm25_from_norm(xs[e], __ldg(ca.norm + d), cl.idf);
                     if (DISMAX && gr.member) {
-                        bool_dismax_member(s_m, s_t, any, j * 4 + e, v, oc);
+                        bool_dismax_member(s_m[(j * 4 + e) * SA_TERM_THREADS], s_t[(j * 4 + e) * SA_TERM_THREADS], any,
+                                           j * 4 + e, v, oc);
                     } else if (OCCUR) {
                         bool_fold_occur(acc[j * 4 + e], hits[j], req, veto, j * 4 + e, v, oc);
                     } else {
@@ -529,7 +534,8 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
                     // bm25.pyx:20-25 over every doc (NaN / inf / -0.0 of exotic parameters)
                     if (!cl.sparse) v = d < a.n_docs ? bm25_one(xs[e], __ldg(ca.doc_lens + d), p) : 0.0f;
                     if (DISMAX && gr.member) {
-                        bool_dismax_member(s_m, s_t, any, j * 4 + e, v, oc);
+                        bool_dismax_member(s_m[(j * 4 + e) * SA_TERM_THREADS], s_t[(j * 4 + e) * SA_TERM_THREADS], any,
+                                           j * 4 + e, v, oc);
                     } else if (OCCUR) {
                         bool_fold_occur(acc[j * 4 + e], hits[j], req, veto, j * 4 + e, v, oc);
                     } else {
@@ -607,6 +613,156 @@ bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const Bool
         __shared__ unsigned long long s_g[3];
         bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, FEATURE, COUNT, DEEP>(a, occ, fld, grp, s_dyn, s_g, nb, wh, feat, cn);
     }
+}
+
+// ----------------------------------------------------------------------------------- scoring at given documents
+// sa_score_docs_bool evaluates the tile fold at a list of documents: one thread per (query, doc), one CTA per 256 docs
+// of one query, every clause looked up at the doc and folded with the tile fold's own device functions, so each value
+// is bit for bit the one bool_tile ranks from (its step 4 at one doc).  A clause absent from a tile, which the tile
+// fold skips, is folded here with its value +0 at the doc: the same result wherever a doc ranks.
+
+// What bool_docs_kernel reads besides BoolArgs.  The per-clause arrays are those of the call's form, NULL above it, as
+// bool_run_group passes them.
+struct BoolDocs {
+    const BoolOccur *occ;
+    const BoolField *fld;
+    const BoolGroup *grp;
+    const BoolFeature *feat;
+    const u32 *nest;         // per clause: 1 for a nested clause (BoolNest::nested); NULL: no nested node
+    const u32 *child;        // per clause: a nested clause's child, as its slot in its query's node list
+    const u32 *node_start;   // per top-level query q: its nested nodes are node_list[node_start[q] .. node_start[q + 1])
+    const u32 *node_list;    // each query's nested nodes, deepest first, as indices of their BoolArgs::queries entries
+    const u32 *docs;         // [n_queries][n_per]: global doc ids in the index's range, or SA_NO_DOC
+    float *out;              // [n_queries][n_per]
+    u32 n_per, chunks;       // docs per query; CTAs per query, ceil(n_per / SA_TERM_THREADS)
+};
+
+// A term clause's tf at local doc dl, read as bool_scatter_term reads it: the doc's record in its tile's slice of the
+// tf table, or the popcounts of the doc's run of posting words; the first of either found by binary search, the words
+// within the tile's slice where the term has a tile directory and within the whole list otherwise.  Returns
+// SA_DOCS_FOUND | tf where the doc is in the list, 0 where it is not.  `ca`: the clause's field (bool_set_field).
+#define SA_DOCS_FOUND (1ull << 32)
+__device__ __forceinline__ u64 bool_docs_tf(const BoolArgs &ca, const BoolClause &cl, u32 dl) {
+    if (cl.n_words == 0) return 0;
+    const u32 tile = dl / SA_TILE_DOCS, rel = dl % SA_TILE_DOCS;
+    if (bool_uses_recs(ca, cl)) {
+        const u32 *__restrict__ dir = ca.rec_dir + cl.dir_off + tile;
+        const u32 *__restrict__ recs = ca.recs + cl.rec_off;
+        u32 lo = __ldg(dir), end = __ldg(dir + 1), hi = end;
+        while (lo < hi) {
+            const u32 mid = (lo + hi) >> 1;
+            if ((__ldg(recs + mid) >> SA_REC_TF_BITS) < rel) lo = mid + 1;
+            else hi = mid;
+        }
+        if (lo == end) return 0;
+        const u32 r = __ldg(recs + lo);
+        return (r >> SA_REC_TF_BITS) == rel ? SA_DOCS_FOUND | (r & SA_REC_TF_MASK) : 0;
+    }
+    const u64 *__restrict__ words = ca.words + cl.word_off;
+    u64 lo = 0, end = cl.n_words;
+    if (cl.dir_off != SA_NO_DIR) {
+        const u32 *__restrict__ dir = ca.tile_dir + cl.dir_off + tile;
+        lo = __ldg(dir);
+        end = __ldg(dir + 1);
+    }
+    const u64 doc = ca.doc_base + dl;                              // as stored in the words
+    u64 hi = end;
+    while (lo < hi) {
+        const u64 mid = (lo + hi) >> 1;
+        if ((__ldg(words + mid) >> SA_KEY_SHIFT) < doc) lo = mid + 1;
+        else hi = mid;
+    }
+    u32 tf = 0;
+    bool found = false;
+    for (u64 j = lo; j < end; j++) {
+        const u64 w = __ldg(words + j);
+        if ((w >> SA_KEY_SHIFT) != doc) break;
+        tf += (u32)__popcll(w & SA_LSB_MASK);
+        found = true;
+    }
+    return found ? SA_DOCS_FOUND | tf : 0;
+}
+
+// Clause c's value v at local doc dl, as bool_tile's step 3 gives it: a nested clause its child's ranked value (in the
+// thread's strip `mine`, slot x.child[c]), a feature clause f(x), a phrase clause BM25 of its count row, a term clause
+// BM25 of its tf -- from the cached norm where the clause is sparse-safe (+0 off its list), else bm25_one at every doc.
+__device__ __forceinline__ float bool_docs_value(const BoolArgs &a, const BoolDocs &x, u32 c, const BoolClause &cl,
+                                                 u32 dl, const float *mine) {
+    if (x.nest && x.nest[c]) return mine[x.child[c] * SA_TERM_THREADS];
+    if (x.feat && cl.row == SA_BOOL_FEATURE_ROW) {
+        const BoolFeature &f = x.feat[c];
+        return bool_feature_value(f, __ldg(f.values + dl));
+    }
+    BoolArgs view = a;
+    if (x.fld) bool_set_field<true>(view, x.fld, cl.field);
+    if (cl.row != SA_BOOL_NO_ROW) {
+        const float r = __ldg(a.rows + (u64)cl.row * a.row_stride + dl);
+        return r > 0.0f ? bm25_from_norm(r, __ldg(view.norm + dl), cl.idf) : 0.0f;
+    }
+    const u64 found_tf = bool_docs_tf(view, cl, dl);
+    const u32 tf = (u32)found_tf;
+    if (cl.sparse) return found_tf ? bm25_from_norm((float)tf, __ldg(view.norm + dl), cl.idf) : 0.0f;
+    Bm25Params p = view.bm25;
+    p.idf = cl.idf;
+    return bm25_one((float)tf, __ldg(view.doc_lens + dl), p);     // bm25.pyx:20-25 over every doc
+}
+
+// The value node bq ranks local doc dl with: its clauses folded in order (bool_fold_occur, or a DisMax group's
+// bool_dismax_member and bool_dismax_doc_end, at the one doc i = 0), +0 where it does not rank.
+__device__ __forceinline__ float bool_docs_node(const BoolArgs &a, const BoolDocs &x, const BoolQuery bq, u32 dl,
+                                                const float *mine) {
+    float acc = 0.0f, m = 0.0f, t = 0.0f;   // the sum; the current DisMax group's running max and sum
+    u32 hits = 0, req = 1u, veto = 0, any = 0;
+    for (u32 c = bq.c0; c < bq.c0 + bq.n; c++) {
+        const BoolClause cl = a.clauses[c];
+        const float v = bool_docs_value(a, x, c, cl, dl, mine);
+        const BoolOccur oc = x.occ ? x.occ[c] : BoolOccur{1.0f, SA_OCCUR_SHOULD};
+        const BoolGroup gr = x.grp ? x.grp[c] : BoolGroup{0.0f, 0u, 0u, 0u};
+        if (gr.member) {
+            bool_dismax_member(m, t, any, 0, v, oc);
+            if (gr.last) {
+                bool_dismax_doc_end(acc, hits, req, veto, 0, any, m, t, gr.tie, oc.occur);
+                any = 0;
+            }
+        } else {
+            bool_fold_occur(acc, hits, req, veto, 0, v, oc);
+        }
+    }
+    return ((req & ~veto) & 1u) && (hits & 0xFFu) >= bq.mm && acc > 0.0f ? acc : 0.0f;
+}
+
+// The thread's pair (q, j): its index q * x.n_per + j in docs and out, and its query q, from the CTA and thread
+// indices read afresh (asm volatile): values computed once at the start stayed live across the fold's division
+// calls (the slow path of __fdiv_rn is a subroutine) and spilled.
+__device__ __forceinline__ u64 bool_docs_at(const BoolDocs &x, u32 q0, u32 *q) {
+    unsigned b, t;
+    asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(b));
+    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+    *q = q0 + b / x.chunks;
+    return (u64)*q * x.n_per + (b % x.chunks) * SA_TERM_THREADS + t;
+}
+
+// Pairs (q, j) of queries [q0, q0 + gridDim.x / x.chunks), j < x.n_per: out = the value query q ranks doc docs[q][j]
+// with, its nested nodes evaluated first, deepest first, each into the thread's strip of s_nest (slot i at
+// [i * SA_TERM_THREADS]); SA_NO_DOC gives +0.
+__global__ void __launch_bounds__(SA_TERM_THREADS)
+bool_docs_kernel(const BoolArgs a, const BoolDocs x, u32 q0) {
+    extern __shared__ float s_nest[];
+    if ((blockIdx.x % x.chunks) * SA_TERM_THREADS + threadIdx.x >= x.n_per) return;   // no barrier follows
+    u32 q;
+    const u32 doc = __ldg(x.docs + bool_docs_at(x, q0, &q));
+    float v = 0.0f;
+    if (doc != SA_NO_DOC) {
+        const u32 dl = doc - (u32)a.doc_base;                      // ids are u32: doc_base + n_docs <= 2^32
+        if (x.nest) {
+            const u32 n0 = x.node_start[q], n1 = x.node_start[q + 1];
+            for (u32 i = n0; i < n1; i++)
+                s_nest[(i - n0) * SA_TERM_THREADS + threadIdx.x] =
+                    bool_docs_node(a, x, a.queries[x.node_list[i]], dl, s_nest + threadIdx.x);
+        }
+        v = bool_docs_node(a, x, a.queries[q], dl, s_nest + threadIdx.x);
+    }
+    x.out[bool_docs_at(x, q0, &q)] = v;
 }
 
 // ------------------------------------------------------------------------------------------------------------ host
@@ -800,6 +956,32 @@ int bool_build_rows(const BoolCall &X, const BoolPlan &P, const BoolInput &in, u
     return SA_OK;
 }
 
+// The kernels' BoolArgs of an uploaded call, without a top-k context: the lead index's lists, norms and BM25
+// parameters below BOOL_FIELDS (the field-table forms read them per clause), the rows, and every query's descriptor
+// from queries[0] on.
+BoolArgs bool_args(const BoolCall &X, const BoolPlan &P) {
+    sa_index *ix = X.lead();
+    BoolArgs a;
+    memset(&a, 0, sizeof(a));
+    if (P.form < BOOL_FIELDS) {
+        a.words = ix->d_words.as<u64>();
+        a.tile_dir = ix->d_tile_dir.as<u32>();
+        a.recs = ix->d_recs.as<u32>();
+        a.rec_dir = ix->d_rec_dir.as<u32>();
+        a.norm = ix->d_norm.as<float>();
+        a.doc_lens = ix->d_doc_lens.as<float>();
+        a.bm25 = make_bm25(1.0f, X.avgdl[0], X.k1[0], X.b[0], ix->doc_lens_nonneg);
+    }
+    const char *d = X.S->desc.as<const char>();
+    a.rows = X.S->rows.as<float>();
+    a.row_stride = sa_padded_docs(ix->n_docs);
+    a.n_docs = ix->n_docs;
+    a.doc_base = ix->doc_base;
+    a.clauses = (const BoolClause *)(d + P.descs.clauses);
+    a.queries = (const BoolQuery *)(d + P.descs.queries);
+    return a;
+}
+
 // Queries [q0, q1) with `slots` candidate slots per tile: their rows, the tile kernel and the selection, enqueued.
 // count: the first pass of a counting call, the top-level launch counting into the call's rows.
 int bool_run_group(const BoolCall &X, const BoolPlan &P, const BoolInput &in, const WhereMask &where, u32 slots,
@@ -811,24 +993,9 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const BoolInput &in, co
     if ((rc = bool_build_rows(X, P, in, q0, q1))) return rc;
     if ((rc = X.cand->reserve(cand_bytes(n_tiles, nq, slots)))) return rc;
     TopkCtx t = make_topk_ctx(X.cand->p, n_tiles, nq, slots, in.k, P.result.ovf(S.d_keys.p) + q0);
-    BoolArgs a;
-    memset(&a, 0, sizeof(a));
-    if (P.form < BOOL_FIELDS) {             // the field-table kernels read these per clause from the field table
-        a.words = ix->d_words.as<u64>();
-        a.tile_dir = ix->d_tile_dir.as<u32>();
-        a.recs = ix->d_recs.as<u32>();
-        a.rec_dir = ix->d_rec_dir.as<u32>();
-        a.norm = ix->d_norm.as<float>();
-        a.doc_lens = ix->d_doc_lens.as<float>();
-        a.bm25 = make_bm25(1.0f, X.avgdl[0], X.k1[0], X.b[0], ix->doc_lens_nonneg);
-    }
+    BoolArgs a = bool_args(X, P);
     const char *d = S.desc.as<const char>();
-    const BoolQuery *queries = (const BoolQuery *)(d + P.descs.queries);
-    a.rows = S.rows.as<float>();
-    a.row_stride = sa_padded_docs(ix->n_docs);
-    a.n_docs = ix->n_docs;
-    a.doc_base = ix->doc_base;
-    a.clauses = (const BoolClause *)(d + P.descs.clauses);
+    const BoolQuery *queries = a.queries;
     a.queries = queries + q0;
     a.topk = t;
     WhereMask wh = where;                   // row 0 of the launch is query q0's
@@ -1260,6 +1427,170 @@ int bool_topk(const BoolCall &X, const BoolInput &in) {
     return bool_collect(X, P, in, where);
 }
 
+// The most nested nodes one top-level query of sa_score_docs_bool may hold (query.SA_BOOL_MAX_NESTED): the kernel keeps
+// their values per thread in dynamic shared memory, 64 x 256 floats at most.
+#define SA_BOOL_DOCS_MAX_NESTED 64
+
+// sa_score_docs_bool reads the phrase clauses' count rows and no nested node's: the phrase rows alone, numbered within
+// launch groups of at most ~4 GB of rows, replace the plan's rows and groups (whose group size also bounds top-k
+// candidate memory, which scoring at docs has none of).
+void bool_docs_rows(const BoolCall &X, const BoolInput &in, BoolPlan &P) {
+    const u32 n_queries = in.n_queries;
+    const u64 stride = sa_padded_docs(X.lead()->n_docs);
+    const u64 group_rows = std::max<u64>(1, (4ull << 30) / (stride * sizeof(float)));
+    std::vector<std::vector<u32>> nodes(n_queries);                  // each top-level query's nodes
+    for (u32 q = 0; q < n_queries; q++) nodes[q].push_back(q);
+    for (u32 n : P.nested) nodes[P.root[n]].push_back(n);
+    auto phrase = [&](u32 c) {
+        const u32 row = P.clauses[c].row;
+        return row != SA_BOOL_NO_ROW && row != SA_BOOL_FEATURE_ROW && !in.nested(c);
+    };
+    P.group_start.assign(1, 0);
+    P.max_rows = 0;
+    u64 rows = 0;
+    for (u32 q = 0; q < n_queries; q++) {
+        u64 need = 0;
+        for (u32 n : nodes[q])
+            for (u32 c = in.node_clause_starts[n]; c < in.node_clause_starts[n + 1]; c++) need += phrase(c);
+        if (q > P.group_start.back() && rows + need > group_rows) {
+            P.group_start.push_back(q);
+            rows = 0;
+        }
+        for (u32 n : nodes[q])
+            for (u32 c = in.node_clause_starts[n]; c < in.node_clause_starts[n + 1]; c++)
+                if (phrase(c)) P.clauses[c].row = (u32)rows++;
+        P.max_rows = std::max(P.max_rows, (u32)rows);
+    }
+    P.group_start.push_back(n_queries);
+}
+
+// Both score-docs entry points, with the call's indexes locked and their device current: the refusals, the outputs
+// zeroed, then the plan with phrase rows alone, its upload, the nested nodes' lists and the docs in two copies, per
+// launch group its phrase rows and one bool_docs_kernel launch, and the scores in one copy.
+int bool_score_docs(const BoolCall &X, const BoolInput &in, const u32 *docs, u32 n_per, float *out) {
+    sa_index *lead = X.lead();
+    BoolState &S = *X.S;
+    const u32 nq = in.n_queries;
+    const u64 n = (u64)nq * n_per;
+    BoolChecked chk;
+    int rc;
+    if ((rc = bool_check(X, in, &chk))) return rc;
+    SA_CHECK(n < (1ull << 31), "n_queries * n_per_query (%llu) must be below 2^31", (unsigned long long)n);
+    for (u64 i = 0; i < n; i++)
+        SA_CHECK(docs[i] == SA_NO_DOC || (docs[i] >= lead->doc_base && docs[i] - lead->doc_base < lead->n_docs),
+                 "docs[%llu] = %u is neither SA_NO_DOC nor a doc of the index ([%llu, %llu))", (unsigned long long)i,
+                 docs[i], (unsigned long long)lead->doc_base, (unsigned long long)(lead->doc_base + lead->n_docs));
+    const u32 n_nodes = in.n_nodes;
+    if (in.clause_node) {                  // each top-level query's nested nodes (references point forward)
+        std::vector<u32> root(n_nodes), count(nq, 0);
+        for (u32 node = 0; node < n_nodes; node++) {
+            if (node < nq) root[node] = node;
+            else count[root[node]]++;
+            for (u32 c = in.node_clause_starts[node]; c < in.node_clause_starts[node + 1]; c++)
+                if (in.nested(c)) root[in.clause_node[c]] = root[node];
+        }
+        for (u32 q = 0; q < nq; q++)
+            SA_CHECK(count[q] <= SA_BOOL_DOCS_MAX_NESTED, "query %u: at most %d nested nodes, not %u", q,
+                     SA_BOOL_DOCS_MAX_NESTED, count[q]);
+    }
+    std::fill(out, out + n, 0.0f);
+    if (chk.empty || n == 0) return SA_OK;
+    BoolPlan P = bool_plan(X, in, chk);
+    bool_docs_rows(X, in, P);
+    WhereMask where;
+    if ((rc = bool_upload(X, in, P, &where))) return rc;
+    // node lists in P.nested's order (deepest first per query), slots by position, each nested clause's child slot
+    std::vector<u32> node_start(nq + 1, 0), node_list, child;
+    size_t max_nested = 0;
+    if (in.clause_node) {
+        std::vector<std::vector<u32>> per_q(nq);
+        for (size_t i = 0; i < P.nested.size(); i++) per_q[P.root[P.nested[i]]].push_back((u32)i);
+        std::vector<u32> slot(n_nodes, 0);
+        for (u32 q = 0; q < nq; q++) {
+            node_start[q] = (u32)node_list.size();
+            for (u32 i : per_q[q]) {
+                slot[P.nested[i]] = (u32)(node_list.size() - node_start[q]);
+                node_list.push_back(nq + i);
+            }
+            max_nested = std::max(max_nested, per_q[q].size());
+        }
+        node_start[nq] = (u32)node_list.size();
+        const u32 c_end = in.node_clause_starts[n_nodes];
+        child.assign(c_end, 0);
+        for (u32 c = 0; c < c_end; c++)
+            if (in.nested(c)) child[c] = slot[in.clause_node[c]];
+    }
+    // d_docs: the docs, the scores, then node_start, node_list and child
+    const size_t docs_at = 0, out_at = (n * 4 + 255) & ~(size_t)255, lists_at = out_at + ((n * 4 + 255) & ~(size_t)255);
+    std::vector<u32> lists_h(node_start);
+    lists_h.insert(lists_h.end(), node_list.begin(), node_list.end());
+    lists_h.insert(lists_h.end(), child.begin(), child.end());
+    if ((rc = S.d_docs.reserve(lists_at + lists_h.size() * sizeof(u32))) || (rc = X.h_pinned->reserve(n * 4)))
+        return rc;
+    char *dd = S.d_docs.as<char>();
+    memcpy(X.h_pinned->p, docs, n * sizeof(u32));
+    SA_CUDA(cudaMemcpyAsync(dd + docs_at, X.h_pinned->p, n * sizeof(u32), cudaMemcpyHostToDevice, lead->stream));
+    if (in.clause_node)
+        SA_CUDA(cudaMemcpyAsync(dd + lists_at, lists_h.data(), lists_h.size() * sizeof(u32), cudaMemcpyHostToDevice,
+                                lead->stream));
+    const char *d = S.desc.as<const char>();
+    const u32 *lists_d = (const u32 *)(dd + lists_at);
+    BoolDocs x;
+    x.occ = P.form >= BOOL_OCCUR ? (const BoolOccur *)(d + P.descs.occur) : nullptr;
+    x.fld = P.form >= BOOL_FIELDS ? (const BoolField *)(d + P.descs.fields) : nullptr;
+    x.grp = P.form >= BOOL_DISMAX ? (const BoolGroup *)(d + P.descs.groups) : nullptr;
+    x.feat = P.features.empty() ? nullptr : (const BoolFeature *)(d + P.descs.features);
+    x.nest = in.clause_node ? (const u32 *)(d + P.descs.nest) : nullptr;
+    x.node_start = lists_d;
+    x.node_list = lists_d + nq + 1;
+    x.child = x.node_list + node_list.size();
+    x.docs = (const u32 *)(dd + docs_at);
+    x.out = (float *)(dd + out_at);
+    x.n_per = n_per;
+    x.chunks = (n_per + SA_TERM_THREADS - 1) / SA_TERM_THREADS;
+    const size_t smem = max_nested * SA_TERM_THREADS * sizeof(float);
+    if (smem > 48 * 1024)
+        SA_CUDA(cudaFuncSetAttribute(bool_docs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const BoolArgs a = bool_args(X, P);
+    for (size_t g = 0; g + 1 < P.group_start.size(); g++) {
+        const u32 q0 = P.group_start[g], q1 = P.group_start[g + 1];
+        if ((rc = bool_build_rows(X, P, in, q0, q1))) return rc;
+        bool_docs_kernel<<<(q1 - q0) * x.chunks, SA_TERM_THREADS, smem, lead->stream>>>(a, x, q0);
+        SA_CUDA(cudaGetLastError());
+        lead->stats.total_launches++;
+    }
+    SA_CUDA(cudaMemcpyAsync(X.h_pinned->p, x.out, n * sizeof(float), cudaMemcpyDeviceToHost, lead->stream));
+    SA_CUDA(cudaStreamSynchronize(lead->stream));
+    memcpy(out, X.h_pinned->p, n * sizeof(float));
+    return SA_OK;
+}
+
+// f(X) under the multi's lock, with its state and candidate buffer, and field 0's pinned staging.  Fields that share
+// an index share its norm cache, which holds one parameter set; each index is locked once, in address order, and its
+// stream swapped to the multi's for the whole call.
+template <typename F>
+int bool_multi_call(sa_multi *m, const float *avg_doc_len, const float *k1, const float *b, F f) {
+    std::lock_guard<std::mutex> g(m->mu);
+    SA_CUDA(cudaSetDevice(m->device));
+    const u32 n_fields = (u32)m->fields.size();
+    std::vector<sa_index *> distinct;
+    for (u32 i = 0; i < n_fields; i++) {
+        for (u32 e = 0; e < i; e++)
+            SA_CHECK(m->fields[e] != m->fields[i] ||
+                     (avg_doc_len[e] == avg_doc_len[i] && k1[e] == k1[i] && b[e] == b[i]),
+                     "fields %u and %u share an index but not their BM25 parameters", e, i);
+        if (std::find(distinct.begin(), distinct.end(), m->fields[i]) == distinct.end()) distinct.push_back(m->fields[i]);
+    }
+    std::sort(distinct.begin(), distinct.end());
+    std::vector<std::unique_ptr<FieldGuard>> guards;
+    for (sa_index *ix : distinct) guards.emplace_back(new FieldGuard(ix, m->stream));
+    if (!m->boolq) m->boolq.reset(new BoolState());
+    const BoolCall X{m->fields, std::vector<float>(avg_doc_len, avg_doc_len + n_fields),
+                     std::vector<float>(k1, k1 + n_fields), std::vector<float>(b, b + n_fields), true, m->boolq.get(),
+                     &m->cand, &m->fields[0]->h_pinned};
+    return f(X);
+}
+
 }  // namespace
 
 // bool_topk under the index's own lock, with its state and buffers.
@@ -1315,29 +1646,62 @@ extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, uint32_t n_nodes, con
                                 clause_idf && clause_weight && clause_occur && mm), "NULL argument");
     SA_CHECK(k >= 1 && k <= SA_TOPK_DEEP_MAX, "k must be in [1, %d]", SA_TOPK_DEEP_MAX);
     if (n_redone) *n_redone = 0;
-    std::lock_guard<std::mutex> g(m->mu);
-    SA_CUDA(cudaSetDevice(m->device));
-    const u32 n_fields = (u32)m->fields.size();
-    // fields that share an index share its norm cache, which holds one parameter set; each index is locked once, in
-    // address order, and its stream swapped to the multi's for the whole call
-    std::vector<sa_index *> distinct;
-    for (u32 f = 0; f < n_fields; f++) {
-        for (u32 e = 0; e < f; e++)
-            SA_CHECK(m->fields[e] != m->fields[f] ||
-                     (avg_doc_len[e] == avg_doc_len[f] && k1[e] == k1[f] && b[e] == b[f]),
-                     "fields %u and %u share an index but not their BM25 parameters", e, f);
-        if (std::find(distinct.begin(), distinct.end(), m->fields[f]) == distinct.end()) distinct.push_back(m->fields[f]);
-    }
-    std::sort(distinct.begin(), distinct.end());
-    std::vector<std::unique_ptr<FieldGuard>> guards;
-    for (sa_index *ix : distinct) guards.emplace_back(new FieldGuard(ix, m->stream));
-    if (!m->boolq) m->boolq.reset(new BoolState());
-    const BoolCall X{m->fields, std::vector<float>(avg_doc_len, avg_doc_len + n_fields),
-                     std::vector<float>(k1, k1 + n_fields), std::vector<float>(b, b + n_fields), true, m->boolq.get(),
-                     &m->cand, &m->fields[0]->h_pinned};
-    const BoolInput in{n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
-                       clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
-                       where_bits, where_n, where_stride, out_docs, out_scores, n_redone, n_facets, facet_field,
-                       facet_slot, out_total, out_facet_counts};
-    return bool_topk(X, in);
+    return bool_multi_call(m, avg_doc_len, k1, b, [&](const BoolCall &X) {
+        const BoolInput in{n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
+                           clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
+                           where_bits, where_n, where_stride, out_docs, out_scores, n_redone, n_facets, facet_field,
+                           facet_slot, out_total, out_facet_counts};
+        return bool_topk(X, in);
+    });
+}
+
+// The value query q ranks doc docs[q * n_per_query + j] with, for each pair: bool_score_docs under the index's lock.
+// Reference: postings.py:652 `score`, indexed at the candidates (arr.score(q)[docs[q]]).
+extern "C" int sa_score_docs_bool(sa_index *ix, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                  const uint32_t *clause_node, const uint32_t *clause_terms,
+                                  const uint32_t *clause_term_starts, const float *clause_idf,
+                                  const float *clause_weight, const uint8_t *clause_occur,
+                                  const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
+                                  uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b,
+                                  const uint32_t *docs, uint32_t n_per_query, float *out_scores) {
+    SA_CHECK(!clause_weight == !clause_occur, "clause_weight and clause_occur are both given or both NULL");
+    SA_CHECK(!clause_group == !clause_tie && (!clause_group || clause_occur),
+             "clause_group and clause_tie are both given (with clause_occur) or both NULL");
+    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
+             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
+    SA_CHECK(ix && ((u64)n_queries * n_per_query == 0 || (docs && out_scores)), "NULL argument");
+    SA_CHECK(n_nodes == 0 || (node_clause_starts && clause_terms && clause_term_starts && clause_idf && mm),
+             "NULL argument");
+    std::lock_guard<std::mutex> g(ix->mu);
+    SA_CUDA(cudaSetDevice(ix->device));
+    if (!ix->boolq) ix->boolq.reset(new BoolState());
+    const BoolCall X{{ix}, {avg_doc_len}, {k1}, {b}, false, ix->boolq.get(), &ix->cand, &ix->h_pinned};
+    const BoolInput in{n_nodes, node_clause_starts, clause_node, nullptr, clause_terms, clause_term_starts, clause_idf,
+                       clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, 1, nullptr, 0, 0,
+                       nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr};
+    return bool_score_docs(X, in, docs, n_per_query, out_scores);
+}
+
+// sa_score_docs_bool over the fields of a multi, under its lock, as sa_multi_score_batch_topk_bool.
+extern "C" int sa_multi_score_docs_bool(sa_multi *m, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                        const uint32_t *clause_node, const uint32_t *clause_field,
+                                        const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                        const float *clause_idf, const float *clause_weight,
+                                        const uint8_t *clause_occur, const uint32_t *clause_group,
+                                        const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
+                                        uint32_t slop, const float *avg_doc_len, const float *k1, const float *b,
+                                        const uint32_t *docs, uint32_t n_per_query, float *out_scores) {
+    SA_CHECK(!clause_group == !clause_tie, "clause_group and clause_tie are both given or both NULL");
+    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
+             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
+    SA_CHECK(m && avg_doc_len && k1 && b && ((u64)n_queries * n_per_query == 0 || (docs && out_scores)),
+             "NULL argument");
+    SA_CHECK(n_nodes == 0 || (node_clause_starts && clause_field && clause_terms && clause_term_starts &&
+                                clause_idf && clause_weight && clause_occur && mm), "NULL argument");
+    return bool_multi_call(m, avg_doc_len, k1, b, [&](const BoolCall &X) {
+        const BoolInput in{n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
+                           clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, 1,
+                           nullptr, 0, 0, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr, nullptr};
+        return bool_score_docs(X, in, docs, n_per_query, out_scores);
+    });
 }

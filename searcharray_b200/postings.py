@@ -326,6 +326,37 @@ class _PreparedBool:
         out = docs, scores, n_redone.value
         return out if self.counts is None else out + (self.counts.hits(),)
 
+    def score_docs(self, docs, slop):
+        """Makes the score-docs call on the same descriptors (sa_score_docs_bool, sa_multi_score_docs_bool): float32
+        [Q, K], the value each query ranks each of its docs with.  docs: uint32 [Q, K] (check_docs)."""
+        b = self.batch
+        out = np.empty(docs.shape, dtype=np.float32)
+        opt = lambda a, p: None if a is None else p(a)      # noqa: E731
+        entry = _lib.lib().sa_score_docs_bool if not self.c_field else _lib.lib().sa_multi_score_docs_bool
+        _lib.check(entry(
+            self.handle, len(b.node_starts) - 1, _lib.p_u32(b.node_starts), opt(b.clause_node, _lib.p_u32),
+            *self.c_field, _lib.p_u32(self.terms), _lib.p_u32(self.c_starts), _lib.p_f32(self.idfs),
+            opt(b.weights, _lib.p_f32), opt(b.occurs, _lib.p_u8), opt(b.groups, _lib.p_u32), opt(b.ties, _lib.p_f32),
+            _lib.p_u32(b.mm), b.n_queries, int(slop), *self.bm25, _lib.p_u32(docs), docs.shape[1], _lib.p_f32(out)))
+        return out
+
+
+def check_docs(docs, n_queries, doc_base, n_docs):
+    """The docs of score_docs / fields_score_docs, checked before any device work: an integer array of shape
+    (n_queries, K) (TypeError for another dtype, ValueError for another shape), each id NO_DOC or a doc of the array,
+    doc_base <= id < doc_base + n_docs (ValueError).  Returns them as contiguous uint32."""
+    d = np.asarray(docs)
+    if d.dtype.kind not in "iu":
+        raise TypeError(f"docs must be an integer array, not dtype {d.dtype}")
+    if d.ndim != 2 or d.shape[0] != n_queries:
+        raise ValueError(f"docs must have shape ({n_queries}, K), one row per query, not {d.shape}")
+    bad = ~((d == _lib.NO_DOC) | ((d >= doc_base) & (d < doc_base + n_docs)))
+    if bad.any():
+        q, j = np.argwhere(bad)[0]
+        raise ValueError(f"docs[{q}, {j}] = {d[q, j]} is neither NO_DOC nor a doc id in [{doc_base}, "
+                         f"{doc_base + n_docs})")
+    return np.ascontiguousarray(d, dtype=np.uint32)
+
 
 class DeviceIndex:
     """Owns one sa_index handle (one shard in one GPU's HBM)."""
@@ -768,7 +799,8 @@ class SearchArray(ExtensionArray):
         return names.index(name)
 
     # -------------------------------------------------- batched, HBM-resident path
-    def search_topk(self, queries, k=10, similarity: Similarity = default_bm25, slop=0, where=None, facets=None):
+    def search_topk(self, queries, k=10, similarity: Similarity = default_bm25, slop=0, where=None, facets=None,
+                    rescore=None):
         """queries: list of str (term) or list[str] (phrase).  Returns (docs uint32[Q,k],
         scores float32[Q,k]): per query the k best scores > 0, by score descending then id ascending, empty
         slots NO_DOC / 0.  Scores never leave HBM except the top-k (sa_score_batch_topk).
@@ -829,9 +861,18 @@ class SearchArray(ExtensionArray):
         that ranks them without `facets`.  On a view (NotImplementedError), under another similarity than
         bm25_similarity (TypeError), and for a name not set, a name given twice or more than 4 names (ValueError),
         the call is refused before any device work.  On a shard the counts are the shard's own docs.  facets=None
-        (the default) returns (docs, scores) as above."""
+        (the default) returns (docs, scores) as above.
+
+        rescore: a query.Rescore re-ranks each query's top window by a second query scored at the window's docs
+        (score_docs), Elasticsearch's `rescore`: the call above at k=rescore.window, with `where` and `facets`, then
+        the top k by c = float32(query_weight * s1) + float32(rescore_weight * s2) (c desc, id asc); the scores
+        returned are c, the hits pass 1's.  A rescore with another number of queries, a window outside [k, 1,024],
+        a view or a similarity other than bm25_similarity is refused before any device work.  On a shard the window
+        is the shard's own top window."""
         from .query import DISMAX, NESTED, OCCUR, OR_AND, Feature, bool_form, check_k, has_dismax, has_field, is_boolean
         k = check_k(k)
+        if rescore is not None:
+            return self._search_topk_rescore(queries, k, similarity, slop, where, facets, rescore)
         queries = list(queries)
         for q in queries:
             if isinstance(q, Feature):
@@ -877,6 +918,58 @@ class SearchArray(ExtensionArray):
                 for f in facets:
                     hits.facets[f][sel] = out[3].facets[f]
         return (docs, scores) if hits is None else (docs, scores, hits)
+
+    def score_docs(self, queries, docs, slop=0, similarity: Similarity = default_bm25):
+        """The value each query ranks each of its candidate docs with, the second stage after search_topk (reranker
+        features, window rescoring): out[q, j] == S_q[docs[q, j]], S_q the dense vector search_topk ranks query q from
+        (.score for a term or phrase, the boolean composition for an Or / And / Bool / DisMax or nested query with
+        Feature clauses), +0 where the doc does not rank.  So score_docs(queries, search_topk(queries, k)[0]) returns
+        search_topk's scores bit for bit.  It replaces `arr.score(q)[docs[q]]` without a dense row per query: every
+        (query, doc) is evaluated on the device from the index's lists (sa_score_docs_bool); only phrase clauses build
+        their count rows, as search_topk does.
+
+        docs: an integer array of shape (len(queries), K), ids as search_topk returns them (global doc ids on a
+        shard), NO_DOC giving 0; duplicates and any order are allowed.  Returns float32 (len(queries), K).  Another
+        dtype (TypeError), another shape or an id out of range (ValueError), a view (NotImplementedError) and a
+        similarity other than bm25_similarity (TypeError) are refused before any device work."""
+        from .query import Feature, Or, has_field, is_boolean
+        queries = list(queries)
+        for q in queries:
+            if isinstance(q, Feature):
+                raise TypeError(f"a Feature is a clause, not a query: write Bool(should=[{q!r}])")
+        if any(has_field(q) for q in queries if is_boolean(q)):
+            raise ValueError("a Field clause names a DataFrame column: score queries over columns with "
+                             "solr.fields_score_docs(frame, queries, rows), not SearchArray.score_docs")
+        self._check_score_docs(similarity)
+        docs = check_docs(docs, len(queries), self.doc_base, len(self))
+        if docs.size == 0:
+            return np.zeros(docs.shape, dtype=np.float32)
+        # plain queries as one-clause Or nodes, which score as .score does: one call at the batch's heaviest form
+        nodes = [q if is_boolean(q) else Or([q]) for q in queries]
+        with self._shared["lock"]:
+            return self._prepare_bool(nodes, similarity).score_docs(docs, slop)
+
+    def _check_score_docs(self, similarity):
+        """score_docs' refusals of the array and the similarity (the boolean path's)."""
+        if self.rows is not None:
+            raise NotImplementedError("score_docs on a view (arr[mask]) is not supported yet; compose .score() on "
+                                      "the view")
+        if not isinstance(similarity, Bm25Similarity):
+            raise TypeError(f"score_docs supports bm25_similarity only, not {similarity!r}")
+
+    def _search_topk_rescore(self, queries, k, similarity, slop, where, facets, rescore):
+        """search_topk with `rescore` (query.Rescore): pass 1 at k=rescore.window, score_docs of the rescore queries
+        at its docs, then the combine and order of query.rescore_window; hits are pass 1's."""
+        from .query import Rescore, rescore_window
+        if not isinstance(rescore, Rescore):
+            raise TypeError(f"rescore is a query.Rescore, not {rescore!r}")
+        queries = list(queries)
+        rescore.check(len(queries), k)
+        self._check_score_docs(similarity)
+        out = self.search_topk(queries, rescore.window, similarity, slop, where, facets)
+        s2 = self.score_docs(rescore.queries, out[0], slop=rescore.slop, similarity=similarity)
+        docs, scores = rescore_window(out[0], out[1], s2, rescore.query_weight, rescore.rescore_weight, k)
+        return (docs, scores) + tuple(out[2:])
 
     @staticmethod
     def _check_topk_similarity(similarity):

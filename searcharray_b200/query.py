@@ -552,6 +552,65 @@ def feature_terms(clauses, slot):
     return out
 
 
+class Rescore:
+    """Window rescoring, as Elasticsearch's `rescore` and Solr's `rq={!rerank}`: the `rescore=` argument of
+    SearchArray.search_topk and solr.fields_topk.  Per query q, the call without `rescore` at k=window ranks the
+    window (pass 1, with its `where=` and `facets=`; hits are pass 1's); s2 is queries[q] scored at the window's docs
+    (SearchArray.score_docs / solr.fields_score_docs, with this slop); each doc's combined score is
+    c = float32(query_weight * s1) + float32(rescore_weight * s2), each product rounded to float32, then the sum; and
+    the result is the top k of the window by (c desc, id asc), with c as its scores and empty slots NO_DOC / 0.
+
+    queries: one query per query of the call, of any form score_docs takes (Field clauses under fields_topk).  window:
+    an int in [k, 1,024] (checked at the call).  Weights are rounded to float32 once and must be finite, with
+    query_weight > 0 and rescore_weight >= 0, so that every c of a ranked doc is > 0 (ValueError otherwise)."""
+
+    def __init__(self, queries, window=100, query_weight=1.0, rescore_weight=1.0, slop=0):
+        self.queries = list(queries)
+        if isinstance(window, bool) or not isinstance(window, (int, np.integer)):
+            raise ValueError(f"a rescore window is an int in [k, {TOPK_MAX}], not {window!r}")
+        self.window = int(window)
+        for name, w in (("query_weight", query_weight), ("rescore_weight", rescore_weight)):
+            if isinstance(w, bool) or not isinstance(w, (int, float, np.integer, np.floating)):
+                raise ValueError(f"{name} is a finite number, not {w!r}")
+            with np.errstate(over="ignore"):
+                w32 = np.float32(w)
+            if not (math.isfinite(float(w)) and np.isfinite(w32)):
+                raise ValueError(f"{name} is finite (in float32), not {w!r}")
+        self.query_weight, self.rescore_weight = np.float32(query_weight), np.float32(rescore_weight)
+        if not self.query_weight > 0:
+            raise ValueError(f"query_weight must be > 0, not {query_weight!r}")
+        if not self.rescore_weight >= 0:
+            raise ValueError(f"rescore_weight must be >= 0, not {rescore_weight!r}")
+        self.slop = slop
+
+    def check(self, n_queries, k):
+        """ValueError unless there is one rescore query per query and k <= window <= TOPK_MAX."""
+        if len(self.queries) != n_queries:
+            raise ValueError(f"Rescore has {len(self.queries)} queries for a call of {n_queries}: one per query")
+        if not k <= self.window <= TOPK_MAX:
+            raise ValueError(f"a rescore window is in [k, {TOPK_MAX}] = [{k}, {TOPK_MAX}], not {self.window}")
+
+    def __repr__(self):
+        return (f"Rescore({self.queries!r}, window={self.window}, query_weight={float(self.query_weight)!r}, "
+                f"rescore_weight={float(self.rescore_weight)!r}, slop={self.slop!r})")
+
+
+def rescore_window(docs, s1, s2, query_weight, rescore_weight, k):
+    """Rescore's combine and order on the host: per row, c = float32(query_weight * s1) + float32(rescore_weight * s2)
+    over the window's docs (uint32 [Q, W], NO_DOC in empty slots, whose c is 0), and the first k by (c desc, id asc)
+    from one argsort of the keys (c_bits << 32) | ~doc.  Returns (docs uint32 [Q, k], c float32 [Q, k])."""
+    from ._lib import NO_DOC
+    docs = np.asarray(docs, dtype=np.uint32)
+    empty = docs == NO_DOC
+    c = np.float32(query_weight) * np.asarray(s1, dtype=np.float32) + np.float32(rescore_weight) * np.asarray(
+        s2, dtype=np.float32)
+    c = np.where(empty, np.float32(0), c).astype(np.float32)
+    # c >= +0 for every doc (s1 > 0, weights and s2 >= 0), so its bits order as it does; an empty slot's key is 0
+    keys = (c.view(np.uint32).astype(np.uint64) << np.uint64(32)) | (~docs).astype(np.uint64)
+    order = np.argsort(~keys, axis=1, kind="stable")[:, :k]
+    return np.take_along_axis(docs, order, axis=1), np.take_along_axis(c, order, axis=1)
+
+
 # The largest k of the batched top-k (search_topk, fields_topk, edismax_topk): SA_TOPK_DEEP_MAX of
 # include/searcharray_b200.h.  Above 32 every tile keeps its exact top k (the deep collectors).
 TOPK_MAX = 1024

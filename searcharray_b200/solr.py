@@ -19,7 +19,7 @@ import numpy as np
 import pandas as pd
 
 from . import _lib
-from .postings import SearchArray, _check_dismax, _PreparedBool, check_facet_keys, pack_where
+from .postings import SearchArray, _check_dismax, _PreparedBool, check_docs, check_facet_keys, pack_where
 from .similarity import Bm25Similarity, Similarity, compute_idf, default_bm25
 
 
@@ -509,9 +509,44 @@ def _fields_topk(frame, queries, k, similarity, slop, where=None, facets=None):
                              None if facets is None else [(p, slot_of[p[0]], p[1]) for p in facets], multi).run(k, slop)
 
 
+def fields_score_docs(frame: pd.DataFrame, queries, rows,
+                      similarity: Union[Similarity, Dict[str, Similarity]] = default_bm25, slop: int = 0):
+    """SearchArray.score_docs over the columns of `frame`: out[q, j] == S_q[rows[q, j]], S_q the composition
+    fields_topk ranks query q from (+0 where the row does not rank), so fields_score_docs(frame, queries,
+    fields_topk(frame, queries, k)[0]) returns fields_topk's scores bit for bit (sa_multi_score_docs_bool).  queries
+    and similarity as in fields_topk, under its refusals and column checks.  rows: an integer array of shape
+    (len(queries), K), ids as fields_topk returns them (global doc ids on a shard), NO_DOC giving 0.  Returns float32
+    (len(queries), K).  Another dtype (TypeError), another shape or an id out of range (ValueError) is refused
+    before any device work."""
+    queries = list(queries)
+    batch, slot_of, arrays, sims = _fields_plan(frame, queries, similarity)
+    rows = check_docs(rows, len(queries), arrays[0].doc_base, len(frame))
+    if rows.size == 0:
+        return np.zeros(rows.shape, dtype=np.float32)
+    multi = _multi_for(arrays)
+    with _locked(multi, arrays):
+        return _PreparedBool(arrays, sims, _clause_slots(batch, slot_of), queries, batch,
+                             multi=multi).score_docs(rows, slop)
+
+
+def _fields_topk_rescore(frame, queries, k, similarity, slop, where, facets, rescore):
+    """fields_topk with `rescore` (query.Rescore), as SearchArray.search_topk's: pass 1 at k=rescore.window,
+    fields_score_docs of the rescore queries at its rows, then query.rescore_window; hits are pass 1's."""
+    from .query import Rescore, rescore_window
+    if not isinstance(rescore, Rescore):
+        raise TypeError(f"rescore is a query.Rescore, not {rescore!r}")
+    queries = list(queries)
+    rescore.check(len(queries), k)
+    _fields_plan(frame, rescore.queries, similarity)        # the rescore queries' refusals, before pass 1
+    out = fields_topk(frame, queries, rescore.window, similarity, slop, where, facets)
+    s2 = fields_score_docs(frame, rescore.queries, out[0], similarity, rescore.slop)
+    docs, scores = rescore_window(out[0], out[1], s2, rescore.query_weight, rescore.rescore_weight, k)
+    return (docs, scores) + tuple(out[2:])
+
+
 def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
                 similarity: Union[Similarity, Dict[str, Similarity]] = default_bm25, slop: int = 0, where=None,
-                facets=None):
+                facets=None, rescore=None):
     """Batched Or / And / Bool queries whose clauses are on several columns of `frame` -- Lucene's
     `+title:star overview:war -overview:trek`, or Elasticsearch's most_fields `title:alien^2 overview:alien` -- ranked
     on the device in one batch.  Every clause is a query.Field(field, term or phrase), or a Boost of one; phrases match
@@ -548,9 +583,14 @@ def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
     or not; it takes part in the column checks above.  rows and scores are bit for bit those of the call without
     `facets`.  A pair whose name is not set, a pair given twice or more than 4 pairs is a ValueError before any device
     work.  k: 1 <= k <= query.TOPK_MAX (1,024), as in SearchArray.search_topk; another k is a ValueError before any
-    device work."""
+    device work.
+
+    rescore: a query.Rescore of queries of this form, as in SearchArray.search_topk -- the top k of the window
+    fields_topk ranks at k=rescore.window, by the combined score c; hits are pass 1's."""
     from .query import check_k
     k = check_k(k)
+    if rescore is not None:
+        return _fields_topk_rescore(frame, queries, k, similarity, slop, where, facets, rescore)
     if facets is not None:
         docs, scores, _, hits = _fields_topk(frame, queries, k, similarity, slop, where, facets)
         return docs, scores, hits
