@@ -235,6 +235,18 @@ int sa_score_batch_topk_sim(sa_index *index, int kind, const uint32_t *terms, co
  * range are SA_ERR_ARG before any device work.  Only the boolean entry points read reserved ids; every other entry
  * point takes them as the out-of-range term ids they are.
  *
+ * Range and In clauses (Elasticsearch's range and terms filters, Lucene's point range and TermInSetQuery): leaves
+ * scored as a constant, v = 1.0f where the clause matches and +0 elsewhere, otherwise as a feature clause (counted
+ * once towards mm, w * v added under MUST / SHOULD, a leaf's role under FILTER / MUST_NOT, not a DisMax member of a
+ * group of two or more); clause_idf[c] must be 0.  A range clause has exactly three entries: SA_RANGE_TERM(slot),
+ * then the float32 bit patterns of lo and hi; it matches where the value x of feature column `slot` has x > 0 and
+ * lo <= x <= hi (NaN bits are refused; -inf / +inf leave a side open).  An In clause is SA_IN_TERM(slot) followed by
+ * one or more codes of facet column `slot` (sa_index_set_facet), each below the facet's n_buckets, duplicates
+ * allowed; it matches where the doc's code is one of them (a doc without a value never does).  A range whose
+ * column's tile bounds miss [lo, hi], or an In whose codes are not in the tile, is absent from the tile, and under
+ * MUST / FILTER the tile is published empty before any list is read (sa_stats.filter_tiles).  A wrong entry count,
+ * NaN bits, a code out of range, a slot not set and a non-zero parameter are SA_ERR_ARG before any device work.
+ *
  * Hit and facet counts (n_facets, facet_field, facet_slot, out_total and out_facet_counts, the last arguments; out_total
  * non-NULL): Lucene's totalHits and Elasticsearch's terms aggregations, counted where the fold decides which docs
  * rank.  out_total[q] is the number of docs query q ranks (the docs whose score the top k is taken from: s > 0 and
@@ -257,10 +269,10 @@ int sa_score_batch_topk_sim(sa_index *index, int kind, const uint32_t *terms, co
 #define SA_OCCUR_FILTER 2
 #define SA_OCCUR_MUST_NOT 3
 #define SA_NO_NODE 0xFFFFFFFFu
-/* Per-document feature columns of an index (popularity, votes, a quality score), read by the feature clauses above.
- * sa_index_set_feature copies values[0 .. n_values) (n_values == the index's n_docs; each finite and >= 0, 0 meaning
- * the doc lacks the feature) into slot `slot` (< SA_MAX_FEATURES), replacing what the slot held, and records per
- * 8,192-doc tile whether any value is > 0.  The index owns the copy and frees it with itself.  A bad argument, or an
+/* Per-document feature columns of an index (popularity, votes, a quality score), read by the feature and range
+ * clauses above.  sa_index_set_feature copies values[0 .. n_values) (n_values == the index's n_docs; each finite and
+ * >= 0, 0 meaning the doc lacks the feature) into slot `slot` (< SA_MAX_FEATURES), replacing what the slot held, and
+ * records per 8,192-doc tile whether any value is > 0 and the min and max of those values.  The index owns the copy and frees it with itself.  A bad argument, or an
  * index whose n_terms reaches SA_FEATURE_TERM_BASE, is SA_ERR_ARG and leaves the index as it was. */
 #define SA_MAX_FEATURES 16
 #define SA_FEATURE_TERM_BASE 0xFF000000u
@@ -268,12 +280,16 @@ int sa_score_batch_topk_sim(sa_index *index, int kind, const uint32_t *terms, co
 #define SA_FEATURE_SATURATION 1
 #define SA_FEATURE_LOG 2
 #define SA_FEATURE_TERM(fn, slot) (SA_FEATURE_TERM_BASE | ((uint32_t)(fn) << 8) | (uint32_t)(slot))
+#define SA_FEATURE_RANGE 0x10
+#define SA_FEATURE_IN 0x11
+#define SA_RANGE_TERM(slot) SA_FEATURE_TERM(SA_FEATURE_RANGE, slot)   /* a feature slot */
+#define SA_IN_TERM(slot) SA_FEATURE_TERM(SA_FEATURE_IN, slot)         /* a facet slot */
 int sa_index_set_feature(sa_index *index, uint32_t slot, const float *values, uint64_t n_values);
 /* Per-document facet columns of an index (a language, a decade, a category), counted by the facet counts above.
  * sa_index_set_facet copies codes[0 .. n_values) (n_values == the index's n_docs) into slot `slot`
  * (< SA_MAX_FACETS), replacing what the slot held: a code in [0, n_buckets) is the doc's bucket, -1 means the doc has
- * no value.  1 <= n_buckets <= SA_FACET_MAX_BUCKETS.  The index owns the copy (uint16 per doc) and frees it with
- * itself.  A bad argument is SA_ERR_ARG and leaves the index as it was. */
+ * no value.  1 <= n_buckets <= SA_FACET_MAX_BUCKETS.  The index owns the copy (uint16 per doc) and, per 8,192-doc
+ * tile, a 1,024-bit set of the codes present (read by In clauses), and frees them with itself.  A bad argument is SA_ERR_ARG and leaves the index as it was. */
 #define SA_MAX_FACETS 8
 #define SA_FACET_MAX_BUCKETS 1024
 int sa_index_set_facet(sa_index *index, uint32_t slot, const int32_t *codes, uint64_t n_values, uint32_t n_buckets);
@@ -351,6 +367,9 @@ typedef struct {
     /* (query, tile) pairs whose candidates the deep collector took (k > 32: the tile's exact top k, sorted), over
      * every batched top-k entry point */
     uint64_t deep_tiles;
+    /* (node, tile) pairs of the boolean entry points' first passes published empty because a MUST / FILTER range or
+     * In clause was absent from the tile (its column's tile bounds or code set miss the clause) */
+    uint64_t filter_tiles;
 } sa_stats;
 int sa_stats_reset(sa_index *index);
 int sa_stats_get(sa_index *index, sa_stats *out);

@@ -9,5 +9,5 @@ from .postings import Hits, SearchArray, Terms, TermsDtype, ws_tokenizer  # noqa
 from .similarity import (Similarity, bm25_similarity, bm25_impact, bm25_legacy_similarity,  # noqa: F401
                          classic_similarity, compute_idf, default_bm25)
 from .indexing import HostIndex, TermDict, TermMissingError  # noqa: F401
-from .query import And, Bool, Boost, DisMax, Feature, Field, Or, Rescore  # noqa: F401
+from .query import And, Bool, Boost, DisMax, Feature, Field, In, Or, Range, Rescore  # noqa: F401
 from .solr import fields_score_docs, fields_topk  # noqa: F401

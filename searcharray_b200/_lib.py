@@ -29,7 +29,8 @@ class SaStats(ctypes.Structure):
                 ("phrase_kernel_launches", c_u64), ("total_launches", c_u64),
                 ("phrase_cont_words", c_u64), ("phrase_matched_docs", c_u64), ("phrase_tile_launches", c_u64),
                 ("bool_instances", c_u64), ("sim_instances", c_u64), ("term_kernel_groups", c_u64),
-                ("deep_tiles", c_u64)]
+                ("deep_tiles", c_u64),
+                ("filter_tiles", c_u64)]
 
 
 # name -> (restype, argtypes); must list EVERY symbol include/searcharray_b200.h declares

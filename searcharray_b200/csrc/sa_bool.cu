@@ -54,6 +54,14 @@
 // of a batch's queries on one tile read the same 32 KB) and put v = f(x) into the shared tile, which the term clauses'
 // fold then reads as it reads BM25 scores.  An Or / And batch with a feature runs as OCCUR.
 //
+// Range and In clauses (filters on a feature or a facet column, scored 1.0f where they match) run in the same
+// instances, as feature clauses whose BoolFeature::fn is SA_FEATURE_RANGE or SA_FEATURE_IN.  Presence: a range is
+// present iff its column's tile flag is set and the tile's [min, max] of values > 0 meets [lo, hi]; an In iff its
+// 32-word code set meets the tile's (one word per lane, __any_sync).  A MUST / FILTER range or In absent from a tile
+// publishes it empty before any list is read, as a mask does, and the tile is counted in the call's skip counter
+// (sa_stats.filter_tiles).  In the fold a range's owners read their float4s of the column, and an In's owners their
+// four uint16 codes as one 8-byte load, testing each against the clause's set with cached loads.
+//
 // COUNT: hit and facet counts (an entry point's out_total non-NULL), in instances of their own (the FEATURE instances
 // with COUNT, an Or / And batch running as OCCUR) so that a batch without counts runs the instances above unchanged.
 // After the tile's collect, s_tile still holds the ranked values (+0 where a doc does not rank); each thread turns its
@@ -126,12 +134,19 @@ struct BoolNest {
     u32 n_tiles;
 };
 
-// A feature clause's column and function (FEATURE instances only), per clause as a.clauses; unused at other clauses.
+// A feature, range or In clause's column and function (FEATURE instances only), per clause as a.clauses; unused at
+// other clauses.
 struct BoolFeature {
-    const float *values;    // the column, float [padded n_docs], zero past n_docs
-    const u32 *tiles;       // its tile flags: 1 where some value of the tile is > 0
+    const float *values;    // feature / range: the column, float [padded n_docs], zero past n_docs
+    const u32 *tiles;       // feature / range: its tile flags (1 where some value of the tile is > 0); In: the facet's
+                            // tile code sets, SA_FACET_SET_WORDS words per tile
     float param;            // SA_FEATURE_SATURATION: pivot; SA_FEATURE_LOG: scaling factor
     u32 fn;                 // SA_FEATURE_*
+    const float2 *bounds;   // range: per tile the (min, max) of the column's values > 0
+    float lo, hi;           // range: the clause matches where x > 0 and lo <= x <= hi
+    const unsigned short *codes;    // In: the facet column, uint16 [padded n_docs], SA_FACET_NONE for no value
+    const u32 *set;         // In: the clause's codes, SA_FACET_SET_WORDS words (in the call's descriptors)
+    u32 *skipped;           // the call's count of (node, tile) pairs an absent MUST / FILTER range or In made empty
 };
 
 // The counts of a COUNT launch: per query of the launch its total and its facet rows, each facet's column and the
@@ -188,17 +203,48 @@ __device__ __forceinline__ void bool_scatter_term(const BoolArgs &a, const BoolC
 }
 
 // FEATURE: v of a doc whose feature value is x: +0 where x is 0, else x, x / (x + pivot) rounded step by step, or
-// log(s + x) in double rounded once (Lucene's FeatureField functions).
+// log(s + x) in double rounded once (Lucene's FeatureField functions); a range clause's 1.0f where lo <= x <= hi.
 __device__ __forceinline__ float bool_feature_value(const BoolFeature &f, float x) {
     if (!(x > 0.0f)) return 0.0f;
+    if (f.fn == SA_FEATURE_RANGE) return f.lo <= x && x <= f.hi ? 1.0f : 0.0f;
     if (f.fn == SA_FEATURE_SATURATION) return __fdiv_rn(x, __fadd_rn(x, f.param));
     if (f.fn == SA_FEATURE_LOG) return __double2float_rn(log(__dadd_rn((double)f.param, (double)x)));
     return x;
 }
 
-// FEATURE: a feature clause's v at the thread's own docs into s_tile (each thread its own float4s, which it reads
-// back in the fold).  Not unrolled: the fold's registers stay live across it.
+// FEATURE: an In clause's v at a doc whose code is c: 1.0f where c is in the clause's set (never for SA_FACET_NONE).
+__device__ __forceinline__ float bool_in_value(const BoolFeature &f, unsigned short c) {
+    return c != SA_FACET_NONE && ((__ldg(f.set + (c >> 5)) >> (c & 31)) & 1u) ? 1.0f : 0.0f;
+}
+
+// FEATURE: whether a feature, range or In clause is present in the tile (warp-uniform, every lane of the warp calls):
+// its column's tile flag, and for a range the tile's bounds meeting [lo, hi]; for an In its set meeting the tile's.
+__device__ __forceinline__ u32 bool_feature_present(const BoolFeature &f, u32 tile, unsigned lane) {
+    if (f.fn == SA_FEATURE_IN) {
+        const u32 w = __ldg(f.tiles + (u64)tile * SA_FACET_SET_WORDS + lane) & __ldg(f.set + lane);
+        return __any_sync(0xFFFFFFFFu, w != 0) ? 1u : 0u;
+    }
+    if (!__ldg(f.tiles + tile)) return 0;
+    if (f.fn != SA_FEATURE_RANGE) return 1;
+    const float2 b = __ldg(f.bounds + tile);
+    return b.x <= f.hi && b.y >= f.lo ? 1u : 0u;
+}
+
+// FEATURE: a feature, range or In clause's v at the thread's own docs into s_tile (each thread its own float4s, which
+// it reads back in the fold; an In clause's four codes in one 8-byte load).  Not unrolled: the fold's registers stay
+// live across it.
 __device__ __forceinline__ void bool_feature_tile(const BoolFeature &f, u32 tile_doc0, float4 *s_tile4) {
+    if (f.fn == SA_FEATURE_IN) {
+        const ushort4 *__restrict__ c4 = reinterpret_cast<const ushort4 *>(f.codes + tile_doc0);
+#pragma unroll 1
+        for (int j = 0; j < SA_TILE_DOCS / SA_TERM_THREADS / 4; j++) {
+            const unsigned g = threadIdx.x + j * SA_TERM_THREADS;
+            const ushort4 c = __ldg(c4 + g);
+            s_tile4[g] = make_float4(bool_in_value(f, c.x), bool_in_value(f, c.y), bool_in_value(f, c.z),
+                                     bool_in_value(f, c.w));
+        }
+        return;
+    }
     const float4 *__restrict__ v4 = reinterpret_cast<const float4 *>(f.values + tile_doc0);
 #pragma unroll 1
     for (int j = 0; j < SA_TILE_DOCS / SA_TERM_THREADS / 4; j++) {
@@ -401,10 +447,13 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
         bool_set_field<FIELDS>(view, fld, cl.field);
         const BoolArgs &ca = FIELDS ? view : a;
         u32 lo = 0, hi = 0;
+        bool filt = false;                  // FEATURE: a range or In clause
         if (NESTED && nb.nested[bq.c0 + c]) {
             hi = nb.flags[(u64)cl.row * nb.n_tiles + tile] != 0;   // the child ranks a doc of the tile
         } else if (FEATURE && cl.row == SA_BOOL_FEATURE_ROW) {
-            hi = __ldg(feat[bq.c0 + c].tiles + tile) != 0;          // some doc of the tile has a value > 0
+            const BoolFeature &f = feat[bq.c0 + c];
+            hi = bool_feature_present(f, tile, lane);               // some doc of the tile can match
+            filt = f.fn >= SA_FEATURE_RANGE;
         } else if (cl.row != SA_BOOL_NO_ROW) {
             hi = 1;                                                 // a phrase row counts as present
         } else if (cl.n_words == 0) {
@@ -435,6 +484,11 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
             } else if (hi > lo) {
                 atomicAdd(&s_present, 1u);
             }
+            // bit 24: an absent MUST / FILTER range or In (above the OCCUR counts, <= 64 << 16)
+            if (FEATURE && filt && hi <= lo) {
+                const u32 o = occ[bq.c0 + c].occur;
+                if (o == SA_OCCUR_MUST || o == SA_OCCUR_FILTER) atomicOr(&s_present, 1u << 24);
+            }
         }
     }
     __syncthreads();
@@ -443,6 +497,7 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
     //    (DISMAX: fewer SHOULD groups with a member in the tile than mm, or a MUST / FILTER group without one)
     if (DISMAX ? ((u32)__popcll(s_g_present & s_g_should) < bq.mm || (s_g_req & ~s_g_present) != 0)
                : OCCUR ? ((s_present & 0xFFFFu) < bq.mm || (s_present >> 16) != 0) : s_present < bq.mm) {   // CTA-uniform
+        if (FEATURE && (s_present >> 24) && bool_fresh_tid() == 0) atomicAdd(feat[bq.c0].skipped, 1u);
         if (NESTED && nb.store != nullptr) {                        // a nested node: its flag only
             if (tid == 0) nb.flags[(u64)bq.pad * nb.n_tiles + tile] = 0;
             return;
@@ -684,13 +739,14 @@ __device__ __forceinline__ u64 bool_docs_tf(const BoolArgs &ca, const BoolClause
 }
 
 // Clause c's value v at local doc dl, as bool_tile's step 3 gives it: a nested clause its child's ranked value (in the
-// thread's strip `mine`, slot x.child[c]), a feature clause f(x), a phrase clause BM25 of its count row, a term clause
+// thread's strip `mine`, slot x.child[c]), a feature, range or In clause its v, a phrase clause BM25 of its count row, a term clause
 // BM25 of its tf -- from the cached norm where the clause is sparse-safe (+0 off its list), else bm25_one at every doc.
 __device__ __forceinline__ float bool_docs_value(const BoolArgs &a, const BoolDocs &x, u32 c, const BoolClause &cl,
                                                  u32 dl, const float *mine) {
     if (x.nest && x.nest[c]) return mine[x.child[c] * SA_TERM_THREADS];
     if (x.feat && cl.row == SA_BOOL_FEATURE_ROW) {
         const BoolFeature &f = x.feat[c];
+        if (f.fn == SA_FEATURE_IN) return bool_in_value(f, __ldg(f.codes + dl));
         return bool_feature_value(f, __ldg(f.values + dl));
     }
     BoolArgs view = a;
@@ -845,6 +901,11 @@ struct BoolCall {
 
 bool bool_is_feature_term(u32 t) { return t >= SA_FEATURE_TERM_BASE && t != SA_NO_TERM; }
 
+// What a leaf clause is, decided from its entries in one place (BoolInput::kind): a term (one id), a phrase (several
+// ids, or one feature id among several entries, which bool_check refuses), a feature (one reserved id), a range (a
+// reserved id of SA_FEATURE_RANGE, then its bounds' bits) or an In (a reserved id of SA_FEATURE_IN, then its codes).
+enum BoolKind { KIND_TERM, KIND_PHRASE, KIND_FEATURE, KIND_RANGE, KIND_IN };
+
 // A call's arrays and scalars as its entry point was given them, in the entry points' argument order.
 // clause_weight / clause_occur NULL: Or / And, every clause SHOULD with weight 1, mm over all.  clause_field NULL:
 // every clause on field 0.  clause_group / clause_tie non-NULL (with clause_occur): DisMax groups, on a field table.
@@ -873,7 +934,19 @@ struct BoolInput {
     u32 field(u32 c) const { return clause_field ? clause_field[c] : 0; }
     const u32 *terms(u32 c) const { return clause_terms + clause_term_starts[c]; }
     u32 n_terms(u32 c) const { return clause_term_starts[c + 1] - clause_term_starts[c]; }
-    bool feature(u32 c) const { return n_terms(c) == 1 && bool_is_feature_term(terms(c)[0]); }
+    // clause c's kind (a leaf with at least one entry)
+    BoolKind kind(u32 c) const {
+        const u32 t = terms(c)[0], n = n_terms(c);
+        if (bool_is_feature_term(t)) {
+            const u32 fn = (t >> 8) & 0xFFFFu;
+            if (fn == SA_FEATURE_RANGE) return KIND_RANGE;
+            if (fn == SA_FEATURE_IN) return KIND_IN;
+            if (n == 1) return KIND_FEATURE;
+        }
+        return n == 1 ? KIND_TERM : KIND_PHRASE;
+    }
+    // a feature, range or In clause: a column of its field's index, scored without BM25
+    bool column(u32 c) const { return kind(c) >= KIND_FEATURE; }
     // clause c of a node with clauses [c0, c1) is a member of a DisMax group of two or more clauses
     bool member(u32 c, u32 c0, u32 c1) const {
         return clause_group && ((c > c0 && clause_group[c] == clause_group[c - 1]) ||
@@ -883,18 +956,19 @@ struct BoolInput {
 
 // What bool_check learns of a call for the steps after it.
 struct BoolChecked {
-    bool features = false;  // some clause is a feature
+    bool features = false;  // some clause is a feature, range or In
     bool empty = false;     // nothing can rank: no query, no doc, or every field's avgdl 0 and no feature
     BoolCount count{};      // counting: the facets' columns and bins (the rows are placed per launch)
 };
 
 // Where each descriptor array of a call starts, in bytes, in BoolState::desc and in the host block it is uploaded
 // from in one copy: one section per array, each 256-byte aligned.
-struct BoolDescs { size_t clauses, queries, occur, groups, nest, fields, features, bytes; };
+struct BoolDescs { size_t clauses, queries, occur, groups, nest, fields, features, sets, bytes; };
 
 // The result block of a call, in BoolState::d_keys and downloaded whole into the pinned staging: the keys
 // [n_queries][k], then the overflow flags [n_queries] and, counting, the totals [n_queries] and the facet rows
-// [n_queries][n_bins].  `base` is either copy.
+// [n_queries][n_bins], then the tiles absent range and In filters made empty (BoolFeature::skipped).  `base` is either
+// copy.
 struct BoolResult {
     size_t n_keys, n_queries, n_bins;
     bool counting;
@@ -902,7 +976,8 @@ struct BoolResult {
     u32 *ovf(void *base) const { return (u32 *)(keys(base) + n_keys); }
     u32 *total(void *base) const { return ovf(base) + n_queries; }
     u32 *counts(void *base) const { return total(base) + n_queries; }
-    size_t bytes() const { return n_keys * sizeof(u64) + n_queries * sizeof(u32) * (counting ? 2 + n_bins : 1); }
+    u32 *skipped(void *base) const { return ovf(base) + n_queries * (counting ? 2 + n_bins : 1); }
+    size_t bytes() const { return n_keys * sizeof(u64) + (n_queries * (counting ? 2 + n_bins : 1) + 1) * sizeof(u32); }
 };
 
 struct BoolPlan {
@@ -919,7 +994,9 @@ struct BoolPlan {
     std::vector<u32> nested;            // nested nodes by (launch group, depth desc, top-level query);
                                         // queries[n_queries + i] is nested[i]'s descriptor
     std::vector<u32> nest;              // per clause, as clauses: 1 for a nested clause (BOOL_NESTED)
-    std::vector<BoolFeature> features;  // per clause, as clauses, when a clause is a feature (the FEATURE instances)
+    std::vector<BoolFeature> features;  // per clause, as clauses, when a clause is a feature, range or In (the FEATURE
+                                        // instances); an In's `set` and every `skipped` are placed by bool_upload
+    std::vector<u32> sets;              // the In clauses' code sets in clause order, SA_FACET_SET_WORDS words each
     std::vector<char> field_sparse;     // per field slot: 1 with a sparse-safe clause (its norms are cached)
     BoolCount count{};                  // the facet table of bool_check
     BoolDescs descs{};
@@ -1067,6 +1144,34 @@ int bool_check_feature(const sa_index *ix, u32 c, u32 term, float param) {
     return SA_OK;
 }
 
+// A range clause's entries (its reserved id, then the bits of lo and hi) and parameter, on index ix: SA_ERR_ARG unless
+// its slot is a feature set on ix, it has three entries, neither bound is NaN and the parameter is 0.
+int bool_check_range(const sa_index *ix, u32 c, const u32 *e, u32 n, float param) {
+    const u32 slot = e[0] & 0xFFu;
+    SA_CHECK(slot < SA_MAX_FEATURES && (ix->feature_set >> slot & 1u), "clause %u: feature slot %u is not set", c,
+             slot);
+    SA_CHECK(n == 3, "clause %u: a range clause has 3 entries (id, lo, hi), not %u", c, n);
+    float lo, hi;
+    memcpy(&lo, e + 1, sizeof(float));
+    memcpy(&hi, e + 2, sizeof(float));
+    SA_CHECK(!std::isnan(lo) && !std::isnan(hi), "clause %u: a range bound is NaN", c);
+    SA_CHECK(param == 0.0f, "clause %u: a range clause takes no parameter (0)", c);
+    return SA_OK;
+}
+
+// An In clause's entries (its reserved id, then its codes) and parameter, on index ix: SA_ERR_ARG unless its slot is a
+// facet set on ix, it has a code, every code is below the facet's n_buckets and the parameter is 0.
+int bool_check_in(const sa_index *ix, u32 c, const u32 *e, u32 n, float param) {
+    const u32 slot = e[0] & 0xFFu;
+    SA_CHECK(slot < SA_MAX_FACETS && (ix->facet_set >> slot & 1u), "clause %u: facet slot %u is not set", c, slot);
+    SA_CHECK(n >= 2, "clause %u: an In clause has at least one code", c);
+    for (u32 i = 1; i < n; i++)
+        SA_CHECK(e[i] < ix->facet_buckets[slot], "clause %u: code %u is not below the facet's %u buckets", c, e[i],
+                 ix->facet_buckets[slot]);
+    SA_CHECK(param == 0.0f, "clause %u: an In clause takes no parameter (0)", c);
+    return SA_OK;
+}
+
 // Bm25Params::sparse_ok of a clause with idf `idf` on field f.
 bool bool_sparse(const BoolCall &X, u32 f, float idf) {
     return make_bm25(idf, X.avgdl[f], X.k1[f], X.b[f], X.ix[f]->doc_lens_nonneg).sparse_ok != 0;
@@ -1152,13 +1257,17 @@ int bool_check(const BoolCall &X, const BoolInput &in, BoolChecked *out) {
     for (u32 c = c_begin; c < c_end; c++) {
         if (in.nested(c)) continue;
         const u32 nt = in.n_terms(c);
-        SA_CHECK(in.clause_term_starts[c + 1] > in.clause_term_starts[c] && nt <= SA_MAX_PHRASE_TERMS,
-                 "clause %u: bad number of terms", c);
+        SA_CHECK(in.clause_term_starts[c + 1] > in.clause_term_starts[c], "clause %u: bad number of terms", c);
+        const BoolKind kind = in.kind(c);
+        SA_CHECK(kind == KIND_IN || nt <= SA_MAX_PHRASE_TERMS, "clause %u: bad number of terms", c);
         const u32 f = in.field(c);
         SA_CHECK(f < n_fields, "clause %u: field %u out of range (%u fields)", c, f, n_fields);
         const u32 *tids = in.terms(c);
-        if (in.feature(c)) {
-            if ((rc = bool_check_feature(X.ix[f], c, tids[0], in.clause_idf[c]))) return rc;
+        if (kind >= KIND_FEATURE) {
+            if (kind == KIND_FEATURE) rc = bool_check_feature(X.ix[f], c, tids[0], in.clause_idf[c]);
+            else if (kind == KIND_RANGE) rc = bool_check_range(X.ix[f], c, tids, nt, in.clause_idf[c]);
+            else rc = bool_check_in(X.ix[f], c, tids, nt, in.clause_idf[c]);
+            if (rc) return rc;
             SA_CHECK(!dismax || ((c == c_begin || in.clause_group[c - 1] != in.clause_group[c]) &&
                                  (c + 1 == c_end || in.clause_group[c + 1] != in.clause_group[c])),
                      "clause %u: a feature clause is not a DisMax member", c);
@@ -1178,7 +1287,7 @@ int bool_check(const BoolCall &X, const BoolInput &in, BoolChecked *out) {
     for (u32 n = 0; n < n_nodes; n++) {
         for (u32 c = starts[n]; c < starts[n + 1]; c++) {
             const u32 f = in.field(c);
-            if (in.nested(c) || in.feature(c) || X.avgdl[f] == 0.0f) continue;
+            if (in.nested(c) || in.column(c) || X.avgdl[f] == 0.0f) continue;
             const bool sparse = bool_sparse(X, f, in.clause_idf[c]);
             SA_CHECK(in.n_terms(c) == 1 || sparse, "phrase queries in a batch need ordinary BM25 parameters (k1 > 0, 0 <= b < 1, finite idf)");
             SA_CHECK(!in.member(c, starts[n], starts[n + 1]) || sparse, "clause %u: DisMax members need ordinary BM25 "
@@ -1204,6 +1313,7 @@ BoolDescs bool_descs(const BoolPlan &P, size_t n_fields) {
     L.nest = section(P.nest.size() * sizeof(u32));
     L.fields = section((P.form >= BOOL_FIELDS ? n_fields : 0) * sizeof(BoolField));
     L.features = section(P.features.size() * sizeof(BoolFeature));
+    L.sets = section(P.sets.size() * sizeof(u32));
     L.bytes = end;
     return L;
 }
@@ -1241,7 +1351,7 @@ BoolPlan bool_plan(const BoolCall &X, const BoolInput &in, const BoolChecked &ch
                 P.depth[in.clause_node[c]] = P.depth[n] + 1;
                 continue;
             }
-            q_rows[P.root[n]] += in.n_terms(c) > 1 && X.avgdl[in.field(c)] != 0.0f;
+            q_rows[P.root[n]] += in.kind(c) == KIND_PHRASE && X.avgdl[in.field(c)] != 0.0f;
         }
     }
     P.group_start.push_back(0);
@@ -1295,12 +1405,27 @@ BoolPlan bool_plan(const BoolCall &X, const BoolInput &in, const BoolChecked &ch
             if (dismax)
                 P.groups.push_back(BoolGroup{in.clause_tie[in.clause_group[c]], in.clause_group[c] - c0, member ? 1u : 0u,
                                              member && (c + 1 == c1 || in.clause_group[c + 1] != in.clause_group[c]) ? 1u : 0u});
-            if (in.feature(c)) {            // its column on its field's index
+            if (in.column(c)) {             // its column on its field's index
                 const u32 slot = tids[0] & 0xFFu, fn = (tids[0] >> 8) & 0xFFFFu;
                 P.features.resize(c_end);
-                P.features[P.clauses.size()] = BoolFeature{ix->d_features[slot].as<float>(),
-                                                           ix->d_feature_tiles.as<u32>() + (size_t)slot * n_tiles,
-                                                           in.clause_idf[c], fn};
+                BoolFeature &bf = P.features[P.clauses.size()];
+                bf.fn = fn;
+                if (fn == SA_FEATURE_IN) {
+                    bf.codes = ix->d_facets[slot].as<const unsigned short>();
+                    bf.tiles = ix->d_facet_tiles[slot].as<u32>();
+                    const size_t at = P.sets.size();
+                    P.sets.resize(at + SA_FACET_SET_WORDS, 0u);
+                    for (u32 i = 1; i < nt; i++) P.sets[at + (tids[i] >> 5)] |= 1u << (tids[i] & 31);
+                } else {
+                    bf.values = ix->d_features[slot].as<float>();
+                    bf.tiles = ix->d_feature_tiles.as<u32>() + (size_t)slot * n_tiles;
+                    bf.param = in.clause_idf[c];
+                    if (fn == SA_FEATURE_RANGE) {
+                        bf.bounds = ix->d_feature_bounds.as<float2>() + (size_t)slot * n_tiles;
+                        memcpy(&bf.lo, tids + 1, sizeof(float));
+                        memcpy(&bf.hi, tids + 2, sizeof(float));
+                    }
+                }
                 P.clauses.push_back(BoolClause{0, 0, SA_NO_DIR, SA_NO_DIR, 0.0f, SA_BOOL_FEATURE_ROW, 1u, f});
                 continue;
             }
@@ -1347,7 +1472,15 @@ int bool_upload(const BoolCall &X, const BoolInput &in, const BoolPlan &P, Where
     put(P.descs.occur, P.occur);
     put(P.descs.groups, P.groups);
     put(P.descs.nest, P.nest);
-    put(P.descs.features, P.features);
+    // each In clause's set in the descriptors, and the call's skip counter in its result block
+    std::vector<BoolFeature> feats(P.features);
+    size_t n_sets = 0;
+    for (BoolFeature &f : feats) {
+        f.skipped = P.result.skipped(S.d_keys.p);
+        if (f.codes) f.set = (const u32 *)(S.desc.as<const char>() + P.descs.sets) + SA_FACET_SET_WORDS * n_sets++;
+    }
+    put(P.descs.features, feats);
+    put(P.descs.sets, P.sets);
     if (P.form >= BOOL_FIELDS) {
         std::vector<BoolField> fields;
         for (u32 f = 0; f < n_fields; f++) {
@@ -1387,6 +1520,7 @@ int bool_collect(const BoolCall &X, const BoolPlan &P, const BoolInput &in, cons
     SA_CUDA(cudaStreamSynchronize(lead->stream));
     const std::vector<u32> ovf(R.ovf(h), R.ovf(h) + nq);
     sa_unpack_keys(R.keys(h), R.n_keys, in.out_docs, in.out_scores);
+    lead->stats.filter_tiles += *R.skipped(h);
     if (R.counting) {
         memcpy(in.out_total, R.total(h), (size_t)nq * sizeof(u32));
         if (R.n_bins) memcpy(in.out_facet_counts, R.counts(h), (size_t)nq * R.n_bins * sizeof(u32));

@@ -172,6 +172,7 @@ struct Bm25Params {
 // A query against one shard, as the kernels see it.
 #define SA_NO_DIR 0xFFFFFFFFFFFFFFFFull
 #define SA_FACET_NONE 0xFFFFu           // a facet column's code of a doc without a value (sa_index::d_facets)
+#define SA_FACET_SET_WORDS (SA_FACET_MAX_BUCKETS / 32)   // u32 words of a set of facet codes, one bit per code
 struct TermQuery {
     u64 word_off;      // offset of the term's first word in d_words
     u64 n_words;       // 0 => unknown term (zeros)
@@ -224,13 +225,18 @@ struct sa_index {
     bool norm_valid = false;
     // feature columns (sa_index_set_feature, sa_feature.cu): slot s, when bit s of feature_set is set, is
     // d_features[s] (float [padded n_docs], zero past n_docs) and its tile flags d_feature_tiles[s * n_tiles + t]
-    // (1: some doc of tile t has a value > 0)
+    // (1: some doc of tile t has a value > 0) and bounds d_feature_bounds[s * n_tiles + t] (the min and max of the
+    // tile's values > 0, read by range clauses)
     DevBuf d_features[SA_MAX_FEATURES];
     DevBuf d_feature_tiles;          // u32 [SA_MAX_FEATURES * n_tiles]
+    DevBuf d_feature_bounds;         // float2 [SA_MAX_FEATURES * n_tiles]
     u32 feature_set = 0;
     // facet columns (sa_index_set_facet, sa_feature.cu): slot s, when bit s of facet_set is set, is d_facets[s]
-    // (uint16 [padded n_docs], a doc's bucket or 0xFFFF for none, 0xFFFF past n_docs) with facet_buckets[s] buckets
+    // (uint16 [padded n_docs], a doc's bucket or 0xFFFF for none, 0xFFFF past n_docs) with facet_buckets[s] buckets,
+    // and d_facet_tiles[s] the codes present in each tile (u32 [n_tiles][SA_FACET_SET_WORDS], bit c: code c), read by
+    // In clauses
     DevBuf d_facets[SA_MAX_FACETS];
+    DevBuf d_facet_tiles[SA_MAX_FACETS];
     u32 facet_buckets[SA_MAX_FACETS] = {};
     u32 facet_set = 0;
     // host mirrors for query set-up

@@ -1,30 +1,73 @@
 // sa_feature.cu -- per-document columns of an index: feature columns (sa_index_set_feature), read by the feature
-// clauses of the batched boolean queries, and facet columns (sa_index_set_facet), read by their counting pass
-// (sa_bool.cu).
+// and range clauses of the batched boolean queries, and facet columns (sa_index_set_facet), read by their counting
+// pass and their In clauses (sa_bool.cu).
 //
 // A feature column is stored as float[padded n_docs], zero past n_docs, so the tile fold's float4 loads of a whole
 // tile need no bounds test.  Beside it, one u32 flag per (slot, tile): whether any value of the tile is > 0.  The fold
 // takes a feature clause as present in a tile iff its flag is set, as it takes a term clause present where its list
-// has a doc, so min-should-match and MUST pruning skip the tiles where the feature is absent.
+// has a doc, so min-should-match and MUST pruning skip the tiles where the feature is absent.  And per (slot, tile)
+// the min and max of the tile's values > 0: a range clause is present iff the flag is set and [min, max] meets it.
 //
 // A facet column is stored as uint16[padded n_docs], 0xFFFF for "no value" and past n_docs, so the counting pass
-// reads a thread's four docs as one 8-byte load with no bounds test.
+// reads a thread's four docs as one 8-byte load with no bounds test.  Beside it, per tile, the set of codes present
+// (1,024 bits): an In clause is present in a tile iff its codes meet that set.
 #include <cmath>
 
 #include "sa_term.cuh"
 
-// One CTA per tile: flags[tile] = 1 iff any of the tile's values is > 0.
+// One CTA per tile: flags[tile] = 1 iff any of the tile's values is > 0, and bounds[tile] = (min, max) of those
+// values ((+inf, 0) where there is none).  Values are >= 0, so the bits of the positive ones order as the values do.
 __global__ void __launch_bounds__(SA_TERM_THREADS) feature_tiles_kernel(const float *__restrict__ values,
-                                                                         u32 *__restrict__ flags) {
+                                                                         u32 *__restrict__ flags,
+                                                                         float2 *__restrict__ bounds) {
+    __shared__ u32 s_lo[SA_TERM_THREADS / 32], s_hi[SA_TERM_THREADS / 32];
     const float4 *v4 = reinterpret_cast<const float4 *>(values + (u64)blockIdx.x * SA_TILE_DOCS);
-    bool any = false;
+    u32 lo = 0x7F800000u, hi = 0;          // +inf, +0
 #pragma unroll
     for (int j = 0; j < SA_TILE_DOCS / SA_TERM_THREADS / 4; j++) {
         const float4 x = __ldg(v4 + threadIdx.x + j * SA_TERM_THREADS);
-        any = any || x.x > 0.0f || x.y > 0.0f || x.z > 0.0f || x.w > 0.0f;
+        const float xs[4] = {x.x, x.y, x.z, x.w};
+#pragma unroll
+        for (int e = 0; e < 4; e++) {
+            if (!(xs[e] > 0.0f)) continue;
+            lo = min(lo, __float_as_uint(xs[e]));
+            hi = max(hi, __float_as_uint(xs[e]));
+        }
     }
-    const int found = __syncthreads_or(any);
-    if (threadIdx.x == 0) flags[blockIdx.x] = found ? 1u : 0u;
+    lo = __reduce_min_sync(0xFFFFFFFFu, lo);
+    hi = __reduce_max_sync(0xFFFFFFFFu, hi);
+    if ((threadIdx.x & 31) == 0) {
+        s_lo[threadIdx.x >> 5] = lo;
+        s_hi[threadIdx.x >> 5] = hi;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < SA_TERM_THREADS / 32; w++) {
+            lo = min(lo, s_lo[w]);
+            hi = max(hi, s_hi[w]);
+        }
+        flags[blockIdx.x] = hi != 0 ? 1u : 0u;
+        bounds[blockIdx.x] = make_float2(__uint_as_float(lo), __uint_as_float(hi));
+    }
+}
+
+// One CTA per tile: sets[tile * SA_FACET_SET_WORDS + w] bit b set iff code 32 w + b is some doc's of the tile.
+__global__ void __launch_bounds__(SA_TERM_THREADS) facet_tiles_kernel(const unsigned short *__restrict__ codes,
+                                                                       u32 *__restrict__ sets) {
+    __shared__ u32 s_set[SA_FACET_SET_WORDS];
+    if (threadIdx.x < SA_FACET_SET_WORDS) s_set[threadIdx.x] = 0;
+    __syncthreads();
+    const ushort4 *c4 = reinterpret_cast<const ushort4 *>(codes + (u64)blockIdx.x * SA_TILE_DOCS);
+#pragma unroll
+    for (int j = 0; j < SA_TILE_DOCS / SA_TERM_THREADS / 4; j++) {
+        const ushort4 c = __ldg(c4 + threadIdx.x + j * SA_TERM_THREADS);
+        const unsigned short cs[4] = {c.x, c.y, c.z, c.w};
+#pragma unroll
+        for (int e = 0; e < 4; e++)
+            if (cs[e] != SA_FACET_NONE) atomicOr(s_set + (cs[e] >> 5), 1u << (cs[e] & 31));
+    }
+    __syncthreads();
+    if (threadIdx.x < SA_FACET_SET_WORDS) sets[(u64)blockIdx.x * SA_FACET_SET_WORDS + threadIdx.x] = s_set[threadIdx.x];
 }
 
 extern "C" int sa_index_set_feature(sa_index *ix, uint32_t slot, const float *values, uint64_t n_values) {
@@ -46,6 +89,11 @@ extern "C" int sa_index_set_feature(sa_index *ix, uint32_t slot, const float *va
             return rc;
         SA_CUDA(cudaMemsetAsync(ix->d_feature_tiles.p, 0, ix->d_feature_tiles.cap, ix->stream));
     }
+    if (!ix->d_feature_bounds.p) {
+        if ((rc = ix->d_feature_bounds.allocate(std::max<size_t>((size_t)SA_MAX_FEATURES * n_tiles * sizeof(float2), 16))))
+            return rc;
+        SA_CUDA(cudaMemsetAsync(ix->d_feature_bounds.p, 0, ix->d_feature_bounds.cap, ix->stream));
+    }
     // into a new buffer, which replaces the slot's once it is filled: a failure leaves the slot as it was
     DevBuf col;
     if ((rc = col.allocate(std::max<size_t>(padded * sizeof(float), 16)))) return rc;
@@ -55,7 +103,8 @@ extern "C" int sa_index_set_feature(sa_index *ix, uint32_t slot, const float *va
     }
     u32 *flags = ix->d_feature_tiles.as<u32>() + (size_t)slot * n_tiles;
     if (n_tiles) {
-        feature_tiles_kernel<<<n_tiles, SA_TERM_THREADS, 0, ix->stream>>>(col.as<float>(), flags);
+        feature_tiles_kernel<<<n_tiles, SA_TERM_THREADS, 0, ix->stream>>>(
+            col.as<float>(), flags, ix->d_feature_bounds.as<float2>() + (size_t)slot * n_tiles);
         SA_CUDA(cudaGetLastError());
         ix->stats.total_launches++;
     }
@@ -83,12 +132,21 @@ extern "C" int sa_index_set_facet(sa_index *ix, uint32_t slot, const int32_t *co
     }
     SA_CUDA(cudaSetDevice(ix->device));
     // into a new buffer, which replaces the slot's once it is filled: a failure leaves the slot as it was
-    DevBuf d;
+    const u32 n_tiles = sa_n_tiles(ix->n_docs);
+    DevBuf d, sets;
     int rc;
-    if ((rc = d.allocate(col.size() * sizeof(uint16_t)))) return rc;
+    if ((rc = d.allocate(col.size() * sizeof(uint16_t))) ||
+        (rc = sets.allocate(std::max<size_t>((size_t)n_tiles * SA_FACET_SET_WORDS * sizeof(u32), 16))))
+        return rc;
     SA_CUDA(cudaMemcpyAsync(d.p, col.data(), col.size() * sizeof(uint16_t), cudaMemcpyHostToDevice, ix->stream));
+    if (n_tiles) {
+        facet_tiles_kernel<<<n_tiles, SA_TERM_THREADS, 0, ix->stream>>>(d.as<unsigned short>(), sets.as<u32>());
+        SA_CUDA(cudaGetLastError());
+        ix->stats.total_launches++;
+    }
     SA_CUDA(cudaStreamSynchronize(ix->stream));     // `col` is a local
     ix->d_facets[slot] = std::move(d);
+    ix->d_facet_tiles[slot] = std::move(sets);
     ix->facet_buckets[slot] = n_buckets;
     ix->facet_set |= 1u << slot;
     return SA_OK;

@@ -248,8 +248,8 @@ def _check_dismax(members, clauses, clause_slot, arrays, sims, idfs=None):
 class _PreparedBool:
     """One call of sa_score_batch_topk_bool over one SearchArray, or of sa_multi_score_batch_topk_bool over the columns
     of a solr.fields_topk plan, prepared from a flattened batch (query.BoolBatch): each clause's term ids, term starts
-    and float32 idf from its own column, as that column's .score takes them, the feature columns its clauses read and
-    the counts it fills.  Build it and run it with the arrays' locks held (the array's lock; solr._locked for a
+    and float32 idf from its own column, as that column's .score takes them, the feature and facet columns its clauses
+    read and the counts it fills.  Build it and run it with the arrays' locks held (the array's lock; solr._locked for a
     multi)."""
 
     def __init__(self, arrays, sims, clause_slot, queries, batch, where=None, facets=None, multi=None):
@@ -257,13 +257,13 @@ class _PreparedBool:
         of batch, its slot (0 for a nested clause).  batch: queries flattened (query.flatten_bool).  where: a packed
         mask (pack_where), None: no mask.  facets: (key in Hits.facets, slot, name) triples, None: no counting.
         multi: the solr._Multi over arrays for fields_topk, None for one array.  A facet or feature name not set on its
-        slot's array, and DisMax members whose idf is not sparse-safe, are ValueErrors, the names checked before any
-        device work."""
+        slot's array, an In code past its facet's buckets, and DisMax members whose idf is not sparse-safe, are
+        ValueErrors, the names and codes checked before any device work."""
         from .query import Field, dismax_members
         self.arrays, self.batch, self.where = arrays, batch, where
         self.counts = None if facets is None else _Counts(facets, arrays, batch.n_queries)
         clauses = batch.clauses
-        feats = self.features(clauses, clause_slot, arrays)
+        feats = self.columns(clauses, clause_slot, arrays)
         text = np.asarray([i for i, c in enumerate(clauses) if c is not None and i not in feats], dtype=np.int64)
         n_terms, self.idfs = np.zeros(len(clauses), dtype=np.int64), np.zeros(len(clauses), dtype=np.float32)
         slot_terms = []
@@ -275,18 +275,20 @@ class _PreparedBool:
             n_terms[idx], self.idfs[idx] = np.diff(starts), idf
             slot_terms.append((idx, t, starts))
         f = list(feats)
-        n_terms[f], self.idfs[f] = 1, [param for _, param in feats.values()]
+        n_terms[f], self.idfs[f] = [len(e) for e, _ in feats.values()], [param for _, param in feats.values()]
         self.c_starts = np.concatenate([[0], np.cumsum(n_terms)]).astype(np.uint32)
-        # each slot's text clauses' terms from their clause's start on, each feature clause's reserved id at its start
+        # each slot's text clauses' terms from their clause's start on, each column clause's entries from its start
         self.terms = np.empty(int(self.c_starts[-1]), dtype=np.uint32)
         for idx, t, starts in slot_terms:
             first = self.c_starts[idx].astype(np.int64) - starts[:-1]
             self.terms[np.repeat(first, np.diff(starts)) + np.arange(len(t))] = t
-        self.terms[self.c_starts[f]] = [tid for tid, _ in feats.values()]
+        for i, (e, _) in feats.items():
+            self.terms[self.c_starts[i]:self.c_starts[i] + len(e)] = e
         if batch.groups is not None:
             _check_dismax(dismax_members(queries), clauses, clause_slot, arrays, sims, self.idfs)
         for s in {int(clause_slot[i]) for i in feats}:
             arrays[s]._device().sync_features(arrays[s].host)
+            arrays[s]._device().sync_facets(arrays[s].host)         # In clauses read facet columns
         if self.counts is not None:
             for s in set(self.counts.fields.tolist()):
                 arrays[s]._device().sync_facets(arrays[s].host)
@@ -300,6 +302,14 @@ class _PreparedBool:
             self.c_field = (_lib.p_u32(clause_slot),)
             self.bm25 = tuple(_lib.p_f32(np.asarray(v, dtype=np.float32)) for v in
                               ([a.avg_doc_length for a in arrays], [s.k1 for s in sims], [s.b for s in sims]))
+
+    @staticmethod
+    def columns(clauses, clause_slot, arrays):
+        """The Feature, Range and In clauses as query.column_terms encodes them, each on its slot's index: {index:
+        (clause entries, float32 parameter)}; ValueError for a name not set there or an In code past its buckets."""
+        from .query import column_terms
+        return column_terms(clauses, lambda i, c: arrays[clause_slot[i]]._feature_slot(c.name),
+                            lambda i, c: arrays[clause_slot[i]]._facet_slot(c.name))
 
     @staticmethod
     def features(clauses, clause_slot, arrays):
@@ -339,6 +349,17 @@ class _PreparedBool:
             opt(b.weights, _lib.p_f32), opt(b.occurs, _lib.p_u8), opt(b.groups, _lib.p_u32), opt(b.ties, _lib.p_f32),
             _lib.p_u32(b.mm), b.n_queries, int(slop), *self.bm25, _lib.p_u32(docs), docs.shape[1], _lib.p_f32(out)))
         return out
+
+
+def _refuse_column_queries(queries):
+    """TypeError for a Feature, Range or In given as a query of its own rather than as a clause."""
+    from .query import Feature, In, Range
+    for q in queries:
+        if isinstance(q, Feature):
+            raise TypeError(f"a Feature is a clause, not a query: write Bool(should=[{q!r}])")
+        if isinstance(q, (Range, In)):
+            raise TypeError(f"a {type(q).__name__} is a filter clause, not a query: write Bool(filter=[{q!r}]) with "
+                            "a must or should clause")
 
 
 def check_docs(docs, n_queries, doc_base, n_docs):
@@ -839,6 +860,14 @@ class SearchArray(ExtensionArray):
         An Or / And / Bool may be a clause of another, at any depth (Or([And(["star", "wars"]), And(["star", "trek"])])):
         it scores what it would rank as a query of its own and matches where that is > 0; see query.Or.
 
+        query.Feature, query.Range and query.In are clauses over the array's columns (set_feature, set_facet): a
+        per-doc signal added to the score, a numeric range and a set of facet codes, the last two scoring 1 where they
+        match.  Bool(must=[Or(["star", "wars"])], filter=[Range("year", gte=1977, lt=1990), In("lang", [en, fr])])
+        ranks as the same query with the matching `where=` mask, evaluated per doc on the device with no mask copied;
+        unlike a mask they also work under must_not, should (a boosted language or recency preference) and in nested
+        queries.  Each is refused as a query of its own (TypeError), as a DisMax member, and for a name not set or an
+        In code past the facet's buckets (ValueError), before any device work.
+
         where: a document filter -- a boolean array-like (a boolean pd.Series too) of shape (len(self),), one mask for
         the batch, or (len(queries), len(self)), one per query -- ranks each query only among the docs its mask
         allows, as Lucene's filter context does: the result is the top k of np.where(mask_q, S_q, 0), S_q being what
@@ -869,14 +898,12 @@ class SearchArray(ExtensionArray):
         returned are c, the hits pass 1's.  A rescore with another number of queries, a window outside [k, 1,024],
         a view or a similarity other than bm25_similarity is refused before any device work.  On a shard the window
         is the shard's own top window."""
-        from .query import DISMAX, NESTED, OCCUR, OR_AND, Feature, bool_form, check_k, has_dismax, has_field, is_boolean
+        from .query import DISMAX, NESTED, OCCUR, OR_AND, bool_form, check_k, has_dismax, has_field, is_boolean
         k = check_k(k)
         if rescore is not None:
             return self._search_topk_rescore(queries, k, similarity, slop, where, facets, rescore)
         queries = list(queries)
-        for q in queries:
-            if isinstance(q, Feature):
-                raise TypeError(f"a Feature is a clause, not a query: write Bool(should=[{q!r}])")
+        _refuse_column_queries(queries)
         if facets is not None:
             facets = check_facet_keys(facets, "facet names")
         bits = None if where is None else pack_where(where, len(self), len(queries))
@@ -923,7 +950,7 @@ class SearchArray(ExtensionArray):
         """The value each query ranks each of its candidate docs with, the second stage after search_topk (reranker
         features, window rescoring): out[q, j] == S_q[docs[q, j]], S_q the dense vector search_topk ranks query q from
         (.score for a term or phrase, the boolean composition for an Or / And / Bool / DisMax or nested query with
-        Feature clauses), +0 where the doc does not rank.  So score_docs(queries, search_topk(queries, k)[0]) returns
+        Feature, Range and In clauses), +0 where the doc does not rank.  So score_docs(queries, search_topk(queries, k)[0]) returns
         search_topk's scores bit for bit.  It replaces `arr.score(q)[docs[q]]` without a dense row per query: every
         (query, doc) is evaluated on the device from the index's lists (sa_score_docs_bool); only phrase clauses build
         their count rows, as search_topk does.
@@ -932,11 +959,9 @@ class SearchArray(ExtensionArray):
         shard), NO_DOC giving 0; duplicates and any order are allowed.  Returns float32 (len(queries), K).  Another
         dtype (TypeError), another shape or an id out of range (ValueError), a view (NotImplementedError) and a
         similarity other than bm25_similarity (TypeError) are refused before any device work."""
-        from .query import Feature, Or, has_field, is_boolean
+        from .query import Or, has_field, is_boolean
         queries = list(queries)
-        for q in queries:
-            if isinstance(q, Feature):
-                raise TypeError(f"a Feature is a clause, not a query: write Bool(should=[{q!r}])")
+        _refuse_column_queries(queries)
         if any(has_field(q) for q in queries if is_boolean(q)):
             raise ValueError("a Field clause names a DataFrame column: score queries over columns with "
                              "solr.fields_score_docs(frame, queries, rows), not SearchArray.score_docs")

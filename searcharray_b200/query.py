@@ -9,9 +9,12 @@ composition.  Field(field, clause) names the DataFrame column a clause scores on
 (solr.fields_topk, sa_multi_score_batch_topk_bool).  DisMax(clauses, tie) is one clause scored by its best member
 plus tie times the others (Lucene's DisjunctionMaxQuery).  An Or / And / Bool may itself be a clause of another (a
 nested query, scored by what it ranks as a query of its own).  Feature(name, function) is a leaf scored by a
-per-document numeric column registered with SearchArray.set_feature (Lucene's FeatureField).  The device entry points
-take the queries flattened for their form (bool_form, flatten_bool)."""
+per-document numeric column registered with SearchArray.set_feature (Lucene's FeatureField).  Range(name, ...) and
+In(name, codes) are filter leaves over a feature column and a facet column (SearchArray.set_facet), scored 1 where
+they match (Elasticsearch's range and terms queries).  The device entry points take the queries flattened for their
+form (bool_form, flatten_bool)."""
 import math
+import numbers
 from typing import List, NamedTuple, Optional, Union
 
 import numpy as np
@@ -32,14 +35,15 @@ SA_MAX_FACETS = 8                 # include/searcharray_b200.h: facet columns of
 SA_FACET_MAX_BUCKETS = 1024       # include/searcharray_b200.h
 SA_BOOL_MAX_FACETS = 4            # include/searcharray_b200.h: facets counted in one call
 FEATURE_FUNCTIONS = {"linear": 0, "saturation": 1, "log": 2}     # SA_FEATURE_LINEAR, _SATURATION, _LOG
+SA_FEATURE_RANGE, SA_FEATURE_IN = 0x10, 0x11                       # include/searcharray_b200.h
 
 Clause = Union[str, List[str]]
 
 
 def _clause(c):
-    """A clause as search_topk's query form: str (term) or list[str] (phrase), a Feature, a Field of one, a DisMax, or
-    a nested Or / And / Bool; anything else is a TypeError."""
-    if isinstance(c, (str, Feature, Field, DisMax, Or, Bool)):
+    """A clause as search_topk's query form: str (term) or list[str] (phrase), a Feature, Range or In, a Field of one,
+    a DisMax, or a nested Or / And / Bool; anything else is a TypeError."""
+    if isinstance(c, (str, Feature, Range, In, Field, DisMax, Or, Bool)):
         return c
     if isinstance(c, (list, tuple)) and c and all(isinstance(t, str) for t in c):
         return list(c)
@@ -59,7 +63,8 @@ class Feature:
     str a TypeError.  A Feature is a leaf like a term: it matches where v > 0, counts once towards mm, adds w * v under
     must / should (Boost(Feature(...), w)) and plays a leaf's role under filter / must_not.  It is accepted in Or,
     And, every list of Bool and nested queries; in solr.fields_topk as Field(column, Feature(...)), the column whose
-    index holds the values.  It is not a DisMax member (TypeError), and not a query of its own in search_topk
+    index holds the values.  Range and In, the filter leaves over the same columns and over facet columns, are
+    accepted and refused exactly where a Feature is.  It is not a DisMax member (TypeError), and not a query of its own in search_topk
     (TypeError: write Bool(should=[Feature(...)])).  apply(x) is the transform in numpy."""
 
     def __init__(self, name, function="linear", pivot=None, scaling_factor=None):
@@ -112,9 +117,162 @@ class Feature:
         return f"Feature({self.name!r}, {self.function!r}{extra})"
 
 
+def _bits(x):
+    """The bit pattern of float32 x as an int (the C ABI's encoding of a range bound)."""
+    return int(np.float32(x).view(np.uint32))
+
+
+def _f32_bound(a, up, strict):
+    """The float32 nearest a in one direction, as a float: up, the least float32 >= a (> a if strict); down, the
+    greatest float32 <= a (< a if strict).  +-inf beyond float32's range, so that x >= result is exactly x >= a
+    (x > a, x <= a, x < a) for every finite float32 x."""
+    big = float(np.finfo(np.float32).max)
+    if a > big:
+        return math.inf
+    if a < -big:
+        return -math.inf
+    f = np.float32(a)
+    with np.errstate(over="ignore"):        # past the largest float32: inf, as wanted
+        f = _f32_step(f, a, up, strict)
+    return float(f)
+
+
+def _f32_step(f, a, up, strict):
+    """f, the float32 nearest a, stepped one float32 outward where it lies on the wrong side of a."""
+    if up and (float(f) < a or (strict and float(f) == a)):
+        f = np.nextafter(f, np.float32(np.inf))
+    if not up and (float(f) > a or (strict and float(f) == a)):
+        f = np.nextafter(f, np.float32(-np.inf))
+    return f
+
+
+class Range:
+    """A filter leaf over a feature column (SearchArray.set_feature): Elasticsearch's range query, Lucene's point range.
+    It matches the docs whose value x in column `name` is inside the bounds given -- gt (x > gt), gte (x >= gte), lt
+    (x < lt), lte (x <= lte) -- and never a doc whose value is 0 (the column's "no value", as Elasticsearch skips docs
+    without the field).  The comparison is exact between x (a float32, widened to float64) and each bound as given:
+    the device compares x with float32 bounds rounded outward (bounds()), which selects the same docs.  Columns hold
+    float32, so a value above 2^24 (epoch seconds, say) was rounded when it was set.
+
+    At least one bound; gt with gte, or lt with lte, a NaN or infinite bound is a ValueError; a bound that is a bool or
+    not a real number a TypeError.  An empty range (gte=5, lt=5) is accepted and matches nothing.  It scores as a
+    constant: 1 where it matches, 0 elsewhere, and is otherwise a leaf like a Feature -- it counts once towards mm, adds
+    w * 1 under must / should (Boost(Range(...), w)), and plays a leaf's role under filter / must_not.  It is accepted
+    and refused where a Feature is (not a DisMax member, not a query of its own: write Bool(filter=[...])); in
+    solr.fields_topk as Field(column, Range(...)).  match(x) is the filter in numpy."""
+
+    def __init__(self, name, gt=None, gte=None, lt=None, lte=None):
+        if not isinstance(name, str):
+            raise TypeError(f"a range's column name is a str, not {name!r}")
+        given = {}
+        for key, v in (("gt", gt), ("gte", gte), ("lt", lt), ("lte", lte)):
+            if v is None:
+                continue
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, numbers.Real):
+                raise TypeError(f"a range bound is a real number, not {key}={v!r}")
+            try:
+                x = float(v)
+            except OverflowError:           # an int beyond float64: beyond every float32 too
+                x = math.inf if v > 0 else -math.inf
+            else:
+                if not math.isfinite(x):
+                    raise ValueError(f"a range bound is finite, not {key}={v!r}")
+            given[key] = x
+        if not given:
+            raise ValueError("a range needs at least one bound (gt, gte, lt or lte)")
+        if "gt" in given and "gte" in given:
+            raise ValueError("a range takes gt or gte, not both")
+        if "lt" in given and "lte" in given:
+            raise ValueError("a range takes lt or lte, not both")
+        self.name = name
+        self.gt, self.gte, self.lt, self.lte = (given.get(k) for k in ("gt", "gte", "lt", "lte"))
+
+    def bounds(self):
+        """(lo, hi): the float32 interval [lo, hi] (as floats) the device tests x against, the bounds rounded
+        outward; -inf / +inf where a side is open or a bound lies beyond float32's range."""
+        lo, hi = -math.inf, math.inf
+        if self.gte is not None:
+            lo = _f32_bound(self.gte, True, False)
+        if self.gt is not None:
+            lo = _f32_bound(self.gt, True, True)
+        if self.lte is not None:
+            hi = _f32_bound(self.lte, False, False)
+        if self.lt is not None:
+            hi = _f32_bound(self.lt, False, True)
+        return lo, hi
+
+    def entries(self, slot):
+        """The clause entries of the C ABI on feature slot `slot`: SA_RANGE_TERM(slot), then lo's and hi's bits."""
+        lo, hi = self.bounds()
+        return [SA_FEATURE_TERM_BASE | (SA_FEATURE_RANGE << 8) | int(slot), _bits(lo), _bits(hi)]
+
+    def match(self, x):
+        """bool[len(x)]: where the float32 values x (widened to float64) are > 0 and inside the bounds."""
+        x = np.asarray(x, dtype=np.float32).astype(np.float64)
+        m = x > 0
+        if self.gt is not None:
+            m &= x > self.gt
+        if self.gte is not None:
+            m &= x >= self.gte
+        if self.lt is not None:
+            m &= x < self.lt
+        if self.lte is not None:
+            m &= x <= self.lte
+        return m
+
+    def __repr__(self):
+        shown = "".join(f", {k}={v!r}" for k, v in (("gt", self.gt), ("gte", self.gte), ("lt", self.lt),
+                                                    ("lte", self.lte)) if v is not None)
+        return f"Range({self.name!r}{shown})"
+
+
+class In:
+    """A filter leaf over a facet column (SearchArray.set_facet): Elasticsearch's terms query on a keyword field,
+    Lucene's TermInSetQuery.  It matches the docs whose code in column `name` is one of `codes`, never a doc without a
+    value (code -1).  codes: a non-empty list (tuple, or integer array) of ints >= 0, duplicates allowed; each must be
+    below the facet's n_buckets, which is checked when the call is prepared (ValueError, before any device work).  A
+    non-list or a non-int code is a TypeError, an empty list or a negative code a ValueError.  It scores and is
+    accepted and refused as Range.  match(codes) is the filter in numpy."""
+
+    def __init__(self, name, codes):
+        if not isinstance(name, str):
+            raise TypeError(f"a facet name is a str, not {name!r}")
+        if isinstance(codes, np.ndarray):
+            if codes.dtype.kind not in "iu":
+                raise TypeError(f"In codes are ints, not dtype {codes.dtype}")
+            codes = codes.tolist()
+        if not isinstance(codes, (list, tuple)):
+            raise TypeError(f"In codes are a list of ints, not {codes!r}")
+        out = []
+        for c in codes:
+            if isinstance(c, (bool, np.bool_)) or not isinstance(c, (int, np.integer)):
+                raise TypeError(f"an In code is an int, not {c!r}")
+            out.append(int(c))
+        if not out:
+            raise ValueError("an In clause needs at least one code")
+        if min(out) < 0:
+            raise ValueError(f"In codes are >= 0: {out}")
+        self.name, self.codes = name, out
+
+    def entries(self, slot):
+        """The clause entries of the C ABI on facet slot `slot`: SA_IN_TERM(slot), then the codes."""
+        return [SA_FEATURE_TERM_BASE | (SA_FEATURE_IN << 8) | int(slot)] + self.codes
+
+    def match(self, codes):
+        """bool[len(codes)]: where the codes (-1: no value) are in the set."""
+        codes = np.asarray(codes)
+        return (codes >= 0) & np.isin(codes, self.codes)
+
+    def __repr__(self):
+        return f"In({self.name!r}, {self.codes!r})"
+
+
+COLUMN_CLAUSES = (Feature, Range, In)     # leaves scored from a column of the index, not from its postings
+
+
 def _is_feature(c):
-    """Whether a clause (without its Boost) is a Feature or a Field of one."""
-    return isinstance(c, Feature) or (isinstance(c, Field) and isinstance(c.clause, Feature))
+    """Whether a clause (without its Boost) is a Feature, Range or In, or a Field of one."""
+    return isinstance(c, COLUMN_CLAUSES) or (isinstance(c, Field) and isinstance(c.clause, COLUMN_CLAUSES))
 
 
 class Field:
@@ -122,7 +280,8 @@ class Field:
     frame[field].array.score(clause) scores it -- Lucene's `title:star`.  Accepted wherever a clause is (Or, And, the
     four lists of Bool) by solr.fields_topk, which needs every clause to name its field; SearchArray.search_topk
     refuses it.  A boosted field clause is Boost(Field(field, clause), weight); a Field holds no Boost or Field.
-    Field(field, Feature(...)) is a feature clause whose values are those set on that column's index."""
+    Field(field, Feature(...)) is a feature clause whose values are those set on that column's index, and
+    Field(field, Range(...)) / Field(field, In(...)) filter on that index's feature / facet columns."""
 
     def __init__(self, field, clause):
         if not isinstance(field, str):
@@ -369,7 +528,8 @@ def has_dismax(q):
 
 
 def has_feature(q):
-    """Whether a boolean query holds a feature clause (Feature, or Field of one), nested queries included."""
+    """Whether a boolean query holds a column clause (Feature, Range or In, or a Field of one), nested queries
+    included: such a query runs at least at the OCCUR form."""
     return any(_is_feature(c) for c in _leaves(q))
 
 
@@ -411,8 +571,8 @@ def _form(clauses, occur):
 class BoolBatch(NamedTuple):
     """Boolean queries as sa_score_batch_topk_bool takes them (flatten_bool).  Arrays the form does not use are None,
     passed as NULL."""
-    clauses: list                   # per clause: search_topk's query form (str, list[str] or Feature); None for a
-                                    # nested clause
+    clauses: list                   # per clause: search_topk's query form (str, list[str], Feature, Range or In);
+                                    # None for a nested clause
     node_starts: np.ndarray         # uint32: node n's clauses are [node_starts[n], node_starts[n + 1])
     clause_node: Optional[np.ndarray]   # uint32 per clause: its nested node, else SA_NO_NODE (NESTED)
     mm: np.ndarray                  # uint32 per node
@@ -540,16 +700,33 @@ def check_dismax_members(members, params):
                              f"{c!r} has k1={float(k1)}, b={float(b)}, idf={float(idf)}")
 
 
-def feature_terms(clauses, slot):
-    """The feature leaves of a flattened clause list (BoolBatch.clauses) as the C entry points take them:
-    {index: (reserved term id, float32 parameter)}.  slot(i, feature) -> the feature's slot on clause i's index (it
-    raises ValueError for a name that is not set there)."""
+def column_terms(clauses, feature_slot, facet_slot):
+    """The Feature, Range and In leaves of a flattened clause list (BoolBatch.clauses) as the C entry points take
+    them: {index: (clause entries, float32 parameter)} -- a Feature's reserved term id with its parameter, a Range's
+    SA_RANGE_TERM and bound bits, an In's SA_IN_TERM and codes, the last two with parameter 0.  feature_slot(i, c) ->
+    the slot of c's feature column on clause i's index; facet_slot(i, c) -> (slot, n_buckets) of c's facet column
+    there; each raises ValueError for a name that is not set.  An In code >= n_buckets is a ValueError."""
     out = {}
     for i, c in enumerate(clauses):
         f = c.clause if isinstance(c, Field) else c
         if isinstance(f, Feature):
-            out[i] = (f.term_id(slot(i, f)), f.param)
+            out[i] = ([f.term_id(feature_slot(i, f))], f.param)
+        elif isinstance(f, Range):
+            out[i] = (f.entries(feature_slot(i, f)), np.float32(0))
+        elif isinstance(f, In):
+            slot, n_buckets = facet_slot(i, f)
+            if max(f.codes) >= n_buckets:
+                raise ValueError(f"{f!r}: codes are below facet {f.name!r}'s {n_buckets} buckets")
+            out[i] = (f.entries(slot), np.float32(0))
     return out
+
+
+def feature_terms(clauses, slot):
+    """The feature leaves of a flattened clause list (BoolBatch.clauses) as the C entry points take them:
+    {index: (reserved term id, float32 parameter)}.  slot(i, feature) -> the feature's slot on clause i's index (it
+    raises ValueError for a name that is not set there).  column_terms restricted to Feature clauses."""
+    only = [c if isinstance(c.clause if isinstance(c, Field) else c, Feature) else None for c in clauses]
+    return {i: (e[0], p) for i, (e, p) in column_terms(only, slot, None).items()}
 
 
 class Rescore:

@@ -473,7 +473,7 @@ def _fields_plan(frame, queries, similarity, extra=()):
     clause_slot = _clause_slots(batch, slot_of)
     if batch.groups is not None:          # DisMax members: sparse-safe k1 / b on their fields
         _check_dismax(dismax_members(queries), batch.clauses, clause_slot, slot_arrays, slot_sims)
-    _PreparedBool.features(batch.clauses, clause_slot, slot_arrays)      # feature names set on their columns
+    _PreparedBool.columns(batch.clauses, clause_slot, slot_arrays)   # feature / facet names set, In codes in range
     return batch, slot_of, slot_arrays, slot_sims
 
 
@@ -515,7 +515,8 @@ def fields_score_docs(frame: pd.DataFrame, queries, rows,
     fields_topk ranks query q from (+0 where the row does not rank), so fields_score_docs(frame, queries,
     fields_topk(frame, queries, k)[0]) returns fields_topk's scores bit for bit (sa_multi_score_docs_bool).  queries
     and similarity as in fields_topk, under its refusals and column checks.  rows: an integer array of shape
-    (len(queries), K), ids as fields_topk returns them (global doc ids on a shard), NO_DOC giving 0.  Returns float32
+    (len(queries), K), ids as fields_topk returns them (global doc ids on a shard), NO_DOC giving 0; Feature, Range and
+    In clauses are evaluated at each row as fields_topk folds them.  Returns float32
     (len(queries), K).  Another dtype (TypeError), another shape or an id out of range (ValueError) is refused
     before any device work."""
     queries = list(queries)
@@ -568,6 +569,10 @@ def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
 
     An Or / And / Bool may be a clause of another, at any depth, as in SearchArray.search_topk: edismax's qf + pf as
     Bool(must=[Or([DisMax(...), DisMax(...)], mm="75%")], should=[Boost(Field("title", ["a", "b"]), 3)]).
+
+    Field(column, Feature(...)), Field(column, Range(...)) and Field(column, In(...)) read the feature or facet
+    columns set on that column's index (SearchArray.set_feature / set_facet), as in SearchArray.search_topk:
+    Bool(must=[Field("title", "alien")], filter=[Field("title", Range("year", gte=1980))]).
 
     where: a document filter, as in SearchArray.search_topk -- a boolean array-like (a boolean pd.Series too) of
     shape (len(frame),), one mask for the batch, or (len(queries), len(frame)), one per query.  Per query the
