@@ -336,16 +336,6 @@ __device__ __forceinline__ unsigned bool_fresh_tid() {
     return t;
 }
 
-// A (query, tile) where nothing ranks: no candidates, bound 0.  FRESH: thread 0 found by bool_fresh_tid.
-template <bool FRESH = false>
-__device__ __forceinline__ void bool_publish_empty(const TopkCtx &t, u32 q, u32 tile) {
-    if ((FRESH ? bool_fresh_tid() : threadIdx.x) == 0) {
-        const u64 t_idx = (u64)q * t.n_tiles + tile;
-        t.tile_cnt[t_idx] = 0;
-        t.tile_max[t_idx] = 0;
-    }
-}
-
 // COUNT: the counting pass of one (query, tile), after flush_tile_collect (whose last barrier follows its last read
 // of s_tile): s_tile holds the tile's ranked values, +0 where a doc does not rank.  All threads must call.
 __device__ __forceinline__ void bool_count_tile(const BoolCount &cn, float *s_tile) {
@@ -436,7 +426,7 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
         // no allowed doc in the tile: nothing ranks, and no list is read (contiguous filters skip whole tiles)
         allow = where_word(wh, q, tile);
         if (!__syncthreads_or(allow != 0)) {
-            bool_publish_empty<true>(a.topk, q, tile);
+            publish_empty_tile(a.topk, q, tile, bool_fresh_tid());
             return;
         }
     } else {
@@ -502,7 +492,7 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
             if (tid == 0) nb.flags[(u64)bq.pad * nb.n_tiles + tile] = 0;
             return;
         }
-        bool_publish_empty(a.topk, q, tile);
+        publish_empty_tile(a.topk, q, tile, threadIdx.x);
         return;
     }
 

@@ -457,15 +457,7 @@ phrase_kernel(const PhraseArgs a) {
     for (u32 tile = tile0; tile < tile1; tile++) {
         const u64 t_abs1 = a.doc_base + (u64)tile * SA_TILE_DOCS + SA_TILE_DOCS;
         if (next_doc >= t_abs1) {
-            float4 *__restrict__ out4 = reinterpret_cast<float4 *>(out + (u64)tile * SA_TILE_DOCS);
-            const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-            for (int i = 0; i < SA_TILE_DOCS / PT / 4; i++) __stcs(out4 + tid + i * PT, z);
-            if (a.topk.k && tid == 0) {
-                const u64 t_idx = (u64)row * a.topk.n_tiles + tile;
-                a.topk.tile_cnt[t_idx] = 0;
-                a.topk.tile_max[t_idx] = 0;
-            }
+            store_empty_tile<PT>(out + (u64)tile * SA_TILE_DOCS, a.topk, row, tile);
             continue;
         }
         // first entry at or past the end of this tile: gallop from the cursor, then bisect (uniform)
@@ -672,15 +664,7 @@ phrase_tile_kernel(const PhraseArgs a) {
 #pragma unroll
     for (int w = 0; w < PT / 32; w++) { total += s_wmatch[w]; holders += min(s_wmatch[w], 32u); }
     if (total == 0) {
-        float4 *__restrict__ out4 = reinterpret_cast<float4 *>(out + (u64)tile * SA_TILE_DOCS);
-        const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int i = 0; i < SA_TILE_DOCS / PT / 4; i++) __stcs(out4 + tid + i * PT, z);
-        if (a.topk.k && tid == 0) {
-            const u64 t_idx = (u64)row * a.topk.n_tiles + tile;
-            a.topk.tile_cnt[t_idx] = 0;
-            a.topk.tile_max[t_idx] = 0;
-        }
+        store_empty_tile<PT>(out + (u64)tile * SA_TILE_DOCS, a.topk, row, tile);
         return;
     }
     flush_tile_collect<true, DEEP>(s_tile, out + (u64)tile * SA_TILE_DOCS, a.topk, row, tile, my_max, total, holders, s_top,

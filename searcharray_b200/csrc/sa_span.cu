@@ -763,15 +763,7 @@ span_tiles_kernel(const SpanArgs a) {
     for (u32 tile = tile0; tile < tile1; tile++) {
         const u64 t0 = (u64)tile * SA_TILE_DOCS, t1 = t0 + SA_TILE_DOCS;
         if (sorted && next_doc >= t1) {                                   // no match in this tile
-            float4 *__restrict__ out4 = reinterpret_cast<float4 *>(out + t0);
-            const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-            for (int i = 0; i < SA_TILE_DOCS / SA_TERM_THREADS / 4; i++) __stcs(out4 + tid + i * SA_TERM_THREADS, z);
-            if (a.topk.k && tid == 0) {
-                const u64 t_idx = (u64)row * a.topk.n_tiles + tile;
-                a.topk.tile_cnt[t_idx] = 0;
-                a.topk.tile_max[t_idx] = 0;
-            }
+            store_empty_tile<SA_TERM_THREADS>(out + t0, a.topk, row, tile);
             continue;
         }
 #pragma unroll

@@ -20,7 +20,9 @@
 //      for docs that do not contain the term;
 //   3. the tile is flushed once with 16-byte streaming stores; while it passes through registers
 //      every score >= a running, provably valid lower bound of the k-th best score is appended to
-//      the query's top-k candidate list (sa_topk.cu), so the dense vector is never re-read.
+//      the query's top-k candidate list (sa_topk.cu), so the dense vector is never re-read.  This is
+//      flush_tile_collect (sa_term.cuh), shared with the other tile kernels; the kernel's finish step
+//      forms the final scores on the way.
 // The grid is one-dimensional, Q * n_tiles CTAs walked in groups of G consecutive queries: inside a group the query
 // runs fastest, then the tile, then the group.  The CTAs in flight (about 6 per SM) then cover about 6 * SMs / G
 // neighbouring tiles of G rows: dense terms (issue-bound CTAs) and sparse terms (store-bound CTAs) overlap, and a
@@ -43,7 +45,7 @@ __device__ __forceinline__ bool payload_keep(u64 w, u64 lo, u64 hi) {
     return v >= lo && v <= hi;
 }
 
-// DEEP: k > SA_TOPK_MAX, the tile's candidates from deep_tile_collect (step 3').
+// DEEP: k > SA_TOPK_MAX, the tile's candidates from deep_tile_collect (through flush_tile_collect).
 template <int MODE, bool ALL_DOCS, bool FILTER, bool DEEP>
 __global__ void __launch_bounds__(SA_TERM_THREADS, DEEP ? SA_TERM_DEEP_CTAS_PER_SM : SA_TERM_CTAS_PER_SM)
 term_tile_kernel(const TermBatchArgs a) {
@@ -297,74 +299,11 @@ term_tile_kernel(const TermBatchArgs a) {
     }
     }
 
-    if constexpr (DEEP) {
-        // 3'. flush the tile's final scores -- de-negated on staged-norm tiles, formed over every doc on the ALL_DOCS
-        //     path -- and write them back to the tile, which the deep collector then ranks.  The barrier: a thread's
-        //     float4s hold scores other threads stored
-        __syncthreads();
-        float4 *__restrict__ out4 = reinterpret_cast<float4 *>(a.out + (u64)q * a.out_stride + tile_doc0);
-#pragma unroll
-        for (int jj = 0; jj < SA_TILE_DOCS / SA_TERM_THREADS / 4; jj++) {
-            const unsigned g = tid + jj * SA_TERM_THREADS;
-            float4 v = reinterpret_cast<const float4 *>(s_out)[g];
-            if (staged_norm) {
-                v.x = __float_as_int(v.x) < 0 ? -v.x : 0.0f;
-                v.y = __float_as_int(v.y) < 0 ? -v.y : 0.0f;
-                v.z = __float_as_int(v.z) < 0 ? -v.z : 0.0f;
-                v.w = __float_as_int(v.w) < 0 ? -v.w : 0.0f;
-            }
-            if (ALL_DOCS && MODE == TERM_MODE_SCORE) {
-                Bm25Params p = a.bm25;
-                p.idf = tq.idf;
-                const u64 d = (u64)tile_doc0 + (u64)g * 4;
-                const float *dl = a.doc_lens + d;
-                v.x = (d + 0 < a.n_docs) ? bm25_one(v.x, dl[0], p) : 0.0f;
-                v.y = (d + 1 < a.n_docs) ? bm25_one(v.y, dl[1], p) : 0.0f;
-                v.z = (d + 2 < a.n_docs) ? bm25_one(v.z, dl[2], p) : 0.0f;
-                v.w = (d + 3 < a.n_docs) ? bm25_one(v.w, dl[3], p) : 0.0f;
-            }
-            __stcs(out4 + g, v);
-            reinterpret_cast<float4 *>(s_out)[g] = v;
-        }
-        __syncthreads();
-        deep_tile_collect(s_out, a.topk, q, tile);
-        return;
-    }
-
-    // 3. top-k.  A tile with no more words than candidate slots needs no bound: every positive
-    //    score fits.  Otherwise each warp publishes its largest thread maxima and every warp
-    //    derives the same tile bound; scores >= bound are this tile's candidates.
-    const u32 k = a.topk.k;
-    // CTA-uniform (<= k postings: all fit).  Keeping every positive score of tiles with up to `slots` postings instead
-    // was measured slower (df/N 1e-2: 9.9 vs 9.2 us/query): candidates cost more than the bound.
-    const bool need_bound = k && (hi - lo) > k;
-    // threads that can hold a score: one per record / posting word, or one per quad of records on the dense tf-table path
-    const u32 M = tile_bound_width(k, quads ? (hi - lo) / 4u : (hi - lo));
-    if (need_bound) {
-        u32 v = my_max;
-        for (u32 r = 0; r < M; r++) {
-            u32 m = warp_pop_max(v);
-            if (lane == r) s_top[warp * 8 + r] = m;
-        }
-    }
-    if (k && tid == 0) { s_ncand = 0; s_tile_max = 0; }
-    __syncthreads();
-    float thr_f = 0.0f;
-    if (k) {
-        u32 thr = 1u;                                   // >= 1: skip zeros (scores are >= +0.0)
-        if (need_bound) thr = max(cta_kth_bound(s_top, k, M == 8u), 1u);
-        thr_f = __uint_as_float(thr);
-    }
-    u64 *__restrict__ my_cand = nullptr;
-    if (k) my_cand = a.topk.tile_cand + ((u64)q * a.topk.n_tiles + tile) * a.topk.slots;
-
-    // 4. flush the tile: 16-byte streaming stores (the padded buffer makes the tile always in bounds)
-    u32 cand_max = 0;
-    float4 *__restrict__ out4 = reinterpret_cast<float4 *>(a.out + (u64)q * a.out_stride + tile_doc0);
-#pragma unroll
-    for (int jj = 0; jj < SA_TILE_DOCS / SA_TERM_THREADS / 4; jj++) {
-        const unsigned g = tid + jj * SA_TERM_THREADS;
-        float4 v = reinterpret_cast<const float4 *>(s_out)[g];
+    // 3. flush the tile and collect its top-k candidates.  A tile with no more postings than k needs no bound: every
+    //    positive score fits.  (Keeping every positive score of tiles with up to `slots` postings instead was measured
+    //    slower, df/N 1e-2: 9.9 vs 9.2 us/query: candidates cost more than the bound.)  Threads that can hold a score:
+    //    one per record / posting word, or one per quad of records on the dense tf-table path.
+    auto finish = [&](unsigned g, float4 &v) {
         if (staged_norm) {                                  // sign set: a (negated) score; clear: a leftover norm
             v.x = __float_as_int(v.x) < 0 ? -v.x : 0.0f;
             v.y = __float_as_int(v.y) < 0 ? -v.y : 0.0f;
@@ -382,38 +321,12 @@ term_tile_kernel(const TermBatchArgs a) {
             v.z = (d + 2 < a.n_docs) ? bm25_one(v.z, dl[2], p) : 0.0f;
             v.w = (d + 3 < a.n_docs) ? bm25_one(v.w, dl[3], p) : 0.0f;
         }
-        __stcs(out4 + g, v);
-        if (k) {
-            // NaN compares false; negatives are below thr_f > 0
-            if ((v.x >= thr_f) | (v.y >= thr_f) | (v.z >= thr_f) | (v.w >= thr_f)) {
-                const float vs[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                for (int e = 0; e < 4; e++) {
-                    if (vs[e] >= thr_f) {
-                        u32 slot = atomicAdd(&s_ncand, 1u);           // shared-memory atomic
-                        if (slot < a.topk.slots)
-                            my_cand[slot] = ((u64)__float_as_uint(vs[e]) << 32) |
-                                            (u64)(0xFFFFFFFFu - (tile_doc0 + g * 4 + e));
-                        cand_max = max(cand_max, __float_as_uint(vs[e]));
-                    }
-                }
-            }
-        }
-    }
-    if (k) {
-        if (cand_max) atomicMax(&s_tile_max, cand_max);
-        __syncthreads();
-        if (s_ncand > a.topk.slots && !(ALL_DOCS && MODE == TERM_MODE_SCORE))    // CTA-uniform: ties at the bound
-            tile_collect_ties_retry(s_out, staged_norm, __float_as_uint(thr_f), a.topk, my_cand, tile_doc0, s_top,
-                                    &s_ncand, &s_tile_max);
-        if (tid == 0) {
-            const u32 n = s_ncand;
-            const u64 t_idx = (u64)q * a.topk.n_tiles + tile;
-            a.topk.tile_cnt[t_idx] = min(n, a.topk.slots);
-            a.topk.tile_max[t_idx] = s_tile_max;
-            if (n > a.topk.slots) a.topk.overflow[q] = 1u;
-        }
-    }
+    };
+    // ALL_DOCS scores take no tie retry, which would evaluate BM25 over the tile again: a tile whose ties overflow
+    // sends its query to the exact re-run (the padded row makes the tile always in bounds)
+    flush_tile_collect<true, DEEP>(s_out, a.out + (u64)q * a.out_stride + tile_doc0, a.topk, q, tile, my_max, hi - lo,
+                                   quads ? (hi - lo) / 4u : hi - lo, s_top, &s_ncand, &s_tile_max, finish,
+                                   !(ALL_DOCS && MODE == TERM_MODE_SCORE));
 }
 
 // per-doc BM25 length norm, the inner part of bm25.pyx:21-23 with the same rounding sequence

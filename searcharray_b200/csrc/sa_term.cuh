@@ -3,6 +3,7 @@
 // scores ranked by a float32 proxy (classic similarity, edismax).
 #pragma once
 #include <cmath>
+#include <type_traits>
 
 #include "sa_common.cuh"
 
@@ -314,6 +315,34 @@ __device__ K radix_kth_largest(u32 k, u32 *s_hist, K *s_prefix, u32 *s_krem, V v
     return *s_prefix;
 }
 
+// Thread 0's publication of one (row, tile) for topk_select_kernel: cnt candidates in the tile's slots, max_bits the
+// best one's score bits (0: none).  overflow: the tile had more candidates than slots, so its row takes the exact
+// host-side re-run.
+__device__ __forceinline__ void publish_tile(const TopkCtx &t, u32 row, u32 tile, u32 cnt, u32 max_bits,
+                                             bool overflow = false) {
+    const u64 t_idx = (u64)row * t.n_tiles + tile;
+    t.tile_cnt[t_idx] = cnt;
+    t.tile_max[t_idx] = max_bits;
+    if (overflow) t.overflow[row] = 1u;
+}
+
+// A (row, tile) where nothing ranks: no candidates, bound 0.  tid: the calling thread's index (the boolean kernels
+// read it afresh, bool_fresh_tid, so that the test holds no register live through their fold).
+__device__ __forceinline__ void publish_empty_tile(const TopkCtx &t, u32 row, u32 tile, unsigned tid) {
+    if (tid == 0) publish_tile(t, row, tile, 0, 0);
+}
+
+// A (row, tile) without a match: the caller's THREADS threads store its dense tile as zeros straight from registers
+// (no shared tile, no barrier), and it is published empty when the launch collects a top k.
+template <u32 THREADS>
+__device__ __forceinline__ void store_empty_tile(float *__restrict__ out_tile, const TopkCtx &t, u32 row, u32 tile) {
+    const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int i = 0; i < SA_TILE_DOCS / THREADS / 4; i++)
+        __stcs(reinterpret_cast<float4 *>(out_tile) + threadIdx.x + i * THREADS, z);
+    if (t.k) publish_empty_tile(t, row, tile, threadIdx.x);
+}
+
 // The deep tile collector (k > SA_TOPK_MAX): the tile's EXACT top k by key score_bits << 32 | ~doc, written as one run
 // sorted by key, descending, so that topk_select_kernel<true> reads only the prefix of each run above its threshold.
 // s_tile holds the tile's final float32 scores (a doc ranks iff its score is > 0; NaN never does).  With n ranked
@@ -370,10 +399,7 @@ __device__ __forceinline__ void deep_tile_collect(const float *s_tile, const Top
     const u64 t_idx = (u64)row * t.n_tiles + tile;
     u64 *__restrict__ run = t.tile_cand + t_idx * t.slots;
     for (u32 i = tid; i < m; i += blockDim.x) run[i] = s_run[i];
-    if (tid == 0) {
-        t.tile_cnt[t_idx] = m;
-        t.tile_max[t_idx] = m ? (u32)(s_run[0] >> 32) : 0u;
-    }
+    if (tid == 0) publish_tile(t, row, tile, m, m ? (u32)(s_run[0] >> 32) : 0u);
     __syncthreads();
 }
 
@@ -419,54 +445,62 @@ __device__ __forceinline__ u32 cta_kth_bound(const u32 *s_top /*[8][8]*/, u32 k,
     return kth;
 }
 
+// The tile bound: every warp publishes the M largest of its threads' values v into s_top (M = 4 or 8,
+// tile_bound_width), then, after a barrier, every warp derives the k-th largest of them (cta_kth_bound), at least 1.
+// need = false (CTA-uniform): no bound, 1.  With k > 0 thread 0 also clears the tile's candidate count and maximum
+// before the barrier.  The barrier is taken either way, so what the CTA stored to shared memory before the call is
+// visible after it.  All SA_TERM_THREADS threads call.
+__device__ __forceinline__ u32 tile_bound(u32 v, bool need, u32 M, u32 k, u32 *s_top, u32 *s_ncand, u32 *s_tile_max) {
+    const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (need) {
+        for (u32 r = 0; r < M; r++) {
+            const u32 m = warp_pop_max(v);
+            if (lane == r) s_top[warp * 8 + r] = m;
+        }
+    }
+    if (k && threadIdx.x == 0) { *s_ncand = 0; *s_tile_max = 0; }
+    __syncthreads();
+    return need ? max(cta_kth_bound(s_top, k, M == 8u), 1u) : 1u;
+}
+
 // Candidate-slot overflow caused by TIES at the tile bound (BM25 scores are a function of (tf, doc_len) only, so
 // exact ties among thousands of docs are normal): the tile is still in shared memory, so the CTA collects
 // again, now breaking ties the way the final ranking does -- lower doc id first.  Scores above the bound are
 // all kept; of the docs AT the bound only those with a local index <= the k-th smallest such index (a bound
 // derived from the threads' smallest tied docs, which are distinct docs) are kept: a superset of what the
-// top-k can take from this tile.  `negated`: the tile holds -score for scored docs and a positive leftover
-// norm elsewhere (term kernel, staged norms).  All SA_TERM_THREADS threads call; returns with the slots,
-// *s_ncand and *s_tile_max rewritten (the caller publishes them).  Still more than `slots` -> the caller
-// flags the query for the exact host-side re-run, as before.
-__device__ __forceinline__ void tile_collect_ties_retry(const float *s_out, bool negated, u32 thr_bits, const TopkCtx &t,
+// top-k can take from this tile.  finish: flush_tile_collect's, applied to the tile again.  All SA_TERM_THREADS
+// threads call; returns with the slots, *s_ncand and *s_tile_max rewritten (the caller publishes them).  Still
+// more than `slots` -> the caller flags the query for the exact host-side re-run, as before.
+template <typename F>
+__device__ __forceinline__ void tile_collect_ties_retry(const float *s_out, F finish, u32 thr_bits, const TopkCtx &t,
                                                         u64 *__restrict__ my_cand, u32 tile_doc0, u32 *s_top,
                                                         u32 *s_ncand, u32 *s_tile_max) {
-    const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const unsigned tid = threadIdx.x;
     const float thr_f = __uint_as_float(thr_bits);
     u32 best = 0;                                   // 0xFFFFFFFF - smallest tied local doc of this thread (0 = none)
 #pragma unroll
     for (int jj = 0; jj < SA_TILE_DOCS / SA_TERM_THREADS / 4; jj++) {
         const unsigned g = tid + jj * SA_TERM_THREADS;
-        const float4 raw = reinterpret_cast<const float4 *>(s_out)[g];
-        const float vs[4] = {raw.x, raw.y, raw.z, raw.w};
+        float4 v = reinterpret_cast<const float4 *>(s_out)[g];
+        finish(g, v);
+        const float vs[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-        for (int e = 0; e < 4; e++) {
-            const float v = negated ? (__float_as_int(vs[e]) < 0 ? -vs[e] : 0.0f) : vs[e];
-            if (v == thr_f) best = max(best, 0xFFFFFFFFu - (g * 4 + e));
-        }
+        for (int e = 0; e < 4; e++)
+            if (vs[e] == thr_f) best = max(best, 0xFFFFFFFFu - (g * 4 + e));
     }
-    const u32 M = 8u;
-    __syncthreads();                                // s_top may still be read by a slow warp of the first pass
-    {
-        u32 v = best;
-        for (u32 r = 0; r < M; r++) {
-            u32 m = warp_pop_max(v);
-            if (lane == r) s_top[warp * 8 + r] = m;
-        }
-    }
-    if (tid == 0) { *s_ncand = 0; *s_tile_max = 0; }
-    __syncthreads();
-    const u32 kth = cta_kth_bound(s_top, t.k, true);   // 0: fewer than k threads hold a tie -> keep every tie
-    const u32 doc_bound = kth ? 0xFFFFFFFFu - kth : 0xFFFFFFFFu;
+    __syncthreads();                                // every thread has read the caller's *s_ncand
+    // fewer than k threads hold a tie: the bound is 1, above every local doc -> keep every tie
+    const u32 doc_bound = 0xFFFFFFFFu - tile_bound(best, true, 8u, t.k, s_top, s_ncand, s_tile_max);
     u32 cand_max = 0;
 #pragma unroll
     for (int jj = 0; jj < SA_TILE_DOCS / SA_TERM_THREADS / 4; jj++) {
         const unsigned g = tid + jj * SA_TERM_THREADS;
-        const float4 raw = reinterpret_cast<const float4 *>(s_out)[g];
-        const float vs[4] = {raw.x, raw.y, raw.z, raw.w};
+        float4 fv = reinterpret_cast<const float4 *>(s_out)[g];
+        finish(g, fv);
+        const float vs[4] = {fv.x, fv.y, fv.z, fv.w};
 #pragma unroll
         for (int e = 0; e < 4; e++) {
-            const float v = negated ? (__float_as_int(vs[e]) < 0 ? -vs[e] : 0.0f) : vs[e];
+            const float v = vs[e];
             if (v > thr_f || (v == thr_f && g * 4 + e <= doc_bound)) {
                 u32 slot = atomicAdd(s_ncand, 1u);
                 if (slot < t.slots)
@@ -485,55 +519,59 @@ __device__ __forceinline__ void tile_collect_ties_retry(const float *s_out, bool
 // `n_holders`: how many threads can hold a score (not how many scores there are).
 __device__ __forceinline__ u32 tile_bound_width(u32 k, u32 n_holders) { return (k <= 10 && n_holders >= SA_TERM_THREADS) ? 4u : 8u; }
 
-// Flush one shared-memory score tile to its dense row with 16-byte streaming stores and, on the way,
-// collect the tile's top-k candidates (private slots, count, maximum): the same step the term kernel
-// ends with, shared with the phrase kernel.  `my_max` = largest score bits this thread put into the
-// tile, `n_items` = number of scores in the tile, `n_holders` = how many threads can hold one of them.  All SA_TERM_THREADS threads must call.
+// The finish step of flush_tile_collect that leaves the tile as it is.
+struct TileIdentity {
+    __device__ __forceinline__ void operator()(unsigned, float4 &) const {}
+};
+
+// Flush one shared-memory score tile to its dense row with 16-byte streaming stores and, on the way, collect the
+// tile's top-k candidates (private slots, count, maximum): the step every float32 tile kernel ends with.
+// finish(g, v) turns float4 g of the tile (docs 4 g .. 4 g + 3) into the final scores that are stored and collected
+// (the term kernel's: staged-norm tiles hold negated scores, ALL_DOCS tiles term frequencies); the default,
+// TileIdentity, takes the tile as it is.  `my_max` = largest final score bits this thread put into the tile,
+// `n_items` = number of scores in the tile, `n_holders` = how many threads can hold one of them.  All SA_TERM_THREADS
+// threads must call.
 // STORE = false: collect only (out_tile unused); the tile stays in shared memory for the tie retry either way.
-// DEEP: k > SA_TOPK_MAX, the tile's candidates from deep_tile_collect (my_max, n_items and n_holders unused).
-template <bool STORE = true, bool DEEP = false>
-__device__ __forceinline__ void flush_tile_collect(const float *s_out, float *__restrict__ out_tile, const TopkCtx &t,
+// DEEP: k > SA_TOPK_MAX, the tile's candidates from deep_tile_collect (my_max, n_items and n_holders unused); a
+// finish other than TileIdentity writes the final scores back to the tile for it.
+// ties_retry = false: a tile whose ties at the bound overflow the slots flags its row for the exact re-run at once,
+// without the tie retry (which applies finish to the whole tile again).
+template <bool STORE = true, bool DEEP = false, typename F = TileIdentity>
+__device__ __forceinline__ void flush_tile_collect(float *s_out, float *__restrict__ out_tile, const TopkCtx &t,
                                                    u32 row, u32 tile, u32 my_max, u32 n_items, u32 n_holders, u32 *s_top,
-                                                   u32 *s_ncand, u32 *s_tile_max) {
-    const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+                                                   u32 *s_ncand, u32 *s_tile_max, F finish = F(),
+                                                   bool ties_retry = true) {
+    constexpr bool FINISH = !std::is_same<F, TileIdentity>::value;
+    const unsigned tid = threadIdx.x;
+    float4 *s_out4 = reinterpret_cast<float4 *>(s_out);
     if constexpr (DEEP) {
         __syncthreads();                                             // the tile as every thread stored it
-        if constexpr (STORE) {
 #pragma unroll
-            for (int jj = 0; jj < SA_TILE_DOCS / SA_TERM_THREADS / 4; jj++)
-                __stcs(reinterpret_cast<float4 *>(out_tile) + tid + jj * SA_TERM_THREADS,
-                       reinterpret_cast<const float4 *>(s_out)[tid + jj * SA_TERM_THREADS]);
+        for (int jj = 0; jj < SA_TILE_DOCS / SA_TERM_THREADS / 4; jj++) {
+            const unsigned g = tid + jj * SA_TERM_THREADS;
+            float4 v = s_out4[g];
+            finish(g, v);
+            if constexpr (STORE) __stcs(reinterpret_cast<float4 *>(out_tile) + tid + jj * SA_TERM_THREADS, v);
+            if constexpr (FINISH) s_out4[g] = v;
         }
+        if constexpr (FINISH) __syncthreads();                       // the final scores, as every thread wrote them
         deep_tile_collect(s_out, t, row, tile);
         return;
     }
     const u32 k = t.k;
     const u32 tile_doc0 = tile * SA_TILE_DOCS;
-    const bool need_bound = k && n_items > k;                        // CTA-uniform
-    const u32 M = tile_bound_width(k, n_holders);
-    if (need_bound) {
-        u32 v = my_max;
-        for (u32 r = 0; r < M; r++) {
-            u32 m = warp_pop_max(v);
-            if (lane == r) s_top[warp * 8 + r] = m;
-        }
-    }
-    if (k && tid == 0) { *s_ncand = 0; *s_tile_max = 0; }
-    __syncthreads();
-    float thr_f = 0.0f;
-    if (k) {
-        u32 thr = 1u;
-        if (need_bound) thr = max(cta_kth_bound(s_top, k, M == 8u), 1u);
-        thr_f = __uint_as_float(thr);
-    }
+    // the barrier inside also orders the tile's stores before the reads below
+    const float thr_f = __uint_as_float(tile_bound(my_max, k && n_items > k, tile_bound_width(k, n_holders), k, s_top, s_ncand, s_tile_max));
     u64 *__restrict__ my_cand = k ? t.tile_cand + ((u64)row * t.n_tiles + tile) * t.slots : nullptr;
     float4 *__restrict__ out4 = reinterpret_cast<float4 *>(out_tile);
     u32 cand_max = 0;
 #pragma unroll
     for (int jj = 0; jj < SA_TILE_DOCS / SA_TERM_THREADS / 4; jj++) {
         const unsigned g = tid + jj * SA_TERM_THREADS;
-        const float4 v = reinterpret_cast<const float4 *>(s_out)[g];
+        float4 v = s_out4[g];
+        finish(g, v);
         if constexpr (STORE) __stcs(out4 + g, v);
+        // NaN compares false; scores <= 0 are below thr_f > 0
         if (k && ((v.x >= thr_f) | (v.y >= thr_f) | (v.z >= thr_f) | (v.w >= thr_f))) {
             const float vs[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
@@ -550,14 +588,12 @@ __device__ __forceinline__ void flush_tile_collect(const float *s_out, float *__
     if (k) {
         if (cand_max) atomicMax(s_tile_max, cand_max);
         __syncthreads();
-        if (*s_ncand > t.slots)                                      // CTA-uniform: ties at the bound (see above)
-            tile_collect_ties_retry(s_out, false, __float_as_uint(thr_f), t, my_cand, tile_doc0, s_top, s_ncand, s_tile_max);
+        if (ties_retry && *s_ncand > t.slots)                        // CTA-uniform: ties at the bound (see above)
+            tile_collect_ties_retry(s_out, finish, __float_as_uint(thr_f), t, my_cand, tile_doc0, s_top, s_ncand,
+                                    s_tile_max);
         if (tid == 0) {
             const u32 n = *s_ncand;
-            const u64 t_idx = (u64)row * t.n_tiles + tile;
-            t.tile_cnt[t_idx] = min(n, t.slots);
-            t.tile_max[t_idx] = *s_tile_max;
-            if (n > t.slots) t.overflow[row] = 1u;
+            publish_tile(t, row, tile, min(n, t.slots), *s_tile_max, n > t.slots);
         }
     }
     __syncthreads();
@@ -583,7 +619,7 @@ template <bool DEEP = false, typename F>
 __device__ __forceinline__ void collect_tile_f64(const u32 (&key)[SA_TILE_DOCS / SA_TERM_THREADS], u32 my_max,
                                                  u32 n_items, const TopkCtx &t, u64 *__restrict__ tile_d, u32 row,
                                                  u32 tile, u32 *s_top, u32 *s_ncand, u32 *s_tile_max, F score) {
-    const unsigned tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const unsigned tid = threadIdx.x;
     u32 thr;
     if constexpr (DEEP) {
         __shared__ u32 s_hist[256], s_kth, s_krem;
@@ -596,17 +632,7 @@ __device__ __forceinline__ void collect_tile_f64(const u32 (&key)[SA_TILE_DOCS /
         __syncthreads();
         thr = max(kth, 1u);
     } else {
-    const bool need_bound = n_items > t.k;                           // CTA-uniform
-    if (need_bound) {
-        u32 v = my_max;
-        for (u32 r = 0; r < 8; r++) {
-            const u32 m = warp_pop_max(v);
-            if (lane == r) s_top[warp * 8 + r] = m;
-        }
-    }
-    if (tid == 0) { *s_ncand = 0; *s_tile_max = 0; }
-    __syncthreads();
-    thr = need_bound ? max(cta_kth_bound(s_top, t.k, true), 1u) : 1u;
+        thr = tile_bound(my_max, n_items > t.k, 8u, t.k, s_top, s_ncand, s_tile_max);
     }
     const u64 slot0 = ((u64)row * t.n_tiles + tile) * t.slots;
     u32 cand_max = 0;
@@ -627,11 +653,6 @@ __device__ __forceinline__ void collect_tile_f64(const u32 (&key)[SA_TILE_DOCS /
     }
     if (cand_max) atomicMax(s_tile_max, cand_max);
     __syncthreads();
-    if (tid == 0) {
-        const u64 t_idx = (u64)row * t.n_tiles + tile;
-        t.tile_cnt[t_idx] = min(*s_ncand, t.slots);
-        t.tile_max[t_idx] = *s_tile_max;
-        if (*s_ncand > t.slots) t.overflow[row] = 1u;
-    }
+    if (tid == 0) publish_tile(t, row, tile, min(*s_ncand, t.slots), *s_tile_max, *s_ncand > t.slots);
 }
 #endif
