@@ -302,6 +302,36 @@ int sa_score_batch_topk_bool(sa_index *index, uint32_t n_nodes, const uint32_t *
                              uint32_t *out_docs, float *out_scores, uint32_t *n_redone, uint32_t n_facets,
                              const uint32_t *facet_field, const uint32_t *facet_slot, uint32_t *out_total,
                              uint32_t *out_facet_counts);
+/* Per-document group columns of an index (a franchise, a parent SKU, a site), read by the collapsed top-k below.
+ * sa_index_set_group copies codes[0 .. n_values) (n_values == the index's n_docs) into slot `slot` (< SA_MAX_GROUPS),
+ * replacing what the slot held: a code in [0, 2^31 - 1) is the doc's group, -1 means the doc belongs to no group.  The
+ * index owns the copy (uint32 per doc, SA_GROUP_NONE for -1 and past n_docs) and frees it with itself.  A bad
+ * argument is SA_ERR_ARG and leaves the index as it was. */
+#define SA_MAX_GROUPS 4
+#define SA_GROUP_NONE 0xFFFFFFFFu
+int sa_index_set_group(sa_index *index, uint32_t slot, const int32_t *codes, uint64_t n_values);
+/* Collapsed top-k (Elasticsearch's collapse, Solr's collapsing query parser with nullPolicy=expand): one result per
+ * group of group column `group_slot` (sa_index_set_group).  The arguments after group_slot are
+ * sa_score_batch_topk_bool's, in its order and under its refusals.  Per query let S_q be the dense vector
+ * sa_score_batch_topk_bool ranks from (mask applied).  The ranked docs are those with S_q > 0; a group's leader is its
+ * ranked doc with the highest S_q, ties to the lower doc id; a ranked doc whose code is SA_GROUP_NONE is a group of its
+ * own.  Result: the k best leaders by (score desc, doc id asc), with the ids and float32 scores the call without
+ * collapsing returns for those docs, empty slots SA_NO_DOC / 0.  So a column of distinct codes, or one of SA_GROUP_NONE
+ * only, returns sa_score_batch_topk_bool's result bit for bit, and the first k' results at k are the result at k'.
+ * The hit and facet counts count documents, not groups: they equal sa_score_batch_topk_bool's.  Each (query, tile)
+ * keeps its exact k best leaders (a group's global leader is among the k best leaders of its tile whenever the group
+ * is in the global top k), so nothing overflows and *n_redone is always 0.  On a shard the groups are collapsed over
+ * the shard's own docs.  A slot not set is SA_ERR_ARG before any device work. */
+int sa_score_batch_topk_bool_collapse(sa_index *index, uint32_t group_slot, uint32_t n_nodes,
+                                      const uint32_t *node_clause_starts, const uint32_t *clause_node,
+                                      const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                      const float *clause_idf, const float *clause_weight, const uint8_t *clause_occur,
+                                      const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
+                                      uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b,
+                                      uint32_t k, const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
+                                      uint32_t *out_docs, float *out_scores, uint32_t *n_redone, uint32_t n_facets,
+                                      const uint32_t *facet_field, const uint32_t *facet_slot, uint32_t *out_total,
+                                      uint32_t *out_facet_counts);
 /* Scoring at given documents, the second stage after a batched top-k (reranker features, window rescoring): replaces
  * the reference's `arr.score(q)[docs[q]]` (postings.py:652 `score`, indexed at the candidates) without a dense row.
  * The descriptor arguments are sa_score_batch_topk_bool's, in its order and under its refusals; in place of k, the
@@ -355,7 +385,8 @@ typedef struct {
      * search regime alone ran, phrase_kernel_launches > phrase_tile_launches after one = a re-run in the search regime */
     uint64_t phrase_tile_launches;
     /* the bool_tile_kernel instances launched (sa_bool.cu, bool_kernel): bit variant * 10 + form * 2 + masked, with
-     * form 0 Or / And, 1 roles and weights, 2 fields, 3 DisMax, 4 nested and variant 0 plain, 1 FEATURE, 2 COUNT */
+     * form 0 Or / And, 1 roles and weights, 2 fields, 3 DisMax, 4 nested and variant 0 plain, 1 FEATURE, 2 COUNT,
+     * 3 COLLAPSE */
     uint64_t bool_instances;
     /* the sim_tile_kernel / sim_where_tile_kernel instances launched (sa_view.cu, launch_sim_tiles): bit
      * 2 * kind + masked, kind the SA_SIM_* value (0 impact, 1 legacy, 2 classic, 3 BM25, also the BM25 batch's phrase
@@ -370,6 +401,12 @@ typedef struct {
     /* (node, tile) pairs of the boolean entry points' first passes published empty because a MUST / FILTER range or
      * In clause was absent from the tile (its column's tile bounds or code set miss the clause) */
     uint64_t filter_tiles;
+    /* (query, tile) pairs whose leaders the collapse collector took (sa_score_batch_topk_bool_collapse and its
+     * multi-field twin) */
+    uint64_t collapse_tiles;
+    /* windows the collapse walk took past the first, in the tiles and in the per-query select: a tile or a query
+     * whose best ranked docs crowd into few groups walks its docs in several windows */
+    uint64_t collapse_windows;
 } sa_stats;
 int sa_stats_reset(sa_index *index);
 int sa_stats_get(sa_index *index, sa_stats *out);
@@ -464,6 +501,22 @@ int sa_multi_score_batch_topk_bool(sa_multi *multi, uint32_t n_nodes, const uint
                                    uint64_t where_stride, uint32_t *out_docs, float *out_scores, uint32_t *n_redone,
                                    uint32_t n_facets, const uint32_t *facet_field, const uint32_t *facet_slot,
                                    uint32_t *out_total, uint32_t *out_facet_counts);
+/* sa_score_batch_topk_bool_collapse over the fields of a multi: group column group_slot of field group_field's index
+ * (a field slot of the multi), then sa_multi_score_batch_topk_bool's arguments in its order.  A field out of range or a
+ * slot not set on its index is SA_ERR_ARG before any device work. */
+int sa_multi_score_batch_topk_bool_collapse(sa_multi *multi, uint32_t group_field, uint32_t group_slot,
+                                            uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                            const uint32_t *clause_node, const uint32_t *clause_field,
+                                            const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                            const float *clause_idf, const float *clause_weight,
+                                            const uint8_t *clause_occur, const uint32_t *clause_group,
+                                            const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
+                                            uint32_t slop, const float *avg_doc_len, const float *k1, const float *b,
+                                            uint32_t k, const uint32_t *where_bits, uint64_t where_n,
+                                            uint64_t where_stride, uint32_t *out_docs, float *out_scores,
+                                            uint32_t *n_redone, uint32_t n_facets, const uint32_t *facet_field,
+                                            const uint32_t *facet_slot, uint32_t *out_total,
+                                            uint32_t *out_facet_counts);
 /* sa_score_docs_bool over the fields of a multi: sa_multi_score_batch_topk_bool's descriptor arguments up to b, then
  * the docs (global ids of the fields' document set), n_per_query and out_scores, under sa_score_docs_bool's contract
  * with sa_multi_score_batch_topk_bool as the top-k it matches. */

@@ -30,7 +30,7 @@ class SaStats(ctypes.Structure):
                 ("phrase_cont_words", c_u64), ("phrase_matched_docs", c_u64), ("phrase_tile_launches", c_u64),
                 ("bool_instances", c_u64), ("sim_instances", c_u64), ("term_kernel_groups", c_u64),
                 ("deep_tiles", c_u64),
-                ("filter_tiles", c_u64)]
+                ("filter_tiles", c_u64), ("collapse_tiles", c_u64), ("collapse_windows", c_u64)]
 
 
 # name -> (restype, argtypes); must list EVERY symbol include/searcharray_b200.h declares
@@ -64,6 +64,10 @@ SIGNATURES = {
     "sa_score_batch_topk_bool": (c_int, [P_void, c_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8, P_u32, P_f32,
                                          P_u32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32, P_u32, c_u64, c_u64, P_u32,
                                          P_f32, P_u32, c_u32, P_u32, P_u32, P_u32, P_u32]),
+    "sa_index_set_group": (c_int, [P_void, c_u32, P_i32, c_u64]),
+    "sa_score_batch_topk_bool_collapse": (c_int, [P_void, c_u32, c_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8,
+                                                  P_u32, P_f32, P_u32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32, P_u32,
+                                                  c_u64, c_u64, P_u32, P_f32, P_u32, c_u32, P_u32, P_u32, P_u32, P_u32]),
     "sa_score_docs_bool": (c_int, [P_void, c_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8, P_u32, P_f32, P_u32,
                                    c_u32, c_u32, c_f32, c_f32, c_f32, P_u32, c_u32, P_f32]),
     "sa_batch_upload": (c_int, [P_void, P_u32, P_u32, P_f32, c_u32, c_u32, c_f32, c_f32, c_f32, c_u32]),
@@ -98,6 +102,10 @@ SIGNATURES = {
     "sa_multi_score_batch_topk_bool": (c_int, [P_void, c_u32, P_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8,
                                                P_u32, P_f32, P_u32, c_u32, c_u32, P_f32, P_f32, P_f32, c_u32, P_u32,
                                                c_u64, c_u64, P_u32, P_f32, P_u32, c_u32, P_u32, P_u32, P_u32, P_u32]),
+    "sa_multi_score_batch_topk_bool_collapse": (c_int, [P_void, c_u32, c_u32, c_u32, P_u32, P_u32, P_u32, P_u32, P_u32,
+                                                        P_f32, P_f32, P_u8, P_u32, P_f32, P_u32, c_u32, c_u32, P_f32,
+                                                        P_f32, P_f32, c_u32, P_u32, c_u64, c_u64, P_u32, P_f32, P_u32,
+                                                        c_u32, P_u32, P_u32, P_u32, P_u32]),
     "sa_multi_score_docs_bool": (c_int, [P_void, c_u32, P_u32, P_u32, P_u32, P_u32, P_u32, P_f32, P_f32, P_u8, P_u32,
                                          P_f32, P_u32, c_u32, c_u32, P_f32, P_f32, P_f32, P_u32, c_u32, P_f32]),
     "sa_op_popcount64_reduce": (c_int, [P_u64, c_u64, c_int, P_u64, P_f32, P_u64]),

@@ -160,6 +160,13 @@ struct BoolCount {
     u32 n_facets, n_bins;
 };
 
+// The group column of a collapse launch (COLLAPSE instances only): per index-local doc its code or SA_GROUP_NONE
+// (sa_index::d_groups), and the call's count of walk windows past the first (BoolResult::windows).
+struct BoolCollapse {
+    const u32 *groups;
+    u32 *windows;
+};
+
 struct BoolState {
     DevBuf desc;         // the call's descriptor arrays, one section each (BoolDescs)
     DevBuf d_keys;       // the call's result block (BoolResult): one device-to-host copy
@@ -393,12 +400,16 @@ __device__ __forceinline__ void bool_count_tile(const BoolCount &cn, float *s_ti
 // WHERE: only docs whose bit of the mask row of query blockIdx.x is set rank (never in a store pass).  FEATURE (with
 // OCCUR): clauses whose row is SA_BOOL_FEATURE_ROW score their column feat[clause] (BoolFeature).  COUNT (with
 // FEATURE): the collected tile is counted into `cn` (bool_count_tile).  DEEP: k > SA_TOPK_MAX, the tile's candidates
-// from deep_tile_collect.
-template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, bool FEATURE, bool COUNT, bool DEEP>
+// from deep_tile_collect.  COLLAPSE: the tile's k best group leaders (collapse_tile_collect over the group column
+// co.groups, its hash in s_dyn, free once the fold is done), then, when the launch counts (cn.total non-NULL, a
+// CTA-uniform test), the tile's hits and facets as COUNT counts them.
+template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, bool FEATURE, bool COUNT, bool DEEP,
+          bool COLLAPSE = false>
 __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__restrict__ occ,
                                           const BoolField *__restrict__ fld, const BoolGroup *__restrict__ grp,
                                           float *s_dyn, unsigned long long *s_g, const BoolNest nb, const WhereMask wh,
-                                          const BoolFeature *__restrict__ feat, const BoolCount cn) {
+                                          const BoolFeature *__restrict__ feat, const BoolCount cn,
+                                          const BoolCollapse co) {
     constexpr int PER = SA_TILE_DOCS / SA_TERM_THREADS / 4;        // float4 groups per thread
     __shared__ __align__(16) float s_tile[SA_TILE_DOCS];
     __shared__ u32 s_lo[SA_BOOL_MAX_CLAUSES], s_hi[SA_BOOL_MAX_CLAUSES];
@@ -624,6 +635,11 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
         if (tid == 0) nb.flags[(u64)bq.pad * nb.n_tiles + tile] = ranked ? 1u : 0u;
         return;
     }
+    if constexpr (COLLAPSE) {
+        collapse_tile_collect(s_tile, a.topk, q, tile, co.groups, reinterpret_cast<u32 *>(s_dyn), co.windows);
+        if (cn.total != nullptr) bool_count_tile(cn, s_tile);
+        return;
+    }
     flush_tile_collect<false, DEEP>(s_tile, nullptr, a.topk, q, tile, my_max, SA_TILE_DOCS, 0, s_top, &s_ncand,
                                     &s_tile_max);
     if (COUNT) bool_count_tile(cn, s_tile);
@@ -632,7 +648,8 @@ __device__ __forceinline__ void bool_tile(const BoolArgs &a, const BoolOccur *__
 // Every instance of the fold: bool_tile with every argument, of which it reads those its flags name (the others are
 // NULL and never read).  MIN_CTAS holds an instance to the CTAs per SM it was tuned for (0: no minimum); bool_kernel
 // lists the instances.  DISMAX: the groups' running max and sum live in SA_BOOL_DISMAX_SMEM bytes of dynamic shared
-// memory (a thread's strips, owner-only, so no extra barriers).
+// memory (a thread's strips, owner-only, so no extra barriers).  COLLAPSE: the collector's hash in the same dynamic
+// memory (bool_smem).
 #define SA_BOOL_DISMAX_SMEM (2 * SA_TILE_DOCS * sizeof(float))
 
 // bool_tile's s_g placed ahead of the fold's own shared arrays.  Where the compiler places a __shared__ array follows
@@ -645,18 +662,19 @@ __device__ __forceinline__ unsigned long long *bool_s_g_first() {
 }
 
 template <bool OCCUR, bool FIELDS, bool DISMAX, bool NESTED, bool WHERE, bool FEATURE, bool COUNT, bool DEEP,
-          int MIN_CTAS>
+          int MIN_CTAS, bool COLLAPSE = false>
 __global__ void __launch_bounds__(SA_TERM_THREADS, MIN_CTAS)
 bool_tile_kernel(const BoolArgs a, const BoolOccur *__restrict__ occ, const BoolField *__restrict__ fld,
                  const BoolGroup *__restrict__ grp, const BoolNest nb, const WhereMask wh,
-                 const BoolFeature *__restrict__ feat, const BoolCount cn) {
+                 const BoolFeature *__restrict__ feat, const BoolCount cn, const BoolCollapse co) {
     extern __shared__ __align__(16) float s_dyn[];
     if constexpr (DISMAX && !WHERE && !FEATURE) {
-        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, FEATURE, COUNT, DEEP>(a, occ, fld, grp, s_dyn,
-                                                                        bool_s_g_first<NESTED, DEEP>(), nb, wh, feat, cn);
+        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, FEATURE, COUNT, DEEP, COLLAPSE>(
+            a, occ, fld, grp, s_dyn, bool_s_g_first<NESTED, DEEP>(), nb, wh, feat, cn, co);
     } else {
         __shared__ unsigned long long s_g[3];
-        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, FEATURE, COUNT, DEEP>(a, occ, fld, grp, s_dyn, s_g, nb, wh, feat, cn);
+        bool_tile<OCCUR, FIELDS, DISMAX, NESTED, WHERE, FEATURE, COUNT, DEEP, COLLAPSE>(a, occ, fld, grp, s_dyn, s_g, nb,
+                                                                                  wh, feat, cn, co);
     }
 }
 
@@ -819,20 +837,23 @@ namespace {
 enum BoolForm { BOOL_OR_AND, BOOL_OCCUR, BOOL_FIELDS, BOOL_DISMAX, BOOL_NESTED };
 
 // The instances of a form: plain; FEATURE, for a batch with feature clauses; COUNT (with FEATURE), for the first pass
-// of a counting call.  The last two exist from BOOL_OCCUR up.
-enum BoolVariant { BOOL_PLAIN, BOOL_FEATURE, BOOL_COUNT };
+// of a counting call; COLLAPSE (with FEATURE from BOOL_OCCUR up, counting at run time), for the top-level launch of a
+// collapsed call.  FEATURE and COUNT exist from BOOL_OCCUR up.
+enum BoolVariant { BOOL_PLAIN, BOOL_FEATURE, BOOL_COUNT, BOOL_COLLAPSE };
 
 typedef void (*BoolKernel)(BoolArgs, const BoolOccur *, const BoolField *, const BoolGroup *, BoolNest, WhereMask,
-                           const BoolFeature *, BoolCount);
+                           const BoolFeature *, BoolCount, BoolCollapse);
 
 // The instance a launch of `form` runs, with or without a document mask.  The fields instance is held to three CTAs per
 // SM, as the single-field roles instance runs (80 registers, no spills; at two, 90 registers, it ran 23-24% slower);
 // the DisMax and nested ones to two (DESIGN.md sections 3.10.3, 3.10.4); each masked instance to its unmasked
 // instance's CTAs per SM (section 3.11); the FEATURE and COUNT instances to their form's (three for the roles form).
-// A nested call's store passes run the unmasked nested instance.
+// The COLLAPSE instances (one depth: DEEP is unused) run at two CTAs per SM, which their shared memory allows (the
+// tile, the window's run and a 32 KB hash: ~74 KB); at three the roles and fields ones spilled 336 bytes.  A nested
+// call's store passes run the unmasked nested instance.
 template <bool DEEP>
 BoolKernel bool_instance(BoolForm form, bool masked, BoolVariant variant) {
-    static const BoolKernel instances[3][5][2] = {
+    static const BoolKernel instances[4][5][2] = {
         {
             {bool_tile_kernel<false, false, false, false, false, false, false, DEEP, 0>,
              bool_tile_kernel<false, false, false, false, true, false, false, DEEP, 2>},
@@ -867,6 +888,18 @@ BoolKernel bool_instance(BoolForm form, bool masked, BoolVariant variant) {
             {bool_tile_kernel<true, true, true, true, false, true, true, DEEP, 2>,
              bool_tile_kernel<true, true, true, true, true, true, true, DEEP, 2>},
         },
+        {
+            {bool_tile_kernel<false, false, false, false, false, false, false, false, 2, true>,
+             bool_tile_kernel<false, false, false, false, true, false, false, false, 2, true>},
+            {bool_tile_kernel<true, false, false, false, false, true, false, false, 2, true>,
+             bool_tile_kernel<true, false, false, false, true, true, false, false, 2, true>},
+            {bool_tile_kernel<true, true, false, false, false, true, false, false, 2, true>,
+             bool_tile_kernel<true, true, false, false, true, true, false, false, 2, true>},
+            {bool_tile_kernel<true, true, true, false, false, true, false, false, 2, true>,
+             bool_tile_kernel<true, true, true, false, true, true, false, false, 2, true>},
+            {bool_tile_kernel<true, true, true, true, false, true, false, false, 2, true>,
+             bool_tile_kernel<true, true, true, true, true, true, false, false, 2, true>},
+        },
     };
     return instances[variant][form][masked];
 }
@@ -874,6 +907,13 @@ BoolKernel bool_instance(BoolForm form, bool masked, BoolVariant variant) {
 // deep: k > SA_TOPK_MAX, the instance whose tiles collect with deep_tile_collect
 BoolKernel bool_kernel(BoolForm form, bool masked, BoolVariant variant, bool deep) {
     return deep ? bool_instance<true>(form, masked, variant) : bool_instance<false>(form, masked, variant);
+}
+
+// The dynamic shared memory of an instance: the DisMax groups' strips from BOOL_DISMAX up, and a COLLAPSE instance's
+// hash (collapse_tile_collect), which reuses the strips once the fold is done.
+size_t bool_smem(BoolForm form, bool collapse) {
+    const size_t fold = form >= BOOL_DISMAX ? SA_BOOL_DISMAX_SMEM : 0;
+    return collapse ? std::max<size_t>(fold, SA_COLLAPSE_TILE_SMEM) : fold;
 }
 
 // The fields of one call and where the call keeps its state.  The single-index entry point passes one field and the
@@ -901,7 +941,8 @@ enum BoolKind { KIND_TERM, KIND_PHRASE, KIND_FEATURE, KIND_RANGE, KIND_IN };
 // every clause on field 0.  clause_group / clause_tie non-NULL (with clause_occur): DisMax groups, on a field table.
 // clause_node non-NULL (with the DisMax arrays): n_nodes nodes, the first n_queries top-level, clause c being nested
 // node clause_node[c] unless SA_NO_NODE; otherwise n_nodes == n_queries.  where_bits non-NULL: the document mask.
-// out_total non-NULL: hit counts, and counts over the n_facets facets.
+// out_total non-NULL: hit counts, and counts over the n_facets facets.  groups non-NULL: a collapsed call on that group
+// column (index-local ids), set by the collapse entry points.
 struct BoolInput {
     u32 n_nodes;
     const u32 *node_clause_starts, *clause_node, *clause_field, *clause_terms, *clause_term_starts;
@@ -919,6 +960,7 @@ struct BoolInput {
     u32 n_facets;
     const u32 *facet_field, *facet_slot;
     u32 *out_total, *out_facet_counts;
+    const u32 *groups;
 
     bool nested(u32 c) const { return clause_node && clause_node[c] != SA_NO_NODE; }
     u32 field(u32 c) const { return clause_field ? clause_field[c] : 0; }
@@ -957,8 +999,8 @@ struct BoolDescs { size_t clauses, queries, occur, groups, nest, fields, feature
 
 // The result block of a call, in BoolState::d_keys and downloaded whole into the pinned staging: the keys
 // [n_queries][k], then the overflow flags [n_queries] and, counting, the totals [n_queries] and the facet rows
-// [n_queries][n_bins], then the tiles absent range and In filters made empty (BoolFeature::skipped).  `base` is either
-// copy.
+// [n_queries][n_bins], then the tiles absent range and In filters made empty (BoolFeature::skipped) and the collapse
+// walk's windows past the first (BoolCollapse::windows).  `base` is either copy.
 struct BoolResult {
     size_t n_keys, n_queries, n_bins;
     bool counting;
@@ -967,12 +1009,13 @@ struct BoolResult {
     u32 *total(void *base) const { return ovf(base) + n_queries; }
     u32 *counts(void *base) const { return total(base) + n_queries; }
     u32 *skipped(void *base) const { return ovf(base) + n_queries * (counting ? 2 + n_bins : 1); }
-    size_t bytes() const { return n_keys * sizeof(u64) + (n_queries * (counting ? 2 + n_bins : 1) + 1) * sizeof(u32); }
+    u32 *windows(void *base) const { return skipped(base) + 1; }
+    size_t bytes() const { return n_keys * sizeof(u64) + (n_queries * (counting ? 2 + n_bins : 1) + 2) * sizeof(u32); }
 };
 
 struct BoolPlan {
     BoolForm form = BOOL_OR_AND;
-    u32 slots = 0;                      // candidate slots per tile of a first pass
+    u32 slots = 0;                      // candidate slots per tile of a first pass (k when collapsing)
     std::vector<BoolClause> clauses;
     std::vector<BoolQuery> queries;
     std::vector<u32> group_start;       // queries [group_start[i], group_start[i + 1]) share one launch and its rows
@@ -1072,7 +1115,6 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const BoolInput &in, co
     const BoolField *fld = P.form >= BOOL_FIELDS ? (const BoolField *)(d + P.descs.fields) : nullptr;
     const BoolGroup *grp = P.form >= BOOL_DISMAX ? (const BoolGroup *)(d + P.descs.groups) : nullptr;
     BoolNest nb{nullptr, nullptr, nullptr, 0};
-    const size_t smem = P.form >= BOOL_DISMAX ? SA_BOOL_DISMAX_SMEM : 0;
     const BoolFeature *feat = P.features.empty() ? nullptr : (const BoolFeature *)(d + P.descs.features);
     BoolCount cn = P.count;                 // counting: the call's rows, from query q0's in the counting launch
     if (in.out_total) {
@@ -1080,12 +1122,17 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const BoolInput &in, co
         cn.total = P.result.total(S.d_keys.p) + row0;
         cn.counts = P.result.counts(S.d_keys.p) + (u64)row0 * cn.n_bins;
     }
+    const BoolCollapse co{in.groups, P.result.windows(S.d_keys.p)};
     auto launch = [&](bool c, bool masked, u32 n_q, const BoolArgs &args, const BoolNest &n, const WhereMask &w) -> int {
-        const BoolVariant variant = bool_variant(P, c);
-        bool_kernel(P.form, masked, variant, in.k > SA_TOPK_MAX)<<<dim3(n_q, n_tiles), SA_TERM_THREADS, smem,
-                                                                    ix->stream>>>(args, occ, fld, grp, n, w, feat, cn);
+        // a collapsed call's top-level launch collapses (and counts where cn.total is set: a collapse is never re-run)
+        const bool collapse = in.groups && !n.store;
+        const BoolVariant variant = collapse ? BOOL_COLLAPSE : bool_variant(P, c);
+        bool_kernel(P.form, masked, variant, in.k > SA_TOPK_MAX)<<<dim3(n_q, n_tiles), SA_TERM_THREADS,
+                                                                    bool_smem(P.form, collapse), ix->stream>>>(
+            args, occ, fld, grp, n, w, feat, cn, co);
         SA_CUDA(cudaGetLastError());
-        if (in.k > SA_TOPK_MAX && !n.store) ix->stats.deep_tiles += (u64)n_q * n_tiles;
+        if (collapse) ix->stats.collapse_tiles += (u64)n_q * n_tiles;
+        else if (in.k > SA_TOPK_MAX && !n.store) ix->stats.deep_tiles += (u64)n_q * n_tiles;
         ix->stats.total_launches++;
         ix->stats.bool_instances |= 1ull << (variant * 10 + P.form * 2 + (masked ? 1 : 0));
         return SA_OK;
@@ -1107,13 +1154,16 @@ int bool_run_group(const BoolCall &X, const BoolPlan &P, const BoolInput &in, co
         nb.store = nullptr;
     }
     if ((rc = launch(count, wh.bits != nullptr, nq, a, nb, wh))) return rc;
-    return launch_topk_select(ix, t, nq, ix->doc_base, P.result.keys(S.d_keys.p) + (size_t)q0 * in.k, nullptr);
+    u64 *keys = P.result.keys(S.d_keys.p) + (size_t)q0 * in.k;
+    if (in.groups) return launch_topk_collapse(ix, t, nq, ix->doc_base, in.groups, keys, co.windows);
+    return launch_topk_select(ix, t, nq, ix->doc_base, keys, nullptr);
 }
 
-// The DisMax instances' dynamic shared memory above the default 48 KB, and the carveout that fits two CTAs per SM
-// (~2 x 98 KB of shared memory), on the current device (function attributes are per device).
-int bool_dismax_smem(BoolKernel kernel) {
-    SA_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SA_BOOL_DISMAX_SMEM));
+// An instance's dynamic shared memory (`bytes`, above what fits the default 48 KB with its static arrays), and the
+// carveout that fits its CTAs per SM (two DisMax CTAs: ~2 x 98 KB), on the current device (function attributes are
+// per device).
+int bool_set_smem(BoolKernel kernel, size_t bytes) {
+    SA_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
     SA_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout,
                                  (int)cudaSharedmemCarveoutMaxShared));
     return SA_OK;
@@ -1315,14 +1365,15 @@ BoolPlan bool_plan(const BoolCall &X, const BoolInput &in, const BoolChecked &ch
     const u32 n_nodes = in.n_nodes, n_queries = in.n_queries, n_fields = (u32)X.ix.size();
     const u32 *starts = in.node_clause_starts;
     const bool occur = in.clause_occur != nullptr, dismax = in.clause_group != nullptr;
-    // an Or / And batch with a feature clause or counts runs as roles and weights, every clause SHOULD with weight 1
-    const bool roles = occur || chk.features || in.out_total != nullptr;
+    // an Or / And batch with a feature clause, or counts without collapsing (whose Or / And instance counts), runs as
+    // roles and weights, every clause SHOULD with weight 1
+    const bool roles = occur || chk.features || (in.out_total != nullptr && !in.groups);
     auto role = [&](u32 c) {
         return occur ? BoolOccur{in.clause_weight[c], in.clause_occur[c]} : BoolOccur{1.0f, SA_OCCUR_SHOULD};
     };
     BoolPlan P;
     const u32 n_tiles = sa_n_tiles(X.lead()->n_docs);
-    P.slots = sa_topk_slots(in.k);
+    P.slots = in.groups ? in.k : sa_topk_slots(in.k);     // a collapse tile keeps its k best leaders
     const u64 stride = sa_padded_docs(X.lead()->n_docs);
     const u32 group_q = (u32)std::min<u64>(65535, std::max<u64>(1, (1ull << 30) / ((u64)n_tiles * (P.slots * sizeof(u64) + 8))));
     const u32 group_rows = (u32)std::max<u64>(1, (4ull << 30) / (stride * sizeof(float)));
@@ -1488,10 +1539,13 @@ int bool_upload(const BoolCall &X, const BoolInput &in, const BoolPlan &P, Where
         // the first pass's variant and that of the store passes and re-runs, each masked only when the call is
         const BoolVariant first = bool_variant(P, in.out_total != nullptr), rest = bool_variant(P, false);
         for (int masked = 0; masked <= (where->bits != nullptr); masked++)
-            if ((rc = bool_dismax_smem(bool_kernel(P.form, masked, first, in.k > SA_TOPK_MAX))) ||
-                (rest != first && (rc = bool_dismax_smem(bool_kernel(P.form, masked, rest, in.k > SA_TOPK_MAX)))))
+            if ((rc = bool_set_smem(bool_kernel(P.form, masked, first, in.k > SA_TOPK_MAX), SA_BOOL_DISMAX_SMEM)) ||
+                (rest != first &&
+                 (rc = bool_set_smem(bool_kernel(P.form, masked, rest, in.k > SA_TOPK_MAX), SA_BOOL_DISMAX_SMEM))))
                 return rc;
     }
+    for (int masked = 0; in.groups && masked <= (where->bits != nullptr); masked++)
+        if ((rc = bool_set_smem(bool_kernel(P.form, masked, BOOL_COLLAPSE, false), bool_smem(P.form, true)))) return rc;
     SA_CUDA(cudaMemsetAsync(P.result.ovf(S.d_keys.p), 0, P.result.bytes() - P.result.n_keys * sizeof(u64),
                             lead->stream));
     return SA_OK;
@@ -1511,6 +1565,7 @@ int bool_collect(const BoolCall &X, const BoolPlan &P, const BoolInput &in, cons
     const std::vector<u32> ovf(R.ovf(h), R.ovf(h) + nq);
     sa_unpack_keys(R.keys(h), R.n_keys, in.out_docs, in.out_scores);
     lead->stats.filter_tiles += *R.skipped(h);
+    lead->stats.collapse_windows += *R.windows(h);
     if (R.counting) {
         memcpy(in.out_total, R.total(h), (size_t)nq * sizeof(u32));
         if (R.n_bins) memcpy(in.out_facet_counts, R.counts(h), (size_t)nq * R.n_bins * sizeof(u32));
@@ -1717,17 +1772,17 @@ int bool_multi_call(sa_multi *m, const float *avg_doc_len, const float *k1, cons
 
 }  // namespace
 
-// bool_topk under the index's own lock, with its state and buffers.
-extern "C" int sa_score_batch_topk_bool(sa_index *ix, uint32_t n_nodes, const uint32_t *node_clause_starts,
-                                        const uint32_t *clause_node, const uint32_t *clause_terms,
-                                        const uint32_t *clause_term_starts, const float *clause_idf,
-                                        const float *clause_weight, const uint8_t *clause_occur,
-                                        const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
-                                        uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b,
-                                        uint32_t k, const uint32_t *where_bits, uint64_t where_n,
-                                        uint64_t where_stride, uint32_t *out_docs, float *out_scores,
-                                        uint32_t *n_redone, uint32_t n_facets, const uint32_t *facet_field,
-                                        const uint32_t *facet_slot, uint32_t *out_total, uint32_t *out_facet_counts) {
+// bool_topk under the index's own lock, with its state and buffers; collapsed on the index's group column
+// *group_slot where group_slot is not NULL.
+static int bool_topk_index(sa_index *ix, const uint32_t *group_slot, uint32_t n_nodes,
+                           const uint32_t *node_clause_starts, const uint32_t *clause_node, const uint32_t *clause_terms,
+                           const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
+                           const uint8_t *clause_occur, const uint32_t *clause_group, const float *clause_tie,
+                           const uint32_t *mm, uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b,
+                           uint32_t k, const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
+                           uint32_t *out_docs, float *out_scores, uint32_t *n_redone, uint32_t n_facets,
+                           const uint32_t *facet_field, const uint32_t *facet_slot, uint32_t *out_total,
+                           uint32_t *out_facet_counts) {
     SA_CHECK(!clause_weight == !clause_occur, "clause_weight and clause_occur are both given or both NULL");
     SA_CHECK(!clause_group == !clause_tie && (!clause_group || clause_occur),
              "clause_group and clause_tie are both given (with clause_occur) or both NULL");
@@ -1742,14 +1797,86 @@ extern "C" int sa_score_batch_topk_bool(sa_index *ix, uint32_t n_nodes, const ui
     SA_CUDA(cudaSetDevice(ix->device));
     if (!ix->boolq) ix->boolq.reset(new BoolState());
     const BoolCall X{{ix}, {avg_doc_len}, {k1}, {b}, false, ix->boolq.get(), &ix->cand, &ix->h_pinned};
-    const BoolInput in{n_nodes, node_clause_starts, clause_node, nullptr, clause_terms, clause_term_starts, clause_idf,
-                       clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k, where_bits,
-                       where_n, where_stride, out_docs, out_scores, n_redone, n_facets, facet_field, facet_slot,
-                       out_total, out_facet_counts};
+    BoolInput in{n_nodes, node_clause_starts, clause_node, nullptr, clause_terms, clause_term_starts, clause_idf,
+                 clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k, where_bits,
+                 where_n, where_stride, out_docs, out_scores, n_redone, n_facets, facet_field, facet_slot,
+                 out_total, out_facet_counts, nullptr};
+    if (group_slot) {
+        SA_CHECK(*group_slot < SA_MAX_GROUPS && (ix->group_set >> *group_slot & 1u), "group slot %u is not set",
+                 *group_slot);
+        in.groups = ix->d_groups[*group_slot].as<const u32>();
+    }
     return bool_topk(X, in);
 }
 
-// bool_topk under the multi's lock, with its state and candidate buffer.
+extern "C" int sa_score_batch_topk_bool(sa_index *ix, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                                        const uint32_t *clause_node, const uint32_t *clause_terms,
+                                        const uint32_t *clause_term_starts, const float *clause_idf,
+                                        const float *clause_weight, const uint8_t *clause_occur,
+                                        const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
+                                        uint32_t n_queries, uint32_t slop, float avg_doc_len, float k1, float b,
+                                        uint32_t k, const uint32_t *where_bits, uint64_t where_n,
+                                        uint64_t where_stride, uint32_t *out_docs, float *out_scores,
+                                        uint32_t *n_redone, uint32_t n_facets, const uint32_t *facet_field,
+                                        const uint32_t *facet_slot, uint32_t *out_total, uint32_t *out_facet_counts) {
+    return bool_topk_index(ix, nullptr, n_nodes, node_clause_starts, clause_node, clause_terms, clause_term_starts,
+                           clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop,
+                           avg_doc_len, k1, b, k, where_bits, where_n, where_stride, out_docs, out_scores, n_redone,
+                           n_facets, facet_field, facet_slot, out_total, out_facet_counts);
+}
+
+extern "C" int sa_score_batch_topk_bool_collapse(sa_index *ix, uint32_t group_slot, uint32_t n_nodes,
+                                                 const uint32_t *node_clause_starts, const uint32_t *clause_node,
+                                                 const uint32_t *clause_terms, const uint32_t *clause_term_starts,
+                                                 const float *clause_idf, const float *clause_weight,
+                                                 const uint8_t *clause_occur, const uint32_t *clause_group,
+                                                 const float *clause_tie, const uint32_t *mm, uint32_t n_queries,
+                                                 uint32_t slop, float avg_doc_len, float k1, float b, uint32_t k,
+                                                 const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride,
+                                                 uint32_t *out_docs, float *out_scores, uint32_t *n_redone,
+                                                 uint32_t n_facets, const uint32_t *facet_field,
+                                                 const uint32_t *facet_slot, uint32_t *out_total,
+                                                 uint32_t *out_facet_counts) {
+    return bool_topk_index(ix, &group_slot, n_nodes, node_clause_starts, clause_node, clause_terms, clause_term_starts,
+                           clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop,
+                           avg_doc_len, k1, b, k, where_bits, where_n, where_stride, out_docs, out_scores, n_redone,
+                           n_facets, facet_field, facet_slot, out_total, out_facet_counts);
+}
+
+// bool_topk under the multi's lock, with its state and candidate buffer; collapsed on group column group[1] of field
+// group[0]'s index where group is not NULL.
+static int bool_topk_multi(sa_multi *m, const uint32_t *group, uint32_t n_nodes, const uint32_t *node_clause_starts,
+                           const uint32_t *clause_node, const uint32_t *clause_field, const uint32_t *clause_terms,
+                           const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
+                           const uint8_t *clause_occur, const uint32_t *clause_group, const float *clause_tie,
+                           const uint32_t *mm, uint32_t n_queries, uint32_t slop, const float *avg_doc_len,
+                           const float *k1, const float *b, uint32_t k, const uint32_t *where_bits, uint64_t where_n,
+                           uint64_t where_stride, uint32_t *out_docs, float *out_scores, uint32_t *n_redone,
+                           uint32_t n_facets, const uint32_t *facet_field, const uint32_t *facet_slot,
+                           uint32_t *out_total, uint32_t *out_facet_counts) {
+    SA_CHECK(!clause_group == !clause_tie, "clause_group and clause_tie are both given or both NULL");
+    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
+             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
+    SA_CHECK(m && out_docs && out_scores && avg_doc_len && k1 && b, "NULL argument");
+    SA_CHECK(n_nodes == 0 || (node_clause_starts && clause_field && clause_terms && clause_term_starts &&
+                                clause_idf && clause_weight && clause_occur && mm), "NULL argument");
+    SA_CHECK(k >= 1 && k <= SA_TOPK_DEEP_MAX, "k must be in [1, %d]", SA_TOPK_DEEP_MAX);
+    if (n_redone) *n_redone = 0;
+    return bool_multi_call(m, avg_doc_len, k1, b, [&](const BoolCall &X) {
+        BoolInput in{n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
+                     clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
+                     where_bits, where_n, where_stride, out_docs, out_scores, n_redone, n_facets, facet_field,
+                     facet_slot, out_total, out_facet_counts, nullptr};
+        if (group) {
+            SA_CHECK(group[0] < X.ix.size(), "group field %u out of range (%u fields)", group[0], (u32)X.ix.size());
+            SA_CHECK(group[1] < SA_MAX_GROUPS && (X.ix[group[0]]->group_set >> group[1] & 1u),
+                     "group slot %u is not set on field %u", group[1], group[0]);
+            in.groups = X.ix[group[0]]->d_groups[group[1]].as<const u32>();
+        }
+        return bool_topk(X, in);
+    });
+}
+
 extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, uint32_t n_nodes, const uint32_t *node_clause_starts,
                                               const uint32_t *clause_node, const uint32_t *clause_field,
                                               const uint32_t *clause_terms, const uint32_t *clause_term_starts,
@@ -1762,21 +1889,26 @@ extern "C" int sa_multi_score_batch_topk_bool(sa_multi *m, uint32_t n_nodes, con
                                               uint32_t *n_redone, uint32_t n_facets, const uint32_t *facet_field,
                                               const uint32_t *facet_slot, uint32_t *out_total,
                                               uint32_t *out_facet_counts) {
-    SA_CHECK(!clause_group == !clause_tie, "clause_group and clause_tie are both given or both NULL");
-    SA_CHECK(clause_node ? clause_group != nullptr : n_nodes == n_queries,
-             "clause_node needs the DisMax arrays; without it n_nodes == n_queries");
-    SA_CHECK(m && out_docs && out_scores && avg_doc_len && k1 && b, "NULL argument");
-    SA_CHECK(n_nodes == 0 || (node_clause_starts && clause_field && clause_terms && clause_term_starts &&
-                                clause_idf && clause_weight && clause_occur && mm), "NULL argument");
-    SA_CHECK(k >= 1 && k <= SA_TOPK_DEEP_MAX, "k must be in [1, %d]", SA_TOPK_DEEP_MAX);
-    if (n_redone) *n_redone = 0;
-    return bool_multi_call(m, avg_doc_len, k1, b, [&](const BoolCall &X) {
-        const BoolInput in{n_nodes, node_clause_starts, clause_node, clause_field, clause_terms, clause_term_starts,
-                           clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm, n_queries, slop, k,
-                           where_bits, where_n, where_stride, out_docs, out_scores, n_redone, n_facets, facet_field,
-                           facet_slot, out_total, out_facet_counts};
-        return bool_topk(X, in);
-    });
+    return bool_topk_multi(m, nullptr, n_nodes, node_clause_starts, clause_node, clause_field, clause_terms,
+                           clause_term_starts, clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm,
+                           n_queries, slop, avg_doc_len, k1, b, k, where_bits, where_n, where_stride, out_docs,
+                           out_scores, n_redone, n_facets, facet_field, facet_slot, out_total, out_facet_counts);
+}
+
+extern "C" int sa_multi_score_batch_topk_bool_collapse(
+    sa_multi *m, uint32_t group_field, uint32_t group_slot, uint32_t n_nodes, const uint32_t *node_clause_starts,
+    const uint32_t *clause_node, const uint32_t *clause_field, const uint32_t *clause_terms,
+    const uint32_t *clause_term_starts, const float *clause_idf, const float *clause_weight,
+    const uint8_t *clause_occur, const uint32_t *clause_group, const float *clause_tie, const uint32_t *mm,
+    uint32_t n_queries, uint32_t slop, const float *avg_doc_len, const float *k1, const float *b, uint32_t k,
+    const uint32_t *where_bits, uint64_t where_n, uint64_t where_stride, uint32_t *out_docs, float *out_scores,
+    uint32_t *n_redone, uint32_t n_facets, const uint32_t *facet_field, const uint32_t *facet_slot,
+    uint32_t *out_total, uint32_t *out_facet_counts) {
+    const uint32_t group[2] = {group_field, group_slot};
+    return bool_topk_multi(m, group, n_nodes, node_clause_starts, clause_node, clause_field, clause_terms,
+                           clause_term_starts, clause_idf, clause_weight, clause_occur, clause_group, clause_tie, mm,
+                           n_queries, slop, avg_doc_len, k1, b, k, where_bits, where_n, where_stride, out_docs,
+                           out_scores, n_redone, n_facets, facet_field, facet_slot, out_total, out_facet_counts);
 }
 
 // The value query q ranks doc docs[q * n_per_query + j] with, for each pair: bool_score_docs under the index's lock.

@@ -239,6 +239,10 @@ struct sa_index {
     DevBuf d_facet_tiles[SA_MAX_FACETS];
     u32 facet_buckets[SA_MAX_FACETS] = {};
     u32 facet_set = 0;
+    // group columns (sa_index_set_group, sa_feature.cu): slot s, when bit s of group_set is set, is d_groups[s]
+    // (u32 [padded n_docs], a doc's group or SA_GROUP_NONE, SA_GROUP_NONE past n_docs), read by the collapsed top-k
+    DevBuf d_groups[SA_MAX_GROUPS];
+    u32 group_set = 0;
     // host mirrors for query set-up
     std::vector<u64> h_off, h_len;
     std::vector<u32> h_df;

@@ -11,6 +11,10 @@
 // A facet column is stored as uint16[padded n_docs], 0xFFFF for "no value" and past n_docs, so the counting pass
 // reads a thread's four docs as one 8-byte load with no bounds test.  Beside it, per tile, the set of codes present
 // (1,024 bits): an In clause is present in a tile iff its codes meet that set.
+//
+// A group column (sa_index_set_group) is stored as u32[padded n_docs], SA_GROUP_NONE for "no group" and past n_docs;
+// the collapsed top-k reads it by doc id, for the docs of its windows only.
+#include <climits>
 #include <cmath>
 
 #include "sa_term.cuh"
@@ -149,5 +153,29 @@ extern "C" int sa_index_set_facet(sa_index *ix, uint32_t slot, const int32_t *co
     ix->d_facet_tiles[slot] = std::move(sets);
     ix->facet_buckets[slot] = n_buckets;
     ix->facet_set |= 1u << slot;
+    return SA_OK;
+}
+
+extern "C" int sa_index_set_group(sa_index *ix, uint32_t slot, const int32_t *codes, uint64_t n_values) {
+    SA_CHECK(ix && (codes || n_values == 0), "NULL argument");
+    SA_CHECK(slot < SA_MAX_GROUPS, "group slot %u out of range (%d slots)", slot, SA_MAX_GROUPS);
+    std::lock_guard<std::mutex> g(ix->mu);
+    SA_CHECK(n_values == ix->n_docs, "a group column has one code per doc: %llu codes for %llu docs",
+             (unsigned long long)n_values, (unsigned long long)ix->n_docs);
+    std::vector<u32> col(std::max<u64>(sa_padded_docs(ix->n_docs), 4), SA_GROUP_NONE);
+    for (u64 i = 0; i < n_values; i++) {
+        SA_CHECK(codes[i] >= -1 && codes[i] != INT32_MAX, "group code %llu (%d) is not -1 or in [0, 2^31 - 1)",
+                 (unsigned long long)i, codes[i]);
+        if (codes[i] >= 0) col[i] = (u32)codes[i];
+    }
+    SA_CUDA(cudaSetDevice(ix->device));
+    // into a new buffer, which replaces the slot's once it is filled: a failure leaves the slot as it was
+    DevBuf d;
+    int rc;
+    if ((rc = d.allocate(col.size() * sizeof(u32)))) return rc;
+    SA_CUDA(cudaMemcpyAsync(d.p, col.data(), col.size() * sizeof(u32), cudaMemcpyHostToDevice, ix->stream));
+    SA_CUDA(cudaStreamSynchronize(ix->stream));     // `col` is a local
+    ix->d_groups[slot] = std::move(d);
+    ix->group_set |= 1u << slot;
     return SA_OK;
 }

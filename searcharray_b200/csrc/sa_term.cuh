@@ -6,6 +6,7 @@
 #include <type_traits>
 
 #include "sa_common.cuh"
+#include "sa_scan.cuh"
 
 #define SA_TILE_DOCS 8192          // docs per CTA tile (32 KB of float32 scores)
 #define SA_TERM_UNROLL 4           // 30-word windows loaded per warp before processing
@@ -84,6 +85,11 @@ int sa_ensure_norm(sa_index *ix, float k1, float b, float avg_doc_len);
 int launch_topk_select(sa_index *ix, const TopkCtx &t, u32 n_queries, u64 doc_base, u64 *d_out_keys,
                        const u32 *d_out_index);
 u32 sa_topk_slots(u32 k);
+// The collapsed top k of each query from the runs of collapse_tile_collect (tile slots == k): the k best distinct
+// groups' leaders, keys as topk_select_kernel writes them to d_out_keys[q * k ..]; groups: the group column
+// (index-local ids); *d_windows counts the walk's windows past the first (see sa_topk.cu).
+int launch_topk_collapse(sa_index *ix, const TopkCtx &t, u32 n_queries, u64 doc_base, const u32 *groups,
+                         u64 *d_out_keys, u32 *d_windows);
 // Slots of a tile of collect_tile_f64: `shallow` for k <= SA_TOPK_MAX, max(k, 256) above (the deep bound keeps the k
 // best keys plus their ties)
 inline u32 sa_topk_slots_f64(u32 k, u32 shallow) { return k > SA_TOPK_MAX ? std::max(k, 256u) : shallow; }
@@ -400,6 +406,151 @@ __device__ __forceinline__ void deep_tile_collect(const float *s_tile, const Top
     u64 *__restrict__ run = t.tile_cand + t_idx * t.slots;
     for (u32 i = tid; i < m; i += blockDim.x) run[i] = s_run[i];
     if (tid == 0) publish_tile(t, row, tile, m, m ? (u32)(s_run[0] >> 32) : 0u);
+    __syncthreads();
+}
+
+// ---- collapse (sa_score_batch_topk_bool_collapse): one leader per group, taken by a walk over ranked keys in
+// descending order, window by window.  The groups taken so far and those of the current window live in a
+// shared-memory hash of 2^bits (code, position) pairs: s_hash[0 .. 2^bits) the codes (SA_COLLAPSE_EMPTY: a free
+// slot; group codes are below 2^31 - 1) and s_hash[2^bits .. 2^(bits+1)) per code 0 once taken, otherwise 1 + the
+// least window position holding it.
+#define SA_COLLAPSE_EMPTY 0xFFFFFFFFu
+#define SA_COLLAPSE_TILE_HASH_BITS 12      // a tile: <= k taken + SA_TOPK_DEEP_MAX in a window = 2,048 codes
+#define SA_COLLAPSE_TILE_SMEM ((2u << SA_COLLAPSE_TILE_HASH_BITS) * sizeof(u32))   // 32 KB of dynamic memory
+
+// Every thread of the CTA calls: every slot free.
+__device__ __forceinline__ void collapse_hash_clear(u32 *s_hash, u32 bits) {
+    for (u32 i = threadIdx.x; i < (2u << bits); i += blockDim.x) s_hash[i] = SA_COLLAPSE_EMPTY;
+}
+
+// The slot of code g (not SA_GROUP_NONE), inserted if absent: open addressing with linear probes.
+__device__ __forceinline__ u32 collapse_slot(u32 *s_hash, u32 bits, u32 g) {
+    const u32 mask = (1u << bits) - 1;
+    u32 h = (g * 0x9E3779B1u) >> (32 - bits);
+    for (;;) {
+        const u32 prev = atomicCAS(s_hash + h, SA_COLLAPSE_EMPTY, g);
+        if (prev == SA_COLLAPSE_EMPTY || prev == g) return h;
+        h = (h + 1) & mask;
+    }
+}
+
+// One window of the walk: s_win[0, m) ranked run keys (score_bits << 32 | ~doc, doc index-local) sorted descending,
+// m <= NT * PER, thread t owning positions PER t .. PER t + PER - 1.  A key is a leader iff its doc's code (groups[doc])
+// is SA_GROUP_NONE, or is not taken and no earlier position of the window holds it.  The leaders go, in order, to
+// ranks taken, taken + 1, ... below k through emit(rank, key); every code of the window is then taken.  Returns the
+// new number of leaders (<= k).  Every thread of the NT-thread CTA calls; returns after a barrier.
+template <int NT, int PER, typename E>
+__device__ __forceinline__ u32 collapse_window(const u64 *s_win, u32 m, const u32 *__restrict__ groups, u32 *s_hash,
+                                               u32 bits, u32 taken, u32 k, E emit) {
+    __shared__ u32 s_warp[NT / 32];
+    u32 *s_pos = s_hash + (1u << bits);
+    const u32 p0 = threadIdx.x * PER;
+    u32 slot[PER];
+#pragma unroll
+    for (int j = 0; j < PER; j++) {
+        slot[j] = SA_COLLAPSE_EMPTY;
+        if (p0 + j >= m) continue;
+        const u32 g = __ldg(groups + (0xFFFFFFFFu - (u32)s_win[p0 + j]));
+        if (g == SA_GROUP_NONE) continue;
+        slot[j] = collapse_slot(s_hash, bits, g);
+        atomicMin(s_pos + slot[j], p0 + j + 1);
+    }
+    __syncthreads();
+    u32 keep = 0;
+#pragma unroll
+    for (int j = 0; j < PER; j++)
+        if (p0 + j < m && (slot[j] == SA_COLLAPSE_EMPTY || s_pos[slot[j]] == p0 + j + 1)) keep |= 1u << j;
+    u32 total;
+    u32 r = taken + block_exclusive_sum<NT>((u32)__popc(keep), s_warp, total);
+#pragma unroll
+    for (int j = 0; j < PER; j++)
+        if ((keep >> j) & 1u) {
+            if (r < k) emit(r, s_win[p0 + j]);
+            r++;
+        }
+    __syncthreads();                                                 // every test above read s_pos
+#pragma unroll
+    for (int j = 0; j < PER; j++)
+        if (slot[j] != SA_COLLAPSE_EMPTY) s_pos[slot[j]] = 0;
+    __syncthreads();
+    return min(taken + total, k);
+}
+
+// The collapse tile collector: the tile's EXACT k best leaders (collapse_window) as one run sorted by key, descending,
+// with tile_cnt = its length and tile_max = its first score, as deep_tile_collect publishes its run.  A group whose
+// global leader d lies in this tile has fewer than k groups above it in the tile (each of them ranks above it
+// globally), so it is among the tile's k best leaders: topk_collapse_kernel's select over the runs is exact.  The
+// ranked keys are walked in windows of SA_TOPK_DEEP_MAX, each the next keys below the last window's least (a radix
+// select over the 48-bit keys of deep_tile_collect, sorted in s_run), until k leaders are taken or the ranked docs
+// run out.  groups: the group column (index-local ids); s_hash: SA_COLLAPSE_TILE_SMEM bytes; *windows counts the
+// windows past the first.  s_tile holds the tile's final scores, as deep_tile_collect takes them, and is not written.
+// All SA_TERM_THREADS threads call; returns after a barrier.
+__device__ __forceinline__ void collapse_tile_collect(const float *s_tile, const TopkCtx &t, u32 row, u32 tile,
+                                                      const u32 *__restrict__ groups, u32 *s_hash, u32 *windows) {
+    __shared__ u64 s_run[SA_TOPK_DEEP_MAX];
+    __shared__ u32 s_hist[256];
+    __shared__ u64 s_prefix;
+    __shared__ u32 s_krem, s_n, s_m, s_max;
+    const unsigned tid = threadIdx.x;
+    const u32 k = t.k, tile_doc0 = tile * SA_TILE_DOCS;
+    u64 hi = ~0ull;                                                  // keys below hi are still to walk
+    auto visit = [&](auto f) {
+#pragma unroll
+        for (int jj = 0; jj < SA_TILE_DOCS / SA_TERM_THREADS / 4; jj++) {
+            const unsigned g = tid + jj * SA_TERM_THREADS;
+            const float4 v = reinterpret_cast<const float4 *>(s_tile)[g];
+            const float vs[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+            for (int e = 0; e < 4; e++) {
+                const u64 key = ((u64)__float_as_uint(vs[e]) << 16) | (u64)(0xFFFFu - (g * 4 + e));
+                if (vs[e] > 0.0f && key < hi) f(key);
+            }
+        }
+    };
+    __syncthreads();                           // the tile as every thread stored it; the fold's dynamic memory is free
+    collapse_hash_clear(s_hash, SA_COLLAPSE_TILE_HASH_BITS);
+    if (tid == 0) { s_n = 0; s_max = 0; }
+    __syncthreads();
+    u32 mine = 0;
+    visit([&](u64) { mine++; });
+    mine = __reduce_add_sync(0xffffffffu, mine);
+    if ((tid & 31) == 0 && mine) atomicAdd(&s_n, mine);
+    __syncthreads();
+    // CTA-uniform: s_n is written only before the barrier above.  Each window gathers through its own counter s_m,
+    // which thread 0 clears when every thread is past the previous window's gather (the barriers of the sort and of
+    // collapse_window lie between), and which nothing reads but the gather's atomics after the barrier that follows
+    // the clear; with lo = 0 no radix select runs, so a shared counter would race with this read of s_n
+    u32 n = s_n, taken = 0, w = 0;
+    u64 *__restrict__ run = t.tile_cand + ((u64)row * t.n_tiles + tile) * t.slots;
+    while (taken < k && n > 0) {
+        const u32 m = min(n, (u32)SA_TOPK_DEEP_MAX);
+        const u64 lo = n > m ? radix_kth_largest<u64, 48>(m, s_hist, &s_prefix, &s_krem, visit) : 0ull;
+        if (tid == 0) s_m = 0;
+        __syncthreads();
+        visit([&](u64 key) {
+            if (key >= lo)
+                s_run[atomicAdd(&s_m, 1u)] = ((key >> 16) << 32) |
+                                             (u64)(0xFFFFFFFFu - (tile_doc0 + 0xFFFFu - (u32)(key & 0xFFFFu)));
+        });
+        u32 n2 = 1;
+        while (n2 < m) n2 <<= 1;
+        __syncthreads();
+        for (u32 i = m + tid; i < n2; i += blockDim.x) s_run[i] = 0ull;
+        __syncthreads();
+        bitonic_sort_desc_smem(s_run, n2);
+        taken = collapse_window<SA_TERM_THREADS, SA_TOPK_DEEP_MAX / SA_TERM_THREADS>(
+            s_run, m, groups, s_hash, SA_COLLAPSE_TILE_HASH_BITS, taken, k, [&](u32 r, u64 key) {
+                run[r] = key;
+                if (r == 0) s_max = (u32)(key >> 32);
+            });
+        n -= m;
+        hi = lo;
+        w++;
+    }
+    if (tid == 0) {
+        publish_tile(t, row, tile, taken, s_max);
+        if (w > 1) atomicAdd(windows, w - 1);
+    }
     __syncthreads();
 }
 

@@ -151,6 +151,83 @@ topk_select_kernel(TopkCtx t, u64 doc_base, u64 *__restrict__ out_keys, const u3
     }
 }
 
+// The collapsed top k of query q (collapse_tile_collect's runs, one leader per group and tile): the tile maxima bound
+// nothing here (two tiles' best docs may share a group), so every run key takes part.  The keys are walked in
+// descending order in windows of SEL_SMEM_KEYS -- each the next keys below the last window's least, from a radix
+// select over the 64-bit keys, gathered from the run prefixes (for_each_candidate<true>) and sorted -- and each window
+// keeps its leaders (collapse_window) until k groups are taken.  A group's best key over the runs is its global
+// leader, so the result is exact.  The hash holds <= k taken codes plus a window's 4,096 (dynamic memory,
+// SEL_COLLAPSE_SMEM).  Result keys as topk_select_kernel writes them, 0 past the last leader.
+#define SEL_COLLAPSE_HASH_BITS 13
+#define SEL_COLLAPSE_SMEM ((2u << SEL_COLLAPSE_HASH_BITS) * sizeof(u32))   // 64 KB
+__global__ void __launch_bounds__(SEL_THREADS)
+topk_collapse_kernel(TopkCtx t, const u32 *__restrict__ groups, u64 doc_base, u64 *__restrict__ out_keys,
+                     u32 *windows) {
+    __shared__ u64 s_keys[SEL_SMEM_KEYS];
+    __shared__ u32 s_hist[256];
+    __shared__ u64 s_prefix;
+    __shared__ u32 s_krem, s_n, s_m;
+    extern __shared__ u32 s_hash[];
+    const u32 q = blockIdx.x, k = t.k;
+    u64 *__restrict__ out = out_keys + (u64)q * k;
+    u64 hi = ~0ull;                                                  // keys below hi are still to walk
+    auto visit = [&](auto f) {
+        for_each_candidate<true>(t, q, 1u, [&](u64 key) {
+            if (key < hi) f(key);
+        });
+    };
+    collapse_hash_clear(s_hash, SEL_COLLAPSE_HASH_BITS);
+    if (threadIdx.x == 0) s_n = 0;
+    __syncthreads();
+    u32 mine = 0;
+    visit([&](u64) { mine++; });
+    mine = __reduce_add_sync(0xffffffffu, mine);
+    if ((threadIdx.x & 31) == 0 && mine) atomicAdd(&s_n, mine);
+    __syncthreads();
+    // CTA-uniform: s_n is written only before the barrier above; each window gathers through its own counter s_m, as
+    // collapse_tile_collect does (a shared counter cleared here would race with this read when no radix select runs)
+    u32 n = s_n, taken = 0, w = 0;
+    while (taken < k && n > 0) {
+        const u32 m = min(n, (u32)SEL_SMEM_KEYS);
+        const u64 lo = n > m ? radix_kth_largest<u64, 64>(m, s_hist, &s_prefix, &s_krem, visit) : 0ull;
+        if (threadIdx.x == 0) s_m = 0;
+        __syncthreads();
+        for_each_candidate<true>(t, q, max((u32)(lo >> 32), 1u), [&](u64 key) {
+            if (key >= lo && key < hi) s_keys[atomicAdd(&s_m, 1u)] = key;
+        });
+        u32 n2 = 1;
+        while (n2 < m) n2 <<= 1;
+        __syncthreads();
+        for (u32 i = m + threadIdx.x; i < n2; i += blockDim.x) s_keys[i] = 0ull;
+        __syncthreads();
+        bitonic_sort_desc_smem(s_keys, n2);
+        taken = collapse_window<SEL_THREADS, SEL_SMEM_KEYS / SEL_THREADS>(
+            s_keys, m, groups, s_hash, SEL_COLLAPSE_HASH_BITS, taken, k,
+            [&](u32 r, u64 key) { out[r] = key - doc_base; });      // (~local) - base == ~(local + base)
+        n -= m;
+        hi = lo;
+        w++;
+    }
+    for (u32 i = taken + threadIdx.x; i < k; i += blockDim.x) out[i] = 0ull;
+    if (threadIdx.x == 0 && w > 1) atomicAdd(windows, w - 1);
+}
+
+int launch_topk_collapse(sa_index *ix, const TopkCtx &t, u32 n_queries, u64 doc_base, const u32 *groups,
+                         u64 *d_out_keys, u32 *d_windows) {
+    if (n_queries == 0) return SA_OK;
+    SA_CHECK(t.k <= SA_TOPK_DEEP_MAX && t.slots == t.k, "collapse: k = %u, %u slots", t.k, t.slots);
+    SA_CUDA(cudaFuncSetAttribute(topk_collapse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)SEL_COLLAPSE_SMEM));
+    KernelTimer tm(ix, 1);
+    topk_collapse_kernel<<<n_queries, SEL_THREADS, SEL_COLLAPSE_SMEM, ix->stream>>>(t, groups, doc_base, d_out_keys,
+                                                                                     d_windows);
+    SA_CUDA(cudaGetLastError());
+    tm.stop();
+    ix->stats.topk_kernel_launches++;
+    ix->stats.total_launches++;
+    return SA_OK;
+}
+
 typedef unsigned __int128 u128;
 
 // The exact top k of a query whose candidates carry a float32 PROXY of a float64 score (collect_tile_f64: classic

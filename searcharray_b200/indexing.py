@@ -67,6 +67,9 @@ class HostIndex:
         # per-doc facet columns (SearchArray.set_facet): name -> (int32[n_docs] codes, -1: no value; n_buckets); a
         # name's slot on the device index is its position in this dict
         self.facets = {}
+        # per-doc group columns (SearchArray.set_group): name -> int32[n_docs] codes, -1: no group; a name's slot on
+        # the device index is its position in this dict
+        self.groups = {}
 
     # ---- on-disk posting words (reference phrase/memmap_arrays.py:145-208, MemoryMappedArrays): the words
     #      array written once to `<data_dir>/<n>.dat`, mapped back read-only; pickling stores the file name
@@ -95,6 +98,7 @@ class HostIndex:
         self.__dict__.update(st)
         self.__dict__.setdefault("features", {})
         self.__dict__.setdefault("facets", {})
+        self.__dict__.setdefault("groups", {})
         if st.get("words_file"):
             self._map_words()
 
@@ -128,6 +132,7 @@ class HostIndex:
         out = HostIndex(words, offs, lens, self.doc_lens[doc_lo:doc_hi], self.term_dict, self.avg_doc_length)
         out.features = {name: v[doc_lo:doc_hi].copy() for name, v in self.features.items()}
         out.facets = {name: (c[doc_lo:doc_hi].copy(), nb) for name, (c, nb) in self.facets.items()}
+        out.groups = {name: c[doc_lo:doc_hi].copy() for name, c in self.groups.items()}
         return out
 
 

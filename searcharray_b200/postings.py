@@ -252,16 +252,19 @@ class _PreparedBool:
     read and the counts it fills.  Build it and run it with the arrays' locks held (the array's lock; solr._locked for a
     multi)."""
 
-    def __init__(self, arrays, sims, clause_slot, queries, batch, where=None, facets=None, multi=None):
+    def __init__(self, arrays, sims, clause_slot, queries, batch, where=None, facets=None, multi=None, group=None):
         """arrays, sims: per slot its SearchArray and similarity (one array: one slot).  clause_slot: uint32 per clause
         of batch, its slot (0 for a nested clause).  batch: queries flattened (query.flatten_bool).  where: a packed
         mask (pack_where), None: no mask.  facets: (key in Hits.facets, slot, name) triples, None: no counting.
-        multi: the solr._Multi over arrays for fields_topk, None for one array.  A facet or feature name not set on its
-        slot's array, an In code past its facet's buckets, and DisMax members whose idf is not sparse-safe, are
+        multi: the solr._Multi over arrays for fields_topk, None for one array.  group: (slot, name) of a group column
+        set on arrays[slot] (set_group) to collapse on, None: no collapsing.  A facet, feature or group name not set on
+        its slot's array, an In code past its facet's buckets, and DisMax members whose idf is not sparse-safe, are
         ValueErrors, the names and codes checked before any device work."""
         from .query import Field, dismax_members
         self.arrays, self.batch, self.where = arrays, batch, where
         self.counts = None if facets is None else _Counts(facets, arrays, batch.n_queries)
+        # the collapse entry point's leading arguments: the group column's slot (and its field slot on a multi)
+        self.group = None if group is None else (group[0], arrays[group[0]]._group_slot(group[1]))
         clauses = batch.clauses
         feats = self.columns(clauses, clause_slot, arrays)
         text = np.asarray([i for i, c in enumerate(clauses) if c is not None and i not in feats], dtype=np.int64)
@@ -292,6 +295,8 @@ class _PreparedBool:
         if self.counts is not None:
             for s in set(self.counts.fields.tolist()):
                 arrays[s]._device().sync_facets(arrays[s].host)
+        if self.group is not None:
+            arrays[self.group[0]]._device().sync_groups(arrays[self.group[0]].host)
         for arr in arrays:          # a sliced view of the same column may have left its row filter installed
             arr._apply_rows(arr._device())
         if multi is None:
@@ -302,6 +307,12 @@ class _PreparedBool:
             self.c_field = (_lib.p_u32(clause_slot),)
             self.bm25 = tuple(_lib.p_f32(np.asarray(v, dtype=np.float32)) for v in
                               ([a.avg_doc_length for a in arrays], [s.k1 for s in sims], [s.b for s in sims]))
+        self.group_args = ()
+        if self.group is not None:
+            lib = _lib.lib()
+            self.entry = lib.sa_score_batch_topk_bool_collapse if multi is None else \
+                lib.sa_multi_score_batch_topk_bool_collapse
+            self.group_args = self.group[1:] if multi is None else self.group
 
     @staticmethod
     def columns(clauses, clause_slot, arrays):
@@ -328,10 +339,11 @@ class _PreparedBool:
         opt = lambda a, p: None if a is None else p(a)      # noqa: E731
         p_w, stride = _where_args(self.where)
         _lib.check(self.entry(
-            self.handle, len(b.node_starts) - 1, _lib.p_u32(b.node_starts), opt(b.clause_node, _lib.p_u32),
-            *self.c_field, _lib.p_u32(self.terms), _lib.p_u32(self.c_starts), _lib.p_f32(self.idfs),
-            opt(b.weights, _lib.p_f32), opt(b.occurs, _lib.p_u8), opt(b.groups, _lib.p_u32), opt(b.ties, _lib.p_f32),
-            _lib.p_u32(b.mm), b.n_queries, int(slop), *self.bm25, k, p_w, len(self.arrays[0]), stride,
+            self.handle, *self.group_args, len(b.node_starts) - 1, _lib.p_u32(b.node_starts),
+            opt(b.clause_node, _lib.p_u32), *self.c_field, _lib.p_u32(self.terms), _lib.p_u32(self.c_starts),
+            _lib.p_f32(self.idfs), opt(b.weights, _lib.p_f32), opt(b.occurs, _lib.p_u8), opt(b.groups, _lib.p_u32),
+            opt(b.ties, _lib.p_f32), _lib.p_u32(b.mm), b.n_queries, int(slop), *self.bm25, k, p_w, len(self.arrays[0]),
+            stride,
             _lib.p_u32(docs), _lib.p_f32(scores), ctypes.byref(n_redone), *_Counts.args(self.counts)))
         out = docs, scores, n_redone.value
         return out if self.counts is None else out + (self.counts.hits(),)
@@ -397,6 +409,8 @@ class DeviceIndex:
         self.sync_features(host)
         self.facets = {}            # slot -> the host codes last uploaded there
         self.sync_facets(host)
+        self.groups = {}            # slot -> the host codes last uploaded there
+        self.sync_groups(host)
 
     def sync_features(self, host: HostIndex):
         """Uploads every feature column of `host` that this index does not hold yet (sa_index_set_feature)."""
@@ -411,6 +425,13 @@ class DeviceIndex:
             if self.facets.get(slot) is not codes:
                 _lib.check(_lib.lib().sa_index_set_facet(self.handle, slot, _lib.p_i32(codes), len(codes), n_buckets))
                 self.facets[slot] = codes
+
+    def sync_groups(self, host: HostIndex):
+        """Uploads every group column of `host` that this index does not hold yet (sa_index_set_group)."""
+        for slot, codes in enumerate(host.groups.values()):
+            if self.groups.get(slot) is not codes:
+                _lib.check(_lib.lib().sa_index_set_group(self.handle, slot, _lib.p_i32(codes), len(codes)))
+                self.groups[slot] = codes
 
     @staticmethod
     def _destroy(handle):
@@ -805,6 +826,43 @@ class SearchArray(ExtensionArray):
             if self._shared["dev"] is not None:
                 self._shared["dev"].sync_facets(self.host)
 
+    def set_group(self, name, codes) -> None:
+        """Registers a per-document group column -- a franchise, a parent SKU, a site -- that search_topk and
+        solr.fields_topk collapse on with `collapse=`, returning one document per group.  codes: one integer per doc
+        of the array (on a shard, per row of the shard) in [-1, 2^31 - 1); -1 means the doc belongs to no group, and
+        each such doc is a group of its own.  A non-integer dtype is a TypeError; another length, a code out of range
+        or more than 4 names per index a ValueError, all before any device work.  Setting a name again replaces it.
+        Refused (ValueError) on a view, whose positions are not the index's docs.  The codes live with the index
+        (copies, pickles and shard slices carry them) and go to the device when it is first used, or at once if it
+        already is."""
+        from .query import SA_MAX_GROUPS
+        if not isinstance(name, str):
+            raise TypeError(f"a group name is a str, not {name!r}")
+        if self.rows is not None:
+            raise ValueError("set_group on a view (arr[mask]) is not supported: set it on the whole array")
+        c = np.asarray(codes)
+        if c.dtype.kind not in "iu":
+            raise TypeError(f"group codes are integers, not dtype {c.dtype}")
+        if c.shape != (self.host.n_docs,):
+            raise ValueError(f"a group column has one code per doc: shape ({self.host.n_docs},), not {c.shape}")
+        if len(c) and (int(c.min()) < -1 or int(c.max()) >= 2 ** 31 - 1):
+            raise ValueError(f"group codes are -1 (no group) or in [0, 2^31 - 1): {name!r} holds "
+                             f"[{int(c.min())}, {int(c.max())}]")
+        groups = self.host.groups
+        if name not in groups and len(groups) >= SA_MAX_GROUPS:
+            raise ValueError(f"an index holds at most {SA_MAX_GROUPS} group columns")
+        with self._shared["lock"]:
+            groups[name] = np.ascontiguousarray(c, dtype=np.int32).copy()
+            if self._shared["dev"] is not None:
+                self._shared["dev"].sync_groups(self.host)
+
+    def _group_slot(self, name):
+        """The slot of group column `name` on this array's index; ValueError if it is not set."""
+        names = list(self.host.groups)
+        if name not in names:
+            raise ValueError(f"group column {name!r} is not set on this array (set_group); set: {names}")
+        return names.index(name)
+
     def _facet_slot(self, name):
         """(slot, n_buckets) of facet `name` on this array's index; ValueError if it is not set."""
         names = list(self.host.facets)
@@ -821,7 +879,7 @@ class SearchArray(ExtensionArray):
 
     # -------------------------------------------------- batched, HBM-resident path
     def search_topk(self, queries, k=10, similarity: Similarity = default_bm25, slop=0, where=None, facets=None,
-                    rescore=None):
+                    rescore=None, collapse=None):
         """queries: list of str (term) or list[str] (phrase).  Returns (docs uint32[Q,k],
         scores float32[Q,k]): per query the k best scores > 0, by score descending then id ascending, empty
         slots NO_DOC / 0.  Scores never leave HBM except the top-k (sa_score_batch_topk).
@@ -897,9 +955,29 @@ class SearchArray(ExtensionArray):
         the top k by c = float32(query_weight * s1) + float32(rescore_weight * s2) (c desc, id asc); the scores
         returned are c, the hits pass 1's.  A rescore with another number of queries, a window outside [k, 1,024],
         a view or a similarity other than bm25_similarity is refused before any device work.  On a shard the window
-        is the shard's own top window."""
+        is the shard's own top window.
+
+        collapse: the name of a group column (set_group) to return one document per group, as Elasticsearch's
+        `collapse` and Solr's collapsing query parser (nullPolicy=expand) do.  Per query, of the docs with S_q > 0
+        (S_q as above, `where` applied) each group's leader is its doc with the highest S_q, ties to the lower id; a
+        doc whose code is -1 is a group of its own; the result is the k best leaders by (score desc, id asc), with the
+        ids and float32 scores the call without `collapse` returns for them, and NO_DOC / 0 past the last group.  So
+        the first k' results at k are those at k', and score_docs at the returned docs returns their scores.  With
+        `facets`, hits count documents, not groups (Elasticsearch's hits.total under collapse): they equal the hits
+        of the call without `collapse`.  Every query form the boolean path takes is accepted, with or without `where`
+        and `facets`; plain queries then rank as one-clause Or queries through the boolean fold.  Each tile of 8,192
+        docs keeps its exact k best leaders on the device, so the result is exact whatever the group sizes.  A name
+        that is not a str (TypeError), a name not set (ValueError), a view (NotImplementedError), a similarity other
+        than bm25_similarity (TypeError) and `collapse` with `rescore` (ValueError) are refused before any device
+        work.  On a shard the groups are collapsed over the shard's own docs: shards are not merged with
+        deduplication."""
         from .query import DISMAX, NESTED, OCCUR, OR_AND, bool_form, check_k, has_dismax, has_field, is_boolean
         k = check_k(k)
+        if collapse is not None:
+            if rescore is not None:
+                raise ValueError("collapse cannot be combined with rescore")
+            if not isinstance(collapse, str):
+                raise TypeError(f"collapse is the name of a group column (a str), not {collapse!r}")
         if rescore is not None:
             return self._search_topk_rescore(queries, k, similarity, slop, where, facets, rescore)
         queries = list(queries)
@@ -908,7 +986,7 @@ class SearchArray(ExtensionArray):
             facets = check_facet_keys(facets, "facet names")
         bits = None if where is None else pack_where(where, len(self), len(queries))
         kind = np.asarray([bool_form(q) if is_boolean(q) else 0 for q in queries])     # 0: plain
-        if facets is None and not kind.any():
+        if facets is None and collapse is None and not kind.any():
             self._check_topk_similarity(similarity)
             if self.rows is not None or not isinstance(similarity, Bm25Similarity):
                 return self._search_topk_sim(queries, k, similarity, slop, bits)
@@ -923,6 +1001,8 @@ class SearchArray(ExtensionArray):
                                           "compose .score() on the view")
             if not isinstance(similarity, Bm25Similarity):
                 raise TypeError(f"boolean queries support bm25_similarity only, not {similarity!r}")
+            if collapse is not None:
+                self._group_slot(collapse)
         hits = None if facets is None else Hits(np.zeros(len(queries), dtype=np.int64), {
             f: np.zeros((len(queries), self._facet_slot(f)[1]), dtype=np.int64) for f in facets})
         if any(has_dismax(q) for q, kd in zip(queries, kind) if kd >= DISMAX):      # k1 / b before any device work
@@ -935,10 +1015,10 @@ class SearchArray(ExtensionArray):
             if not sel.any():
                 continue
             part = [q for q, s in zip(queries, sel) if s]
-            if kd == 0 and bits is None and facets is None:
+            if kd == 0 and bits is None and facets is None and collapse is None:
                 docs[sel], scores[sel] = self._search_topk_plain(part, k, similarity, slop)
                 continue
-            out = self._search_topk_bool(part, k, similarity, slop, _where_part(bits, sel), facets)
+            out = self._search_topk_bool(part, k, similarity, slop, _where_part(bits, sel), facets, collapse)
             docs[sel], scores[sel] = out[:2]
             if hits is not None:
                 hits.total[sel] = out[3].total
@@ -1017,21 +1097,23 @@ class SearchArray(ExtensionArray):
                                                       _lib.p_u32(docs), _lib.p_f32(scores)))
         return docs, scores
 
-    def _prepare_bool(self, queries, similarity, where=None, facets=None):
+    def _prepare_bool(self, queries, similarity, where=None, facets=None, collapse=None):
         """Boolean queries of any forms, or plain ones (a batch of their own) as one-clause Or nodes, which score
         exactly as .score(q, slop=slop), as one sa_score_batch_topk_bool call flattened for the heaviest form among
         them (query.bool_form, flatten_bool): a _PreparedBool.  where: a packed mask (pack_where).  facets: facet names
-        (check_facet_keys) whose Hits the call returns.  Call it, and run the call, with the lock held."""
+        (check_facet_keys) whose Hits the call returns.  collapse: a group column's name, collapsed on
+        (sa_score_batch_topk_bool_collapse).  Call it, and run the call, with the lock held."""
         from .query import OR_AND, bool_form, flatten_bool, is_boolean
         batch = flatten_bool(queries, max((bool_form(q) for q in queries if is_boolean(q)), default=OR_AND))
         return _PreparedBool([self], [similarity], np.zeros(len(batch.clauses), dtype=np.uint32), queries, batch,
-                             where, None if facets is None else [(f, 0, f) for f in facets])
+                             where, None if facets is None else [(f, 0, f) for f in facets],
+                             group=None if collapse is None else (0, collapse))
 
-    def _search_topk_bool(self, queries, k, similarity, slop, where=None, facets=None):
+    def _search_topk_bool(self, queries, k, similarity, slop, where=None, facets=None, collapse=None):
         """_prepare_bool's call, made with the lock held: (docs, scores, queries re-run exactly), and the Hits with
         facets."""
         with self._shared["lock"]:
-            return self._prepare_bool(queries, similarity, where, facets).run(k, slop)
+            return self._prepare_bool(queries, similarity, where, facets, collapse).run(k, slop)
 
     def _topk_queries(self, queries, idf):
         """The queries as the batched top-k entries take them: term ids, start offsets and, per query, idf(dfs) of

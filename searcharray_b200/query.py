@@ -34,6 +34,7 @@ SA_FEATURE_TERM_BASE = 0xFF000000
 SA_MAX_FACETS = 8                 # include/searcharray_b200.h: facet columns of one index
 SA_FACET_MAX_BUCKETS = 1024       # include/searcharray_b200.h
 SA_BOOL_MAX_FACETS = 4            # include/searcharray_b200.h: facets counted in one call
+SA_MAX_GROUPS = 4                 # include/searcharray_b200.h: group columns of one index
 FEATURE_FUNCTIONS = {"linear": 0, "saturation": 1, "log": 2}     # SA_FEATURE_LINEAR, _SATURATION, _LOG
 SA_FEATURE_RANGE, SA_FEATURE_IN = 0x10, 0x11                       # include/searcharray_b200.h
 

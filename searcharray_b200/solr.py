@@ -493,20 +493,32 @@ def _facet_pairs(frame, facets):
     return facets
 
 
-def _fields_topk(frame, queries, k, similarity, slop, where=None, facets=None):
+def _collapse_pair(frame, collapse):
+    """fields_topk's collapse= as a (column, name) pair, checked before any device work: a pair (TypeError) whose
+    column is a SearchArray column of the frame (get_field) on whose index the group column is set (ValueError)."""
+    if not (isinstance(collapse, tuple) and len(collapse) == 2 and isinstance(collapse[1], str)):
+        raise TypeError(f"collapse of fields_topk is a (column, name) pair, not {collapse!r}")
+    get_field(frame, collapse[0])._group_slot(collapse[1])
+    return collapse
+
+
+def _fields_topk(frame, queries, k, similarity, slop, where=None, facets=None, collapse=None):
     """fields_topk and the number of queries re-run exactly (candidate overflow); with facets (a list of
-    (column, name) pairs), (docs, scores, queries re-run, Hits)."""
+    (column, name) pairs), (docs, scores, queries re-run, Hits).  collapse: a (column, name) pair, collapsed on."""
     queries = list(queries)
     if where is not None:
         where = pack_where(where, len(frame), len(queries))
     if facets is not None:
         facets = _facet_pairs(frame, facets)
-    batch, slot_of, arrays, sims = _fields_plan(frame, queries, similarity,
-                                                extra=[] if facets is None else [c for c, _ in facets])
+    if collapse is not None:
+        collapse = _collapse_pair(frame, collapse)
+    extra = ([] if facets is None else [c for c, _ in facets]) + ([] if collapse is None else [collapse[0]])
+    batch, slot_of, arrays, sims = _fields_plan(frame, queries, similarity, extra=extra)
     multi = _multi_for(arrays)
     with _locked(multi, arrays):
         return _PreparedBool(arrays, sims, _clause_slots(batch, slot_of), queries, batch, where,
-                             None if facets is None else [(p, slot_of[p[0]], p[1]) for p in facets], multi).run(k, slop)
+                             None if facets is None else [(p, slot_of[p[0]], p[1]) for p in facets], multi,
+                             None if collapse is None else (slot_of[collapse[0]], collapse[1])).run(k, slop)
 
 
 def fields_score_docs(frame: pd.DataFrame, queries, rows,
@@ -547,7 +559,7 @@ def _fields_topk_rescore(frame, queries, k, similarity, slop, where, facets, res
 
 def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
                 similarity: Union[Similarity, Dict[str, Similarity]] = default_bm25, slop: int = 0, where=None,
-                facets=None, rescore=None):
+                facets=None, rescore=None, collapse=None):
     """Batched Or / And / Bool queries whose clauses are on several columns of `frame` -- Lucene's
     `+title:star overview:war -overview:trek`, or Elasticsearch's most_fields `title:alien^2 overview:alien` -- ranked
     on the device in one batch.  Every clause is a query.Field(field, term or phrase), or a Boost of one; phrases match
@@ -591,13 +603,21 @@ def fields_topk(frame: pd.DataFrame, queries, k: int = 10,
     device work.
 
     rescore: a query.Rescore of queries of this form, as in SearchArray.search_topk -- the top k of the window
-    fields_topk ranks at k=rescore.window, by the combined score c; hits are pass 1's."""
+    fields_topk ranks at k=rescore.window, by the combined score c; hits are pass 1's.
+
+    collapse: a (column, name) pair naming a group column set on that column (SearchArray.set_group): one row per
+    group, as in SearchArray.search_topk -- the k best group leaders of S_q above, hits counting rows.  The column may
+    be any SearchArray column of the frame, read by a clause or not; it takes part in the column checks above.  A value
+    that is not a pair (TypeError), a name not set (ValueError) and `collapse` with `rescore` (ValueError) are refused
+    before any device work.  On a shard the groups are collapsed over the shard's own rows."""
     from .query import check_k
     k = check_k(k)
+    if collapse is not None and rescore is not None:
+        raise ValueError("collapse cannot be combined with rescore")
     if rescore is not None:
         return _fields_topk_rescore(frame, queries, k, similarity, slop, where, facets, rescore)
     if facets is not None:
-        docs, scores, _, hits = _fields_topk(frame, queries, k, similarity, slop, where, facets)
+        docs, scores, _, hits = _fields_topk(frame, queries, k, similarity, slop, where, facets, collapse)
         return docs, scores, hits
-    docs, scores, _ = _fields_topk(frame, queries, k, similarity, slop, where)
+    docs, scores, _ = _fields_topk(frame, queries, k, similarity, slop, where, collapse=collapse)
     return docs, scores
